@@ -2,6 +2,7 @@
 """bench.py -- SGD samples/sec on RCV1-shaped synthetic sparse data (BASELINE.json's metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--batch 256] [--mode sync]
+                   [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]/[2]): sync mode, RCV1-shaped synthetic rows (47 236 features, 700 000
 rows of which the first 80 % train -- Main.scala:52 --, ~0.2 % non-zeros), batch 256 per GPU, lambda 1e-5,
@@ -74,7 +75,13 @@ def parse():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--no-extras", action="store_true", help="skip sweep / async / parity / rpc_seam / e2e_fit sub-records")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU path only")
     if a.batch is None:
         a.batch = 256 if a.mode == "sync" else 1        # BASELINE.json configs[1]/[2] and configs[3]
     return a
@@ -85,7 +92,7 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def ncu_traffic(kernel_key: str):
@@ -103,7 +110,7 @@ def ncu_traffic(kernel_key: str):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md's clocks line), read every 25 ms from NVML
+    """SM clock and throttle reasons DURING the timed region, read every 25 ms from NVML
     in this process -- the same counters `nvidia-smi --query-gpu=clocks.sm,clocks_event_reasons.*` prints, without a
     looping nvidia-smi process next to the launching rank (whose peers spin for it inside the fused multi-GPU kernel).
     `nvidia-smi -lms 20` remains the fallback when NVML cannot be loaded."""
@@ -201,13 +208,21 @@ def nvlink_counters(device: int):
         return None
 
 
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """One DIR/<name>.npy per array (float64, the dtype the C ABI returns): same arguments, same inputs, so two builds
+    can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 def sync_config(args, world, n_train, B, S):
     """The `config` object of a sync line -- shared by the GPU arm and the reference arm so that they name the same
     workload."""
     return {"workload": f"sync SGD (configs[{1 if world == 1 else 2}]): RCV1-shaped synthetic, {DIM} feats, "
                         f"{args.rows} rows ({n_train} train), ~0.2% nnz, batch {B} per GPU",
             "mode": "sync", "batch_per_gpu": B, "sgd_steps_per_bench_step": S, "lambda": LAMBDA, "lr": LR,
-            "parallelism": f"dp{world}", "l2": "inputs (train CSR 0.43 GB) larger than the 126 MB L2; rows drawn at random",
+            "parallelism": f"dp{world}", "l2": "inputs (train CSR 0.43 GB) larger than the 50 MB L2; rows drawn at random",
             "values": "fp32", "state": "fp64"}
 
 
@@ -519,6 +534,8 @@ def bench_async(args, ctx, data, n_train, d, group, rank, local_rank, world):
     value = samples_total / (ms_dev * 1e-3)
     e2e_value = samples_total / wall
     w_master = ctx.async_master_weights() if rank == 0 else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"master_weights": w_master})
     hbm_peak, peak_src = peaks()
     mean_bytes = data.algorithmic_bytes() / data.n_rows
     achieved = (args.steps * U * B * mean_bytes) / (ms_dev * 1e-3) / 1e9     # per GPU
@@ -538,7 +555,7 @@ def bench_async(args, ctx, data, n_train, d, group, rank, local_rank, world):
             "config": {"workload": f"async Hogwild (configs[3]): RCV1-shaped synthetic, {DIM} feats, {args.rows} rows, batch {B}, "
                                    f"one worker per GPU, {args.lanes} Hogwild lanes per GPU, peer replica writes over NVLink",
                        "mode": "async", "batch": B, "lr": LR, "updates_per_gpu_per_step": U, "lanes": args.lanes,
-                       "parallelism": f"dp{world}", "l2": "rows drawn at random from 0.43 GB of CSR (larger than the 126 MB L2)"},
+                       "parallelism": f"dp{world}", "l2": "rows drawn at random from 0.43 GB of CSR (larger than the 50 MB L2)"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(assigned.nbytes), "d2h_bytes_per_step": 0,
                     "api": "dsgd_start_async ... dsgd_stop_async (C ABI)"},
             "gpu_launches": int(launches),
@@ -667,6 +684,8 @@ def main():
     value = samples_total / (ms * 1e-3)
     w_after = ctx.get_weights()
     last_losses = ctx.read_losses(S)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"weights": w_after, "step_losses": last_losses})
 
     # ---- leg 2: end to end through the C-ABI call with host buffers (e2e) --------------------------------
     ctx.set_weights(np.zeros(data.dim))

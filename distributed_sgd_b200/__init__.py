@@ -1,4 +1,4 @@
-"""distributed_sgd_b200 -- B200-native data-parallel SGD hot path behind the surface of
+"""distributed_sgd_b200 -- H100-native data-parallel SGD hot path behind the surface of
 zifeo/distributed-sgd's Slave / Master / SparseSVM (see DESIGN.md, INTEGRATION.md, include/dsgd.h).
 
 (The directory is named with an underscore because `distributed-sgd_b200` is not an importable

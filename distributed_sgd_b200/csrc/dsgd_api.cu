@@ -1,4 +1,4 @@
-// dsgd_api.cu -- the C ABI declared in include/dsgd.h over the sm_100a kernels in dsgd_kernels.cuh.
+// dsgd_api.cu -- the C ABI declared in include/dsgd.h over the sm_90a kernels in dsgd_kernels.cuh.
 // There is no CPU path in this library: without a usable GPU dsgd_create fails with DSGD_ERR_CUDA.
 #include "../../include/dsgd.h"
 
@@ -223,8 +223,8 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return bail("cudaGetDeviceProperties", e);
   ctx->sm_count = prop.multiProcessorCount;
   ctx->dev_name = prop.name;
-  if (prop.major != 10)
-    { int rc = fail(nullptr, DSGD_ERR_CUDA, "dsgd_create: device %d is sm_%d%d; this library is built for sm_100a only",
+  if (prop.major != 9 || prop.minor != 0)   // sm_90a code loads on compute capability 9.0 only
+    { int rc = fail(nullptr, DSGD_ERR_CUDA, "dsgd_create: device %d is sm_%d%d; this library is built for sm_90a only",
                     device, prop.major, prop.minor); delete ctx; return rc; }
   if ((e = cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   if (flags & DSGD_FLAG_ASYNC) {   // the worker loop's stream and the service stream exist in async mode only: streams
@@ -302,7 +302,7 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   if (!ctx) return "{}";
   char buf[512];
   snprintf(buf, sizeof buf,
-           "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_100a\", \"dim\": %d, \"rank\": %d, "
+           "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\"}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
            (long long)ctx->nnz);
@@ -599,7 +599,6 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
   sp.rows_log2 = 5;
   while (sp.rows_log2 > 3 && ((n + (1 << sp.rows_log2) - 1) >> sp.rows_log2) < 6 * n_warps_all) --sp.rows_log2;
   // the last fifth of the pass goes out in blocks of half the size (not below 8 rows): warps end closer together.
-  // (Measured r2q: 2 to 6 blocks per warp and a tail of 0 to 35 % all land within 1 % of each other, profiles/r2_streaming.md.)
   sp.tail_log2 = std::max(3, sp.rows_log2 - 1);
   sp.n_big = sp.tail_log2 < sp.rows_log2 ? ((n - n / 5) >> sp.rows_log2) : ((n + (1 << sp.rows_log2) - 1) >> sp.rows_log2);
   const int64_t n_blk = sp.n_big + cdiv(std::max<int64_t>(0, n - (sp.n_big << sp.rows_log2)), (int64_t)1 << sp.tail_log2);
@@ -779,8 +778,8 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
   return DSGD_OK;
 }
 
-// CTAs of the persistent kernel: one per SM (measured in round 1 with tools/sweep_persist.py: fastest at batch 64, 256
-// and 1024); every CTA owns at most kMaxRowsPerCta rows of a step.  0: the batch is too large for this kernel.
+// CTAs of the persistent kernel: one per SM (fastest at batch 64, 256 and 1024 when it was
+// measured); every CTA owns at most kMaxRowsPerCta rows of a step.  0: the batch is too large for this kernel.
 static int persist_grid(const dsgd_ctx *ctx, int64_t batch) {
   const int g = ctx->grid_limit > 0 ? std::min(ctx->grid_limit, ctx->sm_count) : ctx->sm_count;
   if (cdiv(batch, kMaxRowsPerCta) > g) return 0;

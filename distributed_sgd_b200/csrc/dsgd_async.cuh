@@ -62,7 +62,7 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long &s) {
 
 // `Random.shuffle(indices) take batchSize` (core/Slave.scala:86-88): the first B images of a keyed pseudo-random permutation
 // of [0, n) (dsgd_feistel.h).  The rejection loop of round 1 compared each candidate with all earlier ones on one lane:
-// 1.9 ms per batch of 256, 10 ms per batch of 1024 (profiles/r2_sweep.md).
+// milliseconds per batch of 256 or 1024.
 // One row of a batch, requested one row ahead of its use: window bounds, label and the first 128 pairs.
 struct AsyncBatchRow {
   int64_t s0, s1;

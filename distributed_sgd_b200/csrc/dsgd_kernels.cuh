@@ -1,4 +1,4 @@
-// dsgd_kernels.cuh -- sm_100a kernels of the SGD hot path (see DESIGN.md for the layout and rooflines).
+// dsgd_kernels.cuh -- sm_90a kernels of the SGD hot path (see DESIGN.md for the layout and rooflines).
 //
 // Device layout of the rows ("row windows"): one array of 8-byte (col:int32, val:fp32) pairs, each row
 // padded with (col = last col, val = 0) pairs to a multiple of 2 pairs so that every row window starts on
@@ -6,9 +6,9 @@
 // rp16[r] is the window start in 16-byte units.  A val == 0 pair is arithmetically inert everywhere:
 // it adds 0 to the dot product and is skipped by the scatter.
 //
-// State vectors (w, g, d) are fp64 and live in L2 (3 x 378 KB on a 126 MB L2); the HBM stream is the
+// State vectors (w, g, d) are fp64 and live in L2 (3 x 378 KB on a 50 MB L2); the HBM stream is the
 // row windows only.  All reference arithmetic cited as path:line under
-// /root/reference/src/main/scala/epfl/distributed/.
+// src/main/scala/epfl/distributed/ of the reference repository.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

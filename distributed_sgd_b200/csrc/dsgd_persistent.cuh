@@ -4,8 +4,8 @@
 // (core/Master.scala:179-198) together with the slave's gradient request (core/Slave.scala:142-157):
 // no launch, no host round trip and exactly ONE grid-wide barrier per SGD step -- on one GPU and on K GPUs.
 //
-// Measured facts this design answers (profiles/r1c_summary.md, tools/microbench.cu on a B200): L2 hit 307 cycles;
-// a gpu-scope release/acquire grid barrier ~2300 cycles; the step is a chain of dependent latencies, so the
+// Latencies this design answers (tools/microbench.cu measures them): an L2 hit and a gpu-scope grid barrier each cost
+// hundreds to thousands of cycles; the step is a chain of dependent latencies, so the
 // kernel removes links from the chain:
 //   * PRODUCER warp (one per CTA): row windows do not depend on the weights, so it walks the sample ids
 //     kStages steps ahead -- ids -> row pointers -> one TMA bulk copy (cp.async.bulk, mbarrier
@@ -20,14 +20,10 @@
 //     to a small EXACT fixed-point accumulator (three 40-bit limbs per value, 64-bit integer REDs, striped over 8 copies)
 //     before it arrives at the grid barrier: integer sums do not depend on the order of arrival, so there is nothing to
 //     sort out afterwards -- update warp 0 of every CTA reads the 512 bytes after the barrier (one L2 round trip,
-//     overlapped with the consumers' first gathers) and has c.  Measured history (profiles/r2_timeline.md): round 1 summed
-//     148 fp64 partials from one shared area after the barrier, c arrived 1 880 cycles into the interval; a second counter
-//     barrier among the update warps serialised with the grid barrier (+2 200 cycles per step); an all-to-all flag barrier
-//     carrying the partials took 5 100 cycles from the last arrival to the first exit against 2 450 for the counter.
-//   * GRID BARRIER: one release arrival on a counter, relaxed polling.  With an acquire fence after the poll a barrier
-//     costs 2 412 cycles for 148 CTAs on a B200 (tools/microbench.cu: 1 721 for 2 CTAs -- it is fences and L2 round trips,
-//     not contention; cooperative groups' grid.sync() 2 472; +1 300 with 448 REDs per CTA in flight); the acquire fence
-//     is not needed here (see grid_barrier_arrive_wait) and leaving it out saved 1 400 cycles per step.  The barrier is
+//     overlapped with the consumers' first gathers) and has c.  (Summing fp64 partials from a shared area after the
+//     barrier, a second counter barrier among the update warps and an all-to-all flag barrier were all slower.)
+//   * GRID BARRIER: one release arrival on a counter, relaxed polling.  Its cost is fences and L2 round trips, not
+//     contention (tools/microbench.cu); the acquire fence is not needed here (see grid_barrier_arrive_wait).  The barrier is
 //     still the largest single item of a step.
 //
 // One GPU (kMulti == false), interval I_t between grid barrier t-1 and t, W_t = weights step t differentiates at:
@@ -35,7 +31,7 @@
 //   updaters : W_t buffer <- update(W_{t-1}, g_{t-1}, c_{t-1}); zero g_{t+1}'s buffer; c_t, ||W_t||^2
 //   W and g of a column sit side by side in one 16-byte record {W, g} (three rotating record arrays): a consumer needs
 //   ONE 128-bit gather per non-zero -- the scattered 8-byte accesses of a CTA's non-zeros are what its time grows with
-//   (measured: 5 cycles per pair with two gathers and one RED, profiles/r2_timeline.md).
+//   (two gathers and one RED per pair were measured slower).
 //
 // K GPUs (kMulti == true; one process or ctx per GPU, every rank's receive area mapped into every peer over
 // NVLink), interval I_T:
@@ -210,8 +206,7 @@ __device__ __forceinline__ double apply_update(double wv, double graw, double c,
 // There is no acquire fence after the poll.  What follows the barrier reads mutable global data only with instructions
 // that are served by L2 -- ld.global.cg / ld.relaxed.gpu / red / the LL words' ld.relaxed.sys -- never through L1, and a
 // thread cannot issue them before the branch on the polled value resolves, so they reach L2 after the arrival they
-// observed, which every peer performed after its own writes (release).  The fence cost 1 400 cycles per step (measured:
-// last arrival -> first exit 1 728 ns with it, 928 ns without; profiles/r2_timeline.md); the trajectories are checked
+// observed, which every peer performed after its own writes (release).  Leaving the fence out shortens every barrier; the trajectories are checked
 // against the oracle to 1e-12 over hundreds of steps in the tests and in every bench run (`parity`).
 // Returns false if the watchdog fired.
 __device__ __forceinline__ bool grid_barrier_arrive_wait(unsigned *bar, unsigned target, int *abort_flag, long long timeout) {
@@ -232,11 +227,11 @@ __device__ __forceinline__ bool grid_barrier_arrive_wait(unsigned *bar, unsigned
 // ---- order-free exact sums of the per-CTA partials -------------------------------------------------------------------
 // A double v with |v| < 2^52 is cut into three integers: |v| = l2 + l1 * 2^-40 + l0 * 2^-80, l1 and l0 in [0, 2^40] (l0
 // rounded: resolution 2^-80), every cut exact in fp64 arithmetic; negative v contribute the negated limbs.  The limbs of
-// 148 CTAs are added with 64-bit integer REDs (no overflow: 148 * 2^40 < 2^48) and converted back once.  One accumulator
+// all CTAs are added with 64-bit integer REDs (no overflow while CTAs < 2^8: 2^8 * 2^40 = 2^48) and converted back once.  One accumulator
 // = 8 x u64 = 64 bytes {sd.l0, sd.l1, sd.l2, sn.l0, sn.l1, sn.l2, overflow count, pad} on its own 128-byte line: every CTA
-// adds ONE partial per step (148 same-address REDs per limb: ~400 cycles at 2.7 cycles each, tools/microbench.cu) and
+// adds ONE partial per step (one same-address RED per CTA and limb, tools/microbench.cu) and
 // reads the 64 bytes back with ONE coalesced request.  (First cut: 8 striped copies read with 16-byte loads = 2 368
-// requests on 4 lines after every barrier: c arrived 2 170 cycles into the interval, profiles/r2_timeline.md.)
+// requests on 4 lines after every barrier: c arrived later.)
 constexpr int kAccStride = 16;   // u64 words between the three rotating accumulators (128 bytes)
 __device__ __forceinline__ void red_add_u64(unsigned long long *p, unsigned long long v) {
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
@@ -382,7 +377,7 @@ struct FetchLL {
     }
   }
   // All pending words are REQUESTED before any is looked at (a request and its check written together compile into
-  // one dependent round trip per word: nvcc reuses the destination registers -- measured, profiles/r2_multi_gpu.md).
+  // one dependent round trip per word: nvcc reuses the destination registers).
   __device__ __forceinline__ void get4(const uint2 (&pr)[4], double (&wv)[4]) {
     unsigned pend = 0;   // bit u: word of pair u not published yet; all pending words are re-requested together
 #pragma unroll
@@ -785,8 +780,8 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
             const unsigned long long *bm0 = p.xbm[me] + (size_t)parp * p.xwords + (size_t)col_word;
             const unsigned long long *vl0 = p.xval[me] + 2 * ((size_t)parp * p.xstride + (size_t)j_col);
             // All K-1 bitmap words are requested together and re-requested together until every one carries this step's
-            // tag: the wait is the LATEST peer plus one poll, not a poll per peer in turn (with one peer polled after the
-            // other the 8-GPU step spent 13 600 cycles here, profiles/r2_multi_gpu.md).  Polling HARDER does not pay:
+            // tag: the wait is the LATEST peer plus one poll, not a poll per peer in turn (polling one peer after the
+            // other costs a round trip per peer).  Polling HARDER does not pay:
             // a second request set half a round trip behind the first made the 2-GPU step 8.6 -> 13.5 us, and requesting
             // every thread's value word along with the bitmap word (66 000 more requests per round) 8.5 -> 8.6 us --
             // the polled lines are the ones the NVLink writes are landing in.

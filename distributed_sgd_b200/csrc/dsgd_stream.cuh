@@ -15,8 +15,8 @@
 //     busy).  A lane accumulates its units of the open row; the warp reduces once per ROW END (one 5-step butterfly
 //     of ONE float), not per load, and the row's lane just keeps the sum: predictions, counters and gates of the 32
 //     rows are worked out by 32 lanes in parallel after the block's stream.  The kernel is ISSUE-bound before it is
-//     HBM-bound (ncu: round 2's first cut 108 warp instructions per 64 pairs = 131 us per evaluation pass; 100.8 us at
-//     70; 88.7 us at ~55, profiles/r2_streaming.md), so every per-slot instruction counts: groups that lie inside the block
+//     HBM-bound (fewer warp instructions per 64 pairs made the evaluation
+//     pass faster at every step), so every per-slot instruction counts: groups that lie inside the block
 //     carry no bounds predicates (only a block's last group does), a slot without a row end adds its products with one
 //     FADD, and a pass over CONSECUTIVE rows (kContig: evaluation) needs no row lookup for its loads at all -- the windows
 //     are back to back in the pair array -- so its four loads leave before the row-end masks are even computed.
@@ -31,9 +31,8 @@
 //   * Scatter (gradient): rows that pass the gate are re-walked after the block's stream (their units are in
 //     L1/L2) and y*x goes to g with fp64 REDs.  On trained weights few rows pass (the misclassified ones) and the pass
 //     runs at the streaming rate; on untrained weights every row passes and the fp64 RED rate at L2 bounds it
-//     (0.45 per SM-cycle, tools/microbench.cu).  Per-CTA fixed-point accumulators in shared memory for the most
-//     frequent columns were measured and dropped: 162 -> 160 us on 262 144 rows, 58 -> 64 us on 65 536
-//     (profiles/r2_streaming.md).
+//     (tools/microbench.cu).  Per-CTA fixed-point accumulators in shared memory for the most frequent columns were
+//     measured and dropped (no net gain).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -197,7 +196,7 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
     // row of each lane's unit, then the 128-bit loads -- all issued before the first is used (64 KB in flight per SM).
     // Groups that lie entirely inside the block (kFull) carry no bounds predicates; the block's last group does.
     // (A software-prefetched form -- group g + 1 fetched before group g is processed, 768 threads x 80 registers -- was
-    // measured SLOWER: 118.9 us against 107.4 us per evaluation pass, profiles/r2_streaming.md: the lost warps cost more
+    // measured SLOWER per evaluation pass: the lost warps cost more
     // latency hiding than the deeper queue bought.)
     auto do_group = [&](auto full_tag, const int v0) {
       constexpr bool kFull = decltype(full_tag)::value;

@@ -1,7 +1,7 @@
 """ctypes binding of libdsgd.so (the C ABI in include/dsgd.h) and libdsgd_host.so (data preparation).
 
 This is the only place the Python host touches native code.  There is no fallback: if libdsgd.so is
-missing or no B200 is usable, the call raises (NativeLibraryMissing / DsgdError) -- nothing in this
+missing or no H100 is usable, the call raises (NativeLibraryMissing / DsgdError) -- nothing in this
 package computes the hot path on the CPU.
 """
 from __future__ import annotations
@@ -59,7 +59,7 @@ _EXC = {ERR_INVALID: DsgdInvalid, ERR_STATE: DsgdState, ERR_EMPTY: DsgdEmpty, ER
 
 
 def build(verbose: bool = False) -> None:
-    """Compile libdsgd.so (nvcc, sm_100a) and libdsgd_host.so (gcc) in-tree."""
+    """Compile libdsgd.so (nvcc, sm_90a) and libdsgd_host.so (gcc) in-tree."""
     r = subprocess.run(["make", "-C", os.path.join(_PKG, "csrc"), "all"], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout)
@@ -135,7 +135,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise NativeLibraryMissing(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  There is no CPU fallback for the hot path.")
+                "(nvcc, sm_90a).  There is no CPU fallback for the hot path.")
         l = C.CDLL(LIB_PATH)
         for name, args in ABI.items():
             fn = getattr(l, name)  # AttributeError here == header and library disagree

@@ -1,10 +1,10 @@
 /*
- * dsgd.h -- C ABI of the B200-native data-parallel SGD hot path (libdsgd.so).
+ * dsgd.h -- C ABI of the H100-native (sm_90a) data-parallel SGD hot path (libdsgd.so).
  *
  * This is the drop-in boundary for zifeo/distributed-sgd's hot path.  The reference has no FFI of its
  * own (it is 100 % Scala over gRPC, SURVEY.md F1/F2); the seams this ABI sits behind are the handlers of
  * its gRPC `Slave` service and the step body of `Master.fit`.  Every entry point names the reference
- * interface it replaces (path:line under /root/reference/src/main/).  INTEGRATION.md shows the JNI /
+ * interface it replaces (path:line under the reference repository's src/main/).  INTEGRATION.md shows the JNI /
  * Scala binding a maintainer would add; distributed_sgd_b200/ is the Python host that mirrors the
  * reference's Slave / Master / SparseSVM surface over this ABI.
  *

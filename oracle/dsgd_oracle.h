@@ -15,7 +15,7 @@
  * "key absent from the reference's Map".  CSR column c stands for the reference's 1-based feature
  * key c+1; dimSparsity is passed already shifted into the weight index space (see
  * dsgd_oracle_dim_sparsity).  Citations are path:line under
- * /root/reference/src/main/scala/epfl/distributed/.
+ * src/main/scala/epfl/distributed/ of the reference repository.
  */
 #ifndef DSGD_ORACLE_H
 #define DSGD_ORACLE_H

@@ -14,7 +14,7 @@ route through the oracle).  PARITY STATUS: "parity unpinned" for SparseSVM / Sla
 Master (the reference has zero tests there, SURVEY.md 8c); pinned only for the L0 vector
 algebra by VecTests.
 
-Citations are path:line under /root/reference/src/main/scala/epfl/distributed/.
+Citations are path:line under src/main/scala/epfl/distributed/ of the reference.
 """
 from __future__ import annotations
 

@@ -14,7 +14,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); select with -m gpu")
 
 
 def random_csr(rng, n_rows, dim, max_nnz=12, min_nnz=1, allow_empty=False, dup_values=False):

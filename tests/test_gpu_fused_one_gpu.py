@@ -1,12 +1,12 @@
 """The fused K-rank sync kernel (sparse LL exchange through peer memory, dsgd_persistent.cuh kMulti) exercised on ONE GPU:
 K device contexts share the GPU (each limited to 1/K of the SMs with dsgd_set_grid_limit, attached to each other with
 dsgd_xchg_attach), one host thread per context like one JVM thread per Slave.  The ranks' kernels run concurrently and
-exchange exactly as they do over NVLink -- the receive areas just live in the same HBM -- so the driver's single-GPU test
-box runs the multi-rank path for real: trajectories against the oracle's K-worker master step (core/Master.scala:184-197),
+exchange exactly as they do over NVLink -- the receive areas just live in the same HBM -- so a single-GPU
+machine runs the multi-rank path for real: trajectories against the oracle's K-worker master step (core/Master.scala:184-197),
 bit-identical replicas, several launches in a row (global step counter, receive parities), short last batches.
 K stops at 3 here: four spinning kernels sharing one GPU hit the device-side watchdog in 2 of 9 sessions (CUDA does not
 promise co-scheduling of independent kernels; cooperative launch is per kernel) -- four and eight ranks are checked on real
-GPUs by bench.py's parity record and whole-run replays (profiles/r2_multi_gpu.md).  A watchdog time-out is retried once.
+GPUs by bench.py's parity record and whole-run replays.  A watchdog time-out is retried once.
 """
 import threading
 

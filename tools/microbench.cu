@@ -1,5 +1,5 @@
-// Dev microbenchmarks for the latency model of the persistent SGD kernel (sm_100a).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench microbench.cu && ./microbench
+// Dev microbenchmarks for the latency model of the persistent SGD kernel (sm_90a).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench microbench.cu && ./microbench
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cstdlib>
@@ -330,7 +330,7 @@ int main() {
     CK(cudaFree(d));
   }
   unsigned *bar; CK(cudaMalloc(&bar, 1024));
-  for (int G : {2, 8, 32, 64, 148}) {
+  for (int G : {2, 8, 32, 64, 132}) {
     long long r[4];
     for (int mode = 0; mode < 3; ++mode) {
       CK(cudaMemset(bar, 0, 1024));
@@ -346,7 +346,7 @@ int main() {
     printf("ping-pong round trip (release add -> acquire poll, two CTAs): %lld cyc\n", *out); }
   double *bd; float *bf; CK(cudaMalloc(&bd, 8 << 20)); CK(cudaMalloc(&bf, 4 << 20)); CK(cudaMemset(bd, 0, 8 << 20)); CK(cudaMemset(bf, 0, 4 << 20));
   for (int n_addr : {1, 16, 1024, 47236, 1 << 20}) {
-    for (int blocks : {32, 148}) {
+    for (int blocks : {32, 132}) {
       int reps = 64;
       k_red<double><<<blocks, 256>>>(bd, n_addr, reps, out); CK(cudaDeviceSynchronize()); long long a = *out;
       k_red<float><<<blocks, 256>>>(bf, n_addr, reps, out); CK(cudaDeviceSynchronize()); long long b = *out;
@@ -372,7 +372,7 @@ int main() {
     run((void *)k_barrier2<8, true, true>, "flags per 8 CTAs + 1 RED/thread:");
   }
   for (int threads : {256, 1024})
-    for (int blocks : {8, 16, 32, 74, 148}) {
+    for (int blocks : {8, 16, 32, 66, 132}) {
       int reps = 64, n_addr = 47236;
       k_red<double><<<blocks, threads>>>(bd, n_addr, reps, out); CK(cudaDeviceSynchronize()); long long a = *out;
       k_gather<<<blocks, threads>>>(bd, n_addr, reps, out, bd + n_addr); CK(cudaDeviceSynchronize()); long long b = *out;

@@ -1,6 +1,6 @@
 """Static SASS facts per kernel of libdsgd.so (cuobjdump -sass / -res-usage): the mnemonics that prove TMA bulk copies,
 mbarriers, fp64 reductions without a return value, system-scope LL stores, and the absence of tensor-core instructions.
-    python tools/sass_table.py > profiles/r2_sass_evidence.md"""
+    python tools/sass_table.py > sass_evidence.md"""
 import collections
 import os
 import re
@@ -34,8 +34,8 @@ usage = {}
 for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+)", res):
     usage[demangle(m.group(1))] = (int(m.group(2)), int(m.group(3)), int(m.group(4)))
 
-print("# SASS evidence, round 2 (`cuobjdump -sass distributed_sgd_b200/libdsgd.so`, sm_100a, nvcc 12.9; `tools/sass_table.py`)\n")
-print("What the mnemonics prove (B200_PROFILING.md): `UBLKCP` = TMA bulk copy (`cp.async.bulk`), `SYNCS.*` = mbarrier (`arrive.expect_tx`,\n"
+print("# SASS evidence (`cuobjdump -sass distributed_sgd_b200/libdsgd.so`, sm_90a, nvcc 12.9; `tools/sass_table.py`)\n")
+print("What the mnemonics prove: `UBLKCP` = TMA bulk copy (`cp.async.bulk`), `SYNCS.*` = mbarrier (`arrive.expect_tx`,\n"
       "`try_wait`), `REDG.E.ADD.F64` = fp64 reduction at L2 WITHOUT a return value (gradient scatter; at `.SYS` scope the async peer-replica\n"
       "writes), `..STRONG.SYS` loads/stores = the LL words of the multi-GPU exchange (`st.relaxed.sys` / `ld.relaxed.sys`), `REDUX` = the\n"
       "warp or-reductions of the flat stream.  `ATOMG` = atomics WITH a return value: the streaming kernels' block tickets and nothing on\n"

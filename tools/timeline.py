@@ -24,7 +24,7 @@ def report(tl_all, B, ms, S, world):
         v = (t[:, k] - t[:, 0])[t[:, k] > 0]
         if len(v):
             print(f"  {NAMES[k]:48s} +{np.mean(v):8.0f} cycles (min {v.min()}, max {v.max()})")
-    G = 148
+    G = 132   # one CTA per SM of an H100
     for k in range(4):
         a, b, nz = per_cta[k, :G, 0], per_cta[k, :G, 1], per_cta[k, :G, 2]
         if not a.any():
