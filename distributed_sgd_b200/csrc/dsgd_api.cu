@@ -10,6 +10,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -37,7 +38,6 @@ struct dsgd_ctx {
 
   // rows
   int64_t n_rows = 0, nnz = 0, n_pairs = 0;
-  bool rows_unique = false;   // every row's columns are strictly increasing (no duplicate keys: the reference's rows are Maps)
   uint32_t *rp16 = nullptr;
   uint2 *pairs = nullptr;
   int8_t *label = nullptr;
@@ -92,6 +92,7 @@ struct dsgd_ctx {
   int32_t *a_rows = nullptr, *a_assigned = nullptr, *a_replay = nullptr;
   int64_t a_rows_cap = 0, a_assigned_cap = 0, a_replay_cap = 0;
   int32_t *u_idx = nullptr; double *u_val = nullptr; int64_t u_cap = 0;  // update_grad staging
+  std::mutex u_mu;                  // dsgd_update_grad: one call at a time stages, launches and waits
   bool a_running = false;
   cudaEvent_t a_ev0 = nullptr, a_ev1 = nullptr;
 
@@ -398,10 +399,15 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
   for (int64_t k = 0; k < nnz; ++k)
     NEED(col[k] >= 0 && col[k] < ctx->dim, DSGD_ERR_RANGE, "dsgd_load_csr: column %d at position %lld outside [0,%d)",
          col[k], (long long)k, ctx->dim);
-  bool unique = true;
-  for (int64_t r = 0; r < n_rows && unique; ++r)
-    for (int64_t k = row_ptr[r] + 1; k < row_ptr[r + 1]; ++k)
-      if (col[k] <= col[k - 1]) { unique = false; break; }
+  {  // the reference's rows are Maps: a key occurs once per row (any order); per-column stamp of the last row that held it
+    std::vector<int64_t> seen((size_t)ctx->dim, -1);
+    for (int64_t r = 0; r < n_rows; ++r)
+      for (int64_t k = row_ptr[r]; k < row_ptr[r + 1]; ++k) {
+        NEED(seen[(size_t)col[k]] != r, DSGD_ERR_INVALID, "dsgd_load_csr: row %lld repeats column %d (position %lld)",
+             (long long)r, col[k], (long long)k);
+        seen[(size_t)col[k]] = r;
+      }
+  }
   CU(cudaSetDevice(ctx->device));
   for (void *p : {(void *)ctx->rp16, (void *)ctx->pairs, (void *)ctx->label, (void *)ctx->yabs}) if (p) CU(cudaFree(p));
   ctx->rp16 = nullptr; ctx->pairs = nullptr; ctx->label = nullptr; ctx->yabs = nullptr;
@@ -427,7 +433,7 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream));
   CU(cudaFree(d_rp)); CU(cudaFree(d_col)); CU(cudaFree(d_val));
-  ctx->n_rows = n_rows; ctx->nnz = nnz; ctx->n_pairs = n_pairs; ctx->rows_unique = unique;
+  ctx->n_rows = n_rows; ctx->nnz = nnz; ctx->n_pairs = n_pairs;
   return DSGD_OK;
 }
 
@@ -1264,7 +1270,6 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   AsyncParams ap;
   ap.rp16 = ctx->rp16; ap.pairs = ctx->pairs; ap.label = ctx->label; ap.d = ctx->d; ap.dim = ctx->dim;
   ap.assigned = assigned; ap.n_assigned = n_assigned; ap.replay = replay; ap.batch = batch; ap.lr = lr; ap.lambda = ctx->lambda;
-  ap.rows_unique = ctx->rows_unique ? 1 : 0;
   int nr = 0;
   ap.replica[nr++] = ctx->w;
   for (int r = 0; r < ctx->world && r < kMaxReplicas - 1; ++r)
@@ -1283,9 +1288,8 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   CU(cudaStreamSynchronize(ctx->stream));  // inputs in place before the loop's own stream starts
   if (!ctx->a_ev0) { CU(cudaEventCreate(&ctx->a_ev0)); CU(cudaEventCreate(&ctx->a_ev1)); }
   CU(cudaEventRecord(ctx->a_ev0, st));
-  // batch 1 on rows with unique columns (what the reference's Map rows are): the delta of every non-zero is formed straight
-  // from the pair, without the per-lane scratch vector
-  if (batch == 1 && ctx->rows_unique) k_async_worker_b1<<<cdiv(lanes, 4), 128, 0, st>>>(ap);
+  // batch 1: the delta of every non-zero is formed straight from the pair, without the per-lane scratch vector
+  if (batch == 1) k_async_worker_b1<<<cdiv(lanes, 4), 128, 0, st>>>(ap);
   else k_async_worker<<<cdiv(lanes, 4), 128, 0, st>>>(ap);
   CU(cudaEventRecord(ctx->a_ev1, st));
   LAUNCHED();
@@ -1378,6 +1382,9 @@ extern "C" int dsgd_async_elapsed_ms(dsgd_ctx *ctx, float *elapsed_ms) {
 
 extern "C" int dsgd_update_grad(dsgd_ctx *ctx, const int32_t *idx, const double *val, int64_t nnz) {
   if (!ctx) return DSGD_ERR_INVALID;
+  // concurrent callers (a gRPC server's thread pool) share the staging buffers: the next call may refill or regrow them only
+  // after this call's kernel has finished reading them
+  std::lock_guard<std::mutex> lock(ctx->u_mu);
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot update gradient: slave is in synchronous mode.");
   NEED(nnz >= 0 && (nnz == 0 || (idx && val)), DSGD_ERR_INVALID, "dsgd_update_grad: bad arguments");
   for (int64_t k = 0; k < nnz; ++k)

@@ -13,6 +13,14 @@
 // the reference's strictly sequential loop).  c = 2*lambda*(w . d) needs the whole weight vector every iteration
 // in the reference; each replica instead carries S = w . d in a control slot, and whoever applies a delta to a
 // replica also applies  S -= sum_j delta_j d_j  to it -- O(nnz) instead of O(dim), same value up to fp64 rounding.
+//
+// Every replica update of the reference builds a new Sparse (`weights.single.transform(_ - gradUpdate)`, core/Slave.scala:
+// 101, 180; `grad - gradUpdate`, core/ml/GradState.scala:8), so an entry with |w - delta| <= 1e-20 leaves the map.  A red.add
+// cannot filter its result; instead the lane checks its snapshot wv of the entry after sending -delta: when wv - delta is tiny
+// and nonzero it sends that residual as well, so the entry lands on exactly 0 (async_apply_key).  Every replica, the outbox
+// and S receive the same amounts.  The check follows the red.adds, so the common case waits for nothing new.  With one lane the
+// snapshot is the entry, so this is the reference's arithmetic exactly; with concurrent lanes another lane may move the entry
+// between the snapshot and the red.add (DESIGN.md 4.4).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -50,8 +58,19 @@ struct AsyncParams {
   volatile int *stop;       // raised by dsgd_stop_async
   unsigned long long *claimed;  // next iteration number to claim (lanes race for iterations)
   unsigned long long *done;     // iterations finished by this worker
-  int rows_unique;              // every row's columns are distinct (checked when the rows were loaded)
 };
+
+// w -= delta on key j of every replica, the result filtered against the snapshot wv (math/Sparse.scala:108-118); sd += the
+// amount times d_j
+__device__ __forceinline__ void async_apply_key(const AsyncParams &p, int j, double wv, double delta, double dj, double &sd) {
+  for (int q = 0; q < p.n_replicas; ++q) red_add_f64_sys(&p.replica[q][j], -delta);
+  sd += delta * dj;
+  const double nw = wv - delta;
+  if (nw != 0.0 && fabs(nw) <= kEps) {   // the entry would keep a residual the reference's new Sparse drops
+    for (int q = 0; q < p.n_replicas; ++q) red_add_f64_sys(&p.replica[q][j], -nw);
+    sd += nw * dj;
+  }
+}
 
 __device__ __forceinline__ unsigned long long mix64(unsigned long long &s) {
   unsigned long long z = (s += 0x9E3779B97F4A7C15ull);
@@ -146,30 +165,23 @@ __global__ void __launch_bounds__(128) k_async_worker(const AsyncParams p) {
         }
         dot = warp_sum(dot);
         if (!(cur.y * dot < 0.0)) {  // SparseSVM.scala:28
-          // Vec.sum: left fold, filter after each +.  A column occurs once per row (unique-column rows) or in consecutive
-          // pairs of the same lane stride; the read-modify-write below is per lane, in pair order, as before
-          auto add_pair = [&](const uint2 pr) {
-            const double gv = filt(filt((double)__uint_as_float(pr.y)) * cur.y);
-            if (gv != 0.0) scratch[pr.x] = filt(scratch[pr.x] + gv);
-          };
-          if (p.rows_unique) {
-            // distinct columns inside a row: the lane's four read-modify-writes are independent -- all four scratch entries
-            // are requested before the first is used (one L2 round trip instead of four dependent ones)
-            double gv[4], sv[4];
+          // Vec.sum: left fold in batch order, filter after each +.  A column occurs once per row (dsgd_load_csr rejects
+          // repeated keys), so the lane's four read-modify-writes are independent -- all four scratch entries are requested
+          // before the first is used (one L2 round trip instead of four dependent ones)
+          double gv[4], sv[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              gv[u] = (cur.s0 + lane + 32 * u < cur.s1) ? filt(filt((double)__uint_as_float(cur.pre[u].y)) * cur.y) : 0.0;
-              sv[u] = (gv[u] != 0.0) ? scratch[cur.pre[u].x] : 0.0;
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              if (gv[u] != 0.0) scratch[cur.pre[u].x] = filt(sv[u] + gv[u]);
-          } else {
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              if (cur.s0 + lane + 32 * u < cur.s1) add_pair(cur.pre[u]);
+          for (int u = 0; u < 4; ++u) {
+            gv[u] = (cur.s0 + lane + 32 * u < cur.s1) ? filt(filt((double)__uint_as_float(cur.pre[u].y)) * cur.y) : 0.0;
+            sv[u] = (gv[u] != 0.0) ? scratch[cur.pre[u].x] : 0.0;
           }
-          for (int64_t k = cur.s0 + 128 + lane; k < cur.s1; k += 32) add_pair(p.pairs[k]);
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+            if (gv[u] != 0.0) scratch[cur.pre[u].x] = filt(sv[u] + gv[u]);
+          for (int64_t k = cur.s0 + 128 + lane; k < cur.s1; k += 32) {
+            const uint2 pr = p.pairs[k];
+            const double g = filt(filt((double)__uint_as_float(pr.y)) * cur.y);
+            if (g != 0.0) scratch[pr.x] = filt(scratch[pr.x] + g);
+          }
         }
         __syncwarp();
         cur = nxt;
@@ -182,48 +194,33 @@ __global__ void __launch_bounds__(128) k_async_worker(const AsyncParams p) {
       AsyncBatchRow cur = async_fetch_batch_row(p, rows, 0, B, lane);
       for (int b = 0; b < B; ++b) {
         const AsyncBatchRow nxt = async_fetch_batch_row(p, rows, b + 1, B, lane);
-        auto apply_pair = [&](const uint2 pr) {
-          // a padding pair repeats the row's last column with val == 0: only the real pair may claim the key
-          if (filt((double)__uint_as_float(pr.y)) == 0.0) return;
-          const double v = scratch[pr.x];
-          if (v != 0.0) {
-            scratch[pr.x] = 0.0;                        // claim the key: later duplicates of the column see 0
-            double m = filt(v / (double)B);             // Vec.mean = sum / size (math/Vec.scala:139)
-            if (m != 0.0 && add_c) m = filt(m + c);     // regularize on the surviving keys
-            const double delta = filt(m * p.lr);        // learningRate * (...)
-            if (delta != 0.0) {
-              for (int q = 0; q < p.n_replicas; ++q) red_add_f64_sys(&p.replica[q][pr.x], -delta);
-              sd += delta * p.d[pr.x];
-            }
-          }
+        // the key's summed value v, its dimSparsity factor and the replica's snapshot wv of it -> delta applied to every
+        // replica; the first row of the batch that holds the key claims it (the next rows see 0)
+        auto apply_key = [&](const int j, const double v, const double dj, const double wv) {
+          scratch[j] = 0.0;                           // claim the key
+          double m = filt(v / (double)B);             // Vec.mean = sum / size (math/Vec.scala:139)
+          if (m != 0.0 && add_c) m = filt(m + c);     // regularize on the surviving keys
+          const double delta = filt(m * p.lr);        // learningRate * (...)
+          if (delta != 0.0) async_apply_key(p, j, wv, delta, dj, sd);
         };
-        if (p.rows_unique) {
-          double v4[4], d4[4];
-          bool live[4];
+        double v4[4], d4[4], w4[4];
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {   // the lane's four entries and their dimSparsity factors: requested together
-            live[u] = (cur.s0 + lane + 32 * u < cur.s1) && filt((double)__uint_as_float(cur.pre[u].y)) != 0.0;
-            v4[u] = live[u] ? scratch[cur.pre[u].x] : 0.0;
-            d4[u] = live[u] ? __ldg(&p.d[cur.pre[u].x]) : 0.0;
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (v4[u] != 0.0) {
-              scratch[cur.pre[u].x] = 0.0;                  // claim the key (the next rows of the batch see 0)
-              double m = filt(v4[u] / (double)B);
-              if (m != 0.0 && add_c) m = filt(m + c);
-              const double delta = filt(m * p.lr);
-              if (delta != 0.0) {
-                for (int q = 0; q < p.n_replicas; ++q) red_add_f64_sys(&p.replica[q][cur.pre[u].x], -delta);
-                sd += delta * d4[u];
-              }
-            }
-        } else {
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (cur.s0 + lane + 32 * u < cur.s1) apply_pair(cur.pre[u]);
+        for (int u = 0; u < 4; ++u) {   // the lane's four entries, their dimSparsity factors and weights: requested together
+          // a padding pair repeats the row's last column with val == 0: only the real pair may claim the key
+          const bool live = (cur.s0 + lane + 32 * u < cur.s1) && filt((double)__uint_as_float(cur.pre[u].y)) != 0.0;
+          v4[u] = live ? scratch[cur.pre[u].x] : 0.0;
+          d4[u] = live ? __ldg(&p.d[cur.pre[u].x]) : 0.0;
+          w4[u] = live ? __ldcg(&w[cur.pre[u].x]) : 0.0;
         }
-        for (int64_t k = cur.s0 + 128 + lane; k < cur.s1; k += 32) apply_pair(p.pairs[k]);
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (v4[u] != 0.0) apply_key(cur.pre[u].x, v4[u], d4[u], w4[u]);
+        for (int64_t k = cur.s0 + 128 + lane; k < cur.s1; k += 32) {
+          const uint2 pr = p.pairs[k];
+          if (filt((double)__uint_as_float(pr.y)) == 0.0) continue;
+          const double v = scratch[pr.x];
+          if (v != 0.0) apply_key(pr.x, v, p.d[pr.x], __ldcg(&w[pr.x]));
+        }
         __syncwarp();
         cur = nxt;
       }
@@ -332,20 +329,21 @@ __global__ void __launch_bounds__(128) k_async_worker_b1(const AsyncParams p) {
     // ---- delta = lr * regularize(y * x / 1, w); apply to every replica (core/Slave.scala:92-105) ----
     double sd = 0.0;
     if (!(y * dot < 0.0)) {
-      auto push = [&](uint2 pr) {
+      // wv: the snapshot of the entry the dot product used (reloaded for the pairs past the first 128)
+      auto push = [&](uint2 pr, double wv) {
         const double xv = filt((double)__uint_as_float(pr.y));
         if (xv == 0.0) return;                          // padding pair (or an explicit zero): no key
         double m = filt(filt(xv * y) / 1.0);            // Vec.sum of one vector, Vec.mean = sum / size
         if (m != 0.0 && add_c) m = filt(m + c);
         const double delta = filt(m * p.lr);
-        if (delta != 0.0) {
-          for (int q = 0; q < p.n_replicas; ++q) red_add_f64_sys(&p.replica[q][pr.x], -delta);
-          sd += delta * __ldg(&p.d[pr.x]);
-        }
+        if (delta != 0.0) async_apply_key(p, pr.x, wv, delta, __ldg(&p.d[pr.x]), sd);
       };
 #pragma unroll
-      for (int u = 0; u < kAsyncPre; ++u) push(cur.pre[u]);
-      for (int64_t k = cur.s0 + lane + 32 * kAsyncPre; k < cur.s1; k += 32) push(__ldg(&p.pairs[k]));
+      for (int u = 0; u < kAsyncPre; ++u) push(cur.pre[u], wv[u]);
+      for (int64_t k = cur.s0 + lane + 32 * kAsyncPre; k < cur.s1; k += 32) {
+        const uint2 pr = __ldg(&p.pairs[k]);
+        push(pr, __ldcg(&w[pr.x]));
+      }
     }
     sd = warp_sum(sd);
     if (lane == 0) {
@@ -371,8 +369,13 @@ __global__ void __launch_bounds__(256) k_async_apply_delta(double *__restrict__ 
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x) {
     const double v = filt(val[k]);
     if (v != 0.0) {
-      atomicAdd_system(&w[idx[k]], -v);
+      // w - v, filtered: a tiny nonzero result is taken out as well, so the entry lands on exactly 0
+      const double nw = atomicAdd_system(&w[idx[k]], -v) - v;
       sd += v * d[idx[k]];
+      if (nw != 0.0 && fabs(nw) <= kEps) {
+        atomicAdd_system(&w[idx[k]], -nw);
+        sd += nw * d[idx[k]];
+      }
     }
   }
   sd = block_sum<256>(sd, red);

@@ -153,7 +153,8 @@ int dsgd_synth_fill(const dsgd_synth_params *p, const int64_t *row_ptr, int32_t 
  * go through .toMap, the LAST line of a rowId decides (quirk Q10).
  * Keys in the file are the reference's 1-based feature ids; they are stored 0-based (key - 1).
  *
- * Two-call protocol: dsgd_rcv1_count sizes the arrays, dsgd_rcv1_parse fills them. */
+ * Two-call protocol: dsgd_rcv1_count sizes the arrays (nnz counts every pair, an upper bound), dsgd_rcv1_parse fills them;
+ * its row_ptr[n_rows] is the number of distinct keys stored. */
 int dsgd_rcv1_count(const char *vectors_path, int64_t *n_rows, int64_t *nnz) {
   FILE *f = fopen(vectors_path, "r");
   if (!f) return -1;
@@ -195,10 +196,18 @@ int dsgd_rcv1_parse(const char *vectors_path, int32_t dim, int64_t n_rows, int64
       if (end == s) { free(line); fclose(f); return -3; }
       s = end;
       if (key < 1 || key > dim) { free(line); fclose(f); return -4; }  /* Sparse.apply allows key == size (Q11) */
-      if (k >= nnz) { free(line); fclose(f); return -2; }
-      col[k] = (int32_t)(key - 1); val[k] = (float)v; ++k;
+      /* the reference builds a Map per row (.toMap, Dataset.scala:26-32): a repeated key keeps its last value.  Keys come
+       * sorted in RCV1 files, so a key above the row's last one is new without a search */
+      int64_t at = k;
+      if (k > row_ptr[r] && (int32_t)(key - 1) <= col[k - 1])
+        for (int64_t q = row_ptr[r]; q < k; ++q)
+          if (col[q] == (int32_t)(key - 1)) { at = q; break; }
+      if (at == k) {
+        if (k >= nnz) { free(line); fclose(f); return -2; }
+        col[k] = (int32_t)(key - 1); ++k;
+      }
+      val[at] = (float)v;
     }
-    /* the reference builds a Map per row: duplicate keys keep the last value; keys come sorted in RCV1 files */
     row_ptr[++r] = k;
   }
   free(line);

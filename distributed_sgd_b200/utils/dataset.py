@@ -101,7 +101,9 @@ def _read_vectors(path: str, dim: int):
                            ids.ctypes.data_as(C.c_void_p))
     if rc != 0:
         raise ValueError(f"{path}: malformed RCV1 vectors file (code {rc})")
-    return row_ptr, col, val, ids
+    # the count is an upper bound: a key repeated within a line is stored once
+    nnz = int(row_ptr[-1])
+    return row_ptr, col[:nnz], val[:nnz], ids
 
 
 def rcv1(folder: str, full: bool = True, features_count: int = RCV1_FEATURES) -> Data:

@@ -25,6 +25,8 @@
  *  - Threading: calls on one ctx are serialised by the caller, except dsgd_update_grad,
  *    dsgd_get_weights, dsgd_async_updates and dsgd_stop_async, which are safe while the async loop runs
  *    (the reference serves them from its 8-thread pool concurrently with asyncTask, core/Slave.scala:24-30).
+ *    dsgd_update_grad may also be called from several threads at once: the calls take a lock of the ctx and
+ *    each delta is applied exactly once.
  */
 #ifndef DSGD_H
 #define DSGD_H
@@ -96,7 +98,9 @@ int dsgd_debug_timeline(dsgd_ctx *ctx, long long *out);
 int dsgd_stream_exact_rows(dsgd_ctx *ctx, int64_t *rows);
 
 /* ---- data: the `data: Array[(Vec, Int)]` constructor argument (core/Slave.scala:20; Main.scala:138,149).
- *      Rows are repacked on the device into 16-byte aligned (col, val) windows.  label in {-1, +1}. ------ */
+ *      Rows are repacked on the device into 16-byte aligned (col, val) windows.  label in {-1, +1}.  A row is
+ *      a Map in the reference: a column repeated within one row (in any order) is DSGD_ERR_INVALID; columns
+ *      need not be sorted. ------------------------------------------------------------------------------- */
 int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const int64_t *row_ptr, const int32_t *col,
                   const float *val, const int8_t *label);
 
@@ -212,7 +216,8 @@ int dsgd_async_running(dsgd_ctx *ctx, int *running);
 int dsgd_async_elapsed_ms(dsgd_ctx *ctx, float *elapsed_ms);
 /* SlaveImpl.updateGrad / AsyncMasterGrpcImpl.updateGrad (core/Slave.scala:177-185; core/MasterAsync.scala:
  * 164-177): weights -= delta for a sparse delta given as (idx, val) pairs, applied to this context's own replica (a host-side
- * sender -- e.g. a gRPC colleague -- uses it; GPU peers write the replica directly over NVLink). */
+ * sender -- e.g. a gRPC colleague -- uses it; GPU peers write the replica directly over NVLink).  Like the reference's new Sparse,
+ * an entry whose result is |w - v| <= 1e-20 becomes exactly 0.  Safe from several threads at once (see Threading). */
 int dsgd_update_grad(dsgd_ctx *ctx, const int32_t *idx, const double *val, int64_t nnz);
 /* GradState.updates (core/ml/GradState.scala:8; core/MasterAsync.scala:165): updates the master replica has
  * received if this ctx hosts or has imported it, else the updates this worker has made. */

@@ -81,6 +81,27 @@ def test_rcv1_text_round_trip(tmp_path):                      # utils/Dataset.sc
     assert back.label[0] == 1 and back.label[1] == -1
 
 
+def test_rcv1_repeated_key_keeps_the_last_value(tmp_path):   # utils/Dataset.scala:26-32: each row goes through .toMap
+    """A key repeated on one line is stored once with its last value (0.25 over 0.5, in either position); a last value of
+    1e-25 is stored as such and the 1e-20 filter of every consumer drops the key.  With repeats in the train file, the
+    rows of the test files that follow it must still line up (the parsed arrays are shorter than the pair count)."""
+    lines = {"lyrl2004_vectors_train.dat": ["10  3:0.5 7:1 3:0.25", "11  5:1 5:1e-25 9:2", "12  2:0.5 8:0.5 2:0.25 8:0.75"],
+             "lyrl2004_vectors_test_pt0.dat": ["13  1:1 4:0.5"], "lyrl2004_vectors_test_pt1.dat": ["14  6:0.125"],
+             "lyrl2004_vectors_test_pt2.dat": ["15  9:4 9:3"], "lyrl2004_vectors_test_pt3.dat": ["16  2:1"]}
+    for name, rows in lines.items():
+        (tmp_path / name).write_text("\n".join(rows) + "\n")
+    (tmp_path / "rcv1-v2.topics.qrels").write_text("".join(f"CCAT {i} 1\n" for i in range(10, 17)))
+    d = rcv1(str(tmp_path), full=True, features_count=10)
+    assert d.n_rows == 7 and d.row_ptr.tolist() == [0, 2, 4, 6, 8, 9, 10, 11]
+    assert len(d.col) == len(d.val) == 11
+    rows = [dict(zip(d.col[a:b].tolist(), d.val[a:b].tolist())) for a, b in zip(d.row_ptr[:-1], d.row_ptr[1:])]
+    assert rows[0] == {2: 0.25, 6: 1.0}                         # key 3 (column 2): the last value wins
+    assert rows[2] == {1: 0.25, 7: 0.75}
+    assert set(rows[1]) == {4, 8} and rows[1][8] == 2.0 and 0 < rows[1][4] <= 1e-20   # key 5 ends at 1e-25: filtered
+    assert rows[3] == {0: 1.0, 3: 0.5} and rows[4] == {5: 0.125} and rows[5] == {8: 3.0} and rows[6] == {1: 1.0}
+    assert (d.label == 1).all()
+
+
 class _RecCtx:
     """Stand-in device context that records what MasterSync would send to the GPU (no arithmetic)."""
 
