@@ -16,13 +16,31 @@ import numpy as np
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
 from ..ml.grad_state import GradState
 from ..ml.sparse_svm import SparseSVM
-from ..native import NativeCtx
+from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
 from ..utils.dataset import Data
 from .group import Group
 from .slave import Slave
 
 EarlyStopping = Callable[[Sequence[float]], bool]
 Split = Callable[[int, int], List[range]]
+
+_M64 = (1 << 64) - 1
+
+
+def sampled_key(seed: int, t: int) -> int:
+    """Key of the t-th device-drawn sample of a Master seeded with `seed` (Master.local_sampled_*).  splitmix64's finaliser
+    over seed * phi + (t + 1) * c (mod 2^64, c odd): for one seed it maps different t to different keys, and every rank
+    computes the same key from the same (seed, t)."""
+    z = (int(seed) * 0x9E3779B97F4A7C15 + (int(t) + 1) * 0xD1B54A32D192ED03) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def sample_shard(k: int, world: int, rank: int):
+    """Positions [lo, hi) of a k-row sample that rank `rank` of `world` evaluates: the shards are disjoint and cover
+    [0, k), and their sizes differ by at most one."""
+    return (k * rank) // world, (k * (rank + 1)) // world
 
 
 class EpochDraw(list):
@@ -90,6 +108,7 @@ class Master:
         self.seed = int(seed)
         self.rng = np.random.default_rng(seed)
         self._epochs_drawn = 0
+        self._sampled_draws = 0   # t of sampled_key: device-drawn evaluation samples so far (apart from the epoch draws)
         # jvm_exact: draw the batches with java.util.Random(seed) + Scala 2.12's Random.shuffle, the stream a reference
         # run consumes (SURVEY.md 8f N4); default: numpy's generator (statistically the same draws, much faster)
         self.jvm = None
@@ -138,6 +157,52 @@ class Master:
     def local_loss_accuracy(self, weights=None, test_data: bool = False):
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         return self._eval_rows(weights, b, e)
+
+    def _eval_sample(self, weights, samples_count: int, test_data: bool):
+        """(loss, accuracy) on a fresh sample of min(samples_count, n) of the working rows, or None when that is empty.
+        Every call draws anew, as every reference call reshuffles.  Default: the sample is drawn on the device with
+        sampled_key(seed, t), t counting this Master's draws (the epoch draws of `fit` are separate).  jvm_exact: the ids are
+        `Random.shuffle(indices) take k` from the java.util.Random stream `fit` also draws from.  Rank r of W evaluates
+        positions sample_shard(k, W, r); the integer counters are summed over ranks."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        n = e - b
+        k = min(int(samples_count), n)
+        ids = None
+        if self.jvm is not None:
+            # the reference shuffles every index before `take`: the stream moves by one shuffle whatever k is
+            ids = self.jvm.shuffle(np.arange(n, dtype=np.int32))[:max(k, 0)] + np.int32(b)
+        if k <= 0:
+            return None
+        lo, hi = sample_shard(k, self.group.world, self.group.rank)
+        if ids is None:
+            key = sampled_key(self.seed, self._sampled_draws)
+            self._sampled_draws += 1
+        if hi <= lo:
+            h, c, n2 = 0, 0, 0.0
+        elif ids is None:
+            h, c, n2 = self.ctx.eval_sampled_counts(b, e, key, lo, hi, weights)
+        else:
+            h, c, n2 = self.ctx.eval_samples_counts(ids[lo:hi], weights)
+        hs, cs = self.group.all_reduce_sum([h, c])
+        n2 = self.group.all_reduce_max(n2)  # identical on every rank that evaluated; 0 on idle ranks
+        return self.model.lam * n2 + hs / k, cs / k
+
+    def local_sampled_loss(self, weights, samples_count: int, test_data: bool = False) -> float:
+        """Master.localSampledLoss (core/Master.scala:109-112).  An empty sample raises DsgdEmpty, as the reference's
+        `reduce` on an empty list throws."""
+        return self.local_sampled_loss_accuracy(weights, samples_count, test_data)[0]
+
+    def local_sampled_accuracy(self, weights, samples_count: int, test_data: bool = False) -> float:
+        """Master.localSampledAccuracy (core/Master.scala:114-118).  An empty sample gives nan (the reference's 0.0 / 0)."""
+        r = self._eval_sample(weights, samples_count, test_data)
+        return float("nan") if r is None else r[1]
+
+    def local_sampled_loss_accuracy(self, weights, samples_count: int, test_data: bool = False):
+        """(loss, accuracy) on ONE sample, drawn once for both numbers.  An empty sample raises DsgdEmpty."""
+        r = self._eval_sample(weights, samples_count, test_data)
+        if r is None:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
+        return r
 
     def predict(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> dict:
         """Master.predict (core/Master.scala:61-75): idx -> prediction over the training rows; each worker

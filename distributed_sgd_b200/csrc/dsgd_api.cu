@@ -64,6 +64,9 @@ struct dsgd_ctx {
   int64_t losses_cap = 0;
   double *preds = nullptr;
   int64_t preds_cap = 0;
+  // row ids of a sampled evaluation (drawn on the device or copied from the host): never the staged stream above
+  int32_t *eval_ids = nullptr;
+  int64_t eval_ids_cap = 0;
 
   ncclComm_t comm = nullptr;
 
@@ -287,7 +290,7 @@ extern "C" int dsgd_destroy(dsgd_ctx *ctx) {
   void *ptrs[] = {ctx->rp16, ctx->pairs, ctx->label, ctx->yabs, ctx->w, ctx->g, ctx->d, ctx->w_req, ctx->w32, ctx->w32_req, ctx->n_exact, ctx->scal,
                   ctx->cnt, ctx->partial, ctx->out2, ctx->gsum, ctx->p_wbuf[0], ctx->p_wbuf[1], ctx->p_gbuf[0],
                   ctx->p_gbuf[1], ctx->p_gbuf[2], ctx->p_rec[0], ctx->p_rec[1], ctx->p_rec[2], ctx->p_acc, ctx->p_hinge, ctx->p_bar, ctx->x_stats, ctx->samples,
-                  ctx->losses, ctx->preds};
+                  ctx->losses, ctx->preds, ctx->eval_ids};
   for (void *p : ptrs) if (p) cudaFree(p);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -590,6 +593,7 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
     CU(cudaFuncSetAttribute(k_stream_rows<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU(cudaFuncSetAttribute(k_stream_rows<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU(cudaFuncSetAttribute(k_stream_rows<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     ctx->stream_ready = true;
   }
   NEED(kContig == (samples_dev == nullptr), DSGD_ERR_INVALID, "stream_launch: sample list / row range mismatch");
@@ -678,21 +682,20 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
   return DSGD_OK;
 }
 
-static int eval_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double out[5]) {
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval: no rows loaded");
-  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
-       "dsgd_eval: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
-  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "dsgd_eval: empty range (reduce on an empty collection throws in the reference)");
-  CU(cudaSetDevice(ctx->device));
-  const int64_t n = row_end - row_begin;
-  const double *wd, *cd, *nd;
-  const float *w32d;
+// One evaluation pass over rows [row_begin, row_begin + n) (ids == nullptr) or over the n row ids at the device address
+// `ids`, then the shared tail: out = {loss, accuracy, hinge sum, correct count, ||w||^2}, and the counters cleared for the
+// next pass (k_loss_scalar).
+static int eval_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t row_begin, int64_t n, double out[5]) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  const float *w32d = nullptr;
   int rc;
   if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
   if (stream_eligible(ctx, n)) {
-    if ((rc = stream_launch<false, false, true>(ctx, nullptr, row_begin, n, wd, w32d, nullptr, nullptr))) return rc;
+    rc = ids ? stream_launch<false, false, false>(ctx, ids, 0, n, wd, w32d, nullptr, nullptr)
+             : stream_launch<false, false, true>(ctx, nullptr, row_begin, n, wd, w32d, nullptr, nullptr);
+    if (rc) return rc;
   } else {
-    k_rows<false, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, nullptr, row_begin, n,
+    k_rows<false, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n,
                                                                      wd, nullptr, nullptr, ctx->cnt);
     LAUNCHED();
   }
@@ -702,6 +705,21 @@ static int eval_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t 
   CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return DSGD_OK;
+}
+
+static int eval_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double out[5]) {
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval: no rows loaded");
+  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
+       "dsgd_eval: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
+  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "dsgd_eval: empty range (reduce on an empty collection throws in the reference)");
+  CU(cudaSetDevice(ctx->device));
+  return eval_pass(ctx, w, nullptr, row_begin, row_end - row_begin, out);
+}
+
+static void put_counts(const double out[5], int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+  if (hinge_sum) *hinge_sum = (int64_t)out[2];
+  if (correct) *correct = (int64_t)out[3];
+  if (norm_squared) *norm_squared = out[4];
 }
 
 extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
@@ -721,14 +739,60 @@ extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begi
   double out[5];
   int rc = eval_impl(ctx, w, row_begin, row_end, out);
   if (rc) return rc;
-  if (hinge_sum) *hinge_sum = (int64_t)out[2];
-  if (correct) *correct = (int64_t)out[3];
-  if (norm_squared) *norm_squared = out[4];
+  put_counts(out, hinge_sum, correct, norm_squared);
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                        int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
+                                        double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_sampled_counts: no rows loaded");
+  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
+       "dsgd_eval_sampled_counts: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end,
+       (long long)ctx->n_rows);
+  const int64_t n = row_end - row_begin;
+  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_sampled_counts: empty row range");
+  NEED(n <= (int64_t)UINT32_MAX, DSGD_ERR_INVALID, "dsgd_eval_sampled_counts: %lld rows; the draw permutes 32-bit positions",
+       (long long)n);
+  NEED(pos_begin >= 0 && pos_end <= n, DSGD_ERR_INVALID, "dsgd_eval_sampled_counts: positions [%lld,%lld) outside [0,%lld)",
+       (long long)pos_begin, (long long)pos_end, (long long)n);
+  NEED(pos_end > pos_begin, DSGD_ERR_EMPTY, "dsgd_eval_sampled_counts: no positions (reduce on an empty collection throws)");
+  CU(cudaSetDevice(ctx->device));
+  const int64_t k = pos_end - pos_begin;
+  int rc = ensure_i32(ctx, &ctx->eval_ids, &ctx->eval_ids_cap, k);
+  if (rc) return rc;
+  k_draw_rows<<<cdiv(k, 256), 256, 0, ctx->stream>>>(ctx->eval_ids, k, (uint32_t)pos_begin,
+                                                      dsgd_feistel_half_bits((uint64_t)n), key, (uint32_t)n, row_begin);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  double out[5];
+  if ((rc = eval_pass(ctx, w, ctx->eval_ids, 0, k, out))) return rc;
+  put_counts(out, hinge_sum, correct, norm_squared);
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_samples_counts: no rows loaded");
+  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_eval_samples_counts: bad arguments");
+  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_samples_counts: empty sample (reduce on an empty collection throws)");
+  for (int64_t i = 0; i < n; ++i)
+    NEED(samples[i] >= 0 && samples[i] < ctx->n_rows, DSGD_ERR_RANGE, "sample index %d at position %lld outside [0,%lld)",
+         samples[i], (long long)i, (long long)ctx->n_rows);
+  CU(cudaSetDevice(ctx->device));
+  int rc = ensure_i32(ctx, &ctx->eval_ids, &ctx->eval_ids_cap, n);
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(ctx->eval_ids, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  double out[5];
+  if ((rc = eval_pass(ctx, w, ctx->eval_ids, 0, n, out))) return rc;
+  put_counts(out, hinge_sum, correct, norm_squared);
   return DSGD_OK;
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all
-// streaming passes of this ctx so far).
+// streaming passes of this ctx so far: forward, gradient, and the full and sampled evaluations).
 extern "C" int dsgd_stream_exact_rows(dsgd_ctx *ctx, int64_t *rows) {
   if (!ctx || !rows) return DSGD_ERR_INVALID;
   unsigned long long host = 0;

@@ -2,7 +2,8 @@
  * in random order are pi(0), ..., pi(B - 1) of a keyed pseudo-random PERMUTATION pi of [0, n) -- a 4-round Feistel network on
  * the next even power of two, walked until the image falls inside [0, n) (a bijection restricted to its cycles through
  * [0, n) stays a bijection).  Distinct by construction, O(1) per position, every lane of a warp draws its own positions.
- * Plain C, compiled by nvcc into the async worker (dsgd_async.cuh) and by gcc into libdsgd_host.so (dsgd_feistel_pos), where
+ * Plain C, compiled by nvcc into the async worker (dsgd_async.cuh) and the sampled evaluation's draw (k_draw_rows,
+ * dsgd_kernels.cuh), and by gcc into libdsgd_host.so (dsgd_feistel_pos), where
  * tests/test_host_logic.py checks the permutation property on the very same source. */
 #ifndef DSGD_FEISTEL_H
 #define DSGD_FEISTEL_H

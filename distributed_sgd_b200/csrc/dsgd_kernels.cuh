@@ -13,6 +13,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dsgd_feistel.h"
+
 namespace dsgd {
 
 constexpr double kEps = 1e-20;  // math/Sparse.scala:104
@@ -349,6 +351,16 @@ __global__ void __launch_bounds__(256) k_repack(const int64_t *__restrict__ row_
       yabs[r] = label[r] < 0 ? -a : a;
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_draw_rows: positions [pos_begin, pos_begin + n_pos) of a keyed permutation of [0, n) as row ids (Master.scala:
+// 109-118: `Random.shuffle(workingData.indices) take samplesCount`, dsgd_feistel.h).  One thread per position.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_draw_rows(int32_t *__restrict__ ids, int64_t n_pos, uint32_t pos_begin,
+                                                   int half_bits, uint64_t key, uint32_t n, int64_t row_begin) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_pos) ids[i] = (int32_t)(row_begin + (int64_t)dsgd_feistel(pos_begin + (uint32_t)i, half_bits, key, n));
 }
 
 __global__ void __launch_bounds__(256) k_to_f32(const double *__restrict__ src, float *__restrict__ dst, int n) {

@@ -25,6 +25,12 @@ object DsgdNative {
   @native def eval(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, lossAcc: Array[Double]): Int
   @native def evalCounts(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, hingeCorrect: Array[Long],
                          normSquared: Array[Double]): Int
+  // Master.localSampledLoss / localSampledAccuracy: positions [posBegin, posEnd) of a sample of rows [rowBegin, rowEnd)
+  // drawn on the device with `key`, or a list of row ids the JVM drew itself (its own Random); same counters as evalCounts
+  @native def evalSampledCounts(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                posEnd: Long, hingeCorrect: Array[Long], normSquared: Array[Double]): Int
+  @native def evalSamplesCounts(ctx: Long, w: Array[Double], samples: Array[Int], hingeCorrect: Array[Long],
+                                normSquared: Array[Double]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

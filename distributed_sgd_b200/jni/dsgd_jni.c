@@ -137,6 +137,31 @@ FN(evalCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegi
   free(bw.p);
   return rc;
 }
+FN(evalSampledCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                      jlong posBegin, jlong posEnd, jlongArray hingeCorrect, jdoubleArray normSquared) {
+  buf_t bw = in_Double(env, w), bc = out_Long(env, hingeCorrect), bn = out_Double(env, normSquared);
+  int rc = DSGD_ERR_NOMEM;               /* core/Master.scala:109-118, sample drawn on the device: positions [posBegin, posEnd) */
+  if (!(bw.bad | bc.bad | bn.bad))
+    rc = (bc.n < 2 || bn.n < 1) ? DSGD_ERR_INVALID
+                                : dsgd_eval_sampled_counts(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                           (int64_t *)bc.p, (int64_t *)bc.p + 1, bn.p);
+  back_Long(env, hingeCorrect, bc, rc);
+  back_Double(env, normSquared, bn, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray hingeCorrect,
+                      jdoubleArray normSquared) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bc = out_Long(env, hingeCorrect), bn = out_Double(env, normSquared);
+  int rc = DSGD_ERR_NOMEM;               /* the same counters over row ids the JVM drew with its own Random */
+  if (!(bw.bad | bs.bad | bc.bad | bn.bad))
+    rc = (bc.n < 2 || bn.n < 1) ? DSGD_ERR_INVALID
+                                : dsgd_eval_samples_counts(CTX(h), bw.p, bs.p, bs.n, (int64_t *)bc.p, (int64_t *)bc.p + 1, bn.p);
+  back_Long(env, hingeCorrect, bc, rc);
+  back_Double(env, normSquared, bn, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
 
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {

@@ -95,6 +95,8 @@ ABI = {
     "dsgd_gradient": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64)],
     "dsgd_eval": [_vp, _vp, _i64, _i64, C.POINTER(_f64), C.POINTER(_f64)],
     "dsgd_eval_counts": [_vp, _vp, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_eval_sampled_counts": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_eval_samples_counts": [_vp, _vp, _vp, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -311,6 +313,25 @@ class NativeCtx:
         h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
         w = self._w(w)
         self._ck(self._l.dsgd_eval_counts(self._h, _ptr(w), row_begin, row_end, C.byref(h), C.byref(c), C.byref(n2)))
+        return h.value, c.value, n2.value
+
+    def eval_sampled_counts(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                            w=None) -> Tuple[int, int, float]:
+        """(hinge sum, correct count, ||w||^2) over positions [pos_begin, pos_end) of the sample drawn on the device from rows
+        [row_begin, row_end) with `key` (dsgd_eval_sampled_counts)."""
+        h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_sampled_counts(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
+                                                  pos_begin, pos_end, C.byref(h), C.byref(c), C.byref(n2)))
+        return h.value, c.value, n2.value
+
+    def eval_samples_counts(self, samples, w=None) -> Tuple[int, int, float]:
+        """The same counters over a list of row ids; repeats count every time (dsgd_eval_samples_counts)."""
+        samples = _arr(samples, np.int32)
+        h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_samples_counts(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
+                                                  C.byref(n2)))
         return h.value, c.value, n2.value
 
     # -- sync --

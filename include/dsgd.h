@@ -93,8 +93,9 @@ int dsgd_set_grid_limit(dsgd_ctx *ctx, int32_t n_ctas);
  * pairs of the CTA's rows, spare} per CTA; this copies the last launch's DSGD_TIMELINE_WORDS int64 words out. */
 #define DSGD_TIMELINE_WORDS (256 * 16 + 4 * 160 * 4)
 int dsgd_debug_timeline(dsgd_ctx *ctx, long long *out);
-/* Diagnostic: rows the streaming pass (forward / gradient / eval of 2048 rows or more) recomputed in fp64 because the
- * sign of their fp32 dot product was inside the rounding band; cumulative since dsgd_create. */
+/* Diagnostic: rows the streaming pass (forward / gradient / eval / sampled eval of 2048 rows or more) recomputed in fp64
+ * because the sign of their fp32 dot product was inside the rounding band; cumulative since dsgd_create, every streaming
+ * pass counted. */
 int dsgd_stream_exact_rows(dsgd_ctx *ctx, int64_t *rows);
 
 /* ---- data: the `data: Array[(Vec, Int)]` constructor argument (core/Slave.scala:20; Main.scala:138,149).
@@ -134,6 +135,23 @@ int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end
  * ||w||^2, so that a host can combine row shards evaluated on different GPUs without rounding. */
 int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *hinge_sum,
                      int64_t *correct, double *norm_squared);
+
+/* ---- Master.localSampledLoss / localSampledAccuracy (core/Master.scala:109-118) on a sample drawn on the device:
+ *      position i of the draw is row row_begin + dsgd_feistel(i, half_bits(n), key, n), n = row_end - row_begin, a keyed
+ *      permutation of the range (`Random.shuffle(indices) take k` without a shuffle, dsgd_feistel.h).  Evaluates positions
+ *      [pos_begin, pos_end), so ranks that draw with the same key can split one sample between them; returns the same
+ *      exact counters as dsgd_eval_counts.  w == NULL: resident weights.  The drawn ids go to a buffer of their own: a
+ *      sample stream staged with dsgd_stage_samples is left intact.  Errors: no rows loaded -> DSGD_ERR_STATE; range
+ *      outside the loaded rows -> DSGD_ERR_RANGE; n == 0 or pos_end <= pos_begin -> DSGD_ERR_EMPTY; pos_begin < 0,
+ *      pos_end > n, or n >= 2^32 -> DSGD_ERR_INVALID. */
+int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                             int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
+                             double *norm_squared);
+/* The same counters over a caller's list of n row ids; repeats are allowed and every occurrence counts.  For a host that
+ * draws the sample itself (the JVM-exact draw, or a JVM master using its own Random).  n == 0 -> DSGD_ERR_EMPTY; an id
+ * outside the loaded rows -> DSGD_ERR_RANGE before anything is launched.  The staged sample stream is left intact. */
+int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *hinge_sum,
+                             int64_t *correct, double *norm_squared);
 
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
