@@ -1143,6 +1143,17 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
            (long long)n_per_step, (long long)tot);
     }
   }
+  const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
+  const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
+  const bool fused = ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
+                     persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step));
+  // Ranks wired with the peer exchange only have no communicator for the step-by-step path below: refuse before anything
+  // is launched instead of reaching the allreduce without one.
+  NEED(ctx->world == 1 || ctx->comm || n_steps == 0 || fused, DSGD_ERR_STATE,
+       "dsgd_sync_steps: world > 1 without dsgd_comm_init, and the fused peer-exchange kernel cannot take this step "
+       "(it needs one worker per rank, batch <= %d x %d CTAs and dim + 1 <= %d x CTAs; batch %lld, dim %d)",
+       kMaxRowsPerCta, ctx->grid_limit > 0 ? std::min(ctx->grid_limit, ctx->sm_count) : ctx->sm_count,
+       (kPCons + kPUpd) * 32, (long long)n_per_step, ctx->dim);
   CU(cudaSetDevice(ctx->device));
   if (want_losses) {
     int rc = ensure_f64(ctx, &ctx->losses, &ctx->losses_cap, n_steps);
@@ -1150,14 +1161,11 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
   }
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
-  const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
-  const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
   if (single && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel
     return persist_run(ctx, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses : nullptr);
   }
-  if (ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
-      persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step))) {
+  if (fused) {
     // one worker per GPU, every peer's exchange block mapped: aggregate inside the persistent kernel over NVLink
     return persist_run_multi(ctx, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses : nullptr);
   }

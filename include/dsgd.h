@@ -162,7 +162,9 @@ int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYTES]);
 /* Peer exchange for the FUSED multi-GPU step: each rank exports its receive area, the host transports the handles, every rank imports every other rank's.  Once all world-1 peers
  * are attached, sync steps with one worker per GPU run as one persistent kernel per call that sums the workers'
  * replies directly out of peer memory over NVLink (no NCCL call, no launch per step; only the non-zero entries of a
- * reply travel); otherwise the NCCL allreduce path is used.  Up to 8 ranks (one NVSwitch box).  dsgd_xchg_attach is
+ * reply travel); otherwise the NCCL allreduce path is used, which needs dsgd_comm_init: without a communicator, a step
+ * the fused kernel cannot take (batch above 32 x CTAs per rank, dim + 1 above 448 x CTAs, several workers on a rank)
+ * fails with DSGD_ERR_STATE before anything is launched.  Up to 8 ranks (one NVSwitch box).  dsgd_xchg_attach is
  * the same-process form. */
 int dsgd_xchg_export(dsgd_ctx *ctx, uint8_t handle[DSGD_IPC_HANDLE_BYTES]);
 int dsgd_xchg_import(dsgd_ctx *ctx, int peer_rank, const uint8_t handle[DSGD_IPC_HANDLE_BYTES]);
