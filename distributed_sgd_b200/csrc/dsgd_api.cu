@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "dsgd_kernels.cuh"
@@ -22,6 +23,72 @@
 
 using namespace dsgd;
 
+struct dsgd_ctx;
+
+namespace {  // internal linkage: none of these types or their instantiations is exported from the library
+
+// Device memory owned by a ctx (or, for a temporary, by one call). The destructor frees it; it runs with the ctx's device
+// current (dsgd_destroy and the failure path of dsgd_create set it, and a call sets it before it allocates).
+template <class T>
+struct dev_buf {
+  T *p = nullptr;
+  int64_t cap = 0;  // elements
+  dev_buf() = default;
+  dev_buf(const dev_buf &) = delete;
+  dev_buf &operator=(const dev_buf &) = delete;
+  ~dev_buf() { release(); }
+  operator T *() const { return p; }
+  cudaError_t release() {
+    if (!p) return cudaSuccess;
+    const cudaError_t e = cudaFree(p);
+    if (e == cudaSuccess) { p = nullptr; cap = 0; }
+    return e;
+  }
+  // replaces the allocation with one of n elements (contents undefined)
+  cudaError_t alloc(int64_t n) {
+    cudaError_t e = release();
+    if (e != cudaSuccess) return e;
+    T *q = nullptr;
+    if ((e = cudaMalloc(&q, sizeof(T) * (size_t)n)) == cudaSuccess) { p = q; cap = n; }
+    return e;
+  }
+  // at least n elements: a smaller buffer is replaced by one of max(n, min_cap), zero-filled on ctx->stream if `zero`
+  int grow(dsgd_ctx *ctx, int64_t n, int64_t min_cap, bool zero = false);
+};
+
+// A stream or event owned by a ctx, destroyed with it.
+template <class H, cudaError_t (*Destroy)(H)>
+struct cuda_handle {
+  H h = nullptr;
+  cuda_handle() = default;
+  cuda_handle(cuda_handle &&o) noexcept : h(o.h) { o.h = nullptr; }
+  cuda_handle(const cuda_handle &) = delete;
+  cuda_handle &operator=(const cuda_handle &) = delete;
+  ~cuda_handle() { if (h) Destroy(h); }
+  operator H() const { return h; }
+};
+using owned_stream = cuda_handle<cudaStream_t, cudaStreamDestroy>;
+using owned_event = cuda_handle<cudaEvent_t, cudaEventDestroy>;
+
+// A peer's buffer as this ctx addresses it: mapped from another process with cudaIpcOpenMemHandle (the mapping is closed
+// when it is replaced or destroyed), or a pointer into another ctx of this process (not owned).
+struct peer_ptr {
+  double *p = nullptr;
+  bool via_ipc = false;
+  peer_ptr() = default;
+  peer_ptr(const peer_ptr &) = delete;
+  peer_ptr &operator=(const peer_ptr &) = delete;
+  ~peer_ptr() { set(nullptr, false); }
+  operator double *() const { return p; }
+  void set(double *q, bool ipc) {
+    if (p && via_ipc) cudaIpcCloseMemHandle(p);
+    p = q;
+    via_ipc = ipc;
+  }
+};
+
+}  // namespace
+
 struct dsgd_ctx {
   int device = 0;
   int32_t dim = 0;
@@ -31,89 +98,81 @@ struct dsgd_ctx {
   int sm_count = 0;
   std::string dev_name;
 
-  cudaStream_t own_stream = nullptr;
+  owned_stream own_stream;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  owned_event ev0, ev1;
   int64_t launches = 0;
 
   // rows
   int64_t n_rows = 0, nnz = 0, n_pairs = 0;
-  uint32_t *rp16 = nullptr;
-  uint2 *pairs = nullptr;
-  int8_t *label = nullptr;
-  float *yabs = nullptr;   // label * sum_j |x_j| per row (dsgd_kernels.cuh: k_repack)
+  dev_buf<uint32_t> rp16;
+  dev_buf<uint2> pairs;
+  dev_buf<int8_t> label;
+  dev_buf<float> yabs;   // label * sum_j |x_j| per row (dsgd_kernels.cuh: k_repack)
 
   // state (fp64, L2 resident) -- g has dim + 2 slots (hinge sum and batch size ride in the allreduce)
-  double *w = nullptr, *g = nullptr, *d = nullptr, *w_req = nullptr;
-  float *w32 = nullptr, *w32_req = nullptr;
-  unsigned long long *n_exact = nullptr;  // rows that took the exact fallback in streaming passes (diagnostic)
+  dev_buf<double> w, g, d, w_req;
+  dev_buf<float> w32, w32_req;
+  dev_buf<unsigned long long> n_exact;  // rows that took the exact fallback in streaming passes (diagnostic)
   bool stream_ready = false;
-  double *scal = nullptr;
-  unsigned long long *cnt = nullptr;
-  double *partial = nullptr;  // 2 doubles per k_update block
-  double *out2 = nullptr;     // loss, acc, hinge sum, correct count, ||w||^2
-  double *gsum = nullptr;     // master-side running sum of worker replies (dim + 2)
+  dev_buf<double> scal;
+  dev_buf<unsigned long long> cnt;
+  dev_buf<double> partial;  // 2 doubles per k_update block
+  dev_buf<double> out2;     // loss, acc, hinge sum, correct count, ||w||^2
+  dev_buf<double> gsum;     // master-side running sum of worker replies (dim + 2)
   std::vector<int32_t> worker_counts;  // logical workers on this ctx (empty: one worker, whole slice)
   int32_t n_local = 1, k_total = 0;    // k_total == 0: world
   bool have_d = false;
 
   // staged sample indices / per-step losses
-  int32_t *samples = nullptr;
-  int64_t samples_cap = 0, samples_n = 0;
-  double *losses = nullptr;
-  int64_t losses_cap = 0;
-  double *preds = nullptr;
-  int64_t preds_cap = 0;
+  dev_buf<int32_t> samples;
+  int64_t samples_n = 0;
+  dev_buf<double> losses;
+  dev_buf<double> preds;
   // row ids of a sampled evaluation (drawn on the device or copied from the host): never the staged stream above
-  int32_t *eval_ids = nullptr;
-  int64_t eval_ids_cap = 0;
+  dev_buf<int32_t> eval_ids;
 
   ncclComm_t comm = nullptr;
 
   // persistent sync kernel resources (allocated on first use)
-  double *p_wbuf[2] = {nullptr, nullptr};            // K GPUs
-  double *p_gbuf[3] = {nullptr, nullptr, nullptr};   // K GPUs
-  double2 *p_rec[3] = {nullptr, nullptr, nullptr};   // one GPU: rotating {W, g} records
-  unsigned long long *p_acc = nullptr;   // fixed-point accumulators of the per-CTA partials [3][kAccStride]
-  unsigned *p_hinge = nullptr;
-  int64_t p_hinge_cap = 0;
-  unsigned *p_bar = nullptr;   // [0]: grid barrier counter, [1]: abort flag
+  dev_buf<double> p_wbuf[2];   // K GPUs
+  dev_buf<double> p_gbuf[3];   // K GPUs
+  dev_buf<double2> p_rec[3];   // one GPU: rotating {W, g} records
+  dev_buf<unsigned long long> p_acc;   // fixed-point accumulators of the per-CTA partials [3][kAccStride]
+  dev_buf<unsigned> p_hinge;
+  dev_buf<unsigned> p_bar;   // [0]: grid barrier counter, [1]: abort flag
   bool p_ready = false;
-  long long *p_tl = nullptr;   // debug timeline (DSGD_PERSIST_TIMELINE)
+  dev_buf<long long> p_tl;   // debug timeline (DSGD_PERSIST_TIMELINE)
 
   // async (Hogwild) mode
-  cudaStream_t astream = nullptr;   // the worker loop
-  cudaStream_t stream2 = nullptr;   // service calls that must not queue behind anything
-  double *m_w = nullptr;            // master replica hosted by this ctx (dsgd_async_host_master)
-  double *outbox = nullptr;         // dsgd_async_outbox_enable: running sum of -delta of THIS worker (a replica-shaped block)
-  double *peer_w[kMaxReplicas] = {};  // [r] = replica of rank r, [world] = master replica; nullptr: not attached
-  bool peer_ipc[kMaxReplicas] = {};
-  int *a_stop = nullptr;
-  unsigned long long *a_cnt = nullptr;   // [0] claimed, [1] done
-  double *a_scratch = nullptr;
-  int64_t a_scratch_lanes = 0;
-  int32_t *a_rows = nullptr, *a_assigned = nullptr, *a_replay = nullptr;
-  int64_t a_rows_cap = 0, a_assigned_cap = 0, a_replay_cap = 0;
-  int32_t *u_idx = nullptr; double *u_val = nullptr; int64_t u_cap = 0;  // update_grad staging
+  owned_stream astream;   // the worker loop
+  owned_stream stream2;   // service calls that must not queue behind anything
+  dev_buf<double> m_w;      // master replica hosted by this ctx (dsgd_async_host_master)
+  dev_buf<double> outbox;   // dsgd_async_outbox_enable: running sum of -delta of THIS worker (a replica-shaped block)
+  peer_ptr peer_w[kMaxReplicas];  // [r] = replica of rank r, [world] = master replica; nullptr: not attached
+  dev_buf<int> a_stop;
+  dev_buf<unsigned long long> a_cnt;   // [0] claimed, [1] done
+  dev_buf<double> a_scratch;           // [lanes][dim]
+  dev_buf<int32_t> a_rows, a_assigned, a_replay;
+  dev_buf<int32_t> u_idx; dev_buf<double> u_val;  // update_grad staging
   std::mutex u_mu;                  // dsgd_update_grad: one call at a time stages, launches and waits
   bool a_running = false;
-  cudaEvent_t a_ev0 = nullptr, a_ev1 = nullptr;
+  owned_event a_ev0, a_ev1;
 
   // sync-mode receive area shared with peers over NVLink: value words [sender][parity][dim + 8] x 16 B, then bitmap
   // words [sender][parity][ceil((dim + 1) / 32)] x 8 B (dsgd_persistent.cuh)
-  double *xblk = nullptr;
-  double *peer_x[kMaxWorld] = {};
-  bool peer_x_ipc[kMaxWorld] = {};
+  dev_buf<double> xblk;
+  peer_ptr peer_x[kMaxWorld];
   int grid_limit = 0;   // dsgd_set_grid_limit: CTAs of the persistent sync kernel (0: one per SM)
   int64_t x_step = 0;   // global step counter of the fused multi-GPU kernel (identical on every rank)
   int64_t x_steps_run = 0;  // SGD steps run by the fused kernel so far (dsgd_xchg_stats)
-  unsigned long long *x_llw = nullptr;  // this rank's weights in LL form, two parities
-  unsigned long long *x_stats = nullptr;  // [0] value words, [1] bitmap words pushed to each peer so far; [2] SGD steps of those launches
+  dev_buf<unsigned long long> x_llw;  // this rank's weights in LL form, two parities
+  dev_buf<unsigned long long> x_stats;  // [0] value words, [1] bitmap words pushed to each peer so far; [2] SGD steps of those launches
 
   // sampled per-launch timing of the gradient kernel
   int32_t prof_every = 0;
   int64_t prof_seen = 0;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
+  std::vector<std::pair<owned_event, owned_event>> prof_events;
   size_t prof_used = 0;
 
   mutable std::string err;
@@ -184,20 +243,45 @@ static int fail(const dsgd_ctx *ctx, int code, const char *fmt, ...) {
   } while (0)
 #define LAUNCHED() (++ctx->launches)
 
+template <class T>
+int dev_buf<T>::grow(dsgd_ctx *ctx, int64_t n, int64_t min_cap, bool zero) {
+  if (cap >= n) return DSGD_OK;
+  CU(alloc(std::max(n, min_cap)));
+  if (zero) CU(cudaMemsetAsync(p, 0, sizeof(T) * (size_t)cap, ctx->stream));
+  return DSGD_OK;
+}
+
 // returns the event pair to bracket this gradient launch with, or nullptr
-static std::pair<cudaEvent_t, cudaEvent_t> *prof_slot(dsgd_ctx *ctx) {
+static std::pair<owned_event, owned_event> *prof_slot(dsgd_ctx *ctx) {
   if (ctx->prof_every <= 0) return nullptr;
   if ((ctx->prof_seen++ % ctx->prof_every) != 0) return nullptr;
   if (ctx->prof_used == ctx->prof_events.size()) {
     if (ctx->prof_events.size() >= 16384) return nullptr;
-    cudaEvent_t a, b;
-    if (cudaEventCreate(&a) != cudaSuccess || cudaEventCreate(&b) != cudaSuccess) return nullptr;
-    ctx->prof_events.emplace_back(a, b);
+    std::pair<owned_event, owned_event> pe;
+    if (cudaEventCreate(&pe.first.h) != cudaSuccess || cudaEventCreate(&pe.second.h) != cudaSuccess) return nullptr;
+    ctx->prof_events.push_back(std::move(pe));
   }
   return &ctx->prof_events[ctx->prof_used++];
 }
 
+// runs `launch` (one gradient kernel launch on ctx->stream) between the events of prof_slot when this launch is sampled
+template <class F>
+static void profiled(dsgd_ctx *ctx, F &&launch) {
+  auto *pe = prof_slot(ctx);
+  if (pe) cudaEventRecord(pe->first, ctx->stream);
+  launch();
+  if (pe) cudaEventRecord(pe->second, ctx->stream);
+}
+
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+
+// every id names a loaded row (the reference indexes its data array with it)
+static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *what) {
+  for (int64_t i = 0; i < n; ++i)
+    NEED(ids[i] >= 0 && ids[i] < ctx->n_rows, DSGD_ERR_RANGE, "%s %d at position %lld outside [0,%lld)", what, ids[i],
+         (long long)i, (long long)ctx->n_rows);
+  return DSGD_OK;
+}
 
 // ---- lifecycle ---------------------------------------------------------------------------------------
 
@@ -219,7 +303,7 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
   ctx->device = device; ctx->dim = dim; ctx->lambda = lambda; ctx->rank = rank; ctx->world = world; ctx->flags = flags;
   auto bail = [&](const char *what, cudaError_t err) {
     int rc = fail(nullptr, DSGD_ERR_CUDA, "dsgd_create: %s: %s", what, cudaGetErrorString(err));
-    delete ctx;
+    delete ctx;   // releases what was made so far
     return rc;
   };
   if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
@@ -230,34 +314,35 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
   if (prop.major != 9 || prop.minor != 0)   // sm_90a code loads on compute capability 9.0 only
     { int rc = fail(nullptr, DSGD_ERR_CUDA, "dsgd_create: device %d is sm_%d%d; this library is built for sm_90a only",
                     device, prop.major, prop.minor); delete ctx; return rc; }
-  if ((e = cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
+  if ((e = cudaStreamCreateWithFlags(&ctx->own_stream.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   if (flags & DSGD_FLAG_ASYNC) {   // the worker loop's stream and the service stream exist in async mode only: streams
                                    // beyond the device's hardware queues (8 by default) alias and serialise each other
-    if ((e = cudaStreamCreateWithFlags(&ctx->astream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
-    if ((e = cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
+    if ((e = cudaStreamCreateWithFlags(&ctx->astream.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
+    if ((e = cudaStreamCreateWithFlags(&ctx->stream2.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   }
-  if ((e = cudaMalloc(&ctx->a_stop, sizeof(int))) != cudaSuccess) return bail("cudaMalloc a_stop", e);
-  if ((e = cudaMalloc(&ctx->a_cnt, sizeof(unsigned long long) * 2)) != cudaSuccess) return bail("cudaMalloc a_cnt", e);
+  if ((e = ctx->a_stop.alloc(1)) != cudaSuccess) return bail("cudaMalloc a_stop", e);
+  if ((e = ctx->a_cnt.alloc(2)) != cudaSuccess) return bail("cudaMalloc a_cnt", e);
   cudaMemsetAsync(ctx->a_stop, 0, sizeof(int), ctx->own_stream);
   cudaMemsetAsync(ctx->a_cnt, 0, sizeof(unsigned long long) * 2, ctx->own_stream);
   ctx->stream = ctx->own_stream;
-  if ((e = cudaEventCreate(&ctx->ev0)) != cudaSuccess) return bail("event", e);
-  if ((e = cudaEventCreate(&ctx->ev1)) != cudaSuccess) return bail("event", e);
-  const size_t vd = sizeof(double) * (size_t)(dim + kReplicaPad);
+  if ((e = cudaEventCreate(&ctx->ev0.h)) != cudaSuccess) return bail("event", e);
+  if ((e = cudaEventCreate(&ctx->ev1.h)) != cudaSuccess) return bail("event", e);
+  const int64_t nv = (int64_t)dim + kReplicaPad;
+  const size_t vd = sizeof(double) * (size_t)nv;
   const int upd_blocks = cdiv(dim, 256);
-  if ((e = cudaMalloc(&ctx->w, vd)) != cudaSuccess) return bail("cudaMalloc w", e);
-  if ((e = cudaMalloc(&ctx->g, vd)) != cudaSuccess) return bail("cudaMalloc g", e);
-  if ((e = cudaMalloc(&ctx->d, vd)) != cudaSuccess) return bail("cudaMalloc d", e);
-  if ((e = cudaMalloc(&ctx->w_req, vd)) != cudaSuccess) return bail("cudaMalloc w_req", e);
-  if ((e = cudaMalloc(&ctx->w32, sizeof(float) * (size_t)(dim + 4))) != cudaSuccess) return bail("cudaMalloc w32", e);
-  if ((e = cudaMalloc(&ctx->w32_req, sizeof(float) * (size_t)(dim + 4))) != cudaSuccess) return bail("cudaMalloc w32_req", e);
-  if ((e = cudaMalloc(&ctx->n_exact, sizeof(unsigned long long) * 2)) != cudaSuccess) return bail("cudaMalloc n_exact", e);
+  if ((e = ctx->w.alloc(nv)) != cudaSuccess) return bail("cudaMalloc w", e);
+  if ((e = ctx->g.alloc(nv)) != cudaSuccess) return bail("cudaMalloc g", e);
+  if ((e = ctx->d.alloc(nv)) != cudaSuccess) return bail("cudaMalloc d", e);
+  if ((e = ctx->w_req.alloc(nv)) != cudaSuccess) return bail("cudaMalloc w_req", e);
+  if ((e = ctx->w32.alloc((int64_t)dim + 4)) != cudaSuccess) return bail("cudaMalloc w32", e);
+  if ((e = ctx->w32_req.alloc((int64_t)dim + 4)) != cudaSuccess) return bail("cudaMalloc w32_req", e);
+  if ((e = ctx->n_exact.alloc(2)) != cudaSuccess) return bail("cudaMalloc n_exact", e);
   cudaMemsetAsync(ctx->n_exact, 0, sizeof(unsigned long long) * 2, ctx->stream);
-  if ((e = cudaMalloc(&ctx->scal, sizeof(double) * kNumScal)) != cudaSuccess) return bail("cudaMalloc scal", e);
-  if ((e = cudaMalloc(&ctx->cnt, sizeof(unsigned long long) * kNumCnt)) != cudaSuccess) return bail("cudaMalloc cnt", e);
-  if ((e = cudaMalloc(&ctx->partial, sizeof(double) * 2 * (size_t)upd_blocks)) != cudaSuccess) return bail("cudaMalloc partial", e);
-  if ((e = cudaMalloc(&ctx->out2, sizeof(double) * 8)) != cudaSuccess) return bail("cudaMalloc out2", e);
-  if ((e = cudaMalloc(&ctx->gsum, vd)) != cudaSuccess) return bail("cudaMalloc gsum", e);
+  if ((e = ctx->scal.alloc(kNumScal)) != cudaSuccess) return bail("cudaMalloc scal", e);
+  if ((e = ctx->cnt.alloc(kNumCnt)) != cudaSuccess) return bail("cudaMalloc cnt", e);
+  if ((e = ctx->partial.alloc(2 * (int64_t)upd_blocks)) != cudaSuccess) return bail("cudaMalloc partial", e);
+  if ((e = ctx->out2.alloc(8)) != cudaSuccess) return bail("cudaMalloc out2", e);
+  if ((e = ctx->gsum.alloc(nv)) != cudaSuccess) return bail("cudaMalloc gsum", e);
   cudaMemsetAsync(ctx->gsum, 0, vd, ctx->stream);
   cudaMemsetAsync(ctx->w, 0, vd, ctx->stream);
   cudaMemsetAsync(ctx->g, 0, vd, ctx->stream);
@@ -276,27 +361,7 @@ extern "C" int dsgd_destroy(dsgd_ctx *ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   if (ctx->comm) nccl().CommDestroy(ctx->comm);
-  for (int r = 0; r < kMaxReplicas; ++r)
-    if (ctx->peer_w[r] && ctx->peer_ipc[r]) cudaIpcCloseMemHandle(ctx->peer_w[r]);
-  for (int r = 0; r < kMaxWorld; ++r)
-    if (ctx->peer_x[r] && ctx->peer_x_ipc[r]) cudaIpcCloseMemHandle(ctx->peer_x[r]);
-  if (ctx->xblk) cudaFree(ctx->xblk);
-  if (ctx->x_llw) cudaFree(ctx->x_llw);
-  void *aptrs[] = {ctx->m_w, ctx->outbox, ctx->a_stop, ctx->a_cnt, ctx->a_scratch, ctx->a_rows, ctx->a_assigned, ctx->a_replay, ctx->u_idx, ctx->u_val};
-  for (void *q : aptrs) if (q) cudaFree(q);
-  if (ctx->a_ev0) { cudaEventDestroy(ctx->a_ev0); cudaEventDestroy(ctx->a_ev1); }
-  if (ctx->astream) cudaStreamDestroy(ctx->astream);
-  if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-  void *ptrs[] = {ctx->rp16, ctx->pairs, ctx->label, ctx->yabs, ctx->w, ctx->g, ctx->d, ctx->w_req, ctx->w32, ctx->w32_req, ctx->n_exact, ctx->scal,
-                  ctx->cnt, ctx->partial, ctx->out2, ctx->gsum, ctx->p_wbuf[0], ctx->p_wbuf[1], ctx->p_gbuf[0],
-                  ctx->p_gbuf[1], ctx->p_gbuf[2], ctx->p_rec[0], ctx->p_rec[1], ctx->p_rec[2], ctx->p_acc, ctx->p_hinge, ctx->p_bar, ctx->x_stats, ctx->samples,
-                  ctx->losses, ctx->preds, ctx->eval_ids};
-  for (void *p : ptrs) if (p) cudaFree(p);
-  if (ctx->ev0) cudaEventDestroy(ctx->ev0);
-  if (ctx->ev1) cudaEventDestroy(ctx->ev1);
-  for (auto &pe : ctx->prof_events) { cudaEventDestroy(pe.first); cudaEventDestroy(pe.second); }
-  if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-  delete ctx;
+  delete ctx;   // its members free the device buffers, streams, events and peer mappings
   return DSGD_OK;
 }
 
@@ -412,17 +477,17 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
       }
   }
   CU(cudaSetDevice(ctx->device));
-  for (void *p : {(void *)ctx->rp16, (void *)ctx->pairs, (void *)ctx->label, (void *)ctx->yabs}) if (p) CU(cudaFree(p));
-  ctx->rp16 = nullptr; ctx->pairs = nullptr; ctx->label = nullptr; ctx->yabs = nullptr;
+  // all of the previous rows go before any of the new ones is allocated
+  CU(ctx->rp16.release()); CU(ctx->pairs.release()); CU(ctx->label.release()); CU(ctx->yabs.release());
   const int64_t n_pairs = (int64_t)acc * 2;
-  CU(cudaMalloc(&ctx->rp16, sizeof(uint32_t) * ((size_t)n_rows + 1)));
-  CU(cudaMalloc(&ctx->pairs, sizeof(uint2) * (size_t)std::max<int64_t>(n_pairs, 1)));
-  CU(cudaMalloc(&ctx->label, (size_t)n_rows));
-  CU(cudaMalloc(&ctx->yabs, sizeof(float) * (size_t)n_rows));
-  int64_t *d_rp = nullptr; int32_t *d_col = nullptr; float *d_val = nullptr;
-  CU(cudaMalloc(&d_rp, sizeof(int64_t) * ((size_t)n_rows + 1)));
-  CU(cudaMalloc(&d_col, sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1)));
-  CU(cudaMalloc(&d_val, sizeof(float) * (size_t)std::max<int64_t>(nnz, 1)));
+  CU(ctx->rp16.alloc(n_rows + 1));
+  CU(ctx->pairs.alloc(std::max<int64_t>(n_pairs, 1)));
+  CU(ctx->label.alloc(n_rows));
+  CU(ctx->yabs.alloc(n_rows));
+  dev_buf<int64_t> d_rp; dev_buf<int32_t> d_col; dev_buf<float> d_val;
+  CU(d_rp.alloc(n_rows + 1));
+  CU(d_col.alloc(std::max<int64_t>(nnz, 1)));
+  CU(d_val.alloc(std::max<int64_t>(nnz, 1)));
   CU(cudaMemcpyAsync(d_rp, row_ptr, sizeof(int64_t) * ((size_t)n_rows + 1), cudaMemcpyHostToDevice, ctx->stream));
   if (nnz) {
     CU(cudaMemcpyAsync(d_col, col, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, ctx->stream));
@@ -435,18 +500,22 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream));
-  CU(cudaFree(d_rp)); CU(cudaFree(d_col)); CU(cudaFree(d_val));
+  CU(d_rp.release()); CU(d_col.release()); CU(d_val.release());
   ctx->n_rows = n_rows; ctx->nnz = nnz; ctx->n_pairs = n_pairs;
   return DSGD_OK;
 }
 
+// c and ||w||^2 of the weights `w` into scal[c_slot] and scal[nrm_slot], and their fp32 shadow into w32
+static void launch_prepare(dsgd_ctx *ctx, const double *w, float *w32, int c_slot, int nrm_slot) {
+  k_prepare<1024><<<1, 1024, 0, ctx->stream>>>(w, ctx->d, ctx->dim, ctx->lambda, ctx->scal + c_slot, ctx->scal + nrm_slot);
+  LAUNCHED();
+  k_to_f32<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(w, w32, ctx->dim);
+  LAUNCHED();
+}
+
 // recompute c and ||w||^2 of the resident weights, refresh the fp32 shadow
 static int refresh_resident(dsgd_ctx *ctx) {
-  k_prepare<1024><<<1, 1024, 0, ctx->stream>>>(ctx->w, ctx->d, ctx->dim, ctx->lambda, ctx->scal + kScalC,
-                                                ctx->scal + kScalNrm2);
-  LAUNCHED();
-  k_to_f32<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->dim);
-  LAUNCHED();
+  launch_prepare(ctx, ctx->w, ctx->w32, kScalC, kScalNrm2);
   if (ctx->flags & DSGD_FLAG_ASYNC) {
     k_async_init_ctl<1024><<<1, 1024, 0, ctx->stream>>>(ctx->w, ctx->d, ctx->dim);
     LAUNCHED();
@@ -473,8 +542,8 @@ extern "C" int dsgd_compute_dim_sparsity(dsgd_ctx *ctx, int64_t n_train, double 
   NEED(n_train >= 0 && n_train <= ctx->n_rows, DSGD_ERR_RANGE, "dsgd_compute_dim_sparsity: n_train %lld outside [0,%lld]",
        (long long)n_train, (long long)ctx->n_rows);
   CU(cudaSetDevice(ctx->device));
-  unsigned *df = nullptr;
-  CU(cudaMalloc(&df, sizeof(unsigned) * (size_t)ctx->dim));
+  dev_buf<unsigned> df;
+  CU(df.alloc(ctx->dim));
   CU(cudaMemsetAsync(df, 0, sizeof(unsigned) * (size_t)ctx->dim, ctx->stream));
   uint32_t end16 = 0;
   CU(cudaMemcpyAsync(&end16, ctx->rp16 + n_train, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -493,7 +562,7 @@ extern "C" int dsgd_compute_dim_sparsity(dsgd_ctx *ctx, int64_t n_train, double 
   if (rc) return rc;
   if (d_out) CU(cudaMemcpyAsync(d_out, ctx->d, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  CU(cudaFree(df));
+  CU(df.release());
   return DSGD_OK;
 }
 
@@ -519,35 +588,14 @@ extern "C" int dsgd_get_weights(dsgd_ctx *ctx, double *w) {
 
 // ---- sample staging ----------------------------------------------------------------------------------
 
-static int ensure_i32(dsgd_ctx *ctx, int32_t **buf, int64_t *cap, int64_t n) {
-  if (*cap >= n) return DSGD_OK;
-  if (*buf) CU(cudaFree(*buf));
-  *buf = nullptr; *cap = 0;
-  const int64_t want = std::max<int64_t>(n, 1024);
-  CU(cudaMalloc(buf, sizeof(int32_t) * (size_t)want));
-  *cap = want;
-  return DSGD_OK;
-}
-static int ensure_f64(dsgd_ctx *ctx, double **buf, int64_t *cap, int64_t n) {
-  if (*cap >= n) return DSGD_OK;
-  if (*buf) CU(cudaFree(*buf));
-  *buf = nullptr; *cap = 0;
-  const int64_t want = std::max<int64_t>(n, 1024);
-  CU(cudaMalloc(buf, sizeof(double) * (size_t)want));
-  *cap = want;
-  return DSGD_OK;
-}
-
 extern "C" int dsgd_stage_samples(dsgd_ctx *ctx, const int32_t *samples, int64_t n) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_stage_samples: no rows loaded");
   NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_stage_samples: bad arguments");
-  for (int64_t i = 0; i < n; ++i)
-    NEED(samples[i] >= 0 && samples[i] < ctx->n_rows, DSGD_ERR_RANGE, "sample index %d at position %lld outside [0,%lld)",
-         samples[i], (long long)i, (long long)ctx->n_rows);
-  CU(cudaSetDevice(ctx->device));
-  int rc = ensure_i32(ctx, &ctx->samples, &ctx->samples_cap, n);
+  int rc = check_ids(ctx, samples, n, "sample index");
   if (rc) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->samples.grow(ctx, n, 1024))) return rc;
   if (n) CU(cudaMemcpyAsync(ctx->samples, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   ctx->samples_n = n;
   return DSGD_OK;
@@ -564,11 +612,7 @@ static int request_weights(dsgd_ctx *ctx, const double *w, const double **w_dev,
   }
   if (w32_dev) *w32_dev = ctx->w32_req;
   CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
-  k_prepare<1024><<<1, 1024, 0, ctx->stream>>>(ctx->w_req, ctx->d, ctx->dim, ctx->lambda, ctx->scal + kScalReqC,
-                                                ctx->scal + kScalReqNrm2);
-  LAUNCHED();
-  k_to_f32<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w_req, ctx->w32_req, ctx->dim);
-  LAUNCHED();
+  launch_prepare(ctx, ctx->w_req, ctx->w32_req, kScalReqC, kScalReqNrm2);
   CU(cudaGetLastError());
   *w_dev = ctx->w_req; *c_dev = ctx->scal + kScalReqC; *nrm_dev = ctx->scal + kScalReqNrm2;
   return DSGD_OK;
@@ -599,7 +643,7 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
   NEED(kContig == (samples_dev == nullptr), DSGD_ERR_INVALID, "stream_launch: sample list / row range mismatch");
   StreamParams sp;
   memset(&sp, 0, sizeof sp);
-  sp.rp16 = ctx->rp16; sp.units = reinterpret_cast<const uint4 *>(ctx->pairs); sp.yabs = ctx->yabs;
+  sp.rp16 = ctx->rp16; sp.units = reinterpret_cast<const uint4 *>(ctx->pairs.p); sp.yabs = ctx->yabs;
   sp.samples = samples_dev; sp.row_begin = row_begin; sp.n = n;
   sp.w = w_dev; sp.w32 = w32_dev; sp.dim = ctx->dim;
   sp.g = g; sp.preds = preds; sp.cnt = ctx->cnt; sp.n_exact = ctx->n_exact; sp.next_block = ctx->n_exact + 1;
@@ -613,10 +657,7 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
   sp.n_big = sp.tail_log2 < sp.rows_log2 ? ((n - n / 5) >> sp.rows_log2) : ((n + (1 << sp.rows_log2) - 1) >> sp.rows_log2);
   const int64_t n_blk = sp.n_big + cdiv(std::max<int64_t>(0, n - (sp.n_big << sp.rows_log2)), (int64_t)1 << sp.tail_log2);
   const int grid = (int)std::min<int64_t>(ctx->sm_count, std::max<int64_t>(1, cdiv(n_blk, kStreamThreads / 32)));
-  auto *pe = prof_slot(ctx);
-  if (pe) cudaEventRecord(pe->first, ctx->stream);
-  k_stream_rows<kScatter, kPreds, kContig><<<grid, kStreamThreads, smem, ctx->stream>>>(sp);
-  if (pe) cudaEventRecord(pe->second, ctx->stream);
+  profiled(ctx, [&] { k_stream_rows<kScatter, kPreds, kContig><<<grid, kStreamThreads, smem, ctx->stream>>>(sp); });
   LAUNCHED();
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -630,7 +671,7 @@ extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *sampl
   if (n == 0) return DSGD_OK;
   int rc = dsgd_stage_samples(ctx, samples, n);
   if (rc) return rc;
-  rc = ensure_f64(ctx, &ctx->preds, &ctx->preds_cap, n);
+  rc = ctx->preds.grow(ctx, n, 1024);
   if (rc) return rc;
   const double *wd, *cd, *nd;
   const float *w32d;
@@ -760,7 +801,7 @@ extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t 
   NEED(pos_end > pos_begin, DSGD_ERR_EMPTY, "dsgd_eval_sampled_counts: no positions (reduce on an empty collection throws)");
   CU(cudaSetDevice(ctx->device));
   const int64_t k = pos_end - pos_begin;
-  int rc = ensure_i32(ctx, &ctx->eval_ids, &ctx->eval_ids_cap, k);
+  int rc = ctx->eval_ids.grow(ctx, k, 1024);
   if (rc) return rc;
   k_draw_rows<<<cdiv(k, 256), 256, 0, ctx->stream>>>(ctx->eval_ids, k, (uint32_t)pos_begin,
                                                       dsgd_feistel_half_bits((uint64_t)n), key, (uint32_t)n, row_begin);
@@ -778,12 +819,10 @@ extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const in
   NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_samples_counts: no rows loaded");
   NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_eval_samples_counts: bad arguments");
   NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_samples_counts: empty sample (reduce on an empty collection throws)");
-  for (int64_t i = 0; i < n; ++i)
-    NEED(samples[i] >= 0 && samples[i] < ctx->n_rows, DSGD_ERR_RANGE, "sample index %d at position %lld outside [0,%lld)",
-         samples[i], (long long)i, (long long)ctx->n_rows);
-  CU(cudaSetDevice(ctx->device));
-  int rc = ensure_i32(ctx, &ctx->eval_ids, &ctx->eval_ids_cap, n);
+  int rc = check_ids(ctx, samples, n, "sample index");
   if (rc) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
   CU(cudaMemcpyAsync(ctx->eval_ids, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   double out[5];
   if ((rc = eval_pass(ctx, w, ctx->eval_ids, 0, n, out))) return rc;
@@ -836,28 +875,22 @@ static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIME
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
   if (!ctx->p_ready) {
-    const size_t vd = sizeof(double) * (size_t)(ctx->dim + 2);
-    for (int i = 0; i < 2; ++i) CU(cudaMalloc(&ctx->p_wbuf[i], vd));
+    const int64_t nv = (int64_t)ctx->dim + 2;
+    const size_t vd = sizeof(double) * (size_t)nv;
+    for (int i = 0; i < 2; ++i) CU(ctx->p_wbuf[i].alloc(nv));
     for (int i = 0; i < 3; ++i) {
-      CU(cudaMalloc(&ctx->p_gbuf[i], vd));
+      CU(ctx->p_gbuf[i].alloc(nv));
       CU(cudaMemsetAsync(ctx->p_gbuf[i], 0, vd, ctx->stream));
-      CU(cudaMalloc(&ctx->p_rec[i], 2 * vd));
+      CU(ctx->p_rec[i].alloc(nv));
       CU(cudaMemsetAsync(ctx->p_rec[i], 0, 2 * vd, ctx->stream));
     }
-    CU(cudaMalloc(&ctx->p_acc, sizeof(unsigned long long) * 3 * kAccStride));
-    CU(cudaMalloc(&ctx->p_bar, sizeof(unsigned) * 4));
+    CU(ctx->p_acc.alloc(3 * kAccStride));
+    CU(ctx->p_bar.alloc(4));
     CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
-  if (ctx->p_hinge_cap < n_steps) {
-    if (ctx->p_hinge) CU(cudaFree(ctx->p_hinge));
-    ctx->p_hinge = nullptr;
-    const int64_t want = std::max<int64_t>(n_steps, 4096);
-    CU(cudaMalloc(&ctx->p_hinge, sizeof(unsigned) * (size_t)want));
-    ctx->p_hinge_cap = want;
-  }
-  return DSGD_OK;
+  return ctx->p_hinge.grow(ctx, n_steps, 4096);
 }
 
 // CTAs of the persistent kernel: one per SM (fastest at batch 64, 256 and 1024 when it was
@@ -883,10 +916,47 @@ static cudaError_t persist_launch(dsgd_ctx *ctx, void *fn, int G, void **args) {
   return cudaLaunchCooperativeKernel(fn, dim3(G), dim3((kPCons + kPUpd + 1) * 32), args, sizeof(PSmem), ctx->stream);
 }
 
-// fields shared by the one-GPU and the K-GPU launch
-static int persist_params(dsgd_ctx *ctx, PersistParams &pp, const int32_t *samples_dev, int64_t n_per_step, int64_t n_steps,
-                          double lr, double *losses_dev, int G) {
-  (void)G;
+// ---- fused K-GPU loop: all ranks run the persistent kernel and exchange gradients through peer memory ----
+// exported block of a rank (in 8-byte words): value words [sender][parity][dim + 8] x 2, then bitmap words
+// [sender][parity][ceil((dim + 1) / 32)]
+static size_t xblk_stride(const dsgd_ctx *ctx) { return (size_t)(ctx->dim + kReplicaPad); }
+static size_t xblk_words(const dsgd_ctx *ctx) { return ((size_t)ctx->dim + 1 + 31) / 32; }
+static size_t xblk_bm_offset(const dsgd_ctx *ctx) { return 2 * (size_t)kMaxWorld * 2 * xblk_stride(ctx); }
+static size_t xblk_doubles(const dsgd_ctx *ctx) { return xblk_bm_offset(ctx) + (size_t)kMaxWorld * 2 * xblk_words(ctx); }
+
+static int xblk_ensure(dsgd_ctx *ctx) {
+  if (ctx->xblk) return DSGD_OK;
+  CU(cudaSetDevice(ctx->device));
+  CU(ctx->xblk.alloc((int64_t)xblk_doubles(ctx)));
+  CU(cudaMemset(ctx->xblk, 0, sizeof(double) * xblk_doubles(ctx)));
+  CU(ctx->x_stats.alloc(4));
+  CU(cudaMemset(ctx->x_stats, 0, sizeof(unsigned long long) * 4));
+  return DSGD_OK;
+}
+
+static int xllw_ensure(dsgd_ctx *ctx) {
+  if (ctx->x_llw) return DSGD_OK;
+  CU(ctx->x_llw.alloc(2 * 2 * (int64_t)xblk_stride(ctx)));
+  CU(cudaMemsetAsync(ctx->x_llw, 0, 2 * 2 * sizeof(unsigned long long) * xblk_stride(ctx), ctx->stream));
+  return DSGD_OK;
+}
+
+static bool xchg_complete(const dsgd_ctx *ctx) {
+  if (ctx->world <= 1 || ctx->world > kMaxWorld || !ctx->xblk) return false;
+  for (int r = 0; r < ctx->world; ++r)
+    if (r != ctx->rank && !ctx->peer_x[r]) return false;
+  return true;
+}
+
+// One launch of the persistent kernel for n_steps SGD steps: on one GPU, or (multi) the fused K-GPU kernel in which every
+// rank aggregates the gradients through the exchange blocks of its peers.
+static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, int64_t n_per_step, int64_t n_steps,
+                       double lr, double *losses_dev) {
+  int rc = persist_prepare(ctx, n_steps);
+  if (rc) return rc;
+  const int G = persist_grid(ctx, n_per_step);
+  NEED((uint64_t)G * (uint64_t)(n_steps + 2) < (1ull << 32), DSGD_ERR_INVALID, "dsgd_sync_steps: too many steps for one launch");
+  PersistParams pp;
   memset(&pp, 0, sizeof pp);
   pp.rp16 = ctx->rp16; pp.pairs = ctx->pairs; pp.label = ctx->label; pp.samples = samples_dev;
   pp.n_steps = n_steps; pp.batch = (int32_t)n_per_step; pp.dim = ctx->dim;
@@ -900,102 +970,47 @@ static int persist_params(dsgd_ctx *ctx, PersistParams &pp, const int32_t *sampl
   CU(cudaMemsetAsync(ctx->p_hinge, 0, sizeof(unsigned) * (size_t)n_steps, ctx->stream));
   CU(cudaMemsetAsync(ctx->p_bar, 0, sizeof(unsigned) * 4, ctx->stream));
   if (persist_timeline()) {
-    if (!ctx->p_tl) CU(cudaMalloc(&ctx->p_tl, sizeof(long long) * kTlWords));
+    if (!ctx->p_tl) CU(ctx->p_tl.alloc(kTlWords));
     CU(cudaMemsetAsync(ctx->p_tl, 0, sizeof(long long) * kTlWords, ctx->stream));
     pp.tl = ctx->p_tl;
   }
-  return DSGD_OK;
-}
-
-static int persist_run(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t n_per_step, int64_t n_steps, double lr,
-                       double *losses_dev) {
-  int rc = persist_prepare(ctx, n_steps);
-  if (rc) return rc;
-  const int G = persist_grid(ctx, n_per_step);
-  NEED((uint64_t)G * (uint64_t)(n_steps + 2) < (1ull << 32), DSGD_ERR_INVALID, "dsgd_sync_steps: too many steps for one launch");
-  PersistParams pp;
-  if ((rc = persist_params(ctx, pp, samples_dev, n_per_step, n_steps, lr, losses_dev, G))) return rc;
-  k_rec_init<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w, ctx->dim, ctx->p_rec[0], ctx->p_rec[1], ctx->p_rec[2]);
-  LAUNCHED();
-  pp.k_den = 1.0;
-  pp.timeout_cycles = 4000000000ll;  // ~2 s at 1.9 GHz: a healthy barrier takes well under a microsecond
-  void *args[] = {&pp};
-  auto *pe = prof_slot(ctx);
-  if (pe) cudaEventRecord(pe->first, ctx->stream);
-  CU(persist_launch(ctx, (void *)DSGD_PERSIST_KERNEL(false), G, args));
-  if (pe) cudaEventRecord(pe->second, ctx->stream);
-  LAUNCHED();
-  return DSGD_OK;
-}
-
-// ---- fused K-GPU loop: all ranks run the persistent kernel and exchange gradients through peer memory ----
-// exported block of a rank (in 8-byte words): value words [sender][parity][dim + 8] x 2, then bitmap words
-// [sender][parity][ceil((dim + 1) / 32)]
-static size_t xblk_stride(const dsgd_ctx *ctx) { return (size_t)(ctx->dim + kReplicaPad); }
-static size_t xblk_words(const dsgd_ctx *ctx) { return ((size_t)ctx->dim + 1 + 31) / 32; }
-static size_t xblk_bm_offset(const dsgd_ctx *ctx) { return 2 * (size_t)kMaxWorld * 2 * xblk_stride(ctx); }
-static size_t xblk_doubles(const dsgd_ctx *ctx) { return xblk_bm_offset(ctx) + (size_t)kMaxWorld * 2 * xblk_words(ctx); }
-
-static int xblk_ensure(dsgd_ctx *ctx) {
-  if (ctx->xblk) return DSGD_OK;
-  CU(cudaSetDevice(ctx->device));
-  CU(cudaMalloc(&ctx->xblk, sizeof(double) * xblk_doubles(ctx)));
-  CU(cudaMemset(ctx->xblk, 0, sizeof(double) * xblk_doubles(ctx)));
-  CU(cudaMalloc(&ctx->x_stats, sizeof(unsigned long long) * 4));
-  CU(cudaMemset(ctx->x_stats, 0, sizeof(unsigned long long) * 4));
-  return DSGD_OK;
-}
-
-static int xllw_ensure(dsgd_ctx *ctx) {
-  if (ctx->x_llw) return DSGD_OK;
-  CU(cudaMalloc(&ctx->x_llw, 2 * 2 * sizeof(unsigned long long) * xblk_stride(ctx)));
-  CU(cudaMemsetAsync(ctx->x_llw, 0, 2 * 2 * sizeof(unsigned long long) * xblk_stride(ctx), ctx->stream));
-  return DSGD_OK;
-}
-
-static bool xchg_complete(const dsgd_ctx *ctx) {
-  if (ctx->world <= 1 || ctx->world > kMaxWorld || !ctx->xblk) return false;
-  for (int r = 0; r < ctx->world; ++r)
-    if (r != ctx->rank && !ctx->peer_x[r]) return false;
-  return true;
-}
-
-static int persist_run_multi(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t n_per_step, int64_t n_steps, double lr,
-                             double *losses_dev) {
-  int rc = persist_prepare(ctx, n_steps);
-  if (rc) return rc;
-  const int G = persist_grid(ctx, n_per_step);
-  NEED((uint64_t)G * (uint64_t)(n_steps + 2) < (1ull << 32), DSGD_ERR_INVALID, "dsgd_sync_steps: too many steps for one launch");
-  PersistParams pp;
-  if ((rc = persist_params(ctx, pp, samples_dev, n_per_step, n_steps, lr, losses_dev, G))) return rc;
-  // the kernel's first interval reads the host-provided weights from wbuf[0] and publishes them in LL form
-  CU(cudaMemcpyAsync(ctx->p_wbuf[0], ctx->w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToDevice, ctx->stream));
-  pp.k_den = (double)ctx->world;
-  pp.timeout_cycles = 20000000000ll;  // ~10 s: covers a peer that launches late
-  pp.world = ctx->world; pp.rank = ctx->rank; pp.step_base = ctx->x_step;
-  pp.xstride = (int)xblk_stride(ctx);
-  pp.xwords = (int)xblk_words(ctx);
-  for (int r = 0; r < ctx->world; ++r) {
-    unsigned long long *blk = reinterpret_cast<unsigned long long *>((r == ctx->rank) ? ctx->xblk : ctx->peer_x[r]);
-    pp.xval[r] = blk;
-    pp.xbm[r] = blk + xblk_bm_offset(ctx);
+  if (!multi) {
+    k_rec_init<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w, ctx->dim, ctx->p_rec[0], ctx->p_rec[1], ctx->p_rec[2]);
+    LAUNCHED();
+    pp.k_den = 1.0;
+    pp.timeout_cycles = 4000000000ll;  // ~2 s at 1.9 GHz: a healthy barrier takes well under a microsecond
+  } else {
+    // the kernel's first interval reads the host-provided weights from wbuf[0] and publishes them in LL form
+    CU(cudaMemcpyAsync(ctx->p_wbuf[0], ctx->w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToDevice, ctx->stream));
+    pp.k_den = (double)ctx->world;
+    pp.timeout_cycles = 20000000000ll;  // ~10 s: covers a peer that launches late
+    pp.world = ctx->world; pp.rank = ctx->rank; pp.step_base = ctx->x_step;
+    pp.xstride = (int)xblk_stride(ctx);
+    pp.xwords = (int)xblk_words(ctx);
+    for (int r = 0; r < ctx->world; ++r) {
+      unsigned long long *blk = reinterpret_cast<unsigned long long *>((r == ctx->rank) ? ctx->xblk.p : ctx->peer_x[r].p);
+      pp.xval[r] = blk;
+      pp.xbm[r] = blk + xblk_bm_offset(ctx);
+    }
+    if ((rc = xllw_ensure(ctx))) return rc;
+    pp.llw[0] = ctx->x_llw;
+    pp.llw[1] = ctx->x_llw + 2 * xblk_stride(ctx);
+    pp.xstats = ctx->x_stats;
   }
-  if ((rc = xllw_ensure(ctx))) return rc;
-  pp.llw[0] = ctx->x_llw;
-  pp.llw[1] = ctx->x_llw + 2 * xblk_stride(ctx);
-  pp.xstats = ctx->x_stats;
   void *args[] = {&pp};
-  auto *pe = prof_slot(ctx);
-  if (pe) cudaEventRecord(pe->first, ctx->stream);
-  CU(persist_launch(ctx, (void *)DSGD_PERSIST_KERNEL(true), G, args));
-  if (pe) cudaEventRecord(pe->second, ctx->stream);
+  void *fn = multi ? (void *)DSGD_PERSIST_KERNEL(true) : (void *)DSGD_PERSIST_KERNEL(false);
+  cudaError_t launch_err = cudaSuccess;
+  profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
+  CU(launch_err);
   LAUNCHED();
-  // The next launch must not meet LL words carrying tags this one used (the host may install new weights in between): the
-  // step counter jumps.  By 6: a multiple of 3 keeps the rotation of the three gradient buffers (the dirty one is re-zeroed
-  // before use), and an EVEN jump makes the first push of launch n+1 (its second interval) land in the receive parity that
-  // a slow peer is NOT reading in launch n's last interval (+3 put them on the same one: ADVICE.md round 1).
-  ctx->x_step += n_steps + 6;
-  ctx->x_steps_run += n_steps;
+  if (multi) {
+    // The next launch must not meet LL words carrying tags this one used (the host may install new weights in between): the
+    // step counter jumps.  By 6: a multiple of 3 keeps the rotation of the three gradient buffers (the dirty one is re-zeroed
+    // before use), and an EVEN jump makes the first push of launch n+1 (its second interval) land in the receive parity that
+    // a slow peer is NOT reading in launch n's last interval (+3 put them on the same one: ADVICE.md round 1).
+    ctx->x_step += n_steps + 6;
+    ctx->x_steps_run += n_steps;
+  }
   return DSGD_OK;
 }
 
@@ -1003,11 +1018,11 @@ extern "C" int dsgd_reserve(dsgd_ctx *ctx, int64_t n_samples, int64_t n_steps) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(n_samples >= 0 && n_steps >= 0, DSGD_ERR_INVALID, "dsgd_reserve: negative size");
   CU(cudaSetDevice(ctx->device));
-  int rc = ensure_i32(ctx, &ctx->samples, &ctx->samples_cap, n_samples);
+  int rc = ctx->samples.grow(ctx, n_samples, 1024);
   if (rc) return rc;
-  if ((rc = ensure_f64(ctx, &ctx->losses, &ctx->losses_cap, n_steps))) return rc;
+  if ((rc = ctx->losses.grow(ctx, n_steps, 1024))) return rc;
   if ((rc = persist_prepare(ctx, n_steps))) return rc;
-  if (persist_timeline() && !ctx->p_tl) CU(cudaMalloc(&ctx->p_tl, sizeof(long long) * kTlWords));
+  if (persist_timeline() && !ctx->p_tl) CU(ctx->p_tl.alloc(kTlWords));
   if (ctx->world > 1 && !(ctx->flags & DSGD_FLAG_ASYNC)) {
     if ((rc = xblk_ensure(ctx))) return rc;
     if ((rc = xllw_ensure(ctx))) return rc;
@@ -1039,6 +1054,30 @@ extern "C" int dsgd_xchg_stats(dsgd_ctx *ctx, int64_t *value_words, int64_t *bit
   return DSGD_OK;
 }
 
+// ---- peer memory: buffers of other ranks, mapped from another process or attached from this one ----
+
+static int open_ipc(dsgd_ctx *ctx, peer_ptr &slot, const uint8_t handle[DSGD_IPC_HANDLE_BYTES]) {
+  cudaIpcMemHandle_t h;
+  memcpy(&h, handle, sizeof h);
+  void *ptr = nullptr;
+  CU(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
+  slot.set(static_cast<double *>(ptr), true);
+  return DSGD_OK;
+}
+
+// makes ctx's device current and lets it address the memory of peer's device
+static int enable_peer_access(dsgd_ctx *ctx, const dsgd_ctx *peer, const char *who) {
+  CU(cudaSetDevice(ctx->device));
+  if (peer->device == ctx->device) return DSGD_OK;
+  int can = 0;
+  CU(cudaDeviceCanAccessPeer(&can, ctx->device, peer->device));
+  NEED(can, DSGD_ERR_CUDA, "%s: device %d cannot access device %d", who, ctx->device, peer->device);
+  cudaError_t e = cudaDeviceEnablePeerAccess(peer->device, 0);
+  if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CU(e);
+  (void)cudaGetLastError();
+  return DSGD_OK;
+}
+
 extern "C" int dsgd_xchg_export(dsgd_ctx *ctx, uint8_t handle[DSGD_IPC_HANDLE_BYTES]) {
   if (!ctx || !handle) return DSGD_ERR_INVALID;
   NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_xchg_export: ctx is in async mode");
@@ -1056,14 +1095,7 @@ extern "C" int dsgd_xchg_import(dsgd_ctx *ctx, int peer_rank, const uint8_t hand
        "dsgd_xchg_import: bad peer rank %d", peer_rank);
   int rc = xblk_ensure(ctx);
   if (rc) return rc;
-  cudaIpcMemHandle_t h;
-  memcpy(&h, handle, sizeof h);
-  void *ptr = nullptr;
-  CU(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-  if (ctx->peer_x[peer_rank] && ctx->peer_x_ipc[peer_rank]) cudaIpcCloseMemHandle(ctx->peer_x[peer_rank]);
-  ctx->peer_x[peer_rank] = static_cast<double *>(ptr);
-  ctx->peer_x_ipc[peer_rank] = true;
-  return DSGD_OK;
+  return open_ipc(ctx, ctx->peer_x[peer_rank], handle);
 }
 
 extern "C" int dsgd_xchg_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer) {
@@ -1074,17 +1106,8 @@ extern "C" int dsgd_xchg_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer) {
   int rc = xblk_ensure(ctx);
   if (rc) return rc;
   if ((rc = xblk_ensure(peer))) { ctx->err = peer->err; return rc; }
-  CU(cudaSetDevice(ctx->device));
-  if (peer->device != ctx->device) {
-    int can = 0;
-    CU(cudaDeviceCanAccessPeer(&can, ctx->device, peer->device));
-    NEED(can, DSGD_ERR_CUDA, "dsgd_xchg_attach: device %d cannot access device %d", ctx->device, peer->device);
-    cudaError_t e = cudaDeviceEnablePeerAccess(peer->device, 0);
-    if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CU(e);
-    (void)cudaGetLastError();
-  }
-  ctx->peer_x[peer_rank] = peer->xblk;
-  ctx->peer_x_ipc[peer_rank] = false;
+  if ((rc = enable_peer_access(ctx, peer, "dsgd_xchg_attach"))) return rc;
+  ctx->peer_x[peer_rank].set(peer->xblk, false);
   return DSGD_OK;
 }
 
@@ -1156,29 +1179,25 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
        (kPCons + kPUpd) * 32, (long long)n_per_step, ctx->dim);
   CU(cudaSetDevice(ctx->device));
   if (want_losses) {
-    int rc = ensure_f64(ctx, &ctx->losses, &ctx->losses_cap, n_steps);
+    int rc = ctx->losses.grow(ctx, n_steps, 1024);
     if (rc) return rc;
   }
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
-  if (single && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) {
-    // one worker on one GPU: the whole run of steps is one persistent cooperative kernel
-    return persist_run(ctx, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses : nullptr);
-  }
-  if (fused) {
-    // one worker per GPU, every peer's exchange block mapped: aggregate inside the persistent kernel over NVLink
-    return persist_run_multi(ctx, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses : nullptr);
+  if ((single && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
+    // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
+    // exchange block mapped (fused): the same kernel aggregates over NVLink
+    return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses.p : nullptr);
   }
   for (int64_t s = 0; s < n_steps; ++s) {
     const int32_t *smp = ctx->samples + first + s * n_per_step;
     double *loss_dev = want_losses ? ctx->losses + s : nullptr;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
-      auto *pe = prof_slot(ctx);
-      if (pe) cudaEventRecord(pe->first, ctx->stream);
-      k_rows<true, false><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp, 0,
-                                                                               n_per_step, ctx->w, ctx->g, nullptr, ctx->cnt);
-      if (pe) cudaEventRecord(pe->second, ctx->stream);
+      profiled(ctx, [&] {
+        k_rows<true, false><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp, 0,
+                                                                                 n_per_step, ctx->w, ctx->g, nullptr, ctx->cnt);
+      });
       LAUNCHED();
       k_update<true><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->g, ctx->d, ctx->dim, ctx->lambda, lr, 1.0,
                                                           ctx->scal, ctx->cnt, ctx->partial, (double)n_per_step, loss_dev);
@@ -1188,11 +1207,10 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     int64_t off = 0;
     for (int32_t v = 0; v < ctx->n_local; ++v) {
       const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
-      auto *pe = prof_slot(ctx);
-      if (pe) cudaEventRecord(pe->first, ctx->stream);
-      k_rows<true, false><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0, nv,
-                                                                       ctx->w, ctx->g, nullptr, ctx->cnt);
-      if (pe) cudaEventRecord(pe->second, ctx->stream);
+      profiled(ctx, [&] {
+        k_rows<true, false><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0, nv,
+                                                                         ctx->w, ctx->g, nullptr, ctx->cnt);
+      });
       LAUNCHED();
       k_finish_acc<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt, (double)nv,
                                                         v == 0 ? 1 : 0);
@@ -1212,7 +1230,7 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
 
 extern "C" int dsgd_read_losses(dsgd_ctx *ctx, double *losses_out, int64_t n_steps) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(losses_out && n_steps >= 0 && n_steps <= ctx->losses_cap, DSGD_ERR_INVALID, "dsgd_read_losses: bad arguments");
+  NEED(losses_out && n_steps >= 0 && n_steps <= ctx->losses.cap, DSGD_ERR_INVALID, "dsgd_read_losses: bad arguments");
   CU(cudaSetDevice(ctx->device));
   if (n_steps)
     CU(cudaMemcpyAsync(losses_out, ctx->losses, sizeof(double) * (size_t)n_steps, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1240,23 +1258,13 @@ extern "C" int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, 
 
 // ---- async (Hogwild) mode -------------------------------------------------------------------------------------
 
-static int ensure_dev(dsgd_ctx *ctx, void **buf, int64_t *cap, int64_t n, size_t elt) {
-  if (*cap >= n) return DSGD_OK;
-  if (*buf) CU(cudaFree(*buf));
-  *buf = nullptr; *cap = 0;
-  const int64_t want = std::max<int64_t>(n, 1024);
-  CU(cudaMalloc(buf, elt * (size_t)want));
-  *cap = want;
-  return DSGD_OK;
-}
-
 extern "C" int dsgd_async_host_master(dsgd_ctx *ctx, const double *w0) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot host the async master replica: ctx is in synchronous mode.");
   NEED(w0, DSGD_ERR_INVALID, "dsgd_async_host_master: w0 is NULL");
   NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_async_host_master: dimSparsity not set");
   CU(cudaSetDevice(ctx->device));
-  if (!ctx->m_w) CU(cudaMalloc(&ctx->m_w, sizeof(double) * (size_t)(ctx->dim + kReplicaPad)));
+  if (!ctx->m_w) CU(ctx->m_w.alloc((int64_t)ctx->dim + kReplicaPad));
   CU(cudaMemsetAsync(ctx->m_w, 0, sizeof(double) * (size_t)(ctx->dim + kReplicaPad), ctx->stream));
   CU(cudaMemcpyAsync(ctx->m_w, w0, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
   k_async_init_ctl<1024><<<1, 1024, 0, ctx->stream>>>(ctx->m_w, ctx->d, ctx->dim);
@@ -1273,7 +1281,7 @@ extern "C" int dsgd_ipc_export(dsgd_ctx *ctx, int which, uint8_t handle[DSGD_IPC
   NEED(which == DSGD_REPLICA_SELF || ctx->m_w, DSGD_ERR_STATE, "dsgd_ipc_export: this ctx does not host the master replica");
   CU(cudaSetDevice(ctx->device));
   cudaIpcMemHandle_t h;
-  CU(cudaIpcGetMemHandle(&h, which == DSGD_REPLICA_SELF ? ctx->w : ctx->m_w));
+  CU(cudaIpcGetMemHandle(&h, which == DSGD_REPLICA_SELF ? ctx->w.p : ctx->m_w.p));
   memcpy(handle, &h, sizeof h);
   return DSGD_OK;
 }
@@ -1285,14 +1293,7 @@ extern "C" int dsgd_ipc_import(dsgd_ctx *ctx, int peer_rank, const uint8_t handl
   NEED(peer_rank != ctx->rank, DSGD_ERR_INVALID, "dsgd_ipc_import: a worker does not import its own replica");
   NEED(!ctx->a_running, DSGD_ERR_STATE, "dsgd_ipc_import: async computation is running");
   CU(cudaSetDevice(ctx->device));
-  cudaIpcMemHandle_t h;
-  memcpy(&h, handle, sizeof h);
-  void *ptr = nullptr;
-  CU(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-  if (ctx->peer_w[peer_rank] && ctx->peer_ipc[peer_rank]) cudaIpcCloseMemHandle(ctx->peer_w[peer_rank]);
-  ctx->peer_w[peer_rank] = static_cast<double *>(ptr);
-  ctx->peer_ipc[peer_rank] = true;
-  return DSGD_OK;
+  return open_ipc(ctx, ctx->peer_w[peer_rank], handle);
 }
 
 extern "C" int dsgd_peer_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer, int which) {
@@ -1301,18 +1302,14 @@ extern "C" int dsgd_peer_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer, in
        "dsgd_peer_attach: peer_rank %d outside [0,%d]", peer_rank, ctx->world);
   NEED(which == DSGD_REPLICA_SELF || peer->m_w, DSGD_ERR_STATE, "dsgd_peer_attach: peer does not host the master replica");
   NEED(peer->dim == ctx->dim, DSGD_ERR_INVALID, "dsgd_peer_attach: dimension mismatch");
-  CU(cudaSetDevice(ctx->device));
-  if (peer->device != ctx->device) {
-    int can = 0;
-    CU(cudaDeviceCanAccessPeer(&can, ctx->device, peer->device));
-    NEED(can, DSGD_ERR_CUDA, "dsgd_peer_attach: device %d cannot access device %d", ctx->device, peer->device);
-    cudaError_t e = cudaDeviceEnablePeerAccess(peer->device, 0);
-    if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CU(e);
-    (void)cudaGetLastError();
-  }
-  ctx->peer_w[peer_rank] = which == DSGD_REPLICA_SELF ? peer->w : peer->m_w;
-  ctx->peer_ipc[peer_rank] = false;
+  int rc = enable_peer_access(ctx, peer, "dsgd_peer_attach");
+  if (rc) return rc;
+  ctx->peer_w[peer_rank].set(which == DSGD_REPLICA_SELF ? peer->w.p : peer->m_w.p, false);
   return DSGD_OK;
+}
+
+static double *master_replica(dsgd_ctx *ctx) {
+  return ctx->m_w ? ctx->m_w.p : (ctx->world < kMaxReplicas ? ctx->peer_w[ctx->world].p : nullptr);
 }
 
 static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned, int64_t n_assigned, const int32_t *replay,
@@ -1329,14 +1326,8 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
     rc = refresh_resident(ctx);  // also S = w . d and the control slots of the replica
     if (rc) return rc;
   }  // else: keep the resident replica (already initialised; deltas peers pushed since then must survive)
-  if (ctx->a_scratch_lanes < lanes) {
-    if (ctx->a_scratch) CU(cudaFree(ctx->a_scratch));
-    ctx->a_scratch = nullptr; ctx->a_scratch_lanes = 0;
-    CU(cudaMalloc(&ctx->a_scratch, sizeof(double) * (size_t)lanes * (size_t)ctx->dim));
-    CU(cudaMemsetAsync(ctx->a_scratch, 0, sizeof(double) * (size_t)lanes * (size_t)ctx->dim, ctx->stream));
-    ctx->a_scratch_lanes = lanes;
-  }
-  if ((rc = ensure_dev(ctx, (void **)&ctx->a_rows, &ctx->a_rows_cap, (int64_t)lanes * batch, sizeof(int32_t)))) return rc;
+  if ((rc = ctx->a_scratch.grow(ctx, (int64_t)lanes * ctx->dim, 1, true))) return rc;
+  if ((rc = ctx->a_rows.grow(ctx, (int64_t)lanes * batch, 1024))) return rc;
   CU(cudaMemsetAsync(ctx->a_stop, 0, sizeof(int), ctx->stream));
   CU(cudaMemsetAsync(ctx->a_cnt, 0, sizeof(unsigned long long) * 2, ctx->stream));
   AsyncParams ap;
@@ -1347,8 +1338,7 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   for (int r = 0; r < ctx->world && r < kMaxReplicas - 1; ++r)
     if (r != ctx->rank && ctx->peer_w[r]) ap.replica[nr++] = ctx->peer_w[r];
   ap.master_slot = -1;
-  double *master = ctx->m_w ? ctx->m_w : (ctx->world < kMaxReplicas ? ctx->peer_w[ctx->world] : nullptr);
-  if (master) { ap.master_slot = nr; ap.replica[nr++] = master; }
+  if (double *master = master_replica(ctx)) { ap.master_slot = nr; ap.replica[nr++] = master; }
   if (ctx->outbox) {   // colleagues reached over the host: one more target of every delta, relayed by the host in batches
     NEED(nr < kMaxReplicas, DSGD_ERR_INVALID, "dsgd_start_async: no replica slot left for the outbox");
     ap.replica[nr++] = ctx->outbox;
@@ -1358,7 +1348,7 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   ap.scratch = ctx->a_scratch; ap.batch_rows = ctx->a_rows; ap.n_lanes = lanes; ap.max_updates = max_updates; ap.seed = seed;
   ap.stop = ctx->a_stop; ap.claimed = ctx->a_cnt; ap.done = ctx->a_cnt + 1;
   CU(cudaStreamSynchronize(ctx->stream));  // inputs in place before the loop's own stream starts
-  if (!ctx->a_ev0) { CU(cudaEventCreate(&ctx->a_ev0)); CU(cudaEventCreate(&ctx->a_ev1)); }
+  if (!ctx->a_ev0) { CU(cudaEventCreate(&ctx->a_ev0.h)); CU(cudaEventCreate(&ctx->a_ev1.h)); }
   CU(cudaEventRecord(ctx->a_ev0, st));
   // batch 1: the delta of every non-zero is formed straight from the pair, without the per-lane scratch vector
   if (batch == 1) k_async_worker_b1<<<cdiv(lanes, 4), 128, 0, st>>>(ap);
@@ -1375,12 +1365,10 @@ extern "C" int dsgd_start_async(dsgd_ctx *ctx, const double *w0, const int32_t *
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot initialize async computation: slave is in synchronous mode.");
   NEED(assigned && n_assigned >= 1, DSGD_ERR_EMPTY, "dsgd_start_async: no samples assigned (Random.nextInt(0) throws)");
   NEED(n_assigned <= ctx->n_rows, DSGD_ERR_RANGE, "dsgd_start_async: more assigned samples than rows");
-  for (int64_t i = 0; i < n_assigned; ++i)
-    NEED(assigned[i] >= 0 && assigned[i] < ctx->n_rows, DSGD_ERR_RANGE, "assigned sample %d at position %lld outside [0,%lld)",
-         assigned[i], (long long)i, (long long)ctx->n_rows);
-  CU(cudaSetDevice(ctx->device));
-  int rc = ensure_dev(ctx, (void **)&ctx->a_assigned, &ctx->a_assigned_cap, n_assigned, sizeof(int32_t));
+  int rc = check_ids(ctx, assigned, n_assigned, "assigned sample");
   if (rc) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->a_assigned.grow(ctx, n_assigned, 1024))) return rc;
   CU(cudaMemcpyAsync(ctx->a_assigned, assigned, sizeof(int32_t) * (size_t)n_assigned, cudaMemcpyHostToDevice, ctx->stream));
   if (batch > n_assigned) batch = (int32_t)n_assigned;  // `take batchSize` of a shorter shuffle
   rc = async_launch(ctx, w0, ctx->a_assigned, n_assigned, nullptr, batch, lr, concurrency, max_updates, seed, ctx->astream);
@@ -1395,12 +1383,10 @@ extern "C" int dsgd_async_replay(dsgd_ctx *ctx, const double *w0, const int32_t 
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot initialize async computation: slave is in synchronous mode.");
   NEED(samples && batch >= 1 && n_updates >= 1, DSGD_ERR_EMPTY, "dsgd_async_replay: empty sequence");
   const int64_t n = (int64_t)batch * n_updates;
-  for (int64_t i = 0; i < n; ++i)
-    NEED(samples[i] >= 0 && samples[i] < ctx->n_rows, DSGD_ERR_RANGE, "sample index %d at position %lld outside [0,%lld)",
-         samples[i], (long long)i, (long long)ctx->n_rows);
-  CU(cudaSetDevice(ctx->device));
-  int rc = ensure_dev(ctx, (void **)&ctx->a_replay, &ctx->a_replay_cap, n, sizeof(int32_t));
+  int rc = check_ids(ctx, samples, n, "sample index");
   if (rc) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->a_replay.grow(ctx, n, 1024))) return rc;
   CU(cudaMemcpyAsync(ctx->a_replay, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   rc = async_launch(ctx, w0, nullptr, 1, ctx->a_replay, batch, lr, 1, n_updates, 0, ctx->stream);
   if (rc) return rc;
@@ -1434,10 +1420,8 @@ extern "C" int dsgd_stop_async(dsgd_ctx *ctx) {
   CU(cudaStreamSynchronize(ctx->stream2));
   CU(cudaStreamSynchronize(ctx->astream));
   ctx->a_running = false;
-  k_prepare<1024><<<1, 1024, 0, ctx->stream>>>(ctx->w, ctx->d, ctx->dim, ctx->lambda, ctx->scal + kScalC, ctx->scal + kScalNrm2);
-  LAUNCHED();
-  k_to_f32<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->dim);
-  LAUNCHED();
+  // not refresh_resident: its k_async_init_ctl would zero the update counter the loop just advanced
+  launch_prepare(ctx, ctx->w, ctx->w32, kScalC, kScalNrm2);
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream));
   return DSGD_OK;
@@ -1463,15 +1447,9 @@ extern "C" int dsgd_update_grad(dsgd_ctx *ctx, const int32_t *idx, const double 
     NEED(idx[k] >= 0 && idx[k] < ctx->dim, DSGD_ERR_RANGE, "dsgd_update_grad: key %d outside [0,%d)", idx[k], ctx->dim);
   if (nnz == 0) return DSGD_OK;
   CU(cudaSetDevice(ctx->device));
-  if (ctx->u_cap < nnz) {
-    if (ctx->u_idx) CU(cudaFree(ctx->u_idx));
-    if (ctx->u_val) CU(cudaFree(ctx->u_val));
-    ctx->u_idx = nullptr; ctx->u_val = nullptr; ctx->u_cap = 0;
-    const int64_t want = std::max<int64_t>(nnz, 4096);
-    CU(cudaMalloc(&ctx->u_idx, sizeof(int32_t) * (size_t)want));
-    CU(cudaMalloc(&ctx->u_val, sizeof(double) * (size_t)want));
-    ctx->u_cap = want;
-  }
+  int rc = ctx->u_idx.grow(ctx, nnz, 4096);
+  if (rc) return rc;
+  if ((rc = ctx->u_val.grow(ctx, nnz, 4096))) return rc;
   CU(cudaMemcpyAsync(ctx->u_idx, idx, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, ctx->stream2));
   CU(cudaMemcpyAsync(ctx->u_val, val, sizeof(double) * (size_t)nnz, cudaMemcpyHostToDevice, ctx->stream2));
   k_async_apply_delta<<<std::min(cdiv(nnz, 256), 64), 256, 0, ctx->stream2>>>(ctx->w, ctx->dim, ctx->d, ctx->u_idx, ctx->u_val, nnz, 0);
@@ -1479,10 +1457,6 @@ extern "C" int dsgd_update_grad(dsgd_ctx *ctx, const int32_t *idx, const double 
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(ctx->stream2));
   return DSGD_OK;
-}
-
-static double *master_replica(dsgd_ctx *ctx) {
-  return ctx->m_w ? ctx->m_w : (ctx->world < kMaxReplicas ? ctx->peer_w[ctx->world] : nullptr);
 }
 
 extern "C" int dsgd_async_updates(dsgd_ctx *ctx, int64_t *count) {
@@ -1503,7 +1477,7 @@ extern "C" int dsgd_async_outbox_enable(dsgd_ctx *ctx) {
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "dsgd_async_outbox_enable: ctx is in synchronous mode");
   NEED(!ctx->a_running, DSGD_ERR_STATE, "dsgd_async_outbox_enable: async computation is running");
   CU(cudaSetDevice(ctx->device));
-  if (!ctx->outbox) CU(cudaMalloc(&ctx->outbox, sizeof(double) * (size_t)(ctx->dim + kReplicaPad)));
+  if (!ctx->outbox) CU(ctx->outbox.alloc((int64_t)ctx->dim + kReplicaPad));
   CU(cudaMemsetAsync(ctx->outbox, 0, sizeof(double) * (size_t)(ctx->dim + kReplicaPad), ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return DSGD_OK;
