@@ -9,12 +9,13 @@ control flow over a handful of scalars per epoch (losses, accuracies, the stoppi
 """
 from __future__ import annotations
 
-from typing import Callable, List, Optional, Sequence
+from typing import Callable, List, Optional, Sequence, Union
 
 import numpy as np
 
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
 from ..ml.grad_state import GradState
+from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
 from ..utils.dataset import Data
@@ -91,10 +92,12 @@ class EpochDraw(list):
 class Master:
     """core/Master.scala:19-255 (abstract).  `Master.apply` (Master.scala:259-271) is `Master.create`."""
 
-    def __init__(self, node: int, data: Data, test_data: Data, model: SparseSVM, expected_node_count: int, *,
+    def __init__(self, node: int, data: Data, test_data: Data, model: Union[SparseSVM, SparseLogistic],
+                 expected_node_count: int, *,
                  slave: Slave, group: Optional[Group] = None, seed: int = 0, log: Optional[Callable[[str], None]] = None,
                  jvm_exact: bool = False, attach: bool = True):
         self.node, self.model, self.expected_node_count = node, model, expected_node_count
+        self.logistic = isinstance(model, SparseLogistic)
         self.n_train, self.n_test = data.n_rows, test_data.n_rows
         self.dim = data.dim
         self.slave = slave
@@ -131,17 +134,35 @@ class Master:
         return (MasterAsync if is_async else MasterSync)(node, data, test_data, model, node_count, **kw)
 
     # ---- evaluation ------------------------------------------------------------------------------------
+    def _local_eval(self, call: str, *args):
+        """(loss sum, correct count, ||w||^2) of this rank's share: ctx.<call>_counts for the SVM (its loss sum is the
+        integer hinge sum), ctx.<call>_sums for SparseLogistic."""
+        return getattr(self.ctx, call + ("_sums" if self.logistic else "_counts"))(*args)
+
+    def _combine(self, h, c, n2, *rows):
+        """(loss sum, correct[, rows], ||w||^2) over all ranks; ||w||^2 is identical on every rank that evaluated and 0 on idle
+        ranks: its maximum.  SVM: the sums are integers below 2^53, exact in any order (all-reduce).  Logistic: the loss
+        sums are not integers, so the partials are gathered and added in rank order and every rank gets the same bits --
+        ranks whose stopping rule saw different losses would leave `fit` at different epochs and hang the next collective."""
+        if not self.logistic:
+            return (*self.group.all_reduce_sum([h, c, *rows]), self.group.all_reduce_max(n2))
+        mine = np.array([h, c, *rows, n2], dtype=np.float64)
+        parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
+        sums = [0.0] * (mine.size - 1)
+        for p in parts:
+            sums = [s + float(v) for s, v in zip(sums, p[:-1])]
+        return (*sums, max(float(p[-1]) for p in parts))
+
     def _eval_rows(self, weights, begin: int, end: int):
-        """Row-sharded pass: each rank evaluates a contiguous share, integer counters are summed."""
+        """Row-sharded pass: each rank evaluates a contiguous share, the loss sums and counters are summed."""
         W, r = self.group.world, self.group.rank
         n = end - begin
         lo, hi = begin + (n * r) // W, begin + (n * (r + 1)) // W
         if hi > lo:
-            h, c, n2 = self.ctx.eval_counts(lo, hi, weights)
+            h, c, n2 = self._local_eval("eval", lo, hi, weights)
         else:
             h, c, n2 = 0, 0, 0.0
-        hs, cs = self.group.all_reduce_sum([h, c])
-        n2 = self.group.all_reduce_max(n2)  # identical on every rank that evaluated; 0 on idle ranks
+        hs, cs, n2 = self._combine(h, c, n2)
         return self.model.lam * n2 + hs / n, cs / n
 
     def local_loss(self, weights=None, test_data: bool = False) -> float:
@@ -163,7 +184,7 @@ class Master:
         Every call draws anew, as every reference call reshuffles.  Default: the sample is drawn on the device with
         sampled_key(seed, t), t counting this Master's draws (the epoch draws of `fit` are separate).  jvm_exact: the ids are
         `Random.shuffle(indices) take k` from the java.util.Random stream `fit` also draws from.  Rank r of W evaluates
-        positions sample_shard(k, W, r); the integer counters are summed over ranks."""
+        positions sample_shard(k, W, r); the loss sums and counters are summed over ranks."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         n = e - b
         k = min(int(samples_count), n)
@@ -180,11 +201,10 @@ class Master:
         if hi <= lo:
             h, c, n2 = 0, 0, 0.0
         elif ids is None:
-            h, c, n2 = self.ctx.eval_sampled_counts(b, e, key, lo, hi, weights)
+            h, c, n2 = self._local_eval("eval_sampled", b, e, key, lo, hi, weights)
         else:
-            h, c, n2 = self.ctx.eval_samples_counts(ids[lo:hi], weights)
-        hs, cs = self.group.all_reduce_sum([h, c])
-        n2 = self.group.all_reduce_max(n2)  # identical on every rank that evaluated; 0 on idle ranks
+            h, c, n2 = self._local_eval("eval_samples", ids[lo:hi], weights)
+        hs, cs, n2 = self._combine(h, c, n2)
         return self.model.lam * n2 + hs / k, cs / k
 
     def local_sampled_loss(self, weights, samples_count: int, test_data: bool = False) -> float:
@@ -232,11 +252,10 @@ class Master:
         groups = split_strategy(self.n_train, self.group.world)
         mine = groups[self.group.rank] if self.group.rank < len(groups) else range(0)
         if len(mine):
-            h, c, n2 = self.ctx.eval_counts(mine.start, mine.stop, weights)
+            h, c, n2 = self._local_eval("eval", mine.start, mine.stop, weights)
         else:
             h, c, n2 = 0, 0, 0.0
-        hs, cs, ns = self.group.all_reduce_sum([h, c, len(mine)])
-        n2 = self.group.all_reduce_max(n2)
+        hs, cs, ns, n2 = self._combine(h, c, n2, len(mine))
         return self.model.lam * n2 + hs / ns, cs / ns
 
 
@@ -347,7 +366,12 @@ class MasterAsync(Master):
     """core/MasterAsync.scala -- Hogwild: every worker runs its loop on its GPU and pushes deltas into every peer
     replica and into the master replica (hosted on rank 0's GPU) over NVLink; the master logic polls the update
     counter, evaluates the master replica on the test rows every `check_every` updates with a leaky average, keeps
-    the best weights, and stops on `n_train * max_epoch` updates or the early-stopping rule."""
+    the best weights, and stops on `n_train * max_epoch` updates or the early-stopping rule.  SparseSVM only."""
+
+    def __init__(self, node, data, test_data, model, expected_node_count, **kw):
+        if isinstance(model, SparseLogistic):
+            raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
+        super().__init__(node, data, test_data, model, expected_node_count, **kw)
 
     def _attach_replicas(self):
         from ..native import REPLICA_MASTER, REPLICA_SELF

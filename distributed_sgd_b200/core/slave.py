@@ -7,17 +7,18 @@ library through the C ABI; there is no arithmetic in this file.
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Union
 
 import numpy as np
 
+from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import NativeCtx
 from ..utils.dataset import Data
 
 
 class Slave:
-    def __init__(self, node: int, master: int, data: Data, model: SparseSVM, is_async: bool = False, *,
+    def __init__(self, node: int, master: int, data: Data, model: Union[SparseSVM, SparseLogistic], is_async: bool = False, *,
                  world: int = 1, device: Optional[int] = None, test_data: Optional[Data] = None,
                  ctx: Optional[NativeCtx] = None):
         """`new Slave(node, master, data, model, async)` (core/Slave.scala:20; Main.scala:138,149).
@@ -27,7 +28,11 @@ class Slave:
         Q13).  test_data (extension): rows appended after the training rows so the same device context can
         serve Master.localLoss(testData) -- they are never sampled.  ctx (extension): a device context that already
         holds exactly these rows (train rows followed by the test rows) and its dimSparsity.
+        model: SparseSVM, or SparseLogistic (sync mode only).
         """
+        logistic = isinstance(model, SparseLogistic)
+        if logistic and is_async:
+            raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
         self.node, self.master, self.model, self.is_async, self.world = node, master, model, is_async, world
         self.n_train = data.n_rows
         self.n_test = test_data.n_rows if test_data is not None else 0
@@ -35,12 +40,14 @@ class Slave:
         if ctx is not None:
             if ctx.n_rows != self.n_train + self.n_test or ctx.dim != data.dim:
                 raise ValueError("Slave: the given device context does not hold these rows")
+            if getattr(ctx, "logistic", False) != logistic:
+                raise ValueError("Slave: the given device context was created for another model")
             self.ctx = ctx
             if model.dim_sparsity is None:
                 model.dim_sparsity = ctx.compute_dim_sparsity(self.n_train)
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
-                             is_async=is_async)
+                             is_async=is_async, logistic=logistic)
         if test_data is not None:
             row_ptr = np.concatenate([data.row_ptr, test_data.row_ptr[1:] + data.row_ptr[-1]])
             col = np.concatenate([data.col[:data.nnz], test_data.col[:test_data.nnz]])

@@ -275,6 +275,8 @@ static void profiled(dsgd_ctx *ctx, F &&launch) {
 
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
+
 // every id names a loaded row (the reference indexes its data array with it)
 static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *what) {
   for (int64_t i = 0; i < n; ++i)
@@ -292,6 +294,8 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
   if (dim <= 0) return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: dim must be positive (got %d)", dim);
   if (world <= 0 || rank < 0 || rank >= world)
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: bad rank/world %d/%d", rank, world);
+  if ((flags & DSGD_FLAG_LOGISTIC) && (flags & DSGD_FLAG_ASYNC))
+    return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports the SVM model only");
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
   if (e != cudaSuccess || n_dev == 0)
@@ -372,9 +376,10 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   char buf[512];
   snprintf(buf, sizeof buf,
            "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
-           "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\"}",
+           "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
+           "\"model\": \"%s\"}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
-           (long long)ctx->nnz);
+           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm");
   ctx->info = buf;
   return ctx->info.c_str();
 }
@@ -702,16 +707,27 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
   const double *wd, *cd, *nd;
   const float *w32d;
   if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  if (stream_eligible(ctx, n)) {
+  const bool logistic = is_logistic(ctx);
+  if (logistic) {
+    k_rows_logistic<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->samples, 0, n,
+                                                                      wd, ctx->g, ctx->cnt);
+    LAUNCHED();
+  } else if (stream_eligible(ctx, n)) {
     if ((rc = stream_launch<true, false, false>(ctx, ctx->samples, 0, n, wd, w32d, ctx->g, nullptr))) return rc;
   } else {
     k_rows<true, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->samples, 0, n,
                                                                     wd, ctx->g, nullptr, ctx->cnt);
     LAUNCHED();
   }
-  k_finish<<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, cd, ctx->cnt, (double)n);
+  const int fin_blocks = cdiv(ctx->dim + 1, 256);
+  if (logistic) {
+    k_finish_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, cd, ctx->cnt, (double)n);
+    k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
+  } else {
+    k_finish<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, cd, ctx->cnt, (double)n);
+    k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
+  }
   LAUNCHED();
-  k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(grad_out, ctx->g, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
@@ -724,14 +740,18 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
 }
 
 // One evaluation pass over rows [row_begin, row_begin + n) (ids == nullptr) or over the n row ids at the device address
-// `ids`, then the shared tail: out = {loss, accuracy, hinge sum, correct count, ||w||^2}, and the counters cleared for the
-// next pass (k_loss_scalar).
+// `ids`, then the shared tail: out = {loss, accuracy, loss sum, correct count, ||w||^2}, and the counters cleared for the
+// next pass (k_loss_scalar).  The SVM's loss sum is the hinge sum, an integer.
 static int eval_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t row_begin, int64_t n, double out[5]) {
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   const float *w32d = nullptr;
   int rc;
   if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  if (stream_eligible(ctx, n)) {
+  if (is_logistic(ctx)) {   // the fp32 streaming pass decides signs only; the logistic loss needs the dot's value
+    k_rows_logistic<false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n,
+                                                                       wd, nullptr, ctx->cnt);
+    LAUNCHED();
+  } else if (stream_eligible(ctx, n)) {
     rc = ids ? stream_launch<false, false, false>(ctx, ids, 0, n, wd, w32d, nullptr, nullptr)
              : stream_launch<false, false, true>(ctx, nullptr, row_begin, n, wd, w32d, nullptr, nullptr);
     if (rc) return rc;
@@ -740,7 +760,8 @@ static int eval_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t
                                                                      wd, nullptr, nullptr, ctx->cnt);
     LAUNCHED();
   }
-  k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
+  if (is_logistic(ctx)) k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
+  else k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
@@ -757,8 +778,20 @@ static int eval_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t 
   return eval_pass(ctx, w, nullptr, row_begin, row_end - row_begin, out);
 }
 
+// the *_counts calls report integer hinge sums, which only the SVM has
+static int counts_model(dsgd_ctx *ctx, const char *fn) {
+  NEED(!is_logistic(ctx), DSGD_ERR_STATE, "%s: the logistic model's loss sum is not an integer; use the *_sums call", fn);
+  return DSGD_OK;
+}
+
 static void put_counts(const double out[5], int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
   if (hinge_sum) *hinge_sum = (int64_t)out[2];
+  if (correct) *correct = (int64_t)out[3];
+  if (norm_squared) *norm_squared = out[4];
+}
+
+static void put_sums(const double out[5], double *loss_sum, int64_t *correct, double *norm_squared) {
+  if (loss_sum) *loss_sum = out[2];
   if (correct) *correct = (int64_t)out[3];
   if (norm_squared) *norm_squared = out[4];
 }
@@ -778,27 +811,33 @@ extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begi
                                 int64_t *correct, double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
   double out[5];
-  int rc = eval_impl(ctx, w, row_begin, row_end, out);
-  if (rc) return rc;
+  int rc = counts_model(ctx, "dsgd_eval_counts");
+  if (rc || (rc = eval_impl(ctx, w, row_begin, row_end, out))) return rc;
   put_counts(out, hinge_sum, correct, norm_squared);
   return DSGD_OK;
 }
 
-extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                        int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
-                                        double *norm_squared) {
+extern "C" int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_sum,
+                              int64_t *correct, double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_sampled_counts: no rows loaded");
+  double out[5];
+  int rc = eval_impl(ctx, w, row_begin, row_end, out);
+  if (rc) return rc;
+  put_sums(out, loss_sum, correct, norm_squared);
+  return DSGD_OK;
+}
+
+static int eval_sampled_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                             int64_t pos_begin, int64_t pos_end, double out[5], const char *fn) {
+  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
   NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
-       "dsgd_eval_sampled_counts: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end,
-       (long long)ctx->n_rows);
+       "%s: rows [%lld,%lld) outside [0,%lld)", fn, (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
   const int64_t n = row_end - row_begin;
-  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_sampled_counts: empty row range");
-  NEED(n <= (int64_t)UINT32_MAX, DSGD_ERR_INVALID, "dsgd_eval_sampled_counts: %lld rows; the draw permutes 32-bit positions",
-       (long long)n);
-  NEED(pos_begin >= 0 && pos_end <= n, DSGD_ERR_INVALID, "dsgd_eval_sampled_counts: positions [%lld,%lld) outside [0,%lld)",
+  NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty row range", fn);
+  NEED(n <= (int64_t)UINT32_MAX, DSGD_ERR_INVALID, "%s: %lld rows; the draw permutes 32-bit positions", fn, (long long)n);
+  NEED(pos_begin >= 0 && pos_end <= n, DSGD_ERR_INVALID, "%s: positions [%lld,%lld) outside [0,%lld)", fn,
        (long long)pos_begin, (long long)pos_end, (long long)n);
-  NEED(pos_end > pos_begin, DSGD_ERR_EMPTY, "dsgd_eval_sampled_counts: no positions (reduce on an empty collection throws)");
+  NEED(pos_end > pos_begin, DSGD_ERR_EMPTY, "%s: no positions (reduce on an empty collection throws)", fn);
   CU(cudaSetDevice(ctx->device));
   const int64_t k = pos_end - pos_begin;
   int rc = ctx->eval_ids.grow(ctx, k, 1024);
@@ -807,26 +846,62 @@ extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t 
                                                       dsgd_feistel_half_bits((uint64_t)n), key, (uint32_t)n, row_begin);
   LAUNCHED();
   CU(cudaGetLastError());
+  return eval_pass(ctx, w, ctx->eval_ids, 0, k, out);
+}
+
+extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                        int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
+                                        double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
   double out[5];
-  if ((rc = eval_pass(ctx, w, ctx->eval_ids, 0, k, out))) return rc;
+  int rc = counts_model(ctx, "dsgd_eval_sampled_counts");
+  if (rc || (rc = eval_sampled_impl(ctx, w, row_begin, row_end, key, pos_begin, pos_end, out, "dsgd_eval_sampled_counts")))
+    return rc;
   put_counts(out, hinge_sum, correct, norm_squared);
   return DSGD_OK;
 }
 
-extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
-                                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+extern "C" int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                      int64_t pos_begin, int64_t pos_end, double *loss_sum, int64_t *correct,
+                                      double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_samples_counts: no rows loaded");
-  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_eval_samples_counts: bad arguments");
-  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_samples_counts: empty sample (reduce on an empty collection throws)");
+  double out[5];
+  int rc = eval_sampled_impl(ctx, w, row_begin, row_end, key, pos_begin, pos_end, out, "dsgd_eval_sampled_sums");
+  if (rc) return rc;
+  put_sums(out, loss_sum, correct, norm_squared);
+  return DSGD_OK;
+}
+
+static int eval_samples_impl(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double out[5],
+                             const char *fn) {
+  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
+  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "%s: bad arguments", fn);
+  NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty sample (reduce on an empty collection throws)", fn);
   int rc = check_ids(ctx, samples, n, "sample index");
   if (rc) return rc;
   CU(cudaSetDevice(ctx->device));
   if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
   CU(cudaMemcpyAsync(ctx->eval_ids, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  return eval_pass(ctx, w, ctx->eval_ids, 0, n, out);
+}
+
+extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
   double out[5];
-  if ((rc = eval_pass(ctx, w, ctx->eval_ids, 0, n, out))) return rc;
+  int rc = counts_model(ctx, "dsgd_eval_samples_counts");
+  if (rc || (rc = eval_samples_impl(ctx, w, samples, n, out, "dsgd_eval_samples_counts"))) return rc;
   put_counts(out, hinge_sum, correct, norm_squared);
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
+                                      int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  double out[5];
+  int rc = eval_samples_impl(ctx, w, samples, n, out, "dsgd_eval_samples_sums");
+  if (rc) return rc;
+  put_sums(out, loss_sum, correct, norm_squared);
   return DSGD_OK;
 }
 
@@ -1168,7 +1243,11 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
   }
   const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
-  const bool fused = ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
+  // the persistent and fused kernels are SVM-only: a logistic ctx always takes the per-step path below
+  const bool logistic = is_logistic(ctx);
+  NEED(!logistic || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
+       "dsgd_sync_steps: the logistic model takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
+  const bool fused = !logistic && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
                      persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step));
   // Ranks wired with the peer exchange only have no communicator for the step-by-step path below: refuse before anything
   // is launched instead of reaching the allreduce without one.
@@ -1184,7 +1263,7 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
   }
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
-  if ((single && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
+  if ((single && !logistic && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
     // exchange block mapped (fused): the same kernel aggregates over NVLink
     return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses.p : nullptr);
@@ -1194,6 +1273,18 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     double *loss_dev = want_losses ? ctx->losses + s : nullptr;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
+      if (logistic) {
+        profiled(ctx, [&] {
+          k_rows_logistic<true><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp,
+                                                                                      0, n_per_step, ctx->w, ctx->g, ctx->cnt);
+        });
+        LAUNCHED();
+        k_update<true, kLogistic><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->g, ctx->d, ctx->dim, ctx->lambda,
+                                                                       lr, 1.0, ctx->scal, ctx->cnt, ctx->partial,
+                                                                       (double)n_per_step, loss_dev);
+        LAUNCHED();
+        continue;
+      }
       profiled(ctx, [&] {
         k_rows<true, false><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp, 0,
                                                                                  n_per_step, ctx->w, ctx->g, nullptr, ctx->cnt);
@@ -1207,6 +1298,18 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     int64_t off = 0;
     for (int32_t v = 0; v < ctx->n_local; ++v) {
       const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
+      if (logistic) {
+        profiled(ctx, [&] {
+          k_rows_logistic<true><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0,
+                                                                              nv, ctx->w, ctx->g, ctx->cnt);
+        });
+        LAUNCHED();
+        k_finish_acc_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
+                                                                   (double)nv, v == 0 ? 1 : 0);
+        LAUNCHED();
+        off += nv;
+        continue;
+      }
       profiled(ctx, [&] {
         k_rows<true, false><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0, nv,
                                                                          ctx->w, ctx->g, nullptr, ctx->cnt);
@@ -1220,8 +1323,13 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
     if (ctx->world > 1)
       NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    k_update<false><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->gsum, ctx->d, ctx->dim, ctx->lambda, lr,
-                                                         (double)k_total, ctx->scal, ctx->cnt, ctx->partial, 0.0, loss_dev);
+    if (logistic)
+      k_update<false, kLogistic><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->gsum, ctx->d, ctx->dim,
+                                                                      ctx->lambda, lr, (double)k_total, ctx->scal, ctx->cnt,
+                                                                      ctx->partial, 0.0, loss_dev);
+    else
+      k_update<false><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->gsum, ctx->d, ctx->dim, ctx->lambda, lr,
+                                                           (double)k_total, ctx->scal, ctx->cnt, ctx->partial, 0.0, loss_dev);
     LAUNCHED();
   }
   CU(cudaGetLastError());

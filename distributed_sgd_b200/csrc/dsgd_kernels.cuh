@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include "dsgd_feistel.h"
+#include "dsgd_fixed.cuh"
 
 namespace dsgd {
 
@@ -32,8 +33,27 @@ enum Cnt : int {
   kCntHinge = 0,    // sum of per-sample hinge losses of the running batch (integers: 0, 1 or 2 each)
   kCntCorrect = 1,  // #{pred == y}
   kCntTicket = 2,   // last-block ticket of k_update
-  kNumCnt = 8
+  kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
+  kNumCnt = 16
 };
+static_assert(kCntLoss + kLossAccWords <= kNumCnt, "counter block");
+
+// Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
+constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
+constexpr int kLogistic = 1;   // SparseLogistic: softplus loss, gradient x * (y * sigmoid(y * x.w))
+
+// Sum of the per-sample losses of the running batch or pass, and its reset
+template <int kModel>
+__device__ __forceinline__ double batch_loss_sum(const unsigned long long *cnt) {
+  return kModel == kLogistic ? acc_value(cnt + kCntLoss) : (double)cnt[kCntHinge];
+}
+template <int kModel>
+__device__ __forceinline__ void clear_batch_loss(unsigned long long *cnt) {
+  cnt[kCntHinge] = 0ull;
+  if (kModel == kLogistic)
+#pragma unroll
+    for (int i = 0; i < kLossAccWords; ++i) cnt[kCntLoss + i] = 0ull;
+}
 
 __device__ __forceinline__ double filt(double v) { return fabs(v) > kEps ? v : 0.0; }  // Sparse.scala:108-118
 
@@ -154,12 +174,73 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
 }
 
 // ---------------------------------------------------------------------------------------------------
+// SparseLogistic, one sample with z = y * (x . w):  loss softplus(z) = max(z, 0) + log1p(exp(-|z|)),
+// backward x * (y * sigmoid(z)).  Both stable for any z; fp64 exp / log1p (no fast-math intrinsics), the formulas of the
+// oracle.
+// ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double softplus(double z) { return (z > 0.0 ? z : 0.0) + log1p(exp(-fabs(z))); }
+__device__ __forceinline__ double sigmoid(double t) {
+  if (t >= 0.0) return 1.0 / (1.0 + exp(-t));
+  const double e = exp(t);
+  return e / (1.0 + e);
+}
+
+// k_rows_logistic: the per-sample body of a gradient request or an evaluation pass for SparseLogistic.  One warp per row
+// window, fp64 dot with the L2-resident weights (the logistic loss and sigmoid need the dot's value, not only its sign: the
+// fp32 streaming pass of dsgd_stream.cuh is SVM-only).  Lane 0 counts correct predictions and adds softplus(z) to fixed-
+// point limbs in registers, pushed once per warp (dsgd_fixed.cuh): the loss sum does not depend on which warp took which
+// row.  kScatter: every row adds its filtered x * (y * sigmoid(z)) to g with fp64 REDs (no gate: every row contributes).
+// samples == nullptr walks rows [row_begin, row_begin + n).
+// ---------------------------------------------------------------------------------------------------
+template <bool kScatter>
+__global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                       const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                       int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                       double *__restrict__ g, unsigned long long *__restrict__ cnt) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned correct = 0;  // lane 0 only
+  unsigned long long lim[kAccLimbs] = {0, 0, 0, 0, 0}, ovf = 0;
+  for (int64_t i = warp0; i < n; i += nwarps) {
+    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
+    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+    double dot = 0.0;
+    for (int64_t k = b + lane; k < e; k += 32) {
+      const uint2 pr = pairs[k];
+      const double xv = filt((double)__uint_as_float(pr.y));
+      dot += filt(xv * w[pr.x]);  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
+    }
+    dot = warp_sum(dot);
+    const double y = (double)label[r];
+    const double z = y * dot;
+    if (lane == 0) {
+      correct += (unsigned)(pred_of(dot) == (int)y);
+      acc_add_local(lim, ovf, softplus(z));
+    }
+    if (kScatter) {
+      const double s = y * sigmoid(z);
+      for (int64_t k = b + lane; k < e; k += 32) {
+        const uint2 pr = pairs[k];
+        const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);  // x * s: mapValues + constructor filter
+        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
+      }
+    }
+  }
+  if (lane == 0) {
+    if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
+    acc_flush_local(cnt + kCntLoss, lim, ovf);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // k_finish: regularize in place -- r_j = g_j + c on the keys that survived the 1e-20 filter
 // (SparseSVM.scala:31; math/Vec.scala:65-75).  Also publishes the batch's hinge sum and size in
 // g[dim], g[dim+1] so that they ride along in the gradient allreduce.
 // ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
-                                                const unsigned long long *__restrict__ cnt, double n_samples) {
+template <int kModel>
+__device__ __forceinline__ void finish_body(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
+                                            const unsigned long long *__restrict__ cnt, double n_samples) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const double c = *scal_c;
   const bool add_c = (c != 0.0) && (fabs(c) > kEps);
@@ -168,9 +249,17 @@ __global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim,
     if (v != 0.0 && add_c) v = filt(v + c);
     g[j] = v;
   } else if (j == dim) {
-    g[dim] = (double)cnt[kCntHinge];
+    g[dim] = batch_loss_sum<kModel>(cnt);
     g[dim + 1] = n_samples;
   }
+}
+__global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
+                                                const unsigned long long *__restrict__ cnt, double n_samples) {
+  finish_body<kSvm>(g, dim, scal_c, cnt, n_samples);
+}
+__global__ void __launch_bounds__(256) k_finish_logistic(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
+                                                         const unsigned long long *__restrict__ cnt, double n_samples) {
+  finish_body<kLogistic>(g, dim, scal_c, cnt, n_samples);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -179,9 +268,10 @@ __global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim,
 // addition (Vec.sum is a left fold of `+`, math/Vec.scala:128-131), g cleared for the next worker.
 // Slots [dim], [dim+1] of `sum` carry the hinge total and the sample count of the step.
 // ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, double *__restrict__ sum, int dim,
-                                                    const double *__restrict__ scal_c,
-                                                    unsigned long long *__restrict__ cnt, double n_samples, int first) {
+template <int kModel>
+__device__ __forceinline__ void finish_acc_body(double *__restrict__ g, double *__restrict__ sum, int dim,
+                                                const double *__restrict__ scal_c, unsigned long long *__restrict__ cnt,
+                                                double n_samples, int first) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const double c = *scal_c;
   const bool add_c = (c != 0.0) && (fabs(c) > kEps);
@@ -192,12 +282,23 @@ __global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, doub
     if (raw != 0.0) g[j] = 0.0;
     sum[j] = first ? v : filt(sum[j] + v);
   } else if (j == dim) {
-    const double h = (double)cnt[kCntHinge];
+    const double h = batch_loss_sum<kModel>(cnt);
     sum[dim] = first ? h : sum[dim] + h;
     sum[dim + 1] = first ? n_samples : sum[dim + 1] + n_samples;
-    cnt[kCntHinge] = 0ull;
+    clear_batch_loss<kModel>(cnt);
     cnt[kCntCorrect] = 0ull;
   }
+}
+__global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, double *__restrict__ sum, int dim,
+                                                    const double *__restrict__ scal_c,
+                                                    unsigned long long *__restrict__ cnt, double n_samples, int first) {
+  finish_acc_body<kSvm>(g, sum, dim, scal_c, cnt, n_samples, first);
+}
+__global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict__ g, double *__restrict__ sum, int dim,
+                                                             const double *__restrict__ scal_c,
+                                                             unsigned long long *__restrict__ cnt, double n_samples,
+                                                             int first) {
+  finish_acc_body<kLogistic>(g, sum, dim, scal_c, cnt, n_samples, first);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -207,8 +308,9 @@ __global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, doub
 // next step needs no separate reduction; per-step loss = lambda*||w_before||^2 + hinge/total written.
 //   kFuseRegularize: the buffer holds the raw local sum (single worker): apply regularize() here.
 //   otherwise it holds sum_k r^(k) (already regularized per worker, then allreduced).
+//   kModel: where the batch's loss sum comes from (batch_loss_sum).
 // ---------------------------------------------------------------------------------------------------
-template <bool kFuseRegularize>
+template <bool kFuseRegularize, int kModel = kSvm>
 __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32,
                                                 double *__restrict__ g, const double *__restrict__ d, int dim,
                                                 double lambda, double lr, double inv_k_den, double *__restrict__ scal,
@@ -260,7 +362,7 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
       // per-step loss on the weights the gradient was taken at (SparseSVM.scala:20-23; SURVEY.md F5)
       double hinge, total;
       if (kFuseRegularize) {
-        hinge = (double)cnt[kCntHinge];
+        hinge = batch_loss_sum<kModel>(cnt);
         total = n_samples_local;
       } else {
         hinge = g[dim];
@@ -271,7 +373,7 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
       if (loss_out) *loss_out = lambda * scal[kScalNrm2] + hinge / total;
       scal[kScalC] = lambda * 2.0 * sd;
       scal[kScalNrm2] = sn;
-      cnt[kCntHinge] = 0ull;
+      clear_batch_loss<kModel>(cnt);
       cnt[kCntCorrect] = 0ull;
       cnt[kCntTicket] = 0ull;
     }
@@ -279,17 +381,27 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_loss_scalar: loss = lambda*||w||^2 + hinge/n, acc = correct/n from the integer counters.
+// k_loss_scalar: loss = lambda*||w||^2 + loss sum/n, acc = correct/n from the counters (SVM: hinge sum, an integer;
+// logistic: the fixed-point sum of the softplus losses).
 // ---------------------------------------------------------------------------------------------------
-__global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
-                              double lambda, double n, double *__restrict__ out2) {
-  out2[0] = lambda * (*scal_nrm2) + (double)cnt[kCntHinge] / n;
+template <int kModel>
+__device__ __forceinline__ void loss_scalar_body(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
+                                                 double lambda, double n, double *__restrict__ out2) {
+  out2[0] = lambda * (*scal_nrm2) + batch_loss_sum<kModel>(cnt) / n;
   out2[1] = (double)cnt[kCntCorrect] / n;
-  out2[2] = (double)cnt[kCntHinge];   // exact: counts are far below 2^53
+  out2[2] = batch_loss_sum<kModel>(cnt);   // SVM: exact, counts are far below 2^53
   out2[3] = (double)cnt[kCntCorrect];
   out2[4] = *scal_nrm2;
-  cnt[kCntHinge] = 0ull;
+  clear_batch_loss<kModel>(cnt);
   cnt[kCntCorrect] = 0ull;
+}
+__global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
+                              double lambda, double n, double *__restrict__ out2) {
+  loss_scalar_body<kSvm>(scal_nrm2, cnt, lambda, n, out2);
+}
+__global__ void k_loss_scalar_logistic(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
+                                       double lambda, double n, double *__restrict__ out2) {
+  loss_scalar_body<kLogistic>(scal_nrm2, cnt, lambda, n, out2);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -51,6 +51,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dsgd_fixed.cuh"
 #include "dsgd_kernels.cuh"
 
 namespace dsgd {
@@ -222,77 +223,6 @@ __device__ __forceinline__ bool grid_barrier_arrive_wait(unsigned *bar, unsigned
     }
   }
   return ok;
-}
-
-// ---- order-free exact sums of the per-CTA partials -------------------------------------------------------------------
-// A double v with |v| < 2^52 is cut into five integers: |v| = l4 + l3 * 2^-40 + l2 * 2^-80 + l1 * 2^-120 + l0 * 2^-160,
-// l3..l0 in [0, 2^40] (l0 rounded: resolution 2^-160), every cut exact in fp64 arithmetic; negative v contribute the
-// negated limbs.  The limbs of all CTAs are added with 64-bit integer REDs (no overflow while CTAs < 2^8: 2^8 * 2^40 = 2^48)
-// and converted back once.  Five limbs rather than three: at 2^-80 a partial ||W||^2 of weights around 1e-12 lost most of its
-// digits and one of weights around 1e-13 read 0, while the k_update<true> path of larger batches sums in fp64 -- the same
-// weights reported different losses at batch 32 G and 32 G + 1.  2^-160 keeps the relative error of ||W||^2 below 1e-15
-// down to weights around 1e-16.  Zero limbs are not sent, so small partials cost no more REDs than before.
-// One accumulator = 11 x u64 = 88 bytes {sd.l0..l4, sn.l0..l4, overflow count} on its own 128-byte line: every CTA adds ONE
-// partial per step (one same-address RED per CTA and non-zero limb, tools/microbench.cu) and reads the 96 bytes from the
-// line's start back with ONE coalesced request.  (First cut: 8 striped copies read with 16-byte loads = 2 368 requests on
-// 4 lines after every barrier: c arrived later.)
-constexpr int kAccStride = 16;   // u64 words between the three rotating accumulators (128 bytes)
-constexpr int kAccLimbs = 5;
-constexpr int kAccWords = 2 * kAccLimbs + 1;   // 11: {sd limbs, sn limbs, overflow}
-static_assert(kAccWords + 1 <= kAccStride, "acc_read loads the accumulator and one pad word");
-__device__ __forceinline__ void red_add_u64(unsigned long long *p, unsigned long long v) {
-  asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void acc_push_one(unsigned long long *limbs, unsigned long long *ovf, double v) {
-  if (!(fabs(v) < 4503599627370496.0)) {   // 2^52; also NaN / inf: the sum is reported as NaN
-    red_add_u64(ovf, 1ull);
-    return;
-  }
-  const bool neg = v < 0.0;                // negative values add the negated limbs (two's complement wraps)
-  auto put = [&](unsigned long long *dst, double limb) {
-    if (limb != 0.0) {
-      const unsigned long long u = (unsigned long long)(long long)limb;
-      red_add_u64(dst, neg ? (0ull - u) : u);
-    }
-  };
-  // F_i = floor(|v| * 2^(40 i)): scaling by a power of two and floor are exact.  Limb 4 - i is F_i - 2^40 F_(i-1), an
-  // integer below 2^40 and therefore exact too; the lowest limb rounds, at 2^-160.  The limbs are cut side by side rather
-  // than one from the remainder of the other: this runs just before the CTA's arrival at the grid barrier.
-  const double a = fabs(v);
-  double F[kAccLimbs - 1];
-#pragma unroll
-  for (int i = 0; i < kAccLimbs - 1; ++i) F[i] = floor(a * __longlong_as_double((1023ll + 40 * i) << 52));
-  put(limbs + kAccLimbs - 1, F[0]);
-#pragma unroll
-  for (int i = 1; i < kAccLimbs - 1; ++i) put(limbs + kAccLimbs - 1 - i, F[i] - F[i - 1] * 0x1p40);
-  put(limbs + 0, rint(a * 0x1p160) - F[kAccLimbs - 2] * 0x1p40);   // [0, 2^40]
-}
-__device__ __forceinline__ void acc_push(unsigned long long *acc, double sd, double sn) {
-  acc_push_one(acc, acc + 2 * kAccLimbs, sd);
-  acc_push_one(acc + kAccLimbs, acc + 2 * kAccLimbs, sn);
-}
-// Called by a whole warp; all lanes return the two sums (identical in every CTA: integer additions commute).
-__device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane, double &sd, double &sn) {
-  unsigned long long q0 = 0, q1 = 0;
-  if (lane < (kAccWords + 1) / 2)   // 6 lanes x 16 bytes = the 88-byte accumulator (and a pad word) in one request
-    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(q0), "=l"(q1) : "l"(acc + 2 * lane) : "memory");
-  // Word k = 2 lane + h is limb k % 5 of sd (k < 5) or of sn (5 <= k < 10), worth 2^(40 (k % 5) - 160); every limb sum is
-  // below 2^48 in magnitude, so its conversion and scaling are exact.  Each lane adds its own two words first, so the
-  // sums take six shuffles: sd = (limbs 0+1 + limbs 2+3) + limb 4, sn = (limb 0 + limbs 1+2) + limbs 3+4.  Word 10 counts
-  // the partials that could not be summed.
-  auto limb = [](unsigned long long q, int k) {
-    return (double)(long long)q * __longlong_as_double((long long)(1023 - 160 + 40 * (k % kAccLimbs)) << 52);
-  };
-  const double lo = limb(q0, 2 * lane), hi = limb(q1, 2 * lane + 1), pair = lo + hi;
-  const double s01 = __shfl_sync(0xffffffffu, pair, 0), s23 = __shfl_sync(0xffffffffu, pair, 1);
-  const double s4 = __shfl_sync(0xffffffffu, lo, 2), n0 = __shfl_sync(0xffffffffu, hi, 2);
-  const double n12 = __shfl_sync(0xffffffffu, pair, 3), n34 = __shfl_sync(0xffffffffu, pair, 4);
-  sd = (s01 + s23) + s4;
-  sn = (n0 + n12) + n34;
-  if (__any_sync(0xffffffffu, lane == kAccWords / 2 && q0 != 0)) {
-    sd = __longlong_as_double(0x7ff8000000000000ll);
-    sn = sd;
-  }
 }
 
 constexpr int kChunkPairs = 128;             // 4 pairs per lane per chunk

@@ -10,6 +10,9 @@ object DsgdNative {
 
   // every native returns the C ABI's status code; 0 = OK, negative = DSGD_ERR_*  (include/dsgd.h).  Arrays are copied in
   // before and out after the call (Get/Set<Type>ArrayRegion): nothing is pinned while a call blocks on the GPU.
+  // flags: FlagAsync | FlagLogistic (DSGD_FLAG_*); FlagLogistic selects SparseLogistic instead of SparseSVM (sync mode only)
+  final val FlagAsync = 1
+  final val FlagLogistic = 2
   @native def create(device: Int, dim: Int, lambda: Double, rank: Int, world: Int, flags: Int): Long
   @native def destroy(ctx: Long): Int
   @native def lastError(ctx: Long): String
@@ -31,6 +34,14 @@ object DsgdNative {
                                 posEnd: Long, hingeCorrect: Array[Long], normSquared: Array[Double]): Int
   @native def evalSamplesCounts(ctx: Long, w: Array[Double], samples: Array[Int], hingeCorrect: Array[Long],
                                 normSquared: Array[Double]): Int
+  // the same passes for either model (the *Counts forms refuse a logistic ctx): lossSumNormSquared = {sum of the per-sample
+  // losses, ||w||^2}, correct = {#correct}
+  @native def evalSums(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, lossSumNormSquared: Array[Double],
+                       correct: Array[Long]): Int
+  @native def evalSampledSums(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                              posEnd: Long, lossSumNormSquared: Array[Double], correct: Array[Long]): Int
+  @native def evalSamplesSums(ctx: Long, w: Array[Double], samples: Array[Int], lossSumNormSquared: Array[Double],
+                              correct: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

@@ -162,6 +162,47 @@ FN(evalSamplesCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintAr
   free(bw.p); free(bs.p);
   return rc;
 }
+/* The *Sums forms serve either model (the *Counts forms refuse a logistic ctx): lossSumNormSquared(0) = sum of the per-sample
+ * losses, (1) = ||w||^2; correct(0) = #correct. */
+FN(evalSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray lossSumNormSquared,
+             jlongArray correct) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, lossSumNormSquared), bc = out_Long(env, correct);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad))
+    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
+                                : dsgd_eval_sums(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (int64_t *)bc.p, (double *)bs.p + 1);
+  back_Double(env, lossSumNormSquared, bs, rc);
+  back_Long(env, correct, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                    jlong posBegin, jlong posEnd, jdoubleArray lossSumNormSquared, jlongArray correct) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, lossSumNormSquared), bc = out_Long(env, correct);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad))
+    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
+                                : dsgd_eval_sampled_sums(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                         (double *)bs.p, (int64_t *)bc.p, (double *)bs.p + 1);
+  back_Double(env, lossSumNormSquared, bs, rc);
+  back_Long(env, correct, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray lossSumNormSquared,
+                    jlongArray correct) {
+  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, lossSumNormSquared),
+        bc = out_Long(env, correct);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bi.bad | bs.bad | bc.bad))
+    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
+                                : dsgd_eval_samples_sums(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (int64_t *)bc.p,
+                                                         (double *)bs.p + 1);
+  back_Double(env, lossSumNormSquared, bs, rc);
+  back_Long(env, correct, bc, rc);
+  free(bw.p); free(bi.p);
+  return rc;
+}
 
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {

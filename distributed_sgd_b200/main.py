@@ -25,11 +25,14 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
              async_concurrency: int = 64, jvm_exact: bool = False, inspect=None) -> dict:
     """Main.scenario (Main.scala:70-120).  inspect (tests): called as inspect("master", master) once the master exists
     and as inspect("done", (master, state)) before the device context is released."""
-    from . import EarlyStopping, Master, Slave, SparseSVM
+    from . import EarlyStopping, Master, Slave, SparseLogistic, SparseSVM
     from .core import Group
 
+    if cfg.model == "logistic" and cfg.is_async:
+        raise ValueError("model = logistic: asynchronous (Hogwild) training supports the svm model only")
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
-    model = SparseSVM(cfg.lam)                                                 # dimSparsity: computed by the Slave on the device
+    # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
+    model = SparseLogistic(cfg.lam) if cfg.model == "logistic" else SparseSVM(cfg.lam)
     slave = Slave(rank, 0, train, model, cfg.is_async, world=world, device=device, test_data=test)
     master = Master.create(rank, train, test, model, cfg.is_async, cfg.node_count, slave=slave, group=Group(), seed=seed,
                            log=(log if rank == 0 else None), jvm_exact=jvm_exact)
@@ -37,7 +40,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         inspect("master", master)
     w0 = np.zeros(data.dim)                                                    # data(0)._1.zerosLike (Main.scala:74)
     report = {"config": {k: getattr(cfg, k) for k in ("batch_size", "learning_rate", "lam", "node_count", "is_async",
-                                                      "max_epochs", "check_every", "leaky_loss", "patience", "conv_delta")},
+                                                      "max_epochs", "check_every", "leaky_loss", "patience", "conv_delta",
+                                                      "model")},
               "rows": {"train": train.n_rows, "test": test.n_rows}, "world": world}
     report["initial_loss"] = master.distributed_loss(w0)                      # Main.scala:75-76
     report["initial_accuracy"] = master.distributed_accuracy(w0)              # Main.scala:77-78

@@ -22,6 +22,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "dsgd.h")
 UNIQUE_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
 FLAG_ASYNC = 1
+FLAG_LOGISTIC = 2
 REPLICA_SELF, REPLICA_MASTER = 0, 1
 
 OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM, ERR_TIMEOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8
@@ -97,6 +98,9 @@ ABI = {
     "dsgd_eval_counts": [_vp, _vp, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_eval_sampled_counts": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_eval_samples_counts": [_vp, _vp, _vp, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_eval_sums": [_vp, _vp, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_eval_sampled_sums": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_eval_samples_sums": [_vp, _vp, _vp, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -187,13 +191,16 @@ def _arr(a, dtype, n: Optional[int] = None, what: str = "array") -> np.ndarray:
 
 
 class NativeCtx:
-    """One dsgd_ctx == one GPU worker (a reference Slave with its SparseSVM)."""
+    """One dsgd_ctx == one GPU worker (a reference Slave with its SparseSVM, or with a SparseLogistic if `logistic`)."""
 
-    def __init__(self, device: int, dim: int, lam: float, rank: int = 0, world: int = 1, is_async: bool = False):
+    def __init__(self, device: int, dim: int, lam: float, rank: int = 0, world: int = 1, is_async: bool = False,
+                 logistic: bool = False):
         self._l = lib()
         self._h = C.c_void_p()
         self.dim, self.lam, self.rank, self.world, self.device = int(dim), float(lam), int(rank), int(world), int(device)
-        rc = self._l.dsgd_create(C.byref(self._h), device, dim, lam, rank, world, FLAG_ASYNC if is_async else 0)
+        self.logistic = bool(logistic)
+        flags = (FLAG_ASYNC if is_async else 0) | (FLAG_LOGISTIC if logistic else 0)
+        rc = self._l.dsgd_create(C.byref(self._h), device, dim, lam, rank, world, flags)
         if rc != OK:
             msg = (self._l.dsgd_last_error(None) or b"").decode()
             self._h = C.c_void_p()
@@ -332,6 +339,32 @@ class NativeCtx:
         w = self._w(w)
         self._ck(self._l.dsgd_eval_samples_counts(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
                                                   C.byref(n2)))
+        return h.value, c.value, n2.value
+
+    def eval_sums(self, row_begin: int, row_end: int, w=None) -> Tuple[float, int, float]:
+        """(loss sum, correct count, ||w||^2) over rows [row_begin, row_end), for either model (dsgd_eval_sums)."""
+        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_sums(self._h, _ptr(w), row_begin, row_end, C.byref(h), C.byref(c), C.byref(n2)))
+        return h.value, c.value, n2.value
+
+    def eval_sampled_sums(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                          w=None) -> Tuple[float, int, float]:
+        """(loss sum, correct count, ||w||^2) over positions [pos_begin, pos_end) of the device-drawn sample
+        (dsgd_eval_sampled_sums)."""
+        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_sampled_sums(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
+                                                pos_begin, pos_end, C.byref(h), C.byref(c), C.byref(n2)))
+        return h.value, c.value, n2.value
+
+    def eval_samples_sums(self, samples, w=None) -> Tuple[float, int, float]:
+        """(loss sum, correct count, ||w||^2) over a list of row ids; repeats count every time (dsgd_eval_samples_sums)."""
+        samples = _arr(samples, np.int32)
+        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_samples_sums(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
+                                                C.byref(n2)))
         return h.value, c.value, n2.value
 
     # -- sync --

@@ -31,6 +31,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     leaky_loss: float = 0.9
     conv_delta: float = 0.01
     patience: int = 5
+    model: str = "svm"            # extension: "svm" (SparseSVM) or "logistic" (SparseLogistic, sync mode only)
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -42,7 +43,9 @@ _KEYS = {
     "async": ("is_async", "DSGD_ASYNC"), "record": ("record", "DSGD_RECORD"), "max-epochs": ("max_epochs", "DSGD_MAX_EPOCHS"),
     "check-every": ("check_every", "DSGD_CHECK_EVERY"), "leaky-loss": ("leaky_loss", "DSGD_LEAKY_LOSS"),
     "patience": ("patience", "DSGD_PATIENCE"), "conv-delta": ("conv_delta", "DSGD_CONV_DELTA"),
+    "model": ("model", "DSGD_MODEL"),
 }
+MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
 
 
@@ -104,4 +107,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
             raise KeyError(f"unknown key dsgd.{key}")
         field = _KEYS[key][0]
         setattr(cfg, field, _coerce(field, value))
+    if cfg.model not in MODELS:
+        raise ValueError(f"model: expected one of {', '.join(MODELS)}, got {cfg.model!r}")
     return cfg

@@ -52,6 +52,12 @@ extern "C" {
 
 /* dsgd_create flags */
 #define DSGD_FLAG_ASYNC 1u /* the `async` constructor argument of Slave / Master (core/Slave.scala:20) */
+/* The model is SparseLogistic instead of SparseSVM: per-sample loss softplus(z) = log(1 + e^z) and gradient
+ * x * (y * sigmoid(z)), z = y * (x . w); prediction, regularize() and the sync step are the SVM's.  Every call that depends
+ * on the model follows it: dsgd_gradient, dsgd_eval, the dsgd_eval_*_sums calls, the sync steps and their losses.  A logistic
+ * ctx takes the per-step sync path (never the persistent or fused kernel), so world > 1 needs dsgd_comm_init.  Combined with
+ * DSGD_FLAG_ASYNC, dsgd_create fails with DSGD_ERR_INVALID (async mode supports the SVM model only). */
+#define DSGD_FLAG_LOGISTIC 2u
 
 typedef struct dsgd_ctx dsgd_ctx;
 
@@ -152,6 +158,16 @@ int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, 
  * outside the loaded rows -> DSGD_ERR_RANGE before anything is launched.  The staged sample stream is left intact. */
 int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *hinge_sum,
                              int64_t *correct, double *norm_squared);
+/* The three *_counts calls above report the hinge sum as an integer, which only the SVM has: on a DSGD_FLAG_LOGISTIC ctx they
+ * fail with DSGD_ERR_STATE.  The *_sums forms take the same arguments and report the sum of the per-sample losses as a double
+ * instead, for either model (for the SVM, the hinge sum: an exact integer held in a double).  The logistic sum is added in
+ * fixed point on the device, so a pass returns the same bits whatever the order in which its rows are taken. */
+int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_sum, int64_t *correct,
+                   double *norm_squared);
+int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                           int64_t pos_begin, int64_t pos_end, double *loss_sum, int64_t *correct, double *norm_squared);
+int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
+                           int64_t *correct, double *norm_squared);
 
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
