@@ -1,6 +1,8 @@
 // dsgd_fixed.cuh -- order-free exact sums: doubles cut into fixed-point limbs and added as 64-bit integers.
 // Used by the persistent sync kernel (its per-CTA partials of W.d and ||W||^2, dsgd_persistent.cuh) and by the logistic row
-// kernel (the per-sample logistic losses of a batch or an evaluation pass, dsgd_kernels.cuh).
+// kernel (the per-sample logistic losses of a batch or an evaluation pass, dsgd_kernels.cuh).  The loss sum, at the end of
+// this file: resolution 2^-160 per value, within one ulp of the exact sum (exact when that is a double) for any pass of values
+// in [0, 2^52) the ABI accepts, NaN if a value is NaN, infinite or 2^52 or more.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -82,36 +84,49 @@ __device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane
 }
 
 // ---- one sum of many non-negative values (the logistic losses of a pass) -------------------------------------------------
-// Layout: kAccLimbs limb words, then one overflow count.  A thread adds its values' limbs in registers (acc_add_local) and
-// pushes them once (acc_flush_local); the sum has the same bits whatever the grid, the work split or the order of arrival.
-// Limb sums reach n * 2^40 (2^60 for 2^20 values): acc_value propagates the carries in integer arithmetic first, so that
-// every limb it converts is below 2^40 (the top one below 2^52 + n) and the only rounding is that of the final additions.
-constexpr int kLossAccWords = kAccLimbs + 1;
-__device__ __forceinline__ void acc_add_local(unsigned long long (&lim)[kAccLimbs], unsigned long long &ovf, double v) {
-  if (!(v >= 0.0 && v < 4503599627370496.0)) { ++ovf; return; }   // NaN, inf, >= 2^52 (or negative): reported as NaN
-  acc_cut(v, [&](int k, double limb) { lim[k] += (unsigned long long)(long long)limb; });
+// Each value v in [0, 2^52) contributes R(v) = rint(v * 2^160) * 2^-160 (acc_cut's limbs, resolution 2^-160: a value below
+// 2^-161 adds exactly 0); NaN, inf and values >= 2^52 are counted instead and the sum reads NaN.  Six limb words, limb k
+// worth 2^(40 k - 160): limbs 0..3 as acc_cut cuts them, the integer part split into limb 4 (its low 40 bits) and limb 5; then
+// one overflow count.  A thread adds its values' limbs in registers (acc_add_local) and propagates the carries after every
+// value, so that limbs 0..4 stay below 2^40 and limb 5 grows by at most 2^13 per value; it pushes them once
+// (acc_flush_local).  The words then hold below warps * 2^40 (limbs 0..4) and n * 2^13 (limb 5): no u64 wraps for any grid
+// of fewer than 2^24 warps and any n below 2^50, far beyond what fits on a device.  Integer additions commute, so the sum has
+// the same bits whatever the grid, the work split or the order of arrival; acc_value propagates the carries once more and
+// converts the limbs from the top down: the result is within one ulp of the exact sum of the R(v), and equal to it whenever
+// that sum is a double (every partial sum is then a prefix of its bits).
+constexpr int kLossLimbs = kAccLimbs + 1;
+constexpr int kLossAccWords = kLossLimbs + 1;   // 7: {limbs 0..5, overflow}
+constexpr unsigned long long kLimbMask = (1ull << 40) - 1;
+__device__ __forceinline__ void acc_carry(unsigned long long (&q)[kLossLimbs]) {
+#pragma unroll
+  for (int i = 0; i < kLossLimbs - 1; ++i) {   // limbs 0..4 into [0, 2^40)
+    q[i + 1] += q[i] >> 40;
+    q[i] &= kLimbMask;
+  }
 }
-__device__ __forceinline__ void acc_flush_local(unsigned long long *acc, const unsigned long long (&lim)[kAccLimbs],
+__device__ __forceinline__ void acc_add_local(unsigned long long (&lim)[kLossLimbs], unsigned long long &ovf, double v) {
+  if (!(v >= 0.0 && v < 4503599627370496.0)) { ++ovf; return; }   // NaN, inf, >= 2^52 (or negative): reported as NaN
+  // limbs 0..3 below 2^40 + 1, limb 4 (the integer part) below 2^52: no register passes 2^53 before the carries
+  acc_cut(v, [&](int k, double limb) { lim[k] += (unsigned long long)(long long)limb; });
+  acc_carry(lim);
+}
+__device__ __forceinline__ void acc_flush_local(unsigned long long *acc, const unsigned long long (&lim)[kLossLimbs],
                                                 unsigned long long ovf) {
 #pragma unroll
-  for (int i = 0; i < kAccLimbs; ++i)
+  for (int i = 0; i < kLossLimbs; ++i)
     if (lim[i]) red_add_u64(acc + i, lim[i]);
-  if (ovf) red_add_u64(acc + kAccLimbs, ovf);
+  if (ovf) red_add_u64(acc + kLossLimbs, ovf);
 }
 // One thread: the value of a kLossAccWords accumulator.
 __device__ __forceinline__ double acc_value(const unsigned long long *acc) {
-  if (acc[kAccLimbs] != 0ull) return __longlong_as_double(0x7ff8000000000000ll);
-  unsigned long long q[kAccLimbs];
+  if (acc[kLossLimbs] != 0ull) return __longlong_as_double(0x7ff8000000000000ll);
+  unsigned long long q[kLossLimbs];
 #pragma unroll
-  for (int i = 0; i < kAccLimbs; ++i) q[i] = acc[i];
+  for (int i = 0; i < kLossLimbs; ++i) q[i] = acc[i];
+  acc_carry(q);
+  double s = (double)q[kLossLimbs - 1] * 0x1p40;   // exact while the sum is below 2^93
 #pragma unroll
-  for (int i = 0; i < kAccLimbs - 1; ++i) {   // carries: limbs 0..3 into [0, 2^40)
-    q[i + 1] += q[i] >> 40;
-    q[i] &= (1ull << 40) - 1;
-  }
-  double s = acc_limb(q[kAccLimbs - 1], kAccLimbs - 1);
-#pragma unroll
-  for (int i = kAccLimbs - 2; i >= 0; --i) s += acc_limb(q[i], i);
+  for (int i = kLossLimbs - 2; i >= 0; --i) s += (double)q[i] * __longlong_as_double((long long)(1023 - 160 + 40 * i) << 52);
   return s;
 }
 

@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restric
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned correct = 0;  // lane 0 only
-  unsigned long long lim[kAccLimbs] = {0, 0, 0, 0, 0}, ovf = 0;
+  unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
   for (int64_t i = warp0; i < n; i += nwarps) {
     const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
     const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
