@@ -1120,8 +1120,8 @@ extern "C" int dsgd_xchg_stats(dsgd_ctx *ctx, int64_t *value_words, int64_t *bit
   unsigned long long host[2] = {0, 0};
   if (ctx->x_stats) {
     CU(cudaSetDevice(ctx->device));
+    CU(cudaMemcpyAsync(host, ctx->x_stats, sizeof host, cudaMemcpyDeviceToHost, ctx->stream));   // see persist_check
     CU(cudaStreamSynchronize(ctx->stream));
-    CU(cudaMemcpy(host, ctx->x_stats, sizeof host, cudaMemcpyDeviceToHost));
   }
   if (value_words) *value_words = (int64_t)host[0];
   if (bitmap_words) *bitmap_words = (int64_t)host[1];
@@ -1189,7 +1189,12 @@ extern "C" int dsgd_xchg_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer) {
 static int persist_check(dsgd_ctx *ctx) {  // after a stream sync: did a device-side wait hit its watchdog?
   if (!ctx->p_ready) return DSGD_OK;
   unsigned host[2] = {0, 0};
-  CU(cudaMemcpy(host, ctx->p_bar, sizeof host, cudaMemcpyDeviceToHost));
+  // On this ctx's stream, not the legacy default stream: ranks sharing one GPU each run on their own stream, and a rank
+  // reads this between two launches while a peer's next launch already spins waiting for it.  The legacy stream can share a
+  // hardware queue with that peer's stream; a copy queued behind the spinning kernel holds this rank back until the peer's
+  // watchdog ends it, and both launches fail with DSGD_ERR_TIMEOUT.
+  CU(cudaMemcpyAsync(host, ctx->p_bar, sizeof host, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
   NEED(host[1] == 0, DSGD_ERR_TIMEOUT, "persistent sync kernel: a device-side wait (grid barrier, peer word) hit its watchdog");
   return DSGD_OK;
 }

@@ -8,54 +8,17 @@ K stops at 3 here: four spinning kernels sharing one GPU hit the device-side wat
 promise co-scheduling of independent kernels; cooperative launch is per kernel) -- four and eight ranks are checked on real
 GPUs by bench.py's parity record and whole-run replays.  A watchdog time-out is retried once.
 """
-import threading
-
 import numpy as np
 import pytest
 
-from helpers import make_pair
+from helpers import make_pair, retry_once_if_not_coscheduled, run_ranks, xchg_model
 
 pytestmark = pytest.mark.gpu
 
 
-def _run_ranks(fns):
-    errs = [None] * len(fns)
-
-    def wrap(i):
-        try:
-            fns[i]()
-        except BaseException as e:  # noqa: BLE001 -- reported below
-            errs[i] = e
-
-    th = [threading.Thread(target=wrap, args=(i,)) for i in range(len(fns))]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join(timeout=120)
-    for e in errs:
-        if e is not None:
-            raise e
-    assert not any(t.is_alive() for t in th), "a rank hangs"
-
-
-def _retry_once_if_not_coscheduled(attempt):
-    """K spinning kernels sharing ONE GPU need all their CTAs resident at once; CUDA does not promise that for independent
-    plain launches (on real multi-GPU boxes every rank has its own GPU and a cooperative launch).  A run that ends in the
-    device-side watchdog is repeated once with fresh contexts; a second time-out fails the test."""
-    from distributed_sgd_b200.native import DsgdError, ERR_TIMEOUT
-    try:
-        return attempt()
-    except DsgdError as e:
-        if getattr(e, "code", None) == ERR_TIMEOUT:
-            import warnings
-            warnings.warn("fused ranks were not co-scheduled on the shared GPU (watchdog); retrying once")
-            return attempt()
-        raise
-
-
 @pytest.mark.parametrize("K,batch,dim", [(2, 48, 20000), (2, 7, 3000), (3, 33, 9000), (3, 64, 11000)])
 def test_fused_k_ranks_on_one_gpu_match_oracle(K, batch, dim):
-    _retry_once_if_not_coscheduled(lambda: _fused_k_ranks(K, batch, dim))
+    retry_once_if_not_coscheduled(lambda: _fused_k_ranks(K, batch, dim))
 
 
 def _fused_k_ranks(K, batch, dim):
@@ -92,22 +55,28 @@ def _fused_k_ranks(K, batch, dim):
             out[r] = (np.concatenate(ls), ctx.get_weights())
         return run
 
+    # contexts are closed on every way out: one left to the garbage collector would be destroyed (a device-wide sync) on
+    # whatever thread collects it, possibly a rank thread of a later test whose peers are spinning
     try:
-        _run_ranks([rank_fn(r) for r in range(K)])
-    except BaseException:
+        run_ranks([rank_fn(r) for r in range(K)])
+        stats = [c.xchg_stats() for c in ctxs]
+    finally:
         for c in ctxs:
             c.close()
-        raise
     for r in range(K):
         losses, w = out[r]
         np.testing.assert_allclose(losses, losses_ref, rtol=1e-12, atol=0)
         assert np.array_equal(w != 0, w_ref != 0)
         np.testing.assert_allclose(w, w_ref, rtol=1e-11, atol=1e-15)
         assert np.array_equal(w, out[0][1]), "weight replicas differ across ranks"
-    v, b, n = ctxs[0].xchg_stats()
-    assert n == steps and b > 0 and 0 < v < n * (dim + 1), "the exchange is expected to be sparse"
-    for c in ctxs:
-        c.close()
+    # the words each rank pushed to each peer: its filtered raw reply's support + the counter column, one bitmap word per
+    # 32 columns, every step (helpers.xchg_model)
+    per_rank = idx.reshape(steps, K, batch)
+    calls = [([per_rank[a:b, r, :] for r in range(K)], None) for a, b in zip(cuts[:-1], cuts[1:])]
+    model = xchg_model(orc, w0, calls, lr)
+    for r in range(K):
+        assert stats[r] == model[r], (r, stats[r], model[r])
+        assert model[r][0] < steps * (dim + 1), "the exchange is expected to be sparse"
 
 
 def test_fused_ranks_exact_cancellation_and_empty_support():
@@ -144,10 +113,16 @@ def test_fused_ranks_exact_cancellation_and_empty_support():
             out[r] = (ls, ctxs[r].get_weights())
         return run
 
-    _run_ranks([rank_fn(0), rank_fn(1)])
+    try:
+        run_ranks([rank_fn(0), rank_fn(1)])
+        stats = [c.xchg_stats() for c in ctxs]
+    finally:
+        for c in ctxs:
+            c.close()
     for r in range(2):
         np.testing.assert_allclose(out[r][0], losses_ref, rtol=1e-13, atol=0)
         np.testing.assert_allclose(out[r][1], w_ref, rtol=1e-13, atol=1e-300)
     assert np.array_equal(out[0][1], out[1][1])
-    for c in ctxs:
-        c.close()
+    model = xchg_model(orc, w0, [([idx[:, 0:2], idx[:, 2:4]], None)], lr)
+    for r in range(2):
+        assert stats[r] == model[r], (r, stats[r], model[r])

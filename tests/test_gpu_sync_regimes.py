@@ -18,12 +18,10 @@ E. Ranks wired with the peer exchange only refuse steps the fused kernel cannot 
 Tolerances (README): losses rtol 1e-12, supports exact, weights rtol 1e-11 / atol 1e-15; bit for bit where the values are
 dyadic and every sum is exact.
 """
-import threading
-
 import numpy as np
 import pytest
 
-from helpers import data_from_csr, make_pair
+from helpers import data_from_csr, fused_ranks, make_pair
 
 pytestmark = pytest.mark.gpu
 
@@ -72,76 +70,13 @@ def _fits_fused(dim, G):
     return ((dim + 1 + G - 1) // G + 31) // 32 * 32 <= SLICE_MAX
 
 
-# ---- two ranks of the fused exchange on one GPU (the pattern of test_gpu_fused_one_gpu.py) -----------------------------
-
-def _run_ranks(fns):
-    errs = [None] * len(fns)
-
-    def wrap(i):
-        try:
-            fns[i]()
-        except BaseException as e:  # noqa: BLE001 -- reported below
-            errs[i] = e
-
-    th = [threading.Thread(target=wrap, args=(i,)) for i in range(len(fns))]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join(timeout=120)
-    for e in errs:
-        if e is not None:
-            raise e
-    assert not any(t.is_alive() for t in th), "a rank hangs"
-
-
-def _retry_once_if_not_coscheduled(attempt):
-    """Two spinning kernels sharing one GPU need all their CTAs resident at once, which CUDA does not promise for independent
-    plain launches: a run that ends in the device-side watchdog is repeated once with fresh contexts."""
-    from distributed_sgd_b200.native import DsgdError, ERR_TIMEOUT
-    try:
-        return attempt()
-    except DsgdError as e:
-        if getattr(e, "code", None) == ERR_TIMEOUT:
-            import warnings
-            warnings.warn("fused ranks were not co-scheduled on the shared GPU (watchdog); retrying once")
-            return attempt()
-        raise
-
+# ---- two ranks of the fused exchange on one GPU (helpers.fused_ranks) --------------------------------------------------
 
 def _fused_run(data, lam, d, G, w0, per_rank, lr):
-    """per_rank[r]: int32 [steps, batch_r] of rank r.  Runs both ranks, checks the replicas are identical, returns rank 0's
-    (losses, weights)."""
-    steps = per_rank[0].shape[0]
-
-    def attempt():
-        ctxs = []
-        for r in range(2):
-            ctx, _ = _pair(data, lam, d, rank=r, world=2)
-            ctx.set_grid_limit(G)
-            ctx.reserve(per_rank[r].size, steps)   # no cudaMalloc (a device-wide sync) once the ranks wait for each other
-            ctxs.append(ctx)
-        ctxs[0].xchg_attach(1, ctxs[1])
-        ctxs[1].xchg_attach(0, ctxs[0])
-        out = [None, None]
-
-        def rank_fn(r):
-            def run():
-                ctxs[r].set_weights(w0)
-                ls = ctxs[r].sync_steps(per_rank[r].reshape(-1), per_rank[r].shape[1], steps, lr)
-                out[r] = (ls, ctxs[r].get_weights())
-            return run
-
-        try:
-            _run_ranks([rank_fn(0), rank_fn(1)])
-        finally:
-            for c in ctxs:
-                c.close()
-        return out
-
-    out = _retry_once_if_not_coscheduled(attempt)
-    assert np.array_equal(out[0][1], out[1][1]), "weight replicas differ across ranks"
-    np.testing.assert_array_equal(out[0][0], out[1][0])
-    return out[0]
+    """per_rank[r]: int32 [steps, batch_r] of rank r.  Runs both ranks in one launch (fused_ranks checks the replicas are
+    identical), returns rank 0's (losses, weights)."""
+    res = fused_ranks(data, lam, d, [G, G], w0, [(per_rank, None)], lr)
+    return res["losses"][0], res["w"][0]
 
 
 def _fused_oracle(orc, w0, per_rank, lr):
