@@ -284,12 +284,19 @@ class MasterSync(Master):
 
     def fit(self, initial_weights: np.ndarray, max_epochs: int, batch_size: int, learning_rate: float,
             stopping_criterion: EarlyStopping, split_strategy: Split = SplitStrategy.vanilla, *,
-            virtual_workers: int = 1, on_epoch: Optional[Callable[[int, dict], None]] = None) -> GradState:
+            virtual_workers: int = 1, on_epoch: Optional[Callable[[int, dict], None]] = None,
+            average_from: Optional[int] = None) -> GradState:
         """Master.fit (core/Master.scala:120-218).
 
         virtual_workers (extension): logical reference workers per GPU, so that `node-count` can exceed the
         number of GPUs (K = world * virtual_workers).
+        average_from (extension): averaged SGD from epoch `average_from` (0-based) on.  The device adds the weights after
+        every step of that epoch and of the later ones to a running sum (ctx.average_begin); the per-epoch evaluations, and
+        so the stopping rule, then see the mean of those weights, and `fit` returns it.  history["averaged_steps"] holds
+        the number of steps averaged.  None: the last weights, as in the reference.
         """
+        if average_from is not None and not 0 <= average_from < max_epochs:
+            raise ValueError(f"average_from must lie in [0, max_epochs = {max_epochs}), got {average_from}")
         W, r, V = self.group.world, self.group.rank, virtual_workers
         K = W * V
         groups = split_strategy(self.n_train, K)             # Master.scala:136 (may hold fewer than K groups)
@@ -308,58 +315,71 @@ class MasterSync(Master):
         from concurrent.futures import ThreadPoolExecutor
         prefetch = ThreadPoolExecutor(1) if self.jvm is None else None
         pending = None
-        while True:
-            if losses:
-                self.log(f"loss after epoch {epoch}: {losses[0]}")
-                self.log(f"acc after epoch {epoch}: {accs[0]}")
-            if epoch >= max_epochs or stopping_criterion(test_losses):   # Master.scala:154,166
-                self.log("Reached max number of epochs: stopping computation" if epoch >= max_epochs
-                         else "Converged to target: stopping computation")
-                self.history = {"losses": losses[::-1], "test_losses": test_losses[::-1], "accs": accs[::-1],
-                                "test_accs": test_accs[::-1]}
-                if prefetch is not None:
-                    prefetch.shutdown(wait=True)
-                # `losses.head` throws on an empty list in the reference (max_epochs == 0)
-                return state.finish(losses[0])
-            steps = pending.result() if pending is not None else self.draw_epoch(groups, batch_size)
-            pending = None
-            if not isinstance(steps, EpochDraw):
-                steps = EpochDraw.from_steps(steps)
-            if prefetch is not None and epoch + 1 < max_epochs:
-                # the draws of epoch e + 1 do not depend on epoch e: make them while the GPU runs epoch e
-                pending = prefetch.submit(self.draw_epoch, groups, batch_size, self._epochs_drawn)
-            counts = steps.counts                                                 # [steps, k_total]
-            if counts.size and (counts[:, :k_total] == 0).any():
-                raise ValueError("Cannot sum an empty list of vectors")  # Vec.scala:129 via Master.scala:187 (Q7)
-            # consecutive steps with identical counts for ALL workers go to the device in one call; the boundaries come
-            # from the global shape so that every rank issues the same sequence of calls (the fused multi-GPU kernel
-            # numbers its exchange tags by call)
-            n_steps = counts.shape[0]
-            change = np.flatnonzero((counts[1:] != counts[:-1]).any(axis=1)) + 1 if n_steps > 1 else np.zeros(0, dtype=np.int64)
-            bounds = [0, *change.tolist(), n_steps]
-            for i, j in zip(bounds[:-1], bounds[1:]):
-                if j == i:
-                    continue
-                shape = [int(counts[i, k]) for k in my_groups]
-                if my_groups:
-                    g0, g1 = my_groups[0], my_groups[-1] + 1
-                    if all(c == steps.ids.shape[2] for c in shape):
-                        flat = np.ascontiguousarray(steps.ids[i:j, g0:g1, :]).reshape(-1)
+        averaging, n_averaged = False, 0   # averaging: average_begin was called, so average_end on every way out
+        try:
+            while True:
+                if losses:
+                    self.log(f"loss after epoch {epoch}: {losses[0]}")
+                    self.log(f"acc after epoch {epoch}: {accs[0]}")
+                if epoch >= max_epochs or stopping_criterion(test_losses):   # Master.scala:154,166
+                    self.log("Reached max number of epochs: stopping computation" if epoch >= max_epochs
+                             else "Converged to target: stopping computation")
+                    self.history = {"losses": losses[::-1], "test_losses": test_losses[::-1], "accs": accs[::-1],
+                                    "test_accs": test_accs[::-1]}
+                    if average_from is not None:
+                        self.history["averaged_steps"] = n_averaged
+                    if prefetch is not None:
+                        prefetch.shutdown(wait=True)
+                    # `losses.head` throws on an empty list in the reference (max_epochs == 0)
+                    return state.finish(losses[0])
+                if epoch == average_from:
+                    self.ctx.average_begin()    # the steps of this epoch and of every later one are averaged
+                    averaging = True
+                steps = pending.result() if pending is not None else self.draw_epoch(groups, batch_size)
+                pending = None
+                if not isinstance(steps, EpochDraw):
+                    steps = EpochDraw.from_steps(steps)
+                if prefetch is not None and epoch + 1 < max_epochs:
+                    # the draws of epoch e + 1 do not depend on epoch e: make them while the GPU runs epoch e
+                    pending = prefetch.submit(self.draw_epoch, groups, batch_size, self._epochs_drawn)
+                counts = steps.counts                                                 # [steps, k_total]
+                if counts.size and (counts[:, :k_total] == 0).any():
+                    raise ValueError("Cannot sum an empty list of vectors")  # Vec.scala:129 via Master.scala:187 (Q7)
+                # consecutive steps with identical counts for ALL workers go to the device in one call; the boundaries come
+                # from the global shape so that every rank issues the same sequence of calls (the fused multi-GPU kernel
+                # numbers its exchange tags by call)
+                n_steps = counts.shape[0]
+                change = np.flatnonzero((counts[1:] != counts[:-1]).any(axis=1)) + 1 if n_steps > 1 else np.zeros(0, dtype=np.int64)
+                bounds = [0, *change.tolist(), n_steps]
+                for i, j in zip(bounds[:-1], bounds[1:]):
+                    if j == i:
+                        continue
+                    shape = [int(counts[i, k]) for k in my_groups]
+                    if my_groups:
+                        g0, g1 = my_groups[0], my_groups[-1] + 1
+                        if all(c == steps.ids.shape[2] for c in shape):
+                            flat = np.ascontiguousarray(steps.ids[i:j, g0:g1, :]).reshape(-1)
+                        else:
+                            flat = np.concatenate([steps.ids[s, k, :counts[s, k]] for s in range(i, j) for k in my_groups])
                     else:
-                        flat = np.concatenate([steps.ids[s, k, :counts[s, k]] for s in range(i, j) for k in my_groups])
-                else:
-                    flat = np.zeros(0, dtype=np.int32)
-                self.ctx.set_workers(shape, k_total)
-                ls = self.ctx.sync_steps(flat, int(sum(shape)), j - i, learning_rate, want_losses=True)
-                self.step_losses.append(ls)
-            w = None  # evaluate the resident weights
-            tl, ta = self.local_loss_accuracy(w, test_data=False)        # Master.scala:206-207
-            vl, va = self.local_loss_accuracy(w, test_data=True)         # Master.scala:208-209
-            losses.insert(0, tl); accs.insert(0, ta); test_losses.insert(0, vl); test_accs.insert(0, va)
-            epoch += 1
-            state = state.replace_grad(self.ctx.get_weights())          # Master.scala:205
-            if on_epoch:
-                on_epoch(epoch, {"loss": tl, "acc": ta, "test_loss": vl, "test_acc": va})
+                        flat = np.zeros(0, dtype=np.int32)
+                    self.ctx.set_workers(shape, k_total)
+                    ls = self.ctx.sync_steps(flat, int(sum(shape)), j - i, learning_rate, want_losses=True)
+                    self.step_losses.append(ls)
+                # evaluate the resident weights, or while averaging the mean of the averaged steps' weights
+                w = None
+                if averaging:
+                    w, n_averaged = self.ctx.average_weights()
+                tl, ta = self.local_loss_accuracy(w, test_data=False)        # Master.scala:206-207
+                vl, va = self.local_loss_accuracy(w, test_data=True)         # Master.scala:208-209
+                losses.insert(0, tl); accs.insert(0, ta); test_losses.insert(0, vl); test_accs.insert(0, va)
+                epoch += 1
+                state = state.replace_grad(self.ctx.get_weights() if w is None else w)   # Master.scala:205
+                if on_epoch:
+                    on_epoch(epoch, {"loss": tl, "acc": ta, "test_loss": vl, "test_acc": va})
+        finally:
+            if averaging:
+                self.ctx.average_end()
 
 
 class MasterAsync(Master):

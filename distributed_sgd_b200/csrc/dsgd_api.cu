@@ -7,6 +7,7 @@
 #include <nccl.h>  // types only: the library itself is bound at run time (see nccl_api)
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -143,6 +144,12 @@ struct dsgd_ctx {
   dev_buf<unsigned> p_bar;   // [0]: grid barrier counter, [1]: abort flag
   bool p_ready = false;
   dev_buf<long long> p_tl;   // debug timeline (DSGD_PERSIST_TIMELINE)
+
+  // averaged SGD: per-column fp64 sum of the weights after every sync step since dsgd_average_begin (which allocates it),
+  // and the count
+  dev_buf<double> avg;
+  bool avg_on = false;        // the sync steps add to avg
+  int64_t avg_n = 0;
 
   // async (Hogwild) mode
   owned_stream astream;   // the worker loop
@@ -945,7 +952,7 @@ extern "C" int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYT
 // ---- persistent sync loop (dsgd_persistent.cuh) ----------------------------------------------------------------
 constexpr int kPCons = 8, kPUpd = 6, kPStages = 8, kPStagePairs = 2560, kPMaxChunks = 128;
 using PSmem = PersistSmem<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks>;
-#define DSGD_PERSIST_KERNEL(multi) k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, multi>
+#define DSGD_PERSIST_KERNEL(multi, avg) k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, multi, avg>
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -961,8 +968,10 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
     }
     CU(ctx->p_acc.alloc(3 * kAccStride));
     CU(ctx->p_bar.alloc(4));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
   return ctx->p_hinge.grow(ctx, n_steps, 4096);
@@ -1073,11 +1082,18 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.xstats = ctx->x_stats;
   }
   void *args[] = {&pp};
-  void *fn = multi ? (void *)DSGD_PERSIST_KERNEL(true) : (void *)DSGD_PERSIST_KERNEL(false);
+  void *fn;
+  if (ctx->avg_on) {   // the averaging instantiations only while averaging is on: otherwise the kernels of before run
+    pp.avg = ctx->avg;
+    fn = multi ? (void *)DSGD_PERSIST_KERNEL(true, true) : (void *)DSGD_PERSIST_KERNEL(false, true);
+  } else {
+    fn = multi ? (void *)DSGD_PERSIST_KERNEL(true, false) : (void *)DSGD_PERSIST_KERNEL(false, false);
+  }
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
   CU(launch_err);
   LAUNCHED();
+  if (ctx->avg_on) ctx->avg_n += n_steps;
   if (multi) {
     // The next launch must not meet LL words carrying tags this one used (the host may install new weights in between): the
     // step counter jumps.  By 6: a multiple of 3 keeps the rotation of the three gradient buffers (the dirty one is re-zeroed
@@ -1273,6 +1289,17 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     // exchange block mapped (fused): the same kernel aggregates over NVLink
     return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses.p : nullptr);
   }
+  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights
+  auto update = [&](auto kernel, auto kernel_avg, double *gbuf, double k_den, double n_local, double *loss_dev) {
+    if (ctx->avg_on)
+      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr, k_den,
+                                                      ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
+    else
+      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr, k_den, ctx->scal,
+                                                  ctx->cnt, ctx->partial, n_local, loss_dev);
+    LAUNCHED();
+    if (ctx->avg_on) ++ctx->avg_n;
+  };
   for (int64_t s = 0; s < n_steps; ++s) {
     const int32_t *smp = ctx->samples + first + s * n_per_step;
     double *loss_dev = want_losses ? ctx->losses + s : nullptr;
@@ -1284,10 +1311,7 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
                                                                                       0, n_per_step, ctx->w, ctx->g, ctx->cnt);
         });
         LAUNCHED();
-        k_update<true, kLogistic><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->g, ctx->d, ctx->dim, ctx->lambda,
-                                                                       lr, 1.0, ctx->scal, ctx->cnt, ctx->partial,
-                                                                       (double)n_per_step, loss_dev);
-        LAUNCHED();
+        update(k_update<true, kLogistic>, k_update_avg<true, kLogistic>, ctx->g, 1.0, (double)n_per_step, loss_dev);
         continue;
       }
       profiled(ctx, [&] {
@@ -1295,9 +1319,7 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
                                                                                  n_per_step, ctx->w, ctx->g, nullptr, ctx->cnt);
       });
       LAUNCHED();
-      k_update<true><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->g, ctx->d, ctx->dim, ctx->lambda, lr, 1.0,
-                                                          ctx->scal, ctx->cnt, ctx->partial, (double)n_per_step, loss_dev);
-      LAUNCHED();
+      update(k_update<true>, k_update_avg<true>, ctx->g, 1.0, (double)n_per_step, loss_dev);
       continue;
     }
     int64_t off = 0;
@@ -1329,13 +1351,9 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
     if (ctx->world > 1)
       NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
     if (logistic)
-      k_update<false, kLogistic><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->gsum, ctx->d, ctx->dim,
-                                                                      ctx->lambda, lr, (double)k_total, ctx->scal, ctx->cnt,
-                                                                      ctx->partial, 0.0, loss_dev);
+      update(k_update<false, kLogistic>, k_update_avg<false, kLogistic>, ctx->gsum, (double)k_total, 0.0, loss_dev);
     else
-      k_update<false><<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, ctx->gsum, ctx->d, ctx->dim, ctx->lambda, lr,
-                                                           (double)k_total, ctx->scal, ctx->cnt, ctx->partial, 0.0, loss_dev);
-    LAUNCHED();
+      update(k_update<false>, k_update_avg<false>, ctx->gsum, (double)k_total, 0.0, loss_dev);
   }
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -1367,6 +1385,50 @@ extern "C" int dsgd_sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_
 
 extern "C" int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, double lr, double *loss_out) {
   return dsgd_sync_steps(ctx, samples, n, 1, lr, loss_out);
+}
+
+// ---- averaged SGD: the sync step kernels add the new weights of every step to ctx->avg while ctx->avg_on ----------------
+
+extern "C" int dsgd_average_begin(dsgd_ctx *ctx) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_average_begin: ctx is in async mode (averaging is sync-mode only)");
+  ctx->avg_on = false;   // a failure below leaves averaging off and nothing to read
+  ctx->avg_n = 0;
+  CU(cudaSetDevice(ctx->device));
+  if (!ctx->avg) CU(ctx->avg.alloc(ctx->dim));
+  CU(cudaMemsetAsync(ctx->avg, 0, sizeof(double) * (size_t)ctx->dim, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  ctx->avg_on = true;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_average_end(dsgd_ctx *ctx) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_average_end: ctx is in async mode (averaging is sync-mode only)");
+  ctx->avg_on = false;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_average_weights(dsgd_ctx *ctx, double *avg_out, int64_t *n_steps_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_average_weights: ctx is in async mode (averaging is sync-mode only)");
+  NEED(ctx->avg, DSGD_ERR_STATE, "dsgd_average_weights: dsgd_average_begin was never called");
+  NEED(ctx->avg_n > 0, DSGD_ERR_EMPTY, "dsgd_average_weights: no sync step since dsgd_average_begin (the mean of an empty list)");
+  if (avg_out) {
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaMemcpyAsync(avg_out, ctx->avg, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    int rc = persist_check(ctx);   // the sums of a launch that hit its watchdog are garbage
+    if (rc) return rc;
+    // one IEEE division per column, then the constructor filter of a new Sparse (Sparse.scala:108-118)
+    const double n = (double)ctx->avg_n;
+    for (int32_t j = 0; j < ctx->dim; ++j) {
+      const double v = avg_out[j] / n;
+      avg_out[j] = std::fabs(v) > kEps ? v : 0.0;
+    }
+  }
+  if (n_steps_out) *n_steps_out = ctx->avg_n;
+  return DSGD_OK;
 }
 
 // ---- async (Hogwild) mode -------------------------------------------------------------------------------------

@@ -309,13 +309,14 @@ __global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict_
 //   kFuseRegularize: the buffer holds the raw local sum (single worker): apply regularize() here.
 //   otherwise it holds sum_k r^(k) (already regularized per worker, then allreduced).
 //   kModel: where the batch's loss sum comes from (batch_loss_sum).
+//   kAvg (k_update_avg): also avg_j <- avg_j + w_j of the NEW weights, every column (averaged SGD, dsgd_average_begin).
 // ---------------------------------------------------------------------------------------------------
-template <bool kFuseRegularize, int kModel = kSvm>
-__global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32,
-                                                double *__restrict__ g, const double *__restrict__ d, int dim,
-                                                double lambda, double lr, double inv_k_den, double *__restrict__ scal,
-                                                unsigned long long *__restrict__ cnt, double *__restrict__ partial,
-                                                double n_samples_local, double *__restrict__ loss_out) {
+template <bool kFuseRegularize, int kModel, bool kAvg>
+__device__ __forceinline__ void update_body(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
+                                            const double *__restrict__ d, int dim, double lambda, double lr, double inv_k_den,
+                                            double *__restrict__ scal, unsigned long long *__restrict__ cnt,
+                                            double *__restrict__ partial, double n_samples_local,
+                                            double *__restrict__ loss_out, double *__restrict__ avg) {
   __shared__ double red[8];
   __shared__ bool is_last;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -338,6 +339,7 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
       w[j] = wn;
       w32[j] = (float)wn;
     }
+    if (kAvg) avg[j] = avg[j] + wn;
     pd = filt(wn * d[j]);
     pn = wn * wn;
   }
@@ -378,6 +380,25 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
       cnt[kCntTicket] = 0ull;
     }
   }
+}
+template <bool kFuseRegularize, int kModel = kSvm>
+__global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32,
+                                                double *__restrict__ g, const double *__restrict__ d, int dim,
+                                                double lambda, double lr, double inv_k_den, double *__restrict__ scal,
+                                                unsigned long long *__restrict__ cnt, double *__restrict__ partial,
+                                                double n_samples_local, double *__restrict__ loss_out) {
+  update_body<kFuseRegularize, kModel, false>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
+                                              loss_out, nullptr);
+}
+template <bool kFuseRegularize, int kModel = kSvm>
+__global__ void __launch_bounds__(256) k_update_avg(double *__restrict__ w, float *__restrict__ w32,
+                                                    double *__restrict__ g, const double *__restrict__ d, int dim,
+                                                    double lambda, double lr, double inv_k_den, double *__restrict__ scal,
+                                                    unsigned long long *__restrict__ cnt, double *__restrict__ partial,
+                                                    double n_samples_local, double *__restrict__ loss_out,
+                                                    double *__restrict__ avg) {
+  update_body<kFuseRegularize, kModel, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
+                                             loss_out, avg);
 }
 
 // ---------------------------------------------------------------------------------------------------

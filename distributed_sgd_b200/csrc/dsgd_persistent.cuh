@@ -89,6 +89,8 @@ struct PersistParams {
   int xstride, xwords;
   unsigned long long *llw[2];             // this rank's weights as LL words, double-buffered by step parity
   unsigned long long *xstats;             // [0] value words, [1] bitmap words this rank pushed to ONE peer (diagnostic)
+  // ---- averaged SGD (kAvg); last, so that the parameter offsets of the other instantiations stay where they were ----
+  double *avg;                            // [dim] running sum of W_t over the averaged steps: read at launch, written at exit
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -465,7 +467,11 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
   return hinge;
 }
 
-template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti>
+// kAvg: averaged SGD -- every column's p.avg[j] += W_t[j] for t = 1 .. S (W_0, the launch's starting weights, is not
+// added), in step order, in plain fp64.  One GPU: the update threads keep the sums of their register columns in registers
+// (loaded at launch start, stored in the epilogue); the columns past the register ones read-modify-write p.avg every step.
+// K GPUs: the column thread keeps its column's sum in a register.
+template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -601,20 +607,30 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   // "the g half seen last interval was non-zero"); K GPUs, column threads: W_{T-1}[j_col] and d[j_col]
   constexpr int kUpdCols = 2;
   double wreg[kUpdCols], dreg[kUpdCols];
+  double areg[kUpdCols];   // kAvg: running sums of the same columns
   int ttl[kUpdCols];
   bool gnz[kUpdCols];
 #pragma unroll
   for (int i = 0; i < kUpdCols; ++i) {
     wreg[i] = dreg[i] = 0.0;
+    areg[i] = 0.0;
     ttl[i] = 0;
     gnz[i] = false;
     if constexpr (!kMulti) {
       const int j = u0 + i * n_upd;
-      if (is_upd && j < p.dim) { wreg[i] = __ldcg(&p.rec[2][j].x); dreg[i] = __ldg(&p.d[j]); }
+      if (is_upd && j < p.dim) {
+        wreg[i] = __ldcg(&p.rec[2][j].x);
+        dreg[i] = __ldg(&p.d[j]);
+        if constexpr (kAvg) areg[i] = p.avg[j];
+      }
     }
   }
   if constexpr (kMulti) {
-    if (col_act && j_col < p.dim) { wreg[0] = __ldcg(&p.wbuf[0][j_col]); dreg[0] = __ldg(&p.d[j_col]); }
+    if (col_act && j_col < p.dim) {
+      wreg[0] = __ldcg(&p.wbuf[0][j_col]);
+      dreg[0] = __ldg(&p.d[j_col]);
+      if constexpr (kAvg) areg[0] = p.avg[j_col];
+    }
   }
 
   // rotating buffer indices kept as small integers (64-bit % 3 per warp and step is ~100 instructions on the critical path)
@@ -824,6 +840,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
                   wn = filt(wn - step);
                 }
                 wreg[0] = wn;
+                if constexpr (kAvg) areg[0] = areg[0] + wn;   // W_T, T >= base + 1
                 ll_store(LWcur + 2 * (size_t)j_col, wn, wtag);
                 pd = filt(wn * dreg[0]);
                 pn = wn * wn;
@@ -894,6 +911,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
             if (ttl[i] > 0) { Rcur[j].x = wreg[i]; --ttl[i]; }
             if (gnz[i]) Rnext[j].y = 0.0;          // held g_{t-2}, read for the last time during interval t-1
             gnz[i] = gv[i] != 0.0;
+            if constexpr (kAvg) if (!first) areg[i] = areg[i] + wreg[i];   // W_t, t >= 1
             pd += filt(wreg[i] * dreg[i]);
             pn += wreg[i] * wreg[i];
           }
@@ -903,6 +921,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           const double wn = apply_update(r.x, r.y, c_prev, add_c, p.k_den, lr);
           Rcur[j].x = wn;
           Rnext[j].y = 0.0;
+          if constexpr (kAvg) if (!first) p.avg[j] = p.avg[j] + wn;
           pd += filt(wn * __ldg(&p.d[j]));
           pn += wn * wn;
         }
@@ -967,12 +986,19 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       atomicAdd(&p.xstats[0], st_val);
       atomicAdd(&p.xstats[1], st_bm);
     }
+    if constexpr (kAvg) {
+      if (col_act && j_col < p.dim) p.avg[j_col] = areg[0];
+    }
   } else if (is_upd) {
     const double2 *Rfin = p.rec[ti_prev];
 #pragma unroll
     for (int i = 0; i < kUpdCols; ++i) {
       const int j = u0 + i * n_upd;
-      if (j < p.dim) { p.w_out[j] = wreg[i]; p.w32_out[j] = (float)wreg[i]; }
+      if (j < p.dim) {
+        p.w_out[j] = wreg[i];
+        p.w32_out[j] = (float)wreg[i];
+        if constexpr (kAvg) p.avg[j] = areg[i];
+      }
     }
     for (int j = u0 + kUpdCols * n_upd; j < p.dim; j += n_upd) {
       const double wv = __ldcg(&Rfin[j]).x;

@@ -263,6 +263,19 @@ FN(syncSteps)(JNIEnv *env, jobject self, jlong h, jintArray samples, jlong n_per
   free(bs.p);
   return rc;
 }
+/* averaged SGD: begin zeroes the device-side sum, every following sync step adds its new weights; avg(dim) = the mean,
+ * nSteps(0) = the number of steps averaged (either array may be null) */
+FN(averageBegin)(JNIEnv *env, jobject self, jlong h) { return dsgd_average_begin(CTX(h)); }
+FN(averageEnd)(JNIEnv *env, jobject self, jlong h) { return dsgd_average_end(CTX(h)); }
+FN(averageWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray avg, jlongArray nSteps) {
+  buf_t ba = out_Double(env, avg), bn = out_Long(env, nSteps);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(ba.bad | bn.bad))
+    rc = (bn.p && bn.n < 1) ? DSGD_ERR_INVALID : dsgd_average_weights(CTX(h), (double *)ba.p, (int64_t *)bn.p);
+  back_Double(env, avg, ba, rc);
+  back_Long(env, nSteps, bn, rc);
+  return rc;
+}
 
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {

@@ -30,6 +30,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
 
     if cfg.model == "logistic" and cfg.is_async:
         raise ValueError("model = logistic: asynchronous (Hogwild) training supports the svm model only")
+    if cfg.average_from >= 0 and cfg.is_async:
+        raise ValueError("average-from: averaged SGD is a sync-mode option; asynchronous (Hogwild) training does not average")
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
     model = SparseLogistic(cfg.lam) if cfg.model == "logistic" else SparseSVM(cfg.lam)
@@ -54,7 +56,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         if cfg.node_count % world:
             raise ValueError(f"node-count {cfg.node_count} is not a multiple of the {world} GPU processes")
         state = master.fit(w0, cfg.max_epochs, cfg.batch_size, cfg.learning_rate, stop,
-                           virtual_workers=cfg.node_count // world)
+                           virtual_workers=cfg.node_count // world,
+                           average_from=cfg.average_from if cfg.average_from >= 0 else None)
     report["fit_seconds"] = time.perf_counter() - t0                          # Measure.durationLog(log, "fit") (Main.scala:80)
     w1 = state.grad
     report["history"] = {k: [float(x) for x in v] for k, v in getattr(master, "history", {}).items()
@@ -62,6 +65,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     report["final_test_loss"], report["final_test_accuracy"] = master.local_loss_accuracy(w1, test_data=True)  # :115-118
     report["final_weights_nonzero"] = int(np.count_nonzero(w1))
     report["updates"] = state.updates
+    if "averaged_steps" in getattr(master, "history", {}):
+        report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
     if inspect:
         inspect("done", (master, state))
     slave.stop()

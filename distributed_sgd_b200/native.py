@@ -117,6 +117,9 @@ ABI = {
     "dsgd_stage_samples": [_vp, _vp, _i64],
     "dsgd_sync_steps_staged": [_vp, _i64, _i64, _i64, _f64, C.c_int],
     "dsgd_read_losses": [_vp, _vp, _i64],
+    "dsgd_average_begin": [_vp],
+    "dsgd_average_end": [_vp],
+    "dsgd_average_weights": [_vp, _vp, C.POINTER(_i64)],
     "dsgd_async_host_master": [_vp, _vp],
     "dsgd_ipc_export": [_vp, C.c_int, _vp],
     "dsgd_ipc_import": [_vp, C.c_int, _vp],
@@ -458,6 +461,22 @@ class NativeCtx:
         out = np.zeros(n_steps, dtype=np.float64)
         self._ck(self._l.dsgd_read_losses(self._h, _ptr(out), n_steps))
         return out
+
+    # -- averaged SGD (sync mode) --
+    def average_begin(self):
+        """Zero the running sum of the weights and its step count; every following sync step adds its new weights."""
+        self._ck(self._l.dsgd_average_begin(self._h))
+
+    def average_end(self):
+        """Stop adding to the sum; the sum and the count stay readable."""
+        self._ck(self._l.dsgd_average_end(self._h))
+
+    def average_weights(self) -> Tuple[np.ndarray, int]:
+        """(mean of the weights after every step averaged since average_begin, number of those steps)."""
+        out = np.zeros(self.dim, dtype=np.float64)
+        n = C.c_int64()
+        self._ck(self._l.dsgd_average_weights(self._h, _ptr(out), C.byref(n)))
+        return out, n.value
 
     # -- async --
     def async_host_master(self, w0):

@@ -32,6 +32,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     conv_delta: float = 0.01
     patience: int = 5
     model: str = "svm"            # extension: "svm" (SparseSVM) or "logistic" (SparseLogistic, sync mode only)
+    average_from: int = -1        # extension: averaged SGD from this epoch (0-based) on, sync mode only; -1: off
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -43,7 +44,7 @@ _KEYS = {
     "async": ("is_async", "DSGD_ASYNC"), "record": ("record", "DSGD_RECORD"), "max-epochs": ("max_epochs", "DSGD_MAX_EPOCHS"),
     "check-every": ("check_every", "DSGD_CHECK_EVERY"), "leaky-loss": ("leaky_loss", "DSGD_LEAKY_LOSS"),
     "patience": ("patience", "DSGD_PATIENCE"), "conv-delta": ("conv_delta", "DSGD_CONV_DELTA"),
-    "model": ("model", "DSGD_MODEL"),
+    "model": ("model", "DSGD_MODEL"), "average-from": ("average_from", "DSGD_AVERAGE_FROM"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -109,4 +110,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         setattr(cfg, field, _coerce(field, value))
     if cfg.model not in MODELS:
         raise ValueError(f"model: expected one of {', '.join(MODELS)}, got {cfg.model!r}")
+    if cfg.average_from < -1:
+        raise ValueError(f"average-from: expected an epoch >= 0, or -1 for off, got {cfg.average_from}")
     return cfg

@@ -215,6 +215,21 @@ int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int
                            int want_losses);
 int dsgd_read_losses(dsgd_ctx *ctx, double *losses_out, int64_t n_steps);
 
+/* ---- averaged SGD (Polyak-Ruppert) on the device, sync mode.  dsgd_average_begin zeroes a per-column fp64 sum A[dim] and
+ *      a step count n; every sync step that runs after it, on any path (persistent, fused K-rank, per-step, logistic),
+ *      then adds the weights after the step to A -- every column, whether the step changed it or not -- and 1 to n.  The
+ *      starting weights of a call are not added.  Per column the additions happen in step order in plain fp64, so the sum
+ *      does not depend on which path ran a step or on how the steps are split into calls.  dsgd_average_end stops the
+ *      accumulation and keeps A and n.  dsgd_set_weights leaves both alone; a call of zero steps adds nothing.
+ *      dsgd_average_weights: avg_out[j] = A[j] / n, with the 1e-20 filter of a new Sparse; n_steps_out = n; either
+ *      pointer may be NULL.  Errors: an async ctx -> DSGD_ERR_STATE (every call); dsgd_average_weights before any
+ *      dsgd_average_begin -> DSGD_ERR_STATE, with n == 0 -> DSGD_ERR_EMPTY.
+ *      The first dsgd_average_begin allocates A with cudaMalloc, which synchronises the whole device: K contexts that
+ *      share ONE GPU call it before their threads start stepping (see dsgd_reserve). ---------------------------------- */
+int dsgd_average_begin(dsgd_ctx *ctx);   /* zero the sum and the count; average every following sync step */
+int dsgd_average_end(dsgd_ctx *ctx);     /* stop averaging; the sum and the count stay readable */
+int dsgd_average_weights(dsgd_ctx *ctx, double *avg_out, int64_t *n_steps_out);
+
 /* ---- async (Hogwild) mode.  Every worker keeps its own weight replica (core/Slave.scala:30) and pushes each
  *      delta to every peer replica and to the master's replica (core/Slave.scala:101-105).  Here replicas are
  *      reached by ADDRESS over NVLink: a rank exports its replica, the host transports the handle, peers import

@@ -1,7 +1,8 @@
 """Dev tool: which kernels of two builds of libdsgd.so differ, instruction for instruction (cuobjdump -sass; addresses and
 encodings ignored).  Used to show that adding template variants leaves the kernels that were verified on the GPU untouched.
     python tools/sass_diff.py old/libdsgd.so distributed_sgd_b200/libdsgd.so
-A kernel that gained trailing default template arguments (e.g. `..., 0>` -> `..., 0, 0>`) is matched by its name prefix."""
+A kernel that gained trailing template arguments 0 or false (e.g. `..., 0>` -> `..., 0, 0>`, `..., false>` ->
+`..., false, false>`) is matched by its name prefix."""
 import re
 import subprocess
 import sys
@@ -26,7 +27,8 @@ def main():
     a, b = kernels(sys.argv[1]), kernels(sys.argv[2])
     differ = 0
     for name, body in sorted(a.items()):
-        cands = [name] if name in b else [n for n in (name.replace("EEEv", "ELi0EEEv", 1), name.replace("EEEv", "ELi0ELi0EEEv", 1)) if n in b]
+        extra = ("ELi0", "ELi0ELi0", "ELb0")
+        cands = [name] if name in b else [n for n in (name.replace("EEEv", e + "EEEv", 1) for e in extra) if n in b]
         if not cands:
             print("only in the first build:", name)
             differ += 1
