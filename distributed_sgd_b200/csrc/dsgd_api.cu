@@ -130,7 +130,8 @@ struct dsgd_ctx {
   int64_t samples_n = 0;
   dev_buf<double> losses;
   dev_buf<double> preds;
-  // row ids of a sampled evaluation (drawn on the device or copied from the host): never the staged stream above
+  // row ids of a request (forward, gradient, a sampled evaluation; drawn on the device or copied from the host): never the
+  // staged stream above
   dev_buf<int32_t> eval_ids;
 
   ncclComm_t comm = nullptr;
@@ -489,6 +490,8 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
       }
   }
   CU(cudaSetDevice(ctx->device));
+  // the staged stream was checked against the previous rows: a shorter set would leave ids past its end in it
+  ctx->samples_n = 0;
   // all of the previous rows go before any of the new ones is allocated
   CU(ctx->rp16.release()); CU(ctx->pairs.release()); CU(ctx->label.release()); CU(ctx->yabs.release());
   const int64_t n_pairs = (int64_t)acc * 2;
@@ -613,17 +616,23 @@ extern "C" int dsgd_stage_samples(dsgd_ctx *ctx, const int32_t *samples, int64_t
   return DSGD_OK;
 }
 
-// weights to use for a request: NULL -> resident; else copy into w_req and compute its scalars
+// weights to use for a request: NULL -> resident; else copy into w_req and compute its scalars.  On an async ctx NULL is a
+// snapshot of the replica taken now, with its scalars computed like those of explicit weights: dsgd_update_grad, a peer's
+// pushes and a loop that ended by itself change the replica without refreshing c, ||w||^2 or the fp32 shadow.
 static int request_weights(dsgd_ctx *ctx, const double *w, const double **w_dev, const double **c_dev,
                            const double **nrm_dev, const float **w32_dev = nullptr) {
   CU(cudaSetDevice(ctx->device));  // every request path passes here: a caller thread may have another device current
-  if (!w) {
+  const bool snapshot = !w && (ctx->flags & DSGD_FLAG_ASYNC);
+  if (!w && !snapshot) {
     *w_dev = ctx->w; *c_dev = ctx->scal + kScalC; *nrm_dev = ctx->scal + kScalNrm2;
     if (w32_dev) *w32_dev = ctx->w32;
     return DSGD_OK;
   }
   if (w32_dev) *w32_dev = ctx->w32_req;
-  CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
+  if (snapshot)
+    CU(cudaMemcpyAsync(ctx->w_req, ctx->w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToDevice, ctx->stream));
+  else
+    CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
   launch_prepare(ctx, ctx->w_req, ctx->w32_req, kScalReqC, kScalReqNrm2);
   CU(cudaGetLastError());
   *w_dev = ctx->w_req; *c_dev = ctx->scal + kScalReqC; *nrm_dev = ctx->scal + kScalReqNrm2;
@@ -677,11 +686,22 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
 
 // ---- forward / gradient / eval -------------------------------------------------------------------------
 
+// the n row ids of a request into eval_ids: the staged stream stays as it was for the next dsgd_sync_steps_staged
+static int request_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn) {
+  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
+  int rc = check_ids(ctx, ids, n, "sample index");
+  if (rc) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
+  CU(cudaMemcpyAsync(ctx->eval_ids, ids, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  return DSGD_OK;
+}
+
 extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *preds_out) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(n >= 0 && (n == 0 || (samples && preds_out)), DSGD_ERR_INVALID, "dsgd_forward: bad arguments");
   if (n == 0) return DSGD_OK;
-  int rc = dsgd_stage_samples(ctx, samples, n);
+  int rc = request_ids(ctx, samples, n, "dsgd_forward");
   if (rc) return rc;
   rc = ctx->preds.grow(ctx, n, 1024);
   if (rc) return rc;
@@ -689,9 +709,9 @@ extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *sampl
   const float *w32d;
   if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
   if (stream_eligible(ctx, n)) {
-    if ((rc = stream_launch<false, true, false>(ctx, ctx->samples, 0, n, wd, w32d, nullptr, ctx->preds))) return rc;
+    if ((rc = stream_launch<false, true, false>(ctx, ctx->eval_ids, 0, n, wd, w32d, nullptr, ctx->preds))) return rc;
   } else {
-    k_rows<false, true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->samples, 0, n,
+    k_rows<false, true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
                                                                     wd, nullptr, ctx->preds, ctx->cnt);
     LAUNCHED();
   }
@@ -709,20 +729,20 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
   NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_gradient: empty batch (Vec.sum of an empty list throws in the reference)");
   NEED(samples, DSGD_ERR_INVALID, "dsgd_gradient: samples is NULL");
   NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_gradient: dimSparsity not set");
-  int rc = dsgd_stage_samples(ctx, samples, n);
+  int rc = request_ids(ctx, samples, n, "dsgd_gradient");
   if (rc) return rc;
   const double *wd, *cd, *nd;
   const float *w32d;
   if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
   const bool logistic = is_logistic(ctx);
   if (logistic) {
-    k_rows_logistic<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->samples, 0, n,
+    k_rows_logistic<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
                                                                       wd, ctx->g, ctx->cnt);
     LAUNCHED();
   } else if (stream_eligible(ctx, n)) {
-    if ((rc = stream_launch<true, false, false>(ctx, ctx->samples, 0, n, wd, w32d, ctx->g, nullptr))) return rc;
+    if ((rc = stream_launch<true, false, false>(ctx, ctx->eval_ids, 0, n, wd, w32d, ctx->g, nullptr))) return rc;
   } else {
-    k_rows<true, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->samples, 0, n,
+    k_rows<true, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
                                                                     wd, ctx->g, nullptr, ctx->cnt);
     LAUNCHED();
   }
@@ -884,11 +904,8 @@ static int eval_samples_impl(dsgd_ctx *ctx, const double *w, const int32_t *samp
   NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
   NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "%s: bad arguments", fn);
   NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty sample (reduce on an empty collection throws)", fn);
-  int rc = check_ids(ctx, samples, n, "sample index");
+  int rc = request_ids(ctx, samples, n, fn);
   if (rc) return rc;
-  CU(cudaSetDevice(ctx->device));
-  if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
-  CU(cudaMemcpyAsync(ctx->eval_ids, samples, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   return eval_pass(ctx, w, ctx->eval_ids, 0, n, out);
 }
 

@@ -494,7 +494,8 @@ class NativeCtx:
         self._ck(self._l.dsgd_peer_attach(self._h, peer_rank, peer._h, which))
 
     def async_replay(self, w0, samples, batch: int, lr: float):
-        w0 = _arr(w0, np.float64, self.dim, "weights")
+        """Replays recorded batches on one lane; w0 None starts from the replica as it is (peers' pushes included)."""
+        w0 = None if w0 is None else _arr(w0, np.float64, self.dim, "weights")
         samples = _arr(samples, np.int32)
         if samples.size % batch:
             raise DsgdInvalid(ERR_INVALID, "async_replay: len(samples) is not a multiple of batch")

@@ -107,7 +107,8 @@ int dsgd_stream_exact_rows(dsgd_ctx *ctx, int64_t *rows);
 /* ---- data: the `data: Array[(Vec, Int)]` constructor argument (core/Slave.scala:20; Main.scala:138,149).
  *      Rows are repacked on the device into 16-byte aligned (col, val) windows.  label in {-1, +1}.  A row is
  *      a Map in the reference: a column repeated within one row (in any order) is DSGD_ERR_INVALID; columns
- *      need not be sorted. ------------------------------------------------------------------------------- */
+ *      need not be sorted.  A reload drops a staged sample stream (dsgd_stage_samples): its ids named the previous
+ *      rows, so stage again before dsgd_sync_steps_staged. ------------------------------------------------------ */
 int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const int64_t *row_ptr, const int32_t *col,
                   const float *val, const int8_t *label);
 
@@ -118,12 +119,16 @@ int dsgd_set_dim_sparsity(dsgd_ctx *ctx, const double *d);
 int dsgd_compute_dim_sparsity(dsgd_ctx *ctx, int64_t n_train, double *d_out);
 
 /* ---- resident weights: GradState.grad on the master (core/ml/GradState.scala:6), `weights` Ref on an
- *      async slave (core/Slave.scala:30) ---------------------------------------------------------------- */
+ *      async slave (core/Slave.scala:30).  w == NULL in a request below (forward, gradient, every evaluation) reads
+ *      the resident weights.  On a DSGD_FLAG_ASYNC ctx it reads a snapshot of the replica taken when the call starts,
+ *      exactly as if that snapshot had been passed as w: dsgd_update_grad, a peer's pushes and a loop that ended by
+ *      itself on max_updates change the replica between calls. ---------------------------------------------- */
 int dsgd_set_weights(dsgd_ctx *ctx, const double *w);
 int dsgd_get_weights(dsgd_ctx *ctx, double *w);
 
 /* ---- SlaveImpl.forward (core/Slave.scala:129-140; SparseSVM.scala:14): preds[i] = -signum(x_i . w).
- *      w == NULL: use the resident weights. ----------------------------------------------------------------- */
+ *      w == NULL: use the resident weights.  The ids go to a buffer of their own, as those of every request do: a
+ *      sample stream staged with dsgd_stage_samples is left intact (this holds for dsgd_gradient too). ---------- */
 int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *preds_out);
 
 /* ---- SlaveImpl.gradient (core/Slave.scala:142-157; SparseSVM.scala:26-31): grad_out[dim] =
@@ -209,7 +214,9 @@ int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, double lr, 
 int dsgd_sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, double lr,
                     double *losses_out);
 /* The same split in three, so a host can keep the index stream resident: stage = H2D of the sample slices
- * (the `samples` field of GradientRequest, protobuf/proto.proto:60-63); run = device only; read = D2H. */
+ * (the `samples` field of GradientRequest, protobuf/proto.proto:60-63); run = device only; read = D2H.  The stream stays
+ * until the next dsgd_stage_samples, dsgd_sync_step or dsgd_sync_steps (which stage their own samples and so replace it)
+ * or dsgd_load_csr (which drops it); the requests (forward, gradient, the evaluations) leave it intact. */
 int dsgd_stage_samples(dsgd_ctx *ctx, const int32_t *samples, int64_t n);
 int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,
                            int want_losses);

@@ -63,13 +63,14 @@ def retry_once_if_not_coscheduled(attempt):
         raise
 
 
-def fused_ranks(data, lam, d, grid_limits, w0, calls, lr, n_train=None, after=None):
+def fused_ranks(data, lam, d, grid_limits, w0, calls, lr, n_train=None, after=None, before=None):
     """Runs K = len(grid_limits) ranks of the fused sync step on one GPU: rank r limited to grid_limits[r] CTAs, every rank
     attached to every other with dsgd_xchg_attach, one host thread each.  d: dimSparsity for every rank (None: computed
     from the first n_train rows).  Every rank starts from w0; calls[i] = (ids, w) is one launch: ids[r] is rank r's int32
     [steps, batch_r] sample ids (steps the same on every rank, batches may differ), w (or None) new weights installed with
-    set_weights on every rank just before the launch.  after(r, ctx), if given, runs on every rank's context once all
-    launches are done, before the contexts are closed.
+    set_weights on every rank just before the launch.  before(r, ctx), if given, runs on every rank's context once the ranks
+    are attached, before the first launch; after(r, ctx) runs on every rank's context once all launches are done, before
+    the contexts are closed.
 
     Checks that the replicas, the losses and the exchange's step counts are identical across ranks, and returns
     dict(losses=[K arrays over all steps], w=[K weights], xstats=[K (value words, bitmap words, steps)], after=[K results])."""
@@ -93,6 +94,9 @@ def fused_ranks(data, lam, d, grid_limits, w0, calls, lr, n_train=None, after=No
                 for q in range(K):
                     if q != r:
                         ctxs[r].xchg_attach(q, ctxs[q])
+            if before is not None:
+                for r in range(K):
+                    before(r, ctxs[r])
             out = [None] * K
 
             def rank_fn(r):
