@@ -15,6 +15,7 @@ import numpy as np
 
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
 from ..ml.grad_state import GradState
+from ..ml.lr_schedule import check_schedule, learning_rates
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
@@ -285,7 +286,8 @@ class MasterSync(Master):
     def fit(self, initial_weights: np.ndarray, max_epochs: int, batch_size: int, learning_rate: float,
             stopping_criterion: EarlyStopping, split_strategy: Split = SplitStrategy.vanilla, *,
             virtual_workers: int = 1, on_epoch: Optional[Callable[[int, dict], None]] = None,
-            average_from: Optional[int] = None) -> GradState:
+            average_from: Optional[int] = None, learning_rate_decay: float = 0.0,
+            learning_rate_power: float = 1.0) -> GradState:
         """Master.fit (core/Master.scala:120-218).
 
         virtual_workers (extension): logical reference workers per GPU, so that `node-count` can exceed the
@@ -294,9 +296,16 @@ class MasterSync(Master):
         every step of that epoch and of the later ones to a running sum (ctx.average_begin); the per-epoch evaluations, and
         so the stopping rule, then see the mean of those weights, and `fit` returns it.  history["averaged_steps"] holds
         the number of steps averaged.  None: the last weights, as in the reference.
+        learning_rate_decay, learning_rate_power (extension): step t of the fit (counted from 0 over every epoch) uses
+        learning_rate / (1 + decay * t)^power (ml/lr_schedule.py), handed to the device as a per-step table
+        (ctx.sync_steps_lr).  decay = 0: the constant learning_rate of the reference, through the scalar calls of before.
+        Together with average_from this is Bottou's averaged SGD (power 0.75 in svmasgd).
         """
         if average_from is not None and not 0 <= average_from < max_epochs:
             raise ValueError(f"average_from must lie in [0, max_epochs = {max_epochs}), got {average_from}")
+        check_schedule(learning_rate_decay, learning_rate_power)
+        decaying = learning_rate_decay > 0.0
+        t_global = 0   # global index of the next step: the schedule's t
         W, r, V = self.group.world, self.group.rank, virtual_workers
         K = W * V
         groups = split_strategy(self.n_train, K)             # Master.scala:136 (may hold fewer than K groups)
@@ -364,7 +373,12 @@ class MasterSync(Master):
                     else:
                         flat = np.zeros(0, dtype=np.int32)
                     self.ctx.set_workers(shape, k_total)
-                    ls = self.ctx.sync_steps(flat, int(sum(shape)), j - i, learning_rate, want_losses=True)
+                    if decaying:   # this call's slice of the fit's table: the same on every rank
+                        lrs = learning_rates(learning_rate, learning_rate_decay, learning_rate_power, t_global, j - i)
+                        ls = self.ctx.sync_steps_lr(flat, int(sum(shape)), lrs, want_losses=True)
+                    else:
+                        ls = self.ctx.sync_steps(flat, int(sum(shape)), j - i, learning_rate, want_losses=True)
+                    t_global += j - i
                     self.step_losses.append(ls)
                 # evaluate the resident weights, or while averaging the mean of the averaged steps' weights
                 w = None

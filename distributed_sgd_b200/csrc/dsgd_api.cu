@@ -129,6 +129,7 @@ struct dsgd_ctx {
   dev_buf<int32_t> samples;
   int64_t samples_n = 0;
   dev_buf<double> losses;
+  dev_buf<double> lrs;      // per-step learning rates of a dsgd_sync_steps_lr call that runs the persistent kernel
   dev_buf<double> preds;
   // row ids of a request (forward, gradient, a sampled evaluation; drawn on the device or copied from the host): never the
   // staged stream above
@@ -969,7 +970,14 @@ extern "C" int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYT
 // ---- persistent sync loop (dsgd_persistent.cuh) ----------------------------------------------------------------
 constexpr int kPCons = 8, kPUpd = 6, kPStages = 8, kPStagePairs = 2560, kPMaxChunks = 128;
 using PSmem = PersistSmem<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks>;
-#define DSGD_PERSIST_KERNEL(multi, avg) k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, multi, avg>
+#define DSGD_PERSIST_KERNEL(multi, avg, lr_table) \
+  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, multi, avg, lr_table>
+// every instantiation, indexed [multi][avg][lr_table]
+static void *const kPersistKernels[2][2][2] = {
+    {{(void *)DSGD_PERSIST_KERNEL(false, false, false), (void *)DSGD_PERSIST_KERNEL(false, false, true)},
+     {(void *)DSGD_PERSIST_KERNEL(false, true, false), (void *)DSGD_PERSIST_KERNEL(false, true, true)}},
+    {{(void *)DSGD_PERSIST_KERNEL(true, false, false), (void *)DSGD_PERSIST_KERNEL(true, false, true)},
+     {(void *)DSGD_PERSIST_KERNEL(true, true, false), (void *)DSGD_PERSIST_KERNEL(true, true, true)}}};
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -985,10 +993,10 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
     }
     CU(ctx->p_acc.alloc(3 * kAccStride));
     CU(ctx->p_bar.alloc(4));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true, false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(false, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    CU(cudaFuncSetAttribute((const void *)DSGD_PERSIST_KERNEL(true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    for (int m = 0; m < 2; ++m)
+      for (int a = 0; a < 2; ++a)
+        for (int l = 0; l < 2; ++l)
+          CU(cudaFuncSetAttribute(kPersistKernels[m][a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
   return ctx->p_hinge.grow(ctx, n_steps, 4096);
@@ -1050,9 +1058,10 @@ static bool xchg_complete(const dsgd_ctx *ctx) {
 }
 
 // One launch of the persistent kernel for n_steps SGD steps: on one GPU, or (multi) the fused K-GPU kernel in which every
-// rank aggregates the gradients through the exchange blocks of its peers.
+// rank aggregates the gradients through the exchange blocks of its peers.  lrs_host (n_steps host values) or nullptr: the
+// per-step rates of dsgd_sync_steps_lr, or the scalar lr for every step.
 static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, int64_t n_per_step, int64_t n_steps,
-                       double lr, double *losses_dev) {
+                       double lr, const double *lrs_host, double *losses_dev) {
   int rc = persist_prepare(ctx, n_steps);
   if (rc) return rc;
   const int G = persist_grid(ctx, n_per_step);
@@ -1098,14 +1107,17 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.llw[1] = ctx->x_llw + 2 * xblk_stride(ctx);
     pp.xstats = ctx->x_stats;
   }
-  void *args[] = {&pp};
-  void *fn;
-  if (ctx->avg_on) {   // the averaging instantiations only while averaging is on: otherwise the kernels of before run
-    pp.avg = ctx->avg;
-    fn = multi ? (void *)DSGD_PERSIST_KERNEL(true, true) : (void *)DSGD_PERSIST_KERNEL(false, true);
-  } else {
-    fn = multi ? (void *)DSGD_PERSIST_KERNEL(true, false) : (void *)DSGD_PERSIST_KERNEL(false, false);
+  // The averaging instantiations only while averaging is on, the table ones only for a table: otherwise the kernels of
+  // before run.
+  if (ctx->avg_on) pp.avg = ctx->avg;
+  if (lrs_host) {
+    if ((rc = ctx->lrs.grow(ctx, n_steps, 1024))) return rc;
+    CU(cudaMemcpyAsync(ctx->lrs, lrs_host, sizeof(double) * (size_t)n_steps, cudaMemcpyHostToDevice, ctx->stream));
+    pp.lrs = ctx->lrs;
+    pp.lr = 0.0;   // not read: interval 0, the only one before lrs[0] is loaded, applies no update
   }
+  void *args[] = {&pp};
+  void *fn = kPersistKernels[multi ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
   CU(launch_err);
@@ -1129,6 +1141,7 @@ extern "C" int dsgd_reserve(dsgd_ctx *ctx, int64_t n_samples, int64_t n_steps) {
   int rc = ctx->samples.grow(ctx, n_samples, 1024);
   if (rc) return rc;
   if ((rc = ctx->losses.grow(ctx, n_steps, 1024))) return rc;
+  if ((rc = ctx->lrs.grow(ctx, n_steps, 1024))) return rc;
   if ((rc = persist_prepare(ctx, n_steps))) return rc;
   if (persist_timeline() && !ctx->p_tl) CU(ctx->p_tl.alloc(kTlWords));
   if (ctx->world > 1 && !(ctx->flags & DSGD_FLAG_ASYNC)) {
@@ -1258,8 +1271,11 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
   return DSGD_OK;
 }
 
-extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,
-                                      int want_losses) {
+// The sync steps of dsgd_sync_steps_staged, and of dsgd_sync_steps_lr with lrs (n_steps host values, step s takes lrs[s])
+// instead of the scalar lr.  The per-step paths pass each step's rate as the kernel argument they always take; the
+// persistent and fused kernels read the table on the device (persist_run).
+static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr, const double *lrs,
+                       int want_losses) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "sync step on a ctx created in async mode");
   NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_sync_steps: dimSparsity not set");
@@ -1304,20 +1320,23 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
   if ((single && !logistic && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
     // exchange block mapped (fused): the same kernel aggregates over NVLink
-    return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, want_losses ? ctx->losses.p : nullptr);
+    return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, lrs,
+                       want_losses ? ctx->losses.p : nullptr);
   }
+  double lr_s = lr;   // the rate of step s
   // k_update, or while averaging k_update_avg: the same update, then avg += the new weights
   auto update = [&](auto kernel, auto kernel_avg, double *gbuf, double k_den, double n_local, double *loss_dev) {
     if (ctx->avg_on)
-      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr, k_den,
+      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
                                                       ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
     else
-      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr, k_den, ctx->scal,
-                                                  ctx->cnt, ctx->partial, n_local, loss_dev);
+      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
+                                                  ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev);
     LAUNCHED();
     if (ctx->avg_on) ++ctx->avg_n;
   };
   for (int64_t s = 0; s < n_steps; ++s) {
+    if (lrs) lr_s = lrs[s];
     const int32_t *smp = ctx->samples + first + s * n_per_step;
     double *loss_dev = want_losses ? ctx->losses + s : nullptr;
     if (single) {
@@ -1376,6 +1395,11 @@ extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_pe
   return DSGD_OK;
 }
 
+extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,
+                                      int want_losses) {
+  return sync_staged(ctx, first, n_per_step, n_steps, lr, nullptr, want_losses);
+}
+
 extern "C" int dsgd_read_losses(dsgd_ctx *ctx, double *losses_out, int64_t n_steps) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(losses_out && n_steps >= 0 && n_steps <= ctx->losses.cap, DSGD_ERR_INVALID, "dsgd_read_losses: bad arguments");
@@ -1386,18 +1410,32 @@ extern "C" int dsgd_read_losses(dsgd_ctx *ctx, double *losses_out, int64_t n_ste
   return persist_check(ctx);
 }
 
-extern "C" int dsgd_sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, double lr,
-                               double *losses_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
+// dsgd_sync_steps, and dsgd_sync_steps_lr with lrs != nullptr
+static int sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, double lr,
+                      const double *lrs, double *losses_out) {
   NEED(n_steps >= 0 && n_per_step >= 0, DSGD_ERR_INVALID, "dsgd_sync_steps: bad arguments");
   NEED(n_per_step > 0 || ctx->n_local == 0, DSGD_ERR_EMPTY,
        "dsgd_sync_steps: empty batch (Vec.sum of an empty list throws in the reference)");
   int rc = dsgd_stage_samples(ctx, samples, n_per_step * n_steps);
   if (rc) return rc;
-  if ((rc = dsgd_sync_steps_staged(ctx, 0, n_per_step, n_steps, lr, losses_out != nullptr))) return rc;
+  if ((rc = sync_staged(ctx, 0, n_per_step, n_steps, lr, lrs, losses_out != nullptr))) return rc;
   if (losses_out) return dsgd_read_losses(ctx, losses_out, n_steps);
   CU(cudaStreamSynchronize(ctx->stream));
   return persist_check(ctx);
+}
+
+extern "C" int dsgd_sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, double lr,
+                               double *losses_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  return sync_steps(ctx, samples, n_per_step, n_steps, lr, nullptr, losses_out);
+}
+
+extern "C" int dsgd_sync_steps_lr(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps,
+                                  const double *lrs, double *losses_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_sync_steps_lr: ctx is in async mode (Hogwild keeps its constant rate)");
+  NEED(lrs || n_steps <= 0, DSGD_ERR_INVALID, "dsgd_sync_steps_lr: lrs is NULL");
+  return sync_steps(ctx, samples, n_per_step, n_steps, 0.0, lrs, losses_out);
 }
 
 extern "C" int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, double lr, double *loss_out) {

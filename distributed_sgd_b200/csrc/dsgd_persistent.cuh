@@ -91,6 +91,8 @@ struct PersistParams {
   unsigned long long *xstats;             // [0] value words, [1] bitmap words this rank pushed to ONE peer (diagnostic)
   // ---- averaged SGD (kAvg); last, so that the parameter offsets of the other instantiations stay where they were ----
   double *avg;                            // [dim] running sum of W_t over the averaged steps: read at launch, written at exit
+  // ---- per-step learning rates (kLrTable); last for the same reason ----
+  const double *lrs;                      // [n_steps]: step s of this launch uses lrs[s] instead of lr
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -471,7 +473,10 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
 // added), in step order, in plain fp64.  One GPU: the update threads keep the sums of their register columns in registers
 // (loaded at launch start, stored in the epilogue); the columns past the register ones read-modify-write p.avg every step.
 // K GPUs: the column thread keeps its column's sum in a register.
-template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg>
+// kLrTable: step s of the launch takes the rate p.lrs[s] instead of p.lr.  Interval t applies the update of step t-1 (the
+// consumers' on-the-fly fetch, the update warps, the K-GPU column threads), so all of them use lrs[t-1]; interval 0
+// applies no update.
+template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -589,7 +594,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   // =========================================================================================================
   // barrier-synchronised warps (consumers + updaters)
   // =========================================================================================================
-  const double lr = p.lr;
+  double lr = p.lr;   // kLrTable: the rate of the update this interval applies (installed after the barrier that opens it)
   const int64_t base = kMulti ? p.step_base : 0;
   unsigned phase = 0;
   // one GPU: the update threads of all CTAs stride over the columns
@@ -653,6 +658,14 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     long long *tl_rec = tl_cta ? p.tl + 256 * 16 + ((t - kTlFirst) * kTlCtas + blockIdx.x) * kTlPerCta : nullptr;
     long long *tl_row = (p.tl && blockIdx.x == 0 && t < 256) ? p.tl + t * 16 : nullptr;
     bool ok = true;
+    // kLrTable: the rate of step t, which interval t+1 applies, requested now, a whole interval before it is needed, and
+    // installed after this interval's barrier.  The load completes while the interval works, so neither the barrier
+    // (whose release arrival orders the thread's earlier memory operations) nor the next interval's update, which is on
+    // the critical path, waits for it.
+    double lr_next = lr;
+    if constexpr (kLrTable) {
+      if (!last) lr_next = __ldg(&p.lrs[t]);
+    }
     if (warp == 0) DSGD_TL(0);
 
     // ---- update warp 0, first thing: c_{T-1} and ||W_{T-1}||^2 from the partials the last barrier delivered ----
@@ -962,6 +975,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     }
     named_bar_sync(3, kSyncThreads);
     if (*(volatile int *)&sm.ok == 0) return;
+    if constexpr (kLrTable) lr = lr_next;
     { const int a = gi_prev; gi_prev = gi_cur; gi_cur = gi_next; gi_next = a; }
     { const int a = ti_prev; ti_prev = ti_cur; ti_cur = ti_next; ti_next = a; }
   }

@@ -52,6 +52,9 @@ object DsgdNative {
   @native def streamExactRows(ctx: Long, out: Array[Long]): Int // diagnostic: rows of streaming passes recomputed in fp64
   @native def setWorkers(ctx: Long, counts: Array[Int], kTotal: Int): Int
   @native def syncSteps(ctx: Long, samples: Array[Int], nPerStep: Long, nSteps: Long, lr: Double, losses: Array[Double]): Int
+  // the same with one learning rate per step: step s uses lrs(s) (every rank passes the same table)
+  @native def syncStepsLr(ctx: Long, samples: Array[Int], nPerStep: Long, nSteps: Long, lrs: Array[Double],
+                          losses: Array[Double]): Int
   // averaged SGD (sync mode): every sync step after averageBegin adds its new weights to a device-side sum until averageEnd;
   // averageWeights: avg = the mean of those weights, nSteps(0) = how many (either may be null)
   @native def averageBegin(ctx: Long): Int

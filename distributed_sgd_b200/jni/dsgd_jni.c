@@ -263,6 +263,19 @@ FN(syncSteps)(JNIEnv *env, jobject self, jlong h, jintArray samples, jlong n_per
   free(bs.p);
   return rc;
 }
+/* the same with a learning rate per step: lrs(s) for step s (a decaying schedule inside one call) */
+FN(syncStepsLr)(JNIEnv *env, jobject self, jlong h, jintArray samples, jlong n_per_step, jlong n_steps, jdoubleArray lrs,
+                jdoubleArray losses) {
+  buf_t bs = in_Int(env, samples), br = in_Double(env, lrs), bl = out_Double(env, losses);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bs.bad | br.bad | bl.bad)) {
+    if ((jlong)bs.n < n_per_step * n_steps || (jlong)br.n < n_steps || (bl.p && (jlong)bl.n < n_steps)) rc = DSGD_ERR_INVALID;
+    else rc = dsgd_sync_steps_lr(CTX(h), bs.p, n_per_step, n_steps, br.p, bl.p);
+  }
+  back_Double(env, losses, bl, rc);
+  free(bs.p); free(br.p);
+  return rc;
+}
 /* averaged SGD: begin zeroes the device-side sum, every following sync step adds its new weights; avg(dim) = the mean,
  * nSteps(0) = the number of steps averaged (either array may be null) */
 FN(averageBegin)(JNIEnv *env, jobject self, jlong h) { return dsgd_average_begin(CTX(h)); }

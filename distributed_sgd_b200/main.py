@@ -32,6 +32,9 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         raise ValueError("model = logistic: asynchronous (Hogwild) training supports the svm model only")
     if cfg.average_from >= 0 and cfg.is_async:
         raise ValueError("average-from: averaged SGD is a sync-mode option; asynchronous (Hogwild) training does not average")
+    if cfg.learning_rate_decay != 0.0 and cfg.is_async:
+        raise ValueError("learning-rate-decay: the decaying learning rate is a sync-mode option; asynchronous (Hogwild) "
+                         "training keeps its constant rate")
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
     model = SparseLogistic(cfg.lam) if cfg.model == "logistic" else SparseSVM(cfg.lam)
@@ -43,7 +46,7 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     w0 = np.zeros(data.dim)                                                    # data(0)._1.zerosLike (Main.scala:74)
     report = {"config": {k: getattr(cfg, k) for k in ("batch_size", "learning_rate", "lam", "node_count", "is_async",
                                                       "max_epochs", "check_every", "leaky_loss", "patience", "conv_delta",
-                                                      "model")},
+                                                      "model", "learning_rate_decay", "learning_rate_power")},
               "rows": {"train": train.n_rows, "test": test.n_rows}, "world": world}
     report["initial_loss"] = master.distributed_loss(w0)                      # Main.scala:75-76
     report["initial_accuracy"] = master.distributed_accuracy(w0)              # Main.scala:77-78
@@ -57,7 +60,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
             raise ValueError(f"node-count {cfg.node_count} is not a multiple of the {world} GPU processes")
         state = master.fit(w0, cfg.max_epochs, cfg.batch_size, cfg.learning_rate, stop,
                            virtual_workers=cfg.node_count // world,
-                           average_from=cfg.average_from if cfg.average_from >= 0 else None)
+                           average_from=cfg.average_from if cfg.average_from >= 0 else None,
+                           learning_rate_decay=cfg.learning_rate_decay, learning_rate_power=cfg.learning_rate_power)
     report["fit_seconds"] = time.perf_counter() - t0                          # Measure.durationLog(log, "fit") (Main.scala:80)
     w1 = state.grad
     report["history"] = {k: [float(x) for x in v] for k, v in getattr(master, "history", {}).items()

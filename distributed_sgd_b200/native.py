@@ -114,6 +114,7 @@ ABI = {
     "dsgd_set_workers": [_vp, _i32, _vp, _i32],
     "dsgd_sync_step": [_vp, _vp, _i64, _f64, C.POINTER(_f64)],
     "dsgd_sync_steps": [_vp, _vp, _i64, _i64, _f64, _vp],
+    "dsgd_sync_steps_lr": [_vp, _vp, _i64, _i64, _vp, _vp],
     "dsgd_stage_samples": [_vp, _vp, _i64],
     "dsgd_sync_steps_staged": [_vp, _i64, _i64, _i64, _f64, C.c_int],
     "dsgd_read_losses": [_vp, _vp, _i64],
@@ -448,6 +449,15 @@ class NativeCtx:
         samples = _arr(samples, np.int32, n_per_step * n_steps, "samples")
         losses = np.zeros(n_steps, dtype=np.float64) if want_losses else None
         self._ck(self._l.dsgd_sync_steps(self._h, _ptr(samples), n_per_step, n_steps, lr, _ptr(losses)))
+        return losses
+
+    def sync_steps_lr(self, samples, n_per_step: int, lrs, want_losses: bool = True):
+        """len(lrs) steps; step s uses the learning rate lrs[s] (exactly len(lrs) one-step sync_steps calls)."""
+        lrs = _arr(lrs, np.float64)
+        n_steps = lrs.size
+        samples = _arr(samples, np.int32, n_per_step * n_steps, "samples")
+        losses = np.zeros(n_steps, dtype=np.float64) if want_losses else None
+        self._ck(self._l.dsgd_sync_steps_lr(self._h, _ptr(samples), n_per_step, n_steps, _ptr(lrs), _ptr(losses)))
         return losses
 
     def stage_samples(self, samples):

@@ -33,6 +33,8 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     patience: int = 5
     model: str = "svm"            # extension: "svm" (SparseSVM) or "logistic" (SparseLogistic, sync mode only)
     average_from: int = -1        # extension: averaged SGD from this epoch (0-based) on, sync mode only; -1: off
+    learning_rate_decay: float = 0.0   # extension: step t uses learning-rate / (1 + decay * t)^power, sync mode only
+    learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -45,6 +47,8 @@ _KEYS = {
     "check-every": ("check_every", "DSGD_CHECK_EVERY"), "leaky-loss": ("leaky_loss", "DSGD_LEAKY_LOSS"),
     "patience": ("patience", "DSGD_PATIENCE"), "conv-delta": ("conv_delta", "DSGD_CONV_DELTA"),
     "model": ("model", "DSGD_MODEL"), "average-from": ("average_from", "DSGD_AVERAGE_FROM"),
+    "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
+    "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -112,4 +116,8 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"model: expected one of {', '.join(MODELS)}, got {cfg.model!r}")
     if cfg.average_from < -1:
         raise ValueError(f"average-from: expected an epoch >= 0, or -1 for off, got {cfg.average_from}")
+    if not cfg.learning_rate_decay >= 0.0:
+        raise ValueError(f"learning-rate-decay: expected a value >= 0, got {cfg.learning_rate_decay}")
+    if not cfg.learning_rate_power > 0.0:
+        raise ValueError(f"learning-rate-power: expected a value > 0, got {cfg.learning_rate_power}")
     return cfg

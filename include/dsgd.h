@@ -85,7 +85,7 @@ int dsgd_launch_count(const dsgd_ctx *ctx, int64_t *count);
 int dsgd_profile_begin(dsgd_ctx *ctx, int32_t sample_every);
 int dsgd_profile_end(dsgd_ctx *ctx, float *mean_ms, int64_t *n_sampled);
 /* Optional: allocate every device buffer the sync path needs for calls of up to n_samples sample ids and n_steps steps
- * now (staging, per-step losses, the persistent kernel's buffers, the exchange's weight words) instead of on first
+ * now (staging, per-step losses and learning rates, the persistent kernel's buffers, the exchange's weight words) instead of on first
  * use.  cudaMalloc synchronises the whole device: a host that drives several contexts on ONE GPU from several threads
  * must reserve before the first fused step, or a rank allocating late waits for a rank that already runs and waits for
  * it.  (One context per GPU never needs this.) */
@@ -213,6 +213,16 @@ int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, double lr, 
  * n_steps * n_per_step indices, step-major.  losses_out (optional) holds n_steps values. */
 int dsgd_sync_steps(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, double lr,
                     double *losses_out);
+/* The same with one learning rate per step (a decaying schedule inside one call): `lrs` holds n_steps rates in host
+ * memory and step s uses lrs[s].  One call gives exactly what n_steps calls of dsgd_sync_steps would, each taking one
+ * step with its scalar lrs[s]: weights, losses, the resident state and the averaging sum and count, bit for bit.  The
+ * arguments are checked as in dsgd_sync_steps; lrs == NULL with n_steps > 0 -> DSGD_ERR_INVALID, an async ctx ->
+ * DSGD_ERR_STATE; the rates themselves are not checked (nor is a scalar lr).  Every rank of a multi-rank step passes
+ * the same table, as every rank passes the same scalar lr to dsgd_sync_steps.  The table is copied to the device on
+ * the ctx's stream into a buffer that dsgd_reserve(.., n_steps) sizes in advance (K contexts sharing ONE GPU reserve
+ * before their threads start stepping, as for the per-step losses). */
+int dsgd_sync_steps_lr(dsgd_ctx *ctx, const int32_t *samples, int64_t n_per_step, int64_t n_steps, const double *lrs,
+                       double *losses_out);
 /* The same split in three, so a host can keep the index stream resident: stage = H2D of the sample slices
  * (the `samples` field of GradientRequest, protobuf/proto.proto:60-63); run = device only; read = D2H.  The stream stays
  * until the next dsgd_stage_samples, dsgd_sync_step or dsgd_sync_steps (which stage their own samples and so replace it)
