@@ -2,6 +2,7 @@
 // There is no CPU path in this library: without a usable GPU dsgd_create fails with DSGD_ERR_CUDA.
 #include "../../include/dsgd.h"
 
+#include <cuda.h>  // driver types only: entry points are looked up through the runtime (load_all_kernels)
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <nccl.h>  // types only: the library itself is bound at run time (see nccl_api)
@@ -305,6 +306,10 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: bad rank/world %d/%d", rank, world);
   if ((flags & DSGD_FLAG_LOGISTIC) && (flags & DSGD_FLAG_ASYNC))
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports the SVM model only");
+  // every async worker pushes each delta into all `world` replicas and the master's, through one table of kMaxReplicas slots
+  if ((flags & DSGD_FLAG_ASYNC) && world > kMaxReplicas - 1)
+    return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports at most %d workers (got world %d)",
+                kMaxReplicas - 1, world);
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
   if (e != cudaSuccess || n_dev == 0)
@@ -1532,6 +1537,8 @@ extern "C" int dsgd_peer_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer, in
        "dsgd_peer_attach: peer_rank %d outside [0,%d]", peer_rank, ctx->world);
   NEED(which == DSGD_REPLICA_SELF || peer->m_w, DSGD_ERR_STATE, "dsgd_peer_attach: peer does not host the master replica");
   NEED(peer->dim == ctx->dim, DSGD_ERR_INVALID, "dsgd_peer_attach: dimension mismatch");
+  // the running loop copied the replica table when it started: a replica attached now would never receive a delta
+  NEED(!ctx->a_running, DSGD_ERR_STATE, "dsgd_peer_attach: async computation is running");
   int rc = enable_peer_access(ctx, peer, "dsgd_peer_attach");
   if (rc) return rc;
   ctx->peer_w[peer_rank].set(which == DSGD_REPLICA_SELF ? peer->w.p : peer->m_w.p, false);
@@ -1542,6 +1549,38 @@ static double *master_replica(dsgd_ctx *ctx) {
   return ctx->m_w ? ctx->m_w.p : (ctx->world < kMaxReplicas ? ctx->peer_w[ctx->world].p : nullptr);
 }
 
+// CUDA loads a kernel when it is first launched (lazy loading, the default since CUDA 12.2), and loading may wait for every
+// kernel running on the device.  An async loop started by dsgd_start_async runs until it is stopped, so the first launch of
+// any other kernel while it runs -- an evaluation of the master's weights in MasterAsync.fit, a request, another context's
+// loop -- would wait for it forever.  Before the first async loop on a device, every kernel of the library is loaded.
+static int load_all_kernels(dsgd_ctx *ctx) {
+  static std::mutex mu;
+  static std::vector<int> done;   // devices whose kernels are loaded in this process
+  std::lock_guard<std::mutex> lock(mu);
+  if (std::find(done.begin(), done.end(), ctx->device) != done.end()) return DSGD_OK;
+  void *get_module = nullptr, *count = nullptr, *enumerate = nullptr, *load = nullptr;
+  cudaDriverEntryPointQueryResult q[4];
+  CU(cudaGetDriverEntryPointByVersion("cuFuncGetModule", &get_module, 12040, cudaEnableDefault, &q[0]));
+  CU(cudaGetDriverEntryPointByVersion("cuModuleGetFunctionCount", &count, 12040, cudaEnableDefault, &q[1]));
+  CU(cudaGetDriverEntryPointByVersion("cuModuleEnumerateFunctions", &enumerate, 12040, cudaEnableDefault, &q[2]));
+  CU(cudaGetDriverEntryPointByVersion("cuFuncLoad", &load, 12040, cudaEnableDefault, &q[3]));
+  for (int i = 0; i < 4; ++i)
+    NEED(q[i] == cudaDriverEntryPointSuccess, DSGD_ERR_CUDA, "async loop: the CUDA driver cannot preload kernels (needs 12.4)");
+  cudaFunction_t any = nullptr;
+  CU(cudaGetFuncBySymbol(&any, reinterpret_cast<const void *>(k_async_worker_b1)));
+  CUmodule mod = nullptr;
+  unsigned n = 0;
+  CUresult r = reinterpret_cast<CUresult (*)(CUmodule *, CUfunction)>(get_module)(&mod, any);
+  if (r == CUDA_SUCCESS) r = reinterpret_cast<CUresult (*)(unsigned *, CUmodule)>(count)(&n, mod);
+  std::vector<CUfunction> fns(n);
+  if (r == CUDA_SUCCESS && n)
+    r = reinterpret_cast<CUresult (*)(CUfunction *, unsigned, CUmodule)>(enumerate)(fns.data(), n, mod);
+  for (unsigned i = 0; i < n && r == CUDA_SUCCESS; ++i) r = reinterpret_cast<CUresult (*)(CUfunction)>(load)(fns[i]);
+  NEED(r == CUDA_SUCCESS, DSGD_ERR_CUDA, "async loop: loading the library's kernels failed (CUresult %d)", (int)r);
+  done.push_back(ctx->device);
+  return DSGD_OK;
+}
+
 static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned, int64_t n_assigned, const int32_t *replay,
                         int32_t batch, double lr, int32_t lanes, int64_t max_updates, uint64_t seed, cudaStream_t st) {
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot initialize async computation: slave is in synchronous mode.");
@@ -1550,7 +1589,8 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   NEED(ctx->pairs && ctx->have_d, DSGD_ERR_STATE, "dsgd_start_async: rows or dimSparsity missing");
   NEED(batch >= 1 && lanes >= 1 && lanes <= 4096, DSGD_ERR_INVALID, "dsgd_start_async: bad arguments");
   CU(cudaSetDevice(ctx->device));
-  int rc = DSGD_OK;
+  int rc = load_all_kernels(ctx);
+  if (rc) return rc;
   if (w0) {  // weights() = request.weights
     CU(cudaMemcpyAsync(ctx->w, w0, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
     rc = refresh_resident(ctx);  // also S = w . d and the control slots of the replica

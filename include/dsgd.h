@@ -254,7 +254,11 @@ int dsgd_average_weights(dsgd_ctx *ctx, double *avg_out, int64_t *n_steps_out);
  *      Replaces the slave<->slave and slave->master channels (core/Slave.scala:23,26; core/Master.scala:
  *      229-233).  `which`: DSGD_REPLICA_SELF = this worker's replica; DSGD_REPLICA_MASTER = the master's replica
  *      (GradState.grad + the update counter, core/MasterAsync.scala:66,164-177), hosted by the ctx that calls
- *      dsgd_async_host_master.  peer_rank in dsgd_ipc_import: 0..world-1, or `world` for the master replica. */
+ *      dsgd_async_host_master.  peer_rank in dsgd_ipc_import: 0..world-1, or `world` for the master replica.
+ *      A worker's delta goes to at most 17 replicas (its own, 15 peers and the master; an outbox takes one of them), so
+ *      dsgd_create with DSGD_FLAG_ASYNC refuses world > 16 with DSGD_ERR_INVALID (sync mode has no such bound).  A running
+ *      loop keeps the replica table it started with: dsgd_ipc_import and dsgd_peer_attach fail with DSGD_ERR_STATE while
+ *      it runs. */
 #define DSGD_REPLICA_SELF 0
 #define DSGD_REPLICA_MASTER 1
 int dsgd_async_host_master(dsgd_ctx *ctx, const double *w0);
@@ -269,7 +273,9 @@ int dsgd_peer_attach(dsgd_ctx *ctx, int peer_rank, dsgd_ctx *peer, int which);
  * `assigned` (core/Slave.scala:84,87; batch > 1 indexes rows by POSITION like the reference, quirk Q6).
  * w0 == NULL keeps the resident replica: initialise every replica with dsgd_set_weights first, then start the
  * loops, and no delta a faster peer pushes early is overwritten (the reference has that start-up race).
- * Returns immediately; the loop runs on its own stream. */
+ * Returns immediately; the loop runs on its own stream.  The first async loop on a device (this call or dsgd_async_replay)
+ * first loads every kernel of the library, so that no later call waits for the running loop to load one (CUDA loads kernels
+ * lazily by default); that needs a driver for CUDA 12.4 or later, else DSGD_ERR_CUDA. */
 int dsgd_start_async(dsgd_ctx *ctx, const double *w0, const int32_t *assigned, int64_t n_assigned, int32_t batch,
                      double lr, int32_t concurrency, int64_t max_updates, uint64_t seed);
 /* The same loop body over a RECORDED sampling sequence (n_updates * batch row ids), one lane, blocking: the

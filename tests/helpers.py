@@ -25,6 +25,131 @@ def data_from_csr(rp, col, val, lab, dim):
                 np.asarray(lab, np.int8), dim)
 
 
+# ---- async (Hogwild) test data ----------------------------------------------------------------------------------------
+
+LENGTHS = [0, 1, 2, 127, 128, 129, 130, 255, 256, 257, 2000]   # pairs: odd lengths get one padding pair
+
+
+def csr(rows, labels, dim):
+    """rows: list of (cols, vals) in storage order."""
+    rp = np.zeros(len(rows) + 1, np.int64)
+    rp[1:] = np.cumsum([len(c) for c, _ in rows])
+    col = np.concatenate([np.asarray(c, np.int32) for c, _ in rows]) if rp[-1] else np.zeros(0, np.int32)
+    val = np.concatenate([np.asarray(v, np.float32) for _, v in rows]) if rp[-1] else np.zeros(0, np.float32)
+    return data_from_csr(rp, col, val, labels, dim)
+
+
+def dyadic(rng, n):
+    return rng.integers(1, 1025, size=n) / 256.0                 # multiples of 2^-8 in [2^-8, 4]
+
+
+def edge_rows(seed, dim=4099, n_rows=330):
+    """Every length of LENGTHS in sorted, descending and random column order; short rows draw their columns from a
+    512-column pool (so the rows of a batch share most of their columns), 2000-long rows from the whole range; every
+    fifth row holds columns 0 and dim - 1."""
+    rng = np.random.default_rng(seed)
+    pool = np.concatenate([[0, dim - 1], rng.choice(np.arange(1, dim - 1), size=510, replace=False)])
+    rows = []
+    for i in range(n_rows):
+        n = LENGTHS[i % len(LENGTHS)]
+        src = pool if n <= len(pool) else np.arange(dim)
+        cols = rng.choice(src, size=n, replace=False)
+        if i % 5 == 0 and n >= 2:
+            rest = cols[(cols != 0) & (cols != dim - 1)][:n - 2]
+            cols = np.concatenate([[0, dim - 1], rest])
+        order = (i // len(LENGTHS)) % 3
+        cols = np.sort(cols) if order == 0 else (np.sort(cols)[::-1] if order == 1 else rng.permutation(cols))
+        rows.append((cols, dyadic(rng, n)))
+    labels = rng.choice(np.array([-1, 1], np.int8), size=n_rows)
+    w0 = np.where(rng.random(dim) < 0.5, rng.integers(-256, 257, size=dim) / 64.0, 0.0)
+    return csr(rows, labels, dim), w0
+
+
+EPS = 1e-20
+
+
+def filter_case(name):
+    """One edge of the reference's 1e-20 filter: (rows, labels, dim, d, lam, lr, w0); a replay makes one update per row,
+    in row order."""
+    dim = 8
+    d = np.zeros(dim)
+    w0 = np.zeros(dim)
+    if name == "residual":            # w - delta = 2^-72 ~ 2.1e-22: the entry must leave the map
+        w0[3] = 2.0 ** -20 + 2.0 ** -72
+        return [([3], [2.0 ** -20])], [1], dim, d, 0.0, 1.0, w0
+    if name == "tiny_product":        # x . w = 2^-80 <= 1e-20 is dropped: dot 0, y = -1 passes the gate
+        w0[2] = 2.0 ** -40
+        return [([2, 5], [2.0 ** -40, 0.5])], [-1], dim, d, 0.0, 1.0, w0
+    if name in ("c_at_eps", "c_above_eps"):   # S = 1, lambda = 1e-20 / 2: c = 1e-20 exactly (not added), or one ulp above
+        w0[0], d[0] = 1.0, 1.0
+        lam = EPS / 2 if name == "c_at_eps" else np.nextafter(EPS / 2, 1.0)
+        return [([4], [2.0 ** -66])], [1], dim, d, lam, 1.0, w0
+    if name == "cancel":              # m + c == 0 on column 1: the key leaves the delta; column 6 moves S for update 2
+        w0[0], d[0], d[1], d[6] = -1.0, 1.0, 0.5, 0.5
+        return [([1, 6], [0.5, 0.25]), ([6, 1], [0.25, 0.5])], [1, 1], dim, d, 0.25, 0.5, w0
+    if name == "tiny_delta":          # (m + c) * lr = 2^-69 <= 1e-20 on column 1: no delta, and S must not move (d = 2^40)
+        w0[0], d[0], d[1] = 2.0 ** -20, 1.0, 2.0 ** 40
+        return [([1, 2], [2.0 ** -40, 1.0]), ([3], [1.0])], [1, 1], dim, d, 2.0 ** -21, 2.0 ** -30, w0
+    raise KeyError(name)
+
+
+FILTER_CASES = ["residual", "tiny_product", "c_at_eps", "c_above_eps", "cancel", "tiny_delta"]
+
+
+def filter_expect(name):
+    """{column: exact weight} after the replay of filter_case(name)."""
+    return {
+        "residual": {3: 0.0},
+        "tiny_product": {2: 2.0 ** -39, 5: 0.5},
+        "c_at_eps": {4: -(2.0 ** -66)},
+        "c_above_eps": {4: -(2.0 ** -66 + np.nextafter(EPS, 1.0))},
+        # update 1: column 1 cancels, column 6 -> 0.125 and S -> -0.9375; update 2 reads that S: c = -0.46875
+        "cancel": {1: -0.015625, 6: 0.234375},
+        "tiny_delta": {1: 0.0, 2: -(1.0 + 2.0 ** -40) * 2.0 ** -30, 3: -(1.0 + 2.0 ** -40) * 2.0 ** -30},
+    }[name]
+
+
+def conservation_rows():
+    """4096 rows of 8 entries 2^-4 over 4096 columns, y = +1: from w0 = 2^10 with lr = 2^-6 the gate always passes and every
+    partial sum of deltas is exact in any order.  Returns (data, entries per row)."""
+    rng = np.random.default_rng(77)
+    dim, n, k = 4096, 4096, 8
+    rows = [(np.sort(rng.choice(dim, size=k, replace=False)), np.full(k, 2.0 ** -4)) for _ in range(n)]
+    return csr(rows, np.ones(n, np.int8), dim), k
+
+
+def async_workers(data, lam, d, K, w0=None, master=True, outbox=False):
+    """K async contexts on device 0 (rank r of world K), `data` loaded and dimSparsity d installed, every context attached
+    to every other's replica with dsgd_peer_attach.  master: rank 0 hosts the master replica and ranks 1..K-1 attach it at
+    peer_rank K.  Every replica, the master's included, starts from w0 (None: zeros); outbox: every worker's outbox is
+    enabled (and empty).  The caller closes the contexts."""
+    from distributed_sgd_b200.native import REPLICA_MASTER, REPLICA_SELF, NativeCtx
+    w0 = np.zeros(data.dim) if w0 is None else np.asarray(w0, np.float64)
+    ctxs = []
+    try:
+        for r in range(K):
+            ctx = NativeCtx(0, data.dim, lam, rank=r, world=K, is_async=True)
+            ctxs.append(ctx)
+            ctx.load_csr(data.row_ptr, data.col, data.val, data.label)
+            ctx.set_dim_sparsity(d)
+            ctx.set_weights(w0)
+        if master:
+            ctxs[0].async_host_master(w0)
+        for r in range(K):
+            for q in range(K):
+                if q != r:
+                    ctxs[r].peer_attach(q, ctxs[q], REPLICA_SELF)
+            if master and r != 0:
+                ctxs[r].peer_attach(K, ctxs[0], REPLICA_MASTER)
+            if outbox:
+                ctxs[r].async_outbox_enable()
+    except BaseException:
+        for c in ctxs:
+            c.close()
+        raise
+    return ctxs
+
+
 # ---- K ranks of the fused peer-exchange sync step sharing one GPU ----------------------------------------------------
 
 def run_ranks(fns):

@@ -14,46 +14,9 @@ import time
 import numpy as np
 import pytest
 
-from helpers import data_from_csr, make_pair
+from helpers import FILTER_CASES, conservation_rows, csr, edge_rows, filter_case, filter_expect, make_pair
 
 pytestmark = pytest.mark.gpu
-
-LENGTHS = [0, 1, 2, 127, 128, 129, 130, 255, 256, 257, 2000]   # pairs: odd lengths get one padding pair
-
-
-def _csr(rows, labels, dim):
-    """rows: list of (cols, vals) in storage order."""
-    rp = np.zeros(len(rows) + 1, np.int64)
-    rp[1:] = np.cumsum([len(c) for c, _ in rows])
-    col = np.concatenate([np.asarray(c, np.int32) for c, _ in rows]) if rp[-1] else np.zeros(0, np.int32)
-    val = np.concatenate([np.asarray(v, np.float32) for _, v in rows]) if rp[-1] else np.zeros(0, np.float32)
-    return data_from_csr(rp, col, val, labels, dim)
-
-
-def _dyadic(rng, n):
-    return rng.integers(1, 1025, size=n) / 256.0                 # multiples of 2^-8 in [2^-8, 4]
-
-
-def _edge_rows(seed, dim=4099, n_rows=330):
-    """Every length of LENGTHS in sorted, descending and random column order; short rows draw their columns from a
-    512-column pool (so the rows of a batch share most of their columns), 2000-long rows from the whole range; every
-    fifth row holds columns 0 and dim - 1."""
-    rng = np.random.default_rng(seed)
-    pool = np.concatenate([[0, dim - 1], rng.choice(np.arange(1, dim - 1), size=510, replace=False)])
-    rows = []
-    for i in range(n_rows):
-        n = LENGTHS[i % len(LENGTHS)]
-        src = pool if n <= len(pool) else np.arange(dim)
-        cols = rng.choice(src, size=n, replace=False)
-        if i % 5 == 0 and n >= 2:
-            rest = cols[(cols != 0) & (cols != dim - 1)][:n - 2]
-            cols = np.concatenate([[0, dim - 1], rest])
-        order = (i // len(LENGTHS)) % 3
-        cols = np.sort(cols) if order == 0 else (np.sort(cols)[::-1] if order == 1 else rng.permutation(cols))
-        rows.append((cols, _dyadic(rng, n)))
-    labels = rng.choice(np.array([-1, 1], np.int8), size=n_rows)
-    w0 = np.where(rng.random(dim) < 0.5, rng.integers(-256, 257, size=dim) / 64.0, 0.0)
-    return _csr(rows, labels, dim), w0
 
 
 def _batches(rng, n_rows, batch, n_updates):
@@ -62,7 +25,7 @@ def _batches(rng, n_rows, batch, n_updates):
 
 @pytest.fixture(scope="module")
 def edge_data():
-    return _edge_rows(21)
+    return edge_rows(21)
 
 
 # ---- a. replay: bit for bit at lambda = 0, and at the stated tolerance with lambda > 0 ---------------------------------
@@ -101,41 +64,11 @@ def test_replay_with_regularizer(edge_data, batch, n_updates):
 
 # ---- b. the 1e-20 filter, one or two hand-built updates through both kernels -------------------------------------------
 
-EPS = 1e-20
-
-
-def _filter_case(name):
-    """(rows, labels, dim, d, lam, lr, w0, n_updates of the replay: each update is the next row)."""
-    dim = 8
-    d = np.zeros(dim)
-    w0 = np.zeros(dim)
-    if name == "residual":            # w - delta = 2^-72 ~ 2.1e-22: the entry must leave the map
-        w0[3] = 2.0 ** -20 + 2.0 ** -72
-        return [([3], [2.0 ** -20])], [1], dim, d, 0.0, 1.0, w0
-    if name == "tiny_product":        # x . w = 2^-80 <= 1e-20 is dropped: dot 0, y = -1 passes the gate
-        w0[2] = 2.0 ** -40
-        return [([2, 5], [2.0 ** -40, 0.5])], [-1], dim, d, 0.0, 1.0, w0
-    if name in ("c_at_eps", "c_above_eps"):   # S = 1, lambda = 1e-20 / 2: c = 1e-20 exactly (not added), or one ulp above
-        w0[0], d[0] = 1.0, 1.0
-        lam = EPS / 2 if name == "c_at_eps" else np.nextafter(EPS / 2, 1.0)
-        return [([4], [2.0 ** -66])], [1], dim, d, lam, 1.0, w0
-    if name == "cancel":              # m + c == 0 on column 1: the key leaves the delta; column 6 moves S for update 2
-        w0[0], d[0], d[1], d[6] = -1.0, 1.0, 0.5, 0.5
-        return [([1, 6], [0.5, 0.25]), ([6, 1], [0.25, 0.5])], [1, 1], dim, d, 0.25, 0.5, w0
-    if name == "tiny_delta":          # (m + c) * lr = 2^-69 <= 1e-20 on column 1: no delta, and S must not move (d = 2^40)
-        w0[0], d[0], d[1] = 2.0 ** -20, 1.0, 2.0 ** 40
-        return [([1, 2], [2.0 ** -40, 1.0]), ([3], [1.0])], [1, 1], dim, d, 2.0 ** -21, 2.0 ** -30, w0
-    raise KeyError(name)
-
-
-FILTER_CASES = ["residual", "tiny_product", "c_at_eps", "c_above_eps", "cancel", "tiny_delta"]
-
-
 def _filter_pair(name):
     from distributed_sgd_b200.native import NativeCtx
     from oracle.oracle import Oracle
-    rows, labels, dim, d, lam, lr, w0 = _filter_case(name)
-    data = _csr(rows, np.asarray(labels, np.int8), dim)
+    rows, labels, dim, d, lam, lr, w0 = filter_case(name)
+    data = csr(rows, np.asarray(labels, np.int8), dim)
     ctx = NativeCtx(0, dim, lam, is_async=True)
     ctx.load_csr(data.row_ptr, data.col, data.val, data.label)
     ctx.set_dim_sparsity(d)
@@ -153,15 +86,7 @@ def test_filter_edges(name, batch):
     ctx.async_replay(w0, idx, batch, lr)
     w = ctx.get_weights()
     w_ref = orc.async_run(w0, idx, batch, lr)
-    expect = {
-        "residual": {3: 0.0},
-        "tiny_product": {2: 2.0 ** -39, 5: 0.5},
-        "c_at_eps": {4: -(2.0 ** -66)},
-        "c_above_eps": {4: -(2.0 ** -66 + np.nextafter(EPS, 1.0))},
-        # update 1: column 1 cancels, column 6 -> 0.125 and S -> -0.9375; update 2 reads that S: c = -0.46875
-        "cancel": {1: -0.015625, 6: 0.234375},
-        "tiny_delta": {1: 0.0, 2: -(1.0 + 2.0 ** -40) * 2.0 ** -30, 3: -(1.0 + 2.0 ** -40) * 2.0 ** -30},
-    }[name]
+    expect = filter_expect(name)
     for j, v in expect.items():
         assert w_ref[j] == v, (j, w_ref[j], v)               # the case is what it says on the oracle
         assert w[j] == v, (j, w[j], v)
@@ -188,7 +113,7 @@ def private_columns():
     """Row i holds only column i (value 1, y = +1); from w0 = 2^10 the gate always passes, and the decrease of column i
     counts how often row i was drawn."""
     n = 2000
-    return _csr([([i], [1.0]) for i in range(n)], np.ones(n, np.int8), n)
+    return csr([([i], [1.0]) for i in range(n)], np.ones(n, np.int8), n)
 
 
 def _run_free(ctx, w0, assigned, batch, lr, n_updates, lanes=1, seed=5):
@@ -242,19 +167,16 @@ def test_device_draw_clips_batch_to_assigned(private_columns, n_assigned, batch)
 # ---- d. Hogwild conservation: concurrent lanes lose and duplicate nothing ----------------------------------------------
 
 @pytest.fixture(scope="module")
-def conservation_rows():
-    rng = np.random.default_rng(77)
-    dim, n, k = 4096, 4096, 8
-    rows = [(np.sort(rng.choice(dim, size=k, replace=False)), np.full(k, 2.0 ** -4)) for _ in range(n)]
-    return _csr(rows, np.ones(n, np.int8), dim), k
+def conservation():
+    return conservation_rows()
 
 
 @pytest.mark.parametrize("batch", [1, 8])
 @pytest.mark.parametrize("lanes", [1, 32, 256])
-def test_hogwild_conservation(conservation_rows, lanes, batch):
+def test_hogwild_conservation(conservation, lanes, batch):
     """Every entry is 2^-4, y = +1, w0 = 2^10, lr = 2^-6: the gate always passes and every partial sum is exact in any
     order.  So the update count, the total decrease, the master replica and the outbox must all be exact."""
-    data, k = conservation_rows
+    data, k = conservation
     ctx, _ = make_pair(data, lam=0.0, is_async=True)
     w0 = np.full(data.dim, 1024.0)
     lr, U = 2.0 ** -6, 20000
@@ -344,9 +266,9 @@ def test_load_csr_rejects_repeated_keys(bad_row):
     from distributed_sgd_b200.native import DsgdInvalid, NativeCtx
     ctx = NativeCtx(0, 10, 0.0, is_async=True)
     good = [([1, 2, 3], [1.0, 1.0, 1.0]), ([3, 1, 2, 9], [1.0, 1.0, 1.0, 1.0])]   # the same keys in two rows: fine
-    data = _csr(good, np.ones(2, np.int8), 10)
+    data = csr(good, np.ones(2, np.int8), 10)
     ctx.load_csr(data.row_ptr, data.col, data.val, data.label)
-    data = _csr(good + [(bad_row, np.ones(len(bad_row)))], np.ones(3, np.int8), 10)
+    data = csr(good + [(bad_row, np.ones(len(bad_row)))], np.ones(3, np.int8), 10)
     with pytest.raises(DsgdInvalid, match="repeats column"):
         ctx.load_csr(data.row_ptr, data.col, data.val, data.label)
     ctx.close()
