@@ -45,6 +45,24 @@ def sample_shard(k: int, world: int, rank: int):
     return (k * rank) // world, (k * (rank + 1)) // world
 
 
+def metrics_dict(words) -> dict:
+    """The result of Master.local_metrics from the native.METRICS_WORDS counts of a dsgd_eval_*metrics call: the eight counts
+    (tp, fn, pos_no_pred, fp, tn, neg_no_pred, u2, nan_scores), precision = TP / (TP + FP), recall = TP / P, f1 = 2 TP /
+    (2 TP + FP + FN + pos_no_pred) -- the harmonic mean of the two where both are defined --, auc = U2 / (2 P N) and accuracy
+    = (TP + TN) / (P + N), with P and N the positive and negative rows.  A ratio whose denominator is 0 is nan, and so is auc
+    when a score is NaN or a class is empty."""
+    tp, fn, pos_none, fp, tn, neg_none, u2, nan = (int(x) for x in words)
+    P, N = tp + fn + pos_none, fp + tn + neg_none
+
+    def ratio(a: int, b: int) -> float:
+        return a / b if b else float("nan")
+
+    auc = float(u2) / float(2 * P * N) if nan == 0 and P and N else float("nan")   # one IEEE division
+    return {"tp": tp, "fn": fn, "pos_no_pred": pos_none, "fp": fp, "tn": tn, "neg_no_pred": neg_none, "u2": u2,
+            "nan_scores": nan, "precision": ratio(tp, tp + fp), "recall": ratio(tp, P),
+            "f1": ratio(2 * tp, 2 * tp + fp + fn + pos_none), "auc": auc, "accuracy": ratio(tp + tn, P + N)}
+
+
 class EpochDraw(list):
     """The batch draws of one epoch: `self[s][k]` = row ids of worker k at step s (a list of lists of int32 arrays, the
     shape the tests and the oracle replay), backed by ONE array `ids[steps, K, batch]` (-1 beyond a short slice) and
@@ -180,25 +198,30 @@ class Master:
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         return self._eval_rows(weights, b, e)
 
-    def _eval_sample(self, weights, samples_count: int, test_data: bool):
-        """(loss, accuracy) on a fresh sample of min(samples_count, n) of the working rows, or None when that is empty.
-        Every call draws anew, as every reference call reshuffles.  Default: the sample is drawn on the device with
-        sampled_key(seed, t), t counting this Master's draws (the epoch draws of `fit` are separate).  jvm_exact: the ids are
-        `Random.shuffle(indices) take k` from the java.util.Random stream `fit` also draws from.  Rank r of W evaluates
-        positions sample_shard(k, W, r); the loss sums and counters are summed over ranks."""
+    def _draw_sample(self, samples_count: int, test_data: bool):
+        """(b, e, k, key, ids): a fresh sample of k = min(samples_count, n) of the working rows [b, e).  Every call draws anew,
+        as every reference call reshuffles.  Default: the sample is drawn on the device with key = sampled_key(seed, t), t
+        counting this Master's draws (the epoch draws of `fit` are separate); k <= 0 consumes no draw.  jvm_exact: ids =
+        `Random.shuffle(indices) take k` from the java.util.Random stream `fit` also draws from (key is None)."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         n = e - b
         k = min(int(samples_count), n)
-        ids = None
+        key = ids = None
         if self.jvm is not None:
             # the reference shuffles every index before `take`: the stream moves by one shuffle whatever k is
             ids = self.jvm.shuffle(np.arange(n, dtype=np.int32))[:max(k, 0)] + np.int32(b)
+        elif k > 0:
+            key = sampled_key(self.seed, self._sampled_draws)
+            self._sampled_draws += 1
+        return b, e, k, key, ids
+
+    def _eval_sample(self, weights, samples_count: int, test_data: bool):
+        """(loss, accuracy) on a fresh sample (_draw_sample), or None when that is empty.  Rank r of W evaluates positions
+        sample_shard(k, W, r); the loss sums and counters are summed over ranks."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
         if k <= 0:
             return None
         lo, hi = sample_shard(k, self.group.world, self.group.rank)
-        if ids is None:
-            key = sampled_key(self.seed, self._sampled_draws)
-            self._sampled_draws += 1
         if hi <= lo:
             h, c, n2 = 0, 0, 0.0
         elif ids is None:
@@ -224,6 +247,26 @@ class Master:
         if r is None:
             raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
         return r
+
+    # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
+    # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank
+    # evaluates the whole range or sample itself.  The counts are exact integers, so every rank returns the same bits without
+    # a collective.
+    def local_metrics(self, weights=None, test_data: bool = False) -> dict:
+        """Confusion counts, precision, recall, F1, ROC AUC and accuracy over the train (or test) rows (metrics_dict).
+        weights None: the resident weights -- in `fit` the last iterate, not the average of average_from."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return metrics_dict(self.ctx.eval_metrics(b, e, weights))
+
+    def local_sampled_metrics(self, weights, samples_count: int, test_data: bool = False) -> dict:
+        """local_metrics on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it (one draw of
+        sampled_key, or the jvm_exact shuffle).  An empty sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled metrics of {samples_count} rows: the sample is empty")
+        if ids is None:
+            return metrics_dict(self.ctx.eval_sampled_metrics(b, e, key, 0, k, weights))
+        return metrics_dict(self.ctx.eval_samples_metrics(ids, weights))
 
     def predict(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> dict:
         """Master.predict (core/Master.scala:61-75): idx -> prediction over the training rows; each worker

@@ -70,6 +70,17 @@ class Slave:
         self._train_ids(samples_idx)
         return self.ctx.forward(samples_idx, weights)
 
+    def margins(self, samples_idx: Sequence[int], weights: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension: the margins x.w in fp64 of the listed rows (forward reports -signum of these)."""
+        self._train_ids(samples_idx)
+        return self.ctx.margins(samples_idx, weights)
+
+    def probabilities(self, samples_idx: Sequence[int], weights: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension, SparseLogistic only (a SparseSVM slave raises DsgdState): P(y = +1 | x) = sigmoid(-x.w) of the listed
+        rows."""
+        self._train_ids(samples_idx)
+        return self.ctx.probabilities(samples_idx, weights)
+
     def gradient(self, weights: Optional[np.ndarray], samples_idx: Sequence[int]) -> np.ndarray:
         """SlaveImpl.gradient (core/Slave.scala:142-157): regularize(sum of backward over the batch)."""
         self._train_ids(samples_idx)

@@ -21,7 +21,10 @@
 #include "dsgd_persistent.cuh"
 #include "dsgd_stream.cuh"
 #include "dsgd_async.cuh"
+#include "dsgd_metrics.cuh"
 #include <cstdlib>
+
+#include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
 
 using namespace dsgd;
 
@@ -135,6 +138,10 @@ struct dsgd_ctx {
   // row ids of a request (forward, gradient, a sampled evaluation; drawn on the device or copied from the host): never the
   // staged stream above
   dev_buf<int32_t> eval_ids;
+  // a metrics pass (dsgd_eval_*metrics, dsgd_metrics.cuh): the score keys (positives from the front, negatives from the back),
+  // the radix sort's alternate keys and temporary storage, and the counter words (MetricWord)
+  dev_buf<unsigned long long> m_keys, m_alt, m_cnt;
+  dev_buf<unsigned char> m_tmp;
 
   ncclComm_t comm = nullptr;
 
@@ -860,8 +867,9 @@ extern "C" int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin,
   return DSGD_OK;
 }
 
-static int eval_sampled_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                             int64_t pos_begin, int64_t pos_end, double out[5], const char *fn) {
+// the argument checks of a sampled evaluation, then positions [pos_begin, pos_end) of its draw as row ids into eval_ids
+static int draw_sample(dsgd_ctx *ctx, int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end,
+                       const char *fn) {
   NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
   NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
        "%s: rows [%lld,%lld) outside [0,%lld)", fn, (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
@@ -879,7 +887,14 @@ static int eval_sampled_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, 
                                                       dsgd_feistel_half_bits((uint64_t)n), key, (uint32_t)n, row_begin);
   LAUNCHED();
   CU(cudaGetLastError());
-  return eval_pass(ctx, w, ctx->eval_ids, 0, k, out);
+  return DSGD_OK;
+}
+
+static int eval_sampled_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                             int64_t pos_begin, int64_t pos_end, double out[5], const char *fn) {
+  int rc = draw_sample(ctx, row_begin, row_end, key, pos_begin, pos_end, fn);
+  if (rc) return rc;
+  return eval_pass(ctx, w, ctx->eval_ids, 0, pos_end - pos_begin, out);
 }
 
 extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -933,6 +948,141 @@ extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int3
   if (rc) return rc;
   put_sums(out, loss_sum, correct, norm_squared);
   return DSGD_OK;
+}
+
+// ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
+
+// Growing a device buffer (cudaMalloc, and cudaFree of the smaller one) waits for the kernels running on the device, so it
+// would wait forever for an async loop that runs until stopped.  The start of an async loop therefore sizes the buffers of
+// the score and metrics calls for n_rows rows (and the sort's storage for them), and a call that would have to grow one while
+// the loop runs -- a list of more ids than rows -- is refused.
+static int reserve_scores(dsgd_ctx *ctx) {
+  const int64_t n = ctx->n_rows;
+  int rc;
+  if ((rc = ctx->eval_ids.grow(ctx, n, 1024)) || (rc = ctx->preds.grow(ctx, n, 1024)) || (rc = ctx->m_keys.grow(ctx, n, 1024)) ||
+      (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)))
+    return rc;
+  size_t tmp = 0;
+  cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
+  CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, kb, (int)n, 0, 64, ctx->stream));
+  return ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16);
+}
+
+static int fits_while_running(dsgd_ctx *ctx, bool fits, const char *fn) {
+  NEED(fits || !ctx->a_running, DSGD_ERR_STATE,
+       "%s: more ids than rows while the async loop runs (the buffers cannot grow until it is stopped)", fn);
+  return DSGD_OK;
+}
+
+// out[i] = x . w (prob: sigmoid(-x . w)) of the n rows samples[i]; the values go through `preds`, the per-row request buffer
+static int scores_impl(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *out, bool prob,
+                       const char *fn) {
+  NEED(out, DSGD_ERR_INVALID, "%s: output is NULL", fn);
+  NEED(!prob || is_logistic(ctx), DSGD_ERR_STATE, "%s: probabilities need the SparseLogistic model (DSGD_FLAG_LOGISTIC)", fn);
+  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
+  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "%s: bad arguments", fn);
+  NEED(n > 0, DSGD_ERR_EMPTY, "%s: no samples", fn);
+  int rc = fits_while_running(ctx, ctx->eval_ids.cap >= n && ctx->preds.cap >= n, fn);
+  if (rc || (rc = request_ids(ctx, samples, n, fn))) return rc;
+  if (rc || (rc = ctx->preds.grow(ctx, n, 1024))) return rc;
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  if ((rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
+  if (prob) k_margins<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->eval_ids, n, wd, ctx->preds);
+  else k_margins<false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->eval_ids, n, wd, ctx->preds);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *margins_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  return scores_impl(ctx, w, samples, n, margins_out, false, "dsgd_margins");
+}
+
+extern "C" int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *probs_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  return scores_impl(ctx, w, samples, n, probs_out, true, "dsgd_probabilities");
+}
+
+// One metrics pass over rows [row_begin, row_begin + n) (ids == nullptr) or over the n row ids at the device address `ids`:
+// scores and counts (k_metrics_score), the two key runs sorted, U2 counted (k_auc_count).  The host reads the run lengths
+// between the scoring and the sort, which takes them from the host.  Launches of the sort's own kernels are not counted in
+// dsgd_launch_count.
+static int metrics_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t row_begin, int64_t n, int64_t *out) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = fits_while_running(ctx, ctx->m_keys.cap >= n && ctx->m_alt.cap >= n && ctx->m_cnt, "metrics pass");
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
+  if ((rc = ctx->m_keys.grow(ctx, n, 1024)) || (rc = ctx->m_alt.grow(ctx, n, 1024)) ||
+      (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)))
+    return rc;
+  CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kMetWords, ctx->stream));
+  const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
+  k_metrics_score<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n, wd, ctx->m_keys,
+                                                 ctx->m_cnt);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long h[kMetWords];
+  CU(cudaMemcpyAsync(h, ctx->m_cnt, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int64_t n_pos = (int64_t)h[kMetPosSlots], n_neg = (int64_t)h[kMetNegSlots];
+  if (n_pos > 0 && n_neg > 0) {   // else no pair: U2 = 0
+    // the positives sit in keys[0, n_pos), the negatives in keys[n - n_neg, n); each run sorts within its own slice of
+    // the two buffers, and Current() is the buffer that holds it sorted.  Sorted positives let the threads of a warp walk
+    // nearly the same search path through the negatives.
+    cub::DoubleBuffer<unsigned long long> kp(ctx->m_keys.p, ctx->m_alt.p);
+    cub::DoubleBuffer<unsigned long long> kn(ctx->m_keys.p + (n - n_neg), ctx->m_alt.p + (n - n_neg));
+    size_t tmp_p = 0, tmp_n = 0;
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_p, kp, (int)n_pos, 0, 64, ctx->stream));
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_n, kn, (int)n_neg, 0, 64, ctx->stream));
+    size_t tmp = std::max(tmp_p, tmp_n);
+    if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, "metrics pass")) ||
+        (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
+      return rc;
+    CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kp, (int)n_pos, 0, 64, ctx->stream));
+    CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kn, (int)n_neg, 0, 64, ctx->stream));
+    const int cgrid = (int)std::min<int64_t>(cdiv(n_pos, 256), (int64_t)ctx->sm_count * 8);
+    k_auc_count<<<cgrid, 256, 0, ctx->stream>>>(kp.Current(), n_pos, kn.Current(), n_neg, ctx->m_cnt + kMetU2);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&h[kMetU2], ctx->m_cnt + kMetU2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  for (int k = 0; k < DSGD_METRICS_WORDS; ++k) out[k] = (int64_t)h[k];
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_metrics: out is NULL");
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_metrics: no rows loaded");
+  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
+       "dsgd_eval_metrics: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
+  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "dsgd_eval_metrics: empty range");
+  CU(cudaSetDevice(ctx->device));
+  return metrics_pass(ctx, w, nullptr, row_begin, row_end - row_begin, out);
+}
+
+extern "C" int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                         int64_t pos_begin, int64_t pos_end, int64_t *out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_sampled_metrics: out is NULL");
+  int rc = draw_sample(ctx, row_begin, row_end, key, pos_begin, pos_end, "dsgd_eval_sampled_metrics");
+  if (rc) return rc;
+  return metrics_pass(ctx, w, ctx->eval_ids, 0, pos_end - pos_begin, out);
+}
+
+extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: out is NULL");
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_samples_metrics: no rows loaded");
+  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: bad arguments");
+  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_samples_metrics: empty sample");
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: %lld ids; at most 2^31 - 1", (long long)n);
+  int rc = fits_while_running(ctx, ctx->eval_ids.cap >= n, "dsgd_eval_samples_metrics");
+  if (rc || (rc = request_ids(ctx, samples, n, "dsgd_eval_samples_metrics"))) return rc;
+  return metrics_pass(ctx, w, ctx->eval_ids, 0, n, out);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all
@@ -1590,7 +1740,7 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   NEED(batch >= 1 && lanes >= 1 && lanes <= 4096, DSGD_ERR_INVALID, "dsgd_start_async: bad arguments");
   CU(cudaSetDevice(ctx->device));
   int rc = load_all_kernels(ctx);
-  if (rc) return rc;
+  if (rc || (rc = reserve_scores(ctx))) return rc;
   if (w0) {  // weights() = request.weights
     CU(cudaMemcpyAsync(ctx->w, w0, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
     rc = refresh_resident(ctx);  // also S = w . d and the control slots of the replica

@@ -1,0 +1,154 @@
+// dsgd_metrics.cuh -- sm_90a kernels of the scoring and ranking-metric calls (dsgd_margins, dsgd_probabilities, the
+// dsgd_eval_*metrics calls; DESIGN.md §4.8).
+//
+// A metrics pass is three steps on the ctx's stream:
+//   1. k_metrics_score: x . w of every row in fp64 (row_margin, the body dsgd_margins runs too), the confusion counts, and
+//      the row's score s = -(x . w) as an order-preserving u64 key -- positives from the front of one key array, negatives
+//      from its back.  NaN scores are counted and not written.
+//   2. cub::DeviceRadixSort::SortKeys on each of the two runs (the host reads their lengths in between).
+//   3. k_auc_count: one thread per positive key, lower_bound / upper_bound in the sorted negatives, U2 in integers.
+// Every word is an integer sum, so the result does not depend on the grid or on the order in which warps take rows.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "dsgd_kernels.cuh"
+
+namespace dsgd {
+
+// Words of dsgd_eval_*metrics (include/dsgd.h) and the two slot counters that follow them in the ctx's counter block
+enum MetricWord : int {
+  kMetTp = 0, kMetFn = 1, kMetPosNone = 2,   // y = +1: pred +1, pred -1, no +-1 prediction (x.w == 0 or NaN)
+  kMetFp = 3, kMetTn = 4, kMetNegNone = 5,   // y = -1: pred +1, pred -1, no +-1 prediction
+  kMetU2 = 6,                                // sum over (positive, negative) pairs of 2*[s_pos > s_neg] + [s_pos == s_neg]
+  kMetNan = 7,                               // rows whose score is NaN
+  kMetPosSlots = 8, kMetNegSlots = 9,        // keys written so far to the positive run / the negative run
+  kMetWords = 16
+};
+
+// x . w of row r for one warp, every lane gets it: the fold of k_rows_logistic (lane-strided partial sums of the filtered
+// products, then the xor butterfly).  dsgd_margins and the metrics pass both call this, so a metrics pass ranks exactly the
+// values dsgd_margins returns for the same rows.
+__device__ __forceinline__ double row_margin(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                             const double *__restrict__ w, int64_t r, int lane) {
+  const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+  double dot = 0.0;
+  for (int64_t k = b + lane; k < e; k += 32) {
+    const uint2 pr = pairs[k];
+    const double xv = filt((double)__uint_as_float(pr.y));
+    dot += filt(xv * w[pr.x]);  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
+  }
+  return warp_sum(dot);
+}
+
+// Order-preserving key of a score: +0 and -0 are one key, and key(a) < key(b) exactly when a < b (for non-NaN scores)
+__device__ __forceinline__ unsigned long long score_key(double s) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(s == 0.0 ? 0.0 : s);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_margins: out[i] = x . w of row samples[i] (kProb: P(y = +1 | x) = sigmoid(-x . w), the model's probability, with the
+// `sigmoid` of the logistic gradient).  One warp per row, in sample order.
+// ---------------------------------------------------------------------------------------------------
+template <bool kProb>
+__global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                 const int32_t *__restrict__ samples, int64_t n,
+                                                 const double *__restrict__ w, double *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t i = warp0; i < n; i += nwarps) {
+    const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    if (lane == 0) out[i] = kProb ? sigmoid(-dot) : dot;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_metrics_score: the scoring step of a metrics pass over rows samples[0..n) (samples == nullptr: rows [row_begin,
+// row_begin + n)).  A warp takes 32 consecutive positions at a time: lane j loads the id and label of position j, the warp
+// computes the 32 dots one after the other and lane j keeps the j-th.  Each lane counts its rows in registers; the counts
+// are flushed once per warp.  The keys go to keys[0..) (y = +1) and keys[..n) backwards (y = -1), their slots claimed with
+// one atomic per warp and class for 32 rows.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_metrics_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                       const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                       int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                       unsigned long long *__restrict__ keys,
+                                                       unsigned long long *__restrict__ cnt) {
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned c[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // this lane's rows, by MetricWord (kMetU2 unused)
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i = g + lane;
+    const bool mine = i < n;
+    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    double dot_own = 0.0;
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const double dot = row_margin(rp16, pairs, w, r, lane);
+      if (lane == j) dot_own = dot;
+    }
+    const bool pos = mine && label[r_own] > 0, neg = mine && !pos;
+    const bool nan = mine && isnan(dot_own);
+    const int p = pred_of(dot_own);   // dsgd_forward's prediction; NaN -> 0
+    c[kMetTp] += pos && p == 1;
+    c[kMetFn] += pos && p == -1;
+    c[kMetPosNone] += pos && p == 0;
+    c[kMetFp] += neg && p == 1;
+    c[kMetTn] += neg && p == -1;
+    c[kMetNegNone] += neg && p == 0;
+    c[kMetNan] += nan;
+    const bool put_pos = pos && !nan, put_neg = neg && !nan;
+    const unsigned bp = __ballot_sync(full, put_pos), bn = __ballot_sync(full, put_neg);
+    unsigned long long base_p = 0, base_n = 0;
+    if (lane == 0) {
+      if (bp) base_p = atomicAdd(&cnt[kMetPosSlots], (unsigned long long)__popc(bp));
+      if (bn) base_n = atomicAdd(&cnt[kMetNegSlots], (unsigned long long)__popc(bn));
+    }
+    base_p = __shfl_sync(full, base_p, 0);
+    base_n = __shfl_sync(full, base_n, 0);
+    const unsigned below = (1u << lane) - 1u;
+    if (put_pos) keys[base_p + __popc(bp & below)] = score_key(-dot_own);
+    if (put_neg) keys[n - 1 - (int64_t)(base_n + __popc(bn & below))] = score_key(-dot_own);
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    if (k == kMetU2) continue;
+    const unsigned s = __reduce_add_sync(full, c[k]);
+    if (lane == 0 && s) atomicAdd(&cnt[k], (unsigned long long)s);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_auc_count: U2 = sum over the positive keys of 2 * #{negative keys below} + #{negative keys equal}, i.e. of
+// lower_bound + upper_bound in the sorted negatives.  One thread per positive key, the sum in a register, one atomic per
+// warp: integer additions, the same bits in any order.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_auc_count(const unsigned long long *__restrict__ pos, int64_t n_pos,
+                                                   const unsigned long long *__restrict__ neg, int64_t n_neg,
+                                                   unsigned long long *__restrict__ u2) {
+  unsigned long long acc = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pos; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = pos[i];
+    int64_t lo = 0, hi = n_neg;   // lower_bound: first negative >= key
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (neg[mid] < key) lo = mid + 1; else hi = mid;
+    }
+    int64_t up = lo, top = n_neg;   // upper_bound: first negative > key, at or after lower_bound
+    while (up < top) {
+      const int64_t mid = (up + top) >> 1;
+      if (neg[mid] <= key) up = mid + 1; else top = mid;
+    }
+    acc += (unsigned long long)(lo + up);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0 && acc) atomicAdd(u2, acc);
+}
+
+}  // namespace dsgd

@@ -42,6 +42,16 @@ object DsgdNative {
                               posEnd: Long, lossSumNormSquared: Array[Double], correct: Array[Long]): Int
   @native def evalSamplesSums(ctx: Long, w: Array[Double], samples: Array[Int], lossSumNormSquared: Array[Double],
                               correct: Array[Long]): Int
+  // scores (out.length >= samples.length): the margins x.w, or P(y = +1 | x) on a FlagLogistic context; ranking metrics
+  // (metrics.length >= MetricsWords): TP, FN, positives without a prediction, FP, TN, negatives without one, U2, NaN rows --
+  // AUC = U2 / (2 P N)
+  final val MetricsWords = 8
+  @native def margins(ctx: Long, w: Array[Double], samples: Array[Int], out: Array[Double]): Int
+  @native def probabilities(ctx: Long, w: Array[Double], samples: Array[Int], out: Array[Double]): Int
+  @native def evalMetrics(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, metrics: Array[Long]): Int
+  @native def evalSampledMetrics(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                 posEnd: Long, metrics: Array[Long]): Int
+  @native def evalSamplesMetrics(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

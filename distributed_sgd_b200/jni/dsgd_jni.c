@@ -203,6 +203,54 @@ FN(evalSamplesSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArra
   free(bw.p); free(bi.p);
   return rc;
 }
+/* scores and ranking metrics, either model: out(i) = x_i . w (margins) or P(y = +1 | x_i) (probabilities, SparseLogistic
+ * only); metrics(0..7) = the DSGD_METRICS_WORDS counts of dsgd_eval_metrics.  An output shorter than that is DSGD_ERR_INVALID. */
+FN(margins)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray out) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bo.bad)) rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_margins(CTX(h), bw.p, bs.p, bs.n, bo.p);
+  back_Double(env, out, bo, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+FN(probabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray out) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bo.bad)) rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_probabilities(CTX(h), bw.p, bs.p, bs.n, bo.p);
+  back_Double(env, out, bo, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+FN(evalMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics) {
+  buf_t bw = in_Double(env, w), bm = out_Long(env, metrics);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bm.bad))
+    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID : dsgd_eval_metrics(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)bm.p);
+  back_Long(env, metrics, bm, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                       jlong posBegin, jlong posEnd, jlongArray metrics) {
+  buf_t bw = in_Double(env, w), bm = out_Long(env, metrics);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bm.bad))
+    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID
+                                   : dsgd_eval_sampled_metrics(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                               (int64_t *)bm.p);
+  back_Long(env, metrics, bm, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bm = out_Long(env, metrics);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bm.bad))
+    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID : dsgd_eval_samples_metrics(CTX(h), bw.p, bs.p, bs.n, (int64_t *)bm.p);
+  back_Long(env, metrics, bm, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
 
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {

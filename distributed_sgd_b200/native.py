@@ -26,6 +26,8 @@ FLAG_LOGISTIC = 2
 REPLICA_SELF, REPLICA_MASTER = 0, 1
 
 OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM, ERR_TIMEOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8
+# words of the dsgd_eval_*metrics calls: TP, FN, positives without a +-1 prediction, FP, TN, negatives without one, U2, NaN rows
+METRICS_WORDS = 8
 
 
 class NativeLibraryMissing(ImportError):
@@ -101,6 +103,11 @@ ABI = {
     "dsgd_eval_sums": [_vp, _vp, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_eval_sampled_sums": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_eval_samples_sums": [_vp, _vp, _vp, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
+    "dsgd_margins": [_vp, _vp, _vp, _i64, _vp],
+    "dsgd_probabilities": [_vp, _vp, _vp, _i64, _vp],
+    "dsgd_eval_metrics": [_vp, _vp, _i64, _i64, _vp],
+    "dsgd_eval_sampled_metrics": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp],
+    "dsgd_eval_samples_metrics": [_vp, _vp, _vp, _i64, _vp],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -370,6 +377,47 @@ class NativeCtx:
         self._ck(self._l.dsgd_eval_samples_sums(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
                                                 C.byref(n2)))
         return h.value, c.value, n2.value
+
+    # -- scores and ranking metrics --
+    def margins(self, samples, w=None) -> np.ndarray:
+        """x . w in fp64 for each listed row (dsgd_margins)."""
+        samples = _arr(samples, np.int32)
+        out = np.zeros(samples.size, dtype=np.float64)
+        w = self._w(w)
+        self._ck(self._l.dsgd_margins(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
+        return out
+
+    def probabilities(self, samples, w=None) -> np.ndarray:
+        """P(y = +1 | x) = sigmoid(-x . w) for each listed row; SparseLogistic contexts only (dsgd_probabilities)."""
+        samples = _arr(samples, np.int32)
+        out = np.zeros(samples.size, dtype=np.float64)
+        w = self._w(w)
+        self._ck(self._l.dsgd_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
+        return out
+
+    def eval_metrics(self, row_begin: int, row_end: int, w=None) -> np.ndarray:
+        """The METRICS_WORDS exact counts over rows [row_begin, row_end) (dsgd_eval_metrics)."""
+        out = np.zeros(METRICS_WORDS, dtype=np.int64)
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_metrics(self._h, _ptr(w), row_begin, row_end, _ptr(out)))
+        return out
+
+    def eval_sampled_metrics(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                             w=None) -> np.ndarray:
+        """The same counts over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_metrics)."""
+        out = np.zeros(METRICS_WORDS, dtype=np.int64)
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_sampled_metrics(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
+                                                   pos_begin, pos_end, _ptr(out)))
+        return out
+
+    def eval_samples_metrics(self, samples, w=None) -> np.ndarray:
+        """The same counts over a list of row ids; repeats count every time (dsgd_eval_samples_metrics)."""
+        samples = _arr(samples, np.int32)
+        out = np.zeros(METRICS_WORDS, dtype=np.int64)
+        w = self._w(w)
+        self._ck(self._l.dsgd_eval_samples_metrics(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
+        return out
 
     # -- sync --
     def set_workers(self, counts, k_total: int = 0):

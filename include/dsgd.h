@@ -174,6 +174,35 @@ int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, in
 int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
                            int64_t *correct, double *norm_squared);
 
+/* ---- scores and ranking metrics, for either model.  The conventions of the evaluations above: w == NULL reads the resident
+ *      weights (on an async ctx, a snapshot taken when the call starts); the ids go to a buffer of their own, so a staged
+ *      sample stream is left intact; no rows loaded -> DSGD_ERR_STATE; an id or a range outside the loaded rows ->
+ *      DSGD_ERR_RANGE, before anything is launched; n == 0 (an empty range, no positions) -> DSGD_ERR_EMPTY; a NULL output
+ *      -> DSGD_ERR_INVALID.  The dot product x_i . w is the fp64 fold of the logistic passes (not the fp32 streaming pass,
+ *      which only decides a sign), and the metrics rank exactly the values dsgd_margins returns for the same rows. ---- */
+/* margins_out[i] = x_i . w in fp64 (the value whose -signum dsgd_forward reports) */
+int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *margins_out);
+/* SparseLogistic only: probs_out[i] = P(y = +1 | x_i) = sigmoid(-x_i . w), with the sigmoid of the logistic gradient; an SVM ctx
+ * -> DSGD_ERR_STATE (its margins are not calibrated probabilities). */
+int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *probs_out);
+
+#define DSGD_METRICS_WORDS 8
+/* out[0] TP  (y=+1, pred=+1)   out[1] FN (y=+1, pred=-1)   out[2] y=+1 with no +-1 prediction (x.w == 0 or NaN)
+ * out[3] FP  (y=-1, pred=+1)   out[4] TN (y=-1, pred=-1)   out[5] y=-1 with no +-1 prediction
+ * out[6] U2 = sum over (positive, negative) pairs of 2*[s_pos > s_neg] + [s_pos == s_neg], s = -x.w, NaN rows left out
+ * out[7] rows whose score is NaN
+ * pred is dsgd_forward's prediction, so out[0] + out[4] is the `correct` of dsgd_eval_* over the same rows.  A NaN row has no
+ * prediction: it counts in out[2] or out[5] and in out[7].  +0 and -0 are one score.  Every word is an exact integer, whatever
+ * the grid or the row order.  ROC AUC = U2 / (2 P N), P = out[0] + out[1] + out[2] positive rows, N = out[3] + out[4] + out[5]
+ * negative rows; it is undefined (NaN) when out[7] > 0 or P or N is 0.
+ * The sampled form draws as dsgd_eval_sampled_counts (its further errors are that call's); the list form counts a repeated id
+ * every time and takes at most 2^31 - 1 ids (DSGD_ERR_INVALID), so U2 <= 2 (n/2)^2 fits in int64.  A pass sorts the scores: it
+ * grows its buffers (two 8-byte keys per row and the sort's storage) on first use, like the other requests. */
+int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out);
+int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                              int64_t pos_begin, int64_t pos_end, int64_t *out);
+int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out);
+
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
  *      (its own RPC), every rank calls dsgd_comm_init.  world == 1 needs neither. -------------------------- */
