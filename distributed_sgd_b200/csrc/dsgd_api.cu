@@ -294,11 +294,11 @@ static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
 
-// every id names a loaded row (the reference indexes its data array with it)
-static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *what) {
+// every id names a loaded row (the reference indexes its data array with it); fn is the entry point
+static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn, const char *what) {
   for (int64_t i = 0; i < n; ++i)
-    NEED(ids[i] >= 0 && ids[i] < ctx->n_rows, DSGD_ERR_RANGE, "%s %d at position %lld outside [0,%lld)", what, ids[i],
-         (long long)i, (long long)ctx->n_rows);
+    NEED(ids[i] >= 0 && ids[i] < ctx->n_rows, DSGD_ERR_RANGE, "%s: %s %d at position %lld outside [0,%lld)", fn, what,
+         ids[i], (long long)i, (long long)ctx->n_rows);
   return DSGD_OK;
 }
 
@@ -340,42 +340,28 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
     { int rc = fail(nullptr, DSGD_ERR_CUDA, "dsgd_create: device %d is sm_%d%d; this library is built for sm_90a only",
                     device, prop.major, prop.minor); delete ctx; return rc; }
   if ((e = cudaStreamCreateWithFlags(&ctx->own_stream.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
+  ctx->stream = ctx->own_stream;
   if (flags & DSGD_FLAG_ASYNC) {   // the worker loop's stream and the service stream exist in async mode only: streams
                                    // beyond the device's hardware queues (8 by default) alias and serialise each other
     if ((e = cudaStreamCreateWithFlags(&ctx->astream.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
     if ((e = cudaStreamCreateWithFlags(&ctx->stream2.h, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   }
-  if ((e = ctx->a_stop.alloc(1)) != cudaSuccess) return bail("cudaMalloc a_stop", e);
-  if ((e = ctx->a_cnt.alloc(2)) != cudaSuccess) return bail("cudaMalloc a_cnt", e);
-  cudaMemsetAsync(ctx->a_stop, 0, sizeof(int), ctx->own_stream);
-  cudaMemsetAsync(ctx->a_cnt, 0, sizeof(unsigned long long) * 2, ctx->own_stream);
-  ctx->stream = ctx->own_stream;
   if ((e = cudaEventCreate(&ctx->ev0.h)) != cudaSuccess) return bail("event", e);
   if ((e = cudaEventCreate(&ctx->ev1.h)) != cudaSuccess) return bail("event", e);
+  // a device buffer of n elements, all of it zeroed on the ctx's stream
+  auto zeroed = [&](auto &buf, int64_t n, const char *what) {
+    if ((e = buf.alloc(n)) == cudaSuccess) e = cudaMemsetAsync(buf.p, 0, sizeof *buf.p * (size_t)n, ctx->stream);
+    return e == cudaSuccess ? DSGD_OK : bail(what, e);
+  };
   const int64_t nv = (int64_t)dim + kReplicaPad;
-  const size_t vd = sizeof(double) * (size_t)nv;
-  const int upd_blocks = cdiv(dim, 256);
-  if ((e = ctx->w.alloc(nv)) != cudaSuccess) return bail("cudaMalloc w", e);
-  if ((e = ctx->g.alloc(nv)) != cudaSuccess) return bail("cudaMalloc g", e);
-  if ((e = ctx->d.alloc(nv)) != cudaSuccess) return bail("cudaMalloc d", e);
-  if ((e = ctx->w_req.alloc(nv)) != cudaSuccess) return bail("cudaMalloc w_req", e);
-  if ((e = ctx->w32.alloc((int64_t)dim + 4)) != cudaSuccess) return bail("cudaMalloc w32", e);
-  if ((e = ctx->w32_req.alloc((int64_t)dim + 4)) != cudaSuccess) return bail("cudaMalloc w32_req", e);
-  if ((e = ctx->n_exact.alloc(2)) != cudaSuccess) return bail("cudaMalloc n_exact", e);
-  cudaMemsetAsync(ctx->n_exact, 0, sizeof(unsigned long long) * 2, ctx->stream);
-  if ((e = ctx->scal.alloc(kNumScal)) != cudaSuccess) return bail("cudaMalloc scal", e);
-  if ((e = ctx->cnt.alloc(kNumCnt)) != cudaSuccess) return bail("cudaMalloc cnt", e);
-  if ((e = ctx->partial.alloc(2 * (int64_t)upd_blocks)) != cudaSuccess) return bail("cudaMalloc partial", e);
-  if ((e = ctx->out2.alloc(8)) != cudaSuccess) return bail("cudaMalloc out2", e);
-  if ((e = ctx->gsum.alloc(nv)) != cudaSuccess) return bail("cudaMalloc gsum", e);
-  cudaMemsetAsync(ctx->gsum, 0, vd, ctx->stream);
-  cudaMemsetAsync(ctx->w, 0, vd, ctx->stream);
-  cudaMemsetAsync(ctx->g, 0, vd, ctx->stream);
-  cudaMemsetAsync(ctx->d, 0, vd, ctx->stream);
-  cudaMemsetAsync(ctx->w_req, 0, vd, ctx->stream);
-  cudaMemsetAsync(ctx->w32, 0, sizeof(float) * (size_t)(dim + 2), ctx->stream);
-  cudaMemsetAsync(ctx->scal, 0, sizeof(double) * kNumScal, ctx->stream);
-  cudaMemsetAsync(ctx->cnt, 0, sizeof(unsigned long long) * kNumCnt, ctx->stream);
+  int rc;
+  if ((rc = zeroed(ctx->a_stop, 1, "a_stop")) || (rc = zeroed(ctx->a_cnt, 2, "a_cnt")) || (rc = zeroed(ctx->w, nv, "w")) ||
+      (rc = zeroed(ctx->g, nv, "g")) || (rc = zeroed(ctx->d, nv, "d")) || (rc = zeroed(ctx->w_req, nv, "w_req")) ||
+      (rc = zeroed(ctx->w32, (int64_t)dim + 4, "w32")) || (rc = zeroed(ctx->w32_req, (int64_t)dim + 4, "w32_req")) ||
+      (rc = zeroed(ctx->n_exact, 2, "n_exact")) || (rc = zeroed(ctx->scal, kNumScal, "scal")) ||
+      (rc = zeroed(ctx->cnt, kNumCnt, "cnt")) || (rc = zeroed(ctx->partial, 2 * (int64_t)cdiv(dim, 256), "partial")) ||
+      (rc = zeroed(ctx->out2, 8, "out2")) || (rc = zeroed(ctx->gsum, nv, "gsum")))
+    return rc;
   if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) return bail("init memset", e);
   *out = ctx;
   return DSGD_OK;
@@ -620,7 +606,7 @@ extern "C" int dsgd_stage_samples(dsgd_ctx *ctx, const int32_t *samples, int64_t
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_stage_samples: no rows loaded");
   NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_stage_samples: bad arguments");
-  int rc = check_ids(ctx, samples, n, "sample index");
+  int rc = check_ids(ctx, samples, n, __func__, "sample index");
   if (rc) return rc;
   CU(cudaSetDevice(ctx->device));
   if ((rc = ctx->samples.grow(ctx, n, 1024))) return rc;
@@ -699,264 +685,49 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
 
 // ---- forward / gradient / eval -------------------------------------------------------------------------
 
-// the n row ids of a request into eval_ids: the staged stream stays as it was for the next dsgd_sync_steps_staged
-static int request_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn) {
-  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
-  int rc = check_ids(ctx, ids, n, "sample index");
-  if (rc) return rc;
-  CU(cudaSetDevice(ctx->device));
-  if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
-  CU(cudaMemcpyAsync(ctx->eval_ids, ids, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  return DSGD_OK;
-}
+// The rows of a request: rows [row_begin, row_begin + n) when ids == nullptr, else the n row ids at the device address ids
+// (in eval_ids: the staged stream stays as it was for the next dsgd_sync_steps_staged).  rows_range, rows_drawn and
+// rows_list check the rows a request names and build its row_set; fn is the entry point, and every message names it.
+struct row_set {
+  const int32_t *ids;
+  int64_t row_begin, n;
+};
 
-extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *preds_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(n >= 0 && (n == 0 || (samples && preds_out)), DSGD_ERR_INVALID, "dsgd_forward: bad arguments");
-  if (n == 0) return DSGD_OK;
-  int rc = request_ids(ctx, samples, n, "dsgd_forward");
-  if (rc) return rc;
-  rc = ctx->preds.grow(ctx, n, 1024);
-  if (rc) return rc;
-  const double *wd, *cd, *nd;
-  const float *w32d;
-  if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  if (stream_eligible(ctx, n)) {
-    if ((rc = stream_launch<false, true, false>(ctx, ctx->eval_ids, 0, n, wd, w32d, nullptr, ctx->preds))) return rc;
-  } else {
-    k_rows<false, true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
-                                                                    wd, nullptr, ctx->preds, ctx->cnt);
-    LAUNCHED();
-  }
-  CU(cudaGetLastError());
-  CU(cudaMemsetAsync(ctx->cnt, 0, sizeof(unsigned long long) * 2, ctx->stream));
-  CU(cudaMemcpyAsync(preds_out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  return DSGD_OK;
-}
-
-extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *grad_out,
-                             double *loss_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(n >= 0 && grad_out, DSGD_ERR_INVALID, "dsgd_gradient: bad arguments");
-  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_gradient: empty batch (Vec.sum of an empty list throws in the reference)");
-  NEED(samples, DSGD_ERR_INVALID, "dsgd_gradient: samples is NULL");
-  NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_gradient: dimSparsity not set");
-  int rc = request_ids(ctx, samples, n, "dsgd_gradient");
-  if (rc) return rc;
-  const double *wd, *cd, *nd;
-  const float *w32d;
-  if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  const bool logistic = is_logistic(ctx);
-  if (logistic) {
-    k_rows_logistic<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
-                                                                      wd, ctx->g, ctx->cnt);
-    LAUNCHED();
-  } else if (stream_eligible(ctx, n)) {
-    if ((rc = stream_launch<true, false, false>(ctx, ctx->eval_ids, 0, n, wd, w32d, ctx->g, nullptr))) return rc;
-  } else {
-    k_rows<true, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ctx->eval_ids, 0, n,
-                                                                    wd, ctx->g, nullptr, ctx->cnt);
-    LAUNCHED();
-  }
-  const int fin_blocks = cdiv(ctx->dim + 1, 256);
-  if (logistic) {
-    k_finish_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, cd, ctx->cnt, (double)n);
-    k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
-  } else {
-    k_finish<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, cd, ctx->cnt, (double)n);
-    k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
-  }
-  LAUNCHED();
-  LAUNCHED();
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(grad_out, ctx->g, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
-  double out2[2];
-  CU(cudaMemcpyAsync(out2, ctx->out2, sizeof out2, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemsetAsync(ctx->g, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  if (loss_out) *loss_out = out2[0];
-  return DSGD_OK;
-}
-
-// One evaluation pass over rows [row_begin, row_begin + n) (ids == nullptr) or over the n row ids at the device address
-// `ids`, then the shared tail: out = {loss, accuracy, loss sum, correct count, ||w||^2}, and the counters cleared for the
-// next pass (k_loss_scalar).  The SVM's loss sum is the hinge sum, an integer.
-static int eval_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t row_begin, int64_t n, double out[5]) {
-  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
-  const float *w32d = nullptr;
-  int rc;
-  if ((rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  if (is_logistic(ctx)) {   // the fp32 streaming pass decides signs only; the logistic loss needs the dot's value
-    k_rows_logistic<false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n,
-                                                                       wd, nullptr, ctx->cnt);
-    LAUNCHED();
-  } else if (stream_eligible(ctx, n)) {
-    rc = ids ? stream_launch<false, false, false>(ctx, ids, 0, n, wd, w32d, nullptr, nullptr)
-             : stream_launch<false, false, true>(ctx, nullptr, row_begin, n, wd, w32d, nullptr, nullptr);
-    if (rc) return rc;
-  } else {
-    k_rows<false, false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n,
-                                                                     wd, nullptr, nullptr, ctx->cnt);
-    LAUNCHED();
-  }
-  if (is_logistic(ctx)) k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
-  else k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nd, ctx->cnt, ctx->lambda, (double)n, ctx->out2);
-  LAUNCHED();
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  return DSGD_OK;
-}
-
-static int eval_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double out[5]) {
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval: no rows loaded");
-  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
-       "dsgd_eval: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
-  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "dsgd_eval: empty range (reduce on an empty collection throws in the reference)");
-  CU(cudaSetDevice(ctx->device));
-  return eval_pass(ctx, w, nullptr, row_begin, row_end - row_begin, out);
-}
-
-// the *_counts calls report integer hinge sums, which only the SVM has
-static int counts_model(dsgd_ctx *ctx, const char *fn) {
-  NEED(!is_logistic(ctx), DSGD_ERR_STATE, "%s: the logistic model's loss sum is not an integer; use the *_sums call", fn);
-  return DSGD_OK;
-}
-
-static void put_counts(const double out[5], int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
-  if (hinge_sum) *hinge_sum = (int64_t)out[2];
-  if (correct) *correct = (int64_t)out[3];
-  if (norm_squared) *norm_squared = out[4];
-}
-
-static void put_sums(const double out[5], double *loss_sum, int64_t *correct, double *norm_squared) {
-  if (loss_sum) *loss_sum = out[2];
-  if (correct) *correct = (int64_t)out[3];
-  if (norm_squared) *norm_squared = out[4];
-}
-
-extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
-                         double *acc_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = eval_impl(ctx, w, row_begin, row_end, out);
-  if (rc) return rc;
-  if (loss_out) *loss_out = out[0];
-  if (acc_out) *acc_out = out[1];
-  return DSGD_OK;
-}
-
-extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *hinge_sum,
-                                int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = counts_model(ctx, "dsgd_eval_counts");
-  if (rc || (rc = eval_impl(ctx, w, row_begin, row_end, out))) return rc;
-  put_counts(out, hinge_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-extern "C" int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_sum,
-                              int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = eval_impl(ctx, w, row_begin, row_end, out);
-  if (rc) return rc;
-  put_sums(out, loss_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-// the argument checks of a sampled evaluation, then positions [pos_begin, pos_end) of its draw as row ids into eval_ids
-static int draw_sample(dsgd_ctx *ctx, int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end,
-                       const char *fn) {
+static int rows_range(dsgd_ctx *ctx, int64_t row_begin, int64_t row_end, const char *fn, row_set *rows) {
   NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
   NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
        "%s: rows [%lld,%lld) outside [0,%lld)", fn, (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
+  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "%s: empty range (reduce on an empty collection throws in the reference)", fn);
+  *rows = {nullptr, row_begin, row_end - row_begin};
+  return DSGD_OK;
+}
+
+// positions [pos_begin, pos_end) of the sample drawn from rows [row_begin, row_end) with `key`, as row ids into eval_ids
+static int rows_drawn(dsgd_ctx *ctx, int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end,
+                      const char *fn, row_set *rows) {
+  int rc = rows_range(ctx, row_begin, row_end, fn, rows);
+  if (rc) return rc;
   const int64_t n = row_end - row_begin;
-  NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty row range", fn);
   NEED(n <= (int64_t)UINT32_MAX, DSGD_ERR_INVALID, "%s: %lld rows; the draw permutes 32-bit positions", fn, (long long)n);
   NEED(pos_begin >= 0 && pos_end <= n, DSGD_ERR_INVALID, "%s: positions [%lld,%lld) outside [0,%lld)", fn,
        (long long)pos_begin, (long long)pos_end, (long long)n);
   NEED(pos_end > pos_begin, DSGD_ERR_EMPTY, "%s: no positions (reduce on an empty collection throws)", fn);
   CU(cudaSetDevice(ctx->device));
   const int64_t k = pos_end - pos_begin;
-  int rc = ctx->eval_ids.grow(ctx, k, 1024);
-  if (rc) return rc;
+  if ((rc = ctx->eval_ids.grow(ctx, k, 1024))) return rc;
   k_draw_rows<<<cdiv(k, 256), 256, 0, ctx->stream>>>(ctx->eval_ids, k, (uint32_t)pos_begin,
                                                       dsgd_feistel_half_bits((uint64_t)n), key, (uint32_t)n, row_begin);
   LAUNCHED();
   CU(cudaGetLastError());
+  *rows = {ctx->eval_ids, 0, k};
   return DSGD_OK;
 }
-
-static int eval_sampled_impl(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                             int64_t pos_begin, int64_t pos_end, double out[5], const char *fn) {
-  int rc = draw_sample(ctx, row_begin, row_end, key, pos_begin, pos_end, fn);
-  if (rc) return rc;
-  return eval_pass(ctx, w, ctx->eval_ids, 0, pos_end - pos_begin, out);
-}
-
-extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                        int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
-                                        double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = counts_model(ctx, "dsgd_eval_sampled_counts");
-  if (rc || (rc = eval_sampled_impl(ctx, w, row_begin, row_end, key, pos_begin, pos_end, out, "dsgd_eval_sampled_counts")))
-    return rc;
-  put_counts(out, hinge_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-extern "C" int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                      int64_t pos_begin, int64_t pos_end, double *loss_sum, int64_t *correct,
-                                      double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = eval_sampled_impl(ctx, w, row_begin, row_end, key, pos_begin, pos_end, out, "dsgd_eval_sampled_sums");
-  if (rc) return rc;
-  put_sums(out, loss_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-static int eval_samples_impl(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double out[5],
-                             const char *fn) {
-  NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
-  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "%s: bad arguments", fn);
-  NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty sample (reduce on an empty collection throws)", fn);
-  int rc = request_ids(ctx, samples, n, fn);
-  if (rc) return rc;
-  return eval_pass(ctx, w, ctx->eval_ids, 0, n, out);
-}
-
-extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
-                                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = counts_model(ctx, "dsgd_eval_samples_counts");
-  if (rc || (rc = eval_samples_impl(ctx, w, samples, n, out, "dsgd_eval_samples_counts"))) return rc;
-  put_counts(out, hinge_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
-                                      int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  double out[5];
-  int rc = eval_samples_impl(ctx, w, samples, n, out, "dsgd_eval_samples_sums");
-  if (rc) return rc;
-  put_sums(out, loss_sum, correct, norm_squared);
-  return DSGD_OK;
-}
-
-// ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
 
 // Growing a device buffer (cudaMalloc, and cudaFree of the smaller one) waits for the kernels running on the device, so it
 // would wait forever for an async loop that runs until stopped.  The start of an async loop therefore sizes the buffers of
-// the score and metrics calls for n_rows rows (and the sort's storage for them), and a call that would have to grow one while
-// the loop runs -- a list of more ids than rows -- is refused.
-static int reserve_scores(dsgd_ctx *ctx) {
+// the request calls for n_rows rows (and the sort's storage for them), and a call that would have to grow one while the
+// loop runs -- a list of more ids than rows -- is refused.
+static int reserve_requests(dsgd_ctx *ctx) {
   const int64_t n = ctx->n_rows;
   int rc;
   if ((rc = ctx->eval_ids.grow(ctx, n, 1024)) || (rc = ctx->preds.grow(ctx, n, 1024)) || (rc = ctx->m_keys.grow(ctx, n, 1024)) ||
@@ -974,53 +745,249 @@ static int fits_while_running(dsgd_ctx *ctx, bool fits, const char *fn) {
   return DSGD_OK;
 }
 
-// out[i] = x . w (prob: sigmoid(-x . w)) of the n rows samples[i]; the values go through `preds`, the per-row request buffer
-static int scores_impl(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *out, bool prob,
-                       const char *fn) {
-  NEED(out, DSGD_ERR_INVALID, "%s: output is NULL", fn);
-  NEED(!prob || is_logistic(ctx), DSGD_ERR_STATE, "%s: probabilities need the SparseLogistic model (DSGD_FLAG_LOGISTIC)", fn);
+// the n row ids at the host address ids, into eval_ids; `preds`: the call also writes one value per id into preds
+static int rows_list(dsgd_ctx *ctx, const int32_t *ids, int64_t n, bool preds, const char *fn, row_set *rows) {
   NEED(ctx->pairs, DSGD_ERR_STATE, "%s: no rows loaded", fn);
-  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "%s: bad arguments", fn);
-  NEED(n > 0, DSGD_ERR_EMPTY, "%s: no samples", fn);
-  int rc = fits_while_running(ctx, ctx->eval_ids.cap >= n && ctx->preds.cap >= n, fn);
-  if (rc || (rc = request_ids(ctx, samples, n, fn))) return rc;
-  if (rc || (rc = ctx->preds.grow(ctx, n, 1024))) return rc;
-  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
-  if ((rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
-  if (prob) k_margins<true><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->eval_ids, n, wd, ctx->preds);
-  else k_margins<false><<<rows_grid(ctx, n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->eval_ids, n, wd, ctx->preds);
+  NEED(n >= 0 && (n == 0 || ids), DSGD_ERR_INVALID, "%s: bad arguments", fn);
+  NEED(n > 0, DSGD_ERR_EMPTY, "%s: empty sample (reduce on an empty collection throws)", fn);
+  int rc = fits_while_running(ctx, ctx->eval_ids.cap >= n && (!preds || ctx->preds.cap >= n), fn);
+  if (rc || (rc = check_ids(ctx, ids, n, fn, "sample index"))) return rc;
+  CU(cudaSetDevice(ctx->device));
+  if ((rc = ctx->eval_ids.grow(ctx, n, 1024))) return rc;
+  CU(cudaMemcpyAsync(ctx->eval_ids, ids, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  if (preds && (rc = ctx->preds.grow(ctx, n, 1024))) return rc;
+  *rows = {ctx->eval_ids, 0, n};
+  return DSGD_OK;
+}
+
+// The fp64 row kernel of model kModel over `rows` with the weights w: counters into cnt; kScatter: the gradient into g;
+// kPreds: the SVM kernel's sign predictions into preds.
+template <int kModel, bool kScatter, bool kPreds = false>
+static void launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, double *preds = nullptr) {
+  static_assert(!(kPreds && kModel == kLogistic), "k_rows_logistic writes no predictions");
+  if constexpr (kModel == kLogistic)
+    k_rows_logistic<kScatter><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids,
+                                                                              rows.row_begin, rows.n, w, g, ctx->cnt);
+  else
+    k_rows<kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids,
+                                                                             rows.row_begin, rows.n, w, g, preds, ctx->cnt);
+  LAUNCHED();
+}
+
+// The row kernel of a request: the fp32 streaming pass over kStreamMinRows rows or more (SVM only: it decides signs, and
+// the logistic loss needs the dot's value), else launch_rows.  Only an evaluation names a range of rows; a gradient or a
+// forward pass always lists them.
+template <int kModel, bool kScatter, bool kPreds = false>
+static int request_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, const float *w32, double *g, double *preds) {
+  if (kModel == kLogistic || !stream_eligible(ctx, rows.n)) {
+    launch_rows<kModel, kScatter, kPreds>(ctx, rows, w, g, preds);
+    return DSGD_OK;
+  }
+  return rows.ids ? stream_launch<kScatter, kPreds, false>(ctx, rows.ids, 0, rows.n, w, w32, g, preds)
+                  : stream_launch<false, false, true>(ctx, nullptr, rows.row_begin, rows.n, w, w32, nullptr, nullptr);
+}
+
+// The pass of a gradient (kScatter: the gradient into g, then k_finish) or of an evaluation over `rows` with the weights of
+// request_weights, then the shared tail: out2 = {loss, accuracy, loss sum, correct count, ||w||^2}, and the counters
+// cleared for the next pass (k_loss_scalar).
+template <int kModel, bool kScatter>
+static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
+  const double *w, *c, *nrm;
+  const float *w32;
+  int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
+  if (rc || (rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr))) return rc;
+  const double n = (double)rows.n;
+  if constexpr (kScatter) {
+    const int fin_blocks = cdiv(ctx->dim + 1, 256);
+    if constexpr (kModel == kLogistic) k_finish_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+    else k_finish<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+    LAUNCHED();
+  }
+  if constexpr (kModel == kLogistic) k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
+  else k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
   LAUNCHED();
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *preds_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(n >= 0 && (n == 0 || (samples && preds_out)), DSGD_ERR_INVALID, "dsgd_forward: bad arguments");
+  if (n == 0) return DSGD_OK;
+  row_set rows;
+  const double *wd, *cd, *nd;
+  const float *w32d;
+  int rc = rows_list(ctx, samples, n, true, __func__, &rows);
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
+  // a prediction is the sign of x . w under either model: the SVM's row kernels
+  if ((rc = request_rows<kSvm, false, true>(ctx, rows, wd, w32d, nullptr, ctx->preds))) return rc;
+  CU(cudaGetLastError());
+  CU(cudaMemsetAsync(ctx->cnt, 0, sizeof(unsigned long long) * 2, ctx->stream));
+  CU(cudaMemcpyAsync(preds_out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *grad_out,
+                             double *loss_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(n >= 0 && grad_out, DSGD_ERR_INVALID, "dsgd_gradient: bad arguments");
+  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_gradient: empty batch (Vec.sum of an empty list throws in the reference)");
+  NEED(samples, DSGD_ERR_INVALID, "dsgd_gradient: samples is NULL");
+  NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_gradient: dimSparsity not set");
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  if (rc || (rc = is_logistic(ctx) ? loss_pass<kLogistic, true>(ctx, w, rows) : loss_pass<kSvm, true>(ctx, w, rows)))
+    return rc;
+  CU(cudaMemcpyAsync(grad_out, ctx->g, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
+  double out2[2];
+  CU(cudaMemcpyAsync(out2, ctx->out2, sizeof out2, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemsetAsync(ctx->g, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (loss_out) *loss_out = out2[0];
+  return DSGD_OK;
+}
+
+// One evaluation pass over `rows`: out = {loss, accuracy, loss sum, correct count, ||w||^2}.  The SVM's loss sum is the
+// hinge sum, an integer.
+static int eval_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double out[5]) {
+  int rc = is_logistic(ctx) ? loss_pass<kLogistic, false>(ctx, w, rows) : loss_pass<kSvm, false>(ctx, w, rows);
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+// The evaluation behind the *_counts and *_sums calls, and their outputs (NULL: not wanted): the loss sum as hinge_sum
+// (*_counts) or as loss_sum (*_sums), the correct count and ||w||^2.
+static int eval_sums(dsgd_ctx *ctx, const double *w, const row_set &rows, double *loss_sum, int64_t *hinge_sum,
+                     int64_t *correct, double *norm_squared) {
+  double out[5];
+  int rc = eval_pass(ctx, w, rows, out);
+  if (rc) return rc;
+  if (loss_sum) *loss_sum = out[2];
+  if (hinge_sum) *hinge_sum = (int64_t)out[2];
+  if (correct) *correct = (int64_t)out[3];
+  if (norm_squared) *norm_squared = out[4];
+  return DSGD_OK;
+}
+
+// the *_counts calls report integer hinge sums, which only the SVM has
+static const char kCountsNeedSvm[] = "%s: the logistic model's loss sum is not an integer; use the *_sums call";
+
+extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
+                         double *acc_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  double out[5];
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  if (rc || (rc = eval_pass(ctx, w, rows, out))) return rc;
+  if (loss_out) *loss_out = out[0];
+  if (acc_out) *acc_out = out[1];
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *hinge_sum,
+                                int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_sum,
+                              int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                        int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
+                                        double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                      int64_t pos_begin, int64_t pos_end, double *loss_sum, int64_t *correct,
+                                      double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
+                                      int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+}
+
+// ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
+
+// out[i] = x . w (prob: sigmoid(-x . w)) of the listed rows; the values go through `preds`, the per-row request buffer
+static int scores_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *out, bool prob) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd);
+  if (rc) return rc;
+  if (prob) k_margins<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
+  else k_margins<false><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return DSGD_OK;
 }
 
 extern "C" int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *margins_out) {
   if (!ctx) return DSGD_ERR_INVALID;
-  return scores_impl(ctx, w, samples, n, margins_out, false, "dsgd_margins");
+  NEED(margins_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, true, __func__, &rows);
+  return rc ? rc : scores_pass(ctx, w, rows, margins_out, false);
 }
 
 extern "C" int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *probs_out) {
   if (!ctx) return DSGD_ERR_INVALID;
-  return scores_impl(ctx, w, samples, n, probs_out, true, "dsgd_probabilities");
+  NEED(probs_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
+  NEED(is_logistic(ctx), DSGD_ERR_STATE, "%s: probabilities need the SparseLogistic model (DSGD_FLAG_LOGISTIC)", __func__);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, true, __func__, &rows);
+  return rc ? rc : scores_pass(ctx, w, rows, probs_out, true);
 }
 
-// One metrics pass over rows [row_begin, row_begin + n) (ids == nullptr) or over the n row ids at the device address `ids`:
-// scores and counts (k_metrics_score), the two key runs sorted, U2 counted (k_auc_count).  The host reads the run lengths
-// between the scoring and the sort, which takes them from the host.  Launches of the sort's own kernels are not counted in
-// dsgd_launch_count.
-static int metrics_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int64_t row_begin, int64_t n, int64_t *out) {
+// One metrics pass over `rows`: scores and counts (k_metrics_score), the two key runs sorted, U2 counted (k_auc_count).  The
+// host reads the run lengths between the scoring and the sort, which takes them from the host.  Launches of the sort's own
+// kernels are not counted in dsgd_launch_count.
+static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *out, const char *fn) {
+  const int64_t n = rows.n;
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
-  int rc = fits_while_running(ctx, ctx->m_keys.cap >= n && ctx->m_alt.cap >= n && ctx->m_cnt, "metrics pass");
+  int rc = fits_while_running(ctx, ctx->m_keys.cap >= n && ctx->m_alt.cap >= n && ctx->m_cnt, fn);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
   if ((rc = ctx->m_keys.grow(ctx, n, 1024)) || (rc = ctx->m_alt.grow(ctx, n, 1024)) ||
       (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)))
     return rc;
   CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kMetWords, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
-  k_metrics_score<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, ids, row_begin, n, wd, ctx->m_keys,
-                                                 ctx->m_cnt);
+  k_metrics_score<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                 ctx->m_keys, ctx->m_cnt);
   LAUNCHED();
   CU(cudaGetLastError());
   unsigned long long h[kMetWords];
@@ -1037,8 +1004,7 @@ static int metrics_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int6
     CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_p, kp, (int)n_pos, 0, 64, ctx->stream));
     CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_n, kn, (int)n_neg, 0, 64, ctx->stream));
     size_t tmp = std::max(tmp_p, tmp_n);
-    if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, "metrics pass")) ||
-        (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
+    if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
       return rc;
     CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kp, (int)n_pos, 0, 64, ctx->stream));
     CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kn, (int)n_neg, 0, 64, ctx->stream));
@@ -1055,34 +1021,28 @@ static int metrics_pass(dsgd_ctx *ctx, const double *w, const int32_t *ids, int6
 
 extern "C" int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_metrics: out is NULL");
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_metrics: no rows loaded");
-  NEED(row_begin >= 0 && row_end <= ctx->n_rows && row_begin <= row_end, DSGD_ERR_RANGE,
-       "dsgd_eval_metrics: rows [%lld,%lld) outside [0,%lld)", (long long)row_begin, (long long)row_end, (long long)ctx->n_rows);
-  NEED(row_end > row_begin, DSGD_ERR_EMPTY, "dsgd_eval_metrics: empty range");
-  CU(cudaSetDevice(ctx->device));
-  return metrics_pass(ctx, w, nullptr, row_begin, row_end - row_begin, out);
+  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
 }
 
 extern "C" int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                          int64_t pos_begin, int64_t pos_end, int64_t *out) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_sampled_metrics: out is NULL");
-  int rc = draw_sample(ctx, row_begin, row_end, key, pos_begin, pos_end, "dsgd_eval_sampled_metrics");
-  if (rc) return rc;
-  return metrics_pass(ctx, w, ctx->eval_ids, 0, pos_end - pos_begin, out);
+  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
 }
 
 extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: out is NULL");
-  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_eval_samples_metrics: no rows loaded");
-  NEED(n >= 0 && (n == 0 || samples), DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: bad arguments");
-  NEED(n > 0, DSGD_ERR_EMPTY, "dsgd_eval_samples_metrics: empty sample");
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "dsgd_eval_samples_metrics: %lld ids; at most 2^31 - 1", (long long)n);
-  int rc = fits_while_running(ctx, ctx->eval_ids.cap >= n, "dsgd_eval_samples_metrics");
-  if (rc || (rc = request_ids(ctx, samples, n, "dsgd_eval_samples_metrics"))) return rc;
-  return metrics_pass(ctx, w, ctx->eval_ids, 0, n, out);
+  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all
@@ -1426,6 +1386,57 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
   return DSGD_OK;
 }
 
+// The per-step path of sync_staged for model kModel: n_steps steps of n_per_step staged ids from smp, step s at the rate
+// lrs[s] (lrs == nullptr: lr), its loss into losses[s] (losses == nullptr: none)
+template <int kModel>
+static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, int64_t n_steps, double lr,
+                         const double *lrs, double *losses, bool single, int32_t k_total) {
+  const int upd_blocks = cdiv(ctx->dim, 256);
+  const int fin_blocks = cdiv(ctx->dim + 1, 256);
+  double lr_s = lr;   // the rate of step s
+  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights
+  auto update = [&](auto kernel, auto kernel_avg, double *gbuf, double k_den, double n_local, double *loss_dev) {
+    if (ctx->avg_on)
+      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
+                                                      ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
+    else
+      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
+                                                  ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev);
+    LAUNCHED();
+    if (ctx->avg_on) ++ctx->avg_n;
+  };
+  for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
+    if (lrs) lr_s = lrs[s];
+    double *loss_dev = losses ? losses + s : nullptr;
+    if (single) {
+      // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
+      profiled(ctx, [&] { launch_rows<kModel, true>(ctx, {smp, 0, n_per_step}, ctx->w, ctx->g); });
+      update(k_update<true, kModel>, k_update_avg<true, kModel>, ctx->g, 1.0, (double)n_per_step, loss_dev);
+      continue;
+    }
+    // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
+    int64_t off = 0;
+    for (int32_t v = 0; v < ctx->n_local; ++v) {
+      const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
+      profiled(ctx, [&] { launch_rows<kModel, true>(ctx, {smp + off, 0, nv}, ctx->w, ctx->g); });
+      if constexpr (kModel == kLogistic)
+        k_finish_acc_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
+                                                                   (double)nv, v == 0 ? 1 : 0);
+      else
+        k_finish_acc<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
+                                                          (double)nv, v == 0 ? 1 : 0);
+      LAUNCHED();
+      off += nv;
+    }
+    if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
+    if (ctx->world > 1)
+      NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
+    update(k_update<false, kModel>, k_update_avg<false, kModel>, ctx->gsum, (double)k_total, 0.0, loss_dev);
+  }
+  CU(cudaGetLastError());
+  return DSGD_OK;
+}
+
 // The sync steps of dsgd_sync_steps_staged, and of dsgd_sync_steps_lr with lrs (n_steps host values, step s takes lrs[s])
 // instead of the scalar lr.  The per-step paths pass each step's rate as the kernel argument they always take; the
 // persistent and fused kernels read the table on the device (persist_run).
@@ -1470,84 +1481,16 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
     int rc = ctx->losses.grow(ctx, n_steps, 1024);
     if (rc) return rc;
   }
-  const int upd_blocks = cdiv(ctx->dim, 256);
-  const int fin_blocks = cdiv(ctx->dim + 1, 256);
   if ((single && !logistic && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
     // exchange block mapped (fused): the same kernel aggregates over NVLink
     return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, lrs,
                        want_losses ? ctx->losses.p : nullptr);
   }
-  double lr_s = lr;   // the rate of step s
-  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights
-  auto update = [&](auto kernel, auto kernel_avg, double *gbuf, double k_den, double n_local, double *loss_dev) {
-    if (ctx->avg_on)
-      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                      ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
-    else
-      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                  ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev);
-    LAUNCHED();
-    if (ctx->avg_on) ++ctx->avg_n;
-  };
-  for (int64_t s = 0; s < n_steps; ++s) {
-    if (lrs) lr_s = lrs[s];
-    const int32_t *smp = ctx->samples + first + s * n_per_step;
-    double *loss_dev = want_losses ? ctx->losses + s : nullptr;
-    if (single) {
-      // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
-      if (logistic) {
-        profiled(ctx, [&] {
-          k_rows_logistic<true><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp,
-                                                                                      0, n_per_step, ctx->w, ctx->g, ctx->cnt);
-        });
-        LAUNCHED();
-        update(k_update<true, kLogistic>, k_update_avg<true, kLogistic>, ctx->g, 1.0, (double)n_per_step, loss_dev);
-        continue;
-      }
-      profiled(ctx, [&] {
-        k_rows<true, false><<<rows_grid(ctx, n_per_step), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp, 0,
-                                                                                 n_per_step, ctx->w, ctx->g, nullptr, ctx->cnt);
-      });
-      LAUNCHED();
-      update(k_update<true>, k_update_avg<true>, ctx->g, 1.0, (double)n_per_step, loss_dev);
-      continue;
-    }
-    int64_t off = 0;
-    for (int32_t v = 0; v < ctx->n_local; ++v) {
-      const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
-      if (logistic) {
-        profiled(ctx, [&] {
-          k_rows_logistic<true><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0,
-                                                                              nv, ctx->w, ctx->g, ctx->cnt);
-        });
-        LAUNCHED();
-        k_finish_acc_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
-                                                                   (double)nv, v == 0 ? 1 : 0);
-        LAUNCHED();
-        off += nv;
-        continue;
-      }
-      profiled(ctx, [&] {
-        k_rows<true, false><<<rows_grid(ctx, nv), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, smp + off, 0, nv,
-                                                                         ctx->w, ctx->g, nullptr, ctx->cnt);
-      });
-      LAUNCHED();
-      k_finish_acc<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt, (double)nv,
-                                                        v == 0 ? 1 : 0);
-      LAUNCHED();
-      off += nv;
-    }
-    if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
-    if (ctx->world > 1)
-      NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    if (logistic)
-      update(k_update<false, kLogistic>, k_update_avg<false, kLogistic>, ctx->gsum, (double)k_total, 0.0, loss_dev);
-    else
-      update(k_update<false>, k_update_avg<false>, ctx->gsum, (double)k_total, 0.0, loss_dev);
-  }
-  CU(cudaGetLastError());
-  return DSGD_OK;
+  const int32_t *smp = ctx->samples + first;
+  double *loss_dev = want_losses ? ctx->losses.p : nullptr;
+  return logistic ? sync_per_step<kLogistic>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
+                  : sync_per_step<kSvm>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
 }
 
 extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,
@@ -1740,7 +1683,7 @@ static int async_launch(dsgd_ctx *ctx, const double *w0, const int32_t *assigned
   NEED(batch >= 1 && lanes >= 1 && lanes <= 4096, DSGD_ERR_INVALID, "dsgd_start_async: bad arguments");
   CU(cudaSetDevice(ctx->device));
   int rc = load_all_kernels(ctx);
-  if (rc || (rc = reserve_scores(ctx))) return rc;
+  if (rc || (rc = reserve_requests(ctx))) return rc;
   if (w0) {  // weights() = request.weights
     CU(cudaMemcpyAsync(ctx->w, w0, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
     rc = refresh_resident(ctx);  // also S = w . d and the control slots of the replica
@@ -1785,7 +1728,7 @@ extern "C" int dsgd_start_async(dsgd_ctx *ctx, const double *w0, const int32_t *
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot initialize async computation: slave is in synchronous mode.");
   NEED(assigned && n_assigned >= 1, DSGD_ERR_EMPTY, "dsgd_start_async: no samples assigned (Random.nextInt(0) throws)");
   NEED(n_assigned <= ctx->n_rows, DSGD_ERR_RANGE, "dsgd_start_async: more assigned samples than rows");
-  int rc = check_ids(ctx, assigned, n_assigned, "assigned sample");
+  int rc = check_ids(ctx, assigned, n_assigned, __func__, "assigned sample");
   if (rc) return rc;
   CU(cudaSetDevice(ctx->device));
   if ((rc = ctx->a_assigned.grow(ctx, n_assigned, 1024))) return rc;
@@ -1803,7 +1746,7 @@ extern "C" int dsgd_async_replay(dsgd_ctx *ctx, const double *w0, const int32_t 
   NEED(ctx->flags & DSGD_FLAG_ASYNC, DSGD_ERR_STATE, "Cannot initialize async computation: slave is in synchronous mode.");
   NEED(samples && batch >= 1 && n_updates >= 1, DSGD_ERR_EMPTY, "dsgd_async_replay: empty sequence");
   const int64_t n = (int64_t)batch * n_updates;
-  int rc = check_ids(ctx, samples, n, "sample index");
+  int rc = check_ids(ctx, samples, n, __func__, "sample index");
   if (rc) return rc;
   CU(cudaSetDevice(ctx->device));
   if ((rc = ctx->a_replay.grow(ctx, n, 1024))) return rc;

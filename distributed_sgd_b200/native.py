@@ -190,6 +190,16 @@ def host_lib():
     return _host
 
 
+def _drawn(row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int) -> tuple:
+    """The row arguments of a sample drawn on the device from rows [row_begin, row_end): the key goes in as 64 bits."""
+    return row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF, pos_begin, pos_end
+
+
+# out-parameters of the dsgd_eval_*counts and dsgd_eval_*sums calls: (hinge sum | loss sum, correct count, ||w||^2)
+_COUNTS = (_i64, _i64, _f64)
+_SUMS = (_f64, _i64, _f64)
+
+
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
@@ -306,10 +316,7 @@ class NativeCtx:
 
     def forward(self, samples, w=None) -> np.ndarray:
         samples = _arr(samples, np.int32)
-        out = np.zeros(samples.size, dtype=np.float64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_forward(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
-        return out
+        return self._request("forward", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
 
     def gradient(self, samples, w=None, want_loss: bool = False):
         samples = _arr(samples, np.int32)
@@ -320,104 +327,77 @@ class NativeCtx:
                                        C.byref(loss) if want_loss else None))
         return (out, loss.value) if want_loss else out
 
-    def eval(self, row_begin: int, row_end: int, w=None) -> Tuple[float, float]:
-        loss, acc = C.c_double(), C.c_double()
+    def _request(self, fn: str, w, rows: tuple, out):
+        """dsgd_<fn>(ctx, w, *rows, out...).  rows: (row_begin, row_end), _drawn(...) or (ids pointer, len(ids)).  out: an
+        array, filled and returned, or ctypes scalar types, passed by reference and returned as a tuple of values."""
         w = self._w(w)
-        self._ck(self._l.dsgd_eval(self._h, _ptr(w), row_begin, row_end, C.byref(loss), C.byref(acc)))
-        return loss.value, acc.value
+        call = getattr(self._l, "dsgd_" + fn)
+        if isinstance(out, np.ndarray):
+            self._ck(call(self._h, _ptr(w), *rows, _ptr(out)))
+            return out
+        vals = [t() for t in out]
+        self._ck(call(self._h, _ptr(w), *rows, *[C.byref(v) for v in vals]))
+        return tuple([v.value for v in vals])
+
+    def eval(self, row_begin: int, row_end: int, w=None) -> Tuple[float, float]:
+        return self._request("eval", w, (row_begin, row_end), (_f64, _f64))
 
     def eval_counts(self, row_begin: int, row_end: int, w=None) -> Tuple[int, int, float]:
         """(hinge sum, correct count, ||w||^2) over rows [row_begin, row_end) -- exact shardable form."""
-        h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_counts(self._h, _ptr(w), row_begin, row_end, C.byref(h), C.byref(c), C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_counts", w, (row_begin, row_end), _COUNTS)
 
     def eval_sampled_counts(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                             w=None) -> Tuple[int, int, float]:
         """(hinge sum, correct count, ||w||^2) over positions [pos_begin, pos_end) of the sample drawn on the device from rows
         [row_begin, row_end) with `key` (dsgd_eval_sampled_counts)."""
-        h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_sampled_counts(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
-                                                  pos_begin, pos_end, C.byref(h), C.byref(c), C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_sampled_counts", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), _COUNTS)
 
     def eval_samples_counts(self, samples, w=None) -> Tuple[int, int, float]:
         """The same counters over a list of row ids; repeats count every time (dsgd_eval_samples_counts)."""
         samples = _arr(samples, np.int32)
-        h, c, n2 = C.c_int64(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_samples_counts(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
-                                                  C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_samples_counts", w, (_ptr(samples), samples.size), _COUNTS)
 
     def eval_sums(self, row_begin: int, row_end: int, w=None) -> Tuple[float, int, float]:
         """(loss sum, correct count, ||w||^2) over rows [row_begin, row_end), for either model (dsgd_eval_sums)."""
-        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_sums(self._h, _ptr(w), row_begin, row_end, C.byref(h), C.byref(c), C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_sums", w, (row_begin, row_end), _SUMS)
 
     def eval_sampled_sums(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                           w=None) -> Tuple[float, int, float]:
         """(loss sum, correct count, ||w||^2) over positions [pos_begin, pos_end) of the device-drawn sample
         (dsgd_eval_sampled_sums)."""
-        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_sampled_sums(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
-                                                pos_begin, pos_end, C.byref(h), C.byref(c), C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_sampled_sums", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), _SUMS)
 
     def eval_samples_sums(self, samples, w=None) -> Tuple[float, int, float]:
         """(loss sum, correct count, ||w||^2) over a list of row ids; repeats count every time (dsgd_eval_samples_sums)."""
         samples = _arr(samples, np.int32)
-        h, c, n2 = C.c_double(), C.c_int64(), C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_samples_sums(self._h, _ptr(w), _ptr(samples), samples.size, C.byref(h), C.byref(c),
-                                                C.byref(n2)))
-        return h.value, c.value, n2.value
+        return self._request("eval_samples_sums", w, (_ptr(samples), samples.size), _SUMS)
 
     # -- scores and ranking metrics --
     def margins(self, samples, w=None) -> np.ndarray:
         """x . w in fp64 for each listed row (dsgd_margins)."""
         samples = _arr(samples, np.int32)
-        out = np.zeros(samples.size, dtype=np.float64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_margins(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
-        return out
+        return self._request("margins", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
 
     def probabilities(self, samples, w=None) -> np.ndarray:
         """P(y = +1 | x) = sigmoid(-x . w) for each listed row; SparseLogistic contexts only (dsgd_probabilities)."""
         samples = _arr(samples, np.int32)
-        out = np.zeros(samples.size, dtype=np.float64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
-        return out
+        return self._request("probabilities", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
 
     def eval_metrics(self, row_begin: int, row_end: int, w=None) -> np.ndarray:
         """The METRICS_WORDS exact counts over rows [row_begin, row_end) (dsgd_eval_metrics)."""
-        out = np.zeros(METRICS_WORDS, dtype=np.int64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_metrics(self._h, _ptr(w), row_begin, row_end, _ptr(out)))
-        return out
+        return self._request("eval_metrics", w, (row_begin, row_end), np.zeros(METRICS_WORDS, dtype=np.int64))
 
     def eval_sampled_metrics(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                              w=None) -> np.ndarray:
         """The same counts over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_metrics)."""
-        out = np.zeros(METRICS_WORDS, dtype=np.int64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_sampled_metrics(self._h, _ptr(w), row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF,
-                                                   pos_begin, pos_end, _ptr(out)))
-        return out
+        return self._request("eval_sampled_metrics", w, _drawn(row_begin, row_end, key, pos_begin, pos_end),
+                             np.zeros(METRICS_WORDS, dtype=np.int64))
 
     def eval_samples_metrics(self, samples, w=None) -> np.ndarray:
         """The same counts over a list of row ids; repeats count every time (dsgd_eval_samples_metrics)."""
         samples = _arr(samples, np.int32)
-        out = np.zeros(METRICS_WORDS, dtype=np.int64)
-        w = self._w(w)
-        self._ck(self._l.dsgd_eval_samples_metrics(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out)))
-        return out
+        return self._request("eval_samples_metrics", w, (_ptr(samples), samples.size),
+                             np.zeros(METRICS_WORDS, dtype=np.int64))
 
     # -- sync --
     def set_workers(self, counts, k_total: int = 0):

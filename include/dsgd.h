@@ -27,6 +27,10 @@
  *    (the reference serves them from its 8-thread pool concurrently with asyncTask, core/Slave.scala:24-30).
  *    dsgd_update_grad may also be called from several threads at once: the calls take a lock of the ctx and
  *    each delta is applied exactly once.
+ *    From dsgd_start_async until dsgd_stop_async, every call that takes a list of row ids (dsgd_forward,
+ *    dsgd_gradient, dsgd_margins, dsgd_probabilities, dsgd_eval_samples_*) refuses a list of more ids than
+ *    loaded rows with DSGD_ERR_STATE: its buffers would have to grow, and growing one waits for every kernel on
+ *    the device, the running loop included.
  */
 #ifndef DSGD_H
 #define DSGD_H
