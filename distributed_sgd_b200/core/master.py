@@ -63,6 +63,30 @@ def metrics_dict(words) -> dict:
             "f1": ratio(2 * tp, 2 * tp + fp + fn + pos_none), "auc": auc, "accuracy": ratio(tp + tn, P + N)}
 
 
+def curve_dict(result) -> dict:
+    """The result of Master.local_curve from a NativeCtx.eval_*curve result: metrics_dict(words) plus average_precision and
+    n_points, and for a full curve pass the points under "curve", highest score first (the scalar counts and rates of
+    metrics_dict keep their keys): thresholds, tp and fp (the rows at or above each threshold) and the derived precision =
+    tp / (tp + fp), recall = tpr = tp / P and fpr = fp / N, with P and N the non-NaN positive and negative rows; a rate whose
+    denominator is 0 is nan."""
+    words, ap = result[0], result[1]
+    out = metrics_dict(words)
+    out["average_precision"] = float(ap)
+    out["n_points"] = int(result[2]) if len(result) == 3 else len(result[2])   # distinct scores
+    if len(result) == 5:
+        thr, tp, fp = result[2], np.asarray(result[3], dtype=np.int64), np.asarray(result[4], dtype=np.int64)
+        P, N = (int(tp[-1]), int(fp[-1])) if len(tp) else (0, 0)
+        nan = float("nan")
+        with np.errstate(divide="ignore", invalid="ignore"):
+            precision = np.where(tp + fp > 0, tp / np.maximum(tp + fp, 1), nan)
+            recall = tp / P if P else np.full(len(tp), nan)
+            fpr = fp / N if N else np.full(len(fp), nan)
+        out["curve"] = {"thresholds": [float(x) for x in thr], "tp": [int(x) for x in tp], "fp": [int(x) for x in fp],
+                        "precision": [float(x) for x in precision], "recall": [float(x) for x in recall],
+                        "tpr": [float(x) for x in recall], "fpr": [float(x) for x in fpr]}
+    return out
+
+
 class EpochDraw(list):
     """The batch draws of one epoch: `self[s][k]` = row ids of worker k at step s (a list of lists of int32 arrays, the
     shape the tests and the oracle replay), backed by ONE array `ids[steps, K, batch]` (-1 beyond a short slice) and
@@ -267,6 +291,22 @@ class Master:
         if ids is None:
             return metrics_dict(self.ctx.eval_sampled_metrics(b, e, key, 0, k, weights))
         return metrics_dict(self.ctx.eval_samples_metrics(ids, weights))
+
+    def local_curve(self, weights=None, test_data: bool = False, curve: bool = True) -> dict:
+        """local_metrics plus average precision, and with `curve` the ROC and precision-recall points over the train (or test)
+        rows (curve_dict).  Like local_metrics, every rank evaluates the whole range."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return curve_dict(self.ctx.eval_curve(b, e, weights, curve=curve))
+
+    def local_sampled_curve(self, weights, samples_count: int, test_data: bool = False, curve: bool = True) -> dict:
+        """local_curve on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
+        sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled curve of {samples_count} rows: the sample is empty")
+        if ids is None:
+            return curve_dict(self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=curve))
+        return curve_dict(self.ctx.eval_samples_curve(ids, weights, curve=curve))
 
     def predict(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> dict:
         """Master.predict (core/Master.scala:61-75): idx -> prediction over the training rows; each worker

@@ -12,6 +12,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <mutex>
 #include <string>
 #include <utility>
@@ -25,6 +26,10 @@
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
+#include <cub/device/device_merge.cuh>       // the curve pass's merge and scan, likewise
+#include <cub/device/device_scan.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 using namespace dsgd;
 
@@ -142,6 +147,12 @@ struct dsgd_ctx {
   // the radix sort's alternate keys and temporary storage, and the counter words (MetricWord)
   dev_buf<unsigned long long> m_keys, m_alt, m_cnt;
   dev_buf<unsigned char> m_tmp;
+  // a curve pass (dsgd_eval_*curve): its counter words (CurveWord), the merged key runs, the exclusive scan of their tie
+  // ends, and the points (sort, merge and scan share m_tmp)
+  dev_buf<unsigned long long> c_cnt, c_merged;
+  dev_buf<int> c_excl;
+  dev_buf<double> c_thr;
+  dev_buf<long long> c_tp, c_fp;
 
   ncclComm_t comm = nullptr;
 
@@ -727,16 +738,33 @@ static int rows_drawn(dsgd_ctx *ctx, int64_t row_begin, int64_t row_end, uint64_
 // would wait forever for an async loop that runs until stopped.  The start of an async loop therefore sizes the buffers of
 // the request calls for n_rows rows (and the sort's storage for them), and a call that would have to grow one while the
 // loop runs -- a list of more ids than rows -- is refused.
+// The curve pass's merge of the two sorted key runs into c_merged, and the exclusive scan of tie_end over the merged keys
+// into c_excl (tmp == nullptr: the storage they need, into bytes).  reserve_requests sizes with these same instantiations.
+static cudaError_t merge_runs(dsgd_ctx *ctx, void *tmp, size_t &bytes, const unsigned long long *pos, int64_t n_pos,
+                              const unsigned long long *neg, int64_t n_neg) {
+  return cub::DeviceMerge::MergeKeys(tmp, bytes, pos, (int)n_pos, neg, (int)n_neg, ctx->c_merged.p, ::cuda::std::less<>{},
+                                     ctx->stream);
+}
+static cudaError_t scan_tie_ends(dsgd_ctx *ctx, void *tmp, size_t &bytes, int64_t n_all) {
+  auto flags = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), tie_end{ctx->c_merged.p, (int)n_all});
+  return cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, ctx->c_excl.p, (int)n_all, ctx->stream);
+}
+
 static int reserve_requests(dsgd_ctx *ctx) {
   const int64_t n = ctx->n_rows;
   int rc;
   if ((rc = ctx->eval_ids.grow(ctx, n, 1024)) || (rc = ctx->preds.grow(ctx, n, 1024)) || (rc = ctx->m_keys.grow(ctx, n, 1024)) ||
-      (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)))
+      (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)) ||
+      (rc = ctx->c_cnt.grow(ctx, kCurWords, kCurWords)) || (rc = ctx->c_merged.grow(ctx, n, 1024)) ||
+      (rc = ctx->c_excl.grow(ctx, n, 1024)) || (rc = ctx->c_thr.grow(ctx, n, 1024)) || (rc = ctx->c_tp.grow(ctx, n, 1024)) ||
+      (rc = ctx->c_fp.grow(ctx, n, 1024)))
     return rc;
-  size_t tmp = 0;
+  size_t tmp = 0, tmp_merge = 0, tmp_scan = 0;
   cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
   CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, kb, (int)n, 0, 64, ctx->stream));
-  return ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16);
+  CU(merge_runs(ctx, nullptr, tmp_merge, ctx->m_keys.p, n - n / 2, ctx->m_alt.p, n / 2));   // sized by the total
+  CU(scan_tie_ends(ctx, nullptr, tmp_scan, n));
+  return ctx->m_tmp.grow(ctx, (int64_t)std::max({tmp, tmp_merge, tmp_scan}), 1 << 16);
 }
 
 static int fits_while_running(dsgd_ctx *ctx, bool fits, const char *fn) {
@@ -973,10 +1001,17 @@ extern "C" int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t 
   return rc ? rc : scores_pass(ctx, w, rows, probs_out, true);
 }
 
-// One metrics pass over `rows`: scores and counts (k_metrics_score), the two key runs sorted, U2 counted (k_auc_count).  The
-// host reads the run lengths between the scoring and the sort, which takes them from the host.  Launches of the sort's own
-// kernels are not counted in dsgd_launch_count.
-static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *out, const char *fn) {
+// The first half of a metrics or a curve pass over `rows`: scores and counts (k_metrics_score), the words and the run
+// lengths read by the host (the sort takes its lengths from the host), and the key runs sorted.  A metrics pass
+// (`each_run` false) sorts only when both runs have keys, since otherwise there is no pair to count; a curve pass sorts
+// every run that has keys.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
+struct sorted_runs {
+  unsigned long long h[kMetWords];   // the counter words as k_metrics_score left them
+  int64_t n_pos, n_neg;
+  const unsigned long long *pos, *neg;   // each run ascending, if it was sorted
+};
+static int score_and_sort(dsgd_ctx *ctx, const double *w, const row_set &rows, bool each_run, const char *fn,
+                          sorted_runs *s) {
   const int64_t n = rows.n;
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = fits_while_running(ctx, ctx->m_keys.cap >= n && ctx->m_alt.cap >= n && ctx->m_cnt, fn);
@@ -990,26 +1025,42 @@ static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int
                                                  ctx->m_keys, ctx->m_cnt);
   LAUNCHED();
   CU(cudaGetLastError());
-  unsigned long long h[kMetWords];
-  CU(cudaMemcpyAsync(h, ctx->m_cnt, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(s->h, ctx->m_cnt, sizeof s->h, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
-  const int64_t n_pos = (int64_t)h[kMetPosSlots], n_neg = (int64_t)h[kMetNegSlots];
-  if (n_pos > 0 && n_neg > 0) {   // else no pair: U2 = 0
-    // the positives sit in keys[0, n_pos), the negatives in keys[n - n_neg, n); each run sorts within its own slice of
-    // the two buffers, and Current() is the buffer that holds it sorted.  Sorted positives let the threads of a warp walk
-    // nearly the same search path through the negatives.
-    cub::DoubleBuffer<unsigned long long> kp(ctx->m_keys.p, ctx->m_alt.p);
-    cub::DoubleBuffer<unsigned long long> kn(ctx->m_keys.p + (n - n_neg), ctx->m_alt.p + (n - n_neg));
+  const int64_t n_pos = (int64_t)s->h[kMetPosSlots], n_neg = (int64_t)s->h[kMetNegSlots];
+  // the positives sit in keys[0, n_pos), the negatives in keys[n - n_neg, n); each run sorts within its own slice of the
+  // two buffers, and Current() is the buffer that holds it sorted
+  cub::DoubleBuffer<unsigned long long> kp(ctx->m_keys.p, ctx->m_alt.p);
+  cub::DoubleBuffer<unsigned long long> kn(ctx->m_keys.p + (n - n_neg), ctx->m_alt.p + (n - n_neg));
+  const bool sort_pos = n_pos > 0 && (each_run || n_neg > 0), sort_neg = n_neg > 0 && (each_run || n_pos > 0);
+  if (sort_pos || sort_neg) {
     size_t tmp_p = 0, tmp_n = 0;
-    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_p, kp, (int)n_pos, 0, 64, ctx->stream));
-    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_n, kn, (int)n_neg, 0, 64, ctx->stream));
+    if (sort_pos) CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_p, kp, (int)n_pos, 0, 64, ctx->stream));
+    if (sort_neg) CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_n, kn, (int)n_neg, 0, 64, ctx->stream));
     size_t tmp = std::max(tmp_p, tmp_n);
     if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
       return rc;
-    CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kp, (int)n_pos, 0, 64, ctx->stream));
-    CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kn, (int)n_neg, 0, 64, ctx->stream));
+    if (sort_pos) CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kp, (int)n_pos, 0, 64, ctx->stream));
+    if (sort_neg) CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kn, (int)n_neg, 0, 64, ctx->stream));
+  }
+  s->n_pos = n_pos;
+  s->n_neg = n_neg;
+  s->pos = kp.Current();
+  s->neg = kn.Current();
+  return DSGD_OK;
+}
+
+// One metrics pass over `rows`: score_and_sort, then U2 counted (k_auc_count).
+static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *out, const char *fn) {
+  sorted_runs s;
+  int rc = score_and_sort(ctx, w, rows, false, fn, &s);
+  if (rc) return rc;
+  unsigned long long *h = s.h;
+  const int64_t n_pos = s.n_pos, n_neg = s.n_neg;
+  if (n_pos > 0 && n_neg > 0) {   // else no pair: U2 = 0
+    // Sorted positives let the threads of a warp walk nearly the same search path through the negatives.
     const int cgrid = (int)std::min<int64_t>(cdiv(n_pos, 256), (int64_t)ctx->sm_count * 8);
-    k_auc_count<<<cgrid, 256, 0, ctx->stream>>>(kp.Current(), n_pos, kn.Current(), n_neg, ctx->m_cnt + kMetU2);
+    k_auc_count<<<cgrid, 256, 0, ctx->stream>>>(s.pos, n_pos, s.neg, n_neg, ctx->m_cnt + kMetU2);
     LAUNCHED();
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(&h[kMetU2], ctx->m_cnt + kMetU2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1017,6 +1068,105 @@ static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int
   }
   for (int k = 0; k < DSGD_METRICS_WORDS; ++k) out[k] = (int64_t)h[k];
   return DSGD_OK;
+}
+
+// One curve pass over `rows` (DESIGN.md §4.9): score_and_sort with every run sorted, then k_curve_count (U2, the limbs of
+// S = sum of v_i, the number of points m) and k_curve_sum.  With thr != nullptr also the points: the runs merged, the
+// exclusive scan of the merged keys' tie ends, k_curve_emit, and the m points copied back at once.  AP = S / P, NaN when a
+// score is NaN or there is no positive row.
+static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *words, double *ap, int64_t *n_points,
+                      double *thr, int64_t *tp, int64_t *fp, const char *fn) {
+  const int64_t n = rows.n;
+  const bool curve = thr != nullptr;
+  int rc = fits_while_running(ctx, ctx->c_cnt && (!curve || (ctx->c_merged.cap >= n && ctx->c_excl.cap >= n &&
+                                                              ctx->c_thr.cap >= n && ctx->c_tp.cap >= n && ctx->c_fp.cap >= n)),
+                              fn);
+  sorted_runs s;
+  if (rc || (rc = score_and_sort(ctx, w, rows, true, fn, &s)) || (rc = ctx->c_cnt.grow(ctx, kCurWords, kCurWords))) return rc;
+  CU(cudaMemsetAsync(ctx->c_cnt, 0, sizeof(unsigned long long) * kCurWords, ctx->stream));
+  const int64_t n_all = s.n_pos + s.n_neg;
+  const int grid = (int)std::min<int64_t>(std::max(cdiv(n_all, 256), 1), (int64_t)ctx->sm_count * 8);
+  k_curve_count<<<grid, 256, 0, ctx->stream>>>(s.pos, s.n_pos, s.neg, s.n_neg, ctx->m_cnt + kMetU2, ctx->c_cnt);
+  LAUNCHED();
+  k_curve_sum<<<1, 1, 0, ctx->stream>>>(ctx->c_cnt);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  if (curve && n_all > 0) {
+    if ((rc = ctx->c_merged.grow(ctx, n, 1024)) || (rc = ctx->c_excl.grow(ctx, n, 1024)) || (rc = ctx->c_thr.grow(ctx, n, 1024)) ||
+        (rc = ctx->c_tp.grow(ctx, n, 1024)) || (rc = ctx->c_fp.grow(ctx, n, 1024)))
+      return rc;
+    size_t tmp_merge = 0, tmp_scan = 0;
+    CU(merge_runs(ctx, nullptr, tmp_merge, s.pos, s.n_pos, s.neg, s.n_neg));
+    CU(scan_tie_ends(ctx, nullptr, tmp_scan, n_all));
+    size_t tmp = std::max(tmp_merge, tmp_scan);
+    if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
+      return rc;
+    CU(merge_runs(ctx, ctx->m_tmp.p, tmp, s.pos, s.n_pos, s.neg, s.n_neg));
+    tmp = std::max(tmp_merge, tmp_scan);
+    CU(scan_tie_ends(ctx, ctx->m_tmp.p, tmp, n_all));
+    k_curve_emit<<<grid, 256, 0, ctx->stream>>>(ctx->c_merged, n_all, ctx->c_excl, s.pos, s.n_pos, s.neg, s.n_neg, ctx->c_cnt,
+                                                ctx->c_thr, ctx->c_tp, ctx->c_fp);
+    LAUNCHED();
+    CU(cudaGetLastError());
+  }
+  unsigned long long c[kCurWords];
+  CU(cudaMemcpyAsync(c, ctx->c_cnt, sizeof c, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&s.h[kMetU2], ctx->m_cnt + kMetU2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int64_t m = (int64_t)c[kCurPoints];
+  if (curve && m > 0) {
+    CU(cudaMemcpyAsync(thr, ctx->c_thr, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(tp, ctx->c_tp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(fp, ctx->c_fp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+  }
+  for (int k = 0; k < DSGD_METRICS_WORDS; ++k) words[k] = (int64_t)s.h[k];
+  const int64_t P = words[kMetTp] + words[kMetFn] + words[kMetPosNone];
+  double S;
+  memcpy(&S, &c[kCurSum], sizeof S);
+  *ap = (words[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
+  *n_points = m;
+  return DSGD_OK;
+}
+
+// the outputs of a curve call: words, ap and the point count always; the three point arrays all or none
+static int curve_outputs(dsgd_ctx *ctx, const int64_t *words, const double *ap, const int64_t *n_points, const double *thr,
+                         const int64_t *tp, const int64_t *fp, const char *fn) {
+  NEED(words && ap && n_points, DSGD_ERR_INVALID, "%s: words_out, ap_out or n_points_out is NULL", fn);
+  NEED(!thr == !tp && !tp == !fp, DSGD_ERR_INVALID,
+       "%s: thr_out, tp_out and fp_out are all NULL (average precision only) or all set", fn);
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *words_out,
+                               double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
+  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                       int64_t pos_begin, int64_t pos_end, int64_t *words_out, double *ap_out,
+                                       int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
+  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
+                                       double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out,
+                                       int64_t *fp_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  if (rc) return rc;
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  if ((rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
+  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
 }
 
 extern "C" int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out) {

@@ -1,5 +1,5 @@
 // dsgd_metrics.cuh -- sm_90a kernels of the scoring and ranking-metric calls (dsgd_margins, dsgd_probabilities, the
-// dsgd_eval_*metrics calls; DESIGN.md §4.8).
+// dsgd_eval_*metrics calls; DESIGN.md §4.8) and of the curve calls (dsgd_eval_*curve; §4.9, at the end of this file).
 //
 // A metrics pass is three steps on the ctx's stream:
 //   1. k_metrics_score: x . w of every row in fp64 (row_margin, the body dsgd_margins runs too), the confusion counts, and
@@ -149,6 +149,118 @@ __global__ void __launch_bounds__(256) k_auc_count(const unsigned long long *__r
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if ((threadIdx.x & 31) == 0 && acc) atomicAdd(u2, acc);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Curves and average precision (the dsgd_eval_*curve calls; DESIGN.md §4.9).  A curve pass scores and sorts as a metrics
+// pass does (both runs sorted even when the other class is empty), then:
+//   4. k_curve_count: one thread per sorted key.  A positive adds U2 as k_auc_count does and v_i = tp_i / (tp_i + fp_i), the
+//      precision at its own score, to fixed-point limbs (dsgd_fixed.cuh); every key that ends a tie group of the union of
+//      the two runs counts one point.
+//   5. k_curve_sum: S = sum of the v_i as a double.
+//   6. (curve wanted) cub::DeviceMerge::MergeKeys of the two runs, cub::DeviceScan::ExclusiveSum of tie_end over the merged
+//      keys, and k_curve_emit: the last key of every tie group writes its point, highest score first.
+// Every count is an integer and S is an order-free fixed-point sum: the result does not depend on the grid.
+// ---------------------------------------------------------------------------------------------------
+
+// Words of a curve pass's own counter block (after the MetricWord block, which holds U2)
+enum CurveWord : int {
+  kCurAcc = 0,                   // [0, kLossAccWords): the limbs of S and their overflow count (acc_add_local)
+  kCurPoints = kLossAccWords,    // m: distinct scores among the non-NaN rows
+  kCurSum = kLossAccWords + 1,   // S as the bits of a double (k_curve_sum)
+  kCurWords = 16
+};
+
+// first index in a[0, n) whose key is >= key
+__device__ __forceinline__ int64_t key_lower_bound(const unsigned long long *__restrict__ a, int64_t n,
+                                                   unsigned long long key) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (a[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// The score of a key: the inverse of score_key (a zero score comes back as +0)
+__device__ __forceinline__ double key_score(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// Thread i < n_pos takes positive key i, thread n_pos + j negative key j.  For a positive at score s: fp = negatives with a
+// score >= s = n_neg - lower_bound(neg, key), tp = positives with a score >= s = n_pos - lower_bound(pos, key) (its own key
+// included, so tp >= 1), v = fl(tp / (tp + fp)) in [1/n, 1].  A key ends a tie group of the union when the next key of its
+// own run differs and, for a positive, no negative has its key (a group shared by both runs ends in the negatives).
+// The counts, U2 and the limbs are reduced over the warp in registers and added once per warp.
+__global__ void __launch_bounds__(256) k_curve_count(const unsigned long long *__restrict__ pos, int64_t n_pos,
+                                                     const unsigned long long *__restrict__ neg, int64_t n_neg,
+                                                     unsigned long long *__restrict__ u2,
+                                                     unsigned long long *__restrict__ cur) {
+  const unsigned full = 0xffffffffu;
+  unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0, pairs = 0, points = 0;
+  const int64_t total = n_pos + n_neg;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i < n_pos) {
+      const unsigned long long key = pos[i];
+      const int64_t lo = key_lower_bound(neg, n_neg, key);
+      int64_t up = lo, top = n_neg;   // upper_bound: first negative > key
+      while (up < top) {
+        const int64_t mid = (up + top) >> 1;
+        if (neg[mid] <= key) up = mid + 1; else top = mid;
+      }
+      pairs += (unsigned long long)(lo + up);
+      const int64_t tp = n_pos - key_lower_bound(pos, i, key), fp = n_neg - lo;
+      acc_add_local(lim, ovf, (double)tp / (double)(tp + fp));
+      points += (i + 1 == n_pos || pos[i + 1] != key) && up == lo;
+    } else {
+      const int64_t j = i - n_pos;
+      points += j + 1 == n_neg || neg[j + 1] != neg[j];
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    pairs += __shfl_xor_sync(full, pairs, o);
+    points += __shfl_xor_sync(full, points, o);
+    ovf += __shfl_xor_sync(full, ovf, o);
+#pragma unroll
+    for (int k = 0; k < kLossLimbs; ++k) lim[k] += __shfl_xor_sync(full, lim[k], o);   // each below 2^45: no carry lost
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (pairs) atomicAdd(u2, pairs);
+    if (points) atomicAdd(cur + kCurPoints, points);
+    acc_flush_local(cur + kCurAcc, lim, ovf);
+  }
+}
+
+// One thread: S (NaN if a value could not be summed, which no v_i in [2^-31, 1] is)
+__global__ void k_curve_sum(unsigned long long *__restrict__ cur) {
+  cur[kCurSum] = (unsigned long long)__double_as_longlong(acc_value(cur + kCurAcc));
+}
+
+// 1 when merged key i is the last of its tie group (the scan's input)
+struct tie_end {
+  const unsigned long long *keys;
+  int n;
+  __device__ __forceinline__ int operator()(int i) const { return i + 1 == n || keys[i] != keys[i + 1]; }
+};
+
+// The last key i of every tie group of the merged runs writes point m - 1 - excl[i] (excl: exclusive scan of tie_end, so
+// the highest score takes point 0): its score, and tp / fp = the keys at or above it in each run.
+__global__ void __launch_bounds__(256) k_curve_emit(const unsigned long long *__restrict__ merged, int64_t n_all,
+                                                    const int *__restrict__ excl,
+                                                    const unsigned long long *__restrict__ pos, int64_t n_pos,
+                                                    const unsigned long long *__restrict__ neg, int64_t n_neg,
+                                                    const unsigned long long *__restrict__ cur, double *__restrict__ thr,
+                                                    long long *__restrict__ tp, long long *__restrict__ fp) {
+  const int64_t m = (int64_t)cur[kCurPoints];
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = merged[i];
+    if (i + 1 < n_all && merged[i + 1] == key) continue;
+    const int64_t k = m - 1 - excl[i];
+    thr[k] = key_score(key);
+    tp[k] = n_pos - key_lower_bound(pos, n_pos, key);
+    fp[k] = n_neg - key_lower_bound(neg, n_neg, key);
+  }
 }
 
 }  // namespace dsgd

@@ -52,6 +52,16 @@ object DsgdNative {
   @native def evalSampledMetrics(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
                                  posEnd: Long, metrics: Array[Long]): Int
   @native def evalSamplesMetrics(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long]): Int
+  // ROC / precision-recall curves: metrics as above, ap(0) = average precision, nPoints(0) = m, and thr / tp / fp(0 until m)
+  // one point per distinct score, highest first.  thr, tp and fp are all null (average precision only) or each at least as
+  // long as the request's rows.
+  @native def evalCurve(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, metrics: Array[Long], ap: Array[Double],
+                        nPoints: Array[Long], thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
+  @native def evalSampledCurve(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                               posEnd: Long, metrics: Array[Long], ap: Array[Double], nPoints: Array[Long],
+                               thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
+  @native def evalSamplesCurve(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long], ap: Array[Double],
+                               nPoints: Array[Long], thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

@@ -251,6 +251,74 @@ FN(evalSamplesMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintA
   free(bw.p); free(bs.p);
   return rc;
 }
+/* curves and average precision: metrics(0..7) as above, ap(0) = average precision, nPoints(0) = m, and thr / tp / fp (0 until
+ * m) the points, highest score first -- all three null for average precision alone, else each at least as long as the
+ * request's rows (n = rowEnd - rowBegin, posEnd - posBegin or samples.length).  A shorter array is DSGD_ERR_INVALID. */
+typedef struct { buf_t m, a, k, t, tp, fp; } curve_bufs;
+static curve_bufs curve_out(JNIEnv *env, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr,
+                            jlongArray tp, jlongArray fp) {
+  curve_bufs c = {out_Long(env, metrics), out_Double(env, ap), out_Long(env, nPoints), out_Double(env, thr),
+                  out_Long(env, tp), out_Long(env, fp)};
+  return c;
+}
+static int curve_bad(const curve_bufs *c) { return c->m.bad | c->a.bad | c->k.bad | c->t.bad | c->tp.bad | c->fp.bad; }
+static int curve_short(const curve_bufs *c, jlong n) {
+  if (c->m.n < DSGD_METRICS_WORDS || c->a.n < 1 || c->k.n < 1) return 1;
+  return (c->t.p && c->t.n < n) || (c->tp.p && c->tp.n < n) || (c->fp.p && c->fp.n < n);
+}
+static void curve_back(JNIEnv *env, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp,
+                       jlongArray fp, curve_bufs *c, int rc) {
+  back_Long(env, metrics, c->m, rc);
+  back_Double(env, ap, c->a, rc);
+  back_Long(env, nPoints, c->k, rc);
+  back_Double(env, thr, c->t, rc);
+  back_Long(env, tp, c->tp, rc);
+  back_Long(env, fp, c->fp, rc);
+}
+FN(evalCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics,
+              jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp, jlongArray fp) {
+  buf_t bw = in_Double(env, w);
+  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | curve_bad(&c)))
+    rc = curve_short(&c, rowEnd - rowBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_curve(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.m.p, (double *)c.a.p, (int64_t *)c.k.p,
+                               (double *)c.t.p, (int64_t *)c.tp.p, (int64_t *)c.fp.p);
+  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                     jlong posBegin, jlong posEnd, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr,
+                     jlongArray tp, jlongArray fp) {
+  buf_t bw = in_Double(env, w);
+  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | curve_bad(&c)))
+    rc = curve_short(&c, posEnd - posBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_curve(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (int64_t *)c.m.p,
+                                       (double *)c.a.p, (int64_t *)c.k.p, (double *)c.t.p, (int64_t *)c.tp.p,
+                                       (int64_t *)c.fp.p);
+  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics,
+                     jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp, jlongArray fp) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | curve_bad(&c)))
+    rc = curve_short(&c, bs.n)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_curve(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.m.p, (double *)c.a.p, (int64_t *)c.k.p,
+                                       (double *)c.t.p, (int64_t *)c.tp.p, (int64_t *)c.fp.p);
+  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
 
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {

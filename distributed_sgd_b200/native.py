@@ -108,6 +108,9 @@ ABI = {
     "dsgd_eval_metrics": [_vp, _vp, _i64, _i64, _vp],
     "dsgd_eval_sampled_metrics": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp],
     "dsgd_eval_samples_metrics": [_vp, _vp, _vp, _i64, _vp],
+    "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -398,6 +401,38 @@ class NativeCtx:
         samples = _arr(samples, np.int32)
         return self._request("eval_samples_metrics", w, (_ptr(samples), samples.size),
                              np.zeros(METRICS_WORDS, dtype=np.int64))
+
+    def _curve(self, fn: str, w, rows: tuple, n: int, curve: bool):
+        """dsgd_<fn>: (words, ap, thr, tp, fp) with the m points of a curve pass over n rows, or (words, ap, m) when not
+        `curve` (the average-precision-only pass)."""
+        w = self._w(w)
+        words = np.zeros(METRICS_WORDS, dtype=np.int64)
+        ap, m = C.c_double(), C.c_int64()
+        thr = np.zeros(max(n, 0), dtype=np.float64) if curve else None
+        tp = np.zeros(max(n, 0), dtype=np.int64) if curve else None
+        fp = np.zeros(max(n, 0), dtype=np.int64) if curve else None
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(words), C.byref(ap), C.byref(m), _ptr(thr),
+                                                 _ptr(tp), _ptr(fp)))
+        if not curve:
+            return words, ap.value, m.value
+        k = m.value
+        return words, ap.value, thr[:k].copy(), tp[:k].copy(), fp[:k].copy()
+
+    def eval_curve(self, row_begin: int, row_end: int, w=None, curve: bool = True):
+        """ROC / precision-recall points and average precision over rows [row_begin, row_end) (dsgd_eval_curve): (words,
+        ap, thr, tp, fp), one point per distinct score, highest first; curve=False: (words, ap, number of points)."""
+        return self._curve("eval_curve", w, (row_begin, row_end), row_end - row_begin, curve)
+
+    def eval_sampled_curve(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None,
+                           curve: bool = True):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_curve)."""
+        return self._curve("eval_sampled_curve", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), pos_end - pos_begin,
+                           curve)
+
+    def eval_samples_curve(self, samples, w=None, curve: bool = True):
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_curve)."""
+        samples = _arr(samples, np.int32)
+        return self._curve("eval_samples_curve", w, (_ptr(samples), samples.size), samples.size, curve)
 
     # -- sync --
     def set_workers(self, counts, k_total: int = 0):

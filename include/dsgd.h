@@ -207,6 +207,28 @@ int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin,
                               int64_t pos_begin, int64_t pos_end, int64_t *out);
 int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out);
 
+/* ---- ROC and precision-recall curves and average precision over the same three row forms, with the conventions and errors
+ *      of the metrics calls above.  Over the non-NaN rows, let t_0 > t_1 > ... > t_(m-1) be the distinct scores s = -x.w
+ *      (+0 and -0 are one score).  Point k: thr_out[k] = t_k (a zero score as +0), tp_out[k] = positive rows with s >= t_k,
+ *      fp_out[k] = negative rows with s >= t_k; the last point counts every non-NaN positive and negative.  ROC is
+ *      (fp / N, tp / P), precision-recall is (tp / (tp + fp), tp / P).  *n_points_out = m <= n, the rows of the request.
+ *      words_out receives the DSGD_METRICS_WORDS words of the metrics call over the same rows, bit for bit.
+ *      *ap_out = average precision, the step-wise sum of (R_k - R_(k-1)) Prec_k: every non-NaN positive row i adds
+ *      v_i = tp_i / (tp_i + fp_i), one IEEE division of the counts at its own score; the v_i are added exactly in fixed point
+ *      (the result is within one ulp of the exact sum, and equal to it when that is a double), and AP = S / P.  AP is NaN when
+ *      a score is NaN or P = 0, and 1 when N = 0.  So AP has the same bits whatever the row order or the grid.
+ *      thr_out, tp_out and fp_out hold at least n entries each, or are all NULL: then only the words, AP and m are computed,
+ *      and nothing of size n is copied back.  Any other mix, or a NULL words_out, ap_out or n_points_out ->
+ *      DSGD_ERR_INVALID.  The list form takes at most 2^31 - 1 ids.  A pass grows its buffers (about 52 bytes per row and the
+ *      sort's, merge's and scan's storage) on first use, except on an async ctx, whose first loop start sizes them. */
+int dsgd_eval_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *words_out, double *ap_out,
+                    int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out);
+int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                            int64_t pos_begin, int64_t pos_end, int64_t *words_out, double *ap_out, int64_t *n_points_out,
+                            double *thr_out, int64_t *tp_out, int64_t *fp_out);
+int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
+                            double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out);
+
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
  *      (its own RPC), every rank calls dsgd_comm_init.  world == 1 needs neither. -------------------------- */
