@@ -156,14 +156,11 @@ __global__ void __launch_bounds__(128) k_async_worker(const AsyncParams p) {
         double wv[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) wv[u] = (cur.pre[u].y << 1) ? __ldcg(&w[cur.pre[u].x]) : 0.0;
-        double dot = 0.0;
+        double acc = 0.0;   // the row fold (dsgd_kernels.cuh): chunk 0 from the registers, the chunks past it from memory
 #pragma unroll
-        for (int u = 0; u < 4; ++u) dot += filt(filt((double)__uint_as_float(cur.pre[u].y)) * wv[u]);
-        for (int64_t k = cur.s0 + 128 + lane; k < cur.s1; k += 32) {   // rows longer than 128 pairs
-          const uint2 pr = p.pairs[k];
-          dot += filt(filt((double)__uint_as_float(pr.y)) * __ldcg(&w[pr.x]));
-        }
-        dot = warp_sum(dot);
+        for (int u = 0; u < 4; ++u) acc += filt(filt((double)__uint_as_float(cur.pre[u].y)) * wv[u]);
+        const double dot = row_fold_from(p.pairs, cur.s0 + kFoldPairs, cur.s1, lane, warp_sum(acc),
+                                         [&](uint32_t c) { return __ldcg(&w[c]); });
         if (!(cur.y * dot < 0.0)) {  // SparseSVM.scala:28
           // Vec.sum: left fold in batch order, filter after each +.  A column occurs once per row (dsgd_load_csr rejects
           // repeated keys), so the lane's four read-modify-writes are independent -- all four scratch entries are requested
@@ -248,6 +245,7 @@ __global__ void __launch_bounds__(128) k_async_worker(const AsyncParams p) {
 // out as fire-and-forget REDs (the reference's updateGrad futures are not awaited either, core/Slave.scala:104-105) and
 // are fenced once, when the loop ends; the stop flag is looked at every 32 iterations.
 constexpr int kAsyncPre = 4;   // pairs per lane held in registers for the next row
+static_assert(32 * kAsyncPre == kFoldPairs, "the registers hold chunk 0 of the row fold");
 struct AsyncRow {
   int64_t s0, s1;
   double y;
@@ -317,14 +315,11 @@ __global__ void __launch_bounds__(128) k_async_worker_b1(const AsyncParams p) {
     double wv[kAsyncPre];
 #pragma unroll
     for (int u = 0; u < kAsyncPre; ++u) wv[u] = (cur.pre[u].y << 1) ? __ldcg(&w[cur.pre[u].x]) : 0.0;
-    double dot = 0.0;
+    double acc = 0.0;   // the row fold (dsgd_kernels.cuh): chunk 0 from the registers, the chunks past it from memory
 #pragma unroll
-    for (int u = 0; u < kAsyncPre; ++u) dot += filt(filt((double)__uint_as_float(cur.pre[u].y)) * wv[u]);
-    for (int64_t k = cur.s0 + lane + 32 * kAsyncPre; k < cur.s1; k += 32) {     // rows longer than 128 pairs
-      const uint2 pr = __ldg(&p.pairs[k]);
-      dot += filt(filt((double)__uint_as_float(pr.y)) * __ldcg(&w[pr.x]));
-    }
-    dot = warp_sum(dot);
+    for (int u = 0; u < kAsyncPre; ++u) acc += filt(filt((double)__uint_as_float(cur.pre[u].y)) * wv[u]);
+    const double dot = row_fold_from(p.pairs, cur.s0 + kFoldPairs, cur.s1, lane, warp_sum(acc),
+                                     [&](uint32_t c) { return __ldcg(&w[c]); });
 
     // ---- delta = lr * regularize(y * x / 1, w); apply to every replica (core/Slave.scala:92-105) ----
     double sd = 0.0;

@@ -79,6 +79,40 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// The row fold: the one fp64 summation order of x . w for a row window on the device, so that a row's margin, prediction
+// and gate are a function of the row and w alone, whichever kernel takes the row and whatever else is in the request.
+//   * The window of L pairs (padding included) is cut into kFoldPairs-pair chunks from its start.
+//   * In chunk c, lane l sums filt(filt(x) * w) over the pairs 128 c + l + 32 u, u = 0 .. 3 in order, from +0.0.
+//   * The xor butterfly 16, 8, 4, 2, 1 reduces the lanes to the chunk partial.
+//   * The dot is 0.0 + part_0 + part_1 + ..., in chunk order.  No partial is -0 (every lane sum starts at +0.0 and filt
+//     never returns -0), so a one-chunk window's dot is its partial.
+// The listed chunks of the persistent sync step (consume_stage, dsgd_persistent.cuh) are this fold with the chunks spread
+// over warps.  row_fold_from continues a fold whose chunks before pair c have been added to dot already (the async workers
+// hold chunk 0 in registers); wt(col) is the weight of column col.  Called by the whole warp; every lane gets the dot.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kFoldPairs = 128;
+template <class Wt>
+__device__ __forceinline__ double row_fold_from(const uint2 *__restrict__ pairs, int64_t c, int64_t e, int lane, double dot,
+                                                Wt &&wt) {
+  const uint2 *__restrict__ src = pairs + c;
+  const int len = (int)(e - c);   // a row window is far below 2^31 pairs
+  for (int c0 = 0; c0 < len; c0 += kFoldPairs) {
+    const int ce = min(c0 + kFoldPairs, len);
+    double acc = 0.0;
+    for (int k = c0 + lane; k < ce; k += 32) {
+      const uint2 pr = __ldg(&src[k]);
+      acc += filt(filt((double)__uint_as_float(pr.y)) * wt(pr.x));  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
+    }
+    dot += warp_sum(acc);
+  }
+  return dot;
+}
+template <class Wt>
+__device__ __forceinline__ double row_fold(const uint2 *__restrict__ pairs, int64_t b, int64_t e, int lane, Wt &&wt) {
+  return row_fold_from(pairs, b, e, lane, 0.0, wt);
+}
+
 // Block-wide sum in a fixed order (deterministic run to run). Result valid in thread 0.
 template <int kThreads>
 __device__ __forceinline__ double block_sum(double v, double *smem /* kThreads/32 */) {
@@ -142,15 +176,9 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
   for (int64_t i = warp0; i < n; i += nwarps) {
     const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
     const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    double dot = 0.0;
-    for (int64_t k = b + lane; k < e; k += 32) {
-      const uint2 pr = pairs[k];
-      const double xv = filt((double)__uint_as_float(pr.y));
-      dot += filt(xv * w[pr.x]);  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
-    }
-    dot = warp_sum(dot);
+    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
     const double y = (double)label[r];
-    const int p = (dot > 0.0) ? -1 : ((dot < 0.0) ? 1 : 0);  // -signum(dot)
+    const int p =(dot > 0.0) ? -1 : ((dot < 0.0) ? 1 : 0);  // -signum(dot)
     if (lane == 0) {
       const int l = 1 - (int)y * p;  // max(0, 1 - y*p), never negative for y,p in {-1,0,1}
       hinge += (unsigned)l;
@@ -205,13 +233,7 @@ __global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restric
   for (int64_t i = warp0; i < n; i += nwarps) {
     const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
     const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    double dot = 0.0;
-    for (int64_t k = b + lane; k < e; k += 32) {
-      const uint2 pr = pairs[k];
-      const double xv = filt((double)__uint_as_float(pr.y));
-      dot += filt(xv * w[pr.x]);  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
-    }
-    dot = warp_sum(dot);
+    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
     const double y = (double)label[r];
     const double z = y * dot;
     if (lane == 0) {

@@ -26,19 +26,13 @@ enum MetricWord : int {
   kMetWords = 16
 };
 
-// x . w of row r for one warp, every lane gets it: the fold of k_rows_logistic (lane-strided partial sums of the filtered
-// products, then the xor butterfly).  dsgd_margins and the metrics pass both call this, so a metrics pass ranks exactly the
-// values dsgd_margins returns for the same rows.
+// x . w of row r for one warp, every lane gets it: the row fold (dsgd_kernels.cuh) that decides the row on every other
+// path.  dsgd_margins and the metrics pass both call this, so a metrics pass ranks exactly the values dsgd_margins returns
+// for the same rows, and its confusion counts are the predictions of every dsgd_eval_* call.
 __device__ __forceinline__ double row_margin(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                              const double *__restrict__ w, int64_t r, int lane) {
   const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-  double dot = 0.0;
-  for (int64_t k = b + lane; k < e; k += 32) {
-    const uint2 pr = pairs[k];
-    const double xv = filt((double)__uint_as_float(pr.y));
-    dot += filt(xv * w[pr.x]);  // (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46)
-  }
-  return warp_sum(dot);
+  return row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
 }
 
 // Order-preserving key of a score: +0 and -0 are one key, and key(a) < key(b) exactly when a < b (for non-NaN scores)

@@ -230,6 +230,7 @@ __device__ __forceinline__ bool grid_barrier_arrive_wait(unsigned *bar, unsigned
 }
 
 constexpr int kChunkPairs = 128;             // 4 pairs per lane per chunk
+static_assert(kChunkPairs == kFoldPairs, "a listed row's chunks are the chunks of the row fold");
 constexpr uint32_t kChunkGlobal = 1u << 31;  // chunk offset flag: read from global, the row did not fit the stage
 constexpr int kMaxRowsPerCta = 32;           // rows of one step per CTA (one producer lane each)
 
@@ -449,12 +450,8 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
     } else if (nch < 0) {
       const uint2 *grow = pairs + (size_t)mt.row_b[m] * 2;
       const int len = mt.row_len[m];
-      double acc = 0.0;
-      for (int k = lane; k < len; k += 32) {
-        const uint2 pr = __ldg(&grow[k]);
-        acc += filt(filt((double)__uint_as_float(pr.y)) * fetch.get1(pr.x));
-      }
-      const double dot = warp_sum(acc);
+      // the row fold (dsgd_kernels.cuh): the dot pass 2 gives the same row when it is listed
+      const double dot = row_fold(grow, 0, len, lane, [&](uint32_t c) { return fetch.get1(c); });
       const int yi = mt.row_y[m];
       const double y = (double)yi;
       if (lane == 0) hinge += (unsigned)(1 - yi * pred_of(dot));

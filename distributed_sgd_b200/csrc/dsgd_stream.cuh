@@ -28,9 +28,11 @@
 //     up, stored with the label in its sign bit: one 4-byte load per row).  The reference also drops every value and
 //     every product with magnitude <= 1e-20 (the Sparse constructor, filt): k_repack stores such values as 0, and the
 //     products the fp32 dot keeps are bounded by 1e-20 per pair, so the band gets 2 * 1e-20 per unit on top.  Rows
-//     whose |dot| is inside that band are recomputed with the fp64 weights from L2 after the block's stream, so every
-//     prediction and gate decision is that of the filtered fp64 arithmetic (tests/test_gpu_streaming.py;
-//     dsgd_stream_exact_rows counts the recomputed rows).
+//     whose |dot| is inside that band are recomputed after the block's stream with the fp64 weights from L2, by the row fold
+//     (dsgd_kernels.cuh) that decides the row on every other path (tests/test_gpu_streaming.py, test_gpu_row_fold.py;
+//     dsgd_stream_exact_rows counts the recomputed rows).  Outside the band the fp32 sign is the row fold's sign: there
+//     |exact x.w| >= band / 3, far above the difference between any two fp64 summation orders, so every prediction and
+//     gate decision of the pass is that of the row fold.
 //   * Scatter (gradient): rows that pass the gate are re-walked after the block's stream (their units are in
 //     L1/L2) and y*x goes to g with fp64 REDs.  On trained weights few rows pass (the misclassified ones) and the pass
 //     runs at the streaming rate; on untrained weights every row passes and the fp64 RED rate at L2 bounds it
@@ -278,13 +280,9 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
       ex &= ex - 1u;
       const uint32_t rb = __shfl_sync(0xffffffffu, b, r);
       const int rl = __shfl_sync(0xffffffffu, len, r);
-      double acc = 0.0;
-      for (int u = lane; u < rl; u += 32) {
-        const uint4 qq = __ldg(&p.units[rb + (uint32_t)u]);
-        acc += filt(filt((double)__uint_as_float(qq.y)) * __ldcg(&p.w[qq.x]));
-        acc += filt(filt((double)__uint_as_float(qq.w)) * __ldcg(&p.w[qq.z]));
-      }
-      const double dot = warp_sum(acc);
+      const int64_t pb = 2 * (int64_t)rb;   // the window in pairs
+      const double dot = row_fold(reinterpret_cast<const uint2 *>(p.units), pb, pb + 2 * (int64_t)rl, lane,
+                                  [&](uint32_t c) { return __ldcg(&p.w[c]); });
       if (lane == r) {
         finalize(pred_of(dot));
         ++n_exact;

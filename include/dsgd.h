@@ -22,6 +22,13 @@
  *    dsgd_load_csr received (the reference addresses a slave by global row id, core/Slave.scala:149).
  *  - Arithmetic: values fp32 (exactly promoted), every accumulation and all state in fp64, like the
  *    reference's spire.math.Number over Double.
+ *  - Every fp64 row dot x . w on the device is the row fold: the row window cut into 128-pair chunks from its start, in
+ *    chunk c lane l sums the filtered products of pairs 128 c + l + 32 u (u = 0..3, in order, from +0.0), an xor
+ *    butterfly per chunk, then 0.0 + the chunk partials in order.  Every request, evaluation, metrics, sync and async
+ *    path uses it (the fp32 streaming pass decides only rows whose sign the fold cannot change), so a row's margin,
+ *    prediction and gate depend on the row and w alone: not on the request size, the grid or the other rows of a step.
+ *    The reference sums in HashMap order; the oracle's index-order fold can differ in the last bits, and in sign where
+ *    the products cancel to within fp64 rounding.
  *  - Threading: calls on one ctx are serialised by the caller, except dsgd_update_grad,
  *    dsgd_get_weights, dsgd_async_updates and dsgd_stop_async, which are safe while the async loop runs
  *    (the reference serves them from its 8-thread pool concurrently with asyncTask, core/Slave.scala:24-30).
@@ -182,8 +189,8 @@ int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *sample
  *      weights (on an async ctx, a snapshot taken when the call starts); the ids go to a buffer of their own, so a staged
  *      sample stream is left intact; no rows loaded -> DSGD_ERR_STATE; an id or a range outside the loaded rows ->
  *      DSGD_ERR_RANGE, before anything is launched; n == 0 (an empty range, no positions) -> DSGD_ERR_EMPTY; a NULL output
- *      -> DSGD_ERR_INVALID.  The dot product x_i . w is the fp64 fold of the logistic passes (not the fp32 streaming pass,
- *      which only decides a sign), and the metrics rank exactly the values dsgd_margins returns for the same rows. ---- */
+ *      -> DSGD_ERR_INVALID.  The dot product x_i . w is the row fold (Conventions), the one that decides the row on every
+ *      other path, and the metrics rank exactly the values dsgd_margins returns for the same rows. ---- */
 /* margins_out[i] = x_i . w in fp64 (the value whose -signum dsgd_forward reports) */
 int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *margins_out);
 /* SparseLogistic only: probs_out[i] = P(y = +1 | x_i) = sigmoid(-x_i . w), with the sigmoid of the logistic gradient; an SVM ctx
