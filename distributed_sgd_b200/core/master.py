@@ -196,7 +196,17 @@ class Master:
             sums = [s + float(v) for s, v in zip(sums, p[:-1])]
         return (*sums, max(float(p[-1]) for p in parts))
 
-    def _eval_rows(self, weights, begin: int, end: int):
+    def _penalty(self, n2: float, weights, want_loss: bool) -> float:
+        """lambda * ||w||^2, plus l1 * ||w||_1 of the same weights (weights None: the resident ones) when the model has an L1
+        penalty.  ||w||_1 is an order-free device sum: the same bits on every rank.  want_loss False (an accuracy query): the
+        loss is not used, so no device pass is made for ||w||_1."""
+        if not self.model.l1:
+            return self.model.lam * n2
+        if not want_loss:
+            return float("nan")
+        return self.model.lam * n2 + self.model.l1 * self.ctx.weights_l1(weights)[0]
+
+    def _eval_rows(self, weights, begin: int, end: int, want_loss: bool = True):
         """Row-sharded pass: each rank evaluates a contiguous share, the loss sums and counters are summed."""
         W, r = self.group.world, self.group.rank
         n = end - begin
@@ -206,7 +216,7 @@ class Master:
         else:
             h, c, n2 = 0, 0, 0.0
         hs, cs, n2 = self._combine(h, c, n2)
-        return self.model.lam * n2 + hs / n, cs / n
+        return self._penalty(n2, weights, want_loss) + hs / n, cs / n
 
     def local_loss(self, weights=None, test_data: bool = False) -> float:
         """Master.localLoss (core/Master.scala:105-107)."""
@@ -216,7 +226,7 @@ class Master:
     def local_accuracy(self, weights=None, test_data: bool = False) -> float:
         """Master.localAccuracy (core/Master.scala:100-103)."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._eval_rows(weights, b, e)[1]
+        return self._eval_rows(weights, b, e, want_loss=False)[1]
 
     def local_loss_accuracy(self, weights=None, test_data: bool = False):
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
@@ -239,7 +249,7 @@ class Master:
             self._sampled_draws += 1
         return b, e, k, key, ids
 
-    def _eval_sample(self, weights, samples_count: int, test_data: bool):
+    def _eval_sample(self, weights, samples_count: int, test_data: bool, want_loss: bool = True):
         """(loss, accuracy) on a fresh sample (_draw_sample), or None when that is empty.  Rank r of W evaluates positions
         sample_shard(k, W, r); the loss sums and counters are summed over ranks."""
         b, e, k, key, ids = self._draw_sample(samples_count, test_data)
@@ -253,7 +263,7 @@ class Master:
         else:
             h, c, n2 = self._local_eval("eval_samples", ids[lo:hi], weights)
         hs, cs, n2 = self._combine(h, c, n2)
-        return self.model.lam * n2 + hs / k, cs / k
+        return self._penalty(n2, weights, want_loss) + hs / k, cs / k
 
     def local_sampled_loss(self, weights, samples_count: int, test_data: bool = False) -> float:
         """Master.localSampledLoss (core/Master.scala:109-112).  An empty sample raises DsgdEmpty, as the reference's
@@ -262,7 +272,7 @@ class Master:
 
     def local_sampled_accuracy(self, weights, samples_count: int, test_data: bool = False) -> float:
         """Master.localSampledAccuracy (core/Master.scala:114-118).  An empty sample gives nan (the reference's 0.0 / 0)."""
-        r = self._eval_sample(weights, samples_count, test_data)
+        r = self._eval_sample(weights, samples_count, test_data, want_loss=False)
         return float("nan") if r is None else r[1]
 
     def local_sampled_loss_accuracy(self, weights, samples_count: int, test_data: bool = False):
@@ -325,13 +335,13 @@ class Master:
 
     def distributed_accuracy(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> float:
         """Master.distributedAccuracy (core/Master.scala:77-85)."""
-        return self._distributed(weights, split_strategy)[1]
+        return self._distributed(weights, split_strategy, want_loss=False)[1]
 
     def distributed_loss(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> float:
         """Master.distributedLoss (core/Master.scala:87-98)."""
         return self._distributed(weights, split_strategy)[0]
 
-    def _distributed(self, weights, split_strategy: Split):
+    def _distributed(self, weights, split_strategy: Split, want_loss: bool = True):
         # same numbers as predict + host-side counting, without shipping N predictions around
         groups = split_strategy(self.n_train, self.group.world)
         mine = groups[self.group.rank] if self.group.rank < len(groups) else range(0)
@@ -340,7 +350,7 @@ class Master:
         else:
             h, c, n2 = 0, 0, 0.0
         hs, cs, ns, n2 = self._combine(h, c, n2, len(mine))
-        return self.model.lam * n2 + hs / ns, cs / ns
+        return self._penalty(n2, weights, want_loss) + hs / ns, cs / ns
 
 
 class MasterSync(Master):
@@ -383,6 +393,8 @@ class MasterSync(Master):
         learning_rate / (1 + decay * t)^power (ml/lr_schedule.py), handed to the device as a per-step table
         (ctx.sync_steps_lr).  decay = 0: the constant learning_rate of the reference, through the scalar calls of before.
         Together with average_from this is Bottou's averaged SGD (power 0.75 in svmasgd).
+        A model with l1 > 0 (the Slave set it on the device) soft-thresholds every weight in every step; the losses then
+        include l1 * ||w||_1 and history["nnz"] holds the non-zero weights of each epoch's evaluated weights.
         """
         if average_from is not None and not 0 <= average_from < max_epochs:
             raise ValueError(f"average_from must lie in [0, max_epochs = {max_epochs}), got {average_from}")
@@ -400,6 +412,7 @@ class MasterSync(Master):
         accs: List[float] = []
         test_losses: List[float] = []
         test_accs: List[float] = []
+        nnz: List[int] = []
         self.step_losses: List[np.ndarray] = []
         epoch = 0
         # a one-thread pool overlaps the next epoch's draw with the current epoch's kernel (not with jvm_exact: that
@@ -420,6 +433,8 @@ class MasterSync(Master):
                                     "test_accs": test_accs[::-1]}
                     if average_from is not None:
                         self.history["averaged_steps"] = n_averaged
+                    if self.model.l1:
+                        self.history["nnz"] = nnz[::-1]
                     if prefetch is not None:
                         prefetch.shutdown(wait=True)
                     # `losses.head` throws on an empty list in the reference (max_epochs == 0)
@@ -470,6 +485,8 @@ class MasterSync(Master):
                 tl, ta = self.local_loss_accuracy(w, test_data=False)        # Master.scala:206-207
                 vl, va = self.local_loss_accuracy(w, test_data=True)         # Master.scala:208-209
                 losses.insert(0, tl); accs.insert(0, ta); test_losses.insert(0, vl); test_accs.insert(0, va)
+                if self.model.l1:
+                    nnz.insert(0, self.ctx.weights_l1(w)[1])
                 epoch += 1
                 state = state.replace_grad(self.ctx.get_weights() if w is None else w)   # Master.scala:205
                 if on_epoch:
@@ -488,6 +505,8 @@ class MasterAsync(Master):
     def __init__(self, node, data, test_data, model, expected_node_count, **kw):
         if isinstance(model, SparseLogistic):
             raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
+        if model.l1:
+            raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
         super().__init__(node, data, test_data, model, expected_node_count, **kw)
 
     def _attach_replicas(self):

@@ -33,6 +33,8 @@ class Slave:
         logistic = isinstance(model, SparseLogistic)
         if logistic and is_async:
             raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
+        if model.l1 and is_async:
+            raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
         self.node, self.master, self.model, self.is_async, self.world = node, master, model, is_async, world
         self.n_train = data.n_rows
         self.n_test = test_data.n_rows if test_data is not None else 0
@@ -45,6 +47,8 @@ class Slave:
             self.ctx = ctx
             if model.dim_sparsity is None:
                 model.dim_sparsity = ctx.compute_dim_sparsity(self.n_train)
+            if model.l1:
+                ctx.set_l1(model.l1)
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
                              is_async=is_async, logistic=logistic)
@@ -60,6 +64,8 @@ class Slave:
             model.dim_sparsity = self.ctx.compute_dim_sparsity(self.n_train)  # Main.scala:54-65 on the device
         else:
             self.ctx.set_dim_sparsity(model.dim_sparsity)
+        if model.l1:
+            self.ctx.set_l1(model.l1)
 
     def stop(self):  # Slave.stop (core/Slave.scala:68-77): releases the device context
         self.ctx.close()

@@ -103,6 +103,7 @@ struct dsgd_ctx {
   int device = 0;
   int32_t dim = 0;
   double lambda = 0.0;
+  double lambda1 = 0.0;   // dsgd_set_l1: the L1 penalty of the sync steps (0: off)
   int rank = 0, world = 1;
   uint32_t flags = 0;
   int sm_count = 0;
@@ -395,9 +396,9 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   snprintf(buf, sizeof buf,
            "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
-           "\"model\": \"%s\"}",
+           "\"model\": \"%s\", \"lambda1\": %.17g}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
-           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm");
+           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1);
   ctx->info = buf;
   return ctx->info.c_str();
 }
@@ -538,9 +539,18 @@ static void launch_prepare(dsgd_ctx *ctx, const double *w, float *w32, int c_slo
   LAUNCHED();
 }
 
-// recompute c and ||w||^2 of the resident weights, refresh the fp32 shadow
+// ||w||_1 of the resident weights into scal[kScalL1], which the per-step L1 update reads for the loss of its step
+static void launch_l1_refresh(dsgd_ctx *ctx) {
+  k_l1_norm<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(ctx->w, ctx->dim, ctx->cnt);
+  LAUNCHED();
+  k_l1_finish<<<1, 1, 0, ctx->stream>>>(ctx->cnt, ctx->scal + kScalL1, nullptr);
+  LAUNCHED();
+}
+
+// recompute c and ||w||^2 (and, with an L1 penalty, ||w||_1) of the resident weights, refresh the fp32 shadow
 static int refresh_resident(dsgd_ctx *ctx) {
   launch_prepare(ctx, ctx->w, ctx->w32, kScalC, kScalNrm2);
+  if (ctx->lambda1 > 0.0) launch_l1_refresh(ctx);
   if (ctx->flags & DSGD_FLAG_ASYNC) {
     k_async_init_ctl<1024><<<1, 1024, 0, ctx->stream>>>(ctx->w, ctx->d, ctx->dim);
     LAUNCHED();
@@ -1243,6 +1253,12 @@ static void *const kPersistKernels[2][2][2] = {
      {(void *)DSGD_PERSIST_KERNEL(false, true, false), (void *)DSGD_PERSIST_KERNEL(false, true, true)}},
     {{(void *)DSGD_PERSIST_KERNEL(true, false, false), (void *)DSGD_PERSIST_KERNEL(true, false, true)},
      {(void *)DSGD_PERSIST_KERNEL(true, true, false), (void *)DSGD_PERSIST_KERNEL(true, true, true)}}};
+// the one-GPU L1 forms (dsgd_set_l1), indexed [avg][lr_table]
+#define DSGD_PERSIST_KERNEL_L1(avg, lr_table) \
+  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, false, avg, lr_table, true>
+static void *const kPersistKernelsL1[2][2] = {
+    {(void *)DSGD_PERSIST_KERNEL_L1(false, false), (void *)DSGD_PERSIST_KERNEL_L1(false, true)},
+    {(void *)DSGD_PERSIST_KERNEL_L1(true, false), (void *)DSGD_PERSIST_KERNEL_L1(true, true)}};
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -1262,6 +1278,9 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
       for (int a = 0; a < 2; ++a)
         for (int l = 0; l < 2; ++l)
           CU(cudaFuncSetAttribute(kPersistKernels[m][a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    for (int a = 0; a < 2; ++a)
+      for (int l = 0; l < 2; ++l)
+        CU(cudaFuncSetAttribute(kPersistKernelsL1[a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
   return ctx->p_hinge.grow(ctx, n_steps, 4096);
@@ -1382,7 +1401,11 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.lr = 0.0;   // not read: interval 0, the only one before lrs[0] is loaded, applies no update
   }
   void *args[] = {&pp};
-  void *fn = kPersistKernels[multi ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
+  // the L1 forms only with a penalty (never fused: sync_staged keeps an L1 ctx off the fused path)
+  const bool l1 = !multi && ctx->lambda1 > 0.0;
+  pp.lambda1 = l1 ? ctx->lambda1 : 0.0;
+  void *fn = l1 ? kPersistKernelsL1[ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0]
+                : kPersistKernels[multi ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
   CU(launch_err);
@@ -1544,9 +1567,19 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
   double lr_s = lr;   // the rate of step s
-  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights
-  auto update = [&](auto kernel, auto kernel_avg, double *gbuf, double k_den, double n_local, double *loss_dev) {
-    if (ctx->avg_on)
+  const bool l1 = ctx->lambda1 > 0.0;
+  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights; with an L1 penalty their _l1
+  // forms, which soft-threshold every column after the update
+  auto update = [&](auto kernel, auto kernel_avg, auto kernel_l1, auto kernel_avg_l1, double *gbuf, double k_den,
+                    double n_local, double *loss_dev) {
+    if (l1 && ctx->avg_on)
+      kernel_avg_l1<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
+                                                         ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg,
+                                                         ctx->lambda1);
+    else if (l1)
+      kernel_l1<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
+                                                     ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->lambda1);
+    else if (ctx->avg_on)
       kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
                                                       ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
     else
@@ -1555,13 +1588,15 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     LAUNCHED();
     if (ctx->avg_on) ++ctx->avg_n;
   };
+
   for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
     if (lrs) lr_s = lrs[s];
     double *loss_dev = losses ? losses + s : nullptr;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
       profiled(ctx, [&] { launch_rows<kModel, true>(ctx, {smp, 0, n_per_step}, ctx->w, ctx->g); });
-      update(k_update<true, kModel>, k_update_avg<true, kModel>, ctx->g, 1.0, (double)n_per_step, loss_dev);
+      update(k_update<true, kModel>, k_update_avg<true, kModel>, k_update_l1<true, kModel>, k_update_avg_l1<true, kModel>,
+             ctx->g, 1.0, (double)n_per_step, loss_dev);
       continue;
     }
     // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
@@ -1581,7 +1616,8 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
     if (ctx->world > 1)
       NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    update(k_update<false, kModel>, k_update_avg<false, kModel>, ctx->gsum, (double)k_total, 0.0, loss_dev);
+    update(k_update<false, kModel>, k_update_avg<false, kModel>, k_update_l1<false, kModel>, k_update_avg_l1<false, kModel>,
+           ctx->gsum, (double)k_total, 0.0, loss_dev);
   }
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -1613,11 +1649,15 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   }
   const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
-  // the persistent and fused kernels are SVM-only: a logistic ctx always takes the per-step path below
+  // the persistent and fused kernels are SVM-only: a logistic ctx always takes the per-step path below.  The fused kernel has
+  // no L1 form: a ctx with an L1 penalty takes the one-GPU persistent kernel's L1 form or the per-step path.
   const bool logistic = is_logistic(ctx);
+  const bool l1 = ctx->lambda1 > 0.0;
   NEED(!logistic || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
        "dsgd_sync_steps: the logistic model takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
-  const bool fused = !logistic && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
+  NEED(!l1 || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
+       "dsgd_sync_steps: the L1 penalty takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
+  const bool fused = !logistic && !l1 && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
                      persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step));
   // Ranks wired with the peer exchange only have no communicator for the step-by-step path below: refuse before anything
   // is launched instead of reaching the allreduce without one.
@@ -1688,6 +1728,57 @@ extern "C" int dsgd_sync_steps_lr(dsgd_ctx *ctx, const int32_t *samples, int64_t
 
 extern "C" int dsgd_sync_step(dsgd_ctx *ctx, const int32_t *samples, int64_t n, double lr, double *loss_out) {
   return dsgd_sync_steps(ctx, samples, n, 1, lr, loss_out);
+}
+
+// ---- the L1 penalty of the sync steps (dsgd_set_l1) and the L1 norm of a weight vector ----------------------------------
+
+extern "C" int dsgd_set_l1(dsgd_ctx *ctx, double lambda1) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE,
+       "dsgd_set_l1: ctx is in async mode (the L1 penalty is a step of the sync paths; Hogwild has no step order)");
+  NEED(std::isfinite(lambda1) && lambda1 >= 0.0, DSGD_ERR_INVALID, "dsgd_set_l1: lambda1 must be finite and >= 0 (got %g)",
+       lambda1);
+  // scal[kScalL1] is kept only while the penalty is on: every step of an L1 ctx and dsgd_set_weights keep it from here on
+  if (lambda1 > 0.0 && !(ctx->lambda1 > 0.0)) {
+    CU(cudaSetDevice(ctx->device));
+    launch_l1_refresh(ctx);
+    CU(cudaGetLastError());
+  }
+  ctx->lambda1 = lambda1;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_dim(const dsgd_ctx *ctx, int32_t *dim_out) {
+  if (!ctx || !dim_out) return DSGD_ERR_INVALID;
+  *dim_out = ctx->dim;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_weights_l1(dsgd_ctx *ctx, const double *w, double *l1_out, int64_t *nnz_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE,
+       "dsgd_weights_l1: ctx is in async mode (the L1 penalty is a step of the sync paths; Hogwild has no step order)");
+  CU(cudaSetDevice(ctx->device));
+  const double *src = ctx->w;
+  if (w) {
+    CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
+    src = ctx->w_req;
+  }
+  // out2[5] = ||w||_1, out2[6] = the count as an int64
+  long long *nnz_dev = reinterpret_cast<long long *>(ctx->out2.p + 6);
+  k_l1_norm<<<cdiv(ctx->dim, 256), 256, 0, ctx->stream>>>(src, ctx->dim, ctx->cnt);
+  LAUNCHED();
+  k_l1_finish<<<1, 1, 0, ctx->stream>>>(ctx->cnt, ctx->out2 + 5, nnz_dev);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  double l1 = 0.0;
+  long long nnz = 0;
+  CU(cudaMemcpyAsync(&l1, ctx->out2 + 5, sizeof l1, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(&nnz, nnz_dev, sizeof nnz, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (l1_out) *l1_out = l1;
+  if (nnz_out) *nnz_out = nnz;
+  return DSGD_OK;
 }
 
 // ---- averaged SGD: the sync step kernels add the new weights of every step to ctx->avg while ctx->avg_on ----------------

@@ -82,6 +82,19 @@ __device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane
     sn = sd;
   }
 }
+// The persistent kernel's L1 form (kL1) keeps a third value in words kAccWords .. kAccWords + 4 of the same accumulator line,
+// its overflows counted in word 2 * kAccLimbs with the other two.  Called by a whole warp; all lanes return the sum.
+__device__ __forceinline__ double acc_read_l1(const unsigned long long *acc, int lane) {
+  unsigned long long q = 0;
+  if (lane < kAccLimbs) asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(q) : "l"(acc + kAccWords + lane) : "memory");
+  const double v = acc_limb(q, lane);
+  const double v0 = __shfl_sync(0xffffffffu, v, 0), v1 = __shfl_sync(0xffffffffu, v, 1), v2 = __shfl_sync(0xffffffffu, v, 2);
+  const double v3 = __shfl_sync(0xffffffffu, v, 3), v4 = __shfl_sync(0xffffffffu, v, 4);
+  const double a = (((v4 + v3) + v2) + v1) + v0;   // from the top limb down
+  unsigned long long o = 0;
+  if (lane == 0) asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(o) : "l"(acc + 2 * kAccLimbs) : "memory");
+  return __shfl_sync(0xffffffffu, o, 0) != 0ull ? __longlong_as_double(0x7ff8000000000000ll) : a;
+}
 
 // ---- one sum of many non-negative values (the logistic losses of a pass) -------------------------------------------------
 // Each value v in [0, 2^52) contributes R(v) = rint(v * 2^160) * 2^-160 (acc_cut's limbs, resolution 2^-160: a value below

@@ -26,6 +26,8 @@ enum Scal : int {
   kScalNrm2 = 1,   // ||w||^2 of the current resident weights (SparseSVM.scala:21)
   kScalReqC = 2,   // same two for a request-supplied weight vector (GradientRequest.weights)
   kScalReqNrm2 = 3,
+  kScalL1 = 4,     // ||w||_1 of the current resident weights: refreshed by every sync call of an L1 ctx (k_l1_norm), then
+                   // kept by its update kernels (k_update_l1)
   kNumScal = 8
 };
 // Slots of the per-ctx counter block (unsigned long long[kNumCnt]).
@@ -34,9 +36,12 @@ enum Cnt : int {
   kCntCorrect = 1,  // #{pred == y}
   kCntTicket = 2,   // last-block ticket of k_update
   kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
-  kNumCnt = 16
+  kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update_l1, k_l1_norm; zero between launches
+  kCntNnz = 23,     // #{w_j != 0} of k_l1_norm; zero between launches
+  kNumCnt = 24
 };
-static_assert(kCntLoss + kLossAccWords <= kNumCnt, "counter block");
+static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kCntNnz && kCntNnz < kNumCnt,
+              "counter block");
 
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
 constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
@@ -56,6 +61,59 @@ __device__ __forceinline__ void clear_batch_loss(unsigned long long *cnt) {
 }
 
 __device__ __forceinline__ double filt(double v) { return fabs(v) > kEps ? v : 0.0; }  // Sparse.scala:108-118
+
+// The proximal step of the L1 penalty at threshold tau = lr * lambda1: u shrunk towards 0 by tau, 0 where |u| <= tau, with the
+// 1e-20 filter of a new Sparse.  tau == 0 (lambda1 == 0, or a zero rate) returns u itself: the step without the penalty.
+__device__ __forceinline__ double soft_threshold(double u, double tau) {
+  if (!(tau > 0.0)) return u;
+  return u > tau ? filt(u - tau) : (u < -tau ? filt(u + tau) : 0.0);
+}
+
+// Adds R(a) of every thread of the block (a in [0, 2^52), dsgd_fixed.cuh) to the kLossAccWords accumulator acc: the limbs are
+// summed in registers, over the warp and over the block, carried once and pushed by thread 0 with one RED per non-zero word,
+// then fenced, so that a ticket thread 0 takes afterwards orders them.  Called by all kThreads threads.
+template <int kThreads>
+__device__ __forceinline__ void acc_push_block(double a, unsigned long long *__restrict__ acc) {
+  __shared__ unsigned long long sh[kThreads / 32][kLossAccWords];
+  unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
+  acc_add_local(lim, ovf, a);   // limbs 0..4 below 2^40, limb 5 below 2^13: a block's sums stay below 2^48
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int i = 0; i < kLossLimbs; ++i) lim[i] += __shfl_xor_sync(0xffffffffu, lim[i], o);
+    ovf += __shfl_xor_sync(0xffffffffu, ovf, o);
+  }
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) {
+#pragma unroll
+    for (int i = 0; i < kLossLimbs; ++i) sh[wid][i] = lim[i];
+    sh[wid][kLossLimbs] = ovf;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int i = 0; i < kLossLimbs; ++i) lim[i] = 0;
+    ovf = 0;
+    for (int w = 0; w < kThreads / 32; ++w) {
+#pragma unroll
+      for (int i = 0; i < kLossLimbs; ++i) lim[i] += sh[w][i];
+      ovf += sh[w][kLossLimbs];
+    }
+    acc_carry(lim);   // limbs 0..4 below 2^40 again: the words of 2^24 blocks cannot wrap
+    acc_flush_local(acc, lim, ovf);
+    __threadfence();
+  }
+}
+// One thread, after every push has landed: the value of the accumulator, which is left zeroed
+__device__ __forceinline__ double acc_take(unsigned long long *acc) {
+  unsigned long long q[kLossAccWords];
+#pragma unroll
+  for (int i = 0; i < kLossAccWords; ++i) {
+    q[i] = __ldcg(acc + i);
+    acc[i] = 0ull;
+  }
+  return acc_value(q);
+}
 
 // Gradient scatter: a reduction WITHOUT a return value.  Written as PTX `red` because nvcc 12.9 compiles atomicAdd(double *)
 // with an unused result to ATOMG (result discarded, but the response still travels back: ncu counted 1.9 M returned sectors
@@ -333,18 +391,22 @@ __global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict_
 //   kModel: where the batch's loss sum comes from (batch_loss_sum).
 //   kAvg (k_update_avg): also avg_j <- avg_j + w_j of the NEW weights, every column (averaged SGD, dsgd_average_begin).
 // ---------------------------------------------------------------------------------------------------
-template <bool kFuseRegularize, int kModel, bool kAvg>
+// kL1 (k_update_l1, k_update_avg_l1): after the update, the proximal step of the L1 penalty lambda1 * ||w||_1 on EVERY column,
+// w_j <- soft_threshold(u_j, lr * lambda1); c, ||w||^2, ||w||_1 and the averaging sum then see the thresholded weights, and
+// the step's loss adds lambda1 * ||w_before||_1 (scal[kScalL1]).  ||w||_1 is summed in fixed-point limbs (acc_push_block), so
+// it has the same bits as k_l1_norm over the same weights.
+template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1 = false>
 __device__ __forceinline__ void update_body(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
                                             const double *__restrict__ d, int dim, double lambda, double lr, double inv_k_den,
                                             double *__restrict__ scal, unsigned long long *__restrict__ cnt,
                                             double *__restrict__ partial, double n_samples_local,
-                                            double *__restrict__ loss_out, double *__restrict__ avg) {
+                                            double *__restrict__ loss_out, double *__restrict__ avg, double lambda1 = 0.0) {
   __shared__ double red[8];
   __shared__ bool is_last;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const double c = scal[kScalC];
   const bool add_c = (c != 0.0) && (fabs(c) > kEps);
-  double pd = 0.0, pn = 0.0;
+  double pd = 0.0, pn = 0.0, pa = 0.0;
   if (j < dim) {
     const double raw = g[j];
     double v = raw;
@@ -353,18 +415,30 @@ __device__ __forceinline__ void update_body(double *__restrict__ w, float *__res
       if (v != 0.0 && add_c) v = filt(v + c);
     }
     double wn = w[j];
+    const double w_before = wn;
     if (raw != 0.0) g[j] = 0.0;
     if (v != 0.0) {
       const double mean = filt(v / inv_k_den);  // Vec.mean: sum / K
       const double step = filt(mean * lr);      // learningRate * grad
       wn = filt(wn - step);                     // batchWeights - ...
-      w[j] = wn;
-      w32[j] = (float)wn;
+      if (!kL1) {
+        w[j] = wn;
+        w32[j] = (float)wn;
+      }
+    }
+    if (kL1) {
+      wn = soft_threshold(wn, lr * lambda1);
+      if (__double_as_longlong(wn) != __double_as_longlong(w_before)) {
+        w[j] = wn;
+        w32[j] = (float)wn;
+      }
+      pa = fabs(wn);
     }
     if (kAvg) avg[j] = avg[j] + wn;
     pd = filt(wn * d[j]);
     pn = wn * wn;
   }
+  if (kL1) acc_push_block<256>(pa, cnt + kCntL1);
   pd = block_sum<256>(pd, red);
   pn = block_sum<256>(pn, red);
   if (threadIdx.x == 0) {
@@ -394,7 +468,12 @@ __device__ __forceinline__ void update_body(double *__restrict__ w, float *__res
         g[dim] = 0.0;
         g[dim + 1] = 0.0;
       }
-      if (loss_out) *loss_out = lambda * scal[kScalNrm2] + hinge / total;
+      if (kL1) {
+        if (loss_out) *loss_out = lambda * scal[kScalNrm2] + lambda1 * scal[kScalL1] + hinge / total;
+        scal[kScalL1] = acc_take(cnt + kCntL1);
+      } else if (loss_out) {
+        *loss_out = lambda * scal[kScalNrm2] + hinge / total;
+      }
       scal[kScalC] = lambda * 2.0 * sd;
       scal[kScalNrm2] = sn;
       clear_batch_loss<kModel>(cnt);
@@ -421,6 +500,44 @@ __global__ void __launch_bounds__(256) k_update_avg(double *__restrict__ w, floa
                                                     double *__restrict__ avg) {
   update_body<kFuseRegularize, kModel, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
                                              loss_out, avg);
+}
+
+template <bool kFuseRegularize, int kModel = kSvm>
+__global__ void __launch_bounds__(256) k_update_l1(double *__restrict__ w, float *__restrict__ w32,
+                                                   double *__restrict__ g, const double *__restrict__ d, int dim,
+                                                   double lambda, double lr, double inv_k_den, double *__restrict__ scal,
+                                                   unsigned long long *__restrict__ cnt, double *__restrict__ partial,
+                                                   double n_samples_local, double *__restrict__ loss_out, double lambda1) {
+  update_body<kFuseRegularize, kModel, false, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
+                                                    n_samples_local, loss_out, nullptr, lambda1);
+}
+template <bool kFuseRegularize, int kModel = kSvm>
+__global__ void __launch_bounds__(256) k_update_avg_l1(double *__restrict__ w, float *__restrict__ w32,
+                                                       double *__restrict__ g, const double *__restrict__ d, int dim,
+                                                       double lambda, double lr, double inv_k_den, double *__restrict__ scal,
+                                                       unsigned long long *__restrict__ cnt, double *__restrict__ partial,
+                                                       double n_samples_local, double *__restrict__ loss_out,
+                                                       double *__restrict__ avg, double lambda1) {
+  update_body<kFuseRegularize, kModel, true, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
+                                                   n_samples_local, loss_out, avg, lambda1);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_l1_norm + k_l1_finish: ||w||_1 = sum_j |w_j| in the fixed-point limbs (exact in any order: every |w_j| > 1e-20 is a
+// multiple of 2^-160) and #{w_j != 0}, over one column per thread; k_l1_finish converts the sum once, writes it to *l1_out
+// and the count to *nnz_out (if not null), and clears the counter words for the next pass.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_l1_norm(const double *__restrict__ w, int dim, unsigned long long *__restrict__ cnt) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const double wj = j < dim ? w[j] : 0.0;
+  acc_push_block<256>(fabs(wj), cnt + kCntL1);
+  const int nz = __syncthreads_count(wj != 0.0);
+  if (threadIdx.x == 0 && nz) atomicAdd(&cnt[kCntNnz], (unsigned long long)nz);
+}
+__global__ void k_l1_finish(unsigned long long *__restrict__ cnt, double *__restrict__ l1_out, long long *__restrict__ nnz_out) {
+  *l1_out = acc_take(cnt + kCntL1);
+  if (nnz_out) *nnz_out = (long long)cnt[kCntNnz];
+  cnt[kCntNnz] = 0ull;
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -93,6 +93,8 @@ struct PersistParams {
   double *avg;                            // [dim] running sum of W_t over the averaged steps: read at launch, written at exit
   // ---- per-step learning rates (kLrTable); last for the same reason ----
   const double *lrs;                      // [n_steps]: step s of this launch uses lrs[s] instead of lr
+  // ---- L1 penalty (kL1, one GPU); last for the same reason ----
+  double lambda1;                         // every update is followed by soft_threshold(., lr * lambda1) on every column
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -277,6 +279,9 @@ constexpr int kTlWords = 256 * 16 + kTlSteps * kTlCtas * kTlPerCta;
 // ---- weight fetch of the consumers: W_t[col] -----------------------------------------------------------------
 // One GPU: the update of step t-1 applied on the fly to (W_{t-1}[col], g_{t-1}[col]); c_{t-1} arrives through an
 // mbarrier (completed during the previous interval, so the wait normally falls through).
+// kL1: the update is followed by the proximal step of the L1 penalty, soft_threshold(., tau), on every column the consumers
+// read -- also on those whose g_{t-1} is 0.
+template <bool kL1 = false>
 struct FetchLocal {
   const double2 *R;   // records {W_{t-1}, g_{t-1}}
   uint64_t *cbar;
@@ -285,6 +290,7 @@ struct FetchLocal {
   int *abort_flag;
   long long timeout;
   double k_den, lr;
+  double tau = 0.0;   // kL1 only
   double c = 0.0;
   bool add_c = false, have_c = false, good = true;
   __device__ __forceinline__ void need_c() {
@@ -304,12 +310,17 @@ struct FetchLocal {
     }
     need_c();
 #pragma unroll
-    for (int u = 0; u < 4; ++u) wv[u] = apply_update(r[u].x, r[u].y, c, add_c, k_den, lr);
+    for (int u = 0; u < 4; ++u) {
+      wv[u] = apply_update(r[u].x, r[u].y, c, add_c, k_den, lr);
+      if constexpr (kL1) wv[u] = soft_threshold(wv[u], tau);
+    }
   }
   __device__ __forceinline__ double get1(uint32_t col) {
     need_c();
     const double2 r = __ldcg(&R[col]);
-    return apply_update(r.x, r.y, c, add_c, k_den, lr);
+    const double wv = apply_update(r.x, r.y, c, add_c, k_den, lr);
+    if constexpr (kL1) return soft_threshold(wv, tau);
+    return wv;
   }
 };
 // K GPUs: the LL word of W_T[col] published by the column's thread of this GPU, spinning on its tag.
@@ -473,9 +484,18 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
 // kLrTable: step s of the launch takes the rate p.lrs[s] instead of p.lr.  Interval t applies the update of step t-1 (the
 // consumers' on-the-fly fetch, the update warps, the K-GPU column threads), so all of them use lrs[t-1]; interval 0
 // applies no update.
-template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable>
+// kL1 (one GPU only): the update of step t-1 is followed by the proximal step of the L1 penalty on EVERY column, tau =
+// lr * lambda1 with the same lr, in both places that apply it (the consumers' FetchLocal and the update warps); interval 0
+// applies none.  A register column whose value changed is stored into the next three record buffers (ttl), as after a
+// gradient update.  ||W_T||_1 travels like W_T . d and ||W_T||^2: fp64 per-warp partials in sm.red[warp - kCons][0] (the
+// consumers' slots, unused on one GPU), summed per CTA by update warp 0 and pushed as fixed-point limbs into words 11..15
+// of the step's accumulator (overflow word 10 shared).  The loss of step t-1 adds lambda1 * ||W_{t-1}||_1.
+template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable,
+          bool kL1 = false>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
+  static_assert(!kL1 || (!kMulti && kUpd <= kCons), "the L1 form is one-GPU only and keeps its partials in the consumers' slots");
+  static_assert(kAccWords + kAccLimbs <= kAccStride, "the L1 limbs follow the accumulator's overflow word");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
 
@@ -667,7 +687,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
 
     // ---- update warp 0, first thing: c_{T-1} and ||W_{T-1}||^2 from the partials the last barrier delivered ----
     if (warp == kCons && !first) {
-      double c_prev, nrm_prev;
+      double c_prev, nrm_prev, l1_prev = 0.0;
       if (kMulti && t == 1) {
         c_prev = p.scal[kScalC];                              // W_base came from the host: k_prepare / previous launch
         nrm_prev = p.scal[kScalNrm2];
@@ -676,29 +696,38 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
         acc_read(acc_prev, lane, sd, sn);
         c_prev = p.lambda * 2.0 * sd;
         nrm_prev = sn;
+        if constexpr (kL1) l1_prev = acc_read_l1(acc_prev, lane);
       }
-      if (blockIdx.x == 0 && lane < kAccWords) acc_next[lane] = 0ull;
+      if (blockIdx.x == 0 && lane < (kL1 ? kAccStride : kAccWords)) acc_next[lane] = 0ull;
       if (lane == 0) {
         sm.c_val[t & 1] = c_prev;
         sm.nrm_val[t & 1] = nrm_prev;
         mbar_arrive(&sm.c_bar[t & 1]);
         // one GPU: loss of step t-1 = lambda*||W_{t-1}||^2 + hinge_{t-1}/batch  (SparseSVM.scala:20-23; SURVEY.md F5)
-        if (!kMulti && p.losses && blockIdx.x == 0)
-          p.losses[t - 1] = p.lambda * nrm_prev + (double)__ldcg(&p.hinge[t - 1]) / (double)B;
+        if (!kMulti && p.losses && blockIdx.x == 0) {
+          if constexpr (kL1)
+            p.losses[t - 1] = p.lambda * nrm_prev + p.lambda1 * l1_prev + (double)__ldcg(&p.hinge[t - 1]) / (double)B;
+          else
+            p.losses[t - 1] = p.lambda * nrm_prev + (double)__ldcg(&p.hinge[t - 1]) / (double)B;
+        }
       }
       __syncwarp();
       DSGD_TL(9);
     }
     double pd = 0.0, pn = 0.0;   // this thread's share of W_T . d and ||W_T||^2
+    double pa = 0.0;             // kL1: its share of ||W_T||_1
+    const double tau = (kL1 && !first) ? lr * p.lambda1 : 0.0;   // interval 0 applies no update and no threshold
     // The CTA's partial {W_T . d, ||W_T||^2}: every warp that owns columns leaves its share in shared memory as soon as its
     // columns are done (no waiting); update warp 0 -- idle until the barrier anyway -- sums them in warp order and adds
     // ONE fixed-point value per CTA to the step's accumulator, well before the arrival.
     auto publish_partial = [&]() {
       pd = warp_sum(pd);
       pn = warp_sum(pn);
+      if constexpr (kL1) pa = warp_sum(pa);
       if (lane == 0) {
         sm.red[warp][0] = pd;
         sm.red[warp][1] = pn;
+        if constexpr (kL1) sm.red[warp - kCons][0] = pa;
         mbar_arrive(&sm.u_bar);
       }
       if (warp == kCons) {
@@ -708,6 +737,12 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
 #pragma unroll
           for (int i = kMulti ? 0 : kCons; i < kCons + kUpd; ++i) { sd += sm.red[i][0]; sn += sm.red[i][1]; }
           if (sd != 0.0 || sn != 0.0) acc_push(acc_cur, sd, sn);
+          if constexpr (kL1) {
+            double sa = 0.0;
+#pragma unroll
+            for (int i = 0; i < kUpd; ++i) sa += sm.red[i][0];
+            if (sa != 0.0) acc_push_one(acc_cur + kAccWords, acc_cur + 2 * kAccLimbs, sa);
+          }
         }
         __syncwarp();
       }
@@ -887,7 +922,8 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           auto &mt = sm.meta[st];
           mbar_wait(&sm.full[st], (unsigned)(((unsigned)t / kStages) & 1u), p.abort_flag, p.timeout_cycles);
           if (warp == 0) DSGD_TL(1);
-          FetchLocal fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
+          FetchLocal<kL1> fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
+          if constexpr (kL1) fetch.tau = tau;
           const unsigned hinge = consume_stage<kCons, kMaxChunks>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
                                                                             lane, warp == 0 ? tl_row : nullptr);
           if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
@@ -918,6 +954,11 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
               wreg[i] = apply_update(wreg[i], gv[i], c_prev, add_c, p.k_den, lr);
               ttl[i] = 3;
             }
+            if constexpr (kL1) {
+              const double wt = soft_threshold(wreg[i], tau);
+              if (__double_as_longlong(wt) != __double_as_longlong(wreg[i])) { wreg[i] = wt; ttl[i] = 3; }
+              pa += fabs(wreg[i]);
+            }
             if (ttl[i] > 0) { Rcur[j].x = wreg[i]; --ttl[i]; }
             if (gnz[i]) Rnext[j].y = 0.0;          // held g_{t-2}, read for the last time during interval t-1
             gnz[i] = gv[i] != 0.0;
@@ -928,7 +969,11 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
         }
         for (int j = u0 + kUpdCols * n_upd; j < p.dim; j += n_upd) {   // more columns than kUpdCols per update thread
           const double2 r = __ldcg(&Rprev[j]);
-          const double wn = apply_update(r.x, r.y, c_prev, add_c, p.k_den, lr);
+          double wn = apply_update(r.x, r.y, c_prev, add_c, p.k_den, lr);
+          if constexpr (kL1) {
+            wn = soft_threshold(wn, tau);
+            pa += fabs(wn);
+          }
           Rcur[j].x = wn;
           Rnext[j].y = 0.0;
           if constexpr (kAvg) if (!first) p.avg[j] = p.avg[j] + wn;
@@ -981,7 +1026,13 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   if (blockIdx.x == 0 && warp == kCons && S > 0) {
     double sd, sn;
     acc_read(p.acc + (size_t)ti_prev * kAccStride, lane, sd, sn);   // partials of W_S: complete at the last barrier
-    if (lane == 0) { p.scal[kScalC] = p.lambda * 2.0 * sd; p.scal[kScalNrm2] = sn; }
+    double l1 = 0.0;
+    if constexpr (kL1) l1 = acc_read_l1(p.acc + (size_t)ti_prev * kAccStride, lane);
+    if (lane == 0) {
+      p.scal[kScalC] = p.lambda * 2.0 * sd;
+      p.scal[kScalNrm2] = sn;
+      if constexpr (kL1) p.scal[kScalL1] = l1;
+    }
   }
   if constexpr (kMulti) {
     const unsigned long long *LW = p.llw[(base + S) & 1];

@@ -80,6 +80,10 @@ object DsgdNative {
   @native def averageBegin(ctx: Long): Int
   @native def averageEnd(ctx: Long): Int
   @native def averageWeights(ctx: Long, avg: Array[Double], nSteps: Array[Long]): Int
+  // L1 penalty of the sync steps (elastic net with lambda): every step soft-thresholds every weight at lr * lambda1;
+  // weightsL1: l1(0) = ||w||_1, nnz(0) = the non-zero weights, of w or (w null) of the resident weights
+  @native def setL1(ctx: Long, lambda1: Double): Int
+  @native def weightsL1(ctx: Long, w: Array[Double], l1: Array[Double], nnz: Array[Long]): Int
   // async (Hogwild) mode
   @native def asyncHostMaster(ctx: Long, w0: Array[Double]): Int
   @native def ipcExport(ctx: Long, which: Int, handle: Array[Byte]): Int

@@ -405,6 +405,23 @@ FN(averageWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray avg, jlongAr
   back_Long(env, nSteps, bn, rc);
   return rc;
 }
+/* L1 penalty of the sync steps: setL1(lambda1 >= 0); weightsL1: l1(0) = ||w||_1 and nnz(0) = the non-zero weights of w (dim
+ * values), or of the resident weights when w is null.  A w of another length than dim, or an empty output array, is
+ * DSGD_ERR_INVALID. */
+FN(setL1)(JNIEnv *env, jobject self, jlong h, jdouble lambda1) { return dsgd_set_l1(CTX(h), lambda1); }
+FN(weightsL1)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jdoubleArray l1, jlongArray nnz) {
+  buf_t bw = in_Double(env, w), bl = out_Double(env, l1), bn = out_Long(env, nnz);
+  int rc = DSGD_ERR_NOMEM;
+  int32_t dim = 0;
+  if (!(bw.bad | bl.bad | bn.bad) && (rc = dsgd_dim(CTX(h), &dim)) == DSGD_OK)
+    rc = (bw.p && (int32_t)bw.n != dim) || (bl.p && bl.n < 1) || (bn.p && bn.n < 1)
+             ? DSGD_ERR_INVALID
+             : dsgd_weights_l1(CTX(h), (const double *)bw.p, (double *)bl.p, (int64_t *)bn.p);
+  back_Double(env, l1, bl, rc);
+  back_Long(env, nnz, bn, rc);
+  free(bw.p);
+  return rc;
+}
 
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {

@@ -35,9 +35,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     if cfg.learning_rate_decay != 0.0 and cfg.is_async:
         raise ValueError("learning-rate-decay: the decaying learning rate is a sync-mode option; asynchronous (Hogwild) "
                          "training keeps its constant rate")
+    if cfg.l1 != 0.0 and cfg.is_async:
+        raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
-    model = SparseLogistic(cfg.lam) if cfg.model == "logistic" else SparseSVM(cfg.lam)
+    model = (SparseLogistic if cfg.model == "logistic" else SparseSVM)(cfg.lam, l1=cfg.l1)
     slave = Slave(rank, 0, train, model, cfg.is_async, world=world, device=device, test_data=test)
     master = Master.create(rank, train, test, model, cfg.is_async, cfg.node_count, slave=slave, group=Group(), seed=seed,
                            log=(log if rank == 0 else None), jvm_exact=jvm_exact)
@@ -46,7 +48,7 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     w0 = np.zeros(data.dim)                                                    # data(0)._1.zerosLike (Main.scala:74)
     report = {"config": {k: getattr(cfg, k) for k in ("batch_size", "learning_rate", "lam", "node_count", "is_async",
                                                       "max_epochs", "check_every", "leaky_loss", "patience", "conv_delta",
-                                                      "model", "learning_rate_decay", "learning_rate_power")},
+                                                      "model", "learning_rate_decay", "learning_rate_power", "l1")},
               "rows": {"train": train.n_rows, "test": test.n_rows}, "world": world}
     report["initial_loss"] = master.distributed_loss(w0)                      # Main.scala:75-76
     report["initial_accuracy"] = master.distributed_accuracy(w0)              # Main.scala:77-78

@@ -16,3 +16,4 @@ import numpy as np
 class SparseSVM:
     lam: float                                  # `lambda`
     dim_sparsity: Optional[np.ndarray] = None   # None: computed on the device from the train rows (Main.scala:54-65)
+    l1: float = 0.0                             # extension: L1 penalty l1 * ||w||_1, a proximal step in every sync step

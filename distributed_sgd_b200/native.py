@@ -131,6 +131,9 @@ ABI = {
     "dsgd_average_begin": [_vp],
     "dsgd_average_end": [_vp],
     "dsgd_average_weights": [_vp, _vp, C.POINTER(_i64)],
+    "dsgd_set_l1": [_vp, _f64],
+    "dsgd_dim": [_vp, C.POINTER(_i32)],
+    "dsgd_weights_l1": [_vp, _vp, C.POINTER(_f64), C.POINTER(_i64)],
     "dsgd_async_host_master": [_vp, _vp],
     "dsgd_ipc_export": [_vp, C.c_int, _vp],
     "dsgd_ipc_import": [_vp, C.c_int, _vp],
@@ -550,6 +553,18 @@ class NativeCtx:
         n = C.c_int64()
         self._ck(self._l.dsgd_average_weights(self._h, _ptr(out), C.byref(n)))
         return out, n.value
+
+    # -- L1 penalty (sync mode) --
+    def set_l1(self, lambda1: float):
+        """Every following sync step soft-thresholds every weight at lr * lambda1 after its update (0: off)."""
+        self._ck(self._l.dsgd_set_l1(self._h, float(lambda1)))
+
+    def weights_l1(self, w=None) -> Tuple[float, int]:
+        """(||w||_1, number of non-zero weights) of w, or of the resident weights when w is None."""
+        w = self._w(w)
+        l1, nnz = C.c_double(), C.c_int64()
+        self._ck(self._l.dsgd_weights_l1(self._h, _ptr(w), C.byref(l1), C.byref(nnz)))
+        return l1.value, nnz.value
 
     # -- async --
     def async_host_master(self, w0):

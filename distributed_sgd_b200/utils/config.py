@@ -35,6 +35,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     average_from: int = -1        # extension: averaged SGD from this epoch (0-based) on, sync mode only; -1: off
     learning_rate_decay: float = 0.0   # extension: step t uses learning-rate / (1 + decay * t)^power, sync mode only
     learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
+    l1: float = 0.0               # extension: L1 penalty l1 * ||w||_1 (lasso; elastic net with lambda), sync mode only
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -49,6 +50,7 @@ _KEYS = {
     "model": ("model", "DSGD_MODEL"), "average-from": ("average_from", "DSGD_AVERAGE_FROM"),
     "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
+    "l1": ("l1", "DSGD_L1"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -120,4 +122,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"learning-rate-decay: expected a value >= 0, got {cfg.learning_rate_decay}")
     if not cfg.learning_rate_power > 0.0:
         raise ValueError(f"learning-rate-power: expected a value > 0, got {cfg.learning_rate_power}")
+    if not (cfg.l1 >= 0.0 and cfg.l1 != float("inf")):
+        raise ValueError(f"l1: expected a finite value >= 0, got {cfg.l1}")
     return cfg

@@ -309,6 +309,28 @@ int dsgd_average_begin(dsgd_ctx *ctx);   /* zero the sum and the count; average 
 int dsgd_average_end(dsgd_ctx *ctx);     /* stop averaging; the sum and the count stay readable */
 int dsgd_average_weights(dsgd_ctx *ctx, double *avg_out, int64_t *n_steps_out);
 
+/* ---- L1 penalty (lasso / elastic net) of the sync steps.  dsgd_set_l1 sets lambda1 >= 0 (0 at creation: every call then
+ *      runs the kernels it ran without this option).  With lambda1 > 0 every sync step, on every path and for both models,
+ *      first does what it does without the penalty -- u_j = filt(w_j - filt(mean_j * lr_t)) on the columns the step touched,
+ *      u_j = w_j elsewhere -- and then takes the proximal step of lambda1 * ||w||_1 on EVERY column with tau = fl(lr_t *
+ *      lambda1) (lr_t the scalar rate or lrs[t]):  w_j = u_j > tau ? filt(u_j - tau) : (u_j < -tau ? filt(u_j + tau) : 0),
+ *      the 1e-20 filter of a new Sparse.  tau == 0 leaves u as it is.  c = 2 lambda (w . d), the averaging sum and the next
+ *      step see the thresholded weights; the step's loss is lambda ||W||^2 + lambda1 ||W||_1 + loss sum / batch at the
+ *      weights the gradient was taken at.  dsgd_gradient and every dsgd_eval_* call are unchanged (the penalty belongs to
+ *      the step).  One worker on one GPU takes the persistent kernel's L1 form up to 32 rows per CTA, the per-step path
+ *      above; the fused K-rank peer exchange has no L1 form, so with world > 1 a ctx with lambda1 > 0 needs dsgd_comm_init
+ *      (a rank wired with the peer exchange only fails with DSGD_ERR_STATE before anything is launched).  The per-step
+ *      path reads ||w||_1 of the weights it starts from off the device: dsgd_set_l1 (turning the penalty on),
+ *      dsgd_set_weights and every step of an L1 ctx keep it.
+ *      dsgd_weights_l1: *l1_out = ||w||_1 (summed in fixed-point limbs: exact before one final rounding, the same bits in any
+ *      order and on every rank) and *nnz_out = #{w_j != 0}, of `w` (dim host values) or with w == NULL of the resident
+ *      weights; either output may be NULL.
+ *      Errors: lambda1 < 0 or not finite -> DSGD_ERR_INVALID; either call on an async ctx -> DSGD_ERR_STATE. ---------------- */
+int dsgd_set_l1(dsgd_ctx *ctx, double lambda1);
+/* *dim_out = the dim the ctx was created with (for bindings that check an array's length before passing it in). */
+int dsgd_dim(const dsgd_ctx *ctx, int32_t *dim_out);
+int dsgd_weights_l1(dsgd_ctx *ctx, const double *w, double *l1_out, int64_t *nnz_out);
+
 /* ---- async (Hogwild) mode.  Every worker keeps its own weight replica (core/Slave.scala:30) and pushes each
  *      delta to every peer replica and to the master's replica (core/Slave.scala:101-105).  Here replicas are
  *      reached by ADDRESS over NVLink: a rank exports its replica, the host transports the handle, peers import
