@@ -14,6 +14,7 @@ from typing import Callable, List, Optional, Sequence, Union
 import numpy as np
 
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
+from ..ml.calibration import Calibration
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
 from ..ml.sparse_logistic import SparseLogistic
@@ -61,6 +62,31 @@ def metrics_dict(words) -> dict:
     return {"tp": tp, "fn": fn, "pos_no_pred": pos_none, "fp": fp, "tn": tn, "neg_no_pred": neg_none, "u2": u2,
             "nan_scores": nan, "precision": ratio(tp, tp + fp), "recall": ratio(tp, P),
             "f1": ratio(2 * tp, 2 * tp + fp + fn + pos_none), "auc": auc, "accuracy": ratio(tp + tn, P + N)}
+
+
+def _calibration(result) -> Calibration:
+    """A NativeCtx.calibrate* result as a Calibration."""
+    a, b, objective, info = result
+    return Calibration(a, b, objective, int(info[0]), int(info[1]), int(info[2]), int(info[3]))
+
+
+def calibration_dict(result) -> dict:
+    """The result of Master.local_calibration from a NativeCtx.eval_*calibration result: brier and log_loss (means over the
+    rows used), ece = sum over the bins of (rows_b / rows) |mean predicted_b - observed frequency_b|, mce = the largest such
+    gap, rows, nan_rows, and bins: edges (n_bins + 1), rows, positives, mean_predicted and observed (NaN for an empty bin)."""
+    sums, bin_rows, bin_pos, bin_psum, words = result
+    n, m = int(words[0]), len(bin_rows)
+    filled = bin_rows > 0
+    den = np.where(filled, bin_rows, 1)
+    mean_p = np.where(filled, bin_psum / den, np.nan)
+    freq = np.where(filled, bin_pos / den, np.nan)
+    gap = np.abs(mean_p - freq)[filled]
+    nan = float("nan")
+    return {"brier": float(sums[0]) / n if n else nan, "log_loss": float(sums[1]) / n if n else nan,
+            "ece": float(np.sum(bin_rows[filled] / n * gap)) if n else nan, "mce": float(np.max(gap)) if n else nan,
+            "rows": n, "nan_rows": int(words[1]),
+            "bins": {"edges": np.arange(m + 1) / m, "rows": bin_rows, "positives": bin_pos, "mean_predicted": mean_p,
+                     "observed": freq}}
 
 
 def curve_dict(result) -> dict:
@@ -317,6 +343,44 @@ class Master:
         if ids is None:
             return curve_dict(self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=curve))
         return curve_dict(self.ctx.eval_samples_curve(ids, weights, curve=curve))
+
+    # ---- calibration (extension) -----------------------------------------------------------------------------------------
+    # Like the ranking metrics, these are not sharded: rows are replicated on every rank and every rank fits or evaluates
+    # the whole range or sample itself.  Every sum over the rows is an order-free fixed-point sum and the arithmetic between
+    # the sums is one fixed sequence, so every rank gets the same bits without a collective.  None of them touches the
+    # weights or the step state: they can be called from `fit`'s on_epoch hook.
+    def calibrate(self, weights=None, test_data: bool = False) -> Calibration:
+        """Platt scaling of the margins over the train (or test) rows: the Calibration (a, b) that makes
+        1 / (1 + exp(a x.w + b)) a probability.  weights None: the resident weights, as in local_metrics."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return _calibration(self.ctx.calibrate(b, e, weights))
+
+    def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False) -> Calibration:
+        """calibrate on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
+        sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled calibration of {samples_count} rows: the sample is empty")
+        if ids is None:
+            return _calibration(self.ctx.calibrate_sampled(b, e, key, 0, k, weights))
+        return _calibration(self.ctx.calibrate_samples(ids, weights))
+
+    def local_calibration(self, calibration: Calibration, weights=None, test_data: bool = False, n_bins: int = 10) -> dict:
+        """How well `calibration` fits the train (or test) rows: Brier score, log loss, expected and maximum calibration
+        error and the reliability bins (calibration_dict).  Every rank evaluates the whole range itself."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return calibration_dict(self.ctx.eval_calibration(b, e, calibration.a, calibration.b, n_bins, weights))
+
+    def local_sampled_calibration(self, calibration: Calibration, weights, samples_count: int, test_data: bool = False,
+                                  n_bins: int = 10) -> dict:
+        """local_calibration on a fresh sample of min(samples_count, n) rows.  An empty sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled calibration quality of {samples_count} rows: the sample is empty")
+        a, bb = calibration.a, calibration.b
+        if ids is None:
+            return calibration_dict(self.ctx.eval_sampled_calibration(b, e, key, 0, k, a, bb, n_bins, weights))
+        return calibration_dict(self.ctx.eval_samples_calibration(ids, a, bb, n_bins, weights))
 
     def predict(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> dict:
         """Master.predict (core/Master.scala:61-75): idx -> prediction over the training rows; each worker

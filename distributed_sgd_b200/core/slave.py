@@ -87,6 +87,13 @@ class Slave:
         self._train_ids(samples_idx)
         return self.ctx.probabilities(samples_idx, weights)
 
+    def calibrated_probabilities(self, samples_idx: Sequence[int], calibration,
+                                 weights: Optional[np.ndarray] = None) -> np.ndarray:
+        """Extension, either model: P(y = +1 | x) = 1 / (1 + exp(a x.w + b)) of the listed rows under `calibration` (a
+        Calibration, e.g. from Master.calibrate)."""
+        self._train_ids(samples_idx)
+        return self.ctx.calibrated_probabilities(samples_idx, calibration.a, calibration.b, weights)
+
     def gradient(self, weights: Optional[np.ndarray], samples_idx: Sequence[int]) -> np.ndarray:
         """SlaveImpl.gradient (core/Slave.scala:142-157): regularize(sum of backward over the batch)."""
         self._train_ids(samples_idx)

@@ -23,6 +23,7 @@
 #include "dsgd_stream.cuh"
 #include "dsgd_async.cuh"
 #include "dsgd_metrics.cuh"
+#include "dsgd_calibrate.cuh"
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
@@ -154,6 +155,12 @@ struct dsgd_ctx {
   dev_buf<int> c_excl;
   dev_buf<double> c_thr;
   dev_buf<long long> c_tp, c_fp;
+  // a calibration fit (dsgd_calibrate*, dsgd_calibrate.cuh): one score and one label per position; the control words (the
+  // counts, the three accumulator lines, the barrier counter and abort flag, the result); and the quality pass's block
+  dev_buf<double> k_score;
+  dev_buf<int8_t> k_lab;
+  dev_buf<unsigned long long> k_ctl, k_eval;
+  int k_fit_occ = 0;   // CTAs of k_calib_fit per SM at its full shared-memory budget (0: not asked yet)
 
   ncclComm_t comm = nullptr;
 
@@ -767,7 +774,7 @@ static int reserve_requests(dsgd_ctx *ctx) {
       (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)) ||
       (rc = ctx->c_cnt.grow(ctx, kCurWords, kCurWords)) || (rc = ctx->c_merged.grow(ctx, n, 1024)) ||
       (rc = ctx->c_excl.grow(ctx, n, 1024)) || (rc = ctx->c_thr.grow(ctx, n, 1024)) || (rc = ctx->c_tp.grow(ctx, n, 1024)) ||
-      (rc = ctx->c_fp.grow(ctx, n, 1024)))
+      (rc = ctx->c_fp.grow(ctx, n, 1024)) || (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)))
     return rc;
   size_t tmp = 0, tmp_merge = 0, tmp_scan = 0;
   cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
@@ -1203,6 +1210,206 @@ extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const i
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
+}
+
+// ---- calibration (dsgd_calibrate.cuh; DESIGN.md §4.11) ---------------------------------------------------------------
+
+// Words of k_ctl: the counts of k_calib_score, the result of k_calib_fit, {barrier counter, abort flag}, the three lines
+constexpr int kCtlCnt = 0, kCtlOut = kCalCntWords, kCtlBar = kCtlOut + kCalOutWords, kCtlAcc = 16;
+constexpr int kCtlWords = kCtlAcc + 3 * kCalLineStride;
+static_assert(kCtlBar + 1 <= kCtlAcc, "k_ctl layout");
+static_assert(kCalMaxBins == DSGD_CALIBRATION_MAX_BINS && kCalOutEvals < kCalOutWords, "calibration layout");
+constexpr int kCalSmemScores = 14336;   // scores (8 bytes) and labels (1 byte) a CTA of k_calib_fit keeps in shared memory: 126 KB
+
+// A cooperative grid cannot be assumed resident beside a kernel that runs until it is stopped.
+static int calibrate_allowed(dsgd_ctx *ctx, const char *fn) {
+  if (!ctx->a_running) return DSGD_OK;
+  CU(cudaSetDevice(ctx->device));
+  const cudaError_t e = cudaStreamQuery(ctx->astream);
+  NEED(e != cudaErrorNotReady, DSGD_ERR_STATE, "%s: the async loop is running (stop it first: the fit is one cooperative launch)", fn);
+  CU(e);
+  return DSGD_OK;
+}
+
+// One fit over `rows`: k_calib_score, the counts read by the host, k_calib_fit, the result read back.
+static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *ab_out, double *objective_out,
+                          int64_t *info_out, const char *fn) {
+  const int64_t n = rows.n;
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd);
+  if (rc || (rc = ctx->k_score.grow(ctx, n, 1024)) || (rc = ctx->k_lab.grow(ctx, n, 1024)) ||
+      (rc = ctx->k_ctl.grow(ctx, kCtlWords, kCtlWords)))
+    return rc;
+  CU(cudaMemsetAsync(ctx->k_ctl, 0, sizeof(unsigned long long) * kCtlWords, ctx->stream));
+  const int sgrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
+  k_calib_score<<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long cnt[kCalCntWords];
+  CU(cudaMemcpyAsync(cnt, ctx->k_ctl + kCtlCnt, sizeof cnt, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int64_t n_pos = (int64_t)cnt[kCalPos], n_neg = (int64_t)cnt[kCalNeg];
+  NEED(n_pos > 0 && n_neg > 0, DSGD_ERR_EMPTY, "%s: %lld positive and %lld negative rows with a score (%lld NaN): a sigmoid needs both classes",
+       fn, (long long)n_pos, (long long)n_neg, (long long)cnt[kCalNan]);
+
+  if (!ctx->k_fit_occ) {
+    const int full = kCalSmemScores * 9;
+    CU(cudaFuncSetAttribute(k_calib_fit, cudaFuncAttributeMaxDynamicSharedMemorySize, full));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->k_fit_occ, k_calib_fit, kCalThreads, (size_t)full));
+    NEED(ctx->k_fit_occ > 0, DSGD_ERR_CUDA, "%s: k_calib_fit does not fit on an SM", fn);
+  }
+  int G = ctx->sm_count * ctx->k_fit_occ;   // resident at the full shared-memory budget, so at any smaller one
+  if (ctx->grid_limit > 0) G = std::min(G, ctx->grid_limit);
+  G = (int)std::min<int64_t>(G, cdiv(n, kCalThreads));
+  CalibFitParams fp;
+  memset(&fp, 0, sizeof fp);
+  fp.score = ctx->k_score; fp.lab = ctx->k_lab; fp.n = n;
+  fp.t_pos = ((double)n_pos + 1.0) / ((double)n_pos + 2.0);
+  fp.t_neg = 1.0 / ((double)n_neg + 2.0);
+  fp.b0 = std::log(((double)n_neg + 1.0) / ((double)n_pos + 1.0));
+  fp.acc = ctx->k_ctl + kCtlAcc;
+  fp.bar = reinterpret_cast<unsigned *>(ctx->k_ctl + kCtlBar);
+  fp.abort_flag = reinterpret_cast<int *>(ctx->k_ctl + kCtlBar) + 1;
+  fp.timeout_cycles = 4000000000ll;   // ~2 s, as the sync step's barrier
+  fp.out = ctx->k_ctl + kCtlOut;
+  fp.smem_cap = (int)std::min<int64_t>(cdiv(n, G), kCalSmemScores);
+  void *args[] = {&fp};
+  CU(cudaLaunchCooperativeKernel((void *)k_calib_fit, dim3(G), dim3(kCalThreads), args, (size_t)fp.smem_cap * 9, ctx->stream));
+  LAUNCHED();
+  unsigned long long out[kCalOutWords + 1];
+  CU(cudaMemcpyAsync(out, ctx->k_ctl + kCtlOut, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  NEED((out[kCalOutWords] >> 32) == 0, DSGD_ERR_TIMEOUT, "%s: the fit's grid barrier hit its watchdog", fn);
+  memcpy(&ab_out[0], &out[kCalOutA], sizeof(double));
+  memcpy(&ab_out[1], &out[kCalOutB], sizeof(double));
+  memcpy(objective_out, &out[kCalOutF], sizeof(double));
+  info_out[0] = (int64_t)out[kCalOutIter];
+  info_out[1] = (int64_t)out[kCalOutStatus];
+  info_out[2] = n_pos + n_neg;
+  info_out[3] = (int64_t)cnt[kCalNan];
+  info_out[4] = (int64_t)out[kCalOutEvals];
+  return DSGD_OK;
+}
+
+#define CALIB_ARGS_OK() \
+  NEED(ab_out && objective_out && info_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__)
+
+extern "C" int dsgd_calibrate(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
+                              double *objective_out, int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_ARGS_OK();
+  row_set rows;
+  int rc = calibrate_allowed(ctx, __func__);
+  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
+  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                      int64_t pos_begin, int64_t pos_end, double *ab_out, double *objective_out,
+                                      int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_ARGS_OK();
+  row_set rows;
+  int rc = calibrate_allowed(ctx, __func__);
+  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
+  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
+                                      double *objective_out, int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = calibrate_allowed(ctx, __func__);
+  if (rc || (rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
+  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+}
+
+extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
+                                             double b, double *probs_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(probs_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
+  NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", __func__, a, b);
+  row_set rows;
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = rows_list(ctx, samples, n, true, __func__, &rows);
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
+  k_calib_prob<<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b, ctx->preds);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+// One quality pass over `rows` at (a, b): k_calib_eval, k_calib_eval_finish, the block read back.
+static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, int32_t n_bins,
+                                    double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                    int64_t *words_out, const char *fn) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = fits_while_running(ctx, ctx->k_eval, fn);
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords))) return rc;
+  CU(cudaMemsetAsync(ctx->k_eval, 0, sizeof(unsigned long long) * kCevWords, ctx->stream));
+  const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);
+  k_calib_eval<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, wd, a, b,
+                                              n_bins, ctx->k_eval);
+  LAUNCHED();
+  k_calib_eval_finish<<<1, kCalMaxBins, 0, ctx->stream>>>(ctx->k_eval, n_bins);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long h[kCevWords];
+  CU(cudaMemcpyAsync(h, ctx->k_eval, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, &h[kCevOutSums], 2 * sizeof(double));
+  for (int i = 0; i < n_bins; ++i) {
+    bin_rows[i] = (int64_t)h[kCevBinRows + i];
+    bin_pos[i] = (int64_t)h[kCevBinPos + i];
+  }
+  memcpy(bin_psum, &h[kCevOutPsum], (size_t)n_bins * sizeof(double));
+  words_out[0] = (int64_t)h[kCevRows];
+  words_out[1] = (int64_t)h[kCevNan];
+  return DSGD_OK;
+}
+
+#define CALIB_EVAL_ARGS_OK()                                                                                            \
+  do {                                                                                                                  \
+    NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);  \
+    NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", __func__, a, b); \
+    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
+  } while (0)
+
+extern "C" int dsgd_eval_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a, double b,
+                                     int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                     int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_EVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                             int64_t pos_begin, int64_t pos_end, double a, double b, int32_t n_bins,
+                                             double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                             int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_EVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
+                                             double b, int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
+                                             double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_EVAL_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all

@@ -62,6 +62,28 @@ object DsgdNative {
                                thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
   @native def evalSamplesCurve(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long], ap: Array[Double],
                                nPoints: Array[Long], thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
+  // calibration (Platt scaling): ab(0..1) = (A, B) of P(y = +1 | x) = 1 / (1 + exp(A x.w + B)), objective(0) = F(A, B),
+  // info(0..4) = iterations, status (0 converged, 1 iteration limit, 2 line search failed, 3 non-finite sum), rows used, NaN
+  // rows, points evaluated.  Quality at (a, b): sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum(0 until
+  // nBins), words(0..1) = rows used and left out.
+  @native def calibrate(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, ab: Array[Double], objective: Array[Double],
+                        info: Array[Long]): Int
+  @native def calibrateSampled(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                               posEnd: Long, ab: Array[Double], objective: Array[Double], info: Array[Long]): Int
+  @native def calibrateSamples(ctx: Long, w: Array[Double], samples: Array[Int], ab: Array[Double], objective: Array[Double],
+                               info: Array[Long]): Int
+  @native def calibratedProbabilities(ctx: Long, w: Array[Double], samples: Array[Int], a: Double, b: Double,
+                                      out: Array[Double]): Int
+  @native def evalCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, a: Double, b: Double, nBins: Int,
+                              sums: Array[Double], binRows: Array[Long], binPos: Array[Long], binPsum: Array[Double],
+                              words: Array[Long]): Int
+  @native def evalSampledCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                     posEnd: Long, a: Double, b: Double, nBins: Int, sums: Array[Double],
+                                     binRows: Array[Long], binPos: Array[Long], binPsum: Array[Double],
+                                     words: Array[Long]): Int
+  @native def evalSamplesCalibration(ctx: Long, w: Array[Double], samples: Array[Int], a: Double, b: Double, nBins: Int,
+                                     sums: Array[Double], binRows: Array[Long], binPos: Array[Long], binPsum: Array[Double],
+                                     words: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

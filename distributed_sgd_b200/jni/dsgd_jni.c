@@ -320,6 +320,136 @@ FN(evalSamplesCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArr
   return rc;
 }
 
+/* calibration: ab(0..1) = (A, B), objective(0) = F(A, B), info(0..4) = the DSGD_CALIBRATION_INFO_WORDS words; probabilities:
+ * out(i) = sigmoid(-(a x_i . w + b)); quality: sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum at least nBins
+ * long, words(0..1) = rows used and left out.  A shorter array is DSGD_ERR_INVALID. */
+typedef struct { buf_t ab, f, info; } calib_bufs;
+static calib_bufs calib_out(JNIEnv *env, jdoubleArray ab, jdoubleArray objective, jlongArray info) {
+  calib_bufs c = {out_Double(env, ab), out_Double(env, objective), out_Long(env, info)};
+  return c;
+}
+static int calib_bad(const calib_bufs *c) { return c->ab.bad | c->f.bad | c->info.bad; }
+static int calib_short(const calib_bufs *c) { return c->ab.n < 2 || c->f.n < 1 || c->info.n < DSGD_CALIBRATION_INFO_WORDS; }
+static void calib_back(JNIEnv *env, jdoubleArray ab, jdoubleArray objective, jlongArray info, calib_bufs *c, int rc) {
+  back_Double(env, ab, c->ab, rc);
+  back_Double(env, objective, c->f, rc);
+  back_Long(env, info, c->info, rc);
+}
+FN(calibrate)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray ab,
+              jdoubleArray objective, jlongArray info) {
+  buf_t bw = in_Double(env, w);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | calib_bad(&c)))
+    rc = calib_short(&c) ? DSGD_ERR_INVALID
+                         : dsgd_calibrate(CTX(h), bw.p, rowBegin, rowEnd, (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                     jlong posBegin, jlong posEnd, jdoubleArray ab, jdoubleArray objective, jlongArray info) {
+  buf_t bw = in_Double(env, w);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | calib_bad(&c)))
+    rc = calib_short(&c) ? DSGD_ERR_INVALID
+                         : dsgd_calibrate_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                  (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray ab,
+                     jdoubleArray objective, jlongArray info) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | calib_bad(&c)))
+    rc = calib_short(&c) ? DSGD_ERR_INVALID
+                         : dsgd_calibrate_samples(CTX(h), bw.p, bs.p, bs.n, (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+FN(calibratedProbabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a, jdouble b,
+                            jdoubleArray out) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bo.bad))
+    rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_calibrated_probabilities(CTX(h), bw.p, bs.p, bs.n, a, b, bo.p);
+  back_Double(env, out, bo, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+typedef struct { buf_t s, r, p, ps, wd; } quality_bufs;
+static quality_bufs quality_out(JNIEnv *env, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
+                                jlongArray words) {
+  quality_bufs q = {out_Double(env, sums), out_Long(env, binRows), out_Long(env, binPos), out_Double(env, binPsum),
+                    out_Long(env, words)};
+  return q;
+}
+static int quality_bad(const quality_bufs *q) { return q->s.bad | q->r.bad | q->p.bad | q->ps.bad | q->wd.bad; }
+/* nBins outside 1 .. DSGD_CALIBRATION_MAX_BINS is the library's DSGD_ERR_INVALID: only the lengths are checked here */
+static int quality_short(const quality_bufs *q, jint nBins) {
+  const jlong m = nBins > 0 ? nBins : 0;
+  return q->s.n < 2 || q->wd.n < 2 || q->r.n < m || q->p.n < m || q->ps.n < m;
+}
+static void quality_back(JNIEnv *env, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
+                         jlongArray words, quality_bufs *q, int rc) {
+  back_Double(env, sums, q->s, rc);
+  back_Long(env, binRows, q->r, rc);
+  back_Long(env, binPos, q->p, rc);
+  back_Double(env, binPsum, q->ps, rc);
+  back_Long(env, words, q->wd, rc);
+}
+FN(evalCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdouble a, jdouble b,
+                    jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
+                    jlongArray words) {
+  buf_t bw = in_Double(env, w);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | quality_bad(&q)))
+    rc = quality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_calibration(CTX(h), bw.p, rowBegin, rowEnd, a, b, nBins, (double *)q.s.p, (int64_t *)q.r.p,
+                                     (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                           jlong posBegin, jlong posEnd, jdouble a, jdouble b, jint nBins, jdoubleArray sums,
+                           jlongArray binRows, jlongArray binPos, jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | quality_bad(&q)))
+    rc = quality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, a, b, nBins,
+                                             (double *)q.s.p, (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p,
+                                             (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a, jdouble b,
+                           jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
+                           jlongArray words) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | quality_bad(&q)))
+    rc = quality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_calibration(CTX(h), bw.p, bs.p, bs.n, a, b, nBins, (double *)q.s.p, (int64_t *)q.r.p,
+                                             (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {
   buf_t b = out_Byte(env, id);

@@ -73,6 +73,23 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     report["updates"] = state.updates
     if "averaged_steps" in getattr(master, "history", {}):
         report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
+    if cfg.calibrate:
+        # a Platt sigmoid fitted on the train rows, judged on the test rows; for the logistic model also against the
+        # model's own probability, the identity link
+        from .ml import Calibration
+        cal = master.calibrate(w1)
+        q = master.local_calibration(cal, w1, test_data=True)
+        report["calibration"] = {"a": cal.a, "b": cal.b, "iterations": cal.iterations, "status": cal.status,
+                                 "test_brier": q["brier"], "test_log_loss": q["log_loss"], "test_ece": q["ece"]}
+        if cfg.model == "logistic":
+            q0 = master.local_calibration(Calibration.identity(), w1, test_data=True)
+            report["calibration"]["identity"] = {"test_brier": q0["brier"], "test_log_loss": q0["log_loss"],
+                                                 "test_ece": q0["ece"]}
+        if rank == 0:
+            log(f"calibration: A = {cal.a:.6g}, B = {cal.b:.6g} ({cal.iterations} Newton iterations, status {cal.status}); "
+                f"test Brier {q['brier']:.6f}, log loss {q['log_loss']:.6f}, ECE {q['ece']:.6f}"
+                + (f"; identity link: Brier {q0['brier']:.6f}, log loss {q0['log_loss']:.6f}, ECE {q0['ece']:.6f}"
+                   if cfg.model == "logistic" else ""))
     if inspect:
         inspect("done", (master, state))
     slave.stop()

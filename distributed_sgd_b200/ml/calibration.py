@@ -1,0 +1,24 @@
+"""A fitted probability link for a trained model: P(y = +1 | x) = 1 / (1 + exp(a x.w + b)) (Platt scaling)."""
+from __future__ import annotations
+
+from dataclasses import dataclass
+
+CONVERGED, ITERATION_LIMIT, LINE_SEARCH_FAILED, NON_FINITE = 0, 1, 2, 3
+
+
+@dataclass(frozen=True)
+class Calibration:
+    """(a, b) and how the fit that produced them ended.  x.w is the margin as Slave.margins returns it: a positive row has
+    a negative x.w, so a fitted `a` is normally positive."""
+    a: float
+    b: float
+    objective: float = float("nan")   # F(a, b), the regularised cross-entropy the fit minimised
+    iterations: int = 0               # accepted Newton steps
+    status: int = CONVERGED           # CONVERGED, ITERATION_LIMIT, LINE_SEARCH_FAILED or NON_FINITE
+    rows: int = 0                     # rows the fit used
+    nan_rows: int = 0                 # rows left out because their margin was NaN
+
+    @staticmethod
+    def identity() -> "Calibration":
+        """(1, 0): the SparseLogistic model's own probability sigmoid(-x.w)."""
+        return Calibration(1.0, 0.0)

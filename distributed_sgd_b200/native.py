@@ -28,6 +28,8 @@ REPLICA_SELF, REPLICA_MASTER = 0, 1
 OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM, ERR_TIMEOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8
 # words of the dsgd_eval_*metrics calls: TP, FN, positives without a +-1 prediction, FP, TN, negatives without one, U2, NaN rows
 METRICS_WORDS = 8
+CALIBRATION_INFO_WORDS = 5   # DSGD_CALIBRATION_INFO_WORDS
+CALIBRATION_MAX_BINS = 64    # DSGD_CALIBRATION_MAX_BINS
 
 
 class NativeLibraryMissing(ImportError):
@@ -108,6 +110,13 @@ ABI = {
     "dsgd_eval_metrics": [_vp, _vp, _i64, _i64, _vp],
     "dsgd_eval_sampled_metrics": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp],
     "dsgd_eval_samples_metrics": [_vp, _vp, _vp, _i64, _vp],
+    "dsgd_calibrate": [_vp, _vp, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_calibrate_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_calibrate_samples": [_vp, _vp, _vp, _i64, _vp, _vp, _vp],
+    "dsgd_calibrated_probabilities": [_vp, _vp, _vp, _i64, _f64, _f64, _vp],
+    "dsgd_eval_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_sampled_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_samples_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
@@ -404,6 +413,67 @@ class NativeCtx:
         samples = _arr(samples, np.int32)
         return self._request("eval_samples_metrics", w, (_ptr(samples), samples.size),
                              np.zeros(METRICS_WORDS, dtype=np.int64))
+
+    # -- calibration --
+    def _calibrate(self, fn: str, w, rows: tuple):
+        """dsgd_<fn>: (A, B, objective, info) of one Platt fit; info = the CALIBRATION_INFO_WORDS words {iterations, status,
+        rows used, NaN rows, points evaluated}."""
+        w = self._w(w)
+        ab = np.zeros(2, dtype=np.float64)
+        info = np.zeros(CALIBRATION_INFO_WORDS, dtype=np.int64)
+        obj = C.c_double()
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(ab), C.byref(obj), _ptr(info)))
+        return float(ab[0]), float(ab[1]), obj.value, info
+
+    def calibrate(self, row_begin: int, row_end: int, w=None):
+        """Platt scaling of x . w over rows [row_begin, row_end) (dsgd_calibrate): (A, B, objective, info) with
+        P(y = +1 | x) = 1 / (1 + exp(A x . w + B))."""
+        return self._calibrate("calibrate", w, (row_begin, row_end))
+
+    def calibrate_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_sampled)."""
+        return self._calibrate("calibrate_sampled", w, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def calibrate_samples(self, samples, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_calibrate_samples)."""
+        samples = _arr(samples, np.int32)
+        return self._calibrate("calibrate_samples", w, (_ptr(samples), samples.size))
+
+    def calibrated_probabilities(self, samples, a: float, b: float, w=None) -> np.ndarray:
+        """sigmoid(-(a x . w + b)) for each listed row, either model (dsgd_calibrated_probabilities)."""
+        samples = _arr(samples, np.int32)
+        w = self._w(w)
+        out = np.zeros(samples.size, dtype=np.float64)
+        self._ck(self._l.dsgd_calibrated_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, float(a), float(b),
+                                                       _ptr(out)))
+        return out
+
+    def _eval_calibration(self, fn: str, w, rows: tuple, a: float, b: float, n_bins: int):
+        """dsgd_<fn>: (sums, bin_rows, bin_pos, bin_psum, words): sums = {Brier, log loss} sums, words = {rows used, rows
+        left out}."""
+        w = self._w(w)
+        m = max(int(n_bins), 1)
+        sums, words = np.zeros(2, dtype=np.float64), np.zeros(2, dtype=np.int64)
+        rows_b, pos_b, psum = np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.float64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, float(a), float(b), int(n_bins), _ptr(sums),
+                                                 _ptr(rows_b), _ptr(pos_b), _ptr(psum), _ptr(words)))
+        return sums, rows_b, pos_b, psum, words
+
+    def eval_calibration(self, row_begin: int, row_end: int, a: float, b: float, n_bins: int = 10, w=None):
+        """Brier and log-loss sums and n_bins reliability bins at (a, b) over rows [row_begin, row_end)
+        (dsgd_eval_calibration)."""
+        return self._eval_calibration("eval_calibration", w, (row_begin, row_end), a, b, n_bins)
+
+    def eval_sampled_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, a: float,
+                                 b: float, n_bins: int = 10, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_calibration)."""
+        return self._eval_calibration("eval_sampled_calibration", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), a, b,
+                                      n_bins)
+
+    def eval_samples_calibration(self, samples, a: float, b: float, n_bins: int = 10, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_calibration)."""
+        samples = _arr(samples, np.int32)
+        return self._eval_calibration("eval_samples_calibration", w, (_ptr(samples), samples.size), a, b, n_bins)
 
     def _curve(self, fn: str, w, rows: tuple, n: int, curve: bool):
         """dsgd_<fn>: (words, ap, thr, tp, fp) with the m points of a curve pass over n rows, or (words, ap, m) when not

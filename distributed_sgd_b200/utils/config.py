@@ -36,6 +36,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     learning_rate_decay: float = 0.0   # extension: step t uses learning-rate / (1 + decay * t)^power, sync mode only
     learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
     l1: float = 0.0               # extension: L1 penalty l1 * ||w||_1 (lasso; elastic net with lambda), sync mode only
+    calibrate: bool = False       # extension: after fit, fit a Platt sigmoid on the train rows and report its test-set quality
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -50,7 +51,7 @@ _KEYS = {
     "model": ("model", "DSGD_MODEL"), "average-from": ("average_from", "DSGD_AVERAGE_FROM"),
     "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
-    "l1": ("l1", "DSGD_L1"),
+    "l1": ("l1", "DSGD_L1"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}

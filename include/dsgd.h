@@ -236,6 +236,52 @@ int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, i
 int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
                             double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out);
 
+/* ---- calibration: scores into probabilities, for either model, over the same three row forms and with the conventions and
+ *      errors of the metrics calls above.  With f = x_i . w exactly as dsgd_margins returns it, a calibration is a pair (A, B)
+ *      and P(y = +1 | x_i) = 1 / (1 + exp(A f + B)), computed as sigmoid(-(A f + B)) with the sigmoid of the logistic gradient.
+ *      A positive row has a negative x . w here, so a fitted A is normally positive, and the SparseLogistic model's own
+ *      probability is the calibration (1, 0) bit for bit.
+ *      dsgd_calibrate* fit (A, B) by Platt scaling as Lin, Lin and Weng (2007) state it: rows whose f is NaN are left out and
+ *      counted; with N+ / N- the remaining positive / negative rows the targets are t = (N+ + 1) / (N+ + 2) and 1 / (N- + 2);
+ *      Newton's method from (0, log((N- + 1) / (N+ + 1))) with a ridge of 1e-12 on the Hessian's diagonal, at most 100
+ *      iterations, a backtracking line search (step 1 halved down to 1e-10, sufficient decrease 1e-4), stopping when both
+ *      gradient components are below 1e-5.  The whole iteration is one cooperative kernel launch.  Every sum over the rows
+ *      is added exactly in fixed point, so ab_out = {A, B}, *objective_out = F(A, B) and the iteration count have the same
+ *      bits for a range, the same ids in any order, any grid limit and either model flag.
+ *      info_out[0] Newton iterations (accepted steps)   info_out[1] status: 0 converged, 1 iteration limit, 2 the line search
+ *      failed (A, B are the last accepted point), 3 a sum was not finite (a term NaN, infinite or >= 2^52: A, B and F are NaN)
+ *      info_out[2] rows used   info_out[3] NaN rows left out   info_out[4] points evaluated (one grid barrier each)
+ *      No positive or no negative row with a score -> DSGD_ERR_EMPTY.  While an async loop runs -> DSGD_ERR_STATE (a
+ *      cooperative grid cannot share the device with a kernel that never ends); after dsgd_stop_async, or once the loop has
+ *      ended by itself, the calls work.  A barrier that hits its watchdog -> DSGD_ERR_TIMEOUT. ---- */
+#define DSGD_CALIBRATION_INFO_WORDS 5
+int dsgd_calibrate(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out, double *objective_out,
+                   int64_t *info_out);
+int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin,
+                           int64_t pos_end, double *ab_out, double *objective_out, int64_t *info_out);
+int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
+                           double *objective_out, int64_t *info_out);
+/* probs_out[i] = sigmoid(-(a x_i . w + b)); a or b not finite -> DSGD_ERR_INVALID.  On a SparseLogistic ctx (1, 0) returns
+ * the bits of dsgd_probabilities.  Works beside a running async loop, like dsgd_margins. */
+int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a, double b,
+                                  double *probs_out);
+/* Calibration quality at (a, b) over the rows whose z = a f + b is not NaN, with p = sigmoid(-z) and o = 1 for a positive row,
+ * 0 otherwise:  sums_out[0] = sum (p - o)^2 (Brier)   sums_out[1] = sum of -log p (o = 1) or -log(1 - p) (o = 0), as the
+ * stable softplus of the logistic loss;  n_bins (1 .. DSGD_CALIBRATION_MAX_BINS, else DSGD_ERR_INVALID) equal-width bins on
+ * [0, 1], bin = min(n_bins - 1, floor(p n_bins)): bin_rows[k] rows, bin_pos[k] positive rows, bin_psum[k] = sum p (n_bins
+ * entries each);  words_out[0] rows used, words_out[1] rows left out.  The counts are exact and the sums are added in fixed
+ * point: the same bits in any row order.  Works beside a running async loop. */
+#define DSGD_CALIBRATION_MAX_BINS 64
+int dsgd_eval_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a, double b,
+                          int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                          int64_t *words_out);
+int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                  int64_t pos_begin, int64_t pos_end, double a, double b, int32_t n_bins, double *sums_out,
+                                  int64_t *bin_rows, int64_t *bin_pos, double *bin_psum, int64_t *words_out);
+int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a, double b,
+                                  int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                  int64_t *words_out);
+
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
  *      (its own RPC), every rank calls dsgd_comm_init.  world == 1 needs neither. -------------------------- */
