@@ -169,7 +169,8 @@ struct dsgd_ctx {
   dev_buf<double> p_gbuf[3];   // K GPUs
   dev_buf<double2> p_rec[3];   // one GPU: rotating {W, g} records
   dev_buf<unsigned long long> p_acc;   // fixed-point accumulators of the per-CTA partials [3][kAccStride]
-  dev_buf<unsigned> p_hinge;
+  dev_buf<unsigned> p_hinge;   // one GPU: hinge count of every step and CTA [n_steps][CTAs]
+  dev_buf<double> p_loss_nrm;  // one GPU: the norms of every step's loss [2][n_steps]
   dev_buf<unsigned> p_bar;   // [0]: grid barrier counter, [1]: abort flag
   bool p_ready = false;
   dev_buf<long long> p_tl;   // debug timeline (DSGD_PERSIST_TIMELINE)
@@ -1490,7 +1491,10 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
         CU(cudaFuncSetAttribute(kPersistKernelsL1[a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
-  return ctx->p_hinge.grow(ctx, n_steps, 4096);
+  // sized for the largest grid (persist_grid), which dsgd_reserve does not know yet
+  int rc = ctx->p_hinge.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count);
+  if (rc) return rc;
+  return ctx->p_loss_nrm.grow(ctx, 2 * n_steps, 2 * 4096);
 }
 
 // CTAs of the persistent kernel: one per SM (fastest at batch 64, 256 and 1024 when it was
@@ -1564,11 +1568,11 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
   pp.wbuf[0] = ctx->p_wbuf[0]; pp.wbuf[1] = ctx->p_wbuf[1];
   for (int i = 0; i < 3; ++i) { pp.gbuf[i] = ctx->p_gbuf[i]; pp.rec[i] = ctx->p_rec[i]; }
   pp.d = ctx->d; pp.acc = ctx->p_acc; pp.bar = ctx->p_bar; pp.hinge = ctx->p_hinge; pp.losses = losses_dev;
+  pp.loss_nrm = ctx->p_loss_nrm;
   pp.w_out = ctx->w; pp.w32_out = ctx->w32; pp.scal = ctx->scal;
   pp.abort_flag = reinterpret_cast<int *>(ctx->p_bar + 1);
   CU(cudaMemsetAsync(ctx->p_acc, 0, sizeof(unsigned long long) * 3 * kAccStride, ctx->stream));
   pp.lambda = ctx->lambda; pp.lr = lr; pp.world = 1;
-  CU(cudaMemsetAsync(ctx->p_hinge, 0, sizeof(unsigned) * (size_t)n_steps, ctx->stream));
   CU(cudaMemsetAsync(ctx->p_bar, 0, sizeof(unsigned) * 4, ctx->stream));
   if (persist_timeline()) {
     if (!ctx->p_tl) CU(ctx->p_tl.alloc(kTlWords));

@@ -62,11 +62,14 @@ __device__ __forceinline__ void acc_push(unsigned long long *acc, double sd, dou
 __device__ __forceinline__ double acc_limb(unsigned long long q, int k) {
   return (double)(long long)q * __longlong_as_double((long long)(1023 - 160 + 40 * (k % kAccLimbs)) << 52);
 }
-// Called by a whole warp; all lanes return the two sums (identical in every CTA: integer additions commute).
-__device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane, double &sd, double &sn) {
-  unsigned long long q0 = 0, q1 = 0;
+// acc_read in two halves, so that a caller can put other loads into the same round trip: acc_load requests the words,
+// acc_sum waits for them and sums.
+__device__ __forceinline__ void acc_load(const unsigned long long *acc, int lane, unsigned long long &q0, unsigned long long &q1) {
+  q0 = 0; q1 = 0;
   if (lane < (kAccWords + 1) / 2)   // 6 lanes x 16 bytes = the 88-byte accumulator (and a pad word) in one request
     asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(q0), "=l"(q1) : "l"(acc + 2 * lane) : "memory");
+}
+__device__ __forceinline__ void acc_sum(unsigned long long q0, unsigned long long q1, int lane, double &sd, double &sn) {
   // Word k = 2 lane + h is limb k % 5 of sd (k < 5) or of sn (5 <= k < 10), worth 2^(40 (k % 5) - 160); every limb sum is
   // below 2^48 in magnitude, so its conversion and scaling are exact.  Each lane adds its own two words first, so the
   // sums take six shuffles: sd = (limbs 0+1 + limbs 2+3) + limb 4, sn = (limb 0 + limbs 1+2) + limbs 3+4.  Word 10 counts
@@ -82,18 +85,31 @@ __device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane
     sn = sd;
   }
 }
+// Called by a whole warp; all lanes return the two sums (identical in every CTA: integer additions commute).
+__device__ __forceinline__ void acc_read(const unsigned long long *acc, int lane, double &sd, double &sn) {
+  unsigned long long q0, q1;
+  acc_load(acc, lane, q0, q1);
+  acc_sum(q0, q1, lane, sd, sn);
+}
 // The persistent kernel's L1 form (kL1) keeps a third value in words kAccWords .. kAccWords + 4 of the same accumulator line,
-// its overflows counted in word 2 * kAccLimbs with the other two.  Called by a whole warp; all lanes return the sum.
-__device__ __forceinline__ double acc_read_l1(const unsigned long long *acc, int lane) {
-  unsigned long long q = 0;
+// its overflows counted in word 2 * kAccLimbs with the other two.  Split like acc_read: acc_load_l1 requests, acc_sum_l1 sums.
+__device__ __forceinline__ void acc_load_l1(const unsigned long long *acc, int lane, unsigned long long &q, unsigned long long &o) {
+  q = 0; o = 0;
   if (lane < kAccLimbs) asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(q) : "l"(acc + kAccWords + lane) : "memory");
+  if (lane == 0) asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(o) : "l"(acc + 2 * kAccLimbs) : "memory");
+}
+__device__ __forceinline__ double acc_sum_l1(unsigned long long q, unsigned long long o, int lane) {
   const double v = acc_limb(q, lane);
   const double v0 = __shfl_sync(0xffffffffu, v, 0), v1 = __shfl_sync(0xffffffffu, v, 1), v2 = __shfl_sync(0xffffffffu, v, 2);
   const double v3 = __shfl_sync(0xffffffffu, v, 3), v4 = __shfl_sync(0xffffffffu, v, 4);
   const double a = (((v4 + v3) + v2) + v1) + v0;   // from the top limb down
-  unsigned long long o = 0;
-  if (lane == 0) asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(o) : "l"(acc + 2 * kAccLimbs) : "memory");
   return __shfl_sync(0xffffffffu, o, 0) != 0ull ? __longlong_as_double(0x7ff8000000000000ll) : a;
+}
+// Called by a whole warp; all lanes return the sum.
+__device__ __forceinline__ double acc_read_l1(const unsigned long long *acc, int lane) {
+  unsigned long long q, o;
+  acc_load_l1(acc, lane, q, o);
+  return acc_sum_l1(q, o, lane);
 }
 
 // ---- one sum of many non-negative values (the logistic losses of a pass) -------------------------------------------------

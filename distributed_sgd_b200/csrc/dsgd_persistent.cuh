@@ -71,7 +71,7 @@ struct PersistParams {
   double2 *rec[3];  // one GPU: rotating records {W, g} per column; on entry all three = {W_init, 0}
   const double *d;
   unsigned long long *acc;  // [3 rotating][kAccStride]: fixed-point accumulators of {W.d, ||W||^2}; zero on entry
-  unsigned *hinge;  // [n_steps], zero on entry (one GPU)
+  unsigned *hinge;  // one GPU: [n_steps][gridDim.x], the hinge count of every step and CTA (every slot is stored)
   double *losses;   // [n_steps] or nullptr
   double *w_out;    // resident weights after the last step
   float *w32_out;
@@ -95,6 +95,8 @@ struct PersistParams {
   const double *lrs;                      // [n_steps]: step s of this launch uses lrs[s] instead of lr
   // ---- L1 penalty (kL1, one GPU); last for the same reason ----
   double lambda1;                         // every update is followed by soft_threshold(., lr * lambda1) on every column
+  // ---- one GPU with losses; last for the same reason ----
+  double *loss_nrm;                       // [2][n_steps]: ||W_t||^2, then (kL1) ||W_t||_1, of every step t of the launch
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -158,6 +160,9 @@ __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_re
 __device__ __forceinline__ void named_bar_sync(int id, int n_threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(int id, int n_threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
+}
 __device__ __forceinline__ long long global_ns() {
   long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -209,7 +214,7 @@ __device__ __forceinline__ double apply_update(double wv, double graw, double c,
 }
 
 // ---- grid barrier among the barrier-synchronised warps of every CTA (the producer warp stays out) -------------------
-// Called by thread 0 between two CTA-level bar.syncs: one RELEASE arrival on a counter, relaxed polling.
+// Called by one thread between two CTA-level barriers: one RELEASE arrival on a counter, relaxed polling.
 // There is no acquire fence after the poll.  What follows the barrier reads mutable global data only with instructions
 // that are served by L2 -- ld.global.cg / ld.relaxed.gpu / red / the LL words' ld.relaxed.sys -- never through L1, and a
 // thread cannot issue them before the branch on the polled value resolves, so they reach L2 after the arrival they
@@ -381,27 +386,41 @@ struct FetchLL {
   }
 };
 
+// The pairs of chunk c, 4 per lane (val 0 past the chunk's end: inert).
+template <int kMaxChunks>
+__device__ __forceinline__ void chunk_pairs(const StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, int c, int lane,
+                                            uint2 (&pr)[4]) {
+  const uint32_t off = mt.ch_off[c];
+  const int n = mt.ch_n[c];
+  const uint2 *src = (off & kChunkGlobal) ? (pairs + (off & ~kChunkGlobal)) : (ring + off);
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int k = u * 32 + lane;
+    pr[u] = (k < n) ? src[k] : make_uint2(0u, 0u);
+  }
+}
+
 // ---- the consumer warps' work on one stage: SlaveImpl.gradient's per-sample body (core/Slave.scala:147-153) ----
 // x.W per row (math/Vec.scala:58), prediction and hinge loss (SparseSVM.scala:14-16), gate (SparseSVM.scala:28),
 // RED of y*x into g (entry of column c at gbase + gstride * c).  A row that is ONE chunk (85 % of them) is gated and
 // scattered by the warp that computed its dot, from the registers that still hold its pairs; rows of several chunks
 // take a second pass after a barrier among the consumer warps (partials summed in chunk order).
+// pre (optional): the pairs of the warp's first chunk, already loaded with chunk_pairs
 template <int kCons, int kMaxChunks, class Fetch>
 __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, double *gbase,
-                                                  const int gstride, Fetch &fetch, int warp, int lane, long long *tl) {
+                                                  const int gstride, Fetch &fetch, int warp, int lane, long long *tl,
+                                                  const uint2 (*pre)[4] = nullptr) {
   const int n_ch = mt.n_chunks;
   unsigned hinge = 0;  // lane 0 only
   // ---- pass 1: dots of this warp's chunks ----
   for (int c = warp; c < n_ch; c += kCons) {
-    const uint32_t off = mt.ch_off[c];
-    const int n = mt.ch_n[c];
-    const uint2 *src = (off & kChunkGlobal) ? (pairs + (off & ~kChunkGlobal)) : (ring + off);
     uint2 pr[4];
     double wv[4];
+    if (pre && c == warp) {
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int k = u * 32 + lane;
-      pr[u] = (k < n) ? src[k] : make_uint2(0u, 0u);  // val 0: inert
+      for (int u = 0; u < 4; ++u) pr[u] = (*pre)[u];
+    } else {
+      chunk_pairs(mt, ring, pairs, c, lane, pr);
     }
     fetch.get4(pr, wv);
     double acc = 0.0;
@@ -655,6 +674,19 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     }
   }
 
+  // one GPU, consumer warps: the pairs of the warp's first chunk of the next step, loaded from the stage while the grid barrier
+  // is still pending (the stage does not depend on the weights), so that the interval starts with the gathers
+  uint2 pre[4];
+  auto prefetch = [&](int64_t tn) {
+    const int st = (int)tn & (kStages - 1);
+    const auto &mt = sm.meta[st];
+    mbar_wait(&sm.full[st], (unsigned)(((unsigned)tn / kStages) & 1u), p.abort_flag, p.timeout_cycles);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) pre[u] = make_uint2(0u, 0u);
+    if (warp < mt.n_chunks) chunk_pairs(mt, &sm.ring[st][0], p.pairs, warp, lane, pre);
+  };
+  if (!kMulti && is_cons && S > 0) prefetch(0);
+
   // rotating buffer indices kept as small integers (64-bit % 3 per warp and step is ~100 instructions on the critical path)
   int gi_prev = (int)((base + 2) % 3), gi_cur = (int)(base % 3), gi_next = (int)((base + 1) % 3);   // K GPUs: by global step
   int ti_prev = 2, ti_cur = 0, ti_next = 1;                                                          // by step of this launch
@@ -685,6 +717,16 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     }
     if (warp == 0) DSGD_TL(0);
 
+    // one GPU, update threads: g_{t-1} of the register columns, requested before anything else.  Update warp 0 then waits
+    // for these loads and the accumulator's below in ONE round trip (the accumulator's asm loads, "memory" clobbers, would
+    // otherwise hold them back until the accumulator had arrived: a second round trip before the CTA's partial is pushed).
+    double gv[kUpdCols];
+#pragma unroll
+    for (int i = 0; i < kUpdCols; ++i) {
+      const int j = u0 + i * n_upd;
+      gv[i] = (!kMulti && is_upd && j < p.dim) ? __ldcg(&Rprev[j].y) : 0.0;
+    }
+
     // ---- update warp 0, first thing: c_{T-1} and ||W_{T-1}||^2 from the partials the last barrier delivered ----
     if (warp == kCons && !first) {
       double c_prev, nrm_prev, l1_prev = 0.0;
@@ -692,23 +734,24 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
         c_prev = p.scal[kScalC];                              // W_base came from the host: k_prepare / previous launch
         nrm_prev = p.scal[kScalNrm2];
       } else {
+        unsigned long long q0, q1, ql = 0, ol = 0;
+        acc_load(acc_prev, lane, q0, q1);
+        if constexpr (kL1) acc_load_l1(acc_prev, lane, ql, ol);   // in the same round trip
         double sd, sn;
-        acc_read(acc_prev, lane, sd, sn);
+        acc_sum(q0, q1, lane, sd, sn);
         c_prev = p.lambda * 2.0 * sd;
         nrm_prev = sn;
-        if constexpr (kL1) l1_prev = acc_read_l1(acc_prev, lane);
+        if constexpr (kL1) l1_prev = acc_sum_l1(ql, ol, lane);
       }
       if (blockIdx.x == 0 && lane < (kL1 ? kAccStride : kAccWords)) acc_next[lane] = 0ull;
       if (lane == 0) {
         sm.c_val[t & 1] = c_prev;
         sm.nrm_val[t & 1] = nrm_prev;
         mbar_arrive(&sm.c_bar[t & 1]);
-        // one GPU: loss of step t-1 = lambda*||W_{t-1}||^2 + hinge_{t-1}/batch  (SparseSVM.scala:20-23; SURVEY.md F5)
+        // one GPU: the norms of the loss of step t-1, which is formed after the last step (epilogue)
         if (!kMulti && p.losses && blockIdx.x == 0) {
-          if constexpr (kL1)
-            p.losses[t - 1] = p.lambda * nrm_prev + p.lambda1 * l1_prev + (double)__ldcg(&p.hinge[t - 1]) / (double)B;
-          else
-            p.losses[t - 1] = p.lambda * nrm_prev + (double)__ldcg(&p.hinge[t - 1]) / (double)B;
+          p.loss_nrm[t - 1] = nrm_prev;
+          if constexpr (kL1) p.loss_nrm[S + t - 1] = l1_prev;
         }
       }
       __syncwarp();
@@ -919,13 +962,11 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       if (is_cons) {
         if (!last) {
           const int st = (int)t & (kStages - 1);
-          auto &mt = sm.meta[st];
-          mbar_wait(&sm.full[st], (unsigned)(((unsigned)t / kStages) & 1u), p.abort_flag, p.timeout_cycles);
-          if (warp == 0) DSGD_TL(1);
+          auto &mt = sm.meta[st];   // full: waited for by prefetch(t)
           FetchLocal<kL1> fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
           if constexpr (kL1) fetch.tau = tau;
           const unsigned hinge = consume_stage<kCons, kMaxChunks>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
-                                                                            lane, warp == 0 ? tl_row : nullptr);
+                                                                            lane, warp == 0 ? tl_row : nullptr, &pre);
           if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
           if (tl_rec && warp == 0 && lane == 0) tl_rec[2] = mt.n_pairs;
           __syncwarp();
@@ -936,13 +977,8 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
         // ---- update warps: W_t <- update(W_{t-1}, g_{t-1}, c_{t-1}).  A thread owns the same (up to kUpdCols) columns for
         //      the whole launch: their W and d stay in registers, only g_{t-1} is read (requested before c is waited
         //      for), and W_t is stored only into the record buffers that do not hold it yet (the three buffers after a
-        //      change), a g half is zeroed only if it was non-zero: most columns of a step cost one 8-byte load ----
-        double gv[kUpdCols];
-#pragma unroll
-        for (int i = 0; i < kUpdCols; ++i) {
-          const int j = u0 + i * n_upd;
-          gv[i] = (j < p.dim) ? __ldcg(&Rprev[j].y) : 0.0;
-        }
+        //      change), a g half is zeroed only if it was non-zero: most columns of a step cost one 8-byte load (gv,
+        //      requested at the top of the interval) ----
         mbar_wait(&sm.c_bar[t & 1], c_par, p.abort_flag, p.timeout_cycles);
         const double c_prev = *(volatile double *)&sm.c_val[t & 1];
         const bool add_c = (c_prev != 0.0) && (fabs(c_prev) > kEps);
@@ -987,9 +1023,16 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
 
     if (!ok) *(volatile int *)&sm.ok = 0;
     if (tl_row && lane == 0) sm.tl_warp[warp] = clock64();
-    named_bar_sync(3, kSyncThreads);
+    // Barrier 3: the CTA's work of the interval is done; only the thread that arrives at the grid barrier waits for it (one GPU:
+    // the consumers arrive and load the next step's first chunk meanwhile).  Barrier 4: the grid barrier has passed.
+    if (!kMulti && is_cons) {
+      named_bar_arrive(3, kSyncThreads);
+      if (t + 1 < S) prefetch(t + 1);
+    } else {
+      named_bar_sync(3, kSyncThreads);
+    }
     ++phase;
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == kCons * 32) {   // update warp 0, lane 0
       if (tl_row) {   // when the slowest consumer warp / update warp of CTA 0 reached the CTA barrier
         long long mc = 0, mu = 0;
         for (int i = 0; i < kCons; ++i) mc = max(mc, sm.tl_warp[i]);
@@ -997,13 +1040,12 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
         tl_row[13] = mc;
         tl_row[14] = mu;
       }
-      if (!last) {   // the CTA's hinge total (and, K GPUs, the step's sample count) ahead of the arrival
-        const unsigned h = sm.hinge_acc;
+      unsigned h = 0;
+      if (!last) {   // the CTA's hinge total; K GPUs add it and the step's sample count to the counter column before arriving
+        h = sm.hinge_acc;
         if constexpr (kMulti) {
           if (h) red_add_f64(&Gcur[p.dim], (double)h);
           if (blockIdx.x == 0) red_add_f64(&Gcur[p.dim], (double)B * 4294967296.0);
-        } else {
-          if (h) atomicAdd(&p.hinge[t], h);
         }
         sm.hinge_acc = 0u;
       }
@@ -1014,8 +1056,12 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       sm.ok = bar_ok ? 1 : 0;
       if (tl_rec) tl_rec[1] = global_ns();
       else if (tl_row) tl_row[7] = clock64();
+      // one GPU: the CTA's hinge count of step t into its own slot, zero included.  A plain store after the barrier: the
+      // release of this arrival does not wait for it (a count shared by all CTAs was one same-address atomic per CTA in front
+      // of every arrival), and the next one finds it long done.  Nothing reads it before the epilogue.
+      if (!kMulti && !last && p.losses) p.hinge[(size_t)t * G + blockIdx.x] = h;
     }
-    named_bar_sync(3, kSyncThreads);
+    named_bar_sync(4, kSyncThreads);
     if (*(volatile int *)&sm.ok == 0) return;
     if constexpr (kLrTable) lr = lr_next;
     { const int a = gi_prev; gi_prev = gi_cur; gi_cur = gi_next; gi_next = a; }
@@ -1032,6 +1078,24 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       p.scal[kScalC] = p.lambda * 2.0 * sd;
       p.scal[kScalNrm2] = sn;
       if constexpr (kL1) p.scal[kScalL1] = l1;
+    }
+  }
+  // one GPU: loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + hinge_s/batch (SparseSVM.scala:20-23; SURVEY.md F5), one
+  // warp per step.  The hinge count is the integer sum of the CTAs' slots, the same in any order.  Every slot and norm was
+  // stored before the last barrier's arrivals, and is read through L2 (see grid_barrier_arrive_wait).
+  if constexpr (!kMulti) {
+    if (p.losses) {
+      for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
+        unsigned h = 0;
+        for (int b = lane; b < G; b += 32) h += __ldcg(&p.hinge[s * G + b]);
+        h = __reduce_add_sync(0xffffffffu, h);
+        if (lane == 0) {
+          if constexpr (kL1)
+            p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + p.lambda1 * __ldcg(&p.loss_nrm[S + s]) + (double)h / (double)B;
+          else
+            p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + (double)h / (double)B;
+        }
+      }
     }
   }
   if constexpr (kMulti) {
