@@ -167,6 +167,9 @@ class Master:
                  jvm_exact: bool = False, attach: bool = True):
         self.node, self.model, self.expected_node_count = node, model, expected_node_count
         self.logistic = isinstance(model, SparseLogistic)
+        # (w_pos, w_neg) as the Slave resolved and installed them; (1, 1): every evaluation makes the calls it made before
+        self.class_weight = getattr(slave, "class_weight", (1.0, 1.0))
+        self.weighted = self.class_weight != (1.0, 1.0)
         self.n_train, self.n_test = data.n_rows, test_data.n_rows
         self.dim = data.dim
         self.slave = slave
@@ -205,8 +208,18 @@ class Master:
     # ---- evaluation ------------------------------------------------------------------------------------
     def _local_eval(self, call: str, *args):
         """(loss sum, correct count, ||w||^2) of this rank's share: ctx.<call>_counts for the SVM (its loss sum is the
-        integer hinge sum), ctx.<call>_sums for SparseLogistic."""
+        integer hinge sum), ctx.<call>_sums for SparseLogistic.  With class weights ctx.<call>_class, and a fourth value:
+        (loss sum of the positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted."""
+        if self.weighted:
+            ce = getattr(self.ctx, call + "_class")(*args)
+            as_sum = float if self.logistic else int   # the SVM's sums are integers: all-reduced exactly
+            return as_sum(ce.loss_pos), ce.correct_pos + ce.correct_neg, ce.norm_squared, as_sum(ce.loss_neg)
         return getattr(self.ctx, call + ("_sums" if self.logistic else "_counts"))(*args)
+
+    def _loss_sum(self, h, *h_neg):
+        """The loss sum of an evaluation from its combined totals: h itself, or with class weights w_pos * h + w_neg * h_neg,
+        formed once from the totals of all ranks."""
+        return self.class_weight[0] * h + self.class_weight[1] * h_neg[0] if h_neg else h
 
     def _combine(self, h, c, n2, *rows):
         """(loss sum, correct[, rows], ||w||^2) over all ranks; ||w||^2 is identical on every rank that evaluated and 0 on idle
@@ -238,11 +251,11 @@ class Master:
         n = end - begin
         lo, hi = begin + (n * r) // W, begin + (n * (r + 1)) // W
         if hi > lo:
-            h, c, n2 = self._local_eval("eval", lo, hi, weights)
+            h, c, n2, *h_neg = self._local_eval("eval", lo, hi, weights)
         else:
-            h, c, n2 = 0, 0, 0.0
-        hs, cs, n2 = self._combine(h, c, n2)
-        return self._penalty(n2, weights, want_loss) + hs / n, cs / n
+            h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
+        hs, cs, *h_neg, n2 = self._combine(h, c, n2, *h_neg)
+        return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / n, cs / n
 
     def local_loss(self, weights=None, test_data: bool = False) -> float:
         """Master.localLoss (core/Master.scala:105-107)."""
@@ -283,13 +296,13 @@ class Master:
             return None
         lo, hi = sample_shard(k, self.group.world, self.group.rank)
         if hi <= lo:
-            h, c, n2 = 0, 0, 0.0
+            h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
         elif ids is None:
-            h, c, n2 = self._local_eval("eval_sampled", b, e, key, lo, hi, weights)
+            h, c, n2, *h_neg = self._local_eval("eval_sampled", b, e, key, lo, hi, weights)
         else:
-            h, c, n2 = self._local_eval("eval_samples", ids[lo:hi], weights)
-        hs, cs, n2 = self._combine(h, c, n2)
-        return self._penalty(n2, weights, want_loss) + hs / k, cs / k
+            h, c, n2, *h_neg = self._local_eval("eval_samples", ids[lo:hi], weights)
+        hs, cs, *h_neg, n2 = self._combine(h, c, n2, *h_neg)
+        return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / k, cs / k
 
     def local_sampled_loss(self, weights, samples_count: int, test_data: bool = False) -> float:
         """Master.localSampledLoss (core/Master.scala:109-112).  An empty sample raises DsgdEmpty, as the reference's
@@ -307,6 +320,35 @@ class Master:
         if r is None:
             raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
         return r
+
+    # ---- per-class report (extension) -------------------------------------------------------------------------------------
+    # Like the ranking metrics below it is not sharded: every rank holds every row and evaluates the whole range or sample,
+    # and the counts are exact integers, so every rank returns the same numbers without a collective.
+    def _class_report(self, ce, weights) -> dict:
+        nan = float("nan")
+        n = ce.n_pos + ce.n_neg
+        rec_pos = ce.correct_pos / ce.n_pos if ce.n_pos else nan
+        rec_neg = ce.correct_neg / ce.n_neg if ce.n_neg else nan
+        pen = self._penalty(ce.norm_squared, weights, True)
+        return {"n_pos": ce.n_pos, "n_neg": ce.n_neg, "correct_pos": ce.correct_pos, "correct_neg": ce.correct_neg,
+                "recall_pos": rec_pos, "recall_neg": rec_neg, "balanced_accuracy": (rec_pos + rec_neg) / 2.0,
+                "accuracy": (ce.correct_pos + ce.correct_neg) / n, "class_weight": self.class_weight,
+                "loss": pen + (ce.loss_pos + ce.loss_neg) / n,
+                "weighted_loss": pen + ce.weighted_loss_sum(*self.class_weight) / n}
+
+    def local_class_report(self, weights=None, test_data: bool = False) -> dict:
+        """Rows, correct predictions and recall per class, balanced accuracy, accuracy, and the loss both unweighted and
+        under the model's class weights, over the train (or test) rows; works whatever the weights are."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return self._class_report(self.ctx.eval_class(b, e, weights), weights)
+
+    def local_sampled_class_report(self, weights, samples_count: int, test_data: bool = False) -> dict:
+        """local_class_report on a fresh sample (_draw_sample).  An empty sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
+        ce = self.ctx.eval_sampled_class(b, e, key, 0, k, weights) if ids is None else self.ctx.eval_samples_class(ids, weights)
+        return self._class_report(ce, weights)
 
     # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
     # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank
@@ -410,11 +452,11 @@ class Master:
         groups = split_strategy(self.n_train, self.group.world)
         mine = groups[self.group.rank] if self.group.rank < len(groups) else range(0)
         if len(mine):
-            h, c, n2 = self._local_eval("eval", mine.start, mine.stop, weights)
+            h, c, n2, *h_neg = self._local_eval("eval", mine.start, mine.stop, weights)
         else:
-            h, c, n2 = 0, 0, 0.0
-        hs, cs, ns, n2 = self._combine(h, c, n2, len(mine))
-        return self._penalty(n2, weights, want_loss) + hs / ns, cs / ns
+            h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
+        hs, cs, ns, *h_neg, n2 = self._combine(h, c, n2, len(mine), *h_neg)
+        return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / ns, cs / ns
 
 
 class MasterSync(Master):
@@ -571,6 +613,9 @@ class MasterAsync(Master):
             raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+        from ..ml.class_weight import resolve_class_weight
+        if resolve_class_weight(getattr(model, "class_weight", None), data.label) != (1.0, 1.0):   # as the Slave decides
+            raise ValueError("class_weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
         super().__init__(node, data, test_data, model, expected_node_count, **kw)
 
     def _attach_replicas(self):

@@ -11,6 +11,7 @@ from typing import Optional, Sequence, Union
 
 import numpy as np
 
+from ..ml.class_weight import resolve_class_weight
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import NativeCtx
@@ -35,6 +36,11 @@ class Slave:
             raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1 and is_async:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+        # (w_pos, w_neg) of the model's class_weight; "balanced" counts the labels of the train rows
+        self.class_weight = resolve_class_weight(getattr(model, "class_weight", None), data.label)
+        weighted = self.class_weight != (1.0, 1.0)
+        if weighted and is_async:
+            raise ValueError("class_weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
         self.node, self.master, self.model, self.is_async, self.world = node, master, model, is_async, world
         self.n_train = data.n_rows
         self.n_test = test_data.n_rows if test_data is not None else 0
@@ -49,6 +55,8 @@ class Slave:
                 model.dim_sparsity = ctx.compute_dim_sparsity(self.n_train)
             if model.l1:
                 ctx.set_l1(model.l1)
+            if weighted:
+                ctx.set_class_weights(*self.class_weight)
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
                              is_async=is_async, logistic=logistic)
@@ -66,6 +74,8 @@ class Slave:
             self.ctx.set_dim_sparsity(model.dim_sparsity)
         if model.l1:
             self.ctx.set_l1(model.l1)
+        if weighted:
+            self.ctx.set_class_weights(*self.class_weight)
 
     def stop(self):  # Slave.stop (core/Slave.scala:68-77): releases the device context
         self.ctx.close()

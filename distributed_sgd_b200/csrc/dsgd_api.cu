@@ -105,6 +105,7 @@ struct dsgd_ctx {
   int32_t dim = 0;
   double lambda = 0.0;
   double lambda1 = 0.0;   // dsgd_set_l1: the L1 penalty of the sync steps (0: off)
+  double cw_pos = 1.0, cw_neg = 1.0;   // dsgd_set_class_weights: the weights of the y = +1 and y = -1 rows
   int rank = 0, world = 1;
   uint32_t flags = 0;
   int sm_count = 0;
@@ -131,6 +132,7 @@ struct dsgd_ctx {
   dev_buf<unsigned long long> cnt;
   dev_buf<double> partial;  // 2 doubles per k_update block
   dev_buf<double> out2;     // loss, acc, hinge sum, correct count, ||w||^2
+  dev_buf<double> cls_out;  // dsgd_eval*_class: ||w||^2, the two loss sums, correct and rows per class (k_class_fold)
   dev_buf<double> gsum;     // master-side running sum of worker replies (dim + 2)
   std::vector<int32_t> worker_counts;  // logical workers on this ctx (empty: one worker, whole slice)
   int32_t n_local = 1, k_total = 0;    // k_total == 0: world
@@ -313,6 +315,8 @@ static void profiled(dsgd_ctx *ctx, F &&launch) {
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
+// the class-weighted kernels run only with weights other than (1, 1)
+static inline bool class_weighted(const dsgd_ctx *ctx) { return !(ctx->cw_pos == 1.0 && ctx->cw_neg == 1.0); }
 
 // every id names a loaded row (the reference indexes its data array with it); fn is the entry point
 static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn, const char *what) {
@@ -380,7 +384,7 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
       (rc = zeroed(ctx->w32, (int64_t)dim + 4, "w32")) || (rc = zeroed(ctx->w32_req, (int64_t)dim + 4, "w32_req")) ||
       (rc = zeroed(ctx->n_exact, 2, "n_exact")) || (rc = zeroed(ctx->scal, kNumScal, "scal")) ||
       (rc = zeroed(ctx->cnt, kNumCnt, "cnt")) || (rc = zeroed(ctx->partial, 2 * (int64_t)cdiv(dim, 256), "partial")) ||
-      (rc = zeroed(ctx->out2, 8, "out2")) || (rc = zeroed(ctx->gsum, nv, "gsum")))
+      (rc = zeroed(ctx->out2, 8, "out2")) || (rc = zeroed(ctx->cls_out, 8, "cls_out")) || (rc = zeroed(ctx->gsum, nv, "gsum")))
     return rc;
   if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) return bail("init memset", e);
   *out = ctx;
@@ -400,13 +404,13 @@ extern "C" const char *dsgd_last_error(const dsgd_ctx *ctx) { return ctx ? ctx->
 
 extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   if (!ctx) return "{}";
-  char buf[512];
+  char buf[640];
   snprintf(buf, sizeof buf,
            "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
-           "\"model\": \"%s\", \"lambda1\": %.17g}",
+           "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g]}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
-           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1);
+           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1, ctx->cw_pos, ctx->cw_neg);
   ctx->info = buf;
   return ctx->info.c_str();
 }
@@ -678,7 +682,7 @@ static bool stream_eligible(const dsgd_ctx *ctx, int64_t n) {
   return n >= kStreamMinRows && stream_smem_bytes(ctx->dim) + 1024 <= 227u * 1024u;
 }
 
-template <bool kScatter, bool kPreds, bool kContig>
+template <bool kScatter, bool kPreds, bool kContig, bool kCls = false>
 static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_begin, int64_t n, const double *w_dev,
                          const float *w32_dev, double *g, double *preds) {
   const size_t smem = stream_smem_bytes(ctx->dim);
@@ -687,6 +691,9 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
     CU(cudaFuncSetAttribute(k_stream_rows<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU(cudaFuncSetAttribute(k_stream_rows<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU(cudaFuncSetAttribute(k_stream_rows<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     ctx->stream_ready = true;
   }
   NEED(kContig == (samples_dev == nullptr), DSGD_ERR_INVALID, "stream_launch: sample list / row range mismatch");
@@ -695,6 +702,7 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
   sp.rp16 = ctx->rp16; sp.units = reinterpret_cast<const uint4 *>(ctx->pairs.p); sp.yabs = ctx->yabs;
   sp.samples = samples_dev; sp.row_begin = row_begin; sp.n = n;
   sp.w = w_dev; sp.w32 = w32_dev; sp.dim = ctx->dim;
+  sp.w_pos = ctx->cw_pos; sp.w_neg = ctx->cw_neg;
   sp.g = g; sp.preds = preds; sp.cnt = ctx->cnt; sp.n_exact = ctx->n_exact; sp.next_block = ctx->n_exact + 1;
   CU(cudaMemsetAsync(ctx->n_exact + 1, 0, sizeof(unsigned long long), ctx->stream));
   // rows per block (the unit of the dynamic work distribution): 32, or fewer when that leaves a warp fewer than ~6 blocks
@@ -706,7 +714,7 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
   sp.n_big = sp.tail_log2 < sp.rows_log2 ? ((n - n / 5) >> sp.rows_log2) : ((n + (1 << sp.rows_log2) - 1) >> sp.rows_log2);
   const int64_t n_blk = sp.n_big + cdiv(std::max<int64_t>(0, n - (sp.n_big << sp.rows_log2)), (int64_t)1 << sp.tail_log2);
   const int grid = (int)std::min<int64_t>(ctx->sm_count, std::max<int64_t>(1, cdiv(n_blk, kStreamThreads / 32)));
-  profiled(ctx, [&] { k_stream_rows<kScatter, kPreds, kContig><<<grid, kStreamThreads, smem, ctx->stream>>>(sp); });
+  profiled(ctx, [&] { k_stream_rows<kScatter, kPreds, kContig, kCls><<<grid, kStreamThreads, smem, ctx->stream>>>(sp); });
   LAUNCHED();
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -820,6 +828,29 @@ static void launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, dou
   LAUNCHED();
 }
 
+// The class-aware row kernel (k_rows_class, or the streaming pass's per-class form) over `rows`, then k_class_fold: with out == nullptr the batch's class-weighted
+// loss sum and correct count are left in cnt for a weighted tail (kCw), else the per-class totals and *nrm go to out.
+// w32 != nullptr (a request): the SVM's pass over kStreamMinRows rows or more is the per-class form of the fp32 streaming pass.
+template <int kModel, bool kScatter>
+static int launch_rows_class(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, const double *nrm = nullptr,
+                             double *out = nullptr, const float *w32 = nullptr) {
+  bool streamed = false;
+  if constexpr (kModel == kSvm) streamed = w32 && stream_eligible(ctx, rows.n);
+  if constexpr (kModel == kSvm) if (streamed) {
+    int rc = rows.ids ? stream_launch<kScatter, false, false, true>(ctx, rows.ids, 0, rows.n, w, w32, g, nullptr)
+                      : stream_launch<false, false, true, true>(ctx, nullptr, rows.row_begin, rows.n, w, w32, nullptr, nullptr);
+    if (rc) return rc;
+  }
+  if (!streamed) {
+    k_rows_class<kModel, kScatter><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+        ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, ctx->cnt, ctx->cw_pos, ctx->cw_neg);
+    LAUNCHED();
+  }
+  k_class_fold<kModel><<<1, 1, 0, ctx->stream>>>(ctx->cnt, ctx->cw_pos, ctx->cw_neg, nrm, out);
+  LAUNCHED();
+  return DSGD_OK;
+}
+
 // The row kernel of a request: the fp32 streaming pass over kStreamMinRows rows or more (SVM only: it decides signs, and
 // the logistic loss needs the dot's value), else launch_rows.  Only an evaluation names a range of rows; a gradient or a
 // forward pass always lists them.
@@ -838,11 +869,21 @@ static int request_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, con
 // cleared for the next pass (k_loss_scalar).
 template <int kModel, bool kScatter>
 static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
-  const double *w, *c, *nrm;
-  const float *w32;
+  const double *w = nullptr, *c = nullptr, *nrm = nullptr;
+  const float *w32 = nullptr;
   int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
-  if (rc || (rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr))) return rc;
+  if (rc) return rc;
   const double n = (double)rows.n;
+  if (kScatter && class_weighted(ctx)) {   // a gradient of a class-weighted model: the fp64 class kernel at any size
+    if ((rc = launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32))) return rc;
+    k_finish_cw<kModel><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+    LAUNCHED();
+    k_loss_scalar_cw<kModel><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    return DSGD_OK;
+  }
+  if ((rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr))) return rc;
   if constexpr (kScatter) {
     const int fin_blocks = cdiv(ctx->dim + 1, 256);
     if constexpr (kModel == kLogistic) k_finish_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
@@ -984,6 +1025,52 @@ extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int3
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+}
+
+// One per-class evaluation pass over `rows` (dsgd_eval*_class): k_rows_class without the scatter, then k_class_fold
+static int class_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *norm_squared, double *loss_sums,
+                      int64_t *counts) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  const float *w32 = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd, &w32);
+  if (rc) return rc;
+  if ((rc = is_logistic(ctx) ? launch_rows_class<kLogistic, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out, w32)
+                             : launch_rows_class<kSvm, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out, w32)))
+    return rc;
+  CU(cudaGetLastError());
+  double out[7];
+  CU(cudaMemcpyAsync(out, ctx->cls_out, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (norm_squared) *norm_squared = out[0];
+  if (loss_sums) { loss_sums[0] = out[1]; loss_sums[1] = out[2]; }
+  if (counts)
+    for (int k = 0; k < 4; ++k) counts[k] = (int64_t)out[3 + k];
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
+                               double *loss_sums_out, int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+}
+
+extern "C" int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                       int64_t pos_begin, int64_t pos_end, double *norm_squared, double *loss_sums_out,
+                                       int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+}
+
+extern "C" int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                       double *norm_squared, double *loss_sums_out, int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
 }
 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
@@ -1467,6 +1554,14 @@ static void *const kPersistKernels[2][2][2] = {
 static void *const kPersistKernelsL1[2][2] = {
     {(void *)DSGD_PERSIST_KERNEL_L1(false, false), (void *)DSGD_PERSIST_KERNEL_L1(false, true)},
     {(void *)DSGD_PERSIST_KERNEL_L1(true, false), (void *)DSGD_PERSIST_KERNEL_L1(true, true)}};
+// the one-GPU class-weighted forms (dsgd_set_class_weights), indexed [l1][avg][lr_table]
+#define DSGD_PERSIST_KERNEL_CW(avg, lr_table, l1) \
+  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, false, avg, lr_table, l1, true>
+static void *const kPersistKernelsCw[2][2][2] = {
+    {{(void *)DSGD_PERSIST_KERNEL_CW(false, false, false), (void *)DSGD_PERSIST_KERNEL_CW(false, true, false)},
+     {(void *)DSGD_PERSIST_KERNEL_CW(true, false, false), (void *)DSGD_PERSIST_KERNEL_CW(true, true, false)}},
+    {{(void *)DSGD_PERSIST_KERNEL_CW(false, false, true), (void *)DSGD_PERSIST_KERNEL_CW(false, true, true)},
+     {(void *)DSGD_PERSIST_KERNEL_CW(true, false, true), (void *)DSGD_PERSIST_KERNEL_CW(true, true, true)}}};
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -1489,6 +1584,10 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
     for (int a = 0; a < 2; ++a)
       for (int l = 0; l < 2; ++l)
         CU(cudaFuncSetAttribute(kPersistKernelsL1[a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    for (int m = 0; m < 2; ++m)
+      for (int a = 0; a < 2; ++a)
+        for (int l = 0; l < 2; ++l)
+          CU(cudaFuncSetAttribute(kPersistKernelsCw[m][a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
   // sized for the largest grid (persist_grid), which dsgd_reserve does not know yet
@@ -1617,6 +1716,9 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
   pp.lambda1 = l1 ? ctx->lambda1 : 0.0;
   void *fn = l1 ? kPersistKernelsL1[ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0]
                 : kPersistKernels[multi ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
+  // the class-weighted forms only with weights other than (1, 1) (never fused: sync_staged keeps such a ctx off that path)
+  pp.w_pos = ctx->cw_pos; pp.w_neg = ctx->cw_neg;
+  if (!multi && class_weighted(ctx)) fn = kPersistKernelsCw[l1 ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
   CU(launch_err);
@@ -1772,7 +1874,8 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
 
 // The per-step path of sync_staged for model kModel: n_steps steps of n_per_step staged ids from smp, step s at the rate
 // lrs[s] (lrs == nullptr: lr), its loss into losses[s] (losses == nullptr: none)
-template <int kModel>
+// kCw: a class-weighted ctx -- every worker's pass is k_rows_class + k_class_fold, and the tails read the weighted loss sum
+template <int kModel, bool kCw>
 static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, int64_t n_steps, double lr,
                          const double *lrs, double *losses, bool single, int32_t k_total) {
   const int upd_blocks = cdiv(ctx->dim, 256);
@@ -1800,22 +1903,30 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     if (ctx->avg_on) ++ctx->avg_n;
   };
 
+  auto rows_pass = [&](const row_set &rows) {
+    if constexpr (kCw) launch_rows_class<kModel, true>(ctx, rows, ctx->w, ctx->g);
+    else launch_rows<kModel, true>(ctx, rows, ctx->w, ctx->g);
+  };
+
   for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
     if (lrs) lr_s = lrs[s];
     double *loss_dev = losses ? losses + s : nullptr;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
-      profiled(ctx, [&] { launch_rows<kModel, true>(ctx, {smp, 0, n_per_step}, ctx->w, ctx->g); });
-      update(k_update<true, kModel>, k_update_avg<true, kModel>, k_update_l1<true, kModel>, k_update_avg_l1<true, kModel>,
-             ctx->g, 1.0, (double)n_per_step, loss_dev);
+      profiled(ctx, [&] { rows_pass({smp, 0, n_per_step}); });
+      update(k_update<true, kModel, kCw>, k_update_avg<true, kModel, kCw>, k_update_l1<true, kModel, kCw>,
+             k_update_avg_l1<true, kModel, kCw>, ctx->g, 1.0, (double)n_per_step, loss_dev);
       continue;
     }
     // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
     int64_t off = 0;
     for (int32_t v = 0; v < ctx->n_local; ++v) {
       const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
-      profiled(ctx, [&] { launch_rows<kModel, true>(ctx, {smp + off, 0, nv}, ctx->w, ctx->g); });
-      if constexpr (kModel == kLogistic)
+      profiled(ctx, [&] { rows_pass({smp + off, 0, nv}); });
+      if constexpr (kCw)
+        k_finish_acc_cw<kModel><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
+                                                                     (double)nv, v == 0 ? 1 : 0);
+      else if constexpr (kModel == kLogistic)
         k_finish_acc_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
                                                                    (double)nv, v == 0 ? 1 : 0);
       else
@@ -1827,8 +1938,8 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
     if (ctx->world > 1)
       NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    update(k_update<false, kModel>, k_update_avg<false, kModel>, k_update_l1<false, kModel>, k_update_avg_l1<false, kModel>,
-           ctx->gsum, (double)k_total, 0.0, loss_dev);
+    update(k_update<false, kModel, kCw>, k_update_avg<false, kModel, kCw>, k_update_l1<false, kModel, kCw>,
+           k_update_avg_l1<false, kModel, kCw>, ctx->gsum, (double)k_total, 0.0, loss_dev);
   }
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -1868,7 +1979,11 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
        "dsgd_sync_steps: the logistic model takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
   NEED(!l1 || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
        "dsgd_sync_steps: the L1 penalty takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
-  const bool fused = !logistic && !l1 && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
+  // Class weights have no form in the fused kernel: with world > 1 a weighted ctx takes the per-step path over NCCL.
+  const bool cw = class_weighted(ctx);
+  NEED(!cw || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
+       "dsgd_sync_steps: class weights take the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
+  const bool fused = !logistic && !l1 && !cw && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
                      persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step));
   // Ranks wired with the peer exchange only have no communicator for the step-by-step path below: refuse before anything
   // is launched instead of reaching the allreduce without one.
@@ -1890,8 +2005,11 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   }
   const int32_t *smp = ctx->samples + first;
   double *loss_dev = want_losses ? ctx->losses.p : nullptr;
-  return logistic ? sync_per_step<kLogistic>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
-                  : sync_per_step<kSvm>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
+  if (cw)
+    return logistic ? sync_per_step<kLogistic, true>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
+                    : sync_per_step<kSvm, true>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
+  return logistic ? sync_per_step<kLogistic, false>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
+                  : sync_per_step<kSvm, false>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
 }
 
 extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,
@@ -1956,6 +2074,26 @@ extern "C" int dsgd_set_l1(dsgd_ctx *ctx, double lambda1) {
     CU(cudaGetLastError());
   }
   ctx->lambda1 = lambda1;
+  return DSGD_OK;
+}
+
+// ---- class weights of the sync steps and of dsgd_gradient ------------------------------------------------------------------
+
+extern "C" int dsgd_set_class_weights(dsgd_ctx *ctx, double w_pos, double w_neg) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE,
+       "dsgd_set_class_weights: ctx is in async mode (class weights belong to the sync paths)");
+  NEED(std::isfinite(w_pos) && w_pos >= 0.0 && std::isfinite(w_neg) && w_neg >= 0.0, DSGD_ERR_INVALID,
+       "dsgd_set_class_weights: weights must be finite and >= 0 (got %g, %g)", w_pos, w_neg);
+  ctx->cw_pos = w_pos;
+  ctx->cw_neg = w_neg;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_get_class_weights(const dsgd_ctx *ctx, double *w_pos_out, double *w_neg_out) {
+  if (!ctx || !w_pos_out || !w_neg_out) return DSGD_ERR_INVALID;
+  *w_pos_out = ctx->cw_pos;
+  *w_neg_out = ctx->cw_neg;
   return DSGD_OK;
 }
 

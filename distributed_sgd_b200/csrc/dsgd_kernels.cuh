@@ -35,25 +35,38 @@ enum Cnt : int {
   kCntHinge = 0,    // sum of per-sample hinge losses of the running batch (integers: 0, 1 or 2 each)
   kCntCorrect = 1,  // #{pred == y}
   kCntTicket = 2,   // last-block ticket of k_update
+  kCntWLoss = 3,    // class-weighted batch: the bits of the double w_pos * L_pos + w_neg * L_neg (k_class_fold), which the
+                    // weighted tails (kCw) read instead of kCntHinge / kCntLoss
   kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
   kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update_l1, k_l1_norm; zero between launches
   kCntNnz = 23,     // #{w_j != 0} of k_l1_norm; zero between launches
-  kNumCnt = 24
+  // per-class counters of k_rows_class, cleared by k_class_fold: index 0 is the class y = +1, index 1 the class y = -1
+  kCntClassN = 24,        // rows
+  kCntClassCorrect = 26,  // #{pred == y}
+  kCntClassHinge = 28,    // SVM: hinge sums (integers)
+  kCntClassLoss = 32,     // logistic: two fixed-point sums of the unweighted losses, kLossAccWords words each
+  kNumCnt = 48
 };
-static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kCntNnz && kCntNnz < kNumCnt,
+static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kCntNnz && kCntNnz < kCntClassN &&
+                  kCntClassLoss + 2 * kLossAccWords <= kNumCnt,
               "counter block");
 
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
 constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
 constexpr int kLogistic = 1;   // SparseLogistic: softplus loss, gradient x * (y * sigmoid(y * x.w))
 
-// Sum of the per-sample losses of the running batch or pass, and its reset
-template <int kModel>
+// Sum of the per-sample losses of the running batch or pass, and its reset.  kCw: the class-weighted sum of k_class_fold.
+template <int kModel, bool kCw = false>
 __device__ __forceinline__ double batch_loss_sum(const unsigned long long *cnt) {
+  if (kCw) return __longlong_as_double((long long)cnt[kCntWLoss]);
   return kModel == kLogistic ? acc_value(cnt + kCntLoss) : (double)cnt[kCntHinge];
 }
-template <int kModel>
+template <int kModel, bool kCw = false>
 __device__ __forceinline__ void clear_batch_loss(unsigned long long *cnt) {
+  if (kCw) {
+    cnt[kCntWLoss] = 0ull;
+    return;
+  }
   cnt[kCntHinge] = 0ull;
   if (kModel == kLogistic)
 #pragma unroll
@@ -314,11 +327,121 @@ __global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restric
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Class weights (dsgd_set_class_weights).  k_rows_class is the row kernel of either model with one weight per class: the dot,
+// the prediction, the SVM's gate and the unweighted per-sample loss are those of k_rows / k_rows_logistic; the scatter value
+// is scaled by the weight of the row's class,
+//   SVM       s = y * w_y          (an exact sign flip of w_y),  added where !(y * dot < 0)
+//   logistic  s = (y * sigmoid(z)) * w_y
+// then filt(filt(x_j) * s) per entry as before, so w_y = 0 adds nothing.  Lane 0 counts rows, correct predictions and the
+// loss per class: the SVM's hinge sums are integers, the logistic sums two fixed-point limb blocks (a row adds its loss to
+// its class's block and an exact 0 to the other), so every per-class total is the same in any order.  kScatter = false is
+// the pass of dsgd_eval*_class, which does not read the weights.
+// k_class_fold, one thread after the pass: L = fl(fl(w_pos * L_pos) + fl(w_neg * L_neg)) into cnt[kCntWLoss] and the correct
+// total into cnt[kCntCorrect] for the weighted tails (out == nullptr), or the per-class totals and ||w||^2 into out[0..6]
+// (an evaluation); the per-class words are cleared either way.
+// ---------------------------------------------------------------------------------------------------
+template <int kModel, bool kScatter>
+__global__ void __launch_bounds__(256) k_rows_class(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                    const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                    int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                    double *__restrict__ g, unsigned long long *__restrict__ cnt,
+                                                    double w_pos, double w_neg) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned n_pos = 0, n_neg = 0, ok_pos = 0, ok_neg = 0, h_pos = 0, h_neg = 0;  // lane 0 only
+  unsigned long long lim_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_pos = 0, ovf_neg = 0;
+  for (int64_t i = warp0; i < n; i += nwarps) {
+    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
+    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
+    const int yi = (int)label[r];
+    const bool pos = yi > 0;
+    const double y = (double)yi;
+    const double z = y * dot;
+    if (lane == 0) {
+      const int p = pred_of(dot);
+      const unsigned ok = (unsigned)(p == yi);
+      if (pos) { ++n_pos; ok_pos += ok; } else { ++n_neg; ok_neg += ok; }
+      if (kModel == kLogistic) {
+        const double l = softplus(z);
+        acc_add_local(lim_pos, ovf_pos, pos ? l : 0.0);
+        acc_add_local(lim_neg, ovf_neg, pos ? 0.0 : l);
+      } else {
+        const unsigned l = (unsigned)(1 - yi * p);
+        if (pos) h_pos += l; else h_neg += l;
+      }
+    }
+    if (kScatter) {
+      const double wy = pos ? w_pos : w_neg;
+      double s;
+      if (kModel == kLogistic) {
+        s = (y * sigmoid(z)) * wy;
+      } else {
+        if (z < 0.0) continue;  // SparseSVM.scala:28
+        s = pos ? wy : -wy;
+      }
+      for (int64_t k = b + lane; k < e; k += 32) {
+        const uint2 pr = pairs[k];
+        const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);
+        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
+      }
+    }
+  }
+  if (lane == 0) {
+    if (n_pos) atomicAdd(&cnt[kCntClassN], (unsigned long long)n_pos);
+    if (n_neg) atomicAdd(&cnt[kCntClassN + 1], (unsigned long long)n_neg);
+    if (ok_pos) atomicAdd(&cnt[kCntClassCorrect], (unsigned long long)ok_pos);
+    if (ok_neg) atomicAdd(&cnt[kCntClassCorrect + 1], (unsigned long long)ok_neg);
+    if (kModel == kLogistic) {
+      acc_flush_local(cnt + kCntClassLoss, lim_pos, ovf_pos);
+      acc_flush_local(cnt + kCntClassLoss + kLossAccWords, lim_neg, ovf_neg);
+    } else {
+      if (h_pos) atomicAdd(&cnt[kCntClassHinge], (unsigned long long)h_pos);
+      if (h_neg) atomicAdd(&cnt[kCntClassHinge + 1], (unsigned long long)h_neg);
+    }
+  }
+}
+
+template <int kModel>
+__global__ void k_class_fold(unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
+                             const double *__restrict__ scal_nrm2, double *__restrict__ out) {
+  double l_pos, l_neg;
+  if (kModel == kLogistic) {
+    l_pos = acc_take(cnt + kCntClassLoss);
+    l_neg = acc_take(cnt + kCntClassLoss + kLossAccWords);
+  } else {
+    l_pos = (double)cnt[kCntClassHinge];   // exact: counts are far below 2^53
+    l_neg = (double)cnt[kCntClassHinge + 1];
+    cnt[kCntClassHinge] = 0ull;
+    cnt[kCntClassHinge + 1] = 0ull;
+  }
+  const unsigned long long ok_pos = cnt[kCntClassCorrect], ok_neg = cnt[kCntClassCorrect + 1];
+  if (out) {
+    out[0] = *scal_nrm2;
+    out[1] = l_pos;
+    out[2] = l_neg;
+    out[3] = (double)ok_pos;
+    out[4] = (double)ok_neg;
+    out[5] = (double)cnt[kCntClassN];
+    out[6] = (double)cnt[kCntClassN + 1];
+  } else {
+    const double a = w_pos * l_pos, b = w_neg * l_neg;
+    cnt[kCntWLoss] = (unsigned long long)__double_as_longlong(a + b);
+    cnt[kCntCorrect] = ok_pos + ok_neg;
+  }
+  cnt[kCntClassN] = 0ull;
+  cnt[kCntClassN + 1] = 0ull;
+  cnt[kCntClassCorrect] = 0ull;
+  cnt[kCntClassCorrect + 1] = 0ull;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // k_finish: regularize in place -- r_j = g_j + c on the keys that survived the 1e-20 filter
 // (SparseSVM.scala:31; math/Vec.scala:65-75).  Also publishes the batch's hinge sum and size in
 // g[dim], g[dim+1] so that they ride along in the gradient allreduce.
 // ---------------------------------------------------------------------------------------------------
-template <int kModel>
+template <int kModel, bool kCw = false>
 __device__ __forceinline__ void finish_body(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
                                             const unsigned long long *__restrict__ cnt, double n_samples) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -329,7 +452,7 @@ __device__ __forceinline__ void finish_body(double *__restrict__ g, int dim, con
     if (v != 0.0 && add_c) v = filt(v + c);
     g[j] = v;
   } else if (j == dim) {
-    g[dim] = batch_loss_sum<kModel>(cnt);
+    g[dim] = batch_loss_sum<kModel, kCw>(cnt);
     g[dim + 1] = n_samples;
   }
 }
@@ -341,6 +464,11 @@ __global__ void __launch_bounds__(256) k_finish_logistic(double *__restrict__ g,
                                                          const unsigned long long *__restrict__ cnt, double n_samples) {
   finish_body<kLogistic>(g, dim, scal_c, cnt, n_samples);
 }
+template <int kModel>   // the class-weighted batch (after k_class_fold)
+__global__ void __launch_bounds__(256) k_finish_cw(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
+                                                   const unsigned long long *__restrict__ cnt, double n_samples) {
+  finish_body<kModel, true>(g, dim, scal_c, cnt, n_samples);
+}
 
 // ---------------------------------------------------------------------------------------------------
 // k_finish_acc: one logical worker's reply folded into the master's running sum.  r = regularize(g) on the
@@ -348,7 +476,7 @@ __global__ void __launch_bounds__(256) k_finish_logistic(double *__restrict__ g,
 // addition (Vec.sum is a left fold of `+`, math/Vec.scala:128-131), g cleared for the next worker.
 // Slots [dim], [dim+1] of `sum` carry the hinge total and the sample count of the step.
 // ---------------------------------------------------------------------------------------------------
-template <int kModel>
+template <int kModel, bool kCw = false>
 __device__ __forceinline__ void finish_acc_body(double *__restrict__ g, double *__restrict__ sum, int dim,
                                                 const double *__restrict__ scal_c, unsigned long long *__restrict__ cnt,
                                                 double n_samples, int first) {
@@ -362,10 +490,10 @@ __device__ __forceinline__ void finish_acc_body(double *__restrict__ g, double *
     if (raw != 0.0) g[j] = 0.0;
     sum[j] = first ? v : filt(sum[j] + v);
   } else if (j == dim) {
-    const double h = batch_loss_sum<kModel>(cnt);
+    const double h = batch_loss_sum<kModel, kCw>(cnt);
     sum[dim] = first ? h : sum[dim] + h;
     sum[dim + 1] = first ? n_samples : sum[dim + 1] + n_samples;
-    clear_batch_loss<kModel>(cnt);
+    clear_batch_loss<kModel, kCw>(cnt);
     cnt[kCntCorrect] = 0ull;
   }
 }
@@ -379,6 +507,12 @@ __global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict_
                                                              unsigned long long *__restrict__ cnt, double n_samples,
                                                              int first) {
   finish_acc_body<kLogistic>(g, sum, dim, scal_c, cnt, n_samples, first);
+}
+template <int kModel>   // the class-weighted batch of one worker: its weighted loss sum joins slot [dim]
+__global__ void __launch_bounds__(256) k_finish_acc_cw(double *__restrict__ g, double *__restrict__ sum, int dim,
+                                                       const double *__restrict__ scal_c,
+                                                       unsigned long long *__restrict__ cnt, double n_samples, int first) {
+  finish_acc_body<kModel, true>(g, sum, dim, scal_c, cnt, n_samples, first);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -395,7 +529,8 @@ __global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict_
 // w_j <- soft_threshold(u_j, lr * lambda1); c, ||w||^2, ||w||_1 and the averaging sum then see the thresholded weights, and
 // the step's loss adds lambda1 * ||w_before||_1 (scal[kScalL1]).  ||w||_1 is summed in fixed-point limbs (acc_push_block), so
 // it has the same bits as k_l1_norm over the same weights.
-template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1 = false>
+//   kCw: the batch's loss sum is the class-weighted one of k_class_fold (batch_loss_sum<kModel, true>).
+template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1 = false, bool kCw = false>
 __device__ __forceinline__ void update_body(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
                                             const double *__restrict__ d, int dim, double lambda, double lr, double inv_k_den,
                                             double *__restrict__ scal, unsigned long long *__restrict__ cnt,
@@ -460,7 +595,7 @@ __device__ __forceinline__ void update_body(double *__restrict__ w, float *__res
       // per-step loss on the weights the gradient was taken at (SparseSVM.scala:20-23; SURVEY.md F5)
       double hinge, total;
       if (kFuseRegularize) {
-        hinge = batch_loss_sum<kModel>(cnt);
+        hinge = batch_loss_sum<kModel, kCw>(cnt);
         total = n_samples_local;
       } else {
         hinge = g[dim];
@@ -476,49 +611,49 @@ __device__ __forceinline__ void update_body(double *__restrict__ w, float *__res
       }
       scal[kScalC] = lambda * 2.0 * sd;
       scal[kScalNrm2] = sn;
-      clear_batch_loss<kModel>(cnt);
+      clear_batch_loss<kModel, kCw>(cnt);
       cnt[kCntCorrect] = 0ull;
       cnt[kCntTicket] = 0ull;
     }
   }
 }
-template <bool kFuseRegularize, int kModel = kSvm>
+template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
 __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32,
                                                 double *__restrict__ g, const double *__restrict__ d, int dim,
                                                 double lambda, double lr, double inv_k_den, double *__restrict__ scal,
                                                 unsigned long long *__restrict__ cnt, double *__restrict__ partial,
                                                 double n_samples_local, double *__restrict__ loss_out) {
-  update_body<kFuseRegularize, kModel, false>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
+  update_body<kFuseRegularize, kModel, false, false, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
                                               loss_out, nullptr);
 }
-template <bool kFuseRegularize, int kModel = kSvm>
+template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
 __global__ void __launch_bounds__(256) k_update_avg(double *__restrict__ w, float *__restrict__ w32,
                                                     double *__restrict__ g, const double *__restrict__ d, int dim,
                                                     double lambda, double lr, double inv_k_den, double *__restrict__ scal,
                                                     unsigned long long *__restrict__ cnt, double *__restrict__ partial,
                                                     double n_samples_local, double *__restrict__ loss_out,
                                                     double *__restrict__ avg) {
-  update_body<kFuseRegularize, kModel, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
+  update_body<kFuseRegularize, kModel, true, false, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
                                              loss_out, avg);
 }
 
-template <bool kFuseRegularize, int kModel = kSvm>
+template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
 __global__ void __launch_bounds__(256) k_update_l1(double *__restrict__ w, float *__restrict__ w32,
                                                    double *__restrict__ g, const double *__restrict__ d, int dim,
                                                    double lambda, double lr, double inv_k_den, double *__restrict__ scal,
                                                    unsigned long long *__restrict__ cnt, double *__restrict__ partial,
                                                    double n_samples_local, double *__restrict__ loss_out, double lambda1) {
-  update_body<kFuseRegularize, kModel, false, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
+  update_body<kFuseRegularize, kModel, false, true, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
                                                     n_samples_local, loss_out, nullptr, lambda1);
 }
-template <bool kFuseRegularize, int kModel = kSvm>
+template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
 __global__ void __launch_bounds__(256) k_update_avg_l1(double *__restrict__ w, float *__restrict__ w32,
                                                        double *__restrict__ g, const double *__restrict__ d, int dim,
                                                        double lambda, double lr, double inv_k_den, double *__restrict__ scal,
                                                        unsigned long long *__restrict__ cnt, double *__restrict__ partial,
                                                        double n_samples_local, double *__restrict__ loss_out,
                                                        double *__restrict__ avg, double lambda1) {
-  update_body<kFuseRegularize, kModel, true, true>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
+  update_body<kFuseRegularize, kModel, true, true, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
                                                    n_samples_local, loss_out, avg, lambda1);
 }
 
@@ -544,15 +679,15 @@ __global__ void k_l1_finish(unsigned long long *__restrict__ cnt, double *__rest
 // k_loss_scalar: loss = lambda*||w||^2 + loss sum/n, acc = correct/n from the counters (SVM: hinge sum, an integer;
 // logistic: the fixed-point sum of the softplus losses).
 // ---------------------------------------------------------------------------------------------------
-template <int kModel>
+template <int kModel, bool kCw = false>
 __device__ __forceinline__ void loss_scalar_body(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
                                                  double lambda, double n, double *__restrict__ out2) {
-  out2[0] = lambda * (*scal_nrm2) + batch_loss_sum<kModel>(cnt) / n;
+  out2[0] = lambda * (*scal_nrm2) + batch_loss_sum<kModel, kCw>(cnt) / n;
   out2[1] = (double)cnt[kCntCorrect] / n;
-  out2[2] = batch_loss_sum<kModel>(cnt);   // SVM: exact, counts are far below 2^53
+  out2[2] = batch_loss_sum<kModel, kCw>(cnt);   // SVM: exact, counts are far below 2^53
   out2[3] = (double)cnt[kCntCorrect];
   out2[4] = *scal_nrm2;
-  clear_batch_loss<kModel>(cnt);
+  clear_batch_loss<kModel, kCw>(cnt);
   cnt[kCntCorrect] = 0ull;
 }
 __global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
@@ -562,6 +697,11 @@ __global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned lon
 __global__ void k_loss_scalar_logistic(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
                                        double lambda, double n, double *__restrict__ out2) {
   loss_scalar_body<kLogistic>(scal_nrm2, cnt, lambda, n, out2);
+}
+template <int kModel>   // the class-weighted batch: out2[2] is the weighted loss sum
+__global__ void k_loss_scalar_cw(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt, double lambda,
+                                 double n, double *__restrict__ out2) {
+  loss_scalar_body<kModel, true>(scal_nrm2, cnt, lambda, n, out2);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -97,6 +97,8 @@ struct PersistParams {
   double lambda1;                         // every update is followed by soft_threshold(., lr * lambda1) on every column
   // ---- one GPU with losses; last for the same reason ----
   double *loss_nrm;                       // [2][n_steps]: ||W_t||^2, then (kL1) ||W_t||_1, of every step t of the launch
+  // ---- class weights (kCw, one GPU); last for the same reason ----
+  double w_pos, w_neg;                    // a row of label y scatters x * (y * w_y); the step's loss is (w_pos H+ + w_neg H-) / batch
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -406,12 +408,18 @@ __device__ __forceinline__ void chunk_pairs(const StageMeta<kMaxChunks> &mt, con
 // scattered by the warp that computed its dot, from the registers that still hold its pairs; rows of several chunks
 // take a second pass after a barrier among the consumer warps (partials summed in chunk order).
 // pre (optional): the pairs of the warp's first chunk, already loaded with chunk_pairs
-template <int kCons, int kMaxChunks, class Fetch>
+// kCw (class weights): a row of label y scatters x * s with s = y * w_y instead of x * y, at all three scatter sites, and its
+// hinge loss is counted in the low 16 bits of the returned word for y = +1 and in the high 16 bits for y = -1.  A CTA holds
+// at most kMaxRowsPerCta = 32 rows of hinge <= 2 per step, so a half holds at most 64 and never carries into the other.
+template <int kCons, int kMaxChunks, bool kCw = false, class Fetch>
 __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, double *gbase,
                                                   const int gstride, Fetch &fetch, int warp, int lane, long long *tl,
-                                                  const uint2 (*pre)[4] = nullptr) {
+                                                  const uint2 (*pre)[4] = nullptr, double w_pos = 1.0, double w_neg = 1.0) {
   const int n_ch = mt.n_chunks;
   unsigned hinge = 0;  // lane 0 only
+  // the scatter scalar of a row, and its hinge loss in its class's half
+  auto scale_of = [&](int yi, double y) { return kCw ? (yi > 0 ? w_pos : -w_neg) : y; };
+  auto hinge_of = [&](int yi, unsigned l) { return kCw ? l << (yi > 0 ? 0 : 16) : l; };
   // ---- pass 1: dots of this warp's chunks ----
   for (int c = warp; c < n_ch; c += kCons) {
     uint2 pr[4];
@@ -434,11 +442,12 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       if (mt.row_nch[row1] == 1) {
         const int yi = mt.row_y[row1];
         const double y = (double)yi;
-        if (lane == 0) hinge += (unsigned)(1 - yi * pred_of(acc));
+        if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(acc)));
         if (!(y * acc < 0.0)) {  // SparseSVM.scala:28
+          const double sc = scale_of(yi, y);
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
-            const double gvv = filt(filt((double)__uint_as_float(pr[u].y)) * y);
+            const double gvv = filt(filt((double)__uint_as_float(pr[u].y)) * sc);
             if (gvv != 0.0) red_add_f64(gbase + (size_t)gstride * pr[u].x, gvv);
           }
         }
@@ -458,14 +467,15 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       for (int i = 0; i < nch; ++i) dot += mt.part[first + i];
       const int yi = mt.row_y[row];
       const double y = (double)yi;
-      if (c == first && lane == 0) hinge += (unsigned)(1 - yi * pred_of(dot));
+      if (c == first && lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)));
       if (!(y * dot < 0.0)) {
+        const double sc = scale_of(yi, y);
         const uint32_t off = mt.ch_off[c];
         const int n = mt.ch_n[c];
         const uint2 *src = (off & kChunkGlobal) ? (pairs + (off & ~kChunkGlobal)) : (ring + off);
         for (int k = lane; k < n; k += 32) {
           const uint2 pr = src[k];
-          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * y);
+          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * sc);
           if (gvv != 0.0) red_add_f64(gbase + (size_t)gstride * pr.x, gvv);
         }
       }
@@ -476,7 +486,7 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
   for (int m = warp; m < mt.n_rows; m += kCons) {
     const int nch = mt.row_nch[m];
     if (nch == 0) {
-      if (lane == 0) hinge += 1u;
+      if (lane == 0) hinge += hinge_of(mt.row_y[m], 1u);
     } else if (nch < 0) {
       const uint2 *grow = pairs + (size_t)mt.row_b[m] * 2;
       const int len = mt.row_len[m];
@@ -484,11 +494,11 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       const double dot = row_fold(grow, 0, len, lane, [&](uint32_t c) { return fetch.get1(c); });
       const int yi = mt.row_y[m];
       const double y = (double)yi;
-      if (lane == 0) hinge += (unsigned)(1 - yi * pred_of(dot));
+      if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)));
       if (!(y * dot < 0.0))
         for (int k = lane; k < len; k += 32) {
           const uint2 pr = __ldg(&grow[k]);
-          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * y);
+          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * scale_of(yi, y));
           if (gvv != 0.0) red_add_f64(gbase + (size_t)gstride * pr.x, gvv);
         }
     }
@@ -509,11 +519,17 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
 // gradient update.  ||W_T||_1 travels like W_T . d and ||W_T||^2: fp64 per-warp partials in sm.red[warp - kCons][0] (the
 // consumers' slots, unused on one GPU), summed per CTA by update warp 0 and pushed as fixed-point limbs into words 11..15
 // of the step's accumulator (overflow word 10 shared).  The loss of step t-1 adds lambda1 * ||W_{t-1}||_1.
+// kCw (one GPU only): class weights -- consume_stage scales every scatter by the weight of the row's label and packs the CTA's
+// hinge counts of the two classes into the halves of the word it already accumulates in sm.hinge_acc and stores in its
+// hinge[t * G + CTA] slot (no new buffer, nothing new on the barrier path); the epilogue's per-step warp splits the halves,
+// sums each over the G slots in integers and forms (w_pos * H+ + w_neg * H-) / batch once.
 template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable,
-          bool kL1 = false>
+          bool kL1 = false, bool kCw = false>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
   static_assert(!kL1 || (!kMulti && kUpd <= kCons), "the L1 form is one-GPU only and keeps its partials in the consumers' slots");
+  static_assert(!kCw || !kMulti, "the class-weighted form is one-GPU only");
+  static_assert(2 * kMaxRowsPerCta < (1 << 16), "a CTA's hinge count of one class fits a 16-bit half");
   static_assert(kAccWords + kAccLimbs <= kAccStride, "the L1 limbs follow the accumulator's overflow word");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
@@ -965,8 +981,8 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           auto &mt = sm.meta[st];   // full: waited for by prefetch(t)
           FetchLocal<kL1> fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
           if constexpr (kL1) fetch.tau = tau;
-          const unsigned hinge = consume_stage<kCons, kMaxChunks>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
-                                                                            lane, warp == 0 ? tl_row : nullptr, &pre);
+          const unsigned hinge = consume_stage<kCons, kMaxChunks, kCw>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
+                                                                       lane, warp == 0 ? tl_row : nullptr, &pre, p.w_pos, p.w_neg);
           if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
           if (tl_rec && warp == 0 && lane == 0) tl_rec[2] = mt.n_pairs;
           __syncwarp();
@@ -1087,13 +1103,30 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     if (p.losses) {
       for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
         unsigned h = 0;
-        for (int b = lane; b < G; b += 32) h += __ldcg(&p.hinge[s * G + b]);
-        h = __reduce_add_sync(0xffffffffu, h);
-        if (lane == 0) {
-          if constexpr (kL1)
-            p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + p.lambda1 * __ldcg(&p.loss_nrm[S + s]) + (double)h / (double)B;
-          else
-            p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + (double)h / (double)B;
+        if constexpr (kCw) {   // the halves are summed apart: G slots of at most 64 each
+          unsigned hn = 0;
+          for (int b = lane; b < G; b += 32) {
+            const unsigned v = __ldcg(&p.hinge[s * G + b]);
+            h += v & 0xffffu;
+            hn += v >> 16;
+          }
+          h = __reduce_add_sync(0xffffffffu, h);
+          hn = __reduce_add_sync(0xffffffffu, hn);
+          if (lane == 0) {
+            const double hp_w = p.w_pos * (double)h, hn_w = p.w_neg * (double)hn;
+            double pen = p.lambda * __ldcg(&p.loss_nrm[s]);
+            if constexpr (kL1) pen = pen + p.lambda1 * __ldcg(&p.loss_nrm[S + s]);
+            p.losses[s] = pen + (hp_w + hn_w) / (double)B;
+          }
+        } else {
+          for (int b = lane; b < G; b += 32) h += __ldcg(&p.hinge[s * G + b]);
+          h = __reduce_add_sync(0xffffffffu, h);
+          if (lane == 0) {
+            if constexpr (kL1)
+              p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + p.lambda1 * __ldcg(&p.loss_nrm[S + s]) + (double)h / (double)B;
+            else
+              p.losses[s] = p.lambda * __ldcg(&p.loss_nrm[s]) + (double)h / (double)B;
+          }
         }
       }
     }

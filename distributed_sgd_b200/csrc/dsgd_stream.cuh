@@ -70,6 +70,8 @@ struct StreamParams {
                                // several blocks (a block is the unit of the dynamic work distribution)
   int64_t n_big;               // blocks [0, n_big) have 1 << rows_log2 rows, the blocks after them 1 << tail_log2: the
   int tail_log2;               // last part of a pass is dealt in smaller pieces, so the warps run dry together
+  // ---- class weights (kCls); last, so that the parameter offsets of the other instantiations stay where they were ----
+  double w_pos, w_neg;         // a row of label y that passes the gate scatters x * (y * w_y)
 };
 
 __host__ __device__ constexpr size_t stream_smem_bytes(int dim) { return (((size_t)dim + 3) & ~(size_t)3) * sizeof(float); }
@@ -77,12 +79,20 @@ __host__ __device__ constexpr size_t stream_smem_bytes(int dim) { return (((size
 // kContig: the rows of the pass are consecutive (samples == nullptr), hence so are their windows in the pair array: unit v
 // of a block sits at (first window) + v and the loads need no row lookup (5 instructions per slot less, and the row-end
 // masks are worked out while the loads are in flight).
-template <bool kScatter, bool kPreds, bool kContig>
+// kCls: the per-class form (dsgd_set_class_weights, dsgd_eval*_class).  Every thread keeps the hinge and correct counts of
+// the y = -1 rows and the rows of each class apart (six counters instead of two), reduced and flushed like the two, into the
+// kCntClass* words that k_class_fold reads; the scatter value is x * (y * w_y).  The rounding band and the fp64
+// recomputation are unchanged: the weight never touches the dot.
+template <bool kScatter, bool kPreds, bool kContig, bool kCls = false>
 __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float *ws = reinterpret_cast<float *>(smem_raw);
   __shared__ float s_wmax[kStreamThreads / 32];
-  __shared__ unsigned long long s_cnt[2];
+  constexpr bool kRows = kCls && !kScatter;   // a gradient reports neither rows nor correct predictions: its per-class form
+                                              // counts the two hinge sums only (1024 threads leave 64 registers each)
+  constexpr int kCounters = kRows ? 6 : (kCls ? 4 : 2);
+  __shared__ unsigned long long s_cnt[kCounters];
+  unsigned hinge_neg = 0, correct_neg = 0, n_pos = 0, n_neg = 0;   // kCls only; hinge and correct then count the y = +1 rows
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
@@ -140,7 +150,7 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = fmaxf(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
     if (lane == 0) s_wmax[warp] = wmax;
-    if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0ull;
+    if (threadIdx.x < kCounters) s_cnt[threadIdx.x] = 0ull;
     __syncthreads();
     wmax = 0.f;
 #pragma unroll
@@ -164,7 +174,8 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
     int opos = lane;            // position of this lane's row inside the block (before compaction)
     // empty rows: dot 0 -> prediction 0, hinge 1, never correct, nothing to scatter (SparseSVM.scala:14-16)
     if (valid && len == 0) {
-      hinge += 1u;
+      if (kCls && (__float_as_uint(ya) >> 31)) { hinge_neg += 1u; if (kRows) ++n_neg; }
+      else { hinge += 1u; if (kRows) ++n_pos; }
       if (kPreds) p.preds[first + lane] = 0.0;
     }
     const unsigned ne_mask = __ballot_sync(0xffffffffu, valid && len > 0);
@@ -263,8 +274,14 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
     // prediction known for this lane's row: counters and the gate (y * dot < 0  <=>  pred == y)
     auto finalize = [&](int pr) {
       pred_mine = pr;
-      hinge += (unsigned)(1 - y * pr);
-      correct += (unsigned)(pr == y);
+      if (kCls && y < 0) {
+        hinge_neg += (unsigned)(1 - y * pr);
+        if (kRows) { correct_neg += (unsigned)(pr == y); ++n_neg; }
+      } else {
+        hinge += (unsigned)(1 - y * pr);
+        if (!kCls || kRows) correct += (unsigned)(pr == y);
+        if (kRows) ++n_pos;
+      }
       do_scatter = kScatter && (pr != y);
     };
     if (valid) {
@@ -299,7 +316,8 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
         sc &= sc - 1u;
         const uint32_t rb = __shfl_sync(0xffffffffu, b, r);
         const int rl = __shfl_sync(0xffffffffu, len, r);
-        const double yy = (double)__shfl_sync(0xffffffffu, y, r);
+        const int yr = __shfl_sync(0xffffffffu, y, r);
+        const double yy = kCls ? (yr > 0 ? p.w_pos : -p.w_neg) : (double)yr;
         for (int u = lane; u < rl; u += 32) {
           const uint4 qq = __ldg(&p.units[rb + (uint32_t)u]);
           scatter_one(qq.x, filt(filt((double)__uint_as_float(qq.y)) * yy));
@@ -314,12 +332,35 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
   hinge = __reduce_add_sync(0xffffffffu, hinge);
   correct = __reduce_add_sync(0xffffffffu, correct);
   n_exact = __reduce_add_sync(0xffffffffu, n_exact);
+  if (kCls) {
+    hinge_neg = __reduce_add_sync(0xffffffffu, hinge_neg);
+    correct_neg = __reduce_add_sync(0xffffffffu, correct_neg);
+    if (lane == 0) {
+      atomicAdd(&s_cnt[kCounters > 2 ? 2 : 0], (unsigned long long)hinge_neg);
+      atomicAdd(&s_cnt[kCounters > 3 ? 3 : 0], (unsigned long long)correct_neg);
+    }
+    if (kRows) {
+      n_pos = __reduce_add_sync(0xffffffffu, n_pos);
+      n_neg = __reduce_add_sync(0xffffffffu, n_neg);
+      if (lane == 0) {
+        atomicAdd(&s_cnt[kCounters - 2], (unsigned long long)n_pos);
+        atomicAdd(&s_cnt[kCounters - 1], (unsigned long long)n_neg);
+      }
+    }
+  }
   if (lane == 0) {
     atomicAdd(&s_cnt[0], (unsigned long long)hinge);
     atomicAdd(&s_cnt[1], (unsigned long long)correct);
     if (p.n_exact && n_exact) atomicAdd(p.n_exact, (unsigned long long)n_exact);
   }
   __syncthreads();
+  if (kCls) {
+    // s_cnt: hinge+, correct+, hinge-, correct-, rows+, rows-
+    const int t = threadIdx.x;
+    const int word = t < 4 ? ((t & 1) ? kCntClassCorrect : kCntClassHinge) + (t >> 1) : kCntClassN + (t - 4);
+    if (t < kCounters && s_cnt[t]) atomicAdd(&p.cnt[word], s_cnt[t]);
+    return;
+  }
   if (threadIdx.x == 0) {
     if (s_cnt[0]) atomicAdd(&p.cnt[kCntHinge], s_cnt[0]);
     if (s_cnt[1]) atomicAdd(&p.cnt[kCntCorrect], s_cnt[1]);

@@ -106,6 +106,17 @@ object DsgdNative {
   // weightsL1: l1(0) = ||w||_1, nnz(0) = the non-zero weights, of w or (w null) of the resident weights
   @native def setL1(ctx: Long, lambda1: Double): Int
   @native def weightsL1(ctx: Long, w: Array[Double], l1: Array[Double], nnz: Array[Long]): Int
+  // class weights of the sync steps and of gradient (both finite and >= 0; (1, 1) by default); out = {wPos, wNeg}.  The
+  // per-class evaluations, either model: sums = {||w||^2, loss sum of the y = +1 rows, of the y = -1 rows} (unweighted),
+  // counts = {correct+, correct-, n+, n-}
+  @native def setClassWeights(ctx: Long, wPos: Double, wNeg: Double): Int
+  @native def getClassWeights(ctx: Long, out: Array[Double]): Int
+  @native def evalClass(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, sums: Array[Double],
+                        counts: Array[Long]): Int
+  @native def evalSampledClass(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                               posEnd: Long, sums: Array[Double], counts: Array[Long]): Int
+  @native def evalSamplesClass(ctx: Long, w: Array[Double], samples: Array[Int], sums: Array[Double],
+                               counts: Array[Long]): Int
   // async (Hogwild) mode
   @native def asyncHostMaster(ctx: Long, w0: Array[Double]): Int
   @native def ipcExport(ctx: Long, which: Int, handle: Array[Byte]): Int

@@ -552,6 +552,57 @@ FN(weightsL1)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jdoubleArray l
   free(bw.p);
   return rc;
 }
+/* Class weights of the sync steps and of gradient: setClassWeights(wPos, wNeg), both finite and >= 0; getClassWeights:
+ * out(0) = wPos, out(1) = wNeg.  The per-class evaluations, either model: sums(0) = ||w||^2, sums(1..2) = the unweighted loss
+ * sums of the y = +1 and y = -1 rows; counts(0..3) = correct+, correct-, n+, n-.  A shorter output is DSGD_ERR_INVALID. */
+FN(setClassWeights)(JNIEnv *env, jobject self, jlong h, jdouble wPos, jdouble wNeg) {
+  return dsgd_set_class_weights(CTX(h), wPos, wNeg);
+}
+FN(getClassWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray out) {
+  buf_t bo = out_Double(env, out);
+  int rc = DSGD_ERR_NOMEM;
+  if (!bo.bad) rc = bo.n < 2 ? DSGD_ERR_INVALID : dsgd_get_class_weights(CTX(h), (double *)bo.p, (double *)bo.p + 1);
+  back_Double(env, out, bo, rc);
+  return rc;
+}
+FN(evalClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray sums,
+              jlongArray counts) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad))
+    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
+                                : dsgd_eval_class(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                     jlong posBegin, jlong posEnd, jdoubleArray sums, jlongArray counts) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad))
+    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
+                                : dsgd_eval_sampled_class(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                          (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray sums,
+                     jlongArray counts) {
+  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bi.bad | bs.bad | bc.bad))
+    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
+                                : dsgd_eval_samples_class(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (double *)bs.p + 1,
+                                                          (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p); free(bi.p);
+  return rc;
+}
 
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {

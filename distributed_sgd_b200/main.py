@@ -37,9 +37,13 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                          "training keeps its constant rate")
     if cfg.l1 != 0.0 and cfg.is_async:
         raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+    from .ml.class_weight import parse_class_weight
+    class_weight = parse_class_weight(cfg.class_weight)
+    if class_weight is not None and cfg.is_async:
+        raise ValueError("class-weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
-    model = (SparseLogistic if cfg.model == "logistic" else SparseSVM)(cfg.lam, l1=cfg.l1)
+    model = (SparseLogistic if cfg.model == "logistic" else SparseSVM)(cfg.lam, l1=cfg.l1, class_weight=class_weight)
     slave = Slave(rank, 0, train, model, cfg.is_async, world=world, device=device, test_data=test)
     master = Master.create(rank, train, test, model, cfg.is_async, cfg.node_count, slave=slave, group=Group(), seed=seed,
                            log=(log if rank == 0 else None), jvm_exact=jvm_exact)
@@ -71,6 +75,14 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     report["final_test_loss"], report["final_test_accuracy"] = master.local_loss_accuracy(w1, test_data=True)  # :115-118
     report["final_weights_nonzero"] = int(np.count_nonzero(w1))
     report["updates"] = state.updates
+    if class_weight is not None:
+        report["class_weight"] = list(slave.class_weight)   # as resolved over the train rows
+        if rank == 0:
+            log(f"class weights: w_pos = {slave.class_weight[0]:.6g}, w_neg = {slave.class_weight[1]:.6g}")
+        report["test_class_report"] = cr = master.local_class_report(w1, test_data=True)
+        if rank == 0:
+            log(f"test rows by class: recall+ {cr['recall_pos']:.4f} ({cr['n_pos']} rows), recall- {cr['recall_neg']:.4f} "
+                f"({cr['n_neg']} rows), balanced accuracy {cr['balanced_accuracy']:.4f}, weighted loss {cr['weighted_loss']:.6f}")
     if "averaged_steps" in getattr(master, "history", {}):
         report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
     if cfg.calibrate:

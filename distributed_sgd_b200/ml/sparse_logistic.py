@@ -20,3 +20,5 @@ class SparseLogistic:
     lam: float                                  # `lambda`
     dim_sparsity: Optional[np.ndarray] = None   # None: computed on the device from the train rows (Main.scala:54-65)
     l1: float = 0.0                             # extension: L1 penalty l1 * ||w||_1, a proximal step in every sync step
+    # extension: one weight per label on backward and loss in sync training: None, (w_pos, w_neg) or "balanced"
+    class_weight: object = None

@@ -10,7 +10,7 @@ import ctypes as C
 import json
 import os
 import subprocess
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import numpy as np
 
@@ -143,6 +143,11 @@ ABI = {
     "dsgd_set_l1": [_vp, _f64],
     "dsgd_dim": [_vp, C.POINTER(_i32)],
     "dsgd_weights_l1": [_vp, _vp, C.POINTER(_f64), C.POINTER(_i64)],
+    "dsgd_set_class_weights": [_vp, _f64, _f64],
+    "dsgd_get_class_weights": [_vp, C.POINTER(_f64), C.POINTER(_f64)],
+    "dsgd_eval_class": [_vp, _vp, _i64, _i64, C.POINTER(_f64), _vp, _vp],
+    "dsgd_eval_sampled_class": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), _vp, _vp],
+    "dsgd_eval_samples_class": [_vp, _vp, _vp, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_async_host_master": [_vp, _vp],
     "dsgd_ipc_export": [_vp, C.c_int, _vp],
     "dsgd_ipc_import": [_vp, C.c_int, _vp],
@@ -212,6 +217,22 @@ def _drawn(row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int)
 
 # out-parameters of the dsgd_eval_*counts and dsgd_eval_*sums calls: (hinge sum | loss sum, correct count, ||w||^2)
 _COUNTS = (_i64, _i64, _f64)
+
+
+class ClassEval(NamedTuple):
+    """One per-class evaluation (dsgd_eval*_class): ||w||^2, the unweighted loss sums and the correct and row counts of the
+    y = +1 and y = -1 rows."""
+    norm_squared: float
+    loss_pos: float
+    loss_neg: float
+    correct_pos: int
+    correct_neg: int
+    n_pos: int
+    n_neg: int
+
+    def weighted_loss_sum(self, w_pos: float, w_neg: float) -> float:
+        return w_pos * self.loss_pos + w_neg * self.loss_neg
+
 _SUMS = (_f64, _i64, _f64)
 
 
@@ -635,6 +656,36 @@ class NativeCtx:
         l1, nnz = C.c_double(), C.c_int64()
         self._ck(self._l.dsgd_weights_l1(self._h, _ptr(w), C.byref(l1), C.byref(nnz)))
         return l1.value, nnz.value
+
+    # -- class weights (sync mode) and the per-class evaluations --
+    def set_class_weights(self, w_pos: float, w_neg: float):
+        """Every following sync step and gradient request scales the gradient and the loss of a row by the weight of its label."""
+        self._ck(self._l.dsgd_set_class_weights(self._h, float(w_pos), float(w_neg)))
+
+    def get_class_weights(self) -> Tuple[float, float]:
+        wp, wn = C.c_double(), C.c_double()
+        self._ck(self._l.dsgd_get_class_weights(self._h, C.byref(wp), C.byref(wn)))
+        return wp.value, wn.value
+
+    def _class(self, fn: str, w, rows: tuple) -> "ClassEval":
+        w = self._w(w)
+        nrm = C.c_double()
+        sums, counts = np.zeros(2, dtype=np.float64), np.zeros(4, dtype=np.int64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(nrm), _ptr(sums), _ptr(counts)))
+        return ClassEval(nrm.value, float(sums[0]), float(sums[1]), *[int(c) for c in counts])
+
+    def eval_class(self, row_begin: int, row_end: int, w=None) -> "ClassEval":
+        """Per-class loss sums (unweighted), correct counts and row counts over rows [row_begin, row_end) (dsgd_eval_class)."""
+        return self._class("eval_class", w, (row_begin, row_end))
+
+    def eval_sampled_class(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None) -> "ClassEval":
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_class)."""
+        return self._class("eval_sampled_class", w, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def eval_samples_class(self, samples, w=None) -> "ClassEval":
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_class)."""
+        samples = _arr(samples, np.int32)
+        return self._class("eval_samples_class", w, (_ptr(samples), samples.size))
 
     # -- async --
     def async_host_master(self, w0):

@@ -36,6 +36,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     learning_rate_decay: float = 0.0   # extension: step t uses learning-rate / (1 + decay * t)^power, sync mode only
     learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
     l1: float = 0.0               # extension: L1 penalty l1 * ||w||_1 (lasso; elastic net with lambda), sync mode only
+    class_weight: str = "none"    # extension: none, balanced or w_pos,w_neg -- one weight per label, sync mode only
     calibrate: bool = False       # extension: after fit, fit a Platt sigmoid on the train rows and report its test-set quality
 
 
@@ -51,7 +52,7 @@ _KEYS = {
     "model": ("model", "DSGD_MODEL"), "average-from": ("average_from", "DSGD_AVERAGE_FROM"),
     "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
-    "l1": ("l1", "DSGD_L1"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
+    "l1": ("l1", "DSGD_L1"), "class-weight": ("class_weight", "DSGD_CLASS_WEIGHT"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -125,4 +126,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"learning-rate-power: expected a value > 0, got {cfg.learning_rate_power}")
     if not (cfg.l1 >= 0.0 and cfg.l1 != float("inf")):
         raise ValueError(f"l1: expected a finite value >= 0, got {cfg.l1}")
+    from ..ml.class_weight import parse_class_weight
+    parse_class_weight(cfg.class_weight)   # raises on a malformed value
     return cfg

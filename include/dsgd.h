@@ -377,6 +377,38 @@ int dsgd_set_l1(dsgd_ctx *ctx, double lambda1);
 int dsgd_dim(const dsgd_ctx *ctx, int32_t *dim_out);
 int dsgd_weights_l1(dsgd_ctx *ctx, const double *w, double *l1_out, int64_t *nnz_out);
 
+/* ---- class weights (sync mode): one weight per label, (w_pos, w_neg) for y = +1 and y = -1, both finite and >= 0, (1, 1)
+ *      when the ctx is created.  Write w_y for the weight of a row's label.  The model's backward and loss follow them:
+ *        SVM       the gate !(y * (x.w) < 0) is unchanged; a row that passes adds filt(filt(x_j) * s), s = y * w_y
+ *        logistic  s = (y * sigmoid(z)) * w_y
+ *        loss      of n rows: lambda ||w||^2 (+ lambda1 ||w||_1) + (w_pos * L_pos + w_neg * L_neg) / n, L_pos and L_neg the
+ *                  per-class sums of the UNWEIGHTED per-sample losses (SVM: integers; logistic: fixed-point sums), each
+ *                  product rounded, then their sum: the divisor is the row count, not the sum of the weights.
+ *      They act in every sync step (per-step losses included) and in dsgd_gradient (grad_out and loss_out).  Predictions,
+ *      margins, probabilities, metrics, curves, calibration and every dsgd_eval* call do not depend on them, and neither do
+ *      regularize, the update, the L1 step, averaging or the rate table, which act on the summed gradient.  At (1, 1) every
+ *      call launches exactly the kernels it launches without this call.  With other weights one worker on one GPU takes the
+ *      persistent kernel's weighted form up to 32 rows per CTA (with averaging, a rate table and L1 as without weights), the
+ *      per-step path above, and large SVM requests the streaming pass's per-class form.  The fused K-rank peer exchange has
+ *      no weighted form: with world > 1 a weighted ctx takes the NCCL path and needs dsgd_comm_init, and a rank wired with
+ *      the peer exchange only fails with DSGD_ERR_STATE before anything is launched.
+ *      Errors: a weight negative, NaN or infinite -> DSGD_ERR_INVALID; the setter on an async ctx -> DSGD_ERR_STATE. -------- */
+int dsgd_set_class_weights(dsgd_ctx *ctx, double w_pos, double w_neg);
+int dsgd_get_class_weights(const dsgd_ctx *ctx, double *w_pos_out, double *w_neg_out);
+/* Per-class evaluation, for either model and whatever the class weights are; rows and weights as in dsgd_eval,
+ * dsgd_eval_sampled_counts and dsgd_eval_samples_counts.  *norm_squared = ||w||^2; loss_sums_out[0..1] = the unweighted loss
+ * sums of the y = +1 and of the y = -1 rows (SVM: exact integers held in doubles; logistic: fixed-point sums, the same bits in
+ * any row order); counts_out[0..3] = correct_pos, correct_neg, n_pos, n_neg.  Any output may be NULL.  The two classes add up
+ * to what dsgd_eval_counts / dsgd_eval_sums report for the same rows (integers exactly), and correct_c / n_c is the recall of
+ * class c. */
+int dsgd_eval_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
+                    double *loss_sums_out, int64_t *counts_out);
+int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                            int64_t pos_begin, int64_t pos_end, double *norm_squared, double *loss_sums_out,
+                            int64_t *counts_out);
+int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *norm_squared,
+                            double *loss_sums_out, int64_t *counts_out);
+
 /* ---- async (Hogwild) mode.  Every worker keeps its own weight replica (core/Slave.scala:30) and pushes each
  *      delta to every peer replica and to the master's replica (core/Slave.scala:101-105).  Here replicas are
  *      reached by ADDRESS over NVLink: a rank exports its replica, the host transports the handle, peers import
