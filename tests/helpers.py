@@ -193,7 +193,8 @@ def fused_ranks(data, lam, d, grid_limits, w0, calls, lr, n_train=None, after=No
     attached to every other with dsgd_xchg_attach, one host thread each.  d: dimSparsity for every rank (None: computed
     from the first n_train rows).  Every rank starts from w0; calls[i] = (ids, w) is one launch: ids[r] is rank r's int32
     [steps, batch_r] sample ids (steps the same on every rank, batches may differ), w (or None) new weights installed with
-    set_weights on every rank just before the launch.  before(r, ctx), if given, runs on every rank's context once the ranks
+    set_weights on every rank just before the launch.  lr: one rate, or an array of one rate per step of every launch (a
+    rate table: dsgd_sync_steps_lr).  before(r, ctx), if given, runs on every rank's context once the ranks
     are attached, before the first launch; after(r, ctx) runs on every rank's context once all launches are done, before
     the contexts are closed.
 
@@ -233,7 +234,10 @@ def fused_ranks(data, lam, d, grid_limits, w0, calls, lr, n_train=None, after=No
                         if w is not None:
                             ctx.set_weights(w)
                         a = np.ascontiguousarray(ids[r], dtype=np.int32)
-                        ls.append(ctx.sync_steps(a.reshape(-1), a.shape[1], a.shape[0], lr))
+                        if np.ndim(lr):
+                            ls.append(ctx.sync_steps_lr(a.reshape(-1), a.shape[1], lr))
+                        else:
+                            ls.append(ctx.sync_steps(a.reshape(-1), a.shape[1], a.shape[0], lr))
                     out[r] = (np.concatenate(ls), ctx.get_weights(), ctx.xchg_stats())
                 return run
 
