@@ -15,6 +15,7 @@
 #include <limits>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -874,25 +875,22 @@ static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
   int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
   if (rc) return rc;
   const double n = (double)rows.n;
-  if (kScatter && class_weighted(ctx)) {   // a gradient of a class-weighted model: the fp64 class kernel at any size
-    if ((rc = launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32))) return rc;
-    k_finish_cw<kModel><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+  // a gradient of a class-weighted model: the fp64 class kernel at any size, and the tails of its weighted loss sum
+  const bool cw = kScatter && class_weighted(ctx);
+  if ((rc = cw ? launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32)
+               : request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr)))
+    return rc;
+  auto tail = [&](auto weighted) {
+    constexpr bool kCw = decltype(weighted)::value;
+    if constexpr (kScatter) {
+      k_finish<kModel, kCw><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+      LAUNCHED();
+    }
+    k_loss_scalar<kModel, kCw><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
     LAUNCHED();
-    k_loss_scalar_cw<kModel><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
-    LAUNCHED();
-    CU(cudaGetLastError());
-    return DSGD_OK;
-  }
-  if ((rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr))) return rc;
-  if constexpr (kScatter) {
-    const int fin_blocks = cdiv(ctx->dim + 1, 256);
-    if constexpr (kModel == kLogistic) k_finish_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
-    else k_finish<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
-    LAUNCHED();
-  }
-  if constexpr (kModel == kLogistic) k_loss_scalar_logistic<<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
-  else k_loss_scalar<<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
-  LAUNCHED();
+  };
+  if (cw) tail(std::true_type{});
+  else tail(std::false_type{});
   CU(cudaGetLastError());
   return DSGD_OK;
 }
@@ -1540,28 +1538,20 @@ extern "C" int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYT
 // ---- persistent sync loop (dsgd_persistent.cuh) ----------------------------------------------------------------
 constexpr int kPCons = 8, kPUpd = 6, kPStages = 8, kPStagePairs = 2560, kPMaxChunks = 128;
 using PSmem = PersistSmem<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks>;
-#define DSGD_PERSIST_KERNEL(multi, avg, lr_table) \
-  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, multi, avg, lr_table>
-// every instantiation, indexed [multi][avg][lr_table]
-static void *const kPersistKernels[2][2][2] = {
-    {{(void *)DSGD_PERSIST_KERNEL(false, false, false), (void *)DSGD_PERSIST_KERNEL(false, false, true)},
-     {(void *)DSGD_PERSIST_KERNEL(false, true, false), (void *)DSGD_PERSIST_KERNEL(false, true, true)}},
-    {{(void *)DSGD_PERSIST_KERNEL(true, false, false), (void *)DSGD_PERSIST_KERNEL(true, false, true)},
-     {(void *)DSGD_PERSIST_KERNEL(true, true, false), (void *)DSGD_PERSIST_KERNEL(true, true, true)}}};
-// the one-GPU L1 forms (dsgd_set_l1), indexed [avg][lr_table]
-#define DSGD_PERSIST_KERNEL_L1(avg, lr_table) \
-  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, false, avg, lr_table, true>
-static void *const kPersistKernelsL1[2][2] = {
-    {(void *)DSGD_PERSIST_KERNEL_L1(false, false), (void *)DSGD_PERSIST_KERNEL_L1(false, true)},
-    {(void *)DSGD_PERSIST_KERNEL_L1(true, false), (void *)DSGD_PERSIST_KERNEL_L1(true, true)}};
-// the one-GPU class-weighted forms (dsgd_set_class_weights), indexed [l1][avg][lr_table]
-#define DSGD_PERSIST_KERNEL_CW(avg, lr_table, l1) \
-  k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, false, avg, lr_table, l1, true>
-static void *const kPersistKernelsCw[2][2][2] = {
-    {{(void *)DSGD_PERSIST_KERNEL_CW(false, false, false), (void *)DSGD_PERSIST_KERNEL_CW(false, true, false)},
-     {(void *)DSGD_PERSIST_KERNEL_CW(true, false, false), (void *)DSGD_PERSIST_KERNEL_CW(true, true, false)}},
-    {{(void *)DSGD_PERSIST_KERNEL_CW(false, false, true), (void *)DSGD_PERSIST_KERNEL_CW(false, true, true)},
-     {(void *)DSGD_PERSIST_KERNEL_CW(true, false, true), (void *)DSGD_PERSIST_KERNEL_CW(true, true, true)}}};
+// Every instantiation of k_sync_persistent, form f = 16 multi + 8 l1 + 4 cw + 2 avg + lr_table.  The fused K-GPU kernel
+// (multi) has no L1 or class-weighted form, so the forms are exactly f < 20.
+constexpr int kPersistForms = 20;
+template <int... F>
+static void *const *persist_forms(std::integer_sequence<int, F...>) {
+  static void *const k[] = {(void *)k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, (F & 16) != 0,
+                                                      (F & 2) != 0, (F & 1) != 0, (F & 8) != 0, (F & 4) != 0>...};
+  return k;
+}
+static void *const *const kPersistKernels = persist_forms(std::make_integer_sequence<int, kPersistForms>{});
+// The form that runs a launch with these options; l1 and cw are not read for the fused kernel.
+static void *persist_kernel(bool multi, bool avg, bool lr_table, bool l1, bool cw) {
+  return kPersistKernels[multi ? 16 + 2 * avg + lr_table : 8 * l1 + 4 * cw + 2 * avg + lr_table];
+}
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -1577,17 +1567,8 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
     }
     CU(ctx->p_acc.alloc(3 * kAccStride));
     CU(ctx->p_bar.alloc(4));
-    for (int m = 0; m < 2; ++m)
-      for (int a = 0; a < 2; ++a)
-        for (int l = 0; l < 2; ++l)
-          CU(cudaFuncSetAttribute(kPersistKernels[m][a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    for (int a = 0; a < 2; ++a)
-      for (int l = 0; l < 2; ++l)
-        CU(cudaFuncSetAttribute(kPersistKernelsL1[a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
-    for (int m = 0; m < 2; ++m)
-      for (int a = 0; a < 2; ++a)
-        for (int l = 0; l < 2; ++l)
-          CU(cudaFuncSetAttribute(kPersistKernelsCw[m][a][l], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+    for (int f = 0; f < kPersistForms; ++f)
+      CU(cudaFuncSetAttribute(kPersistKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
     ctx->p_ready = true;
   }
   // sized for the largest grid (persist_grid), which dsgd_reserve does not know yet
@@ -1711,14 +1692,12 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.lr = 0.0;   // not read: interval 0, the only one before lrs[0] is loaded, applies no update
   }
   void *args[] = {&pp};
-  // the L1 forms only with a penalty (never fused: sync_staged keeps an L1 ctx off the fused path)
+  // the L1 forms only with a penalty, the class-weighted forms only with weights other than (1, 1) (neither fused:
+  // sync_staged keeps such a ctx off the fused path)
   const bool l1 = !multi && ctx->lambda1 > 0.0;
   pp.lambda1 = l1 ? ctx->lambda1 : 0.0;
-  void *fn = l1 ? kPersistKernelsL1[ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0]
-                : kPersistKernels[multi ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
-  // the class-weighted forms only with weights other than (1, 1) (never fused: sync_staged keeps such a ctx off that path)
   pp.w_pos = ctx->cw_pos; pp.w_neg = ctx->cw_neg;
-  if (!multi && class_weighted(ctx)) fn = kPersistKernelsCw[l1 ? 1 : 0][ctx->avg_on ? 1 : 0][lrs_host ? 1 : 0];
+  void *fn = persist_kernel(multi, ctx->avg_on, lrs_host != nullptr, l1, class_weighted(ctx));
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
   CU(launch_err);
@@ -1881,27 +1860,16 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
   double lr_s = lr;   // the rate of step s
-  const bool l1 = ctx->lambda1 > 0.0;
-  // k_update, or while averaging k_update_avg: the same update, then avg += the new weights; with an L1 penalty their _l1
-  // forms, which soft-threshold every column after the update
-  auto update = [&](auto kernel, auto kernel_avg, auto kernel_l1, auto kernel_avg_l1, double *gbuf, double k_den,
-                    double n_local, double *loss_dev) {
-    if (l1 && ctx->avg_on)
-      kernel_avg_l1<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                         ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg,
-                                                         ctx->lambda1);
-    else if (l1)
-      kernel_l1<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                     ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->lambda1);
-    else if (ctx->avg_on)
-      kernel_avg<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                      ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev, ctx->avg);
-    else
-      kernel<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den,
-                                                  ctx->scal, ctx->cnt, ctx->partial, n_local, loss_dev);
-    LAUNCHED();
-    if (ctx->avg_on) ++ctx->avg_n;
-  };
+  // The update of every step, in the form of this call [single][avg][l1]: one worker regularizes its raw gradient in the
+  // update; while averaging the update also adds the new weights to avg; with an L1 penalty it soft-thresholds every column.
+  using Update = decltype(&k_update<true, kModel, false, false, kCw>);
+  static const Update kUpdate[2][2][2] = {
+      {{k_update<false, kModel, false, false, kCw>, k_update<false, kModel, false, true, kCw>},
+       {k_update<false, kModel, true, false, kCw>, k_update<false, kModel, true, true, kCw>}},
+      {{k_update<true, kModel, false, false, kCw>, k_update<true, kModel, false, true, kCw>},
+       {k_update<true, kModel, true, false, kCw>, k_update<true, kModel, true, true, kCw>}}};
+  const Update update = kUpdate[single][ctx->avg_on][ctx->lambda1 > 0.0];
+  double *const avg = ctx->avg_on ? ctx->avg.p : nullptr;
 
   auto rows_pass = [&](const row_set &rows) {
     if constexpr (kCw) launch_rows_class<kModel, true>(ctx, rows, ctx->w, ctx->g);
@@ -1911,35 +1879,33 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
     if (lrs) lr_s = lrs[s];
     double *loss_dev = losses ? losses + s : nullptr;
+    double *gbuf = ctx->g;
+    double k_den = 1.0, n_local = (double)n_per_step;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
       profiled(ctx, [&] { rows_pass({smp, 0, n_per_step}); });
-      update(k_update<true, kModel, kCw>, k_update_avg<true, kModel, kCw>, k_update_l1<true, kModel, kCw>,
-             k_update_avg_l1<true, kModel, kCw>, ctx->g, 1.0, (double)n_per_step, loss_dev);
-      continue;
+    } else {
+      // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
+      int64_t off = 0;
+      for (int32_t v = 0; v < ctx->n_local; ++v) {
+        const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
+        profiled(ctx, [&] { rows_pass({smp + off, 0, nv}); });
+        k_finish_acc<kModel, kCw><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC,
+                                                                       ctx->cnt, (double)nv, v == 0 ? 1 : 0);
+        LAUNCHED();
+        off += nv;
+      }
+      if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
+      if (ctx->world > 1)
+        NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
+      gbuf = ctx->gsum;
+      k_den = (double)k_total;
+      n_local = 0.0;
     }
-    // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
-    int64_t off = 0;
-    for (int32_t v = 0; v < ctx->n_local; ++v) {
-      const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
-      profiled(ctx, [&] { rows_pass({smp + off, 0, nv}); });
-      if constexpr (kCw)
-        k_finish_acc_cw<kModel><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
-                                                                     (double)nv, v == 0 ? 1 : 0);
-      else if constexpr (kModel == kLogistic)
-        k_finish_acc_logistic<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
-                                                                   (double)nv, v == 0 ? 1 : 0);
-      else
-        k_finish_acc<<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC, ctx->cnt,
-                                                          (double)nv, v == 0 ? 1 : 0);
-      LAUNCHED();
-      off += nv;
-    }
-    if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
-    if (ctx->world > 1)
-      NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
-    update(k_update<false, kModel, kCw>, k_update_avg<false, kModel, kCw>, k_update_l1<false, kModel, kCw>,
-           k_update_avg_l1<false, kModel, kCw>, ctx->gsum, (double)k_total, 0.0, loss_dev);
+    update<<<upd_blocks, 256, 0, ctx->stream>>>(ctx->w, ctx->w32, gbuf, ctx->d, ctx->dim, ctx->lambda, lr_s, k_den, ctx->scal,
+                                                ctx->cnt, ctx->partial, n_local, loss_dev, avg, ctx->lambda1);
+    LAUNCHED();
+    if (ctx->avg_on) ++ctx->avg_n;
   }
   CU(cudaGetLastError());
   return DSGD_OK;
@@ -1971,19 +1937,17 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   }
   const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
-  // the persistent and fused kernels are SVM-only: a logistic ctx always takes the per-step path below.  The fused kernel has
-  // no L1 form: a ctx with an L1 penalty takes the one-GPU persistent kernel's L1 form or the per-step path.
+  // The options the fused kernel has no form of, which with world > 1 take the per-step path over NCCL: the persistent and
+  // fused kernels are SVM-only (a logistic ctx always takes the per-step path below), and an L1 penalty or class weights
+  // have only one-GPU persistent forms.  unfused names the first of them that is on.
   const bool logistic = is_logistic(ctx);
-  const bool l1 = ctx->lambda1 > 0.0;
-  NEED(!logistic || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
-       "dsgd_sync_steps: the logistic model takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
-  NEED(!l1 || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
-       "dsgd_sync_steps: the L1 penalty takes the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
-  // Class weights have no form in the fused kernel: with world > 1 a weighted ctx takes the per-step path over NCCL.
   const bool cw = class_weighted(ctx);
-  NEED(!cw || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
-       "dsgd_sync_steps: class weights take the NCCL allreduce path for world > 1, which needs dsgd_comm_init");
-  const bool fused = !logistic && !l1 && !cw && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
+  const char *unfused = logistic ? "the logistic model takes"
+                        : ctx->lambda1 > 0.0 ? "the L1 penalty takes"
+                        : cw ? "class weights take" : nullptr;
+  NEED(!unfused || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
+       "dsgd_sync_steps: %s the NCCL allreduce path for world > 1, which needs dsgd_comm_init", unfused);
+  const bool fused = !unfused && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
                      persist_grid(ctx, n_per_step) > 0 && persist_multi_fits(ctx, persist_grid(ctx, n_per_step));
   // Ranks wired with the peer exchange only have no communicator for the step-by-step path below: refuse before anything
   // is launched instead of reaching the allreduce without one.

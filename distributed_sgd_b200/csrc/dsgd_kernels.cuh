@@ -27,7 +27,7 @@ enum Scal : int {
   kScalReqC = 2,   // same two for a request-supplied weight vector (GradientRequest.weights)
   kScalReqNrm2 = 3,
   kScalL1 = 4,     // ||w||_1 of the current resident weights: refreshed by every sync call of an L1 ctx (k_l1_norm), then
-                   // kept by its update kernels (k_update_l1)
+                   // kept by its update kernels (k_update<..., kL1>)
   kNumScal = 8
 };
 // Slots of the per-ctx counter block (unsigned long long[kNumCnt]).
@@ -38,7 +38,7 @@ enum Cnt : int {
   kCntWLoss = 3,    // class-weighted batch: the bits of the double w_pos * L_pos + w_neg * L_neg (k_class_fold), which the
                     // weighted tails (kCw) read instead of kCntHinge / kCntLoss
   kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
-  kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update_l1, k_l1_norm; zero between launches
+  kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update<..., kL1>, k_l1_norm; zero between launches
   kCntNnz = 23,     // #{w_j != 0} of k_l1_norm; zero between launches
   // per-class counters of k_rows_class, cleared by k_class_fold: index 0 is the class y = +1, index 1 the class y = -1
   kCntClassN = 24,        // rows
@@ -440,10 +440,11 @@ __global__ void k_class_fold(unsigned long long *__restrict__ cnt, double w_pos,
 // k_finish: regularize in place -- r_j = g_j + c on the keys that survived the 1e-20 filter
 // (SparseSVM.scala:31; math/Vec.scala:65-75).  Also publishes the batch's hinge sum and size in
 // g[dim], g[dim+1] so that they ride along in the gradient allreduce.
+//   kModel, kCw: where the batch's loss sum comes from (batch_loss_sum; kCw after k_class_fold).
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kCw = false>
-__device__ __forceinline__ void finish_body(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
-                                            const unsigned long long *__restrict__ cnt, double n_samples) {
+template <int kModel, bool kCw>
+__global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
+                                                const unsigned long long *__restrict__ cnt, double n_samples) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const double c = *scal_c;
   const bool add_c = (c != 0.0) && (fabs(c) > kEps);
@@ -456,30 +457,17 @@ __device__ __forceinline__ void finish_body(double *__restrict__ g, int dim, con
     g[dim + 1] = n_samples;
   }
 }
-__global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
-                                                const unsigned long long *__restrict__ cnt, double n_samples) {
-  finish_body<kSvm>(g, dim, scal_c, cnt, n_samples);
-}
-__global__ void __launch_bounds__(256) k_finish_logistic(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
-                                                         const unsigned long long *__restrict__ cnt, double n_samples) {
-  finish_body<kLogistic>(g, dim, scal_c, cnt, n_samples);
-}
-template <int kModel>   // the class-weighted batch (after k_class_fold)
-__global__ void __launch_bounds__(256) k_finish_cw(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
-                                                   const unsigned long long *__restrict__ cnt, double n_samples) {
-  finish_body<kModel, true>(g, dim, scal_c, cnt, n_samples);
-}
 
 // ---------------------------------------------------------------------------------------------------
 // k_finish_acc: one logical worker's reply folded into the master's running sum.  r = regularize(g) on the
 // worker's own support (SparseSVM.scala:31), then sum <- sum + r with the constructor filter after the
 // addition (Vec.sum is a left fold of `+`, math/Vec.scala:128-131), g cleared for the next worker.
-// Slots [dim], [dim+1] of `sum` carry the hinge total and the sample count of the step.
+// Slots [dim], [dim+1] of `sum` carry the loss total (kCw: the weighted one) and the sample count of the step.
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kCw = false>
-__device__ __forceinline__ void finish_acc_body(double *__restrict__ g, double *__restrict__ sum, int dim,
-                                                const double *__restrict__ scal_c, unsigned long long *__restrict__ cnt,
-                                                double n_samples, int first) {
+template <int kModel, bool kCw>
+__global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, double *__restrict__ sum, int dim,
+                                                    const double *__restrict__ scal_c,
+                                                    unsigned long long *__restrict__ cnt, double n_samples, int first) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const double c = *scal_c;
   const bool add_c = (c != 0.0) && (fabs(c) > kEps);
@@ -497,23 +485,6 @@ __device__ __forceinline__ void finish_acc_body(double *__restrict__ g, double *
     cnt[kCntCorrect] = 0ull;
   }
 }
-__global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, double *__restrict__ sum, int dim,
-                                                    const double *__restrict__ scal_c,
-                                                    unsigned long long *__restrict__ cnt, double n_samples, int first) {
-  finish_acc_body<kSvm>(g, sum, dim, scal_c, cnt, n_samples, first);
-}
-__global__ void __launch_bounds__(256) k_finish_acc_logistic(double *__restrict__ g, double *__restrict__ sum, int dim,
-                                                             const double *__restrict__ scal_c,
-                                                             unsigned long long *__restrict__ cnt, double n_samples,
-                                                             int first) {
-  finish_acc_body<kLogistic>(g, sum, dim, scal_c, cnt, n_samples, first);
-}
-template <int kModel>   // the class-weighted batch of one worker: its weighted loss sum joins slot [dim]
-__global__ void __launch_bounds__(256) k_finish_acc_cw(double *__restrict__ g, double *__restrict__ sum, int dim,
-                                                       const double *__restrict__ scal_c,
-                                                       unsigned long long *__restrict__ cnt, double n_samples, int first) {
-  finish_acc_body<kModel, true>(g, sum, dim, scal_c, cnt, n_samples, first);
-}
 
 // ---------------------------------------------------------------------------------------------------
 // k_update: the master's aggregate + SGD update (core/Master.scala:194,197) fused with the bookkeeping
@@ -523,19 +494,21 @@ __global__ void __launch_bounds__(256) k_finish_acc_cw(double *__restrict__ g, d
 //   kFuseRegularize: the buffer holds the raw local sum (single worker): apply regularize() here.
 //   otherwise it holds sum_k r^(k) (already regularized per worker, then allreduced).
 //   kModel: where the batch's loss sum comes from (batch_loss_sum).
-//   kAvg (k_update_avg): also avg_j <- avg_j + w_j of the NEW weights, every column (averaged SGD, dsgd_average_begin).
-// ---------------------------------------------------------------------------------------------------
-// kL1 (k_update_l1, k_update_avg_l1): after the update, the proximal step of the L1 penalty lambda1 * ||w||_1 on EVERY column,
-// w_j <- soft_threshold(u_j, lr * lambda1); c, ||w||^2, ||w||_1 and the averaging sum then see the thresholded weights, and
-// the step's loss adds lambda1 * ||w_before||_1 (scal[kScalL1]).  ||w||_1 is summed in fixed-point limbs (acc_push_block), so
-// it has the same bits as k_l1_norm over the same weights.
+//   kAvg: also avg_j <- avg_j + w_j of the NEW weights, every column (averaged SGD, dsgd_average_begin); otherwise avg is
+//   nullptr.
+//   kL1: after the update, the proximal step of the L1 penalty lambda1 * ||w||_1 on EVERY column,
+//   w_j <- soft_threshold(u_j, lr * lambda1); c, ||w||^2, ||w||_1 and the averaging sum then see the thresholded weights, and
+//   the step's loss adds lambda1 * ||w_before||_1 (scal[kScalL1]).  ||w||_1 is summed in fixed-point limbs (acc_push_block),
+//   so it has the same bits as k_l1_norm over the same weights.  Otherwise lambda1 is not read.
 //   kCw: the batch's loss sum is the class-weighted one of k_class_fold (batch_loss_sum<kModel, true>).
-template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1 = false, bool kCw = false>
-__device__ __forceinline__ void update_body(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
-                                            const double *__restrict__ d, int dim, double lambda, double lr, double inv_k_den,
-                                            double *__restrict__ scal, unsigned long long *__restrict__ cnt,
-                                            double *__restrict__ partial, double n_samples_local,
-                                            double *__restrict__ loss_out, double *__restrict__ avg, double lambda1 = 0.0) {
+// ---------------------------------------------------------------------------------------------------
+template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1, bool kCw>
+__global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
+                                                const double *__restrict__ d, int dim, double lambda, double lr,
+                                                double inv_k_den, double *__restrict__ scal,
+                                                unsigned long long *__restrict__ cnt, double *__restrict__ partial,
+                                                double n_samples_local, double *__restrict__ loss_out,
+                                                double *__restrict__ avg, double lambda1) {
   __shared__ double red[8];
   __shared__ bool is_last;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -617,45 +590,6 @@ __device__ __forceinline__ void update_body(double *__restrict__ w, float *__res
     }
   }
 }
-template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
-__global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32,
-                                                double *__restrict__ g, const double *__restrict__ d, int dim,
-                                                double lambda, double lr, double inv_k_den, double *__restrict__ scal,
-                                                unsigned long long *__restrict__ cnt, double *__restrict__ partial,
-                                                double n_samples_local, double *__restrict__ loss_out) {
-  update_body<kFuseRegularize, kModel, false, false, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
-                                              loss_out, nullptr);
-}
-template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
-__global__ void __launch_bounds__(256) k_update_avg(double *__restrict__ w, float *__restrict__ w32,
-                                                    double *__restrict__ g, const double *__restrict__ d, int dim,
-                                                    double lambda, double lr, double inv_k_den, double *__restrict__ scal,
-                                                    unsigned long long *__restrict__ cnt, double *__restrict__ partial,
-                                                    double n_samples_local, double *__restrict__ loss_out,
-                                                    double *__restrict__ avg) {
-  update_body<kFuseRegularize, kModel, true, false, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial, n_samples_local,
-                                             loss_out, avg);
-}
-
-template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
-__global__ void __launch_bounds__(256) k_update_l1(double *__restrict__ w, float *__restrict__ w32,
-                                                   double *__restrict__ g, const double *__restrict__ d, int dim,
-                                                   double lambda, double lr, double inv_k_den, double *__restrict__ scal,
-                                                   unsigned long long *__restrict__ cnt, double *__restrict__ partial,
-                                                   double n_samples_local, double *__restrict__ loss_out, double lambda1) {
-  update_body<kFuseRegularize, kModel, false, true, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
-                                                    n_samples_local, loss_out, nullptr, lambda1);
-}
-template <bool kFuseRegularize, int kModel = kSvm, bool kCw = false>
-__global__ void __launch_bounds__(256) k_update_avg_l1(double *__restrict__ w, float *__restrict__ w32,
-                                                       double *__restrict__ g, const double *__restrict__ d, int dim,
-                                                       double lambda, double lr, double inv_k_den, double *__restrict__ scal,
-                                                       unsigned long long *__restrict__ cnt, double *__restrict__ partial,
-                                                       double n_samples_local, double *__restrict__ loss_out,
-                                                       double *__restrict__ avg, double lambda1) {
-  update_body<kFuseRegularize, kModel, true, true, kCw>(w, w32, g, d, dim, lambda, lr, inv_k_den, scal, cnt, partial,
-                                                   n_samples_local, loss_out, avg, lambda1);
-}
 
 // ---------------------------------------------------------------------------------------------------
 // k_l1_norm + k_l1_finish: ||w||_1 = sum_j |w_j| in the fixed-point limbs (exact in any order: every |w_j| > 1e-20 is a
@@ -677,11 +611,11 @@ __global__ void k_l1_finish(unsigned long long *__restrict__ cnt, double *__rest
 
 // ---------------------------------------------------------------------------------------------------
 // k_loss_scalar: loss = lambda*||w||^2 + loss sum/n, acc = correct/n from the counters (SVM: hinge sum, an integer;
-// logistic: the fixed-point sum of the softplus losses).
+// logistic: the fixed-point sum of the softplus losses; kCw: the class-weighted sum of k_class_fold).
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kCw = false>
-__device__ __forceinline__ void loss_scalar_body(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
-                                                 double lambda, double n, double *__restrict__ out2) {
+template <int kModel, bool kCw>
+__global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt, double lambda,
+                              double n, double *__restrict__ out2) {
   out2[0] = lambda * (*scal_nrm2) + batch_loss_sum<kModel, kCw>(cnt) / n;
   out2[1] = (double)cnt[kCntCorrect] / n;
   out2[2] = batch_loss_sum<kModel, kCw>(cnt);   // SVM: exact, counts are far below 2^53
@@ -689,19 +623,6 @@ __device__ __forceinline__ void loss_scalar_body(const double *__restrict__ scal
   out2[4] = *scal_nrm2;
   clear_batch_loss<kModel, kCw>(cnt);
   cnt[kCntCorrect] = 0ull;
-}
-__global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
-                              double lambda, double n, double *__restrict__ out2) {
-  loss_scalar_body<kSvm>(scal_nrm2, cnt, lambda, n, out2);
-}
-__global__ void k_loss_scalar_logistic(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt,
-                                       double lambda, double n, double *__restrict__ out2) {
-  loss_scalar_body<kLogistic>(scal_nrm2, cnt, lambda, n, out2);
-}
-template <int kModel>   // the class-weighted batch: out2[2] is the weighted loss sum
-__global__ void k_loss_scalar_cw(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt, double lambda,
-                                 double n, double *__restrict__ out2) {
-  loss_scalar_body<kModel, true>(scal_nrm2, cnt, lambda, n, out2);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -112,7 +112,7 @@ def test_dyadic_bit_for_bit(dy, S, grid, batch):
         launches = ctx.launch_count() - n0
     finally:
         ctx.set_grid_limit(0)
-    # the persistent kernel (k_rec_init + one launch) up to 32 rows per CTA, else k_rows + k_update_l1 per step
+    # the persistent kernel (k_rec_init + one launch) up to 32 rows per CTA, else k_rows + k_update<..., kL1> per step
     assert launches == (2 if B <= 32 * G else 2 * STEPS), launches
     w_ref, l_ref = L1.sync_steps(orc, w0, ids.reshape(-1), [B], np.full(STEPS, LR), LAM1)
     _same(ctx.get_weights(), w_ref, "weights")

@@ -2,7 +2,9 @@
 encodings ignored).  Used to show that adding template variants leaves the kernels that were verified on the GPU untouched.
     python tools/sass_diff.py old/libdsgd.so distributed_sgd_b200/libdsgd.so
 A kernel that gained trailing template arguments 0 or false (e.g. `..., 0>` -> `..., 0, 0>`, `..., false>` ->
-`..., false, false>`) is matched by its name prefix."""
+`..., false, false>`) is matched by its name prefix.  A kernel with no such counterpart is matched to every kernel of the
+second build with the identical instruction list and reported as renamed; matching by body is many-to-one (two
+instantiations can compile to the same instructions), so it is evidence of a rename, not a proof."""
 import re
 import subprocess
 import sys
@@ -25,17 +27,25 @@ def kernels(path):
 
 def main():
     a, b = kernels(sys.argv[1]), kernels(sys.argv[2])
-    differ = 0
+    by_body = {}
+    for name, body in b.items():
+        by_body.setdefault(tuple(body), []).append(name)
+    differ = renamed = 0
     for name, body in sorted(a.items()):
         extra = ("ELi0", "ELi0ELi0", "ELb0")
         cands = [name] if name in b else [n for n in (name.replace("EEEv", e + "EEEv", 1) for e in extra) if n in b]
         if not cands:
-            print("only in the first build:", name)
-            differ += 1
+            same = by_body.get(tuple(body))
+            if same:
+                print("renamed:", name, "->", " | ".join(sorted(same)))
+                renamed += 1
+            else:
+                print("only in the first build:", name)
+                differ += 1
         elif body != b[cands[0]]:
             print("DIFFERENT:", name, len(body), "->", len(b[cands[0]]), "instructions")
             differ += 1
-    print(f"{len(a)} kernels in the first build, {len(b)} in the second, {differ} differ or are missing")
+    print(f"{len(a)} kernels in the first build, {len(b)} in the second, {renamed} renamed, {differ} differ or are missing")
     return 1 if differ else 0
 
 
