@@ -20,7 +20,7 @@ from ..ml.lr_schedule import check_schedule, learning_rates
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
-from ..utils.dataset import Data
+from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights
 from .group import Group
 from .slave import Slave
 
@@ -169,7 +169,10 @@ class Master:
         self.logistic = isinstance(model, SparseLogistic)
         # (w_pos, w_neg) as the Slave resolved and installed them; (1, 1): every evaluation makes the calls it made before
         self.class_weight = getattr(slave, "class_weight", (1.0, 1.0))
-        self.weighted = self.class_weight != (1.0, 1.0)
+        # the Slave loaded per-row sample weights: every loss evaluation makes the *_weighted calls, whose loss sums already
+        # carry the class weights, so the per-class split below is not used
+        self.sample_weighted = bool(getattr(slave, "sample_weighted", False))
+        self.weighted = self.class_weight != (1.0, 1.0) and not self.sample_weighted
         self.n_train, self.n_test = data.n_rows, test_data.n_rows
         self.dim = data.dim
         self.slave = slave
@@ -209,7 +212,11 @@ class Master:
     def _local_eval(self, call: str, *args):
         """(loss sum, correct count, ||w||^2) of this rank's share: ctx.<call>_counts for the SVM (its loss sum is the
         integer hinge sum), ctx.<call>_sums for SparseLogistic.  With class weights ctx.<call>_class, and a fourth value:
-        (loss sum of the positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted."""
+        (loss sum of the positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted.  With sample
+        weights ctx.<call>_weighted: (S = sum c_i L_i, correct count, ||w||^2)."""
+        if self.sample_weighted:
+            we = getattr(self.ctx, call + "_weighted")(*args)
+            return we.loss_sum, we.correct, we.norm_squared
         if self.weighted:
             ce = getattr(self.ctx, call + "_class")(*args)
             as_sum = float if self.logistic else int   # the SVM's sums are integers: all-reduced exactly
@@ -225,8 +232,9 @@ class Master:
         """(loss sum, correct[, rows], ||w||^2) over all ranks; ||w||^2 is identical on every rank that evaluated and 0 on idle
         ranks: its maximum.  SVM: the sums are integers below 2^53, exact in any order (all-reduce).  Logistic: the loss
         sums are not integers, so the partials are gathered and added in rank order and every rank gets the same bits --
-        ranks whose stopping rule saw different losses would leave `fit` at different epochs and hang the next collective."""
-        if not self.logistic:
+        ranks whose stopping rule saw different losses would leave `fit` at different epochs and hang the next collective.
+        Sample-weighted loss sums are not integers either: they take the logistic path."""
+        if not (self.logistic or self.sample_weighted):
             return (*self.group.all_reduce_sum([h, c, *rows]), self.group.all_reduce_max(n2))
         mine = np.array([h, c, *rows, n2], dtype=np.float64)
         parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
@@ -349,6 +357,31 @@ class Master:
             raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
         ce = self.ctx.eval_sampled_class(b, e, key, 0, k, weights) if ids is None else self.ctx.eval_samples_class(ids, weights)
         return self._class_report(ce, weights)
+
+    # ---- sample-weighted report (extension) -------------------------------------------------------------------------------
+    # Not sharded, like the per-class report: every rank evaluates the whole range or sample, and the fixed-point sums have
+    # the same bits on every rank.
+    def _weighted_report(self, we, weights) -> dict:
+        nan = float("nan")
+        pen = self._penalty(we.norm_squared, weights, True)
+        return {"n": we.n, "weight_sum": we.weight_sum, "weighted_loss": pen + we.loss_sum / we.n,
+                "weighted_accuracy": we.correct_weight / we.weight_sum if we.weight_sum > 0.0 else nan}
+
+    def local_weighted_report(self, weights=None, test_data: bool = False) -> dict:
+        """Rows, the sum of their combined weights c_i = class weight x sample weight, the weighted loss penalty + S / n and
+        the weighted accuracy sum c_i [correct] / sum c_i over the train (or test) rows.  Without sample weights c_i is the
+        class weight."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return self._weighted_report(self.ctx.eval_weighted(b, e, weights), weights)
+
+    def local_sampled_weighted_report(self, weights, samples_count: int, test_data: bool = False) -> dict:
+        """local_weighted_report on a fresh sample (_draw_sample).  An empty sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
+        we = (self.ctx.eval_sampled_weighted(b, e, key, 0, k, weights) if ids is None
+              else self.ctx.eval_samples_weighted(ids, weights))
+        return self._weighted_report(we, weights)
 
     # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
     # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank
@@ -616,6 +649,8 @@ class MasterAsync(Master):
         from ..ml.class_weight import resolve_class_weight
         if resolve_class_weight(getattr(model, "class_weight", None), data.label) != (1.0, 1.0):   # as the Slave decides
             raise ValueError("class_weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
+        if has_sample_weights(data, test_data):   # as the Slave decides
+            raise ValueError(SAMPLE_WEIGHT_ASYNC)
         super().__init__(node, data, test_data, model, expected_node_count, **kw)
 
     def _attach_replicas(self):

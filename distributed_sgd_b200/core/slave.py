@@ -15,7 +15,7 @@ from ..ml.class_weight import resolve_class_weight
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_svm import SparseSVM
 from ..native import NativeCtx
-from ..utils.dataset import Data
+from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights, sample_weights_of
 
 
 class Slave:
@@ -41,6 +41,10 @@ class Slave:
         weighted = self.class_weight != (1.0, 1.0)
         if weighted and is_async:
             raise ValueError("class_weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
+        # per-row sample weights of the train and test rows (a part without them weighs 1 per row)
+        self.sample_weighted = has_sample_weights(data, test_data)
+        if self.sample_weighted and is_async:
+            raise ValueError(SAMPLE_WEIGHT_ASYNC)
         self.node, self.master, self.model, self.is_async, self.world = node, master, model, is_async, world
         self.n_train = data.n_rows
         self.n_test = test_data.n_rows if test_data is not None else 0
@@ -57,6 +61,8 @@ class Slave:
                 ctx.set_l1(model.l1)
             if weighted:
                 ctx.set_class_weights(*self.class_weight)
+            if self.sample_weighted:
+                ctx.set_sample_weights(sample_weights_of(data, test_data))
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
                              is_async=is_async, logistic=logistic)
@@ -76,6 +82,8 @@ class Slave:
             self.ctx.set_l1(model.l1)
         if weighted:
             self.ctx.set_class_weights(*self.class_weight)
+        if self.sample_weighted:
+            self.ctx.set_sample_weights(sample_weights_of(data, test_data))
 
     def stop(self):  # Slave.stop (core/Slave.scala:68-77): releases the device context
         self.ctx.close()

@@ -107,6 +107,7 @@ struct dsgd_ctx {
   double lambda = 0.0;
   double lambda1 = 0.0;   // dsgd_set_l1: the L1 penalty of the sync steps (0: off)
   double cw_pos = 1.0, cw_neg = 1.0;   // dsgd_set_class_weights: the weights of the y = +1 and y = -1 rows
+  bool sw_on = false;   // dsgd_set_sample_weights: sw holds one weight per loaded row, and the sample-weighted forms run
   int rank = 0, world = 1;
   uint32_t flags = 0;
   int sm_count = 0;
@@ -123,6 +124,7 @@ struct dsgd_ctx {
   dev_buf<uint2> pairs;
   dev_buf<int8_t> label;
   dev_buf<float> yabs;   // label * sum_j |x_j| per row (dsgd_kernels.cuh: k_repack)
+  dev_buf<double> sw;    // dsgd_set_sample_weights: one fp64 weight per row (allocated on first use, freed with the rows)
 
   // state (fp64, L2 resident) -- g has dim + 2 slots (hinge sum and batch size ride in the allreduce)
   dev_buf<double> w, g, d, w_req;
@@ -133,7 +135,8 @@ struct dsgd_ctx {
   dev_buf<unsigned long long> cnt;
   dev_buf<double> partial;  // 2 doubles per k_update block
   dev_buf<double> out2;     // loss, acc, hinge sum, correct count, ||w||^2
-  dev_buf<double> cls_out;  // dsgd_eval*_class: ||w||^2, the two loss sums, correct and rows per class (k_class_fold)
+  dev_buf<double> cls_out;  // dsgd_eval*_class: ||w||^2, the two loss sums, correct and rows per class (k_class_fold);
+                            // dsgd_eval*_weighted: ||w||^2, the three weighted sums and the correct count (k_sw_fold)
   dev_buf<double> gsum;     // master-side running sum of worker replies (dim + 2)
   std::vector<int32_t> worker_counts;  // logical workers on this ctx (empty: one worker, whole slice)
   int32_t n_local = 1, k_total = 0;    // k_total == 0: world
@@ -173,6 +176,7 @@ struct dsgd_ctx {
   dev_buf<double2> p_rec[3];   // one GPU: rotating {W, g} records
   dev_buf<unsigned long long> p_acc;   // fixed-point accumulators of the per-CTA partials [3][kAccStride]
   dev_buf<unsigned> p_hinge;   // one GPU: hinge count of every step and CTA [n_steps][CTAs]
+  dev_buf<unsigned long long> p_hcode;   // one GPU with sample weights: the rows' 2-bit hinge codes [n_steps][CTAs]
   dev_buf<double> p_loss_nrm;  // one GPU: the norms of every step's loss [2][n_steps]
   dev_buf<unsigned> p_bar;   // [0]: grid barrier counter, [1]: abort flag
   bool p_ready = false;
@@ -318,6 +322,8 @@ static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
 // the class-weighted kernels run only with weights other than (1, 1)
 static inline bool class_weighted(const dsgd_ctx *ctx) { return !(ctx->cw_pos == 1.0 && ctx->cw_neg == 1.0); }
+// the sample-weighted kernels run whenever weights are loaded, all ones included
+static inline bool sample_weighted(const dsgd_ctx *ctx) { return ctx->sw_on; }
 
 // every id names a loaded row (the reference indexes its data array with it); fn is the entry point
 static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn, const char *what) {
@@ -409,9 +415,10 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   snprintf(buf, sizeof buf,
            "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
-           "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g]}",
+           "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g], \"sample_weights\": %s}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
-           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1, ctx->cw_pos, ctx->cw_neg);
+           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1, ctx->cw_pos, ctx->cw_neg,
+           ctx->sw_on ? "true" : "false");
   ctx->info = buf;
   return ctx->info.c_str();
 }
@@ -516,8 +523,10 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
   CU(cudaSetDevice(ctx->device));
   // the staged stream was checked against the previous rows: a shorter set would leave ids past its end in it
   ctx->samples_n = 0;
+  // the sample weights named the previous rows: the ctx is unweighted again
+  ctx->sw_on = false;
   // all of the previous rows go before any of the new ones is allocated
-  CU(ctx->rp16.release()); CU(ctx->pairs.release()); CU(ctx->label.release()); CU(ctx->yabs.release());
+  CU(ctx->rp16.release()); CU(ctx->pairs.release()); CU(ctx->label.release()); CU(ctx->yabs.release()); CU(ctx->sw.release());
   const int64_t n_pairs = (int64_t)acc * 2;
   CU(ctx->rp16.alloc(n_rows + 1));
   CU(ctx->pairs.alloc(std::max<int64_t>(n_pairs, 1)));
@@ -852,6 +861,22 @@ static int launch_rows_class(dsgd_ctx *ctx, const row_set &rows, const double *w
   return DSGD_OK;
 }
 
+// The sample-weighted row kernel (k_rows_class<..., kSw>) over `rows` at any size, then k_sw_fold: with out == nullptr the
+// batch's weighted loss sum is left in cnt for a weighted tail (kCw), else ||w||^2 (*nrm), the three sums and the correct
+// count go to out.
+template <int kModel, bool kScatter>
+static int launch_rows_sw(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, const double *nrm = nullptr,
+                          double *out = nullptr) {
+  k_rows_class<kModel, kScatter, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+      ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
+      ctx->sw_on ? ctx->sw.p : nullptr);
+  LAUNCHED();
+  k_sw_fold<<<1, 1, 0, ctx->stream>>>(ctx->cnt, nrm, out);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  return DSGD_OK;
+}
+
 // The row kernel of a request: the fp32 streaming pass over kStreamMinRows rows or more (SVM only: it decides signs, and
 // the logistic loss needs the dot's value), else launch_rows.  Only an evaluation names a range of rows; a gradient or a
 // forward pass always lists them.
@@ -875,11 +900,14 @@ static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
   int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
   if (rc) return rc;
   const double n = (double)rows.n;
-  // a gradient of a class-weighted model: the fp64 class kernel at any size, and the tails of its weighted loss sum
-  const bool cw = kScatter && class_weighted(ctx);
-  if ((rc = cw ? launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32)
-               : request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr)))
-    return rc;
+  // a gradient of a class-weighted model: the fp64 class kernel at any size, and the tails of its weighted loss sum; of a
+  // sample-weighted one, the sample-weighted form of that kernel at any size and the same tails
+  const bool sw = kScatter && sample_weighted(ctx);
+  const bool cw = sw || (kScatter && class_weighted(ctx));
+  if (sw) rc = launch_rows_sw<kModel, true>(ctx, rows, w, ctx->g);
+  else if (cw) rc = launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32);
+  else rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr);
+  if (rc) return rc;
   auto tail = [&](auto weighted) {
     constexpr bool kCw = decltype(weighted)::value;
     if constexpr (kScatter) {
@@ -1069,6 +1097,51 @@ extern "C" int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+}
+
+// One weighted evaluation pass over `rows` (dsgd_eval*_weighted): k_rows_class<..., kSw> without the scatter, then
+// k_sw_fold.  Without sample weights the pass reads no weights: every s_i is 1 and c_i = w_y.
+static int weighted_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *norm_squared, double *sums,
+                         int64_t *counts) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd);
+  if (rc) return rc;
+  if ((rc = is_logistic(ctx) ? launch_rows_sw<kLogistic, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out)
+                             : launch_rows_sw<kSvm, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out)))
+    return rc;
+  double out[5];
+  CU(cudaMemcpyAsync(out, ctx->cls_out, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  if (norm_squared) *norm_squared = out[0];
+  if (sums)
+    for (int k = 0; k < 3; ++k) sums[k] = out[1 + k];
+  if (counts) { counts[0] = rows.n; counts[1] = (int64_t)out[4]; }
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
+                                  double *sums_out, int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
+}
+
+extern "C" int dsgd_eval_sampled_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                          int64_t pos_begin, int64_t pos_end, double *norm_squared, double *sums_out,
+                                          int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
+}
+
+extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                          double *norm_squared, double *sums_out, int64_t *counts_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
 }
 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
@@ -1538,20 +1611,29 @@ extern "C" int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYT
 // ---- persistent sync loop (dsgd_persistent.cuh) ----------------------------------------------------------------
 constexpr int kPCons = 8, kPUpd = 6, kPStages = 8, kPStagePairs = 2560, kPMaxChunks = 128;
 using PSmem = PersistSmem<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks>;
-// Every instantiation of k_sync_persistent, form f = 16 multi + 8 l1 + 4 cw + 2 avg + lr_table.  The fused K-GPU kernel
-// (multi) has no L1 or class-weighted form, so the forms are exactly f < 20.
-constexpr int kPersistForms = 20;
+// Every instantiation of k_sync_persistent, form f = 16 multi + 8 l1 + 4 cw + 2 avg + lr_table for f < 20, and the
+// sample-weighted forms f = 20 + 4 l1 + 2 avg + lr_table.  The fused K-GPU kernel (multi) has no L1, class- or
+// sample-weighted form, and the sample-weighted forms include the class weights, so there are exactly 28 forms.
+constexpr int kPersistForms = 28, kPersistSwForm = 20;
+constexpr bool pf_sw(int f) { return f >= kPersistSwForm; }
+constexpr bool pf_multi(int f) { return !pf_sw(f) && (f & 16) != 0; }
+constexpr bool pf_l1(int f) { return pf_sw(f) ? ((f - kPersistSwForm) & 4) != 0 : (f & 8) != 0; }
+constexpr bool pf_cw(int f) { return !pf_sw(f) && (f & 4) != 0; }
 template <int... F>
 static void *const *persist_forms(std::integer_sequence<int, F...>) {
-  static void *const k[] = {(void *)k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, (F & 16) != 0,
-                                                      (F & 2) != 0, (F & 1) != 0, (F & 8) != 0, (F & 4) != 0>...};
+  static void *const k[] = {(void *)k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, pf_multi(F),
+                                                      (F & 2) != 0, (F & 1) != 0, pf_l1(F), pf_cw(F), pf_sw(F)>...};
   return k;
 }
 static void *const *const kPersistKernels = persist_forms(std::make_integer_sequence<int, kPersistForms>{});
-// The form that runs a launch with these options; l1 and cw are not read for the fused kernel.
-static void *persist_kernel(bool multi, bool avg, bool lr_table, bool l1, bool cw) {
-  return kPersistKernels[multi ? 16 + 2 * avg + lr_table : 8 * l1 + 4 * cw + 2 * avg + lr_table];
+// The form that runs a launch with these options; l1, cw and sw are not read for the fused kernel, cw not with sw.
+static int persist_form(bool multi, bool avg, bool lr_table, bool l1, bool cw, bool sw) {
+  if (multi) return 16 + 2 * avg + lr_table;
+  if (sw) return kPersistSwForm + 4 * l1 + 2 * avg + lr_table;
+  return 8 * l1 + 4 * cw + 2 * avg + lr_table;
 }
+// Dynamic shared memory of form f: the sample-weighted forms keep their combined weights and hinge codes past PSmem
+static size_t persist_smem(int f) { return sizeof(PSmem) + (f >= kPersistSwForm ? sizeof(PersistSwSmem<kPStages>) : 0); }
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -1568,12 +1650,14 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
     CU(ctx->p_acc.alloc(3 * kAccStride));
     CU(ctx->p_bar.alloc(4));
     for (int f = 0; f < kPersistForms; ++f)
-      CU(cudaFuncSetAttribute(kPersistKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PSmem)));
+      CU(cudaFuncSetAttribute(kPersistKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)persist_smem(f)));
     ctx->p_ready = true;
   }
   // sized for the largest grid (persist_grid), which dsgd_reserve does not know yet
   int rc = ctx->p_hinge.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count);
   if (rc) return rc;
+  // the hinge codes of the sample-weighted forms, only while sample weights are loaded
+  if (ctx->sw_on && (rc = ctx->p_hcode.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count))) return rc;
   return ctx->p_loss_nrm.grow(ctx, 2 * n_steps, 2 * 4096);
 }
 
@@ -1595,9 +1679,11 @@ static bool persist_multi_fits(const dsgd_ctx *ctx, int G) {
 // grid limit (several contexts sharing one GPU: the K-rank tests on one device) the kernels of the ranks must also run
 // CONCURRENTLY, which cooperative launches of different contexts do not (measured: they serialise and the ranks time
 // out waiting for each other); a plain launch of at most one CTA per SM on an otherwise idle GPU is resident in full too.
-static cudaError_t persist_launch(dsgd_ctx *ctx, void *fn, int G, void **args) {
-  if (ctx->grid_limit > 0) return cudaLaunchKernel(fn, dim3(G), dim3((kPCons + kPUpd + 1) * 32), args, sizeof(PSmem), ctx->stream);
-  return cudaLaunchCooperativeKernel(fn, dim3(G), dim3((kPCons + kPUpd + 1) * 32), args, sizeof(PSmem), ctx->stream);
+static cudaError_t persist_launch(dsgd_ctx *ctx, int form, int G, void **args) {
+  void *fn = kPersistKernels[form];
+  const size_t smem = persist_smem(form);
+  if (ctx->grid_limit > 0) return cudaLaunchKernel(fn, dim3(G), dim3((kPCons + kPUpd + 1) * 32), args, smem, ctx->stream);
+  return cudaLaunchCooperativeKernel(fn, dim3(G), dim3((kPCons + kPUpd + 1) * 32), args, smem, ctx->stream);
 }
 
 // ---- fused K-GPU loop: all ranks run the persistent kernel and exchange gradients through peer memory ----
@@ -1692,14 +1778,17 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.lr = 0.0;   // not read: interval 0, the only one before lrs[0] is loaded, applies no update
   }
   void *args[] = {&pp};
-  // the L1 forms only with a penalty, the class-weighted forms only with weights other than (1, 1) (neither fused:
-  // sync_staged keeps such a ctx off the fused path)
+  // the L1 forms only with a penalty, the class-weighted forms only with weights other than (1, 1), the sample-weighted
+  // forms (which include the class weights) whenever sample weights are loaded (none fused: sync_staged keeps such a ctx
+  // off the fused path)
   const bool l1 = !multi && ctx->lambda1 > 0.0;
   pp.lambda1 = l1 ? ctx->lambda1 : 0.0;
   pp.w_pos = ctx->cw_pos; pp.w_neg = ctx->cw_neg;
-  void *fn = persist_kernel(multi, ctx->avg_on, lrs_host != nullptr, l1, class_weighted(ctx));
+  const bool sw = !multi && sample_weighted(ctx);
+  if (sw) { pp.sw = ctx->sw; pp.hcode = ctx->p_hcode; }
+  const int form = persist_form(multi, ctx->avg_on, lrs_host != nullptr, l1, class_weighted(ctx), sw);
   cudaError_t launch_err = cudaSuccess;
-  profiled(ctx, [&] { launch_err = persist_launch(ctx, fn, G, args); });
+  profiled(ctx, [&] { launch_err = persist_launch(ctx, form, G, args); });
   CU(launch_err);
   LAUNCHED();
   if (ctx->avg_on) ctx->avg_n += n_steps;
@@ -1853,7 +1942,8 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
 
 // The per-step path of sync_staged for model kModel: n_steps steps of n_per_step staged ids from smp, step s at the rate
 // lrs[s] (lrs == nullptr: lr), its loss into losses[s] (losses == nullptr: none)
-// kCw: a class-weighted ctx -- every worker's pass is k_rows_class + k_class_fold, and the tails read the weighted loss sum
+// kCw: a class- or sample-weighted ctx -- every worker's pass is k_rows_class + k_class_fold (with sample weights
+// k_rows_class<..., kSw> + k_sw_fold), and the tails read the weighted loss sum
 template <int kModel, bool kCw>
 static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, int64_t n_steps, double lr,
                          const double *lrs, double *losses, bool single, int32_t k_total) {
@@ -1872,8 +1962,13 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   double *const avg = ctx->avg_on ? ctx->avg.p : nullptr;
 
   auto rows_pass = [&](const row_set &rows) {
-    if constexpr (kCw) launch_rows_class<kModel, true>(ctx, rows, ctx->w, ctx->g);
-    else launch_rows<kModel, true>(ctx, rows, ctx->w, ctx->g);
+    if constexpr (kCw) {
+      if (sample_weighted(ctx)) return launch_rows_sw<kModel, true>(ctx, rows, ctx->w, ctx->g);
+      return launch_rows_class<kModel, true>(ctx, rows, ctx->w, ctx->g);
+    } else {
+      launch_rows<kModel, true>(ctx, rows, ctx->w, ctx->g);
+      return DSGD_OK;
+    }
   };
 
   for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
@@ -1883,13 +1978,17 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     double k_den = 1.0, n_local = (double)n_per_step;
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
-      profiled(ctx, [&] { rows_pass({smp, 0, n_per_step}); });
+      int rc = DSGD_OK;
+      profiled(ctx, [&] { rc = rows_pass({smp, 0, n_per_step}); });
+      if (rc) return rc;
     } else {
       // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
       int64_t off = 0;
       for (int32_t v = 0; v < ctx->n_local; ++v) {
         const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
-        profiled(ctx, [&] { rows_pass({smp + off, 0, nv}); });
+        int rc = DSGD_OK;
+        profiled(ctx, [&] { rc = rows_pass({smp + off, 0, nv}); });
+        if (rc) return rc;
         k_finish_acc<kModel, kCw><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC,
                                                                        ctx->cnt, (double)nv, v == 0 ? 1 : 0);
         LAUNCHED();
@@ -1938,13 +2037,15 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
   // The options the fused kernel has no form of, which with world > 1 take the per-step path over NCCL: the persistent and
-  // fused kernels are SVM-only (a logistic ctx always takes the per-step path below), and an L1 penalty or class weights
-  // have only one-GPU persistent forms.  unfused names the first of them that is on.
+  // fused kernels are SVM-only (a logistic ctx always takes the per-step path below), and an L1 penalty, class weights or
+  // sample weights have only one-GPU persistent forms.  unfused names the first of them that is on.
   const bool logistic = is_logistic(ctx);
-  const bool cw = class_weighted(ctx);
+  const bool sw = sample_weighted(ctx);
+  const bool cw = class_weighted(ctx) || sw;
   const char *unfused = logistic ? "the logistic model takes"
                         : ctx->lambda1 > 0.0 ? "the L1 penalty takes"
-                        : cw ? "class weights take" : nullptr;
+                        : class_weighted(ctx) ? "class weights take"
+                        : sw ? "sample weights take" : nullptr;
   NEED(!unfused || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
        "dsgd_sync_steps: %s the NCCL allreduce path for world > 1, which needs dsgd_comm_init", unfused);
   const bool fused = !unfused && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
@@ -2058,6 +2159,31 @@ extern "C" int dsgd_get_class_weights(const dsgd_ctx *ctx, double *w_pos_out, do
   if (!ctx || !w_pos_out || !w_neg_out) return DSGD_ERR_INVALID;
   *w_pos_out = ctx->cw_pos;
   *w_neg_out = ctx->cw_neg;
+  return DSGD_OK;
+}
+
+// ---- sample weights of the sync steps, of dsgd_gradient and of dsgd_eval*_weighted -------------------------------------
+
+extern "C" int dsgd_set_sample_weights(dsgd_ctx *ctx, const double *sw, int64_t n) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE,
+       "dsgd_set_sample_weights: ctx is in async mode (sample weights belong to the sync paths)");
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_set_sample_weights: no rows loaded");
+  if (!sw && n == 0) {
+    ctx->sw_on = false;
+    return DSGD_OK;
+  }
+  NEED(sw && n == ctx->n_rows, DSGD_ERR_INVALID, "dsgd_set_sample_weights: %lld weights for %lld loaded rows", (long long)n,
+       (long long)ctx->n_rows);
+  for (int64_t i = 0; i < n; ++i)
+    NEED(std::isfinite(sw[i]) && sw[i] >= 0.0, DSGD_ERR_INVALID,
+         "dsgd_set_sample_weights: weight %g of row %lld is not finite and >= 0", sw[i], (long long)i);
+  CU(cudaSetDevice(ctx->device));
+  int rc = ctx->sw.grow(ctx, n, n);
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(ctx->sw, sw, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  ctx->sw_on = true;
   return DSGD_OK;
 }
 

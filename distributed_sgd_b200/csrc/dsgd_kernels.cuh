@@ -45,10 +45,16 @@ enum Cnt : int {
   kCntClassCorrect = 26,  // #{pred == y}
   kCntClassHinge = 28,    // SVM: hinge sums (integers)
   kCntClassLoss = 32,     // logistic: two fixed-point sums of the unweighted losses, kLossAccWords words each
-  kNumCnt = 48
+  // fixed-point sums of k_rows_class<..., kSw> (kLossAccWords words each), taken by k_sw_fold: S = sum R(c_i L_i), and for an
+  // evaluation sum R(c_i [pred_i == y_i]) and sum R(c_i)
+  kCntSwLoss = 48,
+  kCntSwCorrect = 56,
+  kCntSwWeight = 64,
+  kNumCnt = 72
 };
 static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kCntNnz && kCntNnz < kCntClassN &&
-                  kCntClassLoss + 2 * kLossAccWords <= kNumCnt,
+                  kCntClassLoss + 2 * kLossAccWords <= kCntSwLoss && kCntSwLoss + kLossAccWords <= kCntSwCorrect &&
+                  kCntSwCorrect + kLossAccWords <= kCntSwWeight && kCntSwWeight + kLossAccWords <= kNumCnt,
               "counter block");
 
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
@@ -327,6 +333,93 @@ __global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restric
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Sample weights (dsgd_set_sample_weights): k_rows_class<..., kSw>.  Row i has the combined weight c_i = fl(w_y * s_i) (w_y its
+// class weight, s_i its sample weight); the dot, the prediction, the SVM's gate and the unweighted per-sample loss L_i are those
+// of the class form, and the scatter value is c_i in place of w_y:
+//   SVM       s = y * c_i          (an exact sign flip),  added where !(y * dot < 0)
+//   logistic  s = (y * sigmoid(z)) * c_i
+// sw == nullptr (an evaluation of a ctx without sample weights): every s_i is 1.
+// Lane 0 adds R(fl(c_i * L_i)) into one fixed-point limb block (S, kCntSwLoss) and counts the correct rows in kCntCorrect; the
+// evaluation pass (kScatter = false) also adds R(c_i) of the correct rows (kCntSwCorrect) and of every row (kCntSwWeight).
+// Integer additions commute, so every sum has the same bits in any row order or grid.  With s = 1 and w = (1, 1) the SVM's
+// S is the integer hinge sum and the logistic S is k_rows_logistic's limb sum.
+// k_sw_fold, one thread after the pass: S's bits into cnt[kCntWLoss] for the weighted tails (out == nullptr; the correct
+// count stays in kCntCorrect), or {||w||^2, S, sum c_i [correct], sum c_i, correct} into out[0..4] (an evaluation).  The
+// limb blocks, and in an evaluation the correct count, are cleared either way.
+// ---------------------------------------------------------------------------------------------------
+template <int kModel, bool kScatter>
+__device__ __forceinline__ void rows_sample_weighted(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                     const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                     int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                     double *__restrict__ g, unsigned long long *__restrict__ cnt,
+                                                     double w_pos, double w_neg, const double *__restrict__ sw) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned correct = 0;  // lane 0 only
+  unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
+  unsigned long long lim_ok[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_ok = 0;
+  unsigned long long lim_w[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0;
+  for (int64_t i = warp0; i < n; i += nwarps) {
+    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
+    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
+    const int yi = (int)label[r];
+    const bool pos = yi > 0;
+    const double y = (double)yi;
+    const double z = y * dot;
+    const double ci = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r]) : 1.0);   // sw == nullptr: every s_i is 1
+    if (lane == 0) {
+      const int p = pred_of(dot);
+      const bool ok = p == yi;
+      correct += (unsigned)ok;
+      const double l = kModel == kLogistic ? softplus(z) : (double)(1 - yi * p);
+      acc_add_local(lim, ovf, ci * l);
+      if (!kScatter) {
+        acc_add_local(lim_ok, ovf_ok, ok ? ci : 0.0);
+        acc_add_local(lim_w, ovf_w, ci);
+      }
+    }
+    if (kScatter) {
+      double s;
+      if (kModel == kLogistic) {
+        s = (y * sigmoid(z)) * ci;
+      } else {
+        if (z < 0.0) continue;  // SparseSVM.scala:28
+        s = pos ? ci : -ci;
+      }
+      for (int64_t k = b + lane; k < e; k += 32) {
+        const uint2 pr = pairs[k];
+        const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);
+        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
+      }
+    }
+  }
+  if (lane == 0) {
+    if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
+    acc_flush_local(cnt + kCntSwLoss, lim, ovf);
+    if (!kScatter) {
+      acc_flush_local(cnt + kCntSwCorrect, lim_ok, ovf_ok);
+      acc_flush_local(cnt + kCntSwWeight, lim_w, ovf_w);
+    }
+  }
+}
+
+__global__ void k_sw_fold(unsigned long long *__restrict__ cnt, const double *__restrict__ scal_nrm2, double *__restrict__ out) {
+  const double s = acc_take(cnt + kCntSwLoss);
+  if (out) {
+    out[0] = *scal_nrm2;
+    out[1] = s;
+    out[2] = acc_take(cnt + kCntSwCorrect);
+    out[3] = acc_take(cnt + kCntSwWeight);
+    out[4] = (double)cnt[kCntCorrect];
+    cnt[kCntCorrect] = 0ull;
+  } else {
+    cnt[kCntWLoss] = (unsigned long long)__double_as_longlong(s);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Class weights (dsgd_set_class_weights).  k_rows_class is the row kernel of either model with one weight per class: the dot,
 // the prediction, the SVM's gate and the unweighted per-sample loss are those of k_rows / k_rows_logistic; the scatter value
 // is scaled by the weight of the row's class,
@@ -340,12 +433,16 @@ __global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restric
 // total into cnt[kCntCorrect] for the weighted tails (out == nullptr), or the per-class totals and ||w||^2 into out[0..6]
 // (an evaluation); the per-class words are cleared either way.
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kScatter>
+template <int kModel, bool kScatter, bool kSw = false>
 __global__ void __launch_bounds__(256) k_rows_class(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                     int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                     double *__restrict__ g, unsigned long long *__restrict__ cnt,
-                                                    double w_pos, double w_neg) {
+                                                    double w_pos, double w_neg, const double *__restrict__ sw = nullptr) {
+  if constexpr (kSw) {
+    rows_sample_weighted<kModel, kScatter>(rp16, pairs, label, samples, row_begin, n, w, g, cnt, w_pos, w_neg, sw);
+    return;
+  }
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);

@@ -51,6 +51,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "dsgd_fixed.cuh"
 #include "dsgd_kernels.cuh"
 
@@ -99,6 +101,9 @@ struct PersistParams {
   double *loss_nrm;                       // [2][n_steps]: ||W_t||^2, then (kL1) ||W_t||_1, of every step t of the launch
   // ---- class weights (kCw, one GPU); last for the same reason ----
   double w_pos, w_neg;                    // a row of label y scatters x * (y * w_y); the step's loss is (w_pos H+ + w_neg H-) / batch
+  // ---- sample weights (kSw, one GPU); last for the same reason ----
+  const double *sw;                       // [rows]: row i scatters x * (y * c_i), c_i = w_y * sw[i]
+  unsigned long long *hcode;              // [n_steps][gridDim.x]: the 2-bit hinge codes of every step's rows of every CTA
 };
 static_assert(sizeof(PersistParams) <= 4000, "kernel parameter space is 4 KB");
 
@@ -260,6 +265,14 @@ struct StageMeta {
   double part[kMaxChunks];           // pass-1 partial dot of the chunk
 };
 
+// kSw: shared memory past the end of PersistSmem (the other forms launch without it) -- the combined weight c_i of every row of
+// every stage, written by the producer with the stage's metadata, and the 2-bit hinge codes of the CTA's rows of the step
+template <int kStages>
+struct PersistSwSmem {
+  double row_c[kStages][kMaxRowsPerCta];
+  unsigned long long code;
+};
+
 template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks>
 struct PersistSmem {
   uint2 ring[kStages][kStagePairs];
@@ -411,15 +424,26 @@ __device__ __forceinline__ void chunk_pairs(const StageMeta<kMaxChunks> &mt, con
 // kCw (class weights): a row of label y scatters x * s with s = y * w_y instead of x * y, at all three scatter sites, and its
 // hinge loss is counted in the low 16 bits of the returned word for y = +1 and in the high 16 bits for y = -1.  A CTA holds
 // at most kMaxRowsPerCta = 32 rows of hinge <= 2 per step, so a half holds at most 64 and never carries into the other.
-template <int kCons, int kMaxChunks, bool kCw = false, class Fetch>
-__device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, double *gbase,
-                                                  const int gstride, Fetch &fetch, int warp, int lane, long long *tl,
-                                                  const uint2 (*pre)[4] = nullptr, double w_pos = 1.0, double w_neg = 1.0) {
+// kSw (sample weights): row m of the stage scatters x * s with s = y * row_c[m] (row_c: the stage's combined weights), and its
+// hinge loss l in {0, 1, 2} is returned as the code l << 2 m of a 64-bit word: 32 rows x 2 bits, no carries.
+template <int kCons, int kMaxChunks, bool kCw = false, bool kSw = false, class Fetch>
+__device__ __forceinline__ std::conditional_t<kSw, unsigned long long, unsigned> consume_stage(
+    StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, double *gbase, const int gstride, Fetch &fetch, int warp,
+    int lane, long long *tl, const uint2 (*pre)[4] = nullptr, double w_pos = 1.0, double w_neg = 1.0,
+    const double *row_c = nullptr) {
+  static_assert(!(kCw && kSw), "kSw forms the combined weight itself");
+  using Hinge = std::conditional_t<kSw, unsigned long long, unsigned>;
   const int n_ch = mt.n_chunks;
-  unsigned hinge = 0;  // lane 0 only
-  // the scatter scalar of a row, and its hinge loss in its class's half
-  auto scale_of = [&](int yi, double y) { return kCw ? (yi > 0 ? w_pos : -w_neg) : y; };
-  auto hinge_of = [&](int yi, unsigned l) { return kCw ? l << (yi > 0 ? 0 : 16) : l; };
+  Hinge hinge = 0;  // lane 0 only
+  // the scatter scalar of row m, and its hinge loss in its class's half (kCw) or its code (kSw)
+  auto scale_of = [&](int yi, double y, int m) {
+    if constexpr (kSw) return yi > 0 ? row_c[m] : -row_c[m];
+    return kCw ? (yi > 0 ? w_pos : -w_neg) : y;
+  };
+  auto hinge_of = [&](int yi, unsigned l, int m) -> Hinge {
+    if constexpr (kSw) return (Hinge)l << (2 * m);
+    return kCw ? l << (yi > 0 ? 0 : 16) : l;
+  };
   // ---- pass 1: dots of this warp's chunks ----
   for (int c = warp; c < n_ch; c += kCons) {
     uint2 pr[4];
@@ -442,9 +466,9 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       if (mt.row_nch[row1] == 1) {
         const int yi = mt.row_y[row1];
         const double y = (double)yi;
-        if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(acc)));
+        if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(acc)), row1);
         if (!(y * acc < 0.0)) {  // SparseSVM.scala:28
-          const double sc = scale_of(yi, y);
+          const double sc = scale_of(yi, y, row1);
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const double gvv = filt(filt((double)__uint_as_float(pr[u].y)) * sc);
@@ -467,9 +491,9 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       for (int i = 0; i < nch; ++i) dot += mt.part[first + i];
       const int yi = mt.row_y[row];
       const double y = (double)yi;
-      if (c == first && lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)));
+      if (c == first && lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)), row);
       if (!(y * dot < 0.0)) {
-        const double sc = scale_of(yi, y);
+        const double sc = scale_of(yi, y, row);
         const uint32_t off = mt.ch_off[c];
         const int n = mt.ch_n[c];
         const uint2 *src = (off & kChunkGlobal) ? (pairs + (off & ~kChunkGlobal)) : (ring + off);
@@ -486,7 +510,7 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
   for (int m = warp; m < mt.n_rows; m += kCons) {
     const int nch = mt.row_nch[m];
     if (nch == 0) {
-      if (lane == 0) hinge += hinge_of(mt.row_y[m], 1u);
+      if (lane == 0) hinge += hinge_of(mt.row_y[m], 1u, m);
     } else if (nch < 0) {
       const uint2 *grow = pairs + (size_t)mt.row_b[m] * 2;
       const int len = mt.row_len[m];
@@ -494,11 +518,11 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
       const double dot = row_fold(grow, 0, len, lane, [&](uint32_t c) { return fetch.get1(c); });
       const int yi = mt.row_y[m];
       const double y = (double)yi;
-      if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)));
+      if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(dot)), m);
       if (!(y * dot < 0.0))
         for (int k = lane; k < len; k += 32) {
           const uint2 pr = __ldg(&grow[k]);
-          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * scale_of(yi, y));
+          const double gvv = filt(filt((double)__uint_as_float(pr.y)) * scale_of(yi, y, m));
           if (gvv != 0.0) red_add_f64(gbase + (size_t)gstride * pr.x, gvv);
         }
     }
@@ -523,16 +547,26 @@ __device__ __forceinline__ unsigned consume_stage(StageMeta<kMaxChunks> &mt, con
 // hinge counts of the two classes into the halves of the word it already accumulates in sm.hinge_acc and stores in its
 // hinge[t * G + CTA] slot (no new buffer, nothing new on the barrier path); the epilogue's per-step warp splits the halves,
 // sums each over the G slots in integers and forms (w_pos * H+ + w_neg * H-) / batch once.
+// kSw (one GPU only): sample weights -- the producer lane that loads row m's label also loads its sample weight and puts the
+// combined weight c = w_y * sw[id] beside the stage's metadata (PersistSwSmem, past the end of PersistSmem); consume_stage
+// scales every scatter by it and returns the rows' 2-bit hinge codes, which the consumer warps OR into one shared word.  The
+// thread that arrives at the grid barrier stores that word into hcode[t * G + CTA] and clears it after the barrier has passed
+// (nothing new before the arrival); the epilogue's per-step warp re-forms S = sum R(c_i * code_i) of the step in fixed-point
+// limbs from the codes, p.samples, the labels and the weights.  Includes the class weights; never set with kCw.
 template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable,
-          bool kL1 = false, bool kCw = false>
+          bool kL1 = false, bool kCw = false, bool kSw = false>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
   static_assert(!kL1 || (!kMulti && kUpd <= kCons), "the L1 form is one-GPU only and keeps its partials in the consumers' slots");
   static_assert(!kCw || !kMulti, "the class-weighted form is one-GPU only");
+  static_assert(!kSw || (!kMulti && !kCw), "the sample-weighted form is one-GPU only and forms the class weights itself");
+  static_assert(2 * kMaxRowsPerCta <= 64, "a CTA's hinge codes of one step fit one 64-bit word");
   static_assert(2 * kMaxRowsPerCta < (1 << 16), "a CTA's hinge count of one class fits a 16-bit half");
   static_assert(kAccWords + kAccLimbs <= kAccStride, "the L1 limbs follow the accumulator's overflow word");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
+  using SwSmem = PersistSwSmem<kStages>;
+  SwSmem &swm = *reinterpret_cast<SwSmem *>(smem_raw + sizeof(Smem));   // kSw only: launched with the larger size
 
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -556,6 +590,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     sm.c_val[0] = 0.0;   // interval 0 has no pending update (g_{-1} == 0): its c is never used
     sm.nrm_val[0] = 0.0;
     sm.hinge_acc = 0u;
+    if constexpr (kSw) swm.code = 0ull;
     sm.ok = 1;
   }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -571,16 +606,19 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     };
     uint32_t b0 = 0, e0 = 0, b1 = 0, e1 = 0;
     int y0 = 0, y1 = 0;
-    auto load_win = [&](int32_t id, uint32_t &b, uint32_t &e, int &y) {
+    double s0 = 0.0, s1 = 0.0;   // kSw: the sample weights of the two windows
+    auto load_win = [&](int32_t id, uint32_t &b, uint32_t &e, int &y, double &sw) {
       b = 0u; e = 0u; y = 0;
+      if constexpr (kSw) sw = 0.0;
       if (id >= 0) {
         b = __ldg(&p.rp16[id]);
         e = __ldg(&p.rp16[id + 1]);
         y = (int)__ldg(&p.label[id]);
+        if constexpr (kSw) sw = __ldg(&p.sw[id]);
       }
     };
-    load_win(load_id(0), b0, e0, y0);   // window of step t      (stage C input)
-    load_win(load_id(1), b1, e1, y1);   // window of step t + 1  (stage B)
+    load_win(load_id(0), b0, e0, y0, s0);   // window of step t      (stage C input)
+    load_win(load_id(1), b1, e1, y1, s1);   // window of step t + 1  (stage B)
     int32_t id_next = load_id(2);       // sample id of step t + 2 (stage A)
     for (int64_t t = 0; t < S; ++t) {
       const int st = (int)t & (kStages - 1);
@@ -603,6 +641,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       const bool in_ring = listed && (my_pair + len) <= kStagePairs;
       if (lane < n_r) {
         mt.row_y[lane] = y0;
+        if constexpr (kSw) swm.row_c[st][lane] = (y0 > 0 ? p.w_pos : p.w_neg) * s0;
         mt.row_b[lane] = b0;
         mt.row_len[lane] = len;
         mt.row_first[lane] = (short)my_chunk;
@@ -637,7 +676,8 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       if (my_bytes) bulk_g2s(&sm.ring[st][my_pair], p.pairs + (size_t)b0 * 2, my_bytes, &sm.full[st]);
       // advance the register pipeline
       b0 = b1; e0 = e1; y0 = y1;
-      load_win(id_next, b1, e1, y1);
+      if constexpr (kSw) s0 = s1;
+      load_win(id_next, b1, e1, y1, s1);
       id_next = load_id(t + 3);
     }
     return;
@@ -981,9 +1021,14 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           auto &mt = sm.meta[st];   // full: waited for by prefetch(t)
           FetchLocal<kL1> fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
           if constexpr (kL1) fetch.tau = tau;
-          const unsigned hinge = consume_stage<kCons, kMaxChunks, kCw>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
-                                                                       lane, warp == 0 ? tl_row : nullptr, &pre, p.w_pos, p.w_neg);
-          if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
+          const auto hinge = consume_stage<kCons, kMaxChunks, kCw, kSw>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
+                                                                        lane, warp == 0 ? tl_row : nullptr, &pre, p.w_pos, p.w_neg,
+                                                                        kSw ? swm.row_c[st] : nullptr);
+          if constexpr (kSw) {
+            if (lane == 0 && hinge) atomicOr(&swm.code, hinge);
+          } else {
+            if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
+          }
           if (tl_rec && warp == 0 && lane == 0) tl_rec[2] = mt.n_pairs;
           __syncwarp();
           if (lane == 0) mbar_arrive(&sm.empty[st]);
@@ -1076,6 +1121,14 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       // release of this arrival does not wait for it (a count shared by all CTAs was one same-address atomic per CTA in front
       // of every arrival), and the next one finds it long done.  Nothing reads it before the epilogue.
       if (!kMulti && !last && p.losses) p.hinge[(size_t)t * G + blockIdx.x] = h;
+      // kSw: the rows' hinge codes of step t, the same way.  Every consumer warp OR'd its codes in before barrier 3, and the
+      // consumers of step t + 1 start after barrier 4: the word is read and cleared in between.
+      if constexpr (kSw) {
+        if (!last) {
+          if (p.losses) p.hcode[(size_t)t * G + blockIdx.x] = swm.code;
+          swm.code = 0ull;
+        }
+      }
     }
     named_bar_sync(4, kSyncThreads);
     if (*(volatile int *)&sm.ok == 0) return;
@@ -1099,7 +1152,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   // one GPU: loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + hinge_s/batch (SparseSVM.scala:20-23; SURVEY.md F5), one
   // warp per step.  The hinge count is the integer sum of the CTAs' slots, the same in any order.  Every slot and norm was
   // stored before the last barrier's arrivals, and is read through L2 (see grid_barrier_arrive_wait).
-  if constexpr (!kMulti) {
+  if constexpr (!kMulti && !kSw) {
     if (p.losses) {
       for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
         unsigned h = 0;
@@ -1163,6 +1216,38 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       const double wv = __ldcg(&Rfin[j]).x;
       p.w_out[j] = wv;
       p.w32_out[j] = (float)wv;
+    }
+  }
+  // kSw: the loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + S_s / batch, S_s = sum R(c_i * code_i) over the step's rows
+  // (row i of the step is row i / G of CTA i % G), summed in fixed-point limbs: the same bits in any order.  After the weights
+  // are stored, so that the limbs do not share the registers that hold them.
+  if constexpr (kSw) {
+    if (p.losses) {
+      for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
+        unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
+        for (int i = lane; i < B; i += 32) {
+          const int b = i % G, m = i / G;
+          const unsigned code = (unsigned)(__ldcg(&p.hcode[s * G + b]) >> (2 * m)) & 3u;
+          const int32_t id = __ldg(&p.samples[s * B + i]);
+          const double c = (__ldg(&p.label[id]) > 0 ? p.w_pos : p.w_neg) * __ldg(&p.sw[id]);
+          acc_add_local(lim, ovf, c * (double)code);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {   // limbs 0..4 below 2^40 per lane: the warp's sums stay below 2^45
+#pragma unroll
+          for (int k = 0; k < kLossLimbs; ++k) lim[k] += __shfl_xor_sync(0xffffffffu, lim[k], o);
+          ovf += __shfl_xor_sync(0xffffffffu, ovf, o);
+        }
+        if (lane == 0) {
+          unsigned long long q[kLossAccWords];
+#pragma unroll
+          for (int k = 0; k < kLossLimbs; ++k) q[k] = lim[k];
+          q[kLossLimbs] = ovf;
+          double pen = p.lambda * __ldcg(&p.loss_nrm[s]);
+          if constexpr (kL1) pen = pen + p.lambda1 * __ldcg(&p.loss_nrm[S + s]);
+          p.losses[s] = pen + acc_value(q) / (double)B;
+        }
+      }
     }
   }
 }

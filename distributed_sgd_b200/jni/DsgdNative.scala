@@ -117,6 +117,16 @@ object DsgdNative {
                                posEnd: Long, sums: Array[Double], counts: Array[Long]): Int
   @native def evalSamplesClass(ctx: Long, w: Array[Double], samples: Array[Int], sums: Array[Double],
                                counts: Array[Long]): Int
+  // sample weights of the sync steps, of gradient and of the weighted evaluations: one per loaded row (finite and >= 0), null
+  // clears them.  The weighted evaluations, either model: sums = {||w||^2, S = sum c_i L_i, sum c_i [correct], sum c_i},
+  // counts = {rows, correct}
+  @native def setSampleWeights(ctx: Long, sw: Array[Double]): Int
+  @native def evalWeighted(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, sums: Array[Double],
+                           counts: Array[Long]): Int
+  @native def evalSampledWeighted(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                  posEnd: Long, sums: Array[Double], counts: Array[Long]): Int
+  @native def evalSamplesWeighted(ctx: Long, w: Array[Double], samples: Array[Int], sums: Array[Double],
+                                  counts: Array[Long]): Int
   // async (Hogwild) mode
   @native def asyncHostMaster(ctx: Long, w0: Array[Double]): Int
   @native def ipcExport(ctx: Long, which: Int, handle: Array[Byte]): Int

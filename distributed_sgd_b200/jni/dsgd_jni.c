@@ -604,6 +604,58 @@ FN(evalSamplesClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArr
   return rc;
 }
 
+/* Sample weights of the sync steps, of gradient and of the weighted evaluations: setSampleWeights(sw), one weight per loaded
+ * row (finite and >= 0; the library checks the length against the rows), null clears them.  The weighted evaluations, either
+ * model: sums(0) = ||w||^2, sums(1..3) = S = sum c_i L_i, sum c_i [correct], sum c_i; counts(0..1) = rows, correct.  A w
+ * whose length is not dim, or a shorter output, is DSGD_ERR_INVALID. */
+FN(setSampleWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray sw) {
+  buf_t b = in_Double(env, sw);
+  int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_set_sample_weights(CTX(h), (const double *)b.p, b.p ? (int64_t)b.n : 0);
+  free(b.p);
+  return rc;
+}
+/* DSGD_OK when w is null or holds dim values and the outputs are long enough */
+static int weighted_args(jlong h, const buf_t *bw, const buf_t *bs, const buf_t *bc) {
+  int32_t dim = 0;
+  int rc = dsgd_dim(CTX(h), &dim);
+  if (rc) return rc;
+  return ((bw->p && (int32_t)bw->n != dim) || bs->n < 4 || bc->n < 2) ? DSGD_ERR_INVALID : DSGD_OK;
+}
+FN(evalWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray sums,
+                 jlongArray counts) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
+    rc = dsgd_eval_weighted(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                        jlong posBegin, jlong posEnd, jdoubleArray sums, jlongArray counts) {
+  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
+    rc = dsgd_eval_sampled_weighted(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (double *)bs.p,
+                                    (double *)bs.p + 1, (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray sums,
+                        jlongArray counts) {
+  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, sums), bc = out_Long(env, counts);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bi.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
+    rc = dsgd_eval_samples_weighted(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
+  back_Double(env, sums, bs, rc);
+  back_Long(env, counts, bc, rc);
+  free(bw.p); free(bi.p);
+  return rc;
+}
+
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {
   buf_t b = in_Double(env, w0);

@@ -13,6 +13,7 @@ the device), model (:68), initial distributed loss / accuracy (:75-78), fit (:80
 from __future__ import annotations
 
 import argparse
+import dataclasses
 import json
 import os
 import time
@@ -41,6 +42,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     class_weight = parse_class_weight(cfg.class_weight)
     if class_weight is not None and cfg.is_async:
         raise ValueError("class-weight: class weights belong to sync training; asynchronous (Hogwild) training has none")
+    from .utils.dataset import SAMPLE_WEIGHT_ASYNC, load_sample_weights
+    if cfg.sample_weight and cfg.is_async:
+        raise ValueError(SAMPLE_WEIGHT_ASYNC)
+    if cfg.sample_weight:   # one weight per loaded row; the split below carries them
+        data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
     model = (SparseLogistic if cfg.model == "logistic" else SparseSVM)(cfg.lam, l1=cfg.l1, class_weight=class_weight)
@@ -83,6 +89,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         if rank == 0:
             log(f"test rows by class: recall+ {cr['recall_pos']:.4f} ({cr['n_pos']} rows), recall- {cr['recall_neg']:.4f} "
                 f"({cr['n_neg']} rows), balanced accuracy {cr['balanced_accuracy']:.4f}, weighted loss {cr['weighted_loss']:.6f}")
+    if cfg.sample_weight:
+        report["test_weighted_report"] = wr = master.local_weighted_report(w1, test_data=True)
+        if rank == 0:
+            log(f"sample weights: test weight sum {wr['weight_sum']:.6g} over {wr['n']} rows, weighted loss "
+                f"{wr['weighted_loss']:.6f}, weighted accuracy {wr['weighted_accuracy']:.4f}")
     if "averaged_steps" in getattr(master, "history", {}):
         report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
     if cfg.calibrate:

@@ -148,6 +148,10 @@ ABI = {
     "dsgd_eval_class": [_vp, _vp, _i64, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_eval_sampled_class": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_eval_samples_class": [_vp, _vp, _vp, _i64, C.POINTER(_f64), _vp, _vp],
+    "dsgd_set_sample_weights": [_vp, _vp, _i64],
+    "dsgd_eval_weighted": [_vp, _vp, _i64, _i64, C.POINTER(_f64), _vp, _vp],
+    "dsgd_eval_sampled_weighted": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), _vp, _vp],
+    "dsgd_eval_samples_weighted": [_vp, _vp, _vp, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_async_host_master": [_vp, _vp],
     "dsgd_ipc_export": [_vp, C.c_int, _vp],
     "dsgd_ipc_import": [_vp, C.c_int, _vp],
@@ -232,6 +236,17 @@ class ClassEval(NamedTuple):
 
     def weighted_loss_sum(self, w_pos: float, w_neg: float) -> float:
         return w_pos * self.loss_pos + w_neg * self.loss_neg
+
+
+class WeightedEval(NamedTuple):
+    """One weighted evaluation (dsgd_eval*_weighted): ||w||^2, the fixed-point sums over the rows of c_i L_i, of c_i over the
+    correctly predicted rows and of c_i (c_i = class weight x sample weight), and the row and correct counts."""
+    norm_squared: float
+    loss_sum: float
+    correct_weight: float
+    weight_sum: float
+    n: int
+    correct: int
 
 _SUMS = (_f64, _i64, _f64)
 
@@ -686,6 +701,37 @@ class NativeCtx:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_class)."""
         samples = _arr(samples, np.int32)
         return self._class("eval_samples_class", w, (_ptr(samples), samples.size))
+
+    # -- sample weights (sync mode) and the weighted evaluations --
+    def set_sample_weights(self, sw):
+        """One weight per loaded row (finite, >= 0) for every following sync step, gradient request and weighted evaluation;
+        None clears them (dsgd_set_sample_weights)."""
+        if sw is None:
+            self._ck(self._l.dsgd_set_sample_weights(self._h, None, 0))
+            return
+        sw = _arr(sw, np.float64)
+        self._ck(self._l.dsgd_set_sample_weights(self._h, _ptr(sw), sw.size))
+
+    def _weighted(self, fn: str, w, rows: tuple) -> "WeightedEval":
+        w = self._w(w)
+        nrm = C.c_double()
+        sums, counts = np.zeros(3, dtype=np.float64), np.zeros(2, dtype=np.int64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(nrm), _ptr(sums), _ptr(counts)))
+        return WeightedEval(nrm.value, float(sums[0]), float(sums[1]), float(sums[2]), int(counts[0]), int(counts[1]))
+
+    def eval_weighted(self, row_begin: int, row_end: int, w=None) -> "WeightedEval":
+        """Weighted loss, correct-weight and weight sums over rows [row_begin, row_end) (dsgd_eval_weighted)."""
+        return self._weighted("eval_weighted", w, (row_begin, row_end))
+
+    def eval_sampled_weighted(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                              w=None) -> "WeightedEval":
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_weighted)."""
+        return self._weighted("eval_sampled_weighted", w, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def eval_samples_weighted(self, samples, w=None) -> "WeightedEval":
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted)."""
+        samples = _arr(samples, np.int32)
+        return self._weighted("eval_samples_weighted", w, (_ptr(samples), samples.size))
 
     # -- async --
     def async_host_master(self, w0):

@@ -38,6 +38,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     l1: float = 0.0               # extension: L1 penalty l1 * ||w||_1 (lasso; elastic net with lambda), sync mode only
     class_weight: str = "none"    # extension: none, balanced or w_pos,w_neg -- one weight per label, sync mode only
     calibrate: bool = False       # extension: after fit, fit a Platt sigmoid on the train rows and report its test-set quality
+    sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -53,6 +54,7 @@ _KEYS = {
     "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
     "l1": ("l1", "DSGD_L1"), "class-weight": ("class_weight", "DSGD_CLASS_WEIGHT"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
+    "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
 }
 MODELS = ("svm", "logistic")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -128,4 +130,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"l1: expected a finite value >= 0, got {cfg.l1}")
     from ..ml.class_weight import parse_class_weight
     parse_class_weight(cfg.class_weight)   # raises on a malformed value
+    if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
+        raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
     return cfg

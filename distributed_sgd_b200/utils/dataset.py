@@ -29,6 +29,7 @@ class Data:
     val: np.ndarray      # float32[nnz]
     label: np.ndarray    # int8[n_rows], +1 / -1
     dim: int
+    weight: Optional[np.ndarray] = None   # float64[n_rows]: per-row sample weights (finite, >= 0), None: every row weighs 1
 
     @property
     def n_rows(self) -> int:
@@ -45,8 +46,9 @@ class Data:
         """`data.splitAt(n)` (Main.scala:52)."""
         n = max(0, min(int(n), self.n_rows))
         cut = int(self.row_ptr[n])
-        a = Data(self.row_ptr[:n + 1].copy(), self.col[:cut], self.val[:cut], self.label[:n], self.dim)
-        b = Data(self.row_ptr[n:] - cut, self.col[cut:], self.val[cut:], self.label[n:], self.dim)
+        wa, wb = (None, None) if self.weight is None else (self.weight[:n], self.weight[n:])
+        a = Data(self.row_ptr[:n + 1].copy(), self.col[:cut], self.val[:cut], self.label[:n], self.dim, wa)
+        b = Data(self.row_ptr[n:] - cut, self.col[cut:], self.val[cut:], self.label[n:], self.dim, wb)
         return a, b
 
     def head(self, n: int) -> "Data":
@@ -59,6 +61,34 @@ class Data:
         if rows is not None:
             lens = lens[np.asarray(rows, dtype=np.int64)]
         return int(8 * lens.sum() + 16 * lens.size)
+
+
+def has_sample_weights(*parts: Optional["Data"]) -> bool:
+    """Whether any of the given row sets carries per-row sample weights."""
+    return any(p is not None and p.weight is not None for p in parts)
+
+
+def sample_weights_of(*parts: Optional["Data"]) -> np.ndarray:
+    """The sample weights of the given row sets end to end, ones for a set without weights (float64)."""
+    return np.concatenate([np.ones(p.n_rows, dtype=np.float64) if p.weight is None
+                           else np.asarray(p.weight, dtype=np.float64).reshape(-1) for p in parts if p is not None])
+
+
+def load_sample_weights(path: str, n_rows: int) -> np.ndarray:
+    """The sample weights of a `.npy` file: one finite weight >= 0 per row of a set of n_rows rows, as float64."""
+    w = np.load(path, allow_pickle=False)
+    if w.ndim != 1 or w.size != n_rows:
+        raise ValueError(f"sample-weight: {path} holds an array of shape {w.shape}, expected ({n_rows},): one weight per row")
+    if not np.issubdtype(w.dtype, np.number) or np.iscomplexobj(w):
+        raise ValueError(f"sample-weight: {path} holds {w.dtype} values, expected real numbers")
+    w = w.astype(np.float64)
+    bad = np.flatnonzero(~(np.isfinite(w) & (w >= 0.0)))
+    if bad.size:
+        raise ValueError(f"sample-weight: weight {w[bad[0]]!r} of row {int(bad[0])} is not finite and >= 0")
+    return w
+
+
+SAMPLE_WEIGHT_ASYNC = "sample-weight: sample weights belong to sync training; asynchronous (Hogwild) training has none"
 
 
 def synthetic_rcv1(n_rows: int = 700_000, dim: int = RCV1_FEATURES, seed: int = 0, mean_nnz: float = 94.5,

@@ -409,6 +409,43 @@ int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, i
 int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *norm_squared,
                             double *loss_sums_out, int64_t *counts_out);
 
+/* ---- sample weights (sync mode): one weight s_i per loaded row, finite and >= 0, held on the device in fp64.  Without them
+ *      every s_i is 1.  The class weights still apply: row i's combined weight is c_i = fl(w_y * s_i), so s_i = 1 gives
+ *      c_i = w_y exactly.  The model's backward and loss follow c_i:
+ *        SVM       the gate !(y * (x.w) < 0) is unchanged; a row that passes adds filt(filt(x_j) * s), s = y * c_i
+ *        logistic  s = (y * sigmoid(z)) * c_i
+ *        loss      of n rows: lambda ||w||^2 (+ lambda1 ||w||_1) + S / n, S = sum_i R(fl(c_i * L_i)) with L_i the unweighted
+ *                  per-sample loss, added in the fixed-point limbs of the logistic loss sum (the same bits in any row order,
+ *                  grid or rank split; NaN if a term is 2^52 or more).  The divisor is the row count.
+ *      A row of c_i = 0 scatters nothing and still counts in n.  With s = 1 and class weights (1, 1) S is the integer hinge
+ *      sum or the logistic loss sum, so every loss has the bits of the unweighted call.  They act in every sync step and in
+ *      dsgd_gradient; regularize, the update, the L1 step, averaging, the rate table, predictions, margins, metrics, curves,
+ *      calibration and every other dsgd_eval* call do not depend on them.  Loading weights, all ones included, selects the
+ *      sample-weighted kernels: one worker on one GPU takes the persistent kernel's sample-weighted form up to 32 rows per
+ *      CTA (with averaging, a rate table and L1 as without weights), the per-step path above, and dsgd_gradient the fp64
+ *      row kernel at any size (the streaming pass has no sample-weighted form).  The fused K-rank peer exchange has no
+ *      weighted form: with
+ *      world > 1 a weighted ctx needs dsgd_comm_init, and a rank wired with the peer exchange only fails with DSGD_ERR_STATE
+ *      before anything is launched.  dsgd_load_csr drops the weights (they named the previous rows).
+ *      dsgd_set_sample_weights: n == the loaded rows; sw == NULL with n == 0 clears the weights.  The first call allocates
+ *      the weights with cudaMalloc, which synchronises the whole device, and so does the first persistent run with weights
+ *      loaded (its per-step hinge codes): K contexts that share ONE GPU call it, then dsgd_reserve, before their threads
+ *      start stepping.
+ *      Errors: a weight negative, NaN or infinite, or a length other than the loaded rows -> DSGD_ERR_INVALID (checked on the
+ *      host before anything changes); an async ctx or no rows loaded -> DSGD_ERR_STATE. ------------------------------------ */
+int dsgd_set_sample_weights(dsgd_ctx *ctx, const double *sw, int64_t n);
+/* Weighted evaluation, for either model and on any sync ctx; rows and weights as in dsgd_eval_class and its siblings.
+ * *norm_squared = ||w||^2; sums_out[0..2] = S = sum c_i L_i, sum c_i [pred_i == y_i] and sum c_i, each a fixed-point sum (the
+ * same bits in any row order); counts_out[0..1] = rows, correct.  Any output may be NULL.  Without sample weights c_i = w_y;
+ * with class weights (1, 1) as well, S has the bits of dsgd_eval_sums' loss sum and the counts equal dsgd_eval_counts'. */
+int dsgd_eval_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
+                       double *sums_out, int64_t *counts_out);
+int dsgd_eval_sampled_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                               int64_t pos_begin, int64_t pos_end, double *norm_squared, double *sums_out,
+                               int64_t *counts_out);
+int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *norm_squared,
+                               double *sums_out, int64_t *counts_out);
+
 /* ---- async (Hogwild) mode.  Every worker keeps its own weight replica (core/Slave.scala:30) and pushes each
  *      delta to every peer replica and to the master's replica (core/Slave.scala:101-105).  Here replicas are
  *      reached by ADDRESS over NVLink: a rank exports its replica, the host transports the handle, peers import
