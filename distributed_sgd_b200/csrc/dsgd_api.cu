@@ -320,10 +320,25 @@ static void profiled(dsgd_ctx *ctx, F &&launch) {
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
-// the class-weighted kernels run only with weights other than (1, 1)
-static inline bool class_weighted(const dsgd_ctx *ctx) { return !(ctx->cw_pos == 1.0 && ctx->cw_neg == 1.0); }
-// the sample-weighted kernels run whenever weights are loaded, all ones included
-static inline bool sample_weighted(const dsgd_ctx *ctx) { return ctx->sw_on; }
+// class weights other than (1, 1) are set
+static inline bool has_class_weights(const dsgd_ctx *ctx) { return !(ctx->cw_pos == 1.0 && ctx->cw_neg == 1.0); }
+// The weighting of a ctx's training passes: sample-weighted whenever sample weights are loaded, all ones included (their
+// combined weights include the class weights), else class-weighted with class weights other than (1, 1)
+static inline int weighting(const dsgd_ctx *ctx) {
+  return ctx->sw_on ? kSampleWeighted : has_class_weights(ctx) ? kClassWeighted : kUnweighted;
+}
+// The one step from a ctx's run-time model and a weighting to template arguments: f(model, weighting), both as
+// std::integral_constant.  with_model fixes the weighting (an evaluation of one tally); with_forms takes it at run time.
+template <int kWeight, class F>
+static int with_model(const dsgd_ctx *ctx, F &&f) {
+  constexpr std::integral_constant<int, kWeight> weight{};
+  return is_logistic(ctx) ? f(std::integral_constant<int, kLogistic>{}, weight) : f(std::integral_constant<int, kSvm>{}, weight);
+}
+template <class F>
+static int with_forms(const dsgd_ctx *ctx, int weight, F &&f) {
+  return weight == kSampleWeighted ? with_model<kSampleWeighted>(ctx, f)
+         : weight == kClassWeighted ? with_model<kClassWeighted>(ctx, f) : with_model<kUnweighted>(ctx, f);
+}
 
 // every id names a loaded row (the reference indexes its data array with it); fn is the entry point
 static int check_ids(dsgd_ctx *ctx, const int32_t *ids, int64_t n, const char *fn, const char *what) {
@@ -824,101 +839,59 @@ static int rows_list(dsgd_ctx *ctx, const int32_t *ids, int64_t n, bool preds, c
   return DSGD_OK;
 }
 
-// The fp64 row kernel of model kModel over `rows` with the weights w: counters into cnt; kScatter: the gradient into g;
-// kPreds: the SVM kernel's sign predictions into preds.
-template <int kModel, bool kScatter, bool kPreds = false>
-static void launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, double *preds = nullptr) {
-  static_assert(!(kPreds && kModel == kLogistic), "k_rows_logistic writes no predictions");
-  if constexpr (kModel == kLogistic)
-    k_rows_logistic<kScatter><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids,
-                                                                              rows.row_begin, rows.n, w, g, ctx->cnt);
-  else
-    k_rows<kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids,
-                                                                             rows.row_begin, rows.n, w, g, preds, ctx->cnt);
-  LAUNCHED();
-}
-
-// The class-aware row kernel (k_rows_class, or the streaming pass's per-class form) over `rows`, then k_class_fold: with out == nullptr the batch's class-weighted
-// loss sum and correct count are left in cnt for a weighted tail (kCw), else the per-class totals and *nrm go to out.
-// w32 != nullptr (a request): the SVM's pass over kStreamMinRows rows or more is the per-class form of the fp32 streaming pass.
-template <int kModel, bool kScatter>
-static int launch_rows_class(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, const double *nrm = nullptr,
-                             double *out = nullptr, const float *w32 = nullptr) {
+// The row pass of model kModel and weighting kWeight over `rows` with the weights w: counters into cnt; kScatter: the
+// gradient into g; kPreds: the SVM's sign predictions into preds.  w32 != nullptr (a request): an unweighted or
+// class-weighted SVM pass over kStreamMinRows rows or more is the fp32 streaming pass, or its per-class form (SVM only: it
+// decides signs, and the logistic loss needs the dot's value); every other pass is the fp64 k_rows of its model and
+// weighting.  Only an evaluation names a range of rows; a gradient or a forward pass always lists them.  A weighted pass
+// ends with its fold, k_class_fold or k_sw_fold: with out == nullptr the batch's weighted loss sum is left in cnt for a
+// weighted tail (kCw), else the evaluation's totals and *nrm go to out.
+template <int kModel, int kWeight, bool kScatter, bool kPreds = false>
+static int launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, const float *w32, double *g,
+                       double *preds = nullptr, const double *nrm = nullptr, double *out = nullptr) {
   bool streamed = false;
-  if constexpr (kModel == kSvm) streamed = w32 && stream_eligible(ctx, rows.n);
-  if constexpr (kModel == kSvm) if (streamed) {
-    int rc = rows.ids ? stream_launch<kScatter, false, false, true>(ctx, rows.ids, 0, rows.n, w, w32, g, nullptr)
-                      : stream_launch<false, false, true, true>(ctx, nullptr, rows.row_begin, rows.n, w, w32, nullptr, nullptr);
-    if (rc) return rc;
+  if constexpr (kModel == kSvm && kWeight != kSampleWeighted) {
+    constexpr bool kCls = kWeight == kClassWeighted;
+    if ((streamed = w32 && stream_eligible(ctx, rows.n))) {
+      int rc = rows.ids ? stream_launch<kScatter, kPreds, false, kCls>(ctx, rows.ids, 0, rows.n, w, w32, g, preds)
+                        : stream_launch<false, false, true, kCls>(ctx, nullptr, rows.row_begin, rows.n, w, w32, nullptr, nullptr);
+      if (rc) return rc;
+    }
   }
   if (!streamed) {
-    k_rows_class<kModel, kScatter><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
-        ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, ctx->cnt, ctx->cw_pos, ctx->cw_neg);
+    // sw == nullptr without sample weights (an evaluation): every s_i is 1
+    k_rows<kModel, kWeight, kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+        ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
+        ctx->sw_on ? ctx->sw.p : nullptr);
     LAUNCHED();
   }
-  k_class_fold<kModel><<<1, 1, 0, ctx->stream>>>(ctx->cnt, ctx->cw_pos, ctx->cw_neg, nrm, out);
-  LAUNCHED();
-  return DSGD_OK;
-}
-
-// The sample-weighted row kernel (k_rows_class<..., kSw>) over `rows` at any size, then k_sw_fold: with out == nullptr the
-// batch's weighted loss sum is left in cnt for a weighted tail (kCw), else ||w||^2 (*nrm), the three sums and the correct
-// count go to out.
-template <int kModel, bool kScatter>
-static int launch_rows_sw(dsgd_ctx *ctx, const row_set &rows, const double *w, double *g, const double *nrm = nullptr,
-                          double *out = nullptr) {
-  k_rows_class<kModel, kScatter, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
-      ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
-      ctx->sw_on ? ctx->sw.p : nullptr);
-  LAUNCHED();
-  k_sw_fold<<<1, 1, 0, ctx->stream>>>(ctx->cnt, nrm, out);
-  LAUNCHED();
-  CU(cudaGetLastError());
-  return DSGD_OK;
-}
-
-// The row kernel of a request: the fp32 streaming pass over kStreamMinRows rows or more (SVM only: it decides signs, and
-// the logistic loss needs the dot's value), else launch_rows.  Only an evaluation names a range of rows; a gradient or a
-// forward pass always lists them.
-template <int kModel, bool kScatter, bool kPreds = false>
-static int request_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, const float *w32, double *g, double *preds) {
-  if (kModel == kLogistic || !stream_eligible(ctx, rows.n)) {
-    launch_rows<kModel, kScatter, kPreds>(ctx, rows, w, g, preds);
-    return DSGD_OK;
+  if constexpr (kWeight == kClassWeighted) {
+    k_class_fold<kModel><<<1, 1, 0, ctx->stream>>>(ctx->cnt, ctx->cw_pos, ctx->cw_neg, nrm, out);
+    LAUNCHED();
+  } else if constexpr (kWeight == kSampleWeighted) {
+    k_sw_fold<<<1, 1, 0, ctx->stream>>>(ctx->cnt, nrm, out);
+    LAUNCHED();
   }
-  return rows.ids ? stream_launch<kScatter, kPreds, false>(ctx, rows.ids, 0, rows.n, w, w32, g, preds)
-                  : stream_launch<false, false, true>(ctx, nullptr, rows.row_begin, rows.n, w, w32, nullptr, nullptr);
+  return DSGD_OK;
 }
 
 // The pass of a gradient (kScatter: the gradient into g, then k_finish) or of an evaluation over `rows` with the weights of
 // request_weights, then the shared tail: out2 = {loss, accuracy, loss sum, correct count, ||w||^2}, and the counters
-// cleared for the next pass (k_loss_scalar).
-template <int kModel, bool kScatter>
+// cleared for the next pass (k_loss_scalar).  A weighted gradient's tails read its weighted loss sum.
+template <int kModel, int kWeight, bool kScatter>
 static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
   const double *w = nullptr, *c = nullptr, *nrm = nullptr;
   const float *w32 = nullptr;
   int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
-  if (rc) return rc;
+  if (rc || (rc = launch_rows<kModel, kWeight, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr))) return rc;
   const double n = (double)rows.n;
-  // a gradient of a class-weighted model: the fp64 class kernel at any size, and the tails of its weighted loss sum; of a
-  // sample-weighted one, the sample-weighted form of that kernel at any size and the same tails
-  const bool sw = kScatter && sample_weighted(ctx);
-  const bool cw = sw || (kScatter && class_weighted(ctx));
-  if (sw) rc = launch_rows_sw<kModel, true>(ctx, rows, w, ctx->g);
-  else if (cw) rc = launch_rows_class<kModel, true>(ctx, rows, w, ctx->g, nullptr, nullptr, w32);
-  else rc = request_rows<kModel, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr, nullptr);
-  if (rc) return rc;
-  auto tail = [&](auto weighted) {
-    constexpr bool kCw = decltype(weighted)::value;
-    if constexpr (kScatter) {
-      k_finish<kModel, kCw><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
-      LAUNCHED();
-    }
-    k_loss_scalar<kModel, kCw><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
+  constexpr bool kCw = kWeight != kUnweighted;
+  if constexpr (kScatter) {
+    k_finish<kModel, kCw><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
     LAUNCHED();
-  };
-  if (cw) tail(std::true_type{});
-  else tail(std::false_type{});
+  }
+  k_loss_scalar<kModel, kCw><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
+  LAUNCHED();
   CU(cudaGetLastError());
   return DSGD_OK;
 }
@@ -933,7 +906,7 @@ extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *sampl
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
   // a prediction is the sign of x . w under either model: the SVM's row kernels
-  if ((rc = request_rows<kSvm, false, true>(ctx, rows, wd, w32d, nullptr, ctx->preds))) return rc;
+  if ((rc = launch_rows<kSvm, kUnweighted, false, true>(ctx, rows, wd, w32d, nullptr, ctx->preds))) return rc;
   CU(cudaGetLastError());
   CU(cudaMemsetAsync(ctx->cnt, 0, sizeof(unsigned long long) * 2, ctx->stream));
   CU(cudaMemcpyAsync(preds_out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -950,7 +923,9 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
   NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_gradient: dimSparsity not set");
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  if (rc || (rc = is_logistic(ctx) ? loss_pass<kLogistic, true>(ctx, w, rows) : loss_pass<kSvm, true>(ctx, w, rows)))
+  if (rc || (rc = with_forms(ctx, weighting(ctx), [&](auto m, auto wt) {
+               return loss_pass<m, wt, true>(ctx, w, rows);
+             })))
     return rc;
   CU(cudaMemcpyAsync(grad_out, ctx->g, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
   double out2[2];
@@ -964,7 +939,7 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
 // One evaluation pass over `rows`: out = {loss, accuracy, loss sum, correct count, ||w||^2}.  The SVM's loss sum is the
 // hinge sum, an integer.
 static int eval_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double out[5]) {
-  int rc = is_logistic(ctx) ? loss_pass<kLogistic, false>(ctx, w, rows) : loss_pass<kSvm, false>(ctx, w, rows);
+  int rc = with_model<kUnweighted>(ctx, [&](auto m, auto wt) { return loss_pass<m, wt, false>(ctx, w, rows); });
   if (rc) return rc;
   CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1053,24 +1028,35 @@ extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int3
   return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
 }
 
-// One per-class evaluation pass over `rows` (dsgd_eval*_class): k_rows_class without the scatter, then k_class_fold
-static int class_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *norm_squared, double *loss_sums,
+// One evaluation pass of a weighted tally over `rows`: the row kernel without the scatter, then its fold into cls_out.
+// dsgd_eval*_class (kClassWeighted): ||w||^2, the two loss sums, correct and rows per class.  dsgd_eval*_weighted
+// (kSampleWeighted): ||w||^2, the three weighted sums and the correct count; without sample weights the pass reads no
+// weights: every s_i is 1 and c_i = w_y.
+template <int kWeight>
+static int tally_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *norm_squared, double *sums,
                       int64_t *counts) {
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   const float *w32 = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd, &w32);
-  if (rc) return rc;
-  if ((rc = is_logistic(ctx) ? launch_rows_class<kLogistic, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out, w32)
-                             : launch_rows_class<kSvm, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out, w32)))
+  if (rc || (rc = with_model<kWeight>(ctx, [&](auto m, auto wt) {
+               return launch_rows<m, wt, false>(ctx, rows, wd, w32, nullptr, nullptr, nd, ctx->cls_out);
+             })))
     return rc;
   CU(cudaGetLastError());
-  double out[7];
+  constexpr bool kCls = kWeight == kClassWeighted;
+  double out[kCls ? 7 : 5];
   CU(cudaMemcpyAsync(out, ctx->cls_out, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   if (norm_squared) *norm_squared = out[0];
-  if (loss_sums) { loss_sums[0] = out[1]; loss_sums[1] = out[2]; }
-  if (counts)
-    for (int k = 0; k < 4; ++k) counts[k] = (int64_t)out[3 + k];
+  if constexpr (kCls) {
+    if (sums) { sums[0] = out[1]; sums[1] = out[2]; }
+    if (counts)
+      for (int k = 0; k < 4; ++k) counts[k] = (int64_t)out[3 + k];
+  } else {
+    if (sums)
+      for (int k = 0; k < 3; ++k) sums[k] = out[1 + k];
+    if (counts) { counts[0] = rows.n; counts[1] = (int64_t)out[4]; }
+  }
   return DSGD_OK;
 }
 
@@ -1079,7 +1065,7 @@ extern "C" int dsgd_eval_class(dsgd_ctx *ctx, const double *w, int64_t row_begin
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -1088,7 +1074,7 @@ extern "C" int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t r
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
@@ -1096,27 +1082,7 @@ extern "C" int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : class_pass(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
-}
-
-// One weighted evaluation pass over `rows` (dsgd_eval*_weighted): k_rows_class<..., kSw> without the scatter, then
-// k_sw_fold.  Without sample weights the pass reads no weights: every s_i is 1 and c_i = w_y.
-static int weighted_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *norm_squared, double *sums,
-                         int64_t *counts) {
-  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
-  int rc = request_weights(ctx, w, &wd, &cd, &nd);
-  if (rc) return rc;
-  if ((rc = is_logistic(ctx) ? launch_rows_sw<kLogistic, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out)
-                             : launch_rows_sw<kSvm, false>(ctx, rows, wd, nullptr, nd, ctx->cls_out)))
-    return rc;
-  double out[5];
-  CU(cudaMemcpyAsync(out, ctx->cls_out, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  if (norm_squared) *norm_squared = out[0];
-  if (sums)
-    for (int k = 0; k < 3; ++k) sums[k] = out[1 + k];
-  if (counts) { counts[0] = rows.n; counts[1] = (int64_t)out[4]; }
-  return DSGD_OK;
+  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
@@ -1124,7 +1090,7 @@ extern "C" int dsgd_eval_weighted(dsgd_ctx *ctx, const double *w, int64_t row_be
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_sampled_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -1133,7 +1099,7 @@ extern "C" int dsgd_eval_sampled_weighted(dsgd_ctx *ctx, const double *w, int64_
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
@@ -1141,7 +1107,7 @@ extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const 
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : weighted_pass(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
 }
 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
@@ -1611,29 +1577,28 @@ extern "C" int dsgd_comm_init(dsgd_ctx *ctx, const uint8_t id[DSGD_UNIQUE_ID_BYT
 // ---- persistent sync loop (dsgd_persistent.cuh) ----------------------------------------------------------------
 constexpr int kPCons = 8, kPUpd = 6, kPStages = 8, kPStagePairs = 2560, kPMaxChunks = 128;
 using PSmem = PersistSmem<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks>;
-// Every instantiation of k_sync_persistent, form f = 16 multi + 8 l1 + 4 cw + 2 avg + lr_table for f < 20, and the
-// sample-weighted forms f = 20 + 4 l1 + 2 avg + lr_table.  The fused K-GPU kernel (multi) has no L1, class- or
-// sample-weighted form, and the sample-weighted forms include the class weights, so there are exactly 28 forms.
-constexpr int kPersistForms = 28, kPersistSwForm = 20;
-constexpr bool pf_sw(int f) { return f >= kPersistSwForm; }
-constexpr bool pf_multi(int f) { return !pf_sw(f) && (f & 16) != 0; }
-constexpr bool pf_l1(int f) { return pf_sw(f) ? ((f - kPersistSwForm) & 4) != 0 : (f & 8) != 0; }
-constexpr bool pf_cw(int f) { return !pf_sw(f) && (f & 4) != 0; }
+// Every instantiation of k_sync_persistent: the one-GPU forms f = 8 weighting + 4 l1 + 2 avg + lr_table (0..23), and the
+// fused K-GPU kernel (multi), which has no L1 or weighted form, f = 24 + 2 avg + lr_table: exactly 28 forms.
+constexpr int kPersistForms = 28, kPersistFused = 24;
+constexpr bool pf_multi(int f) { return f >= kPersistFused; }
+constexpr int pf_weight(int f) { return pf_multi(f) ? kUnweighted : f / 8; }
+constexpr bool pf_l1(int f) { return (f & 4) != 0; }   // never set in a fused form
 template <int... F>
 static void *const *persist_forms(std::integer_sequence<int, F...>) {
   static void *const k[] = {(void *)k_sync_persistent<kPCons, kPUpd, kPStages, kPStagePairs, kPMaxChunks, pf_multi(F),
-                                                      (F & 2) != 0, (F & 1) != 0, pf_l1(F), pf_cw(F), pf_sw(F)>...};
+                                                      (F & 2) != 0, (F & 1) != 0, pf_l1(F), pf_weight(F)>...};
   return k;
 }
 static void *const *const kPersistKernels = persist_forms(std::make_integer_sequence<int, kPersistForms>{});
-// The form that runs a launch with these options; l1, cw and sw are not read for the fused kernel, cw not with sw.
-static int persist_form(bool multi, bool avg, bool lr_table, bool l1, bool cw, bool sw) {
-  if (multi) return 16 + 2 * avg + lr_table;
-  if (sw) return kPersistSwForm + 4 * l1 + 2 * avg + lr_table;
-  return 8 * l1 + 4 * cw + 2 * avg + lr_table;
+// The form that runs a launch with these options; l1 and weight are not read for the fused kernel.
+static int persist_form(bool multi, bool avg, bool lr_table, bool l1, int weight) {
+  if (multi) return kPersistFused + 2 * avg + lr_table;
+  return 8 * weight + 4 * l1 + 2 * avg + lr_table;
 }
 // Dynamic shared memory of form f: the sample-weighted forms keep their combined weights and hinge codes past PSmem
-static size_t persist_smem(int f) { return sizeof(PSmem) + (f >= kPersistSwForm ? sizeof(PersistSwSmem<kPStages>) : 0); }
+static size_t persist_smem(int f) {
+  return sizeof(PSmem) + (pf_weight(f) == kSampleWeighted ? sizeof(PersistSwSmem<kPStages>) : 0);
+}
 static bool persist_timeline() { static const bool v = getenv("DSGD_PERSIST_TIMELINE") != nullptr; return v; }
 
 static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
@@ -1657,7 +1622,9 @@ static int persist_prepare(dsgd_ctx *ctx, int64_t n_steps) {
   int rc = ctx->p_hinge.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count);
   if (rc) return rc;
   // the hinge codes of the sample-weighted forms, only while sample weights are loaded
-  if (ctx->sw_on && (rc = ctx->p_hcode.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count))) return rc;
+  if (weighting(ctx) == kSampleWeighted &&
+      (rc = ctx->p_hcode.grow(ctx, (int64_t)ctx->sm_count * n_steps, 4096 * (int64_t)ctx->sm_count)))
+    return rc;
   return ctx->p_loss_nrm.grow(ctx, 2 * n_steps, 2 * 4096);
 }
 
@@ -1778,15 +1745,14 @@ static int persist_run(dsgd_ctx *ctx, bool multi, const int32_t *samples_dev, in
     pp.lr = 0.0;   // not read: interval 0, the only one before lrs[0] is loaded, applies no update
   }
   void *args[] = {&pp};
-  // the L1 forms only with a penalty, the class-weighted forms only with weights other than (1, 1), the sample-weighted
-  // forms (which include the class weights) whenever sample weights are loaded (none fused: sync_staged keeps such a ctx
-  // off the fused path)
+  // the L1 forms only with a penalty, the weighted forms only in the ctx's weighting (none fused: sync_staged keeps such a
+  // ctx off the fused path)
   const bool l1 = !multi && ctx->lambda1 > 0.0;
   pp.lambda1 = l1 ? ctx->lambda1 : 0.0;
   pp.w_pos = ctx->cw_pos; pp.w_neg = ctx->cw_neg;
-  const bool sw = !multi && sample_weighted(ctx);
-  if (sw) { pp.sw = ctx->sw; pp.hcode = ctx->p_hcode; }
-  const int form = persist_form(multi, ctx->avg_on, lrs_host != nullptr, l1, class_weighted(ctx), sw);
+  const int weight = multi ? kUnweighted : weighting(ctx);
+  if (weight == kSampleWeighted) { pp.sw = ctx->sw; pp.hcode = ctx->p_hcode; }
+  const int form = persist_form(multi, ctx->avg_on, lrs_host != nullptr, l1, weight);
   cudaError_t launch_err = cudaSuccess;
   profiled(ctx, [&] { launch_err = persist_launch(ctx, form, G, args); });
   CU(launch_err);
@@ -1942,13 +1908,14 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
 
 // The per-step path of sync_staged for model kModel: n_steps steps of n_per_step staged ids from smp, step s at the rate
 // lrs[s] (lrs == nullptr: lr), its loss into losses[s] (losses == nullptr: none)
-// kCw: a class- or sample-weighted ctx -- every worker's pass is k_rows_class + k_class_fold (with sample weights
-// k_rows_class<..., kSw> + k_sw_fold), and the tails read the weighted loss sum
-template <int kModel, bool kCw>
+// kWeight: every worker's pass is k_rows in that weighting (a weighted one followed by its fold, k_class_fold or
+// k_sw_fold), and the tails of a weighted pass (kCw) read its weighted loss sum
+template <int kModel, int kWeight>
 static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, int64_t n_steps, double lr,
                          const double *lrs, double *losses, bool single, int32_t k_total) {
   const int upd_blocks = cdiv(ctx->dim, 256);
   const int fin_blocks = cdiv(ctx->dim + 1, 256);
+  constexpr bool kCw = kWeight != kUnweighted;
   double lr_s = lr;   // the rate of step s
   // The update of every step, in the form of this call [single][avg][l1]: one worker regularizes its raw gradient in the
   // update; while averaging the update also adds the new weights to avg; with an L1 penalty it soft-thresholds every column.
@@ -1961,16 +1928,6 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   const Update update = kUpdate[single][ctx->avg_on][ctx->lambda1 > 0.0];
   double *const avg = ctx->avg_on ? ctx->avg.p : nullptr;
 
-  auto rows_pass = [&](const row_set &rows) {
-    if constexpr (kCw) {
-      if (sample_weighted(ctx)) return launch_rows_sw<kModel, true>(ctx, rows, ctx->w, ctx->g);
-      return launch_rows_class<kModel, true>(ctx, rows, ctx->w, ctx->g);
-    } else {
-      launch_rows<kModel, true>(ctx, rows, ctx->w, ctx->g);
-      return DSGD_OK;
-    }
-  };
-
   for (int64_t s = 0; s < n_steps; ++s, smp += n_per_step) {
     if (lrs) lr_s = lrs[s];
     double *loss_dev = losses ? losses + s : nullptr;
@@ -1979,7 +1936,7 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
       int rc = DSGD_OK;
-      profiled(ctx, [&] { rc = rows_pass({smp, 0, n_per_step}); });
+      profiled(ctx, [&] { rc = launch_rows<kModel, kWeight, true>(ctx, {smp, 0, n_per_step}, ctx->w, nullptr, ctx->g); });
       if (rc) return rc;
     } else {
       // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
@@ -1987,7 +1944,7 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
       for (int32_t v = 0; v < ctx->n_local; ++v) {
         const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
         int rc = DSGD_OK;
-        profiled(ctx, [&] { rc = rows_pass({smp + off, 0, nv}); });
+        profiled(ctx, [&] { rc = launch_rows<kModel, kWeight, true>(ctx, {smp + off, 0, nv}, ctx->w, nullptr, ctx->g); });
         if (rc) return rc;
         k_finish_acc<kModel, kCw><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC,
                                                                        ctx->cnt, (double)nv, v == 0 ? 1 : 0);
@@ -2040,12 +1997,11 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   // fused kernels are SVM-only (a logistic ctx always takes the per-step path below), and an L1 penalty, class weights or
   // sample weights have only one-GPU persistent forms.  unfused names the first of them that is on.
   const bool logistic = is_logistic(ctx);
-  const bool sw = sample_weighted(ctx);
-  const bool cw = class_weighted(ctx) || sw;
+  const int weight = weighting(ctx);
   const char *unfused = logistic ? "the logistic model takes"
                         : ctx->lambda1 > 0.0 ? "the L1 penalty takes"
-                        : class_weighted(ctx) ? "class weights take"
-                        : sw ? "sample weights take" : nullptr;
+                        : has_class_weights(ctx) ? "class weights take"
+                        : weight == kSampleWeighted ? "sample weights take" : nullptr;
   NEED(!unfused || ctx->world == 1 || ctx->comm || n_steps == 0, DSGD_ERR_STATE,
        "dsgd_sync_steps: %s the NCCL allreduce path for world > 1, which needs dsgd_comm_init", unfused);
   const bool fused = !unfused && ctx->world > 1 && ctx->n_local == 1 && k_total == ctx->world && n_steps > 0 && xchg_complete(ctx) &&
@@ -2070,11 +2026,9 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   }
   const int32_t *smp = ctx->samples + first;
   double *loss_dev = want_losses ? ctx->losses.p : nullptr;
-  if (cw)
-    return logistic ? sync_per_step<kLogistic, true>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
-                    : sync_per_step<kSvm, true>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
-  return logistic ? sync_per_step<kLogistic, false>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total)
-                  : sync_per_step<kSvm, false>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
+  return with_forms(ctx, weight, [&](auto m, auto wt) {
+    return sync_per_step<m, wt>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
+  });
 }
 
 extern "C" int dsgd_sync_steps_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t n_steps, double lr,

@@ -40,13 +40,14 @@ enum Cnt : int {
   kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
   kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update<..., kL1>, k_l1_norm; zero between launches
   kCntNnz = 23,     // #{w_j != 0} of k_l1_norm; zero between launches
-  // per-class counters of k_rows_class, cleared by k_class_fold: index 0 is the class y = +1, index 1 the class y = -1
+  // per-class counters of k_rows<..., kClassWeighted, ...>, cleared by k_class_fold: index 0 is the class y = +1, index 1 the
+  // class y = -1
   kCntClassN = 24,        // rows
   kCntClassCorrect = 26,  // #{pred == y}
   kCntClassHinge = 28,    // SVM: hinge sums (integers)
   kCntClassLoss = 32,     // logistic: two fixed-point sums of the unweighted losses, kLossAccWords words each
-  // fixed-point sums of k_rows_class<..., kSw> (kLossAccWords words each), taken by k_sw_fold: S = sum R(c_i L_i), and for an
-  // evaluation sum R(c_i [pred_i == y_i]) and sum R(c_i)
+  // fixed-point sums of k_rows<..., kSampleWeighted, ...> (kLossAccWords words each), taken by k_sw_fold: S = sum R(c_i L_i),
+  // and for an evaluation sum R(c_i [pred_i == y_i]) and sum R(c_i)
   kCntSwLoss = 48,
   kCntSwCorrect = 56,
   kCntSwWeight = 64,
@@ -60,6 +61,10 @@ static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kC
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
 constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
 constexpr int kLogistic = 1;   // SparseLogistic: softplus loss, gradient x * (y * sigmoid(y * x.w))
+// Weighting of a sync pass, a compile-time parameter of the row pass and of the persistent kernel.
+constexpr int kUnweighted = 0;
+constexpr int kClassWeighted = 1;    // dsgd_set_class_weights: row i counts w_y (w_pos or w_neg by its label)
+constexpr int kSampleWeighted = 2;   // dsgd_set_sample_weights: row i counts c_i = fl(w_y * s_i), the class weights included
 
 // Sum of the per-sample losses of the running batch or pass, and its reset.  kCw: the class-weighted sum of k_class_fold.
 template <int kModel, bool kCw = false>
@@ -231,54 +236,6 @@ __global__ void __launch_bounds__(kThreads) k_prepare(const double *__restrict__
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_rows: the per-sample body of SlaveImpl.gradient / SlaveImpl.forward (core/Slave.scala:129-157):
-// one warp per row window; fp64 dot with the L2-resident weights; prediction, hinge loss, gate; scatter
-// y*x into the dense gradient with fp64 reductions at L2 (no return value -> RED, not ATOM).
-//   kScatter: accumulate backward() into g            (SparseSVM.scala:26-29)
-//   kPreds:   write p = -signum(x.w) per sample       (SparseSVM.scala:14)
-// samples == nullptr walks rows [row_begin, row_begin + n).
-// Hinge losses are integers (y, p in {-1,0,1}), so batch loss and accuracy are accumulated as exact
-// integer counters: deterministic regardless of the order in which warps finish.
-// ---------------------------------------------------------------------------------------------------
-template <bool kScatter, bool kPreds>
-__global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                              const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                              int64_t row_begin, int64_t n, const double *__restrict__ w,
-                                              double *__restrict__ g, double *__restrict__ preds,
-                                              unsigned long long *__restrict__ cnt) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  unsigned hinge = 0, correct = 0;  // lane 0 only
-  for (int64_t i = warp0; i < n; i += nwarps) {
-    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
-    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
-    const double y = (double)label[r];
-    const int p =(dot > 0.0) ? -1 : ((dot < 0.0) ? 1 : 0);  // -signum(dot)
-    if (lane == 0) {
-      const int l = 1 - (int)y * p;  // max(0, 1 - y*p), never negative for y,p in {-1,0,1}
-      hinge += (unsigned)l;
-      correct += (unsigned)(p == (int)y);
-      if (kPreds) preds[i] = (double)p;
-    }
-    if (kScatter) {
-      if (!(y * dot < 0.0)) {  // SparseSVM.scala:28: gradient is y*x unless activity < 0
-        for (int64_t k = b + lane; k < e; k += 32) {
-          const uint2 pr = pairs[k];
-          const double gv = filt(filt((double)__uint_as_float(pr.y)) * y);
-          if (gv != 0.0) atomicAdd(&g[pr.x], gv);
-        }
-      }
-    }
-  }
-  if (lane == 0 && (hinge | correct)) {
-    atomicAdd(&cnt[kCntHinge], (unsigned long long)hinge);
-    atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
 // SparseLogistic, one sample with z = y * (x . w):  loss softplus(z) = max(z, 0) + log1p(exp(-|z|)),
 // backward x * (y * sigmoid(z)).  Both stable for any z; fp64 exp / log1p (no fast-math intrinsics), the formulas of the
 // oracle.
@@ -290,121 +247,144 @@ __device__ __forceinline__ double sigmoid(double t) {
   return e / (1.0 + e);
 }
 
-// k_rows_logistic: the per-sample body of a gradient request or an evaluation pass for SparseLogistic.  One warp per row
-// window, fp64 dot with the L2-resident weights (the logistic loss and sigmoid need the dot's value, not only its sign: the
-// fp32 streaming pass of dsgd_stream.cuh is SVM-only).  Lane 0 counts correct predictions and adds softplus(z) to fixed-
-// point limbs in registers, pushed once per warp (dsgd_fixed.cuh): the loss sum does not depend on which warp took which
-// row.  kScatter: every row adds its filtered x * (y * sigmoid(z)) to g with fp64 REDs (no gate: every row contributes).
-// samples == nullptr walks rows [row_begin, row_begin + n).
 // ---------------------------------------------------------------------------------------------------
-template <bool kScatter>
-__global__ void __launch_bounds__(256) k_rows_logistic(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                                       const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                                       int64_t row_begin, int64_t n, const double *__restrict__ w,
-                                                       double *__restrict__ g, unsigned long long *__restrict__ cnt) {
+// k_rows: the per-sample body of SlaveImpl.gradient / SlaveImpl.forward (core/Slave.scala:129-157) for either model and
+// weighting: one warp per row window; fp64 dot with the L2-resident weights (the logistic loss and sigmoid need the dot's
+// value, not only its sign: the fp32 streaming pass of dsgd_stream.cuh is SVM-only); prediction, per-sample loss and gate;
+// scatter into the dense gradient with fp64 reductions at L2 (no return value -> RED, not ATOM).
+//   kScatter: accumulate backward() into g            (SparseSVM.scala:26-29)
+//   kPreds:   write p = -signum(x.w) per sample       (SparseSVM.scala:14); the unweighted SVM pass only
+// samples == nullptr walks rows [row_begin, row_begin + n).
+// The scatter value s of a row, then filt(filt(x_j) * s) per entry, so a zero weight adds nothing:
+//   SVM       s = y, weighted y * c  (an exact sign flip of c),  added where !(y * dot < 0)
+//   logistic  s = y * sigmoid(z), weighted (y * sigmoid(z)) * c,  added for every row
+// where c is the row's weight: w_y with class weights, c_i = fl(w_y * s_i) with sample weights (sw == nullptr, an
+// evaluation of a ctx without sample weights: every s_i is 1).  The unweighted passes do not read w_pos, w_neg or sw, and
+// kScatter = false with class weights is the pass of dsgd_eval*_class, which does not read the weights.
+// Lane 0's tally, the same in any row order or grid (integer counters, or R(.) added to fixed-point limbs in registers
+// and pushed once per warp, dsgd_fixed.cuh):
+//   unweighted      SVM: the hinge sum and the correct count (hinge losses are integers: y, p in {-1,0,1});
+//                   logistic: the correct count and the limbs of softplus(z)
+//   class weights   rows, correct predictions and the unweighted loss per class (SVM: integer hinge sums; logistic: two
+//                   limb blocks, a row adds its loss to its class's block and an exact 0 to the other); k_class_fold
+//                   applies the weights
+//   sample weights  R(fl(c_i * L_i)) into one limb block (S, kCntSwLoss) and the correct count; an evaluation (kScatter =
+//                   false) also R(c_i) of the correct rows (kCntSwCorrect) and of every row (kCntSwWeight).  With s = 1
+//                   and w = (1, 1) the SVM's S is the integer hinge sum and the logistic S the unweighted limb sum.
+// The counters are plain locals of every form, each form using its own: held in a struct, nvcc orders the loop's
+// registers differently, and the forms would no longer compile to the instructions of the separate kernels they replaced.
+// ---------------------------------------------------------------------------------------------------
+template <int kModel, int kWeight, bool kScatter, bool kPreds = false>
+__global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                              const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                              int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                              double *__restrict__ g, double *__restrict__ preds,
+                                              unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
+                                              const double *__restrict__ sw) {
+  static_assert(!kPreds || (kModel == kSvm && kWeight == kUnweighted), "only the unweighted SVM pass writes predictions");
+  constexpr bool kCls = kWeight == kClassWeighted, kSw = kWeight == kSampleWeighted;
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  unsigned correct = 0;  // lane 0 only
+  // lane 0 only
+  unsigned hinge = 0, correct = 0;
   unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
+  unsigned long long lim_ok[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_ok = 0;
+  unsigned long long lim_w[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0;
+  unsigned n_pos = 0, n_neg = 0, ok_pos = 0, ok_neg = 0, h_pos = 0, h_neg = 0;
+  unsigned long long lim_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_pos = 0, ovf_neg = 0;
   for (int64_t i = warp0; i < n; i += nwarps) {
     const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
     const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
     const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
     const double y = (double)label[r];
+    const int yi = (int)label[r];
+    const bool pos = yi > 0;
     const double z = y * dot;
+    const double ci = kSw ? (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r]) : 1.0) : 1.0;
     if (lane == 0) {
-      correct += (unsigned)(pred_of(dot) == (int)y);
-      acc_add_local(lim, ovf, softplus(z));
+      if constexpr (kSw) {
+        const int p = pred_of(dot);
+        const bool ok = p == yi;
+        correct += (unsigned)ok;
+        const double l = kModel == kLogistic ? softplus(z) : (double)(1 - yi * p);
+        acc_add_local(lim, ovf, ci * l);
+        if (!kScatter) {
+          acc_add_local(lim_ok, ovf_ok, ok ? ci : 0.0);
+          acc_add_local(lim_w, ovf_w, ci);
+        }
+      } else if constexpr (kCls) {
+        const int p = pred_of(dot);
+        const unsigned ok = (unsigned)(p == yi);
+        if (pos) { ++n_pos; ok_pos += ok; } else { ++n_neg; ok_neg += ok; }
+        if (kModel == kLogistic) {
+          const double l = softplus(z);
+          acc_add_local(lim_pos, ovf_pos, pos ? l : 0.0);
+          acc_add_local(lim_neg, ovf_neg, pos ? 0.0 : l);
+        } else {
+          const unsigned l = (unsigned)(1 - yi * p);
+          if (pos) h_pos += l; else h_neg += l;
+        }
+      } else if constexpr (kModel == kLogistic) {
+        correct += (unsigned)(pred_of(dot) == (int)y);
+        acc_add_local(lim, ovf, softplus(z));
+      } else {
+        const int p = pred_of(dot);
+        const int yv = (int)y;
+        hinge += (unsigned)(1 - yv * p);  // max(0, 1 - y*p), never negative for y,p in {-1,0,1}
+        correct += (unsigned)(p == yv);
+        if (kPreds) preds[i] = (double)p;
+      }
     }
     if (kScatter) {
-      const double s = y * sigmoid(z);
+      const double c = kCls ? (pos ? w_pos : w_neg) : ci;   // the row's weight
+      double s;
+      if (kModel == kLogistic) {
+        s = kWeight == kUnweighted ? y * sigmoid(z) : (y * sigmoid(z)) * c;
+      } else {
+        if (z < 0.0) continue;  // SparseSVM.scala:28: gradient unless activity < 0
+        s = kWeight == kUnweighted ? y : (pos ? c : -c);
+      }
       for (int64_t k = b + lane; k < e; k += 32) {
         const uint2 pr = pairs[k];
         const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);  // x * s: mapValues + constructor filter
-        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
+        if (gv == 0.0) continue;
+        // the unweighted SVM's atomicAdd compiles to the same RED; red_add_f64 here would reorder the kernel's registers
+        if (kModel == kSvm && kWeight == kUnweighted) atomicAdd(&g[pr.x], gv);
+        else red_add_f64(&g[pr.x], gv);
       }
     }
   }
   if (lane == 0) {
-    if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
-    acc_flush_local(cnt + kCntLoss, lim, ovf);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Sample weights (dsgd_set_sample_weights): k_rows_class<..., kSw>.  Row i has the combined weight c_i = fl(w_y * s_i) (w_y its
-// class weight, s_i its sample weight); the dot, the prediction, the SVM's gate and the unweighted per-sample loss L_i are those
-// of the class form, and the scatter value is c_i in place of w_y:
-//   SVM       s = y * c_i          (an exact sign flip),  added where !(y * dot < 0)
-//   logistic  s = (y * sigmoid(z)) * c_i
-// sw == nullptr (an evaluation of a ctx without sample weights): every s_i is 1.
-// Lane 0 adds R(fl(c_i * L_i)) into one fixed-point limb block (S, kCntSwLoss) and counts the correct rows in kCntCorrect; the
-// evaluation pass (kScatter = false) also adds R(c_i) of the correct rows (kCntSwCorrect) and of every row (kCntSwWeight).
-// Integer additions commute, so every sum has the same bits in any row order or grid.  With s = 1 and w = (1, 1) the SVM's
-// S is the integer hinge sum and the logistic S is k_rows_logistic's limb sum.
-// k_sw_fold, one thread after the pass: S's bits into cnt[kCntWLoss] for the weighted tails (out == nullptr; the correct
-// count stays in kCntCorrect), or {||w||^2, S, sum c_i [correct], sum c_i, correct} into out[0..4] (an evaluation).  The
-// limb blocks, and in an evaluation the correct count, are cleared either way.
-// ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kScatter>
-__device__ __forceinline__ void rows_sample_weighted(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                                     const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                                     int64_t row_begin, int64_t n, const double *__restrict__ w,
-                                                     double *__restrict__ g, unsigned long long *__restrict__ cnt,
-                                                     double w_pos, double w_neg, const double *__restrict__ sw) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  unsigned correct = 0;  // lane 0 only
-  unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;
-  unsigned long long lim_ok[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_ok = 0;
-  unsigned long long lim_w[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0;
-  for (int64_t i = warp0; i < n; i += nwarps) {
-    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
-    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
-    const int yi = (int)label[r];
-    const bool pos = yi > 0;
-    const double y = (double)yi;
-    const double z = y * dot;
-    const double ci = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r]) : 1.0);   // sw == nullptr: every s_i is 1
-    if (lane == 0) {
-      const int p = pred_of(dot);
-      const bool ok = p == yi;
-      correct += (unsigned)ok;
-      const double l = kModel == kLogistic ? softplus(z) : (double)(1 - yi * p);
-      acc_add_local(lim, ovf, ci * l);
-      if (!kScatter) {
-        acc_add_local(lim_ok, ovf_ok, ok ? ci : 0.0);
-        acc_add_local(lim_w, ovf_w, ci);
-      }
-    }
-    if (kScatter) {
-      double s;
+    if constexpr (kCls) {
+      if (n_pos) atomicAdd(&cnt[kCntClassN], (unsigned long long)n_pos);
+      if (n_neg) atomicAdd(&cnt[kCntClassN + 1], (unsigned long long)n_neg);
+      if (ok_pos) atomicAdd(&cnt[kCntClassCorrect], (unsigned long long)ok_pos);
+      if (ok_neg) atomicAdd(&cnt[kCntClassCorrect + 1], (unsigned long long)ok_neg);
       if (kModel == kLogistic) {
-        s = (y * sigmoid(z)) * ci;
+        acc_flush_local(cnt + kCntClassLoss, lim_pos, ovf_pos);
+        acc_flush_local(cnt + kCntClassLoss + kLossAccWords, lim_neg, ovf_neg);
       } else {
-        if (z < 0.0) continue;  // SparseSVM.scala:28
-        s = pos ? ci : -ci;
+        if (h_pos) atomicAdd(&cnt[kCntClassHinge], (unsigned long long)h_pos);
+        if (h_neg) atomicAdd(&cnt[kCntClassHinge + 1], (unsigned long long)h_neg);
       }
-      for (int64_t k = b + lane; k < e; k += 32) {
-        const uint2 pr = pairs[k];
-        const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);
-        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
+    } else if (kSw || kModel == kLogistic) {
+      if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
+      acc_flush_local(cnt + (kSw ? kCntSwLoss : kCntLoss), lim, ovf);
+      if (kSw && !kScatter) {
+        acc_flush_local(cnt + kCntSwCorrect, lim_ok, ovf_ok);
+        acc_flush_local(cnt + kCntSwWeight, lim_w, ovf_w);
       }
-    }
-  }
-  if (lane == 0) {
-    if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
-    acc_flush_local(cnt + kCntSwLoss, lim, ovf);
-    if (!kScatter) {
-      acc_flush_local(cnt + kCntSwCorrect, lim_ok, ovf_ok);
-      acc_flush_local(cnt + kCntSwWeight, lim_w, ovf_w);
+    } else if (hinge | correct) {
+      atomicAdd(&cnt[kCntHinge], (unsigned long long)hinge);
+      atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
     }
   }
 }
 
+// k_sw_fold, one thread after a sample-weighted pass: S's bits into cnt[kCntWLoss] for the weighted tails (out == nullptr;
+// the correct count stays in kCntCorrect), or {||w||^2, S, sum c_i [correct], sum c_i, correct} into out[0..4] (an
+// evaluation).  The limb blocks, and in an evaluation the correct count, are cleared either way.
 __global__ void k_sw_fold(unsigned long long *__restrict__ cnt, const double *__restrict__ scal_nrm2, double *__restrict__ out) {
   const double s = acc_take(cnt + kCntSwLoss);
   if (out) {
@@ -419,87 +399,9 @@ __global__ void k_sw_fold(unsigned long long *__restrict__ cnt, const double *__
   }
 }
 
-// ---------------------------------------------------------------------------------------------------
-// Class weights (dsgd_set_class_weights).  k_rows_class is the row kernel of either model with one weight per class: the dot,
-// the prediction, the SVM's gate and the unweighted per-sample loss are those of k_rows / k_rows_logistic; the scatter value
-// is scaled by the weight of the row's class,
-//   SVM       s = y * w_y          (an exact sign flip of w_y),  added where !(y * dot < 0)
-//   logistic  s = (y * sigmoid(z)) * w_y
-// then filt(filt(x_j) * s) per entry as before, so w_y = 0 adds nothing.  Lane 0 counts rows, correct predictions and the
-// loss per class: the SVM's hinge sums are integers, the logistic sums two fixed-point limb blocks (a row adds its loss to
-// its class's block and an exact 0 to the other), so every per-class total is the same in any order.  kScatter = false is
-// the pass of dsgd_eval*_class, which does not read the weights.
-// k_class_fold, one thread after the pass: L = fl(fl(w_pos * L_pos) + fl(w_neg * L_neg)) into cnt[kCntWLoss] and the correct
-// total into cnt[kCntCorrect] for the weighted tails (out == nullptr), or the per-class totals and ||w||^2 into out[0..6]
-// (an evaluation); the per-class words are cleared either way.
-// ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kScatter, bool kSw = false>
-__global__ void __launch_bounds__(256) k_rows_class(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                                    const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                                    int64_t row_begin, int64_t n, const double *__restrict__ w,
-                                                    double *__restrict__ g, unsigned long long *__restrict__ cnt,
-                                                    double w_pos, double w_neg, const double *__restrict__ sw = nullptr) {
-  if constexpr (kSw) {
-    rows_sample_weighted<kModel, kScatter>(rp16, pairs, label, samples, row_begin, n, w, g, cnt, w_pos, w_neg, sw);
-    return;
-  }
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  unsigned n_pos = 0, n_neg = 0, ok_pos = 0, ok_neg = 0, h_pos = 0, h_neg = 0;  // lane 0 only
-  unsigned long long lim_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_pos = 0, ovf_neg = 0;
-  for (int64_t i = warp0; i < n; i += nwarps) {
-    const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
-    const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
-    const int yi = (int)label[r];
-    const bool pos = yi > 0;
-    const double y = (double)yi;
-    const double z = y * dot;
-    if (lane == 0) {
-      const int p = pred_of(dot);
-      const unsigned ok = (unsigned)(p == yi);
-      if (pos) { ++n_pos; ok_pos += ok; } else { ++n_neg; ok_neg += ok; }
-      if (kModel == kLogistic) {
-        const double l = softplus(z);
-        acc_add_local(lim_pos, ovf_pos, pos ? l : 0.0);
-        acc_add_local(lim_neg, ovf_neg, pos ? 0.0 : l);
-      } else {
-        const unsigned l = (unsigned)(1 - yi * p);
-        if (pos) h_pos += l; else h_neg += l;
-      }
-    }
-    if (kScatter) {
-      const double wy = pos ? w_pos : w_neg;
-      double s;
-      if (kModel == kLogistic) {
-        s = (y * sigmoid(z)) * wy;
-      } else {
-        if (z < 0.0) continue;  // SparseSVM.scala:28
-        s = pos ? wy : -wy;
-      }
-      for (int64_t k = b + lane; k < e; k += 32) {
-        const uint2 pr = pairs[k];
-        const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);
-        if (gv != 0.0) red_add_f64(&g[pr.x], gv);
-      }
-    }
-  }
-  if (lane == 0) {
-    if (n_pos) atomicAdd(&cnt[kCntClassN], (unsigned long long)n_pos);
-    if (n_neg) atomicAdd(&cnt[kCntClassN + 1], (unsigned long long)n_neg);
-    if (ok_pos) atomicAdd(&cnt[kCntClassCorrect], (unsigned long long)ok_pos);
-    if (ok_neg) atomicAdd(&cnt[kCntClassCorrect + 1], (unsigned long long)ok_neg);
-    if (kModel == kLogistic) {
-      acc_flush_local(cnt + kCntClassLoss, lim_pos, ovf_pos);
-      acc_flush_local(cnt + kCntClassLoss + kLossAccWords, lim_neg, ovf_neg);
-    } else {
-      if (h_pos) atomicAdd(&cnt[kCntClassHinge], (unsigned long long)h_pos);
-      if (h_neg) atomicAdd(&cnt[kCntClassHinge + 1], (unsigned long long)h_neg);
-    }
-  }
-}
-
+// k_class_fold, one thread after a class-weighted pass: L = fl(fl(w_pos * L_pos) + fl(w_neg * L_neg)) into cnt[kCntWLoss]
+// and the correct total into cnt[kCntCorrect] for the weighted tails (out == nullptr), or the per-class totals and ||w||^2
+// into out[0..6] (an evaluation); the per-class words are cleared either way.
 template <int kModel>
 __global__ void k_class_fold(unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
                              const double *__restrict__ scal_nrm2, double *__restrict__ out) {

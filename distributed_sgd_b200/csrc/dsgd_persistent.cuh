@@ -99,9 +99,9 @@ struct PersistParams {
   double lambda1;                         // every update is followed by soft_threshold(., lr * lambda1) on every column
   // ---- one GPU with losses; last for the same reason ----
   double *loss_nrm;                       // [2][n_steps]: ||W_t||^2, then (kL1) ||W_t||_1, of every step t of the launch
-  // ---- class weights (kCw, one GPU); last for the same reason ----
+  // ---- class weights (kClassWeighted, one GPU); last for the same reason ----
   double w_pos, w_neg;                    // a row of label y scatters x * (y * w_y); the step's loss is (w_pos H+ + w_neg H-) / batch
-  // ---- sample weights (kSw, one GPU); last for the same reason ----
+  // ---- sample weights (kSampleWeighted, one GPU); last for the same reason ----
   const double *sw;                       // [rows]: row i scatters x * (y * c_i), c_i = w_y * sw[i]
   unsigned long long *hcode;              // [n_steps][gridDim.x]: the 2-bit hinge codes of every step's rows of every CTA
 };
@@ -265,8 +265,9 @@ struct StageMeta {
   double part[kMaxChunks];           // pass-1 partial dot of the chunk
 };
 
-// kSw: shared memory past the end of PersistSmem (the other forms launch without it) -- the combined weight c_i of every row of
-// every stage, written by the producer with the stage's metadata, and the 2-bit hinge codes of the CTA's rows of the step
+// kSampleWeighted: shared memory past the end of PersistSmem (the other forms launch without it) -- the combined weight c_i of
+// every row of every stage, written by the producer with the stage's metadata, and the 2-bit hinge codes of the CTA's rows of
+// the step
 template <int kStages>
 struct PersistSwSmem {
   double row_c[kStages][kMaxRowsPerCta];
@@ -421,28 +422,29 @@ __device__ __forceinline__ void chunk_pairs(const StageMeta<kMaxChunks> &mt, con
 // scattered by the warp that computed its dot, from the registers that still hold its pairs; rows of several chunks
 // take a second pass after a barrier among the consumer warps (partials summed in chunk order).
 // pre (optional): the pairs of the warp's first chunk, already loaded with chunk_pairs
-// kCw (class weights): a row of label y scatters x * s with s = y * w_y instead of x * y, at all three scatter sites, and its
-// hinge loss is counted in the low 16 bits of the returned word for y = +1 and in the high 16 bits for y = -1.  A CTA holds
-// at most kMaxRowsPerCta = 32 rows of hinge <= 2 per step, so a half holds at most 64 and never carries into the other.
-// kSw (sample weights): row m of the stage scatters x * s with s = y * row_c[m] (row_c: the stage's combined weights), and its
-// hinge loss l in {0, 1, 2} is returned as the code l << 2 m of a 64-bit word: 32 rows x 2 bits, no carries.
-template <int kCons, int kMaxChunks, bool kCw = false, bool kSw = false, class Fetch>
-__device__ __forceinline__ std::conditional_t<kSw, unsigned long long, unsigned> consume_stage(
+// kWeight == kClassWeighted: a row of label y scatters x * s with s = y * w_y instead of x * y, at all three scatter sites,
+// and its hinge loss is counted in the low 16 bits of the returned word for y = +1 and in the high 16 bits for y = -1.  A
+// CTA holds at most kMaxRowsPerCta = 32 rows of hinge <= 2 per step, so a half holds at most 64 and never carries into the
+// other.
+// kWeight == kSampleWeighted: row m of the stage scatters x * s with s = y * row_c[m] (row_c: the stage's combined
+// weights), and its hinge loss l in {0, 1, 2} is returned as the code l << 2 m of a 64-bit word: 32 rows x 2 bits, no
+// carries.
+template <int kCons, int kMaxChunks, int kWeight = kUnweighted, class Fetch>
+__device__ __forceinline__ std::conditional_t<kWeight == kSampleWeighted, unsigned long long, unsigned> consume_stage(
     StageMeta<kMaxChunks> &mt, const uint2 *ring, const uint2 *pairs, double *gbase, const int gstride, Fetch &fetch, int warp,
     int lane, long long *tl, const uint2 (*pre)[4] = nullptr, double w_pos = 1.0, double w_neg = 1.0,
     const double *row_c = nullptr) {
-  static_assert(!(kCw && kSw), "kSw forms the combined weight itself");
-  using Hinge = std::conditional_t<kSw, unsigned long long, unsigned>;
+  using Hinge = std::conditional_t<kWeight == kSampleWeighted, unsigned long long, unsigned>;
   const int n_ch = mt.n_chunks;
   Hinge hinge = 0;  // lane 0 only
-  // the scatter scalar of row m, and its hinge loss in its class's half (kCw) or its code (kSw)
+  // the scatter scalar of row m, and its hinge loss in its class's half (class weights) or its code (sample weights)
   auto scale_of = [&](int yi, double y, int m) {
-    if constexpr (kSw) return yi > 0 ? row_c[m] : -row_c[m];
-    return kCw ? (yi > 0 ? w_pos : -w_neg) : y;
+    if constexpr (kWeight == kSampleWeighted) return yi > 0 ? row_c[m] : -row_c[m];
+    return kWeight == kClassWeighted ? (yi > 0 ? w_pos : -w_neg) : y;
   };
   auto hinge_of = [&](int yi, unsigned l, int m) -> Hinge {
-    if constexpr (kSw) return (Hinge)l << (2 * m);
-    return kCw ? l << (yi > 0 ? 0 : 16) : l;
+    if constexpr (kWeight == kSampleWeighted) return (Hinge)l << (2 * m);
+    return kWeight == kClassWeighted ? l << (yi > 0 ? 0 : 16) : l;
   };
   // ---- pass 1: dots of this warp's chunks ----
   for (int c = warp; c < n_ch; c += kCons) {
@@ -543,30 +545,30 @@ __device__ __forceinline__ std::conditional_t<kSw, unsigned long long, unsigned>
 // gradient update.  ||W_T||_1 travels like W_T . d and ||W_T||^2: fp64 per-warp partials in sm.red[warp - kCons][0] (the
 // consumers' slots, unused on one GPU), summed per CTA by update warp 0 and pushed as fixed-point limbs into words 11..15
 // of the step's accumulator (overflow word 10 shared).  The loss of step t-1 adds lambda1 * ||W_{t-1}||_1.
-// kCw (one GPU only): class weights -- consume_stage scales every scatter by the weight of the row's label and packs the CTA's
-// hinge counts of the two classes into the halves of the word it already accumulates in sm.hinge_acc and stores in its
-// hinge[t * G + CTA] slot (no new buffer, nothing new on the barrier path); the epilogue's per-step warp splits the halves,
-// sums each over the G slots in integers and forms (w_pos * H+ + w_neg * H-) / batch once.
-// kSw (one GPU only): sample weights -- the producer lane that loads row m's label also loads its sample weight and puts the
-// combined weight c = w_y * sw[id] beside the stage's metadata (PersistSwSmem, past the end of PersistSmem); consume_stage
-// scales every scatter by it and returns the rows' 2-bit hinge codes, which the consumer warps OR into one shared word.  The
-// thread that arrives at the grid barrier stores that word into hcode[t * G + CTA] and clears it after the barrier has passed
-// (nothing new before the arrival); the epilogue's per-step warp re-forms S = sum R(c_i * code_i) of the step in fixed-point
-// limbs from the codes, p.samples, the labels and the weights.  Includes the class weights; never set with kCw.
+// kWeight == kClassWeighted (one GPU only): class weights -- consume_stage scales every scatter by the weight of the row's
+// label and packs the CTA's hinge counts of the two classes into the halves of the word it already accumulates in
+// sm.hinge_acc and stores in its hinge[t * G + CTA] slot (no new buffer, nothing new on the barrier path); the epilogue's
+// per-step warp splits the halves, sums each over the G slots in integers and forms (w_pos * H+ + w_neg * H-) / batch once.
+// kWeight == kSampleWeighted (one GPU only): sample weights -- the producer lane that loads row m's label also loads its
+// sample weight and puts the combined weight c = w_y * sw[id] beside the stage's metadata (PersistSwSmem, past the end of
+// PersistSmem); consume_stage scales every scatter by it and returns the rows' 2-bit hinge codes, which the consumer warps
+// OR into one shared word.  The thread that arrives at the grid barrier stores that word into hcode[t * G + CTA] and clears
+// it after the barrier has passed (nothing new before the arrival); the epilogue's per-step warp re-forms S = sum R(c_i *
+// code_i) of the step in fixed-point limbs from the codes, p.samples, the labels and the weights.  Includes the class
+// weights.
 template <int kCons, int kUpd, int kStages, int kStagePairs, int kMaxChunks, bool kMulti, bool kAvg, bool kLrTable,
-          bool kL1 = false, bool kCw = false, bool kSw = false>
+          bool kL1 = false, int kWeight = kUnweighted>
 __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(const PersistParams p) {
   using Smem = PersistSmem<kCons, kUpd, kStages, kStagePairs, kMaxChunks>;
   static_assert(!kL1 || (!kMulti && kUpd <= kCons), "the L1 form is one-GPU only and keeps its partials in the consumers' slots");
-  static_assert(!kCw || !kMulti, "the class-weighted form is one-GPU only");
-  static_assert(!kSw || (!kMulti && !kCw), "the sample-weighted form is one-GPU only and forms the class weights itself");
+  static_assert(kWeight == kUnweighted || !kMulti, "the weighted forms are one-GPU only");
   static_assert(2 * kMaxRowsPerCta <= 64, "a CTA's hinge codes of one step fit one 64-bit word");
   static_assert(2 * kMaxRowsPerCta < (1 << 16), "a CTA's hinge count of one class fits a 16-bit half");
   static_assert(kAccWords + kAccLimbs <= kAccStride, "the L1 limbs follow the accumulator's overflow word");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   using SwSmem = PersistSwSmem<kStages>;
-  SwSmem &swm = *reinterpret_cast<SwSmem *>(smem_raw + sizeof(Smem));   // kSw only: launched with the larger size
+  SwSmem &swm = *reinterpret_cast<SwSmem *>(smem_raw + sizeof(Smem));   // sample-weighted only: launched with the larger size
 
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -590,7 +592,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     sm.c_val[0] = 0.0;   // interval 0 has no pending update (g_{-1} == 0): its c is never used
     sm.nrm_val[0] = 0.0;
     sm.hinge_acc = 0u;
-    if constexpr (kSw) swm.code = 0ull;
+    if constexpr (kWeight == kSampleWeighted) swm.code = 0ull;
     sm.ok = 1;
   }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -606,15 +608,15 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
     };
     uint32_t b0 = 0, e0 = 0, b1 = 0, e1 = 0;
     int y0 = 0, y1 = 0;
-    double s0 = 0.0, s1 = 0.0;   // kSw: the sample weights of the two windows
+    double s0 = 0.0, s1 = 0.0;   // sample-weighted: the sample weights of the two windows
     auto load_win = [&](int32_t id, uint32_t &b, uint32_t &e, int &y, double &sw) {
       b = 0u; e = 0u; y = 0;
-      if constexpr (kSw) sw = 0.0;
+      if constexpr (kWeight == kSampleWeighted) sw = 0.0;
       if (id >= 0) {
         b = __ldg(&p.rp16[id]);
         e = __ldg(&p.rp16[id + 1]);
         y = (int)__ldg(&p.label[id]);
-        if constexpr (kSw) sw = __ldg(&p.sw[id]);
+        if constexpr (kWeight == kSampleWeighted) sw = __ldg(&p.sw[id]);
       }
     };
     load_win(load_id(0), b0, e0, y0, s0);   // window of step t      (stage C input)
@@ -641,7 +643,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       const bool in_ring = listed && (my_pair + len) <= kStagePairs;
       if (lane < n_r) {
         mt.row_y[lane] = y0;
-        if constexpr (kSw) swm.row_c[st][lane] = (y0 > 0 ? p.w_pos : p.w_neg) * s0;
+        if constexpr (kWeight == kSampleWeighted) swm.row_c[st][lane] = (y0 > 0 ? p.w_pos : p.w_neg) * s0;
         mt.row_b[lane] = b0;
         mt.row_len[lane] = len;
         mt.row_first[lane] = (short)my_chunk;
@@ -676,7 +678,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       if (my_bytes) bulk_g2s(&sm.ring[st][my_pair], p.pairs + (size_t)b0 * 2, my_bytes, &sm.full[st]);
       // advance the register pipeline
       b0 = b1; e0 = e1; y0 = y1;
-      if constexpr (kSw) s0 = s1;
+      if constexpr (kWeight == kSampleWeighted) s0 = s1;
       load_win(id_next, b1, e1, y1, s1);
       id_next = load_id(t + 3);
     }
@@ -1021,10 +1023,10 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           auto &mt = sm.meta[st];   // full: waited for by prefetch(t)
           FetchLocal<kL1> fetch{Rprev, &sm.c_bar[t & 1], c_par, &sm.c_val[t & 1], p.abort_flag, p.timeout_cycles, p.k_den, lr};
           if constexpr (kL1) fetch.tau = tau;
-          const auto hinge = consume_stage<kCons, kMaxChunks, kCw, kSw>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
-                                                                        lane, warp == 0 ? tl_row : nullptr, &pre, p.w_pos, p.w_neg,
-                                                                        kSw ? swm.row_c[st] : nullptr);
-          if constexpr (kSw) {
+          const auto hinge = consume_stage<kCons, kMaxChunks, kWeight>(mt, &sm.ring[st][0], p.pairs, &Rcur[0].y, 2, fetch, warp,
+                                                                       lane, warp == 0 ? tl_row : nullptr, &pre, p.w_pos, p.w_neg,
+                                                                       kWeight == kSampleWeighted ? swm.row_c[st] : nullptr);
+          if constexpr (kWeight == kSampleWeighted) {
             if (lane == 0 && hinge) atomicOr(&swm.code, hinge);
           } else {
             if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
@@ -1121,9 +1123,9 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       // release of this arrival does not wait for it (a count shared by all CTAs was one same-address atomic per CTA in front
       // of every arrival), and the next one finds it long done.  Nothing reads it before the epilogue.
       if (!kMulti && !last && p.losses) p.hinge[(size_t)t * G + blockIdx.x] = h;
-      // kSw: the rows' hinge codes of step t, the same way.  Every consumer warp OR'd its codes in before barrier 3, and the
-      // consumers of step t + 1 start after barrier 4: the word is read and cleared in between.
-      if constexpr (kSw) {
+      // sample-weighted: the rows' hinge codes of step t, the same way.  Every consumer warp OR'd its codes in before
+      // barrier 3, and the consumers of step t + 1 start after barrier 4: the word is read and cleared in between.
+      if constexpr (kWeight == kSampleWeighted) {
         if (!last) {
           if (p.losses) p.hcode[(size_t)t * G + blockIdx.x] = swm.code;
           swm.code = 0ull;
@@ -1152,11 +1154,11 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   // one GPU: loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + hinge_s/batch (SparseSVM.scala:20-23; SURVEY.md F5), one
   // warp per step.  The hinge count is the integer sum of the CTAs' slots, the same in any order.  Every slot and norm was
   // stored before the last barrier's arrivals, and is read through L2 (see grid_barrier_arrive_wait).
-  if constexpr (!kMulti && !kSw) {
+  if constexpr (!kMulti && kWeight != kSampleWeighted) {
     if (p.losses) {
       for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
         unsigned h = 0;
-        if constexpr (kCw) {   // the halves are summed apart: G slots of at most 64 each
+        if constexpr (kWeight == kClassWeighted) {   // the halves are summed apart: G slots of at most 64 each
           unsigned hn = 0;
           for (int b = lane; b < G; b += 32) {
             const unsigned v = __ldcg(&p.hinge[s * G + b]);
@@ -1218,10 +1220,10 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       p.w32_out[j] = (float)wv;
     }
   }
-  // kSw: the loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + S_s / batch, S_s = sum R(c_i * code_i) over the step's rows
-  // (row i of the step is row i / G of CTA i % G), summed in fixed-point limbs: the same bits in any order.  After the weights
-  // are stored, so that the limbs do not share the registers that hold them.
-  if constexpr (kSw) {
+  // sample-weighted: the loss of step s = lambda*||W_s||^2 (+ lambda1*||W_s||_1) + S_s / batch, S_s = sum R(c_i * code_i)
+  // over the step's rows (row i of the step is row i / G of CTA i % G), summed in fixed-point limbs: the same bits in any
+  // order.  After the weights are stored, so that the limbs do not share the registers that hold them.
+  if constexpr (kWeight == kSampleWeighted) {
     if (p.losses) {
       for (int64_t s = (int64_t)blockIdx.x * (kCons + kUpd) + warp; s < S; s += (int64_t)G * (kCons + kUpd)) {
         unsigned long long lim[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf = 0;

@@ -19,7 +19,8 @@ Writers, each on a context left with its options on (the persistent kernel at ba
 Readers: everything read_all of test_gpu_resident_state.py reads, and margins (below and above 2 048 ids), probabilities
 (logistic), eval_metrics in its three forms, eval_curve with points and AP only, calibrate, calibrated_probabilities and
 eval_calibration (range and list), weights_l1, and on a weighted context eval_class in its three forms and the weighted
-gradient (k_rows_class below 2 048 ids, the streaming pass above).  w == NULL against the weights from get_weights: every
+gradient (k_rows<…, kClassWeighted, …> below 2 048 ids, the streaming pass above).  w == NULL against the weights from
+get_weights: every
 integer word and every value that depends on the weights alone (margins, metrics and curve words, AP, the fit, calibrated
 probabilities, calibration sums and bins, weights_l1) bit for bit; the rest as in test_gpu_resident_state.py.  Those
 against the checkers of oracle/: margins bit for bit on dyadic rows (else within 1e-12 of sum |x_j w_j|), metrics words and

@@ -62,7 +62,7 @@ def test_unit_sample_weights_are_the_unweighted_library(batch, workers, cw, lam)
 @pytest.mark.parametrize("logistic", [False, True])
 def test_unit_sample_weights_gradient_and_evaluations(logistic):
     """Dyadic rows and weights: every SVM gradient sum is exact, so the streaming pass (2 048 ids or more without weights) and
-    k_rows_class<kSw> must give the same bits; the logistic scatter adds in the order of arrival."""
+    k_rows<…, kSampleWeighted, …> must give the same bits; the logistic scatter adds in the order of arrival."""
     data, rng = dyadic_data(21, n_rows=20000)
     w = dyadic_w0(rng, data.dim) / 8.0
     ctx, _ = dyadic_pair(data, 2.0 ** -6, logistic)

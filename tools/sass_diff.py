@@ -4,7 +4,9 @@ encodings ignored).  Used to show that adding template variants leaves the kerne
 A kernel that gained trailing template arguments 0 or false (e.g. `..., 0>` -> `..., 0, 0>`, `..., false>` ->
 `..., false, false>`) is matched by its name prefix.  A kernel with no such counterpart is matched to every kernel of the
 second build with the identical instruction list and reported as renamed; matching by body is many-to-one (two
-instantiations can compile to the same instructions), so it is evidence of a rename, not a proof."""
+instantiations can compile to the same instructions), so it is evidence of a rename, not a proof.
+    --mask-params (before the paths): the body match ignores which kernel parameter an instruction reads (c[0x0][0x...]
+    operands), so a kernel whose parameters moved by a slot is still reported as renamed."""
 import re
 import subprocess
 import sys
@@ -26,16 +28,18 @@ def kernels(path):
 
 
 def main():
-    a, b = kernels(sys.argv[1]), kernels(sys.argv[2])
+    mask = sys.argv[1] == "--mask-params"
+    a, b = kernels(sys.argv[1 + mask]), kernels(sys.argv[2 + mask])
+    key = (lambda body: tuple(re.sub(r"c\[0x0\]\[0x[0-9a-f]+\]", "c[0x0][param]", i) for i in body)) if mask else tuple
     by_body = {}
     for name, body in b.items():
-        by_body.setdefault(tuple(body), []).append(name)
+        by_body.setdefault(key(body), []).append(name)
     differ = renamed = 0
     for name, body in sorted(a.items()):
         extra = ("ELi0", "ELi0ELi0", "ELb0")
         cands = [name] if name in b else [n for n in (name.replace("EEEv", e + "EEEv", 1) for e in extra) if n in b]
         if not cands:
-            same = by_body.get(tuple(body))
+            same = by_body.get(key(body))
             if same:
                 print("renamed:", name, "->", " | ".join(sorted(same)))
                 renamed += 1

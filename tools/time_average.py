@@ -4,7 +4,7 @@ one context (fused: on both ranks' contexts):
 
     persistent kernel, batch 64, 256 and 1024 (2 188 steps per call)
     fallback (k_rows + k_update), batch 32 G + 1, G = SM count (200 steps per call)
-    SparseLogistic, batch 256 (k_rows_logistic + k_update, 200 steps per call)
+    SparseLogistic, batch 256 (k_rows<logistic, …> + k_update, 200 steps per call)
     fused K = 2 on one GPU: two contexts of S / 2 CTAs each, batch 256 per rank (2 188 steps per call).  A CTA of the fused
     kernel owns at most 448 columns, so this case runs on a synthetic set of the same shape at dim 448 (S / 2) - 1.
 

@@ -3,8 +3,10 @@ first 560 000 of them train rows), and one quality figure.  Every timing case ru
 (1, 1), and on, (2, 0.5), alternated on one context:
 
     persistent kernel and its weighted form, batch 64, 256 and 1024 (2 188 steps per call)
-    fallback (k_rows + k_update against k_rows_class + k_class_fold + k_update<kCw>), batch 32 G + 1 (200 steps per call)
-    SparseLogistic, batch 256 (k_rows_logistic against k_rows_class<logistic>, 200 steps per call)
+    fallback (k_rows + k_update against
+        k_rows<svm, kClassWeighted, …> + k_class_fold + k_update<kCw>), batch 32 G + 1 (200 steps per call)
+    SparseLogistic, batch 256 (k_rows<logistic, kUnweighted, …> against
+        k_rows<logistic, kClassWeighted, …>, 200 steps per call)
     dsgd_eval_class against dsgd_eval_counts over the 140 000 test rows and the 560 000 train rows
     dsgd_gradient over 262 144 ids, unweighted and weighted
 

@@ -4,7 +4,7 @@ context:
 
     persistent kernel and its L1 form, batch 64, 256 and 1024 (2 188 steps per call)
     fallback (k_rows + k_update against k_rows + k_update<..., kL1>), batch 32 G + 1, G = SM count (200 steps per call)
-    SparseLogistic, batch 256 (k_rows_logistic + k_update against k_update<..., kL1>, 200 steps per call)
+    SparseLogistic, batch 256 (k_rows<logistic, …> + k_update against k_update<..., kL1>, 200 steps per call)
 
 Each case runs `--warmup` untimed calls per arm, then `--reps` rounds of one timed call per arm (off first, then on), each on
 the host clock between two device synchronisations; every call starts from the same weights.  The card's name and power

@@ -3,10 +3,10 @@ rows, the first 560 000 of them train rows).  Every case runs the same work in t
 weights, all ones, and random weights (uniform in [0, 2)):
 
     one-GPU step, batch 64, 256 and 1024 (2 188 steps per call): the persistent kernel without weights, the per-step path
-        (k_rows_class<kSw> + k_sw_fold + k_update<kCw>) with them
+        (k_rows<…, kSampleWeighted, …> + k_sw_fold + k_update<kCw>) with them
     per-step path, batch 32 G + 1 (200 steps per call): k_rows + k_update against the sample-weighted pass
     SparseLogistic, batch 256 (200 steps per call)
-    dsgd_gradient over 262 144 ids: the streaming pass without weights, k_rows_class<kSw> with them
+    dsgd_gradient over 262 144 ids: the streaming pass without weights, k_rows<…, kSampleWeighted, …> with them
     dsgd_eval_weighted over the 140 000 test rows and the 560 000 train rows (dsgd_eval_counts in the no-weights arm)
 
 Each case runs `--warmup` untimed rounds, then `--reps` rounds of one timed call per arm, each on the host clock between two
