@@ -113,6 +113,37 @@ def curve_dict(result) -> dict:
     return out
 
 
+def weighted_curve_dict(result, curve: bool = True) -> dict:
+    """The result of Master.local_weighted_curve from a NativeCtx.eval_*weighted_curve result (include/dsgd.h): the weighted
+    confusion sums tp, fn, pos_no_pred, fp, tn, neg_no_pred (each row counted by its weight c_i), nan_weight, and with the
+    formulas of metrics_dict on the weights precision = TP / (TP + FP), recall = TP / W+, f1 = 2 TP / (2 TP + FP + FN +
+    pos_no_pred); auc = U2w / (2 W+ W-), average_precision = S_ap / W+, accuracy = the correct rows' weight / weight_sum,
+    weight_sum, n_points and nan_scores (rows).  With `curve` (a result with its points), "curve": thresholds, tp_weight and fp_weight (W+ and W- at
+    or above each threshold), precision, recall and fpr.  A ratio whose denominator is 0 is nan."""
+    tp, fn, pos_none, fp, tn, neg_none, _, nan_w, _, correct, total, wp, wn = (float(x) for x in result.wsums)
+    nan = float("nan")
+
+    def ratio(a: float, b: float) -> float:
+        return a / b if b else nan
+
+    out = {"tp": tp, "fn": fn, "pos_no_pred": pos_none, "fp": fp, "tn": tn, "neg_no_pred": neg_none, "nan_weight": nan_w,
+           "nan_scores": int(result.words[7]), "precision": ratio(tp, tp + fp), "recall": ratio(tp, wp),
+           "f1": ratio(2.0 * tp, 2.0 * tp + fp + fn + pos_none), "auc": float(result.auc),
+           "average_precision": float(result.ap), "accuracy": ratio(correct, total), "weight_sum": total,
+           "n_points": int(result.n_points)}
+    if curve:
+        tpw, fpw = np.asarray(result.tpw, dtype=np.float64), np.asarray(result.fpw, dtype=np.float64)
+        P, N = (float(tpw[-1]), float(fpw[-1])) if len(tpw) else (0.0, 0.0)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            precision = np.where(tpw + fpw > 0, tpw / np.where(tpw + fpw > 0, tpw + fpw, 1.0), nan)
+            recall = tpw / P if P else np.full(len(tpw), nan)
+            fpr = fpw / N if N else np.full(len(fpw), nan)
+        out["curve"] = {"thresholds": [float(x) for x in result.thr], "tp_weight": [float(x) for x in tpw],
+                        "fp_weight": [float(x) for x in fpw], "precision": [float(x) for x in precision],
+                        "recall": [float(x) for x in recall], "fpr": [float(x) for x in fpr]}
+    return out
+
+
 class EpochDraw(list):
     """The batch draws of one epoch: `self[s][k]` = row ids of worker k at step s (a list of lists of int32 arrays, the
     shape the tests and the oracle replay), backed by ONE array `ids[steps, K, batch]` (-1 beyond a short slice) and
@@ -418,6 +449,23 @@ class Master:
         if ids is None:
             return curve_dict(self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=curve))
         return curve_dict(self.ctx.eval_samples_curve(ids, weights, curve=curve))
+
+    def local_weighted_curve(self, weights=None, test_data: bool = False, curve: bool = True) -> dict:
+        """local_curve with every row counted by its weight c_i = class weight x sample weight (weighted_curve_dict).  Not
+        sharded either: every rank evaluates the whole range, and every word is an order-free fixed-point sum, so every
+        rank gets the same bits."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        return weighted_curve_dict(self.ctx.eval_weighted_curve(b, e, weights, curve=curve), curve)
+
+    def local_sampled_weighted_curve(self, weights, samples_count: int, test_data: bool = False, curve: bool = True) -> dict:
+        """local_weighted_curve on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_curve draws it.  An
+        empty sample raises DsgdEmpty."""
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled weighted curve of {samples_count} rows: the sample is empty")
+        if ids is None:
+            return weighted_curve_dict(self.ctx.eval_sampled_weighted_curve(b, e, key, 0, k, weights, curve=curve), curve)
+        return weighted_curve_dict(self.ctx.eval_samples_weighted_curve(ids, weights, curve=curve), curve)
 
     # ---- calibration (extension) -----------------------------------------------------------------------------------------
     # Like the ranking metrics, these are not sharded: rows are replicated on every rank and every rank fits or evaluates

@@ -155,6 +155,10 @@ struct dsgd_ctx {
   // the radix sort's alternate keys and temporary storage, and the counter words (MetricWord)
   dev_buf<unsigned long long> m_keys, m_alt, m_cnt;
   dev_buf<unsigned char> m_tmp;
+  // a weighted curve pass (dsgd_eval_*weighted_curve): each key's weight c in the key's slot and its sort alternate, and the
+  // runs' inclusive prefix sums of R(c) (never grown by an async ctx, which these calls refuse)
+  dev_buf<double> m_val, m_valt;
+  dev_buf<limb_sum> c_pre;
   // a curve pass (dsgd_eval_*curve): its counter words (CurveWord), the merged key runs, the exclusive scan of their tie
   // ends, and the points (sort, merge and scan share m_tmp)
   dev_buf<unsigned long long> c_cnt, c_merged;
@@ -1147,24 +1151,36 @@ extern "C" int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t 
 // lengths read by the host (the sort takes its lengths from the host), and the key runs sorted.  A metrics pass
 // (`each_run` false) sorts only when both runs have keys, since otherwise there is no pair to count; a curve pass sorts
 // every run that has keys.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
+// kSampleWeighted (a weighted curve pass): every key carries its row's c_i, the runs are sorted as (key, c) pairs, and
+// pos_c / neg_c are the sorted weights.
 struct sorted_runs {
   unsigned long long h[kMetWords];   // the counter words as k_metrics_score left them
   int64_t n_pos, n_neg;
   const unsigned long long *pos, *neg;   // each run ascending, if it was sorted
+  const double *pos_c, *neg_c;           // kSampleWeighted: the weights in the order of pos and neg
 };
+template <int kWeight>
 static int score_and_sort(dsgd_ctx *ctx, const double *w, const row_set &rows, bool each_run, const char *fn,
                           sorted_runs *s) {
+  constexpr bool kW = kWeight == kSampleWeighted;
+  constexpr int kWords = kW ? kMetWWords : kMetWords;
   const int64_t n = rows.n;
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = fits_while_running(ctx, ctx->m_keys.cap >= n && ctx->m_alt.cap >= n && ctx->m_cnt, fn);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
   if ((rc = ctx->m_keys.grow(ctx, n, 1024)) || (rc = ctx->m_alt.grow(ctx, n, 1024)) ||
-      (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)))
+      (rc = ctx->m_cnt.grow(ctx, kWords, kWords)))
     return rc;
-  CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kMetWords, ctx->stream));
+  if (kW && ((rc = ctx->m_val.grow(ctx, n, 1024)) || (rc = ctx->m_valt.grow(ctx, n, 1024)))) return rc;
+  CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kWords, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
-  k_metrics_score<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                 ctx->m_keys, ctx->m_cnt);
+  if constexpr (kW)
+    k_metrics_score<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
+                                                            wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
+                                                            ctx->sw_on ? ctx->sw.p : nullptr, ctx->m_val);
+  else
+    k_metrics_score<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
+                                                            wd, ctx->m_keys, ctx->m_cnt);
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(s->h, ctx->m_cnt, sizeof s->h, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1174,28 +1190,37 @@ static int score_and_sort(dsgd_ctx *ctx, const double *w, const row_set &rows, b
   // two buffers, and Current() is the buffer that holds it sorted
   cub::DoubleBuffer<unsigned long long> kp(ctx->m_keys.p, ctx->m_alt.p);
   cub::DoubleBuffer<unsigned long long> kn(ctx->m_keys.p + (n - n_neg), ctx->m_alt.p + (n - n_neg));
+  cub::DoubleBuffer<double> vp(ctx->m_val.p, ctx->m_valt.p);
+  cub::DoubleBuffer<double> vn(kW ? ctx->m_val.p + (n - n_neg) : nullptr, kW ? ctx->m_valt.p + (n - n_neg) : nullptr);
+  // one run sorted: its keys alone, or (kW) its (key, c) pairs
+  auto sort = [&](void *tmp, size_t &bytes, cub::DoubleBuffer<unsigned long long> &k, cub::DoubleBuffer<double> &v, int64_t m) {
+    if constexpr (kW) return cub::DeviceRadixSort::SortPairs(tmp, bytes, k, v, (int)m, 0, 64, ctx->stream);
+    else return cub::DeviceRadixSort::SortKeys(tmp, bytes, k, (int)m, 0, 64, ctx->stream);
+  };
   const bool sort_pos = n_pos > 0 && (each_run || n_neg > 0), sort_neg = n_neg > 0 && (each_run || n_pos > 0);
   if (sort_pos || sort_neg) {
     size_t tmp_p = 0, tmp_n = 0;
-    if (sort_pos) CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_p, kp, (int)n_pos, 0, 64, ctx->stream));
-    if (sort_neg) CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp_n, kn, (int)n_neg, 0, 64, ctx->stream));
+    if (sort_pos) CU(sort(nullptr, tmp_p, kp, vp, n_pos));
+    if (sort_neg) CU(sort(nullptr, tmp_n, kn, vn, n_neg));
     size_t tmp = std::max(tmp_p, tmp_n);
     if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
       return rc;
-    if (sort_pos) CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kp, (int)n_pos, 0, 64, ctx->stream));
-    if (sort_neg) CU(cub::DeviceRadixSort::SortKeys(ctx->m_tmp.p, tmp, kn, (int)n_neg, 0, 64, ctx->stream));
+    if (sort_pos) CU(sort(ctx->m_tmp.p, tmp, kp, vp, n_pos));
+    if (sort_neg) CU(sort(ctx->m_tmp.p, tmp, kn, vn, n_neg));
   }
   s->n_pos = n_pos;
   s->n_neg = n_neg;
   s->pos = kp.Current();
   s->neg = kn.Current();
+  s->pos_c = vp.Current();
+  s->neg_c = vn.Current();
   return DSGD_OK;
 }
 
 // One metrics pass over `rows`: score_and_sort, then U2 counted (k_auc_count).
 static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *out, const char *fn) {
   sorted_runs s;
-  int rc = score_and_sort(ctx, w, rows, false, fn, &s);
+  int rc = score_and_sort<kUnweighted>(ctx, w, rows, false, fn, &s);
   if (rc) return rc;
   unsigned long long *h = s.h;
   const int64_t n_pos = s.n_pos, n_neg = s.n_neg;
@@ -1212,26 +1237,57 @@ static int metrics_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int
   return DSGD_OK;
 }
 
+// The inclusive scan of R(c) over one sorted run's weights into pre (tmp == nullptr: the storage it needs, into bytes).
+static cudaError_t scan_weights(dsgd_ctx *ctx, void *tmp, size_t &bytes, const double *c, limb_sum *pre, int64_t n) {
+  return cub::DeviceScan::InclusiveScan(tmp, bytes, thrust::make_transform_iterator(c, limb_of{}), pre, limb_plus{}, (int)n,
+                                        ctx->stream);
+}
+
 // One curve pass over `rows` (DESIGN.md §4.9): score_and_sort with every run sorted, then k_curve_count (U2, the limbs of
 // S = sum of v_i, the number of points m) and k_curve_sum.  With thr != nullptr also the points: the runs merged, the
 // exclusive scan of the merged keys' tie ends, k_curve_emit, and the m points copied back at once.  AP = S / P, NaN when a
 // score is NaN or there is no positive row.
-static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *words, double *ap, int64_t *n_points,
-                      double *thr, int64_t *tp, int64_t *fp, const char *fn) {
+// kSampleWeighted (§4.14): the same steps in their weighted forms, each run's prefix sums of R(c) scanned into c_pre before
+// k_curve_count (positives at c_pre[0, n_pos), negatives after them); out receives the DSGD_WCURVE_WORDS words instead of
+// AP, and tp / fp the point weights as doubles (k_curve_emit writes their bits into c_tp / c_fp).
+template <int kWeight>
+static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *words, double *out, int64_t *n_points,
+                      double *thr, void *tp, void *fp, const char *fn) {
+  constexpr bool kW = kWeight == kSampleWeighted;
+  constexpr int kWords = kW ? kCurWWords : kCurWords;
   const int64_t n = rows.n;
   const bool curve = thr != nullptr;
   int rc = fits_while_running(ctx, ctx->c_cnt && (!curve || (ctx->c_merged.cap >= n && ctx->c_excl.cap >= n &&
                                                               ctx->c_thr.cap >= n && ctx->c_tp.cap >= n && ctx->c_fp.cap >= n)),
                               fn);
   sorted_runs s;
-  if (rc || (rc = score_and_sort(ctx, w, rows, true, fn, &s)) || (rc = ctx->c_cnt.grow(ctx, kCurWords, kCurWords))) return rc;
-  CU(cudaMemsetAsync(ctx->c_cnt, 0, sizeof(unsigned long long) * kCurWords, ctx->stream));
+  if (rc || (rc = score_and_sort<kWeight>(ctx, w, rows, true, fn, &s)) || (rc = ctx->c_cnt.grow(ctx, kWords, kWords))) return rc;
+  CU(cudaMemsetAsync(ctx->c_cnt, 0, sizeof(unsigned long long) * kWords, ctx->stream));
   const int64_t n_all = s.n_pos + s.n_neg;
   const int grid = (int)std::min<int64_t>(std::max(cdiv(n_all, 256), 1), (int64_t)ctx->sm_count * 8);
-  k_curve_count<<<grid, 256, 0, ctx->stream>>>(s.pos, s.n_pos, s.neg, s.n_neg, ctx->m_cnt + kMetU2, ctx->c_cnt);
-  LAUNCHED();
-  k_curve_sum<<<1, 1, 0, ctx->stream>>>(ctx->c_cnt);
-  LAUNCHED();
+  const limb_sum *pre_pos = nullptr, *pre_neg = nullptr;
+  if constexpr (kW) {
+    if ((rc = ctx->c_pre.grow(ctx, n, 1024))) return rc;
+    pre_pos = ctx->c_pre.p;
+    pre_neg = ctx->c_pre.p + s.n_pos;
+    size_t tmp_p = 0, tmp_n = 0;
+    if (s.n_pos) CU(scan_weights(ctx, nullptr, tmp_p, s.pos_c, ctx->c_pre.p, s.n_pos));
+    if (s.n_neg) CU(scan_weights(ctx, nullptr, tmp_n, s.neg_c, ctx->c_pre.p + s.n_pos, s.n_neg));
+    size_t tmp = std::max(tmp_p, tmp_n);
+    if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+    if (s.n_pos) CU(scan_weights(ctx, ctx->m_tmp.p, tmp, s.pos_c, ctx->c_pre.p, s.n_pos));
+    if (s.n_neg) CU(scan_weights(ctx, ctx->m_tmp.p, tmp, s.neg_c, ctx->c_pre.p + s.n_pos, s.n_neg));
+    k_curve_count<kWeight><<<grid, 256, 0, ctx->stream>>>(s.pos, s.n_pos, s.neg, s.n_neg, ctx->m_cnt + kMetU2, ctx->c_cnt,
+                                                          s.pos_c, pre_pos, pre_neg);
+    LAUNCHED();
+    k_curve_sum<kWeight><<<1, 1, 0, ctx->stream>>>(ctx->c_cnt, s.pos, s.n_pos, s.neg, s.n_neg, pre_pos, pre_neg, ctx->m_cnt);
+    LAUNCHED();
+  } else {
+    k_curve_count<kWeight><<<grid, 256, 0, ctx->stream>>>(s.pos, s.n_pos, s.neg, s.n_neg, ctx->m_cnt + kMetU2, ctx->c_cnt);
+    LAUNCHED();
+    k_curve_sum<kWeight><<<1, 1, 0, ctx->stream>>>(ctx->c_cnt);
+    LAUNCHED();
+  }
   CU(cudaGetLastError());
   if (curve && n_all > 0) {
     if ((rc = ctx->c_merged.grow(ctx, n, 1024)) || (rc = ctx->c_excl.grow(ctx, n, 1024)) || (rc = ctx->c_thr.grow(ctx, n, 1024)) ||
@@ -1246,27 +1302,35 @@ static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64
     CU(merge_runs(ctx, ctx->m_tmp.p, tmp, s.pos, s.n_pos, s.neg, s.n_neg));
     tmp = std::max(tmp_merge, tmp_scan);
     CU(scan_tie_ends(ctx, ctx->m_tmp.p, tmp, n_all));
-    k_curve_emit<<<grid, 256, 0, ctx->stream>>>(ctx->c_merged, n_all, ctx->c_excl, s.pos, s.n_pos, s.neg, s.n_neg, ctx->c_cnt,
-                                                ctx->c_thr, ctx->c_tp, ctx->c_fp);
+    if constexpr (kW)
+      k_curve_emit<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->c_merged, n_all, ctx->c_excl, s.pos, s.n_pos, s.neg, s.n_neg,
+                                                           ctx->c_cnt, ctx->c_thr, ctx->c_tp, ctx->c_fp, pre_pos, pre_neg);
+    else
+      k_curve_emit<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->c_merged, n_all, ctx->c_excl, s.pos, s.n_pos, s.neg, s.n_neg,
+                                                           ctx->c_cnt, ctx->c_thr, ctx->c_tp, ctx->c_fp);
     LAUNCHED();
     CU(cudaGetLastError());
   }
-  unsigned long long c[kCurWords];
+  unsigned long long c[kWords];
   CU(cudaMemcpyAsync(c, ctx->c_cnt, sizeof c, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaMemcpyAsync(&s.h[kMetU2], ctx->m_cnt + kMetU2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   const int64_t m = (int64_t)c[kCurPoints];
-  if (curve && m > 0) {
+  if (curve && m > 0) {   // a weighted pass's c_tp / c_fp hold the bits of doubles: copied as bytes
     CU(cudaMemcpyAsync(thr, ctx->c_thr, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaMemcpyAsync(tp, ctx->c_tp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaMemcpyAsync(fp, ctx->c_fp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
   }
   for (int k = 0; k < DSGD_METRICS_WORDS; ++k) words[k] = (int64_t)s.h[k];
-  const int64_t P = words[kMetTp] + words[kMetFn] + words[kMetPosNone];
-  double S;
-  memcpy(&S, &c[kCurSum], sizeof S);
-  *ap = (words[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
+  if constexpr (kW) {
+    memcpy(out, &c[kCurOut], sizeof(double) * DSGD_WCURVE_WORDS);
+  } else {
+    const int64_t P = words[kMetTp] + words[kMetFn] + words[kMetPosNone];
+    double S;
+    memcpy(&S, &c[kCurSum], sizeof S);
+    *out = (words[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
+  }
   *n_points = m;
   return DSGD_OK;
 }
@@ -1286,7 +1350,7 @@ extern "C" int dsgd_eval_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin
   row_set rows;
   int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
   if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
-  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
 }
 
 extern "C" int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -1296,7 +1360,7 @@ extern "C" int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t r
   row_set rows;
   int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
   if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
-  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
 }
 
 extern "C" int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
@@ -1308,7 +1372,53 @@ extern "C" int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int
   if (rc) return rc;
   NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
   if ((rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
-  return curve_pass(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
+}
+
+// A weighted curve call: the outputs as curve_outputs checks them (wsums_out in ap_out's place, tpw / fpw in tp / fp's), then
+// an async ctx is refused before anything is launched -- its weights are always 1, and growing the pass's buffers would wait
+// for the loop, which runs until stopped.
+static int weighted_curve_args(dsgd_ctx *ctx, const int64_t *words, const double *wsums, const int64_t *n_points,
+                               const double *thr, const double *tpw, const double *fpw, const char *fn) {
+  NEED(words && wsums && n_points, DSGD_ERR_INVALID, "%s: words_out, wsums_out or n_points_out is NULL", fn);
+  NEED(!thr == !tpw && !tpw == !fpw, DSGD_ERR_INVALID,
+       "%s: thr_out, tpw_out and fpw_out are all NULL (the words only) or all set", fn);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (row weights belong to the sync paths)",
+       fn);
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                        int64_t *words_out, double *wsums_out, int64_t *n_points_out, double *thr_out,
+                                        double *tpw_out, double *fpw_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
+  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *words_out,
+                                                double *wsums_out, int64_t *n_points_out, double *thr_out, double *tpw_out,
+                                                double *fpw_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
+  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_weighted_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                int64_t *words_out, double *wsums_out, int64_t *n_points_out,
+                                                double *thr_out, double *tpw_out, double *fpw_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  row_set rows;
+  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  if (rc) return rc;
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  if ((rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
+  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
 }
 
 extern "C" int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out) {

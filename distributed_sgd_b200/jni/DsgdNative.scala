@@ -127,6 +127,18 @@ object DsgdNative {
                                   posEnd: Long, sums: Array[Double], counts: Array[Long]): Int
   @native def evalSamplesWeighted(ctx: Long, w: Array[Double], samples: Array[Int], sums: Array[Double],
                                   counts: Array[Long]): Int
+  // weighted curves, either model: metrics as evalCurve's, wsums(0 until 13) the DSGD_WCURVE_WORDS weighted words, nPoints(0)
+  // = m, thr / tpw / fpw(0 until m) the points (W+ and W- at or above each score); all three null for the words alone, else
+  // each at least as long as the request's rows.  An async ctx is refused.
+  @native def evalWeightedCurve(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, metrics: Array[Long],
+                                wsums: Array[Double], nPoints: Array[Long], thr: Array[Double], tpw: Array[Double],
+                                fpw: Array[Double]): Int
+  @native def evalSampledWeightedCurve(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                       posEnd: Long, metrics: Array[Long], wsums: Array[Double], nPoints: Array[Long],
+                                       thr: Array[Double], tpw: Array[Double], fpw: Array[Double]): Int
+  @native def evalSamplesWeightedCurve(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long],
+                                       wsums: Array[Double], nPoints: Array[Long], thr: Array[Double], tpw: Array[Double],
+                                       fpw: Array[Double]): Int
   // async (Hogwild) mode
   @native def asyncHostMaster(ctx: Long, w0: Array[Double]): Int
   @native def ipcExport(ctx: Long, which: Int, handle: Array[Byte]): Int

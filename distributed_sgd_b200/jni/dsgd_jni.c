@@ -656,6 +656,70 @@ FN(evalSamplesWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jint
   return rc;
 }
 
+/* weighted curves: metrics(0..7) as the curve calls', wsums(0 until DSGD_WCURVE_WORDS) the weighted words, nPoints(0) = m, and
+ * thr / tpw / fpw (0 until m) the points -- all three null for the words alone, else each at least as long as the request's
+ * rows.  w is null or holds dim values.  A shorter array is DSGD_ERR_INVALID, checked before the call. */
+typedef struct { buf_t w, m, s, k, t, tp, fp; } wcurve_bufs;
+static wcurve_bufs wcurve_in(JNIEnv *env, jdoubleArray w, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints,
+                             jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
+  wcurve_bufs c = {in_Double(env, w),      out_Long(env, metrics), out_Double(env, wsums), out_Long(env, nPoints),
+                   out_Double(env, thr),   out_Double(env, tpw),   out_Double(env, fpw)};
+  return c;
+}
+static int wcurve_bad(const wcurve_bufs *c) { return c->w.bad | c->m.bad | c->s.bad | c->k.bad | c->t.bad | c->tp.bad | c->fp.bad; }
+static int wcurve_args(jlong h, const wcurve_bufs *c, jlong n) {
+  int32_t dim = 0;
+  int rc = dsgd_dim(CTX(h), &dim);
+  if (rc) return rc;
+  if ((c->w.p && (int32_t)c->w.n != dim) || c->m.n < DSGD_METRICS_WORDS || c->s.n < DSGD_WCURVE_WORDS || c->k.n < 1)
+    return DSGD_ERR_INVALID;
+  return ((c->t.p && c->t.n < n) || (c->tp.p && c->tp.n < n) || (c->fp.p && c->fp.n < n)) ? DSGD_ERR_INVALID : DSGD_OK;
+}
+static void wcurve_back(JNIEnv *env, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr,
+                        jdoubleArray tpw, jdoubleArray fpw, wcurve_bufs *c, int rc) {
+  back_Long(env, metrics, c->m, rc);
+  back_Double(env, wsums, c->s, rc);
+  back_Long(env, nPoints, c->k, rc);
+  back_Double(env, thr, c->t, rc);
+  back_Double(env, tpw, c->tp, rc);
+  back_Double(env, fpw, c->fp, rc);
+  free(c->w.p);
+}
+FN(evalWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics,
+                      jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
+  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
+  int rc = DSGD_ERR_NOMEM;
+  if (!wcurve_bad(&c) && (rc = wcurve_args(h, &c, rowEnd - rowBegin)) == DSGD_OK)
+    rc = dsgd_eval_weighted_curve(CTX(h), c.w.p, rowBegin, rowEnd, (int64_t *)c.m.p, (double *)c.s.p, (int64_t *)c.k.p,
+                                  (double *)c.t.p, (double *)c.tp.p, (double *)c.fp.p);
+  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
+  return rc;
+}
+FN(evalSampledWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                             jlong posBegin, jlong posEnd, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints,
+                             jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
+  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
+  int rc = DSGD_ERR_NOMEM;
+  if (!wcurve_bad(&c) && (rc = wcurve_args(h, &c, posEnd - posBegin)) == DSGD_OK)
+    rc = dsgd_eval_sampled_weighted_curve(CTX(h), c.w.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (int64_t *)c.m.p,
+                                          (double *)c.s.p, (int64_t *)c.k.p, (double *)c.t.p, (double *)c.tp.p,
+                                          (double *)c.fp.p);
+  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
+  return rc;
+}
+FN(evalSamplesWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics,
+                             jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
+  buf_t bi = in_Int(env, samples);
+  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bi.bad | wcurve_bad(&c)) && (rc = wcurve_args(h, &c, bi.n)) == DSGD_OK)
+    rc = dsgd_eval_samples_weighted_curve(CTX(h), c.w.p, bi.p, bi.n, (int64_t *)c.m.p, (double *)c.s.p, (int64_t *)c.k.p,
+                                          (double *)c.t.p, (double *)c.tp.p, (double *)c.fp.p);
+  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
+  free(bi.p);
+  return rc;
+}
+
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {
   buf_t b = in_Double(env, w0);

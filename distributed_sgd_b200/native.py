@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import math
 import os
 import subprocess
 from typing import NamedTuple, Optional, Tuple
@@ -120,6 +121,9 @@ ABI = {
     "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_weighted_curve": [_vp, _vp, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_sampled_weighted_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_samples_weighted_curve": [_vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -249,6 +253,31 @@ class WeightedEval(NamedTuple):
     correct: int
 
 _SUMS = (_f64, _i64, _f64)
+
+WCURVE_WORDS = 13   # DSGD_WCURVE_WORDS
+
+
+class WeightedCurve(NamedTuple):
+    """One weighted curve (dsgd_eval*_weighted_curve): the metrics words (counts), the DSGD_WCURVE_WORDS weighted words
+    (include/dsgd.h), the number of points m, the points (thresholds, W+(>= t) and W-(>= t); empty arrays for a words-only
+    pass), and the weighted ROC AUC and average precision derived from the words."""
+    words: np.ndarray
+    wsums: np.ndarray
+    n_points: int
+    thr: np.ndarray
+    tpw: np.ndarray
+    fpw: np.ndarray
+    auc: float
+    ap: float
+
+
+def weighted_auc_ap(words, wsums) -> tuple:
+    """(AUC, AP) of a weighted curve: U2w / (2 W+ W-), NaN when a score is NaN or W+ or W- is 0; S_ap / W+, NaN when a score
+    is NaN or W+ is 0, and 1 when W- is 0."""
+    nan, wp, wn = int(words[7]) > 0, float(wsums[11]), float(wsums[12])
+    auc = math.nan if nan or wp == 0.0 or wn == 0.0 else float(wsums[6]) / (2.0 * wp * wn)
+    ap = math.nan if nan or wp == 0.0 else 1.0 if wn == 0.0 else float(wsums[8]) / wp
+    return auc, ap
 
 
 def _ptr(a: Optional[np.ndarray]):
@@ -732,6 +761,32 @@ class NativeCtx:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted)."""
         samples = _arr(samples, np.int32)
         return self._weighted("eval_samples_weighted", w, (_ptr(samples), samples.size))
+
+    def _weighted_curve(self, fn: str, w, rows: tuple, n: int, curve: bool) -> "WeightedCurve":
+        w = self._w(w)
+        words, wsums, m = np.zeros(METRICS_WORDS, dtype=np.int64), np.zeros(WCURVE_WORDS), C.c_int64()
+        pts = [np.zeros(max(n, 0)) if curve else None for _ in range(3)]
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(words), _ptr(wsums), C.byref(m),
+                                                 *[_ptr(a) for a in pts]))
+        k = m.value
+        thr, tpw, fpw = [a[:k].copy() if curve else np.zeros(0) for a in pts]
+        return WeightedCurve(words, wsums, k, thr, tpw, fpw, *weighted_auc_ap(words, wsums))
+
+    def eval_weighted_curve(self, row_begin: int, row_end: int, w=None, curve: bool = True) -> "WeightedCurve":
+        """ROC / precision-recall points, AUC and AP over rows [row_begin, row_end), every row counted by its weight
+        c_i = class weight x sample weight (dsgd_eval_weighted_curve); curve=False: the words only."""
+        return self._weighted_curve("eval_weighted_curve", w, (row_begin, row_end), row_end - row_begin, curve)
+
+    def eval_sampled_weighted_curve(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None,
+                                    curve: bool = True) -> "WeightedCurve":
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_weighted_curve)."""
+        return self._weighted_curve("eval_sampled_weighted_curve", w, _drawn(row_begin, row_end, key, pos_begin, pos_end),
+                                    pos_end - pos_begin, curve)
+
+    def eval_samples_weighted_curve(self, samples, w=None, curve: bool = True) -> "WeightedCurve":
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted_curve)."""
+        samples = _arr(samples, np.int32)
+        return self._weighted_curve("eval_samples_weighted_curve", w, (_ptr(samples), samples.size), samples.size, curve)
 
     # -- async --
     def async_host_master(self, w0):

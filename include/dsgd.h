@@ -236,6 +236,46 @@ int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, i
 int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
                             double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out);
 
+/* ---- weighted curves: the curve calls above with every row counted by its weight, on any sync ctx and for either model.
+ *      Rows, the three row forms, s = -x.w, NaN handling, ties and the m points are exactly those of dsgd_eval_curve.  Row
+ *      i's weight is c_i = fl(w_y * s_i), the class weight of its label times its sample weight (dsgd_set_class_weights,
+ *      dsgd_set_sample_weights): without sample weights c_i = w_y, and with class weights (1, 1) as well c_i = 1.
+ *      R(v) is the fixed-point cut of the loss sums (resolution 2^-160; a value of 2^52 or more, or a NaN, makes its sum
+ *      NaN), and read() converts an exact sum of R values to a double: it depends only on the exact value, so every word has
+ *      the same bits whatever the row order, the grid or the rank.  W+(>= t) = read(sum R(c_i)) over the non-NaN positive
+ *      rows with s >= t; W+(< t), W+(= t) and the W- forms over the negative rows likewise.
+ *      wsums_out[0..12] (DSGD_WCURVE_WORDS), each one read() of one exact sum:
+ *        0 TP weight (positives, s > 0: pred +1)   1 FN weight (s < 0)   2 positives with no prediction (s = +-0 or NaN)
+ *        3 FP weight   4 TN weight   5 negatives with no prediction
+ *        6 U2w = sum over the non-NaN positives of R(fl(c_i B_i)), B_i = read(2 W-(< s_i) + W-(= s_i))
+ *        7 weight of the NaN-score rows
+ *        8 S_ap = sum over the non-NaN positives with c_i > 0 of R(fl(c_i fl(T_i / (T_i + F_i)))), T_i = W+(>= s_i),
+ *          F_i = W-(>= s_i); a zero-weight row adds exactly 0 to every sum and its precision is never formed
+ *        9 weight of the correct rows (TP and TN as one sum)   10 sum of c_i over all rows
+ *        11 W+ and 12 W-: the weight of all positive and of all negative rows, NaN scores included
+ *      Weighted ROC AUC = U2w / (2 W+ W-), NaN when a score is NaN or W+ or W- is 0; weighted AP = S_ap / W+, NaN when a score
+ *      is NaN or W+ = 0, and 1 when W- = 0.  Range: a product term of 2^52 or more makes its word NaN; U2w is finite while
+ *      max c * 2 W- < 2^52.
+ *      words_out receives the DSGD_METRICS_WORDS words of the metrics call over the same rows, bit for bit (counts, not
+ *      weights).  *n_points_out = m; point k: thr_out[k] bit for bit that of dsgd_eval_curve (zero-weight rows still define
+ *      points), tpw_out[k] = W+(>= t_k), fpw_out[k] = W-(>= t_k).  Recent scikit-learn versions drop zero-weight rows before
+ *      they choose thresholds, so their curves can have fewer points; the areas agree.
+ *      At c = 1: words 0..7 are the curve call's words as doubles (U2w = U2), S_ap has the limbs of its S (AP bit for bit)
+ *      and tpw / fpw equal tp / fp.  With integer weights whose products stay below 2^53, U2w is the U2 of the id list in
+ *      which row i appears c_i times.  Words 9 and 10 are dsgd_eval_weighted's sums_out[1] and sums_out[2], bit for bit.
+ *      thr_out, tpw_out and fpw_out hold at least n entries each, or are all NULL (then only the words are computed).  The
+ *      errors are those of dsgd_eval_curve; an async ctx -> DSGD_ERR_STATE before anything is launched.  A pass grows its
+ *      buffers (the curve call's and 72 bytes more per row: c, its sort alternate and the prefix sums) on first use. */
+#define DSGD_WCURVE_WORDS 13
+int dsgd_eval_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *words_out,
+                             double *wsums_out, int64_t *n_points_out, double *thr_out, double *tpw_out, double *fpw_out);
+int dsgd_eval_sampled_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                     int64_t pos_begin, int64_t pos_end, int64_t *words_out, double *wsums_out,
+                                     int64_t *n_points_out, double *thr_out, double *tpw_out, double *fpw_out);
+int dsgd_eval_samples_weighted_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
+                                     double *wsums_out, int64_t *n_points_out, double *thr_out, double *tpw_out,
+                                     double *fpw_out);
+
 /* ---- calibration: scores into probabilities, for either model, over the same three row forms and with the conventions and
  *      errors of the metrics calls above.  With f = x_i . w exactly as dsgd_margins returns it, a calibration is a pair (A, B)
  *      and P(y = +1 | x_i) = 1 / (1 + exp(A f + B)), computed as sigmoid(-(A f + B)) with the sigmoid of the logistic gradient.
