@@ -474,7 +474,9 @@ int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *sampl
  *      Errors: a weight negative, NaN or infinite, or a length other than the loaded rows -> DSGD_ERR_INVALID (checked on the
  *      host before anything changes); an async ctx or no rows loaded -> DSGD_ERR_STATE. ------------------------------------ */
 int dsgd_set_sample_weights(dsgd_ctx *ctx, const double *sw, int64_t n);
-/* Weighted evaluation, for either model and on any sync ctx; rows and weights as in dsgd_eval_class and its siblings.
+/* Weighted evaluation, for either model; rows and weights as in dsgd_eval_class and its siblings.  An async ctx has no
+ * class or sample weights, so there every c_i is 1; w == NULL reads a snapshot of the replica taken when the call starts,
+ * as every other request does there.
  * *norm_squared = ||w||^2; sums_out[0..2] = S = sum c_i L_i, sum c_i [pred_i == y_i] and sum c_i, each a fixed-point sum (the
  * same bits in any row order); counts_out[0..1] = rows, correct.  Any output may be NULL.  Without sample weights c_i = w_y;
  * with class weights (1, 1) as well, S has the bits of dsgd_eval_sums' loss sum and the counts equal dsgd_eval_counts'. */

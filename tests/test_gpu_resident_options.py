@@ -246,15 +246,18 @@ def check_weighted_gradients(ctx, env, orc, w, c, got_res, got_exp, logistic, ex
             assert abs(v - loss_ref) <= 1e-11 * abs(loss_ref), f"{what}: {name} loss ({who}) {v!r} against {loss_ref!r}"
 
 
-def check_all_readers(ctx, env, orc, logistic, exact_resident, exact_oracle, what):
-    """Every reader at w == NULL against the explicit weights, and those against the checkers; returns (w, c)."""
+def check_all_readers(ctx, env, orc, logistic, exact_resident, exact_oracle, what, weighted=None, check_gradients=None):
+    """Every reader at w == NULL against the explicit weights, and those against the checkers; returns (w, c).  weighted:
+    the gradient is weighted (default: by class weights other than (1, 1)), and check_gradients checks it (default:
+    check_weighted_gradients)."""
     w = ctx.get_weights()
-    weighted = ctx.get_class_weights() != (1.0, 1.0)
+    if weighted is None:
+        weighted = ctx.get_class_weights() != (1.0, 1.0)
     resident, explicit = read_all(ctx, env, None, logistic), read_all(ctx, env, w, logistic)
     want, c = oracle_all(orc, env, w, logistic)
     scales = {n: _grad_scale(env, env.data, env.ids[n], c) for n in ("grad_stream", "grad_rows")}
     if weighted:       # the weighted gradient has its own checker; read_all's evaluations are unweighted
-        check_weighted_gradients(ctx, env, orc, w, c, resident, explicit, logistic, exact_oracle, what)
+        (check_gradients or check_weighted_gradients)(ctx, env, orc, w, c, resident, explicit, logistic, exact_oracle, what)
         for d in (resident, explicit, want):
             del d["grad_stream"], d["grad_rows"]
     compare(resident, explicit, exact_resident, f"{what}, w == NULL against the explicit weights", scales)
@@ -288,9 +291,10 @@ def step_ref(ctx, orc, w, ids, batch, lrs, logistic, lam1=None, class_w=None):
     return w_ref, l_ref[0]
 
 
-def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what):
+def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what, ref=None, cmax=None):
     """One step with the context's options on (path "persistent": batch 64; "per_step": 32 G + 1), from the resident state
-    and after set_weights(w) re-derives it: the same weights and loss, and the checker's."""
+    and after set_weights(w) re-derives it: the same weights and loss, and the checker's.  ref: the checker's step, as
+    step_ref takes and returns it; cmax: the largest weight of a row (else the larger class weight)."""
     _one_worker(ctx)
     ctx.set_grid_limit(0)
     ids = env.ids["step"] if path == "persistent" else _big_step(env, S)
@@ -304,7 +308,7 @@ def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what):
     loss, w1 = step()
     ctx.set_weights(w)
     loss_twin, w1_twin = step()
-    w_ref, loss_ref = step_ref(ctx, orc, w, ids, batch, lrs, logistic)
+    w_ref, loss_ref = (ref or step_ref)(ctx, orc, w, ids, batch, lrs, logistic)
     what = f"{what}, next step on the {path} path"
     if exact:
         assert loss == loss_twin == loss_ref, f"{what}: loss {loss!r} / re-set {loss_twin!r} / checker {loss_ref!r}"
@@ -315,7 +319,7 @@ def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what):
         return
     assert abs(loss - loss_twin) <= 1e-12 * abs(loss_twin), f"{what}: loss {loss!r} against {loss_twin!r}"
     assert abs(loss_twin - loss_ref) <= 1e-12 * abs(loss_ref), f"{what}: loss {loss_twin!r} against the checker's {loss_ref!r}"
-    wmax = max(ctx.get_class_weights())
+    wmax = max(ctx.get_class_weights()) if cmax is None else cmax
     tol = 1e-12 * (np.abs(w1_twin) + env.lr * wmax * _grad_scale(env, env.data, ids, c))
     assert np.array_equal(w1 != 0, w1_twin != 0), f"{what}: supports differ"
     bad = np.flatnonzero(np.abs(w1 - w1_twin) > tol)

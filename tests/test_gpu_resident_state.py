@@ -440,46 +440,53 @@ def _wait_for_loop(ctx):
     assert not ctx.async_running(), "the async loop did not end by itself"
 
 
+def async_write(env, writer, peers):
+    """Runs an async writer on the env's async context (peer_push: on two new ranks, appended to peers); returns the
+    context to read and the weights before the writer."""
+    from distributed_sgd_b200.native import REPLICA_SELF
+    rng = np.random.default_rng(len(writer) * 1000 + env.dim + 2)
+    replay = _steps(rng, REPLAY_BATCH, REPLAY_UPDATES)
+    ctx = env.ctx("async")
+    _reset(ctx, env, env.w0, sync=False)
+    w_before = env.w0
+    if writer == "update_grad":                      # SlaveImpl.updateGrad: w -= delta, here onto w1
+        delta = env.w0 - env.w1
+        idx = np.flatnonzero(delta).astype(np.int32)
+        ctx.update_grad(idx, delta[idx])
+    elif writer == "replay_from_replica":
+        ctx.async_replay(None, replay, REPLAY_BATCH, env.lr)
+    elif writer == "replay_from_w0":
+        ctx.set_weights(env.w1)
+        w_before = env.w1
+        ctx.async_replay(env.w0, replay, REPLAY_BATCH, env.lr)
+    elif writer in ("loop_stopped", "loop_ended"):
+        ctx.start_async(None, np.arange(N_ROWS, dtype=np.int32), batch=1, lr=env.lr, concurrency=1,
+                        max_updates=LOOP_UPDATES, seed=env.dim)
+        _wait_for_loop(ctx)
+        if writer == "loop_stopped":
+            ctx.stop_async()
+    elif writer == "peer_push":                      # rank 0's replay pushes every delta into rank 1's replica
+        for r in range(2):
+            p, _ = make_pair(env.data, env.lam, rank=r, world=2, is_async=True)
+            p.set_dim_sparsity(env.d)
+            p.set_weights(env.w0)
+            peers.append(p)
+        peers[0].peer_attach(1, peers[1], REPLICA_SELF)
+        peers[0].async_replay(None, replay, REPLAY_BATCH, env.lr)
+        ctx = peers[1]
+    return ctx, w_before
+
+
 @pytest.mark.parametrize("writer", ASYNC_WRITERS)
 @pytest.mark.parametrize("dim", DIMS)
 @pytest.mark.parametrize("kind", KINDS)
 def test_async(envs, kind, dim, writer):
     """Readers between writers, with no loop running; w == NULL reads the replica as it is when the call starts."""
-    from distributed_sgd_b200.native import REPLICA_SELF
     env = envs(kind, dim)
     what = f"async, {kind}, dim {dim}, {writer}"
-    rng = np.random.default_rng(len(writer) * 1000 + dim + 2)
-    replay = _steps(rng, REPLAY_BATCH, REPLAY_UPDATES)
-    ctx = env.ctx("async")
     peers = []
     try:
-        _reset(ctx, env, env.w0, sync=False)
-        w_before = env.w0
-        if writer == "update_grad":                      # SlaveImpl.updateGrad: w -= delta, here onto w1
-            delta = env.w0 - env.w1
-            idx = np.flatnonzero(delta).astype(np.int32)
-            ctx.update_grad(idx, delta[idx])
-        elif writer == "replay_from_replica":
-            ctx.async_replay(None, replay, REPLAY_BATCH, env.lr)
-        elif writer == "replay_from_w0":
-            ctx.set_weights(env.w1)
-            w_before = env.w1
-            ctx.async_replay(env.w0, replay, REPLAY_BATCH, env.lr)
-        elif writer in ("loop_stopped", "loop_ended"):
-            ctx.start_async(None, np.arange(N_ROWS, dtype=np.int32), batch=1, lr=env.lr, concurrency=1,
-                            max_updates=LOOP_UPDATES, seed=dim)
-            _wait_for_loop(ctx)
-            if writer == "loop_stopped":
-                ctx.stop_async()
-        elif writer == "peer_push":                      # rank 0's replay pushes every delta into rank 1's replica
-            for r in range(2):
-                p, _ = make_pair(env.data, env.lam, rank=r, world=2, is_async=True)
-                p.set_dim_sparsity(env.d)
-                p.set_weights(env.w0)
-                peers.append(p)
-            peers[0].peer_attach(1, peers[1], REPLICA_SELF)
-            peers[0].async_replay(None, replay, REPLAY_BATCH, env.lr)
-            ctx = peers[1]
+        ctx, w_before = async_write(env, writer, peers)
         w_after = ctx.get_weights()
         orc = env.oracle(env.d)
         witness(env, "w", w_before, w_after, env.d, env.d, orc_after=orc)
