@@ -12,7 +12,8 @@
 //     complete_tx) per row into the stage's shared-memory partition, plus a chunk list.
 //   * CONSUMER warps: the CTA's rows of a step are cut into 128-pair chunks dealt round-robin to the
 //     warps.  A row that is ONE chunk (85 % of them) is finished by the warp that holds it in registers: dot,
-//     gate, RED of y*x into g.  Longer rows: partial dots per chunk (fixed order), then gate + scatter per chunk.
+//     gate, RED of y*x into g.  Longer rows: partial dots per chunk (fixed order), then gate + scatter per chunk -- by the
+//     row's own warps after a named barrier of the row's when the stage is at most one chunk per warp, else in a second pass.
 //   * UPDATE warps: weights are double-buffered and gradients triple-buffered in L2 so the update of step
 //     t-1 and the gradient of step t share one barrier interval.
 //   * c_t = 2*lambda*(W_t . d) (SparseSVM.scala:31) is a dot over the whole weight vector that the NEXT interval needs
@@ -247,18 +248,23 @@ constexpr int kChunkPairs = 128;             // 4 pairs per lane per chunk
 static_assert(kChunkPairs == kFoldPairs, "a listed row's chunks are the chunks of the row fold");
 constexpr uint32_t kChunkGlobal = 1u << 31;  // chunk offset flag: read from global, the row did not fit the stage
 constexpr int kMaxRowsPerCta = 32;           // rows of one step per CTA (one producer lane each)
+// Hardware named barriers of the rows of several chunks that their own warps finish (consume_stage): ids 5..15.  0 is
+// __syncthreads, 2 the consumers' second pass, 3 and 4 the CTA's barriers around the grid barrier.
+constexpr int kRowBarFirst = 5, kRowBars = 11;
 
 template <int kMaxChunks>
 struct StageMeta {
   int n_rows;
   int n_chunks;
-  int n_multi;                       // listed rows of more than one chunk (0: the stage needs no second pass)
+  int n_multi;                       // listed rows of more than one chunk
+  int two_pass;                      // 1: the rows of several chunks take the second pass after a barrier of all consumers
   int n_pairs;                       // pairs of the CTA's rows in this stage (diagnostic)
   int row_y[kMaxRowsPerCta];
   uint32_t row_b[kMaxRowsPerCta];    // window start (16-byte units) -- for rows that missed the chunk list
   int row_len[kMaxRowsPerCta];       // pairs, padding included
   short row_first[kMaxRowsPerCta];   // first chunk of the row
   short row_nch[kMaxRowsPerCta];     // chunks of the row; -1: not in the chunk list (whole-row slow path)
+  signed char row_bar[kMaxRowsPerCta];   // named barrier of a row of several chunks finished by its own warps, or -1
   uint32_t ch_off[kMaxChunks];       // pair offset inside the stage partition, or kChunkGlobal | global pair index
   short ch_n[kMaxChunks];            // pairs in the chunk (<= kChunkPairs)
   short ch_row[kMaxChunks];          // local row
@@ -294,7 +300,8 @@ struct PersistSmem {
   do {                                                                                        \
     if (p.tl && blockIdx.x == 0 && lane == 0 && t < 256) p.tl[t * 16 + (slot_)] = clock64(); \
   } while (0)
-constexpr int kTlSteps = 4, kTlFirst = 100, kTlCtas = 160, kTlPerCta = 4;   // per-CTA records of steps 100..103
+// per-CTA records of steps 100..103: {barrier arrival ns, barrier exit ns, pairs of the CTA's rows, chunks | multi-chunk rows << 32}
+constexpr int kTlSteps = 4, kTlFirst = 100, kTlCtas = 160, kTlPerCta = 4;
 constexpr int kTlWords = 256 * 16 + kTlSteps * kTlCtas * kTlPerCta;
 
 // ---- weight fetch of the consumers: W_t[col] -----------------------------------------------------------------
@@ -419,8 +426,13 @@ __device__ __forceinline__ void chunk_pairs(const StageMeta<kMaxChunks> &mt, con
 // ---- the consumer warps' work on one stage: SlaveImpl.gradient's per-sample body (core/Slave.scala:147-153) ----
 // x.W per row (math/Vec.scala:58), prediction and hinge loss (SparseSVM.scala:14-16), gate (SparseSVM.scala:28),
 // RED of y*x into g (entry of column c at gbase + gstride * c).  A row that is ONE chunk (85 % of them) is gated and
-// scattered by the warp that computed its dot, from the registers that still hold its pairs; rows of several chunks
-// take a second pass after a barrier among the consumer warps (partials summed in chunk order).
+// scattered by the warp that computed its dot, from the registers that still hold its pairs.  A row of several chunks:
+//   * per row (the stage lists every row in at most kCons chunks, so a warp holds at most one chunk): the row's warps leave
+//     their partials in part[], meet on the row's own named barrier (row_bar, nch * 32 threads), each sums the row's partials
+//     in chunk order and gates and scatters its own chunk from its registers; the warp of the row's first chunk counts the
+//     hinge.  No warp waits for a row it does not hold, and a warp waits on one barrier at most.
+//   * otherwise (two_pass): a second pass after a barrier among all consumer warps re-reads each chunk's pairs.
+// Both sum the same partials in the same order and issue the same REDs.
 // pre (optional): the pairs of the warp's first chunk, already loaded with chunk_pairs
 // kWeight == kClassWeighted: a row of label y scatters x * s with s = y * w_y instead of x * y, at all three scatter sites,
 // and its hinge loss is counted in the low 16 bits of the returned word for y = +1 and in the high 16 bits for y = -1.  A
@@ -465,10 +477,21 @@ __device__ __forceinline__ std::conditional_t<kWeight == kSampleWeighted, unsign
     if (tl && lane == 0 && c == warp) tl[4] = clock64();   // ... dot reduced
     {
       const int row1 = mt.ch_row[c];
-      if (mt.row_nch[row1] == 1) {
+      const int nch1 = mt.row_nch[row1];
+      int first1 = c;
+      if (nch1 > 1) {   // the row's dot: its chunks' partials in chunk order, once every warp of the row has left its own
+        if (lane == 0) mt.part[c] = acc;
+        const int bar = mt.row_bar[row1];
+        if (bar < 0) continue;   // two_pass
+        named_bar_sync(bar, nch1 * 32);
+        first1 = mt.row_first[row1];
+        acc = 0.0;
+        for (int i = 0; i < nch1; ++i) acc += mt.part[first1 + i];
+      }
+      {
         const int yi = mt.row_y[row1];
         const double y = (double)yi;
-        if (lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(acc)), row1);
+        if (c == first1 && lane == 0) hinge += hinge_of(yi, (unsigned)(1 - yi * pred_of(acc)), row1);
         if (!(y * acc < 0.0)) {  // SparseSVM.scala:28
           const double sc = scale_of(yi, y, row1);
 #pragma unroll
@@ -477,13 +500,11 @@ __device__ __forceinline__ std::conditional_t<kWeight == kSampleWeighted, unsign
             if (gvv != 0.0) red_add_f64(gbase + (size_t)gstride * pr[u].x, gvv);
           }
         }
-        continue;
       }
     }
-    if (lane == 0) mt.part[c] = acc;
   }
-  // ---- pass 2 (rows of several chunks): row dot = chunk partials in order, prediction, gate, scatter ----
-  if (mt.n_multi > 0) {
+  // ---- pass 2 (two_pass: rows of several chunks): row dot = chunk partials in order, prediction, gate, scatter ----
+  if (mt.two_pass) {
     named_bar_sync(2, kCons * 32);
     for (int c = warp; c < n_ch; c += kCons) {
       const int row = mt.ch_row[c];
@@ -565,6 +586,7 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
   static_assert(2 * kMaxRowsPerCta <= 64, "a CTA's hinge codes of one step fit one 64-bit word");
   static_assert(2 * kMaxRowsPerCta < (1 << 16), "a CTA's hinge count of one class fits a 16-bit half");
   static_assert(kAccWords + kAccLimbs <= kAccStride, "the L1 limbs follow the accumulator's overflow word");
+  static_assert(kCons / 2 <= kRowBars, "every row of several chunks in a stage of at most kCons chunks has a named barrier");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   using SwSmem = PersistSwSmem<kStages>;
@@ -663,11 +685,17 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
       // chunks actually written to the list: everything up to the first row that did not fit it
       const int listed_chunks = __reduce_max_sync(0xffffffffu, (lane < n_r && listed) ? (my_chunk + nch) : 0);
       const unsigned multi = __ballot_sync(0xffffffffu, lane < n_r && listed && nch > 1);
+      // the rows of several chunks are finished by their own warps when every row is listed and every consumer warp holds
+      // at most one chunk; each such row gets a named barrier of its own (kCons chunks hold at most kCons / 2 of them)
+      const bool per_row = __all_sync(0xffffffffu, lane >= n_r || listed) && listed_chunks <= kCons;
+      if (lane < n_r)
+        mt.row_bar[lane] = (signed char)((per_row && nch > 1) ? kRowBarFirst + __popc(multi & ((1u << lane) - 1u)) : -1);
       if (lane == 31) mt.n_pairs = ps;
       if (lane == 0) {
         mt.n_rows = n_r;
         mt.n_chunks = listed_chunks;
         mt.n_multi = __popc(multi);
+        mt.two_pass = (multi != 0u && !per_row) ? 1 : 0;
       }
       __syncwarp();  // every lane's metadata is written before lane 0 arrives on the full barrier
       if (lane == 0) {
@@ -1008,7 +1036,10 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
                                                                           warp == 0 ? tl_row : nullptr);
         ok = ok && fetch.good;
         if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
-        if (tl_rec && warp == 0 && lane == 0) tl_rec[2] = mt.n_pairs;
+        if (tl_rec && warp == 0 && lane == 0) {
+          tl_rec[2] = mt.n_pairs;
+          tl_rec[3] = (long long)mt.n_chunks | ((long long)mt.n_multi << 32);
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(&sm.empty[st]);
         if (warp == 0) DSGD_TL(3);
@@ -1031,7 +1062,10 @@ __global__ void __launch_bounds__((kCons + kUpd + 1) * 32, 1) k_sync_persistent(
           } else {
             if (lane == 0 && hinge) atomicAdd(&sm.hinge_acc, hinge);
           }
-          if (tl_rec && warp == 0 && lane == 0) tl_rec[2] = mt.n_pairs;
+          if (tl_rec && warp == 0 && lane == 0) {
+            tl_rec[2] = mt.n_pairs;
+            tl_rec[3] = (long long)mt.n_chunks | ((long long)mt.n_multi << 32);
+          }
           __syncwarp();
           if (lane == 0) mbar_arrive(&sm.empty[st]);
           if (warp == 0) DSGD_TL(3);

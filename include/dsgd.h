@@ -107,7 +107,7 @@ int dsgd_reserve(dsgd_ctx *ctx, int64_t n_samples, int64_t n_steps);
 int dsgd_set_grid_limit(dsgd_ctx *ctx, int32_t n_ctas);
 /* Developer aid (tools/timeline.py): with the environment variable DSGD_PERSIST_TIMELINE set, the persistent sync kernel
  * stamps clock64 per phase (CTA 0, 256 steps x 16 slots) and, for steps 100..103, {barrier arrival ns, barrier exit ns,
- * pairs of the CTA's rows, spare} per CTA; this copies the last launch's DSGD_TIMELINE_WORDS int64 words out. */
+ * pairs of the CTA's rows, chunks of the rows | (rows of more than one chunk << 32)} per CTA; this copies the last launch's DSGD_TIMELINE_WORDS int64 words out. */
 #define DSGD_TIMELINE_WORDS (256 * 16 + 4 * 160 * 4)
 int dsgd_debug_timeline(dsgd_ctx *ctx, long long *out);
 /* Diagnostic: rows the streaming pass (forward / gradient / eval / sampled eval of 2048 rows or more) recomputed in fp64

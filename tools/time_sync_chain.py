@@ -9,7 +9,8 @@ Every build runs in a process of its own (a library is loaded once per process),
 The card's name and power limit come from a read-only nvidia-smi query, and its SM clock from queries taken while the timed
 calls run.  Timeline: cycles from a grid barrier's pass (stamp 7 of the step before) to CTA 0's stamps of the next step,
 averaged over steps 50..250 at each batch; whether the slowest update warp reached the CTA barrier after the slowest consumer
-warp; and CTA 0's place among the arrivals of steps 100..103.  Prints one JSON line.
+warp; CTA 0's place among the arrivals of steps 100..103, and in each of those steps whether the CTAs that arrived last held
+a row of more than one 128-pair chunk.  Prints one JSON line.
 """
 import argparse
 import json
@@ -43,14 +44,32 @@ def timeline_stats(tl):
     d = {k: np.array([t[s, k] for s in ok]) - passed for k in STAMPS}
     out = {"steps": len(ok), "cycles_after_barrier_pass": {STAMPS[k]: round(float(d[k].mean())) for k in STAMPS},
            "update_after_consumers_share": float(np.mean(d[14] > d[13]))}
-    ranks = []
+    ranks, order = [], []
     for k in range(4):
         a = per[k, :, 0]
         G = int(np.count_nonzero(a))
         if G:
             ranks.append(int(np.sum(a[:G] > a[0])))   # CTAs that arrived after CTA 0
+            order.append(arrival_order(a[:G], per[k, :G, 3]))
     out["cta0_arrivals_after_it"] = ranks
+    out["arrival_order_by_multi_chunk_row"] = order
     return out
+
+
+def arrival_order(arrive_ns, chunk_word):
+    """One step's grid-barrier arrivals against whether the CTA held a row of more than one chunk (record word 3: chunks in
+    the low 32 bits, rows of several chunks in the high 32): the share of such CTAs among all, among the latest tenth and
+    as the last to arrive, and the mean arrival rank (0 first, 1 last) of the CTAs with and without one."""
+    import numpy as np
+    G = len(arrive_ns)
+    multi = (chunk_word >> 32) > 0
+    chunks = chunk_word & 0xffffffff
+    rank = np.argsort(np.argsort(arrive_ns, kind="stable"), kind="stable") / max(G - 1, 1)
+    late = np.argsort(arrive_ns, kind="stable")[-max(G // 10, 1):]
+    mean = lambda m: round(float(rank[m].mean()), 3) if m.any() else None
+    return {"ctas": G, "multi_share": round(float(multi.mean()), 3), "multi_share_latest_tenth": round(float(multi[late].mean()), 3),
+            "last_holds_multi": bool(multi[late[-1]]), "mean_rank_multi": mean(multi), "mean_rank_single": mean(~multi),
+            "chunks_latest_tenth": chunks[late].astype(int).tolist(), "max_chunks": int(chunks.max())}
 
 
 def worker(lib_path, reps, timeline):
