@@ -6,8 +6,9 @@ Python package name.)
 """
 from . import native  # noqa: F401
 from .core import Master, MasterAsync, MasterSync, Slave  # noqa: F401
-from .ml import EarlyStopping, GradState, SparseLogistic, SparseSVM, SplitStrategy  # noqa: F401
+from .ml import (EarlyStopping, GradState, SparseLogistic, SparseModifiedHuber, SparseSquaredHinge, SparseSVM,  # noqa: F401
+                 SplitStrategy)
 from .utils import Config, Data, load_config, rcv1, synthetic_rcv1  # noqa: F401
 
-__all__ = ["native", "Master", "MasterAsync", "MasterSync", "Slave", "EarlyStopping", "GradState", "SparseLogistic", "SparseSVM",
-           "SplitStrategy", "Config", "Data", "load_config", "rcv1", "synthetic_rcv1"]
+__all__ = ["native", "Master", "MasterAsync", "MasterSync", "Slave", "EarlyStopping", "GradState", "SparseLogistic",
+           "SparseModifiedHuber", "SparseSquaredHinge", "SparseSVM", "SplitStrategy", "Config", "Data", "load_config", "rcv1", "synthetic_rcv1"]

@@ -18,6 +18,7 @@ from ..ml.calibration import Calibration
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
 from ..ml.sparse_logistic import SparseLogistic
+from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge
 from ..ml.sparse_svm import SparseSVM
 from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
 from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights
@@ -192,12 +193,13 @@ class EpochDraw(list):
 class Master:
     """core/Master.scala:19-255 (abstract).  `Master.apply` (Master.scala:259-271) is `Master.create`."""
 
-    def __init__(self, node: int, data: Data, test_data: Data, model: Union[SparseSVM, SparseLogistic],
+    def __init__(self, node: int, data: Data, test_data: Data, model: Union[SparseSVM, SparseLogistic, SparseSquaredHinge, SparseModifiedHuber],
                  expected_node_count: int, *,
                  slave: Slave, group: Optional[Group] = None, seed: int = 0, log: Optional[Callable[[str], None]] = None,
                  jvm_exact: bool = False, attach: bool = True):
         self.node, self.model, self.expected_node_count = node, model, expected_node_count
-        self.logistic = isinstance(model, SparseLogistic)
+        # every model but SparseSVM has non-integer loss sums: the float *_sums evaluations, gathered in rank order
+        self.logistic = not isinstance(model, SparseSVM)
         # (w_pos, w_neg) as the Slave resolved and installed them; (1, 1): every evaluation makes the calls it made before
         self.class_weight = getattr(slave, "class_weight", (1.0, 1.0))
         # the Slave loaded per-row sample weights: every loss evaluation makes the *_weighted calls, whose loss sums already
@@ -242,7 +244,7 @@ class Master:
     # ---- evaluation ------------------------------------------------------------------------------------
     def _local_eval(self, call: str, *args):
         """(loss sum, correct count, ||w||^2) of this rank's share: ctx.<call>_counts for the SVM (its loss sum is the
-        integer hinge sum), ctx.<call>_sums for SparseLogistic.  With class weights ctx.<call>_class, and a fourth value:
+        integer hinge sum), ctx.<call>_sums for every other model.  With class weights ctx.<call>_class, and a fourth value:
         (loss sum of the positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted.  With sample
         weights ctx.<call>_weighted: (S = sum c_i L_i, correct count, ||w||^2)."""
         if self.sample_weighted:
@@ -690,8 +692,8 @@ class MasterAsync(Master):
     the best weights, and stops on `n_train * max_epoch` updates or the early-stopping rule.  SparseSVM only."""
 
     def __init__(self, node, data, test_data, model, expected_node_count, **kw):
-        if isinstance(model, SparseLogistic):
-            raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
+        if isinstance(model, (SparseLogistic, SparseSquaredHinge, SparseModifiedHuber)):
+            raise ValueError(f"{type(model).__name__}: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
         from ..ml.class_weight import resolve_class_weight

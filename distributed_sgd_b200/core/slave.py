@@ -13,13 +13,15 @@ import numpy as np
 
 from ..ml.class_weight import resolve_class_weight
 from ..ml.sparse_logistic import SparseLogistic
+from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge, model_name
 from ..ml.sparse_svm import SparseSVM
 from ..native import NativeCtx
 from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights, sample_weights_of
 
 
 class Slave:
-    def __init__(self, node: int, master: int, data: Data, model: Union[SparseSVM, SparseLogistic], is_async: bool = False, *,
+    def __init__(self, node: int, master: int, data: Data, model: Union[SparseSVM, SparseLogistic, SparseSquaredHinge, SparseModifiedHuber],
+                 is_async: bool = False, *,
                  world: int = 1, device: Optional[int] = None, test_data: Optional[Data] = None,
                  ctx: Optional[NativeCtx] = None):
         """`new Slave(node, master, data, model, async)` (core/Slave.scala:20; Main.scala:138,149).
@@ -29,11 +31,11 @@ class Slave:
         Q13).  test_data (extension): rows appended after the training rows so the same device context can
         serve Master.localLoss(testData) -- they are never sampled.  ctx (extension): a device context that already
         holds exactly these rows (train rows followed by the test rows) and its dimSparsity.
-        model: SparseSVM, or SparseLogistic (sync mode only).
+        model: SparseSVM, or SparseLogistic, SparseSquaredHinge or SparseModifiedHuber (sync mode only).
         """
-        logistic = isinstance(model, SparseLogistic)
-        if logistic and is_async:
-            raise ValueError("SparseLogistic: asynchronous (Hogwild) training supports SparseSVM only")
+        name = model_name(model)
+        if name != "svm" and is_async:
+            raise ValueError(f"{type(model).__name__}: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1 and is_async:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
         # (w_pos, w_neg) of the model's class_weight; "balanced" counts the labels of the train rows
@@ -52,7 +54,7 @@ class Slave:
         if ctx is not None:
             if ctx.n_rows != self.n_train + self.n_test or ctx.dim != data.dim:
                 raise ValueError("Slave: the given device context does not hold these rows")
-            if getattr(ctx, "logistic", False) != logistic:
+            if getattr(ctx, "model", "logistic" if getattr(ctx, "logistic", False) else "svm") != name:
                 raise ValueError("Slave: the given device context was created for another model")
             self.ctx = ctx
             if model.dim_sparsity is None:
@@ -65,7 +67,7 @@ class Slave:
                 ctx.set_sample_weights(sample_weights_of(data, test_data))
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
-                             is_async=is_async, logistic=logistic)
+                             is_async=is_async, model=name)
         if test_data is not None:
             row_ptr = np.concatenate([data.row_ptr, test_data.row_ptr[1:] + data.row_ptr[-1]])
             col = np.concatenate([data.col[:data.nnz], test_data.col[:test_data.nnz]])
@@ -100,8 +102,8 @@ class Slave:
         return self.ctx.margins(samples_idx, weights)
 
     def probabilities(self, samples_idx: Sequence[int], weights: Optional[np.ndarray] = None) -> np.ndarray:
-        """Extension, SparseLogistic only (a SparseSVM slave raises DsgdState): P(y = +1 | x) = sigmoid(-x.w) of the listed
-        rows."""
+        """Extension, SparseLogistic and SparseModifiedHuber only (other models raise DsgdState): P(y = +1 | x) of the listed
+        rows, sigmoid(-x.w) or (clip(-x.w, -1, 1) + 1) / 2."""
         self._train_ids(samples_idx)
         return self.ctx.probabilities(samples_idx, weights)
 

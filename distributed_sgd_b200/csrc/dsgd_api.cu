@@ -323,7 +323,15 @@ static void profiled(dsgd_ctx *ctx, F &&launch) {
 
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-static inline bool is_logistic(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_LOGISTIC) != 0; }
+// The model of a ctx from its flag (dsgd_create admits at most one model flag), and its name in dsgd_info and messages
+static constexpr uint32_t kModelFlags = DSGD_FLAG_LOGISTIC | DSGD_FLAG_SQUARED_HINGE | DSGD_FLAG_MODIFIED_HUBER;
+static inline int model_of(const dsgd_ctx *ctx) {
+  return (ctx->flags & DSGD_FLAG_LOGISTIC)         ? kLogistic
+         : (ctx->flags & DSGD_FLAG_SQUARED_HINGE)  ? kSquaredHinge
+         : (ctx->flags & DSGD_FLAG_MODIFIED_HUBER) ? kModifiedHuber
+                                                   : kSvm;
+}
+static const char *const kModelNames[] = {"svm", "logistic", "squared_hinge", "modified_huber"};
 // class weights other than (1, 1) are set
 static inline bool has_class_weights(const dsgd_ctx *ctx) { return !(ctx->cw_pos == 1.0 && ctx->cw_neg == 1.0); }
 // The weighting of a ctx's training passes: sample-weighted whenever sample weights are loaded, all ones included (their
@@ -336,7 +344,12 @@ static inline int weighting(const dsgd_ctx *ctx) {
 template <int kWeight, class F>
 static int with_model(const dsgd_ctx *ctx, F &&f) {
   constexpr std::integral_constant<int, kWeight> weight{};
-  return is_logistic(ctx) ? f(std::integral_constant<int, kLogistic>{}, weight) : f(std::integral_constant<int, kSvm>{}, weight);
+  switch (model_of(ctx)) {
+    case kLogistic: return f(std::integral_constant<int, kLogistic>{}, weight);
+    case kSquaredHinge: return f(std::integral_constant<int, kSquaredHinge>{}, weight);
+    case kModifiedHuber: return f(std::integral_constant<int, kModifiedHuber>{}, weight);
+    default: return f(std::integral_constant<int, kSvm>{}, weight);
+  }
 }
 template <class F>
 static int with_forms(const dsgd_ctx *ctx, int weight, F &&f) {
@@ -361,7 +374,9 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
   if (dim <= 0) return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: dim must be positive (got %d)", dim);
   if (world <= 0 || rank < 0 || rank >= world)
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: bad rank/world %d/%d", rank, world);
-  if ((flags & DSGD_FLAG_LOGISTIC) && (flags & DSGD_FLAG_ASYNC))
+  if ((flags & kModelFlags) & ((flags & kModelFlags) - 1))
+    return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: more than one model flag (0x%x)", flags & kModelFlags);
+  if ((flags & kModelFlags) && (flags & DSGD_FLAG_ASYNC))
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports the SVM model only");
   // every async worker pushes each delta into all `world` replicas and the master's, through one table of kMaxReplicas slots
   if ((flags & DSGD_FLAG_ASYNC) && world > kMaxReplicas - 1)
@@ -436,7 +451,7 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
            "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g], \"sample_weights\": %s}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
-           (long long)ctx->nnz, is_logistic(ctx) ? "logistic" : "svm", ctx->lambda1, ctx->cw_pos, ctx->cw_neg,
+           (long long)ctx->nnz, kModelNames[model_of(ctx)], ctx->lambda1, ctx->cw_pos, ctx->cw_neg,
            ctx->sw_on ? "true" : "false");
   ctx->info = buf;
   return ctx->info.c_str();
@@ -965,7 +980,7 @@ static int eval_sums(dsgd_ctx *ctx, const double *w, const row_set &rows, double
 }
 
 // the *_counts calls report integer hinge sums, which only the SVM has
-static const char kCountsNeedSvm[] = "%s: the logistic model's loss sum is not an integer; use the *_sums call";
+static const char kCountsNeedSvm[] = "%s: the %s model's loss sum is not an integer; use the *_sums call";
 
 extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
                          double *acc_out) {
@@ -982,7 +997,7 @@ extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int6
 extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *hinge_sum,
                                 int64_t *correct, double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
   row_set rows;
   int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
   return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
@@ -1000,7 +1015,7 @@ extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t 
                                         int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
                                         double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
   row_set rows;
   int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
   return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
@@ -1018,7 +1033,7 @@ extern "C" int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t ro
 extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                         int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
   if (!ctx) return DSGD_ERR_INVALID;
-  NEED(!is_logistic(ctx), DSGD_ERR_STATE, kCountsNeedSvm, __func__);
+  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
@@ -1116,12 +1131,15 @@ extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const 
 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
 
-// out[i] = x . w (prob: sigmoid(-x . w)) of the listed rows; the values go through `preds`, the per-row request buffer
+// out[i] = x . w (prob: the model's P(y = +1 | x), k_margins) of the listed rows; the values go through `preds`, the per-row
+// request buffer
 static int scores_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *out, bool prob) {
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd);
   if (rc) return rc;
-  if (prob) k_margins<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
+  if (prob && model_of(ctx) == kModifiedHuber)
+    k_margins<true, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
+  else if (prob) k_margins<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
   else k_margins<false><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
   LAUNCHED();
   CU(cudaGetLastError());
@@ -1141,7 +1159,12 @@ extern "C" int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *sampl
 extern "C" int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *probs_out) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(probs_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
-  NEED(is_logistic(ctx), DSGD_ERR_STATE, "%s: probabilities need the SparseLogistic model (DSGD_FLAG_LOGISTIC)", __func__);
+  const int m = model_of(ctx);
+  NEED(m == kLogistic || m == kModifiedHuber, DSGD_ERR_STATE,
+       m == kSvm ? "%s: probabilities need the SparseLogistic model (DSGD_FLAG_LOGISTIC)"
+                 : "%s: the squared_hinge model has no probabilities; they need SparseLogistic (DSGD_FLAG_LOGISTIC) or "
+                   "SparseModifiedHuber (DSGD_FLAG_MODIFIED_HUBER)",
+       __func__);
   row_set rows;
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   return rc ? rc : scores_pass(ctx, w, rows, probs_out, true);
@@ -2104,11 +2127,13 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   const int32_t k_total = ctx->k_total > 0 ? ctx->k_total : ctx->world;
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
   // The options the fused kernel has no form of, which with world > 1 take the per-step path over NCCL: the persistent and
-  // fused kernels are SVM-only (a logistic ctx always takes the per-step path below), and an L1 penalty, class weights or
-  // sample weights have only one-GPU persistent forms.  unfused names the first of them that is on.
-  const bool logistic = is_logistic(ctx);
+  // fused kernels are SVM-only (a ctx of any other model always takes the per-step path below), and an L1 penalty, class
+  // weights or sample weights have only one-GPU persistent forms.  unfused names the first of them that is on.
+  static const char *const kModelTakes[] = {nullptr, "the logistic model takes", "the squared_hinge model takes",
+                                            "the modified_huber model takes"};
+  const int model = model_of(ctx);
   const int weight = weighting(ctx);
-  const char *unfused = logistic ? "the logistic model takes"
+  const char *unfused = model != kSvm ? kModelTakes[model]
                         : ctx->lambda1 > 0.0 ? "the L1 penalty takes"
                         : has_class_weights(ctx) ? "class weights take"
                         : weight == kSampleWeighted ? "sample weights take" : nullptr;
@@ -2128,7 +2153,7 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
     int rc = ctx->losses.grow(ctx, n_steps, 1024);
     if (rc) return rc;
   }
-  if ((single && !logistic && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
+  if ((single && model == kSvm && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
     // exchange block mapped (fused): the same kernel aggregates over NVLink
     return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, lrs,

@@ -37,7 +37,7 @@ enum Cnt : int {
   kCntTicket = 2,   // last-block ticket of k_update
   kCntWLoss = 3,    // class-weighted batch: the bits of the double w_pos * L_pos + w_neg * L_neg (k_class_fold), which the
                     // weighted tails (kCw) read instead of kCntHinge / kCntLoss
-  kCntLoss = 8,     // logistic model: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
+  kCntLoss = 8,     // every model but the SVM: fixed-point sum of the batch's per-sample losses (kLossAccWords words, dsgd_fixed.cuh)
   kCntL1 = 16,      // fixed-point sum of |w_j| (kLossAccWords words): k_update<..., kL1>, k_l1_norm; zero between launches
   kCntNnz = 23,     // #{w_j != 0} of k_l1_norm; zero between launches
   // per-class counters of k_rows<..., kClassWeighted, ...>, cleared by k_class_fold: index 0 is the class y = +1, index 1 the
@@ -45,7 +45,7 @@ enum Cnt : int {
   kCntClassN = 24,        // rows
   kCntClassCorrect = 26,  // #{pred == y}
   kCntClassHinge = 28,    // SVM: hinge sums (integers)
-  kCntClassLoss = 32,     // logistic: two fixed-point sums of the unweighted losses, kLossAccWords words each
+  kCntClassLoss = 32,     // not the SVM: two fixed-point sums of the unweighted losses, kLossAccWords words each
   // fixed-point sums of k_rows<..., kSampleWeighted, ...> (kLossAccWords words each), taken by k_sw_fold: S = sum R(c_i L_i),
   // and for an evaluation sum R(c_i [pred_i == y_i]) and sum R(c_i)
   kCntSwLoss = 48,
@@ -61,6 +61,9 @@ static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kC
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
 constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
 constexpr int kLogistic = 1;   // SparseLogistic: softplus loss, gradient x * (y * sigmoid(y * x.w))
+constexpr int kSquaredHinge = 2;    // SparseSquaredHinge: the L2-loss SVM, loss (1 + z)^2 above z = -1
+constexpr int kModifiedHuber = 3;   // SparseModifiedHuber: (1 + z)^2 on (-1, 1], 4 z above
+// Every model but the SVM has non-integer per-sample losses: they are added in the fixed-point limbs of dsgd_fixed.cuh
 // Weighting of a sync pass, a compile-time parameter of the row pass and of the persistent kernel.
 constexpr int kUnweighted = 0;
 constexpr int kClassWeighted = 1;    // dsgd_set_class_weights: row i counts w_y (w_pos or w_neg by its label)
@@ -70,7 +73,7 @@ constexpr int kSampleWeighted = 2;   // dsgd_set_sample_weights: row i counts c_
 template <int kModel, bool kCw = false>
 __device__ __forceinline__ double batch_loss_sum(const unsigned long long *cnt) {
   if (kCw) return __longlong_as_double((long long)cnt[kCntWLoss]);
-  return kModel == kLogistic ? acc_value(cnt + kCntLoss) : (double)cnt[kCntHinge];
+  return kModel != kSvm ? acc_value(cnt + kCntLoss) : (double)cnt[kCntHinge];
 }
 template <int kModel, bool kCw = false>
 __device__ __forceinline__ void clear_batch_loss(unsigned long long *cnt) {
@@ -79,7 +82,7 @@ __device__ __forceinline__ void clear_batch_loss(unsigned long long *cnt) {
     return;
   }
   cnt[kCntHinge] = 0ull;
-  if (kModel == kLogistic)
+  if (kModel != kSvm)
 #pragma unroll
     for (int i = 0; i < kLossAccWords; ++i) cnt[kCntLoss + i] = 0ull;
 }
@@ -248,8 +251,45 @@ __device__ __forceinline__ double sigmoid(double t) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_rows: the per-sample body of SlaveImpl.gradient / SlaveImpl.forward (core/Slave.scala:129-157) for either model and
-// weighting: one warp per row window; fp64 dot with the L2-resident weights (the logistic loss and sigmoid need the dot's
+// SparseSquaredHinge and SparseModifiedHuber, one sample with z = y * (x . w) and t = fl(1 + z).  The classifier's margin
+// is -z (the prediction is -signum(x . w)), so both losses vanish for z <= -1.  Per-sample loss L and backward scale s
+// (backward x * (y * s), weighted (y * s) * c), each a short chain of correctly rounded fp64 operations in this order:
+//   squared hinge    z <= -1: L = 0, s = 0;   else L = t * t, s = 2 * t
+//   modified Huber   z <= -1: L = 0, s = 0;   -1 < z <= 1: L = t * t, s = 2 * t;   z > 1: L = 4 * z, s = 4
+// The modified Huber loss is continuous at z = 1 (t * t = 4 = 4 * z, 2 * t = 4).  With --fmad=false nothing is contracted,
+// so the C oracle (oracle/dsgd_oracle_margin.c) gives the same bits.
+// ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double sq_hinge_loss(double z) {
+  const double t = 1.0 + z;
+  return z <= -1.0 ? 0.0 : t * t;
+}
+__device__ __forceinline__ double sq_hinge_scale(double z) { return z <= -1.0 ? 0.0 : 2.0 * (1.0 + z); }
+__device__ __forceinline__ double mod_huber_loss(double z) {
+  const double t = 1.0 + z;
+  return z <= -1.0 ? 0.0 : (z <= 1.0 ? t * t : 4.0 * z);
+}
+__device__ __forceinline__ double mod_huber_scale(double z) { return z <= -1.0 ? 0.0 : (z <= 1.0 ? 2.0 * (1.0 + z) : 4.0); }
+
+// The per-sample loss L(z) and backward scale s(z) of a model other than the SVM (whose loss is an integer of the
+// prediction and whose gate is a branch of k_rows)
+template <int kModel>
+__device__ __forceinline__ double row_loss(double z) {
+  static_assert(kModel != kSvm, "the SVM's loss is the integer hinge of its prediction");
+  if constexpr (kModel == kLogistic) return softplus(z);
+  else if constexpr (kModel == kSquaredHinge) return sq_hinge_loss(z);
+  else return mod_huber_loss(z);
+}
+template <int kModel>
+__device__ __forceinline__ double row_scale(double z) {
+  static_assert(kModel != kSvm, "the SVM's scale is its label");
+  if constexpr (kModel == kLogistic) return sigmoid(z);
+  else if constexpr (kModel == kSquaredHinge) return sq_hinge_scale(z);
+  else return mod_huber_scale(z);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_rows: the per-sample body of SlaveImpl.gradient / SlaveImpl.forward (core/Slave.scala:129-157) for every model and
+// weighting: one warp per row window; fp64 dot with the L2-resident weights (every loss but the SVM's needs the dot's
 // value, not only its sign: the fp32 streaming pass of dsgd_stream.cuh is SVM-only); prediction, per-sample loss and gate;
 // scatter into the dense gradient with fp64 reductions at L2 (no return value -> RED, not ATOM).
 //   kScatter: accumulate backward() into g            (SparseSVM.scala:26-29)
@@ -258,19 +298,20 @@ __device__ __forceinline__ double sigmoid(double t) {
 // The scatter value s of a row, then filt(filt(x_j) * s) per entry, so a zero weight adds nothing:
 //   SVM       s = y, weighted y * c  (an exact sign flip of c),  added where !(y * dot < 0)
 //   logistic  s = y * sigmoid(z), weighted (y * sigmoid(z)) * c,  added for every row
+//   squared hinge, modified Huber  s = y * s(z), weighted (y * s(z)) * c (row_scale),  added where z > -1 (s(z) = 0 below)
 // where c is the row's weight: w_y with class weights, c_i = fl(w_y * s_i) with sample weights (sw == nullptr, an
 // evaluation of a ctx without sample weights: every s_i is 1).  The unweighted passes do not read w_pos, w_neg or sw, and
 // kScatter = false with class weights is the pass of dsgd_eval*_class, which does not read the weights.
 // Lane 0's tally, the same in any row order or grid (integer counters, or R(.) added to fixed-point limbs in registers
 // and pushed once per warp, dsgd_fixed.cuh):
 //   unweighted      SVM: the hinge sum and the correct count (hinge losses are integers: y, p in {-1,0,1});
-//                   logistic: the correct count and the limbs of softplus(z)
-//   class weights   rows, correct predictions and the unweighted loss per class (SVM: integer hinge sums; logistic: two
+//                   other models: the correct count and the limbs of L(z) (row_loss)
+//   class weights   rows, correct predictions and the unweighted loss per class (SVM: integer hinge sums; others: two
 //                   limb blocks, a row adds its loss to its class's block and an exact 0 to the other); k_class_fold
 //                   applies the weights
 //   sample weights  R(fl(c_i * L_i)) into one limb block (S, kCntSwLoss) and the correct count; an evaluation (kScatter =
 //                   false) also R(c_i) of the correct rows (kCntSwCorrect) and of every row (kCntSwWeight).  With s = 1
-//                   and w = (1, 1) the SVM's S is the integer hinge sum and the logistic S the unweighted limb sum.
+//                   and w = (1, 1) the SVM's S is the integer hinge sum and any other model's S the unweighted limb sum.
 // The counters are plain locals of every form, each form using its own: held in a struct, nvcc orders the loop's
 // registers differently, and the forms would no longer compile to the instructions of the separate kernels they replaced.
 // ---------------------------------------------------------------------------------------------------
@@ -307,7 +348,9 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
         const int p = pred_of(dot);
         const bool ok = p == yi;
         correct += (unsigned)ok;
-        const double l = kModel == kLogistic ? softplus(z) : (double)(1 - yi * p);
+        double l;
+        if constexpr (kModel != kSvm) l = row_loss<kModel>(z);
+        else l = (double)(1 - yi * p);
         acc_add_local(lim, ovf, ci * l);
         if (!kScatter) {
           acc_add_local(lim_ok, ovf_ok, ok ? ci : 0.0);
@@ -317,17 +360,17 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
         const int p = pred_of(dot);
         const unsigned ok = (unsigned)(p == yi);
         if (pos) { ++n_pos; ok_pos += ok; } else { ++n_neg; ok_neg += ok; }
-        if (kModel == kLogistic) {
-          const double l = softplus(z);
+        if constexpr (kModel != kSvm) {
+          const double l = row_loss<kModel>(z);
           acc_add_local(lim_pos, ovf_pos, pos ? l : 0.0);
           acc_add_local(lim_neg, ovf_neg, pos ? 0.0 : l);
         } else {
           const unsigned l = (unsigned)(1 - yi * p);
           if (pos) h_pos += l; else h_neg += l;
         }
-      } else if constexpr (kModel == kLogistic) {
+      } else if constexpr (kModel != kSvm) {
         correct += (unsigned)(pred_of(dot) == (int)y);
-        acc_add_local(lim, ovf, softplus(z));
+        acc_add_local(lim, ovf, row_loss<kModel>(z));
       } else {
         const int p = pred_of(dot);
         const int yv = (int)y;
@@ -339,8 +382,9 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
     if (kScatter) {
       const double c = kCls ? (pos ? w_pos : w_neg) : ci;   // the row's weight
       double s;
-      if (kModel == kLogistic) {
-        s = kWeight == kUnweighted ? y * sigmoid(z) : (y * sigmoid(z)) * c;
+      if constexpr (kModel != kSvm) {
+        if (kModel != kLogistic && z <= -1.0) continue;   // s = 0: the row scatters nothing
+        s = kWeight == kUnweighted ? y * row_scale<kModel>(z) : (y * row_scale<kModel>(z)) * c;
       } else {
         if (z < 0.0) continue;  // SparseSVM.scala:28: gradient unless activity < 0
         s = kWeight == kUnweighted ? y : (pos ? c : -c);
@@ -361,14 +405,14 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
       if (n_neg) atomicAdd(&cnt[kCntClassN + 1], (unsigned long long)n_neg);
       if (ok_pos) atomicAdd(&cnt[kCntClassCorrect], (unsigned long long)ok_pos);
       if (ok_neg) atomicAdd(&cnt[kCntClassCorrect + 1], (unsigned long long)ok_neg);
-      if (kModel == kLogistic) {
+      if (kModel != kSvm) {
         acc_flush_local(cnt + kCntClassLoss, lim_pos, ovf_pos);
         acc_flush_local(cnt + kCntClassLoss + kLossAccWords, lim_neg, ovf_neg);
       } else {
         if (h_pos) atomicAdd(&cnt[kCntClassHinge], (unsigned long long)h_pos);
         if (h_neg) atomicAdd(&cnt[kCntClassHinge + 1], (unsigned long long)h_neg);
       }
-    } else if (kSw || kModel == kLogistic) {
+    } else if (kSw || kModel != kSvm) {
       if (correct) atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
       acc_flush_local(cnt + (kSw ? kCntSwLoss : kCntLoss), lim, ovf);
       if (kSw && !kScatter) {
@@ -406,7 +450,7 @@ template <int kModel>
 __global__ void k_class_fold(unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
                              const double *__restrict__ scal_nrm2, double *__restrict__ out) {
   double l_pos, l_neg;
-  if (kModel == kLogistic) {
+  if (kModel != kSvm) {
     l_pos = acc_take(cnt + kCntClassLoss);
     l_neg = acc_take(cnt + kCntClassLoss + kLossAccWords);
   } else {
@@ -610,7 +654,7 @@ __global__ void k_l1_finish(unsigned long long *__restrict__ cnt, double *__rest
 
 // ---------------------------------------------------------------------------------------------------
 // k_loss_scalar: loss = lambda*||w||^2 + loss sum/n, acc = correct/n from the counters (SVM: hinge sum, an integer;
-// logistic: the fixed-point sum of the softplus losses; kCw: the class-weighted sum of k_class_fold).
+// other models: the fixed-point sum of their per-sample losses; kCw: the class-weighted sum of k_class_fold).
 // ---------------------------------------------------------------------------------------------------
 template <int kModel, bool kCw>
 __global__ void k_loss_scalar(const double *__restrict__ scal_nrm2, unsigned long long *__restrict__ cnt, double lambda,

@@ -46,10 +46,16 @@ __device__ __forceinline__ unsigned long long score_key(double s) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_margins: out[i] = x . w of row samples[i] (kProb: P(y = +1 | x) = sigmoid(-x . w), the model's probability, with the
-// `sigmoid` of the logistic gradient).  One warp per row, in sample order.
+// k_margins: out[i] = x . w of row samples[i] (kProb: P(y = +1 | x), the model's probability: SparseLogistic's
+// sigmoid(-x . w), with the `sigmoid` of the logistic gradient, or with kHuber SparseModifiedHuber's
+// (clip(-x . w, -1, 1) + 1) / 2, scikit-learn's predict_proba for that loss, NaN for a NaN margin).  One warp per row, in sample order.
 // ---------------------------------------------------------------------------------------------------
-template <bool kProb>
+__device__ __forceinline__ double huber_prob(double dot) {
+  double m = -dot;
+  m = m < -1.0 ? -1.0 : (m > 1.0 ? 1.0 : m);
+  return (m + 1.0) / 2.0;
+}
+template <bool kProb, bool kHuber = false>
 __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                  const int32_t *__restrict__ samples, int64_t n,
                                                  const double *__restrict__ w, double *__restrict__ out) {
@@ -58,7 +64,7 @@ __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t i = warp0; i < n; i += nwarps) {
     const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
-    if (lane == 0) out[i] = kProb ? sigmoid(-dot) : dot;
+    if (lane == 0) out[i] = !kProb ? dot : (kHuber ? huber_prob(dot) : sigmoid(-dot));
   }
 }
 

@@ -10,9 +10,12 @@ object DsgdNative {
 
   // every native returns the C ABI's status code; 0 = OK, negative = DSGD_ERR_*  (include/dsgd.h).  Arrays are copied in
   // before and out after the call (Get/Set<Type>ArrayRegion): nothing is pinned while a call blocks on the GPU.
-  // flags: FlagAsync | FlagLogistic (DSGD_FLAG_*); FlagLogistic selects SparseLogistic instead of SparseSVM (sync mode only)
+  // flags: FlagAsync | one model flag (DSGD_FLAG_*); FlagLogistic, FlagSquaredHinge or FlagModifiedHuber selects
+  // SparseLogistic, SparseSquaredHinge or SparseModifiedHuber instead of SparseSVM (sync mode only, at most one of them)
   final val FlagAsync = 1
   final val FlagLogistic = 2
+  final val FlagSquaredHinge = 4
+  final val FlagModifiedHuber = 8
   @native def create(device: Int, dim: Int, lambda: Double, rank: Int, world: Int, flags: Int): Long
   @native def destroy(ctx: Long): Int
   @native def lastError(ctx: Long): String
@@ -34,7 +37,7 @@ object DsgdNative {
                                 posEnd: Long, hingeCorrect: Array[Long], normSquared: Array[Double]): Int
   @native def evalSamplesCounts(ctx: Long, w: Array[Double], samples: Array[Int], hingeCorrect: Array[Long],
                                 normSquared: Array[Double]): Int
-  // the same passes for either model (the *Counts forms refuse a logistic ctx): lossSumNormSquared = {sum of the per-sample
+  // the same passes for every model (the *Counts forms refuse a ctx of any model but the SVM): lossSumNormSquared = {sum of the per-sample
   // losses, ||w||^2}, correct = {#correct}
   @native def evalSums(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, lossSumNormSquared: Array[Double],
                        correct: Array[Long]): Int
@@ -42,7 +45,7 @@ object DsgdNative {
                               posEnd: Long, lossSumNormSquared: Array[Double], correct: Array[Long]): Int
   @native def evalSamplesSums(ctx: Long, w: Array[Double], samples: Array[Int], lossSumNormSquared: Array[Double],
                               correct: Array[Long]): Int
-  // scores (out.length >= samples.length): the margins x.w, or P(y = +1 | x) on a FlagLogistic context; ranking metrics
+  // scores (out.length >= samples.length): the margins x.w, or P(y = +1 | x) on a FlagLogistic or FlagModifiedHuber context; ranking metrics
   // (metrics.length >= MetricsWords): TP, FN, positives without a prediction, FP, TN, negatives without one, U2, NaN rows --
   // AUC = U2 / (2 P N)
   final val MetricsWords = 8

@@ -26,11 +26,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
              async_concurrency: int = 64, jvm_exact: bool = False, inspect=None) -> dict:
     """Main.scenario (Main.scala:70-120).  inspect (tests): called as inspect("master", master) once the master exists
     and as inspect("done", (master, state)) before the device context is released."""
-    from . import EarlyStopping, Master, Slave, SparseLogistic, SparseSVM
+    from . import EarlyStopping, Master, Slave, SparseLogistic, SparseModifiedHuber, SparseSquaredHinge, SparseSVM
     from .core import Group
 
-    if cfg.model == "logistic" and cfg.is_async:
-        raise ValueError("model = logistic: asynchronous (Hogwild) training supports the svm model only")
+    if cfg.model != "svm" and cfg.is_async:
+        raise ValueError(f"model = {cfg.model}: asynchronous (Hogwild) training supports the svm model only")
     if cfg.average_from >= 0 and cfg.is_async:
         raise ValueError("average-from: averaged SGD is a sync-mode option; asynchronous (Hogwild) training does not average")
     if cfg.learning_rate_decay != 0.0 and cfg.is_async:
@@ -49,7 +49,9 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
-    model = (SparseLogistic if cfg.model == "logistic" else SparseSVM)(cfg.lam, l1=cfg.l1, class_weight=class_weight)
+    model_class = {"logistic": SparseLogistic, "squared_hinge": SparseSquaredHinge,
+                   "modified_huber": SparseModifiedHuber}.get(cfg.model, SparseSVM)
+    model = model_class(cfg.lam, l1=cfg.l1, class_weight=class_weight)
     slave = Slave(rank, 0, train, model, cfg.is_async, world=world, device=device, test_data=test)
     master = Master.create(rank, train, test, model, cfg.is_async, cfg.node_count, slave=slave, group=Group(), seed=seed,
                            log=(log if rank == 0 else None), jvm_exact=jvm_exact)

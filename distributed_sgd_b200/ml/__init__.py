@@ -4,4 +4,5 @@ from .calibration import Calibration  # noqa: F401
 from .grad_state import GradState  # noqa: F401
 from .lr_schedule import learning_rates  # noqa: F401
 from .sparse_logistic import SparseLogistic  # noqa: F401
+from .sparse_margin import SparseModifiedHuber, SparseSquaredHinge  # noqa: F401
 from .sparse_svm import SparseSVM  # noqa: F401

@@ -24,6 +24,10 @@ UNIQUE_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
 FLAG_ASYNC = 1
 FLAG_LOGISTIC = 2
+FLAG_SQUARED_HINGE = 4
+FLAG_MODIFIED_HUBER = 8
+# NativeCtx(model=...) -> the model flag of dsgd_create
+MODEL_FLAGS = {"svm": 0, "logistic": FLAG_LOGISTIC, "squared_hinge": FLAG_SQUARED_HINGE, "modified_huber": FLAG_MODIFIED_HUBER}
 REPLICA_SELF, REPLICA_MASTER = 0, 1
 
 OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM, ERR_TIMEOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8
@@ -292,15 +296,21 @@ def _arr(a, dtype, n: Optional[int] = None, what: str = "array") -> np.ndarray:
 
 
 class NativeCtx:
-    """One dsgd_ctx == one GPU worker (a reference Slave with its SparseSVM, or with a SparseLogistic if `logistic`)."""
+    """One dsgd_ctx == one GPU worker (a reference Slave with its SparseSVM, or with the model named by `model`: "svm",
+    "logistic", "squared_hinge" or "modified_huber"; `logistic=True` is model="logistic")."""
 
     def __init__(self, device: int, dim: int, lam: float, rank: int = 0, world: int = 1, is_async: bool = False,
-                 logistic: bool = False):
+                 logistic: bool = False, model: Optional[str] = None):
+        if model is None:
+            model = "logistic" if logistic else "svm"
+        elif model not in MODEL_FLAGS or (logistic and model != "logistic"):
+            raise ValueError(f"NativeCtx: model must be one of {', '.join(MODEL_FLAGS)} (got {model!r}, logistic={logistic})")
         self._l = lib()
         self._h = C.c_void_p()
         self.dim, self.lam, self.rank, self.world, self.device = int(dim), float(lam), int(rank), int(world), int(device)
-        self.logistic = bool(logistic)
-        flags = (FLAG_ASYNC if is_async else 0) | (FLAG_LOGISTIC if logistic else 0)
+        self.model = model
+        self.logistic = model == "logistic"
+        flags = (FLAG_ASYNC if is_async else 0) | MODEL_FLAGS[model]
         rc = self._l.dsgd_create(C.byref(self._h), device, dim, lam, rank, world, flags)
         if rc != OK:
             msg = (self._l.dsgd_last_error(None) or b"").decode()
@@ -459,7 +469,8 @@ class NativeCtx:
         return self._request("margins", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
 
     def probabilities(self, samples, w=None) -> np.ndarray:
-        """P(y = +1 | x) = sigmoid(-x . w) for each listed row; SparseLogistic contexts only (dsgd_probabilities)."""
+        """P(y = +1 | x) for each listed row (dsgd_probabilities): sigmoid(-x . w) on a SparseLogistic context,
+        (clip(-x . w, -1, 1) + 1) / 2 on a SparseModifiedHuber one; other models raise DsgdState."""
         samples = _arr(samples, np.int32)
         return self._request("probabilities", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
 

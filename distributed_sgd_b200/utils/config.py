@@ -31,7 +31,8 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     leaky_loss: float = 0.9
     conv_delta: float = 0.01
     patience: int = 5
-    model: str = "svm"            # extension: "svm" (SparseSVM) or "logistic" (SparseLogistic, sync mode only)
+    model: str = "svm"            # extension: "svm" (SparseSVM), or "logistic", "squared_hinge" or "modified_huber"
+                                  # (SparseLogistic, SparseSquaredHinge, SparseModifiedHuber; sync mode only)
     average_from: int = -1        # extension: averaged SGD from this epoch (0-based) on, sync mode only; -1: off
     learning_rate_decay: float = 0.0   # extension: step t uses learning-rate / (1 + decay * t)^power, sync mode only
     learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
@@ -56,7 +57,7 @@ _KEYS = {
     "l1": ("l1", "DSGD_L1"), "class-weight": ("class_weight", "DSGD_CLASS_WEIGHT"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
 }
-MODELS = ("svm", "logistic")
+MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}
 
 

@@ -69,6 +69,17 @@ extern "C" {
  * ctx takes the per-step sync path (never the persistent or fused kernel), so world > 1 needs dsgd_comm_init.  Combined with
  * DSGD_FLAG_ASYNC, dsgd_create fails with DSGD_ERR_INVALID (async mode supports the SVM model only). */
 #define DSGD_FLAG_LOGISTIC 2u
+/* The margin models beside it, z = y * (x . w), t = fl(1 + z) (DESIGN.md section 4.15):
+ *   DSGD_FLAG_SQUARED_HINGE   SparseSquaredHinge, the L2-loss SVM: per-sample loss 0 for z <= -1, else t * t; gradient
+ *                             x * (y * s) with s = 0 for z <= -1, else 2 * t.
+ *   DSGD_FLAG_MODIFIED_HUBER  SparseModifiedHuber: loss 0 for z <= -1, t * t for -1 < z <= 1, 4 * z above; s = 0, 2 * t, 4.
+ * Like DSGD_FLAG_LOGISTIC they keep the SVM's prediction, regularize() and sync step, follow it in every call that depends
+ * on the model, add their losses in the fixed-point limbs of the logistic loss sum, are refused by the *_counts calls
+ * (DSGD_ERR_STATE) and take the per-step sync path.  dsgd_probabilities serves SparseModifiedHuber, not
+ * SparseSquaredHinge.  dsgd_create fails with DSGD_ERR_INVALID on more than one model flag, and on any model flag with
+ * DSGD_FLAG_ASYNC. */
+#define DSGD_FLAG_SQUARED_HINGE 4u
+#define DSGD_FLAG_MODIFIED_HUBER 8u
 
 typedef struct dsgd_ctx dsgd_ctx;
 
@@ -174,7 +185,7 @@ int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, 
  * outside the loaded rows -> DSGD_ERR_RANGE before anything is launched.  The staged sample stream is left intact. */
 int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *hinge_sum,
                              int64_t *correct, double *norm_squared);
-/* The three *_counts calls above report the hinge sum as an integer, which only the SVM has: on a DSGD_FLAG_LOGISTIC ctx they
+/* The three *_counts calls above report the hinge sum as an integer, which only the SVM has: on a ctx of any other model they
  * fail with DSGD_ERR_STATE.  The *_sums forms take the same arguments and report the sum of the per-sample losses as a double
  * instead, for either model (for the SVM, the hinge sum: an exact integer held in a double).  The logistic sum is added in
  * fixed point on the device, so a pass returns the same bits whatever the order in which its rows are taken. */
@@ -193,8 +204,9 @@ int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *sample
  *      other path, and the metrics rank exactly the values dsgd_margins returns for the same rows. ---- */
 /* margins_out[i] = x_i . w in fp64 (the value whose -signum dsgd_forward reports) */
 int dsgd_margins(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *margins_out);
-/* SparseLogistic only: probs_out[i] = P(y = +1 | x_i) = sigmoid(-x_i . w), with the sigmoid of the logistic gradient; an SVM ctx
- * -> DSGD_ERR_STATE (its margins are not calibrated probabilities). */
+/* SparseLogistic: probs_out[i] = P(y = +1 | x_i) = sigmoid(-x_i . w), with the sigmoid of the logistic gradient;
+ * SparseModifiedHuber: (clip(-x_i . w, -1, 1) + 1) / 2.  An SVM or squared-hinge ctx -> DSGD_ERR_STATE (its margins are not
+ * probabilities). */
 int dsgd_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *probs_out);
 
 #define DSGD_METRICS_WORDS 8
