@@ -77,7 +77,16 @@ extern "C" {
  * on the model, add their losses in the fixed-point limbs of the logistic loss sum, are refused by the *_counts calls
  * (DSGD_ERR_STATE) and take the per-step sync path.  dsgd_probabilities serves SparseModifiedHuber, not
  * SparseSquaredHinge.  dsgd_create fails with DSGD_ERR_INVALID on more than one model flag, and on any model flag with
- * DSGD_FLAG_ASYNC. */
+ * DSGD_FLAG_ASYNC.
+ * Loss sums and the 2^52 limit: a summed value of 2^52 or more, infinite or NaN makes its sum NaN (the squared hinge
+ * reaches 2^52 at z = 2^26 - 1, modified Huber at z = 2^50; their losses pass it long before the logistic loss does).  The
+ * next pass or step starts from a clean sum.  The unweighted and per-class evaluations sum L_i; a class-weighted gradient or
+ * step sums L_i per class and then takes fl(w_pos * S+) + fl(w_neg * S-); the weighted evaluations (dsgd_eval*_weighted)
+ * and a sample-weighted gradient or step sum fl(c_i * L_i).  So with class weights (2, 1/2) and a row of L in
+ * [2^51, 2^52), the class-weighted loss is finite and the weighted evaluation NaN; with a class weight of 0 and a row of
+ * finite L >= 2^52 in that class, the class-weighted loss is NaN (0 * NaN) and the weighted evaluation adds an exact 0.
+ * At a NaN z the squared hinge's scale is NaN, which the 1e-20 filter drops (no gradient), and modified Huber's is 4 (both
+ * branch tests are false). */
 #define DSGD_FLAG_SQUARED_HINGE 4u
 #define DSGD_FLAG_MODIFIED_HUBER 8u
 

@@ -165,3 +165,37 @@ def sync_steps(orc: Oracle, model, w, idx, counts: Sequence[int], lrs, w_pos: fl
                                                C.c_double(w_neg), _p(_sw(orc, sw)), _p(losses), _p(avg_sum)),
            "margin sync_steps")
     return w, losses
+
+
+class MarginOracle:
+    """One model's checker with the interface of oracle.Oracle (loss_acc, sample_losses, forward, gradient, sync_steps and
+    the rows, lambda and dimSparsity of `orc`), in the weighting (w_pos, w_neg, sw) and with the L1 penalty lambda1 of the
+    steps, so that a test written against an Oracle can take any model of this checker."""
+
+    def __init__(self, orc: Oracle, model, w_pos: float = 1.0, w_neg: float = 1.0, sw=None, lambda1: float = 0.0):
+        self.base, self.model = orc, model
+        self.w_pos, self.w_neg, self.sw, self.lambda1 = w_pos, w_neg, sw, lambda1
+
+    def __getattr__(self, name):
+        return getattr(self.base, name)
+
+    def loss_acc(self, w, idx=None, begin: int = 0, n: Optional[int] = None):
+        return loss_acc(self.base, self.model, w, idx, begin, n)[:2]
+
+    def sample_losses(self, w, idx=None, begin: int = 0, n: Optional[int] = None) -> np.ndarray:
+        return sample_losses(self.base, self.model, w, idx, begin, n)
+
+    def gradient(self, w, idx):
+        """(gradient in the weighting, c = 2 lambda (w . d))"""
+        g, _, _ = gradient(self.base, self.model, w, idx, self.w_pos, self.w_neg, self.sw)
+        wd = self.base._w(w) * self.base.d
+        return g, self.base.lam * 2.0 * float(np.sum(np.where(np.abs(wd) > 1e-20, wd, 0.0)))
+
+    def gradient_loss(self, w, idx) -> float:
+        """The loss a gradient request reports in the weighting"""
+        return gradient(self.base, self.model, w, idx, self.w_pos, self.w_neg, self.sw)[1]
+
+    def sync_steps(self, w, idx, counts: Sequence[int], lr: float, n_steps: int = 1, lrs=None, avg_sum=None):
+        lrs = np.full(n_steps, lr) if lrs is None else lrs
+        return sync_steps(self.base, self.model, w, idx, counts, lrs, self.w_pos, self.w_neg, self.sw,
+                          lambda1=self.lambda1, avg_sum=avg_sum)

@@ -106,14 +106,14 @@ def _abs_oracle(env):
 
 # ---- the readers beyond read_all -----------------------------------------------------------------------------------------
 
-def read_more(ctx, env, w, logistic, weighted):
+def read_more(ctx, env, w, model, weighted):
     """Every reader added since read_all, once, at the weights w (None: resident).  {reader: value}."""
     ids = env.ids
     a, b = CAL_AB
     out = {}
     for name in ("fwd_rows", "fwd_stream"):
         out["margins_" + name] = ctx.margins(ids[name], w)
-    if logistic:
+    if model == "logistic":
         out["probabilities"] = ctx.probabilities(ids["fwd_stream"], w)
     out["metrics_range"] = ctx.eval_metrics(0, N_STREAM, w)
     out["metrics_sampled"] = ctx.eval_sampled_metrics(0, N_ROWS, KEY, 100, 1100, w)
@@ -139,7 +139,7 @@ CLASS_IDS = {"class_range": lambda env: np.arange(N_STREAM), "class_rows": lambd
              "class_sampled": lambda env: env.sampled[:2500], "class_list": lambda env: env.ids["samples"]}
 
 
-def check_more(ctx, env, orc, w, got, logistic, exact, what):
+def check_more(ctx, env, orc, w, got, model, exact, what):
     """The readers of read_more at the explicit weights w against the checkers."""
     ids, data = env.ids, env.data
     bad = []
@@ -151,7 +151,7 @@ def check_more(ctx, env, orc, w, got, logistic, exact, what):
             ok = (np.abs(m - ref) <= 1e-12 * OM.margins(_abs_oracle(env), np.abs(w), idx=ids[name])).all()
         if not ok:
             bad.append(f"margins over {name}: {np.count_nonzero(m != ref)} differ from the checker's")
-    if logistic:
+    if model == "logistic":
         m = ctx.margins(ids["fwd_stream"], w)
         e = np.exp(-np.abs(m))
         ref = np.where(m <= 0, 1.0 / (1.0 + e), e / (1.0 + e))     # sigmoid(-m)
@@ -210,10 +210,10 @@ def check_more(ctx, env, orc, w, got, logistic, exact, what):
         if k not in got:
             continue
         ce = got[k]
-        sums, counts = CW.eval_class(orc, w, f(env), logistic)
+        sums, counts = CW.eval_class(orc, w, f(env), model == "logistic")
         if [ce.correct_pos, ce.correct_neg, ce.n_pos, ce.n_neg] != list(counts):
             bad.append(f"{k}: counts {ce[3:]} against {tuple(counts)}")
-        if logistic:
+        if model == "logistic":
             ok = np.allclose([ce.loss_pos, ce.loss_neg], sums, rtol=1e-12, atol=0)
         else:
             ok = [ce.loss_pos, ce.loss_neg] == list(sums)
@@ -224,13 +224,13 @@ def check_more(ctx, env, orc, w, got, logistic, exact, what):
     assert not bad, f"{what}:\n" + "\n".join(bad)
 
 
-def check_weighted_gradients(ctx, env, orc, w, c, got_res, got_exp, logistic, exact, what):
+def check_weighted_gradients(ctx, env, orc, w, c, got_res, got_exp, model, exact, what):
     """The class-weighted gradient requests at w == NULL and at w against oracle/cw.gradient."""
     wp, wn = ctx.get_class_weights()
     for name in ("grad_stream", "grad_rows"):
         idx = env.ids[name]
         (g_res, l_res), (g, loss) = [(d[name]["grad"], d[name]["loss"]) for d in (got_res, got_exp)]
-        g_ref, loss_ref, _ = CW.gradient(orc, w, idx, wp, wn, logistic=logistic)
+        g_ref, loss_ref, _ = CW.gradient(orc, w, idx, wp, wn, logistic=model == "logistic")
         # the summed magnitudes of a column's terms: each row's is at most max(w_pos, w_neg) |x_j|, and c enters once
         mag = max(wp, wn) * _grad_scale(env, env.data, idx, 0.0) + abs(c)
         if exact:
@@ -246,24 +246,24 @@ def check_weighted_gradients(ctx, env, orc, w, c, got_res, got_exp, logistic, ex
             assert abs(v - loss_ref) <= 1e-11 * abs(loss_ref), f"{what}: {name} loss ({who}) {v!r} against {loss_ref!r}"
 
 
-def check_all_readers(ctx, env, orc, logistic, exact_resident, exact_oracle, what, weighted=None, check_gradients=None):
+def check_all_readers(ctx, env, orc, model, exact_resident, exact_oracle, what, weighted=None, check_gradients=None):
     """Every reader at w == NULL against the explicit weights, and those against the checkers; returns (w, c).  weighted:
     the gradient is weighted (default: by class weights other than (1, 1)), and check_gradients checks it (default:
     check_weighted_gradients)."""
     w = ctx.get_weights()
     if weighted is None:
         weighted = ctx.get_class_weights() != (1.0, 1.0)
-    resident, explicit = read_all(ctx, env, None, logistic), read_all(ctx, env, w, logistic)
-    want, c = oracle_all(orc, env, w, logistic)
+    resident, explicit = read_all(ctx, env, None, model), read_all(ctx, env, w, model)
+    want, c = oracle_all(orc, env, w, model)
     scales = {n: _grad_scale(env, env.data, env.ids[n], c) for n in ("grad_stream", "grad_rows")}
     if weighted:       # the weighted gradient has its own checker; read_all's evaluations are unweighted
-        (check_gradients or check_weighted_gradients)(ctx, env, orc, w, c, resident, explicit, logistic, exact_oracle, what)
+        (check_gradients or check_weighted_gradients)(ctx, env, orc, w, c, resident, explicit, model, exact_oracle, what)
         for d in (resident, explicit, want):
             del d["grad_stream"], d["grad_rows"]
     compare(resident, explicit, exact_resident, f"{what}, w == NULL against the explicit weights", scales)
     compare(explicit, want, exact_oracle, f"{what}, explicit weights against the oracle", scales)
 
-    more_res, more_exp = read_more(ctx, env, None, logistic, weighted), read_more(ctx, env, w, logistic, weighted)
+    more_res, more_exp = read_more(ctx, env, None, model, weighted), read_more(ctx, env, w, model, weighted)
     bad = []
     for k, v in more_exp.items():
         r = more_res[k]
@@ -274,24 +274,24 @@ def check_all_readers(ctx, env, orc, logistic, exact_resident, exact_oracle, wha
         if _bits(r) != _bits(v):
             bad.append(k)
     assert not bad, f"{what}, w == NULL against the explicit weights: {bad}"
-    check_more(ctx, env, orc, w, more_exp, logistic, exact_oracle, f"{what}, explicit weights against the checkers")
+    check_more(ctx, env, orc, w, more_exp, model, exact_oracle, f"{what}, explicit weights against the checkers")
     return w, c
 
 
 # ---- the next step from the resident state --------------------------------------------------------------------------------
 
-def step_ref(ctx, orc, w, ids, batch, lrs, logistic, lam1=None, class_w=None):
+def step_ref(ctx, orc, w, ids, batch, lrs, model, lam1=None, class_w=None):
     """The next step of the checker under the context's options (or those given): (w, loss)."""
     lam1 = ctx.info()["lambda1"] if lam1 is None else lam1
     wp, wn = ctx.get_class_weights() if class_w is None else class_w
     if (wp, wn) != (1.0, 1.0):
-        w_ref, l_ref = CW.sync_steps(orc, w, ids, [batch], lrs, wp, wn, logistic=logistic, lambda1=lam1)
+        w_ref, l_ref = CW.sync_steps(orc, w, ids, [batch], lrs, wp, wn, logistic=model == "logistic", lambda1=lam1)
     else:
-        w_ref, l_ref = L1.sync_steps(orc, w, ids, [batch], lrs, lam1, logistic=logistic)
+        w_ref, l_ref = L1.sync_steps(orc, w, ids, [batch], lrs, lam1, logistic=model == "logistic")
     return w_ref, l_ref[0]
 
 
-def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what, ref=None, cmax=None):
+def check_next_step(ctx, env, orc, S, w, c, exact, path, table, model, what, ref=None, cmax=None):
     """One step with the context's options on (path "persistent": batch 64; "per_step": 32 G + 1), from the resident state
     and after set_weights(w) re-derives it: the same weights and loss, and the checker's.  ref: the checker's step, as
     step_ref takes and returns it; cmax: the largest weight of a row (else the larger class weight)."""
@@ -308,7 +308,7 @@ def check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what, 
     loss, w1 = step()
     ctx.set_weights(w)
     loss_twin, w1_twin = step()
-    w_ref, loss_ref = (ref or step_ref)(ctx, orc, w, ids, batch, lrs, logistic)
+    w_ref, loss_ref = (ref or step_ref)(ctx, orc, w, ids, batch, lrs, model)
     what = f"{what}, next step on the {path} path"
     if exact:
         assert loss == loss_twin == loss_ref, f"{what}: loss {loss!r} / re-set {loss_twin!r} / checker {loss_ref!r}"
@@ -395,27 +395,27 @@ def write(ctx, env, S, writer, rng):
     return env.d
 
 
-def state_witness(ctx, env, orc, S, writer, w_after, logistic):
+def state_witness(ctx, env, orc, S, writer, w_after, model):
     """The next per-step loss under the state from before a writer of state only differs from the right one."""
     lam1, lam1b, _ = consts(env)
     ids = _big_step(env, S)
     lrs = np.array([env.lr])
-    _, right = step_ref(ctx, orc, w_after, ids, ids.size, lrs, logistic)
+    _, right = step_ref(ctx, orc, w_after, ids, ids.size, lrs, model)
     if writer == "set_l1_on":                       # a stale scal[kScalL1] = 0
         stale = right - lam1 * math.fsum(np.abs(w_after))
     elif writer == "set_l1_cycle":                  # a stale ||w0||_1
         stale = right - lam1 * (math.fsum(np.abs(w_after)) - math.fsum(np.abs(env.w0)))
     elif writer == "set_l1_change":
-        _, stale = step_ref(ctx, orc, w_after, ids, ids.size, lrs, logistic, lam1=lam1)
+        _, stale = step_ref(ctx, orc, w_after, ids, ids.size, lrs, model, lam1=lam1)
     else:
-        _, stale = step_ref(ctx, orc, w_after, ids, ids.size, lrs, logistic,
+        _, stale = step_ref(ctx, orc, w_after, ids, ids.size, lrs, model,
                             class_w=(1.0, 1.0) if writer == "cw_on" else CLASS_W)
     assert _moved(right, stale), f"{writer}: the next loss under the stale state ({stale!r}) is the right one ({right!r})"
 
 
-def run_case(ctx_of, env, S, options, writer, logistic):
+def run_case(ctx_of, env, S, options, writer, model):
     kind = env.kind
-    what = f"{'logistic' if logistic else 'SVM'} [{options or 'no options'}], {kind}, dim {env.dim}, {writer}"
+    what = f"{'logistic' if model == 'logistic' else 'SVM'} [{options or 'no options'}], {kind}, dim {env.dim}, {writer}"
     exact = kind == "dyadic" and writer != "compute_dim_sparsity"   # compute_dim_sparsity's d = 1 / (df + 1)
     table = "table" in writer
     for i, path in enumerate(("per_step", "persistent")):
@@ -426,23 +426,23 @@ def run_case(ctx_of, env, S, options, writer, logistic):
             _set_options(ctx, env, options)
             d_after = write(ctx, env, S, writer, rng)
             w_after = ctx.get_weights()
-            orc = env.oracle(d_after, logistic=logistic)
+            orc = env.oracle(d_after, model=model)
             if i == 0:
-                orc_before = env.oracle(env.d, logistic=logistic)
+                orc_before = env.oracle(env.d, model=model)
                 if writer in STATE_ONLY:
-                    state_witness(ctx, env, orc, S, writer, w_after, logistic)
+                    state_witness(ctx, env, orc, S, writer, w_after, model)
                 elif writer == "set_l1_cycle":
                     witness(env, "w", env.w0, w_after, env.d, d_after, orc_before=orc_before, orc_after=orc)
-                    state_witness(ctx, env, orc, S, writer, w_after, logistic)
+                    state_witness(ctx, env, orc, S, writer, w_after, model)
                 else:
                     witness(env, "d" if "dim_sparsity" in writer else "w", env.w0, w_after, env.d, d_after,
                             orc_before=orc_before, orc_after=orc)
                     if ctx.info()["lambda1"] > 0 and "dim_sparsity" not in writer:
                         assert _moved(math.fsum(np.abs(env.w0)), math.fsum(np.abs(w_after))), "||w||_1 does not move"
-                w, c = check_all_readers(ctx, env, orc, logistic, kind == "dyadic", exact, what)
+                w, c = check_all_readers(ctx, env, orc, model, kind == "dyadic", exact, what)
             else:
                 w, c = w_after, 2.0 * env.lam * math.fsum(w_after * d_after)
-            check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what)
+            check_next_step(ctx, env, orc, S, w, c, exact, path, table, model, what)
         finally:
             if own:
                 ctx.close()
@@ -465,7 +465,7 @@ def _ctx_of(env, which):
 def test_svm(envs, S, kind, dim, options, writer):
     env = envs(kind, dim)
     try:
-        run_case(_ctx_of(env, "sync"), env, S, options, writer, False)
+        run_case(_ctx_of(env, "sync"), env, S, options, writer, "svm")
     finally:
         _set_options(env.ctx("sync"), env, "")
 
@@ -476,7 +476,7 @@ def test_logistic(envs, S, dim, options, writer):
     """fp32 rows only: the logistic loss of dyadic rows is not dyadic.  The logistic model always takes the per-step path."""
     env = envs("fp32", dim)
     try:
-        run_case(_ctx_of(env, "logistic"), env, S, options, writer, True)
+        run_case(_ctx_of(env, "logistic"), env, S, options, writer, "logistic")
     finally:
         _set_options(env.ctx("logistic"), env, "")
 
@@ -497,7 +497,7 @@ def test_fused_two_ranks_rate_table(envs, S, kind):
         what = f"fused K = 2 with a rate table, {kind}, rank {r}"
         w = ctx.get_weights()
         witness(env, "w", env.w0, w, env.d, env.d, orc_after=orc)
-        check_all_readers(ctx, env, orc, False, kind == "dyadic", kind == "dyadic", what)
+        check_all_readers(ctx, env, orc, "svm", kind == "dyadic", kind == "dyadic", what)
         return w
 
     res = fused_ranks(env.data, env.lam, env.d, [S // 2, S // 2], env.w0, [(per_rank, None)], lrs, after=after)

@@ -126,7 +126,7 @@ WEIGHTED_IDS = {"we_range": lambda env: np.arange(N_STREAM), "we_rows": lambda e
                 "wc_sampled": lambda env: env.sampled[100:1100], "wc_list": lambda env: env.ids["samples"]}
 
 
-def check_weighted_readers(ctx, env, orc, sw, logistic, exact_resident, exact_oracle, what):
+def check_weighted_readers(ctx, env, orc, sw, model, exact_resident, exact_oracle, what):
     """The weighted readers at w == NULL against the explicit weights, and those against oracle/sw and oracle/wcurve."""
     w = ctx.get_weights()
     wp, wn = ctx.get_class_weights()
@@ -148,10 +148,10 @@ def check_weighted_readers(ctx, env, orc, sw, logistic, exact_resident, exact_or
     for k, v in exp.items():
         ids = WEIGHTED_IDS[k](env)
         if k.startswith("we_"):
-            sums, counts = SW.eval_weighted(orc, w, ids, wp, wn, sw, logistic=logistic)
+            sums, counts = SW.eval_weighted(orc, w, ids, wp, wn, sw, logistic=model == "logistic")
             if [v.n, v.correct] != list(counts) or [v.correct_weight, v.weight_sum] != list(sums[1:]):
                 bad.append(f"{k}: {v} against sums {tuple(sums)}, counts {tuple(counts)}")
-            if not (abs(v.loss_sum - sums[0]) <= 1e-13 * abs(sums[0]) if logistic else v.loss_sum == sums[0]):
+            if not (abs(v.loss_sum - sums[0]) <= 1e-13 * abs(sums[0]) if model == "logistic" else v.loss_sum == sums[0]):
                 bad.append(f"{k}: S {v.loss_sum!r} against {sums[0]!r}")
             if not (v.norm_squared == n2 if exact_oracle else abs(v.norm_squared - n2) <= 1e-12 * n2):
                 bad.append(f"{k}: ||w||^2 {v.norm_squared!r} against {n2!r}")
@@ -168,14 +168,14 @@ def check_weighted_readers(ctx, env, orc, sw, logistic, exact_resident, exact_or
     assert not bad, f"{what}, weighted readers against the checkers:\n" + "\n".join(bad)
 
 
-def check_sw_gradients(sw, ctx, env, orc, w, c, got_res, got_exp, logistic, exact, what):
+def check_sw_gradients(sw, ctx, env, orc, w, c, got_res, got_exp, model, exact, what):
     """The gradient requests at w == NULL and at w against oracle/sw.gradient under the context's class weights and sw."""
     wp, wn = ctx.get_class_weights()
     cvec = OW.weights(env.data.label, wp, wn, sw)
     for name in ("grad_stream", "grad_rows"):
         idx = env.ids[name]
         (g_res, l_res), (g, loss) = [(d[name]["grad"], d[name]["loss"]) for d in (got_res, got_exp)]
-        g_ref, loss_ref, _ = SW.gradient(orc, w, idx, sw, wp, wn, logistic=logistic)
+        g_ref, loss_ref, _ = SW.gradient(orc, w, idx, sw, wp, wn, logistic=model == "logistic")
         if exact:
             assert np.array_equal(g_res, g) and l_res == loss, f"{what}: {name} at w == NULL against the explicit weights"
             assert np.array_equal(g, g_ref) and loss == loss_ref, f"{what}: {name} against the checker"
@@ -192,14 +192,14 @@ def check_sw_gradients(sw, ctx, env, orc, w, c, got_res, got_exp, logistic, exac
 
 # ---- the next step ------------------------------------------------------------------------------------------------------------
 
-def step_ref(ctx, orc, w, ids, batch, lrs, logistic, sw=None, exact=False):
+def step_ref(ctx, orc, w, ids, batch, lrs, model, sw=None, exact=False):
     """The next step of the checker under the context's options: oracle/sw with sample weights loaded (sw), else the
     checker test_gpu_resident_options.step_ref picks from the class weights.  exact: its weights must stay on the grid."""
     assert ctx.info()["sample_weights"] is (sw is not None), "the checker's sample weights are not the context's"
     if sw is None:
-        w_ref, loss = step_ref_unweighted(ctx, orc, w, ids, batch, lrs, logistic)
+        w_ref, loss = step_ref_unweighted(ctx, orc, w, ids, batch, lrs, model)
     else:
-        w_ref, losses = SW.sync_steps(orc, w, ids, [batch], lrs, sw, *ctx.get_class_weights(), logistic=logistic,
+        w_ref, losses = SW.sync_steps(orc, w, ids, [batch], lrs, sw, *ctx.get_class_weights(), logistic=model == "logistic",
                                       lambda1=ctx.info()["lambda1"])
         loss = losses[0]
     if exact:
@@ -268,7 +268,7 @@ def _differs(a, b):
     return abs(a - b) > 1e-9 * max(abs(a), abs(b))
 
 
-def state_witness(env, orc, S, writer, w, sw, class_w, lam1, logistic):
+def state_witness(env, orc, S, writer, w, sw, class_w, lam1, model):
     """The next per-step loss and eval_weighted's S under the state from before a writer of state only differ from the
     right ones (for l1_on only the loss: the evaluation has no penalty)."""
     s0 = sample_weights(env, 0)
@@ -277,19 +277,19 @@ def state_witness(env, orc, S, writer, w, sw, class_w, lam1, logistic):
     lam1_old = 0.0 if writer == "l1_on" else lam1
     ids = _big_step(env, S)
     lrs = np.array([env.lr])
-    right = SW.sync_steps(orc, w, ids, [ids.size], lrs, sw, *class_w, logistic=logistic, lambda1=lam1)[1][0]
-    stale = SW.sync_steps(orc, w, ids, [ids.size], lrs, sw_old, *cw_old, logistic=logistic, lambda1=lam1_old)[1][0]
+    right = SW.sync_steps(orc, w, ids, [ids.size], lrs, sw, *class_w, logistic=model == "logistic", lambda1=lam1)[1][0]
+    stale = SW.sync_steps(orc, w, ids, [ids.size], lrs, sw_old, *cw_old, logistic=model == "logistic", lambda1=lam1_old)[1][0]
     assert _differs(right, stale), f"{writer}: the next loss under the stale state ({stale!r}) is the right one ({right!r})"
     if writer != "l1_on":
         rows = np.arange(N_STREAM)
-        right = SW.eval_weighted(orc, w, rows, *class_w, sw, logistic=logistic)[0][0]
-        stale = SW.eval_weighted(orc, w, rows, *cw_old, sw_old, logistic=logistic)[0][0]
+        right = SW.eval_weighted(orc, w, rows, *class_w, sw, logistic=model == "logistic")[0][0]
+        stale = SW.eval_weighted(orc, w, rows, *cw_old, sw_old, logistic=model == "logistic")[0][0]
         assert _differs(right, stale), f"{writer}: eval_weighted's S under the stale state ({stale!r}) is the right one"
 
 
-def run_case(ctx_of, env, S, options, writer, logistic):
+def run_case(ctx_of, env, S, options, writer, model):
     kind = env.kind
-    what = f"{'logistic' if logistic else 'SVM'} [s {options}], {kind}, dim {env.dim}, {writer}"
+    what = f"{'logistic' if model == 'logistic' else 'SVM'} [s {options}], {kind}, dim {env.dim}, {writer}"
     exact = kind == "dyadic"
     table = "table" in writer
     for i, path in enumerate(("per_step", "persistent")):
@@ -303,24 +303,24 @@ def run_case(ctx_of, env, S, options, writer, logistic):
             assert ctx.info()["sample_weights"] is (sw is not None), f"{what}: sample weights loaded"
             class_w = ctx.get_class_weights()
             w_after = ctx.get_weights()
-            orc = env.oracle(env.d, logistic=logistic)
+            orc = env.oracle(env.d, model=model)
             if exact:
                 on_grid(w_after, what)
             if i == 0:
                 if writer in SW_STATE_ONLY:
-                    state_witness(env, orc, S, writer, w_after, sw, class_w, ctx.info()["lambda1"], logistic)
+                    state_witness(env, orc, S, writer, w_after, sw, class_w, ctx.info()["lambda1"], model)
                 else:
                     step_witness(env, orc, w_after)
                     if ctx.info()["lambda1"] > 0:
                         assert _moved(math.fsum(np.abs(env.w0)), math.fsum(np.abs(w_after))), "||w||_1 does not move"
                 weighted = sw is not None or class_w != (1.0, 1.0)
-                w, c = check_all_readers(ctx, env, orc, logistic, exact, exact, what, weighted=weighted,
+                w, c = check_all_readers(ctx, env, orc, model, exact, exact, what, weighted=weighted,
                                          check_gradients=functools.partial(check_sw_gradients, sw))
-                check_weighted_readers(ctx, env, orc, sw, logistic, exact, exact, what)
+                check_weighted_readers(ctx, env, orc, sw, model, exact, exact, what)
             else:
                 w, c = w_after, 2.0 * env.lam * math.fsum(w_after * env.d)
             cmax = max(class_w) * (1.0 if sw is None else float(sw.max()))
-            check_next_step(ctx, env, orc, S, w, c, exact, path, table, logistic, what,
+            check_next_step(ctx, env, orc, S, w, c, exact, path, table, model, what,
                             ref=functools.partial(step_ref, sw=sw, exact=exact), cmax=cmax)
         finally:
             if own:
@@ -349,7 +349,7 @@ def _clear(ctx, env):
 def test_svm(envs, S, kind, dim, options, writer):
     env = envs(kind, dim)
     try:
-        run_case(_own_ctx_of(env, "sync"), env, S, options, writer, False)
+        run_case(_own_ctx_of(env, "sync"), env, S, options, writer, "svm")
     finally:
         _clear(env.ctx("sync"), env)
 
@@ -360,18 +360,18 @@ def test_logistic(envs, S, dim, options, writer):
     """fp32 rows only: the logistic loss of dyadic rows is not dyadic.  The logistic model always takes the per-step path."""
     env = envs("fp32", dim)
     try:
-        run_case(_own_ctx_of(env, "logistic"), env, S, options, writer, True)
+        run_case(_own_ctx_of(env, "logistic"), env, S, options, writer, "logistic")
     finally:
         _clear(env.ctx("logistic"), env)
 
 
 # ---- the weighted readers after the writers without sample weights -----------------------------------------------------------
 
-def run_unweighted_case(ctx_of, env, S, options, writer, logistic):
+def run_unweighted_case(ctx_of, env, S, options, writer, model):
     """A writer of test_gpu_resident_options.py, then the weighted readers (c_i = w_y).  The witness: a writer that moves the
     weights moves the predictions, c and ||w||^2; a class-weight writer moves eval_weighted's S.  The L1 and dimSparsity
     writers that keep the weights change nothing the weighted readers read, which must still give the bits of the weights."""
-    what = f"{'logistic' if logistic else 'SVM'} [{options or 'no options'}], {env.kind}, dim {env.dim}, {writer}"
+    what = f"{'logistic' if model == 'logistic' else 'SVM'} [{options or 'no options'}], {env.kind}, dim {env.dim}, {writer}"
     rng = np.random.default_rng([zlib.crc32(f"{options}/{writer}".encode()), env.dim])
     ctx, own = ctx_of(writer)
     try:
@@ -381,17 +381,17 @@ def run_unweighted_case(ctx_of, env, S, options, writer, logistic):
         write(ctx, env, S, writer, rng)
         assert ctx.info()["sample_weights"] is False
         w_after = ctx.get_weights()
-        orc = env.oracle(env.d, logistic=logistic)
+        orc = env.oracle(env.d, model=model)
         if writer in ("cw_on", "cw_off"):
             old = (1.0, 1.0) if writer == "cw_on" else CLASS_W
             rows = np.arange(N_STREAM)
-            right = SW.eval_weighted(orc, w_after, rows, *ctx.get_class_weights(), logistic=logistic)[0][0]
-            stale = SW.eval_weighted(orc, w_after, rows, *old, logistic=logistic)[0][0]
+            right = SW.eval_weighted(orc, w_after, rows, *ctx.get_class_weights(), logistic=model == "logistic")[0][0]
+            stale = SW.eval_weighted(orc, w_after, rows, *old, logistic=model == "logistic")[0][0]
             assert _moved(right, stale), f"{what}: S under the old class weights is the right one"
         elif not np.array_equal(w_after, env.w0):
             witness(env, "w", env.w0, w_after, env.d, env.d, orc_before=orc, orc_after=orc)
         exact = env.kind == "dyadic"
-        check_weighted_readers(ctx, env, orc, None, logistic, exact, exact, what)
+        check_weighted_readers(ctx, env, orc, None, model, exact, exact, what)
     finally:
         if own:
             ctx.close()
@@ -403,7 +403,7 @@ def run_unweighted_case(ctx_of, env, S, options, writer, logistic):
 def test_weighted_readers_after_svm_writers(envs, S, kind, dim, options, writer):
     env = envs(kind, dim)
     try:
-        run_unweighted_case(_ctx_of(env, "sync"), env, S, options, writer, False)
+        run_unweighted_case(_ctx_of(env, "sync"), env, S, options, writer, "svm")
     finally:
         _clear(env.ctx("sync"), env)
 
@@ -413,7 +413,7 @@ def test_weighted_readers_after_svm_writers(envs, S, kind, dim, options, writer)
 def test_weighted_readers_after_logistic_writers(envs, S, dim, options, writer):
     env = envs("fp32", dim)
     try:
-        run_unweighted_case(_ctx_of(env, "logistic"), env, S, options, writer, True)
+        run_unweighted_case(_ctx_of(env, "logistic"), env, S, options, writer, "logistic")
     finally:
         _clear(env.ctx("logistic"), env)
 

@@ -108,19 +108,24 @@ class Env:
         }
         self._ctx = {}
 
-    def oracle(self, d, logistic=False, data=None):
+    def oracle(self, d, model="svm", data=None, **weighting):
+        """The checker of `model` ("svm", "logistic", "squared_hinge", "modified_huber") with dimSparsity d; a margin
+        model's takes the weighting of its steps (oracle.margin.MarginOracle)."""
         from oracle.logistic import LogisticOracle
+        from oracle.margin import MarginOracle
         from oracle.oracle import Oracle
         data = self.data if data is None else data
-        orc = (LogisticOracle if logistic else Oracle)(data.row_ptr, data.col, data.val, data.label, self.dim, self.lam)
+        orc = (LogisticOracle if model == "logistic" else Oracle)(data.row_ptr, data.col, data.val, data.label, self.dim,
+                                                                 self.lam)
         orc.set_dim_sparsity(d)
-        return orc
+        return orc if model in ("svm", "logistic") else MarginOracle(orc, model, **weighting)
 
     def ctx(self, which):
-        """'sync', 'logistic' or 'async': one context per kind, reset by the caller."""
+        """'sync' (the SVM), 'async' or another model's name: one context per kind, reset by the caller."""
         if which not in self._ctx:
             from distributed_sgd_b200.native import NativeCtx
-            c = NativeCtx(0, self.dim, self.lam, is_async=which == "async", logistic=which == "logistic")
+            c = NativeCtx(0, self.dim, self.lam, is_async=which == "async",
+                          model=None if which in ("sync", "async") else which)
             c.load_csr(self.data.row_ptr, self.data.col, self.data.val, self.data.label)
             self._ctx[which] = c
         return self._ctx[which]
@@ -190,13 +195,14 @@ def witness(env, what, w_before, w_after, d_before, d_after, orc_before=None, or
 
 # ---- readers -------------------------------------------------------------------------------------------------------------
 
-def read_all(ctx, env, w, logistic):
-    """Every reader once, at the weights w (None: resident).  {reader: {field: value}}."""
+def read_all(ctx, env, w, model):
+    """Every reader once, at the weights w (None: resident).  {reader: {field: value}}.  Every model but the SVM reads the
+    *_sums forms (its loss sum is not an integer)."""
     ids = env.ids
     out = {}
     out["eval_stream"] = dict(zip(("loss", "acc"), ctx.eval(0, N_STREAM, w)))
     out["eval_rows"] = dict(zip(("loss", "acc"), ctx.eval(N_STREAM, N_STREAM + N_SMALL, w)))
-    if logistic:
+    if model != "svm":
         fields = ("loss_sum", "correct", "n2")
         out["sums"] = dict(zip(fields, ctx.eval_sums(0, N_STREAM, w)))
         out["sampled_stream"] = dict(zip(fields, ctx.eval_sampled_sums(0, N_ROWS, KEY, 0, 2500, w)))
@@ -216,8 +222,8 @@ def read_all(ctx, env, w, logistic):
     return out
 
 
-def oracle_all(orc, env, w, logistic):
-    """What read_all must give at the weights w, and c."""
+def oracle_all(orc, env, w, model):
+    """What read_all must give at the weights w, and c.  A margin model's gradient loss is that of its weighting."""
     ids = env.ids
     n2 = math.fsum(w * w)
     out = {}
@@ -225,7 +231,7 @@ def oracle_all(orc, env, w, logistic):
     def sums(idx=None, begin=0, n=None):
         loss, acc = orc.loss_acc(w, idx=idx, begin=begin, n=n)
         k = len(idx) if idx is not None else n
-        if logistic:
+        if model != "svm":
             return {"loss_sum": math.fsum(orc.sample_losses(w, idx=idx, begin=begin, n=n)), "correct": round(acc * k),
                     "n2": n2}
         return {"hinge": round((loss - env.lam * n2) * k), "correct": round(acc * k), "n2": n2}
@@ -241,7 +247,8 @@ def oracle_all(orc, env, w, logistic):
     c = None
     for name in ("grad_stream", "grad_rows"):
         g, c = orc.gradient(w, ids[name])
-        out[name] = {"grad": g, "loss": orc.loss_acc(w, idx=ids[name])[0]}
+        loss = orc.gradient_loss(w, ids[name]) if model not in ("svm", "logistic") else orc.loss_acc(w, idx=ids[name])[0]
+        out[name] = {"grad": g, "loss": loss}
     return out, c
 
 
@@ -281,12 +288,12 @@ def compare(got, want, exact, what, scales):
     assert not bad, "\n".join(bad)
 
 
-def check_readers(ctx, env, orc, logistic, exact_resident, exact_oracle, what, data=None):
+def check_readers(ctx, env, orc, model, exact_resident, exact_oracle, what, data=None):
     """Every reader at w == NULL against the explicit weights, and those against the oracle; returns the weights."""
     w = ctx.get_weights()
-    resident = read_all(ctx, env, None, logistic)
-    explicit = read_all(ctx, env, w, logistic)
-    want, c = oracle_all(orc, env, w, logistic)
+    resident = read_all(ctx, env, None, model)
+    explicit = read_all(ctx, env, w, model)
+    want, c = oracle_all(orc, env, w, model)
     data = env.data if data is None else data
     scales = {n: _grad_scale(env, data, env.ids[n], c) for n in ("grad_stream", "grad_rows")}
     compare(resident, explicit, exact_resident, f"{what}, w == NULL against the explicit weights", scales)
@@ -388,7 +395,7 @@ def test_sync_svm(envs, S, kind, dim, writer):
             witness(env, "d" if "dim_sparsity" in writer else "w", w_before, w_after, env.d, d_after, orc_after=orc)
         # dyadic rows give exact sums, except with compute_dim_sparsity's d = 1 / (df + 1)
         exact_oracle = kind == "dyadic" and writer != "compute_dim_sparsity"
-        w, c = check_readers(ctx, env, orc, False, kind == "dyadic", exact_oracle, what, data=data)
+        w, c = check_readers(ctx, env, orc, "svm", kind == "dyadic", exact_oracle, what, data=data)
         check_next_step(ctx, env, orc, w, c, exact_oracle, what, data=data)
     finally:
         if own is not None:
@@ -420,10 +427,10 @@ def test_logistic(envs, dim, writer):
     elif writer == "set_dim_sparsity":
         ctx.set_dim_sparsity(env.d2)
         d_after = env.d2
-    orc = env.oracle(d_after, logistic=True)
+    orc = env.oracle(d_after, model="logistic")
     witness(env, "d" if writer == "set_dim_sparsity" else "w", env.w0, ctx.get_weights(), env.d, d_after,
-            orc_before=env.oracle(env.d, logistic=True), orc_after=orc)
-    w, c = check_readers(ctx, env, orc, True, False, False, what)
+            orc_before=env.oracle(env.d, model="logistic"), orc_after=orc)
+    w, c = check_readers(ctx, env, orc, "logistic", False, False, what)
     check_next_step(ctx, env, orc, w, c, False, what)
 
 
@@ -490,7 +497,7 @@ def test_async(envs, kind, dim, writer):
         w_after = ctx.get_weights()
         orc = env.oracle(env.d)
         witness(env, "w", w_before, w_after, env.d, env.d, orc_after=orc)
-        check_readers(ctx, env, orc, False, True, kind == "dyadic", what)
+        check_readers(ctx, env, orc, "svm", True, kind == "dyadic", what)
     finally:
         if writer == "loop_ended":
             env.ctx("async").stop_async()
@@ -514,7 +521,7 @@ def test_fused_two_ranks_averaging(envs, S, kind):
         what = f"fused K = 2, {kind}, rank {r}"
         w = ctx.get_weights()
         witness(env, "w", env.w0, w, env.d, env.d, orc_after=orc)
-        check_readers(ctx, env, orc, False, kind == "dyadic", kind == "dyadic", what)
+        check_readers(ctx, env, orc, "svm", kind == "dyadic", kind == "dyadic", what)
         assert ctx.average_weights()[1] == 2
         return w
 
