@@ -14,7 +14,7 @@ from typing import Callable, List, Optional, Sequence, Union
 import numpy as np
 
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
-from ..ml.calibration import Calibration
+from ..ml.calibration import METHODS as CALIBRATION_METHODS, Calibration, IsotonicCalibration
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
 from ..ml.sparse_logistic import SparseLogistic
@@ -69,6 +69,29 @@ def _calibration(result) -> Calibration:
     """A NativeCtx.calibrate* result as a Calibration."""
     a, b, objective, info = result
     return Calibration(a, b, objective, int(info[0]), int(info[1]), int(info[2]), int(info[3]))
+
+
+def _isotonic(result) -> IsotonicCalibration:
+    """A NativeCtx.calibrate_isotonic* result as an IsotonicCalibration."""
+    x, y, block_rows, block_pos, info = result
+    return IsotonicCalibration(x, y, block_rows, block_pos, int(info[0]), int(info[2]), int(info[3]), int(info[4]))
+
+
+def _method(method: str) -> str:
+    if method not in CALIBRATION_METHODS:
+        raise ValueError(f"calibration method: expected one of {', '.join(CALIBRATION_METHODS)}, got {method!r}")
+    return method
+
+
+def isotonic_calibration_dict(result) -> dict:
+    """calibration_dict of a NativeCtx.eval_*isotonic_calibration result, plus infinite_log_loss_rows: the rows whose term
+    -log p (o = 1) or -log(1 - p) (o = 0) is infinite; any such row makes log_loss +inf."""
+    sums, bin_rows, bin_pos, bin_psum, words = result
+    out = calibration_dict((sums, bin_rows, bin_pos, bin_psum, words[:2]))
+    out["infinite_log_loss_rows"] = int(words[2])
+    if words[2]:
+        out["log_loss"] = float("inf")
+    return out
 
 
 def calibration_dict(result) -> dict:
@@ -474,26 +497,38 @@ class Master:
     # the whole range or sample itself.  Every sum over the rows is an order-free fixed-point sum and the arithmetic between
     # the sums is one fixed sequence, so every rank gets the same bits without a collective.  None of them touches the
     # weights or the step state: they can be called from `fit`'s on_epoch hook.
-    def calibrate(self, weights=None, test_data: bool = False) -> Calibration:
-        """Platt scaling of the margins over the train (or test) rows: the Calibration (a, b) that makes
-        1 / (1 + exp(a x.w + b)) a probability.  weights None: the resident weights, as in local_metrics."""
+    def calibrate(self, weights=None, test_data: bool = False, method: str = "sigmoid"):
+        """A calibration of the margins over the train (or test) rows.  method "sigmoid": Platt scaling, the Calibration
+        (a, b) that makes 1 / (1 + exp(a x.w + b)) a probability; "isotonic": isotonic regression, an IsotonicCalibration.
+        weights None: the resident weights, as in local_metrics."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        if _method(method) == "isotonic":
+            return _isotonic(self.ctx.calibrate_isotonic(b, e, weights))
         return _calibration(self.ctx.calibrate(b, e, weights))
 
-    def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False) -> Calibration:
+    def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False, method: str = "sigmoid"):
         """calibrate on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
         sample raises DsgdEmpty."""
+        iso = _method(method) == "isotonic"
         b, e, k, key, ids = self._draw_sample(samples_count, test_data)
         if k <= 0:
             raise DsgdEmpty(ERR_EMPTY, f"sampled calibration of {samples_count} rows: the sample is empty")
         if ids is None:
+            if iso:
+                return _isotonic(self.ctx.calibrate_isotonic_sampled(b, e, key, 0, k, weights))
             return _calibration(self.ctx.calibrate_sampled(b, e, key, 0, k, weights))
+        if iso:
+            return _isotonic(self.ctx.calibrate_isotonic_samples(ids, weights))
         return _calibration(self.ctx.calibrate_samples(ids, weights))
 
-    def local_calibration(self, calibration: Calibration, weights=None, test_data: bool = False, n_bins: int = 10) -> dict:
-        """How well `calibration` fits the train (or test) rows: Brier score, log loss, expected and maximum calibration
-        error and the reliability bins (calibration_dict).  Every rank evaluates the whole range itself."""
+    def local_calibration(self, calibration, weights=None, test_data: bool = False, n_bins: int = 10) -> dict:
+        """How well `calibration` (a Calibration or an IsotonicCalibration) fits the train (or test) rows: Brier score, log
+        loss, expected and maximum calibration error and the reliability bins (calibration_dict; isotonic_calibration_dict
+        for an isotonic map).  Every rank evaluates the whole range itself."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        if isinstance(calibration, IsotonicCalibration):
+            return isotonic_calibration_dict(self.ctx.eval_isotonic_calibration(b, e, calibration.x, calibration.y, n_bins,
+                                                                                weights))
         return calibration_dict(self.ctx.eval_calibration(b, e, calibration.a, calibration.b, n_bins, weights))
 
     def local_sampled_calibration(self, calibration: Calibration, weights, samples_count: int, test_data: bool = False,
@@ -502,6 +537,12 @@ class Master:
         b, e, k, key, ids = self._draw_sample(samples_count, test_data)
         if k <= 0:
             raise DsgdEmpty(ERR_EMPTY, f"sampled calibration quality of {samples_count} rows: the sample is empty")
+        if isinstance(calibration, IsotonicCalibration):
+            x, y = calibration.x, calibration.y
+            if ids is None:
+                return isotonic_calibration_dict(self.ctx.eval_sampled_isotonic_calibration(b, e, key, 0, k, x, y, n_bins,
+                                                                                            weights))
+            return isotonic_calibration_dict(self.ctx.eval_samples_isotonic_calibration(ids, x, y, n_bins, weights))
         a, bb = calibration.a, calibration.b
         if ids is None:
             return calibration_dict(self.ctx.eval_sampled_calibration(b, e, key, 0, k, a, bb, n_bins, weights))

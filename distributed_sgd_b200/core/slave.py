@@ -11,6 +11,7 @@ from typing import Optional, Sequence, Union
 
 import numpy as np
 
+from ..ml.calibration import IsotonicCalibration
 from ..ml.class_weight import resolve_class_weight
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge, model_name
@@ -109,9 +110,11 @@ class Slave:
 
     def calibrated_probabilities(self, samples_idx: Sequence[int], calibration,
                                  weights: Optional[np.ndarray] = None) -> np.ndarray:
-        """Extension, either model: P(y = +1 | x) = 1 / (1 + exp(a x.w + b)) of the listed rows under `calibration` (a
-        Calibration, e.g. from Master.calibrate)."""
+        """Extension, any model: P(y = +1 | x) of the listed rows under `calibration` (from Master.calibrate): a Calibration
+        gives 1 / (1 + exp(a x.w + b)), an IsotonicCalibration numpy.interp(-x.w, x, y)."""
         self._train_ids(samples_idx)
+        if isinstance(calibration, IsotonicCalibration):
+            return self.ctx.isotonic_probabilities(samples_idx, calibration.x, calibration.y, weights)
         return self.ctx.calibrated_probabilities(samples_idx, calibration.a, calibration.b, weights)
 
     def gradient(self, weights: Optional[np.ndarray], samples_idx: Sequence[int]) -> np.ndarray:

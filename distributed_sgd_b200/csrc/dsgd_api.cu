@@ -25,6 +25,7 @@
 #include "dsgd_async.cuh"
 #include "dsgd_metrics.cuh"
 #include "dsgd_calibrate.cuh"
+#include "dsgd_isotonic.cuh"
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
@@ -171,6 +172,13 @@ struct dsgd_ctx {
   dev_buf<int8_t> k_lab;
   dev_buf<unsigned long long> k_ctl, k_eval;
   int k_fit_occ = 0;   // CTAs of k_calib_fit per SM at its full shared-memory budget (0: not asked yet)
+  // an isotonic fit (dsgd_calibrate_isotonic*, dsgd_isotonic.cuh): the hull's two ping-pong vertex buffers, their two
+  // count buffers and the scan of the blocks' X counts; X and Y; the block rows and positives; the X count.  A map applied
+  // to rows (dsgd_isotonic_probabilities, dsgd_eval_isotonic_calibration*): its X and Y
+  dev_buf<int> i_hull;
+  dev_buf<double> i_out, i_map;
+  dev_buf<long long> i_blk;
+  dev_buf<unsigned long long> i_ctl;
 
   ncclComm_t comm = nullptr;
 
@@ -820,6 +828,13 @@ static cudaError_t scan_tie_ends(dsgd_ctx *ctx, void *tmp, size_t &bytes, int64_
   return cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, ctx->c_excl.p, (int)n_all, ctx->stream);
 }
 
+// The isotonic fit's exclusive scan of the X counts of the B blocks of the hull h into excl (tmp == nullptr: the storage it
+// needs, into bytes).
+static cudaError_t scan_x_counts(dsgd_ctx *ctx, void *tmp, size_t &bytes, const int *h, int B, int *excl) {
+  auto counts = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), iso_x_count{h, B});
+  return cub::DeviceScan::ExclusiveSum(tmp, bytes, counts, excl, B, ctx->stream);
+}
+
 static int reserve_requests(dsgd_ctx *ctx) {
   const int64_t n = ctx->n_rows;
   int rc;
@@ -827,14 +842,17 @@ static int reserve_requests(dsgd_ctx *ctx) {
       (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->m_cnt.grow(ctx, kMetWords, kMetWords)) ||
       (rc = ctx->c_cnt.grow(ctx, kCurWords, kCurWords)) || (rc = ctx->c_merged.grow(ctx, n, 1024)) ||
       (rc = ctx->c_excl.grow(ctx, n, 1024)) || (rc = ctx->c_thr.grow(ctx, n, 1024)) || (rc = ctx->c_tp.grow(ctx, n, 1024)) ||
-      (rc = ctx->c_fp.grow(ctx, n, 1024)) || (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)))
+      (rc = ctx->c_fp.grow(ctx, n, 1024)) || (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)) ||
+      (rc = ctx->i_hull.grow(ctx, 5 * (n + 1), 1024)) || (rc = ctx->i_out.grow(ctx, 2 * n, 1024)) ||
+      (rc = ctx->i_blk.grow(ctx, 2 * n, 1024)) || (rc = ctx->i_ctl.grow(ctx, 1, 1)))
     return rc;
-  size_t tmp = 0, tmp_merge = 0, tmp_scan = 0;
+  size_t tmp = 0, tmp_merge = 0, tmp_scan = 0, tmp_iso = 0;
   cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
   CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, kb, (int)n, 0, 64, ctx->stream));
   CU(merge_runs(ctx, nullptr, tmp_merge, ctx->m_keys.p, n - n / 2, ctx->m_alt.p, n / 2));   // sized by the total
   CU(scan_tie_ends(ctx, nullptr, tmp_scan, n));
-  return ctx->m_tmp.grow(ctx, (int64_t)std::max({tmp, tmp_merge, tmp_scan}), 1 << 16);
+  CU(scan_x_counts(ctx, nullptr, tmp_iso, ctx->i_hull.p, (int)n, ctx->i_hull.p));
+  return ctx->m_tmp.grow(ctx, (int64_t)std::max({tmp, tmp_merge, tmp_scan, tmp_iso}), 1 << 16);
 }
 
 static int fits_while_running(dsgd_ctx *ctx, bool fits, const char *fn) {
@@ -1268,18 +1286,19 @@ static cudaError_t scan_weights(dsgd_ctx *ctx, void *tmp, size_t &bytes, const d
 
 // One curve pass over `rows` (DESIGN.md §4.9): score_and_sort with every run sorted, then k_curve_count (U2, the limbs of
 // S = sum of v_i, the number of points m) and k_curve_sum.  With thr != nullptr also the points: the runs merged, the
-// exclusive scan of the merged keys' tie ends, k_curve_emit, and the m points copied back at once.  AP = S / P, NaN when a
+// exclusive scan of the merged keys' tie ends, k_curve_emit, and the m points copied back at once; `device_points` (an
+// isotonic fit): the points are emitted into c_thr / c_tp / c_fp and stay there.  AP = S / P, NaN when a
 // score is NaN or there is no positive row.
 // kSampleWeighted (§4.14): the same steps in their weighted forms, each run's prefix sums of R(c) scanned into c_pre before
 // k_curve_count (positives at c_pre[0, n_pos), negatives after them); out receives the DSGD_WCURVE_WORDS words instead of
 // AP, and tp / fp the point weights as doubles (k_curve_emit writes their bits into c_tp / c_fp).
 template <int kWeight>
 static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *words, double *out, int64_t *n_points,
-                      double *thr, void *tp, void *fp, const char *fn) {
+                      double *thr, void *tp, void *fp, const char *fn, bool device_points = false) {
   constexpr bool kW = kWeight == kSampleWeighted;
   constexpr int kWords = kW ? kCurWWords : kCurWords;
   const int64_t n = rows.n;
-  const bool curve = thr != nullptr;
+  const bool curve = thr != nullptr || device_points;
   int rc = fits_while_running(ctx, ctx->c_cnt && (!curve || (ctx->c_merged.cap >= n && ctx->c_excl.cap >= n &&
                                                               ctx->c_thr.cap >= n && ctx->c_tp.cap >= n && ctx->c_fp.cap >= n)),
                               fn);
@@ -1339,7 +1358,7 @@ static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64
   CU(cudaMemcpyAsync(&s.h[kMetU2], ctx->m_cnt + kMetU2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   const int64_t m = (int64_t)c[kCurPoints];
-  if (curve && m > 0) {   // a weighted pass's c_tp / c_fp hold the bits of doubles: copied as bytes
+  if (thr && m > 0) {   // a weighted pass's c_tp / c_fp hold the bits of doubles: copied as bytes
     CU(cudaMemcpyAsync(thr, ctx->c_thr, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaMemcpyAsync(tp, ctx->c_tp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaMemcpyAsync(fp, ctx->c_fp, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1668,6 +1687,254 @@ extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, con
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+// ---- isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.16) ------------------------------------------------------
+
+// Points of a hull tile: DSGD_ISOTONIC_TILE (1 .. kIsoTileMax) if set, else kIsoTileMax.  The fit has the same bits at every
+// tile size; the variable lets a test see that.
+static int isotonic_tile() {
+  const char *v = getenv("DSGD_ISOTONIC_TILE");
+  const long t = v ? strtol(v, nullptr, 10) : 0;
+  return t >= 1 && t <= kIsoTileMax ? (int)t : kIsoTileMax;
+}
+
+// CTAs of a hull or emit launch of `items` work items: the grid limit if one is set (dsgd_set_grid_limit), else 8 per SM
+static int isotonic_grid(const dsgd_ctx *ctx, int64_t items) {
+  const int64_t cap = ctx->grid_limit > 0 ? ctx->grid_limit : (int64_t)ctx->sm_count * 8;
+  return (int)std::max<int64_t>(1, std::min<int64_t>(items, cap));
+}
+
+// One isotonic fit over `rows`: the curve pass with its points left on the device, the hull (k_iso_tile, then k_iso_merge
+// rounds until one hull is left), the hull's vertex count read back, the scan of the blocks' X counts, k_iso_emit, and the
+// outputs copied back.
+static int isotonic_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *n_points_out, double *x_out,
+                         double *y_out, int64_t *rows_out, int64_t *pos_out, int64_t *info_out, const char *fn) {
+  const int64_t n = rows.n;
+  int rc = fits_while_running(ctx, ctx->i_hull.cap >= 5 * (n + 1) && ctx->i_out.cap >= 2 * n && ctx->i_blk.cap >= 2 * n &&
+                                       ctx->i_ctl,
+                              fn);
+  int64_t words[DSGD_METRICS_WORDS], m = 0;
+  double ap = 0.0;
+  if (rc || (rc = curve_pass<kUnweighted>(ctx, w, rows, words, &ap, &m, nullptr, nullptr, nullptr, fn, true))) return rc;
+  const int64_t nan = words[kMetNan];
+  NEED(m > 0, DSGD_ERR_EMPTY, "%s: all %lld rows have a NaN score", fn, (long long)n);
+  if ((rc = ctx->i_hull.grow(ctx, 5 * (n + 1), 1024)) || (rc = ctx->i_out.grow(ctx, 2 * n, 1024)) ||
+      (rc = ctx->i_blk.grow(ctx, 2 * n, 1024)) || (rc = ctx->i_ctl.grow(ctx, 1, 1)))
+    return rc;
+  const int M = (int)m + 1, S = isotonic_tile(), T = (M + S - 1) / S;
+  int *hv[2] = {ctx->i_hull.p, ctx->i_hull.p + M};
+  int *hc[2] = {ctx->i_hull.p + 2 * (int64_t)M, ctx->i_hull.p + 2 * (int64_t)M + T};
+  int *excl = ctx->i_hull.p + 2 * (int64_t)M + 2 * (int64_t)T;
+  k_iso_tile<<<isotonic_grid(ctx, T), kIsoThreads, (size_t)S * 20, ctx->stream>>>(ctx->c_tp, ctx->c_fp, M, S, hv[0], hc[0]);
+  LAUNCHED();
+  int cur = 0;
+  for (int64_t W = S, h = T; h > 1; W *= 2, h = (h + 1) / 2, cur ^= 1) {
+    k_iso_merge<<<isotonic_grid(ctx, (h + 1) / 2), kIsoThreads, 0, ctx->stream>>>(ctx->c_tp, ctx->c_fp, (int)h, (int)W,
+                                                                                  hv[cur], hc[cur], hv[cur ^ 1], hc[cur ^ 1]);
+    LAUNCHED();
+  }
+  CU(cudaGetLastError());
+  int V = 0;
+  CU(cudaMemcpyAsync(&V, hc[cur], sizeof V, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int B = V - 1;   // the origin and the last point are always vertices: B >= 1
+  NEED(B >= 1 && B <= m, DSGD_ERR_CUDA, "%s: a hull of %d vertices over %lld points", fn, V, (long long)m);
+  size_t tmp = 0;
+  CU(scan_x_counts(ctx, nullptr, tmp, hv[cur], B, excl));
+  if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
+    return rc;
+  CU(scan_x_counts(ctx, ctx->m_tmp.p, tmp, hv[cur], B, excl));
+  double *X = ctx->i_out.p, *Y = ctx->i_out.p + n;
+  long long *br = ctx->i_blk.p, *bp = ctx->i_blk.p + n;
+  k_iso_emit<<<isotonic_grid(ctx, cdiv(B, 256)), 256, 0, ctx->stream>>>(hv[cur], B, excl, ctx->c_thr, ctx->c_tp, ctx->c_fp, X,
+                                                                         Y, br, bp, ctx->i_ctl);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long nx = 0;
+  CU(cudaMemcpyAsync(&nx, ctx->i_ctl, sizeof nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(rows_out, br, sizeof(long long) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(pos_out, bp, sizeof(long long) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  CU(cudaMemcpyAsync(x_out, X, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(y_out, Y, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  *n_points_out = (int64_t)nx;
+  info_out[0] = B;
+  info_out[1] = (int64_t)nx;
+  info_out[2] = n - nan;
+  info_out[3] = nan;
+  info_out[4] = m;
+  return DSGD_OK;
+}
+
+#define ISO_ARGS_OK()                                                                                                 \
+  NEED(n_points_out && x_out && y_out && rows_out && pos_out && info_out, DSGD_ERR_INVALID, "%s: an output is NULL", \
+       __func__)
+
+extern "C" int dsgd_calibrate_isotonic(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                       int64_t *n_points_out, double *x_out, double *y_out, int64_t *rows_out,
+                                       int64_t *pos_out, int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_isotonic_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                               uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *n_points_out,
+                                               double *x_out, double *y_out, int64_t *rows_out, int64_t *pos_out,
+                                               int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_isotonic_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                               int64_t *n_points_out, double *x_out, double *y_out, int64_t *rows_out,
+                                               int64_t *pos_out, int64_t *info_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+}
+
+// A map (X, Y) of k points: X finite and strictly increasing, Y in [0, 1]; copied into i_map (X, then Y)
+static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn) {
+  NEED(X && Y && k >= 1 && k <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: the map needs X and Y of 1 to 2^31 - 1 points", fn);
+  for (int64_t i = 0; i < k; ++i) {
+    NEED(std::isfinite(X[i]) && (i == 0 || X[i] > X[i - 1]), DSGD_ERR_INVALID,
+         "%s: X[%lld] = %g: X must be finite and strictly increasing", fn, (long long)i, X[i]);
+    NEED(Y[i] >= 0.0 && Y[i] <= 1.0, DSGD_ERR_INVALID, "%s: Y[%lld] = %g is not in [0, 1]", fn, (long long)i, Y[i]);
+  }
+  int rc = fits_while_running(ctx, ctx->i_map.cap >= 2 * k, fn);
+  if (rc || (rc = ctx->i_map.grow(ctx, 2 * k, 1024))) return rc;
+  CU(cudaMemcpyAsync(ctx->i_map.p, X, sizeof(double) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->i_map.p + k, Y, sizeof(double) * (size_t)k, cudaMemcpyHostToDevice, ctx->stream));
+  return DSGD_OK;
+}
+
+// Launches kernel<true> with the map in shared memory when it fits, else kernel<false>
+template <class K>
+static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args) {
+  if (k <= kIsoSmemPoints) {
+    const size_t bytes = (size_t)k * 16;
+    cudaError_t e = cudaFuncSetAttribute((const void *)k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+    return cudaLaunchKernel((const void *)k_smem, dim3(grid), dim3(256), args, bytes, stream);
+  }
+  return cudaLaunchKernel((const void *)k_l2, dim3(grid), dim3(256), args, 0, stream);
+}
+
+extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, const double *X,
+                                           const double *Y, int64_t k, double *probs_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(probs_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
+  row_set rows;
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = rows_list(ctx, samples, n, true, __func__, &rows);
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = isotonic_map(ctx, X, Y, k, __func__))) return rc;
+  const double *mx = ctx->i_map.p, *my = ctx->i_map.p + k;
+  int ki = (int)k;
+  double *out = ctx->preds.p;
+  const uint32_t *rp16 = ctx->rp16.p;
+  const uint2 *pairs = ctx->pairs.p;
+  const int32_t *ids = rows.ids;
+  int64_t rn = rows.n;
+  void *args[] = {&rp16, &pairs, &ids, &rn, &wd, &mx, &my, &ki, &out};
+  CU(isotonic_launch(k_iso_prob<true>, k_iso_prob<false>, rows_grid(ctx, rows.n), k, ctx->stream, args));
+  LAUNCHED();
+  CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+// One quality pass over `rows` at the map (X, Y): k_iso_eval, k_calib_eval_finish, the block read back.
+static int isotonic_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, const double *X, const double *Y,
+                                 int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
+                                 double *bin_psum, int64_t *words_out, const char *fn) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = fits_while_running(ctx, ctx->k_eval, fn);
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = isotonic_map(ctx, X, Y, k, fn)) ||
+      (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)))
+    return rc;
+  CU(cudaMemsetAsync(ctx->k_eval, 0, sizeof(unsigned long long) * kCevWords, ctx->stream));
+  const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);
+  const double *mx = ctx->i_map.p, *my = ctx->i_map.p + k;
+  int ki = (int)k, nb = n_bins;
+  unsigned long long *blk = ctx->k_eval.p;
+  const uint32_t *rp16 = ctx->rp16.p;
+  const uint2 *pairs = ctx->pairs.p;
+  const int8_t *label = ctx->label.p;
+  const int32_t *ids = rows.ids;
+  int64_t rb = rows.row_begin, rn = rows.n;
+  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &mx, &my, &ki, &nb, &blk};
+  CU(isotonic_launch(k_iso_eval<true>, k_iso_eval<false>, grid, k, ctx->stream, args));
+  LAUNCHED();
+  k_calib_eval_finish<<<1, kCalMaxBins, 0, ctx->stream>>>(ctx->k_eval, n_bins);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long h[kCevWords];
+  CU(cudaMemcpyAsync(h, ctx->k_eval, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  memcpy(sums_out, &h[kCevOutSums], 2 * sizeof(double));
+  for (int i = 0; i < n_bins; ++i) {
+    bin_rows[i] = (int64_t)h[kCevBinRows + i];
+    bin_pos[i] = (int64_t)h[kCevBinPos + i];
+  }
+  memcpy(bin_psum, &h[kCevOutPsum], (size_t)n_bins * sizeof(double));
+  words_out[0] = (int64_t)h[kCevRows];
+  words_out[1] = (int64_t)h[kCevNan];
+  words_out[2] = (int64_t)h[kCevInf];
+  return DSGD_OK;
+}
+
+#define ISO_EVAL_ARGS_OK()                                                                                              \
+  do {                                                                                                                  \
+    NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);  \
+    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
+  } while (0)
+
+extern "C" int dsgd_eval_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                              const double *X, const double *Y, int64_t k, int32_t n_bins, double *sums_out,
+                                              int64_t *bin_rows, int64_t *bin_pos, double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_EVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc
+            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                      uint64_t key, int64_t pos_begin, int64_t pos_end, const double *X,
+                                                      const double *Y, int64_t k, int32_t n_bins, double *sums_out,
+                                                      int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                                      int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_EVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc
+            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                      const double *X, const double *Y, int64_t k, int32_t n_bins,
+                                                      double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
+                                                      double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_EVAL_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc
+            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all

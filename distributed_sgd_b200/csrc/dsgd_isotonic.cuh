@@ -1,0 +1,321 @@
+// dsgd_isotonic.cuh -- sm_90a kernels of the isotonic calibration calls (dsgd_calibrate_isotonic*,
+// dsgd_isotonic_probabilities, dsgd_eval_isotonic_calibration*; DESIGN.md §4.16).
+//
+// Isotonic regression of 0/1 labels on the score s = -x . w is the upper concave hull of the curve's points: with the m
+// distinct scores t_0 > t_1 > ... > t_(m-1) that a curve pass leaves in c_thr, and tp_k / fp_k the rows with s >= t_k, the
+// points are P_-1 = (0, 0) and P_k = (n_k, tp_k), n_k = tp_k + fp_k.  Here point i of the hull kernels is P_(i-1): point 0 is
+// the origin.  Every coordinate is an integer below 2^31, so the turn test is an int64 cross product and exact, and the hull
+// (vertices strictly above the chord of their neighbours) is one set whatever the algorithm that builds it.  The fit:
+//   1. k_iso_tile: each CTA takes a tile of S consecutive points into shared memory and its thread 0 runs the monotone chain.
+//   2. ceil(log2 tiles) rounds of k_iso_merge: each CTA merges two adjacent hulls -- the bridge (upper common tangent) by a
+//      binary search over the left hull with a binary search over the right one inside it, then the surviving vertices
+//      compacted into the other of two ping-pong buffers.
+//   3. an exclusive scan of every block's X count (1 or 2) and k_iso_emit: X, Y and the block counts, ascending in s.
+// k_iso_prob and k_iso_eval apply a map (X, Y) to rows as numpy.interp does.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "dsgd_calibrate.cuh"
+#include "dsgd_metrics.cuh"
+
+namespace dsgd {
+
+constexpr int kIsoTileMax = 2048;    // points of a tile in shared memory: 16 bytes of coordinates and 4 of stack each (40 KB)
+constexpr int kIsoThreads = 256;
+constexpr int kIsoSmemPoints = 6144; // (X, Y) pairs k_iso_prob / k_iso_eval keep in shared memory (96 KB); more stay in L2
+
+// The coordinates of point i: the origin, or (tp + fp, tp) of curve point i - 1
+__device__ __forceinline__ void iso_point(const long long *__restrict__ tp, const long long *__restrict__ fp, int i,
+                                          long long &x, long long &y) {
+  if (i == 0) { x = 0; y = 0; return; }
+  y = tp[i - 1];
+  x = y + fp[i - 1];
+}
+// (a - o) x (b - o): > 0 when b lies strictly above the line from o through a (x increasing), 0 when the three are collinear.
+// Every coordinate is below 2^31, so each product is below 2^62 and the difference is exact.
+__device__ __forceinline__ long long iso_cross(long long ox, long long oy, long long ax, long long ay, long long bx,
+                                               long long by) {
+  return (ax - ox) * (by - oy) - (ay - oy) * (bx - ox);
+}
+
+// Tile t of S points [t S, min(M, (t + 1) S)): its upper hull by the monotone chain (a point is popped when it lies on or
+// below the chord of its neighbours), vertex indices into hv[t S ..) and their count into hc[t].  Grid-stride over tiles.
+__global__ void __launch_bounds__(kIsoThreads) k_iso_tile(const long long *__restrict__ tp, const long long *__restrict__ fp,
+                                                          int M, int S, int *__restrict__ hv, int *__restrict__ hc) {
+  extern __shared__ __align__(16) unsigned char iso_smem[];
+  long long *sx = reinterpret_cast<long long *>(iso_smem), *sy = sx + S;
+  int *st = reinterpret_cast<int *>(sy + S);
+  __shared__ int s_top;
+  const int T = (M + S - 1) / S;
+  for (int t = blockIdx.x; t < T; t += gridDim.x) {
+    const int b = t * S, len = min(S, M - b);
+    for (int j = threadIdx.x; j < len; j += blockDim.x) iso_point(tp, fp, b + j, sx[j], sy[j]);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int top = 0;
+      for (int j = 0; j < len; ++j) {
+        const long long x = sx[j], y = sy[j];
+        while (top >= 2 && iso_cross(sx[st[top - 2]], sy[st[top - 2]], sx[st[top - 1]], sy[st[top - 1]], x, y) >= 0) --top;
+        st[top++] = j;
+      }
+      s_top = top;
+      hc[t] = top;
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < s_top; j += blockDim.x) hv[b + j] = b + st[j];
+    __syncthreads();
+  }
+}
+
+// One merge round over hulls of width W points (hull g at hv_in[g W ..), hc_in[g] vertices): pair p merges hulls 2p and
+// 2p + 1 into hull p of width 2W at hv_out[2p W ..); an odd last hull is copied.  L = l_0 .. l_(a-1), R = r_0 .. r_(b-1),
+// every x of L below every x of R, each strictly concave.  j(v), the tangent point from a vertex v of L on R: the first j
+// with r_(j+1) strictly below the line v -> r_j (the last of two collinear tangent points).  The bridge's left end: the
+// first i with l_(i+1) not strictly above the line l_i -> r_(j(l_i)), which holds for every i after it and for none before
+// it; the merged hull is l_0 .. l_i, r_(j(l_i)) .. r_(b-1).
+__global__ void __launch_bounds__(kIsoThreads) k_iso_merge(const long long *__restrict__ tp, const long long *__restrict__ fp,
+                                                           int n_hulls, int W, const int *__restrict__ hv_in,
+                                                           const int *__restrict__ hc_in, int *__restrict__ hv_out,
+                                                           int *__restrict__ hc_out) {
+  __shared__ int s_br[2];
+  const int pairs = (n_hulls + 1) / 2;
+  for (int p = blockIdx.x; p < pairs; p += gridDim.x) {
+    const int *L = hv_in + (int64_t)2 * p * W;
+    const int a = hc_in[2 * p];
+    const bool single = 2 * p + 1 >= n_hulls;
+    const int *R = L + W;
+    const int b = single ? 0 : hc_in[2 * p + 1];
+    if (threadIdx.x == 0) {
+      int i_end = a - 1, j_end = 0;
+      if (!single) {
+        auto tangent = [&](long long vx, long long vy) {
+          int lo = 0, hi = b - 1;
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            long long x0, y0, x1, y1;
+            iso_point(tp, fp, R[mid], x0, y0);
+            iso_point(tp, fp, R[mid + 1], x1, y1);
+            if (iso_cross(vx, vy, x0, y0, x1, y1) >= 0) lo = mid + 1; else hi = mid;
+          }
+          return lo;
+        };
+        int lo = 0, hi = a - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          long long vx, vy, ux, uy, rx, ry;
+          iso_point(tp, fp, L[mid], vx, vy);
+          iso_point(tp, fp, L[mid + 1], ux, uy);
+          iso_point(tp, fp, R[tangent(vx, vy)], rx, ry);
+          if (iso_cross(vx, vy, rx, ry, ux, uy) > 0) lo = mid + 1; else hi = mid;
+        }
+        long long vx, vy;
+        iso_point(tp, fp, L[lo], vx, vy);
+        i_end = lo;
+        j_end = tangent(vx, vy);
+      }
+      s_br[0] = i_end;
+      s_br[1] = j_end;
+      hc_out[p] = i_end + 1 + (single ? 0 : b - j_end);
+    }
+    __syncthreads();
+    const int i_end = s_br[0], j_end = s_br[1];
+    int *out = hv_out + (int64_t)2 * p * W;
+    for (int k = threadIdx.x; k <= i_end; k += blockDim.x) out[k] = L[k];
+    if (!single)
+      for (int k = threadIdx.x; k < b - j_end; k += blockDim.x) out[i_end + 1 + k] = R[j_end + k];
+    __syncthreads();
+  }
+}
+
+// X entries of block o (ascending score) of the final hull h_0 .. h_B: 2 when it spans two or more distinct scores, else 1
+struct iso_x_count {
+  const int *h;
+  int B;
+  __device__ __forceinline__ int operator()(int o) const {
+    const int b = B - 1 - o;
+    return 1 + (h[b + 1] - h[b] >= 2);
+  }
+};
+
+// Block o (ascending score) is hull segment b = B - 1 - o, from vertex h_b to h_(b+1): curve points h_b .. h_(b+1) - 1, its
+// highest score thr[h_b] and its lowest thr[h_(b+1) - 1].  p = fl(positives / rows).  excl: the exclusive scan of
+// iso_x_count; the last block writes the number of X entries to *n_x.
+__global__ void __launch_bounds__(256) k_iso_emit(const int *__restrict__ h, int B, const int *__restrict__ excl,
+                                                  const double *__restrict__ thr, const long long *__restrict__ tp,
+                                                  const long long *__restrict__ fp, double *__restrict__ X,
+                                                  double *__restrict__ Y, long long *__restrict__ blk_rows,
+                                                  long long *__restrict__ blk_pos, unsigned long long *__restrict__ n_x) {
+  for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < B; o += gridDim.x * blockDim.x) {
+    const int b = B - 1 - o, i0 = h[b], i1 = h[b + 1];
+    long long x0, y0, x1, y1;
+    iso_point(tp, fp, i0, x0, y0);
+    iso_point(tp, fp, i1, x1, y1);
+    const long long rows = x1 - x0, pos = y1 - y0;
+    const double p = (double)pos / (double)rows;
+    blk_rows[o] = rows;
+    blk_pos[o] = pos;
+    const int at = excl[o];
+    const bool two = i1 - i0 >= 2;
+    X[at] = thr[i1 - 1];
+    Y[at] = p;
+    if (two) {
+      X[at + 1] = thr[i0];
+      Y[at + 1] = p;
+    }
+    if (o == B - 1) *n_x = (unsigned long long)(at + 1 + two);
+  }
+}
+
+// ---- applying a map ----------------------------------------------------------------------------------------------------
+// numpy.interp(s, X, Y) for k >= 1 points, X strictly increasing: NaN for a NaN s, the end values outside [X_0, X_(k-1)],
+// Y_j at s == X_j, and else slope (s - X_j) + Y_j with slope = (Y_(j+1) - Y_j) / (X_(j+1) - X_j), X_j <= s < X_(j+1); a NaN
+// there retries from the right end, and a NaN again between equal Y gives Y_j.  No contraction (--fmad=false).
+__device__ __forceinline__ double iso_interp(double s, const double *X, const double *Y, int k) {
+  if (isnan(s)) return s;
+  if (s <= X[0]) return Y[0];
+  if (s >= X[k - 1]) return Y[k - 1];
+  int lo = 0, hi = k - 1;   // X[lo] <= s < X[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (X[mid] <= s) lo = mid; else hi = mid;
+  }
+  if (X[lo] == s) return Y[lo];
+  const double slope = (Y[lo + 1] - Y[lo]) / (X[lo + 1] - X[lo]);
+  double v = slope * (s - X[lo]) + Y[lo];
+  if (isnan(v)) {
+    v = slope * (s - X[lo + 1]) + Y[lo + 1];
+    if (isnan(v) && Y[lo] == Y[lo + 1]) v = Y[lo];
+  }
+  return v;
+}
+
+// The map in shared memory (kSmem: k <= kIsoSmemPoints) or read through L2
+template <bool kSmem>
+__device__ __forceinline__ void iso_stage(const double *__restrict__ X, const double *__restrict__ Y, int k,
+                                          const double *&xs, const double *&ys) {
+  if constexpr (kSmem) {
+    extern __shared__ __align__(16) unsigned char iso_map[];
+    double *sx = reinterpret_cast<double *>(iso_map), *sy = sx + k;
+    for (int i = threadIdx.x; i < k; i += blockDim.x) {
+      sx[i] = X[i];
+      sy[i] = Y[i];
+    }
+    __syncthreads();
+    xs = sx;
+    ys = sy;
+  } else {
+    xs = X;
+    ys = Y;
+  }
+}
+
+// out[i] = interp(-(x . w)) for row samples[i], x . w the row fold of dsgd_margins.  One warp per row.
+template <bool kSmem>
+__global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                  const int32_t *__restrict__ samples, int64_t n,
+                                                  const double *__restrict__ w, const double *__restrict__ X,
+                                                  const double *__restrict__ Y, int k, double *__restrict__ out) {
+  const double *xs, *ys;
+  iso_stage<kSmem>(X, Y, k, xs, ys);
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t i = warp0; i < n; i += nwarps) {
+    const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    if (lane == 0) out[i] = iso_interp(-dot, xs, ys, k);
+  }
+}
+
+// The quality pass at the map (X, Y): the block of k_calib_eval (CalibEvalWord) with p = interp(s), s = -(x . w); a NaN s
+// leaves the row out.  The log-loss term is -log p (o = 1) or -log1p(-p) (o = 0); a row whose term is infinite (p = 0 with
+// o = 1, p = 1 with o = 0) is counted in kCevInf and adds nothing to the sum.  Positions as in k_calib_eval.
+constexpr int kCevInf = kCevOutPsum + kCalMaxBins;
+static_assert(kCevInf < kCevWords, "the infinite-term count sits after the finished sums");
+template <bool kSmem>
+__global__ void __launch_bounds__(256) k_iso_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                  const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                  int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                  const double *__restrict__ X, const double *__restrict__ Y, int k,
+                                                  int n_bins, unsigned long long *__restrict__ blk) {
+  __shared__ unsigned long long s_rows[kCalMaxBins], s_pos[kCalMaxBins], s_lim[kCalMaxBins][kLossLimbs];
+  const double *xs, *ys;
+  iso_stage<kSmem>(X, Y, k, xs, ys);
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < kCalMaxBins; i += blockDim.x) {
+    s_rows[i] = 0ull;
+    s_pos[i] = 0ull;
+#pragma unroll
+    for (int q = 0; q < kLossLimbs; ++q) s_lim[i][q] = 0ull;
+  }
+  __syncthreads();
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned long long lb[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ll[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_b = 0, ovf_l = 0;
+  unsigned c_rows = 0, c_nan = 0, c_inf = 0;
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i = g + lane;
+    const bool mine = i < n;
+    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    double dot_own = 0.0;
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const double dot = row_margin(rp16, pairs, w, r, lane);
+      if (lane == j) dot_own = dot;
+    }
+    if (!mine) continue;
+    const double s = -dot_own;
+    if (isnan(s)) { ++c_nan; continue; }
+    const bool pos = label[r_own] > 0;
+    const double pr = iso_interp(s, xs, ys, k), o = pos ? 1.0 : 0.0, dlt = pr - o;
+    ++c_rows;
+    acc_add_local(lb, ovf_b, dlt * dlt);
+    const double term = pos ? -log(pr) : -log1p(-pr);
+    if (isinf(term)) ++c_inf;
+    else acc_add_local(ll, ovf_l, term);
+    int bin = (int)floor(pr * (double)n_bins);
+    bin = bin < n_bins - 1 ? bin : n_bins - 1;
+    atomicAdd(&s_rows[bin], 1ull);
+    if (pos) atomicAdd(&s_pos[bin], 1ull);
+    acc_cut(pr, [&](int q, double limb) {
+      if (limb != 0.0) atomicAdd(&s_lim[bin][q], (unsigned long long)(long long)limb);
+    });
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ovf_b += __shfl_xor_sync(full, ovf_b, o);
+    ovf_l += __shfl_xor_sync(full, ovf_l, o);
+#pragma unroll
+    for (int q = 0; q < kLossLimbs; ++q) {
+      lb[q] += __shfl_xor_sync(full, lb[q], o);
+      ll[q] += __shfl_xor_sync(full, ll[q], o);
+    }
+  }
+  c_rows = __reduce_add_sync(full, c_rows);
+  c_nan = __reduce_add_sync(full, c_nan);
+  c_inf = __reduce_add_sync(full, c_inf);
+  if (lane == 0) {
+    acc_flush_local(blk + kCevBrier, lb, ovf_b);
+    acc_flush_local(blk + kCevLog, ll, ovf_l);
+    if (c_rows) atomicAdd(&blk[kCevRows], (unsigned long long)c_rows);
+    if (c_nan) atomicAdd(&blk[kCevNan], (unsigned long long)c_nan);
+    if (c_inf) atomicAdd(&blk[kCevInf], (unsigned long long)c_inf);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n_bins; i += blockDim.x) {
+    if (!s_rows[i]) continue;
+    red_add_u64(blk + kCevBinRows + i, s_rows[i]);
+    if (s_pos[i]) red_add_u64(blk + kCevBinPos + i, s_pos[i]);
+    unsigned long long q[kLossLimbs];
+#pragma unroll
+    for (int t = 0; t < kLossLimbs; ++t) q[t] = s_lim[i][t];
+    acc_carry(q);
+#pragma unroll
+    for (int t = 0; t < kLossLimbs; ++t)
+      if (q[t]) red_add_u64(blk + kCevBinLimbs + i * kLossLimbs + t, q[t]);
+  }
+}
+
+}  // namespace dsgd

@@ -87,6 +87,31 @@ object DsgdNative {
   @native def evalSamplesCalibration(ctx: Long, w: Array[Double], samples: Array[Int], a: Double, b: Double, nBins: Int,
                                      sums: Array[Double], binRows: Array[Long], binPos: Array[Long], binPsum: Array[Double],
                                      words: Array[Long]): Int
+  // isotonic calibration: nPoints(0) = k, x / y(0 until k) the thresholds ascending in s = -x.w and their probabilities,
+  // blockRows / blockPos(0 until blocks), info(0..4) = blocks, points, rows used, NaN rows, distinct scores; x, y, blockRows
+  // and blockPos at least as long as the request's rows.  P(y = +1 | x) = numpy.interp(s, x, y).  Quality at the map (x, y):
+  // as evalCalibration, words(0..2) = rows used, rows left out, rows with an infinite log-loss term.
+  @native def calibrateIsotonic(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, nPoints: Array[Long],
+                                x: Array[Double], y: Array[Double], blockRows: Array[Long], blockPos: Array[Long],
+                                info: Array[Long]): Int
+  @native def calibrateIsotonicSampled(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                       posEnd: Long, nPoints: Array[Long], x: Array[Double], y: Array[Double],
+                                       blockRows: Array[Long], blockPos: Array[Long], info: Array[Long]): Int
+  @native def calibrateIsotonicSamples(ctx: Long, w: Array[Double], samples: Array[Int], nPoints: Array[Long],
+                                       x: Array[Double], y: Array[Double], blockRows: Array[Long], blockPos: Array[Long],
+                                       info: Array[Long]): Int
+  @native def isotonicProbabilities(ctx: Long, w: Array[Double], samples: Array[Int], x: Array[Double], y: Array[Double],
+                                    out: Array[Double]): Int
+  @native def evalIsotonicCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, x: Array[Double],
+                                      y: Array[Double], nBins: Int, sums: Array[Double], binRows: Array[Long],
+                                      binPos: Array[Long], binPsum: Array[Double], words: Array[Long]): Int
+  @native def evalSampledIsotonicCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long,
+                                             posBegin: Long, posEnd: Long, x: Array[Double], y: Array[Double], nBins: Int,
+                                             sums: Array[Double], binRows: Array[Long], binPos: Array[Long],
+                                             binPsum: Array[Double], words: Array[Long]): Int
+  @native def evalSamplesIsotonicCalibration(ctx: Long, w: Array[Double], samples: Array[Int], x: Array[Double],
+                                             y: Array[Double], nBins: Int, sums: Array[Double], binRows: Array[Long],
+                                             binPos: Array[Long], binPsum: Array[Double], words: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

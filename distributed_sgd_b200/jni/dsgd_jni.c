@@ -450,6 +450,139 @@ FN(evalSamplesCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, j
   return rc;
 }
 
+/* isotonic calibration: nPoints(0) = k, x / y(0 until k) the thresholds and their values, blockRows / blockPos(0 until
+ * blocks), info(0..4) = the DSGD_ISOTONIC_INFO_WORDS words; x, y, blockRows and blockPos at least as long as the request's
+ * rows.  Probabilities and quality at the map (x, y): x and y of one length k >= 1; out at least as long as samples; the
+ * quality arrays as for evalCalibration, words(0..2) = rows used, rows left out and rows with an infinite log-loss term.
+ * A shorter array is DSGD_ERR_INVALID. */
+typedef struct { buf_t k, x, y, r, p, info; } iso_bufs;
+static iso_bufs iso_out(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jlongArray blockRows,
+                        jlongArray blockPos, jlongArray info) {
+  iso_bufs c = {out_Long(env, nPoints), out_Double(env, x), out_Double(env, y), out_Long(env, blockRows),
+                out_Long(env, blockPos), out_Long(env, info)};
+  return c;
+}
+static int iso_bad(const iso_bufs *c) { return c->k.bad | c->x.bad | c->y.bad | c->r.bad | c->p.bad | c->info.bad; }
+static int iso_short(const iso_bufs *c, jlong n) {
+  return c->k.n < 1 || c->info.n < DSGD_ISOTONIC_INFO_WORDS || c->x.n < n || c->y.n < n || c->r.n < n || c->p.n < n;
+}
+static void iso_back(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jlongArray blockRows,
+                     jlongArray blockPos, jlongArray info, iso_bufs *c, int rc) {
+  back_Long(env, nPoints, c->k, rc);
+  back_Double(env, x, c->x, rc);
+  back_Double(env, y, c->y, rc);
+  back_Long(env, blockRows, c->r, rc);
+  back_Long(env, blockPos, c->p, rc);
+  back_Long(env, info, c->info, rc);
+}
+FN(calibrateIsotonic)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray nPoints,
+                      jdoubleArray x, jdoubleArray y, jlongArray blockRows, jlongArray blockPos, jlongArray info) {
+  buf_t bw = in_Double(env, w);
+  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | iso_bad(&c)))
+    rc = iso_short(&c, rowEnd - rowBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p,
+                                       (int64_t *)c.r.p, (int64_t *)c.p.p, (int64_t *)c.info.p);
+  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateIsotonicSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                             jlong posBegin, jlong posEnd, jlongArray nPoints, jdoubleArray x, jdoubleArray y,
+                             jlongArray blockRows, jlongArray blockPos, jlongArray info) {
+  buf_t bw = in_Double(env, w);
+  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | iso_bad(&c)))
+    rc = iso_short(&c, posEnd - posBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                               (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p, (int64_t *)c.r.p,
+                                               (int64_t *)c.p.p, (int64_t *)c.info.p);
+  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateIsotonicSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray nPoints,
+                             jdoubleArray x, jdoubleArray y, jlongArray blockRows, jlongArray blockPos, jlongArray info) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | iso_bad(&c)))
+    rc = iso_short(&c, bs.n)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic_samples(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p,
+                                               (int64_t *)c.r.p, (int64_t *)c.p.p, (int64_t *)c.info.p);
+  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+FN(isotonicProbabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray x,
+                          jdoubleArray y, jdoubleArray out) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y),
+        bo = out_Double(env, out);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bx.bad | by.bad | bo.bad))
+    rc = bo.n < bs.n || bx.n != by.n ? DSGD_ERR_INVALID
+                                     : dsgd_isotonic_probabilities(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, bo.p);
+  back_Double(env, out, bo, rc);
+  free(bw.p); free(bs.p); free(bx.p); free(by.p);
+  return rc;
+}
+static int iso_quality_short(const quality_bufs *q, jint nBins, const buf_t *bx, const buf_t *by) {
+  return quality_short(q, nBins) || q->wd.n < DSGD_ISOTONIC_EVAL_WORDS || bx->n != by->n;
+}
+FN(evalIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray x,
+                            jdoubleArray y, jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos,
+                            jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bx.bad | by.bad | quality_bad(&q)))
+    rc = iso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, bx.p, by.p, bx.n, nBins, (double *)q.s.p,
+                                              (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p); free(bx.p); free(by.p);
+  return rc;
+}
+FN(evalSampledIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                                   jlong key, jlong posBegin, jlong posEnd, jdoubleArray x, jdoubleArray y, jint nBins,
+                                   jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
+                                   jlongArray words) {
+  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bx.bad | by.bad | quality_bad(&q)))
+    rc = iso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, bx.p,
+                                                      by.p, bx.n, nBins, (double *)q.s.p, (int64_t *)q.r.p, (int64_t *)q.p.p,
+                                                      (double *)q.ps.p, (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p); free(bx.p); free(by.p);
+  return rc;
+}
+FN(evalSamplesIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray x,
+                                   jdoubleArray y, jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos,
+                                   jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y);
+  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bx.bad | by.bad | quality_bad(&q)))
+    rc = iso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_isotonic_calibration(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, nBins, (double *)q.s.p,
+                                                      (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p,
+                                                      (int64_t *)q.wd.p);
+  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p); free(bs.p); free(bx.p); free(by.p);
+  return rc;
+}
+
 /* ---- sync mode ---- */
 FN(commUniqueId)(JNIEnv *env, jobject self, jbyteArray id) {
   buf_t b = out_Byte(env, id);

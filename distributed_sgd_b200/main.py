@@ -98,13 +98,24 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                 f"{wr['weighted_loss']:.6f}, weighted accuracy {wr['weighted_accuracy']:.4f}")
     if "averaged_steps" in getattr(master, "history", {}):
         report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
-    if cfg.calibrate:
+    if cfg.calibrate and cfg.calibration_method == "isotonic":
+        # an isotonic map fitted on the train rows, judged on the test rows
+        iso = master.calibrate(w1, method="isotonic")
+        q = master.local_calibration(iso, w1, test_data=True)
+        report["calibration"] = {"method": "isotonic", "blocks": iso.blocks, "points": iso.points,
+                                 "distinct_scores": iso.distinct_scores, "test_brier": q["brier"],
+                                 "test_log_loss": q["log_loss"], "test_ece": q["ece"],
+                                 "test_infinite_log_loss_rows": q["infinite_log_loss_rows"]}
+        if rank == 0:
+            log(f"calibration (isotonic): {iso.blocks} blocks over {iso.distinct_scores} distinct train scores; "
+                f"test Brier {q['brier']:.6f}, log loss {q['log_loss']:.6f}, ECE {q['ece']:.6f}")
+    elif cfg.calibrate:
         # a Platt sigmoid fitted on the train rows, judged on the test rows; for the logistic model also against the
         # model's own probability, the identity link
         from .ml import Calibration
         cal = master.calibrate(w1)
         q = master.local_calibration(cal, w1, test_data=True)
-        report["calibration"] = {"a": cal.a, "b": cal.b, "iterations": cal.iterations, "status": cal.status,
+        report["calibration"] = {"method": "sigmoid", "a": cal.a, "b": cal.b, "iterations": cal.iterations, "status": cal.status,
                                  "test_brier": q["brier"], "test_log_loss": q["log_loss"], "test_ece": q["ece"]}
         if cfg.model == "logistic":
             q0 = master.local_calibration(Calibration.identity(), w1, test_data=True)

@@ -1,7 +1,10 @@
-"""A fitted probability link for a trained model: P(y = +1 | x) = 1 / (1 + exp(a x.w + b)) (Platt scaling)."""
+"""Fitted probability links for a trained model: P(y = +1 | x) = 1 / (1 + exp(a x.w + b)) (Platt scaling), or the
+isotonic map numpy.interp(-x.w, x, y) (IsotonicCalibration)."""
 from __future__ import annotations
 
 from dataclasses import dataclass
+
+import numpy as np
 
 CONVERGED, ITERATION_LIMIT, LINE_SEARCH_FAILED, NON_FINITE = 0, 1, 2, 3
 
@@ -22,3 +25,25 @@ class Calibration:
     def identity() -> "Calibration":
         """(1, 0): the SparseLogistic model's own probability sigmoid(-x.w)."""
         return Calibration(1.0, 0.0)
+
+
+METHODS = ("sigmoid", "isotonic")
+
+
+@dataclass(frozen=True, eq=False)
+class IsotonicCalibration:
+    """An isotonic map from the score s = -x.w to P(y = +1 | x) = numpy.interp(s, x, y): x the thresholds ascending (the
+    lowest and highest score of every block), y the block's value at each, and per block (ascending) its rows and positive
+    rows, so that each value is positives / rows.  Compared by identity (it holds arrays)."""
+    x: np.ndarray
+    y: np.ndarray
+    block_rows: np.ndarray
+    block_pos: np.ndarray
+    blocks: int = 0
+    rows: int = 0                     # rows the fit used
+    nan_rows: int = 0                 # rows left out because their margin was NaN
+    distinct_scores: int = 0
+
+    @property
+    def points(self) -> int:
+        return int(self.x.size)

@@ -35,6 +35,8 @@ OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM,
 METRICS_WORDS = 8
 CALIBRATION_INFO_WORDS = 5   # DSGD_CALIBRATION_INFO_WORDS
 CALIBRATION_MAX_BINS = 64    # DSGD_CALIBRATION_MAX_BINS
+ISOTONIC_INFO_WORDS = 5      # DSGD_ISOTONIC_INFO_WORDS: blocks, points, rows used, NaN rows, distinct scores
+ISOTONIC_EVAL_WORDS = 3      # DSGD_ISOTONIC_EVAL_WORDS: rows used, rows left out, rows with an infinite log-loss term
 
 
 class NativeLibraryMissing(ImportError):
@@ -122,6 +124,14 @@ ABI = {
     "dsgd_eval_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_sampled_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_samples_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_isotonic": [_vp, _vp, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_isotonic_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_isotonic_samples": [_vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
+    "dsgd_isotonic_probabilities": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp],
+    "dsgd_eval_isotonic_calibration": [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_sampled_isotonic_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp,
+                                               _vp, _vp],
+    "dsgd_eval_samples_isotonic_calibration": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
@@ -550,6 +560,74 @@ class NativeCtx:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_calibration)."""
         samples = _arr(samples, np.int32)
         return self._eval_calibration("eval_samples_calibration", w, (_ptr(samples), samples.size), a, b, n_bins)
+
+    # -- isotonic calibration --
+    def _calibrate_isotonic(self, fn: str, w, rows: tuple, n: int):
+        """dsgd_<fn>: (x, y, block_rows, block_pos, info) of one isotonic fit over n rows; info = the ISOTONIC_INFO_WORDS
+        words {blocks, points, rows used, NaN rows, distinct scores}."""
+        w = self._w(w)
+        size = max(int(n), 1)
+        x, y = np.zeros(size, dtype=np.float64), np.zeros(size, dtype=np.float64)
+        br, bp = np.zeros(size, dtype=np.int64), np.zeros(size, dtype=np.int64)
+        info, k = np.zeros(ISOTONIC_INFO_WORDS, dtype=np.int64), C.c_int64()
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(k), _ptr(x), _ptr(y), _ptr(br), _ptr(bp),
+                                                 _ptr(info)))
+        nb = int(info[0])
+        return x[:k.value].copy(), y[:k.value].copy(), br[:nb].copy(), bp[:nb].copy(), info
+
+    def calibrate_isotonic(self, row_begin: int, row_end: int, w=None):
+        """Isotonic regression of the labels on s = -x . w over rows [row_begin, row_end) (dsgd_calibrate_isotonic):
+        (x, y, block_rows, block_pos, info), x ascending, P(y = +1 | x) = numpy.interp(s, x, y)."""
+        return self._calibrate_isotonic("calibrate_isotonic", w, (row_begin, row_end), row_end - row_begin)
+
+    def calibrate_isotonic_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_isotonic_sampled)."""
+        return self._calibrate_isotonic("calibrate_isotonic_sampled", w, _drawn(row_begin, row_end, key, pos_begin, pos_end),
+                                        pos_end - pos_begin)
+
+    def calibrate_isotonic_samples(self, samples, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_calibrate_isotonic_samples)."""
+        samples = _arr(samples, np.int32)
+        return self._calibrate_isotonic("calibrate_isotonic_samples", w, (_ptr(samples), samples.size), samples.size)
+
+    def isotonic_probabilities(self, samples, x, y, w=None) -> np.ndarray:
+        """numpy.interp(-x_i . w, x, y) for each listed row, any model (dsgd_isotonic_probabilities)."""
+        samples = _arr(samples, np.int32)
+        x, y = _arr(x, np.float64), _arr(y, np.float64)
+        w = self._w(w)
+        out = np.zeros(samples.size, dtype=np.float64)
+        self._ck(self._l.dsgd_isotonic_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(x), _ptr(y),
+                                                     x.size if x.size == y.size else -1, _ptr(out)))
+        return out
+
+    def _eval_isotonic_calibration(self, fn: str, w, rows: tuple, x, y, n_bins: int):
+        """dsgd_<fn>: (sums, bin_rows, bin_pos, bin_psum, words): sums = {Brier sum, log-loss sum over the finite terms},
+        words = {rows used, rows left out, rows with an infinite term}."""
+        w = self._w(w)
+        x, y = _arr(x, np.float64), _arr(y, np.float64)
+        m = max(int(n_bins), 1)
+        sums, words = np.zeros(2, dtype=np.float64), np.zeros(ISOTONIC_EVAL_WORDS, dtype=np.int64)
+        rows_b, pos_b, psum = np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.float64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1,
+                                                 int(n_bins), _ptr(sums), _ptr(rows_b), _ptr(pos_b), _ptr(psum), _ptr(words)))
+        return sums, rows_b, pos_b, psum, words
+
+    def eval_isotonic_calibration(self, row_begin: int, row_end: int, x, y, n_bins: int = 10, w=None):
+        """Brier and log-loss sums and n_bins reliability bins at the map (x, y) over rows [row_begin, row_end)
+        (dsgd_eval_isotonic_calibration)."""
+        return self._eval_isotonic_calibration("eval_isotonic_calibration", w, (row_begin, row_end), x, y, n_bins)
+
+    def eval_sampled_isotonic_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, x, y,
+                                          n_bins: int = 10, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_isotonic_calibration)."""
+        return self._eval_isotonic_calibration("eval_sampled_isotonic_calibration", w,
+                                               _drawn(row_begin, row_end, key, pos_begin, pos_end), x, y, n_bins)
+
+    def eval_samples_isotonic_calibration(self, samples, x, y, n_bins: int = 10, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_isotonic_calibration)."""
+        samples = _arr(samples, np.int32)
+        return self._eval_isotonic_calibration("eval_samples_isotonic_calibration", w, (_ptr(samples), samples.size), x, y,
+                                               n_bins)
 
     def _curve(self, fn: str, w, rows: tuple, n: int, curve: bool):
         """dsgd_<fn>: (words, ap, thr, tp, fp) with the m points of a curve pass over n rows, or (words, ap, m) when not

@@ -38,7 +38,8 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     learning_rate_power: float = 1.0   # extension: 0 decay is the reference's constant rate
     l1: float = 0.0               # extension: L1 penalty l1 * ||w||_1 (lasso; elastic net with lambda), sync mode only
     class_weight: str = "none"    # extension: none, balanced or w_pos,w_neg -- one weight per label, sync mode only
-    calibrate: bool = False       # extension: after fit, fit a Platt sigmoid on the train rows and report its test-set quality
+    calibrate: bool = False       # extension: after fit, fit a calibration on the train rows and report its test-set quality
+    calibration_method: str = "sigmoid"   # extension: the calibration `calibrate` fits: sigmoid (Platt) or isotonic
     sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
 
 
@@ -55,6 +56,7 @@ _KEYS = {
     "learning-rate-decay": ("learning_rate_decay", "DSGD_LEARNING_RATE_DECAY"),
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
     "l1": ("l1", "DSGD_L1"), "class-weight": ("class_weight", "DSGD_CLASS_WEIGHT"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
+    "calibration-method": ("calibration_method", "DSGD_CALIBRATION_METHOD"),
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
@@ -131,6 +133,10 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"l1: expected a finite value >= 0, got {cfg.l1}")
     from ..ml.class_weight import parse_class_weight
     parse_class_weight(cfg.class_weight)   # raises on a malformed value
+    from ..ml.calibration import METHODS as CALIBRATION_METHODS
+    if cfg.calibration_method not in CALIBRATION_METHODS:
+        raise ValueError(f"calibration-method: expected one of {', '.join(CALIBRATION_METHODS)}, "
+                         f"got {cfg.calibration_method!r}")
     if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
         raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
     return cfg

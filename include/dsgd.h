@@ -343,6 +343,63 @@ int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t 
                                   int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
                                   int64_t *words_out);
 
+/* ---- isotonic calibration: a non-parametric map from the score to a probability, for any model (DESIGN.md §4.16).  The
+ *      rows, the three row forms, the score s = -x . w (f = x . w exactly as dsgd_margins returns it), NaN handling and the
+ *      +0 / -0 rule are those of dsgd_eval_curve.
+ *      Fit: the m distinct non-NaN scores t_0 > ... > t_(m-1) give the points P_k = (n_k, tp_k), n_k = tp_k + fp_k the rows
+ *      with s >= t_k and tp_k the positive ones, and P_-1 = (0, 0).  The blocks are the segments of the upper concave hull of
+ *      P_-1 .. P_(m-1); a hull vertex lies STRICTLY above the chord of its hull neighbours, so collinear points are not
+ *      vertices, two adjacent blocks never have the same exact value, and the block list is unique.  A block is one hull
+ *      segment and spans the distinct scores of the points after its left vertex up to its right one; its value is
+ *      p_b = fl(positives / rows) of its rows, one IEEE division of two exact counts.  p_b does not increase as the score decreases: this is scikit-learn's
+ *      IsotonicRegression(increasing=True, out_of_bounds="clip") fitted on (s, y in {0, 1}).  Every coordinate is an integer
+ *      below 2^31 and every hull test an exact int64 cross product, so the outputs have one bit pattern for a multiset of
+ *      rows, whatever the row form, the row order, the grid limit or the model flag.
+ *      Outputs, ascending in s (scikit-learn's X_thresholds_ / y_thresholds_):  x_out: the lowest and the highest distinct
+ *      score of every block (once when they are the same score; a zero score as +0);  y_out: the block's p_b at each;
+ *      *n_points_out = k, their number (k <= m);  rows_out[j] / pos_out[j]: the rows and positive rows of block j
+ *      (j ascending in s), so that p_j = fl(pos_out[j] / rows_out[j]).  Every output array holds at least n entries.
+ *      info_out (DSGD_ISOTONIC_INFO_WORDS): [0] blocks  [1] points k  [2] rows used  [3] NaN rows left out  [4] distinct
+ *      scores m.  A set of one class is valid (one block, p = 0 or 1); only "no row with a non-NaN score" ->
+ *      DSGD_ERR_EMPTY.  A NULL output -> DSGD_ERR_INVALID.  The list form takes at most 2^31 - 1 ids.  The fit is a curve
+ *      pass that leaves its points on the device, then the hull in parallel: tiles of DSGD_ISOTONIC_TILE points (an
+ *      environment variable, 1 .. 2048, default 2048; the result does not depend on it) and ceil(log2 tiles) merge rounds.
+ *      It grows the curve pass's buffers and about 52 bytes more per row on first use, except on an async ctx, whose first
+ *      loop start sizes them; the launches count in dsgd_launch_count (the scans' own kernels do not). */
+#define DSGD_ISOTONIC_INFO_WORDS 5
+int dsgd_calibrate_isotonic(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *n_points_out,
+                            double *x_out, double *y_out, int64_t *rows_out, int64_t *pos_out, int64_t *info_out);
+int dsgd_calibrate_isotonic_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                    int64_t pos_begin, int64_t pos_end, int64_t *n_points_out, double *x_out, double *y_out,
+                                    int64_t *rows_out, int64_t *pos_out, int64_t *info_out);
+int dsgd_calibrate_isotonic_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *n_points_out,
+                                    double *x_out, double *y_out, int64_t *rows_out, int64_t *pos_out, int64_t *info_out);
+/* Apply: probs_out[i] = numpy.interp(s_i, X, Y) with s_i = -x_i . w and numpy's own arithmetic: a NaN s gives NaN; s <= X_0
+ * gives Y_0 and s >= X_(k-1) gives Y_(k-1) (clip); else j with X_j <= s < X_(j+1) by binary search, s == X_j gives Y_j, and
+ * otherwise slope (s - X_j) + Y_j with slope = (Y_(j+1) - Y_j) / (X_(j+1) - X_j); if that is NaN, slope (s - X_(j+1)) +
+ * Y_(j+1); if that is NaN too and Y_j == Y_(j+1), Y_j.  The library is built without contraction, so this is numpy's
+ * result bit for bit (numpy itself returns Y_0 for a NaN s when k == 1).  X must be finite and strictly increasing, Y in
+ * [0, 1], k >= 1, else DSGD_ERR_INVALID.  Maps of up to 6144 points are held in shared memory, larger ones read through L2.
+ * Works beside a running async loop once a map of k points or more has been applied on the ctx (else DSGD_ERR_STATE). */
+int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, const double *X,
+                                const double *Y, int64_t k, double *probs_out);
+/* Quality at the map (X, Y), with p = the value dsgd_isotonic_probabilities gives and o = 1 for a positive row, 0 otherwise,
+ * over the rows whose s is not NaN: the outputs of dsgd_eval_calibration -- sums_out[0] the Brier sum, the bins as there --
+ * with sums_out[1] = the sum of -log p (o = 1) or -log1p(-p) (o = 0) over the rows whose term is finite.  words_out
+ * (DSGD_ISOTONIC_EVAL_WORDS): [0] rows used  [1] rows left out (NaN s)  [2] rows whose term is infinite (p = 0 with o = 1,
+ * or p = 1 with o = 0): any such row makes the log loss +inf.  The map's checks are those of dsgd_isotonic_probabilities. */
+#define DSGD_ISOTONIC_EVAL_WORDS 3
+int dsgd_eval_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, const double *X,
+                                   const double *Y, int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows,
+                                   int64_t *bin_pos, double *bin_psum, int64_t *words_out);
+int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                           int64_t pos_begin, int64_t pos_end, const double *X, const double *Y, int64_t k,
+                                           int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
+                                           double *bin_psum, int64_t *words_out);
+int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, const double *X,
+                                           const double *Y, int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows,
+                                           int64_t *bin_pos, double *bin_psum, int64_t *words_out);
+
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
  *      (its own RPC), every rank calls dsgd_comm_init.  world == 1 needs neither. -------------------------- */
