@@ -71,6 +71,20 @@ def _calibration(result) -> Calibration:
     return Calibration(a, b, objective, int(info[0]), int(info[1]), int(info[2]), int(info[3]))
 
 
+def _weighted_calibration(result) -> Calibration:
+    """A NativeCtx.calibrate_weighted* result as a weighted Calibration."""
+    a, b, objective, info, wsums = result
+    return Calibration(a, b, objective, int(info[0]), int(info[1]), int(info[2]), int(info[3]), True, float(wsums[0]),
+                       float(wsums[1]), float(wsums[2]))
+
+
+def _weighted_isotonic(result) -> IsotonicCalibration:
+    """A NativeCtx.calibrate_isotonic_weighted* result as a weighted IsotonicCalibration."""
+    x, y, block_w, block_pw, info, wsums = result
+    return IsotonicCalibration(x, y, block_w, block_pw, int(info[0]), int(info[2]), int(info[3]), int(info[4]), True,
+                               float(wsums[0]), float(wsums[1]))
+
+
 def _isotonic(result) -> IsotonicCalibration:
     """A NativeCtx.calibrate_isotonic* result as an IsotonicCalibration."""
     x, y, block_rows, block_pos, info = result
@@ -110,6 +124,29 @@ def calibration_dict(result) -> dict:
             "ece": float(np.sum(bin_rows[filled] / n * gap)) if n else nan, "mce": float(np.max(gap)) if n else nan,
             "rows": n, "nan_rows": int(words[1]),
             "bins": {"edges": np.arange(m + 1) / m, "rows": bin_rows, "positives": bin_pos, "mean_predicted": mean_p,
+                     "observed": freq}}
+
+
+def weighted_calibration_dict(result) -> dict:
+    """The result of Master.local_calibration(weighted=True) from a NativeCtx.eval_*weighted_calibration result, every row
+    counted by its weight: with W = sums[2] the weight of the rows used, brier = S_brier / W, log_loss = S_ll / W (+inf when a
+    row of positive weight has an infinite term, sums[3] > 0), ece = sum over the bins of (W_b / W) |psum_b / W_b - pos_b /
+    W_b|, mce = the largest such gap, rows and nan_rows (counts), weight = W, and bins: edges, weight, positive_weight,
+    mean_predicted and observed (NaN for a bin of zero weight); at an isotonic map also infinite_log_loss_rows."""
+    sums, bin_w, bin_pw, bin_psum, words = result
+    W, m = float(sums[2]), len(bin_w)
+    filled = bin_w > 0
+    den = np.where(filled, bin_w, 1.0)
+    mean_p = np.where(filled, bin_psum / den, np.nan)
+    freq = np.where(filled, bin_pw / den, np.nan)
+    gap = np.abs(mean_p - freq)[filled]
+    nan = float("nan")
+    log_loss = float("inf") if sums[3] > 0 else (float(sums[1]) / W if W else nan)
+    extra = {"infinite_log_loss_rows": int(words[2])} if len(words) > 2 else {}
+    return {**extra, "brier": float(sums[0]) / W if W else nan, "log_loss": log_loss,
+            "ece": float(np.sum(bin_w[filled] / W * gap)) if W else nan, "mce": float(np.max(gap)) if gap.size else nan,
+            "rows": int(words[0]), "nan_rows": int(words[1]), "weight": W,
+            "bins": {"edges": np.arange(m + 1) / m, "weight": bin_w, "positive_weight": bin_pw, "mean_predicted": mean_p,
                      "observed": freq}}
 
 
@@ -497,22 +534,36 @@ class Master:
     # the whole range or sample itself.  Every sum over the rows is an order-free fixed-point sum and the arithmetic between
     # the sums is one fixed sequence, so every rank gets the same bits without a collective.  None of them touches the
     # weights or the step state: they can be called from `fit`'s on_epoch hook.
-    def calibrate(self, weights=None, test_data: bool = False, method: str = "sigmoid"):
+    def calibrate(self, weights=None, test_data: bool = False, method: str = "sigmoid", weighted: bool = False):
         """A calibration of the margins over the train (or test) rows.  method "sigmoid": Platt scaling, the Calibration
         (a, b) that makes 1 / (1 + exp(a x.w + b)) a probability; "isotonic": isotonic regression, an IsotonicCalibration.
-        weights None: the resident weights, as in local_metrics."""
+        weights None: the resident weights, as in local_metrics.  weighted: fitted with every row counted by its weight
+        c_i = class weight x sample weight (dsgd_calibrate_weighted, dsgd_calibrate_isotonic_weighted)."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        if weighted:
+            if _method(method) == "isotonic":
+                return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted(b, e, weights))
+            return _weighted_calibration(self.ctx.calibrate_weighted(b, e, weights))
         if _method(method) == "isotonic":
             return _isotonic(self.ctx.calibrate_isotonic(b, e, weights))
         return _calibration(self.ctx.calibrate(b, e, weights))
 
-    def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False, method: str = "sigmoid"):
+    def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False, method: str = "sigmoid",
+                          weighted: bool = False):
         """calibrate on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
         sample raises DsgdEmpty."""
         iso = _method(method) == "isotonic"
         b, e, k, key, ids = self._draw_sample(samples_count, test_data)
         if k <= 0:
             raise DsgdEmpty(ERR_EMPTY, f"sampled calibration of {samples_count} rows: the sample is empty")
+        if weighted and iso:
+            if ids is None:
+                return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted_sampled(b, e, key, 0, k, weights))
+            return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted_samples(ids, weights))
+        if weighted:
+            if ids is None:
+                return _weighted_calibration(self.ctx.calibrate_weighted_sampled(b, e, key, 0, k, weights))
+            return _weighted_calibration(self.ctx.calibrate_weighted_samples(ids, weights))
         if ids is None:
             if iso:
                 return _isotonic(self.ctx.calibrate_isotonic_sampled(b, e, key, 0, k, weights))
@@ -521,29 +572,48 @@ class Master:
             return _isotonic(self.ctx.calibrate_isotonic_samples(ids, weights))
         return _calibration(self.ctx.calibrate_samples(ids, weights))
 
-    def local_calibration(self, calibration, weights=None, test_data: bool = False, n_bins: int = 10) -> dict:
+    def local_calibration(self, calibration, weights=None, test_data: bool = False, n_bins: int = 10,
+                          weighted: bool = False) -> dict:
         """How well `calibration` (a Calibration or an IsotonicCalibration) fits the train (or test) rows: Brier score, log
         loss, expected and maximum calibration error and the reliability bins (calibration_dict; isotonic_calibration_dict
-        for an isotonic map).  Every rank evaluates the whole range itself."""
+        for an isotonic map).  Every rank evaluates the whole range itself.  weighted: every row counted by its weight c_i
+        (weighted_calibration_dict)."""
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         if isinstance(calibration, IsotonicCalibration):
+            if weighted:
+                return weighted_calibration_dict(self.ctx.eval_weighted_isotonic_calibration(b, e, calibration.x,
+                                                                                             calibration.y, n_bins, weights))
             return isotonic_calibration_dict(self.ctx.eval_isotonic_calibration(b, e, calibration.x, calibration.y, n_bins,
+                                                                                weights))
+        if weighted:
+            return weighted_calibration_dict(self.ctx.eval_weighted_calibration(b, e, calibration.a, calibration.b, n_bins,
                                                                                 weights))
         return calibration_dict(self.ctx.eval_calibration(b, e, calibration.a, calibration.b, n_bins, weights))
 
     def local_sampled_calibration(self, calibration: Calibration, weights, samples_count: int, test_data: bool = False,
-                                  n_bins: int = 10) -> dict:
+                                  n_bins: int = 10, weighted: bool = False) -> dict:
         """local_calibration on a fresh sample of min(samples_count, n) rows.  An empty sample raises DsgdEmpty."""
         b, e, k, key, ids = self._draw_sample(samples_count, test_data)
         if k <= 0:
             raise DsgdEmpty(ERR_EMPTY, f"sampled calibration quality of {samples_count} rows: the sample is empty")
         if isinstance(calibration, IsotonicCalibration):
             x, y = calibration.x, calibration.y
+            if weighted:
+                if ids is None:
+                    return weighted_calibration_dict(self.ctx.eval_sampled_weighted_isotonic_calibration(
+                        b, e, key, 0, k, x, y, n_bins, weights))
+                return weighted_calibration_dict(self.ctx.eval_samples_weighted_isotonic_calibration(ids, x, y, n_bins,
+                                                                                                     weights))
             if ids is None:
                 return isotonic_calibration_dict(self.ctx.eval_sampled_isotonic_calibration(b, e, key, 0, k, x, y, n_bins,
                                                                                             weights))
             return isotonic_calibration_dict(self.ctx.eval_samples_isotonic_calibration(ids, x, y, n_bins, weights))
         a, bb = calibration.a, calibration.b
+        if weighted:
+            if ids is None:
+                return weighted_calibration_dict(self.ctx.eval_sampled_weighted_calibration(b, e, key, 0, k, a, bb, n_bins,
+                                                                                            weights))
+            return weighted_calibration_dict(self.ctx.eval_samples_weighted_calibration(ids, a, bb, n_bins, weights))
         if ids is None:
             return calibration_dict(self.ctx.eval_sampled_calibration(b, e, key, 0, k, a, bb, n_bins, weights))
         return calibration_dict(self.ctx.eval_samples_calibration(ids, a, bb, n_bins, weights))

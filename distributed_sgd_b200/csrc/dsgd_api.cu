@@ -168,14 +168,21 @@ struct dsgd_ctx {
   dev_buf<long long> c_tp, c_fp;
   // a calibration fit (dsgd_calibrate*, dsgd_calibrate.cuh): one score and one label per position; the control words (the
   // counts, the three accumulator lines, the barrier counter and abort flag, the result); and the quality pass's block
-  dev_buf<double> k_score;
+  // (a weighted fit also keeps each position's weight c in k_cw)
+  dev_buf<double> k_score, k_cw;
   dev_buf<int8_t> k_lab;
   dev_buf<unsigned long long> k_ctl, k_eval;
-  int k_fit_occ = 0;   // CTAs of k_calib_fit per SM at its full shared-memory budget (0: not asked yet)
+  int k_fit_occ = 0;     // CTAs of k_calib_fit<false> per SM at its full shared-memory budget (0: not asked yet)
+  int k_fit_occ_w = 0;   // likewise for k_calib_fit<true>
   // an isotonic fit (dsgd_calibrate_isotonic*, dsgd_isotonic.cuh): the hull's two ping-pong vertex buffers, their two
   // count buffers and the scan of the blocks' X counts; X and Y; the block rows and positives; the X count.  A map applied
   // to rows (dsgd_isotonic_probabilities, dsgd_eval_isotonic_calibration*): its X and Y
   dev_buf<int> i_hull;
+  // a weighted isotonic fit: the points' exact coordinates (all m, then the kept ones), their keep flags and its scan, the
+  // kept points' scores, and the blocks' weights and positive weights
+  dev_buf<u256> i_wpt;
+  dev_buf<int> i_wkeep;
+  dev_buf<double> i_wthr, i_wblk;
   dev_buf<double> i_out, i_map;
   dev_buf<long long> i_blk;
   dev_buf<unsigned long long> i_ctl;
@@ -1289,12 +1296,14 @@ static cudaError_t scan_weights(dsgd_ctx *ctx, void *tmp, size_t &bytes, const d
 // exclusive scan of the merged keys' tie ends, k_curve_emit, and the m points copied back at once; `device_points` (an
 // isotonic fit): the points are emitted into c_thr / c_tp / c_fp and stay there.  AP = S / P, NaN when a
 // score is NaN or there is no positive row.
+// runs_out: the sorted runs, for a caller that reads them after the pass.
 // kSampleWeighted (§4.14): the same steps in their weighted forms, each run's prefix sums of R(c) scanned into c_pre before
 // k_curve_count (positives at c_pre[0, n_pos), negatives after them); out receives the DSGD_WCURVE_WORDS words instead of
 // AP, and tp / fp the point weights as doubles (k_curve_emit writes their bits into c_tp / c_fp).
 template <int kWeight>
 static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *words, double *out, int64_t *n_points,
-                      double *thr, void *tp, void *fp, const char *fn, bool device_points = false) {
+                      double *thr, void *tp, void *fp, const char *fn, bool device_points = false,
+                      sorted_runs *runs_out = nullptr) {
   constexpr bool kW = kWeight == kSampleWeighted;
   constexpr int kWords = kW ? kCurWWords : kCurWords;
   const int64_t n = rows.n;
@@ -1373,6 +1382,7 @@ static int curve_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64
     memcpy(&S, &c[kCurSum], sizeof S);
     *out = (words[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
   }
+  if (runs_out) *runs_out = s;   // a weighted isotonic fit reads the sorted runs and their prefix sums
   *n_points = m;
   return DSGD_OK;
 }
@@ -1494,9 +1504,11 @@ extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const i
 // Words of k_ctl: the counts of k_calib_score, the result of k_calib_fit, {barrier counter, abort flag}, the three lines
 constexpr int kCtlCnt = 0, kCtlOut = kCalCntWords, kCtlBar = kCtlOut + kCalOutWords, kCtlAcc = 16;
 constexpr int kCtlWords = kCtlAcc + 3 * kCalLineStride;
+constexpr int kCtlW = kCtlWords, kCtlWWords = kCtlW + kCalWWords;   // a weighted fit's sums of R(c) (CalibWeightWord)
 static_assert(kCtlBar + 1 <= kCtlAcc, "k_ctl layout");
 static_assert(kCalMaxBins == DSGD_CALIBRATION_MAX_BINS && kCalOutEvals < kCalOutWords, "calibration layout");
 constexpr int kCalSmemScores = 14336;   // scores (8 bytes) and labels (1 byte) a CTA of k_calib_fit keeps in shared memory: 126 KB
+constexpr int kCalSmemScoresW = 7552;   // k_calib_fit<true>: score, weight (8 bytes each) and label, within the same 126 KB
 
 // A cooperative grid cannot be assumed resident beside a kernel that runs until it is stopped.
 static int calibrate_allowed(dsgd_ctx *ctx, const char *fn) {
@@ -1508,51 +1520,99 @@ static int calibrate_allowed(dsgd_ctx *ctx, const char *fn) {
   return DSGD_OK;
 }
 
+// read() on the host: the value of six limb words and an overflow count, converted as acc_value converts them (the same
+// operations in the same order, so the same bits): carries, then the limbs from the top down.
+static double fixed_read(const unsigned long long *limbs, unsigned long long ovf) {
+  if (ovf) return std::numeric_limits<double>::quiet_NaN();
+  unsigned long long q[kLossLimbs];
+  for (int i = 0; i < kLossLimbs; ++i) q[i] = limbs[i];
+  for (int i = 0; i < kLossLimbs - 1; ++i) {
+    q[i + 1] += q[i] >> 40;
+    q[i] &= kLimbMask;
+  }
+  double s = (double)q[kLossLimbs - 1] * 0x1p40;
+  for (int i = kLossLimbs - 2; i >= 0; --i) s += (double)q[i] * std::ldexp(1.0, 40 * i - 160);
+  return s;
+}
+
 // One fit over `rows`: k_calib_score, the counts read by the host, k_calib_fit, the result read back.
+// kW: the weighted fit (DESIGN.md §4.17): the targets and start point from W+ and W-, each read() of an exact sum of R(c_i);
+// wsums_out = {W+, W-, the NaN rows' weight}.
+template <bool kW>
 static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *ab_out, double *objective_out,
-                          int64_t *info_out, const char *fn) {
+                          int64_t *info_out, double *wsums_out, const char *fn) {
   const int64_t n = rows.n;
+  const int ctl_words = kW ? kCtlWWords : kCtlWords;
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd);
   if (rc || (rc = ctx->k_score.grow(ctx, n, 1024)) || (rc = ctx->k_lab.grow(ctx, n, 1024)) ||
-      (rc = ctx->k_ctl.grow(ctx, kCtlWords, kCtlWords)))
+      (rc = ctx->k_ctl.grow(ctx, ctl_words, ctl_words)) || (kW && (rc = ctx->k_cw.grow(ctx, n, 1024))))
     return rc;
-  CU(cudaMemsetAsync(ctx->k_ctl, 0, sizeof(unsigned long long) * kCtlWords, ctx->stream));
+  CU(cudaMemsetAsync(ctx->k_ctl, 0, sizeof(unsigned long long) * ctl_words, ctx->stream));
   const int sgrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
-  k_calib_score<<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt);
+  if constexpr (kW)
+    k_calib_score<true><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                        ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
+                                                        ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr, ctx->k_cw,
+                                                        ctx->k_ctl + kCtlW);
+  else
+    k_calib_score<false><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                         ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt);
   LAUNCHED();
   CU(cudaGetLastError());
-  unsigned long long cnt[kCalCntWords];
+  unsigned long long cnt[kCalCntWords], wacc[kCalWWords];
   CU(cudaMemcpyAsync(cnt, ctx->k_ctl + kCtlCnt, sizeof cnt, cudaMemcpyDeviceToHost, ctx->stream));
+  if (kW) CU(cudaMemcpyAsync(wacc, ctx->k_ctl + kCtlW, sizeof wacc, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   const int64_t n_pos = (int64_t)cnt[kCalPos], n_neg = (int64_t)cnt[kCalNeg];
-  NEED(n_pos > 0 && n_neg > 0, DSGD_ERR_EMPTY, "%s: %lld positive and %lld negative rows with a score (%lld NaN): a sigmoid needs both classes",
-       fn, (long long)n_pos, (long long)n_neg, (long long)cnt[kCalNan]);
-
-  if (!ctx->k_fit_occ) {
-    const int full = kCalSmemScores * 9;
-    CU(cudaFuncSetAttribute(k_calib_fit, cudaFuncAttributeMaxDynamicSharedMemorySize, full));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->k_fit_occ, k_calib_fit, kCalThreads, (size_t)full));
-    NEED(ctx->k_fit_occ > 0, DSGD_ERR_CUDA, "%s: k_calib_fit does not fit on an SM", fn);
+  double t_pos, t_neg, b0;
+  if constexpr (kW) {
+    const double w_p = fixed_read(wacc + kCalWPos, wacc[kCalWPos + kLossLimbs]);
+    const double w_n = fixed_read(wacc + kCalWNeg, wacc[kCalWNeg + kLossLimbs]);
+    wsums_out[0] = w_p;
+    wsums_out[1] = w_n;
+    wsums_out[2] = fixed_read(wacc + kCalWNan, wacc[kCalWNan + kLossLimbs]);
+    NEED(w_p != 0.0 && w_n != 0.0, DSGD_ERR_EMPTY,
+         "%s: positive weight %g and negative weight %g among the rows with a score: a sigmoid needs both classes", fn, w_p,
+         w_n);
+    t_pos = (w_p + 1.0) / (w_p + 2.0);
+    t_neg = 1.0 / (w_n + 2.0);
+    b0 = std::log((w_n + 1.0) / (w_p + 1.0));
+  } else {
+    NEED(n_pos > 0 && n_neg > 0, DSGD_ERR_EMPTY, "%s: %lld positive and %lld negative rows with a score (%lld NaN): a sigmoid needs both classes",
+         fn, (long long)n_pos, (long long)n_neg, (long long)cnt[kCalNan]);
+    t_pos = ((double)n_pos + 1.0) / ((double)n_pos + 2.0);
+    t_neg = 1.0 / ((double)n_neg + 2.0);
+    b0 = std::log(((double)n_neg + 1.0) / ((double)n_pos + 1.0));
   }
-  int G = ctx->sm_count * ctx->k_fit_occ;   // resident at the full shared-memory budget, so at any smaller one
+
+  constexpr int cap_max = kW ? kCalSmemScoresW : kCalSmemScores, per_score = kW ? 17 : 9;
+  int &occ = kW ? ctx->k_fit_occ_w : ctx->k_fit_occ;
+  if (!occ) {
+    const int full = cap_max * per_score;
+    CU(cudaFuncSetAttribute((kW ? k_calib_fit_w : k_calib_fit), cudaFuncAttributeMaxDynamicSharedMemorySize, full));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (kW ? k_calib_fit_w : k_calib_fit), kCalThreads, (size_t)full));
+    NEED(occ > 0, DSGD_ERR_CUDA, "%s: k_calib_fit does not fit on an SM", fn);
+  }
+  int G = ctx->sm_count * occ;   // resident at the full shared-memory budget, so at any smaller one
   if (ctx->grid_limit > 0) G = std::min(G, ctx->grid_limit);
   G = (int)std::min<int64_t>(G, cdiv(n, kCalThreads));
   CalibFitParams fp;
   memset(&fp, 0, sizeof fp);
   fp.score = ctx->k_score; fp.lab = ctx->k_lab; fp.n = n;
-  fp.t_pos = ((double)n_pos + 1.0) / ((double)n_pos + 2.0);
-  fp.t_neg = 1.0 / ((double)n_neg + 2.0);
-  fp.b0 = std::log(((double)n_neg + 1.0) / ((double)n_pos + 1.0));
+  fp.t_pos = t_pos;
+  fp.t_neg = t_neg;
+  fp.b0 = b0;
   fp.acc = ctx->k_ctl + kCtlAcc;
   fp.bar = reinterpret_cast<unsigned *>(ctx->k_ctl + kCtlBar);
   fp.abort_flag = reinterpret_cast<int *>(ctx->k_ctl + kCtlBar) + 1;
   fp.timeout_cycles = 4000000000ll;   // ~2 s, as the sync step's barrier
   fp.out = ctx->k_ctl + kCtlOut;
-  fp.smem_cap = (int)std::min<int64_t>(cdiv(n, G), kCalSmemScores);
+  fp.smem_cap = (int)std::min<int64_t>(cdiv(n, G), cap_max);
+  if (kW) fp.cw = ctx->k_cw;
   void *args[] = {&fp};
-  CU(cudaLaunchCooperativeKernel((void *)k_calib_fit, dim3(G), dim3(kCalThreads), args, (size_t)fp.smem_cap * 9, ctx->stream));
+  CU(cudaLaunchCooperativeKernel((void *)(kW ? k_calib_fit_w : k_calib_fit), dim3(G), dim3(kCalThreads), args, (size_t)fp.smem_cap * per_score,
+                                 ctx->stream));
   LAUNCHED();
   unsigned long long out[kCalOutWords + 1];
   CU(cudaMemcpyAsync(out, ctx->k_ctl + kCtlOut, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1579,7 +1639,7 @@ extern "C" int dsgd_calibrate(dsgd_ctx *ctx, const double *w, int64_t row_begin,
   row_set rows;
   int rc = calibrate_allowed(ctx, __func__);
   if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
-  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
 }
 
 extern "C" int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -1590,7 +1650,7 @@ extern "C" int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t ro
   row_set rows;
   int rc = calibrate_allowed(ctx, __func__);
   if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
-  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
 }
 
 extern "C" int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
@@ -1601,7 +1661,51 @@ extern "C" int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int3
   row_set rows;
   int rc = calibrate_allowed(ctx, __func__);
   if (rc || (rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
-  return calibrate_pass(ctx, w, rows, ab_out, objective_out, info_out, __func__);
+  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
+}
+
+// A weighted calibration call: an async ctx is refused before anything is launched (its weights are always 1), as the
+// weighted curves refuse it.
+static int weighted_calibration_allowed(dsgd_ctx *ctx, const char *fn) {
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (row weights belong to the sync paths)",
+       fn);
+  return DSGD_OK;
+}
+
+#define CALIB_W_ARGS_OK()                                                                                               \
+  do {                                                                                                                  \
+    NEED(ab_out && objective_out && info_out && wsums_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);         \
+    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
+    if (rc_) return rc_;                                                                                                \
+  } while (0)
+
+extern "C" int dsgd_calibrate_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
+                                       double *objective_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_W_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                               uint64_t key, int64_t pos_begin, int64_t pos_end, double *ab_out,
+                                               double *objective_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_W_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
+}
+
+extern "C" int dsgd_calibrate_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                               double *ab_out, double *objective_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_W_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
 }
 
 extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
@@ -1687,6 +1791,102 @@ extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, con
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+// One weighted quality pass over `rows`, at (a, b) or (kIso) at the map (X, Y): k_weval, the block read back, every sum
+// read() on the host.
+static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn);
+template <class K>
+static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args);
+template <bool kIso>
+static int weighted_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, const double *X,
+                                 const double *Y, int64_t k, int32_t n_bins, double *sums_out, double *bin_weight,
+                                 double *bin_pos_weight, double *bin_psum, int64_t *words_out, const char *fn) {
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd);
+  if (rc || (kIso && (rc = isotonic_map(ctx, X, Y, k, fn))) || (rc = ctx->k_eval.grow(ctx, kCwvWords, kCwvWords))) return rc;
+  CU(cudaMemsetAsync(ctx->k_eval, 0, sizeof(unsigned long long) * kCwvWords, ctx->stream));
+  const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);
+  const double *mx = kIso ? ctx->i_map.p : nullptr, *my = kIso ? ctx->i_map.p + k : nullptr;
+  int ki = (int)k, nb = n_bins;
+  unsigned long long *blk = ctx->k_eval.p;
+  const uint32_t *rp16 = ctx->rp16.p;
+  const uint2 *pairs = ctx->pairs.p;
+  const int8_t *label = ctx->label.p;
+  const int32_t *ids = rows.ids;
+  int64_t rb = rows.row_begin, rn = rows.n;
+  double cwp = ctx->cw_pos, cwn = ctx->cw_neg;
+  const double *swp = ctx->sw_on ? ctx->sw.p : nullptr;
+  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &cwp, &cwn, &swp};
+  if constexpr (kIso)
+    CU(isotonic_launch(k_weval<true, true>, k_weval<true, false>, grid, k, ctx->stream, args));
+  else
+    CU(cudaLaunchKernel((const void *)k_weval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
+  LAUNCHED();
+  CU(cudaGetLastError());
+  std::vector<unsigned long long> h(kCwvWords);
+  CU(cudaMemcpyAsync(h.data(), ctx->k_eval, sizeof(unsigned long long) * kCwvWords, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  sums_out[0] = fixed_read(&h[kCwvBrier], h[kCwvBrier + kLossLimbs]);
+  sums_out[1] = fixed_read(&h[kCwvLog], h[kCwvLog + kLossLimbs]);
+  sums_out[2] = fixed_read(&h[kCwvW], h[kCwvW + kLossLimbs]);
+  sums_out[3] = fixed_read(&h[kCwvInfW], h[kCwvInfW + kLossLimbs]);   // always 0 at a sigmoid: its term is finite
+  for (int i = 0; i < n_bins; ++i) {
+    const unsigned long long *q = &h[kCwvBins + i * kCwvBinStride], ovf = q[3 * kLossLimbs];
+    bin_weight[i] = fixed_read(q, ovf);
+    bin_pos_weight[i] = fixed_read(q + kLossLimbs, ovf);
+    bin_psum[i] = fixed_read(q + 2 * kLossLimbs, ovf);
+  }
+  words_out[0] = (int64_t)h[kCwvRows];
+  words_out[1] = (int64_t)h[kCwvNan];
+  if (kIso) words_out[2] = (int64_t)h[kCwvInf];
+  return DSGD_OK;
+}
+
+#define CALIB_WEVAL_ARGS_OK()                                                                                           \
+  do {                                                                                                                  \
+    NEED(sums_out && bin_weight && bin_pos_weight && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL",   \
+         __func__);                                                                                                     \
+    NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", __func__, a, b); \
+    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
+    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
+    if (rc_) return rc_;                                                                                                \
+  } while (0)
+
+extern "C" int dsgd_eval_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a,
+                                              double b, int32_t n_bins, double *sums_out, double *bin_weight,
+                                              double *bin_pos_weight, double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_WEVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
+                                                 bin_pos_weight, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                      uint64_t key, int64_t pos_begin, int64_t pos_end, double a, double b,
+                                                      int32_t n_bins, double *sums_out, double *bin_weight,
+                                                      double *bin_pos_weight, double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_WEVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
+                                                 bin_pos_weight, bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_weighted_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                      double a, double b, int32_t n_bins, double *sums_out,
+                                                      double *bin_weight, double *bin_pos_weight, double *bin_psum,
+                                                      int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  CALIB_WEVAL_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
+                                                 bin_pos_weight, bin_psum, words_out, __func__);
 }
 
 // ---- isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.16) ------------------------------------------------------
@@ -1935,6 +2135,212 @@ extern "C" int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const doubl
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc
             : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+}
+
+// ---- weighted isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.17) -----------------------------------------------
+
+// One weighted isotonic fit over `rows`: the weighted curve pass with its points left on the device; the total weight of
+// its non-NaN rows checked against the turn test's bound; every point's exact coordinates and the zero-weight points
+// dropped (k_iso_wpoint, a scan of the keep flags, k_iso_wpack); then the hull and the emit of the unweighted fit in their
+// weighted forms.
+static int isotonic_weighted_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *n_points_out, double *x_out,
+                                  double *y_out, double *wrows_out, double *wpos_out, int64_t *info_out, double *wsums_out,
+                                  const char *fn) {
+  const int64_t n = rows.n;
+  int64_t words[DSGD_METRICS_WORDS], m = 0;
+  double wc[DSGD_WCURVE_WORDS];
+  sorted_runs s;
+  int rc = curve_pass<kSampleWeighted>(ctx, w, rows, words, wc, &m, nullptr, nullptr, nullptr, fn, true, &s);
+  if (rc) return rc;
+  // the totals of the two runs, exact: W+ and W- of the non-NaN rows
+  limb_sum tot[2] = {{{0, 0, 0, 0, 0, 0}, 0}, {{0, 0, 0, 0, 0, 0}, 0}};
+  if (s.n_pos) CU(cudaMemcpyAsync(&tot[0], ctx->c_pre.p + s.n_pos - 1, sizeof(limb_sum), cudaMemcpyDeviceToHost, ctx->stream));
+  if (s.n_neg)
+    CU(cudaMemcpyAsync(&tot[1], ctx->c_pre.p + s.n_pos + s.n_neg - 1, sizeof(limb_sum), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  unsigned long long q[kLossLimbs];
+  for (int k = 0; k < kLossLimbs; ++k) q[k] = tot[0].l[k] + tot[1].l[k];
+  for (int k = 0; k < kLossLimbs - 1; ++k) {
+    q[k + 1] += q[k] >> 40;
+    q[k] &= kLimbMask;
+  }
+  NEED(tot[0].ovf == 0 && tot[1].ovf == 0 && q[kLossLimbs - 1] < (1ull << 56), DSGD_ERR_RANGE,
+       "%s: the rows' total weight is 2^96 or more (or a weight is 2^52 or more): the hull's turn test is exact below that",
+       fn);
+  wsums_out[0] = fixed_read(tot[0].l, 0);
+  wsums_out[1] = fixed_read(tot[1].l, 0);
+  bool any = false;
+  for (int k = 0; k < kLossLimbs; ++k) any |= q[k] != 0;
+  NEED(any, DSGD_ERR_EMPTY, "%s: no row with a non-NaN score has a positive weight (%lld rows, %lld NaN)", fn,
+       (long long)n, (long long)words[kMetNan]);
+  if ((rc = ctx->i_hull.grow(ctx, 5 * (n + 1), 1024)) || (rc = ctx->i_out.grow(ctx, 2 * n, 1024)) ||
+      (rc = ctx->i_wblk.grow(ctx, 2 * n, 1024)) || (rc = ctx->i_ctl.grow(ctx, 4, 4)) || (rc = ctx->i_wpt.grow(ctx, 4 * n, 1024)) ||
+      (rc = ctx->i_wkeep.grow(ctx, 2 * n, 1024)) || (rc = ctx->i_wthr.grow(ctx, n, 1024)))
+    return rc;
+  CU(cudaMemsetAsync(ctx->i_ctl, 0, sizeof(unsigned long long) * 4, ctx->stream));
+  u256 *px = ctx->i_wpt.p, *py = px + n, *qx = px + 2 * n, *qy = px + 3 * n;
+  int *keep = ctx->i_wkeep.p, *kexcl = keep + n;
+  k_iso_wpoint<<<isotonic_grid(ctx, cdiv(std::max<int64_t>(m, s.n_pos + s.n_neg), 256)), 256, 0, ctx->stream>>>(
+      ctx->c_thr, m, s.pos, s.n_pos, s.neg, s.n_neg, ctx->c_pre.p, ctx->c_pre.p + s.n_pos, s.pos_c, s.neg_c, px, py, keep,
+      ctx->i_ctl + 1);
+  LAUNCHED();
+  size_t tmp = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp, keep, kexcl, (int)m, ctx->stream));
+  if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+  CU(cub::DeviceScan::ExclusiveSum(ctx->m_tmp.p, tmp, keep, kexcl, (int)m, ctx->stream));
+  k_iso_wpack<<<isotonic_grid(ctx, cdiv(m, 256)), 256, 0, ctx->stream>>>(m, keep, kexcl, px, py, ctx->c_thr, qx, qy,
+                                                                        ctx->i_wthr, ctx->i_ctl + 2);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long ctl[4];
+  CU(cudaMemcpyAsync(ctl, ctx->i_ctl, sizeof ctl, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int64_t kept = (int64_t)ctl[2];
+  NEED(kept >= 1 && kept <= m, DSGD_ERR_CUDA, "%s: %lld points kept of %lld", fn, (long long)kept, (long long)m);
+  const int M = (int)kept + 1, S = isotonic_tile(), T = (M + S - 1) / S;
+  int *hv[2] = {ctx->i_hull.p, ctx->i_hull.p + M};
+  int *hc[2] = {ctx->i_hull.p + 2 * (int64_t)M, ctx->i_hull.p + 2 * (int64_t)M + T};
+  int *excl = ctx->i_hull.p + 2 * (int64_t)M + 2 * (int64_t)T;
+  const size_t tile_bytes = (size_t)S * (2 * sizeof(u256) + sizeof(int));
+  CU(cudaFuncSetAttribute(k_iso_wtile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_bytes));
+  k_iso_wtile<<<isotonic_grid(ctx, T), kIsoThreads, tile_bytes, ctx->stream>>>(qx, qy, M, S, hv[0], hc[0]);
+  LAUNCHED();
+  int cur = 0;
+  for (int64_t W = S, h = T; h > 1; W *= 2, h = (h + 1) / 2, cur ^= 1) {
+    k_iso_wmerge<<<isotonic_grid(ctx, (h + 1) / 2), kIsoThreads, 0, ctx->stream>>>(qx, qy, (int)h, (int)W, hv[cur], hc[cur],
+                                                                                   hv[cur ^ 1], hc[cur ^ 1]);
+    LAUNCHED();
+  }
+  CU(cudaGetLastError());
+  int V = 0;
+  CU(cudaMemcpyAsync(&V, hc[cur], sizeof V, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int B = V - 1;
+  NEED(B >= 1 && B <= kept, DSGD_ERR_CUDA, "%s: a hull of %d vertices over %lld points", fn, V, (long long)kept);
+  tmp = 0;
+  CU(scan_x_counts(ctx, nullptr, tmp, hv[cur], B, excl));
+  if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+  CU(scan_x_counts(ctx, ctx->m_tmp.p, tmp, hv[cur], B, excl));
+  double *X = ctx->i_out.p, *Y = ctx->i_out.p + n, *bw = ctx->i_wblk.p, *bp = ctx->i_wblk.p + n;
+  k_iso_wemit<<<isotonic_grid(ctx, cdiv(B, 256)), 256, 0, ctx->stream>>>(hv[cur], B, excl, ctx->i_wthr, qx, qy, X, Y, bw, bp,
+                                                                          ctx->i_ctl);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long nx = 0;
+  CU(cudaMemcpyAsync(&nx, ctx->i_ctl, sizeof nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(wrows_out, bw, sizeof(double) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(wpos_out, bp, sizeof(double) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  CU(cudaMemcpyAsync(x_out, X, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(y_out, Y, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  *n_points_out = (int64_t)nx;
+  info_out[0] = B;
+  info_out[1] = (int64_t)nx;
+  info_out[2] = (int64_t)ctl[1];
+  info_out[3] = words[kMetNan];
+  info_out[4] = kept;
+  return DSGD_OK;
+}
+
+#define ISO_W_ARGS_OK()                                                                                               \
+  do {                                                                                                                \
+    NEED(n_points_out && x_out && y_out && wrows_out && wpos_out && info_out && wsums_out, DSGD_ERR_INVALID,          \
+         "%s: an output is NULL", __func__);                                                                          \
+    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                            \
+    if (rc_) return rc_;                                                                                              \
+  } while (0)
+
+extern "C" int dsgd_calibrate_isotonic_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                int64_t *n_points_out, double *x_out, double *y_out, double *wrows_out,
+                                                double *wpos_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_W_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc
+            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
+                                     __func__);
+}
+
+extern "C" int dsgd_calibrate_isotonic_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                        uint64_t key, int64_t pos_begin, int64_t pos_end,
+                                                        int64_t *n_points_out, double *x_out, double *y_out,
+                                                        double *wrows_out, double *wpos_out, int64_t *info_out,
+                                                        double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_W_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc
+            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
+                                     __func__);
+}
+
+extern "C" int dsgd_calibrate_isotonic_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                        int64_t *n_points_out, double *x_out, double *y_out,
+                                                        double *wrows_out, double *wpos_out, int64_t *info_out,
+                                                        double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_W_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc
+            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
+                                     __func__);
+}
+
+#define ISO_WEVAL_ARGS_OK()                                                                                             \
+  do {                                                                                                                  \
+    NEED(sums_out && bin_weight && bin_pos_weight && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL",   \
+         __func__);                                                                                                     \
+    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
+    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
+    if (rc_) return rc_;                                                                                                \
+  } while (0)
+
+extern "C" int dsgd_eval_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                       const double *X, const double *Y, int64_t k, int32_t n_bins,
+                                                       double *sums_out, double *bin_weight, double *bin_pos_weight,
+                                                       double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_WEVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  return rc ? rc
+            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
+                                          bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_sampled_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin,
+                                                               int64_t row_end, uint64_t key, int64_t pos_begin,
+                                                               int64_t pos_end, const double *X, const double *Y, int64_t k,
+                                                               int32_t n_bins, double *sums_out, double *bin_weight,
+                                                               double *bin_pos_weight, double *bin_psum,
+                                                               int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_WEVAL_ARGS_OK();
+  row_set rows;
+  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
+  return rc ? rc
+            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
+                                          bin_psum, words_out, __func__);
+}
+
+extern "C" int dsgd_eval_samples_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples,
+                                                               int64_t n, const double *X, const double *Y, int64_t k,
+                                                               int32_t n_bins, double *sums_out, double *bin_weight,
+                                                               double *bin_pos_weight, double *bin_psum,
+                                                               int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  ISO_WEVAL_ARGS_OK();
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  return rc ? rc
+            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
+                                          bin_psum, words_out, __func__);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all

@@ -79,19 +79,31 @@ __global__ void __launch_bounds__(256) k_calib_prob(const uint32_t *__restrict__
 // ---- k_calib_score -----------------------------------------------------------------------------------------------
 enum CalibWord : int { kCalPos = 0, kCalNeg = 1, kCalNan = 2, kCalCntWords = 4 };
 
+// The weighted fit's three exact sums of R(c_i), each a kLossAccWords block: non-NaN positives, non-NaN negatives, NaN rows
+enum CalibWeightWord : int { kCalWPos = 0, kCalWNeg = kLossAccWords, kCalWNan = 2 * kLossAccWords, kCalWWords = 3 * kLossAccWords };
+
 // score[i] = x . w and lab[i] = the label of position i of the row set (samples == nullptr: rows [row_begin, row_begin + n)),
 // and the counts of non-NaN positives, non-NaN negatives and NaN rows.  A warp takes 32 consecutive positions at a time and
 // lane j keeps the j-th dot, as in k_metrics_score; the counts are flushed once per warp.
+// kW (the weighted fit, DESIGN.md §4.17): cw[i] = c_i = fl(w_y * s_i), the expression of k_metrics_score<kSampleWeighted>
+// (sw == nullptr: every s_i is 1), and R(c_i) added to the three CalibWeightWord sums at wacc; each warp adds its lanes'
+// carried limbs with shuffles (below 2^45 each) and flushes them once.
+template <bool kW>
 __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                      const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                      int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                      double *__restrict__ score, int8_t *__restrict__ lab,
-                                                     unsigned long long *__restrict__ cnt) {
+                                                     unsigned long long *__restrict__ cnt, double w_pos = 1.0,
+                                                     double w_neg = 1.0, const double *__restrict__ sw = nullptr,
+                                                     double *__restrict__ cw = nullptr,
+                                                     unsigned long long *__restrict__ wacc = nullptr) {
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned c_pos = 0, c_neg = 0, c_nan = 0;
+  unsigned long long l_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, l_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0};
+  unsigned long long l_nan[kLossLimbs] = {0, 0, 0, 0, 0, 0}, o_pos = 0, o_neg = 0, o_nan = 0;
   for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
     const int64_t i = g + lane;
     const bool mine = i < n;
@@ -110,11 +122,37 @@ __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict_
       c_nan += nan;
       c_pos += pos && !nan;
       c_neg += !pos && !nan;
+      if constexpr (kW) {
+        const double ci = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r_own]) : 1.0);
+        cw[i] = ci;
+        if (nan) acc_add_local(l_nan, o_nan, ci);
+        else if (pos) acc_add_local(l_pos, o_pos, ci);
+        else acc_add_local(l_neg, o_neg, ci);
+      }
     }
   }
   c_pos = __reduce_add_sync(full, c_pos);
   c_neg = __reduce_add_sync(full, c_neg);
   c_nan = __reduce_add_sync(full, c_nan);
+  if constexpr (kW) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      o_pos += __shfl_xor_sync(full, o_pos, o);
+      o_neg += __shfl_xor_sync(full, o_neg, o);
+      o_nan += __shfl_xor_sync(full, o_nan, o);
+#pragma unroll
+      for (int k = 0; k < kLossLimbs; ++k) {
+        l_pos[k] += __shfl_xor_sync(full, l_pos[k], o);
+        l_neg[k] += __shfl_xor_sync(full, l_neg[k], o);
+        l_nan[k] += __shfl_xor_sync(full, l_nan[k], o);
+      }
+    }
+    if (lane == 0) {
+      acc_flush_local(wacc + kCalWPos, l_pos, o_pos);
+      acc_flush_local(wacc + kCalWNeg, l_neg, o_neg);
+      acc_flush_local(wacc + kCalWNan, l_nan, o_nan);
+    }
+  }
   if (lane == 0) {
     if (c_pos) atomicAdd(&cnt[kCalPos], (unsigned long long)c_pos);
     if (c_neg) atomicAdd(&cnt[kCalNeg], (unsigned long long)c_neg);
@@ -142,6 +180,7 @@ struct CalibFitParams {
   long long timeout_cycles;
   unsigned long long *out;    // CalibOut words (A, B, F as the bits of doubles)
   int smem_cap;               // scores a CTA keeps in shared memory; the rest of its slice stays in global memory
+  const double *cw;           // the weighted fit: n row weights c_i beside the scores (nullptr in the unweighted one)
 };
 
 __device__ __forceinline__ unsigned long long ld_relaxed_gpu_u64(const unsigned long long *p) {
@@ -167,6 +206,8 @@ __device__ __forceinline__ void st_relaxed_gpu_u64(unsigned long long *p, unsign
 // The three lines rotate: evaluation e uses line e % 3.  After barrier e every CTA has finished reading line e - 1 (it read
 // it before it arrived), so block 0 zeroes that line then, for evaluation e + 2; its arrival at barrier e + 1 (release)
 // orders the zeroes before any CTA's REDs of evaluation e + 2.
+// k_calib_fit_w below is this kernel line for line but for its weighted lines: a change here belongs there too
+// (tests/test_calib_fit_twins.py holds the two bodies equal apart from those lines).
 __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit(const CalibFitParams p) {
   extern __shared__ __align__(16) unsigned char cal_smem[];
   double *s_f = reinterpret_cast<double *>(cal_smem);
@@ -229,6 +270,171 @@ __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit(const CalibFitPara
       cal_add(lim[3], ovf, (f * f) * d2);
       cal_add(lim[4], ovf, f * d2);
       cal_add(lim[5], ovf, d2);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      ovf += __shfl_xor_sync(full, ovf, o);
+#pragma unroll
+      for (int s = 0; s < kCalSums; ++s)
+#pragma unroll
+        for (int k = 0; k < kLossLimbs; ++k) lim[s][k] += __shfl_xor_sync(full, lim[s][k], o);   // below 2^45: no carry lost
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int s = 0; s < kCalSums; ++s)
+#pragma unroll
+        for (int k = 0; k < kLossLimbs; ++k)
+          if (lim[s][k]) atomicAdd(&s_red[s * kLossLimbs + k], (unsigned long long)lim[s][k]);
+      if (ovf) atomicAdd(&s_red[kCalLineWords - 1], ovf);
+    }
+    __syncthreads();
+    unsigned long long *line = p.acc + (ev % 3u) * kCalLineStride;
+    if (tid < kCalLineWords) {
+      const unsigned long long v = s_red[tid];
+      if (v) red_add_u64(line + tid, v);
+      s_red[tid] = 0ull;
+    }
+    __syncthreads();
+    if (tid == 0 && !grid_barrier_arrive_wait(p.bar, (ev + 1u) * (unsigned)G, p.abort_flag, p.timeout_cycles)) s_done = -1;
+    __syncthreads();
+    if (s_done < 0) return;
+    if (tid < kCalLineWords) {
+      s_line[tid] = ld_relaxed_gpu_u64(line + tid);
+      if (blockIdx.x == 0) st_relaxed_gpu_u64(p.acc + ((ev + 2u) % 3u) * kCalLineStride + tid, 0ull);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      double S[kCalSums];
+      bool finite = s_line[kCalLineWords - 1] == 0ull;
+#pragma unroll
+      for (int s = 0; s < kCalSums; ++s) S[s] = cal_value(s_line + s * kLossLimbs);
+      bool accept = false, done = false;
+      if (!finite) {
+        status = kCalNonFinite;
+        A = B = F = __longlong_as_double(0x7ff8000000000000ll);
+        done = true;
+      } else if (ev == 0) {
+        accept = true;
+      } else if (S[0] < F + 1e-4 * step * gd) {
+        accept = true;
+        ++iter;
+      } else {
+        step = step / 2.0;
+        if (step < 1e-10) {
+          status = kCalLineSearch;
+          done = true;
+        }
+      }
+      if (accept) {
+        A = pa; B = pb; F = S[0];
+        const double g1 = S[1], g2 = S[2], h11 = S[3] + 1e-12, h21 = S[4], h22 = S[5] + 1e-12;
+        if (fabs(g1) < 1e-5 && fabs(g2) < 1e-5) {
+          status = kCalConverged;
+          done = true;
+        } else if (iter >= kCalMaxIter) {
+          status = kCalIterLimit;
+          done = true;
+        } else {
+          const double det = h11 * h22 - h21 * h21;
+          dA = -(h22 * g1 - h21 * g2) / det;
+          dB = -(h11 * g2 - h21 * g1) / det;
+          gd = g1 * dA + g2 * dB;
+          step = 1.0;
+        }
+      }
+      if (done) {
+        s_done = 1;
+      } else {
+        s_pt[0] = A + step * dA;
+        s_pt[1] = B + step * dB;
+      }
+    }
+    __syncthreads();
+    if (s_done) {
+      if (blockIdx.x == 0 && tid == 0) {
+        p.out[kCalOutA] = (unsigned long long)__double_as_longlong(A);
+        p.out[kCalOutB] = (unsigned long long)__double_as_longlong(B);
+        p.out[kCalOutF] = (unsigned long long)__double_as_longlong(F);
+        p.out[kCalOutIter] = (unsigned long long)iter;
+        p.out[kCalOutStatus] = (unsigned long long)status;
+        p.out[kCalOutEvals] = (unsigned long long)ev + 1ull;
+      }
+      return;
+    }
+  }
+}
+
+// k_calib_fit_w: the weighted fit (DESIGN.md §4.17), k_calib_fit line for line but for three things.  A CTA keeps f, c and y
+// of each score in shared memory (17 bytes instead of 9, so its cap is smaller); a row with R(c) = 0 is skipped before any
+// term is formed; and each of the six terms is added as R(fl(c term)).  The weights change only what a CTA adds to the
+// line, never what it reads from it, so the invariant above holds unchanged.  (A separate kernel rather than a template
+// form: every template form of k_calib_fit compiled its unweighted instructions differently.)
+__global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitParams p) {
+  extern __shared__ __align__(16) unsigned char cal_smem[];
+  double *s_f = reinterpret_cast<double *>(cal_smem);
+  double *s_c = s_f + p.smem_cap;
+  int8_t *s_y = reinterpret_cast<int8_t *>(s_c + p.smem_cap);
+  __shared__ unsigned long long s_red[kCalLineWords];    // the CTA's partial of one evaluation
+  __shared__ unsigned long long s_line[kCalLineWords];   // the accumulator line as read after the barrier
+  __shared__ double s_pt[2];                             // the point to evaluate next
+  __shared__ int s_done;                                 // 1: the fit ended; -1: the watchdog fired
+
+  const unsigned full = 0xffffffffu;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int64_t G = gridDim.x, slice = (p.n + G - 1) / G;
+  const int64_t b = min(p.n, (int64_t)blockIdx.x * slice), e = min(p.n, b + slice);
+  const int m = (int)(e - b), in_smem = min(m, p.smem_cap);
+  for (int i = tid; i < in_smem; i += kCalThreads) {
+    s_f[i] = p.score[b + i];
+    s_c[i] = p.cw[b + i];
+    s_y[i] = p.lab[b + i];
+  }
+  if (tid < kCalLineWords) s_red[tid] = 0ull;
+  if (tid == 0) {
+    s_pt[0] = 0.0;
+    s_pt[1] = p.b0;
+    s_done = 0;
+  }
+  __syncthreads();
+
+  // thread 0's state: the accepted point, its objective, the Newton direction from it and the line search's step
+  double A = 0.0, B = 0.0, F = 0.0, dA = 0.0, dB = 0.0, gd = 0.0, step = 1.0;
+  int iter = 0, status = kCalConverged;
+  for (unsigned ev = 0;; ++ev) {
+    const double pa = s_pt[0], pb = s_pt[1];
+    long long lim[kCalSums][kLossLimbs];
+#pragma unroll
+    for (int s = 0; s < kCalSums; ++s)
+#pragma unroll
+      for (int k = 0; k < kLossLimbs; ++k) lim[s][k] = 0;
+    unsigned long long ovf = 0;
+    for (int i = tid; i < m; i += kCalThreads) {
+      const double f = i < in_smem ? s_f[i] : __ldcg(p.score + b + i);
+      const int8_t y = i < in_smem ? s_y[i] : __ldcg(p.lab + b + i);
+      if (isnan(f)) continue;
+      const double c = i < in_smem ? s_c[i] : __ldcg(p.cw + b + i);
+      if (rint(c * 0x1p160) == 0.0) continue;   // R(c) = 0: the row adds exactly 0 to every sum
+      const double t = y > 0 ? p.t_pos : p.t_neg;
+      const double z = pa * f + pb;
+      double term, pr, qr;   // pr = 1 / (1 + exp(z)) = P(y = +1), qr = 1 - pr, each from the half that does not cancel
+      if (z >= 0.0) {
+        const double ex = exp(-z), den = 1.0 + ex;
+        term = t * z + log1p(ex);
+        pr = ex / den;
+        qr = 1.0 / den;
+      } else {
+        const double ex = exp(z), den = 1.0 + ex;
+        term = (t - 1.0) * z + log1p(ex);
+        pr = 1.0 / den;
+        qr = ex / den;
+      }
+      const double d1 = t - pr, d2 = pr * qr;
+      cal_add(lim[0], ovf, c * term);
+      cal_add(lim[1], ovf, c * (f * d1));
+      cal_add(lim[2], ovf, c * d1);
+      cal_add(lim[3], ovf, c * ((f * f) * d2));
+      cal_add(lim[4], ovf, c * (f * d2));
+      cal_add(lim[5], ovf, c * d2);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

@@ -318,4 +318,384 @@ __global__ void __launch_bounds__(256) k_iso_eval(const uint32_t *__restrict__ r
   }
 }
 
+// ---- the weighted fit (dsgd_calibrate_isotonic_weighted*; DESIGN.md §4.17) ----------------------------------------------
+// A point's coordinates are the exact sums X = W(>= t) and Y = W+(>= t) of the weighted curve pass, integers in units of
+// 2^-160 held in four u64 words (u256).  The hull needs them below 2^256, i.e. a total weight below 2^96; the host refuses
+// more before the hull.  After the zero-weight points are dropped X strictly increases and Y does not decrease along the
+// points, so every difference the turn test forms is >= 0 and the cross product is the comparison of two unsigned 512-bit
+// products: exact.
+struct u256 { unsigned long long w[4]; };
+__device__ __forceinline__ u256 u256_sub(const u256 &a, const u256 &b) {   // a - b, a >= b
+  u256 r;
+  unsigned long long borrow = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const unsigned long long d = a.w[i] - b.w[i], d2 = d - borrow;
+    borrow = (a.w[i] < b.w[i]) | (d < borrow);
+    r.w[i] = d2;
+  }
+  return r;
+}
+__device__ __forceinline__ bool u256_eq(const u256 &a, const u256 &b) {
+  return a.w[0] == b.w[0] && a.w[1] == b.w[1] && a.w[2] == b.w[2] && a.w[3] == b.w[3];
+}
+// a * b as eight words, least significant first
+__device__ __forceinline__ void u256_mul(const u256 &a, const u256 &b, unsigned long long (&r)[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) r[i] = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    unsigned long long carry = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const unsigned long long lo = a.w[i] * b.w[j], hi = __umul64hi(a.w[i], b.w[j]);
+      const unsigned long long s1 = r[i + j] + lo, c1 = s1 < lo;
+      const unsigned long long s2 = s1 + carry, c2 = s2 < carry;
+      r[i + j] = s2;
+      carry = hi + c1 + c2;   // below 2^64: hi <= 2^64 - 2
+    }
+    r[i + 4] = carry;
+  }
+}
+// The sign of (a - o) x (b - o) for points o, a, b in increasing order along the curve: +1 when b lies strictly above the
+// line from o through a, 0 when the three are collinear, -1 below.
+__device__ __forceinline__ int iso_wturn(const u256 &ox, const u256 &oy, const u256 &ax, const u256 &ay, const u256 &bx,
+                                         const u256 &by) {
+  unsigned long long p[8], q[8];
+  u256_mul(u256_sub(ax, ox), u256_sub(by, oy), p);
+  u256_mul(u256_sub(ay, oy), u256_sub(bx, ox), q);
+#pragma unroll
+  for (int i = 7; i >= 0; --i)
+    if (p[i] != q[i]) return p[i] > q[i] ? 1 : -1;
+  return 0;
+}
+// read() of an exact sum given as a u256 in units of 2^-160: its six 40-bit limbs converted as acc_value converts them
+__device__ __forceinline__ double u256_read(const u256 &v) {
+  unsigned long long q[kLossAccWords];
+#pragma unroll
+  for (int k = 0; k < kLossLimbs - 1; ++k) {
+    const int b = 40 * k, wi = b >> 6, sh = b & 63;
+    unsigned long long x = v.w[wi] >> sh;
+    if (sh > 24 && wi < 3) x |= v.w[wi + 1] << (64 - sh);
+    q[k] = x & kLimbMask;
+  }
+  q[kLossLimbs - 1] = (v.w[3] >> 8);   // bits 200 .. 255
+  q[kLossLimbs] = 0;
+  return acc_value(q);
+}
+// A canonical non-negative limb_sum as a u256 (limbs 0..4 in [0, 2^40), limb 5 below 2^56)
+__device__ __forceinline__ u256 u256_of(limb_sum v) {
+#pragma unroll
+  for (int k = 0; k < kLossLimbs - 1; ++k) {
+    v.l[k + 1] += (unsigned long long)((long long)v.l[k] >> 40);
+    v.l[k] &= kLimbMask;
+  }
+  u256 r = {{0, 0, 0, 0}};
+#pragma unroll
+  for (int k = 0; k < kLossLimbs; ++k) {
+    const int b = 40 * k, wi = b >> 6, sh = b & 63;
+    r.w[wi] |= v.l[k] << sh;
+    if (sh > 24 && wi < 3) r.w[wi + 1] |= v.l[k] >> (64 - sh);
+  }
+  return r;
+}
+
+// Point k of the weighted curve pass (thr[k], highest score first): X_k and Y_k from the runs' prefix sums, and keep[k] = 1
+// when its weight increment X_k - X_(k-1) is not zero (X_(-1) = 0).  Also counts the rows of positive weight (R(c) > 0)
+// among the runs' keys into *n_wrows.
+__global__ void __launch_bounds__(256) k_iso_wpoint(const double *__restrict__ thr, int64_t m,
+                                                    const unsigned long long *__restrict__ pos, int64_t n_pos,
+                                                    const unsigned long long *__restrict__ neg, int64_t n_neg,
+                                                    const limb_sum *__restrict__ pre_pos, const limb_sum *__restrict__ pre_neg,
+                                                    const double *__restrict__ pos_c, const double *__restrict__ neg_c,
+                                                    u256 *__restrict__ px, u256 *__restrict__ py, int *__restrict__ keep,
+                                                    unsigned long long *__restrict__ n_wrows) {
+  const limb_sum p_all = limb_prefix(pre_pos, n_pos), n_all = limb_prefix(pre_neg, n_neg);
+  auto at = [&](int64_t k, u256 &x, u256 &y) {
+    const unsigned long long key = score_key(thr[k]);
+    const limb_sum p = limb_add(p_all, limb_prefix(pre_pos, key_lower_bound(pos, n_pos, key)), true);
+    const limb_sum q = limb_add(n_all, limb_prefix(pre_neg, key_lower_bound(neg, n_neg, key)), true);
+    y = u256_of(p);
+    x = u256_of(limb_add(p, q));
+  };
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += stride) {
+    u256 x, y, x0 = {{0, 0, 0, 0}}, y0;
+    at(k, x, y);
+    if (k > 0) at(k - 1, x0, y0);
+    px[k] = x;
+    py[k] = y;
+    keep[k] = !u256_eq(x, x0);
+  }
+  unsigned long long c = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pos + n_neg; i += stride) {
+    const double ci = i < n_pos ? pos_c[i] : neg_c[i - n_pos];
+    c += rint(ci * 0x1p160) != 0.0;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(n_wrows, c);
+}
+// The kept points packed: point excl[k] of (qx, qy, qthr) is point k; the last thread writes the kept count
+__global__ void __launch_bounds__(256) k_iso_wpack(int64_t m, const int *__restrict__ keep, const int *__restrict__ excl,
+                                                   const u256 *__restrict__ px, const u256 *__restrict__ py,
+                                                   const double *__restrict__ thr, u256 *__restrict__ qx,
+                                                   u256 *__restrict__ qy, double *__restrict__ qthr,
+                                                   unsigned long long *__restrict__ n_kept) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+    if (keep[k]) {
+      const int j = excl[k];
+      qx[j] = px[k];
+      qy[j] = py[k];
+      qthr[j] = thr[k];
+    }
+    if (k == m - 1) *n_kept = (unsigned long long)(excl[k] + keep[k]);
+  }
+}
+// Hull point i: the origin, or kept point i - 1
+__device__ __forceinline__ void iso_wpt(const u256 *__restrict__ qx, const u256 *__restrict__ qy, int i, u256 &x, u256 &y) {
+  if (i == 0) { x = u256{{0, 0, 0, 0}}; y = x; return; }
+  x = qx[i - 1];
+  y = qy[i - 1];
+}
+// k_iso_tile over the weighted points: the same monotone chain with the exact multi-word turn test; 68 bytes a point
+__global__ void __launch_bounds__(kIsoThreads) k_iso_wtile(const u256 *__restrict__ qx, const u256 *__restrict__ qy, int M,
+                                                           int S, int *__restrict__ hv, int *__restrict__ hc) {
+  extern __shared__ __align__(16) unsigned char iso_wsmem[];
+  u256 *sx = reinterpret_cast<u256 *>(iso_wsmem), *sy = sx + S;
+  int *st = reinterpret_cast<int *>(sy + S);
+  __shared__ int s_top;
+  const int T = (M + S - 1) / S;
+  for (int t = blockIdx.x; t < T; t += gridDim.x) {
+    const int b = t * S, len = min(S, M - b);
+    for (int j = threadIdx.x; j < len; j += blockDim.x) iso_wpt(qx, qy, b + j, sx[j], sy[j]);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int top = 0;
+      for (int j = 0; j < len; ++j) {
+        while (top >= 2 && iso_wturn(sx[st[top - 2]], sy[st[top - 2]], sx[st[top - 1]], sy[st[top - 1]], sx[j], sy[j]) >= 0)
+          --top;
+        st[top++] = j;
+      }
+      s_top = top;
+      hc[t] = top;
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < s_top; j += blockDim.x) hv[b + j] = b + st[j];
+    __syncthreads();
+  }
+}
+// k_iso_merge over the weighted points: the same bridge search with the exact turn test
+__global__ void __launch_bounds__(kIsoThreads) k_iso_wmerge(const u256 *__restrict__ qx, const u256 *__restrict__ qy,
+                                                            int n_hulls, int W, const int *__restrict__ hv_in,
+                                                            const int *__restrict__ hc_in, int *__restrict__ hv_out,
+                                                            int *__restrict__ hc_out) {
+  __shared__ int s_br[2];
+  const int pairs = (n_hulls + 1) / 2;
+  for (int p = blockIdx.x; p < pairs; p += gridDim.x) {
+    const int *L = hv_in + (int64_t)2 * p * W;
+    const int a = hc_in[2 * p];
+    const bool single = 2 * p + 1 >= n_hulls;
+    const int *R = L + W;
+    const int b = single ? 0 : hc_in[2 * p + 1];
+    if (threadIdx.x == 0) {
+      int i_end = a - 1, j_end = 0;
+      if (!single) {
+        auto tangent = [&](const u256 &vx, const u256 &vy) {
+          int lo = 0, hi = b - 1;
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            u256 x0, y0, x1, y1;
+            iso_wpt(qx, qy, R[mid], x0, y0);
+            iso_wpt(qx, qy, R[mid + 1], x1, y1);
+            if (iso_wturn(vx, vy, x0, y0, x1, y1) >= 0) lo = mid + 1; else hi = mid;
+          }
+          return lo;
+        };
+        int lo = 0, hi = a - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          u256 vx, vy, ux, uy, rx, ry;
+          iso_wpt(qx, qy, L[mid], vx, vy);
+          iso_wpt(qx, qy, L[mid + 1], ux, uy);
+          iso_wpt(qx, qy, R[tangent(vx, vy)], rx, ry);
+          // u strictly above the line v -> r (k_iso_merge's iso_cross(v, r, u) > 0); u comes before r along the curve
+          if (iso_wturn(vx, vy, ux, uy, rx, ry) < 0) lo = mid + 1; else hi = mid;
+        }
+        u256 vx, vy;
+        iso_wpt(qx, qy, L[lo], vx, vy);
+        i_end = lo;
+        j_end = tangent(vx, vy);
+      }
+      s_br[0] = i_end;
+      s_br[1] = j_end;
+      hc_out[p] = i_end + 1 + (single ? 0 : b - j_end);
+    }
+    __syncthreads();
+    const int i_end = s_br[0], j_end = s_br[1];
+    int *out = hv_out + (int64_t)2 * p * W;
+    for (int k = threadIdx.x; k <= i_end; k += blockDim.x) out[k] = L[k];
+    if (!single)
+      for (int k = threadIdx.x; k < b - j_end; k += blockDim.x) out[i_end + 1 + k] = R[j_end + k];
+    __syncthreads();
+  }
+}
+// k_iso_emit over the weighted points: X, Y and each block's weight and positive weight, read() of exact differences;
+// p = fl(read(dY) / read(dX))
+__global__ void __launch_bounds__(256) k_iso_wemit(const int *__restrict__ h, int B, const int *__restrict__ excl,
+                                                   const double *__restrict__ thr, const u256 *__restrict__ qx,
+                                                   const u256 *__restrict__ qy, double *__restrict__ X,
+                                                   double *__restrict__ Y, double *__restrict__ blk_w,
+                                                   double *__restrict__ blk_pw, unsigned long long *__restrict__ n_x) {
+  for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < B; o += gridDim.x * blockDim.x) {
+    const int b = B - 1 - o, i0 = h[b], i1 = h[b + 1];
+    u256 x0, y0, x1, y1;
+    iso_wpt(qx, qy, i0, x0, y0);
+    iso_wpt(qx, qy, i1, x1, y1);
+    const double wr = u256_read(u256_sub(x1, x0)), wp = u256_read(u256_sub(y1, y0));
+    const double p = wp / wr;
+    blk_w[o] = wr;
+    blk_pw[o] = wp;
+    const int at = excl[o];
+    const bool two = i1 - i0 >= 2;
+    X[at] = thr[i1 - 1];
+    Y[at] = p;
+    if (two) {
+      X[at + 1] = thr[i0];
+      Y[at + 1] = p;
+    }
+    if (o == B - 1) *n_x = (unsigned long long)(at + 1 + two);
+  }
+}
+
+// ---- the weighted quality pass (dsgd_eval_*weighted_calibration, dsgd_eval_*weighted_isotonic_calibration) -----------
+// kIso: p = interp(s) at the map (X, Y) and the log-loss term -log p or -log1p(-p), as k_iso_eval; else p = sigmoid(-z),
+// z = a f + b, and the term softplus(+-z), as k_calib_eval.  c_i = fl(w_y * s_i) as in k_calib_score<true>.  A row with
+// R(c) = 0 is counted in kCwvRows and adds nothing else.  The sums add R(fl(c (p - o)^2)), R(fl(c l)) over the finite
+// terms, R(c) over the rows used and R(c) over the rows whose term is infinite (counted in kCwvInf too); bin k adds R(c),
+// R(c) of the positives and R(fl(c p)) to its three limb blocks in shared memory.  A bin value of 2^52 or more is counted
+// in the bin's overflow word; the integer part of a value is split at 2^40 between limbs 4 and 5, so every shared word
+// grows by at most 2^40 per row, as in the unweighted bins.  The host reads every sum with read().
+enum CalibWEvalWord : int {
+  kCwvBrier = 0,                                   // [0, 7): limbs and overflow count of sum R(c (p - o)^2)
+  kCwvLog = kLossAccWords,                         // [7, 14): of sum R(c l), finite terms
+  kCwvW = 2 * kLossAccWords,                       // [14, 21): of sum R(c) over the rows used
+  kCwvInfW = 3 * kLossAccWords,                    // [21, 28): of sum R(c) over the rows whose term is infinite
+  kCwvRows = 4 * kLossAccWords,                    // rows used
+  kCwvNan = kCwvRows + 1,                          // rows left out
+  kCwvInf = kCwvRows + 2,                          // rows of positive weight whose term is infinite
+  kCwvBins = 32,                                   // per bin: kCwvBinStride words {weight, positive weight, sum c p, overflow}
+  kCwvBinStride = 3 * kLossLimbs + 1,
+  kCwvWords = kCwvBins + kCalMaxBins * kCwvBinStride
+};
+// v >= 0 into a bin's limb block in shared memory (limbs 0..5), its overflow counted at *ovf
+__device__ __forceinline__ void cal_bin_add(unsigned long long *lim, unsigned long long *ovf, double v) {
+  if (!(v < 4503599627370496.0)) { atomicAdd(ovf, 1ull); return; }
+  acc_cut(v, [&](int k, double limb) {
+    if (limb == 0.0) return;
+    const unsigned long long u = (unsigned long long)(long long)limb;
+    if (k == kLossLimbs - 2) {
+      if (u & kLimbMask) atomicAdd(&lim[k], u & kLimbMask);
+      if (u >> 40) atomicAdd(&lim[k + 1], u >> 40);
+    } else {
+      atomicAdd(&lim[k], u);
+    }
+  });
+}
+template <bool kIso, bool kSmem>
+__global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                               const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                               int64_t row_begin, int64_t n, const double *__restrict__ w, double a, double b,
+                                               const double *__restrict__ X, const double *__restrict__ Y, int k, int n_bins,
+                                               unsigned long long *__restrict__ blk, double w_pos, double w_neg,
+                                               const double *__restrict__ sw) {
+  __shared__ unsigned long long s_bins[kCalMaxBins * kCwvBinStride];
+  const double *xs = nullptr, *ys = nullptr;
+  if constexpr (kIso) iso_stage<kSmem>(X, Y, k, xs, ys);
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < kCalMaxBins * kCwvBinStride; i += blockDim.x) s_bins[i] = 0ull;
+  __syncthreads();
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned long long lb[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ll[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_b = 0, ovf_l = 0;
+  unsigned long long lw[kLossLimbs] = {0, 0, 0, 0, 0, 0}, li[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0, ovf_i = 0;
+  unsigned c_rows = 0, c_nan = 0, c_inf = 0;
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i = g + lane;
+    const bool mine = i < n;
+    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    double dot_own = 0.0;
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const double dot = row_margin(rp16, pairs, w, r, lane);
+      if (lane == j) dot_own = dot;
+    }
+    if (!mine) continue;
+    const double z = kIso ? -dot_own : a * dot_own + b;   // kIso: the score s
+    if (isnan(z)) { ++c_nan; continue; }
+    ++c_rows;
+    const bool pos = label[r_own] > 0;
+    const double c = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r_own]) : 1.0);
+    if (rint(c * 0x1p160) == 0.0) continue;   // R(c) = 0: the row adds exactly 0 to every sum
+    const double pr = kIso ? iso_interp(z, xs, ys, k) : sigmoid(-z), o = pos ? 1.0 : 0.0, dlt = pr - o;
+    const double term = kIso ? (pos ? -log(pr) : -log1p(-pr)) : softplus(pos ? z : -z);
+    acc_add_local(lb, ovf_b, c * (dlt * dlt));
+    if (kIso && isinf(term)) {
+      ++c_inf;
+      acc_add_local(li, ovf_i, c);
+    } else {
+      acc_add_local(ll, ovf_l, c * term);
+    }
+    acc_add_local(lw, ovf_w, c);
+    int bin = (int)floor(pr * (double)n_bins);
+    bin = bin < n_bins - 1 ? bin : n_bins - 1;
+    unsigned long long *bl = s_bins + bin * kCwvBinStride, *bo = bl + 3 * kLossLimbs;
+    cal_bin_add(bl, bo, c);
+    if (pos) cal_bin_add(bl + kLossLimbs, bo, c);
+    cal_bin_add(bl + 2 * kLossLimbs, bo, c * pr);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ovf_b += __shfl_xor_sync(full, ovf_b, o);
+    ovf_l += __shfl_xor_sync(full, ovf_l, o);
+    ovf_w += __shfl_xor_sync(full, ovf_w, o);
+    ovf_i += __shfl_xor_sync(full, ovf_i, o);
+#pragma unroll
+    for (int q = 0; q < kLossLimbs; ++q) {
+      lb[q] += __shfl_xor_sync(full, lb[q], o);
+      ll[q] += __shfl_xor_sync(full, ll[q], o);
+      lw[q] += __shfl_xor_sync(full, lw[q], o);
+      li[q] += __shfl_xor_sync(full, li[q], o);
+    }
+  }
+  c_rows = __reduce_add_sync(full, c_rows);
+  c_nan = __reduce_add_sync(full, c_nan);
+  c_inf = __reduce_add_sync(full, c_inf);
+  if (lane == 0) {
+    acc_flush_local(blk + kCwvBrier, lb, ovf_b);
+    acc_flush_local(blk + kCwvLog, ll, ovf_l);
+    acc_flush_local(blk + kCwvW, lw, ovf_w);
+    acc_flush_local(blk + kCwvInfW, li, ovf_i);
+    if (c_rows) atomicAdd(&blk[kCwvRows], (unsigned long long)c_rows);
+    if (c_nan) atomicAdd(&blk[kCwvNan], (unsigned long long)c_nan);
+    if (c_inf) atomicAdd(&blk[kCwvInf], (unsigned long long)c_inf);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n_bins * 3; i += blockDim.x) {
+    const int bin = i / 3, s = i % 3;
+    unsigned long long q[kLossLimbs];
+#pragma unroll
+    for (int t = 0; t < kLossLimbs; ++t) q[t] = s_bins[bin * kCwvBinStride + s * kLossLimbs + t];
+    acc_carry(q);
+    unsigned long long *dst = blk + kCwvBins + bin * kCwvBinStride;
+#pragma unroll
+    for (int t = 0; t < kLossLimbs; ++t)
+      if (q[t]) red_add_u64(dst + s * kLossLimbs + t, q[t]);
+    const unsigned long long ov = s_bins[bin * kCwvBinStride + 3 * kLossLimbs];
+    if (s == 0 && ov) red_add_u64(dst + 3 * kLossLimbs, ov);
+  }
+}
+
 }  // namespace dsgd

@@ -87,6 +87,26 @@ object DsgdNative {
   @native def evalSamplesCalibration(ctx: Long, w: Array[Double], samples: Array[Int], a: Double, b: Double, nBins: Int,
                                      sums: Array[Double], binRows: Array[Long], binPos: Array[Long], binPsum: Array[Double],
                                      words: Array[Long]): Int
+  // weighted calibration (every row counted by its weight c_i): the calls above with wsums(0..2) = W+, W- and the NaN rows'
+  // weight added to a fit; weighted quality: sums(0..3) = Brier and log-loss sums, weight used, infinite-term weight (0),
+  // binWeight / binPosWeight / binPsum(0 until nBins), words(0..1) = rows used and left out.
+  @native def calibrateWeighted(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, ab: Array[Double],
+                                objective: Array[Double], info: Array[Long], wsums: Array[Double]): Int
+  @native def calibrateWeightedSampled(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                       posEnd: Long, ab: Array[Double], objective: Array[Double], info: Array[Long],
+                                       wsums: Array[Double]): Int
+  @native def calibrateWeightedSamples(ctx: Long, w: Array[Double], samples: Array[Int], ab: Array[Double],
+                                       objective: Array[Double], info: Array[Long], wsums: Array[Double]): Int
+  @native def evalWeightedCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, a: Double, b: Double,
+                                      nBins: Int, sums: Array[Double], binWeight: Array[Double],
+                                      binPosWeight: Array[Double], binPsum: Array[Double], words: Array[Long]): Int
+  @native def evalSampledWeightedCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long,
+                                             posBegin: Long, posEnd: Long, a: Double, b: Double, nBins: Int,
+                                             sums: Array[Double], binWeight: Array[Double], binPosWeight: Array[Double],
+                                             binPsum: Array[Double], words: Array[Long]): Int
+  @native def evalSamplesWeightedCalibration(ctx: Long, w: Array[Double], samples: Array[Int], a: Double, b: Double,
+                                             nBins: Int, sums: Array[Double], binWeight: Array[Double],
+                                             binPosWeight: Array[Double], binPsum: Array[Double], words: Array[Long]): Int
   // isotonic calibration: nPoints(0) = k, x / y(0 until k) the thresholds ascending in s = -x.w and their probabilities,
   // blockRows / blockPos(0 until blocks), info(0..4) = blocks, points, rows used, NaN rows, distinct scores; x, y, blockRows
   // and blockPos at least as long as the request's rows.  P(y = +1 | x) = numpy.interp(s, x, y).  Quality at the map (x, y):
@@ -112,6 +132,30 @@ object DsgdNative {
   @native def evalSamplesIsotonicCalibration(ctx: Long, w: Array[Double], samples: Array[Int], x: Array[Double],
                                              y: Array[Double], nBins: Int, sums: Array[Double], binRows: Array[Long],
                                              binPos: Array[Long], binPsum: Array[Double], words: Array[Long]): Int
+  // weighted isotonic calibration: blockWeight / blockPosWeight in place of the block counts, wsums(0..1) = W+, W-; weighted
+  // quality at (x, y): sums(0..3), binWeight / binPosWeight / binPsum, words(0..2) as for evalIsotonicCalibration.
+  @native def calibrateIsotonicWeighted(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, nPoints: Array[Long],
+                                        x: Array[Double], y: Array[Double], blockWeight: Array[Double],
+                                        blockPosWeight: Array[Double], info: Array[Long], wsums: Array[Double]): Int
+  @native def calibrateIsotonicWeightedSampled(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long,
+                                               posBegin: Long, posEnd: Long, nPoints: Array[Long], x: Array[Double],
+                                               y: Array[Double], blockWeight: Array[Double], blockPosWeight: Array[Double],
+                                               info: Array[Long], wsums: Array[Double]): Int
+  @native def calibrateIsotonicWeightedSamples(ctx: Long, w: Array[Double], samples: Array[Int], nPoints: Array[Long],
+                                               x: Array[Double], y: Array[Double], blockWeight: Array[Double],
+                                               blockPosWeight: Array[Double], info: Array[Long], wsums: Array[Double]): Int
+  @native def evalWeightedIsotonicCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, x: Array[Double],
+                                              y: Array[Double], nBins: Int, sums: Array[Double], binWeight: Array[Double],
+                                              binPosWeight: Array[Double], binPsum: Array[Double], words: Array[Long]): Int
+  @native def evalSampledWeightedIsotonicCalibration(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long,
+                                                     posBegin: Long, posEnd: Long, x: Array[Double], y: Array[Double],
+                                                     nBins: Int, sums: Array[Double], binWeight: Array[Double],
+                                                     binPosWeight: Array[Double], binPsum: Array[Double],
+                                                     words: Array[Long]): Int
+  @native def evalSamplesWeightedIsotonicCalibration(ctx: Long, w: Array[Double], samples: Array[Int], x: Array[Double],
+                                                     y: Array[Double], nBins: Int, sums: Array[Double],
+                                                     binWeight: Array[Double], binPosWeight: Array[Double],
+                                                     binPsum: Array[Double], words: Array[Long]): Int
   // sync mode: cluster membership (core/Master.scala:222-243) becomes attach / import calls; the step loop one call
   @native def commUniqueId(id: Array[Byte]): Int                       // 128 bytes; rank 0 makes it, every rank commInit()s it
   @native def commInit(ctx: Long, id: Array[Byte]): Int

@@ -450,6 +450,121 @@ FN(evalSamplesCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, j
   return rc;
 }
 
+/* weighted calibration: the calibration natives with wsums(0..2) = W+, W- and the NaN rows' weight added to a fit; quality:
+ * sums(0..3) = weighted Brier and log-loss sums, the weight used and the infinite-term weight, binWeight / binPosWeight /
+ * binPsum at least nBins long (doubles), words(0..1) as there.  A shorter array is DSGD_ERR_INVALID. */
+static int wcalib_short(const calib_bufs *c, const buf_t *ws) { return calib_short(c) || ws->n < DSGD_CALIBRATION_WSUMS; }
+FN(calibrateWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray ab,
+                      jdoubleArray objective, jlongArray info, jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w), ws = out_Double(env, wsums);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | ws.bad | calib_bad(&c)))
+    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
+                               : dsgd_calibrate_weighted(CTX(h), bw.p, rowBegin, rowEnd, (double *)c.ab.p, (double *)c.f.p,
+                                                         (int64_t *)c.info.p, ws.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  back_Double(env, wsums, ws, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateWeightedSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                             jlong posBegin, jlong posEnd, jdoubleArray ab, jdoubleArray objective, jlongArray info,
+                             jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w), ws = out_Double(env, wsums);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | ws.bad | calib_bad(&c)))
+    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
+                               : dsgd_calibrate_weighted_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin,
+                                                                 posEnd, (double *)c.ab.p, (double *)c.f.p,
+                                                                 (int64_t *)c.info.p, ws.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  back_Double(env, wsums, ws, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateWeightedSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray ab,
+                             jdoubleArray objective, jlongArray info, jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), ws = out_Double(env, wsums);
+  calib_bufs c = calib_out(env, ab, objective, info);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | ws.bad | calib_bad(&c)))
+    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
+                               : dsgd_calibrate_weighted_samples(CTX(h), bw.p, bs.p, bs.n, (double *)c.ab.p, (double *)c.f.p,
+                                                                 (int64_t *)c.info.p, ws.p);
+  calib_back(env, ab, objective, info, &c, rc);
+  back_Double(env, wsums, ws, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+typedef struct { buf_t s, wt, pw, ps, wd; } wquality_bufs;
+static wquality_bufs wquality_out(JNIEnv *env, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
+                                  jdoubleArray binPsum, jlongArray words) {
+  wquality_bufs q = {out_Double(env, sums), out_Double(env, binWeight), out_Double(env, binPosWeight),
+                     out_Double(env, binPsum), out_Long(env, words)};
+  return q;
+}
+static int wquality_bad(const wquality_bufs *q) { return q->s.bad | q->wt.bad | q->pw.bad | q->ps.bad | q->wd.bad; }
+static int wquality_short(const wquality_bufs *q, jint nBins) {
+  const jlong m = nBins > 0 ? nBins : 0;
+  return q->s.n < DSGD_WCALIBRATION_SUMS || q->wd.n < 2 || q->wt.n < m || q->pw.n < m || q->ps.n < m;
+}
+static void wquality_back(JNIEnv *env, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
+                          jdoubleArray binPsum, jlongArray words, wquality_bufs *q, int rc) {
+  back_Double(env, sums, q->s, rc);
+  back_Double(env, binWeight, q->wt, rc);
+  back_Double(env, binPosWeight, q->pw, rc);
+  back_Double(env, binPsum, q->ps, rc);
+  back_Long(env, words, q->wd, rc);
+}
+FN(evalWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdouble a,
+                            jdouble b, jint nBins, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
+                            jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | wquality_bad(&q)))
+    rc = wquality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_weighted_calibration(CTX(h), bw.p, rowBegin, rowEnd, a, b, nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p,
+                                              (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                                   jlong key, jlong posBegin, jlong posEnd, jdouble a, jdouble b, jint nBins,
+                                   jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
+                                   jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | wquality_bad(&q)))
+    rc = wquality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_weighted_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, a, b,
+                                                      nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p, (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a,
+                                   jdouble b, jint nBins, jdoubleArray sums, jdoubleArray binWeight,
+                                   jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | wquality_bad(&q)))
+    rc = wquality_short(&q, nBins)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_weighted_calibration(CTX(h), bw.p, bs.p, bs.n, a, b, nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p,
+                                                      (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+
 /* isotonic calibration: nPoints(0) = k, x / y(0 until k) the thresholds and their values, blockRows / blockPos(0 until
  * blocks), info(0..4) = the DSGD_ISOTONIC_INFO_WORDS words; x, y, blockRows and blockPos at least as long as the request's
  * rows.  Probabilities and quality at the map (x, y): x and y of one length k >= 1; out at least as long as samples; the
@@ -579,6 +694,132 @@ FN(evalSamplesIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleAr
                                                       (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p,
                                                       (int64_t *)q.wd.p);
   quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
+  free(bw.p); free(bs.p); free(bx.p); free(by.p);
+  return rc;
+}
+
+/* weighted isotonic calibration: the isotonic natives with blockWeight / blockPosWeight (doubles) in place of the block counts
+ * and wsums(0..1) = W+, W- added to a fit; weighted quality at (x, y): the weighted quality arrays with words(0..2) as for
+ * evalIsotonicCalibration.  A shorter array is DSGD_ERR_INVALID. */
+typedef struct { buf_t k, x, y, r, p, info, ws; } wiso_bufs;
+static wiso_bufs wiso_out(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
+                          jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
+  wiso_bufs c = {out_Long(env, nPoints), out_Double(env, x), out_Double(env, y), out_Double(env, blockWeight),
+                 out_Double(env, blockPosWeight), out_Long(env, info), out_Double(env, wsums)};
+  return c;
+}
+static int wiso_bad(const wiso_bufs *c) {
+  return c->k.bad | c->x.bad | c->y.bad | c->r.bad | c->p.bad | c->info.bad | c->ws.bad;
+}
+static int wiso_short(const wiso_bufs *c, jlong n) {
+  return c->k.n < 1 || c->info.n < DSGD_ISOTONIC_INFO_WORDS || c->ws.n < 2 || c->x.n < n || c->y.n < n || c->r.n < n ||
+         c->p.n < n;
+}
+static void wiso_back(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
+                      jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums, wiso_bufs *c, int rc) {
+  back_Long(env, nPoints, c->k, rc);
+  back_Double(env, x, c->x, rc);
+  back_Double(env, y, c->y, rc);
+  back_Double(env, blockWeight, c->r, rc);
+  back_Double(env, blockPosWeight, c->p, rc);
+  back_Long(env, info, c->info, rc);
+  back_Double(env, wsums, c->ws, rc);
+}
+FN(calibrateIsotonicWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                              jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
+                              jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w);
+  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | wiso_bad(&c)))
+    rc = wiso_short(&c, rowEnd - rowBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic_weighted(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p, c.p.p,
+                                                (int64_t *)c.info.p, c.ws.p);
+  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateIsotonicWeightedSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                                     jlong key, jlong posBegin, jlong posEnd, jlongArray nPoints, jdoubleArray x,
+                                     jdoubleArray y, jdoubleArray blockWeight, jdoubleArray blockPosWeight, jlongArray info,
+                                     jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w);
+  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | wiso_bad(&c)))
+    rc = wiso_short(&c, posEnd - posBegin)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic_weighted_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                        (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p, c.p.p, (int64_t *)c.info.p,
+                                                        c.ws.p);
+  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(calibrateIsotonicWeightedSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples,
+                                     jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
+                                     jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | wiso_bad(&c)))
+    rc = wiso_short(&c, bs.n)
+             ? DSGD_ERR_INVALID
+             : dsgd_calibrate_isotonic_weighted_samples(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p,
+                                                        c.p.p, (int64_t *)c.info.p, c.ws.p);
+  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+static int wiso_quality_short(const wquality_bufs *q, jint nBins, const buf_t *bx, const buf_t *by) {
+  return wquality_short(q, nBins) || q->wd.n < DSGD_ISOTONIC_EVAL_WORDS || bx->n != by->n;
+}
+FN(evalWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                                    jdoubleArray x, jdoubleArray y, jint nBins, jdoubleArray sums, jdoubleArray binWeight,
+                                    jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bx.bad | by.bad | wquality_bad(&q)))
+    rc = wiso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_weighted_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, bx.p, by.p, bx.n, nBins, q.s.p, q.wt.p,
+                                                       q.pw.p, q.ps.p, (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
+  free(bw.p); free(bx.p); free(by.p);
+  return rc;
+}
+FN(evalSampledWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
+                                           jlong key, jlong posBegin, jlong posEnd, jdoubleArray x, jdoubleArray y,
+                                           jint nBins, jdoubleArray sums, jdoubleArray binWeight,
+                                           jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
+  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bx.bad | by.bad | wquality_bad(&q)))
+    rc = wiso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_weighted_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin,
+                                                               posEnd, bx.p, by.p, bx.n, nBins, q.s.p, q.wt.p, q.pw.p,
+                                                               q.ps.p, (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
+  free(bw.p); free(bx.p); free(by.p);
+  return rc;
+}
+FN(evalSamplesWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples,
+                                           jdoubleArray x, jdoubleArray y, jint nBins, jdoubleArray sums,
+                                           jdoubleArray binWeight, jdoubleArray binPosWeight, jdoubleArray binPsum,
+                                           jlongArray words) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y);
+  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | bx.bad | by.bad | wquality_bad(&q)))
+    rc = wiso_quality_short(&q, nBins, &bx, &by)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_weighted_isotonic_calibration(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, nBins, q.s.p,
+                                                               q.wt.p, q.pw.p, q.ps.p, (int64_t *)q.wd.p);
+  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
   free(bw.p); free(bs.p); free(bx.p); free(by.p);
   return rc;
 }

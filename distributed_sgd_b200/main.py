@@ -45,6 +45,9 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     from .utils.dataset import SAMPLE_WEIGHT_ASYNC, load_sample_weights
     if cfg.sample_weight and cfg.is_async:
         raise ValueError(SAMPLE_WEIGHT_ASYNC)
+    if cfg.calibration_weighted and cfg.is_async:
+        raise ValueError("calibration-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
+                         "has none to calibrate by")
     if cfg.sample_weight:   # one weight per loaded row; the split below carries them
         data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
@@ -100,8 +103,9 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         report["averaged_steps"] = int(master.history["averaged_steps"])   # the returned weights are their mean
     if cfg.calibrate and cfg.calibration_method == "isotonic":
         # an isotonic map fitted on the train rows, judged on the test rows
-        iso = master.calibrate(w1, method="isotonic")
-        q = master.local_calibration(iso, w1, test_data=True)
+        wkw = {"weighted": True} if cfg.calibration_weighted else {}   # unweighted: the calls as they always were
+        iso = master.calibrate(w1, method="isotonic", **wkw)
+        q = master.local_calibration(iso, w1, test_data=True, **wkw)
         report["calibration"] = {"method": "isotonic", "blocks": iso.blocks, "points": iso.points,
                                  "distinct_scores": iso.distinct_scores, "test_brier": q["brier"],
                                  "test_log_loss": q["log_loss"], "test_ece": q["ece"],
@@ -113,10 +117,14 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         # a Platt sigmoid fitted on the train rows, judged on the test rows; for the logistic model also against the
         # model's own probability, the identity link
         from .ml import Calibration
-        cal = master.calibrate(w1)
-        q = master.local_calibration(cal, w1, test_data=True)
+        wkw = {"weighted": True} if cfg.calibration_weighted else {}   # unweighted: the calls as they always were
+        cal = master.calibrate(w1, **wkw)
+        q = master.local_calibration(cal, w1, test_data=True, **wkw)
         report["calibration"] = {"method": "sigmoid", "a": cal.a, "b": cal.b, "iterations": cal.iterations, "status": cal.status,
                                  "test_brier": q["brier"], "test_log_loss": q["log_loss"], "test_ece": q["ece"]}
+        if cfg.calibration_weighted:
+            report["calibration"].update(weighted=True, weight_pos=cal.weight_pos, weight_neg=cal.weight_neg,
+                                         test_weight=q["weight"])
         if cfg.model == "logistic":
             q0 = master.local_calibration(Calibration.identity(), w1, test_data=True)
             report["calibration"]["identity"] = {"test_brier": q0["brier"], "test_log_loss": q0["log_loss"],

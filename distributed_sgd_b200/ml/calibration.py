@@ -2,7 +2,7 @@
 isotonic map numpy.interp(-x.w, x, y) (IsotonicCalibration)."""
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 
 import numpy as np
 
@@ -20,6 +20,12 @@ class Calibration:
     status: int = CONVERGED           # CONVERGED, ITERATION_LIMIT, LINE_SEARCH_FAILED or NON_FINITE
     rows: int = 0                     # rows the fit used
     nan_rows: int = 0                 # rows left out because their margin was NaN
+    # a weighted fit (Master.calibrate(weighted=True)): every row counted by its weight c_i; W+ and W- of the rows used and
+    # the weight of the NaN rows.  Left out of repr, so that an unweighted Calibration prints as it always has.
+    weighted: bool = field(default=False, repr=False)
+    weight_pos: float = field(default=0.0, repr=False)
+    weight_neg: float = field(default=0.0, repr=False)
+    nan_weight: float = field(default=0.0, repr=False)
 
     @staticmethod
     def identity() -> "Calibration":
@@ -43,6 +49,12 @@ class IsotonicCalibration:
     rows: int = 0                     # rows the fit used
     nan_rows: int = 0                 # rows left out because their margin was NaN
     distinct_scores: int = 0
+    # a weighted fit (Master.calibrate(method="isotonic", weighted=True)): block_rows / block_pos then hold each block's
+    # weight and positive weight (doubles), rows and distinct_scores count the rows and scores of positive weight, and
+    # weight_pos / weight_neg are W+ and W- of the non-NaN rows.  Left out of repr.
+    weighted: bool = field(default=False, repr=False)
+    weight_pos: float = field(default=0.0, repr=False)
+    weight_neg: float = field(default=0.0, repr=False)
 
     @property
     def points(self) -> int:

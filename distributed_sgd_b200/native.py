@@ -35,6 +35,8 @@ OK, ERR_INVALID, ERR_STATE, ERR_EMPTY, ERR_RANGE, ERR_CUDA, ERR_NCCL, ERR_NOMEM,
 METRICS_WORDS = 8
 CALIBRATION_INFO_WORDS = 5   # DSGD_CALIBRATION_INFO_WORDS
 CALIBRATION_MAX_BINS = 64    # DSGD_CALIBRATION_MAX_BINS
+CALIBRATION_WSUMS = 3        # DSGD_CALIBRATION_WSUMS: W+, W-, the NaN rows' weight
+WCALIBRATION_SUMS = 4        # DSGD_WCALIBRATION_SUMS: weighted Brier and log-loss sums, weight used, infinite-term weight
 ISOTONIC_INFO_WORDS = 5      # DSGD_ISOTONIC_INFO_WORDS: blocks, points, rows used, NaN rows, distinct scores
 ISOTONIC_EVAL_WORDS = 3      # DSGD_ISOTONIC_EVAL_WORDS: rows used, rows left out, rows with an infinite log-loss term
 
@@ -124,6 +126,21 @@ ABI = {
     "dsgd_eval_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_sampled_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_eval_samples_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_weighted": [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_weighted_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_weighted_samples": [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp],
+    "dsgd_eval_weighted_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_sampled_weighted_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp,
+                                               _vp],
+    "dsgd_eval_samples_weighted_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_isotonic_weighted": [_vp, _vp, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_calibrate_isotonic_weighted_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp,
+                                                 _vp, _vp],
+    "dsgd_calibrate_isotonic_weighted_samples": [_vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_weighted_isotonic_calibration": [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
+    "dsgd_eval_sampled_weighted_isotonic_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _i64, _i32, _vp,
+                                                        _vp, _vp, _vp, _vp],
+    "dsgd_eval_samples_weighted_isotonic_calibration": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
     "dsgd_calibrate_isotonic": [_vp, _vp, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
     "dsgd_calibrate_isotonic_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
     "dsgd_calibrate_isotonic_samples": [_vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
@@ -561,6 +578,59 @@ class NativeCtx:
         samples = _arr(samples, np.int32)
         return self._eval_calibration("eval_samples_calibration", w, (_ptr(samples), samples.size), a, b, n_bins)
 
+    # -- weighted calibration --
+    def _calibrate_weighted(self, fn: str, w, rows: tuple):
+        """dsgd_<fn>: (A, B, objective, info, wsums) of one weighted Platt fit; info as _calibrate's, wsums = the
+        CALIBRATION_WSUMS doubles {W+, W-, NaN rows' weight}."""
+        w = self._w(w)
+        ab = np.zeros(2, dtype=np.float64)
+        info = np.zeros(CALIBRATION_INFO_WORDS, dtype=np.int64)
+        wsums = np.zeros(CALIBRATION_WSUMS, dtype=np.float64)
+        obj = C.c_double()
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(ab), C.byref(obj), _ptr(info), _ptr(wsums)))
+        return float(ab[0]), float(ab[1]), obj.value, info, wsums
+
+    def calibrate_weighted(self, row_begin: int, row_end: int, w=None):
+        """Platt scaling with every row counted by its weight c_i over rows [row_begin, row_end) (dsgd_calibrate_weighted)."""
+        return self._calibrate_weighted("calibrate_weighted", w, (row_begin, row_end))
+
+    def calibrate_weighted_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_weighted_sampled)."""
+        return self._calibrate_weighted("calibrate_weighted_sampled", w, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def calibrate_weighted_samples(self, samples, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_calibrate_weighted_samples)."""
+        samples = _arr(samples, np.int32)
+        return self._calibrate_weighted("calibrate_weighted_samples", w, (_ptr(samples), samples.size))
+
+    def _eval_weighted_calibration(self, fn: str, w, rows: tuple, a: float, b: float, n_bins: int):
+        """dsgd_<fn>: (sums, bin_weight, bin_pos_weight, bin_psum, words): sums = the WCALIBRATION_SUMS doubles {Brier sum,
+        log-loss sum, weight used, infinite-term weight}, words = {rows used, rows left out}."""
+        w = self._w(w)
+        m = max(int(n_bins), 1)
+        sums, words = np.zeros(WCALIBRATION_SUMS, dtype=np.float64), np.zeros(2, dtype=np.int64)
+        wb, pwb, psum = np.zeros(m), np.zeros(m), np.zeros(m)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, float(a), float(b), int(n_bins), _ptr(sums),
+                                                 _ptr(wb), _ptr(pwb), _ptr(psum), _ptr(words)))
+        return sums, wb, pwb, psum, words
+
+    def eval_weighted_calibration(self, row_begin: int, row_end: int, a: float, b: float, n_bins: int = 10, w=None):
+        """Weighted Brier and log-loss sums and n_bins weighted reliability bins at (a, b) over rows [row_begin, row_end)
+        (dsgd_eval_weighted_calibration)."""
+        return self._eval_weighted_calibration("eval_weighted_calibration", w, (row_begin, row_end), a, b, n_bins)
+
+    def eval_sampled_weighted_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                                          a: float, b: float, n_bins: int = 10, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_weighted_calibration)."""
+        return self._eval_weighted_calibration("eval_sampled_weighted_calibration", w,
+                                               _drawn(row_begin, row_end, key, pos_begin, pos_end), a, b, n_bins)
+
+    def eval_samples_weighted_calibration(self, samples, a: float, b: float, n_bins: int = 10, w=None):
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted_calibration)."""
+        samples = _arr(samples, np.int32)
+        return self._eval_weighted_calibration("eval_samples_weighted_calibration", w, (_ptr(samples), samples.size), a, b,
+                                               n_bins)
+
     # -- isotonic calibration --
     def _calibrate_isotonic(self, fn: str, w, rows: tuple, n: int):
         """dsgd_<fn>: (x, y, block_rows, block_pos, info) of one isotonic fit over n rows; info = the ISOTONIC_INFO_WORDS
@@ -611,6 +681,64 @@ class NativeCtx:
         self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1,
                                                  int(n_bins), _ptr(sums), _ptr(rows_b), _ptr(pos_b), _ptr(psum), _ptr(words)))
         return sums, rows_b, pos_b, psum, words
+
+    def _calibrate_isotonic_weighted(self, fn: str, w, rows: tuple, n: int):
+        """dsgd_<fn>: (x, y, block_weight, block_pos_weight, info, wsums) of one weighted isotonic fit over n rows; info as
+        _calibrate_isotonic's (rows and scores of positive weight), wsums = {W+, W-}."""
+        w = self._w(w)
+        size = max(int(n), 1)
+        x, y, bw, bp = (np.zeros(size, dtype=np.float64) for _ in range(4))
+        info, k, ws = np.zeros(ISOTONIC_INFO_WORDS, dtype=np.int64), C.c_int64(), np.zeros(2)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(k), _ptr(x), _ptr(y), _ptr(bw), _ptr(bp),
+                                                 _ptr(info), _ptr(ws)))
+        nb = int(info[0])
+        return x[:k.value].copy(), y[:k.value].copy(), bw[:nb].copy(), bp[:nb].copy(), info, ws
+
+    def calibrate_isotonic_weighted(self, row_begin: int, row_end: int, w=None):
+        """Isotonic regression with every row counted by its weight c_i over rows [row_begin, row_end)
+        (dsgd_calibrate_isotonic_weighted)."""
+        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted", w, (row_begin, row_end), row_end - row_begin)
+
+    def calibrate_isotonic_weighted_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                                            w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample."""
+        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted_sampled", w,
+                                                 _drawn(row_begin, row_end, key, pos_begin, pos_end), pos_end - pos_begin)
+
+    def calibrate_isotonic_weighted_samples(self, samples, w=None):
+        """The same over a list of row ids; repeats count every time."""
+        samples = _arr(samples, np.int32)
+        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted_samples", w, (_ptr(samples), samples.size),
+                                                 samples.size)
+
+    def _eval_weighted_isotonic_calibration(self, fn: str, w, rows: tuple, x, y, n_bins: int):
+        """dsgd_<fn>: (sums, bin_weight, bin_pos_weight, bin_psum, words): sums = {Brier sum, log-loss sum over the finite
+        terms, weight used, weight of the infinite terms}, words = {rows used, rows left out, rows with an infinite term}."""
+        w = self._w(w)
+        x, y = _arr(x, np.float64), _arr(y, np.float64)
+        m = max(int(n_bins), 1)
+        sums, words = np.zeros(WCALIBRATION_SUMS), np.zeros(ISOTONIC_EVAL_WORDS, dtype=np.int64)
+        wb, pwb, psum = np.zeros(m), np.zeros(m), np.zeros(m)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1,
+                                                 int(n_bins), _ptr(sums), _ptr(wb), _ptr(pwb), _ptr(psum), _ptr(words)))
+        return sums, wb, pwb, psum, words
+
+    def eval_weighted_isotonic_calibration(self, row_begin: int, row_end: int, x, y, n_bins: int = 10, w=None):
+        """Weighted quality at the isotonic map (x, y) over rows [row_begin, row_end)."""
+        return self._eval_weighted_isotonic_calibration("eval_weighted_isotonic_calibration", w, (row_begin, row_end), x, y,
+                                                        n_bins)
+
+    def eval_sampled_weighted_isotonic_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int,
+                                                   pos_end: int, x, y, n_bins: int = 10, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample."""
+        return self._eval_weighted_isotonic_calibration("eval_sampled_weighted_isotonic_calibration", w,
+                                                        _drawn(row_begin, row_end, key, pos_begin, pos_end), x, y, n_bins)
+
+    def eval_samples_weighted_isotonic_calibration(self, samples, x, y, n_bins: int = 10, w=None):
+        """The same over a list of row ids; repeats count every time."""
+        samples = _arr(samples, np.int32)
+        return self._eval_weighted_isotonic_calibration("eval_samples_weighted_isotonic_calibration", w,
+                                                        (_ptr(samples), samples.size), x, y, n_bins)
 
     def eval_isotonic_calibration(self, row_begin: int, row_end: int, x, y, n_bins: int = 10, w=None):
         """Brier and log-loss sums and n_bins reliability bins at the map (x, y) over rows [row_begin, row_end)

@@ -40,6 +40,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     class_weight: str = "none"    # extension: none, balanced or w_pos,w_neg -- one weight per label, sync mode only
     calibrate: bool = False       # extension: after fit, fit a calibration on the train rows and report its test-set quality
     calibration_method: str = "sigmoid"   # extension: the calibration `calibrate` fits: sigmoid (Platt) or isotonic
+    calibration_weighted: bool = False    # extension: `calibrate` fits and judges with every row counted by its weight
     sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
 
 
@@ -57,6 +58,7 @@ _KEYS = {
     "learning-rate-power": ("learning_rate_power", "DSGD_LEARNING_RATE_POWER"),
     "l1": ("l1", "DSGD_L1"), "class-weight": ("class_weight", "DSGD_CLASS_WEIGHT"), "calibrate": ("calibrate", "DSGD_CALIBRATE"),
     "calibration-method": ("calibration_method", "DSGD_CALIBRATION_METHOD"),
+    "calibration-weighted": ("calibration_weighted", "DSGD_CALIBRATION_WEIGHTED"),
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")

@@ -343,6 +343,51 @@ int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t 
                                   int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
                                   int64_t *words_out);
 
+/* ---- weighted calibration: the Platt fit and its quality pass with every row counted by its weight (DESIGN.md §4.17), on
+ *      any sync ctx and for any model.  Row i's weight is c_i = fl(w_y * s_i), exactly that of the weighted curves: without
+ *      sample weights c_i = w_y, and with class weights (1, 1) as well c_i = 1.  To calibrate on sample weights alone after
+ *      training with class weights, call dsgd_set_class_weights(ctx, 1, 1) first.  R(v) and read() are those of the weighted
+ *      curves; every weighted total below is read() of one exact sum, so it has the same bits whatever the row order, the
+ *      grid or the model flag.  A row has zero weight when R(c_i) = 0 (every c_i of 2^-161 or less): it adds exactly 0 to
+ *      every sum, and no term of it is formed.
+ *      dsgd_calibrate_weighted*: the fit of dsgd_calibrate* with W+ and W-, the weights of the positive and negative rows
+ *      whose f is not NaN, in place of N+ and N-: targets (W+ + 1) / (W+ + 2) and 1 / (W- + 2), start (0, log((W- + 1) /
+ *      (W+ + 1))) -- scikit-learn's weighted priors -- and each of the six sums over the rows adds R(fl(c_i term_i)).  A
+ *      weighted term of 2^52 or more makes its sum non-finite (status 3), and so does a W+ or W- that is not finite.  The
+ *      Newton, ridge, line-search and stop rules are those of dsgd_calibrate; the gradient bound stays 1e-5 in absolute
+ *      terms, so large weights make status 2 likelier.  ab_out, objective_out and info_out as there (info_out[2] and [3]
+ *      count rows, not weights); wsums_out[0..2] = {W+, W-, the weight of the NaN rows}.  W+ = 0 or W- = 0 ->
+ *      DSGD_ERR_EMPTY (wsums_out is set).  An async ctx -> DSGD_ERR_STATE before anything is launched; a NULL output ->
+ *      DSGD_ERR_INVALID.  A fit grows 8 bytes per row more than dsgd_calibrate's.  At c = 1 every output equals
+ *      dsgd_calibrate's bit for bit. */
+#define DSGD_CALIBRATION_WSUMS 3
+int dsgd_calibrate_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
+                            double *objective_out, int64_t *info_out, double *wsums_out);
+int dsgd_calibrate_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                    int64_t pos_begin, int64_t pos_end, double *ab_out, double *objective_out,
+                                    int64_t *info_out, double *wsums_out);
+int dsgd_calibrate_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
+                                    double *objective_out, int64_t *info_out, double *wsums_out);
+/* Weighted quality at (a, b), over the rows of dsgd_eval_calibration with its p, o, bins and arguments:
+ *   sums_out[0] = sum R(fl(c (p - o)^2)) (Brier)   sums_out[1] = sum R(fl(c l)), l the log-loss term of dsgd_eval_calibration
+ *   sums_out[2] = sum R(c) over the rows used       sums_out[3] = 0 (a sigmoid's term is never infinite)
+ *   bin_weight[k] = sum R(c), bin_pos_weight[k] = the same over the positive rows, bin_psum[k] = sum R(fl(c p)), n_bins
+ *   doubles each; a bin value of 2^52 or more makes that bin's three sums NaN, one elsewhere makes its sum NaN.
+ *   words_out[0] rows used, words_out[1] rows left out: counts, as dsgd_eval_calibration's.
+ * At c = 1 the sums and bin_psum equal dsgd_eval_calibration's bit for bit, and the bin weights its bin counts.  Errors are
+ * those of dsgd_eval_calibration; an async ctx -> DSGD_ERR_STATE before anything is launched. */
+#define DSGD_WCALIBRATION_SUMS 4
+int dsgd_eval_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a, double b,
+                                   int32_t n_bins, double *sums_out, double *bin_weight, double *bin_pos_weight,
+                                   double *bin_psum, int64_t *words_out);
+int dsgd_eval_sampled_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                           int64_t pos_begin, int64_t pos_end, double a, double b, int32_t n_bins,
+                                           double *sums_out, double *bin_weight, double *bin_pos_weight, double *bin_psum,
+                                           int64_t *words_out);
+int dsgd_eval_samples_weighted_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
+                                           double b, int32_t n_bins, double *sums_out, double *bin_weight,
+                                           double *bin_pos_weight, double *bin_psum, int64_t *words_out);
+
 /* ---- isotonic calibration: a non-parametric map from the score to a probability, for any model (DESIGN.md §4.16).  The
  *      rows, the three row forms, the score s = -x . w (f = x . w exactly as dsgd_margins returns it), NaN handling and the
  *      +0 / -0 rule are those of dsgd_eval_curve.
@@ -399,6 +444,52 @@ int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64
 int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, const double *X,
                                            const double *Y, int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows,
                                            int64_t *bin_pos, double *bin_psum, int64_t *words_out);
+
+/* ---- weighted isotonic calibration: the isotonic fit and its quality pass with every row counted by its weight c_i, the
+ *      weight of the weighted calibration calls above (DESIGN.md §4.17); on any sync ctx and for any model.
+ *      Fit: the points are the distinct non-NaN scores t_0 > ... > t_(m-1) with the exact sums X_k = W(>= t_k) and
+ *      Y_k = W+(>= t_k) of the weighted curve pass, and P_-1 = (0, 0).  A point whose weight increment X_k - X_(k-1) is
+ *      exactly zero (only zero-weight rows at its score) is dropped before the hull, as scikit-learn drops zero-weight rows,
+ *      so its score never enters X.  The blocks are the segments of the upper concave hull of the rest, with strict
+ *      vertices as in dsgd_calibrate_isotonic; every coordinate is an integer in units of 2^-160 and every turn test an
+ *      exact 512-bit comparison, so the outputs have one bit pattern for a multiset of (row, weight) whatever the row form,
+ *      the row order, the grid limit, the tile size or the model flag.  A block's value is p_b = fl(read(dY) / read(dX));
+ *      at c = 1 this is dsgd_calibrate_isotonic's fl(pos / rows) bit for bit, and every output equals that call's.
+ *      Outputs as dsgd_calibrate_isotonic's, except: wrows_out[j] / wpos_out[j] the block's weight and positive weight (as
+ *      doubles, read() of exact sums); info_out[2] the non-NaN rows of positive weight; info_out[4] the distinct scores
+ *      among them (the points kept); wsums_out[0..1] = {W+, W-} of the non-NaN rows.  The turn test is exact while the total
+ *      weight of the non-NaN rows is below 2^96 (2^64 and far more are accepted): 2^96 or more, or a c_i of 2^52 or more,
+ *      -> DSGD_ERR_RANGE before the hull.  No non-NaN row of positive weight -> DSGD_ERR_EMPTY (one class is valid).  An
+ *      async ctx -> DSGD_ERR_STATE before anything is launched; a NULL output -> DSGD_ERR_INVALID.  DSGD_ISOTONIC_TILE
+ *      applies (the result does not depend on it).  A fit grows about 150 bytes per row more than the weighted curve pass.
+ *      X and Y feed dsgd_isotonic_probabilities unchanged. */
+int dsgd_calibrate_isotonic_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *n_points_out,
+                                     double *x_out, double *y_out, double *wrows_out, double *wpos_out, int64_t *info_out,
+                                     double *wsums_out);
+int dsgd_calibrate_isotonic_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                             int64_t pos_begin, int64_t pos_end, int64_t *n_points_out, double *x_out,
+                                             double *y_out, double *wrows_out, double *wpos_out, int64_t *info_out,
+                                             double *wsums_out);
+int dsgd_calibrate_isotonic_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                             int64_t *n_points_out, double *x_out, double *y_out, double *wrows_out,
+                                             double *wpos_out, int64_t *info_out, double *wsums_out);
+/* Weighted quality at the map (X, Y): dsgd_eval_weighted_calibration's outputs with p and the log-loss term of
+ * dsgd_eval_isotonic_calibration: sums_out[1] adds R(fl(c l)) over the finite terms, sums_out[3] = sum R(c) over the rows of
+ * positive weight whose term is infinite (any such row makes the weighted log loss +inf), words_out
+ * (DSGD_ISOTONIC_EVAL_WORDS) [2] = their number.  The map's checks are those of dsgd_isotonic_probabilities; an async ctx
+ * -> DSGD_ERR_STATE. */
+int dsgd_eval_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, const double *X,
+                                            const double *Y, int64_t k, int32_t n_bins, double *sums_out, double *bin_weight,
+                                            double *bin_pos_weight, double *bin_psum, int64_t *words_out);
+int dsgd_eval_sampled_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                    uint64_t key, int64_t pos_begin, int64_t pos_end, const double *X,
+                                                    const double *Y, int64_t k, int32_t n_bins, double *sums_out,
+                                                    double *bin_weight, double *bin_pos_weight, double *bin_psum,
+                                                    int64_t *words_out);
+int dsgd_eval_samples_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                    const double *X, const double *Y, int64_t k, int32_t n_bins,
+                                                    double *sums_out, double *bin_weight, double *bin_pos_weight,
+                                                    double *bin_psum, int64_t *words_out);
 
 /* ---- communicator for sync mode: replaces the gRPC channels between master and slaves
  *      (core/package.scala:16-21; core/Master.scala:222-243).  Rank 0 makes an id, the host transports it
