@@ -1590,8 +1590,8 @@ static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, d
   int &occ = kW ? ctx->k_fit_occ_w : ctx->k_fit_occ;
   if (!occ) {
     const int full = cap_max * per_score;
-    CU(cudaFuncSetAttribute((kW ? k_calib_fit_w : k_calib_fit), cudaFuncAttributeMaxDynamicSharedMemorySize, full));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (kW ? k_calib_fit_w : k_calib_fit), kCalThreads, (size_t)full));
+    CU(cudaFuncSetAttribute(k_calib_fit<kW>, cudaFuncAttributeMaxDynamicSharedMemorySize, full));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_calib_fit<kW>, kCalThreads, (size_t)full));
     NEED(occ > 0, DSGD_ERR_CUDA, "%s: k_calib_fit does not fit on an SM", fn);
   }
   int G = ctx->sm_count * occ;   // resident at the full shared-memory budget, so at any smaller one
@@ -1611,7 +1611,7 @@ static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, d
   fp.smem_cap = (int)std::min<int64_t>(cdiv(n, G), cap_max);
   if (kW) fp.cw = ctx->k_cw;
   void *args[] = {&fp};
-  CU(cudaLaunchCooperativeKernel((void *)(kW ? k_calib_fit_w : k_calib_fit), dim3(G), dim3(kCalThreads), args, (size_t)fp.smem_cap * per_score,
+  CU(cudaLaunchCooperativeKernel((void *)k_calib_fit<kW>, dim3(G), dim3(kCalThreads), args, (size_t)fp.smem_cap * per_score,
                                  ctx->stream));
   LAUNCHED();
   unsigned long long out[kCalOutWords + 1];
@@ -1725,17 +1725,35 @@ extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, con
   return DSGD_OK;
 }
 
-// One quality pass over `rows` at (a, b): k_calib_eval, k_calib_eval_finish, the block read back.
-static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, int32_t n_bins,
-                                    double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
-                                    int64_t *words_out, const char *fn) {
+// One quality pass over `rows`, at (a, b) or (kIso) at the map (X, Y): k_calib_eval, k_calib_eval_finish, the block read
+// back.  words_out = {rows used, NaN rows} and (kIso) the rows whose log-loss term is infinite.
+static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn);
+template <class K>
+static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args);
+template <bool kIso>
+static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, const double *X,
+                                    const double *Y, int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows,
+                                    int64_t *bin_pos, double *bin_psum, int64_t *words_out, const char *fn) {
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = fits_while_running(ctx, ctx->k_eval, fn);
-  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords))) return rc;
+  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (kIso && (rc = isotonic_map(ctx, X, Y, k, fn))) ||
+      (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)))
+    return rc;
   CU(cudaMemsetAsync(ctx->k_eval, 0, sizeof(unsigned long long) * kCevWords, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);
-  k_calib_eval<<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, wd, a, b,
-                                              n_bins, ctx->k_eval);
+  const double *mx = kIso ? ctx->i_map.p : nullptr, *my = kIso ? ctx->i_map.p + k : nullptr;
+  int ki = (int)k, nb = n_bins;
+  unsigned long long *blk = ctx->k_eval.p;
+  const uint32_t *rp16 = ctx->rp16.p;
+  const uint2 *pairs = ctx->pairs.p;
+  const int8_t *label = ctx->label.p;
+  const int32_t *ids = rows.ids;
+  int64_t rb = rows.row_begin, rn = rows.n;
+  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk};
+  if constexpr (kIso)
+    CU(isotonic_launch(k_calib_eval<true, true>, k_calib_eval<true, false>, grid, k, ctx->stream, args));
+  else
+    CU(cudaLaunchKernel((const void *)k_calib_eval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
   LAUNCHED();
   k_calib_eval_finish<<<1, kCalMaxBins, 0, ctx->stream>>>(ctx->k_eval, n_bins);
   LAUNCHED();
@@ -1751,6 +1769,7 @@ static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_se
   memcpy(bin_psum, &h[kCevOutPsum], (size_t)n_bins * sizeof(double));
   words_out[0] = (int64_t)h[kCevRows];
   words_out[1] = (int64_t)h[kCevNan];
+  if (kIso) words_out[2] = (int64_t)h[kCevInf];
   return DSGD_OK;
 }
 
@@ -1768,7 +1787,8 @@ extern "C" int dsgd_eval_calibration(dsgd_ctx *ctx, const double *w, int64_t row
   CALIB_EVAL_ARGS_OK();
   row_set rows;
   int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
+                                                    bin_pos, bin_psum, words_out, __func__);
 }
 
 extern "C" int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
@@ -1779,7 +1799,8 @@ extern "C" int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int
   CALIB_EVAL_ARGS_OK();
   row_set rows;
   int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
+                                                    bin_pos, bin_psum, words_out, __func__);
 }
 
 extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
@@ -1790,14 +1811,12 @@ extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, con
   NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : calibration_quality_pass(ctx, w, rows, a, b, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
+                                                    bin_pos, bin_psum, words_out, __func__);
 }
 
 // One weighted quality pass over `rows`, at (a, b) or (kIso) at the map (X, Y): k_weval, the block read back, every sum
 // read() on the host.
-static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn);
-template <class K>
-static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args);
 template <bool kIso>
 static int weighted_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, const double *X,
                                  const double *Y, int64_t k, int32_t n_bins, double *sums_out, double *bin_weight,
@@ -1905,9 +1924,59 @@ static int isotonic_grid(const dsgd_ctx *ctx, int64_t items) {
   return (int)std::max<int64_t>(1, std::min<int64_t>(items, cap));
 }
 
-// One isotonic fit over `rows`: the curve pass with its points left on the device, the hull (k_iso_tile, then k_iso_merge
-// rounds until one hull is left), the hull's vertex count read back, the scan of the blocks' X counts, k_iso_emit, and the
-// outputs copied back.
+// The hull and the emit of a fit over `points` points of the point set P (its arrays c0, c1; their scores thr): k_iso_tile,
+// k_iso_merge rounds until one hull is left, the hull's vertex count read back, the scan of the blocks' X counts,
+// k_iso_emit (X and Y into i_out, the blocks' two values into blk and blk + n), and the outputs copied back.  *n_blocks and
+// *n_x: the blocks and the X entries.
+template <class P>
+static int isotonic_hull(dsgd_ctx *ctx, const typename P::Coord *c0, const typename P::Coord *c1, const double *thr,
+                         int64_t points, int64_t n, typename P::Block *blk, double *x_out, double *y_out, void *rows_out,
+                         void *pos_out, int *n_blocks, int64_t *n_x, const char *fn) {
+  const int M = (int)points + 1, S = isotonic_tile(), T = (M + S - 1) / S;
+  int *hv[2] = {ctx->i_hull.p, ctx->i_hull.p + M};
+  int *hc[2] = {ctx->i_hull.p + 2 * (int64_t)M, ctx->i_hull.p + 2 * (int64_t)M + T};
+  int *excl = ctx->i_hull.p + 2 * (int64_t)M + 2 * (int64_t)T;
+  const size_t tile_bytes = (size_t)S * (2 * sizeof(typename P::Coord) + sizeof(int));
+  CU(cudaFuncSetAttribute(k_iso_tile<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_bytes));
+  k_iso_tile<P><<<isotonic_grid(ctx, T), kIsoThreads, tile_bytes, ctx->stream>>>(c0, c1, M, S, hv[0], hc[0]);
+  LAUNCHED();
+  int cur = 0;
+  for (int64_t W = S, h = T; h > 1; W *= 2, h = (h + 1) / 2, cur ^= 1) {
+    k_iso_merge<P><<<isotonic_grid(ctx, (h + 1) / 2), kIsoThreads, 0, ctx->stream>>>(c0, c1, (int)h, (int)W, hv[cur], hc[cur],
+                                                                                     hv[cur ^ 1], hc[cur ^ 1]);
+    LAUNCHED();
+  }
+  CU(cudaGetLastError());
+  int V = 0;
+  CU(cudaMemcpyAsync(&V, hc[cur], sizeof V, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  const int B = V - 1;   // the origin and the last point are always vertices: B >= 1
+  NEED(B >= 1 && B <= points, DSGD_ERR_CUDA, "%s: a hull of %d vertices over %lld points", fn, V, (long long)points);
+  size_t tmp = 0;
+  CU(scan_x_counts(ctx, nullptr, tmp, hv[cur], B, excl));
+  int rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn);
+  if (rc || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+  CU(scan_x_counts(ctx, ctx->m_tmp.p, tmp, hv[cur], B, excl));
+  double *X = ctx->i_out.p, *Y = ctx->i_out.p + n;
+  k_iso_emit<P><<<isotonic_grid(ctx, cdiv(B, 256)), 256, 0, ctx->stream>>>(hv[cur], B, excl, thr, c0, c1, X, Y, blk, blk + n,
+                                                                           ctx->i_ctl);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  unsigned long long nx = 0;
+  CU(cudaMemcpyAsync(&nx, ctx->i_ctl, sizeof nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(rows_out, blk, sizeof(typename P::Block) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(pos_out, blk + n, sizeof(typename P::Block) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  CU(cudaMemcpyAsync(x_out, X, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(y_out, Y, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  *n_blocks = B;
+  *n_x = (int64_t)nx;
+  return DSGD_OK;
+}
+
+// One isotonic fit over `rows`: the curve pass with its points left on the device, then the hull and the emit over its
+// counts (IsoCounts).
 static int isotonic_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *n_points_out, double *x_out,
                          double *y_out, int64_t *rows_out, int64_t *pos_out, int64_t *info_out, const char *fn) {
   const int64_t n = rows.n;
@@ -1922,46 +1991,12 @@ static int isotonic_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, in
   if ((rc = ctx->i_hull.grow(ctx, 5 * (n + 1), 1024)) || (rc = ctx->i_out.grow(ctx, 2 * n, 1024)) ||
       (rc = ctx->i_blk.grow(ctx, 2 * n, 1024)) || (rc = ctx->i_ctl.grow(ctx, 1, 1)))
     return rc;
-  const int M = (int)m + 1, S = isotonic_tile(), T = (M + S - 1) / S;
-  int *hv[2] = {ctx->i_hull.p, ctx->i_hull.p + M};
-  int *hc[2] = {ctx->i_hull.p + 2 * (int64_t)M, ctx->i_hull.p + 2 * (int64_t)M + T};
-  int *excl = ctx->i_hull.p + 2 * (int64_t)M + 2 * (int64_t)T;
-  k_iso_tile<<<isotonic_grid(ctx, T), kIsoThreads, (size_t)S * 20, ctx->stream>>>(ctx->c_tp, ctx->c_fp, M, S, hv[0], hc[0]);
-  LAUNCHED();
-  int cur = 0;
-  for (int64_t W = S, h = T; h > 1; W *= 2, h = (h + 1) / 2, cur ^= 1) {
-    k_iso_merge<<<isotonic_grid(ctx, (h + 1) / 2), kIsoThreads, 0, ctx->stream>>>(ctx->c_tp, ctx->c_fp, (int)h, (int)W,
-                                                                                  hv[cur], hc[cur], hv[cur ^ 1], hc[cur ^ 1]);
-    LAUNCHED();
-  }
-  CU(cudaGetLastError());
-  int V = 0;
-  CU(cudaMemcpyAsync(&V, hc[cur], sizeof V, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  const int B = V - 1;   // the origin and the last point are always vertices: B >= 1
-  NEED(B >= 1 && B <= m, DSGD_ERR_CUDA, "%s: a hull of %d vertices over %lld points", fn, V, (long long)m);
-  size_t tmp = 0;
-  CU(scan_x_counts(ctx, nullptr, tmp, hv[cur], B, excl));
-  if ((rc = fits_while_running(ctx, ctx->m_tmp.cap >= (int64_t)tmp, fn)) || (rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16)))
+  int B = 0;
+  if ((rc = isotonic_hull<IsoCounts>(ctx, ctx->c_tp, ctx->c_fp, ctx->c_thr, m, n, ctx->i_blk.p, x_out, y_out, rows_out,
+                                     pos_out, &B, n_points_out, fn)))
     return rc;
-  CU(scan_x_counts(ctx, ctx->m_tmp.p, tmp, hv[cur], B, excl));
-  double *X = ctx->i_out.p, *Y = ctx->i_out.p + n;
-  long long *br = ctx->i_blk.p, *bp = ctx->i_blk.p + n;
-  k_iso_emit<<<isotonic_grid(ctx, cdiv(B, 256)), 256, 0, ctx->stream>>>(hv[cur], B, excl, ctx->c_thr, ctx->c_tp, ctx->c_fp, X,
-                                                                         Y, br, bp, ctx->i_ctl);
-  LAUNCHED();
-  CU(cudaGetLastError());
-  unsigned long long nx = 0;
-  CU(cudaMemcpyAsync(&nx, ctx->i_ctl, sizeof nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(rows_out, br, sizeof(long long) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(pos_out, bp, sizeof(long long) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  CU(cudaMemcpyAsync(x_out, X, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(y_out, Y, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  *n_points_out = (int64_t)nx;
   info_out[0] = B;
-  info_out[1] = (int64_t)nx;
+  info_out[1] = *n_points_out;
   info_out[2] = n - nan;
   info_out[3] = nan;
   info_out[4] = m;
@@ -2054,46 +2089,6 @@ extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const
   return DSGD_OK;
 }
 
-// One quality pass over `rows` at the map (X, Y): k_iso_eval, k_calib_eval_finish, the block read back.
-static int isotonic_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, const double *X, const double *Y,
-                                 int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
-                                 double *bin_psum, int64_t *words_out, const char *fn) {
-  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
-  int rc = fits_while_running(ctx, ctx->k_eval, fn);
-  if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = isotonic_map(ctx, X, Y, k, fn)) ||
-      (rc = ctx->k_eval.grow(ctx, kCevWords, kCevWords)))
-    return rc;
-  CU(cudaMemsetAsync(ctx->k_eval, 0, sizeof(unsigned long long) * kCevWords, ctx->stream));
-  const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);
-  const double *mx = ctx->i_map.p, *my = ctx->i_map.p + k;
-  int ki = (int)k, nb = n_bins;
-  unsigned long long *blk = ctx->k_eval.p;
-  const uint32_t *rp16 = ctx->rp16.p;
-  const uint2 *pairs = ctx->pairs.p;
-  const int8_t *label = ctx->label.p;
-  const int32_t *ids = rows.ids;
-  int64_t rb = rows.row_begin, rn = rows.n;
-  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &mx, &my, &ki, &nb, &blk};
-  CU(isotonic_launch(k_iso_eval<true>, k_iso_eval<false>, grid, k, ctx->stream, args));
-  LAUNCHED();
-  k_calib_eval_finish<<<1, kCalMaxBins, 0, ctx->stream>>>(ctx->k_eval, n_bins);
-  LAUNCHED();
-  CU(cudaGetLastError());
-  unsigned long long h[kCevWords];
-  CU(cudaMemcpyAsync(h, ctx->k_eval, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  memcpy(sums_out, &h[kCevOutSums], 2 * sizeof(double));
-  for (int i = 0; i < n_bins; ++i) {
-    bin_rows[i] = (int64_t)h[kCevBinRows + i];
-    bin_pos[i] = (int64_t)h[kCevBinPos + i];
-  }
-  memcpy(bin_psum, &h[kCevOutPsum], (size_t)n_bins * sizeof(double));
-  words_out[0] = (int64_t)h[kCevRows];
-  words_out[1] = (int64_t)h[kCevNan];
-  words_out[2] = (int64_t)h[kCevInf];
-  return DSGD_OK;
-}
-
 #define ISO_EVAL_ARGS_OK()                                                                                              \
   do {                                                                                                                  \
     NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);  \
@@ -2108,7 +2103,8 @@ extern "C" int dsgd_eval_isotonic_calibration(dsgd_ctx *ctx, const double *w, in
   row_set rows;
   int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
   return rc ? rc
-            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
+                                             words_out, __func__);
 }
 
 extern "C" int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
@@ -2121,7 +2117,8 @@ extern "C" int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const doubl
   row_set rows;
   int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
   return rc ? rc
-            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
+                                             words_out, __func__);
 }
 
 extern "C" int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
@@ -2134,15 +2131,16 @@ extern "C" int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const doubl
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
   return rc ? rc
-            : isotonic_quality_pass(ctx, w, rows, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out, __func__);
+            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
+                                             words_out, __func__);
 }
 
 // ---- weighted isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.17) -----------------------------------------------
 
 // One weighted isotonic fit over `rows`: the weighted curve pass with its points left on the device; the total weight of
 // its non-NaN rows checked against the turn test's bound; every point's exact coordinates and the zero-weight points
-// dropped (k_iso_wpoint, a scan of the keep flags, k_iso_wpack); then the hull and the emit of the unweighted fit in their
-// weighted forms.
+// dropped (k_iso_wpoint, a scan of the keep flags, k_iso_wpack); then the hull and the emit over the kept points
+// (IsoWeights).
 static int isotonic_weighted_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *n_points_out, double *x_out,
                                   double *y_out, double *wrows_out, double *wpos_out, int64_t *info_out, double *wsums_out,
                                   const char *fn) {
@@ -2197,46 +2195,12 @@ static int isotonic_weighted_pass(dsgd_ctx *ctx, const double *w, const row_set 
   CU(cudaStreamSynchronize(ctx->stream));
   const int64_t kept = (int64_t)ctl[2];
   NEED(kept >= 1 && kept <= m, DSGD_ERR_CUDA, "%s: %lld points kept of %lld", fn, (long long)kept, (long long)m);
-  const int M = (int)kept + 1, S = isotonic_tile(), T = (M + S - 1) / S;
-  int *hv[2] = {ctx->i_hull.p, ctx->i_hull.p + M};
-  int *hc[2] = {ctx->i_hull.p + 2 * (int64_t)M, ctx->i_hull.p + 2 * (int64_t)M + T};
-  int *excl = ctx->i_hull.p + 2 * (int64_t)M + 2 * (int64_t)T;
-  const size_t tile_bytes = (size_t)S * (2 * sizeof(u256) + sizeof(int));
-  CU(cudaFuncSetAttribute(k_iso_wtile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_bytes));
-  k_iso_wtile<<<isotonic_grid(ctx, T), kIsoThreads, tile_bytes, ctx->stream>>>(qx, qy, M, S, hv[0], hc[0]);
-  LAUNCHED();
-  int cur = 0;
-  for (int64_t W = S, h = T; h > 1; W *= 2, h = (h + 1) / 2, cur ^= 1) {
-    k_iso_wmerge<<<isotonic_grid(ctx, (h + 1) / 2), kIsoThreads, 0, ctx->stream>>>(qx, qy, (int)h, (int)W, hv[cur], hc[cur],
-                                                                                   hv[cur ^ 1], hc[cur ^ 1]);
-    LAUNCHED();
-  }
-  CU(cudaGetLastError());
-  int V = 0;
-  CU(cudaMemcpyAsync(&V, hc[cur], sizeof V, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  const int B = V - 1;
-  NEED(B >= 1 && B <= kept, DSGD_ERR_CUDA, "%s: a hull of %d vertices over %lld points", fn, V, (long long)kept);
-  tmp = 0;
-  CU(scan_x_counts(ctx, nullptr, tmp, hv[cur], B, excl));
-  if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
-  CU(scan_x_counts(ctx, ctx->m_tmp.p, tmp, hv[cur], B, excl));
-  double *X = ctx->i_out.p, *Y = ctx->i_out.p + n, *bw = ctx->i_wblk.p, *bp = ctx->i_wblk.p + n;
-  k_iso_wemit<<<isotonic_grid(ctx, cdiv(B, 256)), 256, 0, ctx->stream>>>(hv[cur], B, excl, ctx->i_wthr, qx, qy, X, Y, bw, bp,
-                                                                          ctx->i_ctl);
-  LAUNCHED();
-  CU(cudaGetLastError());
-  unsigned long long nx = 0;
-  CU(cudaMemcpyAsync(&nx, ctx->i_ctl, sizeof nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(wrows_out, bw, sizeof(double) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(wpos_out, bp, sizeof(double) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  CU(cudaMemcpyAsync(x_out, X, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaMemcpyAsync(y_out, Y, sizeof(double) * (size_t)nx, cudaMemcpyDeviceToHost, ctx->stream));
-  CU(cudaStreamSynchronize(ctx->stream));
-  *n_points_out = (int64_t)nx;
+  int B = 0;
+  if ((rc = isotonic_hull<IsoWeights>(ctx, qx, qy, ctx->i_wthr, kept, n, ctx->i_wblk.p, x_out, y_out, wrows_out, wpos_out,
+                                      &B, n_points_out, fn)))
+    return rc;
   info_out[0] = B;
-  info_out[1] = (int64_t)nx;
+  info_out[1] = *n_points_out;
   info_out[2] = (int64_t)ctl[1];
   info_out[3] = words[kMetNan];
   info_out[4] = kept;

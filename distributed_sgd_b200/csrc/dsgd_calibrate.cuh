@@ -9,7 +9,9 @@
 //      launch.  Every evaluation of a point adds its six sums in signed fixed-point limbs (dsgd_fixed.cuh's cut), so they
 //      have the same bits for any grid, work split or row order; every CTA reads the same bits after a grid barrier and
 //      runs the same scalar fp64 code, so all CTAs take the same decisions and (A, B, F, iterations) are order-free too.
-// k_calib_eval is the quality pass at a given (A, B): Brier and log-loss sums in the same limbs, and M equal-width bins.
+// The fit is one kernel template, k_calib_fit<kW>, over counted rows (kW = false) and weighted rows (kW = true).
+// k_calib_eval<kIso, kSmem> (dsgd_isotonic.cuh, beside the maps it applies) is the quality pass at a given (A, B) or
+// isotonic map: Brier and log-loss sums in the same limbs, and M equal-width bins, into the CalibEvalWord block below.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -206,174 +208,17 @@ __device__ __forceinline__ void st_relaxed_gpu_u64(unsigned long long *p, unsign
 // The three lines rotate: evaluation e uses line e % 3.  After barrier e every CTA has finished reading line e - 1 (it read
 // it before it arrived), so block 0 zeroes that line then, for evaluation e + 2; its arrival at barrier e + 1 (release)
 // orders the zeroes before any CTA's REDs of evaluation e + 2.
-// k_calib_fit_w below is this kernel line for line but for its weighted lines: a change here belongs there too
-// (tests/test_calib_fit_twins.py holds the two bodies equal apart from those lines).
+//
+// kW: the weighted fit (DESIGN.md §4.17).  A CTA keeps f, c and y of each score in shared memory (17 bytes instead of 9, so
+// its cap is smaller); a row with R(c) = 0 is skipped before any term is formed; and each of the six terms is added as
+// R(fl(c term)).  The weights change only what a CTA adds to the line, never what it reads from it, so the invariant above
+// holds for both forms.
+template <bool kW>
 __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit(const CalibFitParams p) {
   extern __shared__ __align__(16) unsigned char cal_smem[];
   double *s_f = reinterpret_cast<double *>(cal_smem);
-  int8_t *s_y = reinterpret_cast<int8_t *>(s_f + p.smem_cap);
-  __shared__ unsigned long long s_red[kCalLineWords];    // the CTA's partial of one evaluation
-  __shared__ unsigned long long s_line[kCalLineWords];   // the accumulator line as read after the barrier
-  __shared__ double s_pt[2];                             // the point to evaluate next
-  __shared__ int s_done;                                 // 1: the fit ended; -1: the watchdog fired
-
-  const unsigned full = 0xffffffffu;
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int64_t G = gridDim.x, slice = (p.n + G - 1) / G;
-  const int64_t b = min(p.n, (int64_t)blockIdx.x * slice), e = min(p.n, b + slice);
-  const int m = (int)(e - b), in_smem = min(m, p.smem_cap);
-  for (int i = tid; i < in_smem; i += kCalThreads) {
-    s_f[i] = p.score[b + i];
-    s_y[i] = p.lab[b + i];
-  }
-  if (tid < kCalLineWords) s_red[tid] = 0ull;
-  if (tid == 0) {
-    s_pt[0] = 0.0;
-    s_pt[1] = p.b0;
-    s_done = 0;
-  }
-  __syncthreads();
-
-  // thread 0's state: the accepted point, its objective, the Newton direction from it and the line search's step
-  double A = 0.0, B = 0.0, F = 0.0, dA = 0.0, dB = 0.0, gd = 0.0, step = 1.0;
-  int iter = 0, status = kCalConverged;
-  for (unsigned ev = 0;; ++ev) {
-    const double pa = s_pt[0], pb = s_pt[1];
-    long long lim[kCalSums][kLossLimbs];
-#pragma unroll
-    for (int s = 0; s < kCalSums; ++s)
-#pragma unroll
-      for (int k = 0; k < kLossLimbs; ++k) lim[s][k] = 0;
-    unsigned long long ovf = 0;
-    for (int i = tid; i < m; i += kCalThreads) {
-      const double f = i < in_smem ? s_f[i] : __ldcg(p.score + b + i);
-      const int8_t y = i < in_smem ? s_y[i] : __ldcg(p.lab + b + i);
-      if (isnan(f)) continue;
-      const double t = y > 0 ? p.t_pos : p.t_neg;
-      const double z = pa * f + pb;
-      double term, pr, qr;   // pr = 1 / (1 + exp(z)) = P(y = +1), qr = 1 - pr, each from the half that does not cancel
-      if (z >= 0.0) {
-        const double ex = exp(-z), den = 1.0 + ex;
-        term = t * z + log1p(ex);
-        pr = ex / den;
-        qr = 1.0 / den;
-      } else {
-        const double ex = exp(z), den = 1.0 + ex;
-        term = (t - 1.0) * z + log1p(ex);
-        pr = 1.0 / den;
-        qr = ex / den;
-      }
-      const double d1 = t - pr, d2 = pr * qr;
-      cal_add(lim[0], ovf, term);
-      cal_add(lim[1], ovf, f * d1);
-      cal_add(lim[2], ovf, d1);
-      cal_add(lim[3], ovf, (f * f) * d2);
-      cal_add(lim[4], ovf, f * d2);
-      cal_add(lim[5], ovf, d2);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      ovf += __shfl_xor_sync(full, ovf, o);
-#pragma unroll
-      for (int s = 0; s < kCalSums; ++s)
-#pragma unroll
-        for (int k = 0; k < kLossLimbs; ++k) lim[s][k] += __shfl_xor_sync(full, lim[s][k], o);   // below 2^45: no carry lost
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int s = 0; s < kCalSums; ++s)
-#pragma unroll
-        for (int k = 0; k < kLossLimbs; ++k)
-          if (lim[s][k]) atomicAdd(&s_red[s * kLossLimbs + k], (unsigned long long)lim[s][k]);
-      if (ovf) atomicAdd(&s_red[kCalLineWords - 1], ovf);
-    }
-    __syncthreads();
-    unsigned long long *line = p.acc + (ev % 3u) * kCalLineStride;
-    if (tid < kCalLineWords) {
-      const unsigned long long v = s_red[tid];
-      if (v) red_add_u64(line + tid, v);
-      s_red[tid] = 0ull;
-    }
-    __syncthreads();
-    if (tid == 0 && !grid_barrier_arrive_wait(p.bar, (ev + 1u) * (unsigned)G, p.abort_flag, p.timeout_cycles)) s_done = -1;
-    __syncthreads();
-    if (s_done < 0) return;
-    if (tid < kCalLineWords) {
-      s_line[tid] = ld_relaxed_gpu_u64(line + tid);
-      if (blockIdx.x == 0) st_relaxed_gpu_u64(p.acc + ((ev + 2u) % 3u) * kCalLineStride + tid, 0ull);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      double S[kCalSums];
-      bool finite = s_line[kCalLineWords - 1] == 0ull;
-#pragma unroll
-      for (int s = 0; s < kCalSums; ++s) S[s] = cal_value(s_line + s * kLossLimbs);
-      bool accept = false, done = false;
-      if (!finite) {
-        status = kCalNonFinite;
-        A = B = F = __longlong_as_double(0x7ff8000000000000ll);
-        done = true;
-      } else if (ev == 0) {
-        accept = true;
-      } else if (S[0] < F + 1e-4 * step * gd) {
-        accept = true;
-        ++iter;
-      } else {
-        step = step / 2.0;
-        if (step < 1e-10) {
-          status = kCalLineSearch;
-          done = true;
-        }
-      }
-      if (accept) {
-        A = pa; B = pb; F = S[0];
-        const double g1 = S[1], g2 = S[2], h11 = S[3] + 1e-12, h21 = S[4], h22 = S[5] + 1e-12;
-        if (fabs(g1) < 1e-5 && fabs(g2) < 1e-5) {
-          status = kCalConverged;
-          done = true;
-        } else if (iter >= kCalMaxIter) {
-          status = kCalIterLimit;
-          done = true;
-        } else {
-          const double det = h11 * h22 - h21 * h21;
-          dA = -(h22 * g1 - h21 * g2) / det;
-          dB = -(h11 * g2 - h21 * g1) / det;
-          gd = g1 * dA + g2 * dB;
-          step = 1.0;
-        }
-      }
-      if (done) {
-        s_done = 1;
-      } else {
-        s_pt[0] = A + step * dA;
-        s_pt[1] = B + step * dB;
-      }
-    }
-    __syncthreads();
-    if (s_done) {
-      if (blockIdx.x == 0 && tid == 0) {
-        p.out[kCalOutA] = (unsigned long long)__double_as_longlong(A);
-        p.out[kCalOutB] = (unsigned long long)__double_as_longlong(B);
-        p.out[kCalOutF] = (unsigned long long)__double_as_longlong(F);
-        p.out[kCalOutIter] = (unsigned long long)iter;
-        p.out[kCalOutStatus] = (unsigned long long)status;
-        p.out[kCalOutEvals] = (unsigned long long)ev + 1ull;
-      }
-      return;
-    }
-  }
-}
-
-// k_calib_fit_w: the weighted fit (DESIGN.md §4.17), k_calib_fit line for line but for three things.  A CTA keeps f, c and y
-// of each score in shared memory (17 bytes instead of 9, so its cap is smaller); a row with R(c) = 0 is skipped before any
-// term is formed; and each of the six terms is added as R(fl(c term)).  The weights change only what a CTA adds to the
-// line, never what it reads from it, so the invariant above holds unchanged.  (A separate kernel rather than a template
-// form: every template form of k_calib_fit compiled its unweighted instructions differently.)
-__global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitParams p) {
-  extern __shared__ __align__(16) unsigned char cal_smem[];
-  double *s_f = reinterpret_cast<double *>(cal_smem);
   double *s_c = s_f + p.smem_cap;
-  int8_t *s_y = reinterpret_cast<int8_t *>(s_c + p.smem_cap);
+  int8_t *s_y = reinterpret_cast<int8_t *>(kW ? s_c + p.smem_cap : s_c);
   __shared__ unsigned long long s_red[kCalLineWords];    // the CTA's partial of one evaluation
   __shared__ unsigned long long s_line[kCalLineWords];   // the accumulator line as read after the barrier
   __shared__ double s_pt[2];                             // the point to evaluate next
@@ -386,7 +231,7 @@ __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitPa
   const int m = (int)(e - b), in_smem = min(m, p.smem_cap);
   for (int i = tid; i < in_smem; i += kCalThreads) {
     s_f[i] = p.score[b + i];
-    s_c[i] = p.cw[b + i];
+    if constexpr (kW) s_c[i] = p.cw[b + i];
     s_y[i] = p.lab[b + i];
   }
   if (tid < kCalLineWords) s_red[tid] = 0ull;
@@ -412,8 +257,15 @@ __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitPa
       const double f = i < in_smem ? s_f[i] : __ldcg(p.score + b + i);
       const int8_t y = i < in_smem ? s_y[i] : __ldcg(p.lab + b + i);
       if (isnan(f)) continue;
-      const double c = i < in_smem ? s_c[i] : __ldcg(p.cw + b + i);
-      if (rint(c * 0x1p160) == 0.0) continue;   // R(c) = 0: the row adds exactly 0 to every sum
+      double c = 1.0;
+      if constexpr (kW) {
+        c = i < in_smem ? s_c[i] : __ldcg(p.cw + b + i);
+        if (rint(c * 0x1p160) == 0.0) continue;   // R(c) = 0: the row adds exactly 0 to every sum
+      }
+      auto cw = [&](double v) {   // a term as it is added: c v in the weighted fit
+        if constexpr (kW) return c * v;
+        else return v;
+      };
       const double t = y > 0 ? p.t_pos : p.t_neg;
       const double z = pa * f + pb;
       double term, pr, qr;   // pr = 1 / (1 + exp(z)) = P(y = +1), qr = 1 - pr, each from the half that does not cancel
@@ -429,12 +281,12 @@ __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitPa
         qr = ex / den;
       }
       const double d1 = t - pr, d2 = pr * qr;
-      cal_add(lim[0], ovf, c * term);
-      cal_add(lim[1], ovf, c * (f * d1));
-      cal_add(lim[2], ovf, c * d1);
-      cal_add(lim[3], ovf, c * ((f * f) * d2));
-      cal_add(lim[4], ovf, c * (f * d2));
-      cal_add(lim[5], ovf, c * d2);
+      cal_add(lim[0], ovf, cw(term));
+      cal_add(lim[1], ovf, cw(f * d1));
+      cal_add(lim[2], ovf, cw(d1));
+      cal_add(lim[3], ovf, cw((f * f) * d2));
+      cal_add(lim[4], ovf, cw(f * d2));
+      cal_add(lim[5], ovf, cw(d2));
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -529,105 +381,22 @@ __global__ void __launch_bounds__(kCalThreads, 1) k_calib_fit_w(const CalibFitPa
   }
 }
 
-// ---- k_calib_eval ------------------------------------------------------------------------------------------------
+// ---- the quality pass's block (k_calib_eval, dsgd_isotonic.cuh) ---------------------------------------------------
 constexpr int kCalMaxBins = 64;
 // Words of the quality pass's block
 enum CalibEvalWord : int {
   kCevBrier = 0,                                   // [0, 7): limbs and overflow count of sum (p - o)^2
-  kCevLog = kLossAccWords,                         // [7, 14): of sum softplus(+-z)
+  kCevLog = kLossAccWords,                         // [7, 14): of the finite log-loss terms
   kCevRows = 2 * kLossAccWords,                    // rows used
-  kCevNan = kCevRows + 1,                          // rows left out (a f + b is NaN)
+  kCevNan = kCevRows + 1,                          // rows left out (their argument is NaN)
   kCevBinRows = 16,                                // [16, 80)
   kCevBinPos = kCevBinRows + kCalMaxBins,          // [80, 144)
   kCevBinLimbs = kCevBinPos + kCalMaxBins,         // [144, 528): six limbs of sum p per bin
   kCevOutSums = kCevBinLimbs + kCalMaxBins * kLossLimbs,   // [528, 530): Brier and log-loss sums as the bits of doubles
   kCevOutPsum = kCevOutSums + 2,                   // [530, 594): sum p per bin, likewise (k_calib_eval_finish)
+  kCevInf = kCevOutPsum + kCalMaxBins,             // 594: rows whose log-loss term is infinite (an isotonic map only)
   kCevWords = 640
 };
-
-// The quality pass over rows samples[0..n) (samples == nullptr: rows [row_begin, row_begin + n)) at (a, b) with n_bins
-// equal-width bins: z = a f + b, p = sigmoid(-z), bin = min(n_bins - 1, floor(p n_bins)).  Positions are taken as in
-// k_metrics_score.  The two sums go to register limbs; the bins to shared memory: rows and positives as integers, sum p as
-// limb words added with shared u64 atomics (p <= 1: each limb adds at most 2^40, so a CTA's words hold 2^24 rows without a
-// wrap, and a grid of 8 CTAs per SM leaves a CTA fewer than that for any 32-bit row count).  The CTA propagates each bin's
-// carries and adds its words to the block with REDs.
-__global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                                    const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                                    int64_t row_begin, int64_t n, const double *__restrict__ w, double a,
-                                                    double b, int n_bins, unsigned long long *__restrict__ blk) {
-  __shared__ unsigned long long s_rows[kCalMaxBins], s_pos[kCalMaxBins], s_lim[kCalMaxBins][kLossLimbs];
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < kCalMaxBins; i += blockDim.x) {
-    s_rows[i] = 0ull;
-    s_pos[i] = 0ull;
-#pragma unroll
-    for (int k = 0; k < kLossLimbs; ++k) s_lim[i][k] = 0ull;
-  }
-  __syncthreads();
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  unsigned long long lb[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ll[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_b = 0, ovf_l = 0;
-  unsigned c_rows = 0, c_nan = 0;
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_margin(rp16, pairs, w, r, lane);
-      if (lane == j) dot_own = dot;
-    }
-    if (!mine) continue;
-    const double z = a * dot_own + b;
-    if (isnan(z)) { ++c_nan; continue; }
-    const bool pos = label[r_own] > 0;
-    const double pr = sigmoid(-z), o = pos ? 1.0 : 0.0, dlt = pr - o;
-    ++c_rows;
-    acc_add_local(lb, ovf_b, dlt * dlt);
-    acc_add_local(ll, ovf_l, softplus(pos ? z : -z));
-    int bin = (int)floor(pr * (double)n_bins);
-    bin = bin < n_bins - 1 ? bin : n_bins - 1;
-    atomicAdd(&s_rows[bin], 1ull);
-    if (pos) atomicAdd(&s_pos[bin], 1ull);
-    acc_cut(pr, [&](int k, double limb) {
-      if (limb != 0.0) atomicAdd(&s_lim[bin][k], (unsigned long long)(long long)limb);
-    });
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    ovf_b += __shfl_xor_sync(full, ovf_b, o);
-    ovf_l += __shfl_xor_sync(full, ovf_l, o);
-#pragma unroll
-    for (int k = 0; k < kLossLimbs; ++k) {
-      lb[k] += __shfl_xor_sync(full, lb[k], o);
-      ll[k] += __shfl_xor_sync(full, ll[k], o);
-    }
-  }
-  c_rows = __reduce_add_sync(full, c_rows);
-  c_nan = __reduce_add_sync(full, c_nan);
-  if (lane == 0) {
-    acc_flush_local(blk + kCevBrier, lb, ovf_b);
-    acc_flush_local(blk + kCevLog, ll, ovf_l);
-    if (c_rows) atomicAdd(&blk[kCevRows], (unsigned long long)c_rows);
-    if (c_nan) atomicAdd(&blk[kCevNan], (unsigned long long)c_nan);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < n_bins; i += blockDim.x) {
-    if (!s_rows[i]) continue;
-    red_add_u64(blk + kCevBinRows + i, s_rows[i]);
-    if (s_pos[i]) red_add_u64(blk + kCevBinPos + i, s_pos[i]);
-    unsigned long long q[kLossLimbs];
-#pragma unroll
-    for (int k = 0; k < kLossLimbs; ++k) q[k] = s_lim[i][k];
-    acc_carry(q);
-#pragma unroll
-    for (int k = 0; k < kLossLimbs; ++k)
-      if (q[k]) red_add_u64(blk + kCevBinLimbs + i * kLossLimbs + k, q[k]);
-  }
-}
 
 // The sums of a quality pass as doubles: thread 0 the Brier and log-loss sums, thread i sum p of bin i.
 __global__ void k_calib_eval_finish(unsigned long long *__restrict__ blk, int n_bins) {

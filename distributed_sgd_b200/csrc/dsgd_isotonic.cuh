@@ -11,7 +11,9 @@
 //      binary search over the left hull with a binary search over the right one inside it, then the surviving vertices
 //      compacted into the other of two ping-pong buffers.
 //   3. an exclusive scan of every block's X count (1 or 2) and k_iso_emit: X, Y and the block counts, ascending in s.
-// k_iso_prob and k_iso_eval apply a map (X, Y) to rows as numpy.interp does.
+// The three hull kernels are templates over a point set: k_iso_tile<P>, k_iso_merge<P> and k_iso_emit<P> with P = IsoCounts
+// here, or IsoWeights for the weighted fit (DESIGN.md §4.17).  k_iso_prob<kSmem> applies a map (X, Y) to rows as
+// numpy.interp does, and k_calib_eval<kIso, kSmem> is the quality pass at a sigmoid or at a map.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,40 +25,71 @@ namespace dsgd {
 
 constexpr int kIsoTileMax = 2048;    // points of a tile in shared memory: 16 bytes of coordinates and 4 of stack each (40 KB)
 constexpr int kIsoThreads = 256;
-constexpr int kIsoSmemPoints = 6144; // (X, Y) pairs k_iso_prob / k_iso_eval keep in shared memory (96 KB); more stay in L2
+constexpr int kIsoSmemPoints = 6144; // (X, Y) pairs k_iso_prob / k_calib_eval keep in shared memory (96 KB); more stay in L2
 
-// The coordinates of point i: the origin, or (tp + fp, tp) of curve point i - 1
-__device__ __forceinline__ void iso_point(const long long *__restrict__ tp, const long long *__restrict__ fp, int i,
-                                          long long &x, long long &y) {
-  if (i == 0) { x = 0; y = 0; return; }
-  y = tp[i - 1];
-  x = y + fp[i - 1];
-}
-// (a - o) x (b - o): > 0 when b lies strictly above the line from o through a (x increasing), 0 when the three are collinear.
-// Every coordinate is below 2^31, so each product is below 2^62 and the difference is exact.
-__device__ __forceinline__ long long iso_cross(long long ox, long long oy, long long ax, long long ay, long long bx,
-                                               long long by) {
-  return (ax - ox) * (by - oy) - (ay - oy) * (bx - ox);
-}
+// ---- point sets ----------------------------------------------------------------------------------------------------
+// The hull kernels are templates over a point set P: IsoCounts here (the fit over counted rows) or IsoWeights below (the
+// fit over weighted rows).  A kernel takes P's two arrays and P gives
+//   point(i, x, y): the coordinates of point i (point 0 is the origin), of type P::Coord;
+//   P::Ref: how the hull passes a coordinate it already holds (an int64 by value, a u256 by reference: a copy spills);
+//   turn(o, a, b): a value > 0 when b lies strictly above the line from o through a, 0 when the three are collinear and
+//   < 0 below, for o before a and b along the curve;
+//   above(v, u, r): a value > 0 when u lies strictly above the line from v through r, for v before u and r (the bridge's
+//   test: the sign of (r - v) x (u - v));
+//   block(x0, y0, x1, y1, rows, pos): the values k_iso_emit writes for the hull segment from (x0, y0) to (x1, y1), of type
+//   P::Block, and it returns the segment's probability p.
 
+// Point i: the origin, or (tp + fp, tp) of curve point i - 1.  A block's values are its rows and positives,
+// p = fl(pos / rows).
+struct IsoCounts {
+  using Coord = long long;
+  using Ref = long long;
+  using Block = long long;
+  const long long *__restrict__ tp, *__restrict__ fp;
+  __device__ __forceinline__ void point(int i, long long &x, long long &y) const {
+    if (i == 0) { x = 0; y = 0; return; }
+    y = tp[i - 1];
+    x = y + fp[i - 1];
+  }
+  // (a - o) x (b - o).  Every coordinate is below 2^31, so each product is below 2^62 and the difference is exact.
+  __device__ __forceinline__ static long long turn(Ref ox, Ref oy, Ref ax, Ref ay, Ref bx, Ref by) {
+    return (ax - ox) * (by - oy) - (ay - oy) * (bx - ox);
+  }
+  __device__ __forceinline__ static long long above(Ref vx, Ref vy, Ref ux, Ref uy, Ref rx, Ref ry) {
+    return turn(vx, vy, rx, ry, ux, uy);   // (r - v) x (u - v)
+  }
+  __device__ __forceinline__ static double block(Ref x0, Ref y0, Ref x1, Ref y1, Block &rows, Block &pos) {
+    rows = x1 - x0;
+    pos = y1 - y0;
+    return (double)pos / (double)rows;
+  }
+};
+
+// ---- the hull ------------------------------------------------------------------------------------------------------
+// Every hull kernel takes the point set's two arrays (c0, c1): (tp, fp) of IsoCounts or (qx, qy) of IsoWeights.
 // Tile t of S points [t S, min(M, (t + 1) S)): its upper hull by the monotone chain (a point is popped when it lies on or
 // below the chord of its neighbours), vertex indices into hv[t S ..) and their count into hc[t].  Grid-stride over tiles.
-__global__ void __launch_bounds__(kIsoThreads) k_iso_tile(const long long *__restrict__ tp, const long long *__restrict__ fp,
-                                                          int M, int S, int *__restrict__ hv, int *__restrict__ hc) {
+// Shared memory: S (2 sizeof(P::Coord) + 4) bytes.
+template <class P>
+__global__ void __launch_bounds__(kIsoThreads) k_iso_tile(const typename P::Coord *__restrict__ c0,
+                                                          const typename P::Coord *__restrict__ c1, int M, int S,
+                                                          int *__restrict__ hv, int *__restrict__ hc) {
+  using Coord = typename P::Coord;
+  const P pts{c0, c1};
   extern __shared__ __align__(16) unsigned char iso_smem[];
-  long long *sx = reinterpret_cast<long long *>(iso_smem), *sy = sx + S;
+  Coord *sx = reinterpret_cast<Coord *>(iso_smem), *sy = sx + S;
   int *st = reinterpret_cast<int *>(sy + S);
   __shared__ int s_top;
   const int T = (M + S - 1) / S;
   for (int t = blockIdx.x; t < T; t += gridDim.x) {
     const int b = t * S, len = min(S, M - b);
-    for (int j = threadIdx.x; j < len; j += blockDim.x) iso_point(tp, fp, b + j, sx[j], sy[j]);
+    for (int j = threadIdx.x; j < len; j += blockDim.x) pts.point(b + j, sx[j], sy[j]);
     __syncthreads();
     if (threadIdx.x == 0) {
       int top = 0;
       for (int j = 0; j < len; ++j) {
-        const long long x = sx[j], y = sy[j];
-        while (top >= 2 && iso_cross(sx[st[top - 2]], sy[st[top - 2]], sx[st[top - 1]], sy[st[top - 1]], x, y) >= 0) --top;
+        typename P::Ref x = sx[j], y = sy[j];
+        while (top >= 2 && P::turn(sx[st[top - 2]], sy[st[top - 2]], sx[st[top - 1]], sy[st[top - 1]], x, y) >= 0) --top;
         st[top++] = j;
       }
       s_top = top;
@@ -74,10 +107,13 @@ __global__ void __launch_bounds__(kIsoThreads) k_iso_tile(const long long *__res
 // with r_(j+1) strictly below the line v -> r_j (the last of two collinear tangent points).  The bridge's left end: the
 // first i with l_(i+1) not strictly above the line l_i -> r_(j(l_i)), which holds for every i after it and for none before
 // it; the merged hull is l_0 .. l_i, r_(j(l_i)) .. r_(b-1).
-__global__ void __launch_bounds__(kIsoThreads) k_iso_merge(const long long *__restrict__ tp, const long long *__restrict__ fp,
-                                                           int n_hulls, int W, const int *__restrict__ hv_in,
-                                                           const int *__restrict__ hc_in, int *__restrict__ hv_out,
-                                                           int *__restrict__ hc_out) {
+template <class P>
+__global__ void __launch_bounds__(kIsoThreads) k_iso_merge(const typename P::Coord *__restrict__ c0,
+                                                           const typename P::Coord *__restrict__ c1, int n_hulls, int W,
+                                                           const int *__restrict__ hv_in, const int *__restrict__ hc_in,
+                                                           int *__restrict__ hv_out, int *__restrict__ hc_out) {
+  using Coord = typename P::Coord;
+  const P pts{c0, c1};
   __shared__ int s_br[2];
   const int pairs = (n_hulls + 1) / 2;
   for (int p = blockIdx.x; p < pairs; p += gridDim.x) {
@@ -89,28 +125,28 @@ __global__ void __launch_bounds__(kIsoThreads) k_iso_merge(const long long *__re
     if (threadIdx.x == 0) {
       int i_end = a - 1, j_end = 0;
       if (!single) {
-        auto tangent = [&](long long vx, long long vy) {
+        auto tangent = [&](typename P::Ref vx, typename P::Ref vy) {
           int lo = 0, hi = b - 1;
           while (lo < hi) {
             const int mid = (lo + hi) >> 1;
-            long long x0, y0, x1, y1;
-            iso_point(tp, fp, R[mid], x0, y0);
-            iso_point(tp, fp, R[mid + 1], x1, y1);
-            if (iso_cross(vx, vy, x0, y0, x1, y1) >= 0) lo = mid + 1; else hi = mid;
+            Coord x0, y0, x1, y1;
+            pts.point(R[mid], x0, y0);
+            pts.point(R[mid + 1], x1, y1);
+            if (P::turn(vx, vy, x0, y0, x1, y1) >= 0) lo = mid + 1; else hi = mid;
           }
           return lo;
         };
         int lo = 0, hi = a - 1;
         while (lo < hi) {
           const int mid = (lo + hi) >> 1;
-          long long vx, vy, ux, uy, rx, ry;
-          iso_point(tp, fp, L[mid], vx, vy);
-          iso_point(tp, fp, L[mid + 1], ux, uy);
-          iso_point(tp, fp, R[tangent(vx, vy)], rx, ry);
-          if (iso_cross(vx, vy, rx, ry, ux, uy) > 0) lo = mid + 1; else hi = mid;
+          Coord vx, vy, ux, uy, rx, ry;
+          pts.point(L[mid], vx, vy);
+          pts.point(L[mid + 1], ux, uy);
+          pts.point(R[tangent(vx, vy)], rx, ry);
+          if (P::above(vx, vy, ux, uy, rx, ry) > 0) lo = mid + 1; else hi = mid;
         }
-        long long vx, vy;
-        iso_point(tp, fp, L[lo], vx, vy);
+        Coord vx, vy;
+        pts.point(L[lo], vx, vy);
         i_end = lo;
         j_end = tangent(vx, vy);
       }
@@ -138,21 +174,24 @@ struct iso_x_count {
   }
 };
 
-// Block o (ascending score) is hull segment b = B - 1 - o, from vertex h_b to h_(b+1): curve points h_b .. h_(b+1) - 1, its
-// highest score thr[h_b] and its lowest thr[h_(b+1) - 1].  p = fl(positives / rows).  excl: the exclusive scan of
-// iso_x_count; the last block writes the number of X entries to *n_x.
+// Block o (ascending score) is hull segment b = B - 1 - o, from vertex h_b to h_(b+1): points h_b .. h_(b+1) - 1 of thr, its
+// highest score thr[h_b] and its lowest thr[h_(b+1) - 1]; P::block gives its p and the values blk_rows[o] and blk_pos[o].
+// excl: the exclusive scan of iso_x_count; the last block writes the number of X entries to *n_x.
+template <class P>
 __global__ void __launch_bounds__(256) k_iso_emit(const int *__restrict__ h, int B, const int *__restrict__ excl,
-                                                  const double *__restrict__ thr, const long long *__restrict__ tp,
-                                                  const long long *__restrict__ fp, double *__restrict__ X,
-                                                  double *__restrict__ Y, long long *__restrict__ blk_rows,
-                                                  long long *__restrict__ blk_pos, unsigned long long *__restrict__ n_x) {
+                                                  const double *__restrict__ thr, const typename P::Coord *__restrict__ c0,
+                                                  const typename P::Coord *__restrict__ c1, double *__restrict__ X,
+                                                  double *__restrict__ Y, typename P::Block *__restrict__ blk_rows,
+                                                  typename P::Block *__restrict__ blk_pos,
+                                                  unsigned long long *__restrict__ n_x) {
+  const P pts{c0, c1};
   for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < B; o += gridDim.x * blockDim.x) {
     const int b = B - 1 - o, i0 = h[b], i1 = h[b + 1];
-    long long x0, y0, x1, y1;
-    iso_point(tp, fp, i0, x0, y0);
-    iso_point(tp, fp, i1, x1, y1);
-    const long long rows = x1 - x0, pos = y1 - y0;
-    const double p = (double)pos / (double)rows;
+    typename P::Coord x0, y0, x1, y1;
+    pts.point(i0, x0, y0);
+    pts.point(i1, x1, y1);
+    typename P::Block rows, pos;
+    const double p = P::block(x0, y0, x1, y1, rows, pos);
     blk_rows[o] = rows;
     blk_pos[o] = pos;
     const int at = excl[o];
@@ -227,17 +266,22 @@ __global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ r
   }
 }
 
-// The quality pass at the map (X, Y): the block of k_calib_eval (CalibEvalWord) with p = interp(s), s = -(x . w); a NaN s
-// leaves the row out.  The log-loss term is -log p (o = 1) or -log1p(-p) (o = 0); a row whose term is infinite (p = 0 with
-// o = 1, p = 1 with o = 0) is counted in kCevInf and adds nothing to the sum.  Positions as in k_calib_eval.
-constexpr int kCevInf = kCevOutPsum + kCalMaxBins;
-static_assert(kCevInf < kCevWords, "the infinite-term count sits after the finished sums");
-template <bool kSmem>
-__global__ void __launch_bounds__(256) k_iso_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
-                                                  const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
-                                                  int64_t row_begin, int64_t n, const double *__restrict__ w,
-                                                  const double *__restrict__ X, const double *__restrict__ Y, int k,
-                                                  int n_bins, unsigned long long *__restrict__ blk) {
+// ---- the quality pass (dsgd_eval_calibration*, dsgd_eval_isotonic_calibration*) --------------------------------------
+// The quality pass over rows samples[0..n) (samples == nullptr: rows [row_begin, row_begin + n)) with n_bins equal-width
+// bins into the CalibEvalWord block: bin = min(n_bins - 1, floor(p n_bins)).  At a sigmoid (kIso = false): z = a f + b,
+// p = sigmoid(-z) and the log-loss term softplus(+-z); a NaN z leaves the row out.  At the map (X, Y) (kIso): p = interp(s),
+// s = -f, and the term -log p (o = 1) or -log1p(-p) (o = 0); a NaN s leaves the row out, and a row whose term is infinite
+// (p = 0 with o = 1, p = 1 with o = 0) is counted in kCevInf and adds nothing to the sum.  Positions are taken as in
+// k_metrics_score.  The two sums go to register limbs; the bins to shared memory: rows and positives as integers, sum p as
+// limb words added with shared u64 atomics (p <= 1: each limb adds at most 2^40, so a CTA's words hold 2^24 rows without a
+// wrap, and a grid of 8 CTAs per SM leaves a CTA fewer than that for any 32-bit row count).  The CTA propagates each bin's
+// carries and adds its words to the block with REDs.
+template <bool kIso, bool kSmem>
+__global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                    const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                    int64_t row_begin, int64_t n, const double *__restrict__ w, double a,
+                                                    double b, const double *__restrict__ X, const double *__restrict__ Y,
+                                                    int k, int n_bins, unsigned long long *__restrict__ blk) {
   __shared__ unsigned long long s_rows[kCalMaxBins], s_pos[kCalMaxBins], s_lim[kCalMaxBins][kLossLimbs];
   const double *xs, *ys;
   iso_stage<kSmem>(X, Y, k, xs, ys);
@@ -266,14 +310,14 @@ __global__ void __launch_bounds__(256) k_iso_eval(const uint32_t *__restrict__ r
       if (lane == j) dot_own = dot;
     }
     if (!mine) continue;
-    const double s = -dot_own;
-    if (isnan(s)) { ++c_nan; continue; }
+    const double z = kIso ? -dot_own : a * dot_own + b;   // kIso: the score s
+    if (isnan(z)) { ++c_nan; continue; }
     const bool pos = label[r_own] > 0;
-    const double pr = iso_interp(s, xs, ys, k), o = pos ? 1.0 : 0.0, dlt = pr - o;
+    const double pr = kIso ? iso_interp(z, xs, ys, k) : sigmoid(-z), o = pos ? 1.0 : 0.0, dlt = pr - o;
     ++c_rows;
     acc_add_local(lb, ovf_b, dlt * dlt);
-    const double term = pos ? -log(pr) : -log1p(-pr);
-    if (isinf(term)) ++c_inf;
+    const double term = kIso ? (pos ? -log(pr) : -log1p(-pr)) : softplus(pos ? z : -z);
+    if (kIso && isinf(term)) ++c_inf;
     else acc_add_local(ll, ovf_l, term);
     int bin = (int)floor(pr * (double)n_bins);
     bin = bin < n_bins - 1 ? bin : n_bins - 1;
@@ -295,13 +339,13 @@ __global__ void __launch_bounds__(256) k_iso_eval(const uint32_t *__restrict__ r
   }
   c_rows = __reduce_add_sync(full, c_rows);
   c_nan = __reduce_add_sync(full, c_nan);
-  c_inf = __reduce_add_sync(full, c_inf);
+  if constexpr (kIso) c_inf = __reduce_add_sync(full, c_inf);
   if (lane == 0) {
     acc_flush_local(blk + kCevBrier, lb, ovf_b);
     acc_flush_local(blk + kCevLog, ll, ovf_l);
     if (c_rows) atomicAdd(&blk[kCevRows], (unsigned long long)c_rows);
     if (c_nan) atomicAdd(&blk[kCevNan], (unsigned long long)c_nan);
-    if (c_inf) atomicAdd(&blk[kCevInf], (unsigned long long)c_inf);
+    if (kIso && c_inf) atomicAdd(&blk[kCevInf], (unsigned long long)c_inf);
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n_bins; i += blockDim.x) {
@@ -356,18 +400,6 @@ __device__ __forceinline__ void u256_mul(const u256 &a, const u256 &b, unsigned 
     }
     r[i + 4] = carry;
   }
-}
-// The sign of (a - o) x (b - o) for points o, a, b in increasing order along the curve: +1 when b lies strictly above the
-// line from o through a, 0 when the three are collinear, -1 below.
-__device__ __forceinline__ int iso_wturn(const u256 &ox, const u256 &oy, const u256 &ax, const u256 &ay, const u256 &bx,
-                                         const u256 &by) {
-  unsigned long long p[8], q[8];
-  u256_mul(u256_sub(ax, ox), u256_sub(by, oy), p);
-  u256_mul(u256_sub(ay, oy), u256_sub(bx, ox), q);
-#pragma unroll
-  for (int i = 7; i >= 0; --i)
-    if (p[i] != q[i]) return p[i] > q[i] ? 1 : -1;
-  return 0;
 }
 // read() of an exact sum given as a u256 in units of 2^-160: its six 40-bit limbs converted as acc_value converts them
 __device__ __forceinline__ double u256_read(const u256 &v) {
@@ -452,125 +484,42 @@ __global__ void __launch_bounds__(256) k_iso_wpack(int64_t m, const int *__restr
     if (k == m - 1) *n_kept = (unsigned long long)(excl[k] + keep[k]);
   }
 }
-// Hull point i: the origin, or kept point i - 1
-__device__ __forceinline__ void iso_wpt(const u256 *__restrict__ qx, const u256 *__restrict__ qy, int i, u256 &x, u256 &y) {
-  if (i == 0) { x = u256{{0, 0, 0, 0}}; y = x; return; }
-  x = qx[i - 1];
-  y = qy[i - 1];
-}
-// k_iso_tile over the weighted points: the same monotone chain with the exact multi-word turn test; 68 bytes a point
-__global__ void __launch_bounds__(kIsoThreads) k_iso_wtile(const u256 *__restrict__ qx, const u256 *__restrict__ qy, int M,
-                                                           int S, int *__restrict__ hv, int *__restrict__ hc) {
-  extern __shared__ __align__(16) unsigned char iso_wsmem[];
-  u256 *sx = reinterpret_cast<u256 *>(iso_wsmem), *sy = sx + S;
-  int *st = reinterpret_cast<int *>(sy + S);
-  __shared__ int s_top;
-  const int T = (M + S - 1) / S;
-  for (int t = blockIdx.x; t < T; t += gridDim.x) {
-    const int b = t * S, len = min(S, M - b);
-    for (int j = threadIdx.x; j < len; j += blockDim.x) iso_wpt(qx, qy, b + j, sx[j], sy[j]);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int top = 0;
-      for (int j = 0; j < len; ++j) {
-        while (top >= 2 && iso_wturn(sx[st[top - 2]], sy[st[top - 2]], sx[st[top - 1]], sy[st[top - 1]], sx[j], sy[j]) >= 0)
-          --top;
-        st[top++] = j;
-      }
-      s_top = top;
-      hc[t] = top;
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < s_top; j += blockDim.x) hv[b + j] = b + st[j];
-    __syncthreads();
+// The weighted fit's point set for the hull kernels: point i is the origin, or kept point i - 1 of (qx, qy).  A block's
+// values are its weight and positive weight, read() of exact differences, p = fl(read(dY) / read(dX)).
+struct IsoWeights {
+  using Coord = u256;
+  using Ref = const u256 &;
+  using Block = double;
+  const u256 *__restrict__ qx, *__restrict__ qy;
+  __device__ __forceinline__ void point(int i, u256 &x, u256 &y) const {
+    if (i == 0) { x = u256{{0, 0, 0, 0}}; y = x; return; }
+    x = qx[i - 1];
+    y = qy[i - 1];
   }
-}
-// k_iso_merge over the weighted points: the same bridge search with the exact turn test
-__global__ void __launch_bounds__(kIsoThreads) k_iso_wmerge(const u256 *__restrict__ qx, const u256 *__restrict__ qy,
-                                                            int n_hulls, int W, const int *__restrict__ hv_in,
-                                                            const int *__restrict__ hc_in, int *__restrict__ hv_out,
-                                                            int *__restrict__ hc_out) {
-  __shared__ int s_br[2];
-  const int pairs = (n_hulls + 1) / 2;
-  for (int p = blockIdx.x; p < pairs; p += gridDim.x) {
-    const int *L = hv_in + (int64_t)2 * p * W;
-    const int a = hc_in[2 * p];
-    const bool single = 2 * p + 1 >= n_hulls;
-    const int *R = L + W;
-    const int b = single ? 0 : hc_in[2 * p + 1];
-    if (threadIdx.x == 0) {
-      int i_end = a - 1, j_end = 0;
-      if (!single) {
-        auto tangent = [&](const u256 &vx, const u256 &vy) {
-          int lo = 0, hi = b - 1;
-          while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            u256 x0, y0, x1, y1;
-            iso_wpt(qx, qy, R[mid], x0, y0);
-            iso_wpt(qx, qy, R[mid + 1], x1, y1);
-            if (iso_wturn(vx, vy, x0, y0, x1, y1) >= 0) lo = mid + 1; else hi = mid;
-          }
-          return lo;
-        };
-        int lo = 0, hi = a - 1;
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          u256 vx, vy, ux, uy, rx, ry;
-          iso_wpt(qx, qy, L[mid], vx, vy);
-          iso_wpt(qx, qy, L[mid + 1], ux, uy);
-          iso_wpt(qx, qy, R[tangent(vx, vy)], rx, ry);
-          // u strictly above the line v -> r (k_iso_merge's iso_cross(v, r, u) > 0); u comes before r along the curve
-          if (iso_wturn(vx, vy, ux, uy, rx, ry) < 0) lo = mid + 1; else hi = mid;
-        }
-        u256 vx, vy;
-        iso_wpt(qx, qy, L[lo], vx, vy);
-        i_end = lo;
-        j_end = tangent(vx, vy);
-      }
-      s_br[0] = i_end;
-      s_br[1] = j_end;
-      hc_out[p] = i_end + 1 + (single ? 0 : b - j_end);
-    }
-    __syncthreads();
-    const int i_end = s_br[0], j_end = s_br[1];
-    int *out = hv_out + (int64_t)2 * p * W;
-    for (int k = threadIdx.x; k <= i_end; k += blockDim.x) out[k] = L[k];
-    if (!single)
-      for (int k = threadIdx.x; k < b - j_end; k += blockDim.x) out[i_end + 1 + k] = R[j_end + k];
-    __syncthreads();
+  // The sign of (a - o) x (b - o): o comes before a and b, so every difference is >= 0 and the cross product is the
+  // comparison of two unsigned 512-bit products.
+  __device__ __forceinline__ static int turn(Ref ox, Ref oy, Ref ax, Ref ay, Ref bx, Ref by) {
+    unsigned long long p[8], q[8];
+    u256_mul(u256_sub(ax, ox), u256_sub(by, oy), p);
+    u256_mul(u256_sub(ay, oy), u256_sub(bx, ox), q);
+#pragma unroll
+    for (int i = 7; i >= 0; --i)
+      if (p[i] != q[i]) return p[i] > q[i] ? 1 : -1;
+    return 0;
   }
-}
-// k_iso_emit over the weighted points: X, Y and each block's weight and positive weight, read() of exact differences;
-// p = fl(read(dY) / read(dX))
-__global__ void __launch_bounds__(256) k_iso_wemit(const int *__restrict__ h, int B, const int *__restrict__ excl,
-                                                   const double *__restrict__ thr, const u256 *__restrict__ qx,
-                                                   const u256 *__restrict__ qy, double *__restrict__ X,
-                                                   double *__restrict__ Y, double *__restrict__ blk_w,
-                                                   double *__restrict__ blk_pw, unsigned long long *__restrict__ n_x) {
-  for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < B; o += gridDim.x * blockDim.x) {
-    const int b = B - 1 - o, i0 = h[b], i1 = h[b + 1];
-    u256 x0, y0, x1, y1;
-    iso_wpt(qx, qy, i0, x0, y0);
-    iso_wpt(qx, qy, i1, x1, y1);
-    const double wr = u256_read(u256_sub(x1, x0)), wp = u256_read(u256_sub(y1, y0));
-    const double p = wp / wr;
-    blk_w[o] = wr;
-    blk_pw[o] = wp;
-    const int at = excl[o];
-    const bool two = i1 - i0 >= 2;
-    X[at] = thr[i1 - 1];
-    Y[at] = p;
-    if (two) {
-      X[at + 1] = thr[i0];
-      Y[at + 1] = p;
-    }
-    if (o == B - 1) *n_x = (unsigned long long)(at + 1 + two);
+  __device__ __forceinline__ static int above(Ref vx, Ref vy, Ref ux, Ref uy, Ref rx, Ref ry) {
+    return -turn(vx, vy, ux, uy, rx, ry);   // (r - v) x (u - v) = -((u - v) x (r - v))
   }
-}
+  __device__ __forceinline__ static double block(Ref x0, Ref y0, Ref x1, Ref y1, Block &w, Block &pw) {
+    w = u256_read(u256_sub(x1, x0));
+    pw = u256_read(u256_sub(y1, y0));
+    return pw / w;
+  }
+};
 
 // ---- the weighted quality pass (dsgd_eval_*weighted_calibration, dsgd_eval_*weighted_isotonic_calibration) -----------
-// kIso: p = interp(s) at the map (X, Y) and the log-loss term -log p or -log1p(-p), as k_iso_eval; else p = sigmoid(-z),
-// z = a f + b, and the term softplus(+-z), as k_calib_eval.  c_i = fl(w_y * s_i) as in k_calib_score<true>.  A row with
+// kIso: p = interp(s) at the map (X, Y) and the log-loss term -log p or -log1p(-p); else p = sigmoid(-z), z = a f + b, and
+// the term softplus(+-z); each as k_calib_eval<kIso, kSmem>.  c_i = fl(w_y * s_i) as in k_calib_score<true>.  A row with
 // R(c) = 0 is counted in kCwvRows and adds nothing else.  The sums add R(fl(c (p - o)^2)), R(fl(c l)) over the finite
 // terms, R(c) over the rows used and R(c) over the rows whose term is infinite (counted in kCwvInf too); bin k adds R(c),
 // R(c) of the positives and R(fl(c p)) to its three limb blocks in shared memory.  A bin value of 2^52 or more is counted
