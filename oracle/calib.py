@@ -1,54 +1,21 @@
 """TEST INFRASTRUCTURE ONLY -- the checker of the calibration calls (DESIGN.md §4.11): a ctypes binding of
 oracle/dsgd_oracle_calib.c, and beside it a literal Python restatement (math.fsum sums) that the C checker is tested against.
 
-Both work on an array of scores f = x . w (the device's own dsgd_margins in the GPU tests) and labels.  The library is built by
-__graft_entry__.build(), or on first use: next to its source, or in a temporary directory if that is read-only.  Only tests/
-and tools/ use it; the product package never does.
+Both work on an array of scores f = x . w (the device's own dsgd_margins in the GPU tests) and labels.  The library is
+oracle/oracle.py's libdsgd_oracle.so.  Only tests/ and tools/ use it; the product package never does.
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
-import tempfile
 from typing import NamedTuple
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "dsgd_oracle_calib.c")
-_NAME = "libdsgd_oracle_calib.so"
-# the flags of oracle/Makefile: no fast-math, no contraction
-_CFLAGS = ["-O3", "-march=x86-64-v3", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-Wall", "-Wextra", "-std=gnu11",
-           "-shared"]
+from . import oracle as _oracle
 
 CONVERGED, ITERATION_LIMIT, LINE_SEARCH_FAILED, NON_FINITE = 0, 1, 2, 3
 MAX_ITER, RIDGE, GRAD_EPS, MIN_STEP, ARMIJO = 100, 1e-12, 1e-5, 1e-10, 1e-4
-
-
-def _cc():
-    return "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
-
-
-def _stale(path: str) -> bool:
-    return (not os.path.exists(path)) or os.path.getmtime(path) < os.path.getmtime(_SRC)
-
-
-def build(force: bool = False) -> str:
-    """Compile the calibration checker (gcc only); returns the library's path."""
-    path = os.path.join(_HERE, _NAME)
-    if not force and not _stale(path):
-        return path
-    if not os.access(_HERE, os.W_OK):
-        path = os.path.join(tempfile.gettempdir(), f"dsgd_oracle_calib_{os.getuid()}", _NAME)
-        os.makedirs(os.path.dirname(path), exist_ok=True)
-        if not force and not _stale(path):
-            return path
-    tmp = f"{path}.{os.getpid()}.tmp"
-    subprocess.run([_cc(), *_CFLAGS, "-o", tmp, _SRC, "-lm"], check=True, capture_output=True)
-    os.replace(tmp, path)
-    return path
 
 
 _lib = None
@@ -57,7 +24,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(build())
+        _lib = _oracle.lib()
         _lib.dsgd_oracle_calib_fit.restype = C.c_int
         _lib.dsgd_oracle_calib_sums.restype = None
         _lib.dsgd_oracle_calib_probs.restype = None

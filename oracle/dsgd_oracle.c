@@ -13,21 +13,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#define EPS 1e-20 /* math/Sparse.scala:104 */
-
-static inline double filt(double v) { return fabs(v) > EPS ? v : 0.0; }
-
-/* x . w  = (x * w).sum  (math/Vec.scala:58; math/Sparse.scala:46,20-31): the product map is built first,
- * which drops products with |x_j w_j| <= 1e-20, then folded.  Fold order here is index order (the
- * reference's is HashMap order, not reproducible without a JVM -- SURVEY.md 2.3). */
-static inline double row_dot(const dsgd_oracle_csr *a, int64_t r, const double *w) {
-  double s = 0.0;
-  for (int64_t p = a->row_ptr[r]; p < a->row_ptr[r + 1]; ++p) {
-    double xv = filt((double)a->val[p]); /* the row itself is a Sparse: tiny entries are absent */
-    s += filt(xv * w[a->col[p]]);
-  }
-  return s;
-}
+#include "dsgd_oracle_common.h"   /* EPS, filt, row_dot */
 
 static inline double signum(double v) { return (double)((v > 0.0) - (v < 0.0)); }
 

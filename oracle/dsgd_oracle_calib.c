@@ -6,18 +6,7 @@
  * long double (64-bit significand on x86-64), which is math.fsum quality for these sizes: the error of a sum is far below one
  * ulp of a double before the final rounding.  Rows whose score is NaN are skipped.
  */
-#include <math.h>
-#include <stdint.h>
-
-typedef struct { long double s, c; int bad; } ksum;
-static void k_add(ksum *k, double v) {
-  if (!(fabs(v) < 0x1p52)) { k->bad = 1; return; }   /* NaN, infinite or >= 2^52: the sum reads NaN (DESIGN.md §4.11) */
-  const long double x = (long double)v, t = k->s + x;
-  if (fabsl(k->s) >= fabsl(x)) k->c += (k->s - t) + x;
-  else k->c += (x - t) + k->s;
-  k->s = t;
-}
-static double k_val(const ksum *k) { return k->bad ? NAN : (double)(k->s + k->c); }
+#include "dsgd_oracle_common.h"   /* sigmoid, softplus, ksum */
 
 /* out6 = {F, dF/dA, dF/dB, H_AA, H_AB, H_BB} at (a, b), without the ridge */
 void dsgd_oracle_calib_sums(const double *f, const int8_t *y, int64_t n, double t_pos, double t_neg, double a, double b,
@@ -97,13 +86,6 @@ int dsgd_oracle_calib_fit(const double *f, const int8_t *y, int64_t n, double *a
   info_out[0] = iter; info_out[1] = status; info_out[2] = n_pos + n_neg; info_out[3] = n_nan; info_out[4] = evals;
   return 0;
 }
-
-static double sigmoid(double t) {
-  if (t >= 0.0) return 1.0 / (1.0 + exp(-t));
-  const double e = exp(t);
-  return e / (1.0 + e);
-}
-static double softplus(double z) { return (z > 0.0 ? z : 0.0) + log1p(exp(-fabs(z))); }
 
 /* p_out[i] = sigmoid(-(a f_i + b)) (NaN for a NaN z) */
 void dsgd_oracle_calib_probs(const double *f, int64_t n, double a, double b, double *p_out) {

@@ -1,7 +1,7 @@
 /*
  * TEST INFRASTRUCTURE ONLY -- fp64 CPU restatement of the curves and average precision of include/dsgd.h
- * (dsgd_eval_*curve), the checker of tests/test_gpu_curve.py.  Linked with dsgd_oracle_metrics.c, whose left-fold dots it
- * uses when the caller passes no margins.
+ * (dsgd_eval_*curve), the checker of tests/test_gpu_curve.py.  When the caller passes no margins it uses the left-fold dots
+ * of dsgd_oracle_metrics.c (dsgd_oracle_margins).
  */
 #include <stdlib.h>
 

@@ -7,9 +7,9 @@
  * and every p into the library's fixed-point limbs (resolution 2^-160) and converts the integer sums from the top limb
  * down, so those sums are the library's bit for bit; the log-loss sum is Neumaier-compensated in long double.
  */
-#include <math.h>
-#include <stdint.h>
 #include <stdlib.h>
+
+#include "dsgd_oracle_common.h"   /* fxsum, ksum */
 
 typedef struct { double s; int8_t y; } srow;
 
@@ -108,48 +108,13 @@ void dsgd_oracle_iso_probs(const double *f, int64_t n, const double *X, const do
   for (int64_t i = 0; i < n; ++i) out[i] = interp(-f[i], X, Y, k);
 }
 
-/* ---- the fixed-point sum: limb j worth 2^(40 j - 160), j = 0..5; limbs 0..4 carried into [0, 2^40) ---- */
-typedef struct { uint64_t l[6]; int64_t bad; } lsum;
-static void l_carry(uint64_t *q) {
-  for (int i = 0; i < 5; ++i) {
-    q[i + 1] += q[i] >> 40;
-    q[i] &= (1ull << 40) - 1;
-  }
-}
-static void l_add(lsum *a, double v) {
-  if (!(v >= 0.0 && v < 0x1p52)) { ++a->bad; return; }
-  double F[4];
-  for (int i = 0; i < 4; ++i) F[i] = floor(v * ldexp(1.0, 40 * i));
-  a->l[4] += (uint64_t)F[0];
-  for (int i = 1; i < 4; ++i) a->l[4 - i] += (uint64_t)(F[i] - F[i - 1] * 0x1p40);
-  a->l[0] += (uint64_t)(rint(v * 0x1p160) - F[3] * 0x1p40);
-  l_carry(a->l);
-}
-static double l_value(const lsum *a) {
-  if (a->bad) return NAN;
-  uint64_t q[6];
-  for (int i = 0; i < 6; ++i) q[i] = a->l[i];
-  l_carry(q);
-  double s = (double)q[5] * 0x1p40;
-  for (int i = 4; i >= 0; --i) s += (double)q[i] * ldexp(1.0, 40 * i - 160);
-  return s;
-}
-
-typedef struct { long double s, c; } ksum;
-static void k_add(ksum *k, double v) {
-  const long double x = (long double)v, t = k->s + x;
-  if (fabsl(k->s) >= fabsl(x)) k->c += (k->s - t) + x;
-  else k->c += (x - t) + k->s;
-  k->s = t;
-}
-
 /* The quality pass: sums_out = {Brier sum, log-loss sum over the finite terms}; per bin rows, positives and sum p;
  * words_out = {rows used, rows left out, rows with an infinite term}. */
 void dsgd_oracle_iso_quality(const double *f, const int8_t *y, int64_t n, const double *X, const double *Y, int64_t k,
                              int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
                              int64_t *words_out) {
-  lsum brier = {{0}, 0}, ps[64];
-  ksum ll = {0, 0};
+  fxsum brier = {{0}, 0}, ps[64];
+  ksum ll = {0, 0, 0};
   for (int b = 0; b < n_bins; ++b) { bin_rows[b] = bin_pos[b] = 0; ps[b] = brier; }
   int64_t used = 0, out = 0, inf = 0;
   for (int64_t i = 0; i < n; ++i) {
@@ -158,18 +123,18 @@ void dsgd_oracle_iso_quality(const double *f, const int8_t *y, int64_t n, const 
     const int pos = y[i] > 0;
     const double p = interp(s, X, Y, k), o = pos ? 1.0 : 0.0, d = p - o;
     ++used;
-    l_add(&brier, d * d);
+    fx_add(&brier, d * d);
     const double term = pos ? -log(p) : -log1p(-p);
     if (isinf(term)) ++inf; else k_add(&ll, term);
     int b = (int)floor(p * (double)n_bins);
     b = b < n_bins - 1 ? b : n_bins - 1;
     ++bin_rows[b];
     bin_pos[b] += pos;
-    l_add(&ps[b], p);
+    fx_add(&ps[b], p);
   }
-  sums_out[0] = l_value(&brier);
-  sums_out[1] = (double)(ll.s + ll.c);
-  for (int b = 0; b < n_bins; ++b) bin_psum[b] = l_value(&ps[b]);
+  sums_out[0] = fx_read(brier);
+  sums_out[1] = k_val(&ll);
+  for (int b = 0; b < n_bins; ++b) bin_psum[b] = fx_read(ps[b]);
   words_out[0] = used;
   words_out[1] = out;
   words_out[2] = inf;

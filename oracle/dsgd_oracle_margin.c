@@ -1,6 +1,6 @@
 /*
  * TEST INFRASTRUCTURE ONLY -- see dsgd_oracle_margin.h.  The array restatement of the gradient, the evaluations and the sync
- * step of the margin models, in every weighting; it leaves the other checkers alone.
+ * step of every model, in every weighting, with the L1 step, rate tables and the averaging sum.
  */
 #include "dsgd_oracle_margin.h"
 
@@ -8,23 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#define EPS 1e-20 /* math/Sparse.scala:104 */
-
-static inline double filt(double v) { return fabs(v) > EPS ? v : 0.0; }
-
-/* (x * w).sum: products filtered, then folded in index order */
-static double row_dot(const dsgd_oracle_csr *a, int64_t r, const double *w) {
-  double s = 0.0;
-  for (int64_t p = a->row_ptr[r]; p < a->row_ptr[r + 1]; ++p) s += filt(filt((double)a->val[p]) * w[a->col[p]]);
-  return s;
-}
-
-static inline double softplus(double z) { return (z > 0.0 ? z : 0.0) + log1p(exp(-fabs(z))); }
-static inline double sigmoid(double t) {
-  if (t >= 0.0) return 1.0 / (1.0 + exp(-t));
-  const double e = exp(t);
-  return e / (1.0 + e);
-}
+#include "dsgd_oracle_common.h"
 
 int dsgd_oracle_margin_row(int32_t model, double z, double *loss_out, double *scale_out) {
   const double t = 1.0 + z;
@@ -43,39 +27,20 @@ int dsgd_oracle_margin_row(int32_t model, double z, double *loss_out, double *sc
   return 0;
 }
 
-/* The fixed-point sum of non-negative terms: limbs k = 0..5 worth 2^(40 k - 160), limbs 0..4 kept below 2^40 */
-typedef struct { uint64_t q[6]; int bad; } fxsum;
-#define LIMB_MASK ((1ull << 40) - 1)
-static void fx_carry(uint64_t q[6]) {
-  for (int i = 0; i < 5; ++i) {
-    q[i + 1] += q[i] >> 40;
-    q[i] &= LIMB_MASK;
-  }
-}
-static void fx_add(fxsum *f, double v) {
-  if (!(v >= 0.0 && v < 4503599627370496.0)) { f->bad = 1; return; }   /* NaN, inf, >= 2^52 */
-  double F[4];   /* F_i = floor(v * 2^(40 i)), exact */
-  for (int i = 0; i < 4; ++i) F[i] = floor(ldexp(v, 40 * i));
-  f->q[4] += (uint64_t)F[0];
-  for (int i = 1; i < 4; ++i) f->q[4 - i] += (uint64_t)(F[i] - F[i - 1] * 0x1p40);
-  f->q[0] += (uint64_t)(rint(ldexp(v, 160)) - F[3] * 0x1p40);   /* the one rounding: to 2^-160, ties to even */
-  fx_carry(f->q);
-}
-static double fx_value(const fxsum *f) {
-  if (f->bad) return NAN;
-  uint64_t q[6];
-  memcpy(q, f->q, sizeof q);
-  fx_carry(q);
-  double s = (double)q[5] * 0x1p40;
-  for (int i = 4; i >= 0; --i) s += (double)q[i] * ldexp(1.0, 40 * i - 160);
-  return s;
+double dsgd_oracle_margin_prox(double u, double tau) {
+  if (!(tau > 0.0)) return u;
+  return u > tau ? filt(u - tau) : (u < -tau ? filt(u + tau) : 0.0);
 }
 
-static double l1_norm(const double *w, int32_t dim) {   /* the device's fixed-point sum: every |w_j| > 1e-20 is exact in it */
-  fxsum f;
-  memset(&f, 0, sizeof f);
-  for (int32_t j = 0; j < dim; ++j) fx_add(&f, fabs(w[j]));
-  return fx_value(&f);
+double dsgd_oracle_margin_l1_norm(const double *w, int32_t dim, int64_t *nnz_out) {
+  fxsum f = {{0}, 0};   /* every |w_j| > 1e-20 is exact in it */
+  int64_t nnz = 0;
+  for (int32_t j = 0; j < dim; ++j) {
+    fx_add(&f, fabs(w[j]));
+    nnz += (w[j] != 0.0);
+  }
+  if (nnz_out) *nnz_out = nnz;
+  return fx_read(f);
 }
 
 /* The totals of one pass (pass_rows) */
@@ -90,8 +55,7 @@ typedef struct {
  * the weighting into g (dense, zero on entry), filtered after every addition. */
 static void pass_rows(const dsgd_oracle_csr *a, int32_t model, int32_t weighting, const double *w, const int32_t *idx,
                       int64_t begin, int64_t n, double w_pos, double w_neg, const double *sw, double *g, pass_totals *o) {
-  fxsum fs, fok, fw, fc[2];
-  memset(&fs, 0, sizeof fs); memset(&fok, 0, sizeof fok); memset(&fw, 0, sizeof fw); memset(fc, 0, sizeof fc);
+  fxsum fs = {{0}, 0}, fok = fs, fw = fs, fc[2] = {fs, fs};
   memset(o, 0, sizeof *o);
   for (int64_t i = 0; i < n; ++i) {
     const int64_t r = idx ? idx[i] : begin + i;
@@ -129,16 +93,16 @@ static void pass_rows(const dsgd_oracle_csr *a, int32_t model, int32_t weighting
       if (gv != 0.0) g[a->col[q]] = filt(g[a->col[q]] + gv);
     }
   }
-  o->cls[0] = fx_value(&fc[0]);
-  o->cls[1] = fx_value(&fc[1]);
+  o->cls[0] = fx_read(fc[0]);
+  o->cls[1] = fx_read(fc[1]);
   if (weighting == 1) {
     const double hp = w_pos * o->cls[0], hn = w_neg * o->cls[1];
     o->s = hp + hn;
   } else {
-    o->s = fx_value(&fs);
+    o->s = fx_read(fs);
   }
-  o->ok_w = fx_value(&fok);
-  o->all_w = fx_value(&fw);
+  o->ok_w = fx_read(fok);
+  o->all_w = fx_read(fw);
 }
 
 static int bad_args(const dsgd_oracle_csr *a, int32_t model, int32_t weighting, const int32_t *idx, int64_t begin, int64_t n) {
@@ -196,7 +160,7 @@ int dsgd_oracle_margin_loss_acc(const dsgd_oracle_csr *a, int32_t model, double 
 
 int dsgd_oracle_margin_gradient(const dsgd_oracle_csr *a, int32_t model, int32_t weighting, double lambda, const double *d,
                                 const double *w, const int32_t *idx, int64_t n, double w_pos, double w_neg, const double *sw,
-                                int32_t do_regularize, double *grad_out, double *loss_out, double *s_out) {
+                                int32_t do_regularize, double *grad_out, double *loss_out, double *s_out, double *c_out) {
   int rc = bad_args(a, model, weighting, idx, 0, n);
   if (rc || !idx) return rc ? rc : -3;
   double c, nrm2;
@@ -207,6 +171,7 @@ int dsgd_oracle_margin_gradient(const dsgd_oracle_csr *a, int32_t model, int32_t
   if (do_regularize) regularize(grad_out, a->dim, c);
   if (loss_out) *loss_out = lambda * nrm2 + o.s / (double)n;
   if (s_out) *s_out = o.s;
+  if (c_out) *c_out = c;
   return 0;
 }
 
@@ -261,8 +226,8 @@ int dsgd_oracle_margin_sync_steps(const dsgd_oracle_csr *a, int32_t model, int32
         if (g[j] != 0.0) sum[j] = filt(sum[j] + g[j]);
     }
     if (losses_out) {
-      losses_out[t] = lambda1 > 0.0 ? lambda * nrm2 + lambda1 * l1_norm(w, dim) + h / (double)per_step
-                                    : lambda * nrm2 + h / (double)per_step;
+      const double l1 = lambda1 > 0.0 ? dsgd_oracle_margin_l1_norm(w, dim, NULL) : 0.0;
+      losses_out[t] = lambda1 > 0.0 ? lambda * nrm2 + lambda1 * l1 + h / (double)per_step : lambda * nrm2 + h / (double)per_step;
     }
     const double tau = lr * lambda1;
     for (int32_t j = 0; j < dim; ++j) {
@@ -271,8 +236,7 @@ int dsgd_oracle_margin_sync_steps(const dsgd_oracle_csr *a, int32_t model, int32
         const double mean = filt(sum[j] / (double)n_workers);
         u = filt(u - filt(mean * lr));
       }
-      if (tau > 0.0) u = u > tau ? filt(u - tau) : (u < -tau ? filt(u + tau) : 0.0);
-      w[j] = u;
+      w[j] = dsgd_oracle_margin_prox(u, tau);
       if (avg_sum) avg_sum[j] += w[j];
     }
   }

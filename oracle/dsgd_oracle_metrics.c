@@ -3,21 +3,9 @@
  * dsgd_eval_*metrics), the checker of tests/test_gpu_metrics.py.  Rows are the oracle's CSR (dsgd_oracle.h); the dot is
  * the oracle's left fold (dsgd_oracle.c: row_dot), restated here.
  */
-#include <math.h>
 #include <stdlib.h>
 
-#include "dsgd_oracle.h"
-
-#define EPS 1e-20 /* math/Sparse.scala:104 */
-
-static inline double filt(double v) { return fabs(v) > EPS ? v : 0.0; }
-
-/* x . w = (x * w).sum, folded in index order, products below 1e-20 dropped (math/Vec.scala:58; math/Sparse.scala:46) */
-static double row_dot(const dsgd_oracle_csr *a, int64_t r, const double *w) {
-  double s = 0.0;
-  for (int64_t p = a->row_ptr[r]; p < a->row_ptr[r + 1]; ++p) s += filt(filt((double)a->val[p]) * w[a->col[p]]);
-  return s;
-}
+#include "dsgd_oracle_common.h"   /* row_dot */
 
 static int rows_ok(const dsgd_oracle_csr *a, const int32_t *idx, int64_t begin, int64_t n) {
   if (!idx) return (begin < 0 || begin + n > a->n_rows) ? -2 : 0;

@@ -1,55 +1,23 @@
-"""TEST INFRASTRUCTURE ONLY -- ctypes binding of the fp64 checker of the margin models (oracle/dsgd_oracle_margin.c):
-SparseSquaredHinge and SparseModifiedHuber, and for cross-checks SparseSVM and SparseLogistic, in every weighting.
+"""TEST INFRASTRUCTURE ONLY -- ctypes binding of the fp64 checker of every model's sync path (oracle/dsgd_oracle_margin.c):
+SparseSVM, SparseLogistic, SparseSquaredHinge and SparseModifiedHuber, in every weighting, with the L1 step, rate tables and
+the averaging sum.  The class-weight, sample-weight, L1 and logistic helpers (oracle/cw.py, sw.py, l1.py, logistic.py) are
+calls into this module.
 
 `model` is a name ("svm", "logistic", "squared_hinge", "modified_huber") or its number 0-3.  The weighting of a call is
 the device's: sample-weighted when `sw` is given, else class-weighted when (w_pos, w_neg) != (1, 1), else unweighted.  The
-library is built by __graft_entry__.build(), or on first use: next to its source, or in a temporary directory if that is
-read-only.  Only tests/ and tools/ use this module; the product package never does.
+library is oracle/oracle.py's.  Only tests/ and tools/ use this module; the product package never does.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
 from typing import Optional, Sequence
 
 import numpy as np
 
+from . import oracle as _oracle
 from .oracle import Oracle, _check, _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "dsgd_oracle_margin.c")
-_HDRS = (os.path.join(_HERE, "dsgd_oracle_margin.h"), os.path.join(_HERE, "dsgd_oracle.h"))
-_NAME = "libdsgd_oracle_margin.so"
-# the flags of oracle/Makefile: no fast-math, no contraction
-_CFLAGS = ["-O3", "-march=x86-64-v3", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-Wall", "-Wextra", "-std=gnu11",
-           "-shared"]
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
-
-
-def _cc():
-    return "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
-
-
-def _stale(path: str) -> bool:
-    return (not os.path.exists(path)) or os.path.getmtime(path) < max(os.path.getmtime(f) for f in (_SRC, *_HDRS))
-
-
-def build(force: bool = False) -> str:
-    """Compile the margin-model checker (gcc only); returns the library's path."""
-    path = os.path.join(_HERE, _NAME)
-    if not force and not _stale(path):
-        return path
-    if not os.access(_HERE, os.W_OK):
-        path = os.path.join(tempfile.gettempdir(), f"dsgd_oracle_margin_{os.getuid()}", _NAME)
-        os.makedirs(os.path.dirname(path), exist_ok=True)
-        if not force and not _stale(path):
-            return path
-    tmp = f"{path}.{os.getpid()}.tmp"
-    subprocess.run([_cc(), *_CFLAGS, "-o", tmp, _SRC, "-lm"], check=True, capture_output=True)
-    os.replace(tmp, path)
-    return path
 
 
 _lib = None
@@ -58,9 +26,13 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(build())
+        _lib = _oracle.lib()
         for name in ("row", "sample_losses", "loss_acc", "gradient", "eval", "sync_steps"):
             getattr(_lib, "dsgd_oracle_margin_" + name).restype = C.c_int
+        _lib.dsgd_oracle_margin_prox.restype = C.c_double
+        _lib.dsgd_oracle_margin_prox.argtypes = [C.c_double, C.c_double]
+        _lib.dsgd_oracle_margin_l1_norm.restype = C.c_double
+        _lib.dsgd_oracle_margin_l1_norm.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     return _lib
 
 
@@ -85,6 +57,18 @@ def row(model, z: float):
     l, s = C.c_double(), C.c_double()
     _check(lib().dsgd_oracle_margin_row(C.c_int32(model_number(model)), C.c_double(z), C.byref(l), C.byref(s)), "margin row")
     return l.value, s.value
+
+
+def prox(u: float, tau: float) -> float:
+    """The L1 proximal step of one value at threshold tau, the one the sync steps apply to every column."""
+    return lib().dsgd_oracle_margin_prox(float(u), float(tau))
+
+
+def l1_norm(w):
+    """(||w||_1 as the device's fixed-point sum, #{w_j != 0})."""
+    w = np.ascontiguousarray(w, dtype=np.float64)
+    nnz = C.c_int64()
+    return lib().dsgd_oracle_margin_l1_norm(_p(w), w.size, C.byref(nnz)), nnz.value
 
 
 def sample_losses(orc: Oracle, model, w, idx=None, begin: int = 0, n: Optional[int] = None) -> np.ndarray:
@@ -116,14 +100,19 @@ def loss_acc(orc: Oracle, model, w, idx=None, begin: int = 0, n: Optional[int] =
 
 def gradient(orc: Oracle, model, w, idx, w_pos: float = 1.0, w_neg: float = 1.0, sw=None, regularize: bool = True):
     """(gradient, loss, S) of one request in the weighting of (w_pos, w_neg, sw)."""
+    return _gradient(orc, model, w, idx, w_pos, w_neg, sw, regularize)[:3]
+
+
+def _gradient(orc: Oracle, model, w, idx, w_pos: float = 1.0, w_neg: float = 1.0, sw=None, regularize: bool = True):
+    """(gradient, loss, S, c = 2 lambda (w . d) folded in column order)"""
     idx = orc._idx(idx)
-    g, loss, s = np.zeros(orc.dim, dtype=np.float64), C.c_double(), C.c_double()
+    g, loss, s, c = np.zeros(orc.dim, dtype=np.float64), C.c_double(), C.c_double(), C.c_double()
     _check(lib().dsgd_oracle_margin_gradient(C.byref(orc._csr), C.c_int32(model_number(model)),
                                              C.c_int32(_weighting(sw, w_pos, w_neg)), C.c_double(orc.lam), _p(orc.d),
                                              _p(orc._w(w)), _p(idx), C.c_int64(idx.size), C.c_double(w_pos),
                                              C.c_double(w_neg), _p(_sw(orc, sw)), C.c_int32(1 if regularize else 0), _p(g),
-                                             C.byref(loss), C.byref(s)), "margin gradient")
-    return g, loss.value, s.value
+                                             C.byref(loss), C.byref(s), C.byref(c)), "margin gradient")
+    return g, loss.value, s.value, c.value
 
 
 def eval_class(orc: Oracle, model, w, idx):

@@ -1,30 +1,51 @@
-"""TEST INFRASTRUCTURE ONLY -- ctypes binding of the fp64 C oracle (oracle/dsgd_oracle.c).
+"""TEST INFRASTRUCTURE ONLY -- ctypes binding of the fp64 C oracle (oracle/dsgd_oracle.c), and the one build and load of
+libdsgd_oracle.so, the library every checker of this directory is compiled into (oracle/Makefile).
 
-Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import
-this.  The product package never does.  See oracle/dsgd_oracle.h for the parity status
-("parity unpinned" beyond the VecTests known answers).
+Only tests/, tools/, __graft_entry__ and bench.py's cpu_baseline / --impl reference legs import this.  The product package
+never does.  See oracle/dsgd_oracle.h for the parity status ("parity unpinned" beyond the VecTests known answers).
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
 import subprocess
+import tempfile
 from typing import Optional, Sequence
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB_PATH = os.path.join(_HERE, "libdsgd_oracle.so")
+_NAME = "libdsgd_oracle.so"
+
+
+def _make(*args: str) -> subprocess.CompletedProcess:
+    return subprocess.run(["make", "-C", _HERE, *args], capture_output=True, text=True)
+
+
+def _fresh(path: str) -> bool:
+    """Whether the library at `path` is newer than every source and header oracle/Makefile names."""
+    return _make("-q", f"LIB={path}").returncode == 0
 
 
 def build(force: bool = False) -> str:
-    """Compile the C oracle in place (gcc only, no CUDA)."""
-    src = os.path.join(_HERE, "dsgd_oracle.c")
-    stale = (not os.path.exists(_LIB_PATH)) or os.path.getmtime(_LIB_PATH) < max(
-        os.path.getmtime(src), os.path.getmtime(os.path.join(_HERE, "dsgd_oracle.h")))
-    if force or stale:
-        subprocess.run(["make", "-C", _HERE, "-B", "libdsgd_oracle.so"], check=True, capture_output=True)
-    return _LIB_PATH
+    """Compile every checker into libdsgd_oracle.so with oracle/Makefile (gcc only, no CUDA) when it is missing or older than
+    its sources; returns its path.  The library sits next to its sources, or in a per-user temporary directory when this
+    directory is read-only.  It is written under a temporary name and renamed into place, so a process never loads a
+    half-written file."""
+    path = os.path.join(_HERE, _NAME)
+    if not force and _fresh(path):
+        return path
+    if not os.access(_HERE, os.W_OK):
+        path = os.path.join(tempfile.gettempdir(), f"dsgd_oracle_{os.getuid()}", _NAME)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        if not force and _fresh(path):
+            return path
+    tmp = f"{path}.{os.getpid()}.tmp"
+    r = _make("-B", f"LIB={tmp}")
+    if r.returncode != 0:
+        raise RuntimeError(f"building {_NAME} failed:\n{r.stdout}{r.stderr}")
+    os.replace(tmp, path)
+    return path
 
 
 class _Csr(C.Structure):
@@ -36,11 +57,11 @@ _lib = None
 
 
 def lib():
+    """The loaded library, built on first use.  Every module of this directory loads it through here and sets the restype /
+    argtypes of its own functions."""
     global _lib
     if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
+        _lib = C.CDLL(build())
         for name in ("forward", "loss_acc", "gradient", "sync_step", "sync_steps", "sync_steps_allcores", "async_delta",
                      "async_run", "dim_sparsity"):
             getattr(_lib, "dsgd_oracle_" + name).restype = C.c_int

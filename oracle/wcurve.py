@@ -1,52 +1,20 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes binding of the fp64 weighted-curve checker (oracle/dsgd_oracle_wcurve.c).
 
-`wcurve` answers for rows given by their margins (the device's own, from dsgd_margins), labels and weights c_i; `weights`
-forms c_i = fl(w_y * s_i) as the device does.  The library is built by __graft_entry__.build(), or on first use: next to
-its source, or in a temporary directory if that is read-only.  Only tests/ and tools/ use it; the product package never
-does.
+`wcurve` answers for rows given by their margins (the device's own, from dsgd_margins), labels and weights c_i;
+`weights` forms c_i = fl(w_y * s_i) as the device does.  The library is oracle/oracle.py's libdsgd_oracle.so.  Only tests/
+and tools/ use it; the product package never does.
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import subprocess
-import tempfile
 from typing import NamedTuple
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRCS = (os.path.join(_HERE, "dsgd_oracle_wcurve.c"),)
-_NAME = "libdsgd_oracle_wcurve.so"
-# the flags of oracle/Makefile: no fast-math, no contraction
-_CFLAGS = ["-O3", "-march=x86-64-v3", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-Wall", "-Wextra", "-std=gnu11",
-           "-shared"]
+from . import oracle as _oracle
+
 WCURVE_WORDS = 13
-
-
-def _cc():
-    return "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
-
-
-def _stale(path: str) -> bool:
-    return (not os.path.exists(path)) or os.path.getmtime(path) < max(os.path.getmtime(f) for f in _SRCS)
-
-
-def build(force: bool = False) -> str:
-    """Compile the weighted-curve checker (gcc only); returns the library's path."""
-    path = os.path.join(_HERE, _NAME)
-    if not force and not _stale(path):
-        return path
-    if not os.access(_HERE, os.W_OK):
-        path = os.path.join(tempfile.gettempdir(), f"dsgd_oracle_wcurve_{os.getuid()}", _NAME)
-        os.makedirs(os.path.dirname(path), exist_ok=True)
-        if not force and not _stale(path):
-            return path
-    tmp = f"{path}.{os.getpid()}.tmp"
-    subprocess.run([_cc(), *_CFLAGS, "-o", tmp, *_SRCS, "-lm"], check=True, capture_output=True)
-    os.replace(tmp, path)
-    return path
 
 
 _lib = None
@@ -55,7 +23,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(build())
+        _lib = _oracle.lib()
         _lib.dsgd_oracle_wcurve.restype = C.c_int
         _lib.dsgd_oracle_wcurve_read.restype = C.c_double
         _lib.dsgd_oracle_wcurve_read.argtypes = [C.c_void_p, C.c_int64]

@@ -1,8 +1,9 @@
-"""The class-weight checker (oracle/cw.py, oracle/dsgd_oracle_cw.c), without a GPU:
+"""The class-weight checker (oracle/cw.py, the class weighting of oracle/dsgd_oracle_margin.c), without a GPU:
 
 1. The C checker against the literal restatement over Sparse vectors on dyadic data, both models' paths that are exact there
    (SVM weights and losses bit for bit; logistic weights and losses to rounding), one and several workers, rate tables.
-2. At weights (1, 1) it gives the existing checkers' steps, gradients and evaluations: weights bit for bit.
+2. At weights (1, 1) it gives the unweighted steps, gradients and evaluations: against dsgd_oracle.c for the SVM's gradient
+   and evaluation and against the literal restatements otherwise, weights bit for bit.
 3. Hand-worked cases: a weight of 0 for one class, a product x_j * w_y at exactly 1e-20 and one ulp above, a batch whose
    weighted contributions cancel exactly in a column.
 4. A structural known answer on dyadic data: with (w_pos, w_neg) = (2, 1) the raw gradient sum of a batch equals the unweighted
@@ -13,8 +14,11 @@ import pytest
 
 from oracle import cw as CW
 from oracle import l1 as L1
+from oracle import scala_semantics as S
 from oracle.logistic import LogisticOracle
 from oracle.oracle import Oracle
+from oracle.scala_semantics_logistic import SparseLogistic
+from oracle.scala_semantics_margin import literal_correct
 
 TINY = np.nextafter(1e-20, 1.0)   # the smallest double the 1e-20 filter keeps
 
@@ -36,6 +40,15 @@ def dyadic_problem(seed, n_rows=48, dim=24, cls=Oracle, lam=2.0 ** -6):
     orc.set_dim_sparsity(d)
     w0 = rng.integers(-8, 9, size=dim) / 16.0
     return orc, (rp, col, val, lab, dim, d), w0, rng
+
+
+def literal_model(logistic: bool, lam: float):
+    """The literal SparseSVM or SparseLogistic with the weighted backward of CW.literal_backward (c None: unweighted), as
+    scala_semantics_margin.literal_sync_steps takes a model."""
+    class Weighted(SparseLogistic if logistic else S.SparseSVM):
+        def backward(self, w, x, y, c=None):
+            return CW.literal_backward(w, x, y, 1.0 if c is None else c, logistic)
+    return Weighted(lam, None)
 
 
 @pytest.mark.parametrize("counts", [[8], [5, 3], [4, 3, 2]])
@@ -69,22 +82,30 @@ def test_logistic_c_equals_literal(counts):
 
 
 @pytest.mark.parametrize("logistic", [False, True])
-def test_unit_weights_are_the_existing_checkers(logistic):
-    orc, _, w0, rng = dyadic_problem(5, n_rows=64, cls=LogisticOracle if logistic else Oracle)
+def test_unit_weights_are_the_unweighted_step(logistic):
+    """At weights (1, 1): the steps against oracle/l1.py's literal restatement, with and without the L1 penalty; the gradient
+    and the evaluation against dsgd_oracle.c for the SVM and against scala_semantics_logistic.py for the logistic model."""
+    orc, (rp, col, val, lab, dim, d), w0, rng = dyadic_problem(5, n_rows=64)
     counts, lrs = [6, 4], [0.5, 0.25, 0.125]
     idx = rng.integers(0, 64, size=10 * 3).astype(np.int32)
-    w_cw, l_cw = CW.sync_steps(orc, w0, idx, counts, lrs, 1.0, 1.0, logistic=logistic)
-    w_ref, l_ref = L1.sync_steps(orc, w0, idx, counts, lrs, 0.0, logistic=logistic)
-    assert np.array_equal(w_cw, w_ref)
-    np.testing.assert_allclose(l_cw, l_ref, rtol=0 if not logistic else 1e-15)
-    w_cw, l_cw = CW.sync_steps(orc, w0, idx, counts, lrs, 1.0, 1.0, logistic=logistic, lambda1=2.0 ** -5)
-    w_ref, l_ref = L1.sync_steps(orc, w0, idx, counts, lrs, 2.0 ** -5, logistic=logistic)
-    assert np.array_equal(w_cw, w_ref)
-    np.testing.assert_allclose(l_cw, l_ref, rtol=0 if not logistic else 1e-15)
+    for lambda1 in (0.0, 2.0 ** -5):
+        w_cw, l_cw = CW.sync_steps(orc, w0, idx, counts, lrs, 1.0, 1.0, logistic=logistic, lambda1=lambda1)
+        w_ref, l_ref = L1.literal_sync_steps(rp, col, val, lab, dim, orc.lam, lambda1, d, w0, idx, counts, lrs, logistic=logistic)
+        assert np.array_equal(w_cw, w_ref)
+        np.testing.assert_allclose(l_cw, l_ref, rtol=0 if not logistic else 1e-15)
     g, loss, sums = CW.gradient(orc, w0, idx[:10], 1.0, 1.0, logistic=logistic)
-    g_ref = orc.gradient(w0, idx[:10])
-    assert np.array_equal(g, g_ref[0] if isinstance(g_ref, tuple) else g_ref)
-    loss_ref, acc_ref = orc.loss_acc(w0, idx=idx[:10])
+    if logistic:
+        rows, ids = CW.literal_rows(rp, col, val, dim), [int(i) for i in idx[:10]]
+        w = S.Sparse({j: float(v) for j, v in enumerate(w0)}, dim)
+        model = SparseLogistic(orc.lam, S.Sparse({j: float(v) for j, v in enumerate(d)}, dim))
+        data = [(rows[r], int(lab[r])) for r in range(len(lab))]
+        g_ref = S.slave_gradient(model, data, w, ids)
+        g_ref = [g_ref.get(j) for j in range(dim)]
+        loss_ref, acc_ref = model.loss(w, [data[r] for r in ids]), literal_correct(w, rows, lab, ids) / 10
+    else:
+        g_ref, _ = orc.gradient(w0, idx[:10])
+        loss_ref, acc_ref = orc.loss_acc(w0, idx=idx[:10])
+    assert np.array_equal(g, g_ref)
     np.testing.assert_allclose(loss, loss_ref, rtol=0 if not logistic else 1e-15)
     s, c = CW.eval_class(orc, w0, idx[:10], logistic=logistic)
     assert (c[0] + c[1]) / 10 == acc_ref and c[2] + c[3] == 10

@@ -1,10 +1,11 @@
-"""The checker of the sync step with an L1 penalty (oracle/l1.py, oracle/dsgd_oracle_l1.c), without a GPU:
+"""The checker of the sync step with an L1 penalty (oracle/l1.py, the L1 step of oracle/dsgd_oracle_margin.c), without a GPU:
 
 1. The proximal step on hand-worked values: shrinking by tau, |u| = tau -> 0, u - tau at exactly 1e-20 (filtered) and one ulp
    above (kept), tau = 0 -> u itself (also for values the filter would drop and for -0), the C form equal to the literal one.
 2. The C checker against the literal restatement, both models, one and several workers, scalar rates and tables with zero
    entries: weights bit for bit, losses bit for bit on dyadic data and within 1e-14 on random data.
-3. lambda1 = 0 gives the existing checkers' steps bit for bit (dsgd_oracle_sync_steps, the logistic checker).
+3. lambda1 = 0 gives the plain step bit for bit: dsgd_oracle_sync_steps for the SVM, the literal restatement of
+   scala_semantics_margin.py for the logistic model.
 """
 import math
 
@@ -12,9 +13,12 @@ import numpy as np
 import pytest
 
 from conftest import random_csr
+from oracle import cw as CW
 from oracle import l1 as L1
 from oracle.logistic import LogisticOracle
 from oracle.oracle import Oracle
+from oracle.scala_semantics_margin import literal_sync_steps
+from test_oracle_class_weight import literal_model
 
 TINY = np.nextafter(1e-20, 1.0)   # the smallest double the 1e-20 filter keeps
 
@@ -120,11 +124,17 @@ def test_c_checker_matches_literal(logistic, counts, dyadic, table):
 
 @pytest.mark.parametrize("logistic", [False, True])
 @pytest.mark.parametrize("counts", [[6], [3, 4, 2]])
-def test_lambda1_zero_is_the_existing_step(logistic, counts):
+def test_lambda1_zero_is_the_plain_step(logistic, counts):
+    """lambda1 = 0 gives the step without the penalty: dsgd_oracle.c's for the SVM; for the logistic model the literal
+    restatement over Sparse vectors (scala_semantics_margin.py), whose loss sums are the checker's fixed-point sums."""
     (rp, col, val, lab, dim, lam, lam1, d, w0, idx, lrs), orc = _case(3, False, logistic, counts, 10, False)
     lr = 0.25
     w_c, l_c = L1.sync_steps(orc, w0, idx, counts, np.full(10, lr), 0.0, logistic=logistic)
-    w_r, l_r = orc.sync_steps(w0, idx, counts, lr, n_steps=10)
+    if logistic:
+        w_r, l_r = literal_sync_steps(literal_model(True, lam), CW.literal_rows(rp, col, val, dim), lab, dim, lam, d, w0, idx,
+                                      counts, np.full(10, lr))
+    else:
+        w_r, l_r = orc.sync_steps(w0, idx, counts, lr, n_steps=10)
     assert np.array_equal(w_c, w_r)
     assert np.array_equal(l_c, l_r)
 

@@ -1,5 +1,5 @@
 """SparseLogistic in the oracle: the literal map-based restatement (oracle/scala_semantics_logistic.py) against the C
-restatement (oracle/dsgd_oracle_logistic.c) on random problems, the known answers, margins far out in both directions, and the 1e-20 product filter where sigma(z) * x crosses it."""
+restatement (model 1 of oracle/dsgd_oracle_margin.c, as LogisticOracle) on random problems, the known answers, margins far out in both directions, and the 1e-20 product filter where sigma(z) * x crosses it."""
 import math
 
 import numpy as np

@@ -2,17 +2,16 @@
 1. hand-computed known answers of L(z) and s(z) for both models, both branch points included;
 2. the C checker against the literal restatement over Sparse vectors (oracle/scala_semantics_margin.py) bit for bit on
    random dyadic problems, in every weighting, with L1, the averaging sum and rate tables;
-3. its SVM (0) and logistic (1) forms against the checkers of record of those models (oracle/dsgd_oracle_cw.c and
-   oracle/dsgd_oracle_sw.c), so that its weighted, L1 and averaging machinery is theirs."""
+3. its SVM (0) and logistic (1) forms against the same literal restatement with those models' backward (oracle/cw.py), bit
+   for bit in the class and sample weightings with L1 and the averaging sum."""
 import numpy as np
 import pytest
 
 from oracle import cw as CW
 from oracle import margin as M
-from oracle import sw as SW
 from oracle.scala_semantics_margin import MODEL_CLASSES, literal_correct, literal_pass_loss, literal_sync_steps
 from oracle.scala_semantics import Sparse
-from test_oracle_class_weight import dyadic_problem
+from test_oracle_class_weight import dyadic_problem, literal_model
 from test_oracle_sample_weight import dyadic_weights
 
 MARGIN = ("squared_hinge", "modified_huber")
@@ -125,20 +124,17 @@ def test_sample_losses_match_rows():
 
 @pytest.mark.parametrize("model", [0, 1])
 @pytest.mark.parametrize("weighting", ["class", "sample"])
-def test_models_zero_and_one_are_the_existing_checkers(model, weighting):
-    """The SVM and logistic forms of the margin checker give the trajectories of the checkers of record.  The weights are
-    the same bits; loss sums are added differently (compensated there, fixed point here), so the logistic ones may differ in
-    the last bits."""
-    orc, _, w0, rng = dyadic_problem(52)
+def test_models_zero_and_one_equal_literal(model, weighting):
+    """The SVM and logistic forms of the checker against the literal restatement of the weighted, L1 and averaged steps
+    (scala_semantics_margin.py) with the literal SparseSVM / SparseLogistic: weights, averaging sums and losses bit for
+    bit."""
+    orc, (rp, col, val, lab, dim, d), w0, rng = dyadic_problem(52)
     wp, wn, sw = _weights(weighting, rng, orc.n_rows)
     counts, lrs = [6, 4], [0.25, 0.125, 0.0625]
     idx = rng.integers(0, orc.n_rows, size=sum(counts) * len(lrs)).astype(np.int32)
-    avg_m, avg_o = np.zeros(orc.dim), np.zeros(orc.dim)
+    avg_m, avg_l = np.zeros(orc.dim), [0.0] * dim
     w_m, l_m = M.sync_steps(orc, model, w0, idx, counts, lrs, wp, wn, sw, lambda1=2.0 ** -8, avg_sum=avg_m)
-    if sw is None:
-        w_o, l_o = CW.sync_steps(orc, w0, idx, counts, lrs, wp, wn, logistic=bool(model), lambda1=2.0 ** -8, avg_sum=avg_o)
-    else:
-        w_o, l_o = SW.sync_steps(orc, w0, idx, counts, lrs, sw, wp, wn, logistic=bool(model), lambda1=2.0 ** -8,
-                                 avg_sum=avg_o)
-    assert np.array_equal(w_m, w_o) and np.array_equal(avg_m, avg_o)
-    np.testing.assert_allclose(l_m, l_o, rtol=0 if model == 0 else 1e-15)
+    w_l, l_l = literal_sync_steps(literal_model(model == 1, orc.lam), CW.literal_rows(rp, col, val, dim), lab, dim, orc.lam, d,
+                                  w0, idx, counts, lrs, wp, wn, sw, _code(wp, wn, sw), 2.0 ** -8, avg_l)
+    assert np.array_equal(w_m, np.asarray(w_l)) and np.array_equal(avg_m, np.asarray(avg_l))
+    assert list(l_m) == l_l

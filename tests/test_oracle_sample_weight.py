@@ -1,8 +1,9 @@
-"""The sample-weight checker (oracle/sw.py, oracle/dsgd_oracle_sw.c), without a GPU:
+"""The sample-weight checker (oracle/sw.py, the sample weighting of oracle/dsgd_oracle_margin.c), without a GPU:
 
 1. The C checker against the literal restatement over Sparse vectors on dyadic data with dyadic sample weights (some zero):
    SVM weights and losses bit for bit, logistic to rounding; one and several workers, rate tables; the weighted evaluation.
-2. At sample weights 1 it gives the class-weight checker's steps and gradients: weights and losses bit for bit.
+2. At sample weights 1 it gives the class-weighted steps and gradients of the literal restatements: weights bit for bit,
+   losses bit for bit for the SVM.
 3. Hand-worked cases: a weight of 0, a product x_j * c_i at exactly 1e-20 and one ulp above, and an integer weight k on a row
    equal to that row listed k times.
 """
@@ -13,7 +14,8 @@ from oracle import cw as CW
 from oracle import sw as SW
 from oracle.logistic import LogisticOracle
 from oracle.oracle import Oracle
-from test_oracle_class_weight import TINY, dyadic_problem
+from oracle.scala_semantics_margin import literal_sync_steps
+from test_oracle_class_weight import TINY, dyadic_problem, literal_model
 
 
 def dyadic_weights(rng, n):
@@ -65,24 +67,36 @@ def test_eval_c_equals_literal(logistic, wp, wn):
 
 
 @pytest.mark.parametrize("logistic", [False, True])
-def test_unit_sample_weights_are_the_class_weight_checker(logistic):
-    orc, _, w0, rng = dyadic_problem(5, n_rows=64, cls=LogisticOracle if logistic else Oracle)
+def test_unit_sample_weights_are_the_class_weighted_step(logistic):
+    """At sample weights 1 the steps and the gradient are the class-weighted ones of the literal restatements: oracle/cw.py's
+    without the L1 penalty, scala_semantics_margin.py's with it."""
+    orc, (rp, col, val, lab, dim, d), w0, rng = dyadic_problem(5, n_rows=64)
     counts, lrs = [6, 4], [0.5, 0.25, 0.125]
     idx = rng.integers(0, 64, size=10 * 3).astype(np.int32)
     ones = np.ones(64)
+    rows = CW.literal_rows(rp, col, val, dim)
+    w = SW.Sparse({j: float(v) for j, v in enumerate(w0)}, dim)
+    ids = [int(i) for i in idx[:10]]
     for wp, wn in ((1.0, 1.0), (2.0, 0.5)):
         for lambda1 in (0.0, 2.0 ** -5):
             w_sw, l_sw = SW.sync_steps(orc, w0, idx, counts, lrs, ones, wp, wn, logistic=logistic, lambda1=lambda1)
-            w_cw, l_cw = CW.sync_steps(orc, w0, idx, counts, lrs, wp, wn, logistic=logistic, lambda1=lambda1)
+            if lambda1 == 0.0:
+                w_cw, l_cw = CW.literal_sync_steps(rows, lab, dim, orc.lam, d, w0, idx, counts, lrs, wp, wn, logistic=logistic)
+            else:
+                w_cw, l_cw = literal_sync_steps(literal_model(logistic, orc.lam), rows, lab, dim, orc.lam, d, w0, idx, counts,
+                                                lrs, wp, wn, None, 1 if (wp, wn) != (1.0, 1.0) else 0, lambda1)
             assert np.array_equal(w_sw, w_cw)
             if not logistic:   # dyadic hinge terms: both loss sums exact
                 assert np.array_equal(l_sw, l_cw)
-            else:              # compensated fp64 sums against the fixed-point sum: to rounding
+            else:              # the fixed-point sum against the literal sums: to rounding
                 np.testing.assert_allclose(l_sw, l_cw, rtol=1e-15)
-        g_sw, loss_sw, _ = SW.gradient(orc, w0, idx[:10], None, 2.0, 0.5, logistic=logistic)
-        g_cw, loss_cw, _ = CW.gradient(orc, w0, idx[:10], 2.0, 0.5, logistic=logistic)
-        assert np.array_equal(g_sw, g_cw)
-        np.testing.assert_allclose(loss_sw, loss_cw, rtol=0 if not logistic else 1e-15)
+        g_sw, loss_sw, _ = SW.gradient(orc, w0, idx[:10], None, wp, wn, logistic=logistic)
+        g_cw = SW.vec_sum([CW.literal_backward(w, rows[r], int(lab[r]), wp if lab[r] > 0 else wn, logistic) for r in ids])
+        g_cw = g_cw + g_cw.value_like(orc.lam * 2.0 * w.dot(SW.Sparse({j: float(v) for j, v in enumerate(d)}, dim)))
+        sums, _ = CW.literal_loss_sums(w, rows, lab, ids, logistic)
+        assert np.array_equal(g_sw, [g_cw.get(j) for j in range(dim)])
+        np.testing.assert_allclose(loss_sw, orc.lam * w.norm_squared() + (wp * sums[0] + wn * sums[1]) / 10,
+                                   rtol=0 if not logistic else 1e-15)
 
 
 def test_zero_weight_scatters_nothing_and_still_counts():
