@@ -268,6 +268,9 @@ class Master:
         self.weighted = self.class_weight != (1.0, 1.0) and not self.sample_weighted
         self.n_train, self.n_test = data.n_rows, test_data.n_rows
         self.dim = data.dim
+        # the model fits an intercept (fit_intercept): every weight vector in or out is dim + 1 long, the intercept last
+        self.intercept = bool(getattr(slave, "intercept", False))
+        self.wdim = self.dim + (1 if self.intercept else 0)
         self.slave = slave
         self.ctx: NativeCtx = slave.ctx
         self.group = group or Group()
@@ -698,6 +701,9 @@ class MasterSync(Master):
         """
         if average_from is not None and not 0 <= average_from < max_epochs:
             raise ValueError(f"average_from must lie in [0, max_epochs = {max_epochs}), got {average_from}")
+        if np.asarray(initial_weights).size != self.wdim:
+            raise ValueError(f"initial_weights: expected {self.wdim} values (dim = {self.dim}"
+                             f"{' and the intercept last' if self.intercept else ''}), got {np.asarray(initial_weights).size}")
         check_schedule(learning_rate_decay, learning_rate_power)
         decaying = learning_rate_decay > 0.0
         t_global = 0   # global index of the next step: the schedule's t
@@ -807,6 +813,8 @@ class MasterAsync(Master):
             raise ValueError(f"{type(model).__name__}: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+        if getattr(model, "fit_intercept", False):
+            raise ValueError("fit_intercept: the intercept is fitted by sync training; asynchronous (Hogwild) training has none")
         from ..ml.class_weight import resolve_class_weight
         if resolve_class_weight(getattr(model, "class_weight", None), data.label) != (1.0, 1.0):   # as the Slave decides
             raise ValueError("class_weight: class weights belong to sync training; asynchronous (Hogwild) training has none")

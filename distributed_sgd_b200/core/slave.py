@@ -39,6 +39,9 @@ class Slave:
             raise ValueError(f"{type(model).__name__}: asynchronous (Hogwild) training supports SparseSVM only")
         if model.l1 and is_async:
             raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+        self.intercept = bool(getattr(model, "fit_intercept", False))
+        if self.intercept and is_async:
+            raise ValueError("fit_intercept: the intercept is fitted by sync training; asynchronous (Hogwild) training has none")
         # (w_pos, w_neg) of the model's class_weight; "balanced" counts the labels of the train rows
         self.class_weight = resolve_class_weight(getattr(model, "class_weight", None), data.label)
         weighted = self.class_weight != (1.0, 1.0)
@@ -57,6 +60,8 @@ class Slave:
                 raise ValueError("Slave: the given device context does not hold these rows")
             if getattr(ctx, "model", "logistic" if getattr(ctx, "logistic", False) else "svm") != name:
                 raise ValueError("Slave: the given device context was created for another model")
+            if getattr(ctx, "intercept", False) != self.intercept:
+                raise ValueError("Slave: the given device context does not match the model's fit_intercept")
             self.ctx = ctx
             if model.dim_sparsity is None:
                 model.dim_sparsity = ctx.compute_dim_sparsity(self.n_train)
@@ -68,7 +73,7 @@ class Slave:
                 ctx.set_sample_weights(sample_weights_of(data, test_data))
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
-                             is_async=is_async, model=name)
+                             is_async=is_async, model=name, intercept=self.intercept)
         if test_data is not None:
             row_ptr = np.concatenate([data.row_ptr, test_data.row_ptr[1:] + data.row_ptr[-1]])
             col = np.concatenate([data.col[:data.nnz], test_data.col[:test_data.nnz]])

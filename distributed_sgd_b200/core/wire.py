@@ -186,6 +186,10 @@ class SlaveServicer:
 
     def __init__(self, ctx, n_train: int, is_async: bool, concurrency: int = 1, seed: int = 0,
                  master_target: Optional[str] = None, relay_period: float = 0.05):
+        if getattr(ctx, "intercept", False):
+            # the service's Sparse weight messages are dim long: an intercept would be dropped on every request
+            raise ValueError("SlaveServicer: the Slave service's weight messages carry no intercept; serve a context created "
+                             "without fit_intercept")
         self.ctx, self.n_train, self.is_async = ctx, n_train, is_async
         self.dim = ctx.dim
         self.concurrency, self.seed = concurrency, seed

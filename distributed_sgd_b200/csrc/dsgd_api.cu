@@ -354,17 +354,24 @@ static inline bool has_class_weights(const dsgd_ctx *ctx) { return !(ctx->cw_pos
 static inline int weighting(const dsgd_ctx *ctx) {
   return ctx->sw_on ? kSampleWeighted : has_class_weights(ctx) ? kClassWeighted : kUnweighted;
 }
-// The one step from a ctx's run-time model and a weighting to template arguments: f(model, weighting), both as
-// std::integral_constant.  with_model fixes the weighting (an evaluation of one tally); with_forms takes it at run time.
+// an intercept ctx (DSGD_FLAG_INTERCEPT): every weight vector is dim + 1 long, the intercept last (w[dim] on the device too)
+static inline bool has_icpt(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_INTERCEPT) != 0; }
+static inline int64_t wlen(const dsgd_ctx *ctx) { return (int64_t)ctx->dim + (has_icpt(ctx) ? 1 : 0); }
+// The one step from a ctx's run-time model, intercept and a weighting to template arguments: f(model, weighting,
+// intercept), all three as std::integral_constant.  with_model fixes the weighting (an evaluation of one tally); with_forms
+// takes it at run time.
 template <int kWeight, class F>
 static int with_model(const dsgd_ctx *ctx, F &&f) {
   constexpr std::integral_constant<int, kWeight> weight{};
-  switch (model_of(ctx)) {
-    case kLogistic: return f(std::integral_constant<int, kLogistic>{}, weight);
-    case kSquaredHinge: return f(std::integral_constant<int, kSquaredHinge>{}, weight);
-    case kModifiedHuber: return f(std::integral_constant<int, kModifiedHuber>{}, weight);
-    default: return f(std::integral_constant<int, kSvm>{}, weight);
-  }
+  auto model = [&](auto icpt) {
+    switch (model_of(ctx)) {
+      case kLogistic: return f(std::integral_constant<int, kLogistic>{}, weight, icpt);
+      case kSquaredHinge: return f(std::integral_constant<int, kSquaredHinge>{}, weight, icpt);
+      case kModifiedHuber: return f(std::integral_constant<int, kModifiedHuber>{}, weight, icpt);
+      default: return f(std::integral_constant<int, kSvm>{}, weight, icpt);
+    }
+  };
+  return has_icpt(ctx) ? model(std::true_type{}) : model(std::false_type{});
 }
 template <class F>
 static int with_forms(const dsgd_ctx *ctx, int weight, F &&f) {
@@ -393,6 +400,8 @@ extern "C" int dsgd_create(dsgd_ctx **out, int device, int32_t dim, double lambd
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: more than one model flag (0x%x)", flags & kModelFlags);
   if ((flags & kModelFlags) && (flags & DSGD_FLAG_ASYNC))
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports the SVM model only");
+  if ((flags & DSGD_FLAG_INTERCEPT) && (flags & DSGD_FLAG_ASYNC))
+    return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode has no intercept (DSGD_FLAG_INTERCEPT is sync-mode only)");
   // every async worker pushes each delta into all `world` replicas and the master's, through one table of kMaxReplicas slots
   if ((flags & DSGD_FLAG_ASYNC) && world > kMaxReplicas - 1)
     return fail(nullptr, DSGD_ERR_INVALID, "dsgd_create: async mode supports at most %d workers (got world %d)",
@@ -464,10 +473,11 @@ extern "C" const char *dsgd_info(const dsgd_ctx *ctx) {
   snprintf(buf, sizeof buf,
            "{\"device\": %d, \"name\": \"%s\", \"sm_count\": %d, \"arch\": \"sm_90a\", \"dim\": %d, \"rank\": %d, "
            "\"world\": %d, \"n_rows\": %lld, \"nnz\": %lld, \"state_dtype\": \"f64\", \"value_dtype\": \"f32\", "
-           "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g], \"sample_weights\": %s}",
+           "\"model\": \"%s\", \"lambda1\": %.17g, \"class_weights\": [%.17g, %.17g], \"sample_weights\": %s, "
+           "\"intercept\": %s}",
            ctx->device, ctx->dev_name.c_str(), ctx->sm_count, ctx->dim, ctx->rank, ctx->world, (long long)ctx->n_rows,
            (long long)ctx->nnz, kModelNames[model_of(ctx)], ctx->lambda1, ctx->cw_pos, ctx->cw_neg,
-           ctx->sw_on ? "true" : "false");
+           ctx->sw_on ? "true" : "false", has_icpt(ctx) ? "true" : "false");
   ctx->info = buf;
   return ctx->info.c_str();
 }
@@ -676,7 +686,7 @@ extern "C" int dsgd_set_weights(dsgd_ctx *ctx, const double *w) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(w, DSGD_ERR_INVALID, "dsgd_set_weights: w is NULL");
   CU(cudaSetDevice(ctx->device));
-  CU(cudaMemcpyAsync(ctx->w, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(ctx->w, w, sizeof(double) * (size_t)wlen(ctx), cudaMemcpyHostToDevice, ctx->stream));
   int rc = refresh_resident(ctx);
   if (rc) return rc;
   CU(cudaStreamSynchronize(ctx->stream));
@@ -687,7 +697,7 @@ extern "C" int dsgd_get_weights(dsgd_ctx *ctx, double *w) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(w, DSGD_ERR_INVALID, "dsgd_get_weights: w is NULL");
   CU(cudaSetDevice(ctx->device));
-  CU(cudaMemcpyAsync(w, ctx->w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(w, ctx->w, sizeof(double) * (size_t)wlen(ctx), cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return DSGD_OK;
 }
@@ -723,7 +733,7 @@ static int request_weights(dsgd_ctx *ctx, const double *w, const double **w_dev,
   if (snapshot)
     CU(cudaMemcpyAsync(ctx->w_req, ctx->w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToDevice, ctx->stream));
   else
-    CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)ctx->dim, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->w_req, w, sizeof(double) * (size_t)wlen(ctx), cudaMemcpyHostToDevice, ctx->stream));
   launch_prepare(ctx, ctx->w_req, ctx->w32_req, kScalReqC, kScalReqNrm2);
   CU(cudaGetLastError());
   *w_dev = ctx->w_req; *c_dev = ctx->scal + kScalReqC; *nrm_dev = ctx->scal + kScalReqNrm2;
@@ -737,22 +747,26 @@ static inline int rows_grid(const dsgd_ctx *ctx, int64_t n) {
 // ---- streaming pass (large n): fp32 weights staged in shared memory, one persistent CTA per SM (dsgd_stream.cuh) ----
 constexpr int64_t kStreamMinRows = 2048;
 
+constexpr size_t kStreamMaxSmem = 227u * 1024u - 1024u;   // the weights' staging of the largest eligible dim
 static bool stream_eligible(const dsgd_ctx *ctx, int64_t n) {
-  return n >= kStreamMinRows && stream_smem_bytes(ctx->dim) + 1024 <= 227u * 1024u;
+  return n >= kStreamMinRows && stream_smem_bytes(ctx->dim) <= kStreamMaxSmem;
 }
 
 template <bool kScatter, bool kPreds, bool kContig, bool kCls = false>
 static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_begin, int64_t n, const double *w_dev,
                          const float *w32_dev, double *g, double *preds) {
   const size_t smem = stream_smem_bytes(ctx->dim);
+  // The attribute belongs to the kernel, not to the ctx: every ctx sets the bound of every eligible dim, so that a ctx of a
+  // smaller dim set up later does not lower it under the launches of one of a larger dim.
+  const int max_smem = (int)kStreamMaxSmem;
   if (!ctx->stream_ready) {
-    CU(cudaFuncSetAttribute(k_stream_rows<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<true, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CU(cudaFuncSetAttribute(k_stream_rows<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     ctx->stream_ready = true;
   }
   NEED(kContig == (samples_dev == nullptr), DSGD_ERR_INVALID, "stream_launch: sample list / row range mismatch");
@@ -889,12 +903,13 @@ static int rows_list(dsgd_ctx *ctx, const int32_t *ids, int64_t n, bool preds, c
 // decides signs, and the logistic loss needs the dot's value); every other pass is the fp64 k_rows of its model and
 // weighting.  Only an evaluation names a range of rows; a gradient or a forward pass always lists them.  A weighted pass
 // ends with its fold, k_class_fold or k_sw_fold: with out == nullptr the batch's weighted loss sum is left in cnt for a
-// weighted tail (kCw), else the evaluation's totals and *nrm go to out.
-template <int kModel, int kWeight, bool kScatter, bool kPreds = false>
+// weighted tail (kCw), else the evaluation's totals and *nrm go to out.  kIcpt (an intercept ctx): never the streaming
+// pass, which has no intercept form; k_rows reads the intercept at w[dim].
+template <int kModel, int kWeight, bool kScatter, bool kPreds = false, bool kIcpt = false>
 static int launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, const float *w32, double *g,
                        double *preds = nullptr, const double *nrm = nullptr, double *out = nullptr) {
   bool streamed = false;
-  if constexpr (kModel == kSvm && kWeight != kSampleWeighted) {
+  if constexpr (kModel == kSvm && kWeight != kSampleWeighted && !kIcpt) {
     constexpr bool kCls = kWeight == kClassWeighted;
     if ((streamed = w32 && stream_eligible(ctx, rows.n))) {
       int rc = rows.ids ? stream_launch<kScatter, kPreds, false, kCls>(ctx, rows.ids, 0, rows.n, w, w32, g, preds)
@@ -904,9 +919,14 @@ static int launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, cons
   }
   if (!streamed) {
     // sw == nullptr without sample weights (an evaluation): every s_i is 1
-    k_rows<kModel, kWeight, kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
-        ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
-        ctx->sw_on ? ctx->sw.p : nullptr);
+    if constexpr (kIcpt)
+      k_rows<kModel, kWeight, kScatter, kPreds, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+          ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
+          ctx->sw_on ? ctx->sw.p : nullptr, w + ctx->dim);
+    else
+      k_rows<kModel, kWeight, kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+          ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
+          ctx->sw_on ? ctx->sw.p : nullptr);
     LAUNCHED();
   }
   if constexpr (kWeight == kClassWeighted) {
@@ -922,16 +942,17 @@ static int launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, cons
 // The pass of a gradient (kScatter: the gradient into g, then k_finish) or of an evaluation over `rows` with the weights of
 // request_weights, then the shared tail: out2 = {loss, accuracy, loss sum, correct count, ||w||^2}, and the counters
 // cleared for the next pass (k_loss_scalar).  A weighted gradient's tails read its weighted loss sum.
-template <int kModel, int kWeight, bool kScatter>
+template <int kModel, int kWeight, bool kScatter, bool kIcpt>
 static int loss_pass(dsgd_ctx *ctx, const double *w_host, const row_set &rows) {
   const double *w = nullptr, *c = nullptr, *nrm = nullptr;
   const float *w32 = nullptr;
   int rc = request_weights(ctx, w_host, &w, &c, &nrm, &w32);
-  if (rc || (rc = launch_rows<kModel, kWeight, kScatter>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr))) return rc;
+  if (rc || (rc = launch_rows<kModel, kWeight, kScatter, false, kIcpt>(ctx, rows, w, w32, kScatter ? ctx->g.p : nullptr)))
+    return rc;
   const double n = (double)rows.n;
   constexpr bool kCw = kWeight != kUnweighted;
   if constexpr (kScatter) {
-    k_finish<kModel, kCw><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
+    k_finish<kModel, kCw, kIcpt><<<cdiv(ctx->dim + 1, 256), 256, 0, ctx->stream>>>(ctx->g, ctx->dim, c, ctx->cnt, n);
     LAUNCHED();
   }
   k_loss_scalar<kModel, kCw><<<1, 1, 0, ctx->stream>>>(nrm, ctx->cnt, ctx->lambda, n, ctx->out2);
@@ -949,8 +970,11 @@ extern "C" int dsgd_forward(dsgd_ctx *ctx, const double *w, const int32_t *sampl
   const float *w32d;
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd, &w32d))) return rc;
-  // a prediction is the sign of x . w under either model: the SVM's row kernels
-  if ((rc = launch_rows<kSvm, kUnweighted, false, true>(ctx, rows, wd, w32d, nullptr, ctx->preds))) return rc;
+  // a prediction is the sign of the score under every model: the SVM's row kernels
+  if ((rc = with_model<kUnweighted>(ctx, [&](auto, auto, auto ic) {
+         return launch_rows<kSvm, kUnweighted, false, true, ic>(ctx, rows, wd, w32d, nullptr, ctx->preds);
+       })))
+    return rc;
   CU(cudaGetLastError());
   CU(cudaMemsetAsync(ctx->cnt, 0, sizeof(unsigned long long) * 2, ctx->stream));
   CU(cudaMemcpyAsync(preds_out, ctx->preds, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -967,11 +991,16 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
   NEED(ctx->have_d, DSGD_ERR_STATE, "dsgd_gradient: dimSparsity not set");
   row_set rows;
   int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  if (rc || (rc = with_forms(ctx, weighting(ctx), [&](auto m, auto wt) {
-               return loss_pass<m, wt, true>(ctx, w, rows);
+  if (rc || (rc = with_forms(ctx, weighting(ctx), [&](auto m, auto wt, auto ic) {
+               return loss_pass<m, wt, true, ic>(ctx, w, rows);
              })))
     return rc;
   CU(cudaMemcpyAsync(grad_out, ctx->g, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
+  if (has_icpt(ctx)) {   // the intercept's gradient, and its two sums cleared for the next pass
+    CU(cudaMemcpyAsync(grad_out + ctx->dim, ctx->g + ctx->dim + kIcptSlot, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemsetAsync(ctx->g + ctx->dim + kIcptSlot, 0, sizeof(double), ctx->stream));
+    CU(cudaMemsetAsync(ctx->cnt + kCntIcpt, 0, sizeof(unsigned long long) * 2 * kLossAccWords, ctx->stream));
+  }
   double out2[2];
   CU(cudaMemcpyAsync(out2, ctx->out2, sizeof out2, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaMemsetAsync(ctx->g, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
@@ -983,7 +1012,7 @@ extern "C" int dsgd_gradient(dsgd_ctx *ctx, const double *w, const int32_t *samp
 // One evaluation pass over `rows`: out = {loss, accuracy, loss sum, correct count, ||w||^2}.  The SVM's loss sum is the
 // hinge sum, an integer.
 static int eval_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double out[5]) {
-  int rc = with_model<kUnweighted>(ctx, [&](auto m, auto wt) { return loss_pass<m, wt, false>(ctx, w, rows); });
+  int rc = with_model<kUnweighted>(ctx, [&](auto m, auto wt, auto ic) { return loss_pass<m, wt, false, ic>(ctx, w, rows); });
   if (rc) return rc;
   CU(cudaMemcpyAsync(out, ctx->out2, sizeof(double) * 5, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -1082,8 +1111,8 @@ static int tally_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, doubl
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   const float *w32 = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd, &w32);
-  if (rc || (rc = with_model<kWeight>(ctx, [&](auto m, auto wt) {
-               return launch_rows<m, wt, false>(ctx, rows, wd, w32, nullptr, nullptr, nd, ctx->cls_out);
+  if (rc || (rc = with_model<kWeight>(ctx, [&](auto m, auto wt, auto ic) {
+               return launch_rows<m, wt, false, false, ic>(ctx, rows, wd, w32, nullptr, nullptr, nd, ctx->cls_out);
              })))
     return rc;
   CU(cudaGetLastError());
@@ -1157,12 +1186,21 @@ extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
 
 // out[i] = x . w (prob: the model's P(y = +1 | x), k_margins) of the listed rows; the values go through `preds`, the per-row
-// request buffer
+// request buffer.  On an intercept ctx the score is x . w + beta (k_margins<..., true>)
 static int scores_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double *out, bool prob) {
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd);
   if (rc) return rc;
-  if (prob && model_of(ctx) == kModifiedHuber)
+  const bool huber = model_of(ctx) == kModifiedHuber;
+  if (has_icpt(ctx)) {
+    const double *b = wd + ctx->dim;
+    if (prob && huber)
+      k_margins<true, true, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
+    else if (prob)
+      k_margins<true, false, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
+    else
+      k_margins<false, false, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
+  } else if (prob && huber)
     k_margins<true, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
   else if (prob) k_margins<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
   else k_margins<false><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
@@ -1222,7 +1260,12 @@ static int score_and_sort(dsgd_ctx *ctx, const double *w, const row_set &rows, b
   if (kW && ((rc = ctx->m_val.grow(ctx, n, 1024)) || (rc = ctx->m_valt.grow(ctx, n, 1024)))) return rc;
   CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kWords, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
-  if constexpr (kW)
+  if (has_icpt(ctx))   // the intercept form: the same arguments, every weight vector's intercept at [dim]
+    k_metrics_score<kWeight, true><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin,
+                                                                  n, wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
+                                                                  ctx->sw_on ? ctx->sw.p : nullptr,
+                                                                  kW ? ctx->m_val.p : nullptr, wd + ctx->dim);
+  else if constexpr (kW)
     k_metrics_score<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
                                                             wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
                                                             ctx->sw_on ? ctx->sw.p : nullptr, ctx->m_val);
@@ -1550,7 +1593,13 @@ static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, d
     return rc;
   CU(cudaMemsetAsync(ctx->k_ctl, 0, sizeof(unsigned long long) * ctl_words, ctx->stream));
   const int sgrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
-  if constexpr (kW)
+  if (has_icpt(ctx))
+    k_calib_score<kW, true><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                            ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
+                                                            ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr,
+                                                            kW ? ctx->k_cw.p : nullptr, kW ? ctx->k_ctl + kCtlW : nullptr,
+                                                            wd + ctx->dim);
+  else if constexpr (kW)
     k_calib_score<true><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
                                                         ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
                                                         ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr, ctx->k_cw,
@@ -1717,7 +1766,11 @@ extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, con
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
-  k_calib_prob<<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b, ctx->preds);
+  if (has_icpt(ctx))
+    k_calib_prob<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b,
+                                                                        ctx->preds, wd + ctx->dim);
+  else
+    k_calib_prob<<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b, ctx->preds);
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1749,8 +1802,13 @@ static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_se
   const int8_t *label = ctx->label.p;
   const int32_t *ids = rows.ids;
   int64_t rb = rows.row_begin, rn = rows.n;
-  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk};
-  if constexpr (kIso)
+  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &icpt};
+  if (icpt && kIso)
+    CU(isotonic_launch(k_calib_eval<true, true, true>, k_calib_eval<true, false, true>, grid, k, ctx->stream, args));
+  else if (icpt)
+    CU(cudaLaunchKernel((const void *)k_calib_eval<false, false, true>, dim3(grid), dim3(256), args, 0, ctx->stream));
+  else if constexpr (kIso)
     CU(isotonic_launch(k_calib_eval<true, true>, k_calib_eval<true, false>, grid, k, ctx->stream, args));
   else
     CU(cudaLaunchKernel((const void *)k_calib_eval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
@@ -1836,8 +1894,13 @@ static int weighted_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &
   int64_t rb = rows.row_begin, rn = rows.n;
   double cwp = ctx->cw_pos, cwn = ctx->cw_neg;
   const double *swp = ctx->sw_on ? ctx->sw.p : nullptr;
-  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &cwp, &cwn, &swp};
-  if constexpr (kIso)
+  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &cwp, &cwn, &swp, &icpt};
+  if (icpt && kIso)
+    CU(isotonic_launch(k_weval<true, true, true>, k_weval<true, false, true>, grid, k, ctx->stream, args));
+  else if (icpt)
+    CU(cudaLaunchKernel((const void *)k_weval<false, false, true>, dim3(grid), dim3(256), args, 0, ctx->stream));
+  else if constexpr (kIso)
     CU(isotonic_launch(k_weval<true, true>, k_weval<true, false>, grid, k, ctx->stream, args));
   else
     CU(cudaLaunchKernel((const void *)k_weval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
@@ -2081,8 +2144,12 @@ extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const
   const uint2 *pairs = ctx->pairs.p;
   const int32_t *ids = rows.ids;
   int64_t rn = rows.n;
-  void *args[] = {&rp16, &pairs, &ids, &rn, &wd, &mx, &my, &ki, &out};
-  CU(isotonic_launch(k_iso_prob<true>, k_iso_prob<false>, rows_grid(ctx, rows.n), k, ctx->stream, args));
+  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  void *args[] = {&rp16, &pairs, &ids, &rn, &wd, &mx, &my, &ki, &out, &icpt};
+  if (icpt)
+    CU(isotonic_launch(k_iso_prob<true, true>, k_iso_prob<false, true>, rows_grid(ctx, rows.n), k, ctx->stream, args));
+  else
+    CU(isotonic_launch(k_iso_prob<true>, k_iso_prob<false>, rows_grid(ctx, rows.n), k, ctx->stream, args));
   LAUNCHED();
   CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
@@ -2680,7 +2747,8 @@ extern "C" int dsgd_set_workers(dsgd_ctx *ctx, int32_t n_local, const int32_t *c
 // lrs[s] (lrs == nullptr: lr), its loss into losses[s] (losses == nullptr: none)
 // kWeight: every worker's pass is k_rows in that weighting (a weighted one followed by its fold, k_class_fold or
 // k_sw_fold), and the tails of a weighted pass (kCw) read its weighted loss sum
-template <int kModel, int kWeight>
+// kIcpt: an intercept ctx; its gradient slot g[dim + kIcptSlot] widens the workers' sum and the allreduce by one entry
+template <int kModel, int kWeight, bool kIcpt>
 static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, int64_t n_steps, double lr,
                          const double *lrs, double *losses, bool single, int32_t k_total) {
   const int upd_blocks = cdiv(ctx->dim, 256);
@@ -2689,12 +2757,13 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
   double lr_s = lr;   // the rate of step s
   // The update of every step, in the form of this call [single][avg][l1]: one worker regularizes its raw gradient in the
   // update; while averaging the update also adds the new weights to avg; with an L1 penalty it soft-thresholds every column.
-  using Update = decltype(&k_update<true, kModel, false, false, kCw>);
+  using Update = decltype(&k_update<true, kModel, false, false, kCw, kIcpt>);
   static const Update kUpdate[2][2][2] = {
-      {{k_update<false, kModel, false, false, kCw>, k_update<false, kModel, false, true, kCw>},
-       {k_update<false, kModel, true, false, kCw>, k_update<false, kModel, true, true, kCw>}},
-      {{k_update<true, kModel, false, false, kCw>, k_update<true, kModel, false, true, kCw>},
-       {k_update<true, kModel, true, false, kCw>, k_update<true, kModel, true, true, kCw>}}};
+      {{k_update<false, kModel, false, false, kCw, kIcpt>, k_update<false, kModel, false, true, kCw, kIcpt>},
+       {k_update<false, kModel, true, false, kCw, kIcpt>, k_update<false, kModel, true, true, kCw, kIcpt>}},
+      {{k_update<true, kModel, false, false, kCw, kIcpt>, k_update<true, kModel, false, true, kCw, kIcpt>},
+       {k_update<true, kModel, true, false, kCw, kIcpt>, k_update<true, kModel, true, true, kCw, kIcpt>}}};
+  const size_t g_words = (size_t)ctx->dim + (kIcpt ? kIcptSlot + 1 : 2);
   const Update update = kUpdate[single][ctx->avg_on][ctx->lambda1 > 0.0];
   double *const avg = ctx->avg_on ? ctx->avg.p : nullptr;
 
@@ -2706,7 +2775,9 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
     if (single) {
       // one worker, one GPU: gradient -> (regularize + update) fused, two launches per step
       int rc = DSGD_OK;
-      profiled(ctx, [&] { rc = launch_rows<kModel, kWeight, true>(ctx, {smp, 0, n_per_step}, ctx->w, nullptr, ctx->g); });
+      profiled(ctx, [&] {
+        rc = launch_rows<kModel, kWeight, true, false, kIcpt>(ctx, {smp, 0, n_per_step}, ctx->w, nullptr, ctx->g);
+      });
       if (rc) return rc;
     } else {
       // several workers or ranks: each worker's gradient, regularized and folded into gsum, then the allreduce and the update
@@ -2714,16 +2785,17 @@ static int sync_per_step(dsgd_ctx *ctx, const int32_t *smp, int64_t n_per_step, 
       for (int32_t v = 0; v < ctx->n_local; ++v) {
         const int64_t nv = ctx->worker_counts.empty() ? n_per_step : ctx->worker_counts[(size_t)v];
         int rc = DSGD_OK;
-        profiled(ctx, [&] { rc = launch_rows<kModel, kWeight, true>(ctx, {smp + off, 0, nv}, ctx->w, nullptr, ctx->g); });
+        profiled(ctx, [&] {
+          rc = launch_rows<kModel, kWeight, true, false, kIcpt>(ctx, {smp + off, 0, nv}, ctx->w, nullptr, ctx->g);
+        });
         if (rc) return rc;
-        k_finish_acc<kModel, kCw><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC,
+        k_finish_acc<kModel, kCw, kIcpt><<<fin_blocks, 256, 0, ctx->stream>>>(ctx->g, ctx->gsum, ctx->dim, ctx->scal + kScalC,
                                                                        ctx->cnt, (double)nv, v == 0 ? 1 : 0);
         LAUNCHED();
         off += nv;
       }
-      if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * (size_t)(ctx->dim + 2), ctx->stream));
-      if (ctx->world > 1)
-        NC(nccl().AllReduce(ctx->gsum, ctx->gsum, (size_t)ctx->dim + 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
+      if (ctx->n_local == 0) CU(cudaMemsetAsync(ctx->gsum, 0, sizeof(double) * g_words, ctx->stream));
+      if (ctx->world > 1) NC(nccl().AllReduce(ctx->gsum, ctx->gsum, g_words, ncclDouble, ncclSum, ctx->comm, ctx->stream));
       gbuf = ctx->gsum;
       k_den = (double)k_total;
       n_local = 0.0;
@@ -2765,12 +2837,14 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   const bool single = (ctx->world == 1 && ctx->n_local == 1 && k_total == 1);
   // The options the fused kernel has no form of, which with world > 1 take the per-step path over NCCL: the persistent and
   // fused kernels are SVM-only (a ctx of any other model always takes the per-step path below), and an L1 penalty, class
-  // weights or sample weights have only one-GPU persistent forms.  unfused names the first of them that is on.
+  // weights or sample weights have only one-GPU persistent forms.  An intercept has no persistent form at all: an intercept
+  // ctx always takes the per-step path.  unfused names the first of them that is on.
   static const char *const kModelTakes[] = {nullptr, "the logistic model takes", "the squared_hinge model takes",
                                             "the modified_huber model takes"};
   const int model = model_of(ctx);
   const int weight = weighting(ctx);
   const char *unfused = model != kSvm ? kModelTakes[model]
+                        : has_icpt(ctx) ? "the intercept takes"
                         : ctx->lambda1 > 0.0 ? "the L1 penalty takes"
                         : has_class_weights(ctx) ? "class weights take"
                         : weight == kSampleWeighted ? "sample weights take" : nullptr;
@@ -2790,7 +2864,7 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
     int rc = ctx->losses.grow(ctx, n_steps, 1024);
     if (rc) return rc;
   }
-  if ((single && model == kSvm && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
+  if ((single && model == kSvm && !has_icpt(ctx) && n_steps > 0 && persist_grid(ctx, n_per_step) > 0) || fused) {
     // one worker on one GPU: the whole run of steps is one persistent cooperative kernel; one worker per GPU, every peer's
     // exchange block mapped (fused): the same kernel aggregates over NVLink
     return persist_run(ctx, fused, ctx->samples + first, n_per_step, n_steps, lr, lrs,
@@ -2798,8 +2872,8 @@ static int sync_staged(dsgd_ctx *ctx, int64_t first, int64_t n_per_step, int64_t
   }
   const int32_t *smp = ctx->samples + first;
   double *loss_dev = want_losses ? ctx->losses.p : nullptr;
-  return with_forms(ctx, weight, [&](auto m, auto wt) {
-    return sync_per_step<m, wt>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
+  return with_forms(ctx, weight, [&](auto m, auto wt, auto ic) {
+    return sync_per_step<m, wt, ic>(ctx, smp, n_per_step, n_steps, lr, lrs, loss_dev, single, k_total);
   });
 }
 
@@ -2954,8 +3028,8 @@ extern "C" int dsgd_average_begin(dsgd_ctx *ctx) {
   ctx->avg_on = false;   // a failure below leaves averaging off and nothing to read
   ctx->avg_n = 0;
   CU(cudaSetDevice(ctx->device));
-  if (!ctx->avg) CU(ctx->avg.alloc(ctx->dim));
-  CU(cudaMemsetAsync(ctx->avg, 0, sizeof(double) * (size_t)ctx->dim, ctx->stream));
+  if (!ctx->avg) CU(ctx->avg.alloc(wlen(ctx)));
+  CU(cudaMemsetAsync(ctx->avg, 0, sizeof(double) * (size_t)wlen(ctx), ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   ctx->avg_on = true;
   return DSGD_OK;
@@ -2975,13 +3049,13 @@ extern "C" int dsgd_average_weights(dsgd_ctx *ctx, double *avg_out, int64_t *n_s
   NEED(ctx->avg_n > 0, DSGD_ERR_EMPTY, "dsgd_average_weights: no sync step since dsgd_average_begin (the mean of an empty list)");
   if (avg_out) {
     CU(cudaSetDevice(ctx->device));
-    CU(cudaMemcpyAsync(avg_out, ctx->avg, sizeof(double) * (size_t)ctx->dim, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(avg_out, ctx->avg, sizeof(double) * (size_t)wlen(ctx), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     int rc = persist_check(ctx);   // the sums of a launch that hit its watchdog are garbage
     if (rc) return rc;
     // one IEEE division per column, then the constructor filter of a new Sparse (Sparse.scala:108-118)
     const double n = (double)ctx->avg_n;
-    for (int32_t j = 0; j < ctx->dim; ++j) {
+    for (int64_t j = 0; j < wlen(ctx); ++j) {
       const double v = avg_out[j] / n;
       avg_out[j] = std::fabs(v) > kEps ? v : 0.0;
     }

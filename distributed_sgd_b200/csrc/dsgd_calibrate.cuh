@@ -63,17 +63,19 @@ __device__ __forceinline__ double cal_value(const unsigned long long *words) {
 }
 
 // ---- k_calib_prob ------------------------------------------------------------------------------------------------
-// out[i] = sigmoid(-(a f + b)) for row samples[i], f = x . w: the calibrated probability under either model.  With
+// out[i] = sigmoid(-(a f + b)) for row samples[i], f = x . w (kIcpt: the score with the intercept, row_score): the
+// calibrated probability under either model.  With
 // (a, b) = (1, 0) the argument is -f exactly, i.e. k_margins<true>'s value bit for bit.  One warp per row.
+template <bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_calib_prob(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int32_t *__restrict__ samples, int64_t n,
                                                     const double *__restrict__ w, double a, double b,
-                                                    double *__restrict__ out) {
+                                                    double *__restrict__ out, const double *__restrict__ icpt = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t i = warp0; i < n; i += nwarps) {
-    const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    const double dot = row_score<kIcpt>(rp16, pairs, w, (int64_t)samples[i], lane, icpt);
     if (lane == 0) out[i] = sigmoid(-(a * dot + b));
   }
 }
@@ -90,7 +92,7 @@ enum CalibWeightWord : int { kCalWPos = 0, kCalWNeg = kLossAccWords, kCalWNan = 
 // kW (the weighted fit, DESIGN.md §4.17): cw[i] = c_i = fl(w_y * s_i), the expression of k_metrics_score<kSampleWeighted>
 // (sw == nullptr: every s_i is 1), and R(c_i) added to the three CalibWeightWord sums at wacc; each warp adds its lanes'
 // carried limbs with shuffles (below 2^45 each) and flushes them once.
-template <bool kW>
+template <bool kW, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                      const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                      int64_t row_begin, int64_t n, const double *__restrict__ w,
@@ -98,7 +100,8 @@ __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict_
                                                      unsigned long long *__restrict__ cnt, double w_pos = 1.0,
                                                      double w_neg = 1.0, const double *__restrict__ sw = nullptr,
                                                      double *__restrict__ cw = nullptr,
-                                                     unsigned long long *__restrict__ wacc = nullptr) {
+                                                     unsigned long long *__restrict__ wacc = nullptr,
+                                                     const double *__restrict__ icpt = nullptr) {
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -114,7 +117,7 @@ __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict_
     double dot_own = 0.0;
     for (int j = 0; j < m; ++j) {
       const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_margin(rp16, pairs, w, r, lane);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
       if (lane == j) dot_own = dot;
     }
     if (mine) {

@@ -250,18 +250,19 @@ __device__ __forceinline__ void iso_stage(const double *__restrict__ X, const do
 }
 
 // out[i] = interp(-(x . w)) for row samples[i], x . w the row fold of dsgd_margins.  One warp per row.
-template <bool kSmem>
+template <bool kSmem, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                   const int32_t *__restrict__ samples, int64_t n,
                                                   const double *__restrict__ w, const double *__restrict__ X,
-                                                  const double *__restrict__ Y, int k, double *__restrict__ out) {
+                                                  const double *__restrict__ Y, int k, double *__restrict__ out,
+                                                  const double *__restrict__ icpt = nullptr) {
   const double *xs, *ys;
   iso_stage<kSmem>(X, Y, k, xs, ys);
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t i = warp0; i < n; i += nwarps) {
-    const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    const double dot = row_score<kIcpt>(rp16, pairs, w, (int64_t)samples[i], lane, icpt);
     if (lane == 0) out[i] = iso_interp(-dot, xs, ys, k);
   }
 }
@@ -276,12 +277,13 @@ __global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ r
 // limb words added with shared u64 atomics (p <= 1: each limb adds at most 2^40, so a CTA's words hold 2^24 rows without a
 // wrap, and a grid of 8 CTAs per SM leaves a CTA fewer than that for any 32-bit row count).  The CTA propagates each bin's
 // carries and adds its words to the block with REDs.
-template <bool kIso, bool kSmem>
+template <bool kIso, bool kSmem, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                     int64_t row_begin, int64_t n, const double *__restrict__ w, double a,
                                                     double b, const double *__restrict__ X, const double *__restrict__ Y,
-                                                    int k, int n_bins, unsigned long long *__restrict__ blk) {
+                                                    int k, int n_bins, unsigned long long *__restrict__ blk,
+                                                    const double *__restrict__ icpt = nullptr) {
   __shared__ unsigned long long s_rows[kCalMaxBins], s_pos[kCalMaxBins], s_lim[kCalMaxBins][kLossLimbs];
   const double *xs, *ys;
   iso_stage<kSmem>(X, Y, k, xs, ys);
@@ -306,7 +308,7 @@ __global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__
     double dot_own = 0.0;
     for (int j = 0; j < m; ++j) {
       const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_margin(rp16, pairs, w, r, lane);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
       if (lane == j) dot_own = dot;
     }
     if (!mine) continue;
@@ -551,13 +553,13 @@ __device__ __forceinline__ void cal_bin_add(unsigned long long *lim, unsigned lo
     }
   });
 }
-template <bool kIso, bool kSmem>
+template <bool kIso, bool kSmem, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                int64_t row_begin, int64_t n, const double *__restrict__ w, double a, double b,
                                                const double *__restrict__ X, const double *__restrict__ Y, int k, int n_bins,
                                                unsigned long long *__restrict__ blk, double w_pos, double w_neg,
-                                               const double *__restrict__ sw) {
+                                               const double *__restrict__ sw, const double *__restrict__ icpt = nullptr) {
   __shared__ unsigned long long s_bins[kCalMaxBins * kCwvBinStride];
   const double *xs = nullptr, *ys = nullptr;
   if constexpr (kIso) iso_stage<kSmem>(X, Y, k, xs, ys);
@@ -578,7 +580,7 @@ __global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16
     double dot_own = 0.0;
     for (int j = 0; j < m; ++j) {
       const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_margin(rp16, pairs, w, r, lane);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
       if (lane == j) dot_own = dot;
     }
     if (!mine) continue;

@@ -51,12 +51,19 @@ enum Cnt : int {
   kCntSwLoss = 48,
   kCntSwCorrect = 56,
   kCntSwWeight = 64,
-  kNumCnt = 72
+  // an intercept ctx (kIcpt): the intercept's gradient of the running pass, its positive and its negative parts as two
+  // fixed-point sums (kLossAccWords words each) of k_rows<..., kIcpt>, taken by k_finish, k_finish_acc or k_update
+  kCntIcpt = 72,
+  kNumCnt = 88
 };
 static_assert(kCntLoss + kLossAccWords <= kCntL1 && kCntL1 + kLossAccWords <= kCntNnz && kCntNnz < kCntClassN &&
                   kCntClassLoss + 2 * kLossAccWords <= kCntSwLoss && kCntSwLoss + kLossAccWords <= kCntSwCorrect &&
-                  kCntSwCorrect + kLossAccWords <= kCntSwWeight && kCntSwWeight + kLossAccWords <= kNumCnt,
+                  kCntSwCorrect + kLossAccWords <= kCntSwWeight && kCntSwWeight + kLossAccWords <= kCntIcpt &&
+                  kCntIcpt + 2 * kLossAccWords <= kNumCnt,
               "counter block");
+// Slot of the intercept's gradient in the gradient buffer g and the workers' sum gsum of an intercept ctx: after the loss sum
+// ([dim]) and the batch size ([dim + 1]), which keep their places, so that a plain ctx's buffers do not change.
+constexpr int kIcptSlot = 2;
 
 // Model of a ctx, a compile-time parameter of the kernels whose arithmetic depends on it.
 constexpr int kSvm = 0;        // SparseSVM: hinge loss, integer per-sample losses (SparseSVM.scala:11-33)
@@ -140,6 +147,13 @@ __device__ __forceinline__ double acc_take(unsigned long long *acc) {
     acc[i] = 0ull;
   }
   return acc_value(q);
+}
+// One thread, after a scattering pass of an intercept ctx: the intercept's gradient g_b = filt(P - N) from the two sums of
+// kCntIcpt (both left zeroed), as regularize() leaves an entry that c is never added to
+__device__ __forceinline__ double icpt_take(unsigned long long *cnt) {
+  const double p = acc_take(cnt + kCntIcpt);
+  const double n = acc_take(cnt + kCntIcpt + kLossAccWords);
+  return filt(p - n);
 }
 
 // Gradient scatter: a reduction WITHOUT a return value.  Written as PTX `red` because nvcc 12.9 compiles atomicAdd(double *)
@@ -314,14 +328,18 @@ __device__ __forceinline__ double row_scale(double z) {
 //                   and w = (1, 1) the SVM's S is the integer hinge sum and any other model's S the unweighted limb sum.
 // The counters are plain locals of every form, each form using its own: held in a struct, nvcc orders the loop's
 // registers differently, and the forms would no longer compile to the instructions of the separate kernels they replaced.
+// kIcpt (an intercept ctx, DESIGN.md 4.18): beta = *icpt is the weight of a virtual column of value 1 in every row.  The
+// score is fl(fold + filt(beta)) (the fold's dot, then beta once), and a scattering pass adds each row's filt(s), the value
+// it scatters onto a column with x = 1, to beta's gradient: lane 0 keeps the positive and the negative values in two limb
+// blocks and pushes them once per warp to kCntIcpt (the same bits in any row order or grid).  Otherwise icpt is not read.
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, int kWeight, bool kScatter, bool kPreds = false>
+template <int kModel, int kWeight, bool kScatter, bool kPreds = false, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                               const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                               int64_t row_begin, int64_t n, const double *__restrict__ w,
                                               double *__restrict__ g, double *__restrict__ preds,
                                               unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
-                                              const double *__restrict__ sw) {
+                                              const double *__restrict__ sw, const double *__restrict__ icpt = nullptr) {
   static_assert(!kPreds || (kModel == kSvm && kWeight == kUnweighted), "only the unweighted SVM pass writes predictions");
   constexpr bool kCls = kWeight == kClassWeighted, kSw = kWeight == kSampleWeighted;
   const int lane = threadIdx.x & 31;
@@ -334,10 +352,14 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
   unsigned long long lim_w[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0;
   unsigned n_pos = 0, n_neg = 0, ok_pos = 0, ok_neg = 0, h_pos = 0, h_neg = 0;
   unsigned long long lim_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_pos = 0, ovf_neg = 0;
+  unsigned long long lim_bp[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_bn[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_bp = 0, ovf_bn = 0;
+  double beta = 0.0;
+  if constexpr (kIcpt) beta = filt(__ldg(icpt));
   for (int64_t i = warp0; i < n; i += nwarps) {
     const int64_t r = samples ? (int64_t)samples[i] : row_begin + i;
     const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
-    const double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
+    double dot = row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
+    if constexpr (kIcpt) dot = dot + beta;
     const double y = (double)label[r];
     const int yi = (int)label[r];
     const bool pos = yi > 0;
@@ -389,6 +411,13 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
         if (z < 0.0) continue;  // SparseSVM.scala:28: gradient unless activity < 0
         s = kWeight == kUnweighted ? y : (pos ? c : -c);
       }
+      if constexpr (kIcpt) {
+        const double sb = filt(s);   // filt(filt(1) * s)
+        if (lane == 0) {
+          if (sb > 0.0) acc_add_local(lim_bp, ovf_bp, sb);
+          else if (sb < 0.0) acc_add_local(lim_bn, ovf_bn, -sb);
+        }
+      }
       for (int64_t k = b + lane; k < e; k += 32) {
         const uint2 pr = pairs[k];
         const double gv = filt(filt((double)__uint_as_float(pr.y)) * s);  // x * s: mapValues + constructor filter
@@ -422,6 +451,10 @@ __global__ void __launch_bounds__(256) k_rows(const uint32_t *__restrict__ rp16,
     } else if (hinge | correct) {
       atomicAdd(&cnt[kCntHinge], (unsigned long long)hinge);
       atomicAdd(&cnt[kCntCorrect], (unsigned long long)correct);
+    }
+    if constexpr (kIcpt && kScatter) {
+      acc_flush_local(cnt + kCntIcpt, lim_bp, ovf_bp);
+      acc_flush_local(cnt + kCntIcpt + kLossAccWords, lim_bn, ovf_bn);
     }
   }
 }
@@ -484,8 +517,9 @@ __global__ void k_class_fold(unsigned long long *__restrict__ cnt, double w_pos,
 // (SparseSVM.scala:31; math/Vec.scala:65-75).  Also publishes the batch's hinge sum and size in
 // g[dim], g[dim+1] so that they ride along in the gradient allreduce.
 //   kModel, kCw: where the batch's loss sum comes from (batch_loss_sum; kCw after k_class_fold).
+//   kIcpt: also the intercept's gradient (icpt_take, never regularized) into g[dim + kIcptSlot].
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kCw>
+template <int kModel, bool kCw, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim, const double *__restrict__ scal_c,
                                                 const unsigned long long *__restrict__ cnt, double n_samples) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -498,6 +532,8 @@ __global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim,
   } else if (j == dim) {
     g[dim] = batch_loss_sum<kModel, kCw>(cnt);
     g[dim + 1] = n_samples;
+    if constexpr (kIcpt)   // the request clears the two sums afterwards, with g
+      g[dim + kIcptSlot] = filt(acc_value(cnt + kCntIcpt) - acc_value(cnt + kCntIcpt + kLossAccWords));
   }
 }
 
@@ -506,8 +542,9 @@ __global__ void __launch_bounds__(256) k_finish(double *__restrict__ g, int dim,
 // worker's own support (SparseSVM.scala:31), then sum <- sum + r with the constructor filter after the
 // addition (Vec.sum is a left fold of `+`, math/Vec.scala:128-131), g cleared for the next worker.
 // Slots [dim], [dim+1] of `sum` carry the loss total (kCw: the weighted one) and the sample count of the step.
+// kIcpt: slot [dim + kIcptSlot] folds the intercept's gradients like any other entry (icpt_take, never regularized).
 // ---------------------------------------------------------------------------------------------------
-template <int kModel, bool kCw>
+template <int kModel, bool kCw, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, double *__restrict__ sum, int dim,
                                                     const double *__restrict__ scal_c,
                                                     unsigned long long *__restrict__ cnt, double n_samples, int first) {
@@ -524,6 +561,10 @@ __global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, doub
     const double h = batch_loss_sum<kModel, kCw>(cnt);
     sum[dim] = first ? h : sum[dim] + h;
     sum[dim + 1] = first ? n_samples : sum[dim + 1] + n_samples;
+    if constexpr (kIcpt) {
+      const double v = icpt_take(cnt);
+      sum[dim + kIcptSlot] = first ? v : filt(sum[dim + kIcptSlot] + v);
+    }
     clear_batch_loss<kModel, kCw>(cnt);
     cnt[kCntCorrect] = 0ull;
   }
@@ -544,8 +585,11 @@ __global__ void __launch_bounds__(256) k_finish_acc(double *__restrict__ g, doub
 //   the step's loss adds lambda1 * ||w_before||_1 (scal[kScalL1]).  ||w||_1 is summed in fixed-point limbs (acc_push_block),
 //   so it has the same bits as k_l1_norm over the same weights.  Otherwise lambda1 is not read.
 //   kCw: the batch's loss sum is the class-weighted one of k_class_fold (batch_loss_sum<kModel, true>).
+//   kIcpt: the last block's thread 0 also steps the intercept beta = w[dim] on its gradient g_b (icpt_take with
+//   kFuseRegularize, else g[dim + kIcptSlot]): beta <- filt(beta - filt(filt(g_b / K) * lr)), the other entries' chain
+//   without c and without the L1 step; averaging adds beta to avg[dim].  beta is in neither c, ||w||^2 nor ||w||_1.
 // ---------------------------------------------------------------------------------------------------
-template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1, bool kCw>
+template <bool kFuseRegularize, int kModel, bool kAvg, bool kL1, bool kCw, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *__restrict__ w32, double *__restrict__ g,
                                                 const double *__restrict__ d, int dim, double lambda, double lr,
                                                 double inv_k_den, double *__restrict__ scal,
@@ -627,6 +671,22 @@ __global__ void __launch_bounds__(256) k_update(double *__restrict__ w, float *_
       }
       scal[kScalC] = lambda * 2.0 * sd;
       scal[kScalNrm2] = sn;
+      if constexpr (kIcpt) {
+        double gb;
+        if (kFuseRegularize) {
+          gb = icpt_take(cnt);
+        } else {
+          gb = g[dim + kIcptSlot];
+          g[dim + kIcptSlot] = 0.0;
+        }
+        double beta = w[dim];
+        if (gb != 0.0) {
+          beta = filt(beta - filt(filt(gb / inv_k_den) * lr));
+          w[dim] = beta;
+          w32[dim] = (float)beta;
+        }
+        if (kAvg) avg[dim] = avg[dim] + beta;
+      }
       clear_batch_loss<kModel, kCw>(cnt);
       cnt[kCntCorrect] = 0ull;
       cnt[kCntTicket] = 0ull;

@@ -39,6 +39,16 @@ __device__ __forceinline__ double row_margin(const uint32_t *__restrict__ rp16, 
   return row_fold(pairs, b, e, lane, [&](uint32_t c) { return w[c]; });
 }
 
+// The score of row r: x . w, or on an intercept ctx (kIcpt) fl(x . w + filt(*icpt)), the score of every other reader
+// (k_rows<..., kIcpt>, k_margins<..., kIcpt>).  Otherwise icpt is not read.
+template <bool kIcpt>
+__device__ __forceinline__ double row_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                            const double *__restrict__ w, int64_t r, int lane, const double *__restrict__ icpt) {
+  const double dot = row_margin(rp16, pairs, w, r, lane);
+  if constexpr (kIcpt) return dot + filt(__ldg(icpt));
+  return dot;
+}
+
 // Order-preserving key of a score: +0 and -0 are one key, and key(a) < key(b) exactly when a < b (for non-NaN scores)
 __device__ __forceinline__ unsigned long long score_key(double s) {
   const unsigned long long b = (unsigned long long)__double_as_longlong(s == 0.0 ? 0.0 : s);
@@ -55,15 +65,20 @@ __device__ __forceinline__ double huber_prob(double dot) {
   m = m < -1.0 ? -1.0 : (m > 1.0 ? 1.0 : m);
   return (m + 1.0) / 2.0;
 }
-template <bool kProb, bool kHuber = false>
+// kIcpt (an intercept ctx): the score is fl(x . w + filt(*icpt)), as in k_rows<..., kIcpt>; otherwise icpt is not read.
+template <bool kProb, bool kHuber = false, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                  const int32_t *__restrict__ samples, int64_t n,
-                                                 const double *__restrict__ w, double *__restrict__ out) {
+                                                 const double *__restrict__ w, double *__restrict__ out,
+                                                 const double *__restrict__ icpt = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  double beta = 0.0;
+  if constexpr (kIcpt) beta = filt(__ldg(icpt));
   for (int64_t i = warp0; i < n; i += nwarps) {
-    const double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    double dot = row_margin(rp16, pairs, w, (int64_t)samples[i], lane);
+    if constexpr (kIcpt) dot = dot + beta;
     if (lane == 0) out[i] = !kProb ? dot : (kHuber ? huber_prob(dot) : sigmoid(-dot));
   }
 }
@@ -79,14 +94,15 @@ __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp
 // R(c_i) to the kMetNanPos / kMetNanNeg limbs (each lane flushes its own once).  The weighted confusion sums need nothing
 // more: pred follows the sign of s, so they are read from the runs' prefix sums at the key of +0 (k_curve_sum).
 // ---------------------------------------------------------------------------------------------------
-template <int kWeight>
+template <int kWeight, bool kIcpt = false>
 __global__ void __launch_bounds__(256) k_metrics_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                        const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                        int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                        unsigned long long *__restrict__ keys,
                                                        unsigned long long *__restrict__ cnt, double w_pos = 1.0,
                                                        double w_neg = 1.0, const double *__restrict__ sw = nullptr,
-                                                       double *__restrict__ vals = nullptr) {
+                                                       double *__restrict__ vals = nullptr,
+                                                       const double *__restrict__ icpt = nullptr) {
   static_assert(kWeight == kUnweighted || kWeight == kSampleWeighted, "a metrics pass counts rows or weighs them by c_i");
   constexpr bool kW = kWeight == kSampleWeighted;
   unsigned long long lim_np[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_nn[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_np = 0, ovf_nn = 0;
@@ -103,7 +119,7 @@ __global__ void __launch_bounds__(256) k_metrics_score(const uint32_t *__restric
     double dot_own = 0.0;
     for (int j = 0; j < m; ++j) {
       const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_margin(rp16, pairs, w, r, lane);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
       if (lane == j) dot_own = dot;
     }
     const bool pos = mine && label[r_own] > 0, neg = mine && !pos;

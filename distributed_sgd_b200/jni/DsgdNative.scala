@@ -16,6 +16,11 @@ object DsgdNative {
   final val FlagLogistic = 2
   final val FlagSquaredHinge = 4
   final val FlagModifiedHuber = 8
+  // FlagIntercept (with any one model flag, sync mode only): an unregularised intercept.  Every weight array in or out --
+  // setWeights, getWeights, each request's w, gradient's grad (the intercept's gradient last), averageWeights -- is then
+  // dim + 1 long, the intercept last; d stays dim long.  The shim's own length checks (weightsL1, the weighted evaluations
+  // and curves) take dim + 1 on such a ctx.
+  final val FlagIntercept = 16
   @native def create(device: Int, dim: Int, lambda: Double, rank: Int, world: Int, flags: Int): Long
   @native def destroy(ctx: Long): Int
   @native def lastError(ctx: Long): String

@@ -17,6 +17,7 @@
 #include <stddef.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 #include "dsgd.h"
 
 #define CTX(h) ((dsgd_ctx *)(intptr_t)(h))
@@ -909,15 +910,21 @@ FN(averageWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray avg, jlongAr
   back_Long(env, nSteps, bn, rc);
   return rc;
 }
+/* The length of a weight vector of the ctx: dim, or dim + 1 on a ctx created with DSGD_FLAG_INTERCEPT (dsgd_info names it) */
+static int weight_len(jlong h, int32_t *n) {
+  int rc = dsgd_dim(CTX(h), n);
+  if (rc == DSGD_OK && strstr(dsgd_info(CTX(h)), "\"intercept\": true")) ++*n;
+  return rc;
+}
 /* L1 penalty of the sync steps: setL1(lambda1 >= 0); weightsL1: l1(0) = ||w||_1 and nnz(0) = the non-zero weights of w (dim
- * values), or of the resident weights when w is null.  A w of another length than dim, or an empty output array, is
- * DSGD_ERR_INVALID. */
+ * values, dim + 1 with an intercept, which the norm leaves out), or of the resident weights when w is null.  A w of another
+ * length, or an empty output array, is DSGD_ERR_INVALID. */
 FN(setL1)(JNIEnv *env, jobject self, jlong h, jdouble lambda1) { return dsgd_set_l1(CTX(h), lambda1); }
 FN(weightsL1)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jdoubleArray l1, jlongArray nnz) {
   buf_t bw = in_Double(env, w), bl = out_Double(env, l1), bn = out_Long(env, nnz);
   int rc = DSGD_ERR_NOMEM;
   int32_t dim = 0;
-  if (!(bw.bad | bl.bad | bn.bad) && (rc = dsgd_dim(CTX(h), &dim)) == DSGD_OK)
+  if (!(bw.bad | bl.bad | bn.bad) && (rc = weight_len(h, &dim)) == DSGD_OK)
     rc = (bw.p && (int32_t)bw.n != dim) || (bl.p && bl.n < 1) || (bn.p && bn.n < 1)
              ? DSGD_ERR_INVALID
              : dsgd_weights_l1(CTX(h), (const double *)bw.p, (double *)bl.p, (int64_t *)bn.p);
@@ -988,10 +995,10 @@ FN(setSampleWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray sw) {
   free(b.p);
   return rc;
 }
-/* DSGD_OK when w is null or holds dim values and the outputs are long enough */
+/* DSGD_OK when w is null or holds a weight vector (weight_len values) and the outputs are long enough */
 static int weighted_args(jlong h, const buf_t *bw, const buf_t *bs, const buf_t *bc) {
   int32_t dim = 0;
-  int rc = dsgd_dim(CTX(h), &dim);
+  int rc = weight_len(h, &dim);
   if (rc) return rc;
   return ((bw->p && (int32_t)bw->n != dim) || bs->n < 4 || bc->n < 2) ? DSGD_ERR_INVALID : DSGD_OK;
 }
@@ -1043,7 +1050,7 @@ static wcurve_bufs wcurve_in(JNIEnv *env, jdoubleArray w, jlongArray metrics, jd
 static int wcurve_bad(const wcurve_bufs *c) { return c->w.bad | c->m.bad | c->s.bad | c->k.bad | c->t.bad | c->tp.bad | c->fp.bad; }
 static int wcurve_args(jlong h, const wcurve_bufs *c, jlong n) {
   int32_t dim = 0;
-  int rc = dsgd_dim(CTX(h), &dim);
+  int rc = weight_len(h, &dim);
   if (rc) return rc;
   if ((c->w.p && (int32_t)c->w.n != dim) || c->m.n < DSGD_METRICS_WORDS || c->s.n < DSGD_WCURVE_WORDS || c->k.n < 1)
     return DSGD_ERR_INVALID;

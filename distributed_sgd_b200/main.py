@@ -38,6 +38,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                          "training keeps its constant rate")
     if cfg.l1 != 0.0 and cfg.is_async:
         raise ValueError("l1: the L1 penalty is a step of sync training; asynchronous (Hogwild) training has none")
+    if cfg.fit_intercept and cfg.is_async:
+        raise ValueError("fit-intercept: the intercept is fitted by sync training; asynchronous (Hogwild) training has none")
     from .ml.class_weight import parse_class_weight
     class_weight = parse_class_weight(cfg.class_weight)
     if class_weight is not None and cfg.is_async:
@@ -54,16 +56,17 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     # Main.scala:67-68 ("could use another model"); dimSparsity: computed by the Slave on the device
     model_class = {"logistic": SparseLogistic, "squared_hinge": SparseSquaredHinge,
                    "modified_huber": SparseModifiedHuber}.get(cfg.model, SparseSVM)
-    model = model_class(cfg.lam, l1=cfg.l1, class_weight=class_weight)
+    model = model_class(cfg.lam, l1=cfg.l1, class_weight=class_weight, fit_intercept=cfg.fit_intercept)
     slave = Slave(rank, 0, train, model, cfg.is_async, world=world, device=device, test_data=test)
     master = Master.create(rank, train, test, model, cfg.is_async, cfg.node_count, slave=slave, group=Group(), seed=seed,
                            log=(log if rank == 0 else None), jvm_exact=jvm_exact)
     if inspect:
         inspect("master", master)
-    w0 = np.zeros(data.dim)                                                    # data(0)._1.zerosLike (Main.scala:74)
+    w0 = np.zeros(data.dim + (1 if cfg.fit_intercept else 0))                 # data(0)._1.zerosLike (Main.scala:74)
     report = {"config": {k: getattr(cfg, k) for k in ("batch_size", "learning_rate", "lam", "node_count", "is_async",
                                                       "max_epochs", "check_every", "leaky_loss", "patience", "conv_delta",
-                                                      "model", "learning_rate_decay", "learning_rate_power", "l1")},
+                                                      "model", "learning_rate_decay", "learning_rate_power", "l1",
+                                                      "fit_intercept")},
               "rows": {"train": train.n_rows, "test": test.n_rows}, "world": world}
     report["initial_loss"] = master.distributed_loss(w0)                      # Main.scala:75-76
     report["initial_accuracy"] = master.distributed_accuracy(w0)              # Main.scala:77-78
@@ -84,7 +87,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     report["history"] = {k: [float(x) for x in v] for k, v in getattr(master, "history", {}).items()
                          if isinstance(v, list) and all(isinstance(x, (int, float)) for x in v)}
     report["final_test_loss"], report["final_test_accuracy"] = master.local_loss_accuracy(w1, test_data=True)  # :115-118
-    report["final_weights_nonzero"] = int(np.count_nonzero(w1))
+    report["final_weights_nonzero"] = int(np.count_nonzero(w1[:data.dim]))
+    if cfg.fit_intercept:
+        report["intercept"] = float(w1[data.dim])   # the learned intercept, the last entry of the weights
+        if rank == 0:
+            log(f"intercept: {w1[data.dim]:.6g}")
     report["updates"] = state.updates
     if class_weight is not None:
         report["class_weight"] = list(slave.class_weight)   # as resolved over the train rows

@@ -22,3 +22,5 @@ class SparseLogistic:
     l1: float = 0.0                             # extension: L1 penalty l1 * ||w||_1, a proximal step in every sync step
     # extension: one weight per label on backward and loss in sync training: None, (w_pos, w_neg) or "balanced"
     class_weight: object = None
+    # extension: an unregularised intercept (sync mode): weight vectors are dim + 1 long, the intercept last
+    fit_intercept: bool = False

@@ -26,6 +26,7 @@ FLAG_ASYNC = 1
 FLAG_LOGISTIC = 2
 FLAG_SQUARED_HINGE = 4
 FLAG_MODIFIED_HUBER = 8
+FLAG_INTERCEPT = 16   # an unregularised intercept: weight vectors are dim + 1 long, the intercept last
 # NativeCtx(model=...) -> the model flag of dsgd_create
 MODEL_FLAGS = {"svm": 0, "logistic": FLAG_LOGISTIC, "squared_hinge": FLAG_SQUARED_HINGE, "modified_huber": FLAG_MODIFIED_HUBER}
 REPLICA_SELF, REPLICA_MASTER = 0, 1
@@ -324,10 +325,12 @@ def _arr(a, dtype, n: Optional[int] = None, what: str = "array") -> np.ndarray:
 
 class NativeCtx:
     """One dsgd_ctx == one GPU worker (a reference Slave with its SparseSVM, or with the model named by `model`: "svm",
-    "logistic", "squared_hinge" or "modified_huber"; `logistic=True` is model="logistic")."""
+    "logistic", "squared_hinge" or "modified_huber"; `logistic=True` is model="logistic").  intercept=True: the model fits an
+    unregularised intercept (DSGD_FLAG_INTERCEPT), and every weight vector in or out is wdim = dim + 1 long, the intercept
+    last; d stays dim long."""
 
     def __init__(self, device: int, dim: int, lam: float, rank: int = 0, world: int = 1, is_async: bool = False,
-                 logistic: bool = False, model: Optional[str] = None):
+                 logistic: bool = False, model: Optional[str] = None, intercept: bool = False):
         if model is None:
             model = "logistic" if logistic else "svm"
         elif model not in MODEL_FLAGS or (logistic and model != "logistic"):
@@ -337,7 +340,9 @@ class NativeCtx:
         self.dim, self.lam, self.rank, self.world, self.device = int(dim), float(lam), int(rank), int(world), int(device)
         self.model = model
         self.logistic = model == "logistic"
-        flags = (FLAG_ASYNC if is_async else 0) | MODEL_FLAGS[model]
+        self.intercept = bool(intercept)
+        self.wdim = self.dim + (1 if self.intercept else 0)
+        flags = (FLAG_ASYNC if is_async else 0) | MODEL_FLAGS[model] | (FLAG_INTERCEPT if self.intercept else 0)
         rc = self._l.dsgd_create(C.byref(self._h), device, dim, lam, rank, world, flags)
         if rc != OK:
             msg = (self._l.dsgd_last_error(None) or b"").decode()
@@ -419,17 +424,17 @@ class NativeCtx:
         return out
 
     def set_weights(self, w):
-        w = _arr(w, np.float64, self.dim, "weights")
+        w = _arr(w, np.float64, self.wdim, "weights")
         self._ck(self._l.dsgd_set_weights(self._h, _ptr(w)))
 
     def get_weights(self) -> np.ndarray:
-        out = np.zeros(self.dim, dtype=np.float64)
+        out = np.zeros(self.wdim, dtype=np.float64)
         self._ck(self._l.dsgd_get_weights(self._h, _ptr(out)))
         return out
 
     # -- requests --
     def _w(self, w):
-        return None if w is None else _arr(w, np.float64, self.dim, "weights")
+        return None if w is None else _arr(w, np.float64, self.wdim, "weights")
 
     def forward(self, samples, w=None) -> np.ndarray:
         samples = _arr(samples, np.int32)
@@ -437,7 +442,7 @@ class NativeCtx:
 
     def gradient(self, samples, w=None, want_loss: bool = False):
         samples = _arr(samples, np.int32)
-        out = np.zeros(self.dim, dtype=np.float64)
+        out = np.zeros(self.wdim, dtype=np.float64)
         loss = C.c_double()
         w = self._w(w)
         self._ck(self._l.dsgd_gradient(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out),
@@ -901,7 +906,7 @@ class NativeCtx:
 
     def average_weights(self) -> Tuple[np.ndarray, int]:
         """(mean of the weights after every step averaged since average_begin, number of those steps)."""
-        out = np.zeros(self.dim, dtype=np.float64)
+        out = np.zeros(self.wdim, dtype=np.float64)
         n = C.c_int64()
         self._ck(self._l.dsgd_average_weights(self._h, _ptr(out), C.byref(n)))
         return out, n.value

@@ -42,6 +42,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     calibration_method: str = "sigmoid"   # extension: the calibration `calibrate` fits: sigmoid (Platt) or isotonic
     calibration_weighted: bool = False    # extension: `calibrate` fits and judges with every row counted by its weight
     sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
+    fit_intercept: bool = False   # extension: fit an unregularised intercept (weights dim + 1 long), sync mode only
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -60,6 +61,7 @@ _KEYS = {
     "calibration-method": ("calibration_method", "DSGD_CALIBRATION_METHOD"),
     "calibration-weighted": ("calibration_weighted", "DSGD_CALIBRATION_WEIGHTED"),
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
+    "fit-intercept": ("fit_intercept", "DSGD_FIT_INTERCEPT"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}

@@ -89,6 +89,21 @@ extern "C" {
  * branch tests are false). */
 #define DSGD_FLAG_SQUARED_HINGE 4u
 #define DSGD_FLAG_MODIFIED_HUBER 8u
+/* An unregularised intercept beta, combinable with any one model flag (DESIGN.md section 4.18): the weight of a virtual
+ * column whose value is 1 in every row.  Every score x . w becomes fl(x . w + filt(beta)), beta added once after the row
+ * fold; row i adds filt(s_i) (what it scatters onto a column with x = 1) to beta's gradient; the step is
+ * beta <- filt(beta - filt(filt(g_b / K) * lr)); averaging averages beta too.  beta is in no penalty: not in
+ * lambda * ||w||^2, not in c = 2 lambda (w . d), not in the L1 step, ||w||_1 or its non-zero count.
+ * Lengths: on an intercept ctx every weight vector the ABI reads or writes is dim + 1 doubles, beta last -- dsgd_set_weights,
+ * dsgd_get_weights, the `w` of every request and evaluation, dsgd_average_weights' output, and dsgd_gradient's grad_out
+ * (beta's gradient at [dim]).  d (dsgd_set_dim_sparsity) stays dim long.
+ * Paths: an intercept ctx takes the per-step sync path (never the persistent or fused kernel, so world > 1 needs
+ * dsgd_comm_init; a rank wired with the peer exchange only fails with DSGD_ERR_STATE before any launch) and the fp64 row
+ * kernel for every request (never the fp32 streaming pass).  Every reader scores with beta: dsgd_margins,
+ * dsgd_probabilities, the metrics and curve calls, the Platt, isotonic and weighted calibrations and their probabilities and
+ * quality passes.  dsgd_info reports "intercept": true.  Combined with
+ * DSGD_FLAG_ASYNC, dsgd_create fails with DSGD_ERR_INVALID before it looks for a device. */
+#define DSGD_FLAG_INTERCEPT 16u
 
 typedef struct dsgd_ctx dsgd_ctx;
 
