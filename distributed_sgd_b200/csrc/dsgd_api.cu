@@ -797,7 +797,8 @@ static int stream_launch(dsgd_ctx *ctx, const int32_t *samples_dev, int64_t row_
 
 // The rows of a request: rows [row_begin, row_begin + n) when ids == nullptr, else the n row ids at the device address ids
 // (in eval_ids: the staged stream stays as it was for the next dsgd_sync_steps_staged).  rows_range, rows_drawn and
-// rows_list check the rows a request names and build its row_set; fn is the entry point, and every message names it.
+// rows_list check the rows a request names and build its row_set (an evaluation reaches them through resolve_rows); fn is
+// the entry point, and every message names it.
 struct row_set {
   const int32_t *ids;
   int64_t row_begin, n;
@@ -894,6 +895,39 @@ static int rows_list(dsgd_ctx *ctx, const int32_t *ids, int64_t n, bool preds, c
   CU(cudaMemcpyAsync(ctx->eval_ids, ids, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if (preds && (rc = ctx->preds.grow(ctx, n, 1024))) return rc;
   *rows = {ctx->eval_ids, 0, n};
+  return DSGD_OK;
+}
+
+// The rows an evaluation's caller named, in one of its three forms: a range, a sample drawn from a range, or a host list of
+// ids.  Each family's request function makes its checks once, then resolve_rows builds the row_set.
+struct row_request {
+  enum { kRange, kDrawn, kList } form;
+  int64_t row_begin, row_end;
+  uint64_t key;
+  int64_t pos_begin, pos_end;
+  const int32_t *ids;
+  int64_t n;
+};
+static row_request range_rows(int64_t row_begin, int64_t row_end) {
+  return {row_request::kRange, row_begin, row_end, 0, 0, 0, nullptr, 0};
+}
+static row_request drawn_rows(int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end) {
+  return {row_request::kDrawn, row_begin, row_end, key, pos_begin, pos_end, nullptr, 0};
+}
+static row_request listed_rows(const int32_t *ids, int64_t n) { return {row_request::kList, 0, 0, 0, 0, 0, ids, n}; }
+
+static int resolve_rows(dsgd_ctx *ctx, const row_request &req, const char *fn, row_set *rows) {
+  switch (req.form) {
+    case row_request::kRange: return rows_range(ctx, req.row_begin, req.row_end, fn, rows);
+    case row_request::kDrawn: return rows_drawn(ctx, req.row_begin, req.row_end, req.key, req.pos_begin, req.pos_end, fn, rows);
+    default: return rows_list(ctx, req.ids, req.n, false, fn, rows);
+  }
+}
+
+// the metrics, curve and calibration calls take a list of at most 2^31 - 1 ids; a range or a drawn sample passes
+static int ids_capped(dsgd_ctx *ctx, const row_request &req, const char *fn) {
+  NEED(req.form != row_request::kList || req.n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", fn,
+       (long long)req.n);
   return DSGD_OK;
 }
 
@@ -1036,69 +1070,67 @@ static int eval_sums(dsgd_ctx *ctx, const double *w, const row_set &rows, double
 // the *_counts calls report integer hinge sums, which only the SVM has
 static const char kCountsNeedSvm[] = "%s: the %s model's loss sum is not an integer; use the *_sums call";
 
-extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
-                         double *acc_out) {
+// dsgd_eval: the loss and the accuracy (NULL: not wanted)
+static int eval_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, double *loss_out,
+                        double *acc_out) {
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
   double out[5];
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
+  int rc = resolve_rows(ctx, req, fn, &rows);
   if (rc || (rc = eval_pass(ctx, w, rows, out))) return rc;
   if (loss_out) *loss_out = out[0];
   if (acc_out) *acc_out = out[1];
   return DSGD_OK;
 }
 
+// the *_counts (kCounts: the SVM's integer hinge sum) and *_sums calls
+template <bool kCounts>
+static int sums_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, double *loss_sum,
+                        int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  if constexpr (kCounts) NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, fn, kModelNames[model_of(ctx)]);
+  row_set rows;
+  int rc = resolve_rows(ctx, req, fn, &rows);
+  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, hinge_sum, correct, norm_squared);
+}
+
+extern "C" int dsgd_eval(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_out,
+                         double *acc_out) {
+  return eval_request(ctx, w, range_rows(row_begin, row_end), __func__, loss_out, acc_out);
+}
+
 extern "C" int dsgd_eval_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *hinge_sum,
                                 int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+  return sums_request<true>(ctx, w, range_rows(row_begin, row_end), __func__, nullptr, hinge_sum, correct, norm_squared);
 }
 
 extern "C" int dsgd_eval_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *loss_sum,
                               int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+  return sums_request<false>(ctx, w, range_rows(row_begin, row_end), __func__, loss_sum, nullptr, correct, norm_squared);
 }
 
 extern "C" int dsgd_eval_sampled_counts(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                         int64_t pos_begin, int64_t pos_end, int64_t *hinge_sum, int64_t *correct,
                                         double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+  return sums_request<true>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, nullptr, hinge_sum,
+                            correct, norm_squared);
 }
 
 extern "C" int dsgd_eval_sampled_sums(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                       int64_t pos_begin, int64_t pos_end, double *loss_sum, int64_t *correct,
                                       double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+  return sums_request<false>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, loss_sum, nullptr,
+                             correct, norm_squared);
 }
 
 extern "C" int dsgd_eval_samples_counts(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                         int64_t *hinge_sum, int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(model_of(ctx) == kSvm, DSGD_ERR_STATE, kCountsNeedSvm, __func__, kModelNames[model_of(ctx)]);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, nullptr, hinge_sum, correct, norm_squared);
+  return sums_request<true>(ctx, w, listed_rows(samples, n), __func__, nullptr, hinge_sum, correct, norm_squared);
 }
 
 extern "C" int dsgd_eval_samples_sums(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *loss_sum,
                                       int64_t *correct, double *norm_squared) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : eval_sums(ctx, w, rows, loss_sum, nullptr, correct, norm_squared);
+  return sums_request<false>(ctx, w, listed_rows(samples, n), __func__, loss_sum, nullptr, correct, norm_squared);
 }
 
 // One evaluation pass of a weighted tally over `rows`: the row kernel without the scatter, then its fold into cls_out.
@@ -1133,54 +1165,49 @@ static int tally_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, doubl
   return DSGD_OK;
 }
 
-extern "C" int dsgd_eval_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
-                               double *loss_sums_out, int64_t *counts_out) {
+// dsgd_eval*_class (kClassWeighted) and dsgd_eval*_weighted (kSampleWeighted)
+template <int kWeight>
+static int tally_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, double *norm_squared,
+                         double *sums_out, int64_t *counts_out) {
   if (!ctx) return DSGD_ERR_INVALID;
   row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+  int rc = resolve_rows(ctx, req, fn, &rows);
+  return rc ? rc : tally_pass<kWeight>(ctx, w, rows, norm_squared, sums_out, counts_out);
+}
+
+extern "C" int dsgd_eval_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
+                               double *loss_sums_out, int64_t *counts_out) {
+  return tally_request<kClassWeighted>(ctx, w, range_rows(row_begin, row_end), __func__, norm_squared, loss_sums_out,
+                                       counts_out);
 }
 
 extern "C" int dsgd_eval_sampled_class(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                        int64_t pos_begin, int64_t pos_end, double *norm_squared, double *loss_sums_out,
                                        int64_t *counts_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+  return tally_request<kClassWeighted>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__,
+                                       norm_squared, loss_sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_samples_class(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                        double *norm_squared, double *loss_sums_out, int64_t *counts_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : tally_pass<kClassWeighted>(ctx, w, rows, norm_squared, loss_sums_out, counts_out);
+  return tally_request<kClassWeighted>(ctx, w, listed_rows(samples, n), __func__, norm_squared, loss_sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *norm_squared,
                                   double *sums_out, int64_t *counts_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return tally_request<kSampleWeighted>(ctx, w, range_rows(row_begin, row_end), __func__, norm_squared, sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_sampled_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                           int64_t pos_begin, int64_t pos_end, double *norm_squared, double *sums_out,
                                           int64_t *counts_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return tally_request<kSampleWeighted>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__,
+                                        norm_squared, sums_out, counts_out);
 }
 
 extern "C" int dsgd_eval_samples_weighted(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                           double *norm_squared, double *sums_out, int64_t *counts_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : tally_pass<kSampleWeighted>(ctx, w, rows, norm_squared, sums_out, counts_out);
+  return tally_request<kSampleWeighted>(ctx, w, listed_rows(samples, n), __func__, norm_squared, sums_out, counts_out);
 }
 
 // ---- scores and ranking metrics (dsgd_metrics.cuh) ------------------------------------------------------------------
@@ -1439,37 +1466,6 @@ static int curve_outputs(dsgd_ctx *ctx, const int64_t *words, const double *ap, 
   return DSGD_OK;
 }
 
-extern "C" int dsgd_eval_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *words_out,
-                               double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
-  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-}
-
-extern "C" int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                       int64_t pos_begin, int64_t pos_end, int64_t *words_out, double *ap_out,
-                                       int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
-  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-}
-
-extern "C" int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
-                                       double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out,
-                                       int64_t *fp_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = curve_outputs(ctx, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-  if (rc) return rc;
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  if ((rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
-  return curve_pass<kUnweighted>(ctx, w, rows, words_out, ap_out, n_points_out, thr_out, tp_out, fp_out, __func__);
-}
-
 // A weighted curve call: the outputs as curve_outputs checks them (wsums_out in ap_out's place, tpw / fpw in tp / fp's), then
 // an async ctx is refused before anything is launched -- its weights are always 1, and growing the pass's buffers would wait
 // for the loop, which runs until stopped.
@@ -1483,63 +1479,82 @@ static int weighted_curve_args(dsgd_ctx *ctx, const int64_t *words, const double
   return DSGD_OK;
 }
 
+// dsgd_eval*_curve (kUnweighted: AP into out, the point counts into tp / fp) and dsgd_eval*_weighted_curve (kSampleWeighted:
+// the DSGD_WCURVE_WORDS sums into out, the point weights into tp / fp)
+template <int kWeight, class P>
+static int curve_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, int64_t *words, double *out,
+                         int64_t *n_points, double *thr, P *tp, P *fp) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  int rc;
+  if constexpr (kWeight == kSampleWeighted) rc = weighted_curve_args(ctx, words, out, n_points, thr, tp, fp, fn);
+  else rc = curve_outputs(ctx, words, out, n_points, thr, tp, fp, fn);
+  row_set rows;
+  if (rc || (rc = ids_capped(ctx, req, fn)) || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  return curve_pass<kWeight>(ctx, w, rows, words, out, n_points, thr, tp, fp, fn);
+}
+
+extern "C" int dsgd_eval_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *words_out,
+                               double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
+  return curve_request<kUnweighted>(ctx, w, range_rows(row_begin, row_end), __func__, words_out, ap_out, n_points_out, thr_out,
+                                    tp_out, fp_out);
+}
+
+extern "C" int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                       int64_t pos_begin, int64_t pos_end, int64_t *words_out, double *ap_out,
+                                       int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out) {
+  return curve_request<kUnweighted>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, words_out,
+                                    ap_out, n_points_out, thr_out, tp_out, fp_out);
+}
+
+extern "C" int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
+                                       double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out,
+                                       int64_t *fp_out) {
+  return curve_request<kUnweighted>(ctx, w, listed_rows(samples, n), __func__, words_out, ap_out, n_points_out, thr_out,
+                                    tp_out, fp_out);
+}
+
 extern "C" int dsgd_eval_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                         int64_t *words_out, double *wsums_out, int64_t *n_points_out, double *thr_out,
                                         double *tpw_out, double *fpw_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
-  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
-  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  return curve_request<kSampleWeighted>(ctx, w, range_rows(row_begin, row_end), __func__, words_out, wsums_out, n_points_out,
+                                        thr_out, tpw_out, fpw_out);
 }
 
 extern "C" int dsgd_eval_sampled_weighted_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                 uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *words_out,
                                                 double *wsums_out, int64_t *n_points_out, double *thr_out, double *tpw_out,
                                                 double *fpw_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  row_set rows;
-  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
-  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
-  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  return curve_request<kSampleWeighted>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, words_out,
+                                        wsums_out, n_points_out, thr_out, tpw_out, fpw_out);
 }
 
 extern "C" int dsgd_eval_samples_weighted_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                 int64_t *words_out, double *wsums_out, int64_t *n_points_out,
                                                 double *thr_out, double *tpw_out, double *fpw_out) {
+  return curve_request<kSampleWeighted>(ctx, w, listed_rows(samples, n), __func__, words_out, wsums_out, n_points_out,
+                                        thr_out, tpw_out, fpw_out);
+}
+
+static int metrics_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, int64_t *out) {
   if (!ctx) return DSGD_ERR_INVALID;
+  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", fn);
   row_set rows;
-  int rc = weighted_curve_args(ctx, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
-  if (rc) return rc;
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  if ((rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
-  return curve_pass<kSampleWeighted>(ctx, w, rows, words_out, wsums_out, n_points_out, thr_out, tpw_out, fpw_out, __func__);
+  int rc = ids_capped(ctx, req, fn);
+  if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  return metrics_pass(ctx, w, rows, out, fn);
 }
 
 extern "C" int dsgd_eval_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, int64_t *out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
+  return metrics_request(ctx, w, range_rows(row_begin, row_end), __func__, out);
 }
 
 extern "C" int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
                                          int64_t pos_begin, int64_t pos_end, int64_t *out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
+  return metrics_request(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, out);
 }
 
 extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", __func__);
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : metrics_pass(ctx, w, rows, out, __func__);
+  return metrics_request(ctx, w, listed_rows(samples, n), __func__, out);
 }
 
 // ---- calibration (dsgd_calibrate.cuh; DESIGN.md §4.11) ---------------------------------------------------------------
@@ -1678,41 +1693,6 @@ static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, d
   return DSGD_OK;
 }
 
-#define CALIB_ARGS_OK() \
-  NEED(ab_out && objective_out && info_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__)
-
-extern "C" int dsgd_calibrate(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
-                              double *objective_out, int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_ARGS_OK();
-  row_set rows;
-  int rc = calibrate_allowed(ctx, __func__);
-  if (rc || (rc = rows_range(ctx, row_begin, row_end, __func__, &rows))) return rc;
-  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
-}
-
-extern "C" int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                      int64_t pos_begin, int64_t pos_end, double *ab_out, double *objective_out,
-                                      int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_ARGS_OK();
-  row_set rows;
-  int rc = calibrate_allowed(ctx, __func__);
-  if (rc || (rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows))) return rc;
-  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
-}
-
-extern "C" int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
-                                      double *objective_out, int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = calibrate_allowed(ctx, __func__);
-  if (rc || (rc = rows_list(ctx, samples, n, false, __func__, &rows))) return rc;
-  return calibrate_pass<false>(ctx, w, rows, ab_out, objective_out, info_out, nullptr, __func__);
-}
-
 // A weighted calibration call: an async ctx is refused before anything is launched (its weights are always 1), as the
 // weighted curves refuse it.
 static int weighted_calibration_allowed(dsgd_ctx *ctx, const char *fn) {
@@ -1721,40 +1701,53 @@ static int weighted_calibration_allowed(dsgd_ctx *ctx, const char *fn) {
   return DSGD_OK;
 }
 
-#define CALIB_W_ARGS_OK()                                                                                               \
-  do {                                                                                                                  \
-    NEED(ab_out && objective_out && info_out && wsums_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);         \
-    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
-    if (rc_) return rc_;                                                                                                \
-  } while (0)
+// dsgd_calibrate* and (kW) dsgd_calibrate_weighted*, which also write wsums_out
+template <bool kW>
+static int calibrate_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, double *ab_out,
+                             double *objective_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(ab_out && objective_out && info_out && (!kW || wsums_out), DSGD_ERR_INVALID, "%s: an output is NULL", fn);
+  int rc = kW ? weighted_calibration_allowed(ctx, fn) : DSGD_OK;
+  if (rc || (rc = ids_capped(ctx, req, fn))) return rc;
+  if (!kW && (rc = calibrate_allowed(ctx, fn))) return rc;
+  row_set rows;
+  if ((rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  return calibrate_pass<kW>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, fn);
+}
+
+extern "C" int dsgd_calibrate(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
+                              double *objective_out, int64_t *info_out) {
+  return calibrate_request<false>(ctx, w, range_rows(row_begin, row_end), __func__, ab_out, objective_out, info_out, nullptr);
+}
+
+extern "C" int dsgd_calibrate_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                      int64_t pos_begin, int64_t pos_end, double *ab_out, double *objective_out,
+                                      int64_t *info_out) {
+  return calibrate_request<false>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, ab_out,
+                                  objective_out, info_out, nullptr);
+}
+
+extern "C" int dsgd_calibrate_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double *ab_out,
+                                      double *objective_out, int64_t *info_out) {
+  return calibrate_request<false>(ctx, w, listed_rows(samples, n), __func__, ab_out, objective_out, info_out, nullptr);
+}
 
 extern "C" int dsgd_calibrate_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double *ab_out,
                                        double *objective_out, int64_t *info_out, double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_W_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
+  return calibrate_request<true>(ctx, w, range_rows(row_begin, row_end), __func__, ab_out, objective_out, info_out,
+                                 wsums_out);
 }
 
 extern "C" int dsgd_calibrate_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                uint64_t key, int64_t pos_begin, int64_t pos_end, double *ab_out,
                                                double *objective_out, int64_t *info_out, double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_W_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
+  return calibrate_request<true>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, ab_out,
+                                 objective_out, info_out, wsums_out);
 }
 
 extern "C" int dsgd_calibrate_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                double *ab_out, double *objective_out, int64_t *info_out, double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_W_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : calibrate_pass<true>(ctx, w, rows, ab_out, objective_out, info_out, wsums_out, __func__);
+  return calibrate_request<true>(ctx, w, listed_rows(samples, n), __func__, ab_out, objective_out, info_out, wsums_out);
 }
 
 extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
@@ -1831,48 +1824,6 @@ static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_se
   return DSGD_OK;
 }
 
-#define CALIB_EVAL_ARGS_OK()                                                                                            \
-  do {                                                                                                                  \
-    NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);  \
-    NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", __func__, a, b); \
-    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
-  } while (0)
-
-extern "C" int dsgd_eval_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a, double b,
-                                     int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
-                                     int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_EVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
-                                                    bin_pos, bin_psum, words_out, __func__);
-}
-
-extern "C" int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
-                                             int64_t pos_begin, int64_t pos_end, double a, double b, int32_t n_bins,
-                                             double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
-                                             int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_EVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
-                                                    bin_pos, bin_psum, words_out, __func__);
-}
-
-extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
-                                             double b, int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
-                                             double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_EVAL_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : calibration_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_rows,
-                                                    bin_pos, bin_psum, words_out, __func__);
-}
-
 // One weighted quality pass over `rows`, at (a, b) or (kIso) at the map (X, Y): k_weval, the block read back, every sum
 // read() on the host.
 template <bool kIso>
@@ -1925,50 +1876,71 @@ static int weighted_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &
   return DSGD_OK;
 }
 
-#define CALIB_WEVAL_ARGS_OK()                                                                                           \
-  do {                                                                                                                  \
-    NEED(sums_out && bin_weight && bin_pos_weight && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL",   \
-         __func__);                                                                                                     \
-    NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", __func__, a, b); \
-    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
-    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
-    if (rc_) return rc_;                                                                                                \
-  } while (0)
+// The quality calls: dsgd_eval*_calibration at the sigmoid (a, b), or (kIso) dsgd_eval*_isotonic_calibration at the map
+// (X, Y); counted (B = int64_t: the rows and the positives of each bin), or (kW) weighted (B = double: their weights)
+template <bool kIso, bool kW, class B>
+static int quality_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, double a, double b,
+                           const double *X, const double *Y, int64_t k, int32_t n_bins, double *sums_out, B *bin_rows,
+                           B *bin_pos, double *bin_psum, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", fn);
+  if constexpr (!kIso)
+    NEED(std::isfinite(a) && std::isfinite(b), DSGD_ERR_INVALID, "%s: (a, b) = (%g, %g) is not finite", fn, a, b);
+  NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", fn, (int)n_bins, kCalMaxBins);
+  int rc = kW ? weighted_calibration_allowed(ctx, fn) : DSGD_OK;
+  row_set rows;
+  if (rc || (rc = ids_capped(ctx, req, fn)) || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  if constexpr (kW)
+    return weighted_quality_pass<kIso>(ctx, w, rows, a, b, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
+                                       words_out, fn);
+  else
+    return calibration_quality_pass<kIso>(ctx, w, rows, a, b, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
+                                          words_out, fn);
+}
+
+extern "C" int dsgd_eval_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a, double b,
+                                     int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                     int64_t *words_out) {
+  return quality_request<false, false>(ctx, w, range_rows(row_begin, row_end), __func__, a, b, nullptr, nullptr, 0, n_bins,
+                                       sums_out, bin_rows, bin_pos, bin_psum, words_out);
+}
+
+extern "C" int dsgd_eval_sampled_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                             int64_t pos_begin, int64_t pos_end, double a, double b, int32_t n_bins,
+                                             double *sums_out, int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
+                                             int64_t *words_out) {
+  return quality_request<false, false>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, a, b,
+                                       nullptr, nullptr, 0, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out);
+}
+
+extern "C" int dsgd_eval_samples_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, double a,
+                                             double b, int32_t n_bins, double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
+                                             double *bin_psum, int64_t *words_out) {
+  return quality_request<false, false>(ctx, w, listed_rows(samples, n), __func__, a, b, nullptr, nullptr, 0, n_bins, sums_out,
+                                       bin_rows, bin_pos, bin_psum, words_out);
+}
 
 extern "C" int dsgd_eval_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, double a,
                                               double b, int32_t n_bins, double *sums_out, double *bin_weight,
                                               double *bin_pos_weight, double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_WEVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
-                                                 bin_pos_weight, bin_psum, words_out, __func__);
+  return quality_request<false, true>(ctx, w, range_rows(row_begin, row_end), __func__, a, b, nullptr, nullptr, 0, n_bins,
+                                      sums_out, bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_sampled_weighted_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                       uint64_t key, int64_t pos_begin, int64_t pos_end, double a, double b,
                                                       int32_t n_bins, double *sums_out, double *bin_weight,
                                                       double *bin_pos_weight, double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_WEVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
-                                                 bin_pos_weight, bin_psum, words_out, __func__);
+  return quality_request<false, true>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, a, b,
+                                      nullptr, nullptr, 0, n_bins, sums_out, bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_samples_weighted_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                       double a, double b, int32_t n_bins, double *sums_out,
                                                       double *bin_weight, double *bin_pos_weight, double *bin_psum,
                                                       int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  CALIB_WEVAL_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : weighted_quality_pass<false>(ctx, w, rows, a, b, nullptr, nullptr, 0, n_bins, sums_out, bin_weight,
-                                                 bin_pos_weight, bin_psum, words_out, __func__);
+  return quality_request<false, true>(ctx, w, listed_rows(samples, n), __func__, a, b, nullptr, nullptr, 0, n_bins, sums_out,
+                                      bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 // ---- isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.16) ------------------------------------------------------
@@ -2066,40 +2038,47 @@ static int isotonic_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, in
   return DSGD_OK;
 }
 
-#define ISO_ARGS_OK()                                                                                                 \
-  NEED(n_points_out && x_out && y_out && rows_out && pos_out && info_out, DSGD_ERR_INVALID, "%s: an output is NULL", \
-       __func__)
+static int isotonic_weighted_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, int64_t *n_points_out, double *x_out,
+                                  double *y_out, double *wrows_out, double *wpos_out, int64_t *info_out, double *wsums_out,
+                                  const char *fn);
+
+// dsgd_calibrate_isotonic* (B = int64_t: the blocks' rows and positives) and (kW) dsgd_calibrate_isotonic_weighted*
+// (B = double: their weights; wsums_out too)
+template <bool kW, class B>
+static int isotonic_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, int64_t *n_points_out,
+                            double *x_out, double *y_out, B *rows_out, B *pos_out, int64_t *info_out, double *wsums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(n_points_out && x_out && y_out && rows_out && pos_out && info_out && (!kW || wsums_out), DSGD_ERR_INVALID,
+       "%s: an output is NULL", fn);
+  int rc = kW ? weighted_calibration_allowed(ctx, fn) : DSGD_OK;
+  row_set rows;
+  if (rc || (rc = ids_capped(ctx, req, fn)) || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  if constexpr (kW)
+    return isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, wsums_out, fn);
+  else
+    return isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, fn);
+}
 
 extern "C" int dsgd_calibrate_isotonic(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                        int64_t *n_points_out, double *x_out, double *y_out, int64_t *rows_out,
                                        int64_t *pos_out, int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+  return isotonic_request<false>(ctx, w, range_rows(row_begin, row_end), __func__, n_points_out, x_out, y_out, rows_out,
+                                 pos_out, info_out, nullptr);
 }
 
 extern "C" int dsgd_calibrate_isotonic_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *n_points_out,
                                                double *x_out, double *y_out, int64_t *rows_out, int64_t *pos_out,
                                                int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+  return isotonic_request<false>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, n_points_out,
+                                 x_out, y_out, rows_out, pos_out, info_out, nullptr);
 }
 
 extern "C" int dsgd_calibrate_isotonic_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                int64_t *n_points_out, double *x_out, double *y_out, int64_t *rows_out,
                                                int64_t *pos_out, int64_t *info_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc : isotonic_pass(ctx, w, rows, n_points_out, x_out, y_out, rows_out, pos_out, info_out, __func__);
+  return isotonic_request<false>(ctx, w, listed_rows(samples, n), __func__, n_points_out, x_out, y_out, rows_out, pos_out,
+                                 info_out, nullptr);
 }
 
 // A map (X, Y) of k points: X finite and strictly increasing, Y in [0, 1]; copied into i_map (X, then Y)
@@ -2133,7 +2112,7 @@ extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const
                                            const double *Y, int64_t k, double *probs_out) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(probs_out, DSGD_ERR_INVALID, "%s: output is NULL", __func__);
-  row_set rows;
+  row_set rows{};   // set whenever rows_list succeeds; initialised because GCC's -Wmaybe-uninitialized cannot see that
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd)) || (rc = isotonic_map(ctx, X, Y, k, __func__))) return rc;
@@ -2156,22 +2135,11 @@ extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const
   return DSGD_OK;
 }
 
-#define ISO_EVAL_ARGS_OK()                                                                                              \
-  do {                                                                                                                  \
-    NEED(sums_out && bin_rows && bin_pos && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", __func__);  \
-    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
-  } while (0)
-
 extern "C" int dsgd_eval_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                               const double *X, const double *Y, int64_t k, int32_t n_bins, double *sums_out,
                                               int64_t *bin_rows, int64_t *bin_pos, double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_EVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc
-            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
-                                             words_out, __func__);
+  return quality_request<true, false>(ctx, w, range_rows(row_begin, row_end), __func__, 0.0, 0.0, X, Y, k, n_bins, sums_out,
+                                      bin_rows, bin_pos, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
@@ -2179,27 +2147,16 @@ extern "C" int dsgd_eval_sampled_isotonic_calibration(dsgd_ctx *ctx, const doubl
                                                       const double *Y, int64_t k, int32_t n_bins, double *sums_out,
                                                       int64_t *bin_rows, int64_t *bin_pos, double *bin_psum,
                                                       int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_EVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc
-            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
-                                             words_out, __func__);
+  return quality_request<true, false>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, 0.0, 0.0, X,
+                                      Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_samples_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                       const double *X, const double *Y, int64_t k, int32_t n_bins,
                                                       double *sums_out, int64_t *bin_rows, int64_t *bin_pos,
                                                       double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_EVAL_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc
-            : calibration_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_rows, bin_pos, bin_psum,
-                                             words_out, __func__);
+  return quality_request<true, false>(ctx, w, listed_rows(samples, n), __func__, 0.0, 0.0, X, Y, k, n_bins, sums_out,
+                                      bin_rows, bin_pos, bin_psum, words_out);
 }
 
 // ---- weighted isotonic calibration (dsgd_isotonic.cuh; DESIGN.md §4.17) -----------------------------------------------
@@ -2274,24 +2231,11 @@ static int isotonic_weighted_pass(dsgd_ctx *ctx, const double *w, const row_set 
   return DSGD_OK;
 }
 
-#define ISO_W_ARGS_OK()                                                                                               \
-  do {                                                                                                                \
-    NEED(n_points_out && x_out && y_out && wrows_out && wpos_out && info_out && wsums_out, DSGD_ERR_INVALID,          \
-         "%s: an output is NULL", __func__);                                                                          \
-    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                            \
-    if (rc_) return rc_;                                                                                              \
-  } while (0)
-
 extern "C" int dsgd_calibrate_isotonic_weighted(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                 int64_t *n_points_out, double *x_out, double *y_out, double *wrows_out,
                                                 double *wpos_out, int64_t *info_out, double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_W_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc
-            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
-                                     __func__);
+  return isotonic_request<true>(ctx, w, range_rows(row_begin, row_end), __func__, n_points_out, x_out, y_out, wrows_out,
+                                wpos_out, info_out, wsums_out);
 }
 
 extern "C" int dsgd_calibrate_isotonic_weighted_sampled(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
@@ -2299,49 +2243,24 @@ extern "C" int dsgd_calibrate_isotonic_weighted_sampled(dsgd_ctx *ctx, const dou
                                                         int64_t *n_points_out, double *x_out, double *y_out,
                                                         double *wrows_out, double *wpos_out, int64_t *info_out,
                                                         double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_W_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc
-            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
-                                     __func__);
+  return isotonic_request<true>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, n_points_out,
+                                x_out, y_out, wrows_out, wpos_out, info_out, wsums_out);
 }
 
 extern "C" int dsgd_calibrate_isotonic_weighted_samples(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
                                                         int64_t *n_points_out, double *x_out, double *y_out,
                                                         double *wrows_out, double *wpos_out, int64_t *info_out,
                                                         double *wsums_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_W_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc
-            : isotonic_weighted_pass(ctx, w, rows, n_points_out, x_out, y_out, wrows_out, wpos_out, info_out, wsums_out,
-                                     __func__);
+  return isotonic_request<true>(ctx, w, listed_rows(samples, n), __func__, n_points_out, x_out, y_out, wrows_out, wpos_out,
+                                info_out, wsums_out);
 }
-
-#define ISO_WEVAL_ARGS_OK()                                                                                             \
-  do {                                                                                                                  \
-    NEED(sums_out && bin_weight && bin_pos_weight && bin_psum && words_out, DSGD_ERR_INVALID, "%s: an output is NULL",   \
-         __func__);                                                                                                     \
-    NEED(n_bins >= 1 && n_bins <= kCalMaxBins, DSGD_ERR_INVALID, "%s: %d bins; 1 to %d", __func__, (int)n_bins, kCalMaxBins); \
-    int rc_ = weighted_calibration_allowed(ctx, __func__);                                                              \
-    if (rc_) return rc_;                                                                                                \
-  } while (0)
 
 extern "C" int dsgd_eval_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
                                                        const double *X, const double *Y, int64_t k, int32_t n_bins,
                                                        double *sums_out, double *bin_weight, double *bin_pos_weight,
                                                        double *bin_psum, int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_WEVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_range(ctx, row_begin, row_end, __func__, &rows);
-  return rc ? rc
-            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
-                                          bin_psum, words_out, __func__);
+  return quality_request<true, true>(ctx, w, range_rows(row_begin, row_end), __func__, 0.0, 0.0, X, Y, k, n_bins, sums_out,
+                                     bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_sampled_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, int64_t row_begin,
@@ -2350,13 +2269,8 @@ extern "C" int dsgd_eval_sampled_weighted_isotonic_calibration(dsgd_ctx *ctx, co
                                                                int32_t n_bins, double *sums_out, double *bin_weight,
                                                                double *bin_pos_weight, double *bin_psum,
                                                                int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_WEVAL_ARGS_OK();
-  row_set rows;
-  int rc = rows_drawn(ctx, row_begin, row_end, key, pos_begin, pos_end, __func__, &rows);
-  return rc ? rc
-            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
-                                          bin_psum, words_out, __func__);
+  return quality_request<true, true>(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, 0.0, 0.0, X,
+                                     Y, k, n_bins, sums_out, bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 extern "C" int dsgd_eval_samples_weighted_isotonic_calibration(dsgd_ctx *ctx, const double *w, const int32_t *samples,
@@ -2364,14 +2278,8 @@ extern "C" int dsgd_eval_samples_weighted_isotonic_calibration(dsgd_ctx *ctx, co
                                                                int32_t n_bins, double *sums_out, double *bin_weight,
                                                                double *bin_pos_weight, double *bin_psum,
                                                                int64_t *words_out) {
-  if (!ctx) return DSGD_ERR_INVALID;
-  ISO_WEVAL_ARGS_OK();
-  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
-  row_set rows;
-  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
-  return rc ? rc
-            : weighted_quality_pass<true>(ctx, w, rows, 0.0, 0.0, X, Y, k, n_bins, sums_out, bin_weight, bin_pos_weight,
-                                          bin_psum, words_out, __func__);
+  return quality_request<true, true>(ctx, w, listed_rows(samples, n), __func__, 0.0, 0.0, X, Y, k, n_bins, sums_out,
+                                     bin_weight, bin_pos_weight, bin_psum, words_out);
 }
 
 // Diagnostic: rows the streaming pass recomputed in fp64 because their fp32 dot was inside the rounding band (all

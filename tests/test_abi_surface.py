@@ -30,6 +30,28 @@ def test_ctypes_binding_covers_the_header():
     native.lib()                                   # resolves every bound symbol with its argtypes
 
 
+def row_form_entry_points():
+    """dsgd_eval and the range, drawn-sample and id-list forms of the fifteen evaluation families"""
+    evals = ["counts", "sums", "class", "weighted", "metrics", "curve", "weighted_curve", "calibration",
+             "weighted_calibration", "isotonic_calibration", "weighted_isotonic_calibration"]
+    fits = ["calibrate", "calibrate_weighted", "calibrate_isotonic", "calibrate_isotonic_weighted"]
+    return (["dsgd_eval"] + [f"dsgd_eval{form}_{e}" for e in evals for form in ("", "_sampled", "_samples")]
+            + [f"dsgd_{f}{form}" for f in fits for form in ("", "_sampled", "_samples")])
+
+
+def test_row_form_entry_points_refuse_a_null_ctx():
+    """Every evaluation entry point returns DSGD_ERR_INVALID for a NULL ctx before it reads any other argument."""
+    from distributed_sgd_b200 import native
+    names = row_form_entry_points()
+    assert len(names) == len(set(names)) == 46 and set(names) <= set(declared_symbols())
+    lib = native.lib()
+    for n in names:
+        fn = getattr(lib, n)
+        args = [0.0 if t is C.c_double else 0 if t in (C.c_int32, C.c_int64, C.c_uint64) else None
+                for t in fn.argtypes[1:]]
+        assert fn(None, *args) == native.ERR_INVALID, n
+
+
 def test_no_cpu_fallback_without_gpu():
     import torch
     if torch.cuda.is_available():

@@ -1,13 +1,17 @@
-"""Every request entry point of the C ABI: forward, gradient, the nine evaluations, margins, probabilities and the three
-metrics calls.
+"""Every request entry point of the C ABI: forward, gradient, margins, probabilities, and the 46 evaluation entry points --
+dsgd_eval and fifteen families in three row forms each (a range, a device-drawn sample, a list of ids): counts, sums, the
+per-class and weighted tallies, metrics, curves and weighted curves, the Platt and isotonic fits and their quality passes,
+counted and weighted.
 
 * The kernels one call launches (the dsgd_launch_count delta), on an SVM and a logistic context, over fewer and more ids than
   kStreamMinRows (2048, csrc/dsgd_api.cu) where the SVM's streaming pass takes over; with the resident weights and with the
   same weights passed in, which must give the same bits.  The logistic gradient adds to g with fp64 atomics in the order the
   rows arrive, so its gradient agrees to rounding and its loss (a fixed-point sum) to the bit.
-* The error each bad argument gets on its own, and a message that names the entry point that was called.
+* The error each bad argument gets on its own, a message that names the entry point that was called, and no launch: every
+  check before a pass runs before its first kernel.
 * A list of more ids than rows is refused while an async loop is started, even after the loop ended by itself: growing a
   buffer then would wait for every kernel on the device, and a loop that runs until stopped never ends."""
+import ctypes as C
 import os
 import subprocess
 import sys
@@ -22,24 +26,49 @@ LAM = 1e-4
 N_ROWS = 6000
 KEY = 0x9E3779B97F4A7C15
 SIZES = {"small": 300, "large": 4000}          # ids (or rows) of one call: below and above kStreamMinRows
+SIGMOID = (1.5, -0.25)                         # (a, b) of the Platt quality calls
+MAP = (np.array([-2.0, 0.0, 2.0]), np.array([0.2, 0.5, 0.8]))   # a valid map (X, Y) for the isotonic quality calls
+MAX_BINS = 64                                  # DSGD_CALIBRATION_MAX_BINS
 
-# entry point -> one call over the rows that `ids` stands for, with weights w (None: the resident ones)
-REQUESTS = {
-    "forward": lambda c, ids, w: c.forward(ids, w),
-    "gradient": lambda c, ids, w: c.gradient(ids, w, want_loss=True),
-    "eval": lambda c, ids, w: c.eval(7, 7 + ids.size, w),
-    "eval_counts": lambda c, ids, w: c.eval_counts(7, 7 + ids.size, w),
-    "eval_sums": lambda c, ids, w: c.eval_sums(7, 7 + ids.size, w),
-    "eval_sampled_counts": lambda c, ids, w: c.eval_sampled_counts(7, N_ROWS, KEY, 5, 5 + ids.size, w),
-    "eval_sampled_sums": lambda c, ids, w: c.eval_sampled_sums(7, N_ROWS, KEY, 5, 5 + ids.size, w),
-    "eval_samples_counts": lambda c, ids, w: c.eval_samples_counts(ids, w),
-    "eval_samples_sums": lambda c, ids, w: c.eval_samples_sums(ids, w),
-    "margins": lambda c, ids, w: c.margins(ids, w),
-    "probabilities": lambda c, ids, w: c.probabilities(ids, w),
-    "eval_metrics": lambda c, ids, w: c.eval_metrics(7, 7 + ids.size, w),
-    "eval_sampled_metrics": lambda c, ids, w: c.eval_sampled_metrics(7, N_ROWS, KEY, 5, 5 + ids.size, w),
-    "eval_samples_metrics": lambda c, ids, w: c.eval_samples_metrics(ids, w),
-}
+# The evaluation families: dsgd_<family> over a range, and its drawn-sample and id-list forms (dsgd_eval has only the
+# range form), with the arguments each wrapper takes after the rows
+EVAL_FAMILIES = {"eval_counts": (), "eval_sums": (), "eval_class": (), "eval_weighted": (), "eval_metrics": (),
+                 "eval_curve": (), "eval_weighted_curve": (), "calibrate": (), "calibrate_weighted": (),
+                 "eval_calibration": SIGMOID, "eval_weighted_calibration": SIGMOID, "calibrate_isotonic": (),
+                 "eval_isotonic_calibration": MAP, "calibrate_isotonic_weighted": (),
+                 "eval_weighted_isotonic_calibration": MAP}
+
+
+def row_forms(family):
+    """{entry point: its form} of one evaluation family"""
+    if family.startswith("calibrate"):
+        return {family: "range", family + "_sampled": "drawn", family + "_samples": "list"}
+    rest = family[len("eval_"):]
+    return {family: "range", "eval_sampled_" + rest: "drawn", "eval_samples_" + rest: "list"}
+
+
+FORM = {"forward": "list", "gradient": "list", "eval": "range", "margins": "list", "probabilities": "list"}
+FAMILY = {name: name for name in FORM}
+for _f in EVAL_FAMILIES:
+    FORM.update(row_forms(_f))
+    FAMILY.update({name: _f for name in row_forms(_f)})
+
+
+def _request(name):
+    """one call of entry point `name` over the rows that `ids` stands for, with weights w (None: the resident ones)"""
+    extra, form = EVAL_FAMILIES.get(FAMILY[name], ()), FORM[name]
+    if name in ("forward", "margins", "probabilities"):
+        return lambda c, ids, w: getattr(c, name)(ids, w)
+    if name == "gradient":
+        return lambda c, ids, w: c.gradient(ids, w, want_loss=True)
+    if form == "range":
+        return lambda c, ids, w: getattr(c, name)(7, 7 + ids.size, *extra, w=w)
+    if form == "drawn":
+        return lambda c, ids, w: getattr(c, name)(7, N_ROWS, KEY, 5, 5 + ids.size, *extra, w=w)
+    return lambda c, ids, w: getattr(c, name)(ids, *extra, w=w)
+
+
+REQUESTS = {name: _request(name) for name in FORM}
 SVM_ONLY = {"eval_counts", "eval_sampled_counts", "eval_samples_counts"}
 LOGISTIC_ONLY = {"probabilities"}
 
@@ -48,165 +77,249 @@ LAUNCHES = {
     ('svm', 'large', 'forward'): (1, 3),
     ('svm', 'large', 'gradient'): (3, 5),
     ('svm', 'large', 'eval'): (2, 4),
-    ('svm', 'large', 'eval_counts'): (2, 4),
-    ('svm', 'large', 'eval_sums'): (2, 4),
-    ('svm', 'large', 'eval_sampled_counts'): (3, 5),
-    ('svm', 'large', 'eval_sampled_sums'): (3, 5),
-    ('svm', 'large', 'eval_samples_counts'): (2, 4),
-    ('svm', 'large', 'eval_samples_sums'): (2, 4),
     ('svm', 'large', 'margins'): (1, 3),
+    ('svm', 'large', 'eval_counts'): (2, 4),
+    ('svm', 'large', 'eval_sampled_counts'): (3, 5),
+    ('svm', 'large', 'eval_samples_counts'): (2, 4),
+    ('svm', 'large', 'eval_sums'): (2, 4),
+    ('svm', 'large', 'eval_sampled_sums'): (3, 5),
+    ('svm', 'large', 'eval_samples_sums'): (2, 4),
+    ('svm', 'large', 'eval_class'): (2, 4),
+    ('svm', 'large', 'eval_sampled_class'): (3, 5),
+    ('svm', 'large', 'eval_samples_class'): (2, 4),
+    ('svm', 'large', 'eval_weighted'): (2, 4),
+    ('svm', 'large', 'eval_sampled_weighted'): (3, 5),
+    ('svm', 'large', 'eval_samples_weighted'): (2, 4),
     ('svm', 'large', 'eval_metrics'): (2, 4),
     ('svm', 'large', 'eval_sampled_metrics'): (3, 5),
     ('svm', 'large', 'eval_samples_metrics'): (2, 4),
+    ('svm', 'large', 'eval_curve'): (4, 6),
+    ('svm', 'large', 'eval_sampled_curve'): (5, 7),
+    ('svm', 'large', 'eval_samples_curve'): (4, 6),
+    ('svm', 'large', 'eval_weighted_curve'): (4, 6),
+    ('svm', 'large', 'eval_sampled_weighted_curve'): (5, 7),
+    ('svm', 'large', 'eval_samples_weighted_curve'): (4, 6),
+    ('svm', 'large', 'calibrate'): (2, 4),
+    ('svm', 'large', 'calibrate_sampled'): (3, 5),
+    ('svm', 'large', 'calibrate_samples'): (2, 4),
+    ('svm', 'large', 'calibrate_weighted'): (2, 4),
+    ('svm', 'large', 'calibrate_weighted_sampled'): (3, 5),
+    ('svm', 'large', 'calibrate_weighted_samples'): (2, 4),
+    ('svm', 'large', 'eval_calibration'): (2, 4),
+    ('svm', 'large', 'eval_sampled_calibration'): (3, 5),
+    ('svm', 'large', 'eval_samples_calibration'): (2, 4),
+    ('svm', 'large', 'eval_weighted_calibration'): (1, 3),
+    ('svm', 'large', 'eval_sampled_weighted_calibration'): (2, 4),
+    ('svm', 'large', 'eval_samples_weighted_calibration'): (1, 3),
+    ('svm', 'large', 'calibrate_isotonic'): (7, 9),
+    ('svm', 'large', 'calibrate_isotonic_sampled'): (8, 10),
+    ('svm', 'large', 'calibrate_isotonic_samples'): (7, 9),
+    ('svm', 'large', 'eval_isotonic_calibration'): (2, 4),
+    ('svm', 'large', 'eval_sampled_isotonic_calibration'): (3, 5),
+    ('svm', 'large', 'eval_samples_isotonic_calibration'): (2, 4),
+    ('svm', 'large', 'calibrate_isotonic_weighted'): (9, 11),
+    ('svm', 'large', 'calibrate_isotonic_weighted_sampled'): (10, 12),
+    ('svm', 'large', 'calibrate_isotonic_weighted_samples'): (9, 11),
+    ('svm', 'large', 'eval_weighted_isotonic_calibration'): (1, 3),
+    ('svm', 'large', 'eval_sampled_weighted_isotonic_calibration'): (2, 4),
+    ('svm', 'large', 'eval_samples_weighted_isotonic_calibration'): (1, 3),
     ('svm', 'small', 'forward'): (1, 3),
     ('svm', 'small', 'gradient'): (3, 5),
     ('svm', 'small', 'eval'): (2, 4),
-    ('svm', 'small', 'eval_counts'): (2, 4),
-    ('svm', 'small', 'eval_sums'): (2, 4),
-    ('svm', 'small', 'eval_sampled_counts'): (3, 5),
-    ('svm', 'small', 'eval_sampled_sums'): (3, 5),
-    ('svm', 'small', 'eval_samples_counts'): (2, 4),
-    ('svm', 'small', 'eval_samples_sums'): (2, 4),
     ('svm', 'small', 'margins'): (1, 3),
+    ('svm', 'small', 'eval_counts'): (2, 4),
+    ('svm', 'small', 'eval_sampled_counts'): (3, 5),
+    ('svm', 'small', 'eval_samples_counts'): (2, 4),
+    ('svm', 'small', 'eval_sums'): (2, 4),
+    ('svm', 'small', 'eval_sampled_sums'): (3, 5),
+    ('svm', 'small', 'eval_samples_sums'): (2, 4),
+    ('svm', 'small', 'eval_class'): (2, 4),
+    ('svm', 'small', 'eval_sampled_class'): (3, 5),
+    ('svm', 'small', 'eval_samples_class'): (2, 4),
+    ('svm', 'small', 'eval_weighted'): (2, 4),
+    ('svm', 'small', 'eval_sampled_weighted'): (3, 5),
+    ('svm', 'small', 'eval_samples_weighted'): (2, 4),
     ('svm', 'small', 'eval_metrics'): (2, 4),
     ('svm', 'small', 'eval_sampled_metrics'): (3, 5),
     ('svm', 'small', 'eval_samples_metrics'): (2, 4),
+    ('svm', 'small', 'eval_curve'): (4, 6),
+    ('svm', 'small', 'eval_sampled_curve'): (5, 7),
+    ('svm', 'small', 'eval_samples_curve'): (4, 6),
+    ('svm', 'small', 'eval_weighted_curve'): (4, 6),
+    ('svm', 'small', 'eval_sampled_weighted_curve'): (5, 7),
+    ('svm', 'small', 'eval_samples_weighted_curve'): (4, 6),
+    ('svm', 'small', 'calibrate'): (2, 4),
+    ('svm', 'small', 'calibrate_sampled'): (3, 5),
+    ('svm', 'small', 'calibrate_samples'): (2, 4),
+    ('svm', 'small', 'calibrate_weighted'): (2, 4),
+    ('svm', 'small', 'calibrate_weighted_sampled'): (3, 5),
+    ('svm', 'small', 'calibrate_weighted_samples'): (2, 4),
+    ('svm', 'small', 'eval_calibration'): (2, 4),
+    ('svm', 'small', 'eval_sampled_calibration'): (3, 5),
+    ('svm', 'small', 'eval_samples_calibration'): (2, 4),
+    ('svm', 'small', 'eval_weighted_calibration'): (1, 3),
+    ('svm', 'small', 'eval_sampled_weighted_calibration'): (2, 4),
+    ('svm', 'small', 'eval_samples_weighted_calibration'): (1, 3),
+    ('svm', 'small', 'calibrate_isotonic'): (6, 8),
+    ('svm', 'small', 'calibrate_isotonic_sampled'): (7, 9),
+    ('svm', 'small', 'calibrate_isotonic_samples'): (6, 8),
+    ('svm', 'small', 'eval_isotonic_calibration'): (2, 4),
+    ('svm', 'small', 'eval_sampled_isotonic_calibration'): (3, 5),
+    ('svm', 'small', 'eval_samples_isotonic_calibration'): (2, 4),
+    ('svm', 'small', 'calibrate_isotonic_weighted'): (8, 10),
+    ('svm', 'small', 'calibrate_isotonic_weighted_sampled'): (9, 11),
+    ('svm', 'small', 'calibrate_isotonic_weighted_samples'): (8, 10),
+    ('svm', 'small', 'eval_weighted_isotonic_calibration'): (1, 3),
+    ('svm', 'small', 'eval_sampled_weighted_isotonic_calibration'): (2, 4),
+    ('svm', 'small', 'eval_samples_weighted_isotonic_calibration'): (1, 3),
     ('logistic', 'large', 'forward'): (1, 3),
     ('logistic', 'large', 'gradient'): (3, 5),
     ('logistic', 'large', 'eval'): (2, 4),
+    ('logistic', 'large', 'margins'): (1, 3),
+    ('logistic', 'large', 'probabilities'): (1, 3),
     ('logistic', 'large', 'eval_sums'): (2, 4),
     ('logistic', 'large', 'eval_sampled_sums'): (3, 5),
     ('logistic', 'large', 'eval_samples_sums'): (2, 4),
-    ('logistic', 'large', 'margins'): (1, 3),
-    ('logistic', 'large', 'probabilities'): (1, 3),
+    ('logistic', 'large', 'eval_class'): (2, 4),
+    ('logistic', 'large', 'eval_sampled_class'): (3, 5),
+    ('logistic', 'large', 'eval_samples_class'): (2, 4),
+    ('logistic', 'large', 'eval_weighted'): (2, 4),
+    ('logistic', 'large', 'eval_sampled_weighted'): (3, 5),
+    ('logistic', 'large', 'eval_samples_weighted'): (2, 4),
     ('logistic', 'large', 'eval_metrics'): (2, 4),
     ('logistic', 'large', 'eval_sampled_metrics'): (3, 5),
     ('logistic', 'large', 'eval_samples_metrics'): (2, 4),
+    ('logistic', 'large', 'eval_curve'): (4, 6),
+    ('logistic', 'large', 'eval_sampled_curve'): (5, 7),
+    ('logistic', 'large', 'eval_samples_curve'): (4, 6),
+    ('logistic', 'large', 'eval_weighted_curve'): (4, 6),
+    ('logistic', 'large', 'eval_sampled_weighted_curve'): (5, 7),
+    ('logistic', 'large', 'eval_samples_weighted_curve'): (4, 6),
+    ('logistic', 'large', 'calibrate'): (2, 4),
+    ('logistic', 'large', 'calibrate_sampled'): (3, 5),
+    ('logistic', 'large', 'calibrate_samples'): (2, 4),
+    ('logistic', 'large', 'calibrate_weighted'): (2, 4),
+    ('logistic', 'large', 'calibrate_weighted_sampled'): (3, 5),
+    ('logistic', 'large', 'calibrate_weighted_samples'): (2, 4),
+    ('logistic', 'large', 'eval_calibration'): (2, 4),
+    ('logistic', 'large', 'eval_sampled_calibration'): (3, 5),
+    ('logistic', 'large', 'eval_samples_calibration'): (2, 4),
+    ('logistic', 'large', 'eval_weighted_calibration'): (1, 3),
+    ('logistic', 'large', 'eval_sampled_weighted_calibration'): (2, 4),
+    ('logistic', 'large', 'eval_samples_weighted_calibration'): (1, 3),
+    ('logistic', 'large', 'calibrate_isotonic'): (7, 9),
+    ('logistic', 'large', 'calibrate_isotonic_sampled'): (8, 10),
+    ('logistic', 'large', 'calibrate_isotonic_samples'): (7, 9),
+    ('logistic', 'large', 'eval_isotonic_calibration'): (2, 4),
+    ('logistic', 'large', 'eval_sampled_isotonic_calibration'): (3, 5),
+    ('logistic', 'large', 'eval_samples_isotonic_calibration'): (2, 4),
+    ('logistic', 'large', 'calibrate_isotonic_weighted'): (9, 11),
+    ('logistic', 'large', 'calibrate_isotonic_weighted_sampled'): (10, 12),
+    ('logistic', 'large', 'calibrate_isotonic_weighted_samples'): (9, 11),
+    ('logistic', 'large', 'eval_weighted_isotonic_calibration'): (1, 3),
+    ('logistic', 'large', 'eval_sampled_weighted_isotonic_calibration'): (2, 4),
+    ('logistic', 'large', 'eval_samples_weighted_isotonic_calibration'): (1, 3),
     ('logistic', 'small', 'forward'): (1, 3),
     ('logistic', 'small', 'gradient'): (3, 5),
     ('logistic', 'small', 'eval'): (2, 4),
+    ('logistic', 'small', 'margins'): (1, 3),
+    ('logistic', 'small', 'probabilities'): (1, 3),
     ('logistic', 'small', 'eval_sums'): (2, 4),
     ('logistic', 'small', 'eval_sampled_sums'): (3, 5),
     ('logistic', 'small', 'eval_samples_sums'): (2, 4),
-    ('logistic', 'small', 'margins'): (1, 3),
-    ('logistic', 'small', 'probabilities'): (1, 3),
+    ('logistic', 'small', 'eval_class'): (2, 4),
+    ('logistic', 'small', 'eval_sampled_class'): (3, 5),
+    ('logistic', 'small', 'eval_samples_class'): (2, 4),
+    ('logistic', 'small', 'eval_weighted'): (2, 4),
+    ('logistic', 'small', 'eval_sampled_weighted'): (3, 5),
+    ('logistic', 'small', 'eval_samples_weighted'): (2, 4),
     ('logistic', 'small', 'eval_metrics'): (2, 4),
     ('logistic', 'small', 'eval_sampled_metrics'): (3, 5),
     ('logistic', 'small', 'eval_samples_metrics'): (2, 4),
+    ('logistic', 'small', 'eval_curve'): (4, 6),
+    ('logistic', 'small', 'eval_sampled_curve'): (5, 7),
+    ('logistic', 'small', 'eval_samples_curve'): (4, 6),
+    ('logistic', 'small', 'eval_weighted_curve'): (4, 6),
+    ('logistic', 'small', 'eval_sampled_weighted_curve'): (5, 7),
+    ('logistic', 'small', 'eval_samples_weighted_curve'): (4, 6),
+    ('logistic', 'small', 'calibrate'): (2, 4),
+    ('logistic', 'small', 'calibrate_sampled'): (3, 5),
+    ('logistic', 'small', 'calibrate_samples'): (2, 4),
+    ('logistic', 'small', 'calibrate_weighted'): (2, 4),
+    ('logistic', 'small', 'calibrate_weighted_sampled'): (3, 5),
+    ('logistic', 'small', 'calibrate_weighted_samples'): (2, 4),
+    ('logistic', 'small', 'eval_calibration'): (2, 4),
+    ('logistic', 'small', 'eval_sampled_calibration'): (3, 5),
+    ('logistic', 'small', 'eval_samples_calibration'): (2, 4),
+    ('logistic', 'small', 'eval_weighted_calibration'): (1, 3),
+    ('logistic', 'small', 'eval_sampled_weighted_calibration'): (2, 4),
+    ('logistic', 'small', 'eval_samples_weighted_calibration'): (1, 3),
+    ('logistic', 'small', 'calibrate_isotonic'): (6, 8),
+    ('logistic', 'small', 'calibrate_isotonic_sampled'): (7, 9),
+    ('logistic', 'small', 'calibrate_isotonic_samples'): (6, 8),
+    ('logistic', 'small', 'eval_isotonic_calibration'): (2, 4),
+    ('logistic', 'small', 'eval_sampled_isotonic_calibration'): (3, 5),
+    ('logistic', 'small', 'eval_samples_isotonic_calibration'): (2, 4),
+    ('logistic', 'small', 'calibrate_isotonic_weighted'): (8, 10),
+    ('logistic', 'small', 'calibrate_isotonic_weighted_sampled'): (9, 11),
+    ('logistic', 'small', 'calibrate_isotonic_weighted_samples'): (8, 10),
+    ('logistic', 'small', 'eval_weighted_isotonic_calibration'): (1, 3),
+    ('logistic', 'small', 'eval_sampled_weighted_isotonic_calibration'): (2, 4),
+    ('logistic', 'small', 'eval_samples_weighted_isotonic_calibration'): (1, 3),
 }
 
-FORM = {"forward": "list", "gradient": "list", "eval": "range", "eval_counts": "range", "eval_sums": "range",
-        "eval_sampled_counts": "drawn", "eval_sampled_sums": "drawn", "eval_samples_counts": "list",
-        "eval_samples_sums": "list", "margins": "list", "probabilities": "list", "eval_metrics": "range",
-        "eval_sampled_metrics": "drawn", "eval_samples_metrics": "list"}
-GOOD_ROWS = {"list": [1, 2, 3], "range": (10, 20), "drawn": (10, 20, 1, 0, 5)}
+# the refusals of each row form, one bad argument at a time, and the exception each gets
 BAD_ROWS = {
-    "list": [[0, N_ROWS], [-1, 3], [], "NULL"],
-    "range": [(0, N_ROWS + 1), (-1, 5), (9, 8), (4, 4)],
-    "drawn": [(0, N_ROWS + 1, 1, 0, 5), (-1, 10, 1, 0, 5), (5, 5, 1, 0, 0), (10, 20, 1, -1, 3), (10, 20, 1, 0, 11),
-              (10, 20, 1, 4, 12), (10, 20, 1, 3, 3), (10, 20, 1, 5, 4)],
+    "list": [([0, N_ROWS], "DsgdRange"), ([-1, 3], "DsgdRange"), ([], "DsgdEmpty"), ("NULL", "DsgdInvalid")],
+    "range": [((0, N_ROWS + 1), "DsgdRange"), ((-1, 5), "DsgdRange"), ((9, 8), "DsgdRange"), ((4, 4), "DsgdEmpty")],
+    "drawn": [((0, N_ROWS + 1, 1, 0, 5), "DsgdRange"), ((-1, 10, 1, 0, 5), "DsgdRange"), ((5, 5, 1, 0, 0), "DsgdEmpty"),
+              ((10, 20, 1, -1, 3), "DsgdInvalid"), ((10, 20, 1, 0, 11), "DsgdInvalid"), ((10, 20, 1, 4, 12), "DsgdInvalid"),
+              ((10, 20, 1, 3, 3), "DsgdEmpty"), ((10, 20, 1, 5, 4), "DsgdEmpty")],
 }
-# entry points whose first output pointer must not be NULL
-NEEDS_OUT = {"forward", "gradient", "margins", "probabilities", "eval_metrics", "eval_sampled_metrics",
-             "eval_samples_metrics"}
+GOOD_ROWS = {"list": [1, 2, 3], "range": (10, 20), "drawn": (10, 20, 1, 0, 5)}
 
-# (entry point, context, rows (None: GOOD_ROWS of its form), NULL output, expected exception class name or None)
-ERRORS = [
-    ('forward', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('forward', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('forward', 'svm', [], False, None),
-    ('forward', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('forward', 'empty_svm', None, False, 'DsgdState'),
-    ('forward', 'svm', None, True, 'DsgdInvalid'),
-    ('gradient', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('gradient', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('gradient', 'svm', [], False, 'DsgdEmpty'),
-    ('gradient', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('gradient', 'empty_svm', None, False, 'DsgdState'),
-    ('gradient', 'svm', None, True, 'DsgdInvalid'),
-    ('eval', 'svm', (0, 6001), False, 'DsgdRange'),
-    ('eval', 'svm', (-1, 5), False, 'DsgdRange'),
-    ('eval', 'svm', (9, 8), False, 'DsgdRange'),
-    ('eval', 'svm', (4, 4), False, 'DsgdEmpty'),
-    ('eval', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_counts', 'svm', (0, 6001), False, 'DsgdRange'),
-    ('eval_counts', 'svm', (-1, 5), False, 'DsgdRange'),
-    ('eval_counts', 'svm', (9, 8), False, 'DsgdRange'),
-    ('eval_counts', 'svm', (4, 4), False, 'DsgdEmpty'),
-    ('eval_counts', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_counts', 'logistic', None, False, 'DsgdState'),
-    ('eval_sums', 'svm', (0, 6001), False, 'DsgdRange'),
-    ('eval_sums', 'svm', (-1, 5), False, 'DsgdRange'),
-    ('eval_sums', 'svm', (9, 8), False, 'DsgdRange'),
-    ('eval_sums', 'svm', (4, 4), False, 'DsgdEmpty'),
-    ('eval_sums', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_sampled_counts', 'svm', (0, 6001, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_counts', 'svm', (-1, 10, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_counts', 'svm', (5, 5, 1, 0, 0), False, 'DsgdEmpty'),
-    ('eval_sampled_counts', 'svm', (10, 20, 1, -1, 3), False, 'DsgdInvalid'),
-    ('eval_sampled_counts', 'svm', (10, 20, 1, 0, 11), False, 'DsgdInvalid'),
-    ('eval_sampled_counts', 'svm', (10, 20, 1, 4, 12), False, 'DsgdInvalid'),
-    ('eval_sampled_counts', 'svm', (10, 20, 1, 3, 3), False, 'DsgdEmpty'),
-    ('eval_sampled_counts', 'svm', (10, 20, 1, 5, 4), False, 'DsgdEmpty'),
-    ('eval_sampled_counts', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_sampled_counts', 'logistic', None, False, 'DsgdState'),
-    ('eval_sampled_sums', 'svm', (0, 6001, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_sums', 'svm', (-1, 10, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_sums', 'svm', (5, 5, 1, 0, 0), False, 'DsgdEmpty'),
-    ('eval_sampled_sums', 'svm', (10, 20, 1, -1, 3), False, 'DsgdInvalid'),
-    ('eval_sampled_sums', 'svm', (10, 20, 1, 0, 11), False, 'DsgdInvalid'),
-    ('eval_sampled_sums', 'svm', (10, 20, 1, 4, 12), False, 'DsgdInvalid'),
-    ('eval_sampled_sums', 'svm', (10, 20, 1, 3, 3), False, 'DsgdEmpty'),
-    ('eval_sampled_sums', 'svm', (10, 20, 1, 5, 4), False, 'DsgdEmpty'),
-    ('eval_sampled_sums', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_samples_counts', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('eval_samples_counts', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('eval_samples_counts', 'svm', [], False, 'DsgdEmpty'),
-    ('eval_samples_counts', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('eval_samples_counts', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_samples_counts', 'logistic', None, False, 'DsgdState'),
-    ('eval_samples_sums', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('eval_samples_sums', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('eval_samples_sums', 'svm', [], False, 'DsgdEmpty'),
-    ('eval_samples_sums', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('eval_samples_sums', 'empty_svm', None, False, 'DsgdState'),
-    ('margins', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('margins', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('margins', 'svm', [], False, 'DsgdEmpty'),
-    ('margins', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('margins', 'empty_svm', None, False, 'DsgdState'),
-    ('margins', 'svm', None, True, 'DsgdInvalid'),
-    ('probabilities', 'logistic', [0, 6000], False, 'DsgdRange'),
-    ('probabilities', 'logistic', [-1, 3], False, 'DsgdRange'),
-    ('probabilities', 'logistic', [], False, 'DsgdEmpty'),
-    ('probabilities', 'logistic', 'NULL', False, 'DsgdInvalid'),
-    ('probabilities', 'empty_logistic', None, False, 'DsgdState'),
-    ('probabilities', 'logistic', None, True, 'DsgdInvalid'),
-    ('probabilities', 'svm', None, False, 'DsgdState'),
-    ('eval_metrics', 'svm', (0, 6001), False, 'DsgdRange'),
-    ('eval_metrics', 'svm', (-1, 5), False, 'DsgdRange'),
-    ('eval_metrics', 'svm', (9, 8), False, 'DsgdRange'),
-    ('eval_metrics', 'svm', (4, 4), False, 'DsgdEmpty'),
-    ('eval_metrics', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_metrics', 'svm', None, True, 'DsgdInvalid'),
-    ('eval_sampled_metrics', 'svm', (0, 6001, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_metrics', 'svm', (-1, 10, 1, 0, 5), False, 'DsgdRange'),
-    ('eval_sampled_metrics', 'svm', (5, 5, 1, 0, 0), False, 'DsgdEmpty'),
-    ('eval_sampled_metrics', 'svm', (10, 20, 1, -1, 3), False, 'DsgdInvalid'),
-    ('eval_sampled_metrics', 'svm', (10, 20, 1, 0, 11), False, 'DsgdInvalid'),
-    ('eval_sampled_metrics', 'svm', (10, 20, 1, 4, 12), False, 'DsgdInvalid'),
-    ('eval_sampled_metrics', 'svm', (10, 20, 1, 3, 3), False, 'DsgdEmpty'),
-    ('eval_sampled_metrics', 'svm', (10, 20, 1, 5, 4), False, 'DsgdEmpty'),
-    ('eval_sampled_metrics', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_sampled_metrics', 'svm', None, True, 'DsgdInvalid'),
-    ('eval_samples_metrics', 'svm', [0, 6000], False, 'DsgdRange'),
-    ('eval_samples_metrics', 'svm', [-1, 3], False, 'DsgdRange'),
-    ('eval_samples_metrics', 'svm', [], False, 'DsgdEmpty'),
-    ('eval_samples_metrics', 'svm', 'NULL', False, 'DsgdInvalid'),
-    ('eval_samples_metrics', 'empty_svm', None, False, 'DsgdState'),
-    ('eval_samples_metrics', 'svm', None, True, 'DsgdInvalid'),
-    ('gradient', 'no_d', None, False, 'DsgdState'),
-]
+# family -> the arguments of its entry points after the rows: OUT an output that must not be NULL, None an output that may
+# be (and is left) NULL, else the value passed
+OUT = "out"
+TAIL = {
+    "forward": [OUT], "gradient": [OUT, None], "margins": [OUT], "probabilities": [OUT], "eval": [None, None],
+    "eval_counts": [None] * 3, "eval_sums": [None] * 3, "eval_class": [None] * 3, "eval_weighted": [None] * 3,
+    "eval_metrics": [OUT],
+    "eval_curve": [OUT] * 6, "eval_weighted_curve": [OUT] * 6,         # words, AP or sums, points; thr, tp, fp
+    "calibrate": [OUT] * 3, "calibrate_weighted": [OUT] * 4,
+    "eval_calibration": [*SIGMOID, 10] + [OUT] * 5, "eval_weighted_calibration": [*SIGMOID, 10] + [OUT] * 5,
+    "calibrate_isotonic": [OUT] * 6, "calibrate_isotonic_weighted": [OUT] * 7,
+    "eval_isotonic_calibration": [*MAP, 3, 10] + [OUT] * 5, "eval_weighted_isotonic_calibration": [*MAP, 3, 10] + [OUT] * 5,
+}
+# family -> its bad non-pointer arguments, (position after the rows, value): a non-finite a or b, 0 or too many bins
+_SIGMOID_BAD = [(0, float("inf")), (1, float("nan")), (2, 0), (2, MAX_BINS + 1)]
+_MAP_BAD = [(3, 0), (3, MAX_BINS + 1)]
+BAD_VALUES = {"eval_calibration": _SIGMOID_BAD, "eval_weighted_calibration": _SIGMOID_BAD,
+              "eval_isotonic_calibration": _MAP_BAD, "eval_weighted_isotonic_calibration": _MAP_BAD}
+# families whose row weights belong to the sync paths: an async context is refused (dsgd_eval*_weighted takes one)
+ASYNC_REFUSED = {"eval_weighted_curve", "calibrate_weighted", "eval_weighted_calibration", "calibrate_isotonic_weighted",
+                 "eval_weighted_isotonic_calibration"}
+
+
+def error_cases():
+    """(entry point, context, rows (None: GOOD_ROWS of its form), bad argument (None, or (position after the rows,
+    value)), expected exception class name or None): each bad argument on its own."""
+    cases = []
+    for name in REQUESTS:
+        fam, own = FAMILY[name], "logistic" if name in LOGISTIC_ONLY else "svm"
+        cases += [(name, own, rows, None, None if (name, rows) == ("forward", []) else exc)     # forward of no ids: a no-op
+                  for rows, exc in BAD_ROWS[FORM[name]]]
+        cases.append((name, "empty_" + own, None, None, "DsgdState"))
+        cases += [(name, own, None, (i, None), "DsgdInvalid") for i, v in enumerate(TAIL[fam]) if v is OUT]
+        cases += [(name, own, None, bad, "DsgdInvalid") for bad in BAD_VALUES.get(fam, ())]
+        if fam in ASYNC_REFUSED:
+            cases.append((name, "async", None, None, "DsgdState"))
+        if name in SVM_ONLY:
+            cases.append((name, "logistic", None, None, "DsgdState"))
+        if name in LOGISTIC_ONLY:
+            cases.append((name, "svm", None, None, "DsgdState"))
+    cases.append(("gradient", "no_d", None, None, "DsgdState"))
+    return cases
 
 
 def request_ids(n):
@@ -227,7 +340,7 @@ def entry_points(model):
 
 def make_contexts():
     """model -> (ctx with N_ROWS rows, dimSparsity and resident weights w, w); plus the contexts of the error table:
-    `empty_*` without rows, `no_d` with rows and no dimSparsity."""
+    `empty_*` without rows, `no_d` with rows and no dimSparsity, `async` an async-mode context with rows."""
     from distributed_sgd_b200.native import NativeCtx
     from distributed_sgd_b200.utils import synthetic_rcv1
     data = synthetic_rcv1(n_rows=N_ROWS, seed=31)
@@ -243,6 +356,8 @@ def make_contexts():
         out["empty_" + model] = NativeCtx(0, data.dim, LAM, logistic=model == "logistic")
     out["no_d"] = NativeCtx(0, data.dim, LAM)
     out["no_d"].load_csr(data.row_ptr, data.col, data.val, data.label)
+    out["async"] = NativeCtx(0, data.dim, LAM, is_async=True)
+    out["async"].load_csr(data.row_ptr, data.col, data.val, data.label)
     return out, w
 
 
@@ -259,40 +374,28 @@ def observe_launches(ctxs, w, model, size):
     return out
 
 
-def raw_call(ctx, name, rows, null_out):
-    """dsgd_<name> through ctypes with `rows` in its form and no weights: (exception class name or None, message)."""
+def raw_call(ctx, name, rows, bad):
+    """dsgd_<name> through ctypes with `rows` in its form, no weights, and the arguments of TAIL with `bad` in its place:
+    (exception class name or None, message, launch_count() delta)."""
     from distributed_sgd_b200.native import _EXC
     if FORM[name] == "list":
         ids = None if rows == "NULL" else np.asarray(rows, np.int32)
         args = (None if ids is None else ids.ctypes.data, 3 if ids is None else ids.size)
     else:
         args = tuple(rows)
-    preds, grad, m8 = np.zeros(N_ROWS + 8), np.zeros(ctx.dim), np.zeros(8, np.int64)
-    outs = {"forward": (preds.ctypes.data,), "gradient": (grad.ctypes.data, None), "eval": (None, None),
-            "margins": (preds.ctypes.data,), "probabilities": (preds.ctypes.data,)}.get(name)
-    if outs is None:
-        outs = (m8.ctypes.data,) if "metrics" in name else (None, None, None)
-    if null_out:
-        outs = (None,) + outs[1:]
-    rc = getattr(ctx._l, "dsgd_" + name)(ctx._h, None, *args, *outs)
-    return (None if rc == 0 else _EXC[rc].__name__), (ctx._l.dsgd_last_error(ctx._h) or b"").decode()
-
-
-def error_cases():
-    """(entry point, context, rows, NULL output): each bad argument on its own."""
-    cases = []
-    for name in REQUESTS:
-        own = "logistic" if name in LOGISTIC_ONLY else "svm"
-        cases += [(name, own, rows, False) for rows in BAD_ROWS[FORM[name]]]
-        cases.append((name, "empty_" + own, None, False))
-        if name in NEEDS_OUT:
-            cases.append((name, own, None, True))
-        if name in SVM_ONLY:
-            cases.append((name, "logistic", None, False))
-        if name in LOGISTIC_ONLY:
-            cases.append((name, "svm", None, False))
-    cases.append(("gradient", "no_d", None, False))
-    return cases
+    fn, tail, keep = getattr(ctx._l, "dsgd_" + name), list(TAIL[FAMILY[name]]), []
+    if bad is not None:
+        tail[bad[0]] = bad[1]
+    for i, (v, t) in enumerate(zip(tail, fn.argtypes[-len(tail):])):
+        if v is OUT:                    # room for every output: at most one value per row, of 8 bytes
+            keep.append(np.zeros(max(N_ROWS, ctx.dim) + 8))
+            v = keep[-1]
+        if isinstance(v, np.ndarray):
+            tail[i] = v.ctypes.data if t is C.c_void_p else v.ctypes.data_as(t)
+    before = ctx.launch_count()
+    rc = fn(ctx._h, None, *args, *tail)
+    launched = ctx.launch_count() - before
+    return (None if rc == 0 else _EXC[rc].__name__), (ctx._l.dsgd_last_error(ctx._h) or b"").decode(), launched
 
 
 @pytest.fixture(scope="module")
@@ -315,13 +418,15 @@ def test_launches_and_resident_weights(ctxs, model, size):
 
 
 def test_errors(ctxs):
-    assert len(ERRORS) == len(error_cases())
-    for name, kind, rows, null_out, expected in ERRORS:
+    cases = error_cases()
+    assert len(REQUESTS) == 50 and len(cases) == 529
+    for name, kind, rows, bad, expected in cases:
         ctx = ctxs[0][kind]
-        got, msg = raw_call(ctx, name, GOOD_ROWS[FORM[name]] if rows is None else rows, null_out)
-        assert got == expected, (name, kind, rows, null_out, msg)
+        got, msg, launched = raw_call(ctx, name, GOOD_ROWS[FORM[name]] if rows is None else rows, bad)
+        assert got == expected, (name, kind, rows, bad, msg)
         if expected is not None:
-            assert msg.startswith(f"dsgd_{name}: "), (name, kind, rows, null_out, msg)
+            assert msg.startswith(f"dsgd_{name}: "), (name, kind, rows, bad, msg)
+        assert launched == 0, (name, kind, rows, bad, msg, launched)
     w = ctxs[1]                                       # the contexts still answer after the refusals
     assert bits(ctxs[0]["svm"].eval_sums(0, N_ROWS)) == bits(ctxs[0]["svm"].eval_sums(0, N_ROWS, w))
 
@@ -344,10 +449,12 @@ try:
             raise SystemExit("the loop did not end by itself")
         time.sleep(0.01)
     ids = np.zeros(3001, np.int32)
+    extra = {{"eval_samples_calibration": (1.5, -0.25),
+             "eval_samples_isotonic_calibration": (np.array([-2.0, 0.0, 2.0]), np.array([0.2, 0.5, 0.8]))}}
     refused = []
-    for name in ("forward", "gradient", "eval_samples_counts", "eval_samples_sums", "margins", "eval_samples_metrics"):
+    for name in {names!r}:
         try:
-            getattr(ctx, name)(ids)
+            getattr(ctx, name)(ids, *extra.get(name, ()))
         except DsgdState as e:
             refused.append(name if str(e).split("] ", 1)[1].startswith("dsgd_" + name + ": ") else name + "?")
     print("REFUSED", " ".join(refused))
@@ -356,13 +463,16 @@ finally:
 print("AFTER", len(ctx.forward(ids)))
 ctx.close()
 """
+# the list forms an async context takes
+LOOP_LISTS = ("forward", "gradient", "eval_samples_counts", "eval_samples_sums", "margins", "eval_samples_metrics",
+              "eval_samples_class", "eval_samples_weighted", "eval_samples_curve", "calibrate_samples",
+              "eval_samples_calibration", "calibrate_isotonic_samples", "eval_samples_isotonic_calibration")
 
 
 def test_longer_list_than_rows_is_refused_while_a_loop_is_started():
     """The loop ends by itself on max_updates; the context still counts as running until stop_async, so the list requests
     refuse a list their buffers cannot hold, and take it once the loop is stopped.  The subprocess has a timeout."""
-    r = subprocess.run([sys.executable, "-s", "-c", _LOOP.format(root=ROOT)], cwd=ROOT, capture_output=True, text=True,
-                       timeout=180)
+    r = subprocess.run([sys.executable, "-s", "-c", _LOOP.format(root=ROOT, names=LOOP_LISTS)], cwd=ROOT,
+                       capture_output=True, text=True, timeout=180)
     assert r.returncode == 0, r.stdout + r.stderr
-    assert ("REFUSED forward gradient eval_samples_counts eval_samples_sums margins eval_samples_metrics\nAFTER 3001"
-            in r.stdout), r.stdout + r.stderr
+    assert ("REFUSED " + " ".join(LOOP_LISTS) + "\nAFTER 3001") in r.stdout, r.stdout + r.stderr
