@@ -41,6 +41,50 @@ def sampled_key(seed: int, t: int) -> int:
     return z ^ (z >> 31)
 
 
+def bootstrap_key(seed: int) -> int:
+    """The bootstrap key of a Master seeded with `seed` (Master.local_bootstrap with key=None): sampled_key at t = 2^64 - 1,
+    which no sample draw reaches."""
+    return sampled_key(seed, _M64)
+
+
+# the metrics a bootstrap reports, and whether a larger value is better
+BOOTSTRAP_METRICS = {"accuracy": True, "loss": False, "auc": True, "ap": True, "precision": True, "recall": True, "f1": True}
+
+
+def bootstrap_values(words, ap, loss_sum, penalty: float) -> dict:
+    """Each BOOTSTRAP_METRICS value of every replicate from its native.BOOTSTRAP_WORDS words, AP and loss sum, as
+    metrics_dict forms them from the counts (nan where undefined); loss = penalty + loss sum / replicate size."""
+    w = np.asarray(words, dtype=np.int64).reshape(-1, 9).astype(np.float64)
+    tp, fn, pos_none, fp, tn, neg_none, u2, nan, size = w.T
+    P, N = tp + fn + pos_none, fp + tn + neg_none
+
+    def ratio(a, b):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.where(b > 0, a / np.where(b > 0, b, 1.0), np.nan)
+
+    auc = np.where((nan == 0) & (P > 0) & (N > 0), u2 / np.where(P * N > 0, 2.0 * P * N, 1.0), np.nan)
+    return {"accuracy": ratio(tp + tn, P + N), "loss": penalty + ratio(np.asarray(loss_sum, np.float64), size),
+            "auc": auc, "ap": np.asarray(ap, dtype=np.float64), "precision": ratio(tp, tp + fp), "recall": ratio(tp, P),
+            "f1": ratio(2 * tp, 2 * tp + fp + fn + pos_none)}
+
+
+def bootstrap_summary(estimate: float, reps, level: float) -> dict:
+    """One metric's bootstrap: the full-sample estimate, the percentile interval at `level` (numpy.quantile's default method)
+    over the replicates where the metric is defined and how many those are, the standard error (their standard deviation),
+    and the replicates (nan where undefined)."""
+    reps = np.asarray(reps, dtype=np.float64)
+    ok = reps[~np.isnan(reps)]
+    a = (1.0 - level) / 2.0
+    lo, hi = (float(x) for x in np.quantile(ok, [a, 1.0 - a])) if ok.size else (float("nan"), float("nan"))
+    se = float(np.std(ok, ddof=1)) if ok.size > 1 else float("nan")
+    return {"estimate": float(estimate), "lo": lo, "hi": hi, "se": se, "n_defined": int(ok.size), "replicates": reps}
+
+
+def bootstrap_share(n_boot: int, world: int, rank: int):
+    """Replicates [lo, hi) that rank `rank` of `world` computes: contiguous, disjoint, covering [0, n_boot)."""
+    return (n_boot * rank) // world, (n_boot * (rank + 1)) // world
+
+
 def sample_shard(k: int, world: int, rank: int):
     """Positions [lo, hi) of a k-row sample that rank `rank` of `world` evaluates: the shards are disjoint and cover
     [0, k), and their sizes differ by at most one."""
@@ -531,6 +575,98 @@ class Master:
         if ids is None:
             return weighted_curve_dict(self.ctx.eval_sampled_weighted_curve(b, e, key, 0, k, weights, curve=curve), curve)
         return weighted_curve_dict(self.ctx.eval_samples_weighted_curve(ids, weights, curve=curve), curve)
+
+    # ---- bootstrap (extension) -------------------------------------------------------------------------------------------
+    # Poisson-bootstrap intervals of the ranking metrics, accuracy and loss (dsgd_eval_*bootstrap).  Every rank holds every
+    # row; rank r computes the replicates bootstrap_share(n_boot, W, r) and all are gathered in rank order, so every rank
+    # returns the same bits -- a replicate's bits do not depend on which rank computed it.
+    def _bootstrap_raw(self, call: str, rows: tuple, weights, n_boot: int, key: int):
+        """(words, ap, loss_sum) of replicates [0, n_boot) of ctx.<call>(*rows, key, lo, hi, weights), gathered in rank
+        order."""
+        if n_boot <= 0:
+            raise ValueError(f"n_boot: expected a number of replicates > 0, got {n_boot}")
+        lo, hi = bootstrap_share(int(n_boot), self.group.world, self.group.rank)
+        if hi > lo:
+            words, ap, loss = getattr(self.ctx, call)(*rows, key, lo, hi, weights)
+            mine = np.concatenate([np.asarray(words, np.int64).reshape(-1).view(np.float64), np.asarray(ap, np.float64),
+                                   np.asarray(loss, np.float64)])
+        else:
+            mine = np.zeros(0)
+        parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
+        words, ap, loss = [], [], []
+        for p in parts:
+            k = p.size // 11
+            words.append(p[:9 * k].view(np.int64).reshape(k, 9))
+            ap.append(p[9 * k:10 * k])
+            loss.append(p[10 * k:])
+        return np.concatenate(words), np.concatenate(ap), np.concatenate(loss)
+
+    def _bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int]):
+        """(call, rows, estimates) of one bootstrap request: the whole train (or test) rows, or a fresh sample
+        (_draw_sample); the estimates come from the existing curve and *_sums calls over the same rows."""
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        if samples_count is None:
+            call, rows = "eval_bootstrap", (b, e)
+            cw = self.ctx.eval_curve(b, e, weights, curve=False)
+            sums = self.ctx.eval_sums(b, e, weights)
+        else:
+            b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+            if k <= 0:
+                raise DsgdEmpty(ERR_EMPTY, f"sampled bootstrap of {samples_count} rows: the sample is empty")
+            if ids is None:
+                call, rows = "eval_sampled_bootstrap", (b, e, key, 0, k)
+                cw = self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=False)
+                sums = self.ctx.eval_sampled_sums(b, e, key, 0, k, weights)
+            else:
+                call, rows = "eval_samples_bootstrap", (ids,)
+                cw = self.ctx.eval_samples_curve(ids, weights, curve=False)
+                sums = self.ctx.eval_samples_sums(ids, weights)
+        penalty = self._penalty(sums[2], weights, True)
+        words, ap = cw[0], cw[1]
+        n = int(np.sum(np.asarray(words)[[0, 1, 2, 3, 4, 5]]))
+        est = {k: float(v[0]) for k, v in bootstrap_values(np.concatenate([words, [n]]), [ap], [sums[0]], penalty).items()}
+        return call, rows, est, penalty
+
+    def _bootstrap(self, weights, test_data, samples_count, n_boot, key, level) -> dict:
+        call, rows, est, penalty = self._bootstrap_case(weights, test_data, samples_count)
+        key = bootstrap_key(self.seed) if key is None else int(key)
+        reps = bootstrap_values(*self._bootstrap_raw(call, rows, weights, n_boot, key), penalty)
+        return {m: bootstrap_summary(est[m], reps[m], level) for m in BOOTSTRAP_METRICS}
+
+    def local_bootstrap(self, weights=None, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
+                        level: float = 0.95) -> dict:
+        """Poisson-bootstrap intervals over the test (or train) rows: for each of accuracy, loss (penalty + S / n, the
+        unweighted loss of the *_sums calls), auc, ap, precision, recall and f1 (BOOTSTRAP_METRICS) a dict of the full-sample
+        estimate, the percentile interval [lo, hi] at `level` over the replicates where the metric is defined, n_defined,
+        the standard error se and the raw replicates.  key None: bootstrap_key(seed)."""
+        return self._bootstrap(weights, test_data, None, n_boot, key, level)
+
+    def local_sampled_bootstrap(self, weights, samples_count: int, test_data: bool = True, n_boot: int = 1000,
+                                key: Optional[int] = None, level: float = 0.95) -> dict:
+        """local_bootstrap over a fresh sample of min(samples_count, n) rows (_draw_sample).  An empty sample raises
+        DsgdEmpty."""
+        return self._bootstrap(weights, test_data, samples_count, n_boot, key, level)
+
+    def compare_bootstrap(self, weights_a, weights_b, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
+                          level: float = 0.95) -> dict:
+        """Paired comparison of two weight vectors over the same rows: both are scored with the same bootstrap key, so
+        replicate b resamples the same rows for both.  Per metric: the difference b - a of the estimates, its percentile
+        interval, standard error and defined-replicate count (replicates where the metric is defined for both), and
+        p_better, the share of those replicates in which b is better (higher, or lower for the loss)."""
+        key = bootstrap_key(self.seed) if key is None else int(key)
+        out = {}
+        sides = []
+        for w in (weights_a, weights_b):
+            call, rows, est, penalty = self._bootstrap_case(w, test_data, None)
+            sides.append((est, bootstrap_values(*self._bootstrap_raw(call, rows, w, n_boot, key), penalty)))
+        (ea, ra), (eb, rb) = sides
+        for m, higher in BOOTSTRAP_METRICS.items():
+            d = rb[m] - ra[m]
+            s = bootstrap_summary(eb[m] - ea[m], d, level)
+            ok = d[~np.isnan(d)]
+            s["p_better"] = float(np.mean(ok > 0 if higher else ok < 0)) if ok.size else float("nan")
+            out[m] = s
+        return out
 
     # ---- calibration (extension) -----------------------------------------------------------------------------------------
     # Like the ranking metrics, these are not sharded: rows are replicated on every rank and every rank fits or evaluates

@@ -26,6 +26,7 @@
 #include "dsgd_metrics.cuh"
 #include "dsgd_calibrate.cuh"
 #include "dsgd_isotonic.cuh"
+#include "dsgd_bootstrap.cuh"
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
@@ -186,6 +187,13 @@ struct dsgd_ctx {
   dev_buf<double> i_out, i_map;
   dev_buf<long long> i_blk;
   dev_buf<unsigned long long> i_ctl;
+  // a bootstrap pass (dsgd_eval_*bootstrap, dsgd_bootstrap.cuh; keys in m_keys / m_alt): each position's tag and its sort
+  // alternate, the group starts and (every model but the SVM) the losses by position and in sorted order, and a chunk's
+  // replicate words
+  dev_buf<uint32_t> b_tag, b_tagt;
+  dev_buf<int> b_gs;
+  dev_buf<double> b_loss, b_eloss;
+  dev_buf<unsigned long long> b_out;
 
   ncclComm_t comm = nullptr;
 
@@ -1555,6 +1563,110 @@ extern "C" int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t
 
 extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out) {
   return metrics_request(ctx, w, listed_rows(samples, n), __func__, out);
+}
+
+// ---- bootstrap (dsgd_bootstrap.cuh; DESIGN.md §4.19) --------------------------------------------------------------------
+
+constexpr int64_t kBootChunk = 4096;   // replicates per k_boot_rep launch: its output block stays small whatever n_boot is
+
+// One bootstrap pass over `rows`: positions scored, sorted and arranged once, then replicates [b_begin, b_end) in chunks.
+// Per replicate b (index b - b_begin of the outputs): the DSGD_BOOTSTRAP_WORDS words, AP = S / P under the curve pass's NaN
+// rule, and the loss sum.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
+static int bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, uint64_t bkey, int64_t b_begin, int64_t b_end,
+                          int64_t *words, double *ap, double *loss) {
+  const int64_t n = rows.n;
+  const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
+  int rc = request_weights(ctx, w, &wd, &cd, &nd);
+  if (rc) return rc;
+  const bool kl = model_of(ctx) != kSvm;
+  if ((rc = ctx->m_keys.grow(ctx, n, 1024)) || (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->b_tag.grow(ctx, n, 1024)) ||
+      (rc = ctx->b_tagt.grow(ctx, n, 1024)) || (rc = ctx->b_gs.grow(ctx, n, 1024)) ||
+      (kl && ((rc = ctx->b_loss.grow(ctx, n, 1024)) || (rc = ctx->b_eloss.grow(ctx, n, 1024)))) ||
+      (rc = ctx->b_out.grow(ctx, kBootChunk * kBootOutWords, kBootChunk * kBootOutWords)))
+    return rc;
+  const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 positions per warp
+  rc = with_model<kUnweighted>(ctx, [&](auto m, auto, auto ic) {
+    k_boot_score<m, ic><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                      ctx->m_keys, ctx->b_tag, ctx->b_loss, wd + ctx->dim);
+    LAUNCHED();
+    return DSGD_OK;
+  });
+  if (rc) return rc;
+  CU(cudaGetLastError());
+  cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
+  cub::DoubleBuffer<uint32_t> tb(ctx->b_tag.p, ctx->b_tagt.p);
+  size_t tmp = 0;
+  CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kb, tb, (int)n, 0, 64, ctx->stream));
+  if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+  CU(cub::DeviceRadixSort::SortPairs(ctx->m_tmp.p, tmp, kb, tb, (int)n, 0, 64, ctx->stream));
+  const int agrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
+  if (kl)
+    k_boot_arrange<true><<<agrid, 256, 0, ctx->stream>>>(kb.Current(), tb.Current(), n, ctx->b_loss, ctx->b_gs, ctx->b_eloss);
+  else
+    k_boot_arrange<false><<<agrid, 256, 0, ctx->stream>>>(kb.Current(), tb.Current(), n, nullptr, ctx->b_gs, nullptr);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  std::vector<unsigned long long> h((size_t)(kBootChunk * kBootOutWords));
+  for (int64_t b0 = b_begin; b0 < b_end; b0 += kBootChunk) {
+    const int64_t k = std::min(kBootChunk, b_end - b0);
+    if (kl)
+      k_boot_rep<true><<<(int)k, kBootThreads, 0, ctx->stream>>>(tb.Current(), ctx->b_gs, ctx->b_eloss, n, bkey, b0, ctx->b_out);
+    else
+      k_boot_rep<false><<<(int)k, kBootThreads, 0, ctx->stream>>>(tb.Current(), ctx->b_gs, nullptr, n, bkey, b0, ctx->b_out);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(h.data(), ctx->b_out, sizeof(unsigned long long) * (size_t)(k * kBootOutWords), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (int64_t r = 0; r < k; ++r) {
+      const unsigned long long *o = &h[(size_t)(r * kBootOutWords)];
+      int64_t *wr = words + (b0 - b_begin + r) * DSGD_BOOTSTRAP_WORDS;
+      for (int q = 0; q < DSGD_BOOTSTRAP_WORDS; ++q) wr[q] = (int64_t)o[q];
+      const int64_t P = wr[kMetTp] + wr[kMetFn] + wr[kMetPosNone];
+      double S, L;
+      memcpy(&S, &o[kBootS], sizeof S);
+      memcpy(&L, &o[kBootLoss], sizeof L);
+      ap[b0 - b_begin + r] = (wr[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
+      loss[b0 - b_begin + r] = L;
+    }
+  }
+  return DSGD_OK;
+}
+
+// dsgd_eval*_bootstrap: the outputs and the replicate range, an async ctx while its loop runs (the pass grows its own
+// buffers), then the request's size -- all before anything is launched, the sampled form's draw included
+static int bootstrap_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, uint64_t bkey,
+                             int64_t b_begin, int64_t b_end, int64_t *words, double *ap, double *loss) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(words && ap && loss, DSGD_ERR_INVALID, "%s: words_out, ap_out or loss_out is NULL", fn);
+  NEED(b_begin >= 0, DSGD_ERR_INVALID, "%s: replicates [%lld,%lld) start below 0", fn, (long long)b_begin, (long long)b_end);
+  NEED(b_end > b_begin, DSGD_ERR_EMPTY, "%s: no replicates [%lld,%lld)", fn, (long long)b_begin, (long long)b_end);
+  NEED(!ctx->a_running, DSGD_ERR_STATE, "%s: the async loop runs (the pass's buffers cannot grow until it is stopped)", fn);
+  const int64_t n = req.form == row_request::kRange ? req.row_end - req.row_begin
+                    : req.form == row_request::kDrawn ? req.pos_end - req.pos_begin : req.n;
+  NEED(n <= kBootMaxRows, DSGD_ERR_INVALID, "%s: %lld rows; a bootstrap takes at most 2^26", fn, (long long)n);
+  row_set rows;
+  int rc = resolve_rows(ctx, req, fn, &rows);
+  return rc ? rc : bootstrap_pass(ctx, w, rows, bkey, b_begin, b_end, words, ap, loss);
+}
+
+extern "C" int dsgd_eval_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t bkey,
+                                   int64_t b_begin, int64_t b_end, int64_t *words_out, double *ap_out, double *loss_out) {
+  return bootstrap_request(ctx, w, range_rows(row_begin, row_end), __func__, bkey, b_begin, b_end, words_out, ap_out,
+                           loss_out);
+}
+
+extern "C" int dsgd_eval_sampled_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                           int64_t pos_begin, int64_t pos_end, uint64_t bkey, int64_t b_begin, int64_t b_end,
+                                           int64_t *words_out, double *ap_out, double *loss_out) {
+  return bootstrap_request(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, bkey, b_begin, b_end,
+                           words_out, ap_out, loss_out);
+}
+
+extern "C" int dsgd_eval_samples_bootstrap(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, uint64_t bkey,
+                                           int64_t b_begin, int64_t b_end, int64_t *words_out, double *ap_out,
+                                           double *loss_out) {
+  return bootstrap_request(ctx, w, listed_rows(samples, n), __func__, bkey, b_begin, b_end, words_out, ap_out, loss_out);
 }
 
 // ---- calibration (dsgd_calibrate.cuh; DESIGN.md §4.11) ---------------------------------------------------------------

@@ -1,0 +1,223 @@
+// dsgd_bootstrap.cuh -- sm_90a kernels of the bootstrap calls (dsgd_eval_*bootstrap; DESIGN.md §4.19).
+//
+// Replicate b of a request of n rows is the unweighted evaluation of its expanded list: position i repeated m_i(b) times,
+// m_i(b) the Poisson(1) draw of dsgd_bootstrap.h.  Scoring and sorting do not depend on b, so a bootstrap pass does them once:
+//   1. k_boot_score: the score of every position as k_metrics_score forms it (row_score: the same fold, the same intercept),
+//      its sort key ~score_key(s) (s = -(x . w): highest score first; a NaN score takes the largest key, ~0, and sorts last)
+//      and a 32-bit tag: the position, its confusion word (kMetTp .. kMetNegNone), its SVM hinge 1 - y p in {0, 1, 2} and
+//      a NaN bit.  Every model but the SVM also keeps the row's loss L (row_loss), by position.
+//   2. cub::DeviceRadixSort::SortPairs of (key, tag) over all n positions.
+//   3. k_boot_arrange: in sorted order, the last element of every tie group of non-NaN scores records the index of its
+//      group's first element (-1 elsewhere), and L is gathered into sorted order.
+//   4. k_boot_rep: one CTA per replicate, tile by tile over the sorted elements.  Each element draws its m from its position;
+//      a block scan carries the (positive, negative) mass, packed as P << 32 | N, above and through every element.  At the end
+//      of a group, with A the mass above it and E the mass through it (P_g = E.P - A.P, N_g = E.N - A.N):
+//        U2 += N_g (2 A.P + P_g)               -- 2 per (positive above, negative) pair, 1 per tied pair
+//        S  += P_g R(E.P / (E.P + E.N))        -- when P_g > 0: the precision at the group's score, once per positive copy
+//      and every element adds m to its confusion word, its NaN word and the replicate's size, and m copies of its loss.
+// Every sum is an integer or an order-free fixed-point sum (dsgd_fixed.cuh): a replicate has the same bits on any grid, and
+// they are those of dsgd_eval_samples_metrics / _curve / _sums over the expanded list (tests/test_gpu_bootstrap.py).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <cub/block/block_scan.cuh>
+
+#include "dsgd_bootstrap.h"
+#include "dsgd_kernels.cuh"
+#include "dsgd_metrics.cuh"
+
+namespace dsgd {
+
+constexpr int64_t kBootMaxRows = 1ll << 26;   // with m <= 20: sum m < 2^31 and U2 < 2^61, every word an exact int64
+constexpr uint32_t kBootPosMask = (1u << 26) - 1u;
+constexpr int kBootThreads = 256, kBootItems = 4, kBootTile = kBootThreads * kBootItems;
+// a replicate's output: the DSGD_BOOTSTRAP_WORDS words, then S (the AP sum) and the loss sum as the bits of doubles
+enum BootWord : int { kBootSize = 8, kBootS = 9, kBootLoss = 10, kBootOutWords = 11 };
+static_assert(kMetTp == 0 && kMetNegNone == 5 && kMetU2 == 6 && kMetNan == 7, "a tag's confusion word is a word index");
+
+// ---------------------------------------------------------------------------------------------------
+// k_boot_score: a warp takes 32 consecutive positions at a time, as k_metrics_score does; every position's key and tag go to
+// its own slot, and (kModel != kSvm) loss[i] = L(y (x . w)), the per-row loss of k_rows.
+// ---------------------------------------------------------------------------------------------------
+template <int kModel, bool kIcpt>
+__global__ void __launch_bounds__(256) k_boot_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                    const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
+                                                    int64_t row_begin, int64_t n, const double *__restrict__ w,
+                                                    unsigned long long *__restrict__ keys, uint32_t *__restrict__ tags,
+                                                    double *__restrict__ loss, const double *__restrict__ icpt) {
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i = g + lane;
+    const bool mine = i < n;
+    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    double dot_own = 0.0;
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
+      if (lane == j) dot_own = dot;
+    }
+    if (!mine) continue;
+    const int y = (int)label[r_own];
+    const bool pos = y > 0, nan = isnan(dot_own);
+    const int p = pred_of(dot_own);
+    const uint32_t word = pos ? (p == 1 ? kMetTp : p == -1 ? kMetFn : kMetPosNone) : (p == 1 ? kMetFp : p == -1 ? kMetTn : kMetNegNone);
+    keys[i] = nan ? ~0ull : ~score_key(-dot_own);
+    tags[i] = (uint32_t)i | word << 26 | (uint32_t)(1 - y * p) << 29 | (uint32_t)nan << 31;
+    if constexpr (kModel != kSvm) loss[i] = row_loss<kModel>((double)y * dot_own);
+  }
+}
+
+// k_boot_arrange: gs[j] = the first index of element j's tie group when j ends a group of non-NaN scores, else -1; kLoss:
+// eloss[j] = loss of element j's position
+template <bool kLoss>
+__global__ void __launch_bounds__(256) k_boot_arrange(const unsigned long long *__restrict__ keys,
+                                                      const uint32_t *__restrict__ tags, int64_t n,
+                                                      const double *__restrict__ loss, int *__restrict__ gs,
+                                                      double *__restrict__ eloss) {
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = keys[j];
+    const bool end = key != ~0ull && (j + 1 == n || keys[j + 1] != key);
+    gs[j] = end ? (int)key_lower_bound(keys, j + 1, key) : -1;
+    if constexpr (kLoss) eloss[j] = loss[tags[j] & kBootPosMask];
+  }
+}
+
+// lim += m R(v) (v in [0, 2^52), not NaN), carried: limbs 0..3 of R(v) are below 2^40 + 1, so each product is split at bit 40
+// into its limb and the next.  Limb 4, R(v)'s integer part, is added whole: callers keep m v below 2^63 (v <= 1 for S, m <= 20
+// for a loss).
+__device__ __forceinline__ void acc_add_times(unsigned long long (&lim)[kLossLimbs], double v, unsigned long long m) {
+  acc_cut(v, [&](int k, double limb) {
+    const unsigned long long q = (unsigned long long)(long long)limb, lo = q * m;
+    if (k == kLossLimbs - 2) {
+      lim[k] += lo;
+      return;
+    }
+    lim[k] += lo & kLimbMask;
+    lim[k + 1] += (lo >> 40) | (__umul64hi(q, m) << 24);
+  });
+  acc_carry(lim);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_boot_rep: replicate b0 + blockIdx.x over the n sorted elements; out[kBootOutWords * blockIdx.x ..] its words.  Thread t
+// takes elements 4 t .. 4 t + 3 of each 1024-element tile; incl[] holds the tile's inclusive masses, and a_open the mass
+// through the last group end of the tiles before, which is the mass above any group that began before this tile.
+// ---------------------------------------------------------------------------------------------------
+template <bool kLoss>
+__global__ void __launch_bounds__(kBootThreads) k_boot_rep(const uint32_t *__restrict__ tags, const int *__restrict__ gs,
+                                                           const double *__restrict__ eloss, int64_t n, uint64_t bkey,
+                                                           int64_t b0, unsigned long long *__restrict__ out) {
+  using Scan = cub::BlockScan<unsigned long long, kBootThreads>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+  __shared__ unsigned long long incl[kBootTile];
+  __shared__ long long last_end;
+  __shared__ unsigned long long red[kBootThreads / 32][24];
+  const uint64_t zb = dsgd_boot_stream(bkey, (uint64_t)(b0 + blockIdx.x));
+  const unsigned long long lo32 = 0xffffffffull;
+  unsigned c[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the six confusion words, then NaN and size
+  unsigned long long u2 = 0, hinge = 0, carry = 0, a_open = 0;
+  unsigned long long lim_s[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_l[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_l = 0;
+  for (int64_t t0 = 0; t0 < n; t0 += kBootTile) {
+    const int base = threadIdx.x * kBootItems;
+    uint32_t tag[kBootItems];
+    int g[kBootItems];
+    unsigned m[kBootItems];
+    unsigned long long pn[kBootItems], sum = 0;
+#pragma unroll
+    for (int k = 0; k < kBootItems; ++k) {
+      const int64_t j = t0 + base + k;
+      tag[k] = j < n ? tags[j] : 0u;
+      g[k] = j < n ? gs[j] : -1;
+      m[k] = j < n ? (unsigned)dsgd_boot_m(zb, tag[k] & kBootPosMask) : 0u;
+      pn[k] = ((tag[k] >> 26) & 7u) < 3u ? (unsigned long long)m[k] << 32 : (unsigned long long)m[k];
+      sum += pn[k];
+    }
+    if (threadIdx.x == 0) last_end = -1;
+    unsigned long long excl, total;
+    Scan(scan_tmp).ExclusiveSum(sum, excl, total);
+    unsigned long long run = carry + excl;
+#pragma unroll
+    for (int k = 0; k < kBootItems; ++k) {
+      run += pn[k];
+      incl[base + k] = run;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kBootItems; ++k) {
+      if (m[k]) {
+        c[(tag[k] >> 26) & 7u] += m[k];
+        c[6] += (tag[k] >> 31) * m[k];
+        c[7] += m[k];
+        if constexpr (kLoss) {
+          const double l = eloss[t0 + base + k];
+          if (!(l >= 0.0 && l < 4503599627370496.0)) ovf_l += m[k];   // NaN, inf, >= 2^52: the sum reads NaN
+          else acc_add_times(lim_l, l, m[k]);
+        } else {
+          hinge += (unsigned long long)((tag[k] >> 29) & 3u) * m[k];
+        }
+      }
+      if (g[k] >= 0) {
+        const unsigned long long E = incl[base + k];
+        const unsigned long long A = g[k] > t0 ? incl[g[k] - 1 - t0] : a_open;
+        const unsigned long long Pa = A >> 32, Pt = E >> 32, Nt = E & lo32;
+        const unsigned long long Pg = Pt - Pa, Ng = Nt - (A & lo32);
+        u2 += Ng * (2 * Pa + Pg);
+        if (Pg) acc_add_times(lim_s, (double)Pt / (double)(Pt + Nt), Pg);
+        atomicMax(&last_end, (long long)(t0 + base + k));
+      }
+    }
+    __syncthreads();
+    if (last_end >= 0) a_open = incl[last_end - t0];
+    carry += total;
+    __syncthreads();
+  }
+  // block sums: 8 counts, U2, the hinge sum, S's and the loss's limbs and the loss's overflow count
+  unsigned long long v[24];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) v[k] = c[k];
+  v[8] = u2;
+  v[9] = hinge;
+#pragma unroll
+  for (int k = 0; k < kLossLimbs; ++k) {
+    v[10 + k] = lim_s[k];
+    v[16 + k] = lim_l[k];
+  }
+  v[22] = ovf_l;
+  v[23] = 0;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 23; ++k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if (lane == 0) red[wid][k] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long t[24];
+    for (int k = 0; k < 23; ++k) {
+      t[k] = 0;
+      for (int q = 0; q < kBootThreads / 32; ++q) t[k] += red[q][k];
+    }
+    unsigned long long *o = out + (int64_t)kBootOutWords * blockIdx.x;
+    for (int k = 0; k < 6; ++k) o[k] = t[k];
+    o[kMetU2] = t[8];
+    o[kMetNan] = t[6];
+    o[kBootSize] = t[7];
+    unsigned long long s[kLossAccWords], l[kLossAccWords];
+    for (int k = 0; k < kLossLimbs; ++k) {
+      s[k] = t[10 + k];
+      l[k] = t[16 + k];
+    }
+    s[kLossLimbs] = 0;
+    l[kLossLimbs] = t[22];
+    o[kBootS] = (unsigned long long)__double_as_longlong(acc_value(s));
+    o[kBootLoss] = (unsigned long long)__double_as_longlong(kLoss ? acc_value(l) : (double)t[9]);
+  }
+}
+
+}  // namespace dsgd

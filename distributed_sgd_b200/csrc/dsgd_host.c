@@ -389,3 +389,7 @@ int64_t dsgd_draw_epoch(uint64_t seed, int64_t epoch, int32_t n_groups, const in
 uint32_t dsgd_feistel_pos(uint32_t x, uint64_t n, uint64_t key) {
   return dsgd_feistel(x, dsgd_feistel_half_bits(n), key, (uint32_t)n);
 }
+
+/* ---- the bootstrap calls' Poisson(1) draw (dsgd_bootstrap.h), exported for the tests ---------------------------------- */
+#include "dsgd_bootstrap.h"
+int dsgd_bootstrap_draw(uint64_t key, uint64_t b, uint64_t i) { return dsgd_boot_m(dsgd_boot_stream(key, b), i); }

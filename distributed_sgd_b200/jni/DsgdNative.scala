@@ -70,6 +70,16 @@ object DsgdNative {
                                thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
   @native def evalSamplesCurve(ctx: Long, w: Array[Double], samples: Array[Int], metrics: Array[Long], ap: Array[Double],
                                nPoints: Array[Long], thr: Array[Double], tp: Array[Long], fp: Array[Long]): Int
+  // Poisson bootstrap, either model: replicates [bBegin, bEnd) with key bKey; words(9 j until 9 j + 9) = the metrics words and
+  // the size of replicate bBegin + j, ap(j) its average precision, loss(j) its loss sum.  Each array holds at least the
+  // replicates' entries.
+  @native def evalBootstrap(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, bKey: Long, bBegin: Long, bEnd: Long,
+                            words: Array[Long], ap: Array[Double], loss: Array[Double]): Int
+  @native def evalSampledBootstrap(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long,
+                                   posEnd: Long, bKey: Long, bBegin: Long, bEnd: Long, words: Array[Long],
+                                   ap: Array[Double], loss: Array[Double]): Int
+  @native def evalSamplesBootstrap(ctx: Long, w: Array[Double], samples: Array[Int], bKey: Long, bBegin: Long, bEnd: Long,
+                                   words: Array[Long], ap: Array[Double], loss: Array[Double]): Int
   // calibration (Platt scaling): ab(0..1) = (A, B) of P(y = +1 | x) = 1 / (1 + exp(A x.w + B)), objective(0) = F(A, B),
   // info(0..4) = iterations, status (0 converged, 1 iteration limit, 2 line search failed, 3 non-finite sum), rows used, NaN
   // rows, points evaluated.  Quality at (a, b): sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum(0 until

@@ -321,6 +321,66 @@ FN(evalSamplesCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArr
   return rc;
 }
 
+/* Poisson bootstrap: replicates [bBegin, bEnd) with key bKey; words(9 j .. 9 j + 8) = the DSGD_BOOTSTRAP_WORDS words of
+ * replicate bBegin + j, ap(j) its average precision, loss(j) its loss sum.  An output shorter than the replicates is
+ * DSGD_ERR_INVALID. */
+typedef struct { buf_t m, a, l; } boot_bufs;
+static boot_bufs boot_out(JNIEnv *env, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
+  boot_bufs c = {out_Long(env, words), out_Double(env, ap), out_Double(env, loss)};
+  return c;
+}
+static int boot_bad(const boot_bufs *c) { return c->m.bad | c->a.bad | c->l.bad; }
+static int boot_short(const boot_bufs *c, jlong bBegin, jlong bEnd) {
+  const jlong k = bEnd > bBegin ? bEnd - bBegin : 0;
+  return c->m.n < k * DSGD_BOOTSTRAP_WORDS || c->a.n < k || c->l.n < k;
+}
+static void boot_back(JNIEnv *env, jlongArray words, jdoubleArray ap, jdoubleArray loss, boot_bufs *c, int rc) {
+  back_Long(env, words, c->m, rc);
+  back_Double(env, ap, c->a, rc);
+  back_Double(env, loss, c->l, rc);
+}
+FN(evalBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong bKey, jlong bBegin,
+                  jlong bEnd, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w);
+  boot_bufs c = boot_out(env, words, ap, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | boot_bad(&c)))
+    rc = boot_short(&c, bBegin, bEnd) ? DSGD_ERR_INVALID
+                                      : dsgd_eval_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)bKey, bBegin, bEnd,
+                                                            (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
+  boot_back(env, words, ap, loss, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                         jlong posBegin, jlong posEnd, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
+                         jdoubleArray ap, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w);
+  boot_bufs c = boot_out(env, words, ap, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | boot_bad(&c)))
+    rc = boot_short(&c, bBegin, bEnd)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (uint64_t)bKey,
+                                           bBegin, bEnd, (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
+  boot_back(env, words, ap, loss, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlong bKey, jlong bBegin,
+                         jlong bEnd, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  boot_bufs c = boot_out(env, words, ap, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | boot_bad(&c)))
+    rc = boot_short(&c, bBegin, bEnd) ? DSGD_ERR_INVALID
+                                      : dsgd_eval_samples_bootstrap(CTX(h), bw.p, bs.p, bs.n, (uint64_t)bKey, bBegin, bEnd,
+                                                                    (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
+  boot_back(env, words, ap, loss, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+
 /* calibration: ab(0..1) = (A, B), objective(0) = F(A, B), info(0..4) = the DSGD_CALIBRATION_INFO_WORDS words; probabilities:
  * out(i) = sigmoid(-(a x_i . w + b)); quality: sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum at least nBins
  * long, words(0..1) = rows used and left out.  A shorter array is DSGD_ERR_INVALID. */

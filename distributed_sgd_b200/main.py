@@ -141,6 +141,14 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                 f"test Brier {q['brier']:.6f}, log loss {q['log_loss']:.6f}, ECE {q['ece']:.6f}"
                 + (f"; identity link: Brier {q0['brier']:.6f}, log loss {q0['log_loss']:.6f}, ECE {q0['ece']:.6f}"
                    if cfg.model == "logistic" else ""))
+    if cfg.bootstrap > 0:
+        # Poisson-bootstrap 95 % intervals of the final test metrics (the replicates themselves are not reported)
+        bs = master.local_bootstrap(w1, test_data=True, n_boot=cfg.bootstrap)
+        report["test_bootstrap"] = {m: {k: v for k, v in r.items() if k != "replicates"} for m, r in bs.items()}
+        report["test_bootstrap"]["replicates"] = cfg.bootstrap
+        if rank == 0:
+            log(f"bootstrap ({cfg.bootstrap} replicates, 95 %): " + ", ".join(
+                f"{m} {bs[m]['estimate']:.4f} [{bs[m]['lo']:.4f}, {bs[m]['hi']:.4f}]" for m in ("auc", "ap", "accuracy", "loss")))
     if inspect:
         inspect("done", (master, state))
     slave.stop()

@@ -40,6 +40,8 @@ CALIBRATION_WSUMS = 3        # DSGD_CALIBRATION_WSUMS: W+, W-, the NaN rows' wei
 WCALIBRATION_SUMS = 4        # DSGD_WCALIBRATION_SUMS: weighted Brier and log-loss sums, weight used, infinite-term weight
 ISOTONIC_INFO_WORDS = 5      # DSGD_ISOTONIC_INFO_WORDS: blocks, points, rows used, NaN rows, distinct scores
 ISOTONIC_EVAL_WORDS = 3      # DSGD_ISOTONIC_EVAL_WORDS: rows used, rows left out, rows with an infinite log-loss term
+BOOTSTRAP_WORDS = 9          # DSGD_BOOTSTRAP_WORDS: the METRICS_WORDS of a replicate, then its size (sum of m_i)
+BOOTSTRAP_MAX_ROWS = 1 << 26  # the rows of one bootstrap request
 
 
 class NativeLibraryMissing(ImportError):
@@ -153,6 +155,9 @@ ABI = {
     "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
+    "dsgd_eval_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_eval_sampled_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_eval_samples_bootstrap": [_vp, _vp, _vp, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
     "dsgd_eval_weighted_curve": [_vp, _vp, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_weighted_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_weighted_curve": [_vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
@@ -246,6 +251,8 @@ def host_lib():
         h.dsgd_draw_epoch.argtypes = [C.c_uint64, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _i64]
         h.dsgd_feistel_pos.restype = C.c_uint32
         h.dsgd_feistel_pos.argtypes = [C.c_uint32, C.c_uint64, C.c_uint64]
+        h.dsgd_bootstrap_draw.restype = C.c_int
+        h.dsgd_bootstrap_draw.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64]
         _host = h
     return _host
 
@@ -793,6 +800,35 @@ class NativeCtx:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_curve)."""
         samples = _arr(samples, np.int32)
         return self._curve("eval_samples_curve", w, (_ptr(samples), samples.size), samples.size, curve)
+
+    # -- bootstrap --
+    def _bootstrap(self, fn: str, w, rows: tuple, bkey: int, b_begin: int, b_end: int):
+        """dsgd_<fn>: (words[b_end - b_begin, BOOTSTRAP_WORDS], ap[...], loss_sum[...]) of replicates [b_begin, b_end)."""
+        w = self._w(w)
+        k = max(int(b_end) - int(b_begin), 0)
+        words = np.zeros((max(k, 1), BOOTSTRAP_WORDS), dtype=np.int64)
+        ap = np.zeros(max(k, 1), dtype=np.float64)
+        loss = np.zeros(max(k, 1), dtype=np.float64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin),
+                                                 int(b_end), _ptr(words), _ptr(ap), _ptr(loss)))
+        return words[:k], ap[:k], loss[:k]
+
+    def eval_bootstrap(self, row_begin: int, row_end: int, bkey: int, b_begin: int, b_end: int, w=None):
+        """Poisson-bootstrap replicates [b_begin, b_end) of rows [row_begin, row_end) with key bkey (dsgd_eval_bootstrap):
+        (words, ap, loss_sum), one row per replicate -- the metrics words and size, the average precision and the loss sum of
+        the replicate's expanded list."""
+        return self._bootstrap("eval_bootstrap", w, (row_begin, row_end), bkey, b_begin, b_end)
+
+    def eval_sampled_bootstrap(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, bkey: int,
+                               b_begin: int, b_end: int, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_bootstrap)."""
+        return self._bootstrap("eval_sampled_bootstrap", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), bkey,
+                               b_begin, b_end)
+
+    def eval_samples_bootstrap(self, samples, bkey: int, b_begin: int, b_end: int, w=None):
+        """The same over a list of row ids, position i being list index i (dsgd_eval_samples_bootstrap)."""
+        samples = _arr(samples, np.int32)
+        return self._bootstrap("eval_samples_bootstrap", w, (_ptr(samples), samples.size), bkey, b_begin, b_end)
 
     # -- sync --
     def set_workers(self, counts, k_total: int = 0):

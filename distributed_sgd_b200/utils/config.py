@@ -43,6 +43,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     calibration_weighted: bool = False    # extension: `calibrate` fits and judges with every row counted by its weight
     sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
     fit_intercept: bool = False   # extension: fit an unregularised intercept (weights dim + 1 long), sync mode only
+    bootstrap: int = 0            # extension: Poisson-bootstrap replicates of the final test metrics' intervals; 0: off
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -62,6 +63,7 @@ _KEYS = {
     "calibration-weighted": ("calibration_weighted", "DSGD_CALIBRATION_WEIGHTED"),
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
     "fit-intercept": ("fit_intercept", "DSGD_FIT_INTERCEPT"),
+    "bootstrap": ("bootstrap", "DSGD_BOOTSTRAP"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -141,6 +143,8 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
     if cfg.calibration_method not in CALIBRATION_METHODS:
         raise ValueError(f"calibration-method: expected one of {', '.join(CALIBRATION_METHODS)}, "
                          f"got {cfg.calibration_method!r}")
+    if cfg.bootstrap < 0:
+        raise ValueError(f"bootstrap: expected a number of replicates >= 0 (0: off), got {cfg.bootstrap}")
     if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
         raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
     return cfg

@@ -272,6 +272,34 @@ int dsgd_eval_sampled_curve(dsgd_ctx *ctx, const double *w, int64_t row_begin, i
 int dsgd_eval_samples_curve(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *words_out,
                             double *ap_out, int64_t *n_points_out, double *thr_out, int64_t *tp_out, int64_t *fp_out);
 
+/* ---- Poisson bootstrap of the test metrics over the same three row forms (DESIGN.md §4.19).  Position i of a request is
+ *      r - row_begin (range), the index p - pos_begin of draw position p (sampled) or the list index (list): two calls over the
+ *      same rows with the same bkey resample them identically, whatever weights they score.  Replicate b gives position i the
+ *      multiplicity m_i(b) = #{k in 0..19 : u >= T_k}, u = H(bkey, b, i), T_k = floor(F(k) 2^64), F the Poisson(1) CDF (m <=
+ *      20; the draw and the T_k are in distributed_sgd_b200/csrc/dsgd_bootstrap.h).  Replicate b is defined as the unweighted
+ *      evaluation of the expanded list -- the request's ids with position i repeated m_i(b) times, in position order -- and
+ *      for each b in [b_begin, b_end), at index j = b - b_begin:
+ *        words_out[9 j + 0 .. 7]  the DSGD_METRICS_WORDS of dsgd_eval_samples_metrics over the expanded list, bit for bit
+ *        words_out[9 j + 8]       sum of m_i(b), the replicate's size
+ *        ap_out[j]                *ap_out of dsgd_eval_samples_curve over the expanded list, bit for bit (NaN when a score
+ *                                 is NaN or the replicate has no positive)
+ *        loss_out[j]              the loss sum of dsgd_eval_samples_sums over the expanded list, bit for bit (the SVM's
+ *                                 integer hinge sum; the fixed-point sum of the other models, NaN as there)
+ *      A replicate's bits do not depend on the grid, the row order or which other replicates the call computes.  The pass is
+ *      unweighted: class and sample weights are not read.  All four models, with or without an intercept; the scores are
+ *      those dsgd_margins returns.  Errors: a NULL output, b_begin < 0, or a request of more than 2^26 rows ->
+ *      DSGD_ERR_INVALID; b_end <= b_begin -> DSGD_ERR_EMPTY; an async ctx while its loop runs -> DSGD_ERR_STATE; all before
+ *      anything is launched.  Otherwise the errors and the w == NULL convention are those of the metrics calls.  A pass grows
+ *      its buffers (about 36 bytes per row, 52 for the models other than the SVM, and the sort's storage) on first use. */
+#define DSGD_BOOTSTRAP_WORDS 9
+int dsgd_eval_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t bkey, int64_t b_begin,
+                        int64_t b_end, int64_t *words_out, double *ap_out, double *loss_out);
+int dsgd_eval_sampled_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                int64_t pos_begin, int64_t pos_end, uint64_t bkey, int64_t b_begin, int64_t b_end,
+                                int64_t *words_out, double *ap_out, double *loss_out);
+int dsgd_eval_samples_bootstrap(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, uint64_t bkey,
+                                int64_t b_begin, int64_t b_end, int64_t *words_out, double *ap_out, double *loss_out);
+
 /* ---- weighted curves: the curve calls above with every row counted by its weight, on any sync ctx and for either model.
  *      Rows, the three row forms, s = -x.w, NaN handling, ties and the m points are exactly those of dsgd_eval_curve.  Row
  *      i's weight is c_i = fl(w_y * s_i), the class weight of its label times its sample weight (dsgd_set_class_weights,
