@@ -68,6 +68,51 @@ def bootstrap_values(words, ap, loss_sum, penalty: float) -> dict:
             "f1": ratio(2 * tp, 2 * tp + fp + fn + pos_none)}
 
 
+def weighted_bootstrap_values(words, wsums, loss_sum, penalty: float) -> dict:
+    """Each BOOTSTRAP_METRICS value of every weighted replicate from its two words (size, NaN-score rows), its
+    native.WCURVE_WORDS weighted words and its weighted loss sum, by the formulas of weighted_curve_dict and
+    native.weighted_auc_ap (nan where undefined); loss = penalty + loss sum / replicate size, as in local_weighted_report."""
+    size, nan = np.asarray(words, dtype=np.int64).reshape(-1, 2).astype(np.float64).T
+    tp, fn, pos_none, fp, _, _, u2w, _, s_ap, correct, total, wp, wn = np.asarray(wsums, np.float64).reshape(-1, 13).T
+
+    def ratio(a, b):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.where(b > 0, a / np.where(b > 0, b, 1.0), np.nan)
+
+    with np.errstate(divide="ignore", invalid="ignore"):
+        auc = np.where((nan == 0) & (wp != 0) & (wn != 0), u2w / (2.0 * wp * wn), np.nan)
+        ap = np.where((nan == 0) & (wp != 0), np.where(wn == 0, 1.0, s_ap / wp), np.nan)
+    return {"accuracy": ratio(correct, total), "loss": penalty + ratio(np.asarray(loss_sum, np.float64), size),
+            "auc": auc, "ap": ap, "precision": ratio(tp, tp + fp), "recall": ratio(tp, wp),
+            "f1": ratio(2.0 * tp, 2.0 * tp + fp + fn + pos_none)}
+
+
+# The replicate layout of a bootstrap call, as (int64 words, doubles) per replicate: the unweighted calls return
+# BOOTSTRAP_WORDS words and the AP, the weighted ones the size and NaN rows and the WCURVE_WORDS words; both then a loss sum.
+BOOTSTRAP_LAYOUT = {False: (9, 1), True: (2, 13)}
+
+
+def bootstrap_pack(words, mid, loss) -> np.ndarray:
+    """One rank's replicates as one float64 array: the words' bits, then the middle doubles (AP or the weighted words), then
+    the loss sums, each block replicate-major."""
+    return np.concatenate([np.asarray(words, np.int64).reshape(-1).view(np.float64),
+                           np.asarray(mid, np.float64).reshape(-1), np.asarray(loss, np.float64).reshape(-1)])
+
+
+def bootstrap_unpack(parts, weighted: bool = False):
+    """bootstrap_pack's arrays of every rank, in rank order, back into (words[k, nw], mid, loss[k]) over all replicates:
+    mid is ap[k] (unweighted) or wsums[k, 13] (weighted)."""
+    nw, nm = BOOTSTRAP_LAYOUT[bool(weighted)]
+    words, mid, loss = [], [], []
+    for p in parts:
+        p = np.asarray(p, np.float64)
+        k = p.size // (nw + nm + 1)
+        words.append(p[:nw * k].view(np.int64).reshape(k, nw))
+        mid.append(p[nw * k:(nw + nm) * k].reshape(k, nm) if weighted else p[nw * k:(nw + nm) * k])
+        loss.append(p[(nw + nm) * k:])
+    return np.concatenate(words), np.concatenate(mid), np.concatenate(loss)
+
+
 def bootstrap_summary(estimate: float, reps, level: float) -> dict:
     """One metric's bootstrap: the full-sample estimate, the percentile interval at `level` (numpy.quantile's default method)
     over the replicates where the metric is defined and how many those are, the standard error (their standard deviation),
@@ -580,30 +625,24 @@ class Master:
     # Poisson-bootstrap intervals of the ranking metrics, accuracy and loss (dsgd_eval_*bootstrap).  Every rank holds every
     # row; rank r computes the replicates bootstrap_share(n_boot, W, r) and all are gathered in rank order, so every rank
     # returns the same bits -- a replicate's bits do not depend on which rank computed it.
-    def _bootstrap_raw(self, call: str, rows: tuple, weights, n_boot: int, key: int):
-        """(words, ap, loss_sum) of replicates [0, n_boot) of ctx.<call>(*rows, key, lo, hi, weights), gathered in rank
-        order."""
+    # weighted=True counts every row by its weight c_i = class weight x sample weight (dsgd_eval_*weighted_bootstrap): the
+    # same seven metrics by weighted_curve_dict's formulas, the estimates from the weighted curve and evaluation calls.
+    def _bootstrap_raw(self, call: str, rows: tuple, weights, n_boot: int, key: int, weighted: bool = False):
+        """(words, ap, loss_sum) -- weighted: (words, wsums, loss_sum) -- of replicates [0, n_boot) of
+        ctx.<call>(*rows, key, lo, hi, weights), gathered in rank order."""
         if n_boot <= 0:
             raise ValueError(f"n_boot: expected a number of replicates > 0, got {n_boot}")
         lo, hi = bootstrap_share(int(n_boot), self.group.world, self.group.rank)
-        if hi > lo:
-            words, ap, loss = getattr(self.ctx, call)(*rows, key, lo, hi, weights)
-            mine = np.concatenate([np.asarray(words, np.int64).reshape(-1).view(np.float64), np.asarray(ap, np.float64),
-                                   np.asarray(loss, np.float64)])
-        else:
-            mine = np.zeros(0)
+        mine = bootstrap_pack(*getattr(self.ctx, call)(*rows, key, lo, hi, weights)) if hi > lo else np.zeros(0)
         parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
-        words, ap, loss = [], [], []
-        for p in parts:
-            k = p.size // 11
-            words.append(p[:9 * k].view(np.int64).reshape(k, 9))
-            ap.append(p[9 * k:10 * k])
-            loss.append(p[10 * k:])
-        return np.concatenate(words), np.concatenate(ap), np.concatenate(loss)
+        return bootstrap_unpack(parts, weighted)
 
-    def _bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int]):
+    def _bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int], weighted: bool = False):
         """(call, rows, estimates) of one bootstrap request: the whole train (or test) rows, or a fresh sample
-        (_draw_sample); the estimates come from the existing curve and *_sums calls over the same rows."""
+        (_draw_sample); the estimates come from the existing curve and *_sums calls over the same rows (weighted: the
+        weighted curve and weighted evaluation calls, as local_weighted_curve and local_weighted_report form them)."""
+        if weighted:
+            return self._weighted_bootstrap_case(weights, test_data, samples_count)
         b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
         if samples_count is None:
             call, rows = "eval_bootstrap", (b, e)
@@ -627,38 +666,67 @@ class Master:
         est = {k: float(v[0]) for k, v in bootstrap_values(np.concatenate([words, [n]]), [ap], [sums[0]], penalty).items()}
         return call, rows, est, penalty
 
-    def _bootstrap(self, weights, test_data, samples_count, n_boot, key, level) -> dict:
-        call, rows, est, penalty = self._bootstrap_case(weights, test_data, samples_count)
+    def _weighted_bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int]):
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        if samples_count is None:
+            call, rows = "eval_weighted_bootstrap", (b, e)
+            wc = self.ctx.eval_weighted_curve(b, e, weights, curve=False)
+            we = self.ctx.eval_weighted(b, e, weights)
+        else:
+            b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+            if k <= 0:
+                raise DsgdEmpty(ERR_EMPTY, f"sampled bootstrap of {samples_count} rows: the sample is empty")
+            if ids is None:
+                call, rows = "eval_sampled_weighted_bootstrap", (b, e, key, 0, k)
+                wc = self.ctx.eval_sampled_weighted_curve(b, e, key, 0, k, weights, curve=False)
+                we = self.ctx.eval_sampled_weighted(b, e, key, 0, k, weights)
+            else:
+                call, rows = "eval_samples_weighted_bootstrap", (ids,)
+                wc = self.ctx.eval_samples_weighted_curve(ids, weights, curve=False)
+                we = self.ctx.eval_samples_weighted(ids, weights)
+        curve, report = weighted_curve_dict(wc, curve=False), self._weighted_report(we, weights)
+        est = {"accuracy": curve["accuracy"], "loss": report["weighted_loss"], "auc": curve["auc"],
+               "ap": curve["average_precision"], "precision": curve["precision"], "recall": curve["recall"],
+               "f1": curve["f1"]}
+        return call, rows, est, self._penalty(we.norm_squared, weights, True)
+
+    def _bootstrap(self, weights, test_data, samples_count, n_boot, key, level, weighted=False) -> dict:
+        call, rows, est, penalty = self._bootstrap_case(weights, test_data, samples_count, weighted)
         key = bootstrap_key(self.seed) if key is None else int(key)
-        reps = bootstrap_values(*self._bootstrap_raw(call, rows, weights, n_boot, key), penalty)
+        values = weighted_bootstrap_values if weighted else bootstrap_values
+        reps = values(*self._bootstrap_raw(call, rows, weights, n_boot, key, weighted), penalty)
         return {m: bootstrap_summary(est[m], reps[m], level) for m in BOOTSTRAP_METRICS}
 
     def local_bootstrap(self, weights=None, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
-                        level: float = 0.95) -> dict:
+                        level: float = 0.95, weighted: bool = False) -> dict:
         """Poisson-bootstrap intervals over the test (or train) rows: for each of accuracy, loss (penalty + S / n, the
         unweighted loss of the *_sums calls), auc, ap, precision, recall and f1 (BOOTSTRAP_METRICS) a dict of the full-sample
         estimate, the percentile interval [lo, hi] at `level` over the replicates where the metric is defined, n_defined,
-        the standard error se and the raw replicates.  key None: bootstrap_key(seed)."""
-        return self._bootstrap(weights, test_data, None, n_boot, key, level)
+        the standard error se and the raw replicates.  key None: bootstrap_key(seed).  weighted: every row counted by its
+        weight c_i = class weight x sample weight -- the metrics of local_weighted_curve and the loss of
+        local_weighted_report, resampled with the same multiplicities as the unweighted bootstrap of the same key."""
+        return self._bootstrap(weights, test_data, None, n_boot, key, level, weighted)
 
     def local_sampled_bootstrap(self, weights, samples_count: int, test_data: bool = True, n_boot: int = 1000,
-                                key: Optional[int] = None, level: float = 0.95) -> dict:
+                                key: Optional[int] = None, level: float = 0.95, weighted: bool = False) -> dict:
         """local_bootstrap over a fresh sample of min(samples_count, n) rows (_draw_sample).  An empty sample raises
         DsgdEmpty."""
-        return self._bootstrap(weights, test_data, samples_count, n_boot, key, level)
+        return self._bootstrap(weights, test_data, samples_count, n_boot, key, level, weighted)
 
     def compare_bootstrap(self, weights_a, weights_b, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
-                          level: float = 0.95) -> dict:
+                          level: float = 0.95, weighted: bool = False) -> dict:
         """Paired comparison of two weight vectors over the same rows: both are scored with the same bootstrap key, so
         replicate b resamples the same rows for both.  Per metric: the difference b - a of the estimates, its percentile
         interval, standard error and defined-replicate count (replicates where the metric is defined for both), and
-        p_better, the share of those replicates in which b is better (higher, or lower for the loss)."""
+        p_better, the share of those replicates in which b is better (higher, or lower for the loss).  weighted: as in
+        local_bootstrap."""
         key = bootstrap_key(self.seed) if key is None else int(key)
+        values = weighted_bootstrap_values if weighted else bootstrap_values
         out = {}
         sides = []
         for w in (weights_a, weights_b):
-            call, rows, est, penalty = self._bootstrap_case(w, test_data, None)
-            sides.append((est, bootstrap_values(*self._bootstrap_raw(call, rows, w, n_boot, key), penalty)))
+            call, rows, est, penalty = self._bootstrap_case(w, test_data, None, weighted)
+            sides.append((est, values(*self._bootstrap_raw(call, rows, w, n_boot, key, weighted), penalty)))
         (ea, ra), (eb, rb) = sides
         for m, higher in BOOTSTRAP_METRICS.items():
             d = rb[m] - ra[m]

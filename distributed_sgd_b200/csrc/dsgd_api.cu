@@ -194,6 +194,10 @@ struct dsgd_ctx {
   dev_buf<int> b_gs;
   dev_buf<double> b_loss, b_eloss;
   dev_buf<unsigned long long> b_out;
+  // a weighted bootstrap pass (dsgd_eval_*weighted_bootstrap) also keeps, in sorted order, the last index of every element's
+  // tie group (the first in b_gs) and its weight c (fl(c L) in b_eloss)
+  dev_buf<int> b_gl;
+  dev_buf<double> b_c;
 
   ncclComm_t comm = nullptr;
 
@@ -1569,20 +1573,18 @@ extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const i
 
 constexpr int64_t kBootChunk = 4096;   // replicates per k_boot_rep launch: its output block stays small whatever n_boot is
 
-// One bootstrap pass over `rows`: positions scored, sorted and arranged once, then replicates [b_begin, b_end) in chunks.
-// Per replicate b (index b - b_begin of the outputs): the DSGD_BOOTSTRAP_WORDS words, AP = S / P under the curve pass's NaN
-// rule, and the loss sum.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
-static int bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, uint64_t bkey, int64_t b_begin, int64_t b_end,
-                          int64_t *words, double *ap, double *loss) {
+// The part of a bootstrap pass that does not depend on the replicate: every position of `rows` scored (k_boot_score, with
+// the losses by position in b_loss for every model but the SVM) and the (key, tag) pairs sorted; *kb / *tb hold the sorted
+// keys and tags.  The keys, tags and losses' buffers are grown here.
+static int boot_sorted(dsgd_ctx *ctx, const double *w, const row_set &rows, cub::DoubleBuffer<unsigned long long> *kb,
+                       cub::DoubleBuffer<uint32_t> *tb) {
   const int64_t n = rows.n;
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = request_weights(ctx, w, &wd, &cd, &nd);
   if (rc) return rc;
   const bool kl = model_of(ctx) != kSvm;
   if ((rc = ctx->m_keys.grow(ctx, n, 1024)) || (rc = ctx->m_alt.grow(ctx, n, 1024)) || (rc = ctx->b_tag.grow(ctx, n, 1024)) ||
-      (rc = ctx->b_tagt.grow(ctx, n, 1024)) || (rc = ctx->b_gs.grow(ctx, n, 1024)) ||
-      (kl && ((rc = ctx->b_loss.grow(ctx, n, 1024)) || (rc = ctx->b_eloss.grow(ctx, n, 1024)))) ||
-      (rc = ctx->b_out.grow(ctx, kBootChunk * kBootOutWords, kBootChunk * kBootOutWords)))
+      (rc = ctx->b_tagt.grow(ctx, n, 1024)) || (kl && (rc = ctx->b_loss.grow(ctx, n, 1024))))
     return rc;
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 positions per warp
   rc = with_model<kUnweighted>(ctx, [&](auto m, auto, auto ic) {
@@ -1593,12 +1595,29 @@ static int bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, u
   });
   if (rc) return rc;
   CU(cudaGetLastError());
-  cub::DoubleBuffer<unsigned long long> kb(ctx->m_keys.p, ctx->m_alt.p);
-  cub::DoubleBuffer<uint32_t> tb(ctx->b_tag.p, ctx->b_tagt.p);
+  *kb = cub::DoubleBuffer<unsigned long long>(ctx->m_keys.p, ctx->m_alt.p);
+  *tb = cub::DoubleBuffer<uint32_t>(ctx->b_tag.p, ctx->b_tagt.p);
   size_t tmp = 0;
-  CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kb, tb, (int)n, 0, 64, ctx->stream));
+  CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, *kb, *tb, (int)n, 0, 64, ctx->stream));
   if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
-  CU(cub::DeviceRadixSort::SortPairs(ctx->m_tmp.p, tmp, kb, tb, (int)n, 0, 64, ctx->stream));
+  CU(cub::DeviceRadixSort::SortPairs(ctx->m_tmp.p, tmp, *kb, *tb, (int)n, 0, 64, ctx->stream));
+  return DSGD_OK;
+}
+
+// One bootstrap pass over `rows`: positions scored, sorted and arranged once, then replicates [b_begin, b_end) in chunks.
+// Per replicate b (index b - b_begin of the outputs): the DSGD_BOOTSTRAP_WORDS words, AP = S / P under the curve pass's NaN
+// rule, and the loss sum.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
+static int bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, uint64_t bkey, int64_t b_begin, int64_t b_end,
+                          int64_t *words, double *ap, double *loss) {
+  const int64_t n = rows.n;
+  const bool kl = model_of(ctx) != kSvm;
+  cub::DoubleBuffer<unsigned long long> kb;
+  cub::DoubleBuffer<uint32_t> tb;
+  int rc;
+  if ((rc = ctx->b_gs.grow(ctx, n, 1024)) || (kl && (rc = ctx->b_eloss.grow(ctx, n, 1024))) ||
+      (rc = ctx->b_out.grow(ctx, kBootChunk * kBootOutWords, kBootChunk * kBootOutWords)) ||
+      (rc = boot_sorted(ctx, w, rows, &kb, &tb)))
+    return rc;
   const int agrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
   if (kl)
     k_boot_arrange<true><<<agrid, 256, 0, ctx->stream>>>(kb.Current(), tb.Current(), n, ctx->b_loss, ctx->b_gs, ctx->b_eloss);
@@ -1628,6 +1647,56 @@ static int bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, u
       memcpy(&L, &o[kBootLoss], sizeof L);
       ap[b0 - b_begin + r] = (wr[kMetNan] > 0 || P == 0) ? std::numeric_limits<double>::quiet_NaN() : S / (double)P;
       loss[b0 - b_begin + r] = L;
+    }
+  }
+  return DSGD_OK;
+}
+
+// One weighted bootstrap pass over `rows` (DESIGN.md §4.20): scored and sorted as bootstrap_pass does, each sorted element's
+// tie group, c and fl(c L) arranged once, then replicates [b_begin, b_end) in chunks.  Per replicate b (index j = b - b_begin):
+// words[2 j] = sum m, words[2 j + 1] = the NaN-score rows, wsums[13 j ..] the DSGD_WCURVE_WORDS and loss[j] the weighted loss
+// sum S of the expanded list.  Launches of the sort's own kernels are not counted in dsgd_launch_count.
+static int weighted_bootstrap_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, uint64_t bkey, int64_t b_begin,
+                                   int64_t b_end, int64_t *words, double *wsums, double *loss) {
+  const int64_t n = rows.n;
+  const bool kl = model_of(ctx) != kSvm;
+  cub::DoubleBuffer<unsigned long long> kb;
+  cub::DoubleBuffer<uint32_t> tb;
+  int rc;
+  if ((rc = ctx->b_gs.grow(ctx, n, 1024)) || (rc = ctx->b_gl.grow(ctx, n, 1024)) || (rc = ctx->b_c.grow(ctx, n, 1024)) ||
+      (rc = ctx->b_eloss.grow(ctx, n, 1024)) ||
+      (rc = ctx->b_out.grow(ctx, kBootChunk * kWbOutWords, kBootChunk * kWbOutWords)) ||
+      (rc = boot_sorted(ctx, w, rows, &kb, &tb)))
+    return rc;
+  const int agrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
+  const double *sw = ctx->sw_on ? ctx->sw.p : nullptr;
+  if (kl)
+    k_wboot_arrange<true><<<agrid, 256, 0, ctx->stream>>>(kb.Current(), tb.Current(), n, rows.ids, rows.row_begin, ctx->cw_pos,
+                                                          ctx->cw_neg, sw, ctx->b_loss, ctx->b_gs, ctx->b_gl, ctx->b_c,
+                                                          ctx->b_eloss);
+  else
+    k_wboot_arrange<false><<<agrid, 256, 0, ctx->stream>>>(kb.Current(), tb.Current(), n, rows.ids, rows.row_begin,
+                                                           ctx->cw_pos, ctx->cw_neg, sw, nullptr, ctx->b_gs, ctx->b_gl,
+                                                           ctx->b_c, ctx->b_eloss);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  std::vector<unsigned long long> h((size_t)(kBootChunk * kWbOutWords));
+  for (int64_t b0 = b_begin; b0 < b_end; b0 += kBootChunk) {
+    const int64_t k = std::min(kBootChunk, b_end - b0);
+    k_wboot_rep<<<(int)k, kWbThreads, 0, ctx->stream>>>(kb.Current(), tb.Current(), ctx->b_gs, ctx->b_gl, ctx->b_c,
+                                                         ctx->b_eloss, n, bkey, b0, ctx->b_out);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(h.data(), ctx->b_out, sizeof(unsigned long long) * (size_t)(k * kWbOutWords), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (int64_t r = 0; r < k; ++r) {
+      const unsigned long long *o = &h[(size_t)(r * kWbOutWords)];
+      const int64_t j = b0 - b_begin + r;
+      words[2 * j] = (int64_t)o[kWbSize];
+      words[2 * j + 1] = (int64_t)o[kWbNan];
+      memcpy(&wsums[DSGD_WCURVE_WORDS * j], &o[kWbSums], sizeof(double) * DSGD_WCURVE_WORDS);
+      memcpy(&loss[j], &o[kWbLoss], sizeof(double));
     }
   }
   return DSGD_OK;
@@ -1667,6 +1736,46 @@ extern "C" int dsgd_eval_samples_bootstrap(dsgd_ctx *ctx, const double *w, const
                                            int64_t b_begin, int64_t b_end, int64_t *words_out, double *ap_out,
                                            double *loss_out) {
   return bootstrap_request(ctx, w, listed_rows(samples, n), __func__, bkey, b_begin, b_end, words_out, ap_out, loss_out);
+}
+
+// dsgd_eval*_weighted_bootstrap: the outputs and the replicate range, an async ctx (its weights are always 1, and the pass
+// grows its own buffers), then the request's size -- all before anything is launched, the sampled form's draw included
+static int weighted_bootstrap_request(dsgd_ctx *ctx, const double *w, const row_request &req, const char *fn, uint64_t bkey,
+                                      int64_t b_begin, int64_t b_end, int64_t *words, double *wsums, double *loss) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(words && wsums && loss, DSGD_ERR_INVALID, "%s: words_out, wsums_out or loss_out is NULL", fn);
+  NEED(b_begin >= 0, DSGD_ERR_INVALID, "%s: replicates [%lld,%lld) start below 0", fn, (long long)b_begin, (long long)b_end);
+  NEED(b_end > b_begin, DSGD_ERR_EMPTY, "%s: no replicates [%lld,%lld)", fn, (long long)b_begin, (long long)b_end);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (row weights belong to the sync paths)",
+       fn);
+  const int64_t n = req.form == row_request::kRange ? req.row_end - req.row_begin
+                    : req.form == row_request::kDrawn ? req.pos_end - req.pos_begin : req.n;
+  NEED(n <= kBootMaxRows, DSGD_ERR_INVALID, "%s: %lld rows; a bootstrap takes at most 2^26", fn, (long long)n);
+  row_set rows;
+  int rc = resolve_rows(ctx, req, fn, &rows);
+  return rc ? rc : weighted_bootstrap_pass(ctx, w, rows, bkey, b_begin, b_end, words, wsums, loss);
+}
+
+extern "C" int dsgd_eval_weighted_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t bkey,
+                                            int64_t b_begin, int64_t b_end, int64_t *words_out, double *wsums_out,
+                                            double *loss_out) {
+  return weighted_bootstrap_request(ctx, w, range_rows(row_begin, row_end), __func__, bkey, b_begin, b_end, words_out,
+                                    wsums_out, loss_out);
+}
+
+extern "C" int dsgd_eval_sampled_weighted_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end,
+                                                    uint64_t key, int64_t pos_begin, int64_t pos_end, uint64_t bkey,
+                                                    int64_t b_begin, int64_t b_end, int64_t *words_out, double *wsums_out,
+                                                    double *loss_out) {
+  return weighted_bootstrap_request(ctx, w, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, bkey, b_begin,
+                                    b_end, words_out, wsums_out, loss_out);
+}
+
+extern "C" int dsgd_eval_samples_weighted_bootstrap(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n,
+                                                    uint64_t bkey, int64_t b_begin, int64_t b_end, int64_t *words_out,
+                                                    double *wsums_out, double *loss_out) {
+  return weighted_bootstrap_request(ctx, w, listed_rows(samples, n), __func__, bkey, b_begin, b_end, words_out, wsums_out,
+                                    loss_out);
 }
 
 // ---- calibration (dsgd_calibrate.cuh; DESIGN.md §4.11) ---------------------------------------------------------------

@@ -80,6 +80,16 @@ object DsgdNative {
                                    ap: Array[Double], loss: Array[Double]): Int
   @native def evalSamplesBootstrap(ctx: Long, w: Array[Double], samples: Array[Int], bKey: Long, bBegin: Long, bEnd: Long,
                                    words: Array[Long], ap: Array[Double], loss: Array[Double]): Int
+  // weighted Poisson bootstrap, every row counted by c_i = class weight x sample weight: words(2 j) and words(2 j + 1) = the
+  // size and the NaN-score rows of replicate bBegin + j, wsums(13 j until 13 j + 13) its weighted curve words, loss(j) its
+  // weighted loss sum.  Each array holds at least the replicates' entries.
+  @native def evalWeightedBootstrap(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, bKey: Long, bBegin: Long,
+                                    bEnd: Long, words: Array[Long], wsums: Array[Double], loss: Array[Double]): Int
+  @native def evalSampledWeightedBootstrap(ctx: Long, w: Array[Double], rowBegin: Long, rowEnd: Long, key: Long,
+                                           posBegin: Long, posEnd: Long, bKey: Long, bBegin: Long, bEnd: Long,
+                                           words: Array[Long], wsums: Array[Double], loss: Array[Double]): Int
+  @native def evalSamplesWeightedBootstrap(ctx: Long, w: Array[Double], samples: Array[Int], bKey: Long, bBegin: Long,
+                                           bEnd: Long, words: Array[Long], wsums: Array[Double], loss: Array[Double]): Int
   // calibration (Platt scaling): ab(0..1) = (A, B) of P(y = +1 | x) = 1 / (1 + exp(A x.w + B)), objective(0) = F(A, B),
   // info(0..4) = iterations, status (0 converged, 1 iteration limit, 2 line search failed, 3 non-finite sum), rows used, NaN
   // rows, points evaluated.  Quality at (a, b): sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum(0 until

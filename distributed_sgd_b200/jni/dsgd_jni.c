@@ -381,6 +381,59 @@ FN(evalSamplesBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jin
   return rc;
 }
 
+/* weighted Poisson bootstrap: replicates [bBegin, bEnd) with key bKey; words(2 j), words(2 j + 1) = the size and the NaN-score
+ * rows of replicate bBegin + j, wsums(13 j .. 13 j + 12) its DSGD_WCURVE_WORDS, loss(j) its weighted loss sum.  The buffers
+ * are those of the unweighted bootstrap, with wsums in ap's place.  An output shorter than the replicates is
+ * DSGD_ERR_INVALID. */
+static int wboot_short(const boot_bufs *c, jlong bBegin, jlong bEnd) {
+  const jlong k = bEnd > bBegin ? bEnd - bBegin : 0;
+  return c->m.n < k * 2 || c->a.n < k * DSGD_WCURVE_WORDS || c->l.n < k;
+}
+FN(evalWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong bKey,
+                          jlong bBegin, jlong bEnd, jlongArray words, jdoubleArray wsums, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w);
+  boot_bufs c = boot_out(env, words, wsums, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | boot_bad(&c)))
+    rc = wboot_short(&c, bBegin, bEnd)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_weighted_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p,
+                                            (double *)c.a.p, (double *)c.l.p);
+  boot_back(env, words, wsums, loss, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSampledWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
+                                 jlong posBegin, jlong posEnd, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
+                                 jdoubleArray wsums, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w);
+  boot_bufs c = boot_out(env, words, wsums, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | boot_bad(&c)))
+    rc = wboot_short(&c, bBegin, bEnd)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_sampled_weighted_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
+                                                    (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p, (double *)c.a.p,
+                                                    (double *)c.l.p);
+  boot_back(env, words, wsums, loss, &c, rc);
+  free(bw.p);
+  return rc;
+}
+FN(evalSamplesWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlong bKey,
+                                 jlong bBegin, jlong bEnd, jlongArray words, jdoubleArray wsums, jdoubleArray loss) {
+  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
+  boot_bufs c = boot_out(env, words, wsums, loss);
+  int rc = DSGD_ERR_NOMEM;
+  if (!(bw.bad | bs.bad | boot_bad(&c)))
+    rc = wboot_short(&c, bBegin, bEnd)
+             ? DSGD_ERR_INVALID
+             : dsgd_eval_samples_weighted_bootstrap(CTX(h), bw.p, bs.p, bs.n, (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p,
+                                                    (double *)c.a.p, (double *)c.l.p);
+  boot_back(env, words, wsums, loss, &c, rc);
+  free(bw.p); free(bs.p);
+  return rc;
+}
+
 /* calibration: ab(0..1) = (A, B), objective(0) = F(A, B), info(0..4) = the DSGD_CALIBRATION_INFO_WORDS words; probabilities:
  * out(i) = sigmoid(-(a x_i . w + b)); quality: sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum at least nBins
  * long, words(0..1) = rows used and left out.  A shorter array is DSGD_ERR_INVALID. */

@@ -50,6 +50,9 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     if cfg.calibration_weighted and cfg.is_async:
         raise ValueError("calibration-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
                          "has none to calibrate by")
+    if cfg.bootstrap_weighted and cfg.is_async:
+        raise ValueError("bootstrap-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
+                         "has none to resample by")
     if cfg.sample_weight:   # one weight per loaded row; the split below carries them
         data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
@@ -143,9 +146,12 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                    if cfg.model == "logistic" else ""))
     if cfg.bootstrap > 0:
         # Poisson-bootstrap 95 % intervals of the final test metrics (the replicates themselves are not reported)
-        bs = master.local_bootstrap(w1, test_data=True, n_boot=cfg.bootstrap)
+        bkw = {"weighted": True} if cfg.bootstrap_weighted else {}   # unweighted: the calls as they always were
+        bs = master.local_bootstrap(w1, test_data=True, n_boot=cfg.bootstrap, **bkw)
         report["test_bootstrap"] = {m: {k: v for k, v in r.items() if k != "replicates"} for m, r in bs.items()}
         report["test_bootstrap"]["replicates"] = cfg.bootstrap
+        if cfg.bootstrap_weighted:
+            report["test_bootstrap"]["weighted"] = True
         if rank == 0:
             log(f"bootstrap ({cfg.bootstrap} replicates, 95 %): " + ", ".join(
                 f"{m} {bs[m]['estimate']:.4f} [{bs[m]['lo']:.4f}, {bs[m]['hi']:.4f}]" for m in ("auc", "ap", "accuracy", "loss")))

@@ -158,6 +158,9 @@ ABI = {
     "dsgd_eval_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
     "dsgd_eval_sampled_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
     "dsgd_eval_samples_bootstrap": [_vp, _vp, _vp, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_eval_weighted_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_eval_sampled_weighted_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
+    "dsgd_eval_samples_weighted_bootstrap": [_vp, _vp, _vp, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
     "dsgd_eval_weighted_curve": [_vp, _vp, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_sampled_weighted_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_eval_samples_weighted_curve": [_vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
@@ -1045,6 +1048,36 @@ class NativeCtx:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted_curve)."""
         samples = _arr(samples, np.int32)
         return self._weighted_curve("eval_samples_weighted_curve", w, (_ptr(samples), samples.size), samples.size, curve)
+
+    # -- weighted bootstrap --
+    def _weighted_bootstrap(self, fn: str, w, rows: tuple, bkey: int, b_begin: int, b_end: int):
+        """dsgd_<fn>: (words[b_end - b_begin, 2], wsums[..., WCURVE_WORDS], loss_sum[...]) of replicates [b_begin, b_end)."""
+        w = self._w(w)
+        k = max(int(b_end) - int(b_begin), 0)
+        words = np.zeros((max(k, 1), 2), dtype=np.int64)
+        wsums = np.zeros((max(k, 1), WCURVE_WORDS), dtype=np.float64)
+        loss = np.zeros(max(k, 1), dtype=np.float64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin),
+                                                 int(b_end), _ptr(words), _ptr(wsums), _ptr(loss)))
+        return words[:k], wsums[:k], loss[:k]
+
+    def eval_weighted_bootstrap(self, row_begin: int, row_end: int, bkey: int, b_begin: int, b_end: int, w=None):
+        """Weighted Poisson-bootstrap replicates [b_begin, b_end) of rows [row_begin, row_end) with key bkey, every row
+        counted by c_i = class weight x sample weight (dsgd_eval_weighted_bootstrap): (words, wsums, loss_sum), one row per
+        replicate -- its size and NaN-score rows, the weighted curve words and the weighted loss sum of its expanded list."""
+        return self._weighted_bootstrap("eval_weighted_bootstrap", w, (row_begin, row_end), bkey, b_begin, b_end)
+
+    def eval_sampled_weighted_bootstrap(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
+                                        bkey: int, b_begin: int, b_end: int, w=None):
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_weighted_bootstrap)."""
+        return self._weighted_bootstrap("eval_sampled_weighted_bootstrap", w,
+                                        _drawn(row_begin, row_end, key, pos_begin, pos_end), bkey, b_begin, b_end)
+
+    def eval_samples_weighted_bootstrap(self, samples, bkey: int, b_begin: int, b_end: int, w=None):
+        """The same over a list of row ids, position i being list index i (dsgd_eval_samples_weighted_bootstrap)."""
+        samples = _arr(samples, np.int32)
+        return self._weighted_bootstrap("eval_samples_weighted_bootstrap", w, (_ptr(samples), samples.size), bkey, b_begin,
+                                        b_end)
 
     # -- async --
     def async_host_master(self, w0):

@@ -44,6 +44,7 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     sample_weight: str = ""       # extension: path of a .npy of one weight per loaded row (before the split), sync mode only
     fit_intercept: bool = False   # extension: fit an unregularised intercept (weights dim + 1 long), sync mode only
     bootstrap: int = 0            # extension: Poisson-bootstrap replicates of the final test metrics' intervals; 0: off
+    bootstrap_weighted: bool = False   # extension: the bootstrap counts every row by its weight (class x sample weight)
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -64,6 +65,7 @@ _KEYS = {
     "sample-weight": ("sample_weight", "DSGD_SAMPLE_WEIGHT"),
     "fit-intercept": ("fit_intercept", "DSGD_FIT_INTERCEPT"),
     "bootstrap": ("bootstrap", "DSGD_BOOTSTRAP"),
+    "bootstrap-weighted": ("bootstrap_weighted", "DSGD_BOOTSTRAP_WEIGHTED"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}

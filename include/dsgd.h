@@ -340,6 +340,31 @@ int dsgd_eval_samples_weighted_curve(dsgd_ctx *ctx, const double *w, const int32
                                      double *wsums_out, int64_t *n_points_out, double *thr_out, double *tpw_out,
                                      double *fpw_out);
 
+/* ---- weighted bootstrap: the Poisson bootstrap above with every row counted by its weight c_i = fl(w_y * s_i), the weight
+ *      of the weighted curves (DESIGN.md §4.20).  The rows, positions, multiplicities m_i(b) and expanded lists are those of
+ *      dsgd_eval*_bootstrap: a weighted and an unweighted call with the same bkey resample the same rows.  Replicate b is
+ *      defined as the weighted calls over its expanded list, every copy of row i weighing c_i; for each b in [b_begin, b_end),
+ *      at index j = b - b_begin:
+ *        words_out[2 j]             sum of m_i(b), the rows of the expanded list (the weighted loss's divisor)
+ *        words_out[2 j + 1]         its NaN-score rows (word 7 of dsgd_eval_samples_metrics over it)
+ *        wsums_out[13 j + 0 .. 12]  the DSGD_WCURVE_WORDS of dsgd_eval_samples_weighted_curve over it, bit for bit
+ *        loss_out[j]                sums_out[0] of dsgd_eval_samples_weighted over it, S = sum R(fl(c_i L_i)), bit for bit
+ *      NaN follows those calls: a term of 2^52 or more, inf or NaN makes its word NaN.  With c = 1 the words 0..7, AP and the
+ *      loss are the unweighted replicate's bit for bit, and words_out[2 j] is its size.  A replicate's bits do not depend on
+ *      the grid, the row order or which other replicates the call computes.  All four models, with or without an intercept.
+ *      Errors: a NULL output, b_begin < 0, or a request of more than 2^26 rows -> DSGD_ERR_INVALID; b_end <= b_begin ->
+ *      DSGD_ERR_EMPTY; an async ctx -> DSGD_ERR_STATE; all before anything is launched.  Otherwise the errors and the
+ *      w == NULL convention are those of the metrics calls.  A pass grows its buffers (about 48 bytes per row, 56 for the
+ *      models other than the SVM, and the sort's storage) on first use. */
+int dsgd_eval_weighted_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t bkey,
+                                 int64_t b_begin, int64_t b_end, int64_t *words_out, double *wsums_out, double *loss_out);
+int dsgd_eval_sampled_weighted_bootstrap(dsgd_ctx *ctx, const double *w, int64_t row_begin, int64_t row_end, uint64_t key,
+                                         int64_t pos_begin, int64_t pos_end, uint64_t bkey, int64_t b_begin, int64_t b_end,
+                                         int64_t *words_out, double *wsums_out, double *loss_out);
+int dsgd_eval_samples_weighted_bootstrap(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, uint64_t bkey,
+                                         int64_t b_begin, int64_t b_end, int64_t *words_out, double *wsums_out,
+                                         double *loss_out);
+
 /* ---- calibration: scores into probabilities, for either model, over the same three row forms and with the conventions and
  *      errors of the metrics calls above.  With f = x_i . w exactly as dsgd_margins returns it, a calibration is a pair (A, B)
  *      and P(y = +1 | x_i) = 1 / (1 + exp(A f + B)), computed as sigmoid(-(A f + B)) with the sigmoid of the logistic gradient.
