@@ -369,21 +369,29 @@ static inline int weighting(const dsgd_ctx *ctx) {
 // an intercept ctx (DSGD_FLAG_INTERCEPT): every weight vector is dim + 1 long, the intercept last (w[dim] on the device too)
 static inline bool has_icpt(const dsgd_ctx *ctx) { return (ctx->flags & DSGD_FLAG_INTERCEPT) != 0; }
 static inline int64_t wlen(const dsgd_ctx *ctx) { return (int64_t)ctx->dim + (has_icpt(ctx) ? 1 : 0); }
+// The intercept of the device weight vector wd (its entry [dim]) on an intercept ctx, else nullptr: the icpt argument of
+// every kernel that forms a score
+static inline const double *icpt_of(const dsgd_ctx *ctx, const double *wd) { return has_icpt(ctx) ? wd + ctx->dim : nullptr; }
+// The one step from a ctx's intercept to a template argument: f(std::true_type{}) on an intercept ctx, else
+// f(std::false_type{})
+template <class F>
+static auto with_icpt(const dsgd_ctx *ctx, F &&f) {
+  return has_icpt(ctx) ? f(std::true_type{}) : f(std::false_type{});
+}
 // The one step from a ctx's run-time model, intercept and a weighting to template arguments: f(model, weighting,
 // intercept), all three as std::integral_constant.  with_model fixes the weighting (an evaluation of one tally); with_forms
 // takes it at run time.
 template <int kWeight, class F>
 static int with_model(const dsgd_ctx *ctx, F &&f) {
   constexpr std::integral_constant<int, kWeight> weight{};
-  auto model = [&](auto icpt) {
+  return with_icpt(ctx, [&](auto icpt) {
     switch (model_of(ctx)) {
       case kLogistic: return f(std::integral_constant<int, kLogistic>{}, weight, icpt);
       case kSquaredHinge: return f(std::integral_constant<int, kSquaredHinge>{}, weight, icpt);
       case kModifiedHuber: return f(std::integral_constant<int, kModifiedHuber>{}, weight, icpt);
       default: return f(std::integral_constant<int, kSvm>{}, weight, icpt);
     }
-  };
-  return has_icpt(ctx) ? model(std::true_type{}) : model(std::false_type{});
+  });
 }
 template <class F>
 static int with_forms(const dsgd_ctx *ctx, int weight, F &&f) {
@@ -965,14 +973,9 @@ static int launch_rows(dsgd_ctx *ctx, const row_set &rows, const double *w, cons
   }
   if (!streamed) {
     // sw == nullptr without sample weights (an evaluation): every s_i is 1
-    if constexpr (kIcpt)
-      k_rows<kModel, kWeight, kScatter, kPreds, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
-          ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
-          ctx->sw_on ? ctx->sw.p : nullptr, w + ctx->dim);
-    else
-      k_rows<kModel, kWeight, kScatter, kPreds><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
-          ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
-          ctx->sw_on ? ctx->sw.p : nullptr);
+    k_rows<kModel, kWeight, kScatter, kPreds, kIcpt><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(
+        ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, rows.n, w, g, preds, ctx->cnt, ctx->cw_pos, ctx->cw_neg,
+        ctx->sw_on ? ctx->sw.p : nullptr, icpt_of(ctx, w));
     LAUNCHED();
   }
   if constexpr (kWeight == kClassWeighted) {
@@ -1231,18 +1234,11 @@ static int scores_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, doub
   int rc = request_weights(ctx, w, &wd, &cd, &nd);
   if (rc) return rc;
   const bool huber = model_of(ctx) == kModifiedHuber;
-  if (has_icpt(ctx)) {
-    const double *b = wd + ctx->dim;
-    if (prob && huber)
-      k_margins<true, true, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
-    else if (prob)
-      k_margins<true, false, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
-    else
-      k_margins<false, false, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds, b);
-  } else if (prob && huber)
-    k_margins<true, true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
-  else if (prob) k_margins<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
-  else k_margins<false><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds);
+  with_icpt(ctx, [&](auto ic) {
+    auto kernel = !prob ? k_margins<false, false, ic> : huber ? k_margins<true, true, ic> : k_margins<true, false, ic>;
+    kernel<<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, ctx->preds,
+                                                           icpt_of(ctx, wd));
+  });
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1299,18 +1295,12 @@ static int score_and_sort(dsgd_ctx *ctx, const double *w, const row_set &rows, b
   if (kW && ((rc = ctx->m_val.grow(ctx, n, 1024)) || (rc = ctx->m_valt.grow(ctx, n, 1024)))) return rc;
   CU(cudaMemsetAsync(ctx->m_cnt, 0, sizeof(unsigned long long) * kWords, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
-  if (has_icpt(ctx))   // the intercept form: the same arguments, every weight vector's intercept at [dim]
-    k_metrics_score<kWeight, true><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin,
-                                                                  n, wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
-                                                                  ctx->sw_on ? ctx->sw.p : nullptr,
-                                                                  kW ? ctx->m_val.p : nullptr, wd + ctx->dim);
-  else if constexpr (kW)
-    k_metrics_score<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
-                                                            wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
-                                                            ctx->sw_on ? ctx->sw.p : nullptr, ctx->m_val);
-  else
-    k_metrics_score<kWeight><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
-                                                            wd, ctx->m_keys, ctx->m_cnt);
+  with_icpt(ctx, [&](auto ic) {
+    k_metrics_score<kWeight, ic><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n,
+                                                                wd, ctx->m_keys, ctx->m_cnt, ctx->cw_pos, ctx->cw_neg,
+                                                                ctx->sw_on ? ctx->sw.p : nullptr, kW ? ctx->m_val.p : nullptr,
+                                                                icpt_of(ctx, wd));
+  });
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(s->h, ctx->m_cnt, sizeof s->h, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1589,7 +1579,7 @@ static int boot_sorted(dsgd_ctx *ctx, const double *w, const row_set &rows, cub:
   const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 positions per warp
   rc = with_model<kUnweighted>(ctx, [&](auto m, auto, auto ic) {
     k_boot_score<m, ic><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                      ctx->m_keys, ctx->b_tag, ctx->b_loss, wd + ctx->dim);
+                                                      ctx->m_keys, ctx->b_tag, ctx->b_loss, icpt_of(ctx, wd));
     LAUNCHED();
     return DSGD_OK;
   });
@@ -1829,20 +1819,13 @@ static int calibrate_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, d
     return rc;
   CU(cudaMemsetAsync(ctx->k_ctl, 0, sizeof(unsigned long long) * ctl_words, ctx->stream));
   const int sgrid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);
-  if (has_icpt(ctx))
-    k_calib_score<kW, true><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                            ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
-                                                            ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr,
-                                                            kW ? ctx->k_cw.p : nullptr, kW ? ctx->k_ctl + kCtlW : nullptr,
-                                                            wd + ctx->dim);
-  else if constexpr (kW)
-    k_calib_score<true><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                        ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
-                                                        ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr, ctx->k_cw,
-                                                        ctx->k_ctl + kCtlW);
-  else
-    k_calib_score<false><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
-                                                         ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt);
+  with_icpt(ctx, [&](auto ic) {
+    k_calib_score<kW, ic><<<sgrid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->label, rows.ids, rows.row_begin, n, wd,
+                                                          ctx->k_score, ctx->k_lab, ctx->k_ctl + kCtlCnt, ctx->cw_pos,
+                                                          ctx->cw_neg, ctx->sw_on ? ctx->sw.p : nullptr,
+                                                          kW ? ctx->k_cw.p : nullptr, kW ? ctx->k_ctl + kCtlW : nullptr,
+                                                          icpt_of(ctx, wd));
+  });
   LAUNCHED();
   CU(cudaGetLastError());
   unsigned long long cnt[kCalCntWords], wacc[kCalWWords];
@@ -1980,11 +1963,10 @@ extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, con
   const double *wd = nullptr, *cd = nullptr, *nd = nullptr;
   int rc = rows_list(ctx, samples, n, true, __func__, &rows);
   if (rc || (rc = request_weights(ctx, w, &wd, &cd, &nd))) return rc;
-  if (has_icpt(ctx))
-    k_calib_prob<true><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b,
-                                                                        ctx->preds, wd + ctx->dim);
-  else
-    k_calib_prob<<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b, ctx->preds);
+  with_icpt(ctx, [&](auto ic) {
+    k_calib_prob<ic><<<rows_grid(ctx, rows.n), 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, rows.ids, rows.n, wd, a, b,
+                                                                      ctx->preds, icpt_of(ctx, wd));
+  });
   LAUNCHED();
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1992,11 +1974,20 @@ extern "C" int dsgd_calibrated_probabilities(dsgd_ctx *ctx, const double *w, con
   return DSGD_OK;
 }
 
+static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn);
+// The dynamic shared memory of a kernel that reads a map of k >= 1 points: the map when it fits (the kernel's kSmem form),
+// else none (its kSmem = false form, which reads the map through L2)
+static size_t map_smem(int64_t k) { return k <= kIsoSmemPoints ? (size_t)k * 16 : 0; }
+// Launches kernel on 256-thread CTAs with smem bytes of dynamic shared memory, its limit raised to them first
+static cudaError_t launch_smem(const void *kernel, int grid, size_t smem, cudaStream_t stream, void **args) {
+  if (smem) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaLaunchKernel(kernel, dim3(grid), dim3(256), args, smem, stream);
+}
 // One quality pass over `rows`, at (a, b) or (kIso) at the map (X, Y): k_calib_eval, k_calib_eval_finish, the block read
 // back.  words_out = {rows used, NaN rows} and (kIso) the rows whose log-loss term is infinite.
-static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t k, const char *fn);
-template <class K>
-static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args);
 template <bool kIso>
 static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &rows, double a, double b, const double *X,
                                     const double *Y, int64_t k, int32_t n_bins, double *sums_out, int64_t *bin_rows,
@@ -2016,16 +2007,13 @@ static int calibration_quality_pass(dsgd_ctx *ctx, const double *w, const row_se
   const int8_t *label = ctx->label.p;
   const int32_t *ids = rows.ids;
   int64_t rb = rows.row_begin, rn = rows.n;
-  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  const double *icpt = icpt_of(ctx, wd);
   void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &icpt};
-  if (icpt && kIso)
-    CU(isotonic_launch(k_calib_eval<true, true, true>, k_calib_eval<true, false, true>, grid, k, ctx->stream, args));
-  else if (icpt)
-    CU(cudaLaunchKernel((const void *)k_calib_eval<false, false, true>, dim3(grid), dim3(256), args, 0, ctx->stream));
-  else if constexpr (kIso)
-    CU(isotonic_launch(k_calib_eval<true, true>, k_calib_eval<true, false>, grid, k, ctx->stream, args));
-  else
-    CU(cudaLaunchKernel((const void *)k_calib_eval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
+  const size_t smem = kIso ? map_smem(k) : 0;   // the kSmem form only at a map that fits
+  CU(with_icpt(ctx, [&](auto ic) {
+    auto kernel = smem ? k_calib_eval<kIso, kIso, ic> : k_calib_eval<kIso, false, ic>;
+    return launch_smem((const void *)kernel, grid, smem, ctx->stream, args);
+  }));
   LAUNCHED();
   k_calib_eval_finish<<<1, kCalMaxBins, 0, ctx->stream>>>(ctx->k_eval, n_bins);
   LAUNCHED();
@@ -2066,16 +2054,13 @@ static int weighted_quality_pass(dsgd_ctx *ctx, const double *w, const row_set &
   int64_t rb = rows.row_begin, rn = rows.n;
   double cwp = ctx->cw_pos, cwn = ctx->cw_neg;
   const double *swp = ctx->sw_on ? ctx->sw.p : nullptr;
-  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  const double *icpt = icpt_of(ctx, wd);
   void *args[] = {&rp16, &pairs, &label, &ids, &rb, &rn, &wd, &a, &b, &mx, &my, &ki, &nb, &blk, &cwp, &cwn, &swp, &icpt};
-  if (icpt && kIso)
-    CU(isotonic_launch(k_weval<true, true, true>, k_weval<true, false, true>, grid, k, ctx->stream, args));
-  else if (icpt)
-    CU(cudaLaunchKernel((const void *)k_weval<false, false, true>, dim3(grid), dim3(256), args, 0, ctx->stream));
-  else if constexpr (kIso)
-    CU(isotonic_launch(k_weval<true, true>, k_weval<true, false>, grid, k, ctx->stream, args));
-  else
-    CU(cudaLaunchKernel((const void *)k_weval<false, false>, dim3(grid), dim3(256), args, 0, ctx->stream));
+  const size_t smem = kIso ? map_smem(k) : 0;   // the kSmem form only at a map that fits
+  CU(with_icpt(ctx, [&](auto ic) {
+    auto kernel = smem ? k_weval<kIso, kIso, ic> : k_weval<kIso, false, ic>;
+    return launch_smem((const void *)kernel, grid, smem, ctx->stream, args);
+  }));
   LAUNCHED();
   CU(cudaGetLastError());
   std::vector<unsigned long long> h(kCwvWords);
@@ -2317,18 +2302,6 @@ static int isotonic_map(dsgd_ctx *ctx, const double *X, const double *Y, int64_t
   return DSGD_OK;
 }
 
-// Launches kernel<true> with the map in shared memory when it fits, else kernel<false>
-template <class K>
-static cudaError_t isotonic_launch(K k_smem, K k_l2, int grid, int64_t k, cudaStream_t stream, void **args) {
-  if (k <= kIsoSmemPoints) {
-    const size_t bytes = (size_t)k * 16;
-    cudaError_t e = cudaFuncSetAttribute((const void *)k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
-    return cudaLaunchKernel((const void *)k_smem, dim3(grid), dim3(256), args, bytes, stream);
-  }
-  return cudaLaunchKernel((const void *)k_l2, dim3(grid), dim3(256), args, 0, stream);
-}
-
 extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, const double *X,
                                            const double *Y, int64_t k, double *probs_out) {
   if (!ctx) return DSGD_ERR_INVALID;
@@ -2344,12 +2317,13 @@ extern "C" int dsgd_isotonic_probabilities(dsgd_ctx *ctx, const double *w, const
   const uint2 *pairs = ctx->pairs.p;
   const int32_t *ids = rows.ids;
   int64_t rn = rows.n;
-  const double *icpt = has_icpt(ctx) ? wd + ctx->dim : nullptr;
+  const double *icpt = icpt_of(ctx, wd);
   void *args[] = {&rp16, &pairs, &ids, &rn, &wd, &mx, &my, &ki, &out, &icpt};
-  if (icpt)
-    CU(isotonic_launch(k_iso_prob<true, true>, k_iso_prob<false, true>, rows_grid(ctx, rows.n), k, ctx->stream, args));
-  else
-    CU(isotonic_launch(k_iso_prob<true>, k_iso_prob<false>, rows_grid(ctx, rows.n), k, ctx->stream, args));
+  const size_t smem = map_smem(k);
+  CU(with_icpt(ctx, [&](auto ic) {
+    auto kernel = smem ? k_iso_prob<true, ic> : k_iso_prob<false, ic>;
+    return launch_smem((const void *)kernel, rows_grid(ctx, rows.n), smem, ctx->stream, args);
+  }));
   LAUNCHED();
   CU(cudaMemcpyAsync(probs_out, ctx->preds, sizeof(double) * (size_t)rows.n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));

@@ -3,10 +3,10 @@
 //
 // Replicate b of a request of n rows is the unweighted evaluation of its expanded list: position i repeated m_i(b) times,
 // m_i(b) the Poisson(1) draw of dsgd_bootstrap.h.  Scoring and sorting do not depend on b, so a bootstrap pass does them once:
-//   1. k_boot_score: the score of every position as k_metrics_score forms it (row_score: the same fold, the same intercept),
-//      its sort key ~score_key(s) (s = -(x . w): highest score first; a NaN score takes the largest key, ~0, and sorts last)
-//      and a 32-bit tag: the position, its confusion word (kMetTp .. kMetNegNone), its SVM hinge 1 - y p in {0, 1, 2} and
-//      a NaN bit.  Every model but the SVM also keeps the row's loss L (row_loss), by position.
+//   1. k_boot_score: the score of every position, taken by warp_scores as every scoring pass takes it (the same fold,
+//      the same intercept), its sort key ~score_key(s) (s = -(x . w): highest score first; a NaN score takes the largest
+//      key, ~0, and sorts last) and a 32-bit tag: the position, its confusion word (kMetTp .. kMetNegNone), its SVM hinge
+//      1 - y p in {0, 1, 2} and a NaN bit.  Every model but the SVM also keeps the row's loss L (row_loss), by position.
 //   2. cub::DeviceRadixSort::SortPairs of (key, tag) over all n positions.
 //   3. k_boot_arrange: in sorted order, the last element of every tie group of non-NaN scores records the index of its
 //      group's first element (-1 elsewhere), and L is gathered into sorted order.
@@ -38,8 +38,8 @@ enum BootWord : int { kBootSize = 8, kBootS = 9, kBootLoss = 10, kBootOutWords =
 static_assert(kMetTp == 0 && kMetNegNone == 5 && kMetU2 == 6 && kMetNan == 7, "a tag's confusion word is a word index");
 
 // ---------------------------------------------------------------------------------------------------
-// k_boot_score: a warp takes 32 consecutive positions at a time, as k_metrics_score does; every position's key and tag go to
-// its own slot, and (kModel != kSvm) loss[i] = L(y (x . w)), the per-row loss of k_rows.
+// k_boot_score: the positions taken by warp_scores; every position's key and tag go to its own slot, and (kModel != kSvm)
+// loss[i] = L(y (x . w)), the per-row loss of k_rows.
 // ---------------------------------------------------------------------------------------------------
 template <int kModel, bool kIcpt>
 __global__ void __launch_bounds__(256) k_boot_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
@@ -47,30 +47,16 @@ __global__ void __launch_bounds__(256) k_boot_score(const uint32_t *__restrict__
                                                     int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                     unsigned long long *__restrict__ keys, uint32_t *__restrict__ tags,
                                                     double *__restrict__ loss, const double *__restrict__ icpt) {
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
-      if (lane == j) dot_own = dot;
-    }
-    if (!mine) continue;
-    const int y = (int)label[r_own];
-    const bool pos = y > 0, nan = isnan(dot_own);
-    const int p = pred_of(dot_own);
+  warp_scores<kIcpt>(rp16, pairs, samples, row_begin, n, w, icpt, [&](int64_t i, int64_t r, double dot, bool mine) {
+    if (!mine) return;
+    const int y = (int)label[r];
+    const bool pos = y > 0, nan = isnan(dot);
+    const int p = pred_of(dot);
     const uint32_t word = pos ? (p == 1 ? kMetTp : p == -1 ? kMetFn : kMetPosNone) : (p == 1 ? kMetFp : p == -1 ? kMetTn : kMetNegNone);
-    keys[i] = nan ? ~0ull : ~score_key(-dot_own);
+    keys[i] = nan ? ~0ull : ~score_key(-dot);
     tags[i] = (uint32_t)i | word << 26 | (uint32_t)(1 - y * p) << 29 | (uint32_t)nan << 31;
-    if constexpr (kModel != kSvm) loss[i] = row_loss<kModel>((double)y * dot_own);
-  }
+    if constexpr (kModel != kSvm) loss[i] = row_loss<kModel>((double)y * dot);
+  });
 }
 
 // k_boot_arrange: gs[j] = the first index of element j's tie group when j ends a group of non-NaN scores, else -1; kLoss:
@@ -241,7 +227,7 @@ constexpr int kWbThreads = 256;
 enum WBootWord : int { kWbSize = 0, kWbNan = 1, kWbSums = 2, kWbLoss = kWbSums + 13, kWbOutWords = 16 };
 
 // k_wboot_arrange: gf[j] / gl[j] the first / last index of element j's tie group (-1: a NaN score), ec[j] = c of its row
-// (the expression of k_metrics_score<kSampleWeighted>; sw == nullptr: every s_i is 1) and ecl[j] = fl(c L), the term of
+// (row_weight) and ecl[j] = fl(c L), the term of
 // k_rows<..., kSampleWeighted, ...>: L the loss by position (kLoss) or the SVM's hinge 1 - y p from the tag.
 template <bool kLoss>
 __global__ void __launch_bounds__(256) k_wboot_arrange(const unsigned long long *__restrict__ keys,
@@ -259,7 +245,7 @@ __global__ void __launch_bounds__(256) k_wboot_arrange(const unsigned long long 
     gl[j] = nan ? -1 : (int)(j + key_lower_bound(keys + j, n - j, key + 1) - 1);
     const int64_t p = tag & kBootPosMask, r = samples ? (int64_t)samples[p] : row_begin + p;
     const bool pos = ((tag >> 26) & 7u) < 3u;
-    const double ci = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r]) : 1.0);
+    const double ci = row_weight(pos, w_pos, w_neg, sw, r);
     const double l = kLoss ? loss[p] : (double)((tag >> 29) & 3u);
     ec[j] = ci;
     ecl[j] = ci * l;

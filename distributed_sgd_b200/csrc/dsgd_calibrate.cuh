@@ -66,11 +66,11 @@ __device__ __forceinline__ double cal_value(const unsigned long long *words) {
 // out[i] = sigmoid(-(a f + b)) for row samples[i], f = x . w (kIcpt: the score with the intercept, row_score): the
 // calibrated probability under either model.  With
 // (a, b) = (1, 0) the argument is -f exactly, i.e. k_margins<true>'s value bit for bit.  One warp per row.
-template <bool kIcpt = false>
+template <bool kIcpt>
 __global__ void __launch_bounds__(256) k_calib_prob(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int32_t *__restrict__ samples, int64_t n,
                                                     const double *__restrict__ w, double a, double b,
-                                                    double *__restrict__ out, const double *__restrict__ icpt = nullptr) {
+                                                    double *__restrict__ out, const double *__restrict__ icpt) {
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
@@ -87,55 +87,39 @@ enum CalibWord : int { kCalPos = 0, kCalNeg = 1, kCalNan = 2, kCalCntWords = 4 }
 enum CalibWeightWord : int { kCalWPos = 0, kCalWNeg = kLossAccWords, kCalWNan = 2 * kLossAccWords, kCalWWords = 3 * kLossAccWords };
 
 // score[i] = x . w and lab[i] = the label of position i of the row set (samples == nullptr: rows [row_begin, row_begin + n)),
-// and the counts of non-NaN positives, non-NaN negatives and NaN rows.  A warp takes 32 consecutive positions at a time and
-// lane j keeps the j-th dot, as in k_metrics_score; the counts are flushed once per warp.
-// kW (the weighted fit, DESIGN.md §4.17): cw[i] = c_i = fl(w_y * s_i), the expression of k_metrics_score<kSampleWeighted>
-// (sw == nullptr: every s_i is 1), and R(c_i) added to the three CalibWeightWord sums at wacc; each warp adds its lanes'
-// carried limbs with shuffles (below 2^45 each) and flushes them once.
-template <bool kW, bool kIcpt = false>
+// and the counts of non-NaN positives, non-NaN negatives and NaN rows, the positions taken by warp_scores; the counts are
+// flushed once per warp.
+// kW (the weighted fit, DESIGN.md §4.17): cw[i] = c_i (row_weight), and R(c_i) added to the three CalibWeightWord sums at
+// wacc; each warp adds its lanes' carried limbs with shuffles (below 2^45 each) and flushes them once.
+template <bool kW, bool kIcpt>
 __global__ void __launch_bounds__(256) k_calib_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                      const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                      int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                      double *__restrict__ score, int8_t *__restrict__ lab,
-                                                     unsigned long long *__restrict__ cnt, double w_pos = 1.0,
-                                                     double w_neg = 1.0, const double *__restrict__ sw = nullptr,
-                                                     double *__restrict__ cw = nullptr,
-                                                     unsigned long long *__restrict__ wacc = nullptr,
-                                                     const double *__restrict__ icpt = nullptr) {
+                                                     unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
+                                                     const double *__restrict__ sw, double *__restrict__ cw,
+                                                     unsigned long long *__restrict__ wacc, const double *__restrict__ icpt) {
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned c_pos = 0, c_neg = 0, c_nan = 0;
   unsigned long long l_pos[kLossLimbs] = {0, 0, 0, 0, 0, 0}, l_neg[kLossLimbs] = {0, 0, 0, 0, 0, 0};
   unsigned long long l_nan[kLossLimbs] = {0, 0, 0, 0, 0, 0}, o_pos = 0, o_neg = 0, o_nan = 0;
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
-      if (lane == j) dot_own = dot;
+  warp_scores<kIcpt>(rp16, pairs, samples, row_begin, n, w, icpt, [&](int64_t i, int64_t r, double dot, bool mine) {
+    if (!mine) return;
+    const bool pos = label[r] > 0, nan = isnan(dot);
+    score[i] = dot;
+    lab[i] = pos ? 1 : -1;
+    c_nan += nan;
+    c_pos += pos && !nan;
+    c_neg += !pos && !nan;
+    if constexpr (kW) {
+      const double ci = row_weight(pos, w_pos, w_neg, sw, r);
+      cw[i] = ci;
+      if (nan) acc_add_local(l_nan, o_nan, ci);
+      else if (pos) acc_add_local(l_pos, o_pos, ci);
+      else acc_add_local(l_neg, o_neg, ci);
     }
-    if (mine) {
-      const bool pos = label[r_own] > 0, nan = isnan(dot_own);
-      score[i] = dot_own;
-      lab[i] = pos ? 1 : -1;
-      c_nan += nan;
-      c_pos += pos && !nan;
-      c_neg += !pos && !nan;
-      if constexpr (kW) {
-        const double ci = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r_own]) : 1.0);
-        cw[i] = ci;
-        if (nan) acc_add_local(l_nan, o_nan, ci);
-        else if (pos) acc_add_local(l_pos, o_pos, ci);
-        else acc_add_local(l_neg, o_neg, ci);
-      }
-    }
-  }
+  });
   c_pos = __reduce_add_sync(full, c_pos);
   c_neg = __reduce_add_sync(full, c_neg);
   c_nan = __reduce_add_sync(full, c_nan);

@@ -250,12 +250,12 @@ __device__ __forceinline__ void iso_stage(const double *__restrict__ X, const do
 }
 
 // out[i] = interp(-(x . w)) for row samples[i], x . w the row fold of dsgd_margins.  One warp per row.
-template <bool kSmem, bool kIcpt = false>
+template <bool kSmem, bool kIcpt>
 __global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                   const int32_t *__restrict__ samples, int64_t n,
                                                   const double *__restrict__ w, const double *__restrict__ X,
                                                   const double *__restrict__ Y, int k, double *__restrict__ out,
-                                                  const double *__restrict__ icpt = nullptr) {
+                                                  const double *__restrict__ icpt) {
   const double *xs, *ys;
   iso_stage<kSmem>(X, Y, k, xs, ys);
   const int lane = threadIdx.x & 31;
@@ -272,18 +272,18 @@ __global__ void __launch_bounds__(256) k_iso_prob(const uint32_t *__restrict__ r
 // bins into the CalibEvalWord block: bin = min(n_bins - 1, floor(p n_bins)).  At a sigmoid (kIso = false): z = a f + b,
 // p = sigmoid(-z) and the log-loss term softplus(+-z); a NaN z leaves the row out.  At the map (X, Y) (kIso): p = interp(s),
 // s = -f, and the term -log p (o = 1) or -log1p(-p) (o = 0); a NaN s leaves the row out, and a row whose term is infinite
-// (p = 0 with o = 1, p = 1 with o = 0) is counted in kCevInf and adds nothing to the sum.  Positions are taken as in
-// k_metrics_score.  The two sums go to register limbs; the bins to shared memory: rows and positives as integers, sum p as
+// (p = 0 with o = 1, p = 1 with o = 0) is counted in kCevInf and adds nothing to the sum.  Positions are taken by
+// warp_scores.  The two sums go to register limbs; the bins to shared memory: rows and positives as integers, sum p as
 // limb words added with shared u64 atomics (p <= 1: each limb adds at most 2^40, so a CTA's words hold 2^24 rows without a
 // wrap, and a grid of 8 CTAs per SM leaves a CTA fewer than that for any 32-bit row count).  The CTA propagates each bin's
 // carries and adds its words to the block with REDs.
-template <bool kIso, bool kSmem, bool kIcpt = false>
+template <bool kIso, bool kSmem, bool kIcpt>
 __global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                     int64_t row_begin, int64_t n, const double *__restrict__ w, double a,
                                                     double b, const double *__restrict__ X, const double *__restrict__ Y,
                                                     int k, int n_bins, unsigned long long *__restrict__ blk,
-                                                    const double *__restrict__ icpt = nullptr) {
+                                                    const double *__restrict__ icpt) {
   __shared__ unsigned long long s_rows[kCalMaxBins], s_pos[kCalMaxBins], s_lim[kCalMaxBins][kLossLimbs];
   const double *xs, *ys;
   iso_stage<kSmem>(X, Y, k, xs, ys);
@@ -296,25 +296,13 @@ __global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__
     for (int q = 0; q < kLossLimbs; ++q) s_lim[i][q] = 0ull;
   }
   __syncthreads();
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned long long lb[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ll[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_b = 0, ovf_l = 0;
   unsigned c_rows = 0, c_nan = 0, c_inf = 0;
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
-      if (lane == j) dot_own = dot;
-    }
-    if (!mine) continue;
-    const double z = kIso ? -dot_own : a * dot_own + b;   // kIso: the score s
-    if (isnan(z)) { ++c_nan; continue; }
-    const bool pos = label[r_own] > 0;
+  warp_scores<kIcpt>(rp16, pairs, samples, row_begin, n, w, icpt, [&](int64_t, int64_t r, double dot, bool mine) {
+    if (!mine) return;
+    const double z = kIso ? -dot : a * dot + b;   // kIso: the score s
+    if (isnan(z)) { ++c_nan; return; }
+    const bool pos = label[r] > 0;
     const double pr = kIso ? iso_interp(z, xs, ys, k) : sigmoid(-z), o = pos ? 1.0 : 0.0, dlt = pr - o;
     ++c_rows;
     acc_add_local(lb, ovf_b, dlt * dlt);
@@ -328,7 +316,7 @@ __global__ void __launch_bounds__(256) k_calib_eval(const uint32_t *__restrict__
     acc_cut(pr, [&](int q, double limb) {
       if (limb != 0.0) atomicAdd(&s_lim[bin][q], (unsigned long long)(long long)limb);
     });
-  }
+  });
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ovf_b += __shfl_xor_sync(full, ovf_b, o);
@@ -521,8 +509,8 @@ struct IsoWeights {
 
 // ---- the weighted quality pass (dsgd_eval_*weighted_calibration, dsgd_eval_*weighted_isotonic_calibration) -----------
 // kIso: p = interp(s) at the map (X, Y) and the log-loss term -log p or -log1p(-p); else p = sigmoid(-z), z = a f + b, and
-// the term softplus(+-z); each as k_calib_eval<kIso, kSmem>.  c_i = fl(w_y * s_i) as in k_calib_score<true>.  A row with
-// R(c) = 0 is counted in kCwvRows and adds nothing else.  The sums add R(fl(c (p - o)^2)), R(fl(c l)) over the finite
+// the term softplus(+-z); each as k_calib_eval<kIso, kSmem>, its positions taken by warp_scores.  c_i is row_weight.  A
+// row with R(c) = 0 is counted in kCwvRows and adds nothing else.  The sums add R(fl(c (p - o)^2)), R(fl(c l)) over the finite
 // terms, R(c) over the rows used and R(c) over the rows whose term is infinite (counted in kCwvInf too); bin k adds R(c),
 // R(c) of the positives and R(fl(c p)) to its three limb blocks in shared memory.  A bin value of 2^52 or more is counted
 // in the bin's overflow word; the integer part of a value is split at 2^40 between limbs 4 and 5, so every shared word
@@ -553,13 +541,13 @@ __device__ __forceinline__ void cal_bin_add(unsigned long long *lim, unsigned lo
     }
   });
 }
-template <bool kIso, bool kSmem, bool kIcpt = false>
+template <bool kIso, bool kSmem, bool kIcpt>
 __global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                int64_t row_begin, int64_t n, const double *__restrict__ w, double a, double b,
                                                const double *__restrict__ X, const double *__restrict__ Y, int k, int n_bins,
                                                unsigned long long *__restrict__ blk, double w_pos, double w_neg,
-                                               const double *__restrict__ sw, const double *__restrict__ icpt = nullptr) {
+                                               const double *__restrict__ sw, const double *__restrict__ icpt) {
   __shared__ unsigned long long s_bins[kCalMaxBins * kCwvBinStride];
   const double *xs = nullptr, *ys = nullptr;
   if constexpr (kIso) iso_stage<kSmem>(X, Y, k, xs, ys);
@@ -567,29 +555,17 @@ __global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16
   const int lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < kCalMaxBins * kCwvBinStride; i += blockDim.x) s_bins[i] = 0ull;
   __syncthreads();
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned long long lb[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ll[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_b = 0, ovf_l = 0;
   unsigned long long lw[kLossLimbs] = {0, 0, 0, 0, 0, 0}, li[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_w = 0, ovf_i = 0;
   unsigned c_rows = 0, c_nan = 0, c_inf = 0;
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
-      if (lane == j) dot_own = dot;
-    }
-    if (!mine) continue;
-    const double z = kIso ? -dot_own : a * dot_own + b;   // kIso: the score s
-    if (isnan(z)) { ++c_nan; continue; }
+  warp_scores<kIcpt>(rp16, pairs, samples, row_begin, n, w, icpt, [&](int64_t, int64_t r, double dot, bool mine) {
+    if (!mine) return;
+    const double z = kIso ? -dot : a * dot + b;   // kIso: the score s
+    if (isnan(z)) { ++c_nan; return; }
     ++c_rows;
-    const bool pos = label[r_own] > 0;
-    const double c = (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r_own]) : 1.0);
-    if (rint(c * 0x1p160) == 0.0) continue;   // R(c) = 0: the row adds exactly 0 to every sum
+    const bool pos = label[r] > 0;
+    const double c = row_weight(pos, w_pos, w_neg, sw, r);
+    if (rint(c * 0x1p160) == 0.0) return;   // R(c) = 0: the row adds exactly 0 to every sum
     const double pr = kIso ? iso_interp(z, xs, ys, k) : sigmoid(-z), o = pos ? 1.0 : 0.0, dlt = pr - o;
     const double term = kIso ? (pos ? -log(pr) : -log1p(-pr)) : softplus(pos ? z : -z);
     acc_add_local(lb, ovf_b, c * (dlt * dlt));
@@ -606,7 +582,7 @@ __global__ void __launch_bounds__(256) k_weval(const uint32_t *__restrict__ rp16
     cal_bin_add(bl, bo, c);
     if (pos) cal_bin_add(bl + kLossLimbs, bo, c);
     cal_bin_add(bl + 2 * kLossLimbs, bo, c * pr);
-  }
+  });
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ovf_b += __shfl_xor_sync(full, ovf_b, o);

@@ -49,6 +49,42 @@ __device__ __forceinline__ double row_score(const uint32_t *__restrict__ rp16, c
   return dot;
 }
 
+// The positions of an evaluation pass over rows samples[0..n) (samples == nullptr: rows [row_begin, row_begin + n)).  A
+// warp takes 32 consecutive positions at a time: lane j resolves position j to its row, the warp scores the 32 rows one
+// after the other (row_score) and lane j keeps the j-th score.  Then f(i, r, s, mine) runs on every lane of the warp, so
+// that f may use warp-wide intrinsics: position i, its row r and score s; mine is false past n, where r = 0 and s = 0.
+// Every pass that scores rows in groups takes them here, so a curve, a calibration, a quality pass and a bootstrap rank
+// exactly the scores of dsgd_margins.
+template <bool kIcpt, class F>
+__device__ __forceinline__ void warp_scores(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                            const int32_t *__restrict__ samples, int64_t row_begin, int64_t n,
+                                            const double *__restrict__ w, const double *__restrict__ icpt, F f) {
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i = g + lane;
+    const bool mine = i < n;
+    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    double dot_own = 0.0;
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
+      if (lane == j) dot_own = dot;
+    }
+    f(i, r_own, dot_own, mine);
+  }
+}
+
+// c_r = fl(w_y * s_r), the weight of row r in a weighted evaluation: its class weight (w_pos or w_neg by its label) times
+// its sample weight (sw == nullptr: every s_r is 1).  The training side forms the same value in k_rows<..., kSampleWeighted,
+// ...> and k_sync_persistent, each with its own expression.
+__device__ __forceinline__ double row_weight(bool pos, double w_pos, double w_neg, const double *__restrict__ sw, int64_t r) {
+  return (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r]) : 1.0);
+}
+
 // Order-preserving key of a score: +0 and -0 are one key, and key(a) < key(b) exactly when a < b (for non-NaN scores)
 __device__ __forceinline__ unsigned long long score_key(double s) {
   const unsigned long long b = (unsigned long long)__double_as_longlong(s == 0.0 ? 0.0 : s);
@@ -66,11 +102,11 @@ __device__ __forceinline__ double huber_prob(double dot) {
   return (m + 1.0) / 2.0;
 }
 // kIcpt (an intercept ctx): the score is fl(x . w + filt(*icpt)), as in k_rows<..., kIcpt>; otherwise icpt is not read.
-template <bool kProb, bool kHuber = false, bool kIcpt = false>
+template <bool kProb, bool kHuber, bool kIcpt>
 __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                  const int32_t *__restrict__ samples, int64_t n,
                                                  const double *__restrict__ w, double *__restrict__ out,
-                                                 const double *__restrict__ icpt = nullptr) {
+                                                 const double *__restrict__ icpt) {
   const int lane = threadIdx.x & 31;
   const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
@@ -85,46 +121,32 @@ __global__ void __launch_bounds__(256) k_margins(const uint32_t *__restrict__ rp
 
 // ---------------------------------------------------------------------------------------------------
 // k_metrics_score: the scoring step of a metrics pass over rows samples[0..n) (samples == nullptr: rows [row_begin,
-// row_begin + n)).  A warp takes 32 consecutive positions at a time: lane j loads the id and label of position j, the warp
-// computes the 32 dots one after the other and lane j keeps the j-th.  Each lane counts its rows in registers; the counts
-// are flushed once per warp.  The keys go to keys[0..) (y = +1) and keys[..n) backwards (y = -1), their slots claimed with
-// one atomic per warp and class for 32 rows.
-// kSampleWeighted (the weighted curve pass): each key's row weight c_i = fl(w_y * s_i), the expression of
-// k_rows<..., kSampleWeighted, ...> (sw == nullptr: every s_i is 1), goes to vals[] in the key's slot, and the NaN rows add
-// R(c_i) to the kMetNanPos / kMetNanNeg limbs (each lane flushes its own once).  The weighted confusion sums need nothing
-// more: pred follows the sign of s, so they are read from the runs' prefix sums at the key of +0 (k_curve_sum).
+// row_begin + n)), its positions taken by warp_scores.  Each lane counts its rows in registers; the counts are flushed once
+// per warp.  The keys go to keys[0..) (y = +1) and keys[..n) backwards (y = -1), their slots claimed with one atomic per
+// warp and class for 32 rows.
+// kSampleWeighted (the weighted curve pass): each key's row weight c_i (row_weight) goes to vals[] in the key's slot, and
+// the NaN rows add R(c_i) to the kMetNanPos / kMetNanNeg limbs (each lane flushes its own once).  The weighted confusion
+// sums need nothing more: pred follows the sign of s, so they are read from the runs' prefix sums at the key of +0
+// (k_curve_sum).
 // ---------------------------------------------------------------------------------------------------
-template <int kWeight, bool kIcpt = false>
+template <int kWeight, bool kIcpt>
 __global__ void __launch_bounds__(256) k_metrics_score(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                        const int8_t *__restrict__ label, const int32_t *__restrict__ samples,
                                                        int64_t row_begin, int64_t n, const double *__restrict__ w,
                                                        unsigned long long *__restrict__ keys,
-                                                       unsigned long long *__restrict__ cnt, double w_pos = 1.0,
-                                                       double w_neg = 1.0, const double *__restrict__ sw = nullptr,
-                                                       double *__restrict__ vals = nullptr,
-                                                       const double *__restrict__ icpt = nullptr) {
+                                                       unsigned long long *__restrict__ cnt, double w_pos, double w_neg,
+                                                       const double *__restrict__ sw, double *__restrict__ vals,
+                                                       const double *__restrict__ icpt) {
   static_assert(kWeight == kUnweighted || kWeight == kSampleWeighted, "a metrics pass counts rows or weighs them by c_i");
   constexpr bool kW = kWeight == kSampleWeighted;
   unsigned long long lim_np[kLossLimbs] = {0, 0, 0, 0, 0, 0}, lim_nn[kLossLimbs] = {0, 0, 0, 0, 0, 0}, ovf_np = 0, ovf_nn = 0;
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
-  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   unsigned c[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // this lane's rows, by MetricWord (kMetU2 unused)
-  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
-    const int64_t i = g + lane;
-    const bool mine = i < n;
-    const int64_t r_own = mine ? (samples ? (int64_t)samples[i] : row_begin + i) : 0;
-    const int m = (int)(n - g < 32 ? n - g : 32);
-    double dot_own = 0.0;
-    for (int j = 0; j < m; ++j) {
-      const int64_t r = __shfl_sync(full, r_own, j);
-      const double dot = row_score<kIcpt>(rp16, pairs, w, r, lane, icpt);
-      if (lane == j) dot_own = dot;
-    }
-    const bool pos = mine && label[r_own] > 0, neg = mine && !pos;
-    const bool nan = mine && isnan(dot_own);
-    const int p = pred_of(dot_own);   // dsgd_forward's prediction; NaN -> 0
+  warp_scores<kIcpt>(rp16, pairs, samples, row_begin, n, w, icpt, [&](int64_t, int64_t r, double dot, bool mine) {
+    const bool pos = mine && label[r] > 0, neg = mine && !pos;
+    const bool nan = mine && isnan(dot);
+    const int p = pred_of(dot);   // dsgd_forward's prediction; NaN -> 0
     c[kMetTp] += pos && p == 1;
     c[kMetFn] += pos && p == -1;
     c[kMetPosNone] += pos && p == 0;
@@ -142,16 +164,16 @@ __global__ void __launch_bounds__(256) k_metrics_score(const uint32_t *__restric
     base_p = __shfl_sync(full, base_p, 0);
     base_n = __shfl_sync(full, base_n, 0);
     const unsigned below = (1u << lane) - 1u;
-    if (put_pos) keys[base_p + __popc(bp & below)] = score_key(-dot_own);
-    if (put_neg) keys[n - 1 - (int64_t)(base_n + __popc(bn & below))] = score_key(-dot_own);
+    if (put_pos) keys[base_p + __popc(bp & below)] = score_key(-dot);
+    if (put_neg) keys[n - 1 - (int64_t)(base_n + __popc(bn & below))] = score_key(-dot);
     if constexpr (kW) {
-      const double ci = mine ? (pos ? w_pos : w_neg) * (sw ? __ldg(&sw[r_own]) : 1.0) : 0.0;
+      const double ci = mine ? row_weight(pos, w_pos, w_neg, sw, r) : 0.0;
       if (put_pos) vals[base_p + __popc(bp & below)] = ci;
       if (put_neg) vals[n - 1 - (int64_t)(base_n + __popc(bn & below))] = ci;
       if (nan && pos) acc_add_local(lim_np, ovf_np, ci);
       if (nan && neg) acc_add_local(lim_nn, ovf_nn, ci);
     }
-  }
+  });
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     if (k == kMetU2) continue;

@@ -117,11 +117,14 @@ def row_losses(model, margins, labels) -> np.ndarray:
 
 
 def _loss_sum(model, losses, m) -> float:
-    if any(k > 0 and not (0.0 <= l < 2.0 ** 52) for l, k in zip(losses, m)):
+    """The replicate's loss sum over positions drawn at least once: a position with m = 0 adds nothing, whatever its loss
+    (NaN included), as on the device."""
+    drawn = [(l, int(k)) for l, k in zip(losses, m) if k > 0]
+    if any(not (0.0 <= l < 2.0 ** 52) for l, _ in drawn):
         return float("nan")
     if model in (None, "svm"):
-        return float(sum(int(l) * int(k) for l, k in zip(losses, m)))
-    return float(sum((_r(l) * int(k) for l, k in zip(losses, m)), Fraction(0)))
+        return float(sum(int(l) * k for l, k in drawn))
+    return float(sum((_r(l) * k for l, k in drawn), Fraction(0)))
 
 
 def replicate(orc, model, w, ids, m, margins) -> Replicate:
