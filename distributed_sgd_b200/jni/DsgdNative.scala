@@ -18,8 +18,8 @@ object DsgdNative {
   final val FlagModifiedHuber = 8
   // FlagIntercept (with any one model flag, sync mode only): an unregularised intercept.  Every weight array in or out --
   // setWeights, getWeights, each request's w, gradient's grad (the intercept's gradient last), averageWeights -- is then
-  // dim + 1 long, the intercept last; d stays dim long.  The shim's own length checks (weightsL1, the weighted evaluations
-  // and curves) take dim + 1 on such a ctx.
+  // dim + 1 long, the intercept last; d stays dim long.  The shim checks every array against the length the library
+  // reads or writes (a request's w: null or exactly that length), and returns DSGD_ERR_INVALID before the call otherwise.
   final val FlagIntercept = 16
   @native def create(device: Int, dim: Int, lambda: Double, rank: Int, world: Int, flags: Int): Long
   @native def destroy(ctx: Long): Int

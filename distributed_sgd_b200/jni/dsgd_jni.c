@@ -10,10 +10,14 @@
  * contexts driven from several JVM threads it can deadlock: rank A's kernel waits for rank B's launch while B's thread
  * waits for the collector that A's critical region holds off.)  A NULL array is passed on as NULL / length 0.
  *
- * tests/test_abi_surface.py compiles this file against a minimal stand-in jni.h (tests/jni_mock/) -- a syntax and type
- * check against include/dsgd.h, not a run under a JVM -- and checks that the facade covers the header. */
+ * The library reads and writes the full length the header names through raw pointers, so every array is checked against
+ * that length before the call: a wrong length is DSGD_ERR_INVALID, with nothing launched and nothing copied back.
+ *
+ * tests/test_abi_surface.py compiles this file against a minimal stand-in jni.h (tests/jni_mock/) and checks that the
+ * facade covers the header; tests/test_gpu_jni.py runs it against the library through a stand-in JNIEnv. */
 #ifdef DSGD_HAVE_JNI
 #include <jni.h>
+#include <pthread.h>
 #include <stddef.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -53,6 +57,71 @@ DEF_BUF(Float, jfloat, float)
 DEF_BUF(Double, jdouble, double)
 DEF_BUF(Byte, jbyte, int8_t)
 
+/* rc, or else DSGD_ERR_NOMEM when a copy failed, or else DSGD_ERR_INVALID when an array is too short */
+static int checked(int rc, int bad, int invalid) {
+  return rc != DSGD_OK ? rc : bad ? DSGD_ERR_NOMEM : invalid ? DSGD_ERR_INVALID : DSGD_OK;
+}
+/* a non-null array shorter than n */
+static int short_of(const buf_t *b, jlong n) { return b->p && b->n < n; }
+
+/* The length of a weight vector of the ctx: dim, or dim + 1 on a ctx created with DSGD_FLAG_INTERCEPT, which dsgd_info
+ * names.  dsgd_info rewrites a string the ctx owns, and getWeights may run on several threads at once while the async loop
+ * runs (include/dsgd.h, Threading); the shim is the only caller of dsgd_info and holds info_lock from the call until it has
+ * read the string. */
+static pthread_mutex_t info_lock = PTHREAD_MUTEX_INITIALIZER;
+static int weight_len(jlong h, int32_t *n) {
+  int rc = dsgd_dim(CTX(h), n);
+  if (rc != DSGD_OK) return rc;
+  pthread_mutex_lock(&info_lock);
+  if (strstr(dsgd_info(CTX(h)), "\"intercept\": true")) ++*n;
+  pthread_mutex_unlock(&info_lock);
+  return rc;
+}
+enum { DIM, WEIGHTS };         /* what an array's length is measured against: dim, or the weight length */
+enum { AT_LEAST, EXACTLY };
+/* DSGD_OK when b is null or holds exactly / at least the ctx's dim or weight length values */
+static int sized(jlong h, const buf_t *b, int what, int how) {
+  int32_t n = 0;
+  int rc = b->bad ? DSGD_ERR_NOMEM : !b->p ? DSGD_OK : what == WEIGHTS ? weight_len(h, &n) : dsgd_dim(CTX(h), &n);
+  return checked(rc, 0, b->p && (how == EXACTLY ? b->n != n : b->n < n));
+}
+
+/* The rows a request names: a range [rowBegin, rowEnd), positions [posBegin, posEnd) of the sample drawn on the device
+ * from the range with `key`, or a list of row ids (copied into `ids` when the request opens). */
+typedef struct {
+  enum { RANGE, DRAWN, LIST } form;
+  jlong rowBegin, rowEnd, key, posBegin, posEnd;
+  jintArray samples;
+  buf_t ids;
+} rows_t;
+static rows_t range_rows(jlong rowBegin, jlong rowEnd) { return (rows_t){RANGE, rowBegin, rowEnd, 0, 0, 0, NULL, {0}}; }
+static rows_t drawn_rows(jlong rowBegin, jlong rowEnd, jlong key, jlong posBegin, jlong posEnd) {
+  return (rows_t){DRAWN, rowBegin, rowEnd, key, posBegin, posEnd, NULL, {0}};
+}
+static rows_t list_rows(jintArray samples) { return (rows_t){LIST, 0, 0, 0, 0, 0, samples, {0}}; }
+/* the rows of a call that takes weights and names no rows (setWeights, weightsL1) */
+static rows_t no_rows(void) { return range_rows(0, 0); }
+
+/* One request: the weights w (null: the resident ones, else exactly the weight length) and its rows, copied in. */
+typedef struct { buf_t w; rows_t r; } req_t;
+static int req_open(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, req_t *q) {
+  q->w = in_Double(env, w);
+  q->r = r;
+  q->r.ids = in_Int(env, r.samples);
+  return checked(sized(h, &q->w, WEIGHTS, EXACTLY), q->r.ids.bad, 0);
+}
+static void req_close(req_t *q) { free(q->w.p); free(q->r.ids.p); }
+/* the number of rows a request names */
+static jlong rows_n(const req_t *q) {
+  return q->r.form == RANGE ? q->r.rowEnd - q->r.rowBegin : q->r.form == DRAWN ? q->r.posEnd - q->r.posBegin : q->r.ids.n;
+}
+/* the call of one evaluation family in the request's row form: fn, fn_sampled or fn_samples, the outputs after the rows */
+#define ROW_CALL(h, q, fn, fn_sampled, fn_samples, ...)                                                                   \
+  ((q).r.form == RANGE   ? fn(CTX(h), (q).w.p, (q).r.rowBegin, (q).r.rowEnd, __VA_ARGS__)                                \
+   : (q).r.form == DRAWN ? fn_sampled(CTX(h), (q).w.p, (q).r.rowBegin, (q).r.rowEnd, (uint64_t)(q).r.key, (q).r.posBegin, \
+                                      (q).r.posEnd, __VA_ARGS__)                                                          \
+                         : fn_samples(CTX(h), (q).w.p, (q).r.ids.p, (q).r.ids.n, __VA_ARGS__))
+
 /* ---- lifecycle ---- */
 JNIEXPORT jlong JNICALL Java_epfl_distributed_nativ_DsgdNative_00024_create(JNIEnv *env, jobject self, jint device, jint dim,
                                                                           jdouble lambda, jint rank, jint world, jint flags) {
@@ -68,615 +137,406 @@ JNIEXPORT jstring JNICALL Java_epfl_distributed_nativ_DsgdNative_00024_lastError
 /* ---- data / model ---- */
 FN(loadCsr)(JNIEnv *env, jobject self, jlong h, jlongArray rowPtr, jintArray col, jfloatArray value, jbyteArray label) {
   buf_t rp = in_Long(env, rowPtr), c = in_Int(env, col), v = in_Float(env, value), l = in_Byte(env, label);
-  int rc = DSGD_ERR_NOMEM;                               /* Dataset.rcv1 rows as CSR (utils/Dataset.scala:23-47) */
-  if (!(rp.bad | c.bad | v.bad | l.bad))
-    rc = rp.n < 1 ? DSGD_ERR_INVALID : dsgd_load_csr(CTX(h), rp.n - 1, c.n, rp.p, c.p, v.p, l.p);
+  int rc = checked(DSGD_OK, rp.bad | c.bad | v.bad | l.bad, rp.n < 1 || l.n != rp.n - 1 || v.n != c.n);
+  if (rc == DSGD_OK) rc = dsgd_load_csr(CTX(h), rp.n - 1, c.n, rp.p, c.p, v.p, l.p);   /* Dataset.rcv1 rows as CSR (utils/Dataset.scala:23-47) */
   free(rp.p); free(c.p); free(v.p); free(l.p);
   return rc;
 }
 FN(setDimSparsity)(JNIEnv *env, jobject self, jlong h, jdoubleArray d) {
   buf_t b = in_Double(env, d);
-  int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_set_dim_sparsity(CTX(h), b.p);            /* SparseSVM.dimSparsity */
+  int rc = sized(h, &b, DIM, EXACTLY);
+  if (rc == DSGD_OK) rc = dsgd_set_dim_sparsity(CTX(h), b.p);            /* SparseSVM.dimSparsity */
   free(b.p);
   return rc;
 }
 FN(computeDimSparsity)(JNIEnv *env, jobject self, jlong h, jlong nTrain, jdoubleArray out) {
   buf_t o = out_Double(env, out);
-  int rc = o.bad ? DSGD_ERR_NOMEM : dsgd_compute_dim_sparsity(CTX(h), nTrain, o.p); /* Main.scala:54-65 */
+  int rc = sized(h, &o, DIM, AT_LEAST);
+  if (rc == DSGD_OK) rc = dsgd_compute_dim_sparsity(CTX(h), nTrain, o.p); /* Main.scala:54-65 */
   back_Double(env, out, o, rc);
   return rc;
 }
 FN(setWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray w) {
-  buf_t b = in_Double(env, w);
-  int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_set_weights(CTX(h), b.p);
-  free(b.p);
+  req_t q;
+  int rc = req_open(env, h, w, no_rows(), &q);
+  if (rc == DSGD_OK) rc = dsgd_set_weights(CTX(h), q.w.p);
+  req_close(&q);
   return rc;
 }
 FN(getWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray w) {
   buf_t o = out_Double(env, w);
-  int rc = o.bad ? DSGD_ERR_NOMEM : dsgd_get_weights(CTX(h), o.p);
+  int rc = sized(h, &o, WEIGHTS, AT_LEAST);
+  if (rc == DSGD_OK) rc = dsgd_get_weights(CTX(h), o.p);
   back_Double(env, w, o, rc);
   return rc;
 }
 
 /* ---- requests ---- */
+/* the calls that give one double per listed row; out at least as long as samples */
+typedef int (*per_row_fn)(dsgd_ctx *, const double *, const int32_t *, int64_t, double *);
+static int per_row(JNIEnv *env, jlong h, jdoubleArray w, jintArray samples, jdoubleArray out, per_row_fn fn) {
+  req_t q;
+  buf_t o = out_Double(env, out);
+  int rc = req_open(env, h, w, list_rows(samples), &q);
+  rc = checked(rc, o.bad, o.n < q.r.ids.n);
+  if (rc == DSGD_OK) rc = fn(CTX(h), q.w.p, q.r.ids.p, q.r.ids.n, o.p);
+  back_Double(env, out, o, rc);
+  req_close(&q);
+  return rc;
+}
 FN(gradient)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray grad) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bg = out_Double(env, grad);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bg.bad)) rc = dsgd_gradient(CTX(h), bw.p, bs.p, bs.n, bg.p, NULL);  /* core/Slave.scala:142-157 */
-  back_Double(env, grad, bg, rc);
-  free(bw.p); free(bs.p);
+  req_t q;
+  buf_t g = out_Double(env, grad);
+  int rc = req_open(env, h, w, list_rows(samples), &q);
+  if (rc == DSGD_OK) rc = sized(h, &g, WEIGHTS, AT_LEAST);
+  if (rc == DSGD_OK) rc = dsgd_gradient(CTX(h), q.w.p, q.r.ids.p, q.r.ids.n, g.p, NULL);  /* core/Slave.scala:142-157 */
+  back_Double(env, grad, g, rc);
+  req_close(&q);
   return rc;
 }
 FN(forward)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray preds) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bp = out_Double(env, preds);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bp.bad)) rc = dsgd_forward(CTX(h), bw.p, bs.p, bs.n, bp.p);          /* core/Slave.scala:129-140 */
-  back_Double(env, preds, bp, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return per_row(env, h, w, samples, preds, dsgd_forward);                                 /* core/Slave.scala:129-140 */
 }
 FN(eval)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray lossAcc) {
-  buf_t bw = in_Double(env, w), bo = out_Double(env, lossAcc);          /* lossAcc(0) = loss, lossAcc(1) = accuracy */
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bo.bad))
-    rc = bo.n < 2 ? DSGD_ERR_INVALID
-                  : dsgd_eval(CTX(h), bw.p, rowBegin, rowEnd, (double *)bo.p, (double *)bo.p + 1);  /* core/Master.scala:100-107 */
-  back_Double(env, lossAcc, bo, rc);
-  free(bw.p);
+  req_t q;
+  buf_t o = out_Double(env, lossAcc);                                   /* lossAcc(0) = loss, lossAcc(1) = accuracy */
+  int rc = checked(req_open(env, h, w, range_rows(rowBegin, rowEnd), &q), o.bad, o.n < 2);
+  if (rc == DSGD_OK) rc = dsgd_eval(CTX(h), q.w.p, rowBegin, rowEnd, (double *)o.p, (double *)o.p + 1);  /* core/Master.scala:100-107 */
+  back_Double(env, lossAcc, o, rc);
+  req_close(&q);
+  return rc;
+}
+
+/* exact shardable form: hingeCorrect(0) = hinge sum, (1) = #correct; the sampled form is core/Master.scala:109-118 with
+ * the sample drawn on the device (positions [posBegin, posEnd)), the list form the row ids the JVM drew with its own Random */
+static int req_counts(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray hingeCorrect, jdoubleArray normSquared) {
+  req_t q;
+  buf_t c = out_Long(env, hingeCorrect), n = out_Double(env, normSquared);
+  int rc = checked(req_open(env, h, w, r, &q), c.bad | n.bad, c.n < 2 || n.n < 1);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_counts, dsgd_eval_sampled_counts, dsgd_eval_samples_counts, (int64_t *)c.p,
+                  (int64_t *)c.p + 1, n.p);
+  back_Long(env, hingeCorrect, c, rc);
+  back_Double(env, normSquared, n, rc);
+  req_close(&q);
   return rc;
 }
 FN(evalCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray hingeCorrect,
                jdoubleArray normSquared) {
-  buf_t bw = in_Double(env, w), bc = out_Long(env, hingeCorrect), bn = out_Double(env, normSquared);
-  int rc = DSGD_ERR_NOMEM;               /* exact shardable form: hingeCorrect(0) = hinge sum, (1) = #correct */
-  if (!(bw.bad | bc.bad | bn.bad))
-    rc = (bc.n < 2 || bn.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_counts(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)bc.p, (int64_t *)bc.p + 1, bn.p);
-  back_Long(env, hingeCorrect, bc, rc);
-  back_Double(env, normSquared, bn, rc);
-  free(bw.p);
-  return rc;
+  return req_counts(env, h, w, range_rows(rowBegin, rowEnd), hingeCorrect, normSquared);
 }
 FN(evalSampledCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                       jlong posBegin, jlong posEnd, jlongArray hingeCorrect, jdoubleArray normSquared) {
-  buf_t bw = in_Double(env, w), bc = out_Long(env, hingeCorrect), bn = out_Double(env, normSquared);
-  int rc = DSGD_ERR_NOMEM;               /* core/Master.scala:109-118, sample drawn on the device: positions [posBegin, posEnd) */
-  if (!(bw.bad | bc.bad | bn.bad))
-    rc = (bc.n < 2 || bn.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_sampled_counts(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                           (int64_t *)bc.p, (int64_t *)bc.p + 1, bn.p);
-  back_Long(env, hingeCorrect, bc, rc);
-  back_Double(env, normSquared, bn, rc);
-  free(bw.p);
-  return rc;
+  return req_counts(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), hingeCorrect, normSquared);
 }
 FN(evalSamplesCounts)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray hingeCorrect,
                       jdoubleArray normSquared) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bc = out_Long(env, hingeCorrect), bn = out_Double(env, normSquared);
-  int rc = DSGD_ERR_NOMEM;               /* the same counters over row ids the JVM drew with its own Random */
-  if (!(bw.bad | bs.bad | bc.bad | bn.bad))
-    rc = (bc.n < 2 || bn.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_samples_counts(CTX(h), bw.p, bs.p, bs.n, (int64_t *)bc.p, (int64_t *)bc.p + 1, bn.p);
-  back_Long(env, hingeCorrect, bc, rc);
-  back_Double(env, normSquared, bn, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_counts(env, h, w, list_rows(samples), hingeCorrect, normSquared);
 }
 /* The *Sums forms serve either model (the *Counts forms refuse a logistic ctx): lossSumNormSquared(0) = sum of the per-sample
  * losses, (1) = ||w||^2; correct(0) = #correct. */
+static int req_sums(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray lossSumNormSquared, jlongArray correct) {
+  req_t q;
+  buf_t s = out_Double(env, lossSumNormSquared), c = out_Long(env, correct);
+  int rc = checked(req_open(env, h, w, r, &q), s.bad | c.bad, s.n < 2 || c.n < 1);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_sums, dsgd_eval_sampled_sums, dsgd_eval_samples_sums, (double *)s.p, (int64_t *)c.p,
+                  (double *)s.p + 1);
+  back_Double(env, lossSumNormSquared, s, rc);
+  back_Long(env, correct, c, rc);
+  req_close(&q);
+  return rc;
+}
 FN(evalSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray lossSumNormSquared,
              jlongArray correct) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, lossSumNormSquared), bc = out_Long(env, correct);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad))
-    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_sums(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (int64_t *)bc.p, (double *)bs.p + 1);
-  back_Double(env, lossSumNormSquared, bs, rc);
-  back_Long(env, correct, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_sums(env, h, w, range_rows(rowBegin, rowEnd), lossSumNormSquared, correct);
 }
 FN(evalSampledSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                     jlong posBegin, jlong posEnd, jdoubleArray lossSumNormSquared, jlongArray correct) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, lossSumNormSquared), bc = out_Long(env, correct);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad))
-    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_sampled_sums(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                         (double *)bs.p, (int64_t *)bc.p, (double *)bs.p + 1);
-  back_Double(env, lossSumNormSquared, bs, rc);
-  back_Long(env, correct, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_sums(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), lossSumNormSquared, correct);
 }
 FN(evalSamplesSums)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray lossSumNormSquared,
                     jlongArray correct) {
-  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, lossSumNormSquared),
-        bc = out_Long(env, correct);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bi.bad | bs.bad | bc.bad))
-    rc = (bs.n < 2 || bc.n < 1) ? DSGD_ERR_INVALID
-                                : dsgd_eval_samples_sums(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (int64_t *)bc.p,
-                                                         (double *)bs.p + 1);
-  back_Double(env, lossSumNormSquared, bs, rc);
-  back_Long(env, correct, bc, rc);
-  free(bw.p); free(bi.p);
-  return rc;
+  return req_sums(env, h, w, list_rows(samples), lossSumNormSquared, correct);
 }
 /* scores and ranking metrics, either model: out(i) = x_i . w (margins) or P(y = +1 | x_i) (probabilities, SparseLogistic
  * only); metrics(0..7) = the DSGD_METRICS_WORDS counts of dsgd_eval_metrics.  An output shorter than that is DSGD_ERR_INVALID. */
 FN(margins)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray out) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bo.bad)) rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_margins(CTX(h), bw.p, bs.p, bs.n, bo.p);
-  back_Double(env, out, bo, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return per_row(env, h, w, samples, out, dsgd_margins);
 }
 FN(probabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray out) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bo.bad)) rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_probabilities(CTX(h), bw.p, bs.p, bs.n, bo.p);
-  back_Double(env, out, bo, rc);
-  free(bw.p); free(bs.p);
+  return per_row(env, h, w, samples, out, dsgd_probabilities);
+}
+static int req_metrics(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray metrics) {
+  req_t q;
+  buf_t m = out_Long(env, metrics);
+  int rc = checked(req_open(env, h, w, r, &q), m.bad, m.n < DSGD_METRICS_WORDS);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_metrics, dsgd_eval_sampled_metrics, dsgd_eval_samples_metrics, (int64_t *)m.p);
+  back_Long(env, metrics, m, rc);
+  req_close(&q);
   return rc;
 }
 FN(evalMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics) {
-  buf_t bw = in_Double(env, w), bm = out_Long(env, metrics);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bm.bad))
-    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID : dsgd_eval_metrics(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)bm.p);
-  back_Long(env, metrics, bm, rc);
-  free(bw.p);
-  return rc;
+  return req_metrics(env, h, w, range_rows(rowBegin, rowEnd), metrics);
 }
 FN(evalSampledMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                        jlong posBegin, jlong posEnd, jlongArray metrics) {
-  buf_t bw = in_Double(env, w), bm = out_Long(env, metrics);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bm.bad))
-    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID
-                                   : dsgd_eval_sampled_metrics(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                               (int64_t *)bm.p);
-  back_Long(env, metrics, bm, rc);
-  free(bw.p);
-  return rc;
+  return req_metrics(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), metrics);
 }
 FN(evalSamplesMetrics)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bm = out_Long(env, metrics);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bm.bad))
-    rc = bm.n < DSGD_METRICS_WORDS ? DSGD_ERR_INVALID : dsgd_eval_samples_metrics(CTX(h), bw.p, bs.p, bs.n, (int64_t *)bm.p);
-  back_Long(env, metrics, bm, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_metrics(env, h, w, list_rows(samples), metrics);
 }
 /* curves and average precision: metrics(0..7) as above, ap(0) = average precision, nPoints(0) = m, and thr / tp / fp (0 until
  * m) the points, highest score first -- all three null for average precision alone, else each at least as long as the
  * request's rows (n = rowEnd - rowBegin, posEnd - posBegin or samples.length).  A shorter array is DSGD_ERR_INVALID. */
-typedef struct { buf_t m, a, k, t, tp, fp; } curve_bufs;
-static curve_bufs curve_out(JNIEnv *env, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr,
-                            jlongArray tp, jlongArray fp) {
-  curve_bufs c = {out_Long(env, metrics), out_Double(env, ap), out_Long(env, nPoints), out_Double(env, thr),
-                  out_Long(env, tp), out_Long(env, fp)};
-  return c;
-}
-static int curve_bad(const curve_bufs *c) { return c->m.bad | c->a.bad | c->k.bad | c->t.bad | c->tp.bad | c->fp.bad; }
-static int curve_short(const curve_bufs *c, jlong n) {
-  if (c->m.n < DSGD_METRICS_WORDS || c->a.n < 1 || c->k.n < 1) return 1;
-  return (c->t.p && c->t.n < n) || (c->tp.p && c->tp.n < n) || (c->fp.p && c->fp.n < n);
-}
-static void curve_back(JNIEnv *env, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp,
-                       jlongArray fp, curve_bufs *c, int rc) {
-  back_Long(env, metrics, c->m, rc);
-  back_Double(env, ap, c->a, rc);
-  back_Long(env, nPoints, c->k, rc);
-  back_Double(env, thr, c->t, rc);
-  back_Long(env, tp, c->tp, rc);
-  back_Long(env, fp, c->fp, rc);
+static int req_curve(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray metrics, jdoubleArray ap,
+                     jlongArray nPoints, jdoubleArray thr, jlongArray tp, jlongArray fp) {
+  req_t q;
+  buf_t m = out_Long(env, metrics), a = out_Double(env, ap), k = out_Long(env, nPoints), t = out_Double(env, thr),
+        bt = out_Long(env, tp), bf = out_Long(env, fp);
+  int rc = req_open(env, h, w, r, &q);
+  const jlong n = rows_n(&q);
+  rc = checked(rc, m.bad | a.bad | k.bad | t.bad | bt.bad | bf.bad,
+               m.n < DSGD_METRICS_WORDS || a.n < 1 || k.n < 1 || short_of(&t, n) || short_of(&bt, n) || short_of(&bf, n));
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_curve, dsgd_eval_sampled_curve, dsgd_eval_samples_curve, (int64_t *)m.p, (double *)a.p,
+                  (int64_t *)k.p, (double *)t.p, (int64_t *)bt.p, (int64_t *)bf.p);
+  back_Long(env, metrics, m, rc);
+  back_Double(env, ap, a, rc);
+  back_Long(env, nPoints, k, rc);
+  back_Double(env, thr, t, rc);
+  back_Long(env, tp, bt, rc);
+  back_Long(env, fp, bf, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics,
               jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp, jlongArray fp) {
-  buf_t bw = in_Double(env, w);
-  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | curve_bad(&c)))
-    rc = curve_short(&c, rowEnd - rowBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_curve(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.m.p, (double *)c.a.p, (int64_t *)c.k.p,
-                               (double *)c.t.p, (int64_t *)c.tp.p, (int64_t *)c.fp.p);
-  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_curve(env, h, w, range_rows(rowBegin, rowEnd), metrics, ap, nPoints, thr, tp, fp);
 }
 FN(evalSampledCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                      jlong posBegin, jlong posEnd, jlongArray metrics, jdoubleArray ap, jlongArray nPoints, jdoubleArray thr,
                      jlongArray tp, jlongArray fp) {
-  buf_t bw = in_Double(env, w);
-  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | curve_bad(&c)))
-    rc = curve_short(&c, posEnd - posBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_curve(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (int64_t *)c.m.p,
-                                       (double *)c.a.p, (int64_t *)c.k.p, (double *)c.t.p, (int64_t *)c.tp.p,
-                                       (int64_t *)c.fp.p);
-  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_curve(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), metrics, ap, nPoints, thr, tp, fp);
 }
 FN(evalSamplesCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics,
                      jdoubleArray ap, jlongArray nPoints, jdoubleArray thr, jlongArray tp, jlongArray fp) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  curve_bufs c = curve_out(env, metrics, ap, nPoints, thr, tp, fp);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | curve_bad(&c)))
-    rc = curve_short(&c, bs.n)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_curve(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.m.p, (double *)c.a.p, (int64_t *)c.k.p,
-                                       (double *)c.t.p, (int64_t *)c.tp.p, (int64_t *)c.fp.p);
-  curve_back(env, metrics, ap, nPoints, thr, tp, fp, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_curve(env, h, w, list_rows(samples), metrics, ap, nPoints, thr, tp, fp);
 }
 
 /* Poisson bootstrap: replicates [bBegin, bEnd) with key bKey; words(9 j .. 9 j + 8) = the DSGD_BOOTSTRAP_WORDS words of
  * replicate bBegin + j, ap(j) its average precision, loss(j) its loss sum.  An output shorter than the replicates is
  * DSGD_ERR_INVALID. */
-typedef struct { buf_t m, a, l; } boot_bufs;
-static boot_bufs boot_out(JNIEnv *env, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
-  boot_bufs c = {out_Long(env, words), out_Double(env, ap), out_Double(env, loss)};
-  return c;
-}
-static int boot_bad(const boot_bufs *c) { return c->m.bad | c->a.bad | c->l.bad; }
-static int boot_short(const boot_bufs *c, jlong bBegin, jlong bEnd) {
+static int req_boot(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
+                    jdoubleArray ap, jdoubleArray loss) {
+  req_t q;
+  buf_t m = out_Long(env, words), a = out_Double(env, ap), l = out_Double(env, loss);
   const jlong k = bEnd > bBegin ? bEnd - bBegin : 0;
-  return c->m.n < k * DSGD_BOOTSTRAP_WORDS || c->a.n < k || c->l.n < k;
-}
-static void boot_back(JNIEnv *env, jlongArray words, jdoubleArray ap, jdoubleArray loss, boot_bufs *c, int rc) {
-  back_Long(env, words, c->m, rc);
-  back_Double(env, ap, c->a, rc);
-  back_Double(env, loss, c->l, rc);
+  int rc = checked(req_open(env, h, w, r, &q), m.bad | a.bad | l.bad, m.n < k * DSGD_BOOTSTRAP_WORDS || a.n < k || l.n < k);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_bootstrap, dsgd_eval_sampled_bootstrap, dsgd_eval_samples_bootstrap, (uint64_t)bKey, bBegin,
+                  bEnd, (int64_t *)m.p, (double *)a.p, (double *)l.p);
+  back_Long(env, words, m, rc);
+  back_Double(env, ap, a, rc);
+  back_Double(env, loss, l, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong bKey, jlong bBegin,
                   jlong bEnd, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w);
-  boot_bufs c = boot_out(env, words, ap, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | boot_bad(&c)))
-    rc = boot_short(&c, bBegin, bEnd) ? DSGD_ERR_INVALID
-                                      : dsgd_eval_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)bKey, bBegin, bEnd,
-                                                            (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
-  boot_back(env, words, ap, loss, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_boot(env, h, w, range_rows(rowBegin, rowEnd), bKey, bBegin, bEnd, words, ap, loss);
 }
 FN(evalSampledBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                          jlong posBegin, jlong posEnd, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
                          jdoubleArray ap, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w);
-  boot_bufs c = boot_out(env, words, ap, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | boot_bad(&c)))
-    rc = boot_short(&c, bBegin, bEnd)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (uint64_t)bKey,
-                                           bBegin, bEnd, (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
-  boot_back(env, words, ap, loss, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_boot(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), bKey, bBegin, bEnd, words, ap, loss);
 }
 FN(evalSamplesBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlong bKey, jlong bBegin,
                          jlong bEnd, jlongArray words, jdoubleArray ap, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  boot_bufs c = boot_out(env, words, ap, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | boot_bad(&c)))
-    rc = boot_short(&c, bBegin, bEnd) ? DSGD_ERR_INVALID
-                                      : dsgd_eval_samples_bootstrap(CTX(h), bw.p, bs.p, bs.n, (uint64_t)bKey, bBegin, bEnd,
-                                                                    (int64_t *)c.m.p, (double *)c.a.p, (double *)c.l.p);
-  boot_back(env, words, ap, loss, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_boot(env, h, w, list_rows(samples), bKey, bBegin, bEnd, words, ap, loss);
 }
 
 /* weighted Poisson bootstrap: replicates [bBegin, bEnd) with key bKey; words(2 j), words(2 j + 1) = the size and the NaN-score
- * rows of replicate bBegin + j, wsums(13 j .. 13 j + 12) its DSGD_WCURVE_WORDS, loss(j) its weighted loss sum.  The buffers
- * are those of the unweighted bootstrap, with wsums in ap's place.  An output shorter than the replicates is
- * DSGD_ERR_INVALID. */
-static int wboot_short(const boot_bufs *c, jlong bBegin, jlong bEnd) {
+ * rows of replicate bBegin + j, wsums(13 j .. 13 j + 12) its DSGD_WCURVE_WORDS, loss(j) its weighted loss sum.  An output
+ * shorter than the replicates is DSGD_ERR_INVALID. */
+static int req_wboot(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
+                     jdoubleArray wsums, jdoubleArray loss) {
+  req_t q;
+  buf_t m = out_Long(env, words), s = out_Double(env, wsums), l = out_Double(env, loss);
   const jlong k = bEnd > bBegin ? bEnd - bBegin : 0;
-  return c->m.n < k * 2 || c->a.n < k * DSGD_WCURVE_WORDS || c->l.n < k;
+  int rc = checked(req_open(env, h, w, r, &q), m.bad | s.bad | l.bad, m.n < k * 2 || s.n < k * DSGD_WCURVE_WORDS || l.n < k);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_weighted_bootstrap, dsgd_eval_sampled_weighted_bootstrap,
+                  dsgd_eval_samples_weighted_bootstrap, (uint64_t)bKey, bBegin, bEnd, (int64_t *)m.p, (double *)s.p,
+                  (double *)l.p);
+  back_Long(env, words, m, rc);
+  back_Double(env, wsums, s, rc);
+  back_Double(env, loss, l, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong bKey,
                           jlong bBegin, jlong bEnd, jlongArray words, jdoubleArray wsums, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w);
-  boot_bufs c = boot_out(env, words, wsums, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | boot_bad(&c)))
-    rc = wboot_short(&c, bBegin, bEnd)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_weighted_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p,
-                                            (double *)c.a.p, (double *)c.l.p);
-  boot_back(env, words, wsums, loss, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_wboot(env, h, w, range_rows(rowBegin, rowEnd), bKey, bBegin, bEnd, words, wsums, loss);
 }
 FN(evalSampledWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                                  jlong posBegin, jlong posEnd, jlong bKey, jlong bBegin, jlong bEnd, jlongArray words,
                                  jdoubleArray wsums, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w);
-  boot_bufs c = boot_out(env, words, wsums, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | boot_bad(&c)))
-    rc = wboot_short(&c, bBegin, bEnd)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_weighted_bootstrap(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                    (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p, (double *)c.a.p,
-                                                    (double *)c.l.p);
-  boot_back(env, words, wsums, loss, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_wboot(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), bKey, bBegin, bEnd, words, wsums, loss);
 }
 FN(evalSamplesWeightedBootstrap)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlong bKey,
                                  jlong bBegin, jlong bEnd, jlongArray words, jdoubleArray wsums, jdoubleArray loss) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  boot_bufs c = boot_out(env, words, wsums, loss);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | boot_bad(&c)))
-    rc = wboot_short(&c, bBegin, bEnd)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_weighted_bootstrap(CTX(h), bw.p, bs.p, bs.n, (uint64_t)bKey, bBegin, bEnd, (int64_t *)c.m.p,
-                                                    (double *)c.a.p, (double *)c.l.p);
-  boot_back(env, words, wsums, loss, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_wboot(env, h, w, list_rows(samples), bKey, bBegin, bEnd, words, wsums, loss);
 }
 
 /* calibration: ab(0..1) = (A, B), objective(0) = F(A, B), info(0..4) = the DSGD_CALIBRATION_INFO_WORDS words; probabilities:
  * out(i) = sigmoid(-(a x_i . w + b)); quality: sums(0..1) = Brier and log-loss sums, binRows / binPos / binPsum at least nBins
- * long, words(0..1) = rows used and left out.  A shorter array is DSGD_ERR_INVALID. */
-typedef struct { buf_t ab, f, info; } calib_bufs;
-static calib_bufs calib_out(JNIEnv *env, jdoubleArray ab, jdoubleArray objective, jlongArray info) {
-  calib_bufs c = {out_Double(env, ab), out_Double(env, objective), out_Long(env, info)};
-  return c;
-}
-static int calib_bad(const calib_bufs *c) { return c->ab.bad | c->f.bad | c->info.bad; }
-static int calib_short(const calib_bufs *c) { return c->ab.n < 2 || c->f.n < 1 || c->info.n < DSGD_CALIBRATION_INFO_WORDS; }
-static void calib_back(JNIEnv *env, jdoubleArray ab, jdoubleArray objective, jlongArray info, calib_bufs *c, int rc) {
-  back_Double(env, ab, c->ab, rc);
-  back_Double(env, objective, c->f, rc);
-  back_Long(env, info, c->info, rc);
+ * long, words(0..1) = rows used and left out.  A shorter array is DSGD_ERR_INVALID.  nBins outside
+ * 1 .. DSGD_CALIBRATION_MAX_BINS is the library's DSGD_ERR_INVALID: only the lengths are checked here. */
+static jlong bins_n(jint nBins) { return nBins > 0 ? nBins : 0; }
+static int req_calib(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray ab, jdoubleArray objective,
+                     jlongArray info) {
+  req_t q;
+  buf_t a = out_Double(env, ab), f = out_Double(env, objective), i = out_Long(env, info);
+  int rc = checked(req_open(env, h, w, r, &q), a.bad | f.bad | i.bad,
+                   a.n < 2 || f.n < 1 || i.n < DSGD_CALIBRATION_INFO_WORDS);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_calibrate, dsgd_calibrate_sampled, dsgd_calibrate_samples, (double *)a.p, (double *)f.p,
+                  (int64_t *)i.p);
+  back_Double(env, ab, a, rc);
+  back_Double(env, objective, f, rc);
+  back_Long(env, info, i, rc);
+  req_close(&q);
+  return rc;
 }
 FN(calibrate)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray ab,
               jdoubleArray objective, jlongArray info) {
-  buf_t bw = in_Double(env, w);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | calib_bad(&c)))
-    rc = calib_short(&c) ? DSGD_ERR_INVALID
-                         : dsgd_calibrate(CTX(h), bw.p, rowBegin, rowEnd, (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_calib(env, h, w, range_rows(rowBegin, rowEnd), ab, objective, info);
 }
 FN(calibrateSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                      jlong posBegin, jlong posEnd, jdoubleArray ab, jdoubleArray objective, jlongArray info) {
-  buf_t bw = in_Double(env, w);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | calib_bad(&c)))
-    rc = calib_short(&c) ? DSGD_ERR_INVALID
-                         : dsgd_calibrate_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                  (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_calib(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), ab, objective, info);
 }
 FN(calibrateSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray ab,
                      jdoubleArray objective, jlongArray info) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | calib_bad(&c)))
-    rc = calib_short(&c) ? DSGD_ERR_INVALID
-                         : dsgd_calibrate_samples(CTX(h), bw.p, bs.p, bs.n, (double *)c.ab.p, (double *)c.f.p, (int64_t *)c.info.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_calib(env, h, w, list_rows(samples), ab, objective, info);
 }
 FN(calibratedProbabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a, jdouble b,
                             jdoubleArray out) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bo = out_Double(env, out);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bo.bad))
-    rc = bo.n < bs.n ? DSGD_ERR_INVALID : dsgd_calibrated_probabilities(CTX(h), bw.p, bs.p, bs.n, a, b, bo.p);
-  back_Double(env, out, bo, rc);
-  free(bw.p); free(bs.p);
+  req_t q;
+  buf_t o = out_Double(env, out);
+  int rc = req_open(env, h, w, list_rows(samples), &q);
+  rc = checked(rc, o.bad, o.n < q.r.ids.n);
+  if (rc == DSGD_OK) rc = dsgd_calibrated_probabilities(CTX(h), q.w.p, q.r.ids.p, q.r.ids.n, a, b, o.p);
+  back_Double(env, out, o, rc);
+  req_close(&q);
   return rc;
 }
-typedef struct { buf_t s, r, p, ps, wd; } quality_bufs;
-static quality_bufs quality_out(JNIEnv *env, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
-                                jlongArray words) {
-  quality_bufs q = {out_Double(env, sums), out_Long(env, binRows), out_Long(env, binPos), out_Double(env, binPsum),
-                    out_Long(env, words)};
-  return q;
-}
-static int quality_bad(const quality_bufs *q) { return q->s.bad | q->r.bad | q->p.bad | q->ps.bad | q->wd.bad; }
-/* nBins outside 1 .. DSGD_CALIBRATION_MAX_BINS is the library's DSGD_ERR_INVALID: only the lengths are checked here */
-static int quality_short(const quality_bufs *q, jint nBins) {
-  const jlong m = nBins > 0 ? nBins : 0;
-  return q->s.n < 2 || q->wd.n < 2 || q->r.n < m || q->p.n < m || q->ps.n < m;
-}
-static void quality_back(JNIEnv *env, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
-                         jlongArray words, quality_bufs *q, int rc) {
-  back_Double(env, sums, q->s, rc);
-  back_Long(env, binRows, q->r, rc);
-  back_Long(env, binPos, q->p, rc);
-  back_Double(env, binPsum, q->ps, rc);
-  back_Long(env, words, q->wd, rc);
+static int req_quality(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdouble a, jdouble b, jint nBins, jdoubleArray sums,
+                       jlongArray binRows, jlongArray binPos, jdoubleArray binPsum, jlongArray words) {
+  req_t q;
+  buf_t s = out_Double(env, sums), br = out_Long(env, binRows), bp = out_Long(env, binPos), ps = out_Double(env, binPsum),
+        wd = out_Long(env, words);
+  const jlong m = bins_n(nBins);
+  int rc = checked(req_open(env, h, w, r, &q), s.bad | br.bad | bp.bad | ps.bad | wd.bad,
+                   s.n < 2 || wd.n < 2 || br.n < m || bp.n < m || ps.n < m);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_calibration, dsgd_eval_sampled_calibration, dsgd_eval_samples_calibration, a, b, nBins,
+                  (double *)s.p, (int64_t *)br.p, (int64_t *)bp.p, (double *)ps.p, (int64_t *)wd.p);
+  back_Double(env, sums, s, rc);
+  back_Long(env, binRows, br, rc);
+  back_Long(env, binPos, bp, rc);
+  back_Double(env, binPsum, ps, rc);
+  back_Long(env, words, wd, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdouble a, jdouble b,
                     jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
                     jlongArray words) {
-  buf_t bw = in_Double(env, w);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | quality_bad(&q)))
-    rc = quality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_calibration(CTX(h), bw.p, rowBegin, rowEnd, a, b, nBins, (double *)q.s.p, (int64_t *)q.r.p,
-                                     (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p);
-  return rc;
+  return req_quality(env, h, w, range_rows(rowBegin, rowEnd), a, b, nBins, sums, binRows, binPos, binPsum, words);
 }
 FN(evalSampledCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                            jlong posBegin, jlong posEnd, jdouble a, jdouble b, jint nBins, jdoubleArray sums,
                            jlongArray binRows, jlongArray binPos, jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | quality_bad(&q)))
-    rc = quality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, a, b, nBins,
-                                             (double *)q.s.p, (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p,
-                                             (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p);
-  return rc;
+  return req_quality(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), a, b, nBins, sums, binRows, binPos,
+                     binPsum, words);
 }
 FN(evalSamplesCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a, jdouble b,
                            jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
                            jlongArray words) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | quality_bad(&q)))
-    rc = quality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_calibration(CTX(h), bw.p, bs.p, bs.n, a, b, nBins, (double *)q.s.p, (int64_t *)q.r.p,
-                                             (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_quality(env, h, w, list_rows(samples), a, b, nBins, sums, binRows, binPos, binPsum, words);
 }
 
 /* weighted calibration: the calibration natives with wsums(0..2) = W+, W- and the NaN rows' weight added to a fit; quality:
  * sums(0..3) = weighted Brier and log-loss sums, the weight used and the infinite-term weight, binWeight / binPosWeight /
  * binPsum at least nBins long (doubles), words(0..1) as there.  A shorter array is DSGD_ERR_INVALID. */
-static int wcalib_short(const calib_bufs *c, const buf_t *ws) { return calib_short(c) || ws->n < DSGD_CALIBRATION_WSUMS; }
+static int req_wcalib(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray ab, jdoubleArray objective,
+                      jlongArray info, jdoubleArray wsums) {
+  req_t q;
+  buf_t a = out_Double(env, ab), f = out_Double(env, objective), i = out_Long(env, info), s = out_Double(env, wsums);
+  int rc = checked(req_open(env, h, w, r, &q), a.bad | f.bad | i.bad | s.bad,
+                   a.n < 2 || f.n < 1 || i.n < DSGD_CALIBRATION_INFO_WORDS || s.n < DSGD_CALIBRATION_WSUMS);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_calibrate_weighted, dsgd_calibrate_weighted_sampled, dsgd_calibrate_weighted_samples,
+                  (double *)a.p, (double *)f.p, (int64_t *)i.p, (double *)s.p);
+  back_Double(env, ab, a, rc);
+  back_Double(env, objective, f, rc);
+  back_Long(env, info, i, rc);
+  back_Double(env, wsums, s, rc);
+  req_close(&q);
+  return rc;
+}
 FN(calibrateWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray ab,
                       jdoubleArray objective, jlongArray info, jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w), ws = out_Double(env, wsums);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | ws.bad | calib_bad(&c)))
-    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
-                               : dsgd_calibrate_weighted(CTX(h), bw.p, rowBegin, rowEnd, (double *)c.ab.p, (double *)c.f.p,
-                                                         (int64_t *)c.info.p, ws.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  back_Double(env, wsums, ws, rc);
-  free(bw.p);
-  return rc;
+  return req_wcalib(env, h, w, range_rows(rowBegin, rowEnd), ab, objective, info, wsums);
 }
 FN(calibrateWeightedSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                              jlong posBegin, jlong posEnd, jdoubleArray ab, jdoubleArray objective, jlongArray info,
                              jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w), ws = out_Double(env, wsums);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | ws.bad | calib_bad(&c)))
-    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
-                               : dsgd_calibrate_weighted_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin,
-                                                                 posEnd, (double *)c.ab.p, (double *)c.f.p,
-                                                                 (int64_t *)c.info.p, ws.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  back_Double(env, wsums, ws, rc);
-  free(bw.p);
-  return rc;
+  return req_wcalib(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), ab, objective, info, wsums);
 }
 FN(calibrateWeightedSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray ab,
                              jdoubleArray objective, jlongArray info, jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), ws = out_Double(env, wsums);
-  calib_bufs c = calib_out(env, ab, objective, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | ws.bad | calib_bad(&c)))
-    rc = wcalib_short(&c, &ws) ? DSGD_ERR_INVALID
-                               : dsgd_calibrate_weighted_samples(CTX(h), bw.p, bs.p, bs.n, (double *)c.ab.p, (double *)c.f.p,
-                                                                 (int64_t *)c.info.p, ws.p);
-  calib_back(env, ab, objective, info, &c, rc);
-  back_Double(env, wsums, ws, rc);
-  free(bw.p); free(bs.p);
+  return req_wcalib(env, h, w, list_rows(samples), ab, objective, info, wsums);
+}
+static int req_wquality(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdouble a, jdouble b, jint nBins, jdoubleArray sums,
+                        jdoubleArray binWeight, jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
+  req_t q;
+  buf_t s = out_Double(env, sums), bw = out_Double(env, binWeight), bp = out_Double(env, binPosWeight),
+        ps = out_Double(env, binPsum), wd = out_Long(env, words);
+  const jlong m = bins_n(nBins);
+  int rc = checked(req_open(env, h, w, r, &q), s.bad | bw.bad | bp.bad | ps.bad | wd.bad,
+                   s.n < DSGD_WCALIBRATION_SUMS || wd.n < 2 || bw.n < m || bp.n < m || ps.n < m);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_weighted_calibration, dsgd_eval_sampled_weighted_calibration,
+                  dsgd_eval_samples_weighted_calibration, a, b, nBins, (double *)s.p, (double *)bw.p, (double *)bp.p,
+                  (double *)ps.p, (int64_t *)wd.p);
+  back_Double(env, sums, s, rc);
+  back_Double(env, binWeight, bw, rc);
+  back_Double(env, binPosWeight, bp, rc);
+  back_Double(env, binPsum, ps, rc);
+  back_Long(env, words, wd, rc);
+  req_close(&q);
   return rc;
-}
-typedef struct { buf_t s, wt, pw, ps, wd; } wquality_bufs;
-static wquality_bufs wquality_out(JNIEnv *env, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
-                                  jdoubleArray binPsum, jlongArray words) {
-  wquality_bufs q = {out_Double(env, sums), out_Double(env, binWeight), out_Double(env, binPosWeight),
-                     out_Double(env, binPsum), out_Long(env, words)};
-  return q;
-}
-static int wquality_bad(const wquality_bufs *q) { return q->s.bad | q->wt.bad | q->pw.bad | q->ps.bad | q->wd.bad; }
-static int wquality_short(const wquality_bufs *q, jint nBins) {
-  const jlong m = nBins > 0 ? nBins : 0;
-  return q->s.n < DSGD_WCALIBRATION_SUMS || q->wd.n < 2 || q->wt.n < m || q->pw.n < m || q->ps.n < m;
-}
-static void wquality_back(JNIEnv *env, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
-                          jdoubleArray binPsum, jlongArray words, wquality_bufs *q, int rc) {
-  back_Double(env, sums, q->s, rc);
-  back_Double(env, binWeight, q->wt, rc);
-  back_Double(env, binPosWeight, q->pw, rc);
-  back_Double(env, binPsum, q->ps, rc);
-  back_Long(env, words, q->wd, rc);
 }
 FN(evalWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdouble a,
                             jdouble b, jint nBins, jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
                             jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | wquality_bad(&q)))
-    rc = wquality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_weighted_calibration(CTX(h), bw.p, rowBegin, rowEnd, a, b, nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p,
-                                              (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p);
-  return rc;
+  return req_wquality(env, h, w, range_rows(rowBegin, rowEnd), a, b, nBins, sums, binWeight, binPosWeight, binPsum, words);
 }
 FN(evalSampledWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                                    jlong key, jlong posBegin, jlong posEnd, jdouble a, jdouble b, jint nBins,
                                    jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight,
                                    jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | wquality_bad(&q)))
-    rc = wquality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_weighted_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, a, b,
-                                                      nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p, (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p);
-  return rc;
+  return req_wquality(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), a, b, nBins, sums, binWeight,
+                      binPosWeight, binPsum, words);
 }
 FN(evalSamplesWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdouble a,
                                    jdouble b, jint nBins, jdoubleArray sums, jdoubleArray binWeight,
                                    jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | wquality_bad(&q)))
-    rc = wquality_short(&q, nBins)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_weighted_calibration(CTX(h), bw.p, bs.p, bs.n, a, b, nBins, q.s.p, q.wt.p, q.pw.p, q.ps.p,
-                                                      (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_wquality(env, h, w, list_rows(samples), a, b, nBins, sums, binWeight, binPosWeight, binPsum, words);
 }
 
 /* isotonic calibration: nPoints(0) = k, x / y(0 until k) the thresholds and their values, blockRows / blockPos(0 until
@@ -684,258 +544,175 @@ FN(evalSamplesWeightedCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleAr
  * rows.  Probabilities and quality at the map (x, y): x and y of one length k >= 1; out at least as long as samples; the
  * quality arrays as for evalCalibration, words(0..2) = rows used, rows left out and rows with an infinite log-loss term.
  * A shorter array is DSGD_ERR_INVALID. */
-typedef struct { buf_t k, x, y, r, p, info; } iso_bufs;
-static iso_bufs iso_out(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jlongArray blockRows,
-                        jlongArray blockPos, jlongArray info) {
-  iso_bufs c = {out_Long(env, nPoints), out_Double(env, x), out_Double(env, y), out_Long(env, blockRows),
-                out_Long(env, blockPos), out_Long(env, info)};
-  return c;
-}
-static int iso_bad(const iso_bufs *c) { return c->k.bad | c->x.bad | c->y.bad | c->r.bad | c->p.bad | c->info.bad; }
-static int iso_short(const iso_bufs *c, jlong n) {
-  return c->k.n < 1 || c->info.n < DSGD_ISOTONIC_INFO_WORDS || c->x.n < n || c->y.n < n || c->r.n < n || c->p.n < n;
-}
-static void iso_back(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jlongArray blockRows,
-                     jlongArray blockPos, jlongArray info, iso_bufs *c, int rc) {
-  back_Long(env, nPoints, c->k, rc);
-  back_Double(env, x, c->x, rc);
-  back_Double(env, y, c->y, rc);
-  back_Long(env, blockRows, c->r, rc);
-  back_Long(env, blockPos, c->p, rc);
-  back_Long(env, info, c->info, rc);
+static int req_iso(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray nPoints, jdoubleArray x, jdoubleArray y,
+                   jlongArray blockRows, jlongArray blockPos, jlongArray info) {
+  req_t q;
+  buf_t k = out_Long(env, nPoints), bx = out_Double(env, x), by = out_Double(env, y), br = out_Long(env, blockRows),
+        bp = out_Long(env, blockPos), i = out_Long(env, info);
+  int rc = req_open(env, h, w, r, &q);
+  const jlong n = rows_n(&q);
+  rc = checked(rc, k.bad | bx.bad | by.bad | br.bad | bp.bad | i.bad,
+               k.n < 1 || i.n < DSGD_ISOTONIC_INFO_WORDS || bx.n < n || by.n < n || br.n < n || bp.n < n);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_calibrate_isotonic, dsgd_calibrate_isotonic_sampled, dsgd_calibrate_isotonic_samples,
+                  (int64_t *)k.p, (double *)bx.p, (double *)by.p, (int64_t *)br.p, (int64_t *)bp.p, (int64_t *)i.p);
+  back_Long(env, nPoints, k, rc);
+  back_Double(env, x, bx, rc);
+  back_Double(env, y, by, rc);
+  back_Long(env, blockRows, br, rc);
+  back_Long(env, blockPos, bp, rc);
+  back_Long(env, info, i, rc);
+  req_close(&q);
+  return rc;
 }
 FN(calibrateIsotonic)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray nPoints,
                       jdoubleArray x, jdoubleArray y, jlongArray blockRows, jlongArray blockPos, jlongArray info) {
-  buf_t bw = in_Double(env, w);
-  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | iso_bad(&c)))
-    rc = iso_short(&c, rowEnd - rowBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p,
-                                       (int64_t *)c.r.p, (int64_t *)c.p.p, (int64_t *)c.info.p);
-  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_iso(env, h, w, range_rows(rowBegin, rowEnd), nPoints, x, y, blockRows, blockPos, info);
 }
 FN(calibrateIsotonicSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                              jlong posBegin, jlong posEnd, jlongArray nPoints, jdoubleArray x, jdoubleArray y,
                              jlongArray blockRows, jlongArray blockPos, jlongArray info) {
-  buf_t bw = in_Double(env, w);
-  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | iso_bad(&c)))
-    rc = iso_short(&c, posEnd - posBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                               (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p, (int64_t *)c.r.p,
-                                               (int64_t *)c.p.p, (int64_t *)c.info.p);
-  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_iso(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), nPoints, x, y, blockRows, blockPos, info);
 }
 FN(calibrateIsotonicSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray nPoints,
                              jdoubleArray x, jdoubleArray y, jlongArray blockRows, jlongArray blockPos, jlongArray info) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  iso_bufs c = iso_out(env, nPoints, x, y, blockRows, blockPos, info);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | iso_bad(&c)))
-    rc = iso_short(&c, bs.n)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic_samples(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.k.p, (double *)c.x.p, (double *)c.y.p,
-                                               (int64_t *)c.r.p, (int64_t *)c.p.p, (int64_t *)c.info.p);
-  iso_back(env, nPoints, x, y, blockRows, blockPos, info, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_iso(env, h, w, list_rows(samples), nPoints, x, y, blockRows, blockPos, info);
 }
 FN(isotonicProbabilities)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray x,
                           jdoubleArray y, jdoubleArray out) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y),
-        bo = out_Double(env, out);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bx.bad | by.bad | bo.bad))
-    rc = bo.n < bs.n || bx.n != by.n ? DSGD_ERR_INVALID
-                                     : dsgd_isotonic_probabilities(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, bo.p);
-  back_Double(env, out, bo, rc);
-  free(bw.p); free(bs.p); free(bx.p); free(by.p);
+  req_t q;
+  buf_t bx = in_Double(env, x), by = in_Double(env, y), o = out_Double(env, out);
+  int rc = req_open(env, h, w, list_rows(samples), &q);
+  rc = checked(rc, bx.bad | by.bad | o.bad, o.n < q.r.ids.n || bx.n != by.n);
+  if (rc == DSGD_OK) rc = dsgd_isotonic_probabilities(CTX(h), q.w.p, q.r.ids.p, q.r.ids.n, bx.p, by.p, bx.n, o.p);
+  back_Double(env, out, o, rc);
+  req_close(&q);
+  free(bx.p); free(by.p);
   return rc;
 }
-static int iso_quality_short(const quality_bufs *q, jint nBins, const buf_t *bx, const buf_t *by) {
-  return quality_short(q, nBins) || q->wd.n < DSGD_ISOTONIC_EVAL_WORDS || bx->n != by->n;
+static int req_iso_quality(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray x, jdoubleArray y, jint nBins,
+                           jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum, jlongArray words) {
+  req_t q;
+  buf_t bx = in_Double(env, x), by = in_Double(env, y), s = out_Double(env, sums), br = out_Long(env, binRows),
+        bp = out_Long(env, binPos), ps = out_Double(env, binPsum), wd = out_Long(env, words);
+  const jlong m = bins_n(nBins);
+  int rc = checked(req_open(env, h, w, r, &q), bx.bad | by.bad | s.bad | br.bad | bp.bad | ps.bad | wd.bad,
+                   s.n < 2 || wd.n < DSGD_ISOTONIC_EVAL_WORDS || br.n < m || bp.n < m || ps.n < m || bx.n != by.n);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_isotonic_calibration, dsgd_eval_sampled_isotonic_calibration,
+                  dsgd_eval_samples_isotonic_calibration, bx.p, by.p, bx.n, nBins, (double *)s.p, (int64_t *)br.p,
+                  (int64_t *)bp.p, (double *)ps.p, (int64_t *)wd.p);
+  back_Double(env, sums, s, rc);
+  back_Long(env, binRows, br, rc);
+  back_Long(env, binPos, bp, rc);
+  back_Double(env, binPsum, ps, rc);
+  back_Long(env, words, wd, rc);
+  req_close(&q);
+  free(bx.p); free(by.p);
+  return rc;
 }
 FN(evalIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray x,
                             jdoubleArray y, jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos,
                             jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bx.bad | by.bad | quality_bad(&q)))
-    rc = iso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, bx.p, by.p, bx.n, nBins, (double *)q.s.p,
-                                              (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p, (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p); free(bx.p); free(by.p);
-  return rc;
+  return req_iso_quality(env, h, w, range_rows(rowBegin, rowEnd), x, y, nBins, sums, binRows, binPos, binPsum, words);
 }
 FN(evalSampledIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                                    jlong key, jlong posBegin, jlong posEnd, jdoubleArray x, jdoubleArray y, jint nBins,
                                    jdoubleArray sums, jlongArray binRows, jlongArray binPos, jdoubleArray binPsum,
                                    jlongArray words) {
-  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bx.bad | by.bad | quality_bad(&q)))
-    rc = iso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, bx.p,
-                                                      by.p, bx.n, nBins, (double *)q.s.p, (int64_t *)q.r.p, (int64_t *)q.p.p,
-                                                      (double *)q.ps.p, (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p); free(bx.p); free(by.p);
-  return rc;
+  return req_iso_quality(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), x, y, nBins, sums, binRows, binPos,
+                         binPsum, words);
 }
 FN(evalSamplesIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray x,
                                    jdoubleArray y, jint nBins, jdoubleArray sums, jlongArray binRows, jlongArray binPos,
                                    jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y);
-  quality_bufs q = quality_out(env, sums, binRows, binPos, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bx.bad | by.bad | quality_bad(&q)))
-    rc = iso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_isotonic_calibration(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, nBins, (double *)q.s.p,
-                                                      (int64_t *)q.r.p, (int64_t *)q.p.p, (double *)q.ps.p,
-                                                      (int64_t *)q.wd.p);
-  quality_back(env, sums, binRows, binPos, binPsum, words, &q, rc);
-  free(bw.p); free(bs.p); free(bx.p); free(by.p);
-  return rc;
+  return req_iso_quality(env, h, w, list_rows(samples), x, y, nBins, sums, binRows, binPos, binPsum, words);
 }
 
 /* weighted isotonic calibration: the isotonic natives with blockWeight / blockPosWeight (doubles) in place of the block counts
  * and wsums(0..1) = W+, W- added to a fit; weighted quality at (x, y): the weighted quality arrays with words(0..2) as for
  * evalIsotonicCalibration.  A shorter array is DSGD_ERR_INVALID. */
-typedef struct { buf_t k, x, y, r, p, info, ws; } wiso_bufs;
-static wiso_bufs wiso_out(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
-                          jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
-  wiso_bufs c = {out_Long(env, nPoints), out_Double(env, x), out_Double(env, y), out_Double(env, blockWeight),
-                 out_Double(env, blockPosWeight), out_Long(env, info), out_Double(env, wsums)};
-  return c;
-}
-static int wiso_bad(const wiso_bufs *c) {
-  return c->k.bad | c->x.bad | c->y.bad | c->r.bad | c->p.bad | c->info.bad | c->ws.bad;
-}
-static int wiso_short(const wiso_bufs *c, jlong n) {
-  return c->k.n < 1 || c->info.n < DSGD_ISOTONIC_INFO_WORDS || c->ws.n < 2 || c->x.n < n || c->y.n < n || c->r.n < n ||
-         c->p.n < n;
-}
-static void wiso_back(JNIEnv *env, jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
-                      jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums, wiso_bufs *c, int rc) {
-  back_Long(env, nPoints, c->k, rc);
-  back_Double(env, x, c->x, rc);
-  back_Double(env, y, c->y, rc);
-  back_Double(env, blockWeight, c->r, rc);
-  back_Double(env, blockPosWeight, c->p, rc);
-  back_Long(env, info, c->info, rc);
-  back_Double(env, wsums, c->ws, rc);
+static int req_wiso(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray nPoints, jdoubleArray x, jdoubleArray y,
+                    jdoubleArray blockWeight, jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
+  req_t q;
+  buf_t k = out_Long(env, nPoints), bx = out_Double(env, x), by = out_Double(env, y), bw = out_Double(env, blockWeight),
+        bp = out_Double(env, blockPosWeight), i = out_Long(env, info), s = out_Double(env, wsums);
+  int rc = req_open(env, h, w, r, &q);
+  const jlong n = rows_n(&q);
+  rc = checked(rc, k.bad | bx.bad | by.bad | bw.bad | bp.bad | i.bad | s.bad,
+               k.n < 1 || i.n < DSGD_ISOTONIC_INFO_WORDS || s.n < 2 || bx.n < n || by.n < n || bw.n < n || bp.n < n);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_calibrate_isotonic_weighted, dsgd_calibrate_isotonic_weighted_sampled,
+                  dsgd_calibrate_isotonic_weighted_samples, (int64_t *)k.p, (double *)bx.p, (double *)by.p, (double *)bw.p,
+                  (double *)bp.p, (int64_t *)i.p, (double *)s.p);
+  back_Long(env, nPoints, k, rc);
+  back_Double(env, x, bx, rc);
+  back_Double(env, y, by, rc);
+  back_Double(env, blockWeight, bw, rc);
+  back_Double(env, blockPosWeight, bp, rc);
+  back_Long(env, info, i, rc);
+  back_Double(env, wsums, s, rc);
+  req_close(&q);
+  return rc;
 }
 FN(calibrateIsotonicWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                               jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
                               jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w);
-  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | wiso_bad(&c)))
-    rc = wiso_short(&c, rowEnd - rowBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic_weighted(CTX(h), bw.p, rowBegin, rowEnd, (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p, c.p.p,
-                                                (int64_t *)c.info.p, c.ws.p);
-  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_wiso(env, h, w, range_rows(rowBegin, rowEnd), nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
 }
 FN(calibrateIsotonicWeightedSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                                      jlong key, jlong posBegin, jlong posEnd, jlongArray nPoints, jdoubleArray x,
                                      jdoubleArray y, jdoubleArray blockWeight, jdoubleArray blockPosWeight, jlongArray info,
                                      jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w);
-  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | wiso_bad(&c)))
-    rc = wiso_short(&c, posEnd - posBegin)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic_weighted_sampled(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                        (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p, c.p.p, (int64_t *)c.info.p,
-                                                        c.ws.p);
-  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
-  free(bw.p);
-  return rc;
+  return req_wiso(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), nPoints, x, y, blockWeight, blockPosWeight,
+                  info, wsums);
 }
 FN(calibrateIsotonicWeightedSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples,
                                      jlongArray nPoints, jdoubleArray x, jdoubleArray y, jdoubleArray blockWeight,
                                      jdoubleArray blockPosWeight, jlongArray info, jdoubleArray wsums) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples);
-  wiso_bufs c = wiso_out(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | wiso_bad(&c)))
-    rc = wiso_short(&c, bs.n)
-             ? DSGD_ERR_INVALID
-             : dsgd_calibrate_isotonic_weighted_samples(CTX(h), bw.p, bs.p, bs.n, (int64_t *)c.k.p, c.x.p, c.y.p, c.r.p,
-                                                        c.p.p, (int64_t *)c.info.p, c.ws.p);
-  wiso_back(env, nPoints, x, y, blockWeight, blockPosWeight, info, wsums, &c, rc);
-  free(bw.p); free(bs.p);
-  return rc;
+  return req_wiso(env, h, w, list_rows(samples), nPoints, x, y, blockWeight, blockPosWeight, info, wsums);
 }
-static int wiso_quality_short(const wquality_bufs *q, jint nBins, const buf_t *bx, const buf_t *by) {
-  return wquality_short(q, nBins) || q->wd.n < DSGD_ISOTONIC_EVAL_WORDS || bx->n != by->n;
+static int req_wiso_quality(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray x, jdoubleArray y, jint nBins,
+                            jdoubleArray sums, jdoubleArray binWeight, jdoubleArray binPosWeight, jdoubleArray binPsum,
+                            jlongArray words) {
+  req_t q;
+  buf_t bx = in_Double(env, x), by = in_Double(env, y), s = out_Double(env, sums), bw = out_Double(env, binWeight),
+        bp = out_Double(env, binPosWeight), ps = out_Double(env, binPsum), wd = out_Long(env, words);
+  const jlong m = bins_n(nBins);
+  int rc = checked(req_open(env, h, w, r, &q), bx.bad | by.bad | s.bad | bw.bad | bp.bad | ps.bad | wd.bad,
+                   s.n < DSGD_WCALIBRATION_SUMS || wd.n < DSGD_ISOTONIC_EVAL_WORDS || bw.n < m || bp.n < m || ps.n < m ||
+                       bx.n != by.n);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_weighted_isotonic_calibration, dsgd_eval_sampled_weighted_isotonic_calibration,
+                  dsgd_eval_samples_weighted_isotonic_calibration, bx.p, by.p, bx.n, nBins, (double *)s.p, (double *)bw.p,
+                  (double *)bp.p, (double *)ps.p, (int64_t *)wd.p);
+  back_Double(env, sums, s, rc);
+  back_Double(env, binWeight, bw, rc);
+  back_Double(env, binPosWeight, bp, rc);
+  back_Double(env, binPsum, ps, rc);
+  back_Long(env, words, wd, rc);
+  req_close(&q);
+  free(bx.p); free(by.p);
+  return rc;
 }
 FN(evalWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                                     jdoubleArray x, jdoubleArray y, jint nBins, jdoubleArray sums, jdoubleArray binWeight,
                                     jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bx.bad | by.bad | wquality_bad(&q)))
-    rc = wiso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_weighted_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, bx.p, by.p, bx.n, nBins, q.s.p, q.wt.p,
-                                                       q.pw.p, q.ps.p, (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p); free(bx.p); free(by.p);
-  return rc;
+  return req_wiso_quality(env, h, w, range_rows(rowBegin, rowEnd), x, y, nBins, sums, binWeight, binPosWeight, binPsum,
+                          words);
 }
 FN(evalSampledWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd,
                                            jlong key, jlong posBegin, jlong posEnd, jdoubleArray x, jdoubleArray y,
                                            jint nBins, jdoubleArray sums, jdoubleArray binWeight,
                                            jdoubleArray binPosWeight, jdoubleArray binPsum, jlongArray words) {
-  buf_t bw = in_Double(env, w), bx = in_Double(env, x), by = in_Double(env, y);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bx.bad | by.bad | wquality_bad(&q)))
-    rc = wiso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_sampled_weighted_isotonic_calibration(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin,
-                                                               posEnd, bx.p, by.p, bx.n, nBins, q.s.p, q.wt.p, q.pw.p,
-                                                               q.ps.p, (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p); free(bx.p); free(by.p);
-  return rc;
+  return req_wiso_quality(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), x, y, nBins, sums, binWeight,
+                          binPosWeight, binPsum, words);
 }
 FN(evalSamplesWeightedIsotonicCalibration)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples,
                                            jdoubleArray x, jdoubleArray y, jint nBins, jdoubleArray sums,
                                            jdoubleArray binWeight, jdoubleArray binPosWeight, jdoubleArray binPsum,
                                            jlongArray words) {
-  buf_t bw = in_Double(env, w), bs = in_Int(env, samples), bx = in_Double(env, x), by = in_Double(env, y);
-  wquality_bufs q = wquality_out(env, sums, binWeight, binPosWeight, binPsum, words);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bx.bad | by.bad | wquality_bad(&q)))
-    rc = wiso_quality_short(&q, nBins, &bx, &by)
-             ? DSGD_ERR_INVALID
-             : dsgd_eval_samples_weighted_isotonic_calibration(CTX(h), bw.p, bs.p, bs.n, bx.p, by.p, bx.n, nBins, q.s.p,
-                                                               q.wt.p, q.pw.p, q.ps.p, (int64_t *)q.wd.p);
-  wquality_back(env, sums, binWeight, binPosWeight, binPsum, words, &q, rc);
-  free(bw.p); free(bs.p); free(bx.p); free(by.p);
-  return rc;
+  return req_wiso_quality(env, h, w, list_rows(samples), x, y, nBins, sums, binWeight, binPosWeight, binPsum, words);
 }
 
 /* ---- sync mode ---- */
@@ -1016,17 +793,10 @@ FN(averageBegin)(JNIEnv *env, jobject self, jlong h) { return dsgd_average_begin
 FN(averageEnd)(JNIEnv *env, jobject self, jlong h) { return dsgd_average_end(CTX(h)); }
 FN(averageWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray avg, jlongArray nSteps) {
   buf_t ba = out_Double(env, avg), bn = out_Long(env, nSteps);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(ba.bad | bn.bad))
-    rc = (bn.p && bn.n < 1) ? DSGD_ERR_INVALID : dsgd_average_weights(CTX(h), (double *)ba.p, (int64_t *)bn.p);
+  int rc = checked(sized(h, &ba, WEIGHTS, AT_LEAST), bn.bad, short_of(&bn, 1));
+  if (rc == DSGD_OK) rc = dsgd_average_weights(CTX(h), (double *)ba.p, (int64_t *)bn.p);
   back_Double(env, avg, ba, rc);
   back_Long(env, nSteps, bn, rc);
-  return rc;
-}
-/* The length of a weight vector of the ctx: dim, or dim + 1 on a ctx created with DSGD_FLAG_INTERCEPT (dsgd_info names it) */
-static int weight_len(jlong h, int32_t *n) {
-  int rc = dsgd_dim(CTX(h), n);
-  if (rc == DSGD_OK && strstr(dsgd_info(CTX(h)), "\"intercept\": true")) ++*n;
   return rc;
 }
 /* L1 penalty of the sync steps: setL1(lambda1 >= 0); weightsL1: l1(0) = ||w||_1 and nnz(0) = the non-zero weights of w (dim
@@ -1034,16 +804,13 @@ static int weight_len(jlong h, int32_t *n) {
  * length, or an empty output array, is DSGD_ERR_INVALID. */
 FN(setL1)(JNIEnv *env, jobject self, jlong h, jdouble lambda1) { return dsgd_set_l1(CTX(h), lambda1); }
 FN(weightsL1)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jdoubleArray l1, jlongArray nnz) {
-  buf_t bw = in_Double(env, w), bl = out_Double(env, l1), bn = out_Long(env, nnz);
-  int rc = DSGD_ERR_NOMEM;
-  int32_t dim = 0;
-  if (!(bw.bad | bl.bad | bn.bad) && (rc = weight_len(h, &dim)) == DSGD_OK)
-    rc = (bw.p && (int32_t)bw.n != dim) || (bl.p && bl.n < 1) || (bn.p && bn.n < 1)
-             ? DSGD_ERR_INVALID
-             : dsgd_weights_l1(CTX(h), (const double *)bw.p, (double *)bl.p, (int64_t *)bn.p);
+  req_t q;
+  buf_t bl = out_Double(env, l1), bn = out_Long(env, nnz);
+  int rc = checked(req_open(env, h, w, no_rows(), &q), bl.bad | bn.bad, short_of(&bl, 1) || short_of(&bn, 1));
+  if (rc == DSGD_OK) rc = dsgd_weights_l1(CTX(h), (const double *)q.w.p, (double *)bl.p, (int64_t *)bn.p);
   back_Double(env, l1, bl, rc);
   back_Long(env, nnz, bn, rc);
-  free(bw.p);
+  req_close(&q);
   return rc;
 }
 /* Class weights of the sync steps and of gradient: setClassWeights(wPos, wNeg), both finite and >= 0; getClassWeights:
@@ -1059,165 +826,110 @@ FN(getClassWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray out) {
   back_Double(env, out, bo, rc);
   return rc;
 }
+static int req_class(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray sums, jlongArray counts) {
+  req_t q;
+  buf_t s = out_Double(env, sums), c = out_Long(env, counts);
+  int rc = checked(req_open(env, h, w, r, &q), s.bad | c.bad, s.n < 3 || c.n < 4);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_class, dsgd_eval_sampled_class, dsgd_eval_samples_class, (double *)s.p, (double *)s.p + 1,
+                  (int64_t *)c.p);
+  back_Double(env, sums, s, rc);
+  back_Long(env, counts, c, rc);
+  req_close(&q);
+  return rc;
+}
 FN(evalClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray sums,
               jlongArray counts) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad))
-    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
-                                : dsgd_eval_class(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_class(env, h, w, range_rows(rowBegin, rowEnd), sums, counts);
 }
 FN(evalSampledClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                      jlong posBegin, jlong posEnd, jdoubleArray sums, jlongArray counts) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad))
-    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
-                                : dsgd_eval_sampled_class(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd,
-                                                          (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_class(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), sums, counts);
 }
 FN(evalSamplesClass)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray sums,
                      jlongArray counts) {
-  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bi.bad | bs.bad | bc.bad))
-    rc = (bs.n < 3 || bc.n < 4) ? DSGD_ERR_INVALID
-                                : dsgd_eval_samples_class(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (double *)bs.p + 1,
-                                                          (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p); free(bi.p);
-  return rc;
+  return req_class(env, h, w, list_rows(samples), sums, counts);
 }
 
 /* Sample weights of the sync steps, of gradient and of the weighted evaluations: setSampleWeights(sw), one weight per loaded
  * row (finite and >= 0; the library checks the length against the rows), null clears them.  The weighted evaluations, either
- * model: sums(0) = ||w||^2, sums(1..3) = S = sum c_i L_i, sum c_i [correct], sum c_i; counts(0..1) = rows, correct.  A w
- * whose length is not dim, or a shorter output, is DSGD_ERR_INVALID. */
+ * model: sums(0) = ||w||^2, sums(1..3) = S = sum c_i L_i, sum c_i [correct], sum c_i; counts(0..1) = rows, correct.  A
+ * shorter output is DSGD_ERR_INVALID. */
 FN(setSampleWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray sw) {
   buf_t b = in_Double(env, sw);
   int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_set_sample_weights(CTX(h), (const double *)b.p, b.p ? (int64_t)b.n : 0);
   free(b.p);
   return rc;
 }
-/* DSGD_OK when w is null or holds a weight vector (weight_len values) and the outputs are long enough */
-static int weighted_args(jlong h, const buf_t *bw, const buf_t *bs, const buf_t *bc) {
-  int32_t dim = 0;
-  int rc = weight_len(h, &dim);
-  if (rc) return rc;
-  return ((bw->p && (int32_t)bw->n != dim) || bs->n < 4 || bc->n < 2) ? DSGD_ERR_INVALID : DSGD_OK;
+static int req_weighted(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray sums, jlongArray counts) {
+  req_t q;
+  buf_t s = out_Double(env, sums), c = out_Long(env, counts);
+  int rc = checked(req_open(env, h, w, r, &q), s.bad | c.bad, s.n < 4 || c.n < 2);
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_weighted, dsgd_eval_sampled_weighted, dsgd_eval_samples_weighted, (double *)s.p,
+                  (double *)s.p + 1, (int64_t *)c.p);
+  back_Double(env, sums, s, rc);
+  back_Long(env, counts, c, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jdoubleArray sums,
                  jlongArray counts) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
-    rc = dsgd_eval_weighted(CTX(h), bw.p, rowBegin, rowEnd, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_weighted(env, h, w, range_rows(rowBegin, rowEnd), sums, counts);
 }
 FN(evalSampledWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                         jlong posBegin, jlong posEnd, jdoubleArray sums, jlongArray counts) {
-  buf_t bw = in_Double(env, w), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
-    rc = dsgd_eval_sampled_weighted(CTX(h), bw.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (double *)bs.p,
-                                    (double *)bs.p + 1, (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p);
-  return rc;
+  return req_weighted(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), sums, counts);
 }
 FN(evalSamplesWeighted)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jdoubleArray sums,
                         jlongArray counts) {
-  buf_t bw = in_Double(env, w), bi = in_Int(env, samples), bs = out_Double(env, sums), bc = out_Long(env, counts);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | bi.bad | bs.bad | bc.bad) && (rc = weighted_args(h, &bw, &bs, &bc)) == DSGD_OK)
-    rc = dsgd_eval_samples_weighted(CTX(h), bw.p, bi.p, bi.n, (double *)bs.p, (double *)bs.p + 1, (int64_t *)bc.p);
-  back_Double(env, sums, bs, rc);
-  back_Long(env, counts, bc, rc);
-  free(bw.p); free(bi.p);
-  return rc;
+  return req_weighted(env, h, w, list_rows(samples), sums, counts);
 }
 
 /* weighted curves: metrics(0..7) as the curve calls', wsums(0 until DSGD_WCURVE_WORDS) the weighted words, nPoints(0) = m, and
  * thr / tpw / fpw (0 until m) the points -- all three null for the words alone, else each at least as long as the request's
- * rows.  w is null or holds dim values.  A shorter array is DSGD_ERR_INVALID, checked before the call. */
-typedef struct { buf_t w, m, s, k, t, tp, fp; } wcurve_bufs;
-static wcurve_bufs wcurve_in(JNIEnv *env, jdoubleArray w, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints,
-                             jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
-  wcurve_bufs c = {in_Double(env, w),      out_Long(env, metrics), out_Double(env, wsums), out_Long(env, nPoints),
-                   out_Double(env, thr),   out_Double(env, tpw),   out_Double(env, fpw)};
-  return c;
-}
-static int wcurve_bad(const wcurve_bufs *c) { return c->w.bad | c->m.bad | c->s.bad | c->k.bad | c->t.bad | c->tp.bad | c->fp.bad; }
-static int wcurve_args(jlong h, const wcurve_bufs *c, jlong n) {
-  int32_t dim = 0;
-  int rc = weight_len(h, &dim);
-  if (rc) return rc;
-  if ((c->w.p && (int32_t)c->w.n != dim) || c->m.n < DSGD_METRICS_WORDS || c->s.n < DSGD_WCURVE_WORDS || c->k.n < 1)
-    return DSGD_ERR_INVALID;
-  return ((c->t.p && c->t.n < n) || (c->tp.p && c->tp.n < n) || (c->fp.p && c->fp.n < n)) ? DSGD_ERR_INVALID : DSGD_OK;
-}
-static void wcurve_back(JNIEnv *env, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr,
-                        jdoubleArray tpw, jdoubleArray fpw, wcurve_bufs *c, int rc) {
-  back_Long(env, metrics, c->m, rc);
-  back_Double(env, wsums, c->s, rc);
-  back_Long(env, nPoints, c->k, rc);
-  back_Double(env, thr, c->t, rc);
-  back_Double(env, tpw, c->tp, rc);
-  back_Double(env, fpw, c->fp, rc);
-  free(c->w.p);
+ * rows.  A shorter array is DSGD_ERR_INVALID, checked before the call. */
+static int req_wcurve(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jlongArray metrics, jdoubleArray wsums,
+                      jlongArray nPoints, jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
+  req_t q;
+  buf_t m = out_Long(env, metrics), s = out_Double(env, wsums), k = out_Long(env, nPoints), t = out_Double(env, thr),
+        bt = out_Double(env, tpw), bf = out_Double(env, fpw);
+  int rc = req_open(env, h, w, r, &q);
+  const jlong n = rows_n(&q);
+  rc = checked(rc, m.bad | s.bad | k.bad | t.bad | bt.bad | bf.bad,
+               m.n < DSGD_METRICS_WORDS || s.n < DSGD_WCURVE_WORDS || k.n < 1 || short_of(&t, n) || short_of(&bt, n) ||
+                   short_of(&bf, n));
+  if (rc == DSGD_OK)
+    rc = ROW_CALL(h, q, dsgd_eval_weighted_curve, dsgd_eval_sampled_weighted_curve, dsgd_eval_samples_weighted_curve,
+                  (int64_t *)m.p, (double *)s.p, (int64_t *)k.p, (double *)t.p, (double *)bt.p, (double *)bf.p);
+  back_Long(env, metrics, m, rc);
+  back_Double(env, wsums, s, rc);
+  back_Long(env, nPoints, k, rc);
+  back_Double(env, thr, t, rc);
+  back_Double(env, tpw, bt, rc);
+  back_Double(env, fpw, bf, rc);
+  req_close(&q);
+  return rc;
 }
 FN(evalWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlongArray metrics,
                       jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
-  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
-  int rc = DSGD_ERR_NOMEM;
-  if (!wcurve_bad(&c) && (rc = wcurve_args(h, &c, rowEnd - rowBegin)) == DSGD_OK)
-    rc = dsgd_eval_weighted_curve(CTX(h), c.w.p, rowBegin, rowEnd, (int64_t *)c.m.p, (double *)c.s.p, (int64_t *)c.k.p,
-                                  (double *)c.t.p, (double *)c.tp.p, (double *)c.fp.p);
-  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
-  return rc;
+  return req_wcurve(env, h, w, range_rows(rowBegin, rowEnd), metrics, wsums, nPoints, thr, tpw, fpw);
 }
 FN(evalSampledWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jlong rowBegin, jlong rowEnd, jlong key,
                              jlong posBegin, jlong posEnd, jlongArray metrics, jdoubleArray wsums, jlongArray nPoints,
                              jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
-  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
-  int rc = DSGD_ERR_NOMEM;
-  if (!wcurve_bad(&c) && (rc = wcurve_args(h, &c, posEnd - posBegin)) == DSGD_OK)
-    rc = dsgd_eval_sampled_weighted_curve(CTX(h), c.w.p, rowBegin, rowEnd, (uint64_t)key, posBegin, posEnd, (int64_t *)c.m.p,
-                                          (double *)c.s.p, (int64_t *)c.k.p, (double *)c.t.p, (double *)c.tp.p,
-                                          (double *)c.fp.p);
-  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
-  return rc;
+  return req_wcurve(env, h, w, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), metrics, wsums, nPoints, thr, tpw, fpw);
 }
 FN(evalSamplesWeightedCurve)(JNIEnv *env, jobject self, jlong h, jdoubleArray w, jintArray samples, jlongArray metrics,
                              jdoubleArray wsums, jlongArray nPoints, jdoubleArray thr, jdoubleArray tpw, jdoubleArray fpw) {
-  buf_t bi = in_Int(env, samples);
-  wcurve_bufs c = wcurve_in(env, w, metrics, wsums, nPoints, thr, tpw, fpw);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bi.bad | wcurve_bad(&c)) && (rc = wcurve_args(h, &c, bi.n)) == DSGD_OK)
-    rc = dsgd_eval_samples_weighted_curve(CTX(h), c.w.p, bi.p, bi.n, (int64_t *)c.m.p, (double *)c.s.p, (int64_t *)c.k.p,
-                                          (double *)c.t.p, (double *)c.tp.p, (double *)c.fp.p);
-  wcurve_back(env, metrics, wsums, nPoints, thr, tpw, fpw, &c, rc);
-  free(bi.p);
-  return rc;
+  return req_wcurve(env, h, w, list_rows(samples), metrics, wsums, nPoints, thr, tpw, fpw);
 }
 
 /* ---- async (Hogwild) mode ---- */
 FN(asyncHostMaster)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0) {
   buf_t b = in_Double(env, w0);
-  int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_async_host_master(CTX(h), b.p);   /* GradState of MasterAsync, core/MasterAsync.scala:66 */
+  int rc = sized(h, &b, DIM, EXACTLY);
+  if (rc == DSGD_OK) rc = dsgd_async_host_master(CTX(h), b.p);   /* GradState of MasterAsync, core/MasterAsync.scala:66 */
   free(b.p);
   return rc;
 }
@@ -1240,8 +952,8 @@ FN(peerAttach)(JNIEnv *env, jobject self, jlong h, jint peerRank, jlong peer, ji
 FN(startAsync)(JNIEnv *env, jobject self, jlong h, jdoubleArray w0, jintArray assigned, jint batch, jdouble lr,
                jint concurrency, jlong maxUpdates, jlong seed) {
   buf_t bw = in_Double(env, w0), ba = in_Int(env, assigned);
-  int rc = DSGD_ERR_NOMEM;
-  if (!(bw.bad | ba.bad))
+  int rc = checked(sized(h, &bw, DIM, EXACTLY), ba.bad, 0);
+  if (rc == DSGD_OK)
     rc = dsgd_start_async(CTX(h), bw.p, ba.p, ba.n, batch, lr, concurrency, maxUpdates, (uint64_t)seed);  /* core/Slave.scala:159-175 */
   free(bw.p); free(ba.p);
   return rc;
@@ -1268,7 +980,8 @@ FN(asyncUpdates)(JNIEnv *env, jobject self, jlong h, jlongArray out) {
 }
 FN(asyncMasterWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray out) {
   buf_t b = out_Double(env, out);
-  int rc = b.bad ? DSGD_ERR_NOMEM : dsgd_async_master_weights(CTX(h), b.p);   /* gradState.single().grad, core/MasterAsync.scala:109 */
+  int rc = sized(h, &b, DIM, AT_LEAST);
+  if (rc == DSGD_OK) rc = dsgd_async_master_weights(CTX(h), b.p);   /* gradState.single().grad, core/MasterAsync.scala:109 */
   back_Double(env, out, b, rc);
   return rc;
 }
@@ -1278,7 +991,8 @@ FN(asyncOutboxEnable)(JNIEnv *env, jobject self, jlong h) {
 }
 FN(asyncOutboxRead)(JNIEnv *env, jobject self, jlong h, jdoubleArray out) {
   buf_t b = out_Double(env, out);
-  int rc = b.bad ? DSGD_ERR_NOMEM : (b.n < 1 ? DSGD_ERR_INVALID : dsgd_async_outbox_read(CTX(h), b.p));
+  int rc = sized(h, &b, DIM, AT_LEAST);
+  if (rc == DSGD_OK) rc = dsgd_async_outbox_read(CTX(h), b.p);
   back_Double(env, out, b, rc);
   return rc;
 }

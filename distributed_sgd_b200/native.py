@@ -111,59 +111,10 @@ ABI = {
     "dsgd_forward": [_vp, _vp, _vp, _i64, _vp],
     "dsgd_gradient": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64)],
     "dsgd_eval": [_vp, _vp, _i64, _i64, C.POINTER(_f64), C.POINTER(_f64)],
-    "dsgd_eval_counts": [_vp, _vp, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
-    "dsgd_eval_sampled_counts": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
-    "dsgd_eval_samples_counts": [_vp, _vp, _vp, _i64, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_f64)],
-    "dsgd_eval_sums": [_vp, _vp, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
-    "dsgd_eval_sampled_sums": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
-    "dsgd_eval_samples_sums": [_vp, _vp, _vp, _i64, C.POINTER(_f64), C.POINTER(_i64), C.POINTER(_f64)],
     "dsgd_margins": [_vp, _vp, _vp, _i64, _vp],
     "dsgd_probabilities": [_vp, _vp, _vp, _i64, _vp],
-    "dsgd_eval_metrics": [_vp, _vp, _i64, _i64, _vp],
-    "dsgd_eval_sampled_metrics": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp],
-    "dsgd_eval_samples_metrics": [_vp, _vp, _vp, _i64, _vp],
-    "dsgd_calibrate": [_vp, _vp, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_calibrate_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_calibrate_samples": [_vp, _vp, _vp, _i64, _vp, _vp, _vp],
     "dsgd_calibrated_probabilities": [_vp, _vp, _vp, _i64, _f64, _f64, _vp],
-    "dsgd_eval_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_sampled_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_samples_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_weighted": [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_weighted_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_weighted_samples": [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp],
-    "dsgd_eval_weighted_calibration": [_vp, _vp, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_sampled_weighted_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp,
-                                               _vp],
-    "dsgd_eval_samples_weighted_calibration": [_vp, _vp, _vp, _i64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_isotonic_weighted": [_vp, _vp, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_isotonic_weighted_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp,
-                                                 _vp, _vp],
-    "dsgd_calibrate_isotonic_weighted_samples": [_vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_weighted_isotonic_calibration": [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_sampled_weighted_isotonic_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _i64, _i32, _vp,
-                                                        _vp, _vp, _vp, _vp],
-    "dsgd_eval_samples_weighted_isotonic_calibration": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_isotonic": [_vp, _vp, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_isotonic_sampled": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
-    "dsgd_calibrate_isotonic_samples": [_vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _vp, _vp, _vp, _vp],
     "dsgd_isotonic_probabilities": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp],
-    "dsgd_eval_isotonic_calibration": [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_sampled_isotonic_calibration": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp,
-                                               _vp, _vp],
-    "dsgd_eval_samples_isotonic_calibration": [_vp, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp],
-    "dsgd_eval_curve": [_vp, _vp, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
-    "dsgd_eval_sampled_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
-    "dsgd_eval_samples_curve": [_vp, _vp, _vp, _i64, _vp, C.POINTER(_f64), C.POINTER(_i64), _vp, _vp, _vp],
-    "dsgd_eval_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_sampled_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_samples_bootstrap": [_vp, _vp, _vp, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_weighted_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_sampled_weighted_bootstrap": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_samples_weighted_bootstrap": [_vp, _vp, _vp, _i64, _u64, _i64, _i64, _vp, _vp, _vp],
-    "dsgd_eval_weighted_curve": [_vp, _vp, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
-    "dsgd_eval_sampled_weighted_curve": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
-    "dsgd_eval_samples_weighted_curve": [_vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(_i64), _vp, _vp, _vp],
     "dsgd_comm_unique_id": [_vp],
     "dsgd_comm_init": [_vp, _vp],
     "dsgd_xchg_export": [_vp, _vp],
@@ -189,13 +140,7 @@ ABI = {
     "dsgd_weights_l1": [_vp, _vp, C.POINTER(_f64), C.POINTER(_i64)],
     "dsgd_set_class_weights": [_vp, _f64, _f64],
     "dsgd_get_class_weights": [_vp, C.POINTER(_f64), C.POINTER(_f64)],
-    "dsgd_eval_class": [_vp, _vp, _i64, _i64, C.POINTER(_f64), _vp, _vp],
-    "dsgd_eval_sampled_class": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), _vp, _vp],
-    "dsgd_eval_samples_class": [_vp, _vp, _vp, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_set_sample_weights": [_vp, _vp, _i64],
-    "dsgd_eval_weighted": [_vp, _vp, _i64, _i64, C.POINTER(_f64), _vp, _vp],
-    "dsgd_eval_sampled_weighted": [_vp, _vp, _i64, _i64, _u64, _i64, _i64, C.POINTER(_f64), _vp, _vp],
-    "dsgd_eval_samples_weighted": [_vp, _vp, _vp, _i64, C.POINTER(_f64), _vp, _vp],
     "dsgd_async_host_master": [_vp, _vp],
     "dsgd_ipc_export": [_vp, C.c_int, _vp],
     "dsgd_ipc_import": [_vp, C.c_int, _vp],
@@ -212,6 +157,36 @@ ABI = {
     "dsgd_async_updates": [_vp, C.POINTER(_i64)],
 }
 _RESTYPE = {"dsgd_last_error": C.c_char_p, "dsgd_info": C.c_char_p}
+
+# The evaluation families: each has a range, a drawn-sample and an id-list entry point, (ctx, w) and the rows of that form
+# (_ROW_PREFIX), then the family's own arguments (below)
+_ROW_PREFIX = {"range": [_vp, _vp, _i64, _i64], "drawn": [_vp, _vp, _i64, _i64, _u64, _i64, _i64], "list": [_vp, _vp, _vp, _i64]}
+_PI64, _PF64 = C.POINTER(_i64), C.POINTER(_f64)
+_QUALITY = [_f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp]                  # (a, b), n_bins, the quality outputs
+_ISO_QUALITY = [_vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp]          # the map (x, y, k), n_bins, the quality outputs
+_BOOTSTRAP = [_u64, _i64, _i64, _vp, _vp, _vp]                          # bkey, [b_begin, b_end), the replicate outputs
+_ROW_FAMILIES = {
+    "eval_counts": [_PI64, _PI64, _PF64], "eval_sums": [_PF64, _PI64, _PF64], "eval_class": [_PF64, _vp, _vp],
+    "eval_weighted": [_PF64, _vp, _vp], "eval_metrics": [_vp], "eval_curve": [_vp, _PF64, _PI64, _vp, _vp, _vp],
+    "eval_weighted_curve": [_vp, _vp, _PI64, _vp, _vp, _vp], "eval_bootstrap": _BOOTSTRAP,
+    "eval_weighted_bootstrap": _BOOTSTRAP, "calibrate": [_vp, _vp, _vp], "calibrate_weighted": [_vp, _vp, _vp, _vp],
+    "eval_calibration": _QUALITY, "eval_weighted_calibration": _QUALITY, "calibrate_isotonic": [_PI64] + [_vp] * 5,
+    "calibrate_isotonic_weighted": [_PI64] + [_vp] * 6, "eval_isotonic_calibration": _ISO_QUALITY,
+    "eval_weighted_isotonic_calibration": _ISO_QUALITY,
+}
+
+
+def _row_forms(family: str) -> dict:
+    """{form: entry point} of an evaluation family: dsgd_<fit>, _sampled, _samples for a fit; dsgd_eval_, eval_sampled_,
+    eval_samples_<rest> for the others."""
+    if family.startswith("calibrate"):
+        return {"range": f"dsgd_{family}", "drawn": f"dsgd_{family}_sampled", "list": f"dsgd_{family}_samples"}
+    rest = family[len("eval_"):]
+    return {"range": f"dsgd_eval_{rest}", "drawn": f"dsgd_eval_sampled_{rest}", "list": f"dsgd_eval_samples_{rest}"}
+
+
+ABI.update({name: _ROW_PREFIX[form] + tail for family, tail in _ROW_FAMILIES.items()
+            for form, name in _row_forms(family).items()})
 
 
 def lib():
@@ -260,9 +235,27 @@ def host_lib():
     return _host
 
 
-def _drawn(row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int) -> tuple:
-    """The row arguments of a sample drawn on the device from rows [row_begin, row_end): the key goes in as 64 bits."""
-    return row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF, pos_begin, pos_end
+class _Rows(NamedTuple):
+    """The rows of one request: the C arguments of its form, the number of rows, and the id array those arguments point
+    into (held here so that it outlives the call)."""
+    args: tuple
+    n: int
+    ids: Optional[np.ndarray] = None
+
+
+def _range(row_begin: int, row_end: int) -> _Rows:
+    return _Rows((row_begin, row_end), row_end - row_begin)
+
+
+def _drawn(row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int) -> _Rows:
+    """Positions [pos_begin, pos_end) of a sample drawn on the device from rows [row_begin, row_end): the key goes in as
+    64 bits."""
+    return _Rows((row_begin, row_end, int(key) & 0xFFFFFFFFFFFFFFFF, pos_begin, pos_end), pos_end - pos_begin)
+
+
+def _list(samples) -> _Rows:
+    ids = _arr(samples, np.int32)
+    return _Rows((_ptr(ids), ids.size), ids.size, ids)
 
 
 # out-parameters of the dsgd_eval_*counts and dsgd_eval_*sums calls: (hinge sum | loss sum, correct count, ||w||^2)
@@ -446,37 +439,37 @@ class NativeCtx:
     def _w(self, w):
         return None if w is None else _arr(w, np.float64, self.wdim, "weights")
 
+    def _call(self, fn: str, w, rows: _Rows, *args):
+        """dsgd_<fn>(ctx, w, *rows, *args), checked; w None: the resident weights."""
+        w = self._w(w)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows.args, *args))
+
     def forward(self, samples, w=None) -> np.ndarray:
-        samples = _arr(samples, np.int32)
-        return self._request("forward", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
+        rows = _list(samples)
+        return self._request("forward", w, rows, np.zeros(rows.n, dtype=np.float64))
 
     def gradient(self, samples, w=None, want_loss: bool = False):
-        samples = _arr(samples, np.int32)
         out = np.zeros(self.wdim, dtype=np.float64)
         loss = C.c_double()
-        w = self._w(w)
-        self._ck(self._l.dsgd_gradient(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(out),
-                                       C.byref(loss) if want_loss else None))
+        self._call("gradient", w, _list(samples), _ptr(out), C.byref(loss) if want_loss else None)
         return (out, loss.value) if want_loss else out
 
-    def _request(self, fn: str, w, rows: tuple, out):
-        """dsgd_<fn>(ctx, w, *rows, out...).  rows: (row_begin, row_end), _drawn(...) or (ids pointer, len(ids)).  out: an
-        array, filled and returned, or ctypes scalar types, passed by reference and returned as a tuple of values."""
-        w = self._w(w)
-        call = getattr(self._l, "dsgd_" + fn)
+    def _request(self, fn: str, w, rows: _Rows, out):
+        """dsgd_<fn>(ctx, w, *rows, out...).  out: an array, filled and returned, or ctypes scalar types, passed by reference
+        and returned as a tuple of values."""
         if isinstance(out, np.ndarray):
-            self._ck(call(self._h, _ptr(w), *rows, _ptr(out)))
+            self._call(fn, w, rows, _ptr(out))
             return out
         vals = [t() for t in out]
-        self._ck(call(self._h, _ptr(w), *rows, *[C.byref(v) for v in vals]))
+        self._call(fn, w, rows, *[C.byref(v) for v in vals])
         return tuple([v.value for v in vals])
 
     def eval(self, row_begin: int, row_end: int, w=None) -> Tuple[float, float]:
-        return self._request("eval", w, (row_begin, row_end), (_f64, _f64))
+        return self._request("eval", w, _range(row_begin, row_end), (_f64, _f64))
 
     def eval_counts(self, row_begin: int, row_end: int, w=None) -> Tuple[int, int, float]:
         """(hinge sum, correct count, ||w||^2) over rows [row_begin, row_end) -- exact shardable form."""
-        return self._request("eval_counts", w, (row_begin, row_end), _COUNTS)
+        return self._request("eval_counts", w, _range(row_begin, row_end), _COUNTS)
 
     def eval_sampled_counts(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                             w=None) -> Tuple[int, int, float]:
@@ -486,12 +479,11 @@ class NativeCtx:
 
     def eval_samples_counts(self, samples, w=None) -> Tuple[int, int, float]:
         """The same counters over a list of row ids; repeats count every time (dsgd_eval_samples_counts)."""
-        samples = _arr(samples, np.int32)
-        return self._request("eval_samples_counts", w, (_ptr(samples), samples.size), _COUNTS)
+        return self._request("eval_samples_counts", w, _list(samples), _COUNTS)
 
     def eval_sums(self, row_begin: int, row_end: int, w=None) -> Tuple[float, int, float]:
         """(loss sum, correct count, ||w||^2) over rows [row_begin, row_end), for either model (dsgd_eval_sums)."""
-        return self._request("eval_sums", w, (row_begin, row_end), _SUMS)
+        return self._request("eval_sums", w, _range(row_begin, row_end), _SUMS)
 
     def eval_sampled_sums(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                           w=None) -> Tuple[float, int, float]:
@@ -501,24 +493,23 @@ class NativeCtx:
 
     def eval_samples_sums(self, samples, w=None) -> Tuple[float, int, float]:
         """(loss sum, correct count, ||w||^2) over a list of row ids; repeats count every time (dsgd_eval_samples_sums)."""
-        samples = _arr(samples, np.int32)
-        return self._request("eval_samples_sums", w, (_ptr(samples), samples.size), _SUMS)
+        return self._request("eval_samples_sums", w, _list(samples), _SUMS)
 
     # -- scores and ranking metrics --
     def margins(self, samples, w=None) -> np.ndarray:
         """x . w in fp64 for each listed row (dsgd_margins)."""
-        samples = _arr(samples, np.int32)
-        return self._request("margins", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
+        rows = _list(samples)
+        return self._request("margins", w, rows, np.zeros(rows.n, dtype=np.float64))
 
     def probabilities(self, samples, w=None) -> np.ndarray:
         """P(y = +1 | x) for each listed row (dsgd_probabilities): sigmoid(-x . w) on a SparseLogistic context,
         (clip(-x . w, -1, 1) + 1) / 2 on a SparseModifiedHuber one; other models raise DsgdState."""
-        samples = _arr(samples, np.int32)
-        return self._request("probabilities", w, (_ptr(samples), samples.size), np.zeros(samples.size, dtype=np.float64))
+        rows = _list(samples)
+        return self._request("probabilities", w, rows, np.zeros(rows.n, dtype=np.float64))
 
     def eval_metrics(self, row_begin: int, row_end: int, w=None) -> np.ndarray:
         """The METRICS_WORDS exact counts over rows [row_begin, row_end) (dsgd_eval_metrics)."""
-        return self._request("eval_metrics", w, (row_begin, row_end), np.zeros(METRICS_WORDS, dtype=np.int64))
+        return self._request("eval_metrics", w, _range(row_begin, row_end), np.zeros(METRICS_WORDS, dtype=np.int64))
 
     def eval_sampled_metrics(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                              w=None) -> np.ndarray:
@@ -528,25 +519,22 @@ class NativeCtx:
 
     def eval_samples_metrics(self, samples, w=None) -> np.ndarray:
         """The same counts over a list of row ids; repeats count every time (dsgd_eval_samples_metrics)."""
-        samples = _arr(samples, np.int32)
-        return self._request("eval_samples_metrics", w, (_ptr(samples), samples.size),
-                             np.zeros(METRICS_WORDS, dtype=np.int64))
+        return self._request("eval_samples_metrics", w, _list(samples), np.zeros(METRICS_WORDS, dtype=np.int64))
 
     # -- calibration --
-    def _calibrate(self, fn: str, w, rows: tuple):
+    def _calibrate(self, fn: str, w, rows: _Rows):
         """dsgd_<fn>: (A, B, objective, info) of one Platt fit; info = the CALIBRATION_INFO_WORDS words {iterations, status,
         rows used, NaN rows, points evaluated}."""
-        w = self._w(w)
         ab = np.zeros(2, dtype=np.float64)
         info = np.zeros(CALIBRATION_INFO_WORDS, dtype=np.int64)
         obj = C.c_double()
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(ab), C.byref(obj), _ptr(info)))
+        self._call(fn, w, rows, _ptr(ab), C.byref(obj), _ptr(info))
         return float(ab[0]), float(ab[1]), obj.value, info
 
     def calibrate(self, row_begin: int, row_end: int, w=None):
         """Platt scaling of x . w over rows [row_begin, row_end) (dsgd_calibrate): (A, B, objective, info) with
         P(y = +1 | x) = 1 / (1 + exp(A x . w + B))."""
-        return self._calibrate("calibrate", w, (row_begin, row_end))
+        return self._calibrate("calibrate", w, _range(row_begin, row_end))
 
     def calibrate_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_sampled)."""
@@ -554,33 +542,29 @@ class NativeCtx:
 
     def calibrate_samples(self, samples, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_calibrate_samples)."""
-        samples = _arr(samples, np.int32)
-        return self._calibrate("calibrate_samples", w, (_ptr(samples), samples.size))
+        return self._calibrate("calibrate_samples", w, _list(samples))
 
     def calibrated_probabilities(self, samples, a: float, b: float, w=None) -> np.ndarray:
         """sigmoid(-(a x . w + b)) for each listed row, either model (dsgd_calibrated_probabilities)."""
-        samples = _arr(samples, np.int32)
-        w = self._w(w)
-        out = np.zeros(samples.size, dtype=np.float64)
-        self._ck(self._l.dsgd_calibrated_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, float(a), float(b),
-                                                       _ptr(out)))
+        rows = _list(samples)
+        out = np.zeros(rows.n, dtype=np.float64)
+        self._call("calibrated_probabilities", w, rows, float(a), float(b), _ptr(out))
         return out
 
-    def _eval_calibration(self, fn: str, w, rows: tuple, a: float, b: float, n_bins: int):
+    def _eval_calibration(self, fn: str, w, rows: _Rows, a: float, b: float, n_bins: int):
         """dsgd_<fn>: (sums, bin_rows, bin_pos, bin_psum, words): sums = {Brier, log loss} sums, words = {rows used, rows
         left out}."""
-        w = self._w(w)
         m = max(int(n_bins), 1)
         sums, words = np.zeros(2, dtype=np.float64), np.zeros(2, dtype=np.int64)
         rows_b, pos_b, psum = np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.float64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, float(a), float(b), int(n_bins), _ptr(sums),
-                                                 _ptr(rows_b), _ptr(pos_b), _ptr(psum), _ptr(words)))
+        self._call(fn, w, rows, float(a), float(b), int(n_bins), _ptr(sums), _ptr(rows_b), _ptr(pos_b), _ptr(psum),
+                   _ptr(words))
         return sums, rows_b, pos_b, psum, words
 
     def eval_calibration(self, row_begin: int, row_end: int, a: float, b: float, n_bins: int = 10, w=None):
         """Brier and log-loss sums and n_bins reliability bins at (a, b) over rows [row_begin, row_end)
         (dsgd_eval_calibration)."""
-        return self._eval_calibration("eval_calibration", w, (row_begin, row_end), a, b, n_bins)
+        return self._eval_calibration("eval_calibration", w, _range(row_begin, row_end), a, b, n_bins)
 
     def eval_sampled_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, a: float,
                                  b: float, n_bins: int = 10, w=None):
@@ -590,24 +574,22 @@ class NativeCtx:
 
     def eval_samples_calibration(self, samples, a: float, b: float, n_bins: int = 10, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_calibration)."""
-        samples = _arr(samples, np.int32)
-        return self._eval_calibration("eval_samples_calibration", w, (_ptr(samples), samples.size), a, b, n_bins)
+        return self._eval_calibration("eval_samples_calibration", w, _list(samples), a, b, n_bins)
 
     # -- weighted calibration --
-    def _calibrate_weighted(self, fn: str, w, rows: tuple):
+    def _calibrate_weighted(self, fn: str, w, rows: _Rows):
         """dsgd_<fn>: (A, B, objective, info, wsums) of one weighted Platt fit; info as _calibrate's, wsums = the
         CALIBRATION_WSUMS doubles {W+, W-, NaN rows' weight}."""
-        w = self._w(w)
         ab = np.zeros(2, dtype=np.float64)
         info = np.zeros(CALIBRATION_INFO_WORDS, dtype=np.int64)
         wsums = np.zeros(CALIBRATION_WSUMS, dtype=np.float64)
         obj = C.c_double()
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(ab), C.byref(obj), _ptr(info), _ptr(wsums)))
+        self._call(fn, w, rows, _ptr(ab), C.byref(obj), _ptr(info), _ptr(wsums))
         return float(ab[0]), float(ab[1]), obj.value, info, wsums
 
     def calibrate_weighted(self, row_begin: int, row_end: int, w=None):
         """Platt scaling with every row counted by its weight c_i over rows [row_begin, row_end) (dsgd_calibrate_weighted)."""
-        return self._calibrate_weighted("calibrate_weighted", w, (row_begin, row_end))
+        return self._calibrate_weighted("calibrate_weighted", w, _range(row_begin, row_end))
 
     def calibrate_weighted_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_weighted_sampled)."""
@@ -615,24 +597,21 @@ class NativeCtx:
 
     def calibrate_weighted_samples(self, samples, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_calibrate_weighted_samples)."""
-        samples = _arr(samples, np.int32)
-        return self._calibrate_weighted("calibrate_weighted_samples", w, (_ptr(samples), samples.size))
+        return self._calibrate_weighted("calibrate_weighted_samples", w, _list(samples))
 
-    def _eval_weighted_calibration(self, fn: str, w, rows: tuple, a: float, b: float, n_bins: int):
+    def _eval_weighted_calibration(self, fn: str, w, rows: _Rows, a: float, b: float, n_bins: int):
         """dsgd_<fn>: (sums, bin_weight, bin_pos_weight, bin_psum, words): sums = the WCALIBRATION_SUMS doubles {Brier sum,
         log-loss sum, weight used, infinite-term weight}, words = {rows used, rows left out}."""
-        w = self._w(w)
         m = max(int(n_bins), 1)
         sums, words = np.zeros(WCALIBRATION_SUMS, dtype=np.float64), np.zeros(2, dtype=np.int64)
         wb, pwb, psum = np.zeros(m), np.zeros(m), np.zeros(m)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, float(a), float(b), int(n_bins), _ptr(sums),
-                                                 _ptr(wb), _ptr(pwb), _ptr(psum), _ptr(words)))
+        self._call(fn, w, rows, float(a), float(b), int(n_bins), _ptr(sums), _ptr(wb), _ptr(pwb), _ptr(psum), _ptr(words))
         return sums, wb, pwb, psum, words
 
     def eval_weighted_calibration(self, row_begin: int, row_end: int, a: float, b: float, n_bins: int = 10, w=None):
         """Weighted Brier and log-loss sums and n_bins weighted reliability bins at (a, b) over rows [row_begin, row_end)
         (dsgd_eval_weighted_calibration)."""
-        return self._eval_weighted_calibration("eval_weighted_calibration", w, (row_begin, row_end), a, b, n_bins)
+        return self._eval_weighted_calibration("eval_weighted_calibration", w, _range(row_begin, row_end), a, b, n_bins)
 
     def eval_sampled_weighted_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                                           a: float, b: float, n_bins: int = 10, w=None):
@@ -642,106 +621,92 @@ class NativeCtx:
 
     def eval_samples_weighted_calibration(self, samples, a: float, b: float, n_bins: int = 10, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted_calibration)."""
-        samples = _arr(samples, np.int32)
-        return self._eval_weighted_calibration("eval_samples_weighted_calibration", w, (_ptr(samples), samples.size), a, b,
-                                               n_bins)
+        return self._eval_weighted_calibration("eval_samples_weighted_calibration", w, _list(samples), a, b, n_bins)
 
     # -- isotonic calibration --
-    def _calibrate_isotonic(self, fn: str, w, rows: tuple, n: int):
-        """dsgd_<fn>: (x, y, block_rows, block_pos, info) of one isotonic fit over n rows; info = the ISOTONIC_INFO_WORDS
+    def _calibrate_isotonic(self, fn: str, w, rows: _Rows):
+        """dsgd_<fn>: (x, y, block_rows, block_pos, info) of one isotonic fit over the rows; info = the ISOTONIC_INFO_WORDS
         words {blocks, points, rows used, NaN rows, distinct scores}."""
-        w = self._w(w)
-        size = max(int(n), 1)
+        size = max(int(rows.n), 1)
         x, y = np.zeros(size, dtype=np.float64), np.zeros(size, dtype=np.float64)
         br, bp = np.zeros(size, dtype=np.int64), np.zeros(size, dtype=np.int64)
         info, k = np.zeros(ISOTONIC_INFO_WORDS, dtype=np.int64), C.c_int64()
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(k), _ptr(x), _ptr(y), _ptr(br), _ptr(bp),
-                                                 _ptr(info)))
+        self._call(fn, w, rows, C.byref(k), _ptr(x), _ptr(y), _ptr(br), _ptr(bp), _ptr(info))
         nb = int(info[0])
         return x[:k.value].copy(), y[:k.value].copy(), br[:nb].copy(), bp[:nb].copy(), info
 
     def calibrate_isotonic(self, row_begin: int, row_end: int, w=None):
         """Isotonic regression of the labels on s = -x . w over rows [row_begin, row_end) (dsgd_calibrate_isotonic):
         (x, y, block_rows, block_pos, info), x ascending, P(y = +1 | x) = numpy.interp(s, x, y)."""
-        return self._calibrate_isotonic("calibrate_isotonic", w, (row_begin, row_end), row_end - row_begin)
+        return self._calibrate_isotonic("calibrate_isotonic", w, _range(row_begin, row_end))
 
     def calibrate_isotonic_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None):
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_calibrate_isotonic_sampled)."""
-        return self._calibrate_isotonic("calibrate_isotonic_sampled", w, _drawn(row_begin, row_end, key, pos_begin, pos_end),
-                                        pos_end - pos_begin)
+        return self._calibrate_isotonic("calibrate_isotonic_sampled", w, _drawn(row_begin, row_end, key, pos_begin, pos_end))
 
     def calibrate_isotonic_samples(self, samples, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_calibrate_isotonic_samples)."""
-        samples = _arr(samples, np.int32)
-        return self._calibrate_isotonic("calibrate_isotonic_samples", w, (_ptr(samples), samples.size), samples.size)
+        return self._calibrate_isotonic("calibrate_isotonic_samples", w, _list(samples))
 
     def isotonic_probabilities(self, samples, x, y, w=None) -> np.ndarray:
         """numpy.interp(-x_i . w, x, y) for each listed row, any model (dsgd_isotonic_probabilities)."""
-        samples = _arr(samples, np.int32)
+        rows = _list(samples)
         x, y = _arr(x, np.float64), _arr(y, np.float64)
-        w = self._w(w)
-        out = np.zeros(samples.size, dtype=np.float64)
-        self._ck(self._l.dsgd_isotonic_probabilities(self._h, _ptr(w), _ptr(samples), samples.size, _ptr(x), _ptr(y),
-                                                     x.size if x.size == y.size else -1, _ptr(out)))
+        out = np.zeros(rows.n, dtype=np.float64)
+        self._call("isotonic_probabilities", w, rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1, _ptr(out))
         return out
 
-    def _eval_isotonic_calibration(self, fn: str, w, rows: tuple, x, y, n_bins: int):
+    def _eval_isotonic_calibration(self, fn: str, w, rows: _Rows, x, y, n_bins: int):
         """dsgd_<fn>: (sums, bin_rows, bin_pos, bin_psum, words): sums = {Brier sum, log-loss sum over the finite terms},
         words = {rows used, rows left out, rows with an infinite term}."""
-        w = self._w(w)
         x, y = _arr(x, np.float64), _arr(y, np.float64)
         m = max(int(n_bins), 1)
         sums, words = np.zeros(2, dtype=np.float64), np.zeros(ISOTONIC_EVAL_WORDS, dtype=np.int64)
         rows_b, pos_b, psum = np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.int64), np.zeros(m, dtype=np.float64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1,
-                                                 int(n_bins), _ptr(sums), _ptr(rows_b), _ptr(pos_b), _ptr(psum), _ptr(words)))
+        self._call(fn, w, rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1, int(n_bins), _ptr(sums), _ptr(rows_b),
+                   _ptr(pos_b), _ptr(psum), _ptr(words))
         return sums, rows_b, pos_b, psum, words
 
-    def _calibrate_isotonic_weighted(self, fn: str, w, rows: tuple, n: int):
-        """dsgd_<fn>: (x, y, block_weight, block_pos_weight, info, wsums) of one weighted isotonic fit over n rows; info as
+    def _calibrate_isotonic_weighted(self, fn: str, w, rows: _Rows):
+        """dsgd_<fn>: (x, y, block_weight, block_pos_weight, info, wsums) of one weighted isotonic fit over the rows; info as
         _calibrate_isotonic's (rows and scores of positive weight), wsums = {W+, W-}."""
-        w = self._w(w)
-        size = max(int(n), 1)
+        size = max(int(rows.n), 1)
         x, y, bw, bp = (np.zeros(size, dtype=np.float64) for _ in range(4))
         info, k, ws = np.zeros(ISOTONIC_INFO_WORDS, dtype=np.int64), C.c_int64(), np.zeros(2)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(k), _ptr(x), _ptr(y), _ptr(bw), _ptr(bp),
-                                                 _ptr(info), _ptr(ws)))
+        self._call(fn, w, rows, C.byref(k), _ptr(x), _ptr(y), _ptr(bw), _ptr(bp), _ptr(info), _ptr(ws))
         nb = int(info[0])
         return x[:k.value].copy(), y[:k.value].copy(), bw[:nb].copy(), bp[:nb].copy(), info, ws
 
     def calibrate_isotonic_weighted(self, row_begin: int, row_end: int, w=None):
         """Isotonic regression with every row counted by its weight c_i over rows [row_begin, row_end)
         (dsgd_calibrate_isotonic_weighted)."""
-        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted", w, (row_begin, row_end), row_end - row_begin)
+        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted", w, _range(row_begin, row_end))
 
     def calibrate_isotonic_weighted_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                                             w=None):
         """The same over positions [pos_begin, pos_end) of the device-drawn sample."""
         return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted_sampled", w,
-                                                 _drawn(row_begin, row_end, key, pos_begin, pos_end), pos_end - pos_begin)
+                                                 _drawn(row_begin, row_end, key, pos_begin, pos_end))
 
     def calibrate_isotonic_weighted_samples(self, samples, w=None):
         """The same over a list of row ids; repeats count every time."""
-        samples = _arr(samples, np.int32)
-        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted_samples", w, (_ptr(samples), samples.size),
-                                                 samples.size)
+        return self._calibrate_isotonic_weighted("calibrate_isotonic_weighted_samples", w, _list(samples))
 
-    def _eval_weighted_isotonic_calibration(self, fn: str, w, rows: tuple, x, y, n_bins: int):
+    def _eval_weighted_isotonic_calibration(self, fn: str, w, rows: _Rows, x, y, n_bins: int):
         """dsgd_<fn>: (sums, bin_weight, bin_pos_weight, bin_psum, words): sums = {Brier sum, log-loss sum over the finite
         terms, weight used, weight of the infinite terms}, words = {rows used, rows left out, rows with an infinite term}."""
-        w = self._w(w)
         x, y = _arr(x, np.float64), _arr(y, np.float64)
         m = max(int(n_bins), 1)
         sums, words = np.zeros(WCALIBRATION_SUMS), np.zeros(ISOTONIC_EVAL_WORDS, dtype=np.int64)
         wb, pwb, psum = np.zeros(m), np.zeros(m), np.zeros(m)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1,
-                                                 int(n_bins), _ptr(sums), _ptr(wb), _ptr(pwb), _ptr(psum), _ptr(words)))
+        self._call(fn, w, rows, _ptr(x), _ptr(y), x.size if x.size == y.size else -1, int(n_bins), _ptr(sums), _ptr(wb),
+                   _ptr(pwb), _ptr(psum), _ptr(words))
         return sums, wb, pwb, psum, words
 
     def eval_weighted_isotonic_calibration(self, row_begin: int, row_end: int, x, y, n_bins: int = 10, w=None):
         """Weighted quality at the isotonic map (x, y) over rows [row_begin, row_end)."""
-        return self._eval_weighted_isotonic_calibration("eval_weighted_isotonic_calibration", w, (row_begin, row_end), x, y,
-                                                        n_bins)
+        return self._eval_weighted_isotonic_calibration("eval_weighted_isotonic_calibration", w, _range(row_begin, row_end),
+                                                        x, y, n_bins)
 
     def eval_sampled_weighted_isotonic_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int,
                                                    pos_end: int, x, y, n_bins: int = 10, w=None):
@@ -751,14 +716,13 @@ class NativeCtx:
 
     def eval_samples_weighted_isotonic_calibration(self, samples, x, y, n_bins: int = 10, w=None):
         """The same over a list of row ids; repeats count every time."""
-        samples = _arr(samples, np.int32)
-        return self._eval_weighted_isotonic_calibration("eval_samples_weighted_isotonic_calibration", w,
-                                                        (_ptr(samples), samples.size), x, y, n_bins)
+        return self._eval_weighted_isotonic_calibration("eval_samples_weighted_isotonic_calibration", w, _list(samples), x, y,
+                                                        n_bins)
 
     def eval_isotonic_calibration(self, row_begin: int, row_end: int, x, y, n_bins: int = 10, w=None):
         """Brier and log-loss sums and n_bins reliability bins at the map (x, y) over rows [row_begin, row_end)
         (dsgd_eval_isotonic_calibration)."""
-        return self._eval_isotonic_calibration("eval_isotonic_calibration", w, (row_begin, row_end), x, y, n_bins)
+        return self._eval_isotonic_calibration("eval_isotonic_calibration", w, _range(row_begin, row_end), x, y, n_bins)
 
     def eval_sampled_isotonic_calibration(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, x, y,
                                           n_bins: int = 10, w=None):
@@ -768,21 +732,18 @@ class NativeCtx:
 
     def eval_samples_isotonic_calibration(self, samples, x, y, n_bins: int = 10, w=None):
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_isotonic_calibration)."""
-        samples = _arr(samples, np.int32)
-        return self._eval_isotonic_calibration("eval_samples_isotonic_calibration", w, (_ptr(samples), samples.size), x, y,
-                                               n_bins)
+        return self._eval_isotonic_calibration("eval_samples_isotonic_calibration", w, _list(samples), x, y, n_bins)
 
-    def _curve(self, fn: str, w, rows: tuple, n: int, curve: bool):
-        """dsgd_<fn>: (words, ap, thr, tp, fp) with the m points of a curve pass over n rows, or (words, ap, m) when not
+    def _curve(self, fn: str, w, rows: _Rows, curve: bool):
+        """dsgd_<fn>: (words, ap, thr, tp, fp) with the m points of a curve pass over the rows, or (words, ap, m) when not
         `curve` (the average-precision-only pass)."""
-        w = self._w(w)
+        n = max(rows.n, 0)
         words = np.zeros(METRICS_WORDS, dtype=np.int64)
         ap, m = C.c_double(), C.c_int64()
-        thr = np.zeros(max(n, 0), dtype=np.float64) if curve else None
-        tp = np.zeros(max(n, 0), dtype=np.int64) if curve else None
-        fp = np.zeros(max(n, 0), dtype=np.int64) if curve else None
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(words), C.byref(ap), C.byref(m), _ptr(thr),
-                                                 _ptr(tp), _ptr(fp)))
+        thr = np.zeros(n, dtype=np.float64) if curve else None
+        tp = np.zeros(n, dtype=np.int64) if curve else None
+        fp = np.zeros(n, dtype=np.int64) if curve else None
+        self._call(fn, w, rows, _ptr(words), C.byref(ap), C.byref(m), _ptr(thr), _ptr(tp), _ptr(fp))
         if not curve:
             return words, ap.value, m.value
         k = m.value
@@ -791,36 +752,32 @@ class NativeCtx:
     def eval_curve(self, row_begin: int, row_end: int, w=None, curve: bool = True):
         """ROC / precision-recall points and average precision over rows [row_begin, row_end) (dsgd_eval_curve): (words,
         ap, thr, tp, fp), one point per distinct score, highest first; curve=False: (words, ap, number of points)."""
-        return self._curve("eval_curve", w, (row_begin, row_end), row_end - row_begin, curve)
+        return self._curve("eval_curve", w, _range(row_begin, row_end), curve)
 
     def eval_sampled_curve(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None,
                            curve: bool = True):
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_curve)."""
-        return self._curve("eval_sampled_curve", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), pos_end - pos_begin,
-                           curve)
+        return self._curve("eval_sampled_curve", w, _drawn(row_begin, row_end, key, pos_begin, pos_end), curve)
 
     def eval_samples_curve(self, samples, w=None, curve: bool = True):
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_curve)."""
-        samples = _arr(samples, np.int32)
-        return self._curve("eval_samples_curve", w, (_ptr(samples), samples.size), samples.size, curve)
+        return self._curve("eval_samples_curve", w, _list(samples), curve)
 
     # -- bootstrap --
-    def _bootstrap(self, fn: str, w, rows: tuple, bkey: int, b_begin: int, b_end: int):
+    def _bootstrap(self, fn: str, w, rows: _Rows, bkey: int, b_begin: int, b_end: int):
         """dsgd_<fn>: (words[b_end - b_begin, BOOTSTRAP_WORDS], ap[...], loss_sum[...]) of replicates [b_begin, b_end)."""
-        w = self._w(w)
         k = max(int(b_end) - int(b_begin), 0)
         words = np.zeros((max(k, 1), BOOTSTRAP_WORDS), dtype=np.int64)
         ap = np.zeros(max(k, 1), dtype=np.float64)
         loss = np.zeros(max(k, 1), dtype=np.float64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin),
-                                                 int(b_end), _ptr(words), _ptr(ap), _ptr(loss)))
+        self._call(fn, w, rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin), int(b_end), _ptr(words), _ptr(ap), _ptr(loss))
         return words[:k], ap[:k], loss[:k]
 
     def eval_bootstrap(self, row_begin: int, row_end: int, bkey: int, b_begin: int, b_end: int, w=None):
         """Poisson-bootstrap replicates [b_begin, b_end) of rows [row_begin, row_end) with key bkey (dsgd_eval_bootstrap):
         (words, ap, loss_sum), one row per replicate -- the metrics words and size, the average precision and the loss sum of
         the replicate's expanded list."""
-        return self._bootstrap("eval_bootstrap", w, (row_begin, row_end), bkey, b_begin, b_end)
+        return self._bootstrap("eval_bootstrap", w, _range(row_begin, row_end), bkey, b_begin, b_end)
 
     def eval_sampled_bootstrap(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, bkey: int,
                                b_begin: int, b_end: int, w=None):
@@ -830,8 +787,7 @@ class NativeCtx:
 
     def eval_samples_bootstrap(self, samples, bkey: int, b_begin: int, b_end: int, w=None):
         """The same over a list of row ids, position i being list index i (dsgd_eval_samples_bootstrap)."""
-        samples = _arr(samples, np.int32)
-        return self._bootstrap("eval_samples_bootstrap", w, (_ptr(samples), samples.size), bkey, b_begin, b_end)
+        return self._bootstrap("eval_samples_bootstrap", w, _list(samples), bkey, b_begin, b_end)
 
     # -- sync --
     def set_workers(self, counts, k_total: int = 0):
@@ -972,16 +928,15 @@ class NativeCtx:
         self._ck(self._l.dsgd_get_class_weights(self._h, C.byref(wp), C.byref(wn)))
         return wp.value, wn.value
 
-    def _class(self, fn: str, w, rows: tuple) -> "ClassEval":
-        w = self._w(w)
+    def _class(self, fn: str, w, rows: _Rows) -> "ClassEval":
         nrm = C.c_double()
         sums, counts = np.zeros(2, dtype=np.float64), np.zeros(4, dtype=np.int64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(nrm), _ptr(sums), _ptr(counts)))
+        self._call(fn, w, rows, C.byref(nrm), _ptr(sums), _ptr(counts))
         return ClassEval(nrm.value, float(sums[0]), float(sums[1]), *[int(c) for c in counts])
 
     def eval_class(self, row_begin: int, row_end: int, w=None) -> "ClassEval":
         """Per-class loss sums (unweighted), correct counts and row counts over rows [row_begin, row_end) (dsgd_eval_class)."""
-        return self._class("eval_class", w, (row_begin, row_end))
+        return self._class("eval_class", w, _range(row_begin, row_end))
 
     def eval_sampled_class(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None) -> "ClassEval":
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_class)."""
@@ -989,8 +944,7 @@ class NativeCtx:
 
     def eval_samples_class(self, samples, w=None) -> "ClassEval":
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_class)."""
-        samples = _arr(samples, np.int32)
-        return self._class("eval_samples_class", w, (_ptr(samples), samples.size))
+        return self._class("eval_samples_class", w, _list(samples))
 
     # -- sample weights (sync mode) and the weighted evaluations --
     def set_sample_weights(self, sw):
@@ -1002,16 +956,15 @@ class NativeCtx:
         sw = _arr(sw, np.float64)
         self._ck(self._l.dsgd_set_sample_weights(self._h, _ptr(sw), sw.size))
 
-    def _weighted(self, fn: str, w, rows: tuple) -> "WeightedEval":
-        w = self._w(w)
+    def _weighted(self, fn: str, w, rows: _Rows) -> "WeightedEval":
         nrm = C.c_double()
         sums, counts = np.zeros(3, dtype=np.float64), np.zeros(2, dtype=np.int64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, C.byref(nrm), _ptr(sums), _ptr(counts)))
+        self._call(fn, w, rows, C.byref(nrm), _ptr(sums), _ptr(counts))
         return WeightedEval(nrm.value, float(sums[0]), float(sums[1]), float(sums[2]), int(counts[0]), int(counts[1]))
 
     def eval_weighted(self, row_begin: int, row_end: int, w=None) -> "WeightedEval":
         """Weighted loss, correct-weight and weight sums over rows [row_begin, row_end) (dsgd_eval_weighted)."""
-        return self._weighted("eval_weighted", w, (row_begin, row_end))
+        return self._weighted("eval_weighted", w, _range(row_begin, row_end))
 
     def eval_sampled_weighted(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                               w=None) -> "WeightedEval":
@@ -1020,15 +973,12 @@ class NativeCtx:
 
     def eval_samples_weighted(self, samples, w=None) -> "WeightedEval":
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted)."""
-        samples = _arr(samples, np.int32)
-        return self._weighted("eval_samples_weighted", w, (_ptr(samples), samples.size))
+        return self._weighted("eval_samples_weighted", w, _list(samples))
 
-    def _weighted_curve(self, fn: str, w, rows: tuple, n: int, curve: bool) -> "WeightedCurve":
-        w = self._w(w)
+    def _weighted_curve(self, fn: str, w, rows: _Rows, curve: bool) -> "WeightedCurve":
         words, wsums, m = np.zeros(METRICS_WORDS, dtype=np.int64), np.zeros(WCURVE_WORDS), C.c_int64()
-        pts = [np.zeros(max(n, 0)) if curve else None for _ in range(3)]
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, _ptr(words), _ptr(wsums), C.byref(m),
-                                                 *[_ptr(a) for a in pts]))
+        pts = [np.zeros(max(rows.n, 0)) if curve else None for _ in range(3)]
+        self._call(fn, w, rows, _ptr(words), _ptr(wsums), C.byref(m), *[_ptr(a) for a in pts])
         k = m.value
         thr, tpw, fpw = [a[:k].copy() if curve else np.zeros(0) for a in pts]
         return WeightedCurve(words, wsums, k, thr, tpw, fpw, *weighted_auc_ap(words, wsums))
@@ -1036,36 +986,33 @@ class NativeCtx:
     def eval_weighted_curve(self, row_begin: int, row_end: int, w=None, curve: bool = True) -> "WeightedCurve":
         """ROC / precision-recall points, AUC and AP over rows [row_begin, row_end), every row counted by its weight
         c_i = class weight x sample weight (dsgd_eval_weighted_curve); curve=False: the words only."""
-        return self._weighted_curve("eval_weighted_curve", w, (row_begin, row_end), row_end - row_begin, curve)
+        return self._weighted_curve("eval_weighted_curve", w, _range(row_begin, row_end), curve)
 
     def eval_sampled_weighted_curve(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, w=None,
                                     curve: bool = True) -> "WeightedCurve":
         """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_weighted_curve)."""
         return self._weighted_curve("eval_sampled_weighted_curve", w, _drawn(row_begin, row_end, key, pos_begin, pos_end),
-                                    pos_end - pos_begin, curve)
+                                    curve)
 
     def eval_samples_weighted_curve(self, samples, w=None, curve: bool = True) -> "WeightedCurve":
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_weighted_curve)."""
-        samples = _arr(samples, np.int32)
-        return self._weighted_curve("eval_samples_weighted_curve", w, (_ptr(samples), samples.size), samples.size, curve)
+        return self._weighted_curve("eval_samples_weighted_curve", w, _list(samples), curve)
 
     # -- weighted bootstrap --
-    def _weighted_bootstrap(self, fn: str, w, rows: tuple, bkey: int, b_begin: int, b_end: int):
+    def _weighted_bootstrap(self, fn: str, w, rows: _Rows, bkey: int, b_begin: int, b_end: int):
         """dsgd_<fn>: (words[b_end - b_begin, 2], wsums[..., WCURVE_WORDS], loss_sum[...]) of replicates [b_begin, b_end)."""
-        w = self._w(w)
         k = max(int(b_end) - int(b_begin), 0)
         words = np.zeros((max(k, 1), 2), dtype=np.int64)
         wsums = np.zeros((max(k, 1), WCURVE_WORDS), dtype=np.float64)
         loss = np.zeros(max(k, 1), dtype=np.float64)
-        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(w), *rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin),
-                                                 int(b_end), _ptr(words), _ptr(wsums), _ptr(loss)))
+        self._call(fn, w, rows, int(bkey) & 0xFFFFFFFFFFFFFFFF, int(b_begin), int(b_end), _ptr(words), _ptr(wsums), _ptr(loss))
         return words[:k], wsums[:k], loss[:k]
 
     def eval_weighted_bootstrap(self, row_begin: int, row_end: int, bkey: int, b_begin: int, b_end: int, w=None):
         """Weighted Poisson-bootstrap replicates [b_begin, b_end) of rows [row_begin, row_end) with key bkey, every row
         counted by c_i = class weight x sample weight (dsgd_eval_weighted_bootstrap): (words, wsums, loss_sum), one row per
         replicate -- its size and NaN-score rows, the weighted curve words and the weighted loss sum of its expanded list."""
-        return self._weighted_bootstrap("eval_weighted_bootstrap", w, (row_begin, row_end), bkey, b_begin, b_end)
+        return self._weighted_bootstrap("eval_weighted_bootstrap", w, _range(row_begin, row_end), bkey, b_begin, b_end)
 
     def eval_sampled_weighted_bootstrap(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int,
                                         bkey: int, b_begin: int, b_end: int, w=None):
@@ -1075,9 +1022,7 @@ class NativeCtx:
 
     def eval_samples_weighted_bootstrap(self, samples, bkey: int, b_begin: int, b_end: int, w=None):
         """The same over a list of row ids, position i being list index i (dsgd_eval_samples_weighted_bootstrap)."""
-        samples = _arr(samples, np.int32)
-        return self._weighted_bootstrap("eval_samples_weighted_bootstrap", w, (_ptr(samples), samples.size), bkey, b_begin,
-                                        b_end)
+        return self._weighted_bootstrap("eval_samples_weighted_bootstrap", w, _list(samples), bkey, b_begin, b_end)
 
     # -- async --
     def async_host_master(self, w0):

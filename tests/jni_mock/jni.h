@@ -1,5 +1,6 @@
 /* Minimal STAND-IN for the JDK's jni.h, used only by tests/test_abi_surface.py to type-check
- * distributed_sgd_b200/jni/dsgd_jni.c on a box without a JDK.  It declares just the JNI names that shim uses, with
+ * distributed_sgd_b200/jni/dsgd_jni.c on a box without a JDK, and by tests/test_gpu_jni.py to run it through the stand-in
+ * JNIEnv of jni_env.c.  It declares just the JNI names that shim uses, with
  * the JDK's types on LP64 Linux; the layout of the function table is NOT the real one -- never load a library built
  * against this header into a JVM. */
 #ifndef DSGD_JNI_MOCK_H

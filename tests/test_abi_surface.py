@@ -30,6 +30,28 @@ def test_ctypes_binding_covers_the_header():
     native.lib()                                   # resolves every bound symbol with its argtypes
 
 
+def declared_parameter_kinds():
+    """{name: [kind of each parameter]} of every prototype in include/dsgd.h: ptr, i32, u32, i64, u64 or f64"""
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "dsgd.h")).read(), flags=re.S)
+    scalar = {"int": "i32", "int32_t": "i32", "uint32_t": "u32", "int64_t": "i64", "uint64_t": "u64", "double": "f64"}
+    out = {}
+    for name, params in re.findall(r"^(?:int|const char \*)\s*(dsgd_\w+)\(([^)]*)\);", text, re.M):
+        out[name] = ["ptr" if "*" in p or "[" in p else scalar[p.split()[0]] for p in params.split(",")]
+    return out
+
+
+def test_ctypes_argtypes_match_the_header_prototypes():
+    """Every ABI entry, the generated row forms included, has its prototype's arity and each parameter's kind."""
+    from distributed_sgd_b200 import native
+    kind = {C.c_void_p: "ptr", C.c_char_p: "ptr", C.c_int32: "i32", C.c_uint32: "u32", C.c_int64: "i64", C.c_uint64: "u64",
+            C.c_double: "f64"}
+    declared = declared_parameter_kinds()
+    assert sorted(declared) == declared_symbols()
+    for name, args in native.ABI.items():
+        got = ["ptr" if issubclass(t, C._Pointer) else kind[t] for t in args]
+        assert got == declared[name], name
+
+
 def row_form_entry_points():
     """dsgd_eval and the range, drawn-sample and id-list forms of the fifteen evaluation families"""
     evals = ["counts", "sums", "class", "weighted", "metrics", "curve", "weighted_curve", "calibration",
