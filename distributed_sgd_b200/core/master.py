@@ -15,8 +15,10 @@ import numpy as np
 
 from ..ml import split_strategy as SplitStrategy  # noqa: N812
 from ..ml.calibration import METHODS as CALIBRATION_METHODS, Calibration, IsotonicCalibration
+from ..ml.class_weight import resolve_class_weight
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
+from ..ml.one_vs_rest import OneVsRest, topic_report
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge
 from ..ml.sparse_svm import SparseSVM
@@ -371,6 +373,9 @@ class Master:
         self.seed = int(seed)
         self.rng = np.random.default_rng(seed)
         self._epochs_drawn = 0
+        self._draw_cache = None   # fit_one_vs_rest: {(epoch, batch, groups): EpochDraw}, the draws every topic's fit shares
+        # the Slave's topics (train rows, then test rows), None without any
+        self.topics = getattr(slave, "topics", None)
         self._sampled_draws = 0   # t of sampled_key: device-drawn evaluation samples so far (apart from the epoch draws)
         # jvm_exact: draw the batches with java.util.Random(seed) + Scala 2.12's Random.shuffle, the stream a reference
         # run consumes (SURVEY.md 8f N4); default: numpy's generator (statistically the same draws, much faster)
@@ -567,6 +572,55 @@ class Master:
         we = (self.ctx.eval_sampled_weighted(b, e, key, 0, k, weights) if ids is None
               else self.ctx.eval_samples_weighted(ids, weights))
         return self._weighted_report(we, weights)
+
+    # ---- one-vs-rest topics (extension) ----------------------------------------------------------------------------------
+    def _topic_weights(self, weights) -> np.ndarray:
+        """[T, wdim] weights of every loaded topic, from an OneVsRest (its topics must be the loaded ones, in order) or an
+        array."""
+        if self.topics is None:
+            raise ValueError("topic report: the Slave holds no topics")
+        if isinstance(weights, OneVsRest):
+            if tuple(weights.topics) != self.topics.names:
+                raise ValueError("topic report: the model must hold one weight vector per loaded topic, in their order")
+            weights = weights.weights
+        W = np.ascontiguousarray(weights, dtype=np.float64)
+        if W.shape != (self.topics.n_topics, self.wdim):
+            raise ValueError(f"topic report: weights must be [{self.topics.n_topics}, {self.wdim}], got {W.shape}")
+        return W
+
+    def _topic_words(self, words) -> dict:
+        """The report of the words every rank computed for its share, summed over ranks (integers: every rank gets the same
+        bits)."""
+        total = np.rint(self.group.all_reduce_sum([float(x) for x in words])).astype(np.int64)
+        return topic_report(total, self.topics.names)
+
+    def local_topic_report(self, weights, test_data: bool = True) -> dict:
+        """Multi-label quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train) rows, all
+        topics in one device pass (dsgd_eval_topics): per topic the counts, precision, recall and F1; micro precision,
+        recall and F1, macro F1, subset accuracy, Hamming loss and top-1 accuracy (ml/one_vs_rest.py: topic_report).  Each
+        rank evaluates a contiguous share of the rows, as _eval_rows splits them."""
+        W = self._topic_weights(weights)
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        n, R, r = e - b, self.group.world, self.group.rank
+        lo, hi = b + (n * r) // R, b + (n * (r + 1)) // R
+        words = self.ctx.eval_topics(lo, hi, W) if hi > lo else np.zeros(8 * len(W) + 8, dtype=np.int64)
+        return self._topic_words(words)
+
+    def local_sampled_topic_report(self, weights, samples_count: int, test_data: bool = True) -> dict:
+        """local_topic_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it; rank r of
+        R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
+        W = self._topic_weights(weights)
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled topic report of {samples_count} rows: the sample is empty")
+        lo, hi = sample_shard(k, self.group.world, self.group.rank)
+        if hi <= lo:
+            words = np.zeros(8 * len(W) + 8, dtype=np.int64)
+        elif ids is None:
+            words = self.ctx.eval_sampled_topics(b, e, key, lo, hi, W)
+        else:
+            words = self.ctx.eval_samples_topics(ids[lo:hi], W)
+        return self._topic_words(words)
 
     # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
     # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank
@@ -881,7 +935,63 @@ class MasterSync(Master):
             if [(g.start, g.stop) for g in groups] != [(a, min(a + size, n)) for a in range(0, n, size)]:
                 raise ValueError("jvm_exact draws are defined for SplitStrategy.vanilla groups")
             return EpochDraw.from_steps(self.jvm.sync_epoch(n, len(groups), batch_size, group_size=size))
+        if self._draw_cache is not None:   # the draws do not depend on the labels: one draw per epoch for every topic
+            key = (epoch, batch_size, tuple((g.start, g.stop) for g in groups))
+            if key not in self._draw_cache:
+                self._draw_cache[key] = EpochDraw.draw(self.seed, epoch, groups, batch_size)
+            return self._draw_cache[key]
         return EpochDraw.draw(self.seed, epoch, groups, batch_size)
+
+    def fit_one_vs_rest(self, initial_weights: np.ndarray, max_epochs: int, batch_size: int, learning_rate: float,
+                        stopping_criterion: EarlyStopping, topics=None, **fit_kwargs) -> OneVsRest:
+        """One-vs-rest training of the Slave's topics: for each chosen topic t (topics None: every loaded topic, else their
+        names or indices, in that order) the device labels become "has topic t" (ctx.select_topic), a "balanced"
+        class_weight is resolved again from topic t's train labels, and `fit` runs with the given arguments.  Each fit
+        draws exactly the batches of a fresh MasterSync of the same seed (epoch numbering restarts at 0); the draws do not
+        depend on the labels, so every epoch is drawn once and shared by all topics.  Every rank runs the same sequence.
+        A topic without a positive or without a negative train row, and jvm_exact (its stream is one reference run), are
+        refused before any fit.  The loaded labels and the Slave's class weights are restored afterwards, also when a fit
+        raises."""
+        if self.topics is None:
+            raise ValueError("fit_one_vs_rest: the Slave holds no topics")
+        if self.jvm is not None:
+            raise ValueError("fit_one_vs_rest: jvm_exact draws are one reference run's stream; one-vs-rest fits cannot share it")
+        names = self.topics.names
+        chosen = list(range(len(names))) if topics is None else [names.index(t) if t in names else -1 if isinstance(t, str)
+                                                                  else int(t) for t in topics]
+        if not chosen or any(not 0 <= t < len(names) for t in chosen):
+            raise ValueError(f"fit_one_vs_rest: topics must name loaded topics, got {topics!r}")
+        train = self.topics.rows(0, self.n_train)
+        labels = {t: train.labels(t) for t in chosen}
+        for t in chosen:
+            n_pos = int(np.count_nonzero(labels[t] > 0))
+            if n_pos == 0 or n_pos == self.n_train:
+                raise ValueError(f"fit_one_vs_rest: topic {names[t]!r} has {n_pos} positive train rows of {self.n_train}; "
+                                 "both classes are needed")
+        balanced = getattr(self.model, "class_weight", None) == "balanced"
+        saved = (self.class_weight, self.weighted, getattr(self.slave, "class_weight", self.class_weight))
+        weights, histories = [], []
+        self._draw_cache = {}
+        try:
+            for t in chosen:
+                self.ctx.select_topic(t)
+                if balanced:
+                    cw = resolve_class_weight("balanced", labels[t])
+                    self.ctx.set_class_weights(*cw)
+                    self.class_weight, self.slave.class_weight = cw, cw
+                    self.weighted = cw != (1.0, 1.0) and not self.sample_weighted
+                self._epochs_drawn = 0
+                state = self.fit(initial_weights, max_epochs, batch_size, learning_rate, stopping_criterion, **fit_kwargs)
+                weights.append(np.array(state.grad, dtype=np.float64))
+                histories.append(self.history)
+        finally:
+            self._draw_cache = None
+            self._epochs_drawn = 0
+            self.ctx.select_topic(-1)
+            self.class_weight, self.weighted, self.slave.class_weight = saved
+            if balanced:
+                self.ctx.set_class_weights(*saved[0])
+        return OneVsRest(np.stack(weights), tuple(names[t] for t in chosen), histories)
 
     def fit(self, initial_weights: np.ndarray, max_epochs: int, batch_size: int, learning_rate: float,
             stopping_criterion: EarlyStopping, split_strategy: Split = SplitStrategy.vanilla, *,

@@ -17,7 +17,23 @@ from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge, model_name
 from ..ml.sparse_svm import SparseSVM
 from ..native import NativeCtx
-from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights, sample_weights_of
+from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, Topics, has_sample_weights, sample_weights_of
+
+
+def topics_of(data: Data, test_data: Optional[Data]) -> Optional[Topics]:
+    """The topics of the train rows followed by the test rows, the layout of the device rows; None when no part carries
+    any.  Both parts must carry topics with the same names, or neither."""
+    parts = [data] if test_data is None else [data, test_data]
+    if all(p.topics is None for p in parts):
+        return None
+    if any(p.topics is None for p in parts):
+        raise ValueError("topics: the train and the test rows must both carry topics, or neither")
+    if test_data is None:
+        return data.topics
+    a, b = data.topics, test_data.topics
+    if a.names != b.names:
+        raise ValueError("topics: the train and the test rows carry different topic names")
+    return Topics(np.concatenate([a.ptr, b.ptr[1:] + a.ptr[-1]]), np.concatenate([a.ids, b.ids]), a.names)
 
 
 class Slave:
@@ -51,6 +67,10 @@ class Slave:
         self.sample_weighted = has_sample_weights(data, test_data)
         if self.sample_weighted and is_async:
             raise ValueError(SAMPLE_WEIGHT_ASYNC)
+        # the topics of a multi-label set (one-vs-rest training, Master.local_topic_report), train rows then test rows
+        self.topics = topics_of(data, test_data)
+        if self.topics is not None and is_async:
+            raise ValueError("topics: one-vs-rest training belongs to sync training; asynchronous (Hogwild) training has none")
         self.node, self.master, self.model, self.is_async, self.world = node, master, model, is_async, world
         self.n_train = data.n_rows
         self.n_test = test_data.n_rows if test_data is not None else 0
@@ -71,6 +91,8 @@ class Slave:
                 ctx.set_class_weights(*self.class_weight)
             if self.sample_weighted:
                 ctx.set_sample_weights(sample_weights_of(data, test_data))
+            if self.topics is not None:
+                ctx.load_topics(self.topics.ptr, self.topics.ids, self.topics.n_topics)
             return
         self.ctx = NativeCtx(node if device is None else device, data.dim, model.lam, rank=node, world=world,
                              is_async=is_async, model=name, intercept=self.intercept)
@@ -92,6 +114,8 @@ class Slave:
             self.ctx.set_class_weights(*self.class_weight)
         if self.sample_weighted:
             self.ctx.set_sample_weights(sample_weights_of(data, test_data))
+        if self.topics is not None:
+            self.ctx.load_topics(self.topics.ptr, self.topics.ids, self.topics.n_topics)
 
     def stop(self):  # Slave.stop (core/Slave.scala:68-77): releases the device context
         self.ctx.close()

@@ -27,6 +27,7 @@
 #include "dsgd_calibrate.cuh"
 #include "dsgd_isotonic.cuh"
 #include "dsgd_bootstrap.cuh"
+#include "dsgd_topics.cuh"
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
@@ -127,6 +128,15 @@ struct dsgd_ctx {
   dev_buf<int8_t> label;
   dev_buf<float> yabs;   // label * sum_j |x_j| per row (dsgd_kernels.cuh: k_repack)
   dev_buf<double> sw;    // dsgd_set_sample_weights: one fp64 weight per row (allocated on first use, freed with the rows)
+  // dsgd_load_topics: each row's topic ids (a CSR over the rows, ids ascending within a row), the labels dsgd_load_csr
+  // loaded (dsgd_select_topic(-1) restores them), and the topic count (0: no topics); freed with the rows
+  dev_buf<int64_t> t_ptr;
+  dev_buf<int32_t> t_ids;
+  dev_buf<int8_t> label0;
+  int32_t n_topics = 0;
+  // a topic evaluation (dsgd_eval_*topics): the T weight vectors and the DSGD_TOPIC_WORDS(T) counter words
+  dev_buf<double> t_w;
+  dev_buf<unsigned long long> t_cnt;
 
   // state (fp64, L2 resident) -- g has dim + 2 slots (hinge sum and batch size ride in the allreduce)
   dev_buf<double> w, g, d, w_req;
@@ -604,8 +614,11 @@ extern "C" int dsgd_load_csr(dsgd_ctx *ctx, int64_t n_rows, int64_t nnz, const i
   ctx->samples_n = 0;
   // the sample weights named the previous rows: the ctx is unweighted again
   ctx->sw_on = false;
+  // the topics named the previous rows too
+  ctx->n_topics = 0;
   // all of the previous rows go before any of the new ones is allocated
   CU(ctx->rp16.release()); CU(ctx->pairs.release()); CU(ctx->label.release()); CU(ctx->yabs.release()); CU(ctx->sw.release());
+  CU(ctx->t_ptr.release()); CU(ctx->t_ids.release()); CU(ctx->label0.release());
   const int64_t n_pairs = (int64_t)acc * 2;
   CU(ctx->rp16.alloc(n_rows + 1));
   CU(ctx->pairs.alloc(std::max<int64_t>(n_pairs, 1)));
@@ -1557,6 +1570,117 @@ extern "C" int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t
 
 extern "C" int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out) {
   return metrics_request(ctx, w, listed_rows(samples, n), __func__, out);
+}
+
+// ---- topics (dsgd_topics.cuh; DESIGN.md §4.21) --------------------------------------------------------------------------
+
+// the loaded labels back in ctx->label, and yabs's signs with them
+static int restore_labels(dsgd_ctx *ctx) {
+  k_topic_select<<<cdiv(ctx->n_rows, 256), 256, 0, ctx->stream>>>(ctx->t_ptr, ctx->t_ids, ctx->label0, ctx->n_rows, -1,
+                                                                   ctx->label, ctx->yabs);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_load_topics(dsgd_ctx *ctx, int32_t n_topics, const int64_t *topic_ptr, const int32_t *topic_id) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "dsgd_load_topics: ctx is in async mode (topics belong to the sync paths)");
+  NEED(ctx->pairs, DSGD_ERR_STATE, "dsgd_load_topics: no rows loaded");
+  NEED(n_topics >= 1 && n_topics <= DSGD_MAX_TOPICS, DSGD_ERR_INVALID, "dsgd_load_topics: %d topics; 1 .. %d", n_topics,
+       DSGD_MAX_TOPICS);
+  NEED(topic_ptr, DSGD_ERR_INVALID, "dsgd_load_topics: topic_ptr is NULL");
+  const int64_t n = ctx->n_rows;
+  NEED(topic_ptr[0] == 0, DSGD_ERR_INVALID, "dsgd_load_topics: topic_ptr[0] is %lld, not 0", (long long)topic_ptr[0]);
+  for (int64_t r = 0; r < n; ++r)
+    NEED(topic_ptr[r + 1] >= topic_ptr[r], DSGD_ERR_INVALID, "dsgd_load_topics: topic_ptr not monotone at row %lld",
+         (long long)r);
+  const int64_t nnz = topic_ptr[n];   // the id count
+  NEED(nnz == 0 || topic_id, DSGD_ERR_INVALID, "dsgd_load_topics: topic_id is NULL with %lld ids", (long long)nnz);
+  for (int64_t r = 0; r < n; ++r)
+    for (int64_t k = topic_ptr[r]; k < topic_ptr[r + 1]; ++k) {
+      NEED(topic_id[k] >= 0 && topic_id[k] < n_topics, DSGD_ERR_INVALID,
+           "dsgd_load_topics: topic %d of row %lld outside [0,%d)", topic_id[k], (long long)r, n_topics);
+      NEED(k == topic_ptr[r] || topic_id[k] > topic_id[k - 1], DSGD_ERR_INVALID,
+           "dsgd_load_topics: the topics of row %lld are not strictly ascending at position %lld", (long long)r, (long long)k);
+    }
+  CU(cudaSetDevice(ctx->device));
+  int rc;
+  if (ctx->n_topics > 0) {   // a topic may be selected: the loaded labels go back first, and label0 keeps them
+    if ((rc = restore_labels(ctx))) return rc;
+  } else {
+    CU(ctx->label0.alloc(n));
+    CU(cudaMemcpyAsync(ctx->label0, ctx->label, (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  ctx->n_topics = 0;
+  CU(ctx->t_ptr.alloc(n + 1));
+  CU(ctx->t_ids.alloc(std::max<int64_t>(nnz, 1)));
+  CU(cudaMemcpyAsync(ctx->t_ptr, topic_ptr, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
+  if (nnz) CU(cudaMemcpyAsync(ctx->t_ids, topic_id, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  ctx->n_topics = n_topics;
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_select_topic(dsgd_ctx *ctx, int32_t topic) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE,
+       "dsgd_select_topic: ctx is in async mode (the labels would change under the Hogwild loop)");
+  NEED(ctx->n_topics > 0, DSGD_ERR_STATE, "dsgd_select_topic: no topics loaded");
+  NEED(topic >= -1 && topic < ctx->n_topics, DSGD_ERR_INVALID, "dsgd_select_topic: topic %d outside [-1,%d)", topic,
+       ctx->n_topics);
+  CU(cudaSetDevice(ctx->device));
+  k_topic_select<<<cdiv(ctx->n_rows, 256), 256, 0, ctx->stream>>>(ctx->t_ptr, ctx->t_ids, ctx->label0, ctx->n_rows, topic,
+                                                                   ctx->label, ctx->yabs);
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+// dsgd_eval*_topics: the DSGD_TOPIC_WORDS(T) words into out.  Every refusal comes before anything is launched.
+static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, const row_request &req, const char *fn,
+                          int64_t *out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", fn);
+  NEED(W, DSGD_ERR_INVALID, "%s: W is NULL (the call scores T weight vectors of the caller's)", fn);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (topics belong to the sync paths)", fn);
+  NEED(ctx->n_topics > 0, DSGD_ERR_STATE, "%s: no topics loaded", fn);
+  NEED(n_topics == ctx->n_topics, DSGD_ERR_INVALID, "%s: %d weight vectors for %d loaded topics", fn, n_topics,
+       ctx->n_topics);
+  row_set rows;
+  int rc = ids_capped(ctx, req, fn);
+  if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  const int64_t T = n_topics, words = DSGD_TOPIC_WORDS(T), nw = T * wlen(ctx);
+  if ((rc = ctx->t_w.grow(ctx, nw, 1024)) || (rc = ctx->t_cnt.grow(ctx, words, 1024))) return rc;
+  CU(cudaMemcpyAsync(ctx->t_w, W, sizeof(double) * (size_t)nw, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemsetAsync(ctx->t_cnt, 0, sizeof(unsigned long long) * (size_t)words, ctx->stream));
+  const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
+  const size_t smem = sizeof(unsigned) * (size_t)(T * kTopicWords);
+  with_icpt(ctx, [&](auto ic) {
+    k_topic_eval<ic><<<grid, 256, smem, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids,
+                                                       rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim, ctx->t_cnt);
+  });
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, ctx->t_cnt, sizeof(int64_t) * (size_t)words, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end,
+                                int64_t *out) {
+  return topics_request(ctx, W, n_topics, range_rows(row_begin, row_end), __func__, out);
+}
+
+extern "C" int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end,
+                                        uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *out) {
+  return topics_request(ctx, W, n_topics, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, out);
+}
+
+extern "C" int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
+                                        int64_t *out) {
+  return topics_request(ctx, W, n_topics, listed_rows(samples, n), __func__, out);
 }
 
 // ---- bootstrap (dsgd_bootstrap.cuh; DESIGN.md §4.19) --------------------------------------------------------------------

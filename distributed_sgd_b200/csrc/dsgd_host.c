@@ -232,6 +232,72 @@ int dsgd_rcv1_labels(const char *qrels_path, const int64_t *row_ids, int64_t n_r
   return 0;
 }
 
+/* ---- every qrels line (multi-label topics) ----------------------------------------------------------------------------
+ * The two-call protocol of dsgd_rcv1_count / dsgd_rcv1_parse over a qrels file ("<topic> <doc id> 1" per line):
+ *   dsgd_rcv1_topics_count: *n_lines, the distinct topic names *n_names and the bytes they take with one NUL each.
+ *   dsgd_rcv1_topics_parse: names_out receives the distinct names, NUL-terminated, in first-seen order; line i's topic is
+ *   line_topic[i] (an index into that order) and its document line_doc[i].  The caller maps documents to rows, sorts the
+ *   names and drops repeated (topic, doc) lines.
+ * Both return 0, -1 (cannot open the file or allocate) or -2 (the file holds more than the sizes passed to parse). */
+static int topics_scan(const char *path, int64_t cap_lines, int32_t cap_names, int64_t cap_bytes, char *names_out,
+                       int32_t *line_topic, int64_t *line_doc, int64_t *n_lines, int32_t *n_names, int64_t *n_bytes) {
+  FILE *f = fopen(path, "r");
+  if (!f) return -1;
+  int64_t lines = 0, bytes = 0, cap = 0;
+  int32_t names = 0;
+  int64_t *off = NULL;   /* name k starts at buf + off[k] */
+  char *buf = NULL;
+  int64_t buf_cap = 0;
+  char topic[64]; long long id; int one, rc = 0;
+  while (fscanf(f, "%63s %lld %d", topic, &id, &one) == 3) {
+    int32_t k = 0;
+    while (k < names && strcmp(buf + off[k], topic) != 0) ++k;
+    if (k == names) {   /* a new name */
+      const int64_t len = (int64_t)strlen(topic) + 1;
+      if (names == cap) {
+        cap = cap ? 2 * cap : 256;
+        int64_t *o = (int64_t *)realloc(off, sizeof(int64_t) * (size_t)cap);
+        if (!o) { rc = -1; break; }
+        off = o;
+      }
+      if (bytes + len > buf_cap) {
+        buf_cap = 2 * (bytes + len) + 4096;
+        char *b = (char *)realloc(buf, (size_t)buf_cap);
+        if (!b) { rc = -1; break; }
+        buf = b;
+      }
+      memcpy(buf + bytes, topic, (size_t)len);
+      off[names++] = bytes;
+      bytes += len;
+    }
+    if (line_topic) {
+      if (lines >= cap_lines) { rc = -2; break; }
+      line_topic[lines] = k;
+      line_doc[lines] = (int64_t)id;
+    }
+    ++lines;
+  }
+  fclose(f);
+  if (rc == 0 && names_out) {
+    if (names > cap_names || bytes > cap_bytes) rc = -2;
+    else if (bytes) memcpy(names_out, buf, (size_t)bytes);
+  }
+  free(off);
+  free(buf);
+  if (rc == 0) { *n_lines = lines; *n_names = names; *n_bytes = bytes; }
+  return rc;
+}
+
+int dsgd_rcv1_topics_count(const char *qrels_path, int64_t *n_lines, int32_t *n_names, int64_t *names_bytes) {
+  return topics_scan(qrels_path, 0, 0, 0, NULL, NULL, NULL, n_lines, n_names, names_bytes);
+}
+
+int dsgd_rcv1_topics_parse(const char *qrels_path, int64_t n_lines, int32_t n_names, int64_t names_bytes, char *names_out,
+                           int32_t *line_topic, int64_t *line_doc) {
+  int64_t l, b; int32_t k;
+  return topics_scan(qrels_path, n_lines, n_names, names_bytes, names_out, line_topic, line_doc, &l, &k, &b);
+}
+
 /* Writes rows in the reference's text format (for feeding the same data to a JVM run of the reference). */
 int dsgd_rcv1_write(const char *vectors_path, const char *qrels_path, int64_t n_rows, const int64_t *row_ptr,
                     const int32_t *col, const float *val, const int8_t *label, int64_t first_id) {

@@ -224,6 +224,17 @@ object DsgdNative {
                                   posEnd: Long, sums: Array[Double], counts: Array[Long]): Int
   @native def evalSamplesWeighted(ctx: Long, w: Array[Double], samples: Array[Int], sums: Array[Double],
                                   counts: Array[Long]): Int
+  // topics (sync mode): loadTopics gives every loaded row its topic ids, rows as in loadCsr (topicPtr.length = rows + 1,
+  // topicId.length = topicPtr(rows), ids strictly ascending within a row, each in [0, nTopics)); selectTopic(t) makes the
+  // labels "has topic t" (-1: the loaded ones).  evalTopics: W holds nTopics weight vectors of the weight length, one after
+  // the other (W.length = nTopics * that length); out.length >= 8 * nTopics + 8: per topic the eight metrics words (U2 0),
+  // then rows, rows right for every topic, rows whose top-scored topic is theirs, rows without a topic, rows without a score
+  @native def loadTopics(ctx: Long, nTopics: Int, topicPtr: Array[Long], topicId: Array[Int]): Int
+  @native def selectTopic(ctx: Long, topic: Int): Int
+  @native def evalTopics(ctx: Long, W: Array[Double], nTopics: Int, rowBegin: Long, rowEnd: Long, out: Array[Long]): Int
+  @native def evalSampledTopics(ctx: Long, W: Array[Double], nTopics: Int, rowBegin: Long, rowEnd: Long, key: Long,
+                                posBegin: Long, posEnd: Long, out: Array[Long]): Int
+  @native def evalSamplesTopics(ctx: Long, W: Array[Double], nTopics: Int, samples: Array[Int], out: Array[Long]): Int
   // weighted curves, either model: metrics as evalCurve's, wsums(0 until 13) the DSGD_WCURVE_WORDS weighted words, nPoints(0)
   // = m, thr / tpw / fpw(0 until m) the points (W+ and W- at or above each score); all three null for the words alone, else
   // each at least as long as the request's rows.  An async ctx is refused.

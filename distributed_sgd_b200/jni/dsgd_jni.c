@@ -861,6 +861,57 @@ FN(setSampleWeights)(JNIEnv *env, jobject self, jlong h, jdoubleArray sw) {
   free(b.p);
   return rc;
 }
+/* ---- topics (sync mode) ---- */
+/* the rows loaded on the ctx, which dsgd_info names (read under info_lock, as weight_len reads it) */
+static int loaded_rows(jlong h, jlong *n) {
+  int32_t dim = 0;
+  int rc = dsgd_dim(CTX(h), &dim);
+  if (rc != DSGD_OK) return rc;
+  pthread_mutex_lock(&info_lock);
+  const char *s = strstr(dsgd_info(CTX(h)), "\"n_rows\": ");
+  *n = s ? strtoll(s + strlen("\"n_rows\": "), NULL, 10) : -1;
+  pthread_mutex_unlock(&info_lock);
+  return *n < 0 ? DSGD_ERR_INVALID : DSGD_OK;
+}
+/* topicPtr exactly rows + 1 long, and topicId exactly topicPtr(rows) */
+FN(loadTopics)(JNIEnv *env, jobject self, jlong h, jint nTopics, jlongArray topicPtr, jintArray topicId) {
+  buf_t p = in_Long(env, topicPtr), t = in_Int(env, topicId);
+  jlong n = 0;
+  int rc = checked(loaded_rows(h, &n), p.bad | t.bad, 0);
+  if (rc == DSGD_OK) rc = checked(DSGD_OK, 0, !p.p || p.n != n + 1 || ((const int64_t *)p.p)[n] != (int64_t)t.n);
+  if (rc == DSGD_OK) rc = dsgd_load_topics(CTX(h), nTopics, (const int64_t *)p.p, (const int32_t *)t.p);
+  free(p.p); free(t.p);
+  return rc;
+}
+FN(selectTopic)(JNIEnv *env, jobject self, jlong h, jint topic) { return dsgd_select_topic(CTX(h), topic); }
+/* W exactly nTopics weight vectors long (null: refused by the library), out at least DSGD_TOPIC_WORDS(nTopics) */
+static int req_topics(JNIEnv *env, jlong h, jdoubleArray W, jint nTopics, rows_t r, jlongArray out) {
+  buf_t bw = in_Double(env, W), o = out_Long(env, out);
+  r.ids = in_Int(env, r.samples);
+  int32_t wl = 0;
+  int rc = checked(weight_len(h, &wl), bw.bad | o.bad | r.ids.bad, 0);
+  if (rc == DSGD_OK)
+    rc = checked(DSGD_OK, 0, nTopics < 1 || (bw.p && bw.n != (jlong)nTopics * wl) || o.n < DSGD_TOPIC_WORDS(nTopics));
+  if (rc == DSGD_OK)
+    rc = r.form == RANGE ? dsgd_eval_topics(CTX(h), bw.p, nTopics, r.rowBegin, r.rowEnd, o.p)
+         : r.form == DRAWN ? dsgd_eval_sampled_topics(CTX(h), bw.p, nTopics, r.rowBegin, r.rowEnd, (uint64_t)r.key, r.posBegin,
+                                                      r.posEnd, o.p)
+                           : dsgd_eval_samples_topics(CTX(h), bw.p, nTopics, r.ids.p, r.ids.n, o.p);
+  back_Long(env, out, o, rc);
+  free(bw.p); free(r.ids.p);
+  return rc;
+}
+FN(evalTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jlong rowBegin, jlong rowEnd,
+               jlongArray out) {
+  return req_topics(env, h, W, nTopics, range_rows(rowBegin, rowEnd), out);
+}
+FN(evalSampledTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jlong rowBegin, jlong rowEnd,
+                      jlong key, jlong posBegin, jlong posEnd, jlongArray out) {
+  return req_topics(env, h, W, nTopics, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), out);
+}
+FN(evalSamplesTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jintArray samples, jlongArray out) {
+  return req_topics(env, h, W, nTopics, list_rows(samples), out);
+}
 static int req_weighted(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray sums, jlongArray counts) {
   req_t q;
   buf_t s = out_Double(env, sums), c = out_Long(env, counts);

@@ -53,6 +53,17 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     if cfg.bootstrap_weighted and cfg.is_async:
         raise ValueError("bootstrap-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
                          "has none to resample by")
+    from .ml.one_vs_rest import parse_topics
+    topics = parse_topics(cfg.topics)
+    if topics is not None and cfg.is_async:
+        raise ValueError("topics: one-vs-rest training belongs to sync training; asynchronous (Hogwild) training has none")
+    if topics is None:   # the binary run alone, with the rows as they always were
+        data = dataclasses.replace(data, topics=None)
+    elif data.topics is None:
+        raise ValueError("topics: the data carries no topics (RCV1 is read with them when the key is set; "
+                         "--synthetic-topics N plants them on synthetic rows)")
+    elif topics != "all":
+        data = dataclasses.replace(data, topics=data.topics.select(topics))
     if cfg.sample_weight:   # one weight per loaded row; the split below carries them
         data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
@@ -155,6 +166,22 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
         if rank == 0:
             log(f"bootstrap ({cfg.bootstrap} replicates, 95 %): " + ", ".join(
                 f"{m} {bs[m]['estimate']:.4f} [{bs[m]['lo']:.4f}, {bs[m]['hi']:.4f}]" for m in ("auc", "ap", "accuracy", "loss")))
+    if topics is not None:
+        # one-vs-rest: every topic fitted with the settings of the binary run, then all judged on the test rows in one pass
+        t1 = time.perf_counter()
+        ovr = master.fit_one_vs_rest(w0, cfg.max_epochs, cfg.batch_size, cfg.learning_rate, stop,
+                                     virtual_workers=cfg.node_count // world,
+                                     average_from=cfg.average_from if cfg.average_from >= 0 else None,
+                                     learning_rate_decay=cfg.learning_rate_decay,
+                                     learning_rate_power=cfg.learning_rate_power)
+        fit_s = time.perf_counter() - t1
+        tr = master.local_topic_report(ovr, test_data=True)
+        report["topic_report"] = {"topics": len(ovr.topics), "fit_seconds": fit_s,
+                                  "epochs": [len(h["losses"]) for h in ovr.histories], **tr}
+        if rank == 0:
+            log(f"one-vs-rest ({len(ovr.topics)} topics, {fit_s:.1f} s): test micro F1 {tr['micro_f1']:.4f}, macro F1 "
+                f"{tr['macro_f1']:.4f} over {tr['macro_f1_topics']} topics, subset accuracy {tr['subset_accuracy']:.4f}, "
+                f"Hamming loss {tr['hamming_loss']:.5f}, top-1 accuracy {tr['top1_accuracy']:.4f}")
     if inspect:
         inspect("done", (master, state))
     slave.stop()
@@ -165,11 +192,13 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--conf", default=None, help="application.conf (HOCON `dsgd { }` block); DSGD_* variables override")
     ap.add_argument("--synthetic-rows", type=int, default=0, help="use RCV1-shaped synthetic rows instead of data-path")
+    ap.add_argument("--synthetic-topics", type=int, default=0,
+                    help="with --synthetic-rows: plant this many topics on the rows (utils.synthetic_topics) for `topics`")
     ap.add_argument("--seed", type=int, default=0)                            # Random.setSeed(0) (Main.scala:32)
     ap.add_argument("--jvm-exact", action="store_true",
                     help="sync mode: draw the batches from java.util.Random(seed) + Scala's Random.shuffle like the reference")
     args = ap.parse_args(argv)
-    from .utils import load_config, rcv1, synthetic_rcv1
+    from .utils import load_config, rcv1, synthetic_rcv1, synthetic_topics
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -178,7 +207,13 @@ def main(argv=None) -> int:
         import torch.distributed as dist
         dist.init_process_group(backend="gloo", rank=rank, world_size=world)
     cfg = load_config(args.conf)
-    data = synthetic_rcv1(n_rows=args.synthetic_rows, seed=args.seed) if args.synthetic_rows else rcv1(cfg.data_path, full=cfg.full)
+    from .ml.one_vs_rest import parse_topics
+    if args.synthetic_rows:
+        data = synthetic_rcv1(n_rows=args.synthetic_rows, seed=args.seed)
+        if args.synthetic_topics:
+            data = dataclasses.replace(data, topics=synthetic_topics(data, args.synthetic_topics, seed=args.seed))
+    else:   # every qrels line is read only when one-vs-rest training asks for it
+        data = rcv1(cfg.data_path, full=cfg.full, topics=parse_topics(cfg.topics) is not None)
     report = scenario(cfg, data, rank=rank, world=world, device=local_rank, seed=args.seed,
                       log=lambda s: print(s, flush=True), jvm_exact=args.jvm_exact)
     if rank == 0:

@@ -42,6 +42,12 @@ ISOTONIC_INFO_WORDS = 5      # DSGD_ISOTONIC_INFO_WORDS: blocks, points, rows us
 ISOTONIC_EVAL_WORDS = 3      # DSGD_ISOTONIC_EVAL_WORDS: rows used, rows left out, rows with an infinite log-loss term
 BOOTSTRAP_WORDS = 9          # DSGD_BOOTSTRAP_WORDS: the METRICS_WORDS of a replicate, then its size (sum of m_i)
 BOOTSTRAP_MAX_ROWS = 1 << 26  # the rows of one bootstrap request
+MAX_TOPICS = 1024             # DSGD_MAX_TOPICS
+
+
+def topic_words(n_topics: int) -> int:
+    """DSGD_TOPIC_WORDS(T): eight words per topic, then eight row words"""
+    return 8 * int(n_topics) + 8
 
 
 class NativeLibraryMissing(ImportError):
@@ -155,6 +161,12 @@ ABI = {
     "dsgd_stop_async": [_vp],
     "dsgd_update_grad": [_vp, _vp, _vp, _i64],
     "dsgd_async_updates": [_vp, C.POINTER(_i64)],
+    "dsgd_load_topics": [_vp, _i32, _vp, _vp],
+    "dsgd_select_topic": [_vp, _i32],
+    # the topic family takes T weight vectors and their count before the rows
+    "dsgd_eval_topics": [_vp, _vp, _i32, _i64, _i64, _vp],
+    "dsgd_eval_sampled_topics": [_vp, _vp, _i32, _i64, _i64, _u64, _i64, _i64, _vp],
+    "dsgd_eval_samples_topics": [_vp, _vp, _i32, _vp, _i64, _vp],
 }
 _RESTYPE = {"dsgd_last_error": C.c_char_p, "dsgd_info": C.c_char_p}
 
@@ -224,6 +236,8 @@ def host_lib():
         h.dsgd_rcv1_count.argtypes = [C.c_char_p, C.POINTER(_i64), C.POINTER(_i64)]
         h.dsgd_rcv1_parse.argtypes = [C.c_char_p, _i32, _i64, _i64, _vp, _vp, _vp, _vp]
         h.dsgd_rcv1_labels.argtypes = [C.c_char_p, _vp, _i64, _vp]
+        h.dsgd_rcv1_topics_count.argtypes = [C.c_char_p, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i64)]
+        h.dsgd_rcv1_topics_parse.argtypes = [C.c_char_p, _i64, _i32, _i64, C.c_char_p, _vp, _vp]
         h.dsgd_rcv1_write.argtypes = [C.c_char_p, C.c_char_p, _i64, _vp, _vp, _vp, _vp, _i64]
         h.dsgd_draw_epoch.restype = C.c_int64
         h.dsgd_draw_epoch.argtypes = [C.c_uint64, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _i64]
@@ -352,6 +366,7 @@ class NativeCtx:
             self._h = C.c_void_p()
             raise _EXC.get(rc, DsgdError)(rc, msg)
         self.n_rows = 0
+        self.n_topics = 0
 
     # -- plumbing --
     def _ck(self, rc: int):
@@ -416,6 +431,7 @@ class NativeCtx:
             raise DsgdInvalid(ERR_INVALID, "load_csr: col/val shorter than row_ptr[-1]")
         self._ck(self._l.dsgd_load_csr(self._h, n_rows, nnz, _ptr(row_ptr), _ptr(col), _ptr(val), _ptr(label)))
         self.n_rows = n_rows
+        self.n_topics = 0
 
     def set_dim_sparsity(self, d):
         d = _arr(d, np.float64, self.dim, "dim_sparsity")
@@ -945,6 +961,42 @@ class NativeCtx:
     def eval_samples_class(self, samples, w=None) -> "ClassEval":
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_class)."""
         return self._class("eval_samples_class", w, _list(samples))
+
+    # -- topics (sync mode): one-vs-rest labels and the one-pass multi-label evaluation --
+    def load_topics(self, topic_ptr, topic_id, n_topics: int):
+        """Each loaded row's topic ids (CSR: topic_ptr int64[n_rows + 1], ids strictly ascending within a row, each in
+        [0, n_topics)); the ctx keeps the loaded labels beside them (dsgd_load_topics)."""
+        topic_ptr = _arr(topic_ptr, np.int64, self.n_rows + 1, "topic_ptr")
+        topic_id = _arr(topic_id, np.int32)
+        if topic_id.size != int(topic_ptr[-1]):
+            raise DsgdInvalid(ERR_INVALID, f"load_topics: {topic_id.size} ids, topic_ptr ends at {int(topic_ptr[-1])}")
+        self._ck(self._l.dsgd_load_topics(self._h, int(n_topics), _ptr(topic_ptr), _ptr(topic_id)))
+        self.n_topics = int(n_topics)
+
+    def select_topic(self, topic: int):
+        """Labels "has topic t" (+1 / -1) for every following call; -1: the labels load_csr loaded (dsgd_select_topic)."""
+        self._ck(self._l.dsgd_select_topic(self._h, int(topic)))
+
+    def _topics(self, fn: str, W, rows: _Rows) -> np.ndarray:
+        W = np.ascontiguousarray(W, dtype=np.float64)
+        if W.ndim != 2 or W.shape[1] != self.wdim:
+            raise DsgdInvalid(ERR_INVALID, f"{fn}: W must be [T, {self.wdim}], got {W.shape}")
+        out = np.zeros(topic_words(W.shape[0]), dtype=np.int64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(W), W.shape[0], *rows.args, _ptr(out)))
+        return out
+
+    def eval_topics(self, row_begin: int, row_end: int, W) -> np.ndarray:
+        """The DSGD_TOPIC_WORDS(T) words of the T weight vectors W[T, wdim] over rows [row_begin, row_end): per topic the
+        metrics words for "has topic t" (U2 left 0), then the row words (dsgd_eval_topics)."""
+        return self._topics("eval_topics", W, _range(row_begin, row_end))
+
+    def eval_sampled_topics(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, W) -> np.ndarray:
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_topics)."""
+        return self._topics("eval_sampled_topics", W, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def eval_samples_topics(self, samples, W) -> np.ndarray:
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_topics)."""
+        return self._topics("eval_samples_topics", W, _list(samples))
 
     # -- sample weights (sync mode) and the weighted evaluations --
     def set_sample_weights(self, sw):

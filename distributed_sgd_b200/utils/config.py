@@ -45,6 +45,8 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     fit_intercept: bool = False   # extension: fit an unregularised intercept (weights dim + 1 long), sync mode only
     bootstrap: int = 0            # extension: Poisson-bootstrap replicates of the final test metrics' intervals; 0: off
     bootstrap_weighted: bool = False   # extension: the bootstrap counts every row by its weight (class x sample weight)
+    topics: str = ""              # extension: one-vs-rest training of a multi-label set after the binary run: empty (off),
+                                  # all, or a comma-separated list of topic names; sync mode only
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -66,6 +68,7 @@ _KEYS = {
     "fit-intercept": ("fit_intercept", "DSGD_FIT_INTERCEPT"),
     "bootstrap": ("bootstrap", "DSGD_BOOTSTRAP"),
     "bootstrap-weighted": ("bootstrap_weighted", "DSGD_BOOTSTRAP_WEIGHTED"),
+    "topics": ("topics", "DSGD_TOPICS"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -149,4 +152,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"bootstrap: expected a number of replicates >= 0 (0: off), got {cfg.bootstrap}")
     if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
         raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
+    from ..ml.one_vs_rest import parse_topics
+    parse_topics(cfg.topics)   # raises on a malformed value
     return cfg

@@ -250,6 +250,44 @@ int dsgd_eval_sampled_metrics(dsgd_ctx *ctx, const double *w, int64_t row_begin,
                               int64_t pos_begin, int64_t pos_end, int64_t *out);
 int dsgd_eval_samples_metrics(dsgd_ctx *ctx, const double *w, const int32_t *samples, int64_t n, int64_t *out);
 
+/* ---- Topics: one-vs-rest labels of a multi-label data set (DESIGN.md §4.21).  Sync mode only.
+ *      dsgd_load_topics: the topics of every loaded row as a CSR: row r has the ids topic_id[topic_ptr[r] .. topic_ptr[r+1]),
+ *      strictly ascending, each in [0, n_topics); topic_ptr holds n_rows + 1 entries, topic_ptr[0] = 0, and topic_ptr[n_rows]
+ *      is the id count.  Everything is checked on the host before anything changes on the device: a topic_ptr that is not
+ *      monotone or does not start at 0, an id outside [0, n_topics), ids of a row not strictly ascending, or n_topics outside
+ *      [1, DSGD_MAX_TOPICS] -> DSGD_ERR_INVALID; no rows loaded or an async ctx -> DSGD_ERR_STATE.  The ctx keeps a copy of
+ *      the labels dsgd_load_csr loaded; loading topics again first restores them.  dsgd_load_csr drops the topics.
+ *      dsgd_select_topic(t): label(r) = +1 when row r has topic t, else -1, for every row, and the streaming pass's
+ *      per-row word follows (its sign is the label).  t = -1: the labels dsgd_load_csr loaded.  Every training and
+ *      evaluation path reads the labels when it launches, so after the call every one of them sees exactly the labels a
+ *      ctx freshly loaded with them would.  No topics loaded or an async ctx -> DSGD_ERR_STATE; t outside [-1, T) ->
+ *      DSGD_ERR_INVALID.
+ *      dsgd_eval*_topics: W holds n_topics weight vectors of the weight length (dim, or dim + 1 with the intercept last),
+ *      W_t = W[t * wlen .. (t + 1) * wlen), each the w a caller would pass to dsgd_margins.  Over the rows of the request
+ *      (the three row forms of the metrics calls, with their errors), with y_t = +1 when the row has topic t (from the
+ *      loaded topics, never from the current labels) and p_t the prediction of dsgd_forward for W_t:
+ *        out[8 t .. 8 t + 8)  the DSGD_METRICS_WORDS of dsgd_eval_metrics for the labels y_t and the weights W_t, except
+ *                             out[8 t + 6] (U2), which is 0
+ *        out[8 T + 0]         rows
+ *        out[8 T + 1]         rows with p_t = y_t for every t (p = 0 is never right)
+ *        out[8 T + 2]         rows with a topic whose top-scored topic is one of theirs: the top-scored topic has the lowest
+ *                             x . W_t among the non-NaN scores (the highest score -x . W_t), ties to the lowest t
+ *        out[8 T + 3]         rows with no topic
+ *        out[8 T + 4]         rows with no non-NaN score
+ *        out[8 T + 5 .. 8)    0
+ *      Every word is an exact integer, the same whatever the grid or the row order.  n_topics other than the loaded T or a
+ *      NULL W or out -> DSGD_ERR_INVALID; no topics loaded or an async ctx -> DSGD_ERR_STATE; all before anything is
+ *      launched.  A call copies T * wlen doubles to the device. */
+#define DSGD_MAX_TOPICS 1024
+#define DSGD_TOPIC_WORDS(T) (8 * (int64_t)(T) + 8)
+int dsgd_load_topics(dsgd_ctx *ctx, int32_t n_topics, const int64_t *topic_ptr, const int32_t *topic_id);
+int dsgd_select_topic(dsgd_ctx *ctx, int32_t topic);
+int dsgd_eval_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end, int64_t *out);
+int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end,
+                             uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *out);
+int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
+                             int64_t *out);
+
 /* ---- ROC and precision-recall curves and average precision over the same three row forms, with the conventions and errors
  *      of the metrics calls above.  Over the non-NaN rows, let t_0 > t_1 > ... > t_(m-1) be the distinct scores s = -x.w
  *      (+0 and -0 are one score).  Point k: thr_out[k] = t_k (a zero score as +0), tp_out[k] = positive rows with s >= t_k,
