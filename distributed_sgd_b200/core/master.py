@@ -18,11 +18,11 @@ from ..ml.calibration import METHODS as CALIBRATION_METHODS, Calibration, Isoton
 from ..ml.class_weight import resolve_class_weight
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
-from ..ml.one_vs_rest import OneVsRest, topic_report
+from ..ml.one_vs_rest import OneVsRest, topic_ranking_report, topic_report
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge
 from ..ml.sparse_svm import SparseSVM
-from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx
+from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx, topic_rank_words
 from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights
 from .group import Group
 from .slave import Slave
@@ -621,6 +621,40 @@ class Master:
         else:
             words = self.ctx.eval_samples_topics(ids[lo:hi], W)
         return self._topic_words(words)
+
+    def _topic_ranking_words(self, words, k: int) -> dict:
+        """The ranking report of the words every rank computed for its share, summed over ranks: integers and limbs below
+        2^40 each, so the float64 sum is exact and the merged limbs convert once (topic_ranking_report)."""
+        total = np.rint(self.group.all_reduce_sum([float(x) for x in words])).astype(np.int64)
+        return topic_ranking_report(total, k)
+
+    def local_topic_ranking_report(self, weights, k: int, test_data: bool = True) -> dict:
+        """Multi-label ranking quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train)
+        rows in one device pass (dsgd_eval_topic_ranking): precision@j and recall@j for j = 1..k, label ranking average
+        precision, coverage error and ranking loss (ml/one_vs_rest.py: topic_ranking_report).  Each rank evaluates a
+        contiguous share of the rows, as local_topic_report splits them."""
+        W = self._topic_weights(weights)
+        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        n, R, r = e - b, self.group.world, self.group.rank
+        lo, hi = b + (n * r) // R, b + (n * (r + 1)) // R
+        words = self.ctx.eval_topic_ranking(lo, hi, W, k)[0] if hi > lo else np.zeros(topic_rank_words(k), dtype=np.int64)
+        return self._topic_ranking_words(words, k)
+
+    def local_sampled_topic_ranking_report(self, weights, k: int, samples_count: int, test_data: bool = True) -> dict:
+        """local_topic_ranking_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it;
+        rank r of R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
+        W = self._topic_weights(weights)
+        b, e, m, key, ids = self._draw_sample(samples_count, test_data)
+        if m <= 0:
+            raise DsgdEmpty(ERR_EMPTY, f"sampled topic ranking report of {samples_count} rows: the sample is empty")
+        lo, hi = sample_shard(m, self.group.world, self.group.rank)
+        if hi <= lo:
+            words = np.zeros(topic_rank_words(k), dtype=np.int64)
+        elif ids is None:
+            words = self.ctx.eval_sampled_topic_ranking(b, e, key, lo, hi, W, k)[0]
+        else:
+            words = self.ctx.eval_samples_topic_ranking(ids[lo:hi], W, k)[0]
+        return self._topic_ranking_words(words, k)
 
     # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
     # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank

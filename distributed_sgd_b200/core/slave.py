@@ -131,6 +131,12 @@ class Slave:
         self._train_ids(samples_idx)
         return self.ctx.margins(samples_idx, weights)
 
+    def topics_topk(self, samples_idx: Sequence[int], weights: np.ndarray, k: int):
+        """Extension: (ids int32[n, k], margins float64[n, k]), the k highest-scored topics of each listed row under the
+        [T, wdim] weights (score -x . w_t, ties to the lower t; NaN scores left out, -1 and NaN in their slots)."""
+        self._train_ids(samples_idx)
+        return self.ctx.topics_topk(samples_idx, weights, k)
+
     def probabilities(self, samples_idx: Sequence[int], weights: Optional[np.ndarray] = None) -> np.ndarray:
         """Extension, SparseLogistic and SparseModifiedHuber only (other models raise DsgdState): P(y = +1 | x) of the listed
         rows, sigmoid(-x.w) or (clip(-x.w, -1, 1) + 1) / 2."""

@@ -137,6 +137,10 @@ struct dsgd_ctx {
   // a topic evaluation (dsgd_eval_*topics): the T weight vectors and the DSGD_TOPIC_WORDS(T) counter words
   dev_buf<double> t_w;
   dev_buf<unsigned long long> t_cnt;
+  // a topic ranking (dsgd_eval_*topic_ranking): its words and limb words; dsgd_topics_topk: the n k ids and margins
+  dev_buf<unsigned long long> t_rank;
+  dev_buf<int32_t> t_top_ids;
+  dev_buf<double> t_top_m;
 
   // state (fp64, L2 resident) -- g has dim + 2 slots (hinge sum and batch size ride in the allreduce)
   dev_buf<double> w, g, d, w_req;
@@ -1638,6 +1642,15 @@ extern "C" int dsgd_select_topic(dsgd_ctx *ctx, int32_t topic) {
   return DSGD_OK;
 }
 
+// the T weight vectors W on the device (ctx->t_w)
+static int topic_weights_in(dsgd_ctx *ctx, const double *W, int32_t n_topics) {
+  const int64_t nw = (int64_t)n_topics * wlen(ctx);
+  int rc = ctx->t_w.grow(ctx, nw, 1024);
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(ctx->t_w, W, sizeof(double) * (size_t)nw, cudaMemcpyHostToDevice, ctx->stream));
+  return DSGD_OK;
+}
+
 // dsgd_eval*_topics: the DSGD_TOPIC_WORDS(T) words into out.  Every refusal comes before anything is launched.
 static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, const row_request &req, const char *fn,
                           int64_t *out) {
@@ -1651,9 +1664,8 @@ static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, cons
   row_set rows;
   int rc = ids_capped(ctx, req, fn);
   if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
-  const int64_t T = n_topics, words = DSGD_TOPIC_WORDS(T), nw = T * wlen(ctx);
-  if ((rc = ctx->t_w.grow(ctx, nw, 1024)) || (rc = ctx->t_cnt.grow(ctx, words, 1024))) return rc;
-  CU(cudaMemcpyAsync(ctx->t_w, W, sizeof(double) * (size_t)nw, cudaMemcpyHostToDevice, ctx->stream));
+  const int64_t T = n_topics, words = DSGD_TOPIC_WORDS(T);
+  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->t_cnt.grow(ctx, words, 1024))) return rc;
   CU(cudaMemsetAsync(ctx->t_cnt, 0, sizeof(unsigned long long) * (size_t)words, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
   const size_t smem = sizeof(unsigned) * (size_t)(T * kTopicWords);
@@ -1681,6 +1693,107 @@ extern "C" int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t 
 extern "C" int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
                                         int64_t *out) {
   return topics_request(ctx, W, n_topics, listed_rows(samples, n), __func__, out);
+}
+
+// ---- topic ranking (dsgd_topics.cuh: k_topic_rank; DESIGN.md §4.22) ----------------------------------------------------
+
+static double fixed_read(const unsigned long long *limbs, unsigned long long ovf);   // with the calibration calls, below
+
+static_assert(kRankMaxK == DSGD_TOPIC_RANK_MAX_K && kRankWords == 8 && kLossAccWords == 7, "DSGD_TOPIC_RANK_WORDS layout");
+
+// k_topic_rank's grid for n rows: at least 32 rows per warp
+static int rank_grid(const dsgd_ctx *ctx, int64_t n) {
+  return (int)std::min<int64_t>(cdiv(n, 32 * kRankWarps), (int64_t)ctx->sm_count * 16);
+}
+
+// dsgd_eval*_topic_ranking: the DSGD_TOPIC_RANK_WORDS(k) words into words_out and the 2 + k sums into sums_out.  The limb
+// words leave with their carries propagated (limbs 0..4 in [0, 2^40)) and each sum is fixed_read of its block, acc_value's
+// conversion.  Every refusal comes before anything is launched.
+static int topic_ranking_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, const row_request &req,
+                                 const char *fn, int64_t *words_out, double *sums_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(words_out && sums_out, DSGD_ERR_INVALID, "%s: an output is NULL", fn);
+  NEED(W, DSGD_ERR_INVALID, "%s: W is NULL (the call ranks by T weight vectors of the caller's)", fn);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (topics belong to the sync paths)", fn);
+  NEED(ctx->n_topics > 0, DSGD_ERR_STATE, "%s: no topics loaded", fn);
+  NEED(n_topics == ctx->n_topics, DSGD_ERR_INVALID, "%s: %d weight vectors for %d loaded topics", fn, n_topics,
+       ctx->n_topics);
+  NEED(k >= 1 && k <= std::min(n_topics, (int32_t)DSGD_TOPIC_RANK_MAX_K), DSGD_ERR_INVALID, "%s: k = %d; 1 .. min(T, %d)",
+       fn, k, DSGD_TOPIC_RANK_MAX_K);
+  row_set rows;
+  int rc = ids_capped(ctx, req, fn);
+  if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  const int64_t words = DSGD_TOPIC_RANK_WORDS(k);
+  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->t_rank.grow(ctx, words, 1024))) return rc;
+  CU(cudaMemsetAsync(ctx->t_rank, 0, sizeof(unsigned long long) * (size_t)words, ctx->stream));
+  const size_t smem = sizeof(double) * (size_t)kRankWarps * (size_t)n_topics;
+  with_icpt(ctx, [&](auto ic) {
+    k_topic_rank<ic, false><<<rank_grid(ctx, rows.n), 32 * kRankWarps, smem, ctx->stream>>>(
+        ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids, rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim, k,
+        ctx->t_rank, nullptr, nullptr);
+  });
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(words_out, ctx->t_rank, sizeof(int64_t) * (size_t)words, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  for (int s = 0; s < 2 + k; ++s) {
+    unsigned long long *q = (unsigned long long *)words_out + kRankWords + k + (int64_t)s * kLossAccWords;
+    for (int i = 0; i < kLossLimbs - 1; ++i) {
+      q[i + 1] += q[i] >> 40;
+      q[i] &= kLimbMask;
+    }
+    sums_out[s] = fixed_read(q, q[kLossLimbs]);
+  }
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_eval_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, int64_t row_begin,
+                                       int64_t row_end, int64_t *words_out, double *sums_out) {
+  return topic_ranking_request(ctx, W, n_topics, k, range_rows(row_begin, row_end), __func__, words_out, sums_out);
+}
+
+extern "C" int dsgd_eval_sampled_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, int64_t row_begin,
+                                               int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end,
+                                               int64_t *words_out, double *sums_out) {
+  return topic_ranking_request(ctx, W, n_topics, k, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__,
+                               words_out, sums_out);
+}
+
+extern "C" int dsgd_eval_samples_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k,
+                                               const int32_t *samples, int64_t n, int64_t *words_out, double *sums_out) {
+  return topic_ranking_request(ctx, W, n_topics, k, listed_rows(samples, n), __func__, words_out, sums_out);
+}
+
+extern "C" int dsgd_topics_topk(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, const int32_t *samples, int64_t n,
+                                int32_t *ids_out, double *margins_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(W && ids_out && margins_out, DSGD_ERR_INVALID, "%s: W or an output is NULL", __func__);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (topics belong to the sync paths)",
+       __func__);
+  NEED(n_topics >= 1 && n_topics <= DSGD_MAX_TOPICS, DSGD_ERR_INVALID, "%s: %d topics; 1 .. %d", __func__, n_topics,
+       DSGD_MAX_TOPICS);
+  NEED(k >= 1 && k <= std::min(n_topics, (int32_t)DSGD_TOPIC_RANK_MAX_K), DSGD_ERR_INVALID, "%s: k = %d; 1 .. min(T, %d)",
+       __func__, k, DSGD_TOPIC_RANK_MAX_K);
+  NEED(n <= (int64_t)INT32_MAX, DSGD_ERR_INVALID, "%s: %lld ids; at most 2^31 - 1", __func__, (long long)n);
+  row_set rows;
+  int rc = rows_list(ctx, samples, n, false, __func__, &rows);
+  if (rc) return rc;
+  const int64_t nk = n * k;
+  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->t_top_ids.grow(ctx, nk, 1024)) ||
+      (rc = ctx->t_top_m.grow(ctx, nk, 1024)))
+    return rc;
+  const size_t smem = sizeof(double) * (size_t)kRankWarps * (size_t)n_topics;
+  with_icpt(ctx, [&](auto ic) {
+    k_topic_rank<ic, true><<<rank_grid(ctx, rows.n), 32 * kRankWarps, smem, ctx->stream>>>(
+        ctx->rp16, ctx->pairs, nullptr, nullptr, rows.ids, rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim, k, nullptr,
+        ctx->t_top_ids, ctx->t_top_m);
+  });
+  LAUNCHED();
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(ids_out, ctx->t_top_ids, sizeof(int32_t) * (size_t)nk, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(margins_out, ctx->t_top_m, sizeof(double) * (size_t)nk, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
 }
 
 // ---- bootstrap (dsgd_bootstrap.cuh; DESIGN.md §4.19) --------------------------------------------------------------------

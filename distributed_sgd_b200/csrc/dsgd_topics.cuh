@@ -1,15 +1,19 @@
-// dsgd_topics.cuh -- sm_90a kernels of the topic calls (dsgd_select_topic, dsgd_eval_*topics; DESIGN.md §4.21).
+// dsgd_topics.cuh -- sm_90a kernels of the topic calls (dsgd_select_topic, dsgd_eval_*topics; DESIGN.md §4.21; the
+// ranking calls dsgd_eval_*topic_ranking and dsgd_topics_topk, §4.22).
 //
 // A ctx with topics keeps, beside its rows, each row's topic ids (a CSR, ascending within a row) and a copy of the labels
 // dsgd_load_csr loaded.
 //   * k_topic_select rewrites the binary labels as "has topic t" (t = -1: the loaded labels), and the sign of yabs with them.
 //   * k_topic_eval scores every row against all T weight vectors in one pass and counts, per topic, the eight words of
 //     dsgd_eval_metrics (U2 left 0), then the row words that need every topic of a row at once.
-// Every word is an integer sum, so the result does not depend on the grid, the row order or the work split.
+//   * k_topic_rank ranks every row's topics by the same scores: the top k, or the multi-label ranking words and sums.
+// Every word is an integer sum (the ranking's fractions exact fixed-point sums), so the result does not depend on the grid,
+// the row order or the work split.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dsgd_fixed.cuh"
 #include "dsgd_kernels.cuh"
 #include "dsgd_metrics.cuh"
 
@@ -33,6 +37,22 @@ __device__ __forceinline__ int64_t topic_lower_bound(const int32_t *__restrict__
     if (ids[mid] < t) b = mid + 1; else e = mid;
   }
   return b;
+}
+
+// The score of one row for one weight vector w, by the whole warp (every lane gets it): chunk 0 of the row fold from the
+// registers pre (pair b + lane + 32 u, a zero pair past the window), the chunks past it from memory with row_fold_from.
+// That is the async worker's split of the fold: the same terms in the same order as row_fold, so the score has the bits
+// dsgd_margins returns for w.  kIcpt: fl(x . w + filt(w[dim])), as row_score.
+template <bool kIcpt>
+__device__ __forceinline__ double topic_score(const uint2 *__restrict__ pairs, const uint2 (&pre)[4], int64_t b, int64_t e,
+                                              int lane, const double *__restrict__ w, int32_t dim) {
+  double acc = 0.0;
+#pragma unroll
+  for (int u = 0; u < 4; ++u)
+    acc += filt(filt((double)__uint_as_float(pre[u].y)) * (pre[u].y << 1 ? __ldg(&w[pre[u].x]) : 0.0));
+  double s = row_fold_from(pairs, b + kFoldPairs, e, lane, warp_sum(acc), [&](uint32_t c) { return __ldg(&w[c]); });
+  if constexpr (kIcpt) s = s + filt(__ldg(&w[dim]));
+  return s;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -62,9 +82,7 @@ __global__ void __launch_bounds__(256) k_topic_select(const int64_t *__restrict_
 // W[t * wdim, t * wdim + wdim) (on an intercept ctx the intercept is the last entry).
 //   * A warp takes 32 consecutive positions at a time, as warp_scores does, and walks their rows one after the other.
 //   * Of each row it loads chunk 0 of the row fold (the first kFoldPairs pairs, 4 per lane) into registers once, then folds
-//     it T times: chunk 0 from the registers, the chunks past it from memory with row_fold_from.  That is the async
-//     worker's split of the fold: the same terms in the same order as row_fold, so score_t has the bits dsgd_margins returns
-//     for W_t (and k_metrics_score ranks for it).  kIcpt: score_t = fl(x . W_t + filt(beta_t)), as row_score.
+//     it T times with topic_score, so score_t has the bits dsgd_margins returns for W_t (and k_metrics_score ranks for it).
 //   * y_t comes from the row's ascending topic list, walked alongside t.
 //   * Per-topic counts in shared memory (u32, one atomic per row and topic by lane 0), flushed once per CTA with u64
 //     atomics into cnt[8 t + k].  Row words in lane 0's registers, flushed once per warp into cnt[8 T + k].
@@ -105,13 +123,7 @@ __global__ void __launch_bounds__(256) k_topic_eval(const uint32_t *__restrict__
       double best_dot = 0.0;
       bool best_has = false;
       for (int32_t t = 0; t < T; ++t) {
-        const double *__restrict__ w = W + (int64_t)t * wdim;
-        double acc = 0.0;
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-          acc += filt(filt((double)__uint_as_float(pre[u].y)) * (pre[u].y << 1 ? __ldg(&w[pre[u].x]) : 0.0));
-        double s = row_fold_from(pairs, b + kFoldPairs, e, lane, warp_sum(acc), [&](uint32_t c) { return __ldg(&w[c]); });
-        if constexpr (kIcpt) s = s + filt(__ldg(&w[dim]));
+        const double s = topic_score<kIcpt>(pairs, pre, b, e, lane, W + (int64_t)t * wdim, dim);
         const bool has = tk < te && tids[tk] == t;
         tk += has;
         const int p = pred_of(s);
@@ -140,6 +152,188 @@ __global__ void __launch_bounds__(256) k_topic_eval(const uint32_t *__restrict__
   __syncthreads();
   for (int k = threadIdx.x; k < T * kTopicWords; k += blockDim.x)
     if (s_cnt[k]) atomicAdd(&cnt[k], (unsigned long long)s_cnt[k]);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Ranking a row's topics (dsgd_eval_*topic_ranking, dsgd_topics_topk; DESIGN.md §4.22).  The score of topic t is -m_t, m_t
+// the margin topic_score gives; a higher score ranks first, so the order is the margins ascending, ties to the lower t
+// (+0 and -0 compare equal).  A warp keeps its row's T margins in shared memory, topic t at sc[t]; lane l owns the topics
+// l + 32 q, q < ceil(T / 32), and keeps one bit per owned topic in a 32-bit mask (T <= 1024).
+// ---------------------------------------------------------------------------------------------------
+constexpr int kRankMaxK = 32;   // DSGD_TOPIC_RANK_MAX_K
+constexpr int kRankWarps = 4;   // warps per CTA of k_topic_rank: 4 T doubles of shared memory, at most 32 KB
+constexpr int kRankWords = 8;   // integer row words before the k hit words (DSGD_TOPIC_RANK_WORDS(k) = 8 + k + 7 (2 + k))
+enum TopicRankWord : int {
+  kRkRows = 0,      // rows
+  kRkRanked = 1,    // ranked rows (a topic, no NaN score)
+  kRkNan = 2,       // rows with a NaN score
+  kRkNoTopic = 3,   // rows with no topic and no NaN score
+  kRkAll = 4,       // ranked rows with every topic
+  kRkCoverage = 5,  // sum of max over l in Y of rank_l
+  kRkMisorder = 6   // sum over l in Y of rank_l - L_l
+};
+
+// The first topic of the order among the topics not yet taken (bit q of `taken`: topic lane + 32 q) whose margin is not
+// NaN: its margin into m and its id into t, on every lane; t = -1 when there is none.  Each lane walks its topics in
+// ascending t with a strict <, then the xor butterfly keeps the lower (m, t) pair: a total order, so every lane ends with
+// the same pair.
+__device__ __forceinline__ void warp_first_topic(const double *sc, int32_t T, int nq, int lane, unsigned taken, double &m,
+                                                 int &t) {
+  double bm = 0.0;
+  int bt = -1;
+  for (int q = 0; q < nq; ++q) {
+    const int u = lane + 32 * q;
+    if (u < T && !((taken >> q) & 1u)) {
+      const double v = sc[u];
+      if (!isnan(v) && (bt < 0 || v < bm)) { bm = v; bt = u; }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double om = __shfl_xor_sync(0xffffffffu, bm, o);
+    const int ot = __shfl_xor_sync(0xffffffffu, bt, o);
+    if (ot >= 0 && (bt < 0 || om < bm || (om == bm && ot < bt))) { bm = om; bt = ot; }
+  }
+  m = bm;
+  t = bt;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_topic_rank: rows samples[0..n) (samples == nullptr: rows [row_begin, row_begin + n)) against the T weight vectors W, with
+// the warp-per-row walk of k_topic_eval and topic_score for every margin.  After a row's T margins are in sc:
+//   kTopk: k rounds of warp_first_topic, each taking its topic out; lane 0 writes round j's id and margin to
+//     ids[i k + j], top[i k + j] (i the row's position; -1 and NaN once the non-NaN margins are used up).
+//   else: the ranking words of DSGD_TOPIC_RANK_WORDS(k) into cnt.  A row is ranked when it has a topic (Y, from the loaded
+//     topics) and no NaN margin.  For each l in Y, one pass over the warp's topics counts rank_l = #{u : m_u <= m_l} and
+//     L_l = #{u in Y : m_u <= m_l} (packed in one u32 per lane, added with __reduce_add_sync): n_Y T / 32 shared loads per
+//     lane.  The top-k is k rounds of warp_first_topic; round j's hit comes from the owner lane's Y mask.
+//     Integer words: 0..6 in lane 0's registers, word 8 + j (hits in the first j + 1) in lane j's; flushed once per warp.
+//     Fixed-point sums (acc_add_local, flushed once per warp with acc_flush_local): lane 0 holds A, lane 1 holds B, lane j
+//     holds C_(j+1).  Every term is one IEEE division of two exact integers.
+// Dynamic shared memory: kRankWarps T doubles.
+// ---------------------------------------------------------------------------------------------------
+template <bool kIcpt, bool kTopk>
+__global__ void __launch_bounds__(32 * kRankWarps) k_topic_rank(const uint32_t *__restrict__ rp16,
+                                                               const uint2 *__restrict__ pairs,
+                                                               const int64_t *__restrict__ tptr,
+                                                               const int32_t *__restrict__ tids,
+                                                               const int32_t *__restrict__ samples, int64_t row_begin,
+                                                               int64_t n, const double *__restrict__ W, int32_t T,
+                                                               int32_t dim, int32_t k, unsigned long long *__restrict__ cnt,
+                                                               int32_t *__restrict__ ids, double *__restrict__ top) {
+  extern __shared__ double s_sc[];   // [kRankWarps][T]
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  double *sc = s_sc + (int64_t)(threadIdx.x >> 5) * T;
+  const int nq = (T + 31) >> 5;
+  const int64_t wdim = (int64_t)dim + (kIcpt ? 1 : 0);
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  unsigned long long rw[7] = {0, 0, 0, 0, 0, 0, 0};   // words 0..6 (lane 0's count)
+  unsigned long long hits = 0;                        // word 8 + lane (lane < k)
+  unsigned long long lim_ab[kLossLimbs] = {}, ovf_ab = 0;   // lane 0: A, lane 1: B
+  unsigned long long lim_c[kLossLimbs] = {}, ovf_c = 0;     // lane j < k: C_(j+1)
+  for (int64_t g = warp0 * 32; g < n; g += nwarps * 32) {
+    const int64_t i_own = g + lane;
+    const int64_t r_own = i_own < n ? (samples ? (int64_t)samples[i_own] : row_begin + i_own) : 0;
+    const int m = (int)(n - g < 32 ? n - g : 32);
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j);
+      const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+      uint2 pre[4];   // chunk 0: pair b + lane + 32 u, a zero pair past the window
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int64_t c = b + lane + 32 * u;
+        pre[u] = c < e ? __ldg(&pairs[c]) : make_uint2(0u, 0u);
+      }
+      for (int32_t t = 0; t < T; ++t) {
+        const double s = topic_score<kIcpt>(pairs, pre, b, e, lane, W + (int64_t)t * wdim, dim);
+        if (lane == (t & 31)) sc[t] = s;
+      }
+      __syncwarp();
+      if constexpr (kTopk) {
+        const int64_t i = g + j;
+        unsigned taken = 0;
+        for (int q = 0; q < k; ++q) {
+          double bm;
+          int bt;
+          warp_first_topic(sc, T, nq, lane, taken, bm, bt);
+          if (bt >= 0 && lane == (bt & 31)) taken |= 1u << (bt >> 5);
+          if (lane == 0) {
+            ids[i * k + q] = bt;
+            top[i * k + q] = bt >= 0 ? bm : __longlong_as_double(0x7ff8000000000000ll);
+          }
+        }
+      } else {
+        const int64_t tb = tptr[r], te = tptr[r + 1];
+        const int nY = (int)(te - tb);
+        bool nan = false;
+        for (int q = 0; q < nq; ++q) {
+          const int u = lane + 32 * q;
+          nan = nan || (u < T && isnan(sc[u]));
+        }
+        nan = __any_sync(full, nan);
+        rw[kRkRows] += 1;
+        if (nan) {
+          rw[kRkNan] += 1;
+        } else if (nY == 0) {
+          rw[kRkNoTopic] += 1;
+        } else {
+          unsigned inY = 0;   // bit q: topic lane + 32 q is one of the row's
+          for (int64_t c = tb; c < te; ++c) {
+            const int32_t id = tids[c];
+            if ((id & 31) == lane) inY |= 1u << (id >> 5);
+          }
+          rw[kRkRanked] += 1;
+          rw[kRkAll] += nY == T;
+          int cov = 0;
+          int64_t mis = 0;
+          for (int64_t c = tb; c < te; ++c) {
+            const double ml = sc[tids[c]];
+            unsigned cl = 0;   // low 16 bits: u with m_u <= m_l; high: those in Y
+            for (int q = 0; q < nq; ++q) {
+              const int u = lane + 32 * q;
+              if (u < T && sc[u] <= ml) cl += 1u + (((inY >> q) & 1u) << 16);
+            }
+            cl = __reduce_add_sync(full, cl);
+            const int rank = (int)(cl & 0xffffu), L = (int)(cl >> 16);
+            cov = max(cov, rank);
+            mis += rank - L;
+            if (lane == 0) acc_add_local(lim_ab, ovf_ab, (double)L / (double)(rank * nY));
+          }
+          rw[kRkCoverage] += cov;
+          rw[kRkMisorder] += mis;
+          if (lane == 1 && nY < T) acc_add_local(lim_ab, ovf_ab, (double)mis / (double)((int64_t)nY * (T - nY)));
+          unsigned taken = 0;
+          int h = 0;
+          for (int q = 0; q < k; ++q) {
+            double bm;
+            int bt;
+            warp_first_topic(sc, T, nq, lane, taken, bm, bt);   // bt >= 0: no NaN and k <= T
+            const int owner = bt & 31, bit = bt >> 5;
+            h += (__shfl_sync(full, inY, owner) >> bit) & 1u;
+            if (lane == owner) taken |= 1u << bit;
+            if (lane == q) {
+              hits += h;
+              acc_add_local(lim_c, ovf_c, (double)h / (double)nY);
+            }
+          }
+        }
+      }
+      __syncwarp();   // every lane is done with sc before the next row's margins go in
+    }
+  }
+  if constexpr (!kTopk) {
+    if (lane == 0) {
+#pragma unroll
+      for (int w = 0; w < 7; ++w)
+        if (rw[w]) atomicAdd(&cnt[w], rw[w]);
+    }
+    if (lane < k && hits) atomicAdd(&cnt[kRankWords + lane], hits);
+    unsigned long long *sums = cnt + kRankWords + k;   // A, B, C_1 .. C_k: kLossAccWords words each
+    if (lane < 2) acc_flush_local(sums + lane * kLossAccWords, lim_ab, ovf_ab);
+    if (lane < k) acc_flush_local(sums + (2 + lane) * kLossAccWords, lim_c, ovf_c);
+  }
 }
 
 }  // namespace dsgd

@@ -235,6 +235,19 @@ object DsgdNative {
   @native def evalSampledTopics(ctx: Long, W: Array[Double], nTopics: Int, rowBegin: Long, rowEnd: Long, key: Long,
                                 posBegin: Long, posEnd: Long, out: Array[Long]): Int
   @native def evalSamplesTopics(ctx: Long, W: Array[Double], nTopics: Int, samples: Array[Int], out: Array[Long]): Int
+  // topic ranking (sync mode): W as evalTopics, 1 <= k <= min(nTopics, 32).  evalTopicRanking: words.length >= 8 + k +
+  // 7 * (2 + k) (rows, ranked rows, rows with a NaN score, rows without a topic, ranked rows with every topic, coverage,
+  // mis-ordered pairs, 0, hits in the top j for j = 1..k, then the limbs of A, B, C_1..C_k), sums.length >= 2 + k (their
+  // values).  topicsTopk: ids and margins at least samples.length * k long; row i's first k topics by score (-1 and NaN past
+  // its non-NaN scores); needs no loaded topics
+  @native def evalTopicRanking(ctx: Long, W: Array[Double], nTopics: Int, k: Int, rowBegin: Long, rowEnd: Long,
+                               words: Array[Long], sums: Array[Double]): Int
+  @native def evalSampledTopicRanking(ctx: Long, W: Array[Double], nTopics: Int, k: Int, rowBegin: Long, rowEnd: Long,
+                                      key: Long, posBegin: Long, posEnd: Long, words: Array[Long], sums: Array[Double]): Int
+  @native def evalSamplesTopicRanking(ctx: Long, W: Array[Double], nTopics: Int, k: Int, samples: Array[Int],
+                                      words: Array[Long], sums: Array[Double]): Int
+  @native def topicsTopk(ctx: Long, W: Array[Double], nTopics: Int, k: Int, samples: Array[Int], ids: Array[Int],
+                         margins: Array[Double]): Int
   // weighted curves, either model: metrics as evalCurve's, wsums(0 until 13) the DSGD_WCURVE_WORDS weighted words, nPoints(0)
   // = m, thr / tpw / fpw(0 until m) the points (W+ and W- at or above each score); all three null for the words alone, else
   // each at least as long as the request's rows.  An async ctx is refused.

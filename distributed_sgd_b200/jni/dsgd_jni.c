@@ -912,6 +912,55 @@ FN(evalSampledTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint n
 FN(evalSamplesTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jintArray samples, jlongArray out) {
   return req_topics(env, h, W, nTopics, list_rows(samples), out);
 }
+/* W exactly nTopics weight vectors long (null: refused by the library), words at least DSGD_TOPIC_RANK_WORDS(k) and sums
+ * at least 2 + k (k itself is checked by the library) */
+static int req_topic_ranking(JNIEnv *env, jlong h, jdoubleArray W, jint nTopics, jint k, rows_t r, jlongArray words,
+                             jdoubleArray sums) {
+  buf_t bw = in_Double(env, W), o = out_Long(env, words), s = out_Double(env, sums);
+  r.ids = in_Int(env, r.samples);
+  int32_t wl = 0;
+  int rc = checked(weight_len(h, &wl), bw.bad | o.bad | s.bad | r.ids.bad, 0);
+  if (rc == DSGD_OK)
+    rc = checked(DSGD_OK, 0, nTopics < 1 || k < 1 || k > DSGD_TOPIC_RANK_MAX_K || (bw.p && bw.n != (jlong)nTopics * wl) ||
+                                 o.n < DSGD_TOPIC_RANK_WORDS(k) || s.n < 2 + (jlong)k);
+  if (rc == DSGD_OK)
+    rc = r.form == RANGE ? dsgd_eval_topic_ranking(CTX(h), bw.p, nTopics, k, r.rowBegin, r.rowEnd, o.p, s.p)
+         : r.form == DRAWN ? dsgd_eval_sampled_topic_ranking(CTX(h), bw.p, nTopics, k, r.rowBegin, r.rowEnd, (uint64_t)r.key,
+                                                             r.posBegin, r.posEnd, o.p, s.p)
+                           : dsgd_eval_samples_topic_ranking(CTX(h), bw.p, nTopics, k, r.ids.p, r.ids.n, o.p, s.p);
+  back_Long(env, words, o, rc);
+  back_Double(env, sums, s, rc);
+  free(bw.p); free(r.ids.p);
+  return rc;
+}
+FN(evalTopicRanking)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jint k, jlong rowBegin, jlong rowEnd,
+                     jlongArray words, jdoubleArray sums) {
+  return req_topic_ranking(env, h, W, nTopics, k, range_rows(rowBegin, rowEnd), words, sums);
+}
+FN(evalSampledTopicRanking)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jint k, jlong rowBegin,
+                            jlong rowEnd, jlong key, jlong posBegin, jlong posEnd, jlongArray words, jdoubleArray sums) {
+  return req_topic_ranking(env, h, W, nTopics, k, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), words, sums);
+}
+FN(evalSamplesTopicRanking)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jint k, jintArray samples,
+                            jlongArray words, jdoubleArray sums) {
+  return req_topic_ranking(env, h, W, nTopics, k, list_rows(samples), words, sums);
+}
+/* W exactly nTopics weight vectors long, ids and margins at least samples.length * k */
+FN(topicsTopk)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jint k, jintArray samples, jintArray ids,
+               jdoubleArray margins) {
+  buf_t bw = in_Double(env, W), sm = in_Int(env, samples), oi = out_Int(env, ids), om = out_Double(env, margins);
+  int32_t wl = 0;
+  int rc = checked(weight_len(h, &wl), bw.bad | sm.bad | oi.bad | om.bad, 0);
+  const jlong nk = (jlong)sm.n * (k > 0 ? k : 0);
+  if (rc == DSGD_OK)
+    rc = checked(DSGD_OK, 0, nTopics < 1 || k < 1 || k > DSGD_TOPIC_RANK_MAX_K || (bw.p && bw.n != (jlong)nTopics * wl) ||
+                                 !oi.p || !om.p || oi.n < nk || om.n < nk);
+  if (rc == DSGD_OK) rc = dsgd_topics_topk(CTX(h), bw.p, nTopics, k, sm.p, sm.n, oi.p, om.p);
+  back_Int(env, ids, oi, rc);
+  back_Double(env, margins, om, rc);
+  free(bw.p); free(sm.p);
+  return rc;
+}
 static int req_weighted(JNIEnv *env, jlong h, jdoubleArray w, rows_t r, jdoubleArray sums, jlongArray counts) {
   req_t q;
   buf_t s = out_Double(env, sums), c = out_Long(env, counts);

@@ -53,10 +53,11 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     if cfg.bootstrap_weighted and cfg.is_async:
         raise ValueError("bootstrap-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
                          "has none to resample by")
-    from .ml.one_vs_rest import parse_topics
+    from .ml.one_vs_rest import parse_topic_rank_k, parse_topics
     topics = parse_topics(cfg.topics)
     if topics is not None and cfg.is_async:
         raise ValueError("topics: one-vs-rest training belongs to sync training; asynchronous (Hogwild) training has none")
+    rank_k = parse_topic_rank_k(cfg.topic_rank_k, topics)
     if topics is None:   # the binary run alone, with the rows as they always were
         data = dataclasses.replace(data, topics=None)
     elif data.topics is None:
@@ -64,6 +65,8 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                          "--synthetic-topics N plants them on synthetic rows)")
     elif topics != "all":
         data = dataclasses.replace(data, topics=data.topics.select(topics))
+    if rank_k and rank_k > data.topics.n_topics:
+        raise ValueError(f"topic-rank-k: {rank_k} exceeds the {data.topics.n_topics} topics")
     if cfg.sample_weight:   # one weight per loaded row; the split below carries them
         data = dataclasses.replace(data, weight=load_sample_weights(cfg.sample_weight, data.n_rows))
     train, test = data.split_at(int(data.n_rows * 0.8))                       # Main.scala:52
@@ -182,6 +185,13 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
             log(f"one-vs-rest ({len(ovr.topics)} topics, {fit_s:.1f} s): test micro F1 {tr['micro_f1']:.4f}, macro F1 "
                 f"{tr['macro_f1']:.4f} over {tr['macro_f1_topics']} topics, subset accuracy {tr['subset_accuracy']:.4f}, "
                 f"Hamming loss {tr['hamming_loss']:.5f}, top-1 accuracy {tr['top1_accuracy']:.4f}")
+        if rank_k:
+            rr = master.local_topic_ranking_report(ovr, rank_k, test_data=True)
+            report["topic_ranking"] = rr
+            if rank == 0:
+                log(f"topic ranking (k = {rank_k}, {rr['ranked_rows']} ranked test rows): precision@{rank_k} "
+                    f"{rr['precision_at'][rank_k]:.4f}, recall@{rank_k} {rr['recall_at'][rank_k]:.4f}, LRAP "
+                    f"{rr['lrap']:.4f}, coverage error {rr['coverage_error']:.3f}, ranking loss {rr['ranking_loss']:.5f}")
     if inspect:
         inspect("done", (master, state))
     slave.stop()

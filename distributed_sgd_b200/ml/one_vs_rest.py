@@ -1,7 +1,9 @@
 """One-vs-rest (OvR) models of a multi-label set: one binary model per topic, "has topic t" against the rest.
 
 `MasterSync.fit_one_vs_rest` trains them one topic after another on one device context (dsgd_select_topic switches the
-labels on the device), and `Master.local_topic_report` judges them all in one pass (dsgd_eval_*topics).
+labels on the device), and `Master.local_topic_report` judges them all in one pass (dsgd_eval_*topics).  The ranking of a
+row's topics by their scores is one more pass: `OneVsRest.predict_topk` (dsgd_topics_topk) and
+`Master.local_topic_ranking_report` (dsgd_eval_*topic_ranking, read by `topic_ranking_report`).
 """
 from __future__ import annotations
 
@@ -26,6 +28,12 @@ class OneVsRest:
         for t in range(len(self.topics)):
             out[:, t] = slave.margins(idx, self.weights[t]) < 0.0
         return out
+
+    def predict_topk(self, slave, idx: Sequence[int], k: int):
+        """(ids int32[n, k], margins float64[n, k]): row idx[i]'s k highest-scored topics (score -x . w_t; ties to the lower
+        index), as indices into `topics`, and their margins, in one device pass (Slave.topics_topk, dsgd_topics_topk).
+        Topics with a NaN score are left out; their slots hold -1 and NaN."""
+        return slave.topics_topk(idx, self.weights, k)
 
 
 def parse_topics(raw: str):
@@ -76,3 +84,56 @@ def topic_report(words, names) -> dict:
             "macro_f1": float(np.mean(f1s)) if f1s else float("nan"), "macro_f1_topics": len(f1s),
             "subset_accuracy": ratio(exact, rows), "hamming_loss": ratio(fn + pos_none + fp + neg_none, rows * T),
             "top1_accuracy": ratio(top1, rows - no_topic)}
+
+
+TOPIC_RANK_MAX_K = 32   # DSGD_TOPIC_RANK_MAX_K
+LIMB_BITS, RES_BITS = 40, 160
+
+
+def parse_topic_rank_k(k: int, topics) -> int:
+    """The configuration value `topic-rank-k`: 0 (off) or 1..32, and only with `topics` set (the parsed value)."""
+    k = int(k)
+    if not 0 <= k <= TOPIC_RANK_MAX_K:
+        raise ValueError(f"topic-rank-k: expected 0 (off) or 1 .. {TOPIC_RANK_MAX_K}, got {k}")
+    if k and topics is None:
+        raise ValueError("topic-rank-k: ranks the topics of a one-vs-rest model; set `topics` too")
+    return k
+
+
+def limbs_value(block) -> float:
+    """The value of one fixed-point sum of seven words (limbs 0..5, limb i worth 2^(40 i - 160), then the overflow count),
+    converted exactly as the device's reader acc_value converts it: NaN with an overflow, else the carries propagated, then
+    the limbs added as doubles from the top down.  The limbs may be sums of several calls' limbs."""
+    q = [int(x) for x in np.asarray(block).reshape(-1)[:7]]
+    if q[6]:
+        return float("nan")
+    mask = (1 << LIMB_BITS) - 1
+    for i in range(5):
+        q[i + 1] += q[i] >> LIMB_BITS
+        q[i] &= mask
+    s = float(q[5]) * 2.0 ** LIMB_BITS
+    for i in range(4, -1, -1):
+        s += float(q[i]) * 2.0 ** (LIMB_BITS * i - RES_BITS)
+    return s
+
+
+def topic_ranking_report(words, k: int) -> dict:
+    """The report of a dsgd_eval_*topic_ranking call (or of several, their words added) from its DSGD_TOPIC_RANK_WORDS(k)
+    words.  Over the N ranked rows (a topic and no NaN score): precision@j = hits in the top j / (j N), recall@j = C_j / N,
+    label ranking average precision = A / N, coverage error = coverage / N and ranking loss = B / (N - rows with every
+    topic); NaN where a denominator is 0.  A, B and C_j are the values of their limbs (limbs_value)."""
+    k = int(k)
+    w = np.asarray(words, dtype=np.int64).reshape(-1)
+    if w.size != 8 + k + 7 * (2 + k):
+        raise ValueError(f"topic_ranking_report: {w.size} words for k = {k}, expected {8 + k + 7 * (2 + k)}")
+
+    def ratio(a, b) -> float:
+        return a / b if b else float("nan")
+
+    rows, N, nan_rows, no_topic, every, coverage = (int(x) for x in w[:6])
+    sums = [limbs_value(w[8 + k + 7 * s:8 + k + 7 * s + 7]) for s in range(2 + k)]
+    return {"k": k, "rows": rows, "ranked_rows": N, "rows_with_nan_score": nan_rows, "rows_without_topic": no_topic,
+            "rows_with_every_topic": every,
+            "precision_at": {j: ratio(int(w[8 + j - 1]), j * N) for j in range(1, k + 1)},
+            "recall_at": {j: ratio(sums[2 + j - 1], N) for j in range(1, k + 1)},
+            "lrap": ratio(sums[0], N), "coverage_error": ratio(coverage, N), "ranking_loss": ratio(sums[1], N - every)}

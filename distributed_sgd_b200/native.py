@@ -50,6 +50,14 @@ def topic_words(n_topics: int) -> int:
     return 8 * int(n_topics) + 8
 
 
+TOPIC_RANK_MAX_K = 32         # DSGD_TOPIC_RANK_MAX_K
+
+
+def topic_rank_words(k: int) -> int:
+    """DSGD_TOPIC_RANK_WORDS(k): eight row words, k hit words, then 2 + k fixed-point sums of seven words each"""
+    return 8 + int(k) + 7 * (2 + int(k))
+
+
 class NativeLibraryMissing(ImportError):
     pass
 
@@ -199,6 +207,10 @@ def _row_forms(family: str) -> dict:
 
 ABI.update({name: _ROW_PREFIX[form] + tail for family, tail in _ROW_FAMILIES.items()
             for form, name in _row_forms(family).items()})
+# the topic ranking family takes T weight vectors, their count and k between (ctx, W) and the rows; then words and sums
+ABI.update({name: _ROW_PREFIX[form][:2] + [_i32, _i32] + _ROW_PREFIX[form][2:] + [_vp, _vp]
+            for form, name in _row_forms("eval_topic_ranking").items()})
+ABI["dsgd_topics_topk"] = [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]
 
 
 def lib():
@@ -978,9 +990,7 @@ class NativeCtx:
         self._ck(self._l.dsgd_select_topic(self._h, int(topic)))
 
     def _topics(self, fn: str, W, rows: _Rows) -> np.ndarray:
-        W = np.ascontiguousarray(W, dtype=np.float64)
-        if W.ndim != 2 or W.shape[1] != self.wdim:
-            raise DsgdInvalid(ERR_INVALID, f"{fn}: W must be [T, {self.wdim}], got {W.shape}")
+        W = self._topic_W(fn, W)
         out = np.zeros(topic_words(W.shape[0]), dtype=np.int64)
         self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(W), W.shape[0], *rows.args, _ptr(out)))
         return out
@@ -997,6 +1007,49 @@ class NativeCtx:
     def eval_samples_topics(self, samples, W) -> np.ndarray:
         """The same over a list of row ids; repeats count every time (dsgd_eval_samples_topics)."""
         return self._topics("eval_samples_topics", W, _list(samples))
+
+    def _topic_W(self, fn: str, W) -> np.ndarray:
+        W = np.ascontiguousarray(W, dtype=np.float64)
+        if W.ndim != 2 or W.shape[1] != self.wdim:
+            raise DsgdInvalid(ERR_INVALID, f"{fn}: W must be [T, {self.wdim}], got {W.shape}")
+        return W
+
+    def _topic_ranking(self, fn: str, W, k: int, rows: _Rows) -> Tuple[np.ndarray, np.ndarray]:
+        W = self._topic_W(fn, W)
+        k = int(k)
+        if not 1 <= k <= TOPIC_RANK_MAX_K:
+            raise DsgdInvalid(ERR_INVALID, f"{fn}: k = {k}; 1 .. min(T, {TOPIC_RANK_MAX_K})")
+        words = np.zeros(topic_rank_words(k), dtype=np.int64)
+        sums = np.zeros(2 + k, dtype=np.float64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(W), W.shape[0], k, *rows.args, _ptr(words), _ptr(sums)))
+        return words, sums
+
+    def eval_topic_ranking(self, row_begin: int, row_end: int, W, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """(words, sums) of the ranking of every row's topics by the T weight vectors W[T, wdim] over rows
+        [row_begin, row_end): the DSGD_TOPIC_RANK_WORDS(k) words (row counts, coverage, mis-ordered pairs, hits in the top j,
+        then the limbs of the sums A, B, C_1..C_k) and the 2 + k sums' values (dsgd_eval_topic_ranking)."""
+        return self._topic_ranking("eval_topic_ranking", W, k, _range(row_begin, row_end))
+
+    def eval_sampled_topic_ranking(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, W,
+                                   k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_topic_ranking)."""
+        return self._topic_ranking("eval_sampled_topic_ranking", W, k, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def eval_samples_topic_ranking(self, samples, W, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_topic_ranking)."""
+        return self._topic_ranking("eval_samples_topic_ranking", W, k, _list(samples))
+
+    def topics_topk(self, samples, W, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """(ids int32[n, k], margins float64[n, k]): each listed row's first k topics by score -x . W_t (the margins
+        ascending, ties to the lower t) among its non-NaN scores, and their margins; -1 and NaN past them.  Needs no loaded
+        topics (dsgd_topics_topk)."""
+        W = self._topic_W("topics_topk", W)
+        rows = _list(samples)
+        k = int(k)
+        ids = np.zeros((rows.n, max(k, 0)), dtype=np.int32)
+        m = np.zeros((rows.n, max(k, 0)), dtype=np.float64)
+        self._ck(self._l.dsgd_topics_topk(self._h, _ptr(W), W.shape[0], k, *rows.args, _ptr(ids), _ptr(m)))
+        return ids, m
 
     # -- sample weights (sync mode) and the weighted evaluations --
     def set_sample_weights(self, sw):

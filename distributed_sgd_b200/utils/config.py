@@ -47,6 +47,8 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
     bootstrap_weighted: bool = False   # extension: the bootstrap counts every row by its weight (class x sample weight)
     topics: str = ""              # extension: one-vs-rest training of a multi-label set after the binary run: empty (off),
                                   # all, or a comma-separated list of topic names; sync mode only
+    topic_rank_k: int = 0         # extension: with `topics`, rank every test row's topics and report precision and recall at
+                                  # 1..k, LRAP, coverage error and ranking loss; 0: off, else 1..32
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -69,6 +71,7 @@ _KEYS = {
     "bootstrap": ("bootstrap", "DSGD_BOOTSTRAP"),
     "bootstrap-weighted": ("bootstrap_weighted", "DSGD_BOOTSTRAP_WEIGHTED"),
     "topics": ("topics", "DSGD_TOPICS"),
+    "topic-rank-k": ("topic_rank_k", "DSGD_TOPIC_RANK_K"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -152,6 +155,6 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"bootstrap: expected a number of replicates >= 0 (0: off), got {cfg.bootstrap}")
     if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
         raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
-    from ..ml.one_vs_rest import parse_topics
-    parse_topics(cfg.topics)   # raises on a malformed value
+    from ..ml.one_vs_rest import parse_topic_rank_k, parse_topics
+    parse_topic_rank_k(cfg.topic_rank_k, parse_topics(cfg.topics))   # raises on a malformed value of either
     return cfg

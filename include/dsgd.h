@@ -288,6 +288,50 @@ int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, i
 int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
                              int64_t *out);
 
+/* ---- Ranking a row's topics (DESIGN.md §4.22).  Sync mode only.  For a row and topic t, m_t is the margin dsgd_margins
+ *      returns for W_t, bit for bit (fl(x . W_t + filt(beta_t)) on an intercept ctx), and its score is s_t = -m_t: a higher
+ *      score ranks first, and +0 and -0 are one score.  Y is the row's loaded topics (never the current labels), n_Y = |Y|.
+ *      The order is the topics sorted by s descending, ties to the lower t; top_j is its first j topics.
+ *      rank_l = #{u : s_u >= s_l} (ties count against the row) and L_l = #{u in Y : s_u >= s_l}.  A row is ranked when
+ *      n_Y >= 1 and none of its T scores is NaN.
+ *      dsgd_eval*_topic_ranking: W and n_topics as dsgd_eval*_topics, 1 <= k <= min(T, DSGD_TOPIC_RANK_MAX_K), the rows in
+ *      the three forms of the metrics calls.  words_out holds DSGD_TOPIC_RANK_WORDS(k) int64 words:
+ *        words[0]              rows
+ *        words[1]              ranked rows, N
+ *        words[2]              rows with a NaN score
+ *        words[3]              rows with no topic and no NaN score (words[0] = words[1] + words[2] + words[3])
+ *        words[4]              ranked rows with n_Y = T (they have no ranking-loss pair)
+ *        words[5]              sum over ranked rows of max over l in Y of rank_l (coverage)
+ *        words[6]              sum over ranked rows and l in Y of rank_l - L_l: mis-ordered (own, other) pairs, ties counted
+ *        words[7]              0
+ *        words[8 + j - 1]      sum over ranked rows of |top_j intersect Y|, j = 1 .. k
+ *      then 2 + k fixed-point sums in blocks of 7 words each (limbs 0..5, limb i worth
+ *      2^(40 i - 160), the carries propagated so that limbs 0..4 lie in [0, 2^40), then an overflow count), in the order
+ *        A    over ranked rows and l in Y: fl(L_l / (rank_l n_Y))
+ *        B    over ranked rows with n_Y < T: fl(p_r / (n_Y (T - n_Y))), p_r the row's share of words[6]
+ *        C_j  for j = 1 .. k, over ranked rows: fl(|top_j intersect Y| / n_Y)
+ *      Each term is one IEEE division of two exact integers, summed exactly at a resolution of 2^-160 as the logistic loss
+ *      sum is; sums_out[2 + k] holds each block's value, converted as that sum's reader converts it.  Every output has the
+ *      same bits for any grid, row order or split, and limbs added over several calls (as float64 too: every limb is below
+ *      2^40) give, once the carries are propagated, the limbs of one call over all their rows.  The errors of
+ *      dsgd_eval*_topics, and a k outside [1, min(T, DSGD_TOPIC_RANK_MAX_K)] -> DSGD_ERR_INVALID, before any launch.
+ *      dsgd_topics_topk: for the listed rows (no topics need be loaded: a model can rank new rows), ids_out[i k .. i k + k)
+ *      holds the first k topics of the order over row samples[i]'s non-NaN scores and margins_out their margins, with the
+ *      bits of dsgd_margins; slots past the non-NaN count hold -1 and NaN.  n_topics outside [1, DSGD_MAX_TOPICS], a bad k
+ *      or a NULL array -> DSGD_ERR_INVALID; an async ctx -> DSGD_ERR_STATE; the list's errors as dsgd_margins; all before
+ *      any launch. */
+#define DSGD_TOPIC_RANK_MAX_K 32
+#define DSGD_TOPIC_RANK_WORDS(k) (8 + (int64_t)(k) + 7 * (2 + (int64_t)(k)))
+int dsgd_eval_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, int64_t row_begin, int64_t row_end,
+                            int64_t *words_out, double *sums_out);
+int dsgd_eval_sampled_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, int64_t row_begin,
+                                    int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *words_out,
+                                    double *sums_out);
+int dsgd_eval_samples_topic_ranking(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, const int32_t *samples,
+                                    int64_t n, int64_t *words_out, double *sums_out);
+int dsgd_topics_topk(dsgd_ctx *ctx, const double *W, int32_t n_topics, int32_t k, const int32_t *samples, int64_t n,
+                     int32_t *ids_out, double *margins_out);
+
 /* ---- ROC and precision-recall curves and average precision over the same three row forms, with the conventions and errors
  *      of the metrics calls above.  Over the non-NaN rows, let t_0 > t_1 > ... > t_(m-1) be the distinct scores s = -x.w
  *      (+0 and -0 are one score).  Point k: thr_out[k] = t_k (a zero score as +0), tp_out[k] = positive rows with s >= t_k,
