@@ -9,7 +9,7 @@ control flow over a handful of scalars per epoch (losses, accuracies, the stoppi
 """
 from __future__ import annotations
 
-from typing import Callable, List, Optional, Sequence, Union
+from typing import Callable, List, NamedTuple, Optional, Sequence, Union
 
 import numpy as np
 
@@ -22,7 +22,7 @@ from ..ml.one_vs_rest import OneVsRest, topic_ranking_report, topic_report
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge
 from ..ml.sparse_svm import SparseSVM
-from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx, topic_rank_words
+from ..native import ERR_EMPTY, DsgdEmpty, NativeCtx, row_methods, topic_rank_words, topic_words
 from ..utils.dataset import SAMPLE_WEIGHT_ASYNC, Data, has_sample_weights
 from .group import Group
 from .slave import Slave
@@ -138,6 +138,34 @@ def sample_shard(k: int, world: int, rank: int):
     return (k * rank) // world, (k * (rank + 1)) // world
 
 
+class Rows(NamedTuple):
+    """The rows of one evaluation request, in the form of the entry point that takes them: rows [lo, hi) (key and ids
+    None); positions [lo, hi) of the sample the device draws from rows [b, e) with `key`; or positions [lo, hi) of the row
+    ids `ids`."""
+    lo: int
+    hi: int
+    b: int = 0
+    e: int = 0
+    key: Optional[int] = None
+    ids: Optional[np.ndarray] = None
+
+    def call(self, ctx, family: str, *args, **kw):
+        """ctx's method of `family` (native.row_methods) for this form, over these rows, with the family's arguments."""
+        if self.ids is not None:
+            form, rows = "list", (self.ids[self.lo:self.hi],)
+        elif self.key is not None:
+            form, rows = "drawn", (self.b, self.e, self.key, self.lo, self.hi)
+        else:
+            form, rows = "range", (self.lo, self.hi)
+        return getattr(ctx, row_methods(family)[form])(*rows, *args, **kw)
+
+    def shard(self, world: int, rank: int) -> Optional["Rows"]:
+        """The contiguous share of these rows that rank `rank` of `world` evaluates (sample_shard of the positions), or
+        None when it is empty."""
+        lo, hi = sample_shard(self.hi - self.lo, world, rank)
+        return self._replace(lo=self.lo + lo, hi=self.lo + hi) if hi > lo else None
+
+
 def metrics_dict(words) -> dict:
     """The result of Master.local_metrics from the native.METRICS_WORDS counts of a dsgd_eval_*metrics call: the eight counts
     (tp, fn, pos_no_pred, fp, tn, neg_no_pred, u2, nan_scores), precision = TP / (TP + FP), recall = TP / P, f1 = 2 TP /
@@ -239,6 +267,16 @@ def weighted_calibration_dict(result) -> dict:
             "rows": int(words[0]), "nan_rows": int(words[1]), "weight": W,
             "bins": {"edges": np.arange(m + 1) / m, "weight": bin_w, "positive_weight": bin_pw, "mean_predicted": mean_p,
                      "observed": freq}}
+
+
+# (weighted, isotonic) -> the fit family and its result's converter (Master.calibrate), and the quality family and its
+# result's converter (Master.local_calibration)
+_FITS = {(False, False): ("calibrate", _calibration), (True, False): ("calibrate_weighted", _weighted_calibration),
+         (False, True): ("calibrate_isotonic", _isotonic), (True, True): ("calibrate_isotonic_weighted", _weighted_isotonic)}
+_QUALITY = {(False, False): ("eval_calibration", calibration_dict),
+            (True, False): ("eval_weighted_calibration", weighted_calibration_dict),
+            (False, True): ("eval_isotonic_calibration", isotonic_calibration_dict),
+            (True, True): ("eval_weighted_isotonic_calibration", weighted_calibration_dict)}
 
 
 def curve_dict(result) -> dict:
@@ -399,19 +437,36 @@ class Master:
         return (MasterAsync if is_async else MasterSync)(node, data, test_data, model, node_count, **kw)
 
     # ---- evaluation ------------------------------------------------------------------------------------
-    def _local_eval(self, call: str, *args):
-        """(loss sum, correct count, ||w||^2) of this rank's share: ctx.<call>_counts for the SVM (its loss sum is the
-        integer hinge sum), ctx.<call>_sums for every other model.  With class weights ctx.<call>_class, and a fourth value:
-        (loss sum of the positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted.  With sample
-        weights ctx.<call>_weighted: (S = sum c_i L_i, correct count, ||w||^2)."""
+    def _split(self, test_data: bool):
+        """(b, e): the train rows [0, n_train) or the test rows [n_train, n_train + n_test)."""
+        return (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+
+    def _rows(self, test_data: bool, samples_count: Optional[int] = None, empty: Optional[str] = None) -> Optional[Rows]:
+        """The rows of a request over the train (or test) rows: all of them (samples_count None), or a fresh sample of
+        min(samples_count, n) of them (_draw_sample).  An empty sample raises DsgdEmpty with the message `empty`, or gives
+        None when `empty` is None."""
+        if samples_count is None:
+            return Rows(*self._split(test_data))
+        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
+        if k <= 0:
+            if empty is None:
+                return None
+            raise DsgdEmpty(ERR_EMPTY, empty)
+        return Rows(0, k, b, e, key, ids)
+
+    def _local_eval(self, rows: Rows, weights):
+        """(loss sum, correct count, ||w||^2) of `rows`: the eval_counts family for the SVM (its loss sum is the integer
+        hinge sum), eval_sums for every other model.  With class weights eval_class, and a fourth value: (loss sum of the
+        positive rows, correct count, ||w||^2, loss sum of the negative rows), unweighted.  With sample weights
+        eval_weighted: (S = sum c_i L_i, correct count, ||w||^2)."""
         if self.sample_weighted:
-            we = getattr(self.ctx, call + "_weighted")(*args)
+            we = rows.call(self.ctx, "eval_weighted", weights)
             return we.loss_sum, we.correct, we.norm_squared
         if self.weighted:
-            ce = getattr(self.ctx, call + "_class")(*args)
+            ce = rows.call(self.ctx, "eval_class", weights)
             as_sum = float if self.logistic else int   # the SVM's sums are integers: all-reduced exactly
             return as_sum(ce.loss_pos), ce.correct_pos + ce.correct_neg, ce.norm_squared, as_sum(ce.loss_neg)
-        return getattr(self.ctx, call + ("_sums" if self.logistic else "_counts"))(*args)
+        return rows.call(self.ctx, "eval_sums" if self.logistic else "eval_counts", weights)
 
     def _loss_sum(self, h, *h_neg):
         """The loss sum of an evaluation from its combined totals: h itself, or with class weights w_pos * h + w_neg * h_neg,
@@ -443,38 +498,39 @@ class Master:
             return float("nan")
         return self.model.lam * n2 + self.model.l1 * self.ctx.weights_l1(weights)[0]
 
-    def _eval_rows(self, weights, begin: int, end: int, want_loss: bool = True):
-        """Row-sharded pass: each rank evaluates a contiguous share, the loss sums and counters are summed."""
-        W, r = self.group.world, self.group.rank
-        n = end - begin
-        lo, hi = begin + (n * r) // W, begin + (n * (r + 1)) // W
-        if hi > lo:
-            h, c, n2, *h_neg = self._local_eval("eval", lo, hi, weights)
-        else:
+    def _loss_accuracy(self, weights, rows: Optional[Rows], want_loss: bool = True, grouped: bool = False):
+        """(loss, accuracy) of a row-sharded pass over `rows`: rank r of W evaluates rows.shard(W, r), and the loss sums and
+        counters are combined over ranks.  grouped (distributed_*): `rows` is already this rank's group of a split strategy
+        (None: it has none), and the groups' row counts are combined with the sums."""
+        share = rows if grouped else rows.shard(self.group.world, self.group.rank)
+        if share is None:
             h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
-        hs, cs, *h_neg, n2 = self._combine(h, c, n2, *h_neg)
+        else:
+            h, c, n2, *h_neg = self._local_eval(share, weights)
+        if grouped:
+            hs, cs, n, *h_neg, n2 = self._combine(h, c, n2, 0 if share is None else share.hi - share.lo, *h_neg)
+        else:
+            hs, cs, *h_neg, n2 = self._combine(h, c, n2, *h_neg)
+            n = rows.hi - rows.lo
         return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / n, cs / n
 
     def local_loss(self, weights=None, test_data: bool = False) -> float:
         """Master.localLoss (core/Master.scala:105-107)."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._eval_rows(weights, b, e)[0]
+        return self._loss_accuracy(weights, self._rows(test_data))[0]
 
     def local_accuracy(self, weights=None, test_data: bool = False) -> float:
         """Master.localAccuracy (core/Master.scala:100-103)."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._eval_rows(weights, b, e, want_loss=False)[1]
+        return self._loss_accuracy(weights, self._rows(test_data), want_loss=False)[1]
 
     def local_loss_accuracy(self, weights=None, test_data: bool = False):
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._eval_rows(weights, b, e)
+        return self._loss_accuracy(weights, self._rows(test_data))
 
     def _draw_sample(self, samples_count: int, test_data: bool):
         """(b, e, k, key, ids): a fresh sample of k = min(samples_count, n) of the working rows [b, e).  Every call draws anew,
         as every reference call reshuffles.  Default: the sample is drawn on the device with key = sampled_key(seed, t), t
         counting this Master's draws (the epoch draws of `fit` are separate); k <= 0 consumes no draw.  jvm_exact: ids =
         `Random.shuffle(indices) take k` from the java.util.Random stream `fit` also draws from (key is None)."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
+        b, e = self._split(test_data)
         n = e - b
         k = min(int(samples_count), n)
         key = ids = None
@@ -486,22 +542,6 @@ class Master:
             self._sampled_draws += 1
         return b, e, k, key, ids
 
-    def _eval_sample(self, weights, samples_count: int, test_data: bool, want_loss: bool = True):
-        """(loss, accuracy) on a fresh sample (_draw_sample), or None when that is empty.  Rank r of W evaluates positions
-        sample_shard(k, W, r); the loss sums and counters are summed over ranks."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            return None
-        lo, hi = sample_shard(k, self.group.world, self.group.rank)
-        if hi <= lo:
-            h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
-        elif ids is None:
-            h, c, n2, *h_neg = self._local_eval("eval_sampled", b, e, key, lo, hi, weights)
-        else:
-            h, c, n2, *h_neg = self._local_eval("eval_samples", ids[lo:hi], weights)
-        hs, cs, *h_neg, n2 = self._combine(h, c, n2, *h_neg)
-        return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / k, cs / k
-
     def local_sampled_loss(self, weights, samples_count: int, test_data: bool = False) -> float:
         """Master.localSampledLoss (core/Master.scala:109-112).  An empty sample raises DsgdEmpty, as the reference's
         `reduce` on an empty list throws."""
@@ -509,15 +549,14 @@ class Master:
 
     def local_sampled_accuracy(self, weights, samples_count: int, test_data: bool = False) -> float:
         """Master.localSampledAccuracy (core/Master.scala:114-118).  An empty sample gives nan (the reference's 0.0 / 0)."""
-        r = self._eval_sample(weights, samples_count, test_data, want_loss=False)
-        return float("nan") if r is None else r[1]
+        rows = self._rows(test_data, samples_count)
+        return float("nan") if rows is None else self._loss_accuracy(weights, rows, want_loss=False)[1]
 
     def local_sampled_loss_accuracy(self, weights, samples_count: int, test_data: bool = False):
-        """(loss, accuracy) on ONE sample, drawn once for both numbers.  An empty sample raises DsgdEmpty."""
-        r = self._eval_sample(weights, samples_count, test_data)
-        if r is None:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
-        return r
+        """(loss, accuracy) on ONE sample, drawn once for both numbers; rank r of W evaluates positions sample_shard(k, W,
+        r).  An empty sample raises DsgdEmpty."""
+        return self._loss_accuracy(weights, self._rows(
+            test_data, samples_count, f"sampled evaluation of {samples_count} rows: reduce on an empty collection"))
 
     # ---- per-class report (extension) -------------------------------------------------------------------------------------
     # Like the ranking metrics below it is not sharded: every rank holds every row and evaluates the whole range or sample,
@@ -537,16 +576,12 @@ class Master:
     def local_class_report(self, weights=None, test_data: bool = False) -> dict:
         """Rows, correct predictions and recall per class, balanced accuracy, accuracy, and the loss both unweighted and
         under the model's class weights, over the train (or test) rows; works whatever the weights are."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._class_report(self.ctx.eval_class(b, e, weights), weights)
+        return self._class_report(self._rows(test_data).call(self.ctx, "eval_class", weights), weights)
 
     def local_sampled_class_report(self, weights, samples_count: int, test_data: bool = False) -> dict:
         """local_class_report on a fresh sample (_draw_sample).  An empty sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
-        ce = self.ctx.eval_sampled_class(b, e, key, 0, k, weights) if ids is None else self.ctx.eval_samples_class(ids, weights)
-        return self._class_report(ce, weights)
+        rows = self._rows(test_data, samples_count, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
+        return self._class_report(rows.call(self.ctx, "eval_class", weights), weights)
 
     # ---- sample-weighted report (extension) -------------------------------------------------------------------------------
     # Not sharded, like the per-class report: every rank evaluates the whole range or sample, and the fixed-point sums have
@@ -561,17 +596,12 @@ class Master:
         """Rows, the sum of their combined weights c_i = class weight x sample weight, the weighted loss penalty + S / n and
         the weighted accuracy sum c_i [correct] / sum c_i over the train (or test) rows.  Without sample weights c_i is the
         class weight."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return self._weighted_report(self.ctx.eval_weighted(b, e, weights), weights)
+        return self._weighted_report(self._rows(test_data).call(self.ctx, "eval_weighted", weights), weights)
 
     def local_sampled_weighted_report(self, weights, samples_count: int, test_data: bool = False) -> dict:
         """local_weighted_report on a fresh sample (_draw_sample).  An empty sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
-        we = (self.ctx.eval_sampled_weighted(b, e, key, 0, k, weights) if ids is None
-              else self.ctx.eval_samples_weighted(ids, weights))
-        return self._weighted_report(we, weights)
+        rows = self._rows(test_data, samples_count, f"sampled evaluation of {samples_count} rows: reduce on an empty collection")
+        return self._weighted_report(rows.call(self.ctx, "eval_weighted", weights), weights)
 
     # ---- one-vs-rest topics (extension) ----------------------------------------------------------------------------------
     def _topic_weights(self, weights) -> np.ndarray:
@@ -588,73 +618,47 @@ class Master:
             raise ValueError(f"topic report: weights must be [{self.topics.n_topics}, {self.wdim}], got {W.shape}")
         return W
 
-    def _topic_words(self, words) -> dict:
-        """The report of the words every rank computed for its share, summed over ranks (integers: every rank gets the same
-        bits)."""
+    def _topic_report(self, W: np.ndarray, rows: Rows, k: Optional[int] = None) -> dict:
+        """The topic report (k None) or the topic ranking report at k of the T weight vectors W over `rows`.  Rank r of R
+        evaluates rows.shard(R, r), and the words are summed over ranks: integers and limbs below 2^40, so the float64 sum
+        is exact, every rank gets the same bits and merged limbs convert once (topic_ranking_report)."""
+        share = rows.shard(self.group.world, self.group.rank)
+        if k is None:
+            words = np.zeros(topic_words(len(W)), np.int64) if share is None else share.call(self.ctx, "eval_topics", W)
+        else:
+            words = (np.zeros(topic_rank_words(k), np.int64) if share is None
+                     else share.call(self.ctx, "eval_topic_ranking", W, k)[0])
         total = np.rint(self.group.all_reduce_sum([float(x) for x in words])).astype(np.int64)
-        return topic_report(total, self.topics.names)
+        return topic_report(total, self.topics.names) if k is None else topic_ranking_report(total, k)
 
     def local_topic_report(self, weights, test_data: bool = True) -> dict:
         """Multi-label quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train) rows, all
         topics in one device pass (dsgd_eval_topics): per topic the counts, precision, recall and F1; micro precision,
         recall and F1, macro F1, subset accuracy, Hamming loss and top-1 accuracy (ml/one_vs_rest.py: topic_report).  Each
-        rank evaluates a contiguous share of the rows, as _eval_rows splits them."""
-        W = self._topic_weights(weights)
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        n, R, r = e - b, self.group.world, self.group.rank
-        lo, hi = b + (n * r) // R, b + (n * (r + 1)) // R
-        words = self.ctx.eval_topics(lo, hi, W) if hi > lo else np.zeros(8 * len(W) + 8, dtype=np.int64)
-        return self._topic_words(words)
+        rank evaluates a contiguous share of the rows, as local_loss splits them."""
+        return self._topic_report(self._topic_weights(weights), self._rows(test_data))
 
     def local_sampled_topic_report(self, weights, samples_count: int, test_data: bool = True) -> dict:
-        """local_topic_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it; rank r of
-        R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
+        """local_topic_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it once the
+        weights are checked; rank r of R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
         W = self._topic_weights(weights)
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled topic report of {samples_count} rows: the sample is empty")
-        lo, hi = sample_shard(k, self.group.world, self.group.rank)
-        if hi <= lo:
-            words = np.zeros(8 * len(W) + 8, dtype=np.int64)
-        elif ids is None:
-            words = self.ctx.eval_sampled_topics(b, e, key, lo, hi, W)
-        else:
-            words = self.ctx.eval_samples_topics(ids[lo:hi], W)
-        return self._topic_words(words)
-
-    def _topic_ranking_words(self, words, k: int) -> dict:
-        """The ranking report of the words every rank computed for its share, summed over ranks: integers and limbs below
-        2^40 each, so the float64 sum is exact and the merged limbs convert once (topic_ranking_report)."""
-        total = np.rint(self.group.all_reduce_sum([float(x) for x in words])).astype(np.int64)
-        return topic_ranking_report(total, k)
+        return self._topic_report(W, self._rows(test_data, samples_count,
+                                                f"sampled topic report of {samples_count} rows: the sample is empty"))
 
     def local_topic_ranking_report(self, weights, k: int, test_data: bool = True) -> dict:
         """Multi-label ranking quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train)
         rows in one device pass (dsgd_eval_topic_ranking): precision@j and recall@j for j = 1..k, label ranking average
         precision, coverage error and ranking loss (ml/one_vs_rest.py: topic_ranking_report).  Each rank evaluates a
         contiguous share of the rows, as local_topic_report splits them."""
-        W = self._topic_weights(weights)
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        n, R, r = e - b, self.group.world, self.group.rank
-        lo, hi = b + (n * r) // R, b + (n * (r + 1)) // R
-        words = self.ctx.eval_topic_ranking(lo, hi, W, k)[0] if hi > lo else np.zeros(topic_rank_words(k), dtype=np.int64)
-        return self._topic_ranking_words(words, k)
+        return self._topic_report(self._topic_weights(weights), self._rows(test_data), k)
 
     def local_sampled_topic_ranking_report(self, weights, k: int, samples_count: int, test_data: bool = True) -> dict:
-        """local_topic_ranking_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it;
-        rank r of R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
+        """local_topic_ranking_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it
+        once the weights are checked; rank r of R evaluates positions sample_shard(m, R, r) of the m drawn rows.  An empty
+        sample raises DsgdEmpty."""
         W = self._topic_weights(weights)
-        b, e, m, key, ids = self._draw_sample(samples_count, test_data)
-        if m <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled topic ranking report of {samples_count} rows: the sample is empty")
-        lo, hi = sample_shard(m, self.group.world, self.group.rank)
-        if hi <= lo:
-            words = np.zeros(topic_rank_words(k), dtype=np.int64)
-        elif ids is None:
-            words = self.ctx.eval_sampled_topic_ranking(b, e, key, lo, hi, W, k)[0]
-        else:
-            words = self.ctx.eval_samples_topic_ranking(ids[lo:hi], W, k)[0]
-        return self._topic_ranking_words(words, k)
+        return self._topic_report(W, self._rows(test_data, samples_count,
+                                                f"sampled topic ranking report of {samples_count} rows: the sample is empty"), k)
 
     # ---- ranking metrics (extension) -------------------------------------------------------------------------------------
     # AUC is not a sum over rows, so these are not sharded: rows are replicated on every rank (quirk Q13) and every rank
@@ -663,51 +667,36 @@ class Master:
     def local_metrics(self, weights=None, test_data: bool = False) -> dict:
         """Confusion counts, precision, recall, F1, ROC AUC and accuracy over the train (or test) rows (metrics_dict).
         weights None: the resident weights -- in `fit` the last iterate, not the average of average_from."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return metrics_dict(self.ctx.eval_metrics(b, e, weights))
+        return metrics_dict(self._rows(test_data).call(self.ctx, "eval_metrics", weights))
 
     def local_sampled_metrics(self, weights, samples_count: int, test_data: bool = False) -> dict:
         """local_metrics on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it (one draw of
         sampled_key, or the jvm_exact shuffle).  An empty sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled metrics of {samples_count} rows: the sample is empty")
-        if ids is None:
-            return metrics_dict(self.ctx.eval_sampled_metrics(b, e, key, 0, k, weights))
-        return metrics_dict(self.ctx.eval_samples_metrics(ids, weights))
+        rows = self._rows(test_data, samples_count, f"sampled metrics of {samples_count} rows: the sample is empty")
+        return metrics_dict(rows.call(self.ctx, "eval_metrics", weights))
 
     def local_curve(self, weights=None, test_data: bool = False, curve: bool = True) -> dict:
         """local_metrics plus average precision, and with `curve` the ROC and precision-recall points over the train (or test)
         rows (curve_dict).  Like local_metrics, every rank evaluates the whole range."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return curve_dict(self.ctx.eval_curve(b, e, weights, curve=curve))
+        return curve_dict(self._rows(test_data).call(self.ctx, "eval_curve", weights, curve=curve))
 
     def local_sampled_curve(self, weights, samples_count: int, test_data: bool = False, curve: bool = True) -> dict:
         """local_curve on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
         sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled curve of {samples_count} rows: the sample is empty")
-        if ids is None:
-            return curve_dict(self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=curve))
-        return curve_dict(self.ctx.eval_samples_curve(ids, weights, curve=curve))
+        rows = self._rows(test_data, samples_count, f"sampled curve of {samples_count} rows: the sample is empty")
+        return curve_dict(rows.call(self.ctx, "eval_curve", weights, curve=curve))
 
     def local_weighted_curve(self, weights=None, test_data: bool = False, curve: bool = True) -> dict:
         """local_curve with every row counted by its weight c_i = class weight x sample weight (weighted_curve_dict).  Not
         sharded either: every rank evaluates the whole range, and every word is an order-free fixed-point sum, so every
         rank gets the same bits."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        return weighted_curve_dict(self.ctx.eval_weighted_curve(b, e, weights, curve=curve), curve)
+        return weighted_curve_dict(self._rows(test_data).call(self.ctx, "eval_weighted_curve", weights, curve=curve), curve)
 
     def local_sampled_weighted_curve(self, weights, samples_count: int, test_data: bool = False, curve: bool = True) -> dict:
         """local_weighted_curve on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_curve draws it.  An
         empty sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled weighted curve of {samples_count} rows: the sample is empty")
-        if ids is None:
-            return weighted_curve_dict(self.ctx.eval_sampled_weighted_curve(b, e, key, 0, k, weights, curve=curve), curve)
-        return weighted_curve_dict(self.ctx.eval_samples_weighted_curve(ids, weights, curve=curve), curve)
+        rows = self._rows(test_data, samples_count, f"sampled weighted curve of {samples_count} rows: the sample is empty")
+        return weighted_curve_dict(rows.call(self.ctx, "eval_weighted_curve", weights, curve=curve), curve)
 
     # ---- bootstrap (extension) -------------------------------------------------------------------------------------------
     # Poisson-bootstrap intervals of the ranking metrics, accuracy and loss (dsgd_eval_*bootstrap).  Every rank holds every
@@ -715,74 +704,45 @@ class Master:
     # returns the same bits -- a replicate's bits do not depend on which rank computed it.
     # weighted=True counts every row by its weight c_i = class weight x sample weight (dsgd_eval_*weighted_bootstrap): the
     # same seven metrics by weighted_curve_dict's formulas, the estimates from the weighted curve and evaluation calls.
-    def _bootstrap_raw(self, call: str, rows: tuple, weights, n_boot: int, key: int, weighted: bool = False):
-        """(words, ap, loss_sum) -- weighted: (words, wsums, loss_sum) -- of replicates [0, n_boot) of
-        ctx.<call>(*rows, key, lo, hi, weights), gathered in rank order."""
-        if n_boot <= 0:
-            raise ValueError(f"n_boot: expected a number of replicates > 0, got {n_boot}")
-        lo, hi = bootstrap_share(int(n_boot), self.group.world, self.group.rank)
-        mine = bootstrap_pack(*getattr(self.ctx, call)(*rows, key, lo, hi, weights)) if hi > lo else np.zeros(0)
-        parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
-        return bootstrap_unpack(parts, weighted)
-
-    def _bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int], weighted: bool = False):
-        """(call, rows, estimates) of one bootstrap request: the whole train (or test) rows, or a fresh sample
-        (_draw_sample); the estimates come from the existing curve and *_sums calls over the same rows (weighted: the
-        weighted curve and weighted evaluation calls, as local_weighted_curve and local_weighted_report form them)."""
-        if weighted:
-            return self._weighted_bootstrap_case(weights, test_data, samples_count)
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        if samples_count is None:
-            call, rows = "eval_bootstrap", (b, e)
-            cw = self.ctx.eval_curve(b, e, weights, curve=False)
-            sums = self.ctx.eval_sums(b, e, weights)
-        else:
-            b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-            if k <= 0:
-                raise DsgdEmpty(ERR_EMPTY, f"sampled bootstrap of {samples_count} rows: the sample is empty")
-            if ids is None:
-                call, rows = "eval_sampled_bootstrap", (b, e, key, 0, k)
-                cw = self.ctx.eval_sampled_curve(b, e, key, 0, k, weights, curve=False)
-                sums = self.ctx.eval_sampled_sums(b, e, key, 0, k, weights)
-            else:
-                call, rows = "eval_samples_bootstrap", (ids,)
-                cw = self.ctx.eval_samples_curve(ids, weights, curve=False)
-                sums = self.ctx.eval_samples_sums(ids, weights)
+    def _estimates(self, cw, sums, weights):
+        """(estimates, penalty) of an unweighted bootstrap from the curve words and the *_sums of its rows."""
         penalty = self._penalty(sums[2], weights, True)
         words, ap = cw[0], cw[1]
         n = int(np.sum(np.asarray(words)[[0, 1, 2, 3, 4, 5]]))
         est = {k: float(v[0]) for k, v in bootstrap_values(np.concatenate([words, [n]]), [ap], [sums[0]], penalty).items()}
-        return call, rows, est, penalty
+        return est, penalty
 
-    def _weighted_bootstrap_case(self, weights, test_data: bool, samples_count: Optional[int]):
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        if samples_count is None:
-            call, rows = "eval_weighted_bootstrap", (b, e)
-            wc = self.ctx.eval_weighted_curve(b, e, weights, curve=False)
-            we = self.ctx.eval_weighted(b, e, weights)
-        else:
-            b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-            if k <= 0:
-                raise DsgdEmpty(ERR_EMPTY, f"sampled bootstrap of {samples_count} rows: the sample is empty")
-            if ids is None:
-                call, rows = "eval_sampled_weighted_bootstrap", (b, e, key, 0, k)
-                wc = self.ctx.eval_sampled_weighted_curve(b, e, key, 0, k, weights, curve=False)
-                we = self.ctx.eval_sampled_weighted(b, e, key, 0, k, weights)
-            else:
-                call, rows = "eval_samples_weighted_bootstrap", (ids,)
-                wc = self.ctx.eval_samples_weighted_curve(ids, weights, curve=False)
-                we = self.ctx.eval_samples_weighted(ids, weights)
+    def _weighted_estimates(self, wc, we, weights):
+        """(estimates, penalty) of a weighted bootstrap, as local_weighted_curve and local_weighted_report form them."""
         curve, report = weighted_curve_dict(wc, curve=False), self._weighted_report(we, weights)
         est = {"accuracy": curve["accuracy"], "loss": report["weighted_loss"], "auc": curve["auc"],
                "ap": curve["average_precision"], "precision": curve["precision"], "recall": curve["recall"],
                "f1": curve["f1"]}
-        return call, rows, est, self._penalty(we.norm_squared, weights, True)
+        return est, self._penalty(we.norm_squared, weights, True)
 
-    def _bootstrap(self, weights, test_data, samples_count, n_boot, key, level, weighted=False) -> dict:
-        call, rows, est, penalty = self._bootstrap_case(weights, test_data, samples_count, weighted)
+    # weighted -> (curve family, evaluation family, estimates, replicate family, replicate values)
+    _BOOTSTRAP = {False: ("eval_curve", "eval_sums", _estimates, "eval_bootstrap", bootstrap_values),
+                  True: ("eval_weighted_curve", "eval_weighted", _weighted_estimates, "eval_weighted_bootstrap",
+                         weighted_bootstrap_values)}
+
+    def _bootstrap_case(self, weights, rows: Rows, n_boot: int, key: Optional[int], weighted: bool):
+        """(estimates, replicates) of one bootstrap over `rows`: the estimates from the curve and evaluation calls over the
+        same rows, and every BOOTSTRAP_METRICS value of replicates [0, n_boot) with `key` (None: bootstrap_key(seed)), rank r
+        computing bootstrap_share(n_boot, W, r), gathered in rank order."""
+        weighted = bool(weighted)
+        curve_family, eval_family, estimates, family, values = self._BOOTSTRAP[weighted]
+        est, penalty = estimates(self, rows.call(self.ctx, curve_family, weights, curve=False),
+                                 rows.call(self.ctx, eval_family, weights), weights)
         key = bootstrap_key(self.seed) if key is None else int(key)
-        values = weighted_bootstrap_values if weighted else bootstrap_values
-        reps = values(*self._bootstrap_raw(call, rows, weights, n_boot, key, weighted), penalty)
+        if n_boot <= 0:
+            raise ValueError(f"n_boot: expected a number of replicates > 0, got {n_boot}")
+        lo, hi = bootstrap_share(int(n_boot), self.group.world, self.group.rank)
+        mine = bootstrap_pack(*rows.call(self.ctx, family, key, lo, hi, weights)) if hi > lo else np.zeros(0)
+        parts = [np.frombuffer(b, dtype=np.float64) for b in self.group.all_gather_bytes(mine.tobytes())]
+        return est, values(*bootstrap_unpack(parts, weighted), penalty)
+
+    def _bootstrap(self, weights, rows: Rows, n_boot, key, level, weighted) -> dict:
+        est, reps = self._bootstrap_case(weights, rows, n_boot, key, weighted)
         return {m: bootstrap_summary(est[m], reps[m], level) for m in BOOTSTRAP_METRICS}
 
     def local_bootstrap(self, weights=None, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
@@ -793,13 +753,14 @@ class Master:
         the standard error se and the raw replicates.  key None: bootstrap_key(seed).  weighted: every row counted by its
         weight c_i = class weight x sample weight -- the metrics of local_weighted_curve and the loss of
         local_weighted_report, resampled with the same multiplicities as the unweighted bootstrap of the same key."""
-        return self._bootstrap(weights, test_data, None, n_boot, key, level, weighted)
+        return self._bootstrap(weights, self._rows(test_data), n_boot, key, level, weighted)
 
     def local_sampled_bootstrap(self, weights, samples_count: int, test_data: bool = True, n_boot: int = 1000,
                                 key: Optional[int] = None, level: float = 0.95, weighted: bool = False) -> dict:
         """local_bootstrap over a fresh sample of min(samples_count, n) rows (_draw_sample).  An empty sample raises
         DsgdEmpty."""
-        return self._bootstrap(weights, test_data, samples_count, n_boot, key, level, weighted)
+        rows = self._rows(test_data, samples_count, f"sampled bootstrap of {samples_count} rows: the sample is empty")
+        return self._bootstrap(weights, rows, n_boot, key, level, weighted)
 
     def compare_bootstrap(self, weights_a, weights_b, test_data: bool = True, n_boot: int = 1000, key: Optional[int] = None,
                           level: float = 0.95, weighted: bool = False) -> dict:
@@ -809,13 +770,9 @@ class Master:
         p_better, the share of those replicates in which b is better (higher, or lower for the loss).  weighted: as in
         local_bootstrap."""
         key = bootstrap_key(self.seed) if key is None else int(key)
-        values = weighted_bootstrap_values if weighted else bootstrap_values
+        rows = self._rows(test_data)
+        (ea, ra), (eb, rb) = [self._bootstrap_case(w, rows, n_boot, key, weighted) for w in (weights_a, weights_b)]
         out = {}
-        sides = []
-        for w in (weights_a, weights_b):
-            call, rows, est, penalty = self._bootstrap_case(w, test_data, None, weighted)
-            sides.append((est, values(*self._bootstrap_raw(call, rows, w, n_boot, key, weighted), penalty)))
-        (ea, ra), (eb, rb) = sides
         for m, higher in BOOTSTRAP_METRICS.items():
             d = rb[m] - ra[m]
             s = bootstrap_summary(eb[m] - ea[m], d, level)
@@ -834,38 +791,23 @@ class Master:
         (a, b) that makes 1 / (1 + exp(a x.w + b)) a probability; "isotonic": isotonic regression, an IsotonicCalibration.
         weights None: the resident weights, as in local_metrics.  weighted: fitted with every row counted by its weight
         c_i = class weight x sample weight (dsgd_calibrate_weighted, dsgd_calibrate_isotonic_weighted)."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        if weighted:
-            if _method(method) == "isotonic":
-                return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted(b, e, weights))
-            return _weighted_calibration(self.ctx.calibrate_weighted(b, e, weights))
-        if _method(method) == "isotonic":
-            return _isotonic(self.ctx.calibrate_isotonic(b, e, weights))
-        return _calibration(self.ctx.calibrate(b, e, weights))
+        family, convert = _FITS[bool(weighted), _method(method) == "isotonic"]
+        return convert(self._rows(test_data).call(self.ctx, family, weights))
 
     def sampled_calibrate(self, weights, samples_count: int, test_data: bool = False, method: str = "sigmoid",
                           weighted: bool = False):
-        """calibrate on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it.  An empty
-        sample raises DsgdEmpty."""
-        iso = _method(method) == "isotonic"
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled calibration of {samples_count} rows: the sample is empty")
-        if weighted and iso:
-            if ids is None:
-                return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted_sampled(b, e, key, 0, k, weights))
-            return _weighted_isotonic(self.ctx.calibrate_isotonic_weighted_samples(ids, weights))
-        if weighted:
-            if ids is None:
-                return _weighted_calibration(self.ctx.calibrate_weighted_sampled(b, e, key, 0, k, weights))
-            return _weighted_calibration(self.ctx.calibrate_weighted_samples(ids, weights))
-        if ids is None:
-            if iso:
-                return _isotonic(self.ctx.calibrate_isotonic_sampled(b, e, key, 0, k, weights))
-            return _calibration(self.ctx.calibrate_sampled(b, e, key, 0, k, weights))
-        if iso:
-            return _isotonic(self.ctx.calibrate_isotonic_samples(ids, weights))
-        return _calibration(self.ctx.calibrate_samples(ids, weights))
+        """calibrate on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_metrics draws it once the method
+        is checked.  An empty sample raises DsgdEmpty."""
+        family, convert = _FITS[bool(weighted), _method(method) == "isotonic"]
+        rows = self._rows(test_data, samples_count, f"sampled calibration of {samples_count} rows: the sample is empty")
+        return convert(rows.call(self.ctx, family, weights))
+
+    def _calibration_quality(self, calibration, weights, rows: Rows, n_bins: int, weighted: bool) -> dict:
+        """local_calibration over `rows`: the quality family of the calibration's kind and of `weighted` (_QUALITY)."""
+        isotonic = isinstance(calibration, IsotonicCalibration)
+        family, convert = _QUALITY[bool(weighted), isotonic]
+        params = (calibration.x, calibration.y) if isotonic else (calibration.a, calibration.b)
+        return convert(rows.call(self.ctx, family, *params, n_bins, weights))
 
     def local_calibration(self, calibration, weights=None, test_data: bool = False, n_bins: int = 10,
                           weighted: bool = False) -> dict:
@@ -873,45 +815,14 @@ class Master:
         loss, expected and maximum calibration error and the reliability bins (calibration_dict; isotonic_calibration_dict
         for an isotonic map).  Every rank evaluates the whole range itself.  weighted: every row counted by its weight c_i
         (weighted_calibration_dict)."""
-        b, e = (self.n_train, self.n_train + self.n_test) if test_data else (0, self.n_train)
-        if isinstance(calibration, IsotonicCalibration):
-            if weighted:
-                return weighted_calibration_dict(self.ctx.eval_weighted_isotonic_calibration(b, e, calibration.x,
-                                                                                             calibration.y, n_bins, weights))
-            return isotonic_calibration_dict(self.ctx.eval_isotonic_calibration(b, e, calibration.x, calibration.y, n_bins,
-                                                                                weights))
-        if weighted:
-            return weighted_calibration_dict(self.ctx.eval_weighted_calibration(b, e, calibration.a, calibration.b, n_bins,
-                                                                                weights))
-        return calibration_dict(self.ctx.eval_calibration(b, e, calibration.a, calibration.b, n_bins, weights))
+        return self._calibration_quality(calibration, weights, self._rows(test_data), n_bins, weighted)
 
     def local_sampled_calibration(self, calibration: Calibration, weights, samples_count: int, test_data: bool = False,
                                   n_bins: int = 10, weighted: bool = False) -> dict:
         """local_calibration on a fresh sample of min(samples_count, n) rows.  An empty sample raises DsgdEmpty."""
-        b, e, k, key, ids = self._draw_sample(samples_count, test_data)
-        if k <= 0:
-            raise DsgdEmpty(ERR_EMPTY, f"sampled calibration quality of {samples_count} rows: the sample is empty")
-        if isinstance(calibration, IsotonicCalibration):
-            x, y = calibration.x, calibration.y
-            if weighted:
-                if ids is None:
-                    return weighted_calibration_dict(self.ctx.eval_sampled_weighted_isotonic_calibration(
-                        b, e, key, 0, k, x, y, n_bins, weights))
-                return weighted_calibration_dict(self.ctx.eval_samples_weighted_isotonic_calibration(ids, x, y, n_bins,
-                                                                                                     weights))
-            if ids is None:
-                return isotonic_calibration_dict(self.ctx.eval_sampled_isotonic_calibration(b, e, key, 0, k, x, y, n_bins,
-                                                                                            weights))
-            return isotonic_calibration_dict(self.ctx.eval_samples_isotonic_calibration(ids, x, y, n_bins, weights))
-        a, bb = calibration.a, calibration.b
-        if weighted:
-            if ids is None:
-                return weighted_calibration_dict(self.ctx.eval_sampled_weighted_calibration(b, e, key, 0, k, a, bb, n_bins,
-                                                                                            weights))
-            return weighted_calibration_dict(self.ctx.eval_samples_weighted_calibration(ids, a, bb, n_bins, weights))
-        if ids is None:
-            return calibration_dict(self.ctx.eval_sampled_calibration(b, e, key, 0, k, a, bb, n_bins, weights))
-        return calibration_dict(self.ctx.eval_samples_calibration(ids, a, bb, n_bins, weights))
+        rows = self._rows(test_data, samples_count,
+                          f"sampled calibration quality of {samples_count} rows: the sample is empty")
+        return self._calibration_quality(calibration, weights, rows, n_bins, weighted)
 
     def predict(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> dict:
         """Master.predict (core/Master.scala:61-75): idx -> prediction over the training rows; each worker
@@ -930,22 +841,18 @@ class Master:
 
     def distributed_accuracy(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> float:
         """Master.distributedAccuracy (core/Master.scala:77-85)."""
-        return self._distributed(weights, split_strategy, want_loss=False)[1]
+        return self._loss_accuracy(weights, self._group_rows(split_strategy), want_loss=False, grouped=True)[1]
 
     def distributed_loss(self, weights, split_strategy: Split = SplitStrategy.vanilla) -> float:
         """Master.distributedLoss (core/Master.scala:87-98)."""
-        return self._distributed(weights, split_strategy)[0]
+        return self._loss_accuracy(weights, self._group_rows(split_strategy), grouped=True)[0]
 
-    def _distributed(self, weights, split_strategy: Split, want_loss: bool = True):
-        # same numbers as predict + host-side counting, without shipping N predictions around
+    def _group_rows(self, split_strategy: Split) -> Optional[Rows]:
+        """This rank's group of split_strategy over the train rows, None when it has none: the same numbers as predict +
+        host-side counting, without shipping N predictions around."""
         groups = split_strategy(self.n_train, self.group.world)
         mine = groups[self.group.rank] if self.group.rank < len(groups) else range(0)
-        if len(mine):
-            h, c, n2, *h_neg = self._local_eval("eval", mine.start, mine.stop, weights)
-        else:
-            h, c, n2, *h_neg = (0, 0, 0.0, 0) if self.weighted else (0, 0, 0.0)
-        hs, cs, ns, *h_neg, n2 = self._combine(h, c, n2, len(mine), *h_neg)
-        return self._penalty(n2, weights, want_loss) + self._loss_sum(hs, *h_neg) / ns, cs / ns
+        return Rows(mine.start, mine.stop) if len(mine) else None
 
 
 class MasterSync(Master):

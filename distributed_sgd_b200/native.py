@@ -171,10 +171,6 @@ ABI = {
     "dsgd_async_updates": [_vp, C.POINTER(_i64)],
     "dsgd_load_topics": [_vp, _i32, _vp, _vp],
     "dsgd_select_topic": [_vp, _i32],
-    # the topic family takes T weight vectors and their count before the rows
-    "dsgd_eval_topics": [_vp, _vp, _i32, _i64, _i64, _vp],
-    "dsgd_eval_sampled_topics": [_vp, _vp, _i32, _i64, _i64, _u64, _i64, _i64, _vp],
-    "dsgd_eval_samples_topics": [_vp, _vp, _i32, _vp, _i64, _vp],
 }
 _RESTYPE = {"dsgd_last_error": C.c_char_p, "dsgd_info": C.c_char_p}
 
@@ -196,20 +192,23 @@ _ROW_FAMILIES = {
 }
 
 
-def _row_forms(family: str) -> dict:
-    """{form: entry point} of an evaluation family: dsgd_<fit>, _sampled, _samples for a fit; dsgd_eval_, eval_sampled_,
-    eval_samples_<rest> for the others."""
+def row_methods(family: str) -> dict:
+    """{form: NativeCtx method} of an evaluation family, each bound to the entry point dsgd_<method>: <fit>, <fit>_sampled
+    and <fit>_samples for a fit; eval_<rest>, eval_sampled_<rest> and eval_samples_<rest> for the others."""
     if family.startswith("calibrate"):
-        return {"range": f"dsgd_{family}", "drawn": f"dsgd_{family}_sampled", "list": f"dsgd_{family}_samples"}
+        return {"range": family, "drawn": f"{family}_sampled", "list": f"{family}_samples"}
     rest = family[len("eval_"):]
-    return {"range": f"dsgd_eval_{rest}", "drawn": f"dsgd_eval_sampled_{rest}", "list": f"dsgd_eval_samples_{rest}"}
+    return {"range": f"eval_{rest}", "drawn": f"eval_sampled_{rest}", "list": f"eval_samples_{rest}"}
 
 
-ABI.update({name: _ROW_PREFIX[form] + tail for family, tail in _ROW_FAMILIES.items()
-            for form, name in _row_forms(family).items()})
-# the topic ranking family takes T weight vectors, their count and k between (ctx, W) and the rows; then words and sums
-ABI.update({name: _ROW_PREFIX[form][:2] + [_i32, _i32] + _ROW_PREFIX[form][2:] + [_vp, _vp]
-            for form, name in _row_forms("eval_topic_ranking").items()})
+ABI.update({"dsgd_" + name: _ROW_PREFIX[form] + tail for family, tail in _ROW_FAMILIES.items()
+            for form, name in row_methods(family).items()})
+# the topic family takes T weight vectors and their count between (ctx, W) and the rows, then the words; the topic ranking
+# family takes k after the count, then words and sums
+ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32] + _ROW_PREFIX[form][2:] + [_vp]
+            for form, name in row_methods("eval_topics").items()})
+ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32, _i32] + _ROW_PREFIX[form][2:] + [_vp, _vp]
+            for form, name in row_methods("eval_topic_ranking").items()})
 ABI["dsgd_topics_topk"] = [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]
 
 

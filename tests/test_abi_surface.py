@@ -52,6 +52,17 @@ def test_ctypes_argtypes_match_the_header_prototypes():
         assert got == declared[name], name
 
 
+def test_row_methods_name_a_bound_native_ctx_method_for_every_form():
+    """Master reaches every form of an evaluation family through native.row_methods: each name is a NativeCtx method, and
+    dsgd_<name> is bound."""
+    from distributed_sgd_b200 import native
+    for family in [*native._ROW_FAMILIES, "eval_topics", "eval_topic_ranking"]:
+        methods = native.row_methods(family)
+        assert sorted(methods) == ["drawn", "list", "range"], family
+        for name in methods.values():
+            assert callable(getattr(native.NativeCtx, name, None)) and "dsgd_" + name in native.ABI, name
+
+
 def row_form_entry_points():
     """dsgd_eval and the range, drawn-sample and id-list forms of the fifteen evaluation families"""
     evals = ["counts", "sums", "class", "weighted", "metrics", "curve", "weighted_curve", "calibration",

@@ -110,7 +110,7 @@ def test_package_exports_the_models():
     assert model_name(pkg.SparseSVM(0.1)) == "svm" and model_name(pkg.SparseLogistic(0.1)) == "logistic"
 
 
-def test_master_takes_the_float_sums_for_every_model_but_the_svm():
+def test_local_loss_takes_the_float_sums_for_every_model_but_the_svm():
     """The choice between the integer *_counts and the float *_sums evaluations, made in Master.__init__."""
     import distributed_sgd_b200 as pkg
     from distributed_sgd_b200.core.master import Master
@@ -137,7 +137,7 @@ def test_master_takes_the_float_sums_for_every_model_but_the_svm():
                       (pkg.SparseModifiedHuber, "sums")):
         s = Slave()
         m = Master(0, _stub(10), _stub(4), cls(0.1), 1, slave=s, attach=False)
-        m._local_eval("eval", 0, 10)
+        m.local_loss()
         assert s.ctx.calls == [call]
 
 
