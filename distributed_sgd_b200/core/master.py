@@ -9,6 +9,7 @@ control flow over a handful of scalars per epoch (losses, accuracies, the stoppi
 """
 from __future__ import annotations
 
+import dataclasses
 from typing import Callable, List, NamedTuple, Optional, Sequence, Union
 
 import numpy as np
@@ -18,7 +19,7 @@ from ..ml.calibration import METHODS as CALIBRATION_METHODS, Calibration, Isoton
 from ..ml.class_weight import resolve_class_weight
 from ..ml.grad_state import GradState
 from ..ml.lr_schedule import check_schedule, learning_rates
-from ..ml.one_vs_rest import OneVsRest, topic_ranking_report, topic_report
+from ..ml.one_vs_rest import OneVsRest, threshold_report, topic_ranking_report, topic_report
 from ..ml.sparse_logistic import SparseLogistic
 from ..ml.sparse_margin import SparseModifiedHuber, SparseSquaredHinge
 from ..ml.sparse_svm import SparseSVM
@@ -618,12 +619,28 @@ class Master:
             raise ValueError(f"topic report: weights must be [{self.topics.n_topics}, {self.wdim}], got {W.shape}")
         return W
 
-    def _topic_report(self, W: np.ndarray, rows: Rows, k: Optional[int] = None) -> dict:
-        """The topic report (k None) or the topic ranking report at k of the T weight vectors W over `rows`.  Rank r of R
-        evaluates rows.shard(R, r), and the words are summed over ranks: integers and limbs below 2^40, so the float64 sum
-        is exact, every rank gets the same bits and merged limbs convert once (topic_ranking_report)."""
+    def _topic_thresholds(self, weights, thresholds) -> Optional[np.ndarray]:
+        """The margin thresholds of a topic report: `thresholds` when given, else an OneVsRest's own; None for neither (the
+        binary rule, every tau 0)."""
+        if thresholds is None and isinstance(weights, OneVsRest):
+            thresholds = weights.thresholds
+        if thresholds is None:
+            return None
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64).reshape(-1)
+        if thr.size != self.topics.n_topics or np.isnan(thr).any():
+            raise ValueError(f"topic report: expected {self.topics.n_topics} thresholds, none NaN, got {thr.size}")
+        return thr
+
+    def _topic_report(self, W: np.ndarray, rows: Rows, k: Optional[int] = None, thr: Optional[np.ndarray] = None) -> dict:
+        """The topic report (k None; at the margin thresholds thr when given) or the topic ranking report at k of the T
+        weight vectors W over `rows`.  Rank r of R evaluates rows.shard(R, r), and the words are summed over ranks: integers
+        and limbs below 2^40, so the float64 sum is exact, every rank gets the same bits and merged limbs convert once
+        (topic_ranking_report)."""
         share = rows.shard(self.group.world, self.group.rank)
-        if k is None:
+        if k is None and thr is not None:
+            words = (np.zeros(topic_words(len(W)), np.int64) if share is None
+                     else share.call(self.ctx, "eval_thresholded_topics", W, thr))
+        elif k is None:
             words = np.zeros(topic_words(len(W)), np.int64) if share is None else share.call(self.ctx, "eval_topics", W)
         else:
             words = (np.zeros(topic_rank_words(k), np.int64) if share is None
@@ -631,19 +648,49 @@ class Master:
         total = np.rint(self.group.all_reduce_sum([float(x) for x in words])).astype(np.int64)
         return topic_report(total, self.topics.names) if k is None else topic_ranking_report(total, k)
 
-    def local_topic_report(self, weights, test_data: bool = True) -> dict:
+    def local_topic_report(self, weights, test_data: bool = True, thresholds=None) -> dict:
         """Multi-label quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train) rows, all
         topics in one device pass (dsgd_eval_topics): per topic the counts, precision, recall and F1; micro precision,
         recall and F1, macro F1, subset accuracy, Hamming loss and top-1 accuracy (ml/one_vs_rest.py: topic_report).  Each
-        rank evaluates a contiguous share of the rows, as local_loss splits them."""
-        return self._topic_report(self._topic_weights(weights), self._rows(test_data))
+        rank evaluates a contiguous share of the rows, as local_loss splits them.  With margin thresholds (`thresholds`, or
+        an OneVsRest's own) topic t is predicted present below tau_t (dsgd_eval_thresholded_topics)."""
+        W = self._topic_weights(weights)
+        return self._topic_report(W, self._rows(test_data), thr=self._topic_thresholds(weights, thresholds))
 
-    def local_sampled_topic_report(self, weights, samples_count: int, test_data: bool = True) -> dict:
+    def local_sampled_topic_report(self, weights, samples_count: int, test_data: bool = True, thresholds=None) -> dict:
         """local_topic_report on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it once the
         weights are checked; rank r of R evaluates positions sample_shard(k, R, r).  An empty sample raises DsgdEmpty."""
         W = self._topic_weights(weights)
+        thr = self._topic_thresholds(weights, thresholds)
         return self._topic_report(W, self._rows(test_data, samples_count,
-                                                f"sampled topic report of {samples_count} rows: the sample is empty"))
+                                                f"sampled topic report of {samples_count} rows: the sample is empty"),
+                                  thr=thr)
+
+    def _tune_topic_thresholds(self, weights, W: np.ndarray, rows: Rows, fbr: float):
+        """(OneVsRest with the tuned thresholds, threshold_report) over `rows`.  Not sharded: the rows are replicated on
+        every rank, and every rank tunes over the whole request and gets the same bits."""
+        thr, words = rows.call(self.ctx, "tune_topic_thresholds", W, float(fbr))
+        if isinstance(weights, OneVsRest):
+            model = dataclasses.replace(weights, thresholds=thr)
+        else:
+            model = OneVsRest(W.copy(), self.topics.names, [], thr)
+        return model, threshold_report(words, thr, self.topics.names)
+
+    def tune_topic_thresholds(self, weights, test_data: bool = False, fbr: float = 0.0):
+        """Each topic's F1-optimal margin threshold (SCut with the fbr fallback, dsgd_tune_topic_thresholds) for one-vs-rest
+        weights (an OneVsRest or a [T, wdim] array) over the train (or test) rows: (an OneVsRest with those thresholds,
+        its threshold_report).  Thresholds tuned on the rows the model was fitted on are optimistic: they fit the training
+        margins, which separate better than new rows' do.  To tune on a list of held-out rows, call
+        NativeCtx.tune_topic_thresholds_samples and put the thresholds into the OneVsRest."""
+        W = self._topic_weights(weights)
+        return self._tune_topic_thresholds(weights, W, self._rows(test_data), fbr)
+
+    def sampled_tune_topic_thresholds(self, weights, samples_count: int, test_data: bool = False, fbr: float = 0.0):
+        """tune_topic_thresholds on a fresh sample of min(samples_count, n) rows, drawn as local_sampled_loss draws it once
+        the weights are checked.  An empty sample raises DsgdEmpty."""
+        W = self._topic_weights(weights)
+        return self._tune_topic_thresholds(weights, W, self._rows(
+            test_data, samples_count, f"sampled threshold tuning of {samples_count} rows: the sample is empty"), fbr)
 
     def local_topic_ranking_report(self, weights, k: int, test_data: bool = True) -> dict:
         """Multi-label ranking quality of one-vs-rest weights (an OneVsRest or a [T, wdim] array) over the test (or train)

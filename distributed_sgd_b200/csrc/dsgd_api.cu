@@ -32,6 +32,7 @@
 
 #include <cub/device/device_radix_sort.cuh>  // header-only: its sort kernels are compiled into this library, for sm_90a
 #include <cub/device/device_merge.cuh>       // the curve pass's merge and scan, likewise
+#include <cub/device/device_segmented_radix_sort.cuh>   // the threshold tuning's per-topic sort, likewise
 #include <cub/device/device_scan.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -141,6 +142,12 @@ struct dsgd_ctx {
   dev_buf<unsigned long long> t_rank;
   dev_buf<int32_t> t_top_ids;
   dev_buf<double> t_top_m;
+  // a threshold tuning (dsgd_tune_topic_thresholds*): a group's [G][n] margin keys and has-topic bytes and their sort
+  // alternates, the T thresholds and the 8 T words; a thresholded evaluation (dsgd_eval*_thresholded_topics): the T thresholds
+  dev_buf<unsigned long long> u_keys, u_alt;
+  dev_buf<uint8_t> u_has, u_hasalt;
+  dev_buf<double> u_thr;
+  dev_buf<long long> u_words;
 
   // state (fp64, L2 resident) -- g has dim + 2 slots (hinge sum and batch size ride in the allreduce)
   dev_buf<double> w, g, d, w_req;
@@ -1651,9 +1658,10 @@ static int topic_weights_in(dsgd_ctx *ctx, const double *W, int32_t n_topics) {
   return DSGD_OK;
 }
 
-// dsgd_eval*_topics: the DSGD_TOPIC_WORDS(T) words into out.  Every refusal comes before anything is launched.
-static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, const row_request &req, const char *fn,
-                          int64_t *out) {
+// dsgd_eval*_topics (thresholded false) and dsgd_eval*_thresholded_topics (thresholded: the caller's T thresholds thr): the
+// DSGD_TOPIC_WORDS(T) words into out.  Every refusal comes before anything is launched.
+static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, bool thresholded, const double *thr,
+                          const row_request &req, const char *fn, int64_t *out) {
   if (!ctx) return DSGD_ERR_INVALID;
   NEED(out, DSGD_ERR_INVALID, "%s: out is NULL", fn);
   NEED(W, DSGD_ERR_INVALID, "%s: W is NULL (the call scores T weight vectors of the caller's)", fn);
@@ -1661,17 +1669,30 @@ static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, cons
   NEED(ctx->n_topics > 0, DSGD_ERR_STATE, "%s: no topics loaded", fn);
   NEED(n_topics == ctx->n_topics, DSGD_ERR_INVALID, "%s: %d weight vectors for %d loaded topics", fn, n_topics,
        ctx->n_topics);
+  if (thresholded) {
+    NEED(thr, DSGD_ERR_INVALID, "%s: thresholds is NULL", fn);
+    for (int32_t t = 0; t < n_topics; ++t)
+      NEED(!std::isnan(thr[t]), DSGD_ERR_INVALID, "%s: the threshold of topic %d is NaN", fn, t);
+  }
   row_set rows;
   int rc = ids_capped(ctx, req, fn);
   if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
   const int64_t T = n_topics, words = DSGD_TOPIC_WORDS(T);
-  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->t_cnt.grow(ctx, words, 1024))) return rc;
+  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->t_cnt.grow(ctx, words, 1024)) ||
+      (thresholded && (rc = ctx->u_thr.grow(ctx, T, 1024))))
+    return rc;
   CU(cudaMemsetAsync(ctx->t_cnt, 0, sizeof(unsigned long long) * (size_t)words, ctx->stream));
+  if (thresholded) CU(cudaMemcpyAsync(ctx->u_thr, thr, sizeof(double) * (size_t)T, cudaMemcpyHostToDevice, ctx->stream));
   const int grid = (int)std::min<int64_t>(cdiv(rows.n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
   const size_t smem = sizeof(unsigned) * (size_t)(T * kTopicWords);
   with_icpt(ctx, [&](auto ic) {
-    k_topic_eval<ic><<<grid, 256, smem, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids,
-                                                       rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim, ctx->t_cnt);
+    if (thresholded)
+      k_topic_eval<ic, true><<<grid, 256, smem, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids,
+                                                               rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim,
+                                                               ctx->t_cnt, ctx->u_thr);
+    else
+      k_topic_eval<ic><<<grid, 256, smem, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids,
+                                                         rows.row_begin, rows.n, ctx->t_w, n_topics, ctx->dim, ctx->t_cnt);
   });
   LAUNCHED();
   CU(cudaGetLastError());
@@ -1682,17 +1703,118 @@ static int topics_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, cons
 
 extern "C" int dsgd_eval_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end,
                                 int64_t *out) {
-  return topics_request(ctx, W, n_topics, range_rows(row_begin, row_end), __func__, out);
+  return topics_request(ctx, W, n_topics, false, nullptr, range_rows(row_begin, row_end), __func__, out);
 }
 
 extern "C" int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, int64_t row_begin, int64_t row_end,
                                         uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *out) {
-  return topics_request(ctx, W, n_topics, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__, out);
+  return topics_request(ctx, W, n_topics, false, nullptr, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__,
+                        out);
 }
 
 extern "C" int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
                                         int64_t *out) {
-  return topics_request(ctx, W, n_topics, listed_rows(samples, n), __func__, out);
+  return topics_request(ctx, W, n_topics, false, nullptr, listed_rows(samples, n), __func__, out);
+}
+
+extern "C" int dsgd_eval_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const double *thresholds,
+                                            int64_t row_begin, int64_t row_end, int64_t *out) {
+  return topics_request(ctx, W, n_topics, true, thresholds, range_rows(row_begin, row_end), __func__, out);
+}
+
+extern "C" int dsgd_eval_sampled_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics,
+                                                    const double *thresholds, int64_t row_begin, int64_t row_end,
+                                                    uint64_t key, int64_t pos_begin, int64_t pos_end, int64_t *out) {
+  return topics_request(ctx, W, n_topics, true, thresholds, drawn_rows(row_begin, row_end, key, pos_begin, pos_end),
+                        __func__, out);
+}
+
+extern "C" int dsgd_eval_samples_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics,
+                                                    const double *thresholds, const int32_t *samples, int64_t n,
+                                                    int64_t *out) {
+  return topics_request(ctx, W, n_topics, true, thresholds, listed_rows(samples, n), __func__, out);
+}
+
+// ---- topic threshold tuning (dsgd_topics.cuh: k_topic_keys, k_topic_tune; DESIGN.md §4.23) -------------------------------
+
+static_assert(kTopicWords == 8 && kTuCand == 7, "DSGD_TOPIC_TUNE_WORDS layout");
+
+constexpr int64_t kTuneKeys = 1ll << 27;   // keys per group: G = max(1, min(T, kTuneKeys / n)) topics of n positions
+
+// the start of sorted segment s: segments of n keys each
+struct tune_segment {
+  int64_t n;
+  __host__ __device__ int operator()(int s) const { return (int)(s * n); }
+};
+
+// dsgd_tune_topic_thresholds*: the T thresholds into thr_out and the DSGD_TOPIC_TUNE_WORDS(T) words into words_out, the
+// topics scored, sorted and scanned in groups of G.  Every refusal comes before anything is launched or grown.
+static int tune_request(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr, const row_request &req,
+                        const char *fn, double *thr_out, int64_t *words_out) {
+  if (!ctx) return DSGD_ERR_INVALID;
+  NEED(thr_out && words_out, DSGD_ERR_INVALID, "%s: an output is NULL", fn);
+  NEED(W, DSGD_ERR_INVALID, "%s: W is NULL (the call tunes T weight vectors of the caller's)", fn);
+  NEED(!(ctx->flags & DSGD_FLAG_ASYNC), DSGD_ERR_STATE, "%s: ctx is in async mode (topics belong to the sync paths)", fn);
+  NEED(ctx->n_topics > 0, DSGD_ERR_STATE, "%s: no topics loaded", fn);
+  NEED(n_topics == ctx->n_topics, DSGD_ERR_INVALID, "%s: %d weight vectors for %d loaded topics", fn, n_topics,
+       ctx->n_topics);
+  NEED(fbr >= 0.0 && fbr <= 1.0, DSGD_ERR_INVALID, "%s: fbr = %g; 0 .. 1", fn, fbr);
+  row_set rows;
+  int rc = ids_capped(ctx, req, fn);
+  if (rc || (rc = resolve_rows(ctx, req, fn, &rows))) return rc;
+  const int64_t n = rows.n, T = n_topics, G = std::max<int64_t>(1, std::min<int64_t>(T, kTuneKeys / n));
+  if ((rc = topic_weights_in(ctx, W, n_topics)) || (rc = ctx->u_keys.grow(ctx, G * n, 1024)) ||
+      (rc = ctx->u_alt.grow(ctx, G * n, 1024)) || (rc = ctx->u_has.grow(ctx, G * n, 1024)) ||
+      (rc = ctx->u_hasalt.grow(ctx, G * n, 1024)) || (rc = ctx->u_thr.grow(ctx, T, 1024)) ||
+      (rc = ctx->u_words.grow(ctx, 8 * T, 1024)))
+    return rc;
+  const int grid = (int)std::min<int64_t>(cdiv(n, 256), (int64_t)ctx->sm_count * 8);   // >= 32 rows per warp
+  const auto seg = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), tune_segment{n});
+  for (int64_t t0 = 0; t0 < T; t0 += G) {
+    const int64_t g = std::min(G, T - t0);
+    with_icpt(ctx, [&](auto ic) {
+      k_topic_keys<ic><<<grid, 256, 0, ctx->stream>>>(ctx->rp16, ctx->pairs, ctx->t_ptr, ctx->t_ids, rows.ids,
+                                                      rows.row_begin, n, ctx->t_w, (int32_t)t0, (int32_t)g, ctx->dim,
+                                                      ctx->u_keys, ctx->u_has);
+    });
+    LAUNCHED();
+    CU(cudaGetLastError());
+    cub::DoubleBuffer<unsigned long long> kb(ctx->u_keys.p, ctx->u_alt.p);
+    cub::DoubleBuffer<uint8_t> hb(ctx->u_has.p, ctx->u_hasalt.p);
+    size_t tmp = 0;
+    CU(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tmp, kb, hb, (int)(g * n), (int)g, seg, seg + 1, 0, 64,
+                                                ctx->stream));
+    if ((rc = ctx->m_tmp.grow(ctx, (int64_t)tmp, 1 << 16))) return rc;
+    CU(cub::DeviceSegmentedRadixSort::SortPairs(ctx->m_tmp.p, tmp, kb, hb, (int)(g * n), (int)g, seg, seg + 1, 0, 64,
+                                                ctx->stream));
+    LAUNCHED();
+    k_topic_tune<<<(int)g, kTuneThreads, 0, ctx->stream>>>(kb.Current(), hb.Current(), n, (int32_t)t0, fbr, ctx->u_thr,
+                                                          ctx->u_words);
+    LAUNCHED();
+    CU(cudaGetLastError());
+  }
+  CU(cudaMemcpyAsync(thr_out, ctx->u_thr, sizeof(double) * (size_t)T, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaMemcpyAsync(words_out, ctx->u_words, sizeof(int64_t) * (size_t)(8 * T), cudaMemcpyDeviceToHost, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return DSGD_OK;
+}
+
+extern "C" int dsgd_tune_topic_thresholds(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr, int64_t row_begin,
+                                          int64_t row_end, double *thresholds_out, int64_t *words_out) {
+  return tune_request(ctx, W, n_topics, fbr, range_rows(row_begin, row_end), __func__, thresholds_out, words_out);
+}
+
+extern "C" int dsgd_tune_topic_thresholds_sampled(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr,
+                                                  int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin,
+                                                  int64_t pos_end, double *thresholds_out, int64_t *words_out) {
+  return tune_request(ctx, W, n_topics, fbr, drawn_rows(row_begin, row_end, key, pos_begin, pos_end), __func__,
+                      thresholds_out, words_out);
+}
+
+extern "C" int dsgd_tune_topic_thresholds_samples(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr,
+                                                  const int32_t *samples, int64_t n, double *thresholds_out,
+                                                  int64_t *words_out) {
+  return tune_request(ctx, W, n_topics, fbr, listed_rows(samples, n), __func__, thresholds_out, words_out);
 }
 
 // ---- topic ranking (dsgd_topics.cuh: k_topic_rank; DESIGN.md §4.22) ----------------------------------------------------

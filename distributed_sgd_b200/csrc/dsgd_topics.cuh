@@ -7,11 +7,16 @@
 //   * k_topic_eval scores every row against all T weight vectors in one pass and counts, per topic, the eight words of
 //     dsgd_eval_metrics (U2 left 0), then the row words that need every topic of a row at once.
 //   * k_topic_rank ranks every row's topics by the same scores: the top k, or the multi-label ranking words and sums.
+//   * k_topic_keys, a segmented sort and k_topic_tune place each topic's F1-optimal threshold (§4.23), which k_topic_eval's
+//     thresholded form then applies.
 // Every word is an integer sum (the ranking's fractions exact fixed-point sums), so the result does not depend on the grid,
 // the row order or the work split.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
 
 #include "dsgd_fixed.cuh"
 #include "dsgd_kernels.cuh"
@@ -77,6 +82,10 @@ __global__ void __launch_bounds__(256) k_topic_select(const int64_t *__restrict_
   yabs[r] = copysignf(fabsf(yabs[r]), y < 0 ? -1.0f : 1.0f);
 }
 
+// The thresholded rule of dsgd_eval*_thresholded_topics: present (+1) below tau, absent (-1) above it, none (0) at tau or
+// for a NaN margin.  At tau = +-0 it is pred_of.
+__device__ __forceinline__ int pred_at(double m, double tau) { return m < tau ? 1 : (m > tau ? -1 : 0); }
+
 // ---------------------------------------------------------------------------------------------------
 // k_topic_eval: rows samples[0..n) (samples == nullptr: rows [row_begin, row_begin + n)) against the T weight vectors
 // W[t * wdim, t * wdim + wdim) (on an intercept ctx the intercept is the last entry).
@@ -84,16 +93,19 @@ __global__ void __launch_bounds__(256) k_topic_select(const int64_t *__restrict_
 //   * Of each row it loads chunk 0 of the row fold (the first kFoldPairs pairs, 4 per lane) into registers once, then folds
 //     it T times with topic_score, so score_t has the bits dsgd_margins returns for W_t (and k_metrics_score ranks for it).
 //   * y_t comes from the row's ascending topic list, walked alongside t.
+//   * p_t is pred_of(score_t); kThr: pred_at(score_t, thr[t]) (dsgd_eval*_thresholded_topics).  The top-1 word ranks the
+//     raw scores either way.
 //   * Per-topic counts in shared memory (u32, one atomic per row and topic by lane 0), flushed once per CTA with u64
 //     atomics into cnt[8 t + k].  Row words in lane 0's registers, flushed once per warp into cnt[8 T + k].
 // Dynamic shared memory: 8 T u32 words.
 // ---------------------------------------------------------------------------------------------------
-template <bool kIcpt>
+template <bool kIcpt, bool kThr = false>
 __global__ void __launch_bounds__(256) k_topic_eval(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
                                                     const int64_t *__restrict__ tptr, const int32_t *__restrict__ tids,
                                                     const int32_t *__restrict__ samples, int64_t row_begin, int64_t n,
                                                     const double *__restrict__ W, int32_t T, int32_t dim,
-                                                    unsigned long long *__restrict__ cnt) {
+                                                    unsigned long long *__restrict__ cnt,
+                                                    const double *__restrict__ thr = nullptr) {
   extern __shared__ unsigned s_cnt[];   // [T][kTopicWords]
   for (int k = threadIdx.x; k < T * kTopicWords; k += blockDim.x) s_cnt[k] = 0u;
   __syncthreads();
@@ -126,7 +138,9 @@ __global__ void __launch_bounds__(256) k_topic_eval(const uint32_t *__restrict__
         const double s = topic_score<kIcpt>(pairs, pre, b, e, lane, W + (int64_t)t * wdim, dim);
         const bool has = tk < te && tids[tk] == t;
         tk += has;
-        const int p = pred_of(s);
+        int p;
+        if constexpr (kThr) p = pred_at(s, __ldg(&thr[t]));
+        else p = pred_of(s);
         exact = exact && p == (has ? 1 : -1);
         const bool nan = isnan(s);
         if (!nan && (best < 0 || s < best_dot)) { best = t; best_dot = s; best_has = has; }
@@ -334,6 +348,187 @@ __global__ void __launch_bounds__(32 * kRankWarps) k_topic_rank(const uint32_t *
     if (lane < 2) acc_flush_local(sums + lane * kLossAccWords, lim_ab, ovf_ab);
     if (lane < k) acc_flush_local(sums + (2 + lane) * kLossAccWords, lim_c, ovf_c);
   }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Tuning each topic's threshold (dsgd_tune_topic_thresholds*; DESIGN.md §4.23).  The topics go in groups of G; a group's
+// workspace is a [G][n] array of margin keys and a [G][n] array of has-topic bytes, n the request's positions.
+//   1. k_topic_keys scores every position against the group's weight vectors with topic_score (the bits of dsgd_margins)
+//      and writes score_key(m) (kKeyNaN for a NaN margin: it sorts last) and "row has topic t" at [t - t0][i].
+//   2. A segmented radix sort orders each topic's keys, the bytes with them.
+//   3. k_topic_tune scans one topic's sorted segment per CTA and writes its threshold and its DSGD_TOPIC_TUNE_WORDS.
+// ---------------------------------------------------------------------------------------------------
+constexpr unsigned long long kKeyNaN = ~0ull;   // the key of a NaN margin, above score_key of every other margin
+constexpr int kTuneThreads = 256;               // threads of k_topic_tune
+constexpr int kTuneItems = 8;                   // consecutive positions per thread and tile of k_topic_tune
+enum TopicTuneWord : int {
+  kTuRows = 0, kTuPos = 1, kTuNan = 2, kTuDistinct = 3, kTuTp = 4, kTuPred = 5, kTuStatus = 6, kTuCand = 7
+};
+enum TopicTuneStatus : int { kTuned = 0, kNoPositive = 1, kBelowFbr = 2, kNoMargin = 3 };
+
+// k_topic_keys: positions [0, n) of the rows (samples, or rows [row_begin, row_begin + n)) against topics [t0, t0 + G),
+// walked as k_topic_eval walks them; lane 0 writes position i's key and byte of topic t0 + g at g n + i.
+template <bool kIcpt>
+__global__ void __launch_bounds__(256) k_topic_keys(const uint32_t *__restrict__ rp16, const uint2 *__restrict__ pairs,
+                                                    const int64_t *__restrict__ tptr, const int32_t *__restrict__ tids,
+                                                    const int32_t *__restrict__ samples, int64_t row_begin, int64_t n,
+                                                    const double *__restrict__ W, int32_t t0, int32_t G, int32_t dim,
+                                                    unsigned long long *__restrict__ keys, uint8_t *__restrict__ has) {
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int64_t wdim = (int64_t)dim + (kIcpt ? 1 : 0);
+  const int64_t warp0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t g0 = warp0 * 32; g0 < n; g0 += nwarps * 32) {
+    const int64_t i_own = g0 + lane;
+    const int64_t r_own = i_own < n ? (samples ? (int64_t)samples[i_own] : row_begin + i_own) : 0;
+    const int m = (int)(n - g0 < 32 ? n - g0 : 32);
+    for (int j = 0; j < m; ++j) {
+      const int64_t r = __shfl_sync(full, r_own, j), i = g0 + j;
+      const int64_t b = (int64_t)rp16[r] * 2, e = (int64_t)rp16[r + 1] * 2;
+      uint2 pre[4];   // chunk 0: pair b + lane + 32 u, a zero pair past the window
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int64_t k = b + lane + 32 * u;
+        pre[u] = k < e ? __ldg(&pairs[k]) : make_uint2(0u, 0u);
+      }
+      const int64_t te = tptr[r + 1];
+      int64_t tk = topic_lower_bound(tids, tptr[r], te, t0);   // the row's next topic id at or after t
+      for (int32_t g = 0; g < G; ++g) {
+        const int32_t t = t0 + g;
+        const double s = topic_score<kIcpt>(pairs, pre, b, e, lane, W + (int64_t)t * wdim, dim);
+        const bool y = tk < te && tids[tk] == t;
+        tk += y;
+        if (lane == 0) {
+          keys[(int64_t)g * n + i] = isnan(s) ? kKeyNaN : score_key(s);
+          has[(int64_t)g * n + i] = y;
+        }
+      }
+    }
+  }
+}
+
+// One candidate of a topic: tp and pp = rows with m <= c_j (one past c_j's last position in the sorted segment); j < 0: none
+struct tune_cand {
+  unsigned long long tp, pp;
+  long long j;
+};
+
+// The better of two candidates: the higher F1 = 2 tp / (P + pp), compared exactly by cross-multiplication in 128 bits, and
+// of equal F1 the lower j (the one predicting fewer rows).  A total order on the candidates, so the block's reduction
+// picks the same one in any order.
+__device__ __forceinline__ tune_cand tune_pick(const tune_cand &a, const tune_cand &b, unsigned long long P) {
+  if (b.j < 0) return a;
+  if (a.j < 0) return b;
+  const unsigned __int128 fa = (unsigned __int128)a.tp * (P + b.pp), fb = (unsigned __int128)b.tp * (P + a.pp);
+  if (fa != fb) return fa > fb ? a : b;
+  return a.j < b.j ? a : b;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// k_topic_tune: CTA s scans the sorted segment s (keys and has-topic bytes at s n .. s n + n) of topic t = t0 + s.
+//   * P: a block sum of the bytes (NaN positions included).
+//   * Tiles of kTuneThreads x kTuneItems positions, each thread kTuneItems consecutive ones.  A position ends a group when
+//     its key is not kKeyNaN and the next key (kKeyNaN past the end) differs.  One block scan of (ends << 32 | bytes) gives
+//     at each group end j = ends - 1 and tp_j; pp_j is the position + 1.
+//   * Each thread keeps its best candidate (tune_pick), and remembers candidate 0 and the group end just before the key
+//     of +inf; a block reduction picks the best.
+//   * Thread 0 applies the status rules, places tau (the midpoint rule, +inf for the last candidate) and writes thr[t] and
+//     words[8 t .. 8 t + 8).  The counts at tau = 0 (statuses 1 and 3) are the lower bound of score_key(0.0), P = 0 or no
+//     non-NaN margin making tp 0; a last candidate at +inf counts at tau = +inf the rows below it.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kTuneThreads) k_topic_tune(const unsigned long long *__restrict__ keys,
+                                                             const uint8_t *__restrict__ has, int64_t n, int32_t t0,
+                                                             double fbr, double *__restrict__ thr,
+                                                             long long *__restrict__ words) {
+  using Scan = cub::BlockScan<unsigned long long, kTuneThreads>;
+  using Sum = cub::BlockReduce<unsigned long long, kTuneThreads>;
+  using Best = cub::BlockReduce<tune_cand, kTuneThreads>;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Sum::TempStorage sum;
+    typename Best::TempStorage best;
+  } tmp;
+  __shared__ unsigned long long s_P, s_c0[2], s_inf[2];   // P; candidate 0's (tp, pp); the counts below +inf
+  const unsigned long long *k = keys + (int64_t)blockIdx.x * n;
+  const uint8_t *h = has + (int64_t)blockIdx.x * n;
+  const unsigned long long kInf = score_key(__longlong_as_double(0x7ff0000000000000ll));
+  const unsigned long long lo32 = 0xffffffffull;
+  unsigned long long p = 0;
+  for (int64_t i = threadIdx.x; i < n; i += kTuneThreads) p += h[i];
+  p = Sum(tmp.sum).Sum(p);
+  if (threadIdx.x == 0) {
+    s_P = p;
+    s_c0[0] = s_c0[1] = s_inf[0] = s_inf[1] = 0;
+  }
+  __syncthreads();
+  const unsigned long long P = s_P;
+  tune_cand best{0, 0, -1};
+  unsigned long long carry = 0;   // (ends << 32) | positives before the tile
+  for (int64_t base = 0; base < n; base += (int64_t)kTuneThreads * kTuneItems) {
+    const int64_t i0 = base + (int64_t)threadIdx.x * kTuneItems;
+    unsigned long long kk[kTuneItems + 1], add[kTuneItems], tot = 0;
+#pragma unroll
+    for (int u = 0; u <= kTuneItems; ++u) kk[u] = i0 + u < n ? k[i0 + u] : kKeyNaN;
+#pragma unroll
+    for (int u = 0; u < kTuneItems; ++u) {
+      const bool end = kk[u] != kKeyNaN && kk[u + 1] != kk[u];
+      add[u] = (i0 + u < n ? (unsigned long long)h[i0 + u] : 0ull) + ((unsigned long long)end << 32);
+      tot += add[u];
+    }
+    unsigned long long excl, agg;
+    Scan(tmp.scan).ExclusiveSum(tot, excl, agg);
+    __syncthreads();   // tmp is the next tile's
+    unsigned long long run = carry + excl;
+#pragma unroll
+    for (int u = 0; u < kTuneItems; ++u) {
+      run += add[u];
+      if (add[u] >> 32) {
+        const tune_cand c{run & lo32, (unsigned long long)(i0 + u + 1), (long long)(run >> 32) - 1};
+        best = tune_pick(best, c, P);
+        if (c.j == 0) { s_c0[0] = c.tp; s_c0[1] = c.pp; }
+        if (kk[u + 1] == kInf) { s_inf[0] = c.tp; s_inf[1] = c.pp; }
+      }
+    }
+    carry += agg;
+  }
+  best = Best(tmp.best).Reduce(best, [P](const tune_cand &a, const tune_cand &b) { return tune_pick(a, b, P); });
+  __syncthreads();   // s_c0 and s_inf are written
+  if (threadIdx.x != 0) return;
+  const long long D = (long long)(carry >> 32);
+  long long status, j = -1;
+  unsigned long long tp, pp;
+  double tau = 0.0;
+  if (D == 0 || P == 0) {
+    status = D == 0 ? kNoMargin : kNoPositive;
+    tp = 0;
+    pp = (unsigned long long)key_lower_bound(k, n, score_key(0.0));
+  } else {
+    status = (double)(2 * best.tp) / (double)(P + best.pp) < fbr ? kBelowFbr : kTuned;
+    j = status == kBelowFbr ? 0 : best.j;
+    tp = status == kBelowFbr ? s_c0[0] : best.tp;
+    pp = status == kBelowFbr ? s_c0[1] : best.pp;
+    const unsigned long long kc = k[pp - 1];   // c_j's key
+    if (j == D - 1) {
+      tau = __longlong_as_double(0x7ff0000000000000ll);
+      if (kc == kInf) { tp = s_inf[0]; pp = s_inf[1]; }   // the rows at +inf get no prediction at tau = +inf
+    } else {
+      const double c = key_score(kc), c1 = key_score(k[pp]);
+      const double mid = c / 2.0 + c1 / 2.0;
+      tau = c < mid && mid <= c1 ? mid : c1;
+    }
+  }
+  const int32_t t = t0 + (int32_t)blockIdx.x;
+  long long *w = words + (int64_t)t * 8;
+  w[kTuRows] = n;
+  w[kTuPos] = (long long)P;
+  w[kTuNan] = n - key_lower_bound(k, n, kKeyNaN);
+  w[kTuDistinct] = D;
+  w[kTuTp] = (long long)tp;
+  w[kTuPred] = (long long)pp;
+  w[kTuStatus] = status;
+  w[kTuCand] = j;
+  thr[t] = tau;
 }
 
 }  // namespace dsgd

@@ -235,6 +235,25 @@ object DsgdNative {
   @native def evalSampledTopics(ctx: Long, W: Array[Double], nTopics: Int, rowBegin: Long, rowEnd: Long, key: Long,
                                 posBegin: Long, posEnd: Long, out: Array[Long]): Int
   @native def evalSamplesTopics(ctx: Long, W: Array[Double], nTopics: Int, samples: Array[Int], out: Array[Long]): Int
+  // topic thresholds (sync mode): W as evalTopics.  evalThresholdedTopics: evalTopics' words with topic t predicted present
+  // below thresholds(t) (thresholds.length >= nTopics, no NaN), absent above it, neither at it.  tuneTopicThresholds: each
+  // topic's F1-optimal threshold over the rows into thresholds (length >= nTopics) and 8 words per topic into words (length
+  // >= 8 * nTopics: rows, positives, NaN margins, distinct margins, tp and rows predicted at the threshold, status,
+  // candidate); 0 <= fbr <= 1
+  @native def evalThresholdedTopics(ctx: Long, W: Array[Double], nTopics: Int, thresholds: Array[Double], rowBegin: Long,
+                                    rowEnd: Long, out: Array[Long]): Int
+  @native def evalSampledThresholdedTopics(ctx: Long, W: Array[Double], nTopics: Int, thresholds: Array[Double],
+                                           rowBegin: Long, rowEnd: Long, key: Long, posBegin: Long, posEnd: Long,
+                                           out: Array[Long]): Int
+  @native def evalSamplesThresholdedTopics(ctx: Long, W: Array[Double], nTopics: Int, thresholds: Array[Double],
+                                           samples: Array[Int], out: Array[Long]): Int
+  @native def tuneTopicThresholds(ctx: Long, W: Array[Double], nTopics: Int, fbr: Double, rowBegin: Long, rowEnd: Long,
+                                  thresholds: Array[Double], words: Array[Long]): Int
+  @native def tuneTopicThresholdsSampled(ctx: Long, W: Array[Double], nTopics: Int, fbr: Double, rowBegin: Long,
+                                         rowEnd: Long, key: Long, posBegin: Long, posEnd: Long,
+                                         thresholds: Array[Double], words: Array[Long]): Int
+  @native def tuneTopicThresholdsSamples(ctx: Long, W: Array[Double], nTopics: Int, fbr: Double, samples: Array[Int],
+                                         thresholds: Array[Double], words: Array[Long]): Int
   // topic ranking (sync mode): W as evalTopics, 1 <= k <= min(nTopics, 32).  evalTopicRanking: words.length >= 8 + k +
   // 7 * (2 + k) (rows, ranked rows, rows with a NaN score, rows without a topic, ranked rows with every topic, coverage,
   // mis-ordered pairs, 0, hits in the top j for j = 1..k, then the limbs of A, B, C_1..C_k), sums.length >= 2 + k (their

@@ -912,6 +912,73 @@ FN(evalSampledTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint n
 FN(evalSamplesTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jintArray samples, jlongArray out) {
   return req_topics(env, h, W, nTopics, list_rows(samples), out);
 }
+/* W exactly nTopics weight vectors long (null: refused by the library), thresholds at least nTopics long (null: refused by
+ * the library), out at least DSGD_TOPIC_WORDS(nTopics) */
+static int req_thresholded_topics(JNIEnv *env, jlong h, jdoubleArray W, jint nTopics, jdoubleArray thresholds, rows_t r,
+                                  jlongArray out) {
+  buf_t bw = in_Double(env, W), bt = in_Double(env, thresholds), o = out_Long(env, out);
+  r.ids = in_Int(env, r.samples);
+  int32_t wl = 0;
+  int rc = checked(weight_len(h, &wl), bw.bad | bt.bad | o.bad | r.ids.bad, 0);
+  if (rc == DSGD_OK)
+    rc = checked(DSGD_OK, 0, nTopics < 1 || (bw.p && bw.n != (jlong)nTopics * wl) || (bt.p && bt.n < (jlong)nTopics) ||
+                                 o.n < DSGD_TOPIC_WORDS(nTopics));
+  if (rc == DSGD_OK)
+    rc = r.form == RANGE ? dsgd_eval_thresholded_topics(CTX(h), bw.p, nTopics, bt.p, r.rowBegin, r.rowEnd, o.p)
+         : r.form == DRAWN ? dsgd_eval_sampled_thresholded_topics(CTX(h), bw.p, nTopics, bt.p, r.rowBegin, r.rowEnd,
+                                                                  (uint64_t)r.key, r.posBegin, r.posEnd, o.p)
+                           : dsgd_eval_samples_thresholded_topics(CTX(h), bw.p, nTopics, bt.p, r.ids.p, r.ids.n, o.p);
+  back_Long(env, out, o, rc);
+  free(bw.p); free(bt.p); free(r.ids.p);
+  return rc;
+}
+FN(evalThresholdedTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdoubleArray thresholds,
+                          jlong rowBegin, jlong rowEnd, jlongArray out) {
+  return req_thresholded_topics(env, h, W, nTopics, thresholds, range_rows(rowBegin, rowEnd), out);
+}
+FN(evalSampledThresholdedTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdoubleArray thresholds,
+                                 jlong rowBegin, jlong rowEnd, jlong key, jlong posBegin, jlong posEnd, jlongArray out) {
+  return req_thresholded_topics(env, h, W, nTopics, thresholds, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd), out);
+}
+FN(evalSamplesThresholdedTopics)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdoubleArray thresholds,
+                                 jintArray samples, jlongArray out) {
+  return req_thresholded_topics(env, h, W, nTopics, thresholds, list_rows(samples), out);
+}
+/* W exactly nTopics weight vectors long (null: refused by the library), thresholds at least nTopics and words at least
+ * DSGD_TOPIC_TUNE_WORDS(nTopics) long */
+static int req_tune_topic_thresholds(JNIEnv *env, jlong h, jdoubleArray W, jint nTopics, jdouble fbr, rows_t r,
+                                     jdoubleArray thresholds, jlongArray words) {
+  buf_t bw = in_Double(env, W), t = out_Double(env, thresholds), o = out_Long(env, words);
+  r.ids = in_Int(env, r.samples);
+  int32_t wl = 0;
+  int rc = checked(weight_len(h, &wl), bw.bad | t.bad | o.bad | r.ids.bad, 0);
+  if (rc == DSGD_OK)
+    rc = checked(DSGD_OK, 0, nTopics < 1 || (bw.p && bw.n != (jlong)nTopics * wl) || t.n < (jlong)nTopics ||
+                                 o.n < DSGD_TOPIC_TUNE_WORDS(nTopics));
+  if (rc == DSGD_OK)
+    rc = r.form == RANGE ? dsgd_tune_topic_thresholds(CTX(h), bw.p, nTopics, fbr, r.rowBegin, r.rowEnd, t.p, o.p)
+         : r.form == DRAWN ? dsgd_tune_topic_thresholds_sampled(CTX(h), bw.p, nTopics, fbr, r.rowBegin, r.rowEnd,
+                                                                (uint64_t)r.key, r.posBegin, r.posEnd, t.p, o.p)
+                           : dsgd_tune_topic_thresholds_samples(CTX(h), bw.p, nTopics, fbr, r.ids.p, r.ids.n, t.p, o.p);
+  back_Double(env, thresholds, t, rc);
+  back_Long(env, words, o, rc);
+  free(bw.p); free(r.ids.p);
+  return rc;
+}
+FN(tuneTopicThresholds)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdouble fbr, jlong rowBegin,
+                        jlong rowEnd, jdoubleArray thresholds, jlongArray words) {
+  return req_tune_topic_thresholds(env, h, W, nTopics, fbr, range_rows(rowBegin, rowEnd), thresholds, words);
+}
+FN(tuneTopicThresholdsSampled)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdouble fbr,
+                               jlong rowBegin, jlong rowEnd, jlong key, jlong posBegin, jlong posEnd,
+                               jdoubleArray thresholds, jlongArray words) {
+  return req_tune_topic_thresholds(env, h, W, nTopics, fbr, drawn_rows(rowBegin, rowEnd, key, posBegin, posEnd),
+                                   thresholds, words);
+}
+FN(tuneTopicThresholdsSamples)(JNIEnv *env, jobject self, jlong h, jdoubleArray W, jint nTopics, jdouble fbr,
+                               jintArray samples, jdoubleArray thresholds, jlongArray words) {
+  return req_tune_topic_thresholds(env, h, W, nTopics, fbr, list_rows(samples), thresholds, words);
+}
 /* W exactly nTopics weight vectors long (null: refused by the library), words at least DSGD_TOPIC_RANK_WORDS(k) and sums
  * at least 2 + k (k itself is checked by the library) */
 static int req_topic_ranking(JNIEnv *env, jlong h, jdoubleArray W, jint nTopics, jint k, rows_t r, jlongArray words,

@@ -53,11 +53,12 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
     if cfg.bootstrap_weighted and cfg.is_async:
         raise ValueError("bootstrap-weighted: row weights belong to sync training; an asynchronous (Hogwild) context "
                          "has none to resample by")
-    from .ml.one_vs_rest import parse_topic_rank_k, parse_topics
+    from .ml.one_vs_rest import parse_topic_rank_k, parse_topic_thresholds, parse_topics
     topics = parse_topics(cfg.topics)
     if topics is not None and cfg.is_async:
         raise ValueError("topics: one-vs-rest training belongs to sync training; asynchronous (Hogwild) training has none")
     rank_k = parse_topic_rank_k(cfg.topic_rank_k, topics)
+    thr_mode, thr_fbr = parse_topic_thresholds(cfg.topic_thresholds, cfg.topic_threshold_fbr, topics)
     if topics is None:   # the binary run alone, with the rows as they always were
         data = dataclasses.replace(data, topics=None)
     elif data.topics is None:
@@ -192,6 +193,19 @@ def scenario(cfg, data, *, rank: int = 0, world: int = 1, device: Optional[int] 
                 log(f"topic ranking (k = {rank_k}, {rr['ranked_rows']} ranked test rows): precision@{rank_k} "
                     f"{rr['precision_at'][rank_k]:.4f}, recall@{rank_k} {rr['recall_at'][rank_k]:.4f}, LRAP "
                     f"{rr['lrap']:.4f}, coverage error {rr['coverage_error']:.3f}, ranking loss {rr['ranking_loss']:.5f}")
+        if thr_mode == "scut":
+            # SCut: each topic's F1-optimal margin threshold on the train rows, then the test rows judged at them
+            t1 = time.perf_counter()
+            tuned, summary = master.tune_topic_thresholds(ovr, test_data=False, fbr=thr_fbr)
+            tune_s = time.perf_counter() - t1
+            tt = master.local_topic_report(tuned, test_data=True)
+            report["topic_thresholds"] = {"mode": thr_mode, "fbr": thr_fbr, "tune_seconds": tune_s,
+                                          "thresholds": [float(x) for x in tuned.thresholds], "tuning": summary, "test": tt}
+            if rank == 0:
+                log(f"topic thresholds (scut, fbr {thr_fbr}, {tune_s:.2f} s on the train rows): test micro F1 "
+                    f"{tr['micro_f1']:.4f} -> {tt['micro_f1']:.4f}, macro F1 {tr['macro_f1']:.4f} -> {tt['macro_f1']:.4f}, "
+                    f"subset accuracy {tr['subset_accuracy']:.4f} -> {tt['subset_accuracy']:.4f}, Hamming loss "
+                    f"{tr['hamming_loss']:.5f} -> {tt['hamming_loss']:.5f}")
     if inspect:
         inspect("done", (master, state))
     slave.stop()

@@ -3,30 +3,36 @@
 `MasterSync.fit_one_vs_rest` trains them one topic after another on one device context (dsgd_select_topic switches the
 labels on the device), and `Master.local_topic_report` judges them all in one pass (dsgd_eval_*topics).  The ranking of a
 row's topics by their scores is one more pass: `OneVsRest.predict_topk` (dsgd_topics_topk) and
-`Master.local_topic_ranking_report` (dsgd_eval_*topic_ranking, read by `topic_ranking_report`).
+`Master.local_topic_ranking_report` (dsgd_eval_*topic_ranking, read by `topic_ranking_report`).  `Master.tune_topic_thresholds`
+places each topic's F1-optimal margin threshold (SCut, dsgd_tune_topic_thresholds*, read by `threshold_report`), which
+`OneVsRest.predict` and the topic reports then apply.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 import numpy as np
 
 
 @dataclass
 class OneVsRest:
-    """weights[t] is topic topics[t]'s weight vector (wdim values: dim, then the intercept on an intercept model), and
-    histories[t] the `fit` history of that topic."""
+    """weights[t] is topic topics[t]'s weight vector (wdim values: dim, then the intercept on an intercept model),
+    histories[t] the `fit` history of that topic, and thresholds[t] its margin threshold tau_t (None: every tau is 0, the
+    binary rule)."""
     weights: np.ndarray      # float64[T', wdim]
     topics: tuple            # the topic names, in the order of weights
     histories: List[dict]
+    thresholds: Optional[np.ndarray] = None   # float64[T'] (Master.tune_topic_thresholds)
 
     def predict(self, slave, idx: Sequence[int]) -> np.ndarray:
-        """bool[n, T']: topic t predicted present for row idx[i], i.e. p = +1 (x . w_t < 0), from slave.margins per topic."""
+        """bool[n, T']: topic t predicted present for row idx[i], i.e. p = +1: its margin x . w_t below tau_t (0 without
+        thresholds), from slave.margins per topic."""
         idx = np.asarray(idx, dtype=np.int32).reshape(-1)
         out = np.zeros((idx.size, len(self.topics)), dtype=bool)
         for t in range(len(self.topics)):
-            out[:, t] = slave.margins(idx, self.weights[t]) < 0.0
+            tau = 0.0 if self.thresholds is None else float(self.thresholds[t])
+            out[:, t] = slave.margins(idx, self.weights[t]) < tau
         return out
 
     def predict_topk(self, slave, idx: Sequence[int], k: int):
@@ -137,3 +143,45 @@ def topic_ranking_report(words, k: int) -> dict:
             "precision_at": {j: ratio(int(w[8 + j - 1]), j * N) for j in range(1, k + 1)},
             "recall_at": {j: ratio(sums[2 + j - 1], N) for j in range(1, k + 1)},
             "lrap": ratio(sums[0], N), "coverage_error": ratio(coverage, N), "ranking_loss": ratio(sums[1], N - every)}
+
+
+TOPIC_THRESHOLD_MODES = ("none", "scut")
+THRESHOLD_STATUS = ("tuned", "no positive row", "below fbr", "no margin")   # word 6 of DSGD_TOPIC_TUNE_WORDS
+
+
+def parse_topic_thresholds(mode: str, fbr: float, topics):
+    """The configuration values `topic-thresholds` (none or scut, only with `topics` set) and `topic-threshold-fbr` (in
+    [0, 1], non-zero only with scut): (mode, fbr)."""
+    mode = str(mode).strip().strip('"').strip().lower()
+    if mode not in TOPIC_THRESHOLD_MODES:
+        raise ValueError(f"topic-thresholds: expected one of {', '.join(TOPIC_THRESHOLD_MODES)}, got {mode!r}")
+    if mode != "none" and topics is None:
+        raise ValueError("topic-thresholds: tunes the thresholds of a one-vs-rest model; set `topics` too")
+    fbr = float(fbr)
+    if not 0.0 <= fbr <= 1.0:
+        raise ValueError(f"topic-threshold-fbr: expected a value in [0, 1], got {fbr}")
+    if fbr != 0.0 and mode != "scut":
+        raise ValueError("topic-threshold-fbr: the fallback of SCut tuning; set topic-thresholds = scut too")
+    return mode, fbr
+
+
+def threshold_report(words, thresholds, names) -> dict:
+    """The report of a dsgd_tune_topic_thresholds* call from its thresholds and DSGD_TOPIC_TUNE_WORDS(T) words
+    (T = len(names)).  Per topic: the threshold tau, the status and the chosen candidate j, the distinct non-NaN margins D,
+    the positive rows P, the NaN margins, and tp and the rows predicted present at tau with the tuned F1 = 2 tp / (P +
+    predicted) (nan where that is 0 / 0).  Then the rows and the topic count of each status."""
+    names = tuple(names)
+    T = len(names)
+    w = np.asarray(words, dtype=np.int64).reshape(-1)
+    thr = np.asarray(thresholds, dtype=np.float64).reshape(-1)
+    if w.size != 8 * T or thr.size != T:
+        raise ValueError(f"threshold_report: {w.size} words and {thr.size} thresholds for {T} topics, expected {8 * T} "
+                         f"and {T}")
+    per = {}
+    for t, name in enumerate(names):
+        rows, P, nan, D, tp, pred, status, j = (int(x) for x in w[8 * t:8 * t + 8])
+        per[name] = {"threshold": float(thr[t]), "status": THRESHOLD_STATUS[status], "candidate": j, "distinct_margins": D,
+                     "positives": P, "nan_margins": nan, "tp": tp, "predicted": pred,
+                     "f1": 2 * tp / (P + pred) if P + pred else float("nan")}
+    return {"topics": per, "rows": int(w[0]) if T else 0,
+            "status_counts": {s: sum(v["status"] == s for v in per.values()) for s in THRESHOLD_STATUS}}

@@ -58,6 +58,11 @@ def topic_rank_words(k: int) -> int:
     return 8 + int(k) + 7 * (2 + int(k))
 
 
+def topic_tune_words(n_topics: int) -> int:
+    """DSGD_TOPIC_TUNE_WORDS(T): eight words per topic (rows, P, NaN rows, D, tp, predicted, status, j)"""
+    return 8 * int(n_topics)
+
+
 class NativeLibraryMissing(ImportError):
     pass
 
@@ -193,9 +198,10 @@ _ROW_FAMILIES = {
 
 
 def row_methods(family: str) -> dict:
-    """{form: NativeCtx method} of an evaluation family, each bound to the entry point dsgd_<method>: <fit>, <fit>_sampled
-    and <fit>_samples for a fit; eval_<rest>, eval_sampled_<rest> and eval_samples_<rest> for the others."""
-    if family.startswith("calibrate"):
+    """{form: NativeCtx method} of an evaluation family, each bound to the entry point dsgd_<method>: eval_<rest>,
+    eval_sampled_<rest> and eval_samples_<rest> for an evaluation; <fit>, <fit>_sampled and <fit>_samples for the others
+    (the fits and the tuning)."""
+    if not family.startswith("eval_"):
         return {"range": family, "drawn": f"{family}_sampled", "list": f"{family}_samples"}
     rest = family[len("eval_"):]
     return {"range": f"eval_{rest}", "drawn": f"eval_sampled_{rest}", "list": f"eval_samples_{rest}"}
@@ -210,6 +216,12 @@ ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32] + _ROW_PREFIX[form][2
 ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32, _i32] + _ROW_PREFIX[form][2:] + [_vp, _vp]
             for form, name in row_methods("eval_topic_ranking").items()})
 ABI["dsgd_topics_topk"] = [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]
+# the threshold tuning takes the count and fbr before the rows, then thresholds and words; the thresholded topic family takes
+# the count and the thresholds before the rows, then the words
+ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32, _f64] + _ROW_PREFIX[form][2:] + [_vp, _vp]
+            for form, name in row_methods("tune_topic_thresholds").items()})
+ABI.update({"dsgd_" + name: _ROW_PREFIX[form][:2] + [_i32, _vp] + _ROW_PREFIX[form][2:] + [_vp]
+            for form, name in row_methods("eval_thresholded_topics").items()})
 
 
 def lib():
@@ -1012,6 +1024,53 @@ class NativeCtx:
         if W.ndim != 2 or W.shape[1] != self.wdim:
             raise DsgdInvalid(ERR_INVALID, f"{fn}: W must be [T, {self.wdim}], got {W.shape}")
         return W
+
+    def _thresholded_topics(self, fn: str, W, thresholds, rows: _Rows) -> np.ndarray:
+        W = self._topic_W(fn, W)
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64).reshape(-1)
+        if thr.size != W.shape[0]:
+            raise DsgdInvalid(ERR_INVALID, f"{fn}: {thr.size} thresholds for {W.shape[0]} weight vectors")
+        out = np.zeros(topic_words(W.shape[0]), dtype=np.int64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(W), W.shape[0], _ptr(thr), *rows.args, _ptr(out)))
+        return out
+
+    def eval_thresholded_topics(self, row_begin: int, row_end: int, W, thresholds) -> np.ndarray:
+        """eval_topics with topic t predicted present when its margin is below thresholds[t], absent above it, and not
+        predicted at it or for a NaN margin (dsgd_eval_thresholded_topics)."""
+        return self._thresholded_topics("eval_thresholded_topics", W, thresholds, _range(row_begin, row_end))
+
+    def eval_sampled_thresholded_topics(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, W,
+                                        thresholds) -> np.ndarray:
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_eval_sampled_thresholded_topics)."""
+        return self._thresholded_topics("eval_sampled_thresholded_topics", W, thresholds,
+                                        _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def eval_samples_thresholded_topics(self, samples, W, thresholds) -> np.ndarray:
+        """The same over a list of row ids; repeats count every time (dsgd_eval_samples_thresholded_topics)."""
+        return self._thresholded_topics("eval_samples_thresholded_topics", W, thresholds, _list(samples))
+
+    def _tune(self, fn: str, W, fbr: float, rows: _Rows) -> Tuple[np.ndarray, np.ndarray]:
+        W = self._topic_W(fn, W)
+        thr = np.zeros(W.shape[0], dtype=np.float64)
+        words = np.zeros(topic_tune_words(W.shape[0]), dtype=np.int64)
+        self._ck(getattr(self._l, "dsgd_" + fn)(self._h, _ptr(W), W.shape[0], float(fbr), *rows.args, _ptr(thr),
+                                                  _ptr(words)))
+        return thr, words
+
+    def tune_topic_thresholds(self, row_begin: int, row_end: int, W, fbr: float = 0.0) -> Tuple[np.ndarray, np.ndarray]:
+        """(thresholds float64[T], words int64[8 T]): each topic's F1-optimal margin threshold (SCut, with the fbr fallback)
+        over rows [row_begin, row_end), and per topic the words rows, P, NaN rows, D, tp and rows predicted at the
+        threshold, status and candidate (dsgd_tune_topic_thresholds)."""
+        return self._tune("tune_topic_thresholds", W, fbr, _range(row_begin, row_end))
+
+    def tune_topic_thresholds_sampled(self, row_begin: int, row_end: int, key: int, pos_begin: int, pos_end: int, W,
+                                      fbr: float = 0.0) -> Tuple[np.ndarray, np.ndarray]:
+        """The same over positions [pos_begin, pos_end) of the device-drawn sample (dsgd_tune_topic_thresholds_sampled)."""
+        return self._tune("tune_topic_thresholds_sampled", W, fbr, _drawn(row_begin, row_end, key, pos_begin, pos_end))
+
+    def tune_topic_thresholds_samples(self, samples, W, fbr: float = 0.0) -> Tuple[np.ndarray, np.ndarray]:
+        """The same over a list of row ids; repeats count every time (dsgd_tune_topic_thresholds_samples)."""
+        return self._tune("tune_topic_thresholds_samples", W, fbr, _list(samples))
 
     def _topic_ranking(self, fn: str, W, k: int, rows: _Rows) -> Tuple[np.ndarray, np.ndarray]:
         W = self._topic_W(fn, W)

@@ -49,6 +49,10 @@ class Config:  # field order and names: utils/Config.scala:3-21 (kebab-case in t
                                   # all, or a comma-separated list of topic names; sync mode only
     topic_rank_k: int = 0         # extension: with `topics`, rank every test row's topics and report precision and recall at
                                   # 1..k, LRAP, coverage error and ranking loss; 0: off, else 1..32
+    topic_thresholds: str = "none"   # extension: with `topics`, scut tunes every topic's F1-optimal margin threshold on the
+                                     # train rows after the fit and reports the test topics at them; none: every threshold 0
+    topic_threshold_fbr: float = 0.0   # extension: with scut, a topic whose best train F1 is below this keeps only its
+                                       # top-scored rows (SCutFBR.1); in [0, 1], 0: off
 
 
 # application.conf key -> (Config field, DSGD_* variable)   (resources/application.conf:2-50)
@@ -72,6 +76,8 @@ _KEYS = {
     "bootstrap-weighted": ("bootstrap_weighted", "DSGD_BOOTSTRAP_WEIGHTED"),
     "topics": ("topics", "DSGD_TOPICS"),
     "topic-rank-k": ("topic_rank_k", "DSGD_TOPIC_RANK_K"),
+    "topic-thresholds": ("topic_thresholds", "DSGD_TOPIC_THRESHOLDS"),
+    "topic-threshold-fbr": ("topic_threshold_fbr", "DSGD_TOPIC_THRESHOLD_FBR"),
 }
 MODELS = ("svm", "logistic", "squared_hinge", "modified_huber")
 _TYPES = {f.name: f.type for f in fields(Config)}
@@ -155,6 +161,8 @@ def load_config(path: Optional[str] = None, env: Optional[Dict[str, str]] = None
         raise ValueError(f"bootstrap: expected a number of replicates >= 0 (0: off), got {cfg.bootstrap}")
     if cfg.sample_weight and not cfg.sample_weight.endswith(".npy"):
         raise ValueError(f"sample-weight: expected the path of a .npy file, or empty for off, got {cfg.sample_weight!r}")
-    from ..ml.one_vs_rest import parse_topic_rank_k, parse_topics
-    parse_topic_rank_k(cfg.topic_rank_k, parse_topics(cfg.topics))   # raises on a malformed value of either
+    from ..ml.one_vs_rest import parse_topic_rank_k, parse_topic_thresholds, parse_topics
+    topics = parse_topics(cfg.topics)
+    parse_topic_rank_k(cfg.topic_rank_k, topics)   # raises on a malformed value of any of these
+    parse_topic_thresholds(cfg.topic_thresholds, cfg.topic_threshold_fbr, topics)
     return cfg

@@ -288,6 +288,48 @@ int dsgd_eval_sampled_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, i
 int dsgd_eval_samples_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const int32_t *samples, int64_t n,
                              int64_t *out);
 
+/* ---- Per-topic decision thresholds (DESIGN.md §4.23).  Sync mode only.  For a row and topic t, m_t is the margin
+ *      dsgd_margins returns for W_t, bit for bit (fl(x . W_t + filt(beta_t)) on an intercept ctx).  The thresholded rule at
+ *      tau_t: p_t = +1 (present) when m_t < tau_t, -1 when m_t > tau_t, and 0 (no prediction) when m_t == tau_t or m_t is
+ *      NaN; at tau = +-0 it is dsgd_forward's prediction.
+ *      dsgd_tune_topic_thresholds*: SCut, the F1-optimal threshold of every topic over the rows of the request (the three
+ *      row forms of the metrics calls; a list counts repeats every time).  For topic t, P = rows with topic t (from the
+ *      loaded topics, never the current labels; NaN-margin rows included) and c_0 < ... < c_(D-1) its distinct non-NaN
+ *      margins (+0 and -0 are one).  Candidate j predicts present the pp_j rows with m <= c_j, tp_j of them with the topic;
+ *      its threshold is tau_j = mid = fl(c_j / 2 + c_(j+1) / 2) when c_j < mid <= c_(j+1), else c_(j+1), and tau_(D-1) =
+ *      +inf.  The best candidate has the highest F1_j = 2 tp_j / (P + pp_j), compared exactly, ties to the lowest j.
+ *      Status (word 6) and thresholds_out[t]:
+ *        0 tuned          tau of the best candidate
+ *        1 no positive    P = 0 (and D > 0): tau = 0, j = -1
+ *        2 below fbr      fl(2 tp / (P + pp)) < fbr for the best candidate: tau_0 (SCutFBR.1), j = 0
+ *        3 no margin      D = 0 (no non-NaN margin, or no row): tau = 0, j = -1
+ *      words_out holds DSGD_TOPIC_TUNE_WORDS(T) int64 words, eight per topic at 8 t: rows, P, rows with a NaN margin, D, then
+ *      tp and rows predicted present by the thresholded rule at thresholds_out[t] over the same rows, the status and j.  At
+ *      tau_j the rule predicts candidate j's rows, except a last candidate at c = +inf, whose rows at +inf sit at tau = +inf
+ *      and get no prediction.  Every output has the same bits for a multiset of rows whatever the grid, the row order, the
+ *      form or the topic grouping.  The errors of dsgd_eval*_topics, a NULL output, and fbr NaN or outside [0, 1] ->
+ *      DSGD_ERR_INVALID, all before anything is launched or grown.  Rows are replicated on every rank, and a call tunes over
+ *      its whole request.  The topics go in groups of G = max(1, min(T, floor(2^27 / n))) over n positions: the call keeps
+ *      18 G n bytes of device workspace.
+ *      dsgd_eval*_thresholded_topics: the words of dsgd_eval*_topics with p_t by the thresholded rule at thresholds[t]; the
+ *      exact-match word (8 T + 1) uses these p_t, the top-1 word (8 T + 2) still ranks the raw margins.  Its errors, a NULL
+ *      thresholds or a NaN threshold (+-inf are allowed) -> DSGD_ERR_INVALID, all before anything is launched. */
+#define DSGD_TOPIC_TUNE_WORDS(T) (8 * (int64_t)(T))
+int dsgd_tune_topic_thresholds(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr, int64_t row_begin,
+                               int64_t row_end, double *thresholds_out, int64_t *words_out);
+int dsgd_tune_topic_thresholds_sampled(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr, int64_t row_begin,
+                                       int64_t row_end, uint64_t key, int64_t pos_begin, int64_t pos_end,
+                                       double *thresholds_out, int64_t *words_out);
+int dsgd_tune_topic_thresholds_samples(dsgd_ctx *ctx, const double *W, int32_t n_topics, double fbr,
+                                       const int32_t *samples, int64_t n, double *thresholds_out, int64_t *words_out);
+int dsgd_eval_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const double *thresholds,
+                                 int64_t row_begin, int64_t row_end, int64_t *out);
+int dsgd_eval_sampled_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const double *thresholds,
+                                         int64_t row_begin, int64_t row_end, uint64_t key, int64_t pos_begin,
+                                         int64_t pos_end, int64_t *out);
+int dsgd_eval_samples_thresholded_topics(dsgd_ctx *ctx, const double *W, int32_t n_topics, const double *thresholds,
+                                         const int32_t *samples, int64_t n, int64_t *out);
+
 /* ---- Ranking a row's topics (DESIGN.md §4.22).  Sync mode only.  For a row and topic t, m_t is the margin dsgd_margins
  *      returns for W_t, bit for bit (fl(x . W_t + filt(beta_t)) on an intercept ctx), and its score is s_t = -m_t: a higher
  *      score ranks first, and +0 and -0 are one score.  Y is the row's loaded topics (never the current labels), n_Y = |Y|.
