@@ -22,17 +22,28 @@
 //     are back to back in the pair array -- so its four loads leave before the row-end masks are even computed.
 //   * Blocks are dealt dynamically (one atomic per block, requested a block ahead); the last fifth of a pass goes out in
 //     blocks of half the size so the warps run dry together.
-//   * Exactness against the fp64 arithmetic of the reference: the fp32 result differs from x.w by at most
-//       (D + 1) * 2^-24 * max|w| * sum|x|,   D = units/32 + 9 roundings on the longest add chain, + 1 for rounding w
-//     (first-order bound, 1.5x slack); sum|x| per row is computed once when the rows are loaded (k_repack, rounded
-//     up, stored with the label in its sign bit: one 4-byte load per row).  The reference also drops every value and
-//     every product with magnitude <= 1e-20 (the Sparse constructor, filt): k_repack stores such values as 0, and the
-//     products the fp32 dot keeps are bounded by 1e-20 per pair, so the band gets 2 * 1e-20 per unit on top.  Rows
-//     whose |dot| is inside that band are recomputed after the block's stream with the fp64 weights from L2, by the row fold
-//     (dsgd_kernels.cuh) that decides the row on every other path (tests/test_gpu_streaming.py, test_gpu_row_fold.py;
-//     dsgd_stream_exact_rows counts the recomputed rows).  Outside the band the fp32 sign is the row fold's sign: there
-//     |exact x.w| >= band / 3, far above the difference between any two fp64 summation orders, so every prediction and
-//     gate decision of the pass is that of the row fold.
+//   * Exactness against the fp64 arithmetic of the reference.  Let W = max(max|w32|, 2^-126) over the staged weights and
+//     u = 2^-24.  If the fp32 dot is FINITE, no operation of its chain overflowed (an overflow gives +-inf, and inf + x is
+//     inf or NaN), and no weight the row reads is infinite or NaN (0 * inf and x * NaN are NaN).  Then every rounding is
+//     relative with at most u, or absolute: (float)w is within max(u |w|, 2^-150) <= u W of w, and a product or fma that
+//     lands in fp32's subnormal range is within 2^-150 (sums of fp32 values are exact there).  So the fp32 result differs
+//     from x.w by at most
+//       (D + 1) * u * W * sum|x| + 2 * 2^-150 per unit,   D = units/32 + 9 roundings on the longest add chain
+//     (product, fma, at most units/32 + 1 lane additions, 5 butterfly steps), + 1 for rounding w (first-order bound,
+//     1.5x slack).  sum|x| per row is computed once when the rows are loaded (k_repack, rounded up -- to inf when it
+//     exceeds FLT_MAX -- and stored with the label in its sign bit: one 4-byte load per row).  The reference also drops
+//     every value and every product with magnitude <= 1e-20 (the Sparse constructor, filt): k_repack stores such values
+//     as 0, and the products the fp32 dot keeps are bounded by 1e-20 per pair, so the band gets 2 * 1e-20 per unit on top
+//     (which also covers the subnormal 2^-150 terms).  The band is formed in fp64 from W, which is at least 2^-126, so it
+//     neither underflows (a band of 0 would decide every row of subnormal weights from its fp32 sign) nor overflows.  Rows
+//     whose fp32 dot is not finite or whose |dot| is inside the band are recomputed after the block's stream with the fp64
+//     weights from L2, by the row fold (dsgd_kernels.cuh) that decides the row on every other path
+//     (tests/test_gpu_streaming.py, test_gpu_stream_range.py, test_gpu_row_fold.py; tests/stream_band_model.py restates
+//     this decision on the CPU; dsgd_stream_exact_rows counts the recomputed rows).  Outside the band the fp32 sign is the
+//     row fold's sign: there |exact x.w| >= band / 3, far above the difference between any two fp64 summation orders
+//     (every fp64 product is finite: |x| and |w| are at most FLT_MAX), so every prediction and gate decision of the
+//     pass is that of the row fold.  An infinite weight anywhere makes W, hence every band, infinite (or NaN on a row
+//     whose values were all filtered): the whole pass is recomputed.
 //   * Scatter (gradient): rows that pass the gate are re-walked after the block's stream (their units are in
 //     L1/L2) and y*x goes to g with fp64 REDs.  On trained weights few rows pass (the misclassified ones) and the pass
 //     runs at the streaming rate; on untrained weights every row passes and the fp64 RED rate at L2 bounds it
@@ -156,7 +167,6 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
 #pragma unroll
     for (int i = 0; i < kStreamThreads / 32; ++i) wmax = fmaxf(wmax, s_wmax[i]);
   }
-  const float band_scale = 1.5f * 5.9604645e-8f * wmax;   // 1.5 * 2^-24 * max|w|
   // one gradient entry (SparseSVM.scala:26-29): a reduction without a return value
   auto scatter_one = [&](uint32_t col, double gv) {
     if (gv != 0.0) red_add_f64(&p.g[col], gv);
@@ -285,9 +295,15 @@ __global__ void __launch_bounds__(kStreamThreads, 1) k_stream_rows(const StreamP
       do_scatter = kScatter && (pr != y);
     };
     if (valid) {
-      // rounding band + the products the reference drops (|x_j w_j| <= 1e-20, filt) but the fp32 dot keeps: one per pair
-      const float thresh = band_scale * fabsf(ya) * (float)((len >> 5) + 10) + 2e-20f * (float)len;
-      if (!(fabsf(dot_mine) > thresh)) need_exact = true;   // also catches NaN
+      // rounding band + the products the reference drops (|x_j w_j| <= 1e-20, filt) but the fp32 dot keeps: one per pair.
+      // In fp64, so that neither the band nor its product with yabs underflows or overflows; a dot that is not finite (an
+      // fp32 overflow somewhere in the chain, an inf or NaN weight) says nothing about the fp64 sign.
+      // 1.5 * 2^-24 * max(max|w|, 2^-126): 2^-24 * 2^-126 bounds the rounding of a subnormal weight (formed per row, so
+      // that the stream loop keeps one fp32 register for it, as before)
+      const double band_scale = 1.5 * 5.9604644775390625e-8 * fmax((double)wmax, 1.1754943508222875e-38);
+      const double thresh = band_scale * (double)fabsf(ya) * (double)((len >> 5) + 10) + 2e-20 * (double)len;
+      const float adot = fabsf(dot_mine);
+      if (!(adot <= 3.40282347e38f && (double)adot > thresh)) need_exact = true;   // also catches NaN
       else finalize(dot_mine > 0.f ? -1 : 1);
     }
     // ---- exact recomputation of the rows the fp32 sign could not decide ----
